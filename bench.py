@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Benchmark of the vietTTS hot path on B200 (contract: see the task statement / DESIGN.md §Measurement).
+"""Benchmark of the vietTTS hot path on one or more H100s (DESIGN.md §Measurement).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
 
 Workload (BASELINE.json configs[2], the one the metric is quoted on): per GPU a batch of 32
@@ -17,6 +17,8 @@ rank gets its own 32 utterances; the weights are broadcast once from rank 0 over
            stage time (CUDA events recorded around the stage inside the timed region)
   cpu_baseline: the oracle port (torch CPU restatement of the reference) on the host cores,
            bounded sample of the same workload.
+  --dump-outputs DIR: after the timed steps, the mel and waveform the timed path returned in its last step are written
+           as DIR/mel.npy and DIR/wav.npy (float32); the inputs are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -47,7 +49,9 @@ def peaks():
         d = json.loads(p.read_text())
         return dict(hbm_gbs=d.get("hbm_gbs", 6650.0), bf16_tflops=d.get("bf16_tflops", 1590.0),
                     bf16_tflops_sustained=d.get("bf16_tflops_sustained", 1400.0), source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- not measured; a card run at a lower
+    # power limit sustains less
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source="H100 SXM data sheet (not measured)")
 
 
 def make_batch(batch: int, phonemes: int, seconds: float, seed0: int):
@@ -238,7 +242,7 @@ def workload_config(args, world):
     return dict(workload=f"NAT acoustic + HiFiGAN, {args.phonemes}-phoneme / {args.seconds:g} s utterances, batch {args.batch} per GPU (BASELINE configs[2])",
                 batch_per_gpu=args.batch, phonemes=args.phonemes, mel_frames=n, samples_per_utterance=n * C.HOP,
                 parallelism=f"utterance-sharded x{world}",
-                l2="activations per step (>4 GB) exceed the 126 MB L2; no flush needed", dropout="on-device threefry keep-masks")
+                l2="activations per step (>4 GB) exceed the 50 MB L2; no flush needed", dropout="on-device threefry keep-masks")
 
 
 class Job:
@@ -296,6 +300,17 @@ def time_jobs(jobs, steps, warmup, barrier):
     return ms, ac, hg
 
 
+def dump_outputs(out_dir, job):
+    """What the timed path returned in its last step: the mel [B, N, 80] and the waveform [B, N * 256], float32
+    (13 MB at the default batch)."""
+    import torch
+    torch.cuda.synchronize()
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    np.save(d / "mel.npy", job.mel_t.cpu().numpy().astype(np.float32))
+    np.save(d / "wav.npy", job.wav_t.cpu().numpy().astype(np.float32))
+
+
 def time_e2e(eng, job, steps, out):
     """Wall time of `steps` host-buffer calls (numpy in -> H2D -> kernels -> D2H -> numpy out)."""
     for _ in range(2):
@@ -316,7 +331,7 @@ def stage_rooflines(eng, job, pk, precision):
     ms = eng.substages(False)
     rows, frames = job.B, job.frames
     hbm = pk["hbm_gbs"]
-    tc_ceiling = pk["bf16_tflops_sustained"] / 3.0 if precision != "fp32" else 74.4
+    tc_ceiling = pk["bf16_tflops_sustained"] / 3.0 if precision != "fp32" else 67.0
     out = {}
 
     def tensor(name, key, flop, note=None):
@@ -385,8 +400,6 @@ def run_ours(args):
 
     eng = Engine(local)
     eng.set_precision(args.precision)
-    if args.tc_variant is not None:
-        eng.tc_stats(False, variant=args.tc_variant)
     if args.pairs != "auto":
         eng.set_fused_pairs(args.pairs != "off", kind=None if args.pairs == "off" else args.pairs)
     hp = synthetic.hifigan_params(1234) if rank == 0 else None
@@ -430,6 +443,8 @@ def run_ours(args):
     ms_step, ac_ms, hg_ms = time_jobs([job], args.steps, W, barrier)
     launches = (eng.launch_count() - l0) * args.steps // (args.steps + W)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, job)
     ms_step = allmax(ms_step)
     value = world * job.samples / (ms_step / 1e3)
 
@@ -543,7 +558,7 @@ def run_ours(args):
         mel_info = dict(samples_per_s=MB * S / (mms / 1e3), ms=mms, achieved_gbs=mbytes / (mms / 1e3) / 1e9,
                         peak_gbs=pk["hbm_gbs"], frac_hbm=mbytes / (mms / 1e3) / 1e9 / pk["hbm_gbs"],
                         achieved_tflops_fp32=mflop / (mms / 1e3) / 1e12, batch=MB, samples_per_row=S,
-                        fp32_peak_tflops=74.4, frac_fp32=mflop / (mms / 1e3) / 1e12 / 74.4,
+                        fp32_peak_tflops=67.0, frac_fp32=mflop / (mms / 1e3) / 1e12 / 67.0,
                         note="one warp per frame pair, FFT-1024 = 32 x 32 four-step with register-resident 32-point transforms; arithmetic intensity "
                              "22 FLOP/B sits above the FP32 ridge (11 FLOP/B): the kernel is FP32-issue bound, not HBM bound")
         if stages is not None:
@@ -611,11 +626,11 @@ def run_ours(args):
                 traffic = tj["generator_dram_bytes_per_step"]
                 traffic_src = f"sum of dram__bytes_read+write over the generator launches of one step, ncu launch list of this command ({tp.name}); not re-measured in this run"
                 break
-        ceiling = pk["bf16_tflops_sustained"] / 3.0 if args.precision != "fp32" else 74.4
+        ceiling = pk["bf16_tflops_sustained"] / 3.0 if args.precision != "fp32" else 67.0
         out = dict(
             metric=METRIC, value=value, unit=UNIT, n_gpus=world, steps=args.steps, warmup=W, ms_per_step=ms_step,
             higher_is_better=True, scaling="weak", vs_baseline=None,
-            dtype="f32" if args.precision == "fp32" else "f32 (bf16x3 split products on tcgen05, fp32 accumulate/storage)", data="synthetic",
+            dtype="f32" if args.precision == "fp32" else "f32 (bf16x3 split products on wgmma tensor cores, fp32 accumulate/storage)", data="synthetic",
             rtf=(ms_step / 1e3) / (world * job.samples / C.SAMPLE_RATE),
             config=workload_config(args, world),
             stages_ms=dict(acoustic=ac_ms, hifigan=hg_ms),
@@ -625,17 +640,17 @@ def run_ours(args):
                                           note="same call with a plain numpy result array (the reference's return type): one more host copy")),
             gpu_launches=int(launches),
             roofline=dict(bound="tensor",
-                          kernel=("tcgen05 conv kernels of the generator (tc_conv_kernel, CTA-pair form for C >= 128, + tc_pair2_kernel), all launches of one step (+ conv_post, 1 % of the stage time)"
+                          kernel=("wgmma conv kernels of the generator (tc_conv_kernel + tc_pair_kernel), all launches of one step (+ conv_post, 1 % of the stage time)"
                                   if args.precision != "fp32" else "conv1d_nwc_kernel: the generator launches of one step (+ conv_post)"),
                           achieved=ach, peak=pk["bf16_tflops_sustained"], unit="TFLOP/s", frac=ach / pk["bf16_tflops_sustained"],
                           traffic=traffic, traffic_source=traffic_src,
                           algorithmic_flops_per_step=flops, launch_ms=hg_ms,
                           frac_of_mode_ceiling=ach / ceiling,
                           mode_ceiling=("1/3 of the bf16 peak: bf16x3 issues three bf16 MMAs per algorithmic product" if args.precision != "fp32"
-                                        else "FP32 FMA pipe, nominal 74.4 TFLOP/s"),
-                          peak_source=pk["source"] + ", sustained bf16 dense",
+                                        else "FP32 FMA pipe, 67 TFLOP/s (H100 SXM data sheet)"),
+                          peak_source=pk["source"] + ", bf16 dense",
                           note=("algorithmic fp32 FLOPs; the bf16x3 path issues 3 bf16 MMAs per algorithmic product, so 1/3 of the bf16 peak is its ceiling"
-                                if args.precision != "fp32" else "strict-fp32 path runs on the FP32 FMA pipe (nominal 74 TFLOP/s)")),
+                                if args.precision != "fp32" else "strict-fp32 path runs on the FP32 FMA pipe (67 TFLOP/s, H100 SXM data sheet)")),
             roofline_stages=stages,
             clocks=clocks, weights=dict(bytes=wbytes, broadcast_s=t_w), melspec=mel_info, callers=callers,
             sweep=sweep, strict_fp32=strict, configs=configs or None,
@@ -664,12 +679,13 @@ def main():
     ap.add_argument("--no-sweep", action="store_true", help="skip the batch sweep and the strict-fp32 line")
     ap.add_argument("--no-configs", action="store_true", help="skip BASELINE configs[3] / configs[4]")
     ap.add_argument("--c5-groups", type=int, default=0, help="equal-cost buckets per rank of the mixed-length workload (0 = pick 2..4 by predicted makespan)")
-    ap.add_argument("--pairs", default="auto", choices=["auto", "off", "smem2", "smem2c", "tmem", "smem"],
-                    help="C<=64 ResBlock pairs: auto = library default, off = two conv launches per pair, tmem / smem = fused pair kernel "
-                         "with the A operand in tensor memory / shared memory")
-    ap.add_argument("--tc-variant", type=int, default=None, help="tile-shape variant of tc_conv (tuning aid; default: library default)")
+    ap.add_argument("--pairs", default="auto", choices=["auto", "off", "smem2", "tmem", "smem"],
+                    help="C<=64 ResBlock pairs: auto = library default, off = two conv launches per pair, smem2 / tmem / smem = fused pair "
+                         "kernel with 256-row tiles / the same with conv2's A operand in registers / 128-row tiles")
     ap.add_argument("--precision", default="bf16x3", choices=["bf16x3", "fp32"],
-                    help="conv arithmetic: bf16x3 = tcgen05 split-bf16 with fp32 accumulate (default), fp32 = FMA pipe")
+                    help="conv arithmetic: bf16x3 = split-bf16 on the tensor cores with fp32 accumulate (default), fp32 = FMA pipe")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the mel and waveform of the last timed step as DIR/mel.npy, DIR/wav.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * viettts_b200.h -- C ABI of the B200-native vietTTS hot path (libviettts_b200.so).
+ * viettts_b200.h -- C ABI of the H100-native vietTTS hot path (libviettts_b200.so).
  *
  * The reference (NTT123/vietTTS) has no FFI: its seams for this path are three
  * Python callables.  Each entry point below names the reference interface it
@@ -19,7 +19,7 @@
  *     cudaStream_t passed as void*, NULL = default stream).
  *   - every call returns 0 on success or a negative vtts_status; the message is
  *     available from vtts_last_error().  Nothing throws across the ABI.  There is
- *     NO CPU fallback: without a usable sm_100 device vtts_create fails.
+ *     NO CPU fallback: without a usable sm_90 (H100) device vtts_create fails.
  *   - one context per GPU; a context is not thread-safe; `*_forward` calls are
  *     stream-ordered and asynchronous, `*_host` calls copy H2D/D2H through pinned
  *     staging owned by the context and return after the result is in host memory.
@@ -43,7 +43,7 @@ typedef enum vtts_status {
   VTTS_ERR_BAD_ARG = -1,
   VTTS_ERR_CUDA = -2,
   VTTS_ERR_NOT_LOADED = -3,   /* weights for this stage were not loaded */
-  VTTS_ERR_NO_DEVICE = -4,    /* no CUDA device / not an sm_100 part */
+  VTTS_ERR_NO_DEVICE = -4,    /* no CUDA device / not an sm_90 part */
   VTTS_ERR_OOM = -5,
   VTTS_ERR_NCCL = -6          /* NCCL missing or a collective failed (vtts_broadcast_weights) */
 } vtts_status;
@@ -57,8 +57,8 @@ typedef enum vtts_dropout_mode {
 
 /* arithmetic of the dense conv contractions (97 % of the FLOPs):
  *   FP32    every product and sum in IEEE fp32 on the FMA pipe (conv1d.cu) -- the strict parity mode
- *   BF16X3  tcgen05 tensor cores, each fp32 operand split into bf16 hi+lo, three products
- *           (hi*hi + hi*lo + lo*hi) accumulated in fp32 in TMEM (tc_conv.cu); fp32-class accuracy
+ *   BF16X3  wgmma tensor cores, each fp32 operand split into bf16 hi+lo, three products
+ *           (hi*hi + hi*lo + lo*hi) accumulated in fp32 registers (tc_conv.cu); fp32-class accuracy
  *           (waveform L-inf 2e-5 vs float64), no reduced-precision storage anywhere. */
 typedef enum vtts_precision { VTTS_PRECISION_FP32 = 0, VTTS_PRECISION_BF16X3 = 1 } vtts_precision;
 

@@ -6,7 +6,7 @@ Only `tests/`, `__graft_entry__.smoke()` and `bench.py`'s cpu_baseline /
 `viettts_b200/` imports it; the product path fails loudly when the CUDA library
 is missing.
 
-What each module restates (file:line into /root/reference):
+What each module restates (file:line into the reference tree, NTT123/vietTTS):
 
   hifigan_oracle.py  vietTTS/hifigan/model.py:8-125 (Generator, ResBlock1, get_padding)
                      PINNED: checked against the reference's own importable torch
@@ -18,7 +18,7 @@ What each module restates (file:line into /root/reference):
                      (text2mel.py:85-103), the teacher-forced pass with zoneout
                      (model.py:146-169) and the GTA forward (gta.py:28-41).
                      PINNED TO THE REFERENCE'S OWN SOURCE (wiring), third-party primitives restated:
-                     jax / dm-haiku cannot be installed on either box (profiles/r2_ref_deps_probe_*.json)
+                     jax / dm-haiku cannot be installed on either box
                      and the reference's tests hold no golden vectors for this path, so the golden
                      vectors come from EXECUTING the unmodified vietTTS/nat/{model,text2mel,gta}.py with
                      numpy stand-ins for the jax / haiku API surface they touch (tests/refshim,

@@ -1,6 +1,6 @@
 """CPU restatement of the Haiku HiFiGAN generator.  Test infrastructure only.
 
-Follows /root/reference/vietTTS/hifigan/model.py line by line, in the NWC layout
+Follows the reference's vietTTS/hifigan/model.py line by line, in the NWC layout
 and with the Haiku parameter layout of hk_hifi.pickle:
 
   get_padding      model.py:8-10

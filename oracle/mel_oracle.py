@@ -2,7 +2,7 @@
 
 Pinned to the output of the reference's own dsp.py executed on numpy stand-ins for jax / librosa
 (tests/refshim, tests/golden/nat_ref_gta.npz `logmel`, tests/test_reference_goldens.py).
-Follows /root/reference/vietTTS/nat/dsp.py:
+Follows the reference's vietTTS/nat/dsp.py:
 
   rolling_window   dsp.py:11-25
   batched_stft     dsp.py:65-101  (center=False path; periodic Hann = hanning(1025)[:-1])

@@ -3,7 +3,7 @@
 Pinned to golden vectors produced by executing the reference's own source files on numpy stand-ins
 for jax / haiku (tests/refshim, tests/golden/make_nat_golden.py, tests/test_reference_goldens.py): the
 WIRING below is held to the reference at float64; the dm-haiku / jax primitives it relies on are
-restated (jax / dm-haiku cannot be installed here or on the GPU box: profiles/r2_ref_deps_probe_*.json)
+restated (jax / dm-haiku cannot be installed where this project is tested)
 and cross-checked against torch operators.  float64 mode is the arbiter for the float32 CUDA path.
 
   TokenEncoder.__call__      vietTTS/nat/model.py:26-47

@@ -1,4 +1,4 @@
-"""CPU emulation of the dense-contraction arithmetic modes on the whole HiFiGAN generator (profiles/r1_precision_study.txt).
+"""CPU emulation of the dense-contraction arithmetic modes on the whole HiFiGAN generator.
 
 Every conv / transposed conv of the oracle is replaced by a version that rounds its operands the way a mode does,
 multiplies the rounded operands in float64 (exact products) and rounds each layer output to fp32 -- i.e. the only

@@ -15,7 +15,7 @@ def pytest_configure(config):
         torch.set_num_threads(min(16, os.cpu_count() or 1))
     except Exception:
         pass
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu)")
 
 
 @pytest.fixture(scope="session")

@@ -1,6 +1,6 @@
 """Generate golden vectors for the HiFiGAN path from the REFERENCE ITSELF.
 
-Run in the build container (needs /root/reference; the GPU box does not have it):
+Run where a checkout of NTT123/vietTTS is available (VIETTTS_REFERENCE=<path>):
 
     python tests/golden/make_golden.py
 
@@ -34,7 +34,7 @@ import numpy as np
 import torch
 
 REPO = Path(__file__).resolve().parents[2]
-REF = Path("/root/reference")
+REF = Path(os.environ.get("VIETTTS_REFERENCE", "vietTTS-reference"))   # a checkout of NTT123/vietTTS
 sys.path.insert(0, str(REPO))
 
 from viettts_b200 import synthetic  # noqa: E402

@@ -1,5 +1,5 @@
 """Golden vectors for the NAT / duration / GTA / MelFilter path, produced by EXECUTING THE REFERENCE'S OWN SOURCE
-FILES (`/root/reference/vietTTS/nat/{model,text2mel,gta,dsp}.py`, unmodified) on the synthetic Haiku-layout
+FILES (`vietTTS/nat/{model,text2mel,gta,dsp}.py` of a checkout named by VIETTTS_REFERENCE, unmodified) on the synthetic Haiku-layout
 checkpoints, with `tests/refshim` standing in for the third-party libraries that cannot be installed here
 (jax, dm-haiku, librosa: see tests/refshim/README.md and profiles/r2_ref_deps_probe_*.json).
 
@@ -7,11 +7,12 @@ What this pins: every line of the reference's wiring (it runs as written) and it
 name or shape in the checkpoint layout raises).  What it does not pin: the third-party primitives, which the shim
 restates (cross-checked elsewhere against torch operators).
 
-Run where /root/reference is mounted:   python tests/golden/make_nat_golden.py
+Run with a reference checkout:   VIETTTS_REFERENCE=<path> python tests/golden/make_nat_golden.py
 Writes tests/golden/nat_ref_*.npz (float32 outputs of float64 arithmetic; masks bit-packed).
 """
 from __future__ import annotations
 
+import os
 import pickle
 import sys
 import tempfile
@@ -21,7 +22,7 @@ import numpy as np
 
 HERE = Path(__file__).resolve().parent
 REPO = HERE.parents[1]
-REF = Path("/root/reference")
+REF = Path(os.environ.get("VIETTTS_REFERENCE", "vietTTS-reference"))   # a checkout of NTT123/vietTTS
 sys.path.insert(0, str(REPO / "tests" / "refshim"))   # jax / haiku / librosa stand-ins FIRST
 sys.path.insert(1, str(REF))
 sys.path.insert(2, str(REPO))

@@ -1,5 +1,5 @@
 """Generates tests/golden/text_frontend.json + tests/golden/lexicon_small.txt from the REFERENCE's own text
-front end (runs only where /root/reference exists; the outputs are committed).
+front end (needs a reference checkout named by VIETTTS_REFERENCE; the outputs are committed).
 
 The reference modules cannot be imported (synthesizer.py parses argv at import, nat/config.py and text2mel.py
 import jax/haiku), so the three pure-Python functions are lifted out of their source files with `ast` and
@@ -10,12 +10,13 @@ executed unchanged against a FLAGS namespace built from nat/config.py's own clas
 """
 import ast
 import json
+import os
 import re
 import unicodedata
 from argparse import Namespace
 from pathlib import Path
 
-REF = Path("/root/reference")
+REF = Path(os.environ.get("VIETTTS_REFERENCE", "vietTTS-reference"))   # a checkout of NTT123/vietTTS
 OUT = Path(__file__).resolve().parent
 
 

@@ -1,5 +1,5 @@
-"""The bench.py JSON contract, checked on the committed record of the last B200 run (profiles/r2_bench_1gpu.json, or the
-round-1 record while that does not exist) and on the argument parser.  (The bench itself needs a GPU; the CPU reference
+"""The bench.py JSON contract, checked on the committed record of an H100 run (profiles/h100_bench_1gpu.json) and on
+the argument parser.  (The bench itself needs a GPU; the CPU reference
 arm is exercised by the driver.)"""
 import json
 import subprocess
@@ -10,11 +10,8 @@ REPO = Path(__file__).resolve().parents[1]
 
 
 def _record():
-    for name in ("r2_bench_1gpu.json", "r1_bench_1gpu.json"):
-        p = REPO / "profiles" / name
-        if p.exists():
-            return json.loads(p.read_text()), name
-    raise FileNotFoundError("no bench record under profiles/")
+    name = "h100_bench_1gpu.json"
+    return json.loads((REPO / "profiles" / name).read_text()), name
 
 
 def test_recorded_line_has_every_contract_key():
@@ -36,12 +33,11 @@ def test_recorded_line_has_every_contract_key():
     c = d["cpu_baseline"]
     assert c["kind"] in ("port", "reference") and c["cores"] >= 1 and c["value"] > 0 and c["sample"]
     assert d["gpu_launches"] > 0 and d["gpu_launches"] % d["steps"] == 0     # every step launches the same kernels, all ours
-    if name.startswith("r2"):
-        # round 2: the other BASELINE configs and the per-stage rooflines travel in the same line
-        assert set(d["sweep"]) >= {"1", "8", "32", "128"} and d["strict_fp32"]["value"] > 0
-        assert set(d["configs"]) >= {"c4", "c5"} and d["configs"]["c5"]["padding_frac"] <= 0.08
-        assert {"nat_decoder_scan", "hifigan_stage0", "hifigan_stage3", "hifigan_conv_post", "melspec"} <= set(d["roofline_stages"])
-        assert d["e2e"]["pageable_result"]["value"] > 0
+    # the other BASELINE configs and the per-stage rooflines travel in the same line
+    assert set(d["sweep"]) >= {"1", "8", "32", "128"} and d["strict_fp32"]["value"] > 0
+    assert set(d["configs"]) >= {"c4", "c5"} and d["configs"]["c5"]["padding_frac"] <= 0.08
+    assert {"nat_decoder_scan", "hifigan_stage0", "hifigan_stage3", "hifigan_conv_post", "melspec"} <= set(d["roofline_stages"])
+    assert d["e2e"]["pageable_result"]["value"] > 0
     assert set(d["clocks"]) >= {"sm_mhz", "sm_max_mhz", "reasons"}
     assert not set(d["clocks"]["reasons"]) & {"hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown"}
 

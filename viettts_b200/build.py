@@ -1,4 +1,4 @@
-"""Build recipe for libviettts_b200.so (sm_100a only, built in-tree so that the
+"""Build recipe for libviettts_b200.so (sm_90a only, built in-tree so that the
 .so travels to the GPU box with the repo snapshot)."""
 from __future__ import annotations
 
@@ -10,9 +10,9 @@ from pathlib import Path
 PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 LIB = PKG / "libviettts_b200.so"
-SOURCES = ["api.cu", "conv1d.cu", "tc_conv.cu", "tc_pair.cu", "tc_pair_ts.cu", "tc_pair2.cu", "hifigan.cu", "nat.cu", "melspec.cu"]
+SOURCES = ["api.cu", "conv1d.cu", "tc_conv.cu", "hifigan.cu", "nat.cu", "melspec.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -54,7 +54,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError("nvcc failed (see stderr)")
-    cmd = [nvcc(), "-shared", "-o", str(LIB), *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart", "-ldl"]
+    cmd = [nvcc(), "-shared", "-o", str(LIB), *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-lcudart", "-ldl"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout)

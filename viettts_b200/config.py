@@ -80,5 +80,5 @@ def check_hifigan_config(cfg: dict) -> None:
         if k in cfg and cfg[k] != HIFIGAN[k]:
             raise ValueError(
                 f"hifigan config key {k!r}={cfg[k]!r} differs from the value the "
-                f"sm_100a kernels are specialised on ({HIFIGAN[k]!r})"
+                f"sm_90a kernels are specialised on ({HIFIGAN[k]!r})"
             )

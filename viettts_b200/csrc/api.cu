@@ -252,9 +252,9 @@ int vtts_create(int device, vtts_ctx** out) {
     g_vtts_create_error = std::string("vtts_create: ") + cudaGetErrorString(e);
     return VTTS_ERR_CUDA;
   }
-  if (prop.major != 10) {
+  if (prop.major != 9 || prop.minor != 0) {
     char buf[256];
-    snprintf(buf, sizeof(buf), "vtts_create: device %d is sm_%d%d; this library contains sm_100a code only", device, prop.major, prop.minor);
+    snprintf(buf, sizeof(buf), "vtts_create: device %d is sm_%d%d; this library contains sm_90a code only", device, prop.major, prop.minor);
     g_vtts_create_error = buf;
     return VTTS_ERR_NO_DEVICE;
   }
@@ -264,7 +264,6 @@ int vtts_create(int device, vtts_ctx** out) {
   ctx->cc_major = prop.major;
   ctx->cc_minor = prop.minor;
   ctx->hbm_bytes = prop.totalGlobalMem;
-  if (const char* v = getenv("VTTS_TC_VARIANT")) ctx->tc_variant = atoi(v);   // tuning aid (same values as vtts_debug_tc_stats bits 4..7)
   if ((e = cudaStreamCreateWithFlags(&ctx->own_stream, cudaStreamNonBlocking)) != cudaSuccess) {
     g_vtts_create_error = std::string("vtts_create: ") + cudaGetErrorString(e);
     delete ctx;
@@ -351,8 +350,7 @@ int vtts_debug_tc_stats(vtts_ctx* ctx, int enable, int64_t* host_out_256x16) {
   VTTS_CUDA(cudaMemset(ctx->d_tc_dbg, 0, 256 * 16 * sizeof(long long)));
   ctx->tc_dbg_on = (enable & 1) != 0;
   if (enable & 0x200) ctx->fuse_pairs = (enable >> 10) & 1;        // bit 9 set: bit 10 selects fused ResBlock pairs (tuning aid)
-  if (enable & 0x800) ctx->pair_ts = (enable >> 12) & 3;           // bit 11 set: bits 12..13 select the pair kernel (vtts_ctx::pair_ts)
-  if (enable & 0x100) ctx->tc_variant = (enable >> 4) & 0xF;   // bit 8 set: bits 4..7 select the tile-shape variant (tuning aid)
+  if (enable & 0x800) ctx->pair_ts = (enable >> 12) & 3;           // bit 11 set: bits 12..13 select the pair kernel form (vtts_ctx::pair_ts)
   return VTTS_OK;
 }
 
@@ -397,17 +395,14 @@ int vtts_debug_pair(vtts_ctx* ctx, const float* x_dev, const float* w1_dev, cons
   VTTS_CUDA(cudaSetDevice(ctx->device));
   void* wpk = nullptr;
   const size_t bytes = vtts_tc_packed_elems(k, C, C) * 2;
-  const size_t cb = (vtts_tc_packed_pc_bytes(k, C) + 255) & ~size_t(255);
-  VTTS_CUDA(cudaMalloc(&wpk, 2 * bytes + 2 * cb));
+  VTTS_CUDA(cudaMalloc(&wpk, 2 * bytes));
   int rc = vtts_tc_pack_weights(ctx, w1_dev, wpk, k, C, C, 0, C);
   if (!rc) rc = vtts_tc_pack_weights(ctx, w2_dev, (char*)wpk + bytes, k, C, C, 0, C);
-  if (!rc) rc = vtts_tc_pack_weights_pc(ctx, w1_dev, (char*)wpk + 2 * bytes, k, C);
-  if (!rc) rc = vtts_tc_pack_weights_pc(ctx, w2_dev, (char*)wpk + 2 * bytes + cb, k, C);
   if (rc) { cudaFree(wpk); return rc; }
   TcPairLaunch PL;
   memset(&PL, 0, sizeof(PL));
   PL.nprob = 1; PL.N = C; PL.B = B; PL.T_rows = T; PL.len = len_dev; PL.len_mul = 1; PL.slope = slope;
-  PL.p[0] = TcPairProb{x_dev, wpk, (char*)wpk + bytes, b1_dev, b2_dev, out_dev, k, dil, (char*)wpk + 2 * bytes, (char*)wpk + 2 * bytes + cb};
+  PL.p[0] = TcPairProb{x_dev, wpk, (char*)wpk + bytes, b1_dev, b2_dev, out_dev, k, dil};
   rc = vtts_launch_tc_pair(ctx, PL, nullptr);
   cudaError_t e = cudaDeviceSynchronize();
   cudaFree(wpk);
@@ -819,7 +814,7 @@ int vtts_gta_host(vtts_ctx* ctx, const int16_t* wav_i16, const int32_t* wav_leng
   if (keep_b) memcpy(hp + o_keep, keep_mask, keep_b);
   if (zone_b) memcpy(hp + o_zone, zone_mask, zone_b);
   VTTS_CUDA(cudaMemcpyAsync(dp, hp, in_end, cudaMemcpyHostToDevice, st));
-  pcm16_to_float_kernel<<<148 * 4, 256, 0, st>>>((const int16_t*)(dp + o_wav), (float*)(dp + o_wavf), (size_t)B * S);
+  pcm16_to_float_kernel<<<ctx->sm_count * 4, 256, 0, st>>>((const int16_t*)(dp + o_wav), (float*)(dp + o_wavf), (size_t)B * S);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   rc = vtts_melspec(ctx, (const float*)(dp + o_wavf), B, S, (float*)(dp + o_gt), st);

@@ -152,30 +152,8 @@ int vtts_hifigan_prepare(vtts_ctx* ctx) {
       poff[t] = elems;
       elems += vtts_tc_packed_elems(7, vc::MEL, 256);
     }
-    // CTA-pair layout of the convs the fused pair kernel runs (C <= 64), appended to the same allocation
-    std::vector<size_t> coff(72, 0);
-    size_t cbytes = 0;
-    for (int n = 6; n < 12; ++n) {
-      const int ch = 256 >> (n / 3), kk = vc::hg_rbk(n % 3);
-      for (int q = 0; q < 6; ++q) {
-        coff[n * 6 + q] = cbytes;
-        cbytes += (vtts_tc_packed_pc_bytes(kk, ch) + 255) & ~size_t(255);
-      }
-    }
-    const size_t base_bytes = (elems * 2 + 255) & ~size_t(255);
     if (ctx->hg_wpk) cudaFree(ctx->hg_wpk);
-    VTTS_CUDA(cudaMalloc(&ctx->hg_wpk, base_bytes + cbytes));
-    ctx->hg_wpc_t.assign(72, nullptr);
-    for (int n = 6; n < 12; ++n) {
-      const int ch = 256 >> (n / 3), kk = vc::hg_rbk(n % 3);
-      for (int which = 0; which < 2; ++which)
-        for (int m = 0; m < 3; ++m) {
-          const int q = which * 3 + m;
-          ctx->hg_wpc_t[n * 6 + q] = (char*)ctx->hg_wpk + base_bytes + coff[n * 6 + q];
-          int rc = vtts_tc_pack_weights_pc(ctx, ctx->hg_t[hgi::RB_W(n, which, m)], ctx->hg_wpc_t[n * 6 + q], kk, ch);
-          if (rc) return rc;
-        }
-    }
+    VTTS_CUDA(cudaMalloc(&ctx->hg_wpk, elems * 2));
     ctx->hg_wpk_t.resize(72);
     ctx->hg_wpk_ups.assign(32, nullptr);
     for (int n = 0; n < 12; ++n) {
@@ -312,14 +290,14 @@ int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, i
       const float* src[3];
       for (int j = 0; j < 3; ++j) src[j] = (m == 0) ? hb.X : (m == 1 ? hb.A[par][j] : hb.Bb[j]);
       if (tc && ctx->fuse_pairs && Co <= 64) {
-        // ---- fused pair: conv(d) -> lrelu -> conv(1) -> + x, intermediate kept on chip (tc_pair.cu) ----
+        // ---- fused pair: conv(d) -> lrelu -> conv(1) -> + x, intermediate kept on chip (tc_conv.cu) ----
         TcPairLaunch PL;
         memset(&PL, 0, sizeof(PL));
         PL.nprob = 3; PL.N = Co; PL.B = B; PL.T_rows = rows; PL.len = n_frames; PL.len_mul = scale; PL.slope = 0.1f;
         for (int j = 0; j < 3; ++j) {
           const int kk = vc::hg_rbk(j), n = i * 3 + j;
           PL.p[j] = TcPairProb{src[j], ctx->hg_wpk_t[n * 6 + m], ctx->hg_wpk_t[n * 6 + 3 + m], W[hgi::RB_B(n, 0, m)], W[hgi::RB_B(n, 1, m)],
-                               (m == 1) ? hb.Bb[j] : hb.A[par][j], kk, d, ctx->hg_wpc_t[n * 6 + m], ctx->hg_wpc_t[n * 6 + 3 + m]};
+                               (m == 1) ? hb.Bb[j] : hb.A[par][j], kk, d};
         }
         rc = vtts_launch_tc_pair(ctx, PL, st);
         if (rc) return rc;

@@ -198,14 +198,14 @@ struct EncScanArgs {
 };
 
 // ---- autoregressive decoder scan (model.py:129-142) ------------------------------------------------
-// One cooperative grid of 144 CTAs, up to 32 batch rows per launch.
+// One cooperative grid of 132 CTAs, up to 32 batch rows per launch.
 //   CTAs 0..127   LSTM role: CTA c owns 4 hidden units (16 gate columns) of both layers; its slices of the
 //                 recurrent matrices (768x16 + 1280x16 fp32) live in REGISTERS.  A persistent shared-memory
 //                 buffer holds [p2 | h0 | h1] of all rows; the parts that are already final (h0_{t-1},
 //                 h1_{t-1}) are prefetched while the prenet CTAs work, so only p2 (phase C) and h0_t (phase D)
 //                 are fetched on the critical path.
-//   CTAs 128..143 prenet role: 16 columns each of p1 = drop(relu([h0,h1]_{t-1}.(Wo.W1) + bo.W1))  (phase EA)
-//                 and of p2 = drop(relu(p1.W2))                                                   (phase B)
+//   CTAs 128..131 prenet role: 64 columns each (four blocks of 16) of p1 = drop(relu([h0,h1]_{t-1}.(Wo.W1) + bo.W1))
+//                 (phase EA) and of p2 = drop(relu(p1.W2)) (phase B); their weights are read through L1/L2
 // The output projection mel_t = [h0,h1]_t.Wo + bo is NOT part of the scan: nothing in the recurrence reads mel_t
 // (the prenet consumes the precomposed Wo.W1), so every frame's [h0 | h1] is written to `hout` and one GEMM
 // projects the whole sequence afterwards.  (A projection role inside the scan -- 4 CTAs taking part in every grid
@@ -239,8 +239,10 @@ struct DecScanArgs {
 constexpr int DEC_XR = 32;                 // batch rows per staging group (smem holds the state of one group)
 constexpr int DEC_NG = 4;                  // row groups per launch: up to 128 rows share the three grid barriers of a frame
 constexpr int DEC_KPAD = vc::PRENET + 2 * vc::DEC_H + 4;   // 1284: [p2 | h0 | h1] + pad
-constexpr int DEC_LSTM = 128, DEC_PRE = 16;
-constexpr int DEC_CTAS = DEC_LSTM + DEC_PRE;   // 144
+// 128 LSTM CTAs + 4 prenet CTAs = the 132 SMs of an H100 SXM (a cooperative grid must be co-resident, one CTA per SM)
+constexpr int DEC_LSTM = 128, DEC_PRE = 4;
+constexpr int DEC_CTAS = DEC_LSTM + DEC_PRE;   // 132
+constexpr int DEC_QPC = 16 / DEC_PRE;          // 16-column blocks of the prenet per prenet CTA
 
 // copy rows [0,nr) x [n floats] of a global matrix (row stride `stride`) into smem (row pitch `pitch`, column
 // offset koff); p == nullptr writes zeros.  8 x 16 B loads in flight per thread.
@@ -474,9 +476,9 @@ __device__ __forceinline__ void dec_matmul2(const float* __restrict__ xa, const 
 }
 
 // ---- prenet / projection CTAs: out[32 rows][8 cols] = xs[32][K] . wsm[K][8] ------------------------------
-// thread (rg = tid&3, ks = tid>>2): rows rg+4i (i<8), K slice ks of SL = K/64; weights in smem with one pad
-// row per slice (physical row = k + k/SL).  Result: outv[row*8 + col] for 32 x 8 outputs.
-template <int SL>
+// thread (rg = tid&3, ks = tid>>2): rows rg+4i (i<8), K slice ks of SL = K/64; weight row k at wsm + k * WLD (the 8
+// columns are contiguous).  Result: outv[row*8 + col] for 32 x 8 outputs.
+template <int SL, int WLD>
 __device__ __forceinline__ void pre_gemm8(const float* __restrict__ xs, int pitch, const float* __restrict__ wsm, float* part, float* outv) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int rg = tid & 3, ks = tid >> 2;
@@ -486,7 +488,7 @@ __device__ __forceinline__ void pre_gemm8(const float* __restrict__ xs, int pitc
 #pragma unroll
     for (int c = 0; c < 8; ++c) acc[i][c] = 0.f;
   const float* xk = xs + (size_t)rg * pitch + ks * SL;
-  const float* wk = wsm + (size_t)(ks * SL + ks) * 8;
+  const float* wk = wsm + (size_t)(ks * SL) * WLD;
 #pragma unroll
   for (int kk = 0; kk < SL; kk += 4) {
     float4 xv[8];
@@ -494,8 +496,8 @@ __device__ __forceinline__ void pre_gemm8(const float* __restrict__ xs, int pitc
     for (int i = 0; i < 8; ++i) xv[i] = *reinterpret_cast<const float4*>(xk + (size_t)(4 * i) * pitch + kk);
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
-      const float4 wa = *reinterpret_cast<const float4*>(wk + (size_t)(kk + e) * 8);
-      const float4 wb = *reinterpret_cast<const float4*>(wk + (size_t)(kk + e) * 8 + 4);
+      const float4 wa = __ldg(reinterpret_cast<const float4*>(wk + (size_t)(kk + e) * WLD));
+      const float4 wb = __ldg(reinterpret_cast<const float4*>(wk + (size_t)(kk + e) * WLD + 4));
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const float x = e == 0 ? xv[i].x : (e == 1 ? xv[i].y : (e == 2 ? xv[i].z : xv[i].w));
@@ -548,17 +550,8 @@ __device__ __forceinline__ void pre_gemm8(const float* __restrict__ xs, int pitc
   __syncthreads();
 }
 
-// copy a [K][ncols_src] slice (cols c0..c0+8) of a global per-CTA weight block into smem [K + K/SL][8]
-__device__ __forceinline__ void pre_load_w8(float* wsm, const float* g, int K, int SL, int ld, int c0) {
-  for (int e = threadIdx.x; e < K * 2; e += SCAN_THREADS) {
-    const int k = e >> 1, h = (e & 1) * 4;
-    const float4 v = __ldg(reinterpret_cast<const float4*>(g + (size_t)k * ld + c0 + h));
-    *reinterpret_cast<float4*>(wsm + (size_t)(k + k / SL) * 8 + h) = v;
-  }
-}
-
 // Barrier among the DEC_PRE prenet CTAs only (all co-resident: cooperative launch).  The second prenet layer needs every
-// column block of p1 from its 15 peers but nothing from the 128 LSTM CTAs, so a grid-wide barrier here would put the
+// column block of p1 from its peers but nothing from the 128 LSTM CTAs, so a grid-wide barrier here would put the
 // LSTM CTAs' pre-accumulation (6.2 us at 32 rows) on the critical path and cost a full grid.sync.  `target` is the
 // monotonically growing arrival count; a 2 s time-out traps instead of hanging the GPU.
 __device__ __forceinline__ void prenet_barrier(unsigned int* counter, unsigned int target, int* err) {
@@ -689,25 +682,16 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const Dec
     }
   } else if (c < DEC_LSTM + DEC_PRE) {
     // =============================== prenet role ===============================
-    const int q = c - DEC_LSTM;                        // columns 16q .. 16q+15 of p1 and p2
+    const int q0 = (c - DEC_LSTM) * DEC_QPC;           // column blocks q0 .. q0 + DEC_QPC - 1 (16 columns each) of p1 and p2
     constexpr int XP = H + 4;                          // 516: row pitch of the 512-wide staging buffer
-    constexpr int WCB = (2 * H + 2 * H / 8) * 8;       // (Wo.W1) half-block: 1024 rows + one pad row per 8, x 8 columns
-    constexpr int W2B = (vc::PRENET + NSLICE) * 8;
     float* xs = sm;                                    // [32][XP]: h1_{t-1} (EA), p1 (B), h0_t (D window)
-    float* wcs = xs + 32 * XP;                         // [2][WCB]
-    float* w2s = wcs + 2 * WCB;                        // [2][W2B]
-    float* part = w2s + 2 * W2B;                       // [8][32][8]
+    float* part = xs + 32 * XP;                        // [8][32][8]
     float* outv = part + 8 * 256;                      // [256]
-    float* pp1 = outv + 256;                           // [DEC_NG][2][256] h0 half of p1's pre-activation, computed one phase early
-    for (int hf = 0; hf < 2; ++hf) {
-      pre_load_w8(wcs + (size_t)hf * WCB, a.wc + (size_t)q * 2 * H * 16, 2 * H, 8, 16, hf * 8);
-      pre_load_w8(w2s + (size_t)hf * W2B, a.wp2 + (size_t)q * vc::PRENET * 16, vc::PRENET, 4, 16, hf * 8);
-    }
+    float* pp1 = outv + 256;                           // [DEC_NG][DEC_QPC][2][256] h0 half of p1's pre-activation, one phase early
     for (int e = tid; e < 32 * XP; e += SCAN_THREADS) xs[e] = 0.f;
-    for (int e = tid; e < DEC_NG * 512; e += SCAN_THREADS) pp1[e] = 0.f;
+    for (int e = tid; e < DEC_NG * DEC_QPC * 512; e += SCAN_THREADS) pp1[e] = 0.f;
     __syncthreads();
     const int orow = tid >> 3, ocol = tid & 7;         // output handled by this thread after a pre_gemm8 pass
-    constexpr int H1OFF = (H + H / 8) * 8;             // first padded row of the h1 half inside a WCB block
     const int NG = (B + DEC_XR - 1) / DEC_XR;
     for (int t = 0; t < N; ++t) {
       // ---- phase EA: p1(t) = drop(relu(pp1 + h1_{t-1} . Wc[512:1024] + bc)) ----
@@ -718,17 +702,19 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const Dec
           dec_fetch(xs, XP, 0, a.h1 + ((size_t)((t - 1) & 1) * B + r0) * H, H, H, nb);
           __syncthreads();
 #pragma unroll 1
-          for (int hf = 0; hf < 2; ++hf) {
-            pre_gemm8<8>(xs, XP, wcs + (size_t)hf * WCB + H1OFF, part, outv);
+          for (int qh = 0; qh < 2 * DEC_QPC; ++qh) {
+            const int q = q0 + (qh >> 1), hf = qh & 1;
+            pre_gemm8<8, 16>(xs, XP, a.wc + ((size_t)q * 2 * H + H) * 16 + hf * 8, part, outv);
             if (orow < nb) {
               const int u = q * 16 + hf * 8 + ocol;
-              const float v = fmaxf(outv[tid] + pp1[rg * 512 + hf * 256 + tid] + __ldg(a.bc + u), 0.f);
+              const float v = fmaxf(outv[tid] + pp1[(rg * DEC_QPC * 2 + qh) * 256 + tid] + __ldg(a.bc + u), 0.f);
               a.p1[(size_t)(r0 + orow) * vc::PRENET + u] = v * keep_scale(a.mode, a.keep, a.seed, a.row_base + r0 + orow, t, N, 0, u);
             }
           }
         }
       } else {
-        for (int e = tid; e < B * 16; e += SCAN_THREADS) a.p1[(size_t)(e >> 4) * vc::PRENET + q * 16 + (e & 15)] = 0.f;  // prenet(0) = 0
+        for (int e = tid; e < B * 16 * DEC_QPC; e += SCAN_THREADS)
+          a.p1[(size_t)(e / (16 * DEC_QPC)) * vc::PRENET + q0 * 16 + e % (16 * DEC_QPC)] = 0.f;  // prenet(0) = 0
       }
       DEC_MARK(0)
       prenet_barrier(a.pre_bar, (unsigned)DEC_PRE * (unsigned)(t + 1), a.err);   // every column block of p1(t) is in L2
@@ -740,8 +726,9 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const Dec
         dec_fetch(xs, XP, 0, a.p1 + (size_t)r0 * vc::PRENET, vc::PRENET, vc::PRENET, nb);
         __syncthreads();
 #pragma unroll 1
-        for (int hf = 0; hf < 2; ++hf) {
-          pre_gemm8<4>(xs, XP, w2s + (size_t)hf * W2B, part, outv);
+        for (int qh = 0; qh < 2 * DEC_QPC; ++qh) {
+          const int q = q0 + (qh >> 1), hf = qh & 1;
+          pre_gemm8<4, 16>(xs, XP, a.wp2 + (size_t)q * vc::PRENET * 16 + hf * 8, part, outv);
           if (orow < nb) {
             const int u = q * 16 + hf * 8 + ocol;
             const float v = fmaxf(outv[tid], 0.f);
@@ -761,9 +748,10 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const Dec
         dec_fetch(xs, XP, 0, a.h0 + ((size_t)(t & 1) * B + r0) * H, H, H, nb);
         __syncthreads();
 #pragma unroll 1
-        for (int hf = 0; hf < 2; ++hf) {
-          pre_gemm8<8>(xs, XP, wcs + (size_t)hf * WCB, part, outv);
-          pp1[rg * 512 + hf * 256 + tid] = outv[tid];
+        for (int qh = 0; qh < 2 * DEC_QPC; ++qh) {
+          const int q = q0 + (qh >> 1), hf = qh & 1;
+          pre_gemm8<8, 16>(xs, XP, a.wc + (size_t)q * 2 * H * 16 + hf * 8, part, outv);
+          pp1[(rg * DEC_QPC * 2 + qh) * 256 + tid] = outv[tid];
         }
       }
       __syncthreads();
@@ -930,7 +918,7 @@ constexpr size_t enc_scan_smem() {
 }
 constexpr size_t dec_scan_smem() {
   constexpr size_t lstm = (size_t)DEC_XR * DEC_KPAD + 8 * DEC_XR * NCOL + DEC_XR * NCOL + DEC_NG * (2 * DEC_XR * NCOL + 2 * DEC_XR * UPC);
-  constexpr size_t pre = (size_t)32 * (vc::DEC_H + 4) + 2 * (2 * vc::DEC_H + 2 * vc::DEC_H / 8) * 8 + 2 * (vc::PRENET + NSLICE) * 8 + 8 * 256 + 256 + DEC_NG * 512;
+  constexpr size_t pre = (size_t)32 * (vc::DEC_H + 4) + 8 * 256 + 256 + DEC_NG * DEC_QPC * 512;
   return (lstm > pre ? lstm : pre) * 4;
 }
 
@@ -1297,7 +1285,7 @@ int vtts_acoustic_teacher_run(vtts_ctx* ctx, const int32_t* tokens, const int32_
     return vtts_conv_dispatch(ctx, Lc, &ctx->ac_wpk_t[wp], st);     // tensor-core path in BF16X3 mode, FMA path in FP32 mode
   };
   const size_t act_blocks = (BN * 256 + 255) / 256;
-  const unsigned act_grid = (unsigned)(act_blocks < 148 * 16 ? act_blocks : 148 * 16);
+  const unsigned act_grid = (unsigned)(act_blocks < ctx->sm_count * 16 ? act_blocks : ctx->sm_count * 16);
   int rc = gemm(mels_in, T[aci::PRE1_W], D[D_ZERO], pa, 80, 256, WP_PRE1);
   if (rc) return rc;
   prenet_act_kernel<<<act_grid, 256, 0, st>>>(pa, keep, seed, mode, 0, B, N, pb, 256);

@@ -111,8 +111,6 @@ struct TcLaunch {
                               // the others: generator 19.8 -> 19.1 ms.  1: problems back to back (experiments only)
   int* err;                   // device int: set before trapping on a barrier timeout
   long long* dbg;             // optional [grid][16] per-role stall counters (vtts_debug_tc_stats)
-  int exp;                    // experiment bits of the CTA-pair form (VTTS_PAIR_EXP; 0 in production): 1 = the issuer polls with
-                              // test_wait instead of try_wait, 4 = cluster-scope release on the weight forwarder's arrive (slow)
 };
 
 // ---- fused ResBlock pair (tc_pair.cu): out = conv2(lrelu(conv1(lrelu(x)) + b1)) + b2 + x, C = N channels ----
@@ -124,8 +122,6 @@ struct TcPairProb {
   const float* b2;
   float* out;            // [B][T_rows][N], must differ from x
   int k, dil;
-  const void* w1pc;      // the same weights in the CTA-pair layout (vtts_tc_pack_weights_pc) or null
-  const void* w2pc;
 };
 
 struct TcPairLaunch {
@@ -143,17 +139,15 @@ struct TcPairLaunch {
 
 struct vtts_ctx {
   int device = 0;
-  int precision = 1;            // 0 = strict fp32 (FMA pipe), 1 = bf16x3 on tcgen05 tensor cores (default)
+  int precision = 1;            // 0 = strict fp32 (FMA pipe), 1 = bf16x3 on the tensor cores (wgmma, default)
   int* d_err = nullptr;
   long long* d_tc_dbg = nullptr;   // [256][16] profiling counters of the last tensor-core conv launch
   bool tc_dbg_on = false;
   int fuse_pairs = 1;              // 1 = ResBlock pairs with C <= 64 run in a fused pair kernel (intermediate stays on chip: 8 instead of 20 B of HBM traffic per element pair)
-  int pair_ts = 2;                 // fused pair kernel: 0 tc_pair.cu (one issuer, smem operand), 1 tc_pair_ts.cu (operand in TMEM), 2 tc_pair2.cu (two decoupled pipelines, smem operand),
-                                   // 3 tc_pair2.cu in the CTA-pair form (cta_group::2 over clusters of two SMs)
-  int tc_variant = 3;              // tile-shape variant of the tensor-core conv (see TcCfg): 3 = CTA pairs (cta_group::2) for N >= 128 (default), 1 = single-CTA form, 0 / 2 = older experiments
+  int pair_ts = 2;                 // form of the fused pair kernel (tc_conv.cu): 2 = 256-row tiles (default), 1 = the same with
+                                   // conv2's A operand in registers (register-A wgmma), 0 = 128-row tiles
   void* hg_wpk = nullptr;       // packed tensor-core weights of the 72 resblock convs
   std::vector<void*> hg_wpk_t;
-  std::vector<void*> hg_wpc_t;     // CTA-pair layout of the C <= 64 resblock convs (null for the others)
   std::vector<void*> hg_wpk_ups;   // [stage][phase] packed transposed-conv phase weights
   void* hg_wpk_pre[2] = {nullptr, nullptr};  // conv_pre, two N=256 output tiles
   int sm_count = 0;
@@ -257,16 +251,8 @@ int vtts_launch_conv(vtts_ctx* ctx, const ConvLaunch& L, cudaStream_t st);
 size_t vtts_tc_packed_elems(int k, int Cin, int N);
 int vtts_tc_pack_weights(vtts_ctx* ctx, const float* w, void* dst, int k, int Cin, int Cout_total, int n0, int N);
 int vtts_launch_tc_conv(vtts_ctx* ctx, TcLaunch& L, cudaStream_t st);
-// tc_pair.cu
-int vtts_launch_tc_pair(vtts_ctx* ctx, TcPairLaunch& L, cudaStream_t st);   // dispatches on ctx->pair_ts
-// tc_pair_ts.cu: same operator with the A operand in tensor memory (TS form of tcgen05.mma)
-int vtts_launch_tc_pair_ts(vtts_ctx* ctx, TcPairLaunch& L, cudaStream_t st);
-// tc_pair2.cu: shared-memory operand, conv1 / conv2 as two decoupled pipelines with one issuing warp each
-int vtts_launch_tc_pair2(vtts_ctx* ctx, TcPairLaunch& L, cudaStream_t st);
-int vtts_launch_tc_pair2c(vtts_ctx* ctx, TcPairLaunch& L, cudaStream_t st);   // the same kernel in the CTA-pair form
-// CTA-pair weight layout of a C x C conv for tc_pair2.cu: [chunk][rank][tap][k-half][1.5 C rows][8 bf16]
-size_t vtts_tc_packed_pc_bytes(int k, int C);
-int vtts_tc_pack_weights_pc(vtts_ctx* ctx, const float* w, void* dst, int k, int C);
+// fused ResBlock pair (C = 32 or 64): conv1 -> lrelu -> conv2 -> + x with the intermediate kept in shared memory
+int vtts_launch_tc_pair(vtts_ctx* ctx, TcPairLaunch& L, cudaStream_t st);
 // generic dispatch: runs `L` on the tensor-core path when ctx->precision == 1 and packed weights are given
 // (wpk[prob * ntile + tile], ntile = ceil(Cout/256) tiles of width vtts_tc_tile_n(Cout)), else on the FP32 path
 int vtts_tc_tile_n(int Cout);

@@ -39,7 +39,7 @@ def _np(a, dtype, shape=None, what="array"):
 
 
 class Engine:
-    """A context on one B200.  Not thread-safe (like the C context)."""
+    """A context on one H100.  Not thread-safe (like the C context)."""
 
     def __init__(self, device: int = 0):
         self.lib = _lib.load()
@@ -84,7 +84,7 @@ class Engine:
         return float(ms.value)
 
     def set_precision(self, mode) -> None:
-        """'fp32' (strict, FMA pipe) or 'bf16x3' (tcgen05 tensor cores, split-bf16, fp32 accumulate)."""
+        """'fp32' (strict, FMA pipe) or 'bf16x3' (wgmma tensor cores, split-bf16, fp32 accumulate)."""
         m = {"fp32": PRECISION_FP32, "bf16x3": PRECISION_BF16X3}.get(mode, mode)
         self._ck(self.lib.vtts_set_precision(self.h, int(m)))
 
@@ -108,25 +108,21 @@ class Engine:
                                           B, T, Cc, int(k), int(dil), float(slope), _ptr(out)))
         return out
 
-    PAIR_KERNELS = {"smem": 0, "tmem": 1, "smem2": 2, "smem2c": 3}
+    PAIR_KERNELS = {"smem": 0, "tmem": 1, "smem2": 2}
 
-    def set_fused_pairs(self, on: bool, ts=None, kind: str | None = None):
-        """Run the C <= 64 ResBlock pairs in a fused pair kernel (off: two tensor-core conv launches per pair).
-        kind: "smem2" tc_pair2.cu (two decoupled pipelines, A operand in shared memory; the default), "smem2c" the same kernel
-        in the CTA-pair form (cta_group::2 over clusters of two SMs, half of the weight operand per SM), "tmem"
-        tc_pair_ts.cu (A operand in tensor memory), "smem" tc_pair.cu (first generation).  `ts` is the old spelling
-        (True = "tmem", False = "smem")."""
-        if kind is None:
-            kind = "smem2" if ts is None else ("tmem" if ts else "smem")
-        self._ck(self.lib.vtts_debug_tc_stats(self.h, 0x200 | ((1 if on else 0) << 10) | 0x800 | (self.PAIR_KERNELS[kind] << 12), None))
+    def set_fused_pairs(self, on: bool, kind: str | None = None):
+        """Run the C <= 64 ResBlock pairs in the fused pair kernel (off: two tensor-core conv launches per pair).
+        kind selects its form: "smem2" 256-row tiles (the default), "tmem" the same with conv2's A operand in registers
+        (register-A wgmma), "smem" 128-row tiles."""
+        flags = 0x200 | ((1 if on else 0) << 10)
+        if kind is not None:
+            flags |= 0x800 | (self.PAIR_KERNELS[kind] << 12)
+        self._ck(self.lib.vtts_debug_tc_stats(self.h, flags, None))
 
-    def tc_stats(self, enable=True, variant=None):
-        """Per-CTA stall counters of the last tensor-core conv launch (see vtts_debug_tc_stats);
-        `variant` optionally selects the conv form for later launches: 3 = CTA pairs (cta_group::2) for C >= 128 (default),
-        1 = single-CTA form, 0 / 2 = older tile-shape experiments."""
+    def tc_stats(self, enable=True):
+        """Per-CTA stall counters of the last tensor-core conv launch (see vtts_debug_tc_stats)."""
         out = np.zeros((256, 16), np.int64)
-        flags = (1 if enable else 0) | (0 if variant is None else (0x100 | (int(variant) << 4)))
-        self._ck(self.lib.vtts_debug_tc_stats(self.h, flags, _ptr(out)))
+        self._ck(self.lib.vtts_debug_tc_stats(self.h, 1 if enable else 0, _ptr(out)))
         return out
 
     SUBSTAGES = {1: "acoustic.encoder", 2: "acoustic.upsample", 3: "acoustic.cond_gemm", 4: "acoustic.decoder_scan",

@@ -4,7 +4,7 @@ Same name, argument and return conventions as the reference: `mel2wave(mel)`
 takes an array-like f32 [B,T,80] (B=1 from the CLI), reads the generator config
 and the Haiku-layout checkpoint from the same cwd-relative paths, and returns a
 numpy float32 waveform, squeezed ([256*T] for B=1), in (-1,1).  Differences: the
-forward runs on the sm_100a kernels, and the parsed checkpoint is cached per
+forward runs on the sm_90a kernels, and the parsed checkpoint is cached per
 (path, mtime, size) instead of being re-read on every call."""
 from __future__ import annotations
 

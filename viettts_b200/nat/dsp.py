@@ -3,7 +3,7 @@
 MelFilter(sample_rate, n_fft, n_mels, fmin, fmax)(y): y f32 [B,S] in [-1,1) ->
 log-mel f32 [B,S/256,80].  The filterbank is the librosa-compatible Slaney bank
 (viettts_b200.weights.mel_filterbank); the STFT + filterbank + log run in the
-sm_100a melspec kernel."""
+sm_90a melspec kernel."""
 from __future__ import annotations
 
 import numpy as np

@@ -45,9 +45,9 @@ def bucket_by_length(n_frames, max_pad_frac: float = 0.08, max_rows: int = 128):
     return buckets
 
 
-# measured cost model of one ragged batch on a B200 (bench.py `roofline_stages`): the decoder scan is paid per frame of
+# cost model of one ragged batch, used only to balance buckets (relative weights): the decoder scan is paid per frame of
 # the batch's longest row (sequential, ~20 us per frame for up to 32 rows), everything else per padded row-frame
-SCAN_US_PER_FRAME = 17.0          # + SCAN_US_PER_FRAME_ROW per row of the launch: 17.6 us at 1 row, 18.5 at 8, 21.7 at 32
+SCAN_US_PER_FRAME = 17.0          # + SCAN_US_PER_FRAME_ROW per row of the launch
 SCAN_US_PER_FRAME_ROW = 0.15
 ROW_US_PER_FRAME = 1.9
 

@@ -2,7 +2,7 @@
 
 Same flags as the reference (--text --output --sample-rate --silence-duration --lexicon-file) and the same
 pipeline (synthesizer.py:34-39): normalise -> text2mel -> mel2wave -> 16-bit PCM WAV.  Two additions that the
-B200 path makes worthwhile: `--text-file` synthesises one utterance per input line as ragged batches through a
+GPU path makes worthwhile: `--text-file` synthesises one utterance per input line as ragged batches through a
 single library call per batch (`Engine.tts`), and the WAV writer is built in (the reference needs `soundfile`).
 """
 from __future__ import annotations
@@ -93,7 +93,7 @@ def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_
 
 
 def main(argv=None) -> int:
-    parser = ArgumentParser(description="B200-native vietTTS synthesizer")
+    parser = ArgumentParser(description="H100-native vietTTS synthesizer")
     parser.add_argument("--text", type=str)
     parser.add_argument("--text-file", type=Path, default=None, help="one utterance per line; outputs <output stem>_NNNN.wav")
     parser.add_argument("--output", default="clip.wav", type=Path)

@@ -119,6 +119,34 @@ def test_bad_arguments_raise(eng):
         e2.close()
 
 
+def test_reload_other_checkpoints_then_originals(eng, duration_ckpt, acoustic_ckpt, hifigan_params):
+    """Loading replaces a model's device weights in place: after a second checkpoint and the original again, the
+    acoustic and duration outputs equal those of a fresh engine."""
+    from viettts_b200.engine import Engine
+    tk = np.stack([_tokens(60, 24), _tokens(61, 24)])
+    lens = np.array([24, 17], np.int32)
+    frames, _ = no.seconds_to_frames(eng.predict_duration(tk, lengths=lens))
+    nfs = frames.sum(axis=1, dtype=np.float32).astype(np.int32)
+    fresh = Engine(0)
+    try:
+        fresh.load_duration(duration_ckpt)
+        fresh.load_acoustic(acoustic_ckpt)
+        fresh.set_precision(eng.lib.vtts_get_precision(eng.h))
+        want_dur = fresh.predict_duration(tk, lengths=lens)
+        want_mel = fresh.predict_mel(tk, frames, lengths=lens, n_frames=nfs)
+    finally:
+        fresh.close()
+    try:
+        eng.load_duration(synthetic.duration_ckpt(99))
+        eng.load_acoustic(synthetic.acoustic_ckpt(99))
+        assert not np.array_equal(eng.predict_duration(tk, lengths=lens), want_dur)
+    finally:
+        eng.load_duration(duration_ckpt)
+        eng.load_acoustic(acoustic_ckpt)
+    assert np.array_equal(eng.predict_duration(tk, lengths=lens), want_dur)
+    assert np.array_equal(eng.predict_mel(tk, frames, lengths=lens, n_frames=nfs), want_mel)
+
+
 def _staged_pipeline(eng, tok_row, silence_duration):
     """text2mel.py:85-103 + mel2wave through the separate entry points (dropout off)."""
     tokens = [int(t) for t in tok_row]

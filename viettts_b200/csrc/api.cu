@@ -155,15 +155,20 @@ static int64_t total_floats(const std::vector<TensorSpec>& s) {
   return t;
 }
 
-// copy a contiguous blob (host or device) into per-tensor 256B-aligned device slots
-// device arena of one model: every tensor of `specs` 256 B aligned; returns the arena size in floats
-static size_t arena_floats(const std::vector<TensorSpec>& specs) {
+static std::vector<size_t> spec_floats(const std::vector<TensorSpec>& specs) {
+  std::vector<size_t> n;
+  for (auto& e : specs) n.push_back((size_t)e.n);
+  return n;
+}
+// floats of one arena of vtts_alloc_tensors
+static size_t arena_floats(const std::vector<size_t>& n) {
   size_t total = 0;
-  for (size_t i = 0; i < specs.size(); ++i) total += ((size_t)specs[i].n + 63) & ~size_t(63);
+  for (size_t x : n) total += (x + 63) & ~size_t(63);
   return total;
 }
-static int alloc_arena(vtts_ctx* ctx, const std::vector<TensorSpec>& specs, float** store, std::vector<float*>& ptrs) {
-  const size_t total = arena_floats(specs);
+
+int vtts_alloc_tensors(vtts_ctx* ctx, const std::vector<size_t>& n, float** store, std::vector<float*>& ptrs) {
+  const size_t total = arena_floats(n);
   if (*store) {
     VTTS_CUDA(cudaDeviceSynchronize());
     cudaFree(*store);
@@ -171,28 +176,76 @@ static int alloc_arena(vtts_ctx* ctx, const std::vector<TensorSpec>& specs, floa
   }
   VTTS_CUDA(cudaMalloc(store, total * sizeof(float)));
   VTTS_CUDA(cudaMemset(*store, 0, total * sizeof(float)));
-  ptrs.resize(specs.size());
+  ptrs.resize(n.size());
   size_t off = 0;
-  for (size_t i = 0; i < specs.size(); ++i) {
+  for (size_t i = 0; i < n.size(); ++i) {
     ptrs[i] = *store + off;
-    off += ((size_t)specs[i].n + 63) & ~size_t(63);
+    off += (n[i] + 63) & ~size_t(63);
   }
   return VTTS_OK;
 }
-static int load_blob(vtts_ctx* ctx, const std::vector<TensorSpec>& specs, const float* blob, int64_t n_floats, float** store,
-                     std::vector<float*>& ptrs) {
+
+int vtts_pack_convs(vtts_ctx* ctx, ModelWeights& m, const std::vector<PackSpec>& convs) {
+  size_t bytes = 0;
+  for (auto& c : convs) {
+    if (!c.w) return ctx->fail(VTTS_ERR_BAD_ARG, "packing table entry without a weight");
+    bytes += vtts_tc_conv_packed_bytes(c.k, c.Cin, c.Cout);
+  }
+  if (m.wpk) cudaFree(m.wpk);
+  m.wpk = nullptr;
+  VTTS_CUDA(cudaMalloc(&m.wpk, bytes));
+  char* cur = (char*)m.wpk;
+  m.wpk_t.clear();
+  m.tile0.clear();
+  for (auto& c : convs) {
+    m.tile0.push_back((int)m.wpk_t.size());
+    int rc = vtts_tc_pack_conv(ctx, c.w, c.k, c.Cin, c.Cout, cur, m.wpk_t);
+    if (rc) return rc;
+  }
+  return VTTS_OK;
+}
+
+void vtts_free_weights(ModelWeights& m) {
+  cudaFree(m.blob);
+  cudaFree(m.derived);
+  cudaFree(m.wpk);
+  m = ModelWeights();
+}
+
+namespace {
+// the models of a context, in the bit order of vtts_broadcast_weights
+struct ModelSlot {
+  ModelWeights vtts_ctx::*w;
+  const std::vector<TensorSpec>& (*specs)();
+  int (*prepare)(vtts_ctx*);
+};
+const ModelSlot kModels[3] = {{&vtts_ctx::hg, vtts_hifigan_specs, vtts_hifigan_prepare},
+                              {&vtts_ctx::ac, vtts_acoustic_specs, vtts_acoustic_prepare},
+                              {&vtts_ctx::du, vtts_duration_specs, vtts_duration_prepare}};
+
+// copies a contiguous blob (host or device) into the slot's tensors, then derives and packs
+int load_model(vtts_ctx* ctx, const ModelSlot& ms, const float* blob, int64_t n_floats) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  ModelWeights& m = ctx->*ms.w;
+  const std::vector<TensorSpec>& specs = ms.specs();
+  m.loaded = false;
   if (!blob) return ctx->fail(VTTS_ERR_BAD_ARG, "load: null blob");
   if (n_floats != total_floats(specs))
     return ctx->fail(VTTS_ERR_BAD_ARG, "load: blob has %lld floats, expected %lld", (long long)n_floats, (long long)total_floats(specs));
-  int rc = alloc_arena(ctx, specs, store, ptrs);
+  int rc = vtts_alloc_tensors(ctx, spec_floats(specs), &m.blob, m.t);
   if (rc) return rc;
   int64_t src = 0;
   for (size_t i = 0; i < specs.size(); ++i) {
-    VTTS_CUDA(cudaMemcpy(ptrs[i], blob + src, (size_t)specs[i].n * sizeof(float), cudaMemcpyDefault));
+    VTTS_CUDA(cudaMemcpy(m.t[i], blob + src, (size_t)specs[i].n * sizeof(float), cudaMemcpyDefault));
     src += specs[i].n;
   }
+  rc = ms.prepare(ctx);
+  if (rc) return rc;
+  m.loaded = true;
   return VTTS_OK;
 }
+}  // namespace
 
 // ---- NCCL, bound at run time (the library has no link-time dependency on it: single-GPU users never load it) ----
 namespace {
@@ -292,10 +345,9 @@ int vtts_destroy(vtts_ctx* ctx) {
   if (!ctx) return VTTS_OK;
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
-  cudaFree(ctx->hg_blob); cudaFree(ctx->hg_upsw); cudaFree(ctx->ac_blob); cudaFree(ctx->ac_derived);
-  cudaFree(ctx->du_blob); cudaFree(ctx->du_derived); cudaFree(ctx->du_wpk);
+  for (auto& m : kModels) vtts_free_weights(ctx->*m.w);
   cudaFree(ctx->mel_fb); cudaFree(ctx->mel_lo); cudaFree(ctx->mel_hi); cudaFree(ctx->fft_tw); cudaFree(ctx->hann);
-  cudaFree(ctx->ws); cudaFree(ctx->dstage); cudaFree(ctx->d_err); cudaFree(ctx->hg_wpk); cudaFree(ctx->ac_wpk); cudaFree(ctx->d_tc_dbg);
+  cudaFree(ctx->ws); cudaFree(ctx->dstage); cudaFree(ctx->d_err); cudaFree(ctx->d_tc_dbg);
   if (ctx->hpin) cudaFreeHost(ctx->hpin);
   for (int i = 0; i < vtts_ctx::NSTAGE; ++i) {
     cudaEventDestroy(ctx->ev0[i]);
@@ -415,41 +467,9 @@ int64_t vtts_hifigan_blob_floats(void) { return total_floats(vtts_hifigan_specs(
 int64_t vtts_acoustic_blob_floats(void) { return total_floats(vtts_acoustic_specs()); }
 int64_t vtts_duration_blob_floats(void) { return total_floats(vtts_duration_specs()); }
 
-int vtts_load_hifigan(vtts_ctx* ctx, const float* blob, int64_t n_floats) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  ctx->hg_loaded = false;
-  int rc = load_blob(ctx, vtts_hifigan_specs(), blob, n_floats, &ctx->hg_blob, ctx->hg_t);
-  if (rc) return rc;
-  rc = vtts_hifigan_prepare(ctx);
-  if (rc) return rc;
-  ctx->hg_loaded = true;
-  return VTTS_OK;
-}
-
-int vtts_load_acoustic(vtts_ctx* ctx, const float* blob, int64_t n_floats) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  ctx->ac_loaded = false;
-  int rc = load_blob(ctx, vtts_acoustic_specs(), blob, n_floats, &ctx->ac_blob, ctx->ac_t);
-  if (rc) return rc;
-  rc = vtts_acoustic_prepare(ctx);
-  if (rc) return rc;
-  ctx->ac_loaded = true;
-  return VTTS_OK;
-}
-
-int vtts_load_duration(vtts_ctx* ctx, const float* blob, int64_t n_floats) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  ctx->du_loaded = false;
-  int rc = load_blob(ctx, vtts_duration_specs(), blob, n_floats, &ctx->du_blob, ctx->du_t);
-  if (rc) return rc;
-  rc = vtts_duration_prepare(ctx);
-  if (rc) return rc;
-  ctx->du_loaded = true;
-  return VTTS_OK;
-}
+int vtts_load_hifigan(vtts_ctx* ctx, const float* blob, int64_t n_floats) { return load_model(ctx, kModels[0], blob, n_floats); }
+int vtts_load_acoustic(vtts_ctx* ctx, const float* blob, int64_t n_floats) { return load_model(ctx, kModels[1], blob, n_floats); }
+int vtts_load_duration(vtts_ctx* ctx, const float* blob, int64_t n_floats) { return load_model(ctx, kModels[2], blob, n_floats); }
 
 // One start-up broadcast of the packed weights from `root` (SURVEY.md 8e: the only collective of the path).
 int vtts_broadcast_weights(vtts_ctx* ctx, void* nccl_comm, int root, int is_root, void* stream) {
@@ -465,7 +485,8 @@ int vtts_broadcast_weights(vtts_ctx* ctx, void* nccl_comm, int root, int is_root
   // which models travel: bit 0 hifigan, 1 acoustic, 2 duration (decided by the root's loaded state)
   int32_t* d_flags = nullptr;
   VTTS_CUDA(cudaMalloc(&d_flags, sizeof(int32_t)));
-  int32_t flags = is_root ? ((ctx->hg_loaded ? 1 : 0) | (ctx->ac_loaded ? 2 : 0) | (ctx->du_loaded ? 4 : 0)) : 0;
+  int32_t flags = 0;
+  for (int i = 0; i < 3 && is_root; ++i) flags |= (ctx->*kModels[i].w).loaded ? 1 << i : 0;
   VTTS_CUDA(cudaMemcpyAsync(d_flags, &flags, sizeof(flags), cudaMemcpyHostToDevice, st));
   int rc = nccl_ck(g_nccl.Broadcast(d_flags, d_flags, 1, /*ncclInt32*/ 2, root, nccl_comm, st), "ncclBroadcast(flags)");
   if (rc) { cudaFree(d_flags); return rc; }
@@ -473,33 +494,34 @@ int vtts_broadcast_weights(vtts_ctx* ctx, void* nccl_comm, int root, int is_root
   VTTS_CUDA(cudaStreamSynchronize(st));
   cudaFree(d_flags);
   if (is_root && flags == 0) return ctx->fail(VTTS_ERR_NOT_LOADED, "broadcast_weights: the root context has no weights loaded");
-  struct M { int bit; const std::vector<TensorSpec>* specs; float** store; std::vector<float*>* ptrs; bool* loaded; };
-  M models[3] = {{1, &vtts_hifigan_specs(), &ctx->hg_blob, &ctx->hg_t, &ctx->hg_loaded},
-                 {2, &vtts_acoustic_specs(), &ctx->ac_blob, &ctx->ac_t, &ctx->ac_loaded},
-                 {4, &vtts_duration_specs(), &ctx->du_blob, &ctx->du_t, &ctx->du_loaded}};
   if (!is_root)
-    for (auto& m : models)
-      if (flags & m.bit) {
-        *m.loaded = false;
-        rc = alloc_arena(ctx, *m.specs, m.store, *m.ptrs);
+    for (int i = 0; i < 3; ++i)
+      if (flags & (1 << i)) {
+        ModelWeights& m = ctx->*kModels[i].w;
+        m.loaded = false;
+        rc = vtts_alloc_tensors(ctx, spec_floats(kModels[i].specs()), &m.blob, m.t);
         if (rc) return rc;
       }
   // the arenas have the same layout on every rank (it only depends on the tensor specs): ONE grouped broadcast
   rc = nccl_ck(g_nccl.GroupStart(), "ncclGroupStart");
   if (rc) return rc;
-  for (auto& m : models)
-    if (flags & m.bit) {
-      rc = nccl_ck(g_nccl.Broadcast(*m.store, *m.store, arena_floats(*m.specs), /*ncclFloat32*/ 7, root, nccl_comm, st), "ncclBroadcast(weights)");
+  for (int i = 0; i < 3; ++i)
+    if (flags & (1 << i)) {
+      float* blob = (ctx->*kModels[i].w).blob;
+      rc = nccl_ck(g_nccl.Broadcast(blob, blob, arena_floats(spec_floats(kModels[i].specs())), /*ncclFloat32*/ 7, root, nccl_comm, st),
+                   "ncclBroadcast(weights)");
       if (rc) { g_nccl.GroupEnd(); return rc; }
     }
   rc = nccl_ck(g_nccl.GroupEnd(), "ncclGroupEnd");
   if (rc) return rc;
   VTTS_CUDA(cudaStreamSynchronize(st));
-  if (!is_root) {
-    if (flags & 1) { rc = vtts_hifigan_prepare(ctx); if (rc) return rc; ctx->hg_loaded = true; }
-    if (flags & 2) { rc = vtts_acoustic_prepare(ctx); if (rc) return rc; ctx->ac_loaded = true; }
-    if (flags & 4) { rc = vtts_duration_prepare(ctx); if (rc) return rc; ctx->du_loaded = true; }
-  }
+  if (!is_root)
+    for (int i = 0; i < 3; ++i)
+      if (flags & (1 << i)) {
+        rc = kModels[i].prepare(ctx);
+        if (rc) return rc;
+        (ctx->*kModels[i].w).loaded = true;
+      }
   return VTTS_OK;
 }
 
@@ -543,16 +565,13 @@ int vtts_acoustic_forward(vtts_ctx* ctx, const int32_t* tokens_dev, const int32_
   if (!tokens_dev || !dur_frames_dev || !mel_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic_forward: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
-  size_t need = 0;
-  int rc = vtts_acoustic_run(ctx, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, B, L, N, nullptr, st, nullptr, 0, &need);
-  if (rc) return rc;
   // the acoustic workspace lives after the hifigan one is released: both share ctx->ws, so a
   // synthesize call sizes it for the larger of the two (see vtts_synthesize_host)
-  rc = ctx->ensure_ws(need);
+  int rc = ctx->ensure_ws(vtts_acoustic_ws_bytes(B, L, N));
   if (rc) return rc;
   stage_begin(ctx, 1, st);
   rc = vtts_acoustic_run(ctx, tokens_dev, lengths_dev, dur_frames_dev, n_frames_dev, keep_mask_dev, dropout_mode, seed, B, L, N,
-                         mel_dev, st, ctx->ws, ctx->ws_bytes, nullptr);
+                         mel_dev, st);
   stage_end(ctx, 1, st);
   return rc;
 }
@@ -565,15 +584,11 @@ int vtts_acoustic_teacher_forward(vtts_ctx* ctx, const int32_t* tokens_dev, cons
   if (!tokens_dev || !dur_frames_dev || !mels_in_dev || !mel2_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic_teacher_forward: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
-  size_t need = 0;
-  int rc = vtts_acoustic_teacher_run(ctx, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, B, L, N, nullptr, nullptr, st,
-                                     nullptr, 0, &need);
-  if (rc) return rc;
-  rc = ctx->ensure_ws(need);
+  int rc = ctx->ensure_ws(vtts_acoustic_teacher_ws_bytes(B, L, N));
   if (rc) return rc;
   stage_begin(ctx, 1, st);
   rc = vtts_acoustic_teacher_run(ctx, tokens_dev, lengths_dev, dur_frames_dev, n_frames_dev, mels_in_dev, keep_mask_dev, zone_mask_dev,
-                                 dropout_mode, seed, B, L, N, mel1_dev_or_null, mel2_dev, st, ctx->ws, ctx->ws_bytes, nullptr);
+                                 dropout_mode, seed, B, L, N, mel1_dev_or_null, mel2_dev, st);
   stage_end(ctx, 1, st);
   return rc;
 }
@@ -584,13 +599,10 @@ int vtts_duration_forward(vtts_ctx* ctx, const int32_t* tokens_dev, const int32_
   if (!tokens_dev || !dur_sec_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "duration_forward: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
-  size_t need = 0;
-  int rc = vtts_duration_run(ctx, nullptr, nullptr, B, L, nullptr, st, nullptr, 0, &need);
-  if (rc) return rc;
-  rc = ctx->ensure_ws(need);
+  int rc = ctx->ensure_ws(vtts_duration_ws_bytes(B, L));
   if (rc) return rc;
   stage_begin(ctx, 3, st);
-  rc = vtts_duration_run(ctx, tokens_dev, lengths_dev, B, L, dur_sec_dev, st, ctx->ws, ctx->ws_bytes, nullptr);
+  rc = vtts_duration_run(ctx, tokens_dev, lengths_dev, B, L, dur_sec_dev, st);
   stage_end(ctx, 3, st);
   return rc;
 }

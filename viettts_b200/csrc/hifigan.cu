@@ -99,6 +99,12 @@ void carve(Arena& ar, int B, int T, HgBufs& hb) {
   for (int j = 0; j < 3; ++j) hb.Bb[j] = ar.take<float>(big);
 }
 
+// packing table of the generator: the 72 ResBlock convs in hgi order, the ConvTranspose output phases of the four
+// stages, conv_pre (two N = 256 tiles)
+constexpr int PK_RB(int n, int which, int m) { return n * 6 + which * 3 + m; }
+constexpr int PK_UPS(int i, int r) { return i == 0 ? 72 + r : PK_UPS(i - 1, vc::hg_rate(i - 1)) + r; }
+constexpr int PK_PRE = PK_UPS(4, 0), PK_COUNT = PK_PRE + 1;
+
 }  // namespace
 
 size_t vtts_hifigan_ws_bytes(int B, int T) {
@@ -109,85 +115,36 @@ size_t vtts_hifigan_ws_bytes(int B, int T) {
 }
 
 int vtts_hifigan_prepare(vtts_ctx* ctx) {
-  // repacked transposed-conv weights
-  size_t total = 0;
-  size_t offs[4];
-  int C = vc::HG_C0;
-  for (int i = 0; i < 4; ++i) {
-    offs[i] = total;
-    total += (size_t)vc::hg_rate(i) * 2 * C * (C / 2);
-    C /= 2;
-  }
-  if (ctx->hg_upsw) cudaFree(ctx->hg_upsw);
-  VTTS_CUDA(cudaMalloc(&ctx->hg_upsw, total * sizeof(float)));
-  C = vc::HG_C0;
-  for (int i = 0; i < 4; ++i) {
-    int u = vc::hg_rate(i), K = vc::hg_upk(i);
-    int a = (K + u - 2 + 1) / 2;
-    repack_ups_kernel<<<256, 256>>>(ctx->hg_t[hgi::UPS_W(i)], ctx->hg_upsw + offs[i], u, K, C, C / 2, a);
+  ModelWeights& m = ctx->hg;
+  // derived: the transposed-conv weights of stage i repacked per output phase, [u][2][C][C/2]
+  std::vector<size_t> dn;
+  for (int i = 0, C = vc::HG_C0; i < 4; ++i, C /= 2) dn.push_back((size_t)vc::hg_rate(i) * 2 * C * (C / 2));
+  int rc = vtts_alloc_tensors(ctx, dn, &m.derived, m.d);
+  if (rc) return rc;
+  std::vector<PackSpec> pk(PK_COUNT);
+  for (int i = 0, C = vc::HG_C0; i < 4; ++i, C /= 2) {
+    const int u = vc::hg_rate(i), K = vc::hg_upk(i);
+    repack_ups_kernel<<<256, 256>>>(m.t[hgi::UPS_W(i)], m.d[i], u, K, C, C / 2, (K + u - 2 + 1) / 2);
     VTTS_CUDA(cudaGetLastError());
-    C /= 2;
+    for (int r = 0; r < u; ++r) pk[PK_UPS(i, r)] = {m.d[i] + (size_t)r * 2 * C * (C / 2), 2, C, C / 2};
   }
+  for (int n = 0; n < 12; ++n)
+    for (int which = 0; which < 2; ++which)
+      for (int j = 0; j < 3; ++j) {
+        const int ch = 256 >> (n / 3);
+        pk[PK_RB(n, which, j)] = {m.t[hgi::RB_W(n, which, j)], vc::hg_rbk(n % 3), ch, ch};
+      }
+  pk[PK_PRE] = {m.t[hgi::PRE_W], 7, vc::MEL, vc::HG_C0};
   // ---- tensor-core path: bf16 hi/lo split + canonical K-major packing of every dense conv ----
-  {
-    VTTS_CUDA(cudaDeviceSynchronize());  // hg_upsw must be complete: the phase weights are packed from it
-    size_t elems = 0;
-    std::vector<size_t> eoff(72), uoff(32), poff(2);
-    for (int n = 0; n < 12; ++n) {
-      const int ch = 256 >> (n / 3), kk = vc::hg_rbk(n % 3);
-      for (int q = 0; q < 6; ++q) {
-        eoff[n * 6 + q] = elems;
-        elems += vtts_tc_packed_elems(kk, ch, ch);
-      }
-    }
-    int Cc = vc::HG_C0;
-    for (int i = 0; i < 4; ++i) {
-      for (int r = 0; r < vc::hg_rate(i); ++r) {
-        uoff[i * 8 + r] = elems;
-        elems += vtts_tc_packed_elems(2, Cc, Cc / 2);
-      }
-      Cc /= 2;
-    }
-    for (int t = 0; t < 2; ++t) {
-      poff[t] = elems;
-      elems += vtts_tc_packed_elems(7, vc::MEL, 256);
-    }
-    if (ctx->hg_wpk) cudaFree(ctx->hg_wpk);
-    VTTS_CUDA(cudaMalloc(&ctx->hg_wpk, elems * 2));
-    ctx->hg_wpk_t.resize(72);
-    ctx->hg_wpk_ups.assign(32, nullptr);
-    for (int n = 0; n < 12; ++n) {
-      const int ch = 256 >> (n / 3), kk = vc::hg_rbk(n % 3);
-      for (int which = 0; which < 2; ++which)
-        for (int m = 0; m < 3; ++m) {
-          const int q = which * 3 + m;
-          ctx->hg_wpk_t[n * 6 + q] = (char*)ctx->hg_wpk + eoff[n * 6 + q] * 2;
-          int rc = vtts_tc_pack_weights(ctx, ctx->hg_t[hgi::RB_W(n, which, m)], ctx->hg_wpk_t[n * 6 + q], kk, ch, ch, 0, ch);
-          if (rc) return rc;
-        }
-    }
-    Cc = vc::HG_C0;
-    for (int i = 0; i < 4; ++i) {
-      const int Co = Cc / 2;
-      for (int r = 0; r < vc::hg_rate(i); ++r) {
-        ctx->hg_wpk_ups[i * 8 + r] = (char*)ctx->hg_wpk + uoff[i * 8 + r] * 2;
-        int rc = vtts_tc_pack_weights(ctx, ctx->hg_upsw + offs[i] + (size_t)r * 2 * Cc * Co, ctx->hg_wpk_ups[i * 8 + r], 2, Cc, Co, 0, Co);
-        if (rc) return rc;
-      }
-      Cc = Co;
-    }
-    for (int t = 0; t < 2; ++t) {
-      ctx->hg_wpk_pre[t] = (char*)ctx->hg_wpk + poff[t] * 2;
-      int rc = vtts_tc_pack_weights(ctx, ctx->hg_t[hgi::PRE_W], ctx->hg_wpk_pre[t], 7, vc::MEL, vc::HG_C0, 256 * t, 256);
-      if (rc) return rc;
-    }
-  }
+  VTTS_CUDA(cudaDeviceSynchronize());  // the phase weights are packed from the repacked transposed-conv weights
+  rc = vtts_pack_convs(ctx, m, pk);
+  if (rc) return rc;
   VTTS_CUDA(cudaDeviceSynchronize());
   return VTTS_OK;
 }
 
 int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, int B, int T, float* wav, cudaStream_t st) {
-  if (!ctx->hg_loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "hifigan weights not loaded");
+  if (!ctx->hg.loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "hifigan weights not loaded");
   if (B < 1 || T < 1 || B > 65535) return ctx->fail(VTTS_ERR_BAD_ARG, "hifigan: B=%d T=%d", B, T);
   if ((int64_t)T * 256 > (int64_t)INT32_MAX / 64) return ctx->fail(VTTS_ERR_BAD_ARG, "hifigan: T=%d too long", T);
   size_t need = vtts_hifigan_ws_bytes(B, T);
@@ -196,7 +153,8 @@ int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, i
   Arena ar(ctx->ws, ctx->ws_bytes, false);
   HgBufs hb;
   carve(ar, B, T, hb);
-  auto& W = ctx->hg_t;
+  const ModelWeights& M = ctx->hg;
+  auto& W = M.t;
 
   ConvLaunch L;
   memset(&L, 0, sizeof(L));
@@ -217,7 +175,7 @@ int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, i
     TL.nprob = 2; TL.Cin = vc::MEL; TL.N = 256; TL.in_ld = vc::MEL; TL.out_ld = vc::HG_C0;
     TL.B = B; TL.T_rows = T; TL.rows_out = T; TL.len = n_frames; TL.len_mul = 1; TL.pre_mode = 0; TL.pre_slope = 1.f;
     for (int t = 0; t < 2; ++t)
-      TL.p[t] = TcProb{mel, nullptr, nullptr, ctx->hg_wpk_pre[t], W[hgi::PRE_B] + 256 * t, nullptr, nullptr, nullptr, nullptr, hb.P0 + 256 * t, 7, 1, -3, 1, 0};
+      TL.p[t] = TcProb{mel, nullptr, nullptr, M.tiles(PK_PRE)[t], W[hgi::PRE_B] + 256 * t, nullptr, nullptr, nullptr, nullptr, hb.P0 + 256 * t, 7, 1, -3, 1, 0};
     rc = vtts_launch_tc_conv(ctx, TL, st);
   } else {
     rc = vtts_launch_conv(ctx, L, st);
@@ -228,7 +186,6 @@ int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, i
   int C = vc::HG_C0;      // input channels of the stage
   int rows_in = T;        // rows per batch item entering the stage
   int scale_in = 1;       // rows_in = T*scale_in
-  size_t ups_off = 0;
   for (int i = 0; i < 4; ++i) {
     const int u = vc::hg_rate(i), K = vc::hg_upk(i), Co = C / 2;
     const int a = (K + u - 2 + 1) / 2;
@@ -245,7 +202,7 @@ int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, i
       ConvProb p;
       memset(&p, 0, sizeof(p));
       if (i == 0) { p.x0 = hb.P0; } else { p.x0 = hb.A[par ^ 1][0]; p.x1 = hb.A[par ^ 1][1]; p.x2 = hb.A[par ^ 1][2]; }
-      p.w = ctx->hg_upsw + ups_off + (size_t)r * 2 * C * Co;
+      p.w = M.d[i] + (size_t)r * 2 * C * Co;
       p.bias = W[hgi::UPS_B(i)];
       p.out = hb.X;
       p.k = 2; p.dil = 1; p.in_off = e; p.out_stride = u; p.out_off = r;
@@ -266,10 +223,10 @@ int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, i
         memset(&q, 0, sizeof(q));
         q.x0 = c0.x0; q.x1 = c0.x1; q.x2 = c0.x2; q.bias = c0.bias; q.out = c0.out;
         q.k = 2; q.dil = 1; q.out_stride = u;
-        q.wpk = ctx->hg_wpk_ups[i * 8 + g * nph]; q.in_off = c0.in_off; q.out_off = g * nph;
+        q.wpk = M.tiles(PK_UPS(i, g * nph))[0]; q.in_off = c0.in_off; q.out_off = g * nph;
         for (int ph = 0; ph < nph; ++ph) {
           const int r = g * nph + ph;
-          q.wpk_ph[ph] = ctx->hg_wpk_ups[i * 8 + r];
+          q.wpk_ph[ph] = M.tiles(PK_UPS(i, r))[0];
           q.in_off_ph[ph] = L.p[r].in_off;
           q.out_off_ph[ph] = r;
         }
@@ -280,7 +237,6 @@ int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, i
       rc = vtts_launch_conv(ctx, L, st);
     }
     if (rc) return rc;
-    ups_off += (size_t)u * 2 * C * Co;
 
     // ---- three ResBlock1 (k = 3,7,11), each 3 x [lrelu, conv(d), lrelu, conv(1), +x] ----
     const int rows = rows_in * u;
@@ -296,7 +252,7 @@ int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, i
         PL.nprob = 3; PL.N = Co; PL.B = B; PL.T_rows = rows; PL.len = n_frames; PL.len_mul = scale; PL.slope = 0.1f;
         for (int j = 0; j < 3; ++j) {
           const int kk = vc::hg_rbk(j), n = i * 3 + j;
-          PL.p[j] = TcPairProb{src[j], ctx->hg_wpk_t[n * 6 + m], ctx->hg_wpk_t[n * 6 + 3 + m], W[hgi::RB_B(n, 0, m)], W[hgi::RB_B(n, 1, m)],
+          PL.p[j] = TcPairProb{src[j], M.tiles(PK_RB(n, 0, m))[0], M.tiles(PK_RB(n, 1, m))[0], W[hgi::RB_B(n, 0, m)], W[hgi::RB_B(n, 1, m)],
                                (m == 1) ? hb.Bb[j] : hb.A[par][j], kk, d};
         }
         rc = vtts_launch_tc_pair(ctx, PL, st);
@@ -317,7 +273,7 @@ int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, i
             TcProb p;
             memset(&p, 0, sizeof(p));
             p.x0 = which == 0 ? src[j] : hb.Tb[j];
-            p.wpk = ctx->hg_wpk_t[n * 6 + which * 3 + m];
+            p.wpk = M.tiles(PK_RB(n, which, m))[0];
             p.bias = W[hgi::RB_B(n, which, m)];
             p.resid = which == 0 ? nullptr : src[j];
             p.out = which == 0 ? hb.Tb[j] : ((m == 1) ? hb.Bb[j] : hb.A[par][j]);

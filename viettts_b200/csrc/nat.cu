@@ -922,11 +922,16 @@ constexpr size_t dec_scan_smem() {
   return (lstm > pre ? lstm : pre) * 4;
 }
 
-// derived-weight slots (ctx->ac_d)
+// Slot layout shared by the acoustic and the duration model: the TokenEncoder's derived tensors and packed convs
+// come first in both, so that run_token_encoder reads either slot.
+enum { D_ENC_BNINV0, D_ENC_BNINV1, D_ENC_BNINV2,
+       D_ENC_WHR,     // [2][64][256][16]
+       D_ENC_COUNT };
+enum { PK_ENC_CONV0, PK_ENC_CONV1, PK_ENC_CONV2, PK_ENC_LSTM_F, PK_ENC_LSTM_B, PK_ENC_COUNT };
+
+// derived tensors of the acoustic model (ctx->ac.d)
 enum {
-  D_ENC_BNINV0 = 0, D_ENC_BNINV1, D_ENC_BNINV2,
-  D_POST_BNINV0, D_POST_BNINV1, D_POST_BNINV2, D_POST_BNINV3,
-  D_ENC_WHR,     // [2][64][256][16]
+  D_POST_BNINV0 = D_ENC_COUNT, D_POST_BNINV1, D_POST_BNINV2, D_POST_BNINV3,
   D_DEC_W0R,     // [128][768][16]
   D_DEC_W1R,     // [128][1280][16]
   D_DEC_WC,      // [16][1024][16]  (Wo . W1) columns
@@ -937,60 +942,90 @@ enum {
   D_COUNT
 };
 
-// slots of ctx->ac_wpk_t (tensor-core packed weights)
-enum { WP_ENC = 0, WP_ENCH = 3, WP_DECH = 11, WP_POST0 = 27, WP_POST1 = 29, WP_POST2 = 31, WP_POST3 = 33, WP_POST4 = 35, WP_PROJ = 36,
-       // teacher-forced pass: [cond | p2] rows 0..767 of both decoder LSTMs (8 N=256 tiles each), the two prenet linears
-       WP_TF_L0 = 37, WP_TF_L1 = 45, WP_PRE1 = 53, WP_PRE2 = 54, WP_COUNT = 55 };
+// packing table of the acoustic model (ctx->ac.tiles).  The problems of one multi-problem launch are consecutive
+// entries: the two decoder LSTMs, and the teacher-forced pass's [cond | p2] rows 0..767 of both
+enum { PK_DEC_L0 = PK_ENC_COUNT, PK_DEC_L1, PK_POST0, PK_PROJ = PK_POST0 + 5, PK_TF_L0, PK_TF_L1, PK_PRE1, PK_PRE2, PK_COUNT };
 
 }  // namespace
 
 // TokenEncoder.__call__ (model.py:26-47, is_training=False): embed -> 3 x [conv k3, BN(eval), relu] -> BiLSTM.
-// The acoustic model and the duration model instantiate it with the same dimensions (config.py:11-17), so one
-// implementation serves both; only the weight pointers differ.
-struct EncWeights {
-  const float* embed;
-  const float* conv_w[3];
-  const float* conv_b[3];
-  const float* bn_off[3];
-  const float* bn_mean[3];
-  const float* bn_inv[3];
-  const float *lf_w, *lf_b, *lb_w, *lb_b;   // hk.LSTM linear of the forward / backward core, w[512][1024]
-  const float* whr;                         // [2][64][256][16] recurrent rows, per direction / CTA
-  void* const* wpk_conv;                    // 3 packed conv weights (tensor-core path)
-  void* const* wpk_hoist;                   // 8 packed tiles of the two hoisted input projections
-};
+// The acoustic model and the duration model instantiate it with the same dimensions (config.py:11-17) and their
+// slots share its layout (aci::EMBED .. aci::ENC_LSTM_B_B, D_ENC_*, PK_ENC_*), so one implementation serves both.
+static void encoder_tables(const ModelWeights& m, std::vector<size_t>& dn, std::vector<PackSpec>& pk) {
+  const auto& T = m.t;
+  for (int i = 0; i < 3; ++i) {
+    dn[D_ENC_BNINV0 + i] = 256;
+    pk[PK_ENC_CONV0 + i] = {T[aci::ENC_CONV(i, 0)], 3, 256, 256};
+  }
+  dn[D_ENC_WHR] = (size_t)2 * 64 * 256 * 16;
+  pk[PK_ENC_LSTM_F] = {T[aci::ENC_LSTM_F_W], 1, 256, 1024};
+  pk[PK_ENC_LSTM_B] = {T[aci::ENC_LSTM_B_W], 1, 256, 1024};
+}
 
-static int run_token_encoder(vtts_ctx* ctx, const EncWeights& w, const int32_t* tokens, const int32_t* lengths, int B, int L,
-                             float* e0, float* e1, float* zx, float* enc, cudaStream_t st) {
+static void encoder_derive(const ModelWeights& m) {
+  const auto& T = m.t;
+  for (int i = 0; i < 3; ++i) bn_inv_kernel<<<1, 256>>>(T[aci::ENC_CONV(i, 2)], T[aci::ENC_CONV(i, 5)], m.d[D_ENC_BNINV0 + i], 256);
+  // recurrent weights: rows 256..511 of w[512][1024]
+  repack_cols_kernel<<<256, 256>>>(T[aci::ENC_LSTM_F_W], 1024, 256, 256, m.d[D_ENC_WHR], 64, 16, UPC, 256);
+  repack_cols_kernel<<<256, 256>>>(T[aci::ENC_LSTM_B_W], 1024, 256, 256, m.d[D_ENC_WHR] + (size_t)64 * 256 * 16, 64, 16, UPC, 256);
+}
+
+// ConvProb of a "same"-padded dilation-1 conv of kernel size k (k = 1: a GEMM over rows); the other fields are zero
+static ConvProb conv_prob(const float* x, const float* w, const float* bias, float* out, int k = 1) {
+  ConvProb p;
+  memset(&p, 0, sizeof(p));
+  p.x0 = x; p.w = w; p.bias = bias; p.out = out;
+  p.k = k; p.dil = 1; p.in_off = -(k - 1) / 2; p.out_stride = 1;
+  return p;
+}
+
+// nprob problems of one shape over B sequences of T rows (rows past len[b] are skipped when len is given), through
+// the shared dispatch: tensor-core path in BF16X3 mode (packed tiles `wpk`), FMA path in FP32 mode
+static int run_convs(vtts_ctx* ctx, const ConvProb* p, int nprob, int Cin, int Cout, int B, int T, const int32_t* len,
+                     int post_act, void* const* wpk, cudaStream_t st) {
+  ConvLaunch L;
+  memset(&L, 0, sizeof(L));
+  for (int i = 0; i < nprob; ++i) L.p[i] = p[i];
+  L.nprob = nprob; L.Cin = Cin; L.Cout = Cout; L.B = B; L.T_rows = T; L.rows_out = T;
+  L.len = len; L.len_mul = 1; L.pre_mode = 0; L.pre_slope = 1.f; L.post_act = post_act;
+  return vtts_conv_dispatch(ctx, L, wpk, st);
+}
+
+struct EncBufs { float *e0, *e1, *zx, *enc; };
+
+static void carve_encoder(Arena& ar, size_t BL, EncBufs& e) {
+  e.e0 = ar.take<float>(BL * 256);
+  e.e1 = ar.take<float>(BL * 256);
+  e.zx = ar.take<float>(2 * BL * 1024);
+  e.enc = ar.take<float>(BL * 512);
+}
+
+static int run_token_encoder(vtts_ctx* ctx, const ModelWeights& m, const int32_t* tokens, const int32_t* lengths, int B, int L,
+                             const EncBufs& e, cudaStream_t st) {
+  const auto& T = m.t;
   const size_t BL = (size_t)B * L;
-  embed_kernel<<<(unsigned)((BL + 3) / 4), 256, 0, st>>>(tokens, w.embed, e0, (int)BL);
+  embed_kernel<<<(unsigned)((BL + 3) / 4), 256, 0, st>>>(tokens, T[aci::EMBED], e.e0, (int)BL);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
-  ConvLaunch Lc;
-  float* cur = e0;
-  float* nxt = e1;
+  float* cur = e.e0;
+  float* nxt = e.e1;
   for (int i = 0; i < 3; ++i) {
-    memset(&Lc, 0, sizeof(Lc));
-    Lc.nprob = 1; Lc.Cin = 256; Lc.Cout = 256; Lc.B = B; Lc.T_rows = L; Lc.rows_out = L;
-    Lc.len = lengths; Lc.len_mul = 1; Lc.pre_mode = 0; Lc.pre_slope = 1.f; Lc.post_act = 2;
-    Lc.p[0] = ConvProb{cur, nullptr, nullptr, w.conv_w[i], w.conv_b[i], nullptr, w.bn_mean[i], w.bn_inv[i], w.bn_off[i], nxt, 3, 1, -1, 1, 0};
-    int rc = vtts_conv_dispatch(ctx, Lc, w.wpk_conv + i, st);
+    ConvProb p = conv_prob(cur, T[aci::ENC_CONV(i, 0)], T[aci::ENC_CONV(i, 1)], nxt, 3);
+    p.bn_mean = T[aci::ENC_CONV(i, 4)]; p.bn_inv = m.d[D_ENC_BNINV0 + i]; p.bn_off = T[aci::ENC_CONV(i, 3)];
+    int rc = run_convs(ctx, &p, 1, 256, 256, B, L, lengths, 2, m.tiles(PK_ENC_CONV0 + i), st);
     if (rc) return rc;
     float* tmp = cur; cur = nxt; nxt = tmp;
   }
   // rows past len[b] of `cur` were never written: the scans mask them, but the hoisted GEMM reads them
   // -> harmless garbage confined to rows that are never consumed (k=1 GEMM has no row mixing).
   // ---- hoisted input projections of the two LSTMs: zx[dir] = x . W[0:256] + b ----
-  memset(&Lc, 0, sizeof(Lc));
-  Lc.nprob = 2; Lc.Cin = 256; Lc.Cout = 1024; Lc.B = 1; Lc.T_rows = (int)BL; Lc.rows_out = (int)BL;
-  Lc.len = nullptr; Lc.len_mul = 1; Lc.pre_mode = 0; Lc.pre_slope = 1.f; Lc.post_act = 0;
-  Lc.p[0] = ConvProb{cur, nullptr, nullptr, w.lf_w, w.lf_b, nullptr, nullptr, nullptr, nullptr, zx, 1, 1, 0, 1, 0};
-  Lc.p[1] = ConvProb{cur, nullptr, nullptr, w.lb_w, w.lb_b, nullptr, nullptr, nullptr, nullptr, zx + BL * 1024, 1, 1, 0, 1, 0};
-  int rc = vtts_conv_dispatch(ctx, Lc, w.wpk_hoist, st);
+  const ConvProb hp[2] = {conv_prob(cur, T[aci::ENC_LSTM_F_W], T[aci::ENC_LSTM_F_B], e.zx),
+                          conv_prob(cur, T[aci::ENC_LSTM_B_W], T[aci::ENC_LSTM_B_B], e.zx + BL * 1024)};
+  int rc = run_convs(ctx, hp, 2, 256, 1024, 1, (int)BL, nullptr, 0, m.tiles(PK_ENC_LSTM_F), st);
   if (rc) return rc;
   // ---- BiLSTM scan (forward core + ResetCore'd backward core) ----
   EncScanArgs ea;
-  ea.zx = zx; ea.whr = w.whr; ea.lengths = lengths; ea.out = enc; ea.B = B; ea.L = L;
+  ea.zx = e.zx; ea.whr = m.d[D_ENC_WHR]; ea.lengths = lengths; ea.out = e.enc; ea.B = B; ea.L = L;
   void* args[] = {&ea};
   VTTS_CUDA(cudaLaunchCooperativeKernel((void*)enc_scan_kernel, dim3(SCAN_CTAS), dim3(SCAN_THREADS), args, enc_scan_smem(), st));
   ctx->launches++;
@@ -998,62 +1033,40 @@ static int run_token_encoder(vtts_ctx* ctx, const EncWeights& w, const int32_t* 
 }
 
 int vtts_acoustic_prepare(vtts_ctx* ctx) {
-  const size_t sizes[D_COUNT] = {256, 256, 256, 512, 512, 512, 512,
-                                 (size_t)2 * 64 * 256 * 16, (size_t)128 * 768 * 16, (size_t)128 * 1280 * 16,
-                                 (size_t)16 * 1024 * 16, (size_t)1024 * 256, 256, (size_t)16 * 256 * 16, 2048};
-  size_t total = 0;
-  std::vector<size_t> offs(D_COUNT);
-  for (int i = 0; i < D_COUNT; ++i) {
-    offs[i] = total;
-    total += (sizes[i] + 63) & ~size_t(63);
-  }
-  if (ctx->ac_derived) cudaFree(ctx->ac_derived);
-  VTTS_CUDA(cudaMalloc(&ctx->ac_derived, total * sizeof(float)));
-  ctx->ac_d.resize(D_COUNT);
-  for (int i = 0; i < D_COUNT; ++i) ctx->ac_d[i] = ctx->ac_derived + offs[i];
-  auto& T = ctx->ac_t;
-  for (int i = 0; i < 3; ++i) bn_inv_kernel<<<1, 256>>>(T[aci::ENC_CONV(i, 2)], T[aci::ENC_CONV(i, 5)], ctx->ac_d[D_ENC_BNINV0 + i], 256);
-  for (int i = 0; i < 4; ++i) bn_inv_kernel<<<2, 256>>>(T[aci::POST_CONV(i, 2)], T[aci::POST_CONV(i, 5)], ctx->ac_d[D_POST_BNINV0 + i], 512);
-  // encoder recurrent weights: rows 256..511 of w[512][1024]
-  repack_cols_kernel<<<256, 256>>>(T[aci::ENC_LSTM_F_W], 1024, 256, 256, ctx->ac_d[D_ENC_WHR], 64, 16, UPC, 256);
-  repack_cols_kernel<<<256, 256>>>(T[aci::ENC_LSTM_B_W], 1024, 256, 256, ctx->ac_d[D_ENC_WHR] + (size_t)64 * 256 * 16, 64, 16, UPC, 256);
+  ModelWeights& m = ctx->ac;
+  const auto& T = m.t;
+  std::vector<size_t> dn(D_COUNT);
+  std::vector<PackSpec> pk(PK_COUNT);
+  encoder_tables(m, dn, pk);
+  for (int i = 0; i < 4; ++i) dn[D_POST_BNINV0 + i] = 512;
+  dn[D_DEC_W0R] = (size_t)128 * 768 * 16;
+  dn[D_DEC_W1R] = (size_t)128 * 1280 * 16;
+  dn[D_DEC_WC] = (size_t)16 * 1024 * 16;
+  dn[D_DEC_WCFULL] = (size_t)1024 * 256;
+  dn[D_DEC_BC] = 256;
+  dn[D_DEC_WP2] = (size_t)16 * 256 * 16;
+  dn[D_ZERO] = 2048;
+  pk[PK_DEC_L0] = {T[aci::DEC_L0_W], 1, 512, 2048};
+  pk[PK_DEC_L1] = {T[aci::DEC_L1_W], 1, 512, 2048};
+  for (int i = 0; i < 5; ++i) pk[PK_POST0 + i] = {T[aci::POST_CONV(i, 0)], 5, i == 0 ? 80 : 512, i == 4 ? 80 : 512};
+  pk[PK_PROJ] = {T[aci::PROJ_W], 1, 1024, 80};
+  pk[PK_TF_L0] = {T[aci::DEC_L0_W], 1, 768, 2048};
+  pk[PK_TF_L1] = {T[aci::DEC_L1_W], 1, 768, 2048};
+  pk[PK_PRE1] = {T[aci::PRE1_W], 1, 80, 256};
+  pk[PK_PRE2] = {T[aci::PRE2_W], 1, 256, 256};
+  int rc = vtts_alloc_tensors(ctx, dn, &m.derived, m.d);   // zero-filled: D_ZERO needs no further work
+  if (rc) return rc;
+  encoder_derive(m);
+  for (int i = 0; i < 4; ++i) bn_inv_kernel<<<2, 256>>>(T[aci::POST_CONV(i, 2)], T[aci::POST_CONV(i, 5)], m.d[D_POST_BNINV0 + i], 512);
   // decoder: rows after the 512 cond rows
-  repack_cols_kernel<<<512, 256>>>(T[aci::DEC_L0_W], 2048, 512, 768, ctx->ac_d[D_DEC_W0R], 128, 16, UPC, 512);
-  repack_cols_kernel<<<512, 256>>>(T[aci::DEC_L1_W], 2048, 512, 1280, ctx->ac_d[D_DEC_W1R], 128, 16, UPC, 512);
-  precompose_kernel<<<2 * vc::DEC_H + 1, 256>>>(T[aci::PROJ_W], T[aci::PROJ_B], T[aci::PRE1_W], ctx->ac_d[D_DEC_WCFULL], ctx->ac_d[D_DEC_BC]);
-  repack_cols_kernel<<<256, 256>>>(ctx->ac_d[D_DEC_WCFULL], 256, 0, 1024, ctx->ac_d[D_DEC_WC], 16, 16, 16, 0);
-  repack_cols_kernel<<<64, 256>>>(T[aci::PRE2_W], 256, 0, 256, ctx->ac_d[D_DEC_WP2], 16, 16, 16, 0);
-  VTTS_CUDA(cudaMemset(ctx->ac_d[D_ZERO], 0, 2048 * sizeof(float)));
+  repack_cols_kernel<<<512, 256>>>(T[aci::DEC_L0_W], 2048, 512, 768, m.d[D_DEC_W0R], 128, 16, UPC, 512);
+  repack_cols_kernel<<<512, 256>>>(T[aci::DEC_L1_W], 2048, 512, 1280, m.d[D_DEC_W1R], 128, 16, UPC, 512);
+  precompose_kernel<<<2 * vc::DEC_H + 1, 256>>>(T[aci::PROJ_W], T[aci::PROJ_B], T[aci::PRE1_W], m.d[D_DEC_WCFULL], m.d[D_DEC_BC]);
+  repack_cols_kernel<<<256, 256>>>(m.d[D_DEC_WCFULL], 256, 0, 1024, m.d[D_DEC_WC], 16, 16, 16, 0);
+  repack_cols_kernel<<<64, 256>>>(T[aci::PRE2_W], 256, 0, 256, m.d[D_DEC_WP2], 16, 16, 16, 0);
   VTTS_CUDA(cudaGetLastError());
-  // ---- tensor-core packed weights of the convs and hoisted GEMMs ----
-  {
-    size_t bytes = 3 * vtts_tc_conv_packed_bytes(3, 256, 256) + 2 * vtts_tc_conv_packed_bytes(1, 256, 1024) +
-                   2 * vtts_tc_conv_packed_bytes(1, 512, 2048) + vtts_tc_conv_packed_bytes(5, 80, 512) +
-                   3 * vtts_tc_conv_packed_bytes(5, 512, 512) + vtts_tc_conv_packed_bytes(5, 512, 80) +
-                   vtts_tc_conv_packed_bytes(1, 1024, 80) + 2 * vtts_tc_conv_packed_bytes(1, 768, 2048) +
-                   vtts_tc_conv_packed_bytes(1, 80, 256) + vtts_tc_conv_packed_bytes(1, 256, 256);
-    if (ctx->ac_wpk) cudaFree(ctx->ac_wpk);
-    VTTS_CUDA(cudaMalloc(&ctx->ac_wpk, bytes));
-    char* cur = (char*)ctx->ac_wpk;
-    ctx->ac_wpk_t.clear();
-    int rc = 0;
-    for (int i = 0; i < 3 && !rc; ++i) rc = vtts_tc_pack_conv(ctx, T[aci::ENC_CONV(i, 0)], 3, 256, 256, cur, ctx->ac_wpk_t);
-    if (!rc) rc = vtts_tc_pack_conv(ctx, T[aci::ENC_LSTM_F_W], 1, 256, 1024, cur, ctx->ac_wpk_t);
-    if (!rc) rc = vtts_tc_pack_conv(ctx, T[aci::ENC_LSTM_B_W], 1, 256, 1024, cur, ctx->ac_wpk_t);
-    if (!rc) rc = vtts_tc_pack_conv(ctx, T[aci::DEC_L0_W], 1, 512, 2048, cur, ctx->ac_wpk_t);
-    if (!rc) rc = vtts_tc_pack_conv(ctx, T[aci::DEC_L1_W], 1, 512, 2048, cur, ctx->ac_wpk_t);
-    if (!rc) rc = vtts_tc_pack_conv(ctx, T[aci::POST_CONV(0, 0)], 5, 80, 512, cur, ctx->ac_wpk_t);
-    for (int i = 1; i < 4 && !rc; ++i) rc = vtts_tc_pack_conv(ctx, T[aci::POST_CONV(i, 0)], 5, 512, 512, cur, ctx->ac_wpk_t);
-    if (!rc) rc = vtts_tc_pack_conv(ctx, T[aci::POST_CONV(4, 0)], 5, 512, 80, cur, ctx->ac_wpk_t);
-    if (!rc) rc = vtts_tc_pack_conv(ctx, T[aci::PROJ_W], 1, 1024, 80, cur, ctx->ac_wpk_t);
-    if (!rc) rc = vtts_tc_pack_conv(ctx, T[aci::DEC_L0_W], 1, 768, 2048, cur, ctx->ac_wpk_t);   // rows 0..767 = [cond | p2]
-    if (!rc) rc = vtts_tc_pack_conv(ctx, T[aci::DEC_L1_W], 1, 768, 2048, cur, ctx->ac_wpk_t);
-    if (!rc) rc = vtts_tc_pack_conv(ctx, T[aci::PRE1_W], 1, 80, 256, cur, ctx->ac_wpk_t);
-    if (!rc) rc = vtts_tc_pack_conv(ctx, T[aci::PRE2_W], 1, 256, 256, cur, ctx->ac_wpk_t);
-    if (rc) return rc;
-    if ((int)ctx->ac_wpk_t.size() != WP_COUNT || (size_t)(cur - (char*)ctx->ac_wpk) > bytes)
-      return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: packed weight table has %d entries", (int)ctx->ac_wpk_t.size());
-  }
+  rc = vtts_pack_convs(ctx, m, pk);
+  if (rc) return rc;
   VTTS_CUDA(cudaDeviceSynchronize());
   VTTS_CUDA(cudaFuncSetAttribute(enc_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc_scan_smem()));
   VTTS_CUDA(cudaFuncSetAttribute(decoder_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dec_scan_smem()));
@@ -1061,115 +1074,149 @@ int vtts_acoustic_prepare(vtts_ctx* ctx) {
   return VTTS_OK;
 }
 
-// AcousticModel.postnet (model.py:113-121, is_training=False) + the residual add (:143-144 / :169):
-// mel = melpre + conv5(tanh(bn(conv5(...))));  q0/q1 are [B*N][512] scratch
-static int run_postnet(vtts_ctx* ctx, const float* melpre, const int32_t* n_frames, int B, int N, float* q0, float* q1, float* mel,
-                       cudaStream_t st) {
-  auto& T = ctx->ac_t;
-  auto& D = ctx->ac_d;
-  ConvLaunch Lc;
+// Gaussian upsampling of the encoder output to N frames: columns 0..511 of `out` (row stride out_ld)
+static int run_upsample(vtts_ctx* ctx, const float* enc, const float* dur, const int32_t* lengths, const int32_t* n_frames,
+                        int B, int L, int N, float* out, int out_ld, cudaStream_t st) {
+  dim3 grid((N + UP_F - 1) / UP_F, B);
+  size_t smem = (size_t)(L + UP_F * L) * sizeof(float);
+  if (smem > 200 * 1024) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: L=%d too long for the upsample kernel", L);
+  if (smem > 48 * 1024) VTTS_CUDA(cudaFuncSetAttribute(upsample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  upsample_kernel<<<grid, 256, smem, st>>>(enc, dur, lengths, n_frames, L, N, out, out_ld);
+  ctx->launches++;
+  VTTS_CUDA(cudaGetLastError());
+  return VTTS_OK;
+}
+
+// Output projection of every frame in one GEMM, melpre = [h0 | h1] . Wo + bo (model.py:135; rows past n_frames[b] stay 0),
+// copied to mel1 if given; sub-stage mark `proj_mark` (if >= 0); then AcousticModel.postnet (model.py:113-121,
+// is_training=False) + the residual add (:143-144 / :169): mel = melpre + conv5(tanh(bn(conv5(...)))).
+// q0/q1 are [B*N][512] scratch.
+static int run_projection_postnet(vtts_ctx* ctx, const float* hout, const int32_t* n_frames, int B, int N, float* melpre,
+                                  float* q0, float* q1, float* mel1, int proj_mark, float* mel, cudaStream_t st) {
+  const ModelWeights& m = ctx->ac;
+  const auto& T = m.t;
+  const ConvProb pp = conv_prob(hout, T[aci::PROJ_W], T[aci::PROJ_B], melpre);
+  int rc = run_convs(ctx, &pp, 1, 1024, 80, B, N, n_frames, 0, m.tiles(PK_PROJ), st);
+  if (rc) return rc;
+  if (mel1) VTTS_CUDA(cudaMemcpyAsync(mel1, melpre, (size_t)B * N * 80 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (proj_mark >= 0) ctx->sub_mark(proj_mark, st);
   const float* pin = melpre;
   float* pout = q0;
-  int cin = 80;
   for (int i = 0; i < 5; ++i) {
-    const int cout = i < 4 ? 512 : 80;
-    memset(&Lc, 0, sizeof(Lc));
-    Lc.nprob = 1; Lc.Cin = cin; Lc.Cout = cout; Lc.B = B; Lc.T_rows = N; Lc.rows_out = N;
-    Lc.len = n_frames; Lc.len_mul = 1; Lc.pre_mode = 0; Lc.pre_slope = 1.f; Lc.post_act = i < 4 ? 1 : 0;
-    ConvProb p;
-    memset(&p, 0, sizeof(p));
-    p.x0 = pin; p.w = T[aci::POST_CONV(i, 0)]; p.bias = T[aci::POST_CONV(i, 1)];
-    if (i < 4) { p.bn_mean = T[aci::POST_CONV(i, 4)]; p.bn_inv = D[D_POST_BNINV0 + i]; p.bn_off = T[aci::POST_CONV(i, 3)]; }
-    if (i == 4) { p.resid = melpre; p.out = mel; } else { p.out = pout; }
-    p.k = 5; p.dil = 1; p.in_off = -2; p.out_stride = 1; p.out_off = 0;
-    Lc.p[0] = p;
-    int rc = vtts_conv_dispatch(ctx, Lc, &ctx->ac_wpk_t[i == 0 ? WP_POST0 : (i == 1 ? WP_POST1 : (i == 2 ? WP_POST2 : (i == 3 ? WP_POST3 : WP_POST4)))], st);
+    ConvProb p = conv_prob(pin, T[aci::POST_CONV(i, 0)], T[aci::POST_CONV(i, 1)], i < 4 ? pout : mel, 5);
+    if (i < 4) { p.bn_mean = T[aci::POST_CONV(i, 4)]; p.bn_inv = m.d[D_POST_BNINV0 + i]; p.bn_off = T[aci::POST_CONV(i, 3)]; }
+    else p.resid = melpre;
+    rc = run_convs(ctx, &p, 1, i == 0 ? 80 : 512, i < 4 ? 512 : 80, B, N, n_frames, i < 4 ? 1 : 0, m.tiles(PK_POST0 + i), st);
     if (rc) return rc;
     pin = pout;
     pout = (pout == q0) ? q1 : q0;
-    cin = cout;
   }
   return VTTS_OK;
 }
 
+namespace {
+// Workspace of one pass.  carve() lays it out the same way for sizing (*_ws_bytes) and for the run.
+struct AcBufs {
+  EncBufs e;
+  float *cond, *zc0, *zc1, *melpre, *q0, *q1, *p1, *p2, *hout, *h0, *h1;
+  unsigned int* pre_bar;
+};
+struct TfBufs {
+  EncBufs e;
+  float *xin, *pa, *pb, *zc0, *zc1, *hout, *melpre, *q0, *q1, *h0s, *h1s;
+};
+struct DuBufs {
+  EncBufs e;
+  float* y;
+};
+constexpr int XW = vc::ENC_OUT + vc::PRENET;   // 768: teacher-forced decoder input [cond | prenet(mel)]
+
+void carve(Arena& ar, int B, int L, int N, AcBufs& w) {
+  const size_t BN = (size_t)B * N;
+  carve_encoder(ar, (size_t)B * L, w.e);
+  w.cond = ar.take<float>(BN * 512);
+  w.zc0 = ar.take<float>(BN * 2048);
+  w.zc1 = ar.take<float>(BN * 2048);
+  w.melpre = ar.take<float>(BN * 80);
+  w.q0 = ar.take<float>(BN * 512);
+  w.q1 = ar.take<float>(BN * 512);
+  w.p1 = ar.take<float>((size_t)B * 256);
+  w.p2 = ar.take<float>((size_t)B * 256);
+  w.hout = ar.take<float>(BN * 1024);
+  w.h0 = ar.take<float>((size_t)2 * MAX_ROWS * 512);
+  w.h1 = ar.take<float>((size_t)2 * MAX_ROWS * 512);
+  w.pre_bar = ar.take<unsigned int>(64);
+}
+void carve(Arena& ar, int B, int L, int N, TfBufs& w) {
+  const size_t BN = (size_t)B * N;
+  carve_encoder(ar, (size_t)B * L, w.e);
+  w.xin = ar.take<float>(BN * XW);
+  w.pa = ar.take<float>(BN * 256);
+  w.pb = ar.take<float>(BN * 256);
+  w.zc0 = ar.take<float>(BN * 2048);
+  w.zc1 = ar.take<float>(BN * 2048);
+  w.hout = ar.take<float>(BN * 1024);
+  w.melpre = ar.take<float>(BN * 80);
+  w.q0 = ar.take<float>(BN * 512);
+  w.q1 = ar.take<float>(BN * 512);
+  w.h0s = ar.take<float>((size_t)2 * DEC_XR * 512);
+  w.h1s = ar.take<float>((size_t)2 * DEC_XR * 512);
+}
+void carve(Arena& ar, int B, int L, int, DuBufs& w) {
+  carve_encoder(ar, (size_t)B * L, w.e);
+  w.y = ar.take<float>((size_t)B * L * 256);
+}
+template <class Bufs>
+size_t ws_bytes(int B, int L, int N) {
+  Arena ar(nullptr, 0, true);
+  Bufs w;
+  carve(ar, B, L, N, w);
+  return ar.off + 256;
+}
+template <class Bufs>
+Bufs carve_ws(vtts_ctx* ctx, int B, int L, int N) {
+  Arena ar(ctx->ws, ctx->ws_bytes, false);
+  Bufs w;
+  carve(ar, B, L, N, w);
+  return w;
+}
+}  // namespace
+
+size_t vtts_acoustic_ws_bytes(int B, int L, int N) { return ws_bytes<AcBufs>(B, L, N); }
+size_t vtts_acoustic_teacher_ws_bytes(int B, int L, int N) { return ws_bytes<TfBufs>(B, L, N); }
+size_t vtts_duration_ws_bytes(int B, int L) { return ws_bytes<DuBufs>(B, L, 0); }
+
 int vtts_acoustic_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const float* dur,
                       const int32_t* n_frames, const uint8_t* keep, int mode, uint64_t seed, int B, int L, int N,
-                      float* mel, cudaStream_t st, void* ws_base, size_t ws_cap, size_t* ws_need) {
-  const bool measure = ws_need != nullptr;
-  if (!measure) {
-    if (!ctx->ac_loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "acoustic weights not loaded");
-    if (B < 1 || L < 1 || N < 1 || B > MAX_ROWS)
-      return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: B=%d L=%d N=%d (1 <= B <= %d rows per call; the host layer chunks larger batches)", B, L, N, MAX_ROWS);
-    if (mode < 0 || mode > 2) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: dropout_mode %d", mode);
-    if (mode == VTTS_DROPOUT_MASK && !keep) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: dropout_mode MASK needs keep_mask");
-    if (ctx->sm_count < DEC_CTAS) return ctx->fail(VTTS_ERR_NO_DEVICE, "scan kernels need %d SMs, device has %d", DEC_CTAS, ctx->sm_count);
-  }
-  Arena ar(ws_base, ws_cap, measure);
+                      float* mel, cudaStream_t st) {
+  if (!ctx->ac.loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "acoustic weights not loaded");
+  if (B < 1 || L < 1 || N < 1 || B > MAX_ROWS)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: B=%d L=%d N=%d (1 <= B <= %d rows per call; the host layer chunks larger batches)", B, L, N, MAX_ROWS);
+  if (mode < 0 || mode > 2) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: dropout_mode %d", mode);
+  if (mode == VTTS_DROPOUT_MASK && !keep) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: dropout_mode MASK needs keep_mask");
+  if (ctx->sm_count < DEC_CTAS) return ctx->fail(VTTS_ERR_NO_DEVICE, "scan kernels need %d SMs, device has %d", DEC_CTAS, ctx->sm_count);
+  const AcBufs w = carve_ws<AcBufs>(ctx, B, L, N);
   const size_t BL = (size_t)B * L, BN = (size_t)B * N;
-  float* e0 = ar.take<float>(BL * 256);
-  float* e1 = ar.take<float>(BL * 256);
-  float* zx = ar.take<float>(2 * BL * 1024);
-  float* enc = ar.take<float>(BL * 512);
-  float* cond = ar.take<float>(BN * 512);
-  float* zc0 = ar.take<float>(BN * 2048);
-  float* zc1 = ar.take<float>(BN * 2048);
-  float* melpre = ar.take<float>(BN * 80);
-  float* q0 = ar.take<float>(BN * 512);
-  float* q1 = ar.take<float>(BN * 512);
-  float* p1 = ar.take<float>((size_t)B * 256);
-  float* p2 = ar.take<float>((size_t)B * 256);
-  float* hout = ar.take<float>(BN * 1024);
-  float* h0 = ar.take<float>((size_t)2 * MAX_ROWS * 512);
-  float* h1 = ar.take<float>((size_t)2 * MAX_ROWS * 512);
-  unsigned int* pre_bar = ar.take<unsigned int>(64);
-  if (measure) {
-    *ws_need = ar.off + 256;
-    return VTTS_OK;
-  }
-  auto& T = ctx->ac_t;
-  auto& D = ctx->ac_d;
-  ctx->tap_enc = enc; ctx->tap_enc_n = BL * 512;
-  ctx->tap_cond = cond; ctx->tap_cond_n = BN * 512;
-  ctx->tap_melpre = melpre; ctx->tap_melpre_n = BN * 80;
+  const ModelWeights& m = ctx->ac;
+  const auto& T = m.t;
+  const auto& D = m.d;
+  ctx->tap_enc = w.e.enc; ctx->tap_enc_n = BL * 512;
+  ctx->tap_cond = w.cond; ctx->tap_cond_n = BN * 512;
+  ctx->tap_melpre = w.melpre; ctx->tap_melpre_n = BN * 80;
 
   VTTS_CUDA(cudaMemsetAsync(mel, 0, BN * 80 * sizeof(float), st));
-  VTTS_CUDA(cudaMemsetAsync(cond, 0, BN * 512 * sizeof(float), st));
-  VTTS_CUDA(cudaMemsetAsync(melpre, 0, BN * 80 * sizeof(float), st));
+  VTTS_CUDA(cudaMemsetAsync(w.cond, 0, BN * 512 * sizeof(float), st));
+  VTTS_CUDA(cudaMemsetAsync(w.melpre, 0, BN * 80 * sizeof(float), st));
   ctx->sub_mark(0, st);
-
-  // ---- TokenEncoder (shared with the duration model, run_token_encoder above) ----
-  {
-    EncWeights ew;
-    ew.embed = T[aci::EMBED];
-    for (int i = 0; i < 3; ++i) {
-      ew.conv_w[i] = T[aci::ENC_CONV(i, 0)]; ew.conv_b[i] = T[aci::ENC_CONV(i, 1)];
-      ew.bn_off[i] = T[aci::ENC_CONV(i, 3)]; ew.bn_mean[i] = T[aci::ENC_CONV(i, 4)]; ew.bn_inv[i] = D[D_ENC_BNINV0 + i];
-    }
-    ew.lf_w = T[aci::ENC_LSTM_F_W]; ew.lf_b = T[aci::ENC_LSTM_F_B]; ew.lb_w = T[aci::ENC_LSTM_B_W]; ew.lb_b = T[aci::ENC_LSTM_B_B];
-    ew.whr = D[D_ENC_WHR]; ew.wpk_conv = &ctx->ac_wpk_t[WP_ENC]; ew.wpk_hoist = &ctx->ac_wpk_t[WP_ENCH];
-    int rc = run_token_encoder(ctx, ew, tokens, lengths, B, L, e0, e1, zx, enc, st);
-    if (rc) return rc;
-  }
+  int rc = run_token_encoder(ctx, m, tokens, lengths, B, L, w.e, st);
+  if (rc) return rc;
   ctx->sub_mark(1, st);
-  // ---- Gaussian upsampling ----
-  {
-    dim3 grid((N + UP_F - 1) / UP_F, B);
-    size_t smem = (size_t)(L + UP_F * L) * sizeof(float);
-    if (smem > 200 * 1024) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: L=%d too long for the upsample kernel", L);
-    if (smem > 48 * 1024) VTTS_CUDA(cudaFuncSetAttribute(upsample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    upsample_kernel<<<grid, 256, smem, st>>>(enc, dur, lengths, n_frames, L, N, cond, vc::ENC_OUT);
-    ctx->launches++;
-    VTTS_CUDA(cudaGetLastError());
-  }
+  rc = run_upsample(ctx, w.e.enc, dur, lengths, n_frames, B, L, N, w.cond, vc::ENC_OUT, st);
+  if (rc) return rc;
   ctx->sub_mark(2, st);
   // ---- hoisted cond projections of the decoder LSTMs ----
-  ConvLaunch Lc;
-  memset(&Lc, 0, sizeof(Lc));
-  Lc.nprob = 2; Lc.Cin = 512; Lc.Cout = 2048; Lc.B = 1; Lc.T_rows = (int)BN; Lc.rows_out = (int)BN;
-  Lc.pre_mode = 0; Lc.pre_slope = 1.f; Lc.post_act = 0; Lc.len_mul = 1;
-  Lc.p[0] = ConvProb{cond, nullptr, nullptr, T[aci::DEC_L0_W], T[aci::DEC_L0_B], nullptr, nullptr, nullptr, nullptr, zc0, 1, 1, 0, 1, 0};
-  Lc.p[1] = ConvProb{cond, nullptr, nullptr, T[aci::DEC_L1_W], T[aci::DEC_L1_B], nullptr, nullptr, nullptr, nullptr, zc1, 1, 1, 0, 1, 0};
-  int rc = vtts_conv_dispatch(ctx, Lc, &ctx->ac_wpk_t[WP_DECH], st);
+  const ConvProb hp[2] = {conv_prob(w.cond, T[aci::DEC_L0_W], T[aci::DEC_L0_B], w.zc0), conv_prob(w.cond, T[aci::DEC_L1_W], T[aci::DEC_L1_B], w.zc1)};
+  rc = run_convs(ctx, hp, 2, 512, 2048, 1, (int)BN, nullptr, 0, m.tiles(PK_DEC_L0), st);
   if (rc) return rc;
   ctx->sub_mark(3, st);
   // ---- autoregressive scan: ONE launch for up to DEC_NG * 32 rows (row groups share the grid barriers of a frame) ----
@@ -1177,28 +1224,19 @@ int vtts_acoustic_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengt
     const int nb = B - b0 < DEC_NG * DEC_XR ? B - b0 : DEC_NG * DEC_XR;
     DecScanArgs da;
     memset(&da, 0, sizeof(da));
-    da.zc0 = zc0 + (size_t)b0 * N * 2048; da.zc1 = zc1 + (size_t)b0 * N * 2048;
+    da.zc0 = w.zc0 + (size_t)b0 * N * 2048; da.zc1 = w.zc1 + (size_t)b0 * N * 2048;
     da.w0r = D[D_DEC_W0R]; da.w1r = D[D_DEC_W1R]; da.wc = D[D_DEC_WC]; da.bc = D[D_DEC_BC]; da.wp2 = D[D_DEC_WP2];
     da.keep = keep; da.seed = seed; da.mode = mode;
-    da.p1 = p1; da.p2 = p2; da.h0 = h0; da.h1 = h1; da.hout = hout + (size_t)b0 * N * 1024;
-    da.pre_bar = pre_bar; da.err = ctx->d_err;
-    VTTS_CUDA(cudaMemsetAsync(pre_bar, 0, sizeof(unsigned int), st));
+    da.p1 = w.p1; da.p2 = w.p2; da.h0 = w.h0; da.h1 = w.h1; da.hout = w.hout + (size_t)b0 * N * 1024;
+    da.pre_bar = w.pre_bar; da.err = ctx->d_err;
+    VTTS_CUDA(cudaMemsetAsync(w.pre_bar, 0, sizeof(unsigned int), st));
     da.B = nb; da.N = N; da.row_base = b0; da.dbg = ctx->tc_dbg_on ? ctx->d_tc_dbg : nullptr;
     void* args[] = {&da};
     VTTS_CUDA(cudaLaunchCooperativeKernel((void*)decoder_scan_kernel, dim3(DEC_CTAS), dim3(SCAN_THREADS), args, dec_scan_smem(), st));
     ctx->launches++;
   }
   ctx->sub_mark(4, st);
-  // ---- output projection of every frame in one GEMM: mel_pre = [h0 | h1] . Wo + bo (model.py:135);
-  //      rows past n_frames[b] stay 0 ----
-  memset(&Lc, 0, sizeof(Lc));
-  Lc.nprob = 1; Lc.Cin = 1024; Lc.Cout = 80; Lc.B = B; Lc.T_rows = N; Lc.rows_out = N;
-  Lc.len = n_frames; Lc.len_mul = 1; Lc.pre_mode = 0; Lc.pre_slope = 1.f; Lc.post_act = 0;
-  Lc.p[0] = ConvProb{hout, nullptr, nullptr, T[aci::PROJ_W], T[aci::PROJ_B], nullptr, nullptr, nullptr, nullptr, melpre, 1, 1, 0, 1, 0};
-  rc = vtts_conv_dispatch(ctx, Lc, &ctx->ac_wpk_t[WP_PROJ], st);
-  if (rc) return rc;
-  ctx->sub_mark(5, st);
-  rc = run_postnet(ctx, melpre, n_frames, B, N, q0, q1, mel, st);
+  rc = run_projection_postnet(ctx, w.hout, n_frames, B, N, w.melpre, w.q0, w.q1, nullptr, 5, mel, st);
   if (rc) return rc;
   ctx->sub_mark(6, st);
   return VTTS_OK;
@@ -1209,99 +1247,49 @@ int vtts_acoustic_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengt
 // scan -> projection -> postnet.  mel1 = projection output (may be null), mel2 = mel1 + postnet(mel1).
 int vtts_acoustic_teacher_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const float* dur,
                               const int32_t* n_frames, const float* mels_in, const uint8_t* keep, const uint8_t* zone, int mode,
-                              uint64_t seed, int B, int L, int N, float* mel1, float* mel2, cudaStream_t st, void* ws_base,
-                              size_t ws_cap, size_t* ws_need) {
-  const bool measure = ws_need != nullptr;
-  if (!measure) {
-    if (!ctx->ac_loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "acoustic weights not loaded");
-    if (B < 1 || L < 1 || N < 1 || B > MAX_ROWS)
-      return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic (teacher forced): B=%d L=%d N=%d (1 <= B <= %d rows per call)", B, L, N, MAX_ROWS);
-    if (mode < 0 || mode > 2) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic (teacher forced): dropout_mode %d", mode);
-    if (mode == VTTS_DROPOUT_MASK && (!keep || !zone))
-      return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic (teacher forced): dropout_mode MASK needs keep_mask and zone_mask");
-    if (ctx->sm_count < SCAN_CTAS) return ctx->fail(VTTS_ERR_NO_DEVICE, "scan kernels need %d SMs, device has %d", SCAN_CTAS, ctx->sm_count);
-  }
-  Arena ar(ws_base, ws_cap, measure);
+                              uint64_t seed, int B, int L, int N, float* mel1, float* mel2, cudaStream_t st) {
+  if (!ctx->ac.loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "acoustic weights not loaded");
+  if (B < 1 || L < 1 || N < 1 || B > MAX_ROWS)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic (teacher forced): B=%d L=%d N=%d (1 <= B <= %d rows per call)", B, L, N, MAX_ROWS);
+  if (mode < 0 || mode > 2) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic (teacher forced): dropout_mode %d", mode);
+  if (mode == VTTS_DROPOUT_MASK && (!keep || !zone))
+    return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic (teacher forced): dropout_mode MASK needs keep_mask and zone_mask");
+  if (ctx->sm_count < SCAN_CTAS) return ctx->fail(VTTS_ERR_NO_DEVICE, "scan kernels need %d SMs, device has %d", SCAN_CTAS, ctx->sm_count);
+  const TfBufs w = carve_ws<TfBufs>(ctx, B, L, N);
   const size_t BL = (size_t)B * L, BN = (size_t)B * N;
-  constexpr int XW = vc::ENC_OUT + vc::PRENET;   // 768: decoder input [cond | prenet(mel)]
-  float* e0 = ar.take<float>(BL * 256);
-  float* e1 = ar.take<float>(BL * 256);
-  float* zx = ar.take<float>(2 * BL * 1024);
-  float* enc = ar.take<float>(BL * 512);
-  float* xin = ar.take<float>(BN * XW);
-  float* pa = ar.take<float>(BN * 256);
-  float* pb = ar.take<float>(BN * 256);
-  float* zc0 = ar.take<float>(BN * 2048);
-  float* zc1 = ar.take<float>(BN * 2048);
-  float* hout = ar.take<float>(BN * 1024);
-  float* melpre = ar.take<float>(BN * 80);
-  float* q0 = ar.take<float>(BN * 512);
-  float* q1 = ar.take<float>(BN * 512);
-  float* h0s = ar.take<float>((size_t)2 * DEC_XR * 512);
-  float* h1s = ar.take<float>((size_t)2 * DEC_XR * 512);
-  if (measure) {
-    *ws_need = ar.off + 256;
-    return VTTS_OK;
-  }
-  auto& T = ctx->ac_t;
-  auto& D = ctx->ac_d;
-  ctx->tap_enc = enc; ctx->tap_enc_n = BL * 512;
+  const ModelWeights& m = ctx->ac;
+  const auto& T = m.t;
+  const auto& D = m.d;
+  ctx->tap_enc = w.e.enc; ctx->tap_enc_n = BL * 512;
   ctx->tap_cond = nullptr; ctx->tap_cond_n = 0;
-  ctx->tap_melpre = melpre; ctx->tap_melpre_n = BN * 80;
+  ctx->tap_melpre = w.melpre; ctx->tap_melpre_n = BN * 80;
   VTTS_CUDA(cudaMemsetAsync(mel2, 0, BN * 80 * sizeof(float), st));
   if (mel1) VTTS_CUDA(cudaMemsetAsync(mel1, 0, BN * 80 * sizeof(float), st));
-  VTTS_CUDA(cudaMemsetAsync(xin, 0, BN * XW * sizeof(float), st));
-  VTTS_CUDA(cudaMemsetAsync(melpre, 0, BN * 80 * sizeof(float), st));
+  VTTS_CUDA(cudaMemsetAsync(w.xin, 0, BN * XW * sizeof(float), st));
+  VTTS_CUDA(cudaMemsetAsync(w.melpre, 0, BN * 80 * sizeof(float), st));
   ctx->sub_mark(16, st);
-  {
-    EncWeights ew;
-    ew.embed = T[aci::EMBED];
-    for (int i = 0; i < 3; ++i) {
-      ew.conv_w[i] = T[aci::ENC_CONV(i, 0)]; ew.conv_b[i] = T[aci::ENC_CONV(i, 1)];
-      ew.bn_off[i] = T[aci::ENC_CONV(i, 3)]; ew.bn_mean[i] = T[aci::ENC_CONV(i, 4)]; ew.bn_inv[i] = D[D_ENC_BNINV0 + i];
-    }
-    ew.lf_w = T[aci::ENC_LSTM_F_W]; ew.lf_b = T[aci::ENC_LSTM_F_B]; ew.lb_w = T[aci::ENC_LSTM_B_W]; ew.lb_b = T[aci::ENC_LSTM_B_B];
-    ew.whr = D[D_ENC_WHR]; ew.wpk_conv = &ctx->ac_wpk_t[WP_ENC]; ew.wpk_hoist = &ctx->ac_wpk_t[WP_ENCH];
-    int rc = run_token_encoder(ctx, ew, tokens, lengths, B, L, e0, e1, zx, enc, st);
-    if (rc) return rc;
-  }
-  {  // cond -> columns 0..511 of the decoder input
-    dim3 grid((N + UP_F - 1) / UP_F, B);
-    size_t smem = (size_t)(L + UP_F * L) * sizeof(float);
-    if (smem > 200 * 1024) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: L=%d too long for the upsample kernel", L);
-    if (smem > 48 * 1024) VTTS_CUDA(cudaFuncSetAttribute(upsample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    upsample_kernel<<<grid, 256, smem, st>>>(enc, dur, lengths, n_frames, L, N, xin, XW);
-    ctx->launches++;
-    VTTS_CUDA(cudaGetLastError());
-  }
+  int rc = run_token_encoder(ctx, m, tokens, lengths, B, L, w.e, st);
+  if (rc) return rc;
+  rc = run_upsample(ctx, w.e.enc, dur, lengths, n_frames, B, L, N, w.xin, XW, st);   // cond -> columns 0..511 of the decoder input
+  if (rc) return rc;
   ctx->sub_mark(17, st);
   // ---- prenet over the whole sequence (model.py:95-100,149): two bias-free linears, relu, dropout 0.5 each ----
-  ConvLaunch Lc;
-  auto gemm = [&](const float* x, const float* w, const float* bias, float* out, int cin, int cout, int wp) {
-    memset(&Lc, 0, sizeof(Lc));
-    Lc.nprob = 1; Lc.Cin = cin; Lc.Cout = cout; Lc.B = 1; Lc.T_rows = (int)BN; Lc.rows_out = (int)BN;
-    Lc.pre_mode = 0; Lc.pre_slope = 1.f; Lc.post_act = 0; Lc.len_mul = 1;
-    Lc.p[0] = ConvProb{x, nullptr, nullptr, w, bias, nullptr, nullptr, nullptr, nullptr, out, 1, 1, 0, 1, 0};
-    return vtts_conv_dispatch(ctx, Lc, &ctx->ac_wpk_t[wp], st);     // tensor-core path in BF16X3 mode, FMA path in FP32 mode
-  };
   const size_t act_blocks = (BN * 256 + 255) / 256;
   const unsigned act_grid = (unsigned)(act_blocks < ctx->sm_count * 16 ? act_blocks : ctx->sm_count * 16);
-  int rc = gemm(mels_in, T[aci::PRE1_W], D[D_ZERO], pa, 80, 256, WP_PRE1);
+  const ConvProb pre1 = conv_prob(mels_in, T[aci::PRE1_W], D[D_ZERO], w.pa);
+  rc = run_convs(ctx, &pre1, 1, 80, 256, 1, (int)BN, nullptr, 0, m.tiles(PK_PRE1), st);
   if (rc) return rc;
-  prenet_act_kernel<<<act_grid, 256, 0, st>>>(pa, keep, seed, mode, 0, B, N, pb, 256);
+  prenet_act_kernel<<<act_grid, 256, 0, st>>>(w.pa, keep, seed, mode, 0, B, N, w.pb, 256);
   ctx->launches++;
-  rc = gemm(pb, T[aci::PRE2_W], D[D_ZERO], pa, 256, 256, WP_PRE2);
+  const ConvProb pre2 = conv_prob(w.pb, T[aci::PRE2_W], D[D_ZERO], w.pa);
+  rc = run_convs(ctx, &pre2, 1, 256, 256, 1, (int)BN, nullptr, 0, m.tiles(PK_PRE2), st);
   if (rc) return rc;
-  prenet_act_kernel<<<act_grid, 256, 0, st>>>(pa, keep, seed, mode, 1, B, N, xin + vc::ENC_OUT, XW);
+  prenet_act_kernel<<<act_grid, 256, 0, st>>>(w.pa, keep, seed, mode, 1, B, N, w.xin + vc::ENC_OUT, XW);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   // ---- every input-side product of both LSTMs in one launch: zc = [cond | p2] . W[0:768] + b ----
-  memset(&Lc, 0, sizeof(Lc));
-  Lc.nprob = 2; Lc.Cin = XW; Lc.Cout = 2048; Lc.B = 1; Lc.T_rows = (int)BN; Lc.rows_out = (int)BN;
-  Lc.pre_mode = 0; Lc.pre_slope = 1.f; Lc.post_act = 0; Lc.len_mul = 1;
-  Lc.p[0] = ConvProb{xin, nullptr, nullptr, T[aci::DEC_L0_W], T[aci::DEC_L0_B], nullptr, nullptr, nullptr, nullptr, zc0, 1, 1, 0, 1, 0};
-  Lc.p[1] = ConvProb{xin, nullptr, nullptr, T[aci::DEC_L1_W], T[aci::DEC_L1_B], nullptr, nullptr, nullptr, nullptr, zc1, 1, 1, 0, 1, 0};
-  rc = vtts_conv_dispatch(ctx, Lc, &ctx->ac_wpk_t[WP_TF_L0], st);      // tiles of problem 0 then problem 1: WP_TF_L0 .. WP_TF_L1+7
+  const ConvProb hp[2] = {conv_prob(w.xin, T[aci::DEC_L0_W], T[aci::DEC_L0_B], w.zc0), conv_prob(w.xin, T[aci::DEC_L1_W], T[aci::DEC_L1_B], w.zc1)};
+  rc = run_convs(ctx, hp, 2, XW, 2048, 1, (int)BN, nullptr, 0, m.tiles(PK_TF_L0), st);
   if (rc) return rc;
   ctx->sub_mark(18, st);
   // ---- zoneout scan, <= 32 rows per launch ----
@@ -1309,25 +1297,17 @@ int vtts_acoustic_teacher_run(vtts_ctx* ctx, const int32_t* tokens, const int32_
     const int nb = B - b0 < DEC_XR ? B - b0 : DEC_XR;
     TfScanArgs ta;
     memset(&ta, 0, sizeof(ta));
-    ta.zc0 = zc0 + (size_t)b0 * N * 2048; ta.zc1 = zc1 + (size_t)b0 * N * 2048;
+    ta.zc0 = w.zc0 + (size_t)b0 * N * 2048; ta.zc1 = w.zc1 + (size_t)b0 * N * 2048;
     ta.w0r = D[D_DEC_W0R]; ta.w1r = D[D_DEC_W1R];
     ta.zone = zone; ta.seed = seed; ta.mode = mode;
-    ta.h0s = h0s; ta.h1s = h1s; ta.hout = hout + (size_t)b0 * N * 1024;
+    ta.h0s = w.h0s; ta.h1s = w.h1s; ta.hout = w.hout + (size_t)b0 * N * 1024;
     ta.B = nb; ta.N = N; ta.row_base = b0;
     void* args[] = {&ta};
     VTTS_CUDA(cudaLaunchCooperativeKernel((void*)decoder_tf_scan_kernel, dim3(SCAN_CTAS), dim3(SCAN_THREADS), args, tf_scan_smem(), st));
     ctx->launches++;
   }
   ctx->sub_mark(19, st);
-  // ---- projection over all frames, then the postnet ----
-  memset(&Lc, 0, sizeof(Lc));
-  Lc.nprob = 1; Lc.Cin = 1024; Lc.Cout = 80; Lc.B = B; Lc.T_rows = N; Lc.rows_out = N;
-  Lc.len = n_frames; Lc.len_mul = 1; Lc.pre_mode = 0; Lc.pre_slope = 1.f; Lc.post_act = 0;      // rows past n_frames[b] stay 0
-  Lc.p[0] = ConvProb{hout, nullptr, nullptr, T[aci::PROJ_W], T[aci::PROJ_B], nullptr, nullptr, nullptr, nullptr, melpre, 1, 1, 0, 1, 0};
-  rc = vtts_conv_dispatch(ctx, Lc, &ctx->ac_wpk_t[WP_PROJ], st);
-  if (rc) return rc;
-  if (mel1) VTTS_CUDA(cudaMemcpyAsync(mel1, melpre, BN * 80 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  rc = run_postnet(ctx, melpre, n_frames, B, N, q0, q1, mel2, st);
+  rc = run_projection_postnet(ctx, w.hout, n_frames, B, N, w.melpre, w.q0, w.q1, mel1, -1, mel2, st);
   ctx->sub_mark(20, st);
   return rc;
 }
@@ -1375,93 +1355,47 @@ __global__ void __launch_bounds__(256) duration_head_kernel(const float* __restr
   if (lane == 0) dur[tok] = softplus(s + __ldg(b2));
 }
 
-enum { DU_BNINV0 = 0, DU_BNINV1, DU_BNINV2, DU_WHR, DU_COUNT };
-enum { DWP_ENC = 0, DWP_ENCH = 3, DWP_FC1 = 11, DWP_COUNT = 12 };
+// packing table of the duration model (ctx->du.tiles)
+enum { PK_DU_FC1 = PK_ENC_COUNT, PK_DU_COUNT };
 
 }  // namespace
 
 int vtts_duration_prepare(vtts_ctx* ctx) {
-  const size_t sizes[DU_COUNT] = {256, 256, 256, (size_t)2 * 64 * 256 * 16};
-  size_t total = 0;
-  std::vector<size_t> offs(DU_COUNT);
-  for (int i = 0; i < DU_COUNT; ++i) {
-    offs[i] = total;
-    total += (sizes[i] + 63) & ~size_t(63);
-  }
-  if (ctx->du_derived) cudaFree(ctx->du_derived);
-  VTTS_CUDA(cudaMalloc(&ctx->du_derived, total * sizeof(float)));
-  ctx->du_d.resize(DU_COUNT);
-  for (int i = 0; i < DU_COUNT; ++i) ctx->du_d[i] = ctx->du_derived + offs[i];
-  auto& T = ctx->du_t;
-  for (int i = 0; i < 3; ++i) bn_inv_kernel<<<1, 256>>>(T[aci::ENC_CONV(i, 2)], T[aci::ENC_CONV(i, 5)], ctx->du_d[DU_BNINV0 + i], 256);
-  repack_cols_kernel<<<256, 256>>>(T[aci::ENC_LSTM_F_W], 1024, 256, 256, ctx->du_d[DU_WHR], 64, 16, UPC, 256);
-  repack_cols_kernel<<<256, 256>>>(T[aci::ENC_LSTM_B_W], 1024, 256, 256, ctx->du_d[DU_WHR] + (size_t)64 * 256 * 16, 64, 16, UPC, 256);
+  ModelWeights& m = ctx->du;
+  std::vector<size_t> dn(D_ENC_COUNT);
+  std::vector<PackSpec> pk(PK_DU_COUNT);
+  encoder_tables(m, dn, pk);
+  pk[PK_DU_FC1] = {m.t[dui::FC1_W], 1, 512, 256};
+  int rc = vtts_alloc_tensors(ctx, dn, &m.derived, m.d);
+  if (rc) return rc;
+  encoder_derive(m);
   VTTS_CUDA(cudaGetLastError());
-  {
-    const size_t bytes = 3 * vtts_tc_conv_packed_bytes(3, 256, 256) + 2 * vtts_tc_conv_packed_bytes(1, 256, 1024) +
-                         vtts_tc_conv_packed_bytes(1, 512, 256);
-    if (ctx->du_wpk) cudaFree(ctx->du_wpk);
-    VTTS_CUDA(cudaMalloc(&ctx->du_wpk, bytes));
-    char* cur = (char*)ctx->du_wpk;
-    ctx->du_wpk_t.clear();
-    int rc = 0;
-    for (int i = 0; i < 3 && !rc; ++i) rc = vtts_tc_pack_conv(ctx, T[aci::ENC_CONV(i, 0)], 3, 256, 256, cur, ctx->du_wpk_t);
-    if (!rc) rc = vtts_tc_pack_conv(ctx, T[aci::ENC_LSTM_F_W], 1, 256, 1024, cur, ctx->du_wpk_t);
-    if (!rc) rc = vtts_tc_pack_conv(ctx, T[aci::ENC_LSTM_B_W], 1, 256, 1024, cur, ctx->du_wpk_t);
-    if (!rc) rc = vtts_tc_pack_conv(ctx, T[dui::FC1_W], 1, 512, 256, cur, ctx->du_wpk_t);
-    if (rc) return rc;
-    if ((int)ctx->du_wpk_t.size() != DWP_COUNT || (size_t)(cur - (char*)ctx->du_wpk) > bytes)
-      return ctx->fail(VTTS_ERR_BAD_ARG, "duration: packed weight table has %d entries", (int)ctx->du_wpk_t.size());
-  }
+  rc = vtts_pack_convs(ctx, m, pk);
+  if (rc) return rc;
   VTTS_CUDA(cudaDeviceSynchronize());
   VTTS_CUDA(cudaFuncSetAttribute(enc_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc_scan_smem()));
   return VTTS_OK;
 }
 
 int vtts_duration_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, int B, int L, float* dur_sec,
-                      cudaStream_t st, void* ws_base, size_t ws_cap, size_t* ws_need) {
-  const bool measure = ws_need != nullptr;
-  if (!measure) {
-    if (!ctx->du_loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "duration weights not loaded");
-    if (B < 1 || L < 1 || B > MAX_ROWS)
-      return ctx->fail(VTTS_ERR_BAD_ARG, "duration: B=%d L=%d (1 <= B <= %d rows per call; the host layer chunks larger batches)", B, L, MAX_ROWS);
-    if (ctx->sm_count < SCAN_CTAS) return ctx->fail(VTTS_ERR_NO_DEVICE, "scan kernels need %d SMs, device has %d", SCAN_CTAS, ctx->sm_count);
-  }
-  Arena ar(ws_base, ws_cap, measure);
+                      cudaStream_t st) {
+  if (!ctx->du.loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "duration weights not loaded");
+  if (B < 1 || L < 1 || B > MAX_ROWS)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "duration: B=%d L=%d (1 <= B <= %d rows per call; the host layer chunks larger batches)", B, L, MAX_ROWS);
+  if (ctx->sm_count < SCAN_CTAS) return ctx->fail(VTTS_ERR_NO_DEVICE, "scan kernels need %d SMs, device has %d", SCAN_CTAS, ctx->sm_count);
+  const DuBufs w = carve_ws<DuBufs>(ctx, B, L, 0);
   const size_t BL = (size_t)B * L;
-  float* e0 = ar.take<float>(BL * 256);
-  float* e1 = ar.take<float>(BL * 256);
-  float* zx = ar.take<float>(2 * BL * 1024);
-  float* enc = ar.take<float>(BL * 512);
-  float* y = ar.take<float>(BL * 256);
-  if (measure) {
-    *ws_need = ar.off + 256;
-    return VTTS_OK;
-  }
-  auto& T = ctx->du_t;
-  auto& D = ctx->du_d;
-  EncWeights ew;
-  ew.embed = T[aci::EMBED];
-  for (int i = 0; i < 3; ++i) {
-    ew.conv_w[i] = T[aci::ENC_CONV(i, 0)]; ew.conv_b[i] = T[aci::ENC_CONV(i, 1)];
-    ew.bn_off[i] = T[aci::ENC_CONV(i, 3)]; ew.bn_mean[i] = T[aci::ENC_CONV(i, 4)]; ew.bn_inv[i] = D[DU_BNINV0 + i];
-  }
-  ew.lf_w = T[aci::ENC_LSTM_F_W]; ew.lf_b = T[aci::ENC_LSTM_F_B]; ew.lb_w = T[aci::ENC_LSTM_B_W]; ew.lb_b = T[aci::ENC_LSTM_B_B];
-  ew.whr = D[DU_WHR]; ew.wpk_conv = &ctx->du_wpk_t[DWP_ENC]; ew.wpk_hoist = &ctx->du_wpk_t[DWP_ENCH];
+  const ModelWeights& m = ctx->du;
   // padded encoder rows are never written by the scan: clear them so the projection reads zeros, not stale workspace
-  VTTS_CUDA(cudaMemsetAsync(enc, 0, BL * 512 * sizeof(float), st));
-  int rc = run_token_encoder(ctx, ew, tokens, lengths, B, L, e0, e1, zx, enc, st);
+  VTTS_CUDA(cudaMemsetAsync(w.e.enc, 0, BL * 512 * sizeof(float), st));
+  int rc = run_token_encoder(ctx, m, tokens, lengths, B, L, w.e, st);
   if (rc) return rc;
-  ctx->tap_enc = enc; ctx->tap_enc_n = BL * 512;
+  ctx->tap_enc = w.e.enc; ctx->tap_enc_n = BL * 512;
   // ---- projection head ----
-  ConvLaunch Lc;
-  memset(&Lc, 0, sizeof(Lc));
-  Lc.nprob = 1; Lc.Cin = 512; Lc.Cout = 256; Lc.B = 1; Lc.T_rows = (int)BL; Lc.rows_out = (int)BL;
-  Lc.len = nullptr; Lc.len_mul = 1; Lc.pre_mode = 0; Lc.pre_slope = 1.f; Lc.post_act = 0;
-  Lc.p[0] = ConvProb{enc, nullptr, nullptr, T[dui::FC1_W], T[dui::FC1_B], nullptr, nullptr, nullptr, nullptr, y, 1, 1, 0, 1, 0};
-  rc = vtts_conv_dispatch(ctx, Lc, &ctx->du_wpk_t[DWP_FC1], st);
+  const ConvProb p = conv_prob(w.e.enc, m.t[dui::FC1_W], m.t[dui::FC1_B], w.y);
+  rc = run_convs(ctx, &p, 1, 512, 256, 1, (int)BL, nullptr, 0, m.tiles(PK_DU_FC1), st);
   if (rc) return rc;
-  duration_head_kernel<<<(unsigned)((BL + 7) / 8), 256, 0, st>>>(y, T[dui::FC2_W], T[dui::FC2_B], lengths, B, L, dur_sec);
+  duration_head_kernel<<<(unsigned)((BL + 7) / 8), 256, 0, st>>>(w.y, m.t[dui::FC2_W], m.t[dui::FC2_B], lengths, B, L, dur_sec);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   return VTTS_OK;

@@ -137,6 +137,21 @@ struct TcPairLaunch {
   long long* dbg;
 };
 
+// Device weights of one model: the checkpoint tensors, fp32 tensors derived from them at load, and the bf16 hi/lo
+// tensor-core packing of its convs (vtts_pack_convs).
+struct ModelWeights {
+  float* blob = nullptr;        // checkpoint tensors in canonical order, each 256 B aligned
+  std::vector<float*> t;
+  float* derived = nullptr;     // derived tensors (BN inverses, repacked weights, ...), same layout rules
+  std::vector<float*> d;
+  void* wpk = nullptr;          // packed convs
+  std::vector<void*> wpk_t;     // every N tile of every packed conv, in the order of the packing table
+  std::vector<int> tile0;       // index into wpk_t of the first tile of each entry of the packing table
+  bool loaded = false;
+  // the tiles of packing-table entry `conv`; the tiles of consecutive entries follow each other
+  void* const* tiles(int conv) const { return &wpk_t[tile0[conv]]; }
+};
+
 struct vtts_ctx {
   int device = 0;
   int precision = 1;            // 0 = strict fp32 (FMA pipe), 1 = bf16x3 on the tensor cores (wgmma, default)
@@ -146,10 +161,6 @@ struct vtts_ctx {
   int fuse_pairs = 1;              // 1 = ResBlock pairs with C <= 64 run in a fused pair kernel (intermediate stays on chip: 8 instead of 20 B of HBM traffic per element pair)
   int pair_ts = 2;                 // form of the fused pair kernel (tc_conv.cu): 2 = 256-row tiles (default), 1 = the same with
                                    // conv2's A operand in registers (register-A wgmma), 0 = 128-row tiles
-  void* hg_wpk = nullptr;       // packed tensor-core weights of the 72 resblock convs
-  std::vector<void*> hg_wpk_t;
-  std::vector<void*> hg_wpk_ups;   // [stage][phase] packed transposed-conv phase weights
-  void* hg_wpk_pre[2] = {nullptr, nullptr};  // conv_pre, two N=256 output tiles
   int sm_count = 0;
   int cc_major = 0, cc_minor = 0;
   size_t hbm_bytes = 0;
@@ -158,26 +169,9 @@ struct vtts_ctx {
   cudaStream_t own_stream = nullptr;   // used by the *_host entry points
 
   // ---- weights (device) ----
-  float* hg_blob = nullptr;     // haiku-layout tensors, each 256B aligned inside the arena
-  std::vector<float*> hg_t;     // tensor pointers in canonical order
-  float* hg_upsw = nullptr;     // transposed-conv weights repacked per output phase
-  bool hg_loaded = false;
-
-  float* ac_blob = nullptr;
-  std::vector<float*> ac_t;
-  void* ac_wpk = nullptr;       // packed tensor-core weights of the acoustic model's convs / hoisted GEMMs
-  std::vector<void*> ac_wpk_t;
-  float* ac_derived = nullptr;  // bn inv, repacked recurrent weights, ...
-  std::vector<float*> ac_d;
-  bool ac_loaded = false;
-
-  float* du_blob = nullptr;     // duration model (TokenEncoder + projection head), same layout rules as ac_*
-  std::vector<float*> du_t;
-  void* du_wpk = nullptr;
-  std::vector<void*> du_wpk_t;
-  float* du_derived = nullptr;
-  std::vector<float*> du_d;
-  bool du_loaded = false;
+  ModelWeights hg;              // HiFiGAN generator
+  ModelWeights ac;              // acoustic model
+  ModelWeights du;              // duration model (TokenEncoder + projection head)
 
   // mel filterbank + fft tables
   float* mel_fb = nullptr;      // dense [80][513]
@@ -260,25 +254,35 @@ int vtts_conv_dispatch(vtts_ctx* ctx, const ConvLaunch& L, void* const* wpk, cud
 // packs every N tile of one conv weight; returns the number of tiles, appends device pointers to `out`
 int vtts_tc_pack_conv(vtts_ctx* ctx, const float* w, int k, int Cin, int Cout, char*& cursor, std::vector<void*>& out);
 size_t vtts_tc_conv_packed_bytes(int k, int Cin, int Cout);
+// api.cu: weight slots
+void vtts_free_weights(ModelWeights& m);
+// replaces *store by one zero-filled device allocation holding tensors of n[i] floats, each 256 B aligned
+int vtts_alloc_tensors(vtts_ctx* ctx, const std::vector<size_t>& n, float** store, std::vector<float*>& ptrs);
+// one entry of a model's packing table: conv weight w[k][Cin][Cout]
+struct PackSpec { const float* w; int k, Cin, Cout; };
+// packs every N tile of every entry of `convs` (vtts_tc_pack_conv) into m.wpk and records m.wpk_t / m.tile0
+int vtts_pack_convs(vtts_ctx* ctx, ModelWeights& m, const std::vector<PackSpec>& convs);
 // hifigan.cu
 int vtts_hifigan_prepare(vtts_ctx* ctx);   // derived weights after load
 int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, int B, int T, float* wav, cudaStream_t st);
 size_t vtts_hifigan_ws_bytes(int B, int T);
-// nat.cu
+// nat.cu: the *_run functions carve ctx->ws, which the caller has sized by the matching *_ws_bytes
 int vtts_acoustic_prepare(vtts_ctx* ctx);
+size_t vtts_acoustic_ws_bytes(int B, int L, int N);
 int vtts_acoustic_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const float* dur,
                       const int32_t* n_frames, const uint8_t* keep, int mode, uint64_t seed, int B, int L, int N,
-                      float* mel, cudaStream_t st, void* ws_base, size_t ws_cap, size_t* ws_need);
-// melspec.cu
-int vtts_melspec_prepare(vtts_ctx* ctx);
+                      float* mel, cudaStream_t st);
+size_t vtts_acoustic_teacher_ws_bytes(int B, int L, int N);
 int vtts_acoustic_teacher_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const float* dur,
                               const int32_t* n_frames, const float* mels_in, const uint8_t* keep, const uint8_t* zone, int mode,
-                              uint64_t seed, int B, int L, int N, float* mel1, float* mel2, cudaStream_t st, void* ws_base,
-                              size_t ws_cap, size_t* ws_need);
+                              uint64_t seed, int B, int L, int N, float* mel1, float* mel2, cudaStream_t st);
 int vtts_duration_prepare(vtts_ctx* ctx);
+size_t vtts_duration_ws_bytes(int B, int L);
 // DurationModel.__call__ (model.py:64-70); dur_sec [B][L] seconds, 0 past lengths[b]
 int vtts_duration_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, int B, int L, float* dur_sec,
-                      cudaStream_t st, void* ws_base, size_t ws_cap, size_t* ws_need);
+                      cudaStream_t st);
+// melspec.cu
+int vtts_melspec_prepare(vtts_ctx* ctx);
 int vtts_melspec_run(vtts_ctx* ctx, const float* wav, int B, int S, float* mel, cudaStream_t st);
 
 // canonical blob layouts (weights.cu)
@@ -287,7 +291,7 @@ const std::vector<TensorSpec>& vtts_hifigan_specs();
 const std::vector<TensorSpec>& vtts_acoustic_specs();
 const std::vector<TensorSpec>& vtts_duration_specs();
 
-// indices into ctx->hg_t  (canonical order: pre, ups 0..3, resblocks 0..11 x (c1_0,c1_1,c1_2,c2_0,c2_1,c2_2), post)
+// indices into ctx->hg.t  (canonical order: pre, ups 0..3, resblocks 0..11 x (c1_0,c1_1,c1_2,c2_0,c2_1,c2_2), post)
 namespace hgi {
 constexpr int PRE_W = 0, PRE_B = 1;
 __host__ __device__ constexpr int UPS_W(int i) { return 2 + 2 * i; }
@@ -299,7 +303,7 @@ constexpr int POST_W = 10 + 12 * 12, POST_B = POST_W + 1;
 constexpr int COUNT = POST_B + 1;
 }  // namespace hgi
 
-// indices into ctx->ac_t
+// indices into ctx->ac.t
 namespace aci {
 constexpr int EMBED = 0;
 // encoder conv i: w, b, bn_scale, bn_offset, bn_mean, bn_var
@@ -312,7 +316,7 @@ __host__ __device__ constexpr int POST_CONV(int i, int f) { return 31 + i * 6 + 
 constexpr int COUNT = 31 + 4 * 6 + 2;
 }  // namespace aci
 
-// indices into ctx->du_t (duration model): the TokenEncoder block has the acoustic model's layout (aci::EMBED ..
+// indices into ctx->du.t (duration model): the TokenEncoder block has the acoustic model's layout (aci::EMBED ..
 // aci::ENC_LSTM_B_B), followed by the projection head hk.Sequential([Linear(256), gelu, Linear(1)]) (model.py:60-62)
 namespace dui {
 constexpr int FC1_W = 23, FC1_B = 24, FC2_W = 25, FC2_B = 26;

@@ -138,31 +138,26 @@ class Engine:
         return {name: float(out[i]) for i, name in self.SUBSTAGES.items() if out[i] > 0}
 
     # ---- weights ----
+    def _load(self, fn, pack, src):
+        blob = pack(src) if isinstance(src, dict) else src
+        n = int(blob.size if isinstance(blob, np.ndarray) else blob.numel())
+        if isinstance(blob, np.ndarray):
+            blob = _np(blob, np.float32)
+        self._ck(fn(self.h, _ptr(blob), n))
+
     def load_hifigan(self, params, key=None):
         """params: Haiku-layout dict, a packed float32 numpy blob, or a torch CUDA
         tensor holding the blob (e.g. received through an NCCL broadcast)."""
-        blob = weights.pack_hifigan(params) if isinstance(params, dict) else params
-        n = int(blob.size if isinstance(blob, np.ndarray) else blob.numel())
-        if isinstance(blob, np.ndarray):
-            blob = _np(blob, np.float32)
-        self._ck(self.lib.vtts_load_hifigan(self.h, _ptr(blob), n))
+        self._load(self.lib.vtts_load_hifigan, weights.pack_hifigan, params)
         self._hifigan_key = key if key is not None else object()
 
     def load_acoustic(self, ckpt, key=None):
-        blob = weights.pack_acoustic(ckpt) if isinstance(ckpt, dict) else ckpt
-        n = int(blob.size if isinstance(blob, np.ndarray) else blob.numel())
-        if isinstance(blob, np.ndarray):
-            blob = _np(blob, np.float32)
-        self._ck(self.lib.vtts_load_acoustic(self.h, _ptr(blob), n))
+        self._load(self.lib.vtts_load_acoustic, weights.pack_acoustic, ckpt)
         self._acoustic_key = key if key is not None else object()
 
     def load_duration(self, ckpt, key=None):
         """ckpt: the duration checkpoint dict (params/aux), a packed numpy blob, or a torch CUDA tensor."""
-        blob = weights.pack_duration(ckpt) if isinstance(ckpt, dict) else ckpt
-        n = int(blob.size if isinstance(blob, np.ndarray) else blob.numel())
-        if isinstance(blob, np.ndarray):
-            blob = _np(blob, np.float32)
-        self._ck(self.lib.vtts_load_duration(self.h, _ptr(blob), n))
+        self._load(self.lib.vtts_load_duration, weights.pack_duration, ckpt)
         self._duration_key = key if key is not None else object()
 
     def broadcast_weights(self, nccl_comm, root: int, is_root: bool, stream=None):

@@ -331,6 +331,11 @@ int vtts_create(int device, vtts_ctx** out) {
     delete ctx;
     return VTTS_ERR_CUDA;
   }
+  if (cudaMalloc(&ctx->d_tc_sched, 2 * sizeof(int)) != cudaSuccess || cudaMemset(ctx->d_tc_sched, 0, 2 * sizeof(int)) != cudaSuccess) {
+    g_vtts_create_error = "vtts_create: cannot allocate the tile scheduler counters";
+    delete ctx;
+    return VTTS_ERR_CUDA;
+  }
   if (cudaMalloc(&ctx->d_tc_dbg, 256 * 16 * sizeof(long long)) != cudaSuccess) {
     g_vtts_create_error = "vtts_create: cannot allocate the profiling counters";
     delete ctx;
@@ -347,7 +352,7 @@ int vtts_destroy(vtts_ctx* ctx) {
   cudaDeviceSynchronize();
   for (auto& m : kModels) vtts_free_weights(ctx->*m.w);
   cudaFree(ctx->mel_fb); cudaFree(ctx->mel_lo); cudaFree(ctx->mel_hi); cudaFree(ctx->fft_tw); cudaFree(ctx->hann);
-  cudaFree(ctx->ws); cudaFree(ctx->dstage); cudaFree(ctx->d_err); cudaFree(ctx->d_tc_dbg);
+  cudaFree(ctx->ws); cudaFree(ctx->dstage); cudaFree(ctx->d_err); cudaFree(ctx->d_tc_sched); cudaFree(ctx->d_tc_dbg);
   if (ctx->hpin) cudaFreeHost(ctx->hpin);
   for (int i = 0; i < vtts_ctx::NSTAGE; ++i) {
     cudaEventDestroy(ctx->ev0[i]);

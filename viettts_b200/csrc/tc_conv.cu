@@ -45,6 +45,8 @@ constexpr int NTHREADS = NCONS + 32 + NCONV;  // 384
 constexpr int NA = 4;                         // activation stages
 constexpr int HALO = 64;                      // staged rows beyond the tile: dilation * (k - 1) <= 64
 constexpr int PAIR_OVERLAP = 16;              // pair kernel: rows per tile that only feed conv2's halo (k - 1 <= 16)
+constexpr int NQ = 2;                         // tile-id ring slots
+constexpr int NREADERS = (NCONS + NCONV) / 32;  // warps that read the tile-id ring
 
 template <int N, int MW, int PAIRF>
 struct TcCfg {
@@ -55,7 +57,7 @@ struct TcCfg {
   static constexpr int W_STAGE = N * 64;                    // bytes of one packed (chunk, tap) weight block
   static constexpr int NW = N == 256 ? 4 : 8;               // weight stages
   static constexpr int NCH2 = PAIRF ? N / 16 : 0;           // 16-channel chunks of the on-chip intermediate
-  static constexpr int SMEM_BYTES = NA * A_STAGE + NW * W_STAGE + NCH2 * A_STAGE + (2 * NA + 2 * NW) * 8 + 1024;
+  static constexpr int SMEM_BYTES = NA * A_STAGE + NW * W_STAGE + NCH2 * A_STAGE + (2 * NA + 2 * NW + 2 * NQ) * 8 + NQ * 4 + 1024;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one CTA");
 };
 
@@ -63,6 +65,67 @@ struct Ring {
   uint32_t s = 0, p = 0;
   template <int NS>
   __device__ __forceinline__ void next() { if (++s == NS) { s = 0; p ^= 1; } }
+};
+
+// Tiles are handed out at run time.  A tile's cost depends on its problem (k taps, skipped rows past a row's length),
+// so a fixed tile -> CTA map leaves SMs idle: with 132 CTAs and 3 problems, tile % 3 == blockIdx.x % 3 and each CTA
+// would run one problem only.  The weight-producer lane of each CTA takes tickets from a launch-wide counter and passes
+// every ticket on to the CTA's other roles through the NQ-slot tile-id ring (-1 ends the launch).
+//
+// Ticket order is (batch row, row tile) major, problem, then output phase minor, with the problems sorted by k,
+// descending: CTAs running at the same time work on the same rows, so an input several problems share (the first pair
+// of a ResBlock stage, the ConvTranspose problems) is read from DRAM once and served from L2 to the others.
+struct Tile {
+  int pi, b, tt, ph;   // problem, batch row, row tile, output phase
+};
+__device__ __forceinline__ Tile decode_tile(int t, int nph, int nprob, int tiles_per_row) {
+  Tile d;
+  d.ph = t % nph; t /= nph;
+  d.pi = t % nprob; t /= nprob;
+  d.tt = t % tiles_per_row;
+  d.b = t / tiles_per_row;
+  return d;
+}
+
+// next ticket, or -1 once the launch's tiles are gone.  Tile blockIdx.x is every CTA's first (grid <= ntiles), so no
+// CTA waits for the counter to start; the counter hands out tiles gridDim.x onwards.  The last CTA to run out zeroes
+// both counters for the next launch (launches of a context are stream-ordered, and every CTA has taken its last ticket
+// by then).
+__device__ __forceinline__ int take_ticket(int* sched, int ntiles) {
+  const int t = (int)gridDim.x + atomicAdd(&sched[0], 1);
+  if (t < ntiles) return t;
+  __threadfence();
+  if (atomicAdd(&sched[1], 1) == (int)gridDim.x - 1) {
+    atomicExch(&sched[0], 0);
+    atomicExch(&sched[1], 0);
+  }
+  return -1;
+}
+
+struct TileQueue {
+  int* id;
+  uint64_t* full;    // producer lane arrives after writing id[s]
+  uint64_t* empty;   // lane 0 of every reader warp arrives once it has read id[s]
+  Ring r;
+  // producer lane: publish ticket t (or -1)
+  __device__ __forceinline__ void put(int t, int* err, long long& acc) {
+    mbar_wait_t(&empty[r.s], r.p ^ 1, err, 6, acc);
+    id[r.s] = t;
+    mbar_arrive(&full[r.s]);
+    r.next<NQ>();
+  }
+  // whole reader warp: the next tile id; the slot is released at once, so the ring only bounds how far the producer
+  // runs ahead
+  __device__ __forceinline__ int get(int* err, long long& acc) {
+    int t = 0;
+    if ((threadIdx.x & 31) == 0) {
+      mbar_wait_t(&full[r.s], r.p, err, 6, acc);
+      t = id[r.s];
+      mbar_arrive(&empty[r.s]);
+    }
+    r.next<NQ>();
+    return __shfl_sync(0xffffffffu, t, 0);
+  }
 };
 
 // converters: fill A stage `stage` with rows [row_base, row_base + rows) of channels [c*16, c*16+16) of x0 (+x1+x2)/3,
@@ -207,15 +270,41 @@ __device__ __forceinline__ void consume(float (&acc)[MW][N / 2], int wg, uint32_
   }
 }
 
+// barriers: a_full[NA] a_empty[NA] w_full[nw] w_empty[nw] q_full[NQ] q_empty[NQ], then the NQ tile ids
 __device__ __forceinline__ void init_barriers(uint64_t* bars, int nw) {
   uint64_t* a_full = bars;
   uint64_t* a_empty = bars + NA;
   uint64_t* w_full = bars + 2 * NA;
   uint64_t* w_empty = bars + 2 * NA + nw;
+  uint64_t* q_full = bars + 2 * NA + 2 * nw;
+  uint64_t* q_empty = q_full + NQ;
   for (int i = 0; i < NA; ++i) { mbar_init(&a_full[i], NCONV); mbar_init(&a_empty[i], NCONS / 32); }
   for (int i = 0; i < nw; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], NCONS / 32); }
+  for (int i = 0; i < NQ; ++i) { mbar_init(&q_full[i], 1); mbar_init(&q_empty[i], NREADERS); }
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
+
+__device__ __forceinline__ TileQueue tile_queue(uint64_t* bars, int nw) {
+  uint64_t* q_full = bars + 2 * NA + 2 * nw;
+  return TileQueue{reinterpret_cast<int*>(q_full + 2 * NQ), q_full, q_full + NQ, Ring{}};
+}
+
+// Tile loops of the roles.  The producer lane takes tickets one tile ahead of the tile it streams weights for, so the
+// converters learn their next tile before they finish the current one.
+#define PRODUCER_TILES                                                                     \
+  TileQueue q = tile_queue(bars, NW);                                                      \
+  long long w_q = 0;                                                                       \
+  int t_next = blockIdx.x;                                                                 \
+  q.put(t_next, L.err, w_q);                                                               \
+  auto next_tile = [&]() {                                                                 \
+    const int t = t_next;                                                                  \
+    if (t >= 0) { t_next = take_ticket(L.sched, L.ntiles); q.put(t_next, L.err, w_q); }    \
+    return t;                                                                              \
+  };
+#define READER_TILES                                                                       \
+  TileQueue q = tile_queue(bars, NW);                                                      \
+  long long w_q = 0;                                                                       \
+  auto next_tile = [&]() { return q.get(L.err, w_q); };
 
 // EPI = 0: bias (+ residual) only -- the HiFiGAN generator's hot path.  EPI = 1: bias, eval BatchNorm,
 // tanh / relu, residual, partial N tile (acoustic model convs and GEMMs).
@@ -240,26 +329,20 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
 
   const int nch = L.Cin / 16;
   const int nph = L.nphase > 1 ? L.nphase : 1;
-  const int tiles_per_row = L.tiles_per_row;
-  const int tiles_per_prob = tiles_per_row * L.B;
 
-  // every role walks the same tile sequence; a tile is (problem, batch row, row tile, output phase)
+  // every role walks the same tile sequence (next_tile); a tile is (problem, batch row, row tile, output phase)
 #define TILE_LOOP_BEGIN                                                           \
-  for (int tile = blockIdx.x; tile < L.ntiles; tile += gridDim.x) {               \
-    const int ph = tile % nph;                                                    \
-    const int t2 = tile / nph;                                                    \
-    const int pi = L.problem_major ? t2 / tiles_per_prob : t2 % L.nprob;          \
-    const int rest = L.problem_major ? t2 - pi * tiles_per_prob : t2 / L.nprob;   \
-    const int tt = rest % tiles_per_row;                                          \
-    const int b = rest / tiles_per_row;                                           \
-    const int tau0 = tt * R;                                                      \
+  for (int tile; (tile = next_tile()) >= 0;) {                                    \
+    const Tile td = decode_tile(tile, nph, L.nprob, L.tiles_per_row);              \
+    const int ph = td.ph, b = td.b;                                                 \
+    const int tau0 = td.tt * R;                                                    \
     int valid = L.T_rows;                                                         \
     if (L.len) {                                                                  \
       const int v = L.len[b] * L.len_mul;                                         \
       valid = v < valid ? v : valid;                                              \
     }                                                                             \
     if (tau0 >= valid) continue;                                                  \
-    const TcProb& P = L.p[pi];
+    const TcProb& P = L.p[td.pi];
 #define TILE_LOOP_END }
 
   if (warp == PROD_WARP) {
@@ -267,6 +350,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
     if ((tid & 31) == 0) {
       Ring rw;
       long long w_e = 0;
+      PRODUCER_TILES
       TILE_LOOP_BEGIN
         (void)b; (void)tau0;
         produce_weights<N, NW>(w_st, w_full, w_empty, rw, P.wpk_ph[ph], nch, P.k, L.err, w_e);
@@ -278,6 +362,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
     const int ct = tid - NCONS - 32;
     Ring ra;
     long long w_ae = 0;
+    READER_TILES
     TILE_LOOP_BEGIN
       const int k = P.k, dil = P.dil;
       const size_t in_base = (size_t)b * L.T_rows * L.in_ld;
@@ -302,6 +387,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
     const long long t_begin = clock64();
     const int n_valid = (EPI && L.n_valid > 0) ? L.n_valid : N;
     const int post_act = EPI ? L.post_act : 0;
+    READER_TILES
     TILE_LOOP_BEGIN
       consume<N, MW, RA, NW, true>(acc, wg, smem_u32(a_st), a_full, a_empty, ra, smem_u32(w_st), w_full, w_empty, rw, nch, P.k, P.dil,
                                    L.err, w_a, w_w);
@@ -370,22 +456,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_pair_kernel(const __grid_const
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
   if (tid == 0) init_barriers(bars, NW);
   __syncthreads();
-  const int tiles_per_row = L.tiles_per_row[0];
 
 #define TILE_LOOP_BEGIN                                                   \
-  for (int tile = blockIdx.x; tile < L.ntiles; tile += gridDim.x) {       \
-    const int pi = tile % L.nprob;                                        \
-    const int rest = tile / L.nprob;                                      \
-    const int tt = rest % tiles_per_row;                                  \
-    const int b = rest / tiles_per_row;                                   \
-    const int tau0 = tt * R_OUT;                                          \
+  for (int tile; (tile = next_tile()) >= 0;) {                            \
+    const Tile td = decode_tile(tile, 1, L.nprob, L.tiles_per_row);        \
+    const int b = td.b;                                                    \
+    const int tau0 = td.tt * R_OUT;                                        \
     int valid = L.T_rows;                                                 \
     if (L.len) {                                                          \
       const int v = L.len[b] * L.len_mul;                                 \
       valid = v < valid ? v : valid;                                      \
     }                                                                     \
     if (tau0 >= valid) continue;                                          \
-    const TcPairProb& P = L.p[pi];                                        \
+    const TcPairProb& P = L.p[td.pi];                                      \
     const int k = P.k, dil = P.dil, h2 = (k - 1) / 2;
 #define TILE_LOOP_END }
 
@@ -393,6 +476,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_pair_kernel(const __grid_const
     if ((tid & 31) == 0) {
       Ring rw;
       long long w_e = 0;
+      PRODUCER_TILES
       TILE_LOOP_BEGIN
         (void)b; (void)tau0; (void)dil; (void)h2;
         produce_weights<N, NW>(w_st, w_full, w_empty, rw, P.w1pk, NCH, k, L.err, w_e);
@@ -403,6 +487,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_pair_kernel(const __grid_const
     const int ct = tid - NCONS - 32;
     Ring ra;
     long long w_ae = 0;
+    READER_TILES
     TILE_LOOP_BEGIN
       const float* x = P.x + (size_t)b * L.T_rows * N;
       const int row_base = tau0 - h2 - (k - 1) * dil / 2;
@@ -419,7 +504,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_pair_kernel(const __grid_const
     float acc[MW][N / 2];
     Ring ra, rw;
     long long w_a = 0, w_w = 0;
+    const long long t_begin = clock64();
     const float slope = L.slope;
+    READER_TILES
     TILE_LOOP_BEGIN
       // ---- conv1 over the R intermediate rows ----
       consume<N, MW, RA, NW, true>(acc, wg, smem_u32(a_st), a_full, a_empty, ra, smem_u32(w_st), w_full, w_empty, rw, NCH, k, dil, L.err,
@@ -474,7 +561,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_pair_kernel(const __grid_const
           }
         }
     TILE_LOOP_END
-    if (L.dbg && tid == 0) { L.dbg[(size_t)blockIdx.x * 16 + 2] = w_a; L.dbg[(size_t)blockIdx.x * 16 + 3] = w_w; }
+    if (L.dbg && tid == 0) {
+      long long* d = L.dbg + (size_t)blockIdx.x * 16;
+      d[0] = clock64() - t_begin; d[2] = w_a; d[3] = w_w;
+    }
   }
 #undef TILE_LOOP_BEGIN
 #undef TILE_LOOP_END
@@ -515,8 +605,7 @@ int launch_cfg(vtts_ctx* ctx, TcLaunch& L, cudaStream_t st) {
     }
     if ((L.p[i].k - 1) * L.p[i].dil > HALO) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: halo too large");
   }
-  // static round-robin tile assignment: put the expensive problems (large k) first so that the last, partial
-  // wave of tiles consists of cheap ones
+  // the expensive problems (large k) first: within each row tile they are handed out before the cheap ones
   std::stable_sort(L.p, L.p + L.nprob, [](const TcProb& a, const TcProb& b) { return a.k > b.k; });
   L.tiles_per_row = (L.T_rows + Cfg::R - 1) / Cfg::R;
   L.ntiles = L.nprob * L.tiles_per_row * L.B * nph;
@@ -548,10 +637,10 @@ int launch_pair(vtts_ctx* ctx, TcPairLaunch& L, cudaStream_t st) {
   }
   for (int i = 0; i < L.nprob; ++i)
     if (L.p[i].k - 1 > PAIR_OVERLAP || (L.p[i].k - 1) * L.p[i].dil > HALO) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_pair: halo too large");
-  // expensive problems (large k) first: the last, partial wave of tiles is made of cheap ones
+  // expensive problems (large k) first: within each row tile they are handed out before the cheap ones
   std::stable_sort(L.p, L.p + L.nprob, [](const TcPairProb& a, const TcPairProb& b) { return a.k > b.k; });
-  for (int i = 0; i < 3; ++i) { L.tile_start[i] = 0; L.tiles_per_row[i] = (L.T_rows + Cfg::R_OUT - 1) / Cfg::R_OUT; }
-  L.ntiles = L.nprob * L.tiles_per_row[0] * L.B;
+  L.tiles_per_row = (L.T_rows + Cfg::R_OUT - 1) / Cfg::R_OUT;
+  L.ntiles = L.nprob * L.tiles_per_row * L.B;
   const int grid = L.ntiles < ctx->sm_count ? L.ntiles : ctx->sm_count;
   tc_pair_kernel<N, MW, A2_REGS><<<grid, NTHREADS, Cfg::SMEM_BYTES, st>>>(L);
   ctx->launches++;
@@ -640,13 +729,9 @@ int vtts_launch_tc_conv(vtts_ctx* ctx, TcLaunch& L, cudaStream_t st) {
   if (L.Cin % 16 != 0) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: Cin %d", L.Cin);
   for (int i = 0; i < L.nprob; ++i)
     if (L.p[i].k < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: k");
+  L.sched = ctx->d_tc_sched;
   L.err = ctx->d_err;
   L.dbg = ctx->tc_dbg_on ? ctx->d_tc_dbg : nullptr;
-  {
-    static int pm_env = -1;    // experiment switch: VTTS_TC_PROBLEM_MAJOR=0/1 forces the tile map of every launch
-    if (pm_env < 0) { const char* e = getenv("VTTS_TC_PROBLEM_MAJOR"); pm_env = e ? atoi(e) + 1 : 0; }
-    if (pm_env > 0) L.problem_major = pm_env - 1;
-  }
   switch (L.N) {
     case 256: return launch_n<256>(ctx, L, st);
     case 128: return launch_n<128>(ctx, L, st);
@@ -660,6 +745,7 @@ int vtts_launch_tc_pair(vtts_ctx* ctx, TcPairLaunch& L, cudaStream_t st) {
   if (L.nprob < 1 || L.nprob > 3) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_pair: nprob %d", L.nprob);
   for (int i = 0; i < L.nprob; ++i)
     if (L.p[i].k < 1 || L.p[i].x == L.p[i].out) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_pair: bad problem %d", i);
+  L.sched = ctx->d_tc_sched;
   L.err = ctx->d_err;
   L.dbg = ctx->tc_dbg_on ? ctx->d_tc_dbg : nullptr;
   if (L.N != 32 && L.N != 64) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_pair: C %d unsupported (32 or 64)", L.N);

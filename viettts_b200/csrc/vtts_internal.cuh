@@ -105,10 +105,7 @@ struct TcLaunch {
   int post_act;          // 0 none, 1 tanh, 2 relu (after BN, before the residual)
   int n_valid;           // real output channels of this N tile (<= N); 0 means N
   int tiles_per_row, ntiles;  // filled by the launcher
-  int problem_major;          // tile -> problem map.  0 (default): round robin (problem = tile % nprob): row tile r of every problem
-                              // is in flight at the same time, so an input / residual tensor the problems SHARE (the first pair
-                              // of every ResBlock stage, the ConvTranspose phases) is read from DRAM once and served from L2 to
-                              // the others: generator 19.8 -> 19.1 ms.  1: problems back to back (experiments only)
+  int* sched;                 // device int[2]: the run-time tile scheduler's counters (vtts_ctx::d_tc_sched)
   int* err;                   // device int: set before trapping on a barrier timeout
   long long* dbg;             // optional [grid][16] per-role stall counters (vtts_debug_tc_stats)
 };
@@ -132,7 +129,8 @@ struct TcPairLaunch {
   const int* len;
   int len_mul;
   float slope;
-  int tile_start[3], tiles_per_row[3], ntiles;   // filled by the launcher
+  int tiles_per_row, ntiles;   // filled by the launcher
+  int* sched;
   int* err;
   long long* dbg;
 };
@@ -156,6 +154,10 @@ struct vtts_ctx {
   int device = 0;
   int precision = 1;            // 0 = strict fp32 (FMA pipe), 1 = bf16x3 on the tensor cores (wgmma, default)
   int* d_err = nullptr;
+  // tile scheduler counters of the tensor-core launches: [0] next ticket, [1] CTAs done taking tickets.  Each launch
+  // leaves them at zero.  One pair serves every launch of the context because a context's tensor-core launches never
+  // overlap: they run in order on the one stream of the call that issues them (calls share the workspace, too).
+  int* d_tc_sched = nullptr;
   long long* d_tc_dbg = nullptr;   // [256][16] profiling counters of the last tensor-core conv launch
   bool tc_dbg_on = false;
   int fuse_pairs = 1;              // 1 = ResBlock pairs with C <= 64 run in a fused pair kernel (intermediate stays on chip: 8 instead of 20 B of HBM traffic per element pair)

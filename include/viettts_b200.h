@@ -59,8 +59,15 @@ typedef enum vtts_dropout_mode {
  *   FP32    every product and sum in IEEE fp32 on the FMA pipe (conv1d.cu) -- the strict parity mode
  *   BF16X3  wgmma tensor cores, each fp32 operand split into bf16 hi+lo, three products
  *           (hi*hi + hi*lo + lo*hi) accumulated in fp32 registers (tc_conv.cu); fp32-class accuracy
- *           (waveform L-inf 2e-5 vs float64), no reduced-precision storage anywhere. */
-typedef enum vtts_precision { VTTS_PRECISION_FP32 = 0, VTTS_PRECISION_BF16X3 = 1 } vtts_precision;
+ *           (waveform L-inf 2e-5 vs float64), no reduced-precision storage anywhere.
+ *   FP16    fast mode for the HiFiGAN generator only: its tensor-core convs (conv_pre, the ConvTranspose phases, the 72
+ *           ResBlock convs) take each operand as ONE fp16 value (round to nearest, saturated to +-65504, never inf) and
+ *           issue one wgmma product instead of three, fp32 accumulate.  Stated tolerance: waveform L-inf <= 3e-3 and RMS
+ *           <= 6e-4 against float64 (about 60 dB below the signal), established on synthetic weights; the activation
+ *           range of a real checkpoint is not verified.  conv_post, MelFilter and the acoustic, duration, teacher-forced
+ *           and GTA paths run exactly as in BF16X3 (their error compounds through the autoregressive scan).  The fused
+ *           ResBlock-pair forms other than the default reject this mode with VTTS_ERR_BAD_ARG. */
+typedef enum vtts_precision { VTTS_PRECISION_FP32 = 0, VTTS_PRECISION_BF16X3 = 1, VTTS_PRECISION_FP16 = 2 } vtts_precision;
 
 /* ---- library / context ------------------------------------------------------------ */
 int vtts_version(void);                                  /* ABI version, currently 1 */
@@ -137,14 +144,16 @@ int vtts_melspec(vtts_ctx* ctx, const float* wav_dev, int B, int S, float* mel_d
 int vtts_debug_read(vtts_ctx* ctx, const char* name, float* host_out, int64_t n_floats);
 
 /* test hook: one hk.Conv1D (SAME padding, dilation, optional leaky_relu on the input and residual
- * add) on device buffers through either arithmetic path.  x [B,T,Cin], w Haiku layout [k,Cin,Cout],
+ * add) on device buffers through any arithmetic path (`precision` a vtts_precision; FP16 packs the weights as the
+ * generator's fp16 plane).  x [B,T,Cin], w Haiku layout [k,Cin,Cout],
  * out/resid [B,T,Cout]; len int32 [B] or NULL; pre_slope 1.0 = no input activation.  Synchronous. */
 int vtts_debug_conv1d(vtts_ctx* ctx, int precision, const float* x_dev, const float* w_dev, const float* bias_dev,
                       const float* resid_dev, const int32_t* len_dev, int B, int T, int Cin, int Cout, int k, int dil,
                       float pre_slope, float* out_dev);
 
 /* test hook: one fused ResBlock pair  out = conv2(lrelu(conv1(lrelu(x)) + b1)) + b2 + x  (vietTTS/hifigan/model.py:44-51)
- * on the tensor-core path; x/out [B,T,C] with C in {32,64}, w1/w2 Haiku layout [k,C,C], conv1 dilation `dil`. Synchronous. */
+ * on the tensor-core path; x/out [B,T,C] with C in {32,64}, w1/w2 Haiku layout [k,C,C], conv1 dilation `dil`. Synchronous.
+ * Runs on fp16 operands when the context is in VTTS_PRECISION_FP16, on bf16x3 otherwise. */
 int vtts_debug_pair(vtts_ctx* ctx, const float* x_dev, const float* w1_dev, const float* b1_dev, const float* w2_dev,
                     const float* b2_dev, const int32_t* len_dev, int B, int T, int C, int k, int dil, float slope, float* out_dev);
 

@@ -29,6 +29,14 @@ def _tf32(x):
     return i.view(torch.float32).to(torch.float64)
 
 
+FP16_MAX = 65504.0
+
+
+def _fp16(x):
+    # saturating, like the kernels' conversions (cvt.rn.satfinite): a value past the fp16 range becomes +-65504, not inf
+    return x.to(torch.float32).clamp(-FP16_MAX, FP16_MAX).to(torch.float16).to(torch.float64)
+
+
 def split(x, rnd, terms):
     """x -> [x0, x1, ...] with x0 = rnd(x), x1 = rnd(x - x0), ..."""
     out, rest = [], x.to(torch.float64)
@@ -44,6 +52,7 @@ MODES = {
     "fp32": (None, 1, None),
     "bf16x1": (_bf16, 1, [(0, 0)]),
     "tf32x1": (_tf32, 1, [(0, 0)]),
+    "fp16x1": (_fp16, 1, [(0, 0)]),
     "bf16x3": (_bf16, 2, [(0, 0), (0, 1), (1, 0)]),
     "tf32x3": (_tf32, 2, [(0, 0), (0, 1), (1, 0)]),
     "bf16x6": (_bf16, 3, [(0, 0), (0, 1), (1, 0), (1, 1), (0, 2), (2, 0)]),

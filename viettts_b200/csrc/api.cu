@@ -189,7 +189,7 @@ int vtts_pack_convs(vtts_ctx* ctx, ModelWeights& m, const std::vector<PackSpec>&
   size_t bytes = 0;
   for (auto& c : convs) {
     if (!c.w) return ctx->fail(VTTS_ERR_BAD_ARG, "packing table entry without a weight");
-    bytes += vtts_tc_conv_packed_bytes(c.k, c.Cin, c.Cout);
+    bytes += vtts_tc_conv_packed_bytes(c.k, c.Cin, c.Cout, c.f16);
   }
   if (m.wpk) cudaFree(m.wpk);
   m.wpk = nullptr;
@@ -199,7 +199,7 @@ int vtts_pack_convs(vtts_ctx* ctx, ModelWeights& m, const std::vector<PackSpec>&
   m.tile0.clear();
   for (auto& c : convs) {
     m.tile0.push_back((int)m.wpk_t.size());
-    int rc = vtts_tc_pack_conv(ctx, c.w, c.k, c.Cin, c.Cout, cur, m.wpk_t);
+    int rc = vtts_tc_pack_conv(ctx, c.w, c.k, c.Cin, c.Cout, c.f16, cur, m.wpk_t);
     if (rc) return rc;
   }
   return VTTS_OK;
@@ -376,7 +376,8 @@ int vtts_device_info(vtts_ctx* ctx, int* sm_count, int* cc_major, int* cc_minor,
 
 int vtts_set_precision(vtts_ctx* ctx, int mode) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (mode != VTTS_PRECISION_FP32 && mode != VTTS_PRECISION_BF16X3) return ctx->fail(VTTS_ERR_BAD_ARG, "set_precision: mode %d", mode);
+  if (mode != VTTS_PRECISION_FP32 && mode != VTTS_PRECISION_BF16X3 && mode != VTTS_PRECISION_FP16)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "set_precision: mode %d", mode);
   ctx->precision = mode;
   return VTTS_OK;
 }
@@ -425,14 +426,15 @@ int vtts_debug_conv1d(vtts_ctx* ctx, int precision, const float* x_dev, const fl
     int rc = vtts_launch_conv(ctx, L, nullptr);
     if (rc) return rc;
   } else {
+    const bool f16 = precision == VTTS_PRECISION_FP16;
     void* wpk = nullptr;
-    VTTS_CUDA(cudaMalloc(&wpk, vtts_tc_packed_elems(k, Cin, Cout) * 2));
-    int rc = vtts_tc_pack_weights(ctx, w_dev, wpk, k, Cin, Cout, 0, Cout);
+    VTTS_CUDA(cudaMalloc(&wpk, vtts_tc_packed_elems(k, Cin, Cout, f16) * 2));
+    int rc = vtts_tc_pack_weights(ctx, w_dev, wpk, k, Cin, Cout, 0, Cout, f16);
     if (rc) { cudaFree(wpk); return rc; }
     TcLaunch TL;
     memset(&TL, 0, sizeof(TL));
     TL.nprob = 1; TL.Cin = Cin; TL.N = Cout; TL.in_ld = Cin; TL.out_ld = Cout; TL.B = B; TL.T_rows = T; TL.rows_out = T;
-    TL.len = len_dev; TL.len_mul = 1; TL.pre_mode = pre_slope == 1.0f ? 0 : 1; TL.pre_slope = pre_slope;
+    TL.len = len_dev; TL.len_mul = 1; TL.pre_mode = pre_slope == 1.0f ? 0 : 1; TL.pre_slope = pre_slope; TL.f16 = f16;
     TL.p[0] = TcProb{x_dev, nullptr, nullptr, wpk, bias_dev, resid_dev, nullptr, nullptr, nullptr, out_dev, k, dil, -((k - 1) * dil) / 2, 1, 0};
     rc = vtts_launch_tc_conv(ctx, TL, nullptr);
     cudaError_t e = cudaDeviceSynchronize();
@@ -450,15 +452,16 @@ int vtts_debug_pair(vtts_ctx* ctx, const float* x_dev, const float* w1_dev, cons
                     const float* b2_dev, const int32_t* len_dev, int B, int T, int C, int k, int dil, float slope, float* out_dev) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const bool f16 = ctx->precision == VTTS_PRECISION_FP16;   // the generator's operand format of the context's mode
   void* wpk = nullptr;
-  const size_t bytes = vtts_tc_packed_elems(k, C, C) * 2;
+  const size_t bytes = vtts_tc_packed_elems(k, C, C, f16) * 2;
   VTTS_CUDA(cudaMalloc(&wpk, 2 * bytes));
-  int rc = vtts_tc_pack_weights(ctx, w1_dev, wpk, k, C, C, 0, C);
-  if (!rc) rc = vtts_tc_pack_weights(ctx, w2_dev, (char*)wpk + bytes, k, C, C, 0, C);
+  int rc = vtts_tc_pack_weights(ctx, w1_dev, wpk, k, C, C, 0, C, f16);
+  if (!rc) rc = vtts_tc_pack_weights(ctx, w2_dev, (char*)wpk + bytes, k, C, C, 0, C, f16);
   if (rc) { cudaFree(wpk); return rc; }
   TcPairLaunch PL;
   memset(&PL, 0, sizeof(PL));
-  PL.nprob = 1; PL.N = C; PL.B = B; PL.T_rows = T; PL.len = len_dev; PL.len_mul = 1; PL.slope = slope;
+  PL.nprob = 1; PL.N = C; PL.B = B; PL.T_rows = T; PL.len = len_dev; PL.len_mul = 1; PL.slope = slope; PL.f16 = f16;
   PL.p[0] = TcPairProb{x_dev, wpk, (char*)wpk + bytes, b1_dev, b2_dev, out_dev, k, dil};
   rc = vtts_launch_tc_pair(ctx, PL, nullptr);
   cudaError_t e = cudaDeviceSynchronize();

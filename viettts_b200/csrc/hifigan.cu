@@ -1,5 +1,5 @@
-// HiFiGAN generator forward (strict fp32 path) -- restates Generator.__call__
-// (vietTTS/hifigan/model.py:109-125) on top of the generic conv kernel.
+// HiFiGAN generator forward -- restates Generator.__call__ (vietTTS/hifigan/model.py:109-125) on top of the generic
+// conv kernel (strict fp32) or the tensor-core kernels of tc_conv.cu (bf16x3, or fp16 in VTTS_PRECISION_FP16).
 //
 //   conv_pre                              model.py:110
 //   per stage: lrelu(0.1) -> ups[i]       model.py:112-114   (u output phases, 2 taps each)
@@ -100,7 +100,8 @@ void carve(Arena& ar, int B, int T, HgBufs& hb) {
 }
 
 // packing table of the generator: the 72 ResBlock convs in hgi order, the ConvTranspose output phases of the four
-// stages, conv_pre (two N = 256 tiles)
+// stages, conv_pre (two N = 256 tiles) as bf16 hi/lo planes; then the same PK_COUNT entries again as fp16 planes
+// (VTTS_PRECISION_FP16): entry e + PK_COUNT is the fp16 copy of entry e
 constexpr int PK_RB(int n, int which, int m) { return n * 6 + which * 3 + m; }
 constexpr int PK_UPS(int i, int r) { return i == 0 ? 72 + r : PK_UPS(i - 1, vc::hg_rate(i - 1)) + r; }
 constexpr int PK_PRE = PK_UPS(4, 0), PK_COUNT = PK_PRE + 1;
@@ -121,7 +122,7 @@ int vtts_hifigan_prepare(vtts_ctx* ctx) {
   for (int i = 0, C = vc::HG_C0; i < 4; ++i, C /= 2) dn.push_back((size_t)vc::hg_rate(i) * 2 * C * (C / 2));
   int rc = vtts_alloc_tensors(ctx, dn, &m.derived, m.d);
   if (rc) return rc;
-  std::vector<PackSpec> pk(PK_COUNT);
+  std::vector<PackSpec> pk(2 * PK_COUNT);
   for (int i = 0, C = vc::HG_C0; i < 4; ++i, C /= 2) {
     const int u = vc::hg_rate(i), K = vc::hg_upk(i);
     repack_ups_kernel<<<256, 256>>>(m.t[hgi::UPS_W(i)], m.d[i], u, K, C, C / 2, (K + u - 2 + 1) / 2);
@@ -135,7 +136,11 @@ int vtts_hifigan_prepare(vtts_ctx* ctx) {
         pk[PK_RB(n, which, j)] = {m.t[hgi::RB_W(n, which, j)], vc::hg_rbk(n % 3), ch, ch};
       }
   pk[PK_PRE] = {m.t[hgi::PRE_W], 7, vc::MEL, vc::HG_C0};
-  // ---- tensor-core path: bf16 hi/lo split + canonical K-major packing of every dense conv ----
+  for (int e = 0; e < PK_COUNT; ++e) {
+    pk[PK_COUNT + e] = pk[e];
+    pk[PK_COUNT + e].f16 = true;
+  }
+  // ---- tensor-core path: bf16 hi/lo split (and fp16) + canonical K-major packing of every dense conv ----
   VTTS_CUDA(cudaDeviceSynchronize());  // the phase weights are packed from the repacked transposed-conv weights
   rc = vtts_pack_convs(ctx, m, pk);
   if (rc) return rc;
@@ -168,14 +173,17 @@ int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, i
   L.T_rows = T; L.rows_out = T; L.len_mul = 1;
   L.pre_mode = 0; L.pre_slope = 1.f; L.post_act = 0;
   L.p[0] = ConvProb{mel, nullptr, nullptr, W[hgi::PRE_W], W[hgi::PRE_B], nullptr, nullptr, nullptr, nullptr, hb.P0, 7, 1, -3, 1, 0};
-  const bool tc = ctx->precision == 1;
+  // tensor-core modes: bf16x3 (BF16X3) or one fp16 product (FP16, the packing table's second half)
+  const bool tc = ctx->precision != VTTS_PRECISION_FP32;
+  const int f16 = ctx->precision == VTTS_PRECISION_FP16;
+  const int pk = f16 ? PK_COUNT : 0;
   if (tc) {
     TcLaunch TL;
     memset(&TL, 0, sizeof(TL));
     TL.nprob = 2; TL.Cin = vc::MEL; TL.N = 256; TL.in_ld = vc::MEL; TL.out_ld = vc::HG_C0;
-    TL.B = B; TL.T_rows = T; TL.rows_out = T; TL.len = n_frames; TL.len_mul = 1; TL.pre_mode = 0; TL.pre_slope = 1.f;
+    TL.B = B; TL.T_rows = T; TL.rows_out = T; TL.len = n_frames; TL.len_mul = 1; TL.pre_mode = 0; TL.pre_slope = 1.f; TL.f16 = f16;
     for (int t = 0; t < 2; ++t)
-      TL.p[t] = TcProb{mel, nullptr, nullptr, M.tiles(PK_PRE)[t], W[hgi::PRE_B] + 256 * t, nullptr, nullptr, nullptr, nullptr, hb.P0 + 256 * t, 7, 1, -3, 1, 0};
+      TL.p[t] = TcProb{mel, nullptr, nullptr, M.tiles(pk + PK_PRE)[t], W[hgi::PRE_B] + 256 * t, nullptr, nullptr, nullptr, nullptr, hb.P0 + 256 * t, 7, 1, -3, 1, 0};
     rc = vtts_launch_tc_conv(ctx, TL, st);
   } else {
     rc = vtts_launch_conv(ctx, L, st);
@@ -216,17 +224,17 @@ int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, i
       memset(&TL, 0, sizeof(TL));
       TL.nprob = u / nph; TL.nphase = nph; TL.Cin = C; TL.N = Co; TL.in_ld = C; TL.out_ld = Co;
       TL.B = B; TL.T_rows = rows_in; TL.rows_out = rows_in * u; TL.len = n_frames; TL.len_mul = scale_in;
-      TL.pre_mode = L.pre_mode; TL.pre_slope = 0.1f;
+      TL.pre_mode = L.pre_mode; TL.pre_slope = 0.1f; TL.f16 = f16;
       for (int g = 0; g < u / nph; ++g) {
         const ConvProb& c0 = L.p[g * nph];
         TcProb q;
         memset(&q, 0, sizeof(q));
         q.x0 = c0.x0; q.x1 = c0.x1; q.x2 = c0.x2; q.bias = c0.bias; q.out = c0.out;
         q.k = 2; q.dil = 1; q.out_stride = u;
-        q.wpk = M.tiles(PK_UPS(i, g * nph))[0]; q.in_off = c0.in_off; q.out_off = g * nph;
+        q.wpk = M.tiles(pk + PK_UPS(i, g * nph))[0]; q.in_off = c0.in_off; q.out_off = g * nph;
         for (int ph = 0; ph < nph; ++ph) {
           const int r = g * nph + ph;
-          q.wpk_ph[ph] = M.tiles(PK_UPS(i, r))[0];
+          q.wpk_ph[ph] = M.tiles(pk + PK_UPS(i, r))[0];
           q.in_off_ph[ph] = L.p[r].in_off;
           q.out_off_ph[ph] = r;
         }
@@ -249,10 +257,10 @@ int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, i
         // ---- fused pair: conv(d) -> lrelu -> conv(1) -> + x, intermediate kept on chip (tc_conv.cu) ----
         TcPairLaunch PL;
         memset(&PL, 0, sizeof(PL));
-        PL.nprob = 3; PL.N = Co; PL.B = B; PL.T_rows = rows; PL.len = n_frames; PL.len_mul = scale; PL.slope = 0.1f;
+        PL.nprob = 3; PL.N = Co; PL.B = B; PL.T_rows = rows; PL.len = n_frames; PL.len_mul = scale; PL.slope = 0.1f; PL.f16 = f16;
         for (int j = 0; j < 3; ++j) {
           const int kk = vc::hg_rbk(j), n = i * 3 + j;
-          PL.p[j] = TcPairProb{src[j], M.tiles(PK_RB(n, 0, m))[0], M.tiles(PK_RB(n, 1, m))[0], W[hgi::RB_B(n, 0, m)], W[hgi::RB_B(n, 1, m)],
+          PL.p[j] = TcPairProb{src[j], M.tiles(pk + PK_RB(n, 0, m))[0], M.tiles(pk + PK_RB(n, 1, m))[0], W[hgi::RB_B(n, 0, m)], W[hgi::RB_B(n, 1, m)],
                                (m == 1) ? hb.Bb[j] : hb.A[par][j], kk, d};
         }
         rc = vtts_launch_tc_pair(ctx, PL, st);
@@ -260,20 +268,20 @@ int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, i
         continue;
       }
       if (tc) {
-        // ---- bf16x3 tensor-core path (tc_conv.cu) ----
+        // ---- tensor-core path (tc_conv.cu) ----
         TcLaunch TL;
         for (int which = 0; which < 2; ++which) {
           memset(&TL, 0, sizeof(TL));
           TL.nprob = 3; TL.Cin = Co; TL.N = Co; TL.in_ld = Co; TL.out_ld = Co;
           TL.B = B; TL.T_rows = rows; TL.rows_out = rows; TL.len = n_frames; TL.len_mul = scale;
-          TL.pre_mode = 1; TL.pre_slope = 0.1f;
+          TL.pre_mode = 1; TL.pre_slope = 0.1f; TL.f16 = f16;
           for (int j = 0; j < 3; ++j) {
             const int kk = vc::hg_rbk(j), n = i * 3 + j;
             const int dd = which == 0 ? d : 1;
             TcProb p;
             memset(&p, 0, sizeof(p));
             p.x0 = which == 0 ? src[j] : hb.Tb[j];
-            p.wpk = M.tiles(PK_RB(n, which, m))[0];
+            p.wpk = M.tiles(pk + PK_RB(n, which, m))[0];
             p.bias = W[hgi::RB_B(n, which, m)];
             p.resid = which == 0 ? nullptr : src[j];
             p.out = which == 0 ? hb.Tb[j] : ((m == 1) ? hb.Bb[j] : hb.A[par][j]);

@@ -5,14 +5,18 @@
 // "bf16x3" arithmetic:  every fp32 operand v is split into hi = bf16(v), lo = bf16(v - hi) and the
 // product is accumulated in fp32 as  a_hi*w_hi + a_hi*w_lo + a_lo*w_hi  (the dropped a_lo*w_lo
 // term and the split truncation are ~2^-17 relative -- see DESIGN.md).
+// The generator's fast mode (VTTS_PRECISION_FP16, template flag F16) runs the same kernels with ONE fp16 operand plane:
+// v -> fp16_rn(v) saturated to +-65504, one wgmma .f32.f16.f16 per (chunk, tap, 64-row block) instead of three bf16
+// ones, fp32 accumulators and the same epilogues (waveform error ~1e-3 L-inf, see DESIGN.md §3).
 //
 // GEMM view per tap j:  D[time, cout] += A_j[time, cin] * W_j[cin, cout]
 //   M = 64 time rows per wgmma (one warpgroup), N = Cout tile (32..256), K = 16 channels.
 //   A operand: activations in shared memory, K-major, NO swizzle, rows 16 B apart:
-//       [plane hi|lo][k-half (8 ch)][row][8 x bf16]
+//       [plane hi|lo][k-half (8 ch)][row][8 x bf16]     (fp16: plane 0 only)
 //     so tap j / dilation d is just a start-address offset of j*d*16 bytes in the descriptor (no im2col).
 //   B operand: weights pre-split and pre-packed at load time into the same canonical layout,
-//     streamed with cp.async.bulk (TMA bulk copy) through an mbarrier ring, one tap per stage.
+//     streamed with cp.async.bulk (TMA bulk copy) through an mbarrier ring, one tap per stage
+//     (fp16: one plane, half the bytes per stage; the stage keeps its bf16 size).
 //
 // One persistent CTA per SM, 12 warps:
 //   warps 0-7  two consumer warpgroups: each owns MW x 64 rows of the tile, issues the wgmmas of its rows and runs the
@@ -129,8 +133,8 @@ struct TileQueue {
 };
 
 // converters: fill A stage `stage` with rows [row_base, row_base + rows) of channels [c*16, c*16+16) of x0 (+x1+x2)/3,
-// leaky_relu'd (pre_mode >= 1), zero outside [0, valid)
-template <int RA>
+// leaky_relu'd (pre_mode >= 1), zero outside [0, valid); bf16 hi/lo planes, or one saturated fp16 plane (F16)
+template <int RA, bool F16>
 __device__ __forceinline__ void convert_chunk(uint8_t* stage, int ct, const float* x0, const float* x1, const float* x2, int ld, int c,
                                               int row_base, int rows, int valid, int pre_mode, float slope) {
   constexpr int RSTEP = NCONV / 4;
@@ -167,24 +171,30 @@ __device__ __forceinline__ void convert_chunk(uint8_t* stage, int ct, const floa
         if (pre_mode >= 1) {
           x.x = lrelu(x.x, slope); x.y = lrelu(x.y, slope); x.z = lrelu(x.z, slope); x.w = lrelu(x.w, slope);
         }
-        uint2 hi, lo;
-        split4(x, hi, lo);
-        *reinterpret_cast<uint2*>(st + (size_t)rr * 16) = hi;
-        *reinterpret_cast<uint2*>(st + (size_t)(2 * RA + rr) * 16) = lo;
+        if constexpr (F16) {
+          *reinterpret_cast<uint2*>(st + (size_t)rr * 16) = f16x4_sat(x);
+        } else {
+          uint2 hi, lo;
+          split4(x, hi, lo);
+          *reinterpret_cast<uint2*>(st + (size_t)rr * 16) = hi;
+          *reinterpret_cast<uint2*>(st + (size_t)(2 * RA + rr) * 16) = lo;
+        }
       }
     }
   }
 }
 
 // weight producer: the k packed (chunk, tap) blocks of chunks [0, nch) of one conv, one ring stage each
-template <int N, int NW>
+// (a block is N * 64 bytes of bf16 hi/lo, or N * 32 bytes of fp16)
+template <int N, int NW, bool F16>
 __device__ __forceinline__ void produce_weights(uint8_t* w_st, uint64_t* w_full, uint64_t* w_empty, Ring& rw, const void* wpk, int nch,
                                                 int k, int* err, long long& wait_acc) {
+  constexpr int WB = F16 ? N * 32 : N * 64;
   const uint8_t* src = reinterpret_cast<const uint8_t*>(wpk);
   for (int i = 0; i < nch * k; ++i) {
     mbar_wait_t(&w_empty[rw.s], rw.p ^ 1, err, 4, wait_acc);
-    mbar_expect_tx(&w_full[rw.s], N * 64);
-    bulk_g2s(w_st + rw.s * (N * 64), src + (size_t)i * (N * 64), N * 64, &w_full[rw.s]);
+    mbar_expect_tx(&w_full[rw.s], WB);
+    bulk_g2s(w_st + rw.s * (N * 64), src + (size_t)i * WB, WB, &w_full[rw.s]);
     rw.next<NW>();
   }
 }
@@ -194,12 +204,14 @@ __device__ __forceinline__ void produce_weights(uint8_t* w_st, uint64_t* w_full,
 // otherwise it is chunk c of the fixed buffer at a_st_u32 (the pair kernel's intermediate).
 // A_REGS (fixed buffer only): the A fragments are loaded into registers with ldmatrix and the wgmmas take A from
 // registers, so the tensor core fetches only B from shared memory; each group then retires before the next one loads.
-template <int N, int MW, int RA, int NW, bool A_FROM_RING, bool A_REGS = false>
+// F16: one fp16 product per (chunk, tap, 64-row block); the weight block is [k-half][n][8], so its k-halves are N rows
+// apart.
+template <int N, int MW, int RA, int NW, bool A_FROM_RING, bool A_REGS, bool F16>
 __device__ __forceinline__ void consume(float (&acc)[MW][N / 2], int wg, uint32_t a_st_u32, uint64_t* a_full, uint64_t* a_empty, Ring& ra,
                                         uint32_t w_st_u32, uint64_t* w_full, uint64_t* w_empty, Ring& rw, int nch, int k, int dil,
                                         int* err, long long& w_a, long long& w_w) {
   const uint64_t a_tmpl = make_desc(0, RA * 16, 128);
-  const uint64_t b_tmpl = make_desc(0, 2 * N * 16, 128);   // k-half blocks are 2N rows apart ([hi rows | lo rows])
+  const uint64_t b_tmpl = make_desc(0, (F16 ? 1 : 2) * N * 16, 128);   // k-half blocks are 2N rows apart ([hi rows | lo rows]) or N (fp16)
   const bool lane0 = (threadIdx.x & 31) == 0;
   int pend_w = -1, pend_a = -1;
   for (int c = 0; c < nch; ++c) {
@@ -217,7 +229,7 @@ __device__ __forceinline__ void consume(float (&acc)[MW][N / 2], int wg, uint32_
       const uint64_t b_lo = b_tmpl | (uint64_t)((w_base + N * 16) >> 4);
       const uint32_t first = (c | j) != 0 ? 1u : 0u;
       if constexpr (A_REGS) {
-        static_assert(!A_FROM_RING, "register A operand comes from the fixed buffer");
+        static_assert(!A_FROM_RING && !F16, "register A operand: bf16 planes of the fixed buffer");
         const int lane = threadIdx.x & 31, wl = (threadIdx.x >> 5) & 3;
         uint32_t fa_hi[MW][4], fa_lo[MW][4];
 #pragma unroll
@@ -247,9 +259,13 @@ __device__ __forceinline__ void consume(float (&acc)[MW][N / 2], int wg, uint32_
         const uint32_t row = a_base + ((wg * MW + mt) * 64 + j * dil) * 16;
         const uint64_t a_hi = a_tmpl | (uint64_t)(row >> 4);
         const uint64_t a_lo = a_tmpl | (uint64_t)((row + 2 * RA * 16) >> 4);
-        wgmma<N>(acc[mt], a_hi, b_hi, first);
-        wgmma<N>(acc[mt], a_hi, b_lo, 1u);
-        wgmma<N>(acc[mt], a_lo, b_hi, 1u);
+        if constexpr (F16) {
+          wgmma<N, true>(acc[mt], a_hi, b_hi, first);
+        } else {
+          wgmma<N>(acc[mt], a_hi, b_hi, first);
+          wgmma<N>(acc[mt], a_hi, b_lo, 1u);
+          wgmma<N>(acc[mt], a_lo, b_hi, 1u);
+        }
       }
       wgmma_commit();
       wgmma_wait<1>();            // the previous group has retired: its stages may be refilled
@@ -308,7 +324,7 @@ __device__ __forceinline__ TileQueue tile_queue(uint64_t* bars, int nw) {
 
 // EPI = 0: bias (+ residual) only -- the HiFiGAN generator's hot path.  EPI = 1: bias, eval BatchNorm,
 // tanh / relu, residual, partial N tile (acoustic model convs and GEMMs).
-template <int N, int EPI, int MW>
+template <int N, int EPI, int MW, bool F16>
 __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_constant__ TcLaunch L) {
   using Cfg = TcCfg<N, MW, 0>;
   constexpr int R = Cfg::R, RA = Cfg::RA, NW = Cfg::NW;
@@ -353,7 +369,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
       PRODUCER_TILES
       TILE_LOOP_BEGIN
         (void)b; (void)tau0;
-        produce_weights<N, NW>(w_st, w_full, w_empty, rw, P.wpk_ph[ph], nch, P.k, L.err, w_e);
+        produce_weights<N, NW, F16>(w_st, w_full, w_empty, rw, P.wpk_ph[ph], nch, P.k, L.err, w_e);
       TILE_LOOP_END
       if (L.dbg) L.dbg[(size_t)blockIdx.x * 16 + 4] = w_e;
     }
@@ -370,7 +386,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
       const float* x2 = L.pre_mode == 2 ? P.x2 + in_base : nullptr;
       for (int c = 0; c < nch; ++c) {
         mbar_wait_t(&a_empty[ra.s], ra.p ^ 1, L.err, 5, w_ae);
-        convert_chunk<RA>(a_st + ra.s * Cfg::A_STAGE, ct, P.x0 + in_base, x1, x2, L.in_ld, c, tau0 + P.in_off_ph[ph], R + (k - 1) * dil,
+        convert_chunk<RA, F16>(a_st + ra.s * Cfg::A_STAGE, ct, P.x0 + in_base, x1, x2, L.in_ld, c, tau0 + P.in_off_ph[ph], R + (k - 1) * dil,
                           valid, L.pre_mode, L.pre_slope);
         fence_proxy_async();
         mbar_arrive(&a_full[ra.s]);
@@ -389,8 +405,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
     const int post_act = EPI ? L.post_act : 0;
     READER_TILES
     TILE_LOOP_BEGIN
-      consume<N, MW, RA, NW, true>(acc, wg, smem_u32(a_st), a_full, a_empty, ra, smem_u32(w_st), w_full, w_empty, rw, nch, P.k, P.dil,
-                                   L.err, w_a, w_w);
+      consume<N, MW, RA, NW, true, false, F16>(acc, wg, smem_u32(a_st), a_full, a_empty, ra, smem_u32(w_st), w_full, w_empty, rw, nch, P.k,
+                                               P.dil, L.err, w_a, w_w);
       const size_t out_base = (size_t)b * L.rows_out * L.out_ld;
       const int ostride = P.out_stride, ooff = P.out_off_ph[ph];
       const int row_w = tau0 + wg * MW * 64 + (warp & 3) * 16 + (lane >> 2);
@@ -437,7 +453,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
 // padding at each row's true end (hifigan/model.py:44-51).  A tile stores R_OUT output rows [tau0, tau0 + R_OUT) and
 // computes the intermediate on rows [tau0 - h2, tau0 - h2 + R) (h2 = (k - 1) / 2, conv2's padding) entirely on chip.
 // A2_REGS: conv2 takes its A operand from registers (ldmatrix + register-A wgmma) instead of from shared memory.
-template <int N, int MW, bool A2_REGS>
+// F16: both convs on fp16 operands; the intermediate is one saturated fp16 plane.
+template <int N, int MW, bool A2_REGS, bool F16>
 __global__ void __launch_bounds__(NTHREADS, 1) tc_pair_kernel(const __grid_constant__ TcPairLaunch L) {
   using Cfg = TcCfg<N, MW, 1>;
   constexpr int R = Cfg::R, R_OUT = Cfg::R_OUT, RA = Cfg::RA, NW = Cfg::NW, NCH = N / 16;
@@ -479,8 +496,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_pair_kernel(const __grid_const
       PRODUCER_TILES
       TILE_LOOP_BEGIN
         (void)b; (void)tau0; (void)dil; (void)h2;
-        produce_weights<N, NW>(w_st, w_full, w_empty, rw, P.w1pk, NCH, k, L.err, w_e);
-        produce_weights<N, NW>(w_st, w_full, w_empty, rw, P.w2pk, NCH, k, L.err, w_e);
+        produce_weights<N, NW, F16>(w_st, w_full, w_empty, rw, P.w1pk, NCH, k, L.err, w_e);
+        produce_weights<N, NW, F16>(w_st, w_full, w_empty, rw, P.w2pk, NCH, k, L.err, w_e);
       TILE_LOOP_END
     }
   } else if (warp > PROD_WARP) {
@@ -493,7 +510,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_pair_kernel(const __grid_const
       const int row_base = tau0 - h2 - (k - 1) * dil / 2;
       for (int c = 0; c < NCH; ++c) {
         mbar_wait_t(&a_empty[ra.s], ra.p ^ 1, L.err, 5, w_ae);
-        convert_chunk<RA>(a_st + ra.s * Cfg::A_STAGE, ct, x, nullptr, nullptr, N, c, row_base, R + (k - 1) * dil, valid, 1, L.slope);
+        convert_chunk<RA, F16>(a_st + ra.s * Cfg::A_STAGE, ct, x, nullptr, nullptr, N, c, row_base, R + (k - 1) * dil, valid, 1, L.slope);
         fence_proxy_async();
         mbar_arrive(&a_full[ra.s]);
         ra.next<NA>();
@@ -509,9 +526,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_pair_kernel(const __grid_const
     READER_TILES
     TILE_LOOP_BEGIN
       // ---- conv1 over the R intermediate rows ----
-      consume<N, MW, RA, NW, true>(acc, wg, smem_u32(a_st), a_full, a_empty, ra, smem_u32(w_st), w_full, w_empty, rw, NCH, k, dil, L.err,
-                                   w_a, w_w);
-      // ---- + b1, lrelu, zero outside the row, hi/lo split -> conv2's operand (rows of this warpgroup only) ----
+      consume<N, MW, RA, NW, true, false, F16>(acc, wg, smem_u32(a_st), a_full, a_empty, ra, smem_u32(w_st), w_full, w_empty, rw, NCH, k, dil,
+                                               L.err, w_a, w_w);
+      // ---- + b1, lrelu, zero outside the row, hi/lo split (or fp16) -> conv2's operand (rows of this warpgroup only) ----
       const int lr_w = wg * MW * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
       for (int mt = 0; mt < MW; ++mt)
@@ -526,18 +543,22 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_pair_kernel(const __grid_const
             const float2 bi = __ldg(reinterpret_cast<const float2*>(P.b1 + col));
             const float v0 = inside ? lrelu(acc[mt][jn * 4 + 2 * h] + bi.x, slope) : 0.f;
             const float v1 = inside ? lrelu(acc[mt][jn * 4 + 2 * h + 1] + bi.y, slope) : 0.f;
-            const __nv_bfloat162 hi = __floats2bfloat162_rn(v0, v1);
-            const __nv_bfloat162 lo = __floats2bfloat162_rn(v0 - __low2float(hi), v1 - __high2float(hi));
             uint8_t* dst = mid + (col >> 4) * Cfg::A_STAGE + (((col >> 3) & 1) * RA + lr) * 16 + (col & 7) * 2;
-            *reinterpret_cast<__nv_bfloat162*>(dst) = hi;
-            *reinterpret_cast<__nv_bfloat162*>(dst + 2 * RA * 16) = lo;
+            if constexpr (F16) {
+              *reinterpret_cast<uint32_t*>(dst) = f16x2_sat(v0, v1);
+            } else {
+              const __nv_bfloat162 hi = __floats2bfloat162_rn(v0, v1);
+              const __nv_bfloat162 lo = __floats2bfloat162_rn(v0 - __low2float(hi), v1 - __high2float(hi));
+              *reinterpret_cast<__nv_bfloat162*>(dst) = hi;
+              *reinterpret_cast<__nv_bfloat162*>(dst + 2 * RA * 16) = lo;
+            }
           }
         }
       fence_proxy_async();
       named_bar(1, NCONS);          // conv2 of a row reads intermediate rows of the other warpgroup
       // ---- conv2 (dilation 1) ----
-      consume<N, MW, RA, NW, false, A2_REGS>(acc, wg, smem_u32(mid), a_full, a_empty, ra, smem_u32(w_st), w_full, w_empty, rw, NCH, k, 1, L.err,
-                                    w_a, w_w);
+      consume<N, MW, RA, NW, false, A2_REGS, F16>(acc, wg, smem_u32(mid), a_full, a_empty, ra, smem_u32(w_st), w_full, w_empty, rw, NCH, k, 1,
+                                                  L.err, w_a, w_w);
       named_bar(1, NCONS);          // both warpgroups are done reading the intermediate before the next tile rewrites it
       // ---- + b2 + x ----
       const float* x = P.x + (size_t)b * L.T_rows * N;
@@ -570,30 +591,37 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_pair_kernel(const __grid_const
 #undef TILE_LOOP_END
 }
 
-// fp32 Haiku conv weight w[k][Cin][Cout_total] -> packed bf16 blocks for output columns [n0, n0+N):
-//   [chunk c = Cin/16][tap j][k-half][plane hi|lo][n][8]
-__global__ void pack_w_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ dst, int k, int Cin, int Cout_total, int n0, int N) {
+// fp32 Haiku conv weight w[k][Cin][Cout_total] -> packed blocks for output columns [n0, n0+N):
+//   bf16x3: [chunk c = Cin/16][tap j][k-half][plane hi|lo][n][8] bf16
+//   fp16:   [chunk c = Cin/16][tap j][k-half][n][8] fp16, saturated to +-65504
+template <bool F16>
+__global__ void pack_w_kernel(const float* __restrict__ w, uint16_t* __restrict__ dst, int k, int Cin, int Cout_total, int n0, int N) {
   const size_t total = (size_t)k * Cin * N;
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
     const int n = idx % N;
     const int i = (idx / N) % Cin;
     const int j = idx / ((size_t)N * Cin);
     const float v = (n0 + n) < Cout_total ? w[((size_t)j * Cin + i) * Cout_total + n0 + n] : 0.f;
+    const int c = i / 16, kh = (i % 16) / 8, e = i % 8;
+    if constexpr (F16) {
+      const size_t blk = ((size_t)c * k + j) * (size_t)(2 * N * 8);
+      dst[blk + ((size_t)kh * N + n) * 8 + e] = (uint16_t)(f16x2_sat(v, 0.f) & 0xffffu);
+      continue;
+    }
     const __nv_bfloat16 hi = __float2bfloat16_rn(v);
     const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-    const int c = i / 16, kh = (i % 16) / 8, e = i % 8;
     const size_t blk = ((size_t)c * k + j) * (size_t)(4 * N * 8);
-    dst[blk + ((size_t)(kh * 2 + 0) * N + n) * 8 + e] = hi;   // [k-half][plane hi|lo][n][8]: hi and lo rows of a k-half are
-    dst[blk + ((size_t)(kh * 2 + 1) * N + n) * 8 + e] = lo;   // adjacent, so [W_hi | W_lo] is also one 2N-row operand
+    dst[blk + ((size_t)(kh * 2 + 0) * N + n) * 8 + e] = __bfloat16_as_ushort(hi);   // [k-half][plane hi|lo][n][8]: hi and lo rows of a
+    dst[blk + ((size_t)(kh * 2 + 1) * N + n) * 8 + e] = __bfloat16_as_ushort(lo);   // k-half are adjacent, so [W_hi | W_lo] is also one 2N-row operand
   }
 }
 
-template <int N, int EPI, int MW>
+template <int N, int EPI, int MW, bool F16>
 int launch_cfg(vtts_ctx* ctx, TcLaunch& L, cudaStream_t st) {
   using Cfg = TcCfg<N, MW, 0>;
   static bool attr_done_dev[64] = {};   // function attributes are per device (a process may hold contexts on several GPUs)
   if (!attr_done_dev[ctx->device & 63]) {
-    VTTS_CUDA(cudaFuncSetAttribute(tc_conv_kernel<N, EPI, MW>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    VTTS_CUDA(cudaFuncSetAttribute(tc_conv_kernel<N, EPI, MW, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_done_dev[ctx->device & 63] = true;
   }
   const int nph = L.nphase > 1 ? L.nphase : 1;
@@ -610,7 +638,7 @@ int launch_cfg(vtts_ctx* ctx, TcLaunch& L, cudaStream_t st) {
   L.tiles_per_row = (L.T_rows + Cfg::R - 1) / Cfg::R;
   L.ntiles = L.nprob * L.tiles_per_row * L.B * nph;
   const int grid = L.ntiles < ctx->sm_count ? L.ntiles : ctx->sm_count;
-  tc_conv_kernel<N, EPI, MW><<<grid, NTHREADS, Cfg::SMEM_BYTES, st>>>(L);
+  tc_conv_kernel<N, EPI, MW, F16><<<grid, NTHREADS, Cfg::SMEM_BYTES, st>>>(L);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   return VTTS_OK;
@@ -624,15 +652,18 @@ int launch_n(vtts_ctx* ctx, TcLaunch& L, cudaStream_t st) {
   for (int i = 0; i < L.nprob; ++i) generic |= L.p[i].bn_mean != nullptr;
   if (L.nphase > 4) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: %d phases", L.nphase);
   if (L.nphase > 1 && generic) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: multi-phase tiles use the plain epilogue");
-  return generic ? launch_cfg<N, 1, MW>(ctx, L, st) : launch_cfg<N, 0, MW>(ctx, L, st);
+  // fp16 operands serve the generator, whose convs all use the plain epilogue
+  if (L.f16 && generic) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: fp16 operands use the plain epilogue");
+  if (L.f16) return launch_cfg<N, 0, MW, true>(ctx, L, st);
+  return generic ? launch_cfg<N, 1, MW, false>(ctx, L, st) : launch_cfg<N, 0, MW, false>(ctx, L, st);
 }
 
-template <int N, int MW, bool A2_REGS>
+template <int N, int MW, bool A2_REGS, bool F16 = false>
 int launch_pair(vtts_ctx* ctx, TcPairLaunch& L, cudaStream_t st) {
   using Cfg = TcCfg<N, MW, 1>;
   static bool attr_done_dev[64] = {};
   if (!attr_done_dev[ctx->device & 63]) {
-    VTTS_CUDA(cudaFuncSetAttribute(tc_pair_kernel<N, MW, A2_REGS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    VTTS_CUDA(cudaFuncSetAttribute(tc_pair_kernel<N, MW, A2_REGS, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_done_dev[ctx->device & 63] = true;
   }
   for (int i = 0; i < L.nprob; ++i)
@@ -642,7 +673,7 @@ int launch_pair(vtts_ctx* ctx, TcPairLaunch& L, cudaStream_t st) {
   L.tiles_per_row = (L.T_rows + Cfg::R_OUT - 1) / Cfg::R_OUT;
   L.ntiles = L.nprob * L.tiles_per_row * L.B;
   const int grid = L.ntiles < ctx->sm_count ? L.ntiles : ctx->sm_count;
-  tc_pair_kernel<N, MW, A2_REGS><<<grid, NTHREADS, Cfg::SMEM_BYTES, st>>>(L);
+  tc_pair_kernel<N, MW, A2_REGS, F16><<<grid, NTHREADS, Cfg::SMEM_BYTES, st>>>(L);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   return VTTS_OK;
@@ -650,34 +681,36 @@ int launch_pair(vtts_ctx* ctx, TcPairLaunch& L, cudaStream_t st) {
 
 }  // namespace
 
-size_t vtts_tc_packed_elems(int k, int Cin, int N) { return (size_t)k * Cin * N * 2; }
+size_t vtts_tc_packed_elems(int k, int Cin, int N, bool f16) { return (size_t)k * Cin * N * (f16 ? 1 : 2); }
 
-int vtts_tc_pack_weights(vtts_ctx* ctx, const float* w, void* dst, int k, int Cin, int Cout_total, int n0, int N) {
-  pack_w_kernel<<<256, 256>>>(w, reinterpret_cast<__nv_bfloat16*>(dst), k, Cin, Cout_total, n0, N);
+int vtts_tc_pack_weights(vtts_ctx* ctx, const float* w, void* dst, int k, int Cin, int Cout_total, int n0, int N, bool f16) {
+  if (f16) pack_w_kernel<true><<<256, 256>>>(w, reinterpret_cast<uint16_t*>(dst), k, Cin, Cout_total, n0, N);
+  else pack_w_kernel<false><<<256, 256>>>(w, reinterpret_cast<uint16_t*>(dst), k, Cin, Cout_total, n0, N);
   VTTS_CUDA(cudaGetLastError());
   return VTTS_OK;
 }
 
 int vtts_tc_tile_n(int Cout) { return Cout <= 32 ? 32 : (Cout <= 64 ? 64 : (Cout <= 128 ? 128 : 256)); }
 
-size_t vtts_tc_conv_packed_bytes(int k, int Cin, int Cout) {
+size_t vtts_tc_conv_packed_bytes(int k, int Cin, int Cout, bool f16) {
   const int N = vtts_tc_tile_n(Cout), nt = (Cout + N - 1) / N;
-  return ((vtts_tc_packed_elems(k, Cin, N) * 2 + 255) & ~size_t(255)) * nt;
+  return ((vtts_tc_packed_elems(k, Cin, N, f16) * 2 + 255) & ~size_t(255)) * nt;
 }
 
-int vtts_tc_pack_conv(vtts_ctx* ctx, const float* w, int k, int Cin, int Cout, char*& cursor, std::vector<void*>& out) {
+int vtts_tc_pack_conv(vtts_ctx* ctx, const float* w, int k, int Cin, int Cout, bool f16, char*& cursor, std::vector<void*>& out) {
   const int N = vtts_tc_tile_n(Cout), nt = (Cout + N - 1) / N;
   for (int t = 0; t < nt; ++t) {
-    int rc = vtts_tc_pack_weights(ctx, w, cursor, k, Cin, Cout, t * N, N);
+    int rc = vtts_tc_pack_weights(ctx, w, cursor, k, Cin, Cout, t * N, N, f16);
     if (rc) return rc;
     out.push_back(cursor);
-    cursor += (vtts_tc_packed_elems(k, Cin, N) * 2 + 255) & ~size_t(255);
+    cursor += (vtts_tc_packed_elems(k, Cin, N, f16) * 2 + 255) & ~size_t(255);
   }
   return VTTS_OK;
 }
 
 int vtts_conv_dispatch(vtts_ctx* ctx, const ConvLaunch& L, void* const* wpk, cudaStream_t st) {
-  if (ctx->precision != 1 || wpk == nullptr) return vtts_launch_conv(ctx, L, st);
+  // the fp16 mode covers the generator only: here (acoustic and duration models) it runs bf16x3 like mode 1
+  if (ctx->precision == VTTS_PRECISION_FP32 || wpk == nullptr) return vtts_launch_conv(ctx, L, st);
   const int N = vtts_tc_tile_n(L.Cout), nt = (L.Cout + N - 1) / N;
   TcLaunch TL;
   auto reset = [&]() {
@@ -750,6 +783,10 @@ int vtts_launch_tc_pair(vtts_ctx* ctx, TcPairLaunch& L, cudaStream_t st) {
   L.dbg = ctx->tc_dbg_on ? ctx->d_tc_dbg : nullptr;
   if (L.N != 32 && L.N != 64) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_pair: C %d unsupported (32 or 64)", L.N);
   // vtts_ctx::pair_ts: 2 = 256-row tiles (default), 1 = the same with conv2's A operand in registers, 0 = 128-row tiles
+  if (L.f16) {
+    if (ctx->pair_ts != 2) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_pair: fp16 operands exist for the default pair form (256-row tiles) only, not form %d", ctx->pair_ts);
+    return L.N == 64 ? launch_pair<64, 2, false, true>(ctx, L, st) : launch_pair<32, 2, false, true>(ctx, L, st);
+  }
   if (ctx->pair_ts == 1) return L.N == 64 ? launch_pair<64, 2, true>(ctx, L, st) : launch_pair<32, 2, true>(ctx, L, st);
   if (ctx->pair_ts == 0) return L.N == 64 ? launch_pair<64, 1, false>(ctx, L, st) : launch_pair<32, 1, false>(ctx, L, st);
   return L.N == 64 ? launch_pair<64, 2, false>(ctx, L, st) : launch_pair<32, 2, false>(ctx, L, st);

@@ -75,7 +75,7 @@ struct TcProb {
   const float* x0;
   const float* x1;
   const float* x2;
-  const void* wpk;       // packed bf16 hi/lo weights (vtts_tc_pack_weights)
+  const void* wpk;       // packed weights (vtts_tc_pack_weights) in the launch's operand format
   const float* bias;     // [N]
   const float* resid;    // rows_out x out_ld or null
   const float* bn_mean;  // eval BatchNorm (all three or none), applied after the bias
@@ -104,6 +104,8 @@ struct TcLaunch {
   int nphase;            // phases per tile (1, 2 or 4); 0 means 1
   int post_act;          // 0 none, 1 tanh, 2 relu (after BN, before the residual)
   int n_valid;           // real output channels of this N tile (<= N); 0 means N
+  int f16;               // operand format: 0 = bf16 hi/lo planes, three products (bf16x3); 1 = one fp16 plane, one product
+                         // (the generator's VTTS_PRECISION_FP16; plain epilogue only)
   int tiles_per_row, ntiles;  // filled by the launcher
   int* sched;                 // device int[2]: the run-time tile scheduler's counters (vtts_ctx::d_tc_sched)
   int* err;                   // device int: set before trapping on a barrier timeout
@@ -113,7 +115,7 @@ struct TcLaunch {
 // ---- fused ResBlock pair (tc_pair.cu): out = conv2(lrelu(conv1(lrelu(x)) + b1)) + b2 + x, C = N channels ----
 struct TcPairProb {
   const float* x;        // [B][T_rows][N] input and residual
-  const void* w1pk;      // packed bf16 hi/lo weights of the dilated conv (vtts_tc_pack_weights)
+  const void* w1pk;      // packed weights of the dilated conv (vtts_tc_pack_weights), in the launch's operand format
   const void* w2pk;      // ... of the dilation-1 conv
   const float* b1;
   const float* b2;
@@ -129,14 +131,15 @@ struct TcPairLaunch {
   const int* len;
   int len_mul;
   float slope;
+  int f16;                     // operand format as in TcLaunch (fp16: the default pair form only)
   int tiles_per_row, ntiles;   // filled by the launcher
   int* sched;
   int* err;
   long long* dbg;
 };
 
-// Device weights of one model: the checkpoint tensors, fp32 tensors derived from them at load, and the bf16 hi/lo
-// tensor-core packing of its convs (vtts_pack_convs).
+// Device weights of one model: the checkpoint tensors, fp32 tensors derived from them at load, and the tensor-core
+// packing of its convs (vtts_pack_convs: bf16 hi/lo, and for the generator a second, fp16 copy).
 struct ModelWeights {
   float* blob = nullptr;        // checkpoint tensors in canonical order, each 256 B aligned
   std::vector<float*> t;
@@ -152,7 +155,8 @@ struct ModelWeights {
 
 struct vtts_ctx {
   int device = 0;
-  int precision = 1;            // 0 = strict fp32 (FMA pipe), 1 = bf16x3 on the tensor cores (wgmma, default)
+  int precision = 1;            // 0 = strict fp32 (FMA pipe), 1 = bf16x3 on the tensor cores (wgmma, default),
+                                // 2 = fp16 operands in the generator, bf16x3 everywhere else (vtts_precision)
   int* d_err = nullptr;
   // tile scheduler counters of the tensor-core launches: [0] next ticket, [1] CTAs done taking tickets.  Each launch
   // leaves them at zero.  One pair serves every launch of the context because a context's tensor-core launches never
@@ -244,24 +248,26 @@ struct Arena {
 // conv1d.cu
 int vtts_launch_conv(vtts_ctx* ctx, const ConvLaunch& L, cudaStream_t st);
 // tc_conv.cu
-size_t vtts_tc_packed_elems(int k, int Cin, int N);
-int vtts_tc_pack_weights(vtts_ctx* ctx, const float* w, void* dst, int k, int Cin, int Cout_total, int n0, int N);
+// 16-bit elements of one packed N tile: two bf16 planes, or one fp16 plane (f16)
+size_t vtts_tc_packed_elems(int k, int Cin, int N, bool f16);
+int vtts_tc_pack_weights(vtts_ctx* ctx, const float* w, void* dst, int k, int Cin, int Cout_total, int n0, int N, bool f16);
 int vtts_launch_tc_conv(vtts_ctx* ctx, TcLaunch& L, cudaStream_t st);
 // fused ResBlock pair (C = 32 or 64): conv1 -> lrelu -> conv2 -> + x with the intermediate kept in shared memory
 int vtts_launch_tc_pair(vtts_ctx* ctx, TcPairLaunch& L, cudaStream_t st);
-// generic dispatch: runs `L` on the tensor-core path when ctx->precision == 1 and packed weights are given
-// (wpk[prob * ntile + tile], ntile = ceil(Cout/256) tiles of width vtts_tc_tile_n(Cout)), else on the FP32 path
+// generic dispatch (acoustic and duration models): runs `L` on the bf16x3 tensor-core path when ctx->precision is 1 or 2
+// and packed weights are given (wpk[prob * ntile + tile], ntile = ceil(Cout/256) tiles of width vtts_tc_tile_n(Cout)),
+// else on the FP32 path
 int vtts_tc_tile_n(int Cout);
 int vtts_conv_dispatch(vtts_ctx* ctx, const ConvLaunch& L, void* const* wpk, cudaStream_t st);
 // packs every N tile of one conv weight; returns the number of tiles, appends device pointers to `out`
-int vtts_tc_pack_conv(vtts_ctx* ctx, const float* w, int k, int Cin, int Cout, char*& cursor, std::vector<void*>& out);
-size_t vtts_tc_conv_packed_bytes(int k, int Cin, int Cout);
+int vtts_tc_pack_conv(vtts_ctx* ctx, const float* w, int k, int Cin, int Cout, bool f16, char*& cursor, std::vector<void*>& out);
+size_t vtts_tc_conv_packed_bytes(int k, int Cin, int Cout, bool f16);
 // api.cu: weight slots
 void vtts_free_weights(ModelWeights& m);
 // replaces *store by one zero-filled device allocation holding tensors of n[i] floats, each 256 B aligned
 int vtts_alloc_tensors(vtts_ctx* ctx, const std::vector<size_t>& n, float** store, std::vector<float*>& ptrs);
-// one entry of a model's packing table: conv weight w[k][Cin][Cout]
-struct PackSpec { const float* w; int k, Cin, Cout; };
+// one entry of a model's packing table: conv weight w[k][Cin][Cout], packed as bf16 hi/lo planes or as one fp16 plane
+struct PackSpec { const float* w; int k, Cin, Cout; bool f16 = false; };
 // packs every N tile of every entry of `convs` (vtts_tc_pack_conv) into m.wpk and records m.wpk_t / m.tile0
 int vtts_pack_convs(vtts_ctx* ctx, ModelWeights& m, const std::vector<PackSpec>& convs);
 // hifigan.cu

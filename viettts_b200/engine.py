@@ -19,7 +19,8 @@ def _chunk_seed(seed: int, chunk: int) -> int:
     """Key of the on-device dropout stream for the chunk-th slice of an over-long batch (a distinct 64-bit key per
     chunk: `seed + offset` would alias the next seed's first chunk)."""
     return (int(seed) ^ (chunk * 0x9E3779B97F4A7C15)) & 0xFFFFFFFFFFFFFFFF
-PRECISION_FP32, PRECISION_BF16X3 = 0, 1
+PRECISION_FP32, PRECISION_BF16X3, PRECISION_FP16 = 0, 1, 2
+PRECISIONS = {"fp32": PRECISION_FP32, "bf16x3": PRECISION_BF16X3, "fp16": PRECISION_FP16}
 MAX_ACOUSTIC_ROWS = 128   # rows per vtts_acoustic_forward call (csrc/nat.cu MAX_ROWS)
 
 
@@ -84,8 +85,10 @@ class Engine:
         return float(ms.value)
 
     def set_precision(self, mode) -> None:
-        """'fp32' (strict, FMA pipe) or 'bf16x3' (wgmma tensor cores, split-bf16, fp32 accumulate)."""
-        m = {"fp32": PRECISION_FP32, "bf16x3": PRECISION_BF16X3}.get(mode, mode)
+        """'fp32' (strict, FMA pipe), 'bf16x3' (wgmma tensor cores, split-bf16, fp32 accumulate; the default) or 'fp16'
+        (fast generator: one fp16 product per operand pair, fp32 accumulate, waveform L-inf <= 3e-3 against float64 on
+        synthetic weights; every other model runs as in 'bf16x3')."""
+        m = PRECISIONS.get(mode, mode)
         self._ck(self.lib.vtts_set_precision(self.h, int(m)))
 
     def debug_conv1d(self, precision, x_t, w_t, bias_t, k, dil, pre_slope=1.0, resid_t=None, len_t=None):
@@ -94,13 +97,14 @@ class Engine:
         B, T, Cin = x_t.shape
         Cout = w_t.shape[2]
         out = torch.empty((B, T, Cout), dtype=torch.float32, device=x_t.device)
-        m = {"fp32": PRECISION_FP32, "bf16x3": PRECISION_BF16X3}.get(precision, precision)
+        m = PRECISIONS.get(precision, precision)
         self._ck(self.lib.vtts_debug_conv1d(self.h, int(m), _ptr(x_t), _ptr(w_t), _ptr(bias_t), _ptr(resid_t), _ptr(len_t),
                                             B, T, Cin, Cout, int(k), int(dil), float(pre_slope), _ptr(out)))
         return out
 
     def debug_pair(self, x_t, w1_t, b1_t, w2_t, b2_t, k, dil, slope=0.1, len_t=None):
-        """Test hook: one fused ResBlock pair on torch CUDA tensors (tensor-core path)."""
+        """Test hook: one fused ResBlock pair on torch CUDA tensors (tensor-core path; fp16 operands when the engine is
+        in 'fp16', bf16x3 otherwise)."""
         import torch
         B, T, Cc = x_t.shape
         out = torch.empty_like(x_t)

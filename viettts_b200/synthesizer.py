@@ -4,6 +4,7 @@ Same flags as the reference (--text --output --sample-rate --silence-duration --
 pipeline (synthesizer.py:34-39): normalise -> text2mel -> mel2wave -> 16-bit PCM WAV.  Two additions that the
 GPU path makes worthwhile: `--text-file` synthesises one utterance per input line as ragged batches through a
 single library call per batch (`Engine.tts`), and the WAV writer is built in (the reference needs `soundfile`).
+`--precision fp16` runs the generator in the fast fp16 mode (Engine.set_precision) for either input.
 """
 from __future__ import annotations
 
@@ -103,8 +104,15 @@ def main(argv=None) -> int:
     parser.add_argument("--seed", default=None, type=int,
                         help="prenet dropout: key of the on-device counter stream; default = the checkpoint's rng "
                              "(--text: the reference's own JAX/Haiku mask stream; --text-file: the device stream keyed by those words)")
+    parser.add_argument("--precision", default=None, choices=["bf16x3", "fp16", "fp32"],
+                        help="conv arithmetic (default bf16x3, the library default): bf16x3 = fp32-class split-bf16 tensor-core "
+                             "products; fp16 = fast generator, one fp16 product per operand pair (waveform within ~1e-3 of "
+                             "bf16x3), every other model as bf16x3; fp32 = strict FMA pipe")
     args = parser.parse_args(argv)
     lexicon = args.lexicon_file if args.lexicon_file is not None else config.LEXICON_FILE
+    if args.precision is not None:
+        from .engine import get_engine
+        get_engine().set_precision(args.precision)      # the engine both the --text and the --text-file paths use
 
     if args.text_file is not None:
         lines = [ln for ln in args.text_file.read_text().splitlines() if ln.strip()]

@@ -151,7 +151,19 @@ int vtts_debug_conv1d(vtts_ctx* ctx, int precision, const float* x_dev, const fl
                       const float* resid_dev, const int32_t* len_dev, int B, int T, int Cin, int Cout, int k, int dil,
                       float pre_slope, float* out_dev);
 
-/* test hook: one fused ResBlock pair  out = conv2(lrelu(conv1(lrelu(x)) + b1)) + b2 + x  (vietTTS/hifigan/model.py:44-51)
+/* test hook: nprob convs of one shape through the shared conv dispatcher, the path of every acoustic and duration
+ * conv and hoisted GEMM (packing, N tiles of <= 256 columns, partial last tile, <= 8 problems per launch, eval BatchNorm
+ * and activation epilogue).  Per problem p: x[p] [B,T,Cin], w[p] Haiku layout [k,Cin,Cout], bias[p] [Cout],
+ * bn[p] NULL or [4][Cout] (Haiku scale, offset, mean, var), resid[p] NULL or [B,T,Cout], out[p] [B,T,Cout]; host arrays
+ * of device pointers (bn and resid may be NULL as a whole).  SAME padding with dilation `dil`; post_act 0 none, 1 tanh,
+ * 2 relu, after the BatchNorm and before the residual; len int32 [B] or NULL.  Rows at or past len[b] are not written.
+ * `precision` is a vtts_precision (FP16 runs bf16x3 here, as the model does); the context's own mode is left unchanged.
+ * Synchronous. */
+int vtts_debug_conv_dispatch(vtts_ctx* ctx, int precision, int nprob, const float* const* x, const float* const* w,
+                             const float* const* bias, const float* const* bn, const float* const* resid, float* const* out,
+                             const int32_t* len, int B, int T, int Cin, int Cout, int k, int dil, int post_act);
+
+/* test hook: one fused ResBlock pair out = conv2(lrelu(conv1(lrelu(x)) + b1)) + b2 + x  (vietTTS/hifigan/model.py:44-51)
  * on the tensor-core path; x/out [B,T,C] with C in {32,64}, w1/w2 Haiku layout [k,C,C], conv1 dilation `dil`. Synchronous.
  * Runs on fp16 operands when the context is in VTTS_PRECISION_FP16, on bf16x3 otherwise. */
 int vtts_debug_pair(vtts_ctx* ctx, const float* x_dev, const float* w1_dev, const float* b1_dev, const float* w2_dev,

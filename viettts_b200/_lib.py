@@ -15,6 +15,7 @@ c_ctx = C.c_void_p
 f32p = C.POINTER(C.c_float)
 i32p = C.POINTER(C.c_int32)
 u8p = C.POINTER(C.c_uint8)
+ptrp = C.POINTER(C.c_void_p)   # host array of device pointers
 
 # name -> (restype, argtypes); kept in sync with include/viettts_b200.h by tests/test_abi.py
 SIGNATURES = {
@@ -27,6 +28,8 @@ SIGNATURES = {
     "vtts_get_precision": (C.c_int, [c_ctx]),
     "vtts_debug_conv1d": (C.c_int, [c_ctx, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]),
+    "vtts_debug_conv_dispatch": (C.c_int, [c_ctx, C.c_int, C.c_int, ptrp, ptrp, ptrp, ptrp, ptrp, ptrp, C.c_void_p,
+                                           C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "vtts_debug_tc_stats": (C.c_int, [c_ctx, C.c_int, C.c_void_p]),
     "vtts_debug_substages": (C.c_int, [c_ctx, C.c_int, C.c_void_p]),
     "vtts_debug_pair": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

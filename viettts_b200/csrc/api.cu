@@ -448,6 +448,63 @@ int vtts_debug_conv1d(vtts_ctx* ctx, int precision, const float* x_dev, const fl
   return VTTS_OK;
 }
 
+namespace {
+// vtts_debug_conv_dispatch on the temporary buffer `tmp`: BatchNorm inverses of every problem (nprob x Cout floats, the
+// first inv_bytes), then the packed tiles of every problem, as the model's load and run code prepare them
+int conv_dispatch_on(vtts_ctx* ctx, char* tmp, size_t inv_bytes, int nprob, const float* const* x, const float* const* w,
+                     const float* const* bias, const float* const* bn, const float* const* resid, float* const* out,
+                     const int32_t* len, int B, int T, int Cin, int Cout, int k, int dil, int post_act) {
+  float* inv = reinterpret_cast<float*>(tmp);
+  char* cursor = tmp + inv_bytes;
+  std::vector<void*> wpk;
+  ConvLaunch L;
+  memset(&L, 0, sizeof(L));
+  for (int p = 0; p < nprob; ++p) {
+    int rc = vtts_tc_pack_conv(ctx, w[p], k, Cin, Cout, false, cursor, wpk);
+    if (rc) return rc;
+    ConvProb& q = L.p[p];
+    q.x0 = x[p]; q.w = w[p]; q.bias = bias[p]; q.out = out[p]; q.resid = resid ? resid[p] : nullptr;
+    q.k = k; q.dil = dil; q.in_off = -((k - 1) * dil) / 2; q.out_stride = 1;
+    if (bn && bn[p]) {
+      vtts_bn_inv(bn[p], bn[p] + 3 * Cout, inv + (size_t)p * Cout, Cout);
+      q.bn_mean = bn[p] + 2 * Cout; q.bn_inv = inv + (size_t)p * Cout; q.bn_off = bn[p] + Cout;
+    }
+  }
+  VTTS_CUDA(cudaGetLastError());
+  L.nprob = nprob; L.Cin = Cin; L.Cout = Cout; L.B = B; L.T_rows = T; L.rows_out = T;
+  L.len = len; L.len_mul = 1; L.pre_mode = 0; L.pre_slope = 1.f; L.post_act = post_act;
+  return vtts_conv_dispatch(ctx, L, wpk.data(), nullptr);
+}
+}  // namespace
+
+int vtts_debug_conv_dispatch(vtts_ctx* ctx, int precision, int nprob, const float* const* x, const float* const* w,
+                             const float* const* bias, const float* const* bn, const float* const* resid, float* const* out,
+                             const int32_t* len, int B, int T, int Cin, int Cout, int k, int dil, int post_act) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  if (precision < VTTS_PRECISION_FP32 || precision > VTTS_PRECISION_FP16)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "debug_conv_dispatch: precision %d", precision);
+  if (nprob < 1 || nprob > 8 || !x || !w || !bias || !out)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "debug_conv_dispatch: nprob %d (1..8) and the x, w, bias and out arrays are required", nprob);
+  for (int p = 0; p < nprob; ++p)
+    if (!x[p] || !w[p] || !bias[p] || !out[p]) return ctx->fail(VTTS_ERR_BAD_ARG, "debug_conv_dispatch: null buffer in problem %d", p);
+  if (B < 1 || T < 1 || Cin < 16 || Cin % 16 != 0 || Cout < 4 || Cout % 4 != 0 || k < 1 || dil < 1 || post_act < 0 || post_act > 2)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "debug_conv_dispatch: B=%d T=%d Cin=%d Cout=%d k=%d dil=%d post_act=%d", B, T, Cin, Cout, k, dil,
+                     post_act);
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  const size_t inv_bytes = ((size_t)nprob * Cout * sizeof(float) + 255) & ~size_t(255);
+  char* tmp = nullptr;
+  VTTS_CUDA(cudaMalloc(&tmp, inv_bytes + nprob * vtts_tc_conv_packed_bytes(k, Cin, Cout, false)));
+  const int saved = ctx->precision;
+  ctx->precision = precision;
+  int rc = conv_dispatch_on(ctx, tmp, inv_bytes, nprob, x, w, bias, bn, resid, out, len, B, T, Cin, Cout, k, dil, post_act);
+  ctx->precision = saved;
+  const cudaError_t e = cudaDeviceSynchronize();
+  cudaFree(tmp);
+  if (rc) return rc;
+  if (e != cudaSuccess) return ctx->fail(VTTS_ERR_CUDA, "debug_conv_dispatch: %s", cudaGetErrorString(e));
+  return VTTS_OK;
+}
+
 int vtts_debug_pair(vtts_ctx* ctx, const float* x_dev, const float* w1_dev, const float* b1_dev, const float* w2_dev,
                     const float* b2_dev, const int32_t* len_dev, int B, int T, int C, int k, int dil, float slope, float* out_dev) {
   if (!ctx) return VTTS_ERR_BAD_ARG;

@@ -238,3 +238,14 @@ int vtts_launch_conv(vtts_ctx* ctx, const ConvLaunch& L, cudaStream_t st) {
   if (L.Cout <= 64) return launch_cfg<256, 64>(ctx, L, st);
   return launch_cfg<128, 128>(ctx, L, st);
 }
+
+namespace {
+__global__ void bn_inv_kernel(const float* __restrict__ scale, const float* __restrict__ var, float* __restrict__ inv, int n) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) inv[i] = scale[i] * rsqrtf(var[i] + 1e-5f);
+}
+}  // namespace
+
+void vtts_bn_inv(const float* scale, const float* var, float* inv, int n) {
+  bn_inv_kernel<<<(n + 255) / 256, 256>>>(scale, var, inv, n);
+}

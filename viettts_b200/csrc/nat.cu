@@ -74,11 +74,6 @@ __global__ void embed_kernel(const int32_t* __restrict__ tokens, const float* __
   *reinterpret_cast<float4*>(out + (size_t)tok * vc::ENC_D + c4) = __ldg(reinterpret_cast<const float4*>(emb + (size_t)id * vc::ENC_D + c4));
 }
 
-__global__ void bn_inv_kernel(const float* __restrict__ scale, const float* __restrict__ var, float* __restrict__ inv, int n) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) inv[i] = scale[i] * rsqrtf(var[i] + 1e-5f);
-}
-
 // dst[c][r][q] = src[(row0 + r)*ld + (q / upc)*gate_stride + c*upc + (q % upc)]
 __global__ void repack_cols_kernel(const float* __restrict__ src, int ld, int row0, int nrows, float* __restrict__ dst,
                                    int ncta, int ncols, int upc, int gate_stride) {
@@ -964,7 +959,7 @@ static void encoder_tables(const ModelWeights& m, std::vector<size_t>& dn, std::
 
 static void encoder_derive(const ModelWeights& m) {
   const auto& T = m.t;
-  for (int i = 0; i < 3; ++i) bn_inv_kernel<<<1, 256>>>(T[aci::ENC_CONV(i, 2)], T[aci::ENC_CONV(i, 5)], m.d[D_ENC_BNINV0 + i], 256);
+  for (int i = 0; i < 3; ++i) vtts_bn_inv(T[aci::ENC_CONV(i, 2)], T[aci::ENC_CONV(i, 5)], m.d[D_ENC_BNINV0 + i], 256);
   // recurrent weights: rows 256..511 of w[512][1024]
   repack_cols_kernel<<<256, 256>>>(T[aci::ENC_LSTM_F_W], 1024, 256, 256, m.d[D_ENC_WHR], 64, 16, UPC, 256);
   repack_cols_kernel<<<256, 256>>>(T[aci::ENC_LSTM_B_W], 1024, 256, 256, m.d[D_ENC_WHR] + (size_t)64 * 256 * 16, 64, 16, UPC, 256);
@@ -1057,7 +1052,7 @@ int vtts_acoustic_prepare(vtts_ctx* ctx) {
   int rc = vtts_alloc_tensors(ctx, dn, &m.derived, m.d);   // zero-filled: D_ZERO needs no further work
   if (rc) return rc;
   encoder_derive(m);
-  for (int i = 0; i < 4; ++i) bn_inv_kernel<<<2, 256>>>(T[aci::POST_CONV(i, 2)], T[aci::POST_CONV(i, 5)], m.d[D_POST_BNINV0 + i], 512);
+  for (int i = 0; i < 4; ++i) vtts_bn_inv(T[aci::POST_CONV(i, 2)], T[aci::POST_CONV(i, 5)], m.d[D_POST_BNINV0 + i], 512);
   // decoder: rows after the 512 cond rows
   repack_cols_kernel<<<512, 256>>>(T[aci::DEC_L0_W], 2048, 512, 768, m.d[D_DEC_W0R], 128, 16, UPC, 512);
   repack_cols_kernel<<<512, 256>>>(T[aci::DEC_L1_W], 2048, 512, 1280, m.d[D_DEC_W1R], 128, 16, UPC, 512);

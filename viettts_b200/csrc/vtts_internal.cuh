@@ -247,6 +247,9 @@ struct Arena {
 
 // conv1d.cu
 int vtts_launch_conv(vtts_ctx* ctx, const ConvLaunch& L, cudaStream_t st);
+// ConvProb::bn_inv of an eval BatchNorm: inv[i] = scale[i] * rsqrt(var[i] + 1e-5), n floats, launched on the default
+// stream (load time); the caller checks cudaGetLastError
+void vtts_bn_inv(const float* scale, const float* var, float* inv, int n);
 // tc_conv.cu
 // 16-bit elements of one packed N tile: two bf16 planes, or one fp16 plane (f16)
 size_t vtts_tc_packed_elems(int k, int Cin, int N, bool f16);

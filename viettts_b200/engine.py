@@ -102,6 +102,28 @@ class Engine:
                                             B, T, Cin, Cout, int(k), int(dil), float(pre_slope), _ptr(out)))
         return out
 
+    POST_ACTS = {"none": 0, "tanh": 1, "relu": 2}
+
+    def debug_conv_dispatch(self, precision, xs, ws, biases, k, dil=1, bns=None, resids=None, post_act="none", len_t=None, outs=None):
+        """Test hook: len(xs) convs of one shape through the shared conv dispatcher of the acoustic and duration models,
+        on torch CUDA tensors.  xs[p] [B,T,Cin], ws[p] [k,Cin,Cout], biases[p] [Cout], bns[p] None or [4,Cout] (scale,
+        offset, mean, var), resids[p] None or [B,T,Cout]; post_act 'none', 'tanh' or 'relu'.  Writes outs[p] [B,T,Cout]
+        (allocated when not given) except the rows at or past len_t[b], and returns outs."""
+        import torch
+        n = len(xs)
+        B, T, Cin = xs[0].shape
+        Cout = ws[0].shape[2]
+        if outs is None:
+            outs = [torch.empty((B, T, Cout), dtype=torch.float32, device=xs[0].device) for _ in range(n)]
+
+        def arr(ts):
+            return None if ts is None else (C.c_void_p * n)(*[_ptr(t) for t in ts])
+
+        m = PRECISIONS.get(precision, precision)
+        self._ck(self.lib.vtts_debug_conv_dispatch(self.h, int(m), n, arr(xs), arr(ws), arr(biases), arr(bns), arr(resids), arr(outs),
+                                                   _ptr(len_t), B, T, Cin, Cout, int(k), int(dil), self.POST_ACTS[post_act]))
+        return outs
+
     def debug_pair(self, x_t, w1_t, b1_t, w2_t, b2_t, k, dil, slope=0.1, len_t=None):
         """Test hook: one fused ResBlock pair on torch CUDA tensors (tensor-core path; fp16 operands when the engine is
         in 'fp16', bf16x3 otherwise)."""

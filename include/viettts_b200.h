@@ -184,6 +184,30 @@ int vtts_debug_tc_stats(vtts_ctx* ctx, int enable, int64_t* host_out_256x16);
  *   teacher-forced pass: 17 encoder + upsample, 18 prenet + hoisted GEMMs, 19 zoneout scan, 20 projection + postnet */
 int vtts_debug_substages(vtts_ctx* ctx, int enable, float* ms_out24);
 
+/* ---- streaming generator: push mel frames per stream slot as they arrive ---------------------
+ * A vtts_vocoder_stream holds max_streams independent slots.  Each slot carries every generator layer's context
+ * between pushes, so a push costs only the frames it brings.  A slot that has received P frames since BEGIN, without
+ * END, has emitted max(0, P - D) frames of 256 samples in total (D = vtts_vocoder_stream_lookahead(), the generator's
+ * right receptive field rounded up to whole frames); a push with END emits the rest, so the slot emits exactly P frames.
+ * The emitted samples, concatenated, are bit-identical to vtts_hifigan_forward of the whole mel in the same precision
+ * mode with the fused ResBlock-pair kernel off.  Modes BF16X3 and FP16; FP32 fails with VTTS_ERR_BAD_ARG.
+ * Slots are independent: a slot's output equals that stream run alone.  n_new = 0 without flags leaves a slot idle and
+ * untouched.  flags: bit0 BEGIN (reset the slot; may be combined with END), bit1 END.  Pushing frames or END to a slot
+ * that has not begun, or that has ended, without BEGIN fails with VTTS_ERR_BAD_ARG.  The stream object owns the carried
+ * state (device memory that grows with max_streams * max_chunk_frames); each push also uses the context's workspace. */
+typedef struct vtts_vocoder_stream vtts_vocoder_stream;
+int vtts_vocoder_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_frames, vtts_vocoder_stream** out);
+int vtts_vocoder_stream_destroy(vtts_ctx* ctx, vtts_vocoder_stream* vs);
+int vtts_vocoder_stream_lookahead(void);                     /* D, in mel frames */
+/* mel_dev [S][F][80] (F = max_chunk_frames, rows past n_new[s] ignored); n_new, flags (bit0 BEGIN, bit1 END) and
+ * n_out are HOST int32/uint8/int32 arrays of S = max_streams; wav_dev [S][256*(F+D)], slot s gets 256*n_out[s]
+ * samples from its start.  Stream-ordered, asynchronous apart from reading the host arrays. */
+int vtts_vocoder_stream_push(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float* mel_dev, const int32_t* n_new,
+                             const uint8_t* flags, float* wav_dev, int32_t* n_out, void* stream);
+/* the same on host buffers mel [S][F][80] and wav [S][256*(F+D)]; returns when wav is written */
+int vtts_vocoder_stream_push_host(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float* mel, const int32_t* n_new,
+                                  const uint8_t* flags, float* wav, int32_t* n_out);
+
 /* ---- host-buffer entry points (what a ctypes / cgo / JNI binding calls) ------------------ */
 int vtts_mel2wave_host(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, int B, int T, float* wav);
 int vtts_predict_mel_host(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths,

@@ -7,6 +7,8 @@
 //   lrelu(0.01) -> conv_post -> tanh      model.py:122-124   (conv_post_kernel below)
 #include "vtts_internal.cuh"
 
+using namespace hgpk;
+
 namespace {
 
 // ---- ConvTranspose weight repack: Haiku w[K][Cout][Cin] -> per phase r: [2][Cin][Cout] ----------
@@ -98,13 +100,6 @@ void carve(Arena& ar, int B, int T, HgBufs& hb) {
   for (int j = 0; j < 3; ++j) hb.Tb[j] = ar.take<float>(big);
   for (int j = 0; j < 3; ++j) hb.Bb[j] = ar.take<float>(big);
 }
-
-// packing table of the generator: the 72 ResBlock convs in hgi order, the ConvTranspose output phases of the four
-// stages, conv_pre (two N = 256 tiles) as bf16 hi/lo planes; then the same PK_COUNT entries again as fp16 planes
-// (VTTS_PRECISION_FP16): entry e + PK_COUNT is the fp16 copy of entry e
-constexpr int PK_RB(int n, int which, int m) { return n * 6 + which * 3 + m; }
-constexpr int PK_UPS(int i, int r) { return i == 0 ? 72 + r : PK_UPS(i - 1, vc::hg_rate(i - 1)) + r; }
-constexpr int PK_PRE = PK_UPS(4, 0), PK_COUNT = PK_PRE + 1;
 
 }  // namespace
 

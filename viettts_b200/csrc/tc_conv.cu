@@ -133,10 +133,10 @@ struct TileQueue {
 };
 
 // converters: fill A stage `stage` with rows [row_base, row_base + rows) of channels [c*16, c*16+16) of x0 (+x1+x2)/3,
-// leaky_relu'd (pre_mode >= 1), zero outside [0, valid); bf16 hi/lo planes, or one saturated fp16 plane (F16)
+// leaky_relu'd (pre_mode >= 1), zero outside [lo, valid); bf16 hi/lo planes, or one saturated fp16 plane (F16)
 template <int RA, bool F16>
 __device__ __forceinline__ void convert_chunk(uint8_t* stage, int ct, const float* x0, const float* x1, const float* x2, int ld, int c,
-                                              int row_base, int rows, int valid, int pre_mode, float slope) {
+                                              int row_base, int rows, int lo, int valid, int pre_mode, float slope) {
   constexpr int RSTEP = NCONV / 4;
   const int q = ct & 3;                     // 4-channel group inside the 16-channel chunk
   const int r0 = ct >> 2;
@@ -150,7 +150,7 @@ __device__ __forceinline__ void convert_chunk(uint8_t* stage, int ct, const floa
       const int rr = rr0 + u * RSTEP;
       const int t = row_base + rr;
       v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (rr < rows && t >= 0 && t < valid) {
+      if (rr < rows && t >= lo && t < valid) {
         const size_t off = (size_t)t * ld + coff;
         v[u] = ldg_pf256(x0 + off);
         if (pre_mode == 2) {
@@ -346,19 +346,27 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
   const int nch = L.Cin / 16;
   const int nph = L.nphase > 1 ? L.nphase : 1;
 
-  // every role walks the same tile sequence (next_tile); a tile is (problem, batch row, row tile, output phase)
+  // every role walks the same tile sequence (next_tile); a tile is (problem, batch row, row tile, output phase).
+  // Input rows outside [in_lo, valid) read as zero.  Output row tau is written while tau < valid, or, with per-row
+  // bounds (TcProb::rb, plain epilogue only), while its output row tau * out_stride + out_off stays below out_hi.
+  constexpr bool ROW_BOUNDS = EPI == 0;
 #define TILE_LOOP_BEGIN                                                           \
   for (int tile; (tile = next_tile()) >= 0;) {                                    \
     const Tile td = decode_tile(tile, nph, L.nprob, L.tiles_per_row);              \
     const int ph = td.ph, b = td.b;                                                 \
     const int tau0 = td.tt * R;                                                    \
-    int valid = L.T_rows;                                                         \
-    if (L.len) {                                                                  \
-      const int v = L.len[b] * L.len_mul;                                         \
-      valid = v < valid ? v : valid;                                              \
-    }                                                                             \
-    if (tau0 >= valid) continue;                                                  \
-    const TcProb& P = L.p[td.pi];
+    const TcProb& P = L.p[td.pi];                                                  \
+    int valid = L.T_rows, in_lo = 0, out_hi = 0;                                  \
+    if (ROW_BOUNDS && P.rb) {                                                     \
+      in_lo = P.rb[3 * b]; valid = P.rb[3 * b + 1]; out_hi = P.rb[3 * b + 2];     \
+      if (tau0 * P.out_stride + P.out_off_ph[ph] >= out_hi) continue;             \
+    } else {                                                                      \
+      if (L.len) {                                                                \
+        const int v = L.len[b] * L.len_mul;                                       \
+        valid = v < valid ? v : valid;                                            \
+      }                                                                           \
+      if (tau0 >= valid) continue;                                                \
+    }
 #define TILE_LOOP_END }
 
   if (warp == PROD_WARP) {
@@ -368,7 +376,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
       long long w_e = 0;
       PRODUCER_TILES
       TILE_LOOP_BEGIN
-        (void)b; (void)tau0;
+        (void)b; (void)tau0; (void)in_lo; (void)valid; (void)out_hi;
         produce_weights<N, NW, F16>(w_st, w_full, w_empty, rw, P.wpk_ph[ph], nch, P.k, L.err, w_e);
       TILE_LOOP_END
       if (L.dbg) L.dbg[(size_t)blockIdx.x * 16 + 4] = w_e;
@@ -387,11 +395,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
       for (int c = 0; c < nch; ++c) {
         mbar_wait_t(&a_empty[ra.s], ra.p ^ 1, L.err, 5, w_ae);
         convert_chunk<RA, F16>(a_st + ra.s * Cfg::A_STAGE, ct, P.x0 + in_base, x1, x2, L.in_ld, c, tau0 + P.in_off_ph[ph], R + (k - 1) * dil,
-                          valid, L.pre_mode, L.pre_slope);
+                          in_lo, valid, L.pre_mode, L.pre_slope);
         fence_proxy_async();
         mbar_arrive(&a_full[ra.s]);
         ra.next<NA>();
       }
+      (void)out_hi;
     TILE_LOOP_END
     if (L.dbg && ct == 0) L.dbg[(size_t)blockIdx.x * 16 + 5] = w_ae;
   } else {
@@ -415,7 +424,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int tau = row_w + mt * 64 + 8 * h;
-          if (tau >= valid) continue;
+          if ((ROW_BOUNDS && P.rb) ? tau * ostride + ooff >= out_hi : tau >= valid) continue;
           const size_t orow = out_base + (size_t)(tau * ostride + ooff) * L.out_ld;
 #pragma unroll
           for (int jn = 0; jn < N / 8; ++jn) {
@@ -510,7 +519,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_pair_kernel(const __grid_const
       const int row_base = tau0 - h2 - (k - 1) * dil / 2;
       for (int c = 0; c < NCH; ++c) {
         mbar_wait_t(&a_empty[ra.s], ra.p ^ 1, L.err, 5, w_ae);
-        convert_chunk<RA, F16>(a_st + ra.s * Cfg::A_STAGE, ct, x, nullptr, nullptr, N, c, row_base, R + (k - 1) * dil, valid, 1, L.slope);
+        convert_chunk<RA, F16>(a_st + ra.s * Cfg::A_STAGE, ct, x, nullptr, nullptr, N, c, row_base, R + (k - 1) * dil, 0, valid, 1, L.slope);
         fence_proxy_async();
         mbar_arrive(&a_full[ra.s]);
         ra.next<NA>();
@@ -635,7 +644,7 @@ int launch_cfg(vtts_ctx* ctx, TcLaunch& L, cudaStream_t st) {
   }
   // the expensive problems (large k) first: within each row tile they are handed out before the cheap ones
   std::stable_sort(L.p, L.p + L.nprob, [](const TcProb& a, const TcProb& b) { return a.k > b.k; });
-  L.tiles_per_row = (L.T_rows + Cfg::R - 1) / Cfg::R;
+  L.tiles_per_row = ((L.tile_rows > 0 ? L.tile_rows : L.T_rows) + Cfg::R - 1) / Cfg::R;
   L.ntiles = L.nprob * L.tiles_per_row * L.B * nph;
   const int grid = L.ntiles < ctx->sm_count ? L.ntiles : ctx->sm_count;
   tc_conv_kernel<N, EPI, MW, F16><<<grid, NTHREADS, Cfg::SMEM_BYTES, st>>>(L);
@@ -649,7 +658,12 @@ template <int N>
 int launch_n(vtts_ctx* ctx, TcLaunch& L, cudaStream_t st) {
   constexpr int MW = N >= 256 ? 1 : (N == 128 ? 2 : 4);
   bool generic = L.post_act != 0 || (L.n_valid > 0 && L.n_valid < N);
-  for (int i = 0; i < L.nprob; ++i) generic |= L.p[i].bn_mean != nullptr;
+  bool rb = false;
+  for (int i = 0; i < L.nprob; ++i) {
+    generic |= L.p[i].bn_mean != nullptr;
+    rb |= L.p[i].rb != nullptr;
+  }
+  if (rb && generic) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: per-row bounds use the plain epilogue");
   if (L.nphase > 4) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: %d phases", L.nphase);
   if (L.nphase > 1 && generic) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: multi-phase tiles use the plain epilogue");
   // fp16 operands serve the generator, whose convs all use the plain epilogue

@@ -89,6 +89,10 @@ struct TcProb {
   const void* wpk_ph[4];
   int in_off_ph[4];
   int out_off_ph[4];
+  // optional per-batch-row bounds [B][3] (device int32): input rows outside [rb[3b], rb[3b+1]) read as zero, and output
+  // row tau*out_stride + out_off is written only below rb[3b+2].  Null: rows [0, valid) of the launch for both
+  // (vocoder_stream.cu runs "valid" convs over per-slot windows, whose input and output ranges differ)
+  const int* rb;
 };
 
 struct TcLaunch {
@@ -106,6 +110,7 @@ struct TcLaunch {
   int n_valid;           // real output channels of this N tile (<= N); 0 means N
   int f16;               // operand format: 0 = bf16 hi/lo planes, three products (bf16x3); 1 = one fp16 plane, one product
                          // (the generator's VTTS_PRECISION_FP16; plain epilogue only)
+  int tile_rows;              // output rows tau per batch row to tile over; 0 means T_rows
   int tiles_per_row, ntiles;  // filled by the launcher
   int* sched;                 // device int[2]: the run-time tile scheduler's counters (vtts_ctx::d_tc_sched)
   int* err;                   // device int: set before trapping on a barrier timeout
@@ -313,6 +318,15 @@ __host__ __device__ constexpr int RB_B(int n, int which, int m) { return RB_W(n,
 constexpr int POST_W = 10 + 12 * 12, POST_B = POST_W + 1;
 constexpr int COUNT = POST_B + 1;
 }  // namespace hgi
+
+// packing table of the generator (ctx->hg.tiles): the 72 ResBlock convs in hgi order, the ConvTranspose output phases
+// of the four stages, conv_pre (two N = 256 tiles) as bf16 hi/lo planes; then the same PK_COUNT entries again as fp16
+// planes (VTTS_PRECISION_FP16): entry e + PK_COUNT is the fp16 copy of entry e
+namespace hgpk {
+constexpr int PK_RB(int n, int which, int m) { return n * 6 + which * 3 + m; }
+constexpr int PK_UPS(int i, int r) { return i == 0 ? 72 + r : PK_UPS(i - 1, vc::hg_rate(i - 1)) + r; }
+constexpr int PK_PRE = PK_UPS(4, 0), PK_COUNT = PK_PRE + 1;
+}  // namespace hgpk
 
 // indices into ctx->ac.t
 namespace aci {

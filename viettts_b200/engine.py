@@ -238,6 +238,13 @@ class Engine:
             wav = self.mel2wave(mel[None, a:b])[0]
             yield wav[(t0 - a) * config.HOP: (t1 - a) * config.HOP]
 
+    def open_vocoder_stream(self, max_streams: int, max_chunk_frames: int) -> "VocoderStream":
+        """Stateful streaming generator with `max_streams` independent slots (vtts_vocoder_stream_*): push each slot's
+        new mel frames as they arrive and get back every waveform frame whose receptive field is complete.  Each push
+        costs only the frames it brings; the emitted audio equals `mel2wave` of the whole mel bit for bit (same
+        precision mode, fused pairs off).  Needs the generator weights and the 'bf16x3' or 'fp16' mode."""
+        return VocoderStream(self, max_streams, max_chunk_frames)
+
     def _acoustic_args(self, tokens, dur_frames, lengths, n_frames, masks, seed):
         tokens = _np(tokens, np.int32)
         if tokens.ndim != 2:
@@ -517,6 +524,82 @@ class Engine:
         st = torch.cuda.current_stream(wav_t.device).cuda_stream if stream is None else stream
         self._ck(self.lib.vtts_melspec(self.h, _ptr(wav_t), B, S, _ptr(out), st))
         return out
+
+
+STREAM_BEGIN, STREAM_END = 1, 2
+
+
+class VocoderStream:
+    """Handle of a streaming generator (Engine.open_vocoder_stream).  A slot that has received P frames since BEGIN
+    has emitted max(0, P - lookahead) frames; a push with END emits the rest."""
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int):
+        self.eng = eng
+        self.max_streams, self.max_chunk_frames = int(max_streams), int(max_chunk_frames)
+        self.lookahead = int(eng.lib.vtts_vocoder_stream_lookahead())
+        self.wav_ld = config.HOP * (self.max_chunk_frames + self.lookahead)   # samples per slot of the output buffer
+        h = C.c_void_p()
+        eng._ck(eng.lib.vtts_vocoder_stream_create(eng.h, self.max_streams, self.max_chunk_frames, C.byref(h)))
+        self.h = h
+
+    def _host_args(self, n_new, flags):
+        S = self.max_streams
+        n = _np(n_new, np.int32, (S,), "n_new")
+        f = _np(flags, np.uint8, (S,), "flags")
+        return n, f
+
+    def push(self, mel, n_new, begin=None, end=None) -> list:
+        """mel f32 [S,F',80] (F' <= max_chunk_frames; rows past n_new[s] ignored), n_new int [S], begin / end bool [S]
+        or None.  Returns one float32 array per slot with the samples it emits now (256 per frame)."""
+        S, F = self.max_streams, self.max_chunk_frames
+        mel = _np(mel, np.float32)
+        if mel.ndim != 3 or mel.shape[0] != S or mel.shape[1] > F or mel.shape[2] != config.MEL_DIM:
+            raise ValueError(f"mel must be [{S}, <= {F}, {config.MEL_DIM}], got {mel.shape}")
+        if mel.shape[1] < F:
+            mel = np.concatenate([mel, np.zeros((S, F - mel.shape[1], config.MEL_DIM), np.float32)], axis=1)
+        flags = np.zeros(S, np.uint8)
+        if begin is not None:
+            flags |= np.asarray(begin, bool).astype(np.uint8) * STREAM_BEGIN
+        if end is not None:
+            flags |= np.asarray(end, bool).astype(np.uint8) * STREAM_END
+        n, f = self._host_args(n_new, flags)
+        wav = np.empty((S, self.wav_ld), np.float32)
+        n_out = np.zeros(S, np.int32)
+        self.eng._ck(self.eng.lib.vtts_vocoder_stream_push_host(self.eng.h, self.h, _ptr(mel), _ptr(n), _ptr(f), _ptr(wav), _ptr(n_out)))
+        return [wav[s, : int(n_out[s]) * config.HOP].copy() for s in range(S)]
+
+    def push_device(self, mel_t, n_new, flags, out_t, stream=None) -> np.ndarray:
+        """Device buffers: mel_t f32 CUDA [S,F,80], out_t f32 CUDA [S, 256*(F+lookahead)]; n_new int [S] and flags
+        uint8 [S] (bit0 BEGIN, bit1 END) on the host.  Stream-ordered; returns n_out int32 [S] (frames slot s got at
+        the start of its row of out_t)."""
+        import torch
+        S, F = self.max_streams, self.max_chunk_frames
+        if tuple(mel_t.shape) != (S, F, config.MEL_DIM) or mel_t.dtype != torch.float32 or not mel_t.is_contiguous():
+            raise ValueError(f"mel_t must be contiguous float32 [{S}, {F}, {config.MEL_DIM}]")
+        if tuple(out_t.shape) != (S, self.wav_ld) or out_t.dtype != torch.float32 or not out_t.is_contiguous():
+            raise ValueError(f"out_t must be contiguous float32 [{S}, {self.wav_ld}]")
+        n, f = self._host_args(n_new, flags)
+        n_out = np.zeros(S, np.int32)
+        st = torch.cuda.current_stream(mel_t.device).cuda_stream if stream is None else stream
+        self.eng._ck(self.eng.lib.vtts_vocoder_stream_push(self.eng.h, self.h, _ptr(mel_t), _ptr(n), _ptr(f), _ptr(out_t), _ptr(n_out), st))
+        return n_out
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.eng, "h", None):
+            self.eng._ck(self.eng.lib.vtts_vocoder_stream_destroy(self.eng.h, self.h))
+        self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 _engines: dict = {}

@@ -193,27 +193,30 @@ struct EncScanArgs {
 };
 
 // ---- autoregressive decoder scan (model.py:129-142) ------------------------------------------------
-// One cooperative grid of 132 CTAs, up to 32 batch rows per launch.
-//   CTAs 0..127   LSTM role: CTA c owns 4 hidden units (16 gate columns) of both layers; its slices of the
-//                 recurrent matrices (768x16 + 1280x16 fp32) live in REGISTERS.  A persistent shared-memory
-//                 buffer holds [p2 | h0 | h1] of all rows; the parts that are already final (h0_{t-1},
-//                 h1_{t-1}) are prefetched while the prenet CTAs work, so only p2 (phase C) and h0_t (phase D)
-//                 are fetched on the critical path.
-//   CTAs 128..131 prenet role: 64 columns each (four blocks of 16) of p1 = drop(relu([h0,h1]_{t-1}.(Wo.W1) + bo.W1))
-//                 (phase EA) and of p2 = drop(relu(p1.W2)) (phase B); their weights are read through L1/L2
+// One cooperative grid of 128 CTAs, up to 128 batch rows per launch (row groups of 32).  CTA c owns
+//   * 4 hidden units (16 gate columns) of both LSTM layers; its slices of the recurrent matrices (768x16 + 1280x16
+//     fp32) live in REGISTERS;
+//   * prenet columns 2c and 2c+1 of p1 = drop(relu([h0,h1]_{t-1}.(Wo.W1) + bo.W1)) and of p2 = drop(relu(p1.W2));
+//     those weight slices (1024x2 + 256x2 fp32) live in SHARED memory.
+// A persistent shared-memory buffer holds [p2 | h0 | h1] of one row group.  A frame has four dependent exchanges
+// through L2, each closed by a grid barrier split into arrive and wait (dec_arrive / dec_wait):
+//   A  p1(t) from [h0 | h1]_{t-1}        arrive; zp1 = h1_{t-1}.W1[h1 rows], prefetch zc0[t] / zc1[t]; wait
+//   B  p2(t) from p1(t)                  arrive; wait
+//   C  LSTM0: h0_t                       arrive; wait
+//   D  LSTM1: h1_t                       arrive; zp0 = h0_t.W0[h0 rows] for frame t+1; wait
+// so the products of the state that is already final run while the barrier is open instead of on the critical path
+// (with more than one row group, the last group's only; the others are computed inline while their rows are staged).
 // The output projection mel_t = [h0,h1]_t.Wo + bo is NOT part of the scan: nothing in the recurrence reads mel_t
 // (the prenet consumes the precomposed Wo.W1), so every frame's [h0 | h1] is written to `hout` and one GEMM
-// projects the whole sequence afterwards.  (A projection role inside the scan -- 4 CTAs taking part in every grid
-// barrier -- was the slowest arrival at the C and D barriers for small batches: 15 us per frame at B = 1.)
-// Four grid barriers per frame: EA | B | C (LSTM0) | D (LSTM1).
+// projects the whole sequence afterwards.
 struct DecScanArgs {
   const float* zc0;      // [B][N][2048] cond.W0[0:512] + b0
   const float* zc1;      // [B][N][2048] cond.W1[0:512] + b1
   const float* w0r;      // [128][768][16]   rows 512..1279 of lstm0   ([p2, h0])
   const float* w1r;      // [128][1280][16]  rows 512..1791 of lstm1   ([p2, h0, h1])
-  const float* wc;       // [16][1024][16]   (Wo . W1) columns, 16 per prenet CTA
+  const float* wc;       // [128][1024][2]   (Wo . W1) columns 2c, 2c+1 per CTA
   const float* bc;       // [256]            bo . W1
-  const float* wp2;      // [16][256][16]    prenet fc2 columns
+  const float* wp2;      // [128][256][2]    prenet fc2 columns 2c, 2c+1 per CTA
   const uint8_t* keep;   // [B][N][2][256] or null (indexed with row_base)
   uint64_t seed;
   int mode;
@@ -221,23 +224,22 @@ struct DecScanArgs {
   float* p2;             // [B][256]
   float* h0;             // [2][B][512] compact double-buffered state the recurrence reads (frame parity)
   float* h1;             // [2][B][512]
-  unsigned int* pre_bar; // arrival counter of the prenet CTAs' private barrier (zeroed before the launch)
+  unsigned int* bar;     // arrival counter of the split grid barriers (zeroed before the launch)
   int* err;              // device int set before trapping on a barrier time-out
   float* hout;           // [B][N][1024] decoder outputs [h0_t | h1_t] of every frame (write only): the output projection
                          // runs over the whole tensor as ONE GEMM after the scan
-  int B, N;              // rows of this launch (<= 32), frames
+  int B, N;              // rows of this launch (<= 128), frames
   int row_base;          // first row of this launch inside the full batch (dropout stream indexing)
   int N_total_rows;      // unused
   long long* dbg;        // optional per-CTA phase timers [grid][16]
 };
 
 constexpr int DEC_XR = 32;                 // batch rows per staging group (smem holds the state of one group)
-constexpr int DEC_NG = 4;                  // row groups per launch: up to 128 rows share the three grid barriers of a frame
+constexpr int DEC_NG = 4;                  // row groups per launch: up to 128 rows share the four barriers of a frame
 constexpr int DEC_KPAD = vc::PRENET + 2 * vc::DEC_H + 4;   // 1284: [p2 | h0 | h1] + pad
-// 128 LSTM CTAs + 4 prenet CTAs = the 132 SMs of an H100 SXM (a cooperative grid must be co-resident, one CTA per SM)
-constexpr int DEC_LSTM = 128, DEC_PRE = 4;
-constexpr int DEC_CTAS = DEC_LSTM + DEC_PRE;   // 132
-constexpr int DEC_QPC = 16 / DEC_PRE;          // 16-column blocks of the prenet per prenet CTA
+// a cooperative grid must be co-resident: one CTA per SM, 128 of the 132 SMs of an H100 SXM
+constexpr int DEC_CTAS = 128;
+constexpr int DEC_PCOL = vc::PRENET / DEC_CTAS;   // 2 prenet columns per CTA
 
 // copy rows [0,nr) x [n floats] of a global matrix (row stride `stride`) into smem (row pitch `pitch`, column
 // offset koff); p == nullptr writes zeros.  8 x 16 B loads in flight per thread.
@@ -470,90 +472,63 @@ __device__ __forceinline__ void dec_matmul2(const float* __restrict__ xa, const 
   __syncthreads();
 }
 
-// ---- prenet / projection CTAs: out[32 rows][8 cols] = xs[32][K] . wsm[K][8] ------------------------------
-// thread (rg = tid&3, ks = tid>>2): rows rg+4i (i<8), K slice ks of SL = K/64; weight row k at wsm + k * WLD (the 8
-// columns are contiguous).  Result: outv[row*8 + col] for 32 x 8 outputs.
-template <int SL, int WLD>
-__device__ __forceinline__ void pre_gemm8(const float* __restrict__ xs, int pitch, const float* __restrict__ wsm, float* part, float* outv) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int rg = tid & 3, ks = tid >> 2;
-  float acc[8][8];
+// ---- prenet columns of a CTA: out[r][j] = xs[r][0:K] . w[0:K][j], j = 0, 1, for the staged rows ----------------
+// Warp w owns rows 4w..4w+3 (no cross-warp reduction, no __syncthreads); lane l accumulates k = 128 i + 4 l .. +3
+// (conflict-free float4 reads of xs).  A transposing butterfly (9 shuffles) leaves the sum of row 4w + (l >> 3),
+// column (l >> 2) & 1 in lane l.  w is [K][2] in shared memory.
+template <int K>
+__device__ __forceinline__ float prenet_dot(const float* __restrict__ xs, const float* __restrict__ w, int lane, int warp) {
+  float acc[8];   // [row][col] at 2 * row + col
 #pragma unroll
-  for (int i = 0; i < 8; ++i)
+  for (int v = 0; v < 8; ++v) acc[v] = 0.f;
+  const float* xr = xs + (size_t)(warp * 4) * DEC_KPAD + lane * 4;
+  const float* wr = w + lane * 8;
+#pragma unroll 2
+  for (int i = 0; i < K / 128; ++i) {
+    const float4 wa = *reinterpret_cast<const float4*>(wr + i * 256);       // w[k][0..1], w[k+1][0..1]
+    const float4 wb = *reinterpret_cast<const float4*>(wr + i * 256 + 4);   // w[k+2][0..1], w[k+3][0..1]
 #pragma unroll
-    for (int c = 0; c < 8; ++c) acc[i][c] = 0.f;
-  const float* xk = xs + (size_t)rg * pitch + ks * SL;
-  const float* wk = wsm + (size_t)(ks * SL) * WLD;
-#pragma unroll
-  for (int kk = 0; kk < SL; kk += 4) {
-    float4 xv[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) xv[i] = *reinterpret_cast<const float4*>(xk + (size_t)(4 * i) * pitch + kk);
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float4 wa = __ldg(reinterpret_cast<const float4*>(wk + (size_t)(kk + e) * WLD));
-      const float4 wb = __ldg(reinterpret_cast<const float4*>(wk + (size_t)(kk + e) * WLD + 4));
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float x = e == 0 ? xv[i].x : (e == 1 ? xv[i].y : (e == 2 ? xv[i].z : xv[i].w));
-        acc[i][0] = fmaf(x, wa.x, acc[i][0]); acc[i][1] = fmaf(x, wa.y, acc[i][1]);
-        acc[i][2] = fmaf(x, wa.z, acc[i][2]); acc[i][3] = fmaf(x, wa.w, acc[i][3]);
-        acc[i][4] = fmaf(x, wb.x, acc[i][4]); acc[i][5] = fmaf(x, wb.y, acc[i][5]);
-        acc[i][6] = fmaf(x, wb.z, acc[i][6]); acc[i][7] = fmaf(x, wb.w, acc[i][7]);
-      }
+    for (int r = 0; r < 4; ++r) {
+      const float4 x = *reinterpret_cast<const float4*>(xr + (size_t)r * DEC_KPAD + i * 128);
+      acc[2 * r] = fmaf(x.x, wa.x, acc[2 * r]); acc[2 * r + 1] = fmaf(x.x, wa.y, acc[2 * r + 1]);
+      acc[2 * r] = fmaf(x.y, wa.z, acc[2 * r]); acc[2 * r + 1] = fmaf(x.y, wa.w, acc[2 * r + 1]);
+      acc[2 * r] = fmaf(x.z, wb.x, acc[2 * r]); acc[2 * r + 1] = fmaf(x.z, wb.y, acc[2 * r + 1]);
+      acc[2 * r] = fmaf(x.w, wb.z, acc[2 * r]); acc[2 * r + 1] = fmaf(x.w, wb.w, acc[2 * r + 1]);
     }
   }
-  // butterfly over the 8 K slices of the warp (lane bits 2..4), halving the row set each time
   const bool b4 = lane & 16, b3 = lane & 8, b2 = lane & 4;
-  float a4[4][8];
+  float a4[4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      const float send = b4 ? acc[i][c] : acc[i + 4][c];
-      const float keep = b4 ? acc[i + 4][c] : acc[i][c];
-      a4[i][c] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-    }
-  float a2[2][8];
-#pragma unroll
-  for (int i = 0; i < 2; ++i)
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      const float send = b3 ? a4[i][c] : a4[i + 2][c];
-      const float keep = b3 ? a4[i + 2][c] : a4[i][c];
-      a2[i][c] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-    }
-  float a1[8];
-#pragma unroll
-  for (int c = 0; c < 8; ++c) {
-    const float send = b2 ? a2[0][c] : a2[1][c];
-    const float keep = b2 ? a2[1][c] : a2[0][c];
-    a1[c] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
+  for (int v = 0; v < 4; ++v) {
+    const float send = b4 ? acc[v] : acc[v + 4];
+    const float keep = b4 ? acc[v + 4] : acc[v];
+    a4[v] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
   }
-  // this thread now holds row rg + 4*(lane>>2 & 7) ... = rg + 4*ksl, all 8 columns, summed over the warp's slices
-  const int row = rg + 4 * ((lane >> 2) & 7);
-  float* pw = part + ((size_t)warp * 32 + row) * 8;
-  *reinterpret_cast<float4*>(pw) = make_float4(a1[0], a1[1], a1[2], a1[3]);
-  *reinterpret_cast<float4*>(pw + 4) = make_float4(a1[4], a1[5], a1[6], a1[7]);
-  __syncthreads();
-  {
-    float sum = 0.f;
+  float a2[2];
 #pragma unroll
-    for (int wv = 0; wv < SCAN_THREADS / 32; ++wv) sum += part[(size_t)wv * 256 + tid];
-    outv[tid] = sum;   // tid = row*8 + col
+  for (int v = 0; v < 2; ++v) {
+    const float send = b3 ? a4[v] : a4[v + 2];
+    const float keep = b3 ? a4[v + 2] : a4[v];
+    a2[v] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
   }
-  __syncthreads();
+  float s = (b2 ? a2[1] : a2[0]) + __shfl_xor_sync(0xffffffffu, b2 ? a2[0] : a2[1], 4);
+  s += __shfl_xor_sync(0xffffffffu, s, 2);
+  s += __shfl_xor_sync(0xffffffffu, s, 1);
+  return s;   // value index (lane >> 2) & 7 = 2 * row + col
 }
 
-// Barrier among the DEC_PRE prenet CTAs only (all co-resident: cooperative launch).  The second prenet layer needs every
-// column block of p1 from its peers but nothing from the 128 LSTM CTAs, so a grid-wide barrier here would put the
-// LSTM CTAs' pre-accumulation (6.2 us at 32 rows) on the critical path and cost a full grid.sync.  `target` is the
-// monotonically growing arrival count; a 2 s time-out traps instead of hanging the GPU.
-__device__ __forceinline__ void prenet_barrier(unsigned int* counter, unsigned int target, int* err) {
-  __syncthreads();                                   // this CTA's p1 stores are issued
+// Grid barrier split in two halves (all CTAs are co-resident: cooperative launch).  dec_arrive publishes this CTA's
+// stores and counts it in; work that the barrier does not order can run before dec_wait, which returns once `target`
+// arrivals (a count that grows monotonically over the launch) are in.  A 2 s time-out traps instead of hanging the GPU.
+__device__ __forceinline__ void dec_arrive(unsigned int* counter) {
+  __syncthreads();                                   // this CTA's stores are issued
   if (threadIdx.x == 0) {
     __threadfence();                                 // ... and visible device-wide before the arrival is
     atomicAdd(counter, 1u);
+  }
+}
+__device__ __forceinline__ void dec_wait(const unsigned int* counter, unsigned int target, int* err) {
+  if (threadIdx.x == 0) {
     const long long t0 = clock64();
     unsigned int v;
     do {
@@ -568,192 +543,159 @@ __device__ __forceinline__ void prenet_barrier(unsigned int* counter, unsigned i
   __syncthreads();
 }
 
+__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+
 __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const DecScanArgs a) {
-  cg::grid_group grid = cg::this_grid();
   extern __shared__ __align__(16) float sm[];
   constexpr int H = vc::DEC_H, K0 = vc::PRENET + H, K1 = vc::PRENET + 2 * H;
-  const int c = blockIdx.x, tid = threadIdx.x;
+  const int c = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int B = a.B, N = a.N;
   long long tm[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   long long tq = clock64();
 #define DEC_MARK(i) { const long long tn = clock64(); tm[i] += tn - tq; tq = tn; }
 
-  if (c < DEC_LSTM) {
-    // =============================== LSTM role ===============================
-    float* xs = sm;                                   // [DEC_XR][DEC_KPAD] = [p2 | h0 | h1] of ONE row group at a time
-    float* part = xs + DEC_XR * DEC_KPAD;             // [8][DEC_XR][16]
-    float* zs = part + 8 * DEC_XR * NCOL;             // [DEC_XR][16]
-    float* zp0 = zs + DEC_XR * NCOL;                  // [DEC_NG][DEC_XR][16] pre-accumulated h0_{t-1} . W0[h0 rows]
-    float* zp1 = zp0 + DEC_NG * DEC_XR * NCOL;        // [DEC_NG][DEC_XR][16] pre-accumulated h1_{t-1} . W1[h1 rows]
-    float* cst = zp1 + DEC_NG * DEC_XR * NCOL;        // [DEC_NG][2][DEC_XR][UPC]
-    const int ks = tid >> 2, cgp = tid & 3;
-    constexpr int SLP = vc::PRENET / NSLICE, SLH = H / NSLICE;   // 4, 8
-    // register-resident weight slices, split by input segment so that each segment's product can be
-    // accumulated as soon as that segment is final
-    float w0p[SLP][4], w0h[SLH][4], w1p[SLP][4], w1h0[SLH][4], w1h1[SLH][4];
-    {
-      auto ld = [&](float (&dst)[4], const float* base, int row) {
-        const float4 v = __ldg(reinterpret_cast<const float4*>(base + (size_t)row * NCOL + cgp * 4));
-        dst[0] = v.x; dst[1] = v.y; dst[2] = v.z; dst[3] = v.w;
-      };
-      const float* g0 = a.w0r + (size_t)c * K0 * NCOL;
-      const float* g1 = a.w1r + (size_t)c * K1 * NCOL;
+  float* xs = sm;                                   // [DEC_XR][DEC_KPAD] = [p2 | h0 | h1] of ONE row group at a time
+  float* part = xs + DEC_XR * DEC_KPAD;             // [8][DEC_XR][16]
+  float* zs = part + 8 * DEC_XR * NCOL;             // [DEC_XR][16]
+  float* zp0 = zs + DEC_XR * NCOL;                  // [DEC_NG][DEC_XR][16] pre-accumulated h0_{t-1} . W0[h0 rows]
+  float* zp1 = zp0 + DEC_NG * DEC_XR * NCOL;        // [DEC_NG][DEC_XR][16] pre-accumulated h1_{t-1} . W1[h1 rows]
+  float* cst = zp1 + DEC_NG * DEC_XR * NCOL;        // [DEC_NG][2][DEC_XR][UPC]
+  float* wcs = cst + DEC_NG * 2 * DEC_XR * UPC;     // [1024][2] (Wo . W1) columns 2c, 2c+1
+  float* wp2s = wcs + 2 * H * DEC_PCOL;             // [256][2]  W2 columns 2c, 2c+1
+  const int ks = tid >> 2, cgp = tid & 3;
+  constexpr int SLP = vc::PRENET / NSLICE, SLH = H / NSLICE;   // 4, 8
+  // register-resident weight slices, split by input segment so that each segment's product can be
+  // accumulated as soon as that segment is final
+  float w0p[SLP][4], w0h[SLH][4], w1p[SLP][4], w1h0[SLH][4], w1h1[SLH][4];
+  {
+    auto ld = [&](float (&dst)[4], const float* base, int row) {
+      const float4 v = __ldg(reinterpret_cast<const float4*>(base + (size_t)row * NCOL + cgp * 4));
+      dst[0] = v.x; dst[1] = v.y; dst[2] = v.z; dst[3] = v.w;
+    };
+    const float* g0 = a.w0r + (size_t)c * K0 * NCOL;
+    const float* g1 = a.w1r + (size_t)c * K1 * NCOL;
 #pragma unroll
-      for (int i = 0; i < SLP; ++i) { ld(w0p[i], g0, ks * SLP + i); ld(w1p[i], g1, ks * SLP + i); }
+    for (int i = 0; i < SLP; ++i) { ld(w0p[i], g0, ks * SLP + i); ld(w1p[i], g1, ks * SLP + i); }
 #pragma unroll
-      for (int i = 0; i < SLH; ++i) {
-        ld(w0h[i], g0, vc::PRENET + ks * SLH + i);
-        ld(w1h0[i], g1, vc::PRENET + ks * SLH + i);
-        ld(w1h1[i], g1, vc::PRENET + H + ks * SLH + i);
-      }
+    for (int i = 0; i < SLH; ++i) {
+      ld(w0h[i], g0, vc::PRENET + ks * SLH + i);
+      ld(w1h0[i], g1, vc::PRENET + ks * SLH + i);
+      ld(w1h1[i], g1, vc::PRENET + H + ks * SLH + i);
     }
-    for (int e = tid; e < DEC_NG * 2 * DEC_XR * UPC; e += SCAN_THREADS) cst[e] = 0.f;
-    for (int e = tid; e < DEC_NG * 2 * DEC_XR * NCOL; e += SCAN_THREADS) zp0[e] = 0.f;   // zp0 and zp1 are adjacent
-    for (int e = tid; e < DEC_XR * DEC_KPAD; e += SCAN_THREADS) xs[e] = 0.f;    // rows >= B and the t=0 state are zero
-    __syncthreads();
-    // Rows are processed in groups of DEC_XR (the staging buffer holds one group); all groups of a launch share the
-    // three grid barriers of a frame.  With one group, h0_{t-1} and p2 stay resident in xs between the phases.
-    const int NG = (B + DEC_XR - 1) / DEC_XR;
-    for (int t = 0; t < N; ++t) {
-      // ---- EA window (prenet CTAs are busy): products of the state that is already final ----
-      if (t > 0) {
-        for (int rg = 0; rg < NG; ++rg) {
-          const int r0 = rg * DEC_XR, nb = min(DEC_XR, B - r0), ngroups = (nb + RG - 1) / RG;
-          if (NG > 1) dec_fetch(xs, DEC_KPAD, vc::PRENET, a.h0 + ((size_t)((t - 1) & 1) * B + r0) * H, H, H, nb);
-          dec_fetch(xs, DEC_KPAD, vc::PRENET + H, a.h1 + ((size_t)((t - 1) & 1) * B + r0) * H, H, H, nb);
-          if (NG > 1) __syncthreads();
-          dec_matmul<SLH>(xs + vc::PRENET, w0h, ngroups, part, zp0 + rg * DEC_XR * NCOL, nullptr);     // its barriers also order the h1 fetch
-          dec_matmul<SLH>(xs + vc::PRENET + H, w1h1, ngroups, part, zp1 + rg * DEC_XR * NCOL, nullptr);
-        }
-      }
-      DEC_MARK(0)
-      DEC_MARK(1)
-      DEC_MARK(2)
-      grid.sync();   // p2(t) is ready (the prenet CTAs order their two layers among themselves, see prenet_barrier)
-      DEC_MARK(3)
-      // ---- phase C: LSTM0 = zc0[t] + p2 . W0[p2 rows] + (h0_{t-1} part) ----
+  }
+  {
+    const float4* gc = reinterpret_cast<const float4*>(a.wc + (size_t)c * 2 * H * DEC_PCOL);
+    const float4* g2 = reinterpret_cast<const float4*>(a.wp2 + (size_t)c * vc::PRENET * DEC_PCOL);
+    for (int e = tid; e < 2 * H * DEC_PCOL / 4; e += SCAN_THREADS) reinterpret_cast<float4*>(wcs)[e] = __ldg(gc + e);
+    for (int e = tid; e < vc::PRENET * DEC_PCOL / 4; e += SCAN_THREADS) reinterpret_cast<float4*>(wp2s)[e] = __ldg(g2 + e);
+  }
+  for (int e = tid; e < DEC_NG * 2 * DEC_XR * UPC; e += SCAN_THREADS) cst[e] = 0.f;
+  for (int e = tid; e < DEC_NG * 2 * DEC_XR * NCOL; e += SCAN_THREADS) zp0[e] = 0.f;   // zp0 and zp1 are adjacent
+  for (int e = tid; e < DEC_XR * DEC_KPAD; e += SCAN_THREADS) xs[e] = 0.f;    // rows >= B and the t=0 state are zero
+  __syncthreads();
+  // Rows are processed in groups of DEC_XR (the staging buffer holds one group); all groups of a launch share the
+  // four barriers of a frame.  With one group, h0 and p2 stay resident in xs between the phases.
+  const int NG = (B + DEC_XR - 1) / DEC_XR;
+  const int lastg = NG - 1, nb_last = B - lastg * DEC_XR, ng_last = (nb_last + RG - 1) / RG;
+  const int prow = warp * 4 + (lane >> 3), pj = (lane >> 2) & 1, pu = DEC_PCOL * c + pj;   // prenet_dot result of this lane
+  const bool pw = (lane & 3) == 0;                                                       // ... which this lane stores
+  unsigned int nbar = 0;                                                                 // barriers passed so far
+  for (int t = 0; t < N; ++t) {
+    // ---- phase A: p1(t) = drop(relu([h0 | h1]_{t-1} . Wc + bc)) for this CTA's columns; p1(0) = 0 ----
+    if (t > 0) {
       for (int rg = 0; rg < NG; ++rg) {
         const int r0 = rg * DEC_XR, nb = min(DEC_XR, B - r0), ngroups = (nb + RG - 1) / RG;
-        dec_fetch(xs, DEC_KPAD, 0, a.p2 + (size_t)r0 * vc::PRENET, vc::PRENET, vc::PRENET, nb);
+        if (NG > 1) dec_fetch(xs, DEC_KPAD, vc::PRENET, a.h0 + ((size_t)((t - 1) & 1) * B + r0) * H, H, H, nb);
+        dec_fetch(xs, DEC_KPAD, vc::PRENET + H, a.h1 + ((size_t)((t - 1) & 1) * B + r0) * H, H, H, nb);
         __syncthreads();
-        dec_matmul<SLP>(xs, w0p, ngroups, part, zs, zp0 + rg * DEC_XR * NCOL);
-        if (tid < nb * UPC) {
-          const int r = tid / UPC, uu = tid % UPC, rb = r0 + r;
-          const float* zc = a.zc0 + ((size_t)rb * N + t) * (4 * H) + c * UPC + uu;
-          float* cs = cst + (size_t)rg * 2 * DEC_XR * UPC;
-          float cc = cs[r * UPC + uu];
-          const float h = lstm_cell(zs, r, uu, __ldg(zc), __ldg(zc + H), __ldg(zc + 2 * H), __ldg(zc + 3 * H), cc);
-          cs[r * UPC + uu] = cc;
-          a.h0[((size_t)(t & 1) * B + rb) * H + c * UPC + uu] = h;
-          a.hout[((size_t)rb * N + t) * 2 * H + c * UPC + uu] = h;
+        if (warp * 4 < nb) {
+          const float s = prenet_dot<2 * H>(xs + vc::PRENET, wcs, lane, warp);
+          if (pw && prow < nb) {
+            const float v = fmaxf(s + __ldg(a.bc + pu), 0.f);
+            a.p1[(size_t)(r0 + prow) * vc::PRENET + pu] = v * keep_scale(a.mode, a.keep, a.seed, a.row_base + r0 + prow, t, N, 0, pu);
+          }
         }
-        if (NG > 1) __syncthreads();    // zs and xs are reused by the next group
+        // earlier groups: their h1 leaves xs with the next fetch, so its product is taken now (the barriers inside
+        // dec_matmul also order that fetch after the prenet reads)
+        if (rg < lastg) dec_matmul<SLH>(xs + vc::PRENET + H, w1h1, ngroups, part, zp1 + rg * DEC_XR * NCOL, nullptr);
       }
-      DEC_MARK(4)
-      grid.sync();
-      DEC_MARK(5)
-      // ---- phase D: LSTM1 = zc1[t] + p2 . W1[p2 rows] + h0_t . W1[h0 rows] + (h1_{t-1} part) ----
-      for (int rg = 0; rg < NG; ++rg) {
-        const int r0 = rg * DEC_XR, nb = min(DEC_XR, B - r0), ngroups = (nb + RG - 1) / RG;
-        if (NG > 1) dec_fetch(xs, DEC_KPAD, 0, a.p2 + (size_t)r0 * vc::PRENET, vc::PRENET, vc::PRENET, nb);
-        dec_fetch(xs, DEC_KPAD, vc::PRENET, a.h0 + ((size_t)(t & 1) * B + r0) * H, H, H, nb);
-        __syncthreads();
-        dec_matmul2<SLP, SLH>(xs, w1p, xs + vc::PRENET, w1h0, ngroups, part, zs, zp1 + rg * DEC_XR * NCOL);
-        if (tid < nb * UPC) {
-          const int r = tid / UPC, uu = tid % UPC, rb = r0 + r;
-          const float* zc = a.zc1 + ((size_t)rb * N + t) * (4 * H) + c * UPC + uu;
-          float* cs = cst + (size_t)rg * 2 * DEC_XR * UPC;
-          float cc = cs[(DEC_XR + r) * UPC + uu];
-          const float h = lstm_cell(zs, r, uu, __ldg(zc), __ldg(zc + H), __ldg(zc + 2 * H), __ldg(zc + 3 * H), cc);
-          cs[(DEC_XR + r) * UPC + uu] = cc;
-          a.h1[((size_t)(t & 1) * B + rb) * H + c * UPC + uu] = h;
-          a.hout[((size_t)rb * N + t) * 2 * H + H + c * UPC + uu] = h;
-        }
-        __syncthreads();
-      }
-      DEC_MARK(6)
-      grid.sync();
-      DEC_MARK(7)
+    } else {
+      for (int e = tid; e < B * DEC_PCOL; e += SCAN_THREADS) a.p1[(size_t)(e / DEC_PCOL) * vc::PRENET + DEC_PCOL * c + e % DEC_PCOL] = 0.f;
     }
-  } else if (c < DEC_LSTM + DEC_PRE) {
-    // =============================== prenet role ===============================
-    const int q0 = (c - DEC_LSTM) * DEC_QPC;           // column blocks q0 .. q0 + DEC_QPC - 1 (16 columns each) of p1 and p2
-    constexpr int XP = H + 4;                          // 516: row pitch of the 512-wide staging buffer
-    float* xs = sm;                                    // [32][XP]: h1_{t-1} (EA), p1 (B), h0_t (D window)
-    float* part = xs + 32 * XP;                        // [8][32][8]
-    float* outv = part + 8 * 256;                      // [256]
-    float* pp1 = outv + 256;                           // [DEC_NG][DEC_QPC][2][256] h0 half of p1's pre-activation, one phase early
-    for (int e = tid; e < 32 * XP; e += SCAN_THREADS) xs[e] = 0.f;
-    for (int e = tid; e < DEC_NG * DEC_QPC * 512; e += SCAN_THREADS) pp1[e] = 0.f;
-    __syncthreads();
-    const int orow = tid >> 3, ocol = tid & 7;         // output handled by this thread after a pre_gemm8 pass
-    const int NG = (B + DEC_XR - 1) / DEC_XR;
-    for (int t = 0; t < N; ++t) {
-      // ---- phase EA: p1(t) = drop(relu(pp1 + h1_{t-1} . Wc[512:1024] + bc)) ----
-      if (t > 0) {
-        for (int rg = 0; rg < NG; ++rg) {
-          const int r0 = rg * DEC_XR, nb = min(DEC_XR, B - r0);
-          if (NG > 1) __syncthreads();
-          dec_fetch(xs, XP, 0, a.h1 + ((size_t)((t - 1) & 1) * B + r0) * H, H, H, nb);
-          __syncthreads();
-#pragma unroll 1
-          for (int qh = 0; qh < 2 * DEC_QPC; ++qh) {
-            const int q = q0 + (qh >> 1), hf = qh & 1;
-            pre_gemm8<8, 16>(xs, XP, a.wc + ((size_t)q * 2 * H + H) * 16 + hf * 8, part, outv);
-            if (orow < nb) {
-              const int u = q * 16 + hf * 8 + ocol;
-              const float v = fmaxf(outv[tid] + pp1[(rg * DEC_QPC * 2 + qh) * 256 + tid] + __ldg(a.bc + u), 0.f);
-              a.p1[(size_t)(r0 + orow) * vc::PRENET + u] = v * keep_scale(a.mode, a.keep, a.seed, a.row_base + r0 + orow, t, N, 0, u);
-            }
-          }
-        }
-      } else {
-        for (int e = tid; e < B * 16 * DEC_QPC; e += SCAN_THREADS)
-          a.p1[(size_t)(e / (16 * DEC_QPC)) * vc::PRENET + q0 * 16 + e % (16 * DEC_QPC)] = 0.f;  // prenet(0) = 0
-      }
-      DEC_MARK(0)
-      prenet_barrier(a.pre_bar, (unsigned)DEC_PRE * (unsigned)(t + 1), a.err);   // every column block of p1(t) is in L2
-      DEC_MARK(1)
-      // ---- phase B: p2(t) = drop(relu(p1 . W2)) ----
-      for (int rg = 0; rg < NG; ++rg) {
-        const int r0 = rg * DEC_XR, nb = min(DEC_XR, B - r0);
-        if (NG > 1) __syncthreads();
-        dec_fetch(xs, XP, 0, a.p1 + (size_t)r0 * vc::PRENET, vc::PRENET, vc::PRENET, nb);
-        __syncthreads();
-#pragma unroll 1
-        for (int qh = 0; qh < 2 * DEC_QPC; ++qh) {
-          const int q = q0 + (qh >> 1), hf = qh & 1;
-          pre_gemm8<4, 16>(xs, XP, a.wp2 + (size_t)q * vc::PRENET * 16 + hf * 8, part, outv);
-          if (orow < nb) {
-            const int u = q * 16 + hf * 8 + ocol;
-            const float v = fmaxf(outv[tid], 0.f);
-            a.p2[(size_t)(r0 + orow) * vc::PRENET + u] = v * keep_scale(a.mode, a.keep, a.seed, a.row_base + r0 + orow, t, N, 1, u);
-          }
-        }
-      }
-      DEC_MARK(2)
-      grid.sync();
-      DEC_MARK(3)
-      grid.sync();
-      DEC_MARK(5)
-      // ---- D window: h0_t is final -> its half of p1(t+1)'s pre-activation ----
-      for (int rg = 0; rg < NG; ++rg) {
-        const int r0 = rg * DEC_XR, nb = min(DEC_XR, B - r0);
-        __syncthreads();
-        dec_fetch(xs, XP, 0, a.h0 + ((size_t)(t & 1) * B + r0) * H, H, H, nb);
-        __syncthreads();
-#pragma unroll 1
-        for (int qh = 0; qh < 2 * DEC_QPC; ++qh) {
-          const int q = q0 + (qh >> 1), hf = qh & 1;
-          pre_gemm8<8, 16>(xs, XP, a.wc + (size_t)q * 2 * H * 16 + hf * 8, part, outv);
-          pp1[(rg * DEC_QPC * 2 + qh) * 256 + tid] = outv[tid];
-        }
-      }
+    DEC_MARK(0)
+    dec_arrive(a.bar);
+    if (t > 0) dec_matmul<SLH>(xs + vc::PRENET + H, w1h1, ng_last, part, zp1 + lastg * DEC_XR * NCOL, nullptr);
+    for (int e = tid; e < B * 8; e += SCAN_THREADS) {   // this frame's slices of zc0 / zc1, read in phases C and D
+      const int rb = e >> 3, g = (e >> 1) & 3;
+      prefetch_l2(((e & 1) ? a.zc1 : a.zc0) + ((size_t)rb * N + t) * (4 * H) + g * H + c * UPC);
+    }
+    dec_wait(a.bar, DEC_CTAS * ++nbar, a.err);        // every column of p1(t) is in L2
+    DEC_MARK(1)
+    // ---- phase B: p2(t) = drop(relu(p1(t) . W2)) for this CTA's columns ----
+    for (int rg = 0; rg < NG; ++rg) {
+      const int r0 = rg * DEC_XR, nb = min(DEC_XR, B - r0);
+      if (rg > 0) __syncthreads();    // the previous group's prenet reads are done
+      dec_fetch(xs, DEC_KPAD, 0, a.p1 + (size_t)r0 * vc::PRENET, vc::PRENET, vc::PRENET, nb);
       __syncthreads();
-      DEC_MARK(6)
-      grid.sync();
-      DEC_MARK(7)
+      if (warp * 4 < nb) {
+        const float s = prenet_dot<vc::PRENET>(xs, wp2s, lane, warp);
+        if (pw && prow < nb)
+          a.p2[(size_t)(r0 + prow) * vc::PRENET + pu] = fmaxf(s, 0.f) * keep_scale(a.mode, a.keep, a.seed, a.row_base + r0 + prow, t, N, 1, pu);
+      }
     }
+    DEC_MARK(2)
+    dec_arrive(a.bar);
+    dec_wait(a.bar, DEC_CTAS * ++nbar, a.err);        // every column of p2(t) is in L2
+    DEC_MARK(3)
+    // ---- phase C: LSTM0 = zc0[t] + p2 . W0[p2 rows] + (h0_{t-1} part) ----
+    for (int rg = 0; rg < NG; ++rg) {
+      const int r0 = rg * DEC_XR, nb = min(DEC_XR, B - r0), ngroups = (nb + RG - 1) / RG;
+      dec_fetch(xs, DEC_KPAD, 0, a.p2 + (size_t)r0 * vc::PRENET, vc::PRENET, vc::PRENET, nb);
+      __syncthreads();
+      dec_matmul<SLP>(xs, w0p, ngroups, part, zs, zp0 + rg * DEC_XR * NCOL);
+      if (tid < nb * UPC) {
+        const int r = tid / UPC, uu = tid % UPC, rb = r0 + r;
+        const float* zc = a.zc0 + ((size_t)rb * N + t) * (4 * H) + c * UPC + uu;
+        float* cs = cst + (size_t)rg * 2 * DEC_XR * UPC;
+        float cc = cs[r * UPC + uu];
+        const float h = lstm_cell(zs, r, uu, __ldg(zc), __ldg(zc + H), __ldg(zc + 2 * H), __ldg(zc + 3 * H), cc);
+        cs[r * UPC + uu] = cc;
+        a.h0[((size_t)(t & 1) * B + rb) * H + c * UPC + uu] = h;
+        a.hout[((size_t)rb * N + t) * 2 * H + c * UPC + uu] = h;
+      }
+      if (NG > 1) __syncthreads();    // zs and xs are reused by the next group
+    }
+    DEC_MARK(4)
+    dec_arrive(a.bar);
+    dec_wait(a.bar, DEC_CTAS * ++nbar, a.err);        // h0_t is in L2
+    DEC_MARK(5)
+    // ---- phase D: LSTM1 = zc1[t] + p2 . W1[p2 rows] + h0_t . W1[h0 rows] + (h1_{t-1} part) ----
+    const bool more = t + 1 < N;
+    for (int rg = 0; rg < NG; ++rg) {
+      const int r0 = rg * DEC_XR, nb = min(DEC_XR, B - r0), ngroups = (nb + RG - 1) / RG;
+      if (NG > 1) dec_fetch(xs, DEC_KPAD, 0, a.p2 + (size_t)r0 * vc::PRENET, vc::PRENET, vc::PRENET, nb);
+      dec_fetch(xs, DEC_KPAD, vc::PRENET, a.h0 + ((size_t)(t & 1) * B + r0) * H, H, H, nb);
+      __syncthreads();
+      dec_matmul2<SLP, SLH>(xs, w1p, xs + vc::PRENET, w1h0, ngroups, part, zs, zp1 + rg * DEC_XR * NCOL);
+      if (tid < nb * UPC) {
+        const int r = tid / UPC, uu = tid % UPC, rb = r0 + r;
+        const float* zc = a.zc1 + ((size_t)rb * N + t) * (4 * H) + c * UPC + uu;
+        float* cs = cst + (size_t)rg * 2 * DEC_XR * UPC;
+        float cc = cs[(DEC_XR + r) * UPC + uu];
+        const float h = lstm_cell(zs, r, uu, __ldg(zc), __ldg(zc + H), __ldg(zc + 2 * H), __ldg(zc + 3 * H), cc);
+        cs[(DEC_XR + r) * UPC + uu] = cc;
+        a.h1[((size_t)(t & 1) * B + rb) * H + c * UPC + uu] = h;
+        a.hout[((size_t)rb * N + t) * 2 * H + H + c * UPC + uu] = h;
+      }
+      // earlier groups: h0_t's product for frame t+1 while the rows are staged
+      if (rg < lastg && more) dec_matmul<SLH>(xs + vc::PRENET, w0h, ngroups, part, zp0 + rg * DEC_XR * NCOL, nullptr);
+      __syncthreads();
+    }
+    DEC_MARK(6)
+    dec_arrive(a.bar);
+    if (more) dec_matmul<SLH>(xs + vc::PRENET, w0h, ng_last, part, zp0 + lastg * DEC_XR * NCOL, nullptr);
+    dec_wait(a.bar, DEC_CTAS * ++nbar, a.err);        // h1_t is in L2
+    DEC_MARK(7)
   }
 #undef DEC_MARK
   if (a.dbg && tid == 0)
@@ -912,10 +854,10 @@ constexpr size_t enc_scan_smem() {
   return ((size_t)32 * (vc::ENC_D + 4) + 8 * DEC_XR * NCOL + DEC_XR * NCOL + MAX_ROWS * UPC) * 4;
 }
 constexpr size_t dec_scan_smem() {
-  constexpr size_t lstm = (size_t)DEC_XR * DEC_KPAD + 8 * DEC_XR * NCOL + DEC_XR * NCOL + DEC_NG * (2 * DEC_XR * NCOL + 2 * DEC_XR * UPC);
-  constexpr size_t pre = (size_t)32 * (vc::DEC_H + 4) + 8 * 256 + 256 + DEC_NG * DEC_QPC * 512;
-  return (lstm > pre ? lstm : pre) * 4;
+  return ((size_t)DEC_XR * DEC_KPAD + 8 * DEC_XR * NCOL + DEC_XR * NCOL + DEC_NG * (2 * DEC_XR * NCOL + 2 * DEC_XR * UPC) +
+          (2 * vc::DEC_H + vc::PRENET) * DEC_PCOL) * 4;
 }
+static_assert(dec_scan_smem() <= 227 * 1024, "decoder scan shared memory exceeds the 227 KB of an sm_90 CTA");
 
 // Slot layout shared by the acoustic and the duration model: the TokenEncoder's derived tensors and packed convs
 // come first in both, so that run_token_encoder reads either slot.
@@ -929,10 +871,10 @@ enum {
   D_POST_BNINV0 = D_ENC_COUNT, D_POST_BNINV1, D_POST_BNINV2, D_POST_BNINV3,
   D_DEC_W0R,     // [128][768][16]
   D_DEC_W1R,     // [128][1280][16]
-  D_DEC_WC,      // [16][1024][16]  (Wo . W1) columns
+  D_DEC_WC,      // [128][1024][2]  (Wo . W1) columns 2c, 2c+1 of decoder-scan CTA c
   D_DEC_WCFULL,  // [1024][256] scratch
   D_DEC_BC,      // [256]
-  D_DEC_WP2,     // [128][256][2]
+  D_DEC_WP2,     // [128][256][2]   prenet fc2 columns 2c, 2c+1 of decoder-scan CTA c
   D_ZERO,        // [2048] zeros: bias of the bias-free prenet linears (model.py:88-89) on the generic conv path
   D_COUNT
 };
@@ -1036,10 +978,10 @@ int vtts_acoustic_prepare(vtts_ctx* ctx) {
   for (int i = 0; i < 4; ++i) dn[D_POST_BNINV0 + i] = 512;
   dn[D_DEC_W0R] = (size_t)128 * 768 * 16;
   dn[D_DEC_W1R] = (size_t)128 * 1280 * 16;
-  dn[D_DEC_WC] = (size_t)16 * 1024 * 16;
+  dn[D_DEC_WC] = (size_t)DEC_CTAS * 1024 * DEC_PCOL;
   dn[D_DEC_WCFULL] = (size_t)1024 * 256;
   dn[D_DEC_BC] = 256;
-  dn[D_DEC_WP2] = (size_t)16 * 256 * 16;
+  dn[D_DEC_WP2] = (size_t)DEC_CTAS * 256 * DEC_PCOL;
   dn[D_ZERO] = 2048;
   pk[PK_DEC_L0] = {T[aci::DEC_L0_W], 1, 512, 2048};
   pk[PK_DEC_L1] = {T[aci::DEC_L1_W], 1, 512, 2048};
@@ -1057,8 +999,8 @@ int vtts_acoustic_prepare(vtts_ctx* ctx) {
   repack_cols_kernel<<<512, 256>>>(T[aci::DEC_L0_W], 2048, 512, 768, m.d[D_DEC_W0R], 128, 16, UPC, 512);
   repack_cols_kernel<<<512, 256>>>(T[aci::DEC_L1_W], 2048, 512, 1280, m.d[D_DEC_W1R], 128, 16, UPC, 512);
   precompose_kernel<<<2 * vc::DEC_H + 1, 256>>>(T[aci::PROJ_W], T[aci::PROJ_B], T[aci::PRE1_W], m.d[D_DEC_WCFULL], m.d[D_DEC_BC]);
-  repack_cols_kernel<<<256, 256>>>(m.d[D_DEC_WCFULL], 256, 0, 1024, m.d[D_DEC_WC], 16, 16, 16, 0);
-  repack_cols_kernel<<<64, 256>>>(T[aci::PRE2_W], 256, 0, 256, m.d[D_DEC_WP2], 16, 16, 16, 0);
+  repack_cols_kernel<<<256, 256>>>(m.d[D_DEC_WCFULL], 256, 0, 1024, m.d[D_DEC_WC], DEC_CTAS, DEC_PCOL, DEC_PCOL, 0);
+  repack_cols_kernel<<<64, 256>>>(T[aci::PRE2_W], 256, 0, 256, m.d[D_DEC_WP2], DEC_CTAS, DEC_PCOL, DEC_PCOL, 0);
   VTTS_CUDA(cudaGetLastError());
   rc = vtts_pack_convs(ctx, m, pk);
   if (rc) return rc;
@@ -1114,7 +1056,7 @@ namespace {
 struct AcBufs {
   EncBufs e;
   float *cond, *zc0, *zc1, *melpre, *q0, *q1, *p1, *p2, *hout, *h0, *h1;
-  unsigned int* pre_bar;
+  unsigned int* dec_bar;
 };
 struct TfBufs {
   EncBufs e;
@@ -1140,7 +1082,7 @@ void carve(Arena& ar, int B, int L, int N, AcBufs& w) {
   w.hout = ar.take<float>(BN * 1024);
   w.h0 = ar.take<float>((size_t)2 * MAX_ROWS * 512);
   w.h1 = ar.take<float>((size_t)2 * MAX_ROWS * 512);
-  w.pre_bar = ar.take<unsigned int>(64);
+  w.dec_bar = ar.take<unsigned int>(64);
 }
 void carve(Arena& ar, int B, int L, int N, TfBufs& w) {
   const size_t BN = (size_t)B * N;
@@ -1223,8 +1165,8 @@ int vtts_acoustic_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengt
     da.w0r = D[D_DEC_W0R]; da.w1r = D[D_DEC_W1R]; da.wc = D[D_DEC_WC]; da.bc = D[D_DEC_BC]; da.wp2 = D[D_DEC_WP2];
     da.keep = keep; da.seed = seed; da.mode = mode;
     da.p1 = w.p1; da.p2 = w.p2; da.h0 = w.h0; da.h1 = w.h1; da.hout = w.hout + (size_t)b0 * N * 1024;
-    da.pre_bar = w.pre_bar; da.err = ctx->d_err;
-    VTTS_CUDA(cudaMemsetAsync(w.pre_bar, 0, sizeof(unsigned int), st));
+    da.bar = w.dec_bar; da.err = ctx->d_err;
+    VTTS_CUDA(cudaMemsetAsync(w.dec_bar, 0, sizeof(unsigned int), st));
     da.B = nb; da.N = N; da.row_base = b0; da.dbg = ctx->tc_dbg_on ? ctx->d_tc_dbg : nullptr;
     void* args[] = {&da};
     VTTS_CUDA(cudaLaunchCooperativeKernel((void*)decoder_scan_kernel, dim3(DEC_CTAS), dim3(SCAN_THREADS), args, dec_scan_smem(), st));

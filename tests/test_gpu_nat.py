@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 
+from helpers.threefry import prenet_keep_masks
 from oracle import nat_oracle as no
 from viettts_b200 import synthetic
 
@@ -70,32 +71,11 @@ def test_dropout_off_mode(eng, acoustic_ckpt):
     assert np.abs(mel - ref).max() < MEL_LINF
 
 
-def _threefry2x32(k0, k1, c0, c1):
-    """numpy restatement of the device generator (csrc/nat.cu) for the SEED mode check."""
-    M = np.uint32
-    k0, k1, c0, c1 = (np.asarray(v, dtype=np.uint32) for v in (k0, k1, c0, c1))
-    ks = [k0, k1, M(0x1BD11BDA) ^ k0 ^ k1]
-    x0, x1 = c0 + k0, c1 + k1
-    R = [[13, 15, 26, 6], [17, 29, 16, 24]]
-    with np.errstate(over="ignore"):
-        for blk in range(5):
-            for r in R[blk & 1]:
-                x0 = x0 + x1
-                x1 = (x1 << M(r)) | (x1 >> M(32 - r))
-                x1 = x1 ^ x0
-            x0 = x0 + ks[(blk + 1) % 3]
-            x1 = x1 + ks[(blk + 2) % 3] + M(blk + 1)
-    return x0, x1
-
-
 def test_seed_mode_matches_documented_stream(eng, acoustic_ckpt):
     tk, d, n = _utt(4, 25, 0.8)
     seed = (7 << 32) | 12345
     mel = eng.predict_mel(tk[None], d[None], n_frames=[n], seed=seed)
-    t = np.arange(n, dtype=np.uint32)[:, None, None]
-    lu = (np.arange(2, dtype=np.uint32)[None, :, None] * 256 + np.arange(256, dtype=np.uint32)[None, None, :])
-    o0, _ = _threefry2x32(np.uint32(seed & 0xFFFFFFFF), np.uint32(seed >> 32), t + 0 * lu, lu + 0 * t)
-    masks = (o0 < np.uint32(0x80000000)).astype(np.uint8)[None]
+    masks = prenet_keep_masks(seed, [0], n)
     assert 0.4 < masks.mean() < 0.6
     ref = no.inference(acoustic_ckpt, tk[None], d[None], n, masks).numpy()
     assert np.abs(mel - ref).max() < MEL_LINF
@@ -127,8 +107,9 @@ def test_ragged_batch_equals_single_rows(eng, acoustic_ckpt):
 
 
 def test_batch32_rows_independent(eng, acoustic_ckpt):
-    """Config-3 size (B=32, L=100, N=312): every row must equal that row run alone (bit exact:
-    same kernels, same reduction order), and one row is checked against the oracle."""
+    """Config-3 size (B=32, L=100, N=312): rows 0, 13 and 31 must have the bits of the same row run alone (no kernel of
+    the path sums across rows, and each row's reductions run in an order that does not depend on its position or on
+    the batch size), and one row is checked against the oracle."""
     B = 32
     utts = [_utt(100 + b, 100, 5.0) for b in range(B)]
     tokens = np.stack([u[0] for u in utts])
@@ -140,7 +121,7 @@ def test_batch32_rows_independent(eng, acoustic_ckpt):
     assert np.isfinite(mel).all()
     for b in (0, 13, 31):
         alone = eng.predict_mel(tokens[b : b + 1], dur[b : b + 1], n_frames=nfs[b : b + 1], masks=masks[b : b + 1])
-        assert np.abs(alone[0] - mel[b]).max() < 1e-5
+        assert np.array_equal(alone[0], mel[b]), (b, float(np.abs(alone[0] - mel[b]).max()))
     ref = no.inference(acoustic_ckpt, tokens[7:8], dur[7:8], 312, masks[7:8]).numpy()
     assert np.abs(mel[7] - ref[0]).max() < MEL_LINF
 
@@ -189,7 +170,8 @@ def test_pinned_output_buffer_path(eng, hifigan_params):
 
 
 def test_batch_spanning_two_decoder_launches(eng, acoustic_ckpt):
-    """40 rows = two launches of the 32-row scan kernel: rows must not depend on their launch."""
+    """40 rows = one scan launch with two row groups (32 + 8), the second a single register tile: rows must not depend
+    on their group."""
     B = 40
     utts = [_utt(300 + b, 24, 0.6) for b in range(B)]
     L = 24

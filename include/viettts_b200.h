@@ -48,11 +48,23 @@ typedef enum vtts_status {
   VTTS_ERR_NCCL = -6          /* NCCL missing or a collective failed (vtts_broadcast_weights) */
 } vtts_status;
 
-/* dropout handling for the prenet (vietTTS/nat/model.py:95-100: dropout is live at inference) */
+/* dropout handling for the prenet (vietTTS/nat/model.py:95-100: dropout is live at inference) and, in the
+ * teacher-forced pass, the zoneout of the decoder state (model.py:162-166) */
 typedef enum vtts_dropout_mode {
   VTTS_DROPOUT_OFF = 0,     /* deterministic parity mode: no mask, scale 1 */
   VTTS_DROPOUT_MASK = 1,    /* caller supplies uint8 keep-mask [B,N,2,256]; kept values are scaled by 2 */
-  VTTS_DROPOUT_SEED = 2     /* keep bits drawn on device from threefry2x32(seed; b,t,layer,unit) */
+  VTTS_DROPOUT_SEED = 2,    /* keep bits drawn on device from threefry2x32(key (lo, hi) = seed; b,t,layer,unit) */
+  /* the reference's own JAX/Haiku mask stream, drawn on the device.  seed = (rng[0] << 32) | rng[1], the checkpoint's
+   * `rng` words; threefry key words k0 = seed >> 32, k1 = (uint32)seed (the opposite word order of SEED).  Classic
+   * threefry layout, Haiku next_rng_key() split chain, jax bernoulli bits (viettts_b200/jaxrng.py states the same in numpy).
+   *   inference (acoustic_forward, predict_mel / synthesize / tts_host): frame t, prenet layer l draws
+   *     bernoulli(sub-key 2t + l, 0.5, [1,256]); every row uses these masks, so row b equals the reference run on row b
+   *     alone, independent of B, of the padded N and of its row index.
+   *   teacher forced (acoustic_teacher_forward, gta_host): the reference's whole-batch draws -- 6 sub-keys, keep
+   *     [B,N,256] x2 at p 0.5, then zoneout [B,N,512] x4 at p 0.1 in state order h0, c0, h1, c1 -- over the call's B rows;
+   *     B*N*512 >= 2^32 is rejected.
+   * Mask pointers are ignored and may be NULL. */
+  VTTS_DROPOUT_REFERENCE = 3
 } vtts_dropout_mode;
 
 /* arithmetic of the dense conv contractions (97 % of the FLOPs):
@@ -121,8 +133,8 @@ int vtts_acoustic_forward(vtts_ctx* ctx, const int32_t* tokens_dev, const int32_
 /* AcousticModel.__call__ (vietTTS/nat/model.py:146-169) with is_training=False, the teacher-forced pass gta.py:24-25 runs:
  * mels_in_dev [B,N,80] is the ground-truth mel ALREADY shifted by one frame (gta.py:34-36).  keep_mask_dev uint8
  * [B,N,2,256] prenet keep-masks (kept values x2); zone_mask_dev uint8 [B,N,4,512] zoneout masks in state order
- * (h0, c0, h1, c1), 1 = keep the previous state (Bernoulli(0.1) in the reference, model.py:161-164); mode SEED draws
- * both on the device, OFF disables both.  mel1 = projection output (may be NULL), mel2 = mel1 + postnet(mel1). */
+ * (h0, c0, h1, c1), 1 = keep the previous state (Bernoulli(0.1) in the reference, model.py:161-164); modes SEED and
+ * REFERENCE draw both on the device, OFF disables both.  mel1 = projection output (may be NULL), mel2 = mel1 + postnet(mel1). */
 int vtts_acoustic_teacher_forward(vtts_ctx* ctx, const int32_t* tokens_dev, const int32_t* lengths_dev,
                                   const float* dur_frames_dev, const int32_t* n_frames_dev, const float* mels_in_dev,
                                   const uint8_t* keep_mask_dev, const uint8_t* zone_mask_dev, int dropout_mode, uint64_t seed,
@@ -168,6 +180,12 @@ int vtts_debug_conv_dispatch(vtts_ctx* ctx, int precision, int nprob, const floa
  * Runs on fp16 operands when the context is in VTTS_PRECISION_FP16, on bf16x3 otherwise. */
 int vtts_debug_pair(vtts_ctx* ctx, const float* x_dev, const float* w1_dev, const float* b1_dev, const float* w2_dev,
                     const float* b2_dev, const int32_t* len_dev, int B, int T, int C, int k, int dil, float slope, float* out_dev);
+
+/* test hook: the masks VTTS_DROPOUT_REFERENCE applies for key `seed`, drawn on the device by the scans' own draw
+ * functions, as uint8 (1 = keep).  kind 0: the autoregressive prenet masks [N,2,256] (shared by every row; B ignored);
+ * kind 1: the teacher-forced masks, keep [B,N,2,256] followed by zone [B,N,4,512].  Uses the context's workspace
+ * (later debug_read taps are invalid).  Synchronous. */
+int vtts_debug_dropout_masks(vtts_ctx* ctx, int kind, uint64_t seed, int B, int N, uint8_t* host_out);
 
 /* profiling aid: per-CTA stall counters (SM clocks) of the LAST tensor-core conv launch.
  * Row = CTA, columns: 0 MMA-role total, 1 MMA wait accumulator-free, 2 MMA wait activations, 3 MMA wait
@@ -223,7 +241,8 @@ int vtts_synthesize_host(vtts_ctx* ctx, const int32_t* tokens, const int32_t* le
 /* text2mel (vietTTS/nat/text2mel.py:85-103) + mel2wave (synthesizer.py:36-37) for a batch of token rows in one call:
  * predicted durations -> silence tokens clipped from below at silence_duration, word-end tokens 0 s -> frames ->
  * AcousticModel.inference -> trailing-silence frames cut -> Generator.
- * tokens int32 [B,L]; lengths int32 [B] or NULL; dropout_mode OFF or SEED.  Outputs: dur_sec_out [B,L] adjusted
+ * tokens int32 [B,L]; lengths int32 [B] or NULL; dropout_mode OFF, SEED or REFERENCE (MASK is rejected: the frame
+ * count is only known inside the call).  Outputs: dur_sec_out [B,L] adjusted
  * durations in seconds (may be NULL); n_frames_out int32 [B] frames of each row's waveform; *n_max_out = row pitch in
  * frames; wav = dense [B][256 * n_max] (samples past 256*n_frames_out[b] are 0), capacity B*256*max_frames floats.
  * If n_max > max_frames nothing is synthesized: the call fails with VTTS_ERR_BAD_ARG after setting *n_max_out and

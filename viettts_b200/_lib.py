@@ -32,6 +32,7 @@ SIGNATURES = {
                                            C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "vtts_debug_tc_stats": (C.c_int, [c_ctx, C.c_int, C.c_void_p]),
     "vtts_debug_substages": (C.c_int, [c_ctx, C.c_int, C.c_void_p]),
+    "vtts_debug_dropout_masks": (C.c_int, [c_ctx, C.c_int, C.c_uint64, C.c_int, C.c_int, C.c_void_p]),
     "vtts_debug_pair": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]),
     "vtts_hifigan_blob_floats": (C.c_int64, []),

@@ -647,9 +647,11 @@ int vtts_acoustic_teacher_forward(vtts_ctx* ctx, const int32_t* tokens_dev, cons
                                   float* mel1_dev_or_null, float* mel2_dev, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   if (!tokens_dev || !dur_frames_dev || !mels_in_dev || !mel2_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic_teacher_forward: null pointer");
+  int rc = vtts_teacher_mode_check(ctx, dropout_mode, B, N);
+  if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
-  int rc = ctx->ensure_ws(vtts_acoustic_teacher_ws_bytes(B, L, N));
+  rc = ctx->ensure_ws(vtts_acoustic_teacher_ws_bytes(B, L, N));
   if (rc) return rc;
   stage_begin(ctx, 1, st);
   rc = vtts_acoustic_teacher_run(ctx, tokens_dev, lengths_dev, dur_frames_dev, n_frames_dev, mels_in_dev, keep_mask_dev, zone_mask_dev,
@@ -858,8 +860,10 @@ int vtts_gta_host(vtts_ctx* ctx, const int16_t* wav_i16, const int32_t* wav_leng
     return ctx->fail(VTTS_ERR_BAD_ARG, "gta_host: bad argument (S must be a multiple of %d, >= 512)", vc::HOP);
   if (dropout_mode == VTTS_DROPOUT_MASK && (!keep_mask || !zone_mask)) return ctx->fail(VTTS_ERR_BAD_ARG, "gta_host: MASK mode needs both masks");
   if (!ctx->mel_loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "gta_host: mel filterbank not loaded");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
   const int N = S / vc::HOP;
+  int rc = vtts_teacher_mode_check(ctx, dropout_mode, B, N);
+  if (rc) return rc;
+  VTTS_CUDA(cudaSetDevice(ctx->device));
   Stager s;
   const size_t wav_b = (size_t)B * S * 2, tok_b = (size_t)B * L * 4, len_b = (size_t)B * 4, dur_b = (size_t)B * L * 4, nf_b = (size_t)B * 4;
   const size_t keep_b = dropout_mode == VTTS_DROPOUT_MASK ? (size_t)B * N * 2 * vc::PRENET : 0;
@@ -871,7 +875,7 @@ int vtts_gta_host(vtts_ctx* ctx, const int16_t* wav_i16, const int32_t* wav_leng
   const size_t o_gt = s.take(mel_b), o_out = s.take(mel_b);
   const size_t host_end = s.off;
   const size_t o_wavf = s.take((size_t)B * S * 4), o_in = s.take(mel_b);      // device-only scratch
-  int rc = ctx->ensure_staging(host_end, s.off);
+  rc = ctx->ensure_staging(host_end, s.off);
   if (rc) return rc;
   char* hp = (char*)ctx->hpin;
   char* dp = (char*)ctx->dstage;
@@ -923,8 +927,8 @@ int vtts_tts_host(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, 
   if (!ctx) return VTTS_ERR_BAD_ARG;
   if (!tokens || !n_frames_out || !n_max_out || !wav || B < 1 || L < 1 || max_frames < 1)
     return ctx->fail(VTTS_ERR_BAD_ARG, "tts_host: bad argument");
-  if (dropout_mode != VTTS_DROPOUT_OFF && dropout_mode != VTTS_DROPOUT_SEED)
-    return ctx->fail(VTTS_ERR_BAD_ARG, "tts_host: dropout_mode must be OFF or SEED (the frame count is not known to the caller)");
+  if (dropout_mode != VTTS_DROPOUT_OFF && dropout_mode != VTTS_DROPOUT_SEED && dropout_mode != VTTS_DROPOUT_REFERENCE)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "tts_host: dropout_mode must be OFF, SEED or REFERENCE (the frame count is not known to the caller)");
   VTTS_CUDA(cudaSetDevice(ctx->device));
   std::vector<float> sec((size_t)B * L), frames((size_t)B * L);
   int rc = vtts_predict_duration_host(ctx, tokens, lengths, B, L, sec.data());

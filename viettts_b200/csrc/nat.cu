@@ -52,15 +52,67 @@ __host__ __device__ inline void threefry2x32(uint32_t k0, uint32_t k1, uint32_t 
   o1 = x1;
 }
 
-__device__ __forceinline__ float keep_scale(int mode, const uint8_t* keep, uint64_t seed, int b, int t, int N, int layer, int unit) {
+// jax split(key) in the classic layout: (next key, sub-key) = ((a0, b0), (a1, b1)) with (a0, a1) = threefry(key, (0, 2)),
+// (b0, b1) = threefry(key, (1, 3)); one hk.next_rng_key() call returns the sub-key
+__host__ __device__ inline void jax_split(uint32_t& k0, uint32_t& k1, uint32_t& s0, uint32_t& s1) {
+  uint32_t a0, a1, b0, b1;
+  threefry2x32(k0, k1, 0u, 2u, a0, a1);
+  threefry2x32(k0, k1, 1u, 3u, b0, b1);
+  k0 = a0; k1 = b0; s0 = a1; s1 = b1;
+}
+
+// The one threefry evaluation per mask element of the two on-device streams.
+//   SEED       key (lo, hi) = seed, counter (frame, row << 12 | entry), output 0: a row's stream depends on its row index
+//              in the call and the absolute frame, not on the padded frame count of the batch it happens to share.
+//   REFERENCE  word i of jax random_bits(rkey, n) in the classic layout (n even): i < n/2 is output 0 of
+//              threefry(rkey, (i, i + n/2)), i >= n/2 is output 1 of threefry(rkey, (i - n/2, i)).
+__device__ __forceinline__ uint32_t stream_word(int mode, uint64_t seed, int b, int t, uint32_t entry, uint2 rkey, uint32_t ri, uint32_t rn) {
+  uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32), c0 = (uint32_t)t, c1 = ((uint32_t)b << 12) | entry;
+  bool hi = false;
+  if (mode == VTTS_DROPOUT_REFERENCE) {
+    const uint32_t h = rn >> 1;
+    hi = ri >= h;
+    k0 = rkey.x; k1 = rkey.y; c0 = hi ? ri - h : ri; c1 = c0 + h;
+  }
+  uint32_t o0, o1;
+  threefry2x32(k0, k1, c0, c1, o0, o1);
+  return hi ? o1 : o0;
+}
+
+// prenet dropout scale of (row b, frame t, layer, unit); rkey / ri / rn: the REFERENCE draw this element belongs to
+__device__ __forceinline__ float keep_scale(int mode, const uint8_t* keep, uint64_t seed, int b, int t, int N, int layer, int unit,
+                                            uint2 rkey = make_uint2(0u, 0u), uint32_t ri = 0u, uint32_t rn = 0u) {
   if (mode == VTTS_DROPOUT_OFF) return 1.f;
   if (mode == VTTS_DROPOUT_MASK) return keep[(((size_t)b * N + t) * 2 + layer) * vc::PRENET + unit] ? 2.f : 0.f;
-  uint32_t o0, o1;
-  // counter = (frame, row << 12 | entry): a row's stream depends on its row index in the call and the absolute frame,
-  // not on the padded frame count N of the batch it happens to share
-  (void)N;
-  threefry2x32((uint32_t)seed, (uint32_t)(seed >> 32), (uint32_t)t, ((uint32_t)b << 12) | (uint32_t)(layer * vc::PRENET + unit), o0, o1);
-  return (o0 < 0x80000000u) ? 2.f : 0.f;
+  // bernoulli(0.5) keeps where the word is below 2^31, in both streams
+  return stream_word(mode, seed, b, t, (uint32_t)(layer * vc::PRENET + unit), rkey, ri, rn) < 0x80000000u ? 2.f : 0.f;
+}
+
+// Autoregressive scan, REFERENCE: every row draws what the reference draws for a batch of one -- frame t, layer l uses
+// sub-key 2t + l of the chain (ref_subkey_chain_kernel) and bernoulli(sub, 0.5, [1,256])
+__device__ __forceinline__ float ar_keep_scale(int mode, const uint8_t* keep, uint64_t seed, const uint2* subkeys, int b, int t, int N,
+                                               int layer, int unit) {
+  const uint2 rk = mode == VTTS_DROPOUT_REFERENCE ? subkeys[2 * t + layer] : make_uint2(0u, 0u);
+  return keep_scale(mode, keep, seed, b, t, N, layer, unit, rk, (uint32_t)unit, (uint32_t)vc::PRENET);
+}
+
+// Teacher-forced pass, REFERENCE: the reference draws over the whole batch, bernoulli(key_l, 0.5, [B,N,256]) per layer;
+// b is the row in the call and B its row count (B * N * 512 < 2^32 is checked by the host)
+__device__ __forceinline__ float tf_keep_scale(int mode, const uint8_t* keep, uint64_t seed, uint2 rkey, int b, int t, int B, int N,
+                                               int layer, int unit) {
+  return keep_scale(mode, keep, seed, b, t, N, layer, unit, rkey, ((uint32_t)b * N + t) * vc::PRENET + unit, (uint32_t)B * N * vc::PRENET);
+}
+
+// Sub-keys 0 .. n-1 of the hk.next_rng_key() chain from key (seed >> 32, (uint32)seed), as uint32 pairs.  The chain is
+// sequential: one thread walks it (two independent threefry evaluations per step).
+__global__ void ref_subkey_chain_kernel(uint64_t seed, int n, uint2* __restrict__ out) {
+  if (blockIdx.x != 0 || threadIdx.x != 0) return;
+  uint32_t k0 = (uint32_t)(seed >> 32), k1 = (uint32_t)seed;
+  for (int i = 0; i < n; ++i) {
+    uint32_t s0, s1;
+    jax_split(k0, k1, s0, s1);
+    out[i] = make_uint2(s0, s1);
+  }
 }
 
 // ---- small kernels ---------------------------------------------------------------------------------
@@ -218,6 +270,7 @@ struct DecScanArgs {
   const float* bc;       // [256]            bo . W1
   const float* wp2;      // [128][256][2]    prenet fc2 columns 2c, 2c+1 per CTA
   const uint8_t* keep;   // [B][N][2][256] or null (indexed with row_base)
+  const uint2* subkeys;  // [N][2] REFERENCE sub-keys of the frames' two prenet draws, or null
   uint64_t seed;
   int mode;
   float* p1;             // [B][256]
@@ -612,7 +665,7 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const Dec
           const float s = prenet_dot<2 * H>(xs + vc::PRENET, wcs, lane, warp);
           if (pw && prow < nb) {
             const float v = fmaxf(s + __ldg(a.bc + pu), 0.f);
-            a.p1[(size_t)(r0 + prow) * vc::PRENET + pu] = v * keep_scale(a.mode, a.keep, a.seed, a.row_base + r0 + prow, t, N, 0, pu);
+            a.p1[(size_t)(r0 + prow) * vc::PRENET + pu] = v * ar_keep_scale(a.mode, a.keep, a.seed, a.subkeys, a.row_base + r0 + prow, t, N, 0, pu);
           }
         }
         // earlier groups: their h1 leaves xs with the next fetch, so its product is taken now (the barriers inside
@@ -640,7 +693,7 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const Dec
       if (warp * 4 < nb) {
         const float s = prenet_dot<vc::PRENET>(xs, wp2s, lane, warp);
         if (pw && prow < nb)
-          a.p2[(size_t)(r0 + prow) * vc::PRENET + pu] = fmaxf(s, 0.f) * keep_scale(a.mode, a.keep, a.seed, a.row_base + r0 + prow, t, N, 1, pu);
+          a.p2[(size_t)(r0 + prow) * vc::PRENET + pu] = fmaxf(s, 0.f) * ar_keep_scale(a.mode, a.keep, a.seed, a.subkeys, a.row_base + r0 + prow, t, N, 1, pu);
       }
     }
     DEC_MARK(2)
@@ -730,25 +783,29 @@ struct TfScanArgs {
   const float* w1r;      // [128][1280][16]  rows 512..1791 of lstm1 ([p2, h0, h1]); h0 and h1 rows used
   const uint8_t* zone;   // [B][N][4][512] (h0, c0, h1, c1; 1 = keep the previous state) or null
   uint64_t seed;
-  int mode;              // VTTS_DROPOUT_OFF / MASK / SEED
+  int mode;              // VTTS_DROPOUT_OFF / MASK / SEED / REFERENCE
+  uint2 zkey[4];         // REFERENCE: sub-keys of the four zoneout draws (state order h0, c0, h1, c1)
   float* h0s;            // [2][B][512] zoned hidden state of layer 0, double buffered by frame parity
   float* h1s;            // [2][B][512]
   float* hout;           // [B][N][1024]  decoder outputs [h0n | h1n]
   int B, N;
   int row_base;
+  int B_call;            // rows of the whole call (the REFERENCE draws span the call's batch, not this launch's rows)
 };
 
 constexpr int TF_PITCH = 3 * vc::DEC_H + 4;    // [h0s | h0n | h1s] + pad
 
 // true = keep the previous state.  SEED mode: Bernoulli(0.1) from the same threefry stream as the prenet masks,
-// counter word 1 offset past the prenet's 2*256 entries.
-__device__ __forceinline__ bool zone_keep(int mode, const uint8_t* zone, uint64_t seed, int b, int t, int N, int which, int unit) {
+// counter word 1 offset past the prenet's 2*256 entries.  REFERENCE mode: element (b, t, unit) of the reference's
+// bernoulli(zkey[which], 0.1, [B,N,512]) draw over the call's B rows, with jax's float32 compare.
+__device__ __forceinline__ bool zone_keep(int mode, const uint8_t* zone, uint64_t seed, uint2 rkey, int b, int t, int B, int N, int which,
+                                          int unit) {
   if (mode == VTTS_DROPOUT_OFF) return false;
   if (mode == VTTS_DROPOUT_MASK) return zone[(((size_t)b * N + t) * 4 + which) * vc::DEC_H + unit] != 0;
-  uint32_t o0, o1;
-  (void)N;
-  threefry2x32((uint32_t)seed, (uint32_t)(seed >> 32), (uint32_t)t, ((uint32_t)b << 12) | (uint32_t)(2 * vc::PRENET + which * vc::DEC_H + unit), o0, o1);
-  return o0 < 429496730u;   // 0.1 * 2^32
+  const uint32_t w = stream_word(mode, seed, b, t, (uint32_t)(2 * vc::PRENET + which * vc::DEC_H + unit), rkey,
+                                 ((uint32_t)b * N + t) * vc::DEC_H + unit, (uint32_t)B * N * vc::DEC_H);
+  if (mode == VTTS_DROPOUT_REFERENCE) return __uint_as_float((w >> 9) | 0x3F800000u) - 1.f < 0.1f;
+  return w < 429496730u;   // 0.1 * 2^32
 }
 
 __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_tf_scan_kernel(const TfScanArgs a) {
@@ -805,8 +862,8 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_tf_scan_kernel(const 
         const float c_prev = cst[r * UPC + uu];
         float cc = c_prev;
         const float h = lstm_cell(zs, r, uu, __ldg(zc), __ldg(zc + H), __ldg(zc + 2 * H), __ldg(zc + 3 * H), cc);
-        const bool kh = zone_keep(a.mode, a.zone, a.seed, a.row_base + r, s, N, 0, u);
-        const bool kc = zone_keep(a.mode, a.zone, a.seed, a.row_base + r, s, N, 1, u);
+        const bool kh = zone_keep(a.mode, a.zone, a.seed, a.zkey[0], a.row_base + r, s, a.B_call, N, 0, u);
+        const bool kc = zone_keep(a.mode, a.zone, a.seed, a.zkey[1], a.row_base + r, s, a.B_call, N, 1, u);
         a.hout[((size_t)r * N + s) * 2 * H + u] = h;
         a.h0s[((size_t)(s & 1) * B + r) * H + u] = kh ? xs[(size_t)r * TF_PITCH + u] : h;
         cst[r * UPC + uu] = kc ? c_prev : cc;
@@ -824,8 +881,8 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_tf_scan_kernel(const 
         const float c_prev = cst[(DEC_XR + r) * UPC + uu];
         float cc = c_prev;
         const float h = lstm_cell(zs, r, uu, __ldg(zc), __ldg(zc + H), __ldg(zc + 2 * H), __ldg(zc + 3 * H), cc);
-        const bool kh = zone_keep(a.mode, a.zone, a.seed, a.row_base + r, t, N, 2, u);
-        const bool kc = zone_keep(a.mode, a.zone, a.seed, a.row_base + r, t, N, 3, u);
+        const bool kh = zone_keep(a.mode, a.zone, a.seed, a.zkey[2], a.row_base + r, t, a.B_call, N, 2, u);
+        const bool kc = zone_keep(a.mode, a.zone, a.seed, a.zkey[3], a.row_base + r, t, a.B_call, N, 3, u);
         a.hout[((size_t)r * N + t) * 2 * H + H + u] = h;
         a.h1s[((size_t)(t & 1) * B + r) * H + u] = kh ? xs[(size_t)r * TF_PITCH + 2 * H + u] : h;
         cst[(DEC_XR + r) * UPC + uu] = kc ? c_prev : cc;
@@ -837,14 +894,45 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_tf_scan_kernel(const 
 }
 
 // out[row][c] (row stride out_ld) = relu(x[row][c]) * keep_scale  -- the two prenet dropouts applied to whole sequences
-__global__ void prenet_act_kernel(const float* __restrict__ x, const uint8_t* __restrict__ keep, uint64_t seed, int mode, int layer,
-                                  int B, int N, float* __restrict__ out, int out_ld) {
+// (rkey: the REFERENCE sub-key of this layer's draw)
+__global__ void prenet_act_kernel(const float* __restrict__ x, const uint8_t* __restrict__ keep, uint64_t seed, int mode, uint2 rkey,
+                                  int layer, int B, int N, float* __restrict__ out, int out_ld) {
   const size_t total = (size_t)B * N * vc::PRENET;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int u = (int)(i % vc::PRENET);
     const size_t row = i / vc::PRENET;
     const int b = (int)(row / N), t = (int)(row % N);
-    out[row * out_ld + u] = fmaxf(x[i], 0.f) * keep_scale(mode, keep, seed, b, t, N, layer, u);
+    out[row * out_ld + u] = fmaxf(x[i], 0.f) * tf_keep_scale(mode, keep, seed, rkey, b, t, B, N, layer, u);
+  }
+}
+
+// Test hook kernels: the masks REFERENCE mode applies, through the draw functions of the scans above.
+// [N][2][256] of the autoregressive scan (row 0; every row shares them)
+__global__ void ref_ar_masks_kernel(const uint2* __restrict__ subkeys, int N, uint8_t* __restrict__ out) {
+  const size_t total = (size_t)N * 2 * vc::PRENET;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int u = (int)(i % vc::PRENET), l = (int)((i / vc::PRENET) % 2), t = (int)(i / (2 * vc::PRENET));
+    out[i] = ar_keep_scale(VTTS_DROPOUT_REFERENCE, nullptr, 0, subkeys, 0, t, N, l, u) != 0.f;
+  }
+}
+// teacher-forced pass: keep [B][N][2][256], zone [B][N][4][512]
+__global__ void ref_tf_masks_kernel(uint2 k0, uint2 k1, uint2 z0, uint2 z1, uint2 z2, uint2 z3, int B, int N, uint8_t* __restrict__ keep,
+                                    uint8_t* __restrict__ zone) {
+  const size_t nk = (size_t)B * N * 2 * vc::PRENET, nz = (size_t)B * N * 4 * vc::DEC_H;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nk + nz; i += (size_t)gridDim.x * blockDim.x) {
+    if (i < nk) {
+      const int u = (int)(i % vc::PRENET), l = (int)((i / vc::PRENET) % 2);
+      const size_t row = i / (2 * vc::PRENET);
+      const int b = (int)(row / N), t = (int)(row % N);
+      keep[i] = tf_keep_scale(VTTS_DROPOUT_REFERENCE, nullptr, 0, l ? k1 : k0, b, t, B, N, l, u) != 0.f;
+    } else {
+      const size_t j = i - nk;
+      const int u = (int)(j % vc::DEC_H), w = (int)((j / vc::DEC_H) % 4);
+      const size_t row = j / (4 * vc::DEC_H);
+      const int b = (int)(row / N), t = (int)(row % N);
+      const uint2 zk = w == 0 ? z0 : (w == 1 ? z1 : (w == 2 ? z2 : z3));
+      zone[j] = zone_keep(VTTS_DROPOUT_REFERENCE, nullptr, 0, zk, b, t, B, N, w, u);
+    }
   }
 }
 
@@ -1057,6 +1145,7 @@ struct AcBufs {
   EncBufs e;
   float *cond, *zc0, *zc1, *melpre, *q0, *q1, *p1, *p2, *hout, *h0, *h1;
   unsigned int* dec_bar;
+  uint2* subkeys;   // [N][2] REFERENCE sub-keys
 };
 struct TfBufs {
   EncBufs e;
@@ -1083,6 +1172,7 @@ void carve(Arena& ar, int B, int L, int N, AcBufs& w) {
   w.h0 = ar.take<float>((size_t)2 * MAX_ROWS * 512);
   w.h1 = ar.take<float>((size_t)2 * MAX_ROWS * 512);
   w.dec_bar = ar.take<unsigned int>(64);
+  w.subkeys = ar.take<uint2>((size_t)2 * N);
 }
 void carve(Arena& ar, int B, int L, int N, TfBufs& w) {
   const size_t BN = (size_t)B * N;
@@ -1129,7 +1219,7 @@ int vtts_acoustic_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengt
   if (!ctx->ac.loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "acoustic weights not loaded");
   if (B < 1 || L < 1 || N < 1 || B > MAX_ROWS)
     return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: B=%d L=%d N=%d (1 <= B <= %d rows per call; the host layer chunks larger batches)", B, L, N, MAX_ROWS);
-  if (mode < 0 || mode > 2) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: dropout_mode %d", mode);
+  if (mode < VTTS_DROPOUT_OFF || mode > VTTS_DROPOUT_REFERENCE) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: dropout_mode %d", mode);
   if (mode == VTTS_DROPOUT_MASK && !keep) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: dropout_mode MASK needs keep_mask");
   if (ctx->sm_count < DEC_CTAS) return ctx->fail(VTTS_ERR_NO_DEVICE, "scan kernels need %d SMs, device has %d", DEC_CTAS, ctx->sm_count);
   const AcBufs w = carve_ws<AcBufs>(ctx, B, L, N);
@@ -1156,6 +1246,12 @@ int vtts_acoustic_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengt
   rc = run_convs(ctx, hp, 2, 512, 2048, 1, (int)BN, nullptr, 0, m.tiles(PK_DEC_L0), st);
   if (rc) return rc;
   ctx->sub_mark(3, st);
+  // ---- REFERENCE: the 2N prenet sub-keys of the reference's chain, stream-ordered into the workspace ----
+  if (mode == VTTS_DROPOUT_REFERENCE) {
+    ref_subkey_chain_kernel<<<1, 32, 0, st>>>(seed, 2 * N, w.subkeys);
+    ctx->launches++;
+    VTTS_CUDA(cudaGetLastError());
+  }
   // ---- autoregressive scan: ONE launch for up to DEC_NG * 32 rows (row groups share the grid barriers of a frame) ----
   for (int b0 = 0; b0 < B; b0 += DEC_NG * DEC_XR) {
     const int nb = B - b0 < DEC_NG * DEC_XR ? B - b0 : DEC_NG * DEC_XR;
@@ -1163,7 +1259,7 @@ int vtts_acoustic_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengt
     memset(&da, 0, sizeof(da));
     da.zc0 = w.zc0 + (size_t)b0 * N * 2048; da.zc1 = w.zc1 + (size_t)b0 * N * 2048;
     da.w0r = D[D_DEC_W0R]; da.w1r = D[D_DEC_W1R]; da.wc = D[D_DEC_WC]; da.bc = D[D_DEC_BC]; da.wp2 = D[D_DEC_WP2];
-    da.keep = keep; da.seed = seed; da.mode = mode;
+    da.keep = keep; da.subkeys = w.subkeys; da.seed = seed; da.mode = mode;
     da.p1 = w.p1; da.p2 = w.p2; da.h0 = w.h0; da.h1 = w.h1; da.hout = w.hout + (size_t)b0 * N * 1024;
     da.bar = w.dec_bar; da.err = ctx->d_err;
     VTTS_CUDA(cudaMemsetAsync(w.dec_bar, 0, sizeof(unsigned int), st));
@@ -1179,6 +1275,25 @@ int vtts_acoustic_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengt
   return VTTS_OK;
 }
 
+// the first n sub-keys of the hk.next_rng_key() chain (host side of ref_subkey_chain_kernel, same function)
+static void ref_subkeys_host(uint64_t seed, int n, uint2* out) {
+  uint32_t k0 = (uint32_t)(seed >> 32), k1 = (uint32_t)seed;
+  for (int i = 0; i < n; ++i) {
+    uint32_t s0, s1;
+    jax_split(k0, k1, s0, s1);
+    out[i] = make_uint2(s0, s1);
+  }
+}
+
+int vtts_teacher_mode_check(vtts_ctx* ctx, int mode, int B, int N) {
+  if (mode < VTTS_DROPOUT_OFF || mode > VTTS_DROPOUT_REFERENCE)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic (teacher forced): dropout_mode %d", mode);
+  // the reference's zoneout draws count B*N*512 words with a 32-bit counter
+  if (mode == VTTS_DROPOUT_REFERENCE && (uint64_t)B * (uint64_t)N * vc::DEC_H >= (1ull << 32))
+    return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic (teacher forced): REFERENCE draws need B*N*512 < 2^32 (B=%d N=%d)", B, N);
+  return VTTS_OK;
+}
+
 // AcousticModel.__call__ (model.py:146-169) with is_training=False, as gta.py:24-25 (`val_net`) runs it:
 // encoder -> upsample to the mel length -> prenet of the SHIFTED ground-truth mel (dropout live) -> zoneout decoder
 // scan -> projection -> postnet.  mel1 = projection output (may be null), mel2 = mel1 + postnet(mel1).
@@ -1188,7 +1303,8 @@ int vtts_acoustic_teacher_run(vtts_ctx* ctx, const int32_t* tokens, const int32_
   if (!ctx->ac.loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "acoustic weights not loaded");
   if (B < 1 || L < 1 || N < 1 || B > MAX_ROWS)
     return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic (teacher forced): B=%d L=%d N=%d (1 <= B <= %d rows per call)", B, L, N, MAX_ROWS);
-  if (mode < 0 || mode > 2) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic (teacher forced): dropout_mode %d", mode);
+  int rc = vtts_teacher_mode_check(ctx, mode, B, N);
+  if (rc) return rc;
   if (mode == VTTS_DROPOUT_MASK && (!keep || !zone))
     return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic (teacher forced): dropout_mode MASK needs keep_mask and zone_mask");
   if (ctx->sm_count < SCAN_CTAS) return ctx->fail(VTTS_ERR_NO_DEVICE, "scan kernels need %d SMs, device has %d", SCAN_CTAS, ctx->sm_count);
@@ -1204,8 +1320,11 @@ int vtts_acoustic_teacher_run(vtts_ctx* ctx, const int32_t* tokens, const int32_
   if (mel1) VTTS_CUDA(cudaMemsetAsync(mel1, 0, BN * 80 * sizeof(float), st));
   VTTS_CUDA(cudaMemsetAsync(w.xin, 0, BN * XW * sizeof(float), st));
   VTTS_CUDA(cudaMemsetAsync(w.melpre, 0, BN * 80 * sizeof(float), st));
+  // REFERENCE: the six sub-keys of AcousticModel.__call__ (two prenet dropouts, then the zoneout draws h0, c0, h1, c1)
+  uint2 rk[6] = {};
+  if (mode == VTTS_DROPOUT_REFERENCE) ref_subkeys_host(seed, 6, rk);
   ctx->sub_mark(16, st);
-  int rc = run_token_encoder(ctx, m, tokens, lengths, B, L, w.e, st);
+  rc = run_token_encoder(ctx, m, tokens, lengths, B, L, w.e, st);
   if (rc) return rc;
   rc = run_upsample(ctx, w.e.enc, dur, lengths, n_frames, B, L, N, w.xin, XW, st);   // cond -> columns 0..511 of the decoder input
   if (rc) return rc;
@@ -1216,12 +1335,12 @@ int vtts_acoustic_teacher_run(vtts_ctx* ctx, const int32_t* tokens, const int32_
   const ConvProb pre1 = conv_prob(mels_in, T[aci::PRE1_W], D[D_ZERO], w.pa);
   rc = run_convs(ctx, &pre1, 1, 80, 256, 1, (int)BN, nullptr, 0, m.tiles(PK_PRE1), st);
   if (rc) return rc;
-  prenet_act_kernel<<<act_grid, 256, 0, st>>>(w.pa, keep, seed, mode, 0, B, N, w.pb, 256);
+  prenet_act_kernel<<<act_grid, 256, 0, st>>>(w.pa, keep, seed, mode, rk[0], 0, B, N, w.pb, 256);
   ctx->launches++;
   const ConvProb pre2 = conv_prob(w.pb, T[aci::PRE2_W], D[D_ZERO], w.pa);
   rc = run_convs(ctx, &pre2, 1, 256, 256, 1, (int)BN, nullptr, 0, m.tiles(PK_PRE2), st);
   if (rc) return rc;
-  prenet_act_kernel<<<act_grid, 256, 0, st>>>(w.pa, keep, seed, mode, 1, B, N, w.xin + vc::ENC_OUT, XW);
+  prenet_act_kernel<<<act_grid, 256, 0, st>>>(w.pa, keep, seed, mode, rk[1], 1, B, N, w.xin + vc::ENC_OUT, XW);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   // ---- every input-side product of both LSTMs in one launch: zc = [cond | p2] . W[0:768] + b ----
@@ -1237,8 +1356,9 @@ int vtts_acoustic_teacher_run(vtts_ctx* ctx, const int32_t* tokens, const int32_
     ta.zc0 = w.zc0 + (size_t)b0 * N * 2048; ta.zc1 = w.zc1 + (size_t)b0 * N * 2048;
     ta.w0r = D[D_DEC_W0R]; ta.w1r = D[D_DEC_W1R];
     ta.zone = zone; ta.seed = seed; ta.mode = mode;
+    for (int i = 0; i < 4; ++i) ta.zkey[i] = rk[2 + i];
     ta.h0s = w.h0s; ta.h1s = w.h1s; ta.hout = w.hout + (size_t)b0 * N * 1024;
-    ta.B = nb; ta.N = N; ta.row_base = b0;
+    ta.B = nb; ta.N = N; ta.row_base = b0; ta.B_call = B;
     void* args[] = {&ta};
     VTTS_CUDA(cudaLaunchCooperativeKernel((void*)decoder_tf_scan_kernel, dim3(SCAN_CTAS), dim3(SCAN_THREADS), args, tf_scan_smem(), st));
     ctx->launches++;
@@ -1247,6 +1367,41 @@ int vtts_acoustic_teacher_run(vtts_ctx* ctx, const int32_t* tokens, const int32_
   rc = run_projection_postnet(ctx, w.hout, n_frames, B, N, w.melpre, w.q0, w.q1, mel1, -1, mel2, st);
   ctx->sub_mark(20, st);
   return rc;
+}
+
+// Test hook: the masks REFERENCE mode applies, drawn on the device by the functions the scans call.
+int vtts_debug_dropout_masks(vtts_ctx* ctx, int kind, uint64_t seed, int B, int N, uint8_t* host_out) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  if (!host_out || (kind != 0 && kind != 1) || N < 1 || (kind == 1 && B < 1))
+    return ctx->fail(VTTS_ERR_BAD_ARG, "debug_dropout_masks: kind=%d B=%d N=%d", kind, B, N);
+  if (kind == 1) {
+    const int rc = vtts_teacher_mode_check(ctx, VTTS_DROPOUT_REFERENCE, B, N);
+    if (rc) return rc;
+  }
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  const size_t nk = (size_t)(kind == 0 ? 1 : B) * N * 2 * vc::PRENET, nz = kind == 0 ? 0 : (size_t)B * N * 4 * vc::DEC_H;
+  Arena sz(nullptr, 0, true);
+  sz.take<uint2>((size_t)2 * N);
+  sz.take<uint8_t>(nk + nz);
+  int rc = ctx->ensure_ws(sz.off + 256);
+  if (rc) return rc;
+  Arena ar(ctx->ws, ctx->ws_bytes, false);
+  uint2* subkeys = ar.take<uint2>((size_t)2 * N);
+  uint8_t* d = ar.take<uint8_t>(nk + nz);
+  const size_t blocks = (nk + nz + 255) / 256;
+  const unsigned grid = (unsigned)(blocks < (size_t)ctx->sm_count * 16 ? blocks : (size_t)ctx->sm_count * 16);
+  if (kind == 0) {
+    ref_subkey_chain_kernel<<<1, 32>>>(seed, 2 * N, subkeys);
+    ref_ar_masks_kernel<<<grid, 256>>>(subkeys, N, d);
+  } else {
+    uint2 rk[6];
+    ref_subkeys_host(seed, 6, rk);
+    ref_tf_masks_kernel<<<grid, 256>>>(rk[0], rk[1], rk[2], rk[3], rk[4], rk[5], B, N, d, d + nk);
+  }
+  VTTS_CUDA(cudaGetLastError());
+  VTTS_CUDA(cudaDeviceSynchronize());
+  VTTS_CUDA(cudaMemcpy(host_out, d, nk + nz, cudaMemcpyDeviceToHost));
+  return VTTS_OK;
 }
 
 // =====================================================================================================

@@ -289,6 +289,8 @@ int vtts_acoustic_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengt
                       const int32_t* n_frames, const uint8_t* keep, int mode, uint64_t seed, int B, int L, int N,
                       float* mel, cudaStream_t st);
 size_t vtts_acoustic_teacher_ws_bytes(int B, int L, int N);
+// dropout_mode of a teacher-forced call (0..3; REFERENCE needs B*N*512 < 2^32), checked before any workspace is sized
+int vtts_teacher_mode_check(vtts_ctx* ctx, int mode, int B, int N);
 int vtts_acoustic_teacher_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const float* dur,
                               const int32_t* n_frames, const float* mels_in, const uint8_t* keep, const uint8_t* zone, int mode,
                               uint64_t seed, int B, int L, int N, float* mel1, float* mel2, cudaStream_t st);

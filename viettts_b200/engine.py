@@ -12,13 +12,24 @@ import numpy as np
 
 from . import _lib, config, weights
 
-DROPOUT_OFF, DROPOUT_MASK, DROPOUT_SEED = 0, 1, 2
+DROPOUT_OFF, DROPOUT_MASK, DROPOUT_SEED, DROPOUT_REFERENCE = 0, 1, 2, 3
 
 
 def _chunk_seed(seed: int, chunk: int) -> int:
     """Key of the on-device dropout stream for the chunk-th slice of an over-long batch (a distinct 64-bit key per
     chunk: `seed + offset` would alias the next seed's first chunk)."""
     return (int(seed) ^ (chunk * 0x9E3779B97F4A7C15)) & 0xFFFFFFFFFFFFFFFF
+
+
+def _rng_seed(rng, *others) -> int:
+    """The `seed` argument of VTTS_DROPOUT_REFERENCE for a checkpoint `rng` (uint32[2]): (rng[0] << 32) | rng[1].
+    `others` are the mask / seed arguments of the same call, which must be None alongside `rng`."""
+    if any(o is not None for o in others):
+        raise ValueError("rng= selects the reference's own mask stream; it cannot be combined with masks= or seed=")
+    w = np.asarray(rng).ravel()
+    if w.size != 2 or not np.issubdtype(w.dtype, np.integer):
+        raise ValueError(f"rng must hold exactly two integer words (the checkpoint's uint32[2] rng), got {np.asarray(rng).shape}")
+    return ((int(w[0]) & 0xFFFFFFFF) << 32) | (int(w[1]) & 0xFFFFFFFF)
 PRECISION_FP32, PRECISION_BF16X3, PRECISION_FP16 = 0, 1, 2
 PRECISIONS = {"fp32": PRECISION_FP32, "bf16x3": PRECISION_BF16X3, "fp16": PRECISION_FP16}
 MAX_ACOUSTIC_ROWS = 128   # rows per vtts_acoustic_forward call (csrc/nat.cu MAX_ROWS)
@@ -245,7 +256,8 @@ class Engine:
         precision mode, fused pairs off).  Needs the generator weights and the 'bf16x3' or 'fp16' mode."""
         return VocoderStream(self, max_streams, max_chunk_frames)
 
-    def _acoustic_args(self, tokens, dur_frames, lengths, n_frames, masks, seed):
+    def _acoustic_args(self, tokens, dur_frames, lengths, n_frames, masks, seed, rng=None):
+        ref_seed = None if rng is None else _rng_seed(rng, masks, seed)
         tokens = _np(tokens, np.int32)
         if tokens.ndim != 2:
             raise ValueError("tokens must be [B,L]")
@@ -259,6 +271,8 @@ class Engine:
         N = int(nf.max())
         if N < 1:
             raise ValueError("durations sum to less than one frame")
+        if ref_seed is not None:
+            return tokens, dur, lens, nf, N, None, DROPOUT_REFERENCE, ref_seed
         if masks is not None:
             mode = DROPOUT_MASK
             masks = _np(masks, np.uint8)
@@ -271,12 +285,19 @@ class Engine:
             mode = DROPOUT_OFF
         return tokens, dur, lens, nf, N, masks, mode, int(seed or 0)
 
-    def predict_mel(self, tokens, dur_frames, lengths=None, n_frames=None, masks=None, seed=None) -> np.ndarray:
+    @staticmethod
+    def _call_seed(mode, seed, chunk):
+        # SEED gives every 128-row chunk its own key; the REFERENCE draws do not depend on the row, so every chunk
+        # shares the checkpoint's key
+        return seed if mode == DROPOUT_REFERENCE else _chunk_seed(seed, chunk)
+
+    def predict_mel(self, tokens, dur_frames, lengths=None, n_frames=None, masks=None, seed=None, rng=None) -> np.ndarray:
         """AcousticModel.inference for a (ragged) batch: tokens int [B,L], durations in FRAMES
         [B,L] -> mel f32 [B,N,80] with N = max_b n_frames[b] (rows past n_frames[b] are 0).
         Dropout (live at inference in the reference): `masks` uint8 [B,N,2,256] keep-masks,
-        else `seed` for the on-device threefry stream, else off."""
-        tokens, dur, lens, nf, N, masks, mode, seed = self._acoustic_args(tokens, dur_frames, lengths, n_frames, masks, seed)
+        else `seed` for the on-device threefry stream, else `rng` (the checkpoint's uint32[2]) for the reference's own
+        mask stream drawn on the device (every row gets the masks of the reference run on that row alone), else off."""
+        tokens, dur, lens, nf, N, masks, mode, seed = self._acoustic_args(tokens, dur_frames, lengths, n_frames, masks, seed, rng)
         B, L = tokens.shape
         mel = np.empty((B, N, config.MEL_DIM), np.float32)
         for b0 in range(0, B, MAX_ACOUSTIC_ROWS):
@@ -285,7 +306,7 @@ class Engine:
             out = np.empty((b1 - b0, N, config.MEL_DIM), np.float32)
             self._ck(self.lib.vtts_predict_mel_host(
                 self.h, _ptr(tokens[sl]), _ptr(None if lens is None else lens[sl]), _ptr(dur[sl]), _ptr(nf[sl]),
-                _ptr(None if masks is None else np.ascontiguousarray(masks[sl])), mode, _chunk_seed(seed, b0 // MAX_ACOUSTIC_ROWS),
+                _ptr(None if masks is None else np.ascontiguousarray(masks[sl])), mode, self._call_seed(mode, seed, b0 // MAX_ACOUSTIC_ROWS),
                 b1 - b0, L, N, _ptr(out)))
             mel[sl] = out
         return mel
@@ -324,13 +345,14 @@ class Engine:
 
     _pinned_keepalive: dict = {}
 
-    def synthesize(self, tokens, dur_frames, lengths=None, n_frames=None, masks=None, seed=None, return_mel=False, out=None):
+    def synthesize(self, tokens, dur_frames, lengths=None, n_frames=None, masks=None, seed=None, return_mel=False, out=None, rng=None):
         """predict_mel -> mel2wave with the mel staying on the device.  Returns wav [B,256N]
         (and mel [B,N,80] if return_mel).  `out`: optional preallocated float32 [B,256N] result array
         (ideally from `pinned_empty`); it is validated and written in every path (rows land directly in it).
         In SEED mode row r of a call draws the device stream keyed by (seed, r, frame): an utterance's masks depend on
-        its row index, not on the padded frame count of the batch; MASK / OFF modes are position independent."""
-        tokens, dur, lens, nf, N, masks, mode, seed = self._acoustic_args(tokens, dur_frames, lengths, n_frames, masks, seed)
+        its row index, not on the padded frame count of the batch; MASK / OFF / `rng` (REFERENCE) modes are position
+        independent."""
+        tokens, dur, lens, nf, N, masks, mode, seed = self._acoustic_args(tokens, dur_frames, lengths, n_frames, masks, seed, rng)
         B, L = tokens.shape
         if out is not None and (out.shape != (B, N * config.HOP) or out.dtype != np.float32 or not out.flags.c_contiguous):
             raise ValueError(f"out must be C-contiguous float32 {(B, N * config.HOP)}")
@@ -342,15 +364,17 @@ class Engine:
             # row slices of C-contiguous arrays are contiguous: the library writes straight into the result
             self._ck(self.lib.vtts_synthesize_host(
                 self.h, _ptr(tokens[sl]), _ptr(None if lens is None else lens[sl]), _ptr(dur[sl]), _ptr(nf[sl]),
-                _ptr(None if masks is None else np.ascontiguousarray(masks[sl])), mode, _chunk_seed(seed, b0 // MAX_ACOUSTIC_ROWS),
+                _ptr(None if masks is None else np.ascontiguousarray(masks[sl])), mode, self._call_seed(mode, seed, b0 // MAX_ACOUSTIC_ROWS),
                 b1 - b0, L, N, _ptr(None if mel is None else mel[sl]), _ptr(wav[sl])))
         return (wav, mel) if return_mel else wav
 
-    def tts(self, tokens, lengths=None, silence_duration=-1.0, seed=None, max_frames=None):
+    def tts(self, tokens, lengths=None, silence_duration=-1.0, seed=None, max_frames=None, rng=None):
         """Token rows -> waveforms in ONE library call (vtts_tts_host): duration model, the duration fix-ups of
         text2mel.py:88-97, acoustic model, trailing-silence trim (:99-102) and generator, the mel never leaving
         the device.  tokens int [B,L] (rows padded to L), lengths int [B].  Returns (list of f32 waveforms,
-        durations_sec f32 [B,L])."""
+        durations_sec f32 [B,L]).  Dropout: `seed` for the on-device counter stream (keyed by row index), else `rng`
+        (the checkpoint's uint32[2]) for the reference's own stream (each row as the reference run on it alone), else off."""
+        ref_seed = None if rng is None else _rng_seed(rng, seed)
         tokens = _np(tokens, np.int32)
         if tokens.ndim != 2:
             raise ValueError("tokens must be [B,L]")
@@ -363,6 +387,8 @@ class Engine:
         nmax = C.c_int32(0)
         cap = int(max_frames) if max_frames else max(16, int(L * 0.12 * config.SAMPLE_RATE / config.HOP))
         mode = DROPOUT_SEED if seed is not None else DROPOUT_OFF
+        if ref_seed is not None:
+            mode, seed = DROPOUT_REFERENCE, ref_seed
         for _ in range(2):
             wav = np.empty(B * cap * config.HOP, np.float32)
             rc = self.lib.vtts_tts_host(self.h, _ptr(tokens), _ptr(lens), B, L, float(silence_duration), mode, int(seed or 0),
@@ -375,12 +401,15 @@ class Engine:
         wav = wav[: B * n * config.HOP].reshape(B, n * config.HOP)
         return [wav[b, : int(nf[b]) * config.HOP].copy() for b in range(B)], dur
 
-    def synthesize_many(self, utterances, seed=None, masks=None, max_pad_frac=0.08, max_rows=32):
+    def synthesize_many(self, utterances, seed=None, masks=None, max_pad_frac=0.08, max_rows=32, rng=None):
         """Mixed-length workload (BASELINE configs[4]): `utterances` is a list of (tokens list[int],
         durations_in_frames f32[L]).  They are bucketed by frame count so that padding stays below
         `max_pad_frac`, each bucket runs as one ragged batch, and the waveforms come back in input order
-        (list of np.float32 [256*n_frames_i]).  Row i of any bucket equals utterance i run alone."""
+        (list of np.float32 [256*n_frames_i]).  Row i of any bucket equals utterance i run alone (with `rng`, the
+        reference's own dropout stream, that includes its masks)."""
         from .parallel import bucket_by_length
+        if rng is not None:
+            _rng_seed(rng, masks, seed)
         nfs = [int(np.sum(np.asarray(d, np.float32), dtype=np.float32)) for _, d in utterances]
         out = [None] * len(utterances)
         for bucket in bucket_by_length(nfs, max_pad_frac, max_rows):
@@ -397,25 +426,31 @@ class Engine:
             m = None if masks is None else np.stack([np.asarray(masks[i])[: nf.max()] if np.asarray(masks[i]).shape[0] >= nf.max()
                                                      else np.pad(np.asarray(masks[i]), ((0, nf.max() - np.asarray(masks[i]).shape[0]), (0, 0), (0, 0)))
                                                      for i in bucket])
-            wav = self.synthesize(tok, dur, lengths=lens, n_frames=nf, masks=m, seed=seed)
+            wav = self.synthesize(tok, dur, lengths=lens, n_frames=nf, masks=m, seed=seed, rng=rng)
             for r, i in enumerate(bucket):
                 out[i] = wav[r, : nfs[i] * config.HOP].copy()
         return out
 
-    def _tf_masks(self, B, N, keep_masks, zone_masks, seed):
+    def _tf_masks(self, B, N, keep_masks, zone_masks, seed, rng=None):
+        """(keep, zone, mode, seed) of a teacher-forced call."""
+        if rng is not None:
+            return None, None, DROPOUT_REFERENCE, _rng_seed(rng, keep_masks, zone_masks, seed)
         if keep_masks is not None or zone_masks is not None:
             if keep_masks is None or zone_masks is None:
                 raise ValueError("keep_masks and zone_masks must be given together")
             km = _np(keep_masks, np.uint8, (B, N, 2, config.PRENET_DIM), "keep_masks")
             zm = _np(zone_masks, np.uint8, (B, N, 4, config.ACOUSTIC_DECODER_DIM), "zone_masks")
-            return km, zm, DROPOUT_MASK
-        return None, None, (DROPOUT_SEED if seed is not None else DROPOUT_OFF)
+            return km, zm, DROPOUT_MASK, 0
+        return None, None, (DROPOUT_SEED if seed is not None else DROPOUT_OFF), int(seed or 0)
 
-    def teacher_forced(self, tokens, dur_frames, mels_in, lengths=None, n_frames=None, keep_masks=None, zone_masks=None, seed=None):
+    def teacher_forced(self, tokens, dur_frames, mels_in, lengths=None, n_frames=None, keep_masks=None, zone_masks=None, seed=None,
+                       rng=None):
         """AcousticModel.__call__ (nat/model.py:146-169, is_training=False): tokens int [B,L], durations in frames
         [B,L], mels_in f32 [B,N,80] (ground truth shifted by one frame) -> (mel1, mel2) f32 [B,N,80].
         keep_masks uint8 [B,N,2,256] / zone_masks uint8 [B,N,4,512] (1 = keep previous state), else `seed` for the
-        on-device stream, else both off.  Host buffers; the device work is vtts_acoustic_teacher_forward."""
+        on-device stream, else `rng` (the checkpoint's uint32[2]) for the reference's own whole-batch draws on the
+        device (= jaxrng.teacher_forced_masks(rng, B, N)), else both off.  Host buffers; the device work is
+        vtts_acoustic_teacher_forward."""
         import torch
         tokens = _np(tokens, np.int32)
         B, L = tokens.shape
@@ -425,7 +460,7 @@ class Engine:
             raise ValueError(f"mels_in must be [B,N,{config.MEL_DIM}]")
         if B > MAX_ACOUSTIC_ROWS:
             raise ValueError(f"teacher_forced: at most {MAX_ACOUSTIC_ROWS} rows per call")
-        km, zm, mode = self._tf_masks(B, N, keep_masks, zone_masks, seed)
+        km, zm, mode, seed = self._tf_masks(B, N, keep_masks, zone_masks, seed, rng)
         dev = torch.device("cuda", self.device)
         up = lambda a: None if a is None else torch.from_numpy(np.ascontiguousarray(a)).to(dev)   # noqa: E731
         t_tok, t_dur, t_in = up(tokens), up(_np(dur_frames, np.float32, (B, L), "durations")), up(mels_in)
@@ -436,13 +471,14 @@ class Engine:
         m2 = torch.empty_like(m1)
         st = torch.cuda.current_stream(dev).cuda_stream
         self._ck(self.lib.vtts_acoustic_teacher_forward(self.h, _ptr(t_tok), _ptr(t_len), _ptr(t_dur), _ptr(t_nf), _ptr(t_in), _ptr(t_km),
-                                                        _ptr(t_zm), mode, int(seed or 0), B, L, N, _ptr(m1), _ptr(m2), st))
+                                                        _ptr(t_zm), mode, seed, B, L, N, _ptr(m1), _ptr(m2), st))
         torch.cuda.synchronize(dev)
         return m1.cpu().numpy(), m2.cpu().numpy()
 
-    def gta(self, wav_i16, tokens, dur_sec, lengths=None, wav_lengths=None, keep_masks=None, zone_masks=None, seed=None, return_gt=False):
+    def gta(self, wav_i16, tokens, dur_sec, lengths=None, wav_lengths=None, keep_masks=None, zone_masks=None, seed=None, return_gt=False,
+            rng=None):
         """forward_fn of nat/gta.py:28-44 in one library call: int16 wavs [B,S] + aligned phonemes -> mel2_hat
-        f32 [B,S/256,80] (rows past wav_lengths[b]//256 are 0)."""
+        f32 [B,S/256,80] (rows past wav_lengths[b]//256 are 0).  Masks as in `teacher_forced`."""
         if not self._mel_loaded:
             self.load_mel_filterbank()
         wav = np.ascontiguousarray(np.asarray(wav_i16))
@@ -456,13 +492,13 @@ class Engine:
         if B > MAX_ACOUSTIC_ROWS:
             raise ValueError(f"gta: at most {MAX_ACOUSTIC_ROWS} rows per call")
         N = S // config.HOP
-        km, zm, mode = self._tf_masks(B, N, keep_masks, zone_masks, seed)
+        km, zm, mode, seed = self._tf_masks(B, N, keep_masks, zone_masks, seed, rng)
         lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
         wl = None if wav_lengths is None else _np(wav_lengths, np.int32, (B,), "wav_lengths")
         gt = np.empty((B, N, config.MEL_DIM), np.float32) if return_gt else None
         out = np.empty((B, N, config.MEL_DIM), np.float32)
         self._ck(self.lib.vtts_gta_host(self.h, _ptr(wav), _ptr(wl), _ptr(tokens), _ptr(lens), _ptr(_np(dur_sec, np.float32, (B, L), "durations")),
-                                        _ptr(km), _ptr(zm), mode, int(seed or 0), B, L, S, _ptr(gt), _ptr(out)))
+                                        _ptr(km), _ptr(zm), mode, seed, B, L, S, _ptr(gt), _ptr(out)))
         return (out, gt) if return_gt else out
 
     def melspec(self, wav) -> np.ndarray:
@@ -492,13 +528,30 @@ class Engine:
         self._ck(self.lib.vtts_hifigan_forward(self.h, _ptr(mel_t), _ptr(n_frames_t), B, T, _ptr(out), st))
         return out
 
-    def acoustic_forward(self, tokens_t, dur_t, N, lengths_t=None, n_frames_t=None, masks_t=None, seed=None, out=None, stream=None):
+    def debug_dropout_masks(self, kind, rng, B, N) -> np.ndarray:
+        """Test hook (vtts_debug_dropout_masks): the masks the `rng` (REFERENCE) mode applies, drawn on the device.
+        kind 0: autoregressive prenet masks uint8 [N,2,256]; kind 1: teacher-forced (keep [B,N,2,256], zone [B,N,4,512])."""
+        seed = _rng_seed(rng)
+        nk = (1 if kind == 0 else B) * N * 2 * config.PRENET_DIM
+        nz = 0 if kind == 0 else B * N * 4 * config.ACOUSTIC_DECODER_DIM
+        out = np.empty(nk + nz, np.uint8)
+        self._ck(self.lib.vtts_debug_dropout_masks(self.h, int(kind), seed, int(B), int(N), _ptr(out)))
+        if kind == 0:
+            return out.reshape(N, 2, config.PRENET_DIM)
+        return out[:nk].reshape(B, N, 2, config.PRENET_DIM), out[nk:].reshape(B, N, 4, config.ACOUSTIC_DECODER_DIM)
+
+    def acoustic_forward(self, tokens_t, dur_t, N, lengths_t=None, n_frames_t=None, masks_t=None, seed=None, out=None, stream=None,
+                         rng=None):
+        """vtts_acoustic_forward on torch CUDA tensors, stream-ordered.  Dropout: masks_t, else seed, else rng (the
+        reference's own stream drawn on the device), else off."""
         import torch
         assert tokens_t.is_cuda and tokens_t.dtype == torch.int32 and dur_t.dtype == torch.float32
         B, L = tokens_t.shape
         if out is None:
             out = torch.empty((B, N, config.MEL_DIM), dtype=torch.float32, device=tokens_t.device)
         mode = DROPOUT_MASK if masks_t is not None else (DROPOUT_SEED if seed is not None else DROPOUT_OFF)
+        if rng is not None:
+            mode, seed = DROPOUT_REFERENCE, _rng_seed(rng, masks_t, seed)
         st = torch.cuda.current_stream(tokens_t.device).cuda_stream if stream is None else stream
         self._ck(self.lib.vtts_acoustic_forward(self.h, _ptr(tokens_t), _ptr(lengths_t), _ptr(dur_t), _ptr(n_frames_t),
                                                 _ptr(masks_t), mode, int(seed or 0), B, L, int(N), _ptr(out), st))

@@ -5,8 +5,10 @@ The reference keeps prenet dropout live at inference and seeds it from the check
 (`key, sub = jax.random.split(key)`) and `hk.dropout` draws `jax.random.bernoulli(sub, 0.5, x.shape)`.  Both are
 defined on the counter-based threefry2x32 generator, so the masks are a pure function of the two rng words and can be
 reproduced without JAX.  This module restates that function in numpy (host side; a few hundred thousand block-cipher
-evaluations per utterance) and the masks go to the device through the existing VTTS_DROPOUT_MASK path, which makes the
-drop-in `predict_mel` / GTA `forward_fn` sample-wise (not just statistically) equal to the reference.
+evaluations per utterance).  The library draws the same masks on the device (VTTS_DROPOUT_REFERENCE, `rng=` in
+`Engine`), which makes the drop-in `predict_mel` / GTA `forward_fn` sample-wise (not just statistically) equal to the
+reference; this module is the host oracle the tests compare the device's masks with, and a source of explicit masks
+for the VTTS_DROPOUT_MASK path.
 
 Layout restated (jax/_src/prng.py, the classic layout, `jax_threefry_partitionable=False`, the default of every jax
 release the 2021 reference can run on):

@@ -10,7 +10,7 @@ from pathlib import Path
 
 import numpy as np
 
-from .. import config, jaxrng
+from .. import config
 from .text2mel import checkpoint_rng, load_acoustic
 
 
@@ -20,11 +20,11 @@ def forward_fn(wavs, phonemes, lengths, durations, wav_lengths=None, keep_masks=
     sees `wav_lengths` (the postnet runs over all S/256 frames; gta.py:70-76 only slices `mel[idx, :l]` when saving),
     so `wav_lengths` is accepted for signature compatibility and used by `save_batch` alone.
     Masks: `keep_masks`/`zone_masks` explicitly, else `seed` for the library's on-device stream, else (default) the
-    masks the reference itself draws from the checkpoint's rng (Haiku split chain, `viettts_b200.jaxrng`)."""
+    masks the reference itself draws from the checkpoint's rng (Haiku split chain, whole-batch draws), drawn on the
+    device."""
     engine, _ = load_acoustic(engine)
     if keep_masks is None and seed is None:
-        wavs_a = np.asarray(wavs)
-        keep_masks, zone_masks = jaxrng.teacher_forced_masks(checkpoint_rng(), wavs_a.shape[0], wavs_a.shape[1] // config.HOP)
+        return engine.gta(wavs, phonemes, durations, lengths=lengths, wav_lengths=None, rng=checkpoint_rng())
     return engine.gta(wavs, phonemes, durations, lengths=lengths, wav_lengths=None, keep_masks=keep_masks,
                       zone_masks=zone_masks, seed=seed)
 

@@ -8,20 +8,20 @@ N = int(sum(durations*16000/256)).
 
 Dropout: the reference applies prenet dropout at inference with the
 checkpoint's `rng` through Haiku's split chain on JAX's threefry generator
-(nat/model.py:95-100,132).  That is a pure function of the two rng words, which
-`viettts_b200.jaxrng` restates on the host, so by default `predict_mel` feeds the
-device exactly the keep-masks the reference would draw (sample-wise parity with
-the JAX path, classic threefry layout).  `seed=` selects the library's own
-on-device counter stream instead (no host mask generation, used by the batched
-throughput paths), `masks=` (uint8 [1,N,2,256]) supplies masks explicitly, and
-`dropout=False` is the deterministic mode."""
+(nat/model.py:95-100,132).  That is a pure function of the two rng words, so by
+default `predict_mel` has the device draw exactly the keep-masks the reference
+would draw (the library's REFERENCE dropout mode: sample-wise parity with the JAX
+path, classic threefry layout; `viettts_b200.jaxrng` states the same function in
+numpy).  `seed=` selects the library's own on-device counter stream instead,
+`masks=` (uint8 [1,N,2,256]) supplies masks explicitly, and `dropout=False` is
+the deterministic mode."""
 from __future__ import annotations
 
 import os
 
 import numpy as np
 
-from .. import config, jaxrng
+from .. import config
 from ..engine import get_engine
 from ..weights import load_pickle
 
@@ -72,10 +72,11 @@ def predict_mel(tokens, durations, masks=None, dropout=True, seed=None):
     tokens = np.array(tokens, dtype=np.int32)[None, :]
     d = d.reshape(1, -1)
     if not dropout:
-        masks, seed = None, None
-    elif masks is None and seed is None:
-        # the reference's own stream: hk.next_rng_key() chain from the checkpoint rng, two [1,256] draws per frame
-        masks = jaxrng.inference_keep_masks(checkpoint_rng(), 1, n_frames)
+        return engine.predict_mel(tokens, d, n_frames=[n_frames])
+    if masks is None and seed is None:
+        # the reference's own stream, drawn on the device: hk.next_rng_key() chain from the checkpoint rng, two [1,256]
+        # draws per frame
+        return engine.predict_mel(tokens, d, n_frames=[n_frames], rng=checkpoint_rng())
     return engine.predict_mel(tokens, d, n_frames=[n_frames], masks=masks, seed=seed if masks is None else None)
 
 

@@ -66,15 +66,18 @@ def read_wav(path):
     return np.frombuffer(raw[44:44 + n], "<i2").astype(np.float32) / 32767.0, sr
 
 
-def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_rows=32, engine=None):
+def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_rows=32, engine=None, rng=None):
     """Batched text -> list of waveforms (input order).  Lines are sorted by token count and cut into batches of
-    at most `max_rows` rows so the padding inside a batch stays small; every batch is one `Engine.tts` call."""
+    at most `max_rows` rows so the padding inside a batch stays small; every batch is one `Engine.tts` call.
+    Dropout: `rng` (the checkpoint's uint32[2], `text2mel.checkpoint_rng()`) draws the reference's own mask stream on
+    the device, so each line sounds as it does alone through `text2mel`; otherwise the on-device counter stream keyed
+    by `seed` (default: the checkpoint's rng words), whose masks depend on the line's row in its batch."""
     from .nat import text2mel as t2m
     from .hifigan.mel2wave import load_generator
     engine = t2m.load_duration(engine)
     _, ck_seed = t2m.load_acoustic(engine)
-    if seed is None:
-        seed = ck_seed          # default stream key: the checkpoint's rng words, same as the single --text path
+    if seed is None and rng is None:
+        seed = ck_seed          # default stream key: the checkpoint's rng words
     load_generator(engine)
     toks = [t2m.text2tokens(nat_normalize_text(line), lexicon_file) for line in lines]
     order = sorted(range(len(toks)), key=lambda i: len(toks[i]))
@@ -87,7 +90,7 @@ def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_
         for r, i in enumerate(idx):
             tok[r, : len(toks[i])] = toks[i]
             lens[r] = len(toks[i])
-        waves, _ = engine.tts(tok, lens, silence_duration=silence_duration, seed=seed)
+        waves, _ = engine.tts(tok, lens, silence_duration=silence_duration, seed=seed, rng=rng)
         for r, i in enumerate(idx):
             out[i] = waves[r]
     return out
@@ -103,12 +106,20 @@ def main(argv=None) -> int:
     parser.add_argument("--lexicon-file", default=None)
     parser.add_argument("--seed", default=None, type=int,
                         help="prenet dropout: key of the on-device counter stream; default = the checkpoint's rng "
-                             "(--text: the reference's own JAX/Haiku mask stream; --text-file: the device stream keyed by those words)")
+                             "(--text: the reference's own JAX/Haiku mask stream, drawn on the device; --text-file: the "
+                             "counter stream keyed by those words, see --reference-dropout)")
+    parser.add_argument("--reference-dropout", action="store_true",
+                        help="with --text-file: draw the reference's own JAX/Haiku mask stream from the checkpoint's rng "
+                             "for every line, so each line's audio is the --text audio of that line (not with --seed)")
     parser.add_argument("--precision", default=None, choices=["bf16x3", "fp16", "fp32"],
                         help="conv arithmetic (default bf16x3, the library default): bf16x3 = fp32-class split-bf16 tensor-core "
                              "products; fp16 = fast generator, one fp16 product per operand pair (waveform within ~1e-3 of "
                              "bf16x3), every other model as bf16x3; fp32 = strict FMA pipe")
     args = parser.parse_args(argv)
+    if args.reference_dropout and args.text_file is None:
+        parser.error("--reference-dropout applies to --text-file (--text always uses the reference's stream)")
+    if args.reference_dropout and args.seed is not None:
+        parser.error("--reference-dropout and --seed select different dropout streams; give one")
     lexicon = args.lexicon_file if args.lexicon_file is not None else config.LEXICON_FILE
     if args.precision is not None:
         from .engine import get_engine
@@ -116,7 +127,11 @@ def main(argv=None) -> int:
 
     if args.text_file is not None:
         lines = [ln for ln in args.text_file.read_text().splitlines() if ln.strip()]
-        waves = synthesize_lines(lines, lexicon, args.silence_duration, seed=args.seed)
+        rng = None
+        if args.reference_dropout:
+            from .nat.text2mel import checkpoint_rng
+            rng = checkpoint_rng()
+        waves = synthesize_lines(lines, lexicon, args.silence_duration, seed=args.seed, rng=rng)
         for i, w in enumerate(waves):
             fn = args.output.with_name(f"{args.output.stem}_{i:04d}{args.output.suffix or '.wav'}")
             print("writing output to file", fn)

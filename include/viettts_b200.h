@@ -152,7 +152,9 @@ int vtts_duration_forward(vtts_ctx* ctx, const int32_t* tokens_dev, const int32_
 int vtts_melspec(vtts_ctx* ctx, const float* wav_dev, int B, int S, float* mel_dev, void* stream);
 
 /* optional taps for tests: copy an internal activation of the LAST forward call to host.
- * name: "enc" [B,L,512] (of the last acoustic OR duration call), "cond" [B,N,512], "mel_pre" [B,N,80] (before the postnet). */
+ * name: "enc" [B,L,512] (of the last acoustic OR duration call), "cond" [B,N,512], "mel_pre" [B,N,80] (before the postnet;
+ * after an acoustic stream push: the stream's [max_streams, max_frames, 80] projection outputs, valid for the frames
+ * each slot has scanned). */
 int vtts_debug_read(vtts_ctx* ctx, const char* name, float* host_out, int64_t n_floats);
 
 /* test hook: one hk.Conv1D (SAME padding, dilation, optional leaky_relu on the input and residual
@@ -225,6 +227,45 @@ int vtts_vocoder_stream_push(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float
 /* the same on host buffers mel [S][F][80] and wav [S][256*(F+D)]; returns when wav is written */
 int vtts_vocoder_stream_push_host(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float* mel, const int32_t* n_new,
                                   const uint8_t* flags, float* wav, int32_t* n_out);
+
+/* ---- streaming acoustic model: every slot advances its decoder a few frames per push ---------------------------
+ * A vtts_acoustic_stream holds max_streams (1..128) independent slots.  begin starts utterances in closed slots; each
+ * push advances every open slot by min(F, frames left) decoder steps in ONE scan launch and returns the mel frames whose
+ * postnet receptive field is complete: after P frames scanned a slot has emitted min(n_emit, max(0, P - D_a)) frames
+ * (D_a = vtts_acoustic_stream_lookahead() = 10, the five k = 5 postnet convs), and the push that finishes its scan emits
+ * the rest and closes the slot.  A slot scans min(n_frames, n_emit + D_a) frames.  Each utterance's emitted frames,
+ * concatenated, are bit-identical to the first n_emit frames of vtts_acoustic_forward of that utterance alone, in the
+ * same precision mode (FP32 or BF16X3; FP16 runs as BF16X3) and dropout mode:
+ *   OFF; SEED with the slot index as the row (slot s reproduces row s of a call with the same seed); MASK with the
+ *   masks given at begin; REFERENCE with the key given at create (the sub-key chain of 2 * max_frames keys is drawn once).
+ * Memory: the stream allocates at create, per slot max_frames * (16 KiB zc0 / zc1 + 320 B melpre [+ 512 B MASK keep])
+ * + 8 KiB of carried state, plus per-push buffers that grow with max_streams * max_chunk_frames.  max_frames and
+ * max_tokens are checked against what vtts_acoustic_forward accepts. */
+typedef struct vtts_acoustic_stream vtts_acoustic_stream;
+int vtts_acoustic_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_frames, int max_frames, int max_tokens, int dropout_mode,
+                                uint64_t seed, vtts_acoustic_stream** out);
+int vtts_acoustic_stream_destroy(vtts_ctx* ctx, vtts_acoustic_stream* as);
+int vtts_acoustic_stream_lookahead(void);                    /* D_a = 10 mel frames */
+/* Start nb utterances (host buffers; synchronous, not on the hot path): slots int32 [nb] distinct closed slots; tokens
+ * int32 [nb,L] (L <= max_tokens); lengths int32 [nb] or NULL (= L); dur_frames [nb,L] durations in frames; n_frames
+ * int32 [nb] in [1, max_frames]; n_emit int32 [nb] frames to emit, in [1, n_frames], or NULL (= n_frames); keep uint8
+ * [nb, max(n_frames), 2, 256] (MASK only, else ignored).  Runs the TokenEncoder, the upsample and the hoisted cond
+ * projections of the rows exactly as vtts_acoustic_forward does.  A slot that is still open fails with VTTS_ERR_BAD_ARG. */
+int vtts_acoustic_stream_begin(vtts_ctx* ctx, vtts_acoustic_stream* as, int nb, const int32_t* slots, const int32_t* tokens,
+                               const int32_t* lengths, const float* dur_frames, const int32_t* n_frames, const int32_t* n_emit,
+                               const uint8_t* keep, int L);
+/* mel_dev [S][F + D_a][80] (S = max_streams, F = max_chunk_frames): slot s gets n_out[s] frames from its start (rows
+ * after them are left as they were); n_out HOST int32 [S], set before anything is launched.  Stream-ordered. */
+int vtts_acoustic_stream_push(vtts_ctx* ctx, vtts_acoustic_stream* as, float* mel_dev, int32_t* n_out, void* stream);
+/* the same into a host buffer mel [S][F + D_a][80]; returns when it is written */
+int vtts_acoustic_stream_push_host(vtts_ctx* ctx, vtts_acoustic_stream* as, float* mel, int32_t* n_out);
+/* The duration half of vtts_tts_host for B token rows: predicted durations, silence tokens clipped from below at
+ * silence_duration, word-end tokens 0 s, seconds -> frames, the frame count (summed in double, rounded to float, then
+ * truncated) and the trailing-silence trim.  Outputs: dur_sec_out [B,L] adjusted seconds (may be NULL); dur_frames_out
+ * [B,L] frames (the acoustic model's durations); n_frames_out int32 [B] acoustic frames; n_emit_out int32 [B] frames
+ * left after the trim (what vtts_tts_host vocodes, possibly 0). */
+int vtts_tts_plan(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, int B, int L, float silence_duration, float* dur_sec_out,
+                  float* dur_frames_out, int32_t* n_frames_out, int32_t* n_emit_out);
 
 /* ---- host-buffer entry points (what a ctypes / cgo / JNI binding calls) ------------------ */
 int vtts_mel2wave_host(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, int B, int T, float* wav);

@@ -67,6 +67,15 @@ SIGNATURES = {
     "vtts_vocoder_stream_lookahead": (C.c_int, []),
     "vtts_vocoder_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtts_vocoder_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_acoustic_stream_create": (C.c_int, [c_ctx, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, C.POINTER(C.c_void_p)]),
+    "vtts_acoustic_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
+    "vtts_acoustic_stream_lookahead": (C.c_int, []),
+    "vtts_acoustic_stream_begin": (C.c_int, [c_ctx, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_int]),
+    "vtts_acoustic_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_acoustic_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_tts_plan": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
+                                C.c_void_p]),
     "vtts_launch_count": (C.c_int64, [c_ctx]),
     "vtts_last_stage_ms": (C.c_int, [c_ctx, C.c_int, C.POINTER(C.c_float)]),
 }

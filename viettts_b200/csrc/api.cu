@@ -921,23 +921,21 @@ int vtts_gta_host(vtts_ctx* ctx, const int16_t* wav_i16, const int32_t* wav_leng
 //   predict_duration -> [host: silence clip, word-end zeroing, seconds -> frames, n_frames, trailing-silence trim]
 //   -> AcousticModel.inference -> Generator.  The one unavoidable host round trip is the [B,L] duration matrix:
 //   the frame count N (every later grid size) depends on it.
-int vtts_tts_host(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, int B, int L, float silence_duration,
-                  int dropout_mode, uint64_t seed, int max_frames, float* dur_sec_out, int32_t* n_frames_out,
-                  int32_t* n_max_out, float* wav) {
+int vtts_tts_plan(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, int B, int L, float silence_duration, float* dur_sec_out,
+                  float* dur_frames_out, int32_t* n_frames_out, int32_t* n_emit_out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!tokens || !n_frames_out || !n_max_out || !wav || B < 1 || L < 1 || max_frames < 1)
-    return ctx->fail(VTTS_ERR_BAD_ARG, "tts_host: bad argument");
-  if (dropout_mode != VTTS_DROPOUT_OFF && dropout_mode != VTTS_DROPOUT_SEED && dropout_mode != VTTS_DROPOUT_REFERENCE)
-    return ctx->fail(VTTS_ERR_BAD_ARG, "tts_host: dropout_mode must be OFF, SEED or REFERENCE (the frame count is not known to the caller)");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  std::vector<float> sec((size_t)B * L), frames((size_t)B * L);
-  int rc = vtts_predict_duration_host(ctx, tokens, lengths, B, L, sec.data());
-  if (rc) return rc;
-  std::vector<int32_t> nf_ac(B), nf_voc(B);
-  int n_max = 0;
+  if (!tokens || !dur_frames_out || !n_frames_out || !n_emit_out || B < 1 || L < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "tts_plan: bad argument");
   for (int b = 0; b < B; ++b) {
     const int len = lengths ? lengths[b] : L;
-    if (len < 1 || len > L) return ctx->fail(VTTS_ERR_BAD_ARG, "tts_host: lengths[%d]=%d outside [1,%d]", b, len, L);
+    if (len < 1 || len > L) return ctx->fail(VTTS_ERR_BAD_ARG, "tts_plan: lengths[%d]=%d outside [1,%d]", b, len, L);
+  }
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  std::vector<float> sec((size_t)B * L);
+  int rc = vtts_predict_duration_host(ctx, tokens, lengths, B, L, sec.data());
+  if (rc) return rc;
+  float* frames = dur_frames_out;
+  for (int b = 0; b < B; ++b) {
+    const int len = lengths ? lengths[b] : L;
     double total = 0.0;
     for (int l = 0; l < L; ++l) {
       float d = l < len ? sec[(size_t)b * L + l] : 0.f;
@@ -953,11 +951,27 @@ int vtts_tts_host(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, 
     int trim = 0;
     if (tokens[(size_t)b * L + len - 1] == vc::SIL_INDEX)                                  // text2mel.py:99-102
       trim = (int)((double)sec[(size_t)b * L + len - 1] * 16000.0 / 256.0);
-    nf_ac[b] = n;
-    nf_voc[b] = n - trim > 0 ? n - trim : 0;
-    if (n > n_max) n_max = n;
+    n_frames_out[b] = n;
+    n_emit_out[b] = n - trim > 0 ? n - trim : 0;
   }
   if (dur_sec_out) memcpy(dur_sec_out, sec.data(), sec.size() * sizeof(float));
+  return VTTS_OK;
+}
+
+int vtts_tts_host(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, int B, int L, float silence_duration,
+                  int dropout_mode, uint64_t seed, int max_frames, float* dur_sec_out, int32_t* n_frames_out,
+                  int32_t* n_max_out, float* wav) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  if (!tokens || !n_frames_out || !n_max_out || !wav || B < 1 || L < 1 || max_frames < 1)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "tts_host: bad argument");
+  if (dropout_mode != VTTS_DROPOUT_OFF && dropout_mode != VTTS_DROPOUT_SEED && dropout_mode != VTTS_DROPOUT_REFERENCE)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "tts_host: dropout_mode must be OFF, SEED or REFERENCE (the frame count is not known to the caller)");
+  std::vector<float> frames((size_t)B * L);
+  std::vector<int32_t> nf_ac(B), nf_voc(B);
+  int rc = vtts_tts_plan(ctx, tokens, lengths, B, L, silence_duration, dur_sec_out, frames.data(), nf_ac.data(), nf_voc.data());
+  if (rc) return rc;
+  int n_max = 0;
+  for (int b = 0; b < B; ++b) n_max = std::max(n_max, nf_ac[b]);
   memcpy(n_frames_out, nf_voc.data(), (size_t)B * sizeof(int32_t));
   *n_max_out = n_max;
   if (n_max < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "tts_host: predicted durations sum to less than one frame");

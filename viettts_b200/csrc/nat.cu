@@ -285,6 +285,13 @@ struct DecScanArgs {
   int row_base;          // first row of this launch inside the full batch (dropout stream indexing)
   int N_total_rows;      // unused
   long long* dbg;        // optional per-CTA phase timers [grid][16]
+  // RESUME instantiation only (acoustic_stream.cu): launch row r advances stream slot rows[r].x from absolute frame
+  // rows[r].y by rows[r].z <= N steps (N = the largest); zc0 / zc1 / keep are per slot [S][zstride][...], the dropout
+  // row is the slot, and hout is [B][hstride][1024] by local step
+  const int4* rows;      // [B] (slot, t0, n, -)
+  float* state;          // [S][4][512] carried h0, c0, h1, c1 of every slot: loaded at launch start, stored after a row's last step
+  int zstride;           // frames per slot of zc0 / zc1 / keep (the stream's max_frames)
+  int hstride;           // frames per row of hout (the stream's max_chunk_frames)
 };
 
 constexpr int DEC_XR = 32;                 // batch rows per staging group (smem holds the state of one group)
@@ -598,6 +605,12 @@ __device__ __forceinline__ void dec_wait(const unsigned int* counter, unsigned i
 
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
+// RESUME = false: the one-shot scan of every acoustic entry point (frames 0..N-1 of every row from zero state).
+// RESUME = true: one push of an acoustic stream.  Each row continues its slot from frame t0 for n steps: the carried
+// state is loaded into the compact buffers (parity of frame -1) and cst, and zp0 / zp1 / p1 of the first step are
+// computed from it by the same dec_matmul / prenet_dot calls that produce them from the previous frame in the one-shot
+// scan, so a slot's frames get the one-shot bits.  A row past its n steps stores nothing (its state stays frozen).
+template <bool RESUME>
 __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const DecScanArgs a) {
   extern __shared__ __align__(16) float sm[];
   constexpr int H = vc::DEC_H, K0 = vc::PRENET + H, K1 = vc::PRENET + 2 * H;
@@ -615,6 +628,7 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const Dec
   float* cst = zp1 + DEC_NG * DEC_XR * NCOL;        // [DEC_NG][2][DEC_XR][UPC]
   float* wcs = cst + DEC_NG * 2 * DEC_XR * UPC;     // [1024][2] (Wo . W1) columns 2c, 2c+1
   float* wp2s = wcs + 2 * H * DEC_PCOL;             // [256][2]  W2 columns 2c, 2c+1
+  int4* rtab = reinterpret_cast<int4*>(wp2s + vc::PRENET * DEC_PCOL);   // RESUME: [B] row table (slot, t0, n, -)
   const int ks = tid >> 2, cgp = tid & 3;
   constexpr int SLP = vc::PRENET / NSLICE, SLH = H / NSLICE;   // 4, 8
   // register-resident weight slices, split by input segment so that each segment's product can be
@@ -645,6 +659,8 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const Dec
   for (int e = tid; e < DEC_NG * 2 * DEC_XR * UPC; e += SCAN_THREADS) cst[e] = 0.f;
   for (int e = tid; e < DEC_NG * 2 * DEC_XR * NCOL; e += SCAN_THREADS) zp0[e] = 0.f;   // zp0 and zp1 are adjacent
   for (int e = tid; e < DEC_XR * DEC_KPAD; e += SCAN_THREADS) xs[e] = 0.f;    // rows >= B and the t=0 state are zero
+  if constexpr (RESUME)
+    for (int e = tid; e < B; e += SCAN_THREADS) rtab[e] = __ldg(a.rows + e);
   __syncthreads();
   // Rows are processed in groups of DEC_XR (the staging buffer holds one group); all groups of a launch share the
   // four barriers of a frame.  With one group, h0 and p2 stay resident in xs between the phases.
@@ -653,9 +669,48 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const Dec
   const int prow = warp * 4 + (lane >> 3), pj = (lane >> 2) & 1, pu = DEC_PCOL * c + pj;   // prenet_dot result of this lane
   const bool pw = (lane & 3) == 0;                                                       // ... which this lane stores
   unsigned int nbar = 0;                                                                 // barriers passed so far
+  // per launch row rb at local step t: the row of zc0 / zc1, the row of hout, and the (dropout row, frame) it draws
+  auto zrow = [&](int rb, int t) -> size_t {
+    if constexpr (RESUME) return (size_t)rtab[rb].x * a.zstride + rtab[rb].y + t;
+    else return (size_t)rb * N + t;
+  };
+  auto hrow = [&](int rb, int t) -> size_t {
+    if constexpr (RESUME) return (size_t)rb * a.hstride + t;
+    else return (size_t)rb * N + t;
+  };
+  auto keep_at = [&](int rb, int t, int layer) -> float {
+    if constexpr (RESUME) return ar_keep_scale(a.mode, a.keep, a.seed, a.subkeys, rtab[rb].x, rtab[rb].y + t, a.zstride, layer, pu);
+    else return ar_keep_scale(a.mode, a.keep, a.seed, a.subkeys, a.row_base + rb, t, N, layer, pu);
+  };
+  auto live = [&](int rb, int t) -> bool {
+    if constexpr (RESUME) return t < rtab[rb].z;
+    else return true;
+  };
+  if constexpr (RESUME) {
+    // carried state of this CTA's units -> the compact buffers at the parity of frame -1, and cst
+    for (int e = tid; e < B * UPC; e += SCAN_THREADS) {
+      const int rb = e / UPC, uu = e % UPC, u = c * UPC + uu, r = rb % DEC_XR;
+      const float* s = a.state + (size_t)rtab[rb].x * 4 * H;
+      float* cs = cst + (size_t)(rb / DEC_XR) * 2 * DEC_XR * UPC;
+      a.h0[((size_t)B + rb) * H + u] = s[u];
+      a.h1[((size_t)B + rb) * H + u] = s[2 * H + u];
+      cs[r * UPC + uu] = s[H + u];
+      cs[(DEC_XR + r) * UPC + uu] = s[3 * H + u];
+    }
+    dec_arrive(a.bar);
+    dec_wait(a.bar, DEC_CTAS * ++nbar, a.err);        // every unit of the loaded h0 / h1 is in L2
+    // zp0 = h0_{-1} . W0[h0 rows], as phase D of the previous frame computes it (with one group, h0 stays in xs)
+    for (int rg = 0; rg < NG; ++rg) {
+      const int r0 = rg * DEC_XR, nb = min(DEC_XR, B - r0), ngroups = (nb + RG - 1) / RG;
+      dec_fetch(xs, DEC_KPAD, vc::PRENET, a.h0 + ((size_t)B + r0) * H, H, H, nb);
+      __syncthreads();
+      dec_matmul<SLH>(xs + vc::PRENET, w0h, ngroups, part, zp0 + rg * DEC_XR * NCOL, nullptr);
+    }
+  }
   for (int t = 0; t < N; ++t) {
     // ---- phase A: p1(t) = drop(relu([h0 | h1]_{t-1} . Wc + bc)) for this CTA's columns; p1(0) = 0 ----
-    if (t > 0) {
+    // (RESUME: every step takes this path from the loaded state; a row at absolute frame 0 stores p1 = 0)
+    if (RESUME || t > 0) {
       for (int rg = 0; rg < NG; ++rg) {
         const int r0 = rg * DEC_XR, nb = min(DEC_XR, B - r0), ngroups = (nb + RG - 1) / RG;
         if (NG > 1) dec_fetch(xs, DEC_KPAD, vc::PRENET, a.h0 + ((size_t)((t - 1) & 1) * B + r0) * H, H, H, nb);
@@ -663,9 +718,11 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const Dec
         __syncthreads();
         if (warp * 4 < nb) {
           const float s = prenet_dot<2 * H>(xs + vc::PRENET, wcs, lane, warp);
-          if (pw && prow < nb) {
+          if (pw && prow < nb && live(r0 + prow, t)) {
             const float v = fmaxf(s + __ldg(a.bc + pu), 0.f);
-            a.p1[(size_t)(r0 + prow) * vc::PRENET + pu] = v * ar_keep_scale(a.mode, a.keep, a.seed, a.subkeys, a.row_base + r0 + prow, t, N, 0, pu);
+            float* dst = a.p1 + (size_t)(r0 + prow) * vc::PRENET + pu;
+            if (RESUME && rtab[r0 + prow].y + t == 0) *dst = 0.f;
+            else *dst = v * keep_at(r0 + prow, t, 0);
           }
         }
         // earlier groups: their h1 leaves xs with the next fetch, so its product is taken now (the barriers inside
@@ -677,10 +734,10 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const Dec
     }
     DEC_MARK(0)
     dec_arrive(a.bar);
-    if (t > 0) dec_matmul<SLH>(xs + vc::PRENET + H, w1h1, ng_last, part, zp1 + lastg * DEC_XR * NCOL, nullptr);
+    if (RESUME || t > 0) dec_matmul<SLH>(xs + vc::PRENET + H, w1h1, ng_last, part, zp1 + lastg * DEC_XR * NCOL, nullptr);
     for (int e = tid; e < B * 8; e += SCAN_THREADS) {   // this frame's slices of zc0 / zc1, read in phases C and D
       const int rb = e >> 3, g = (e >> 1) & 3;
-      prefetch_l2(((e & 1) ? a.zc1 : a.zc0) + ((size_t)rb * N + t) * (4 * H) + g * H + c * UPC);
+      if (live(rb, t)) prefetch_l2(((e & 1) ? a.zc1 : a.zc0) + zrow(rb, t) * (4 * H) + g * H + c * UPC);
     }
     dec_wait(a.bar, DEC_CTAS * ++nbar, a.err);        // every column of p1(t) is in L2
     DEC_MARK(1)
@@ -692,8 +749,8 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const Dec
       __syncthreads();
       if (warp * 4 < nb) {
         const float s = prenet_dot<vc::PRENET>(xs, wp2s, lane, warp);
-        if (pw && prow < nb)
-          a.p2[(size_t)(r0 + prow) * vc::PRENET + pu] = fmaxf(s, 0.f) * ar_keep_scale(a.mode, a.keep, a.seed, a.subkeys, a.row_base + r0 + prow, t, N, 1, pu);
+        if (pw && prow < nb && live(r0 + prow, t))
+          a.p2[(size_t)(r0 + prow) * vc::PRENET + pu] = fmaxf(s, 0.f) * keep_at(r0 + prow, t, 1);
       }
     }
     DEC_MARK(2)
@@ -706,15 +763,22 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const Dec
       dec_fetch(xs, DEC_KPAD, 0, a.p2 + (size_t)r0 * vc::PRENET, vc::PRENET, vc::PRENET, nb);
       __syncthreads();
       dec_matmul<SLP>(xs, w0p, ngroups, part, zs, zp0 + rg * DEC_XR * NCOL);
-      if (tid < nb * UPC) {
+      if (tid < nb * UPC && live(r0 + tid / UPC, t)) {
         const int r = tid / UPC, uu = tid % UPC, rb = r0 + r;
-        const float* zc = a.zc0 + ((size_t)rb * N + t) * (4 * H) + c * UPC + uu;
+        const float* zc = a.zc0 + zrow(rb, t) * (4 * H) + c * UPC + uu;
         float* cs = cst + (size_t)rg * 2 * DEC_XR * UPC;
         float cc = cs[r * UPC + uu];
         const float h = lstm_cell(zs, r, uu, __ldg(zc), __ldg(zc + H), __ldg(zc + 2 * H), __ldg(zc + 3 * H), cc);
         cs[r * UPC + uu] = cc;
         a.h0[((size_t)(t & 1) * B + rb) * H + c * UPC + uu] = h;
-        a.hout[((size_t)rb * N + t) * 2 * H + c * UPC + uu] = h;
+        a.hout[hrow(rb, t) * 2 * H + c * UPC + uu] = h;
+        if constexpr (RESUME) {
+          if (t == rtab[rb].z - 1) {   // the row's last step: carry h0, c0
+            float* s = a.state + (size_t)rtab[rb].x * 4 * H + c * UPC + uu;
+            s[0] = h;
+            s[H] = cc;
+          }
+        }
       }
       if (NG > 1) __syncthreads();    // zs and xs are reused by the next group
     }
@@ -730,15 +794,22 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) decoder_scan_kernel(const Dec
       dec_fetch(xs, DEC_KPAD, vc::PRENET, a.h0 + ((size_t)(t & 1) * B + r0) * H, H, H, nb);
       __syncthreads();
       dec_matmul2<SLP, SLH>(xs, w1p, xs + vc::PRENET, w1h0, ngroups, part, zs, zp1 + rg * DEC_XR * NCOL);
-      if (tid < nb * UPC) {
+      if (tid < nb * UPC && live(r0 + tid / UPC, t)) {
         const int r = tid / UPC, uu = tid % UPC, rb = r0 + r;
-        const float* zc = a.zc1 + ((size_t)rb * N + t) * (4 * H) + c * UPC + uu;
+        const float* zc = a.zc1 + zrow(rb, t) * (4 * H) + c * UPC + uu;
         float* cs = cst + (size_t)rg * 2 * DEC_XR * UPC;
         float cc = cs[(DEC_XR + r) * UPC + uu];
         const float h = lstm_cell(zs, r, uu, __ldg(zc), __ldg(zc + H), __ldg(zc + 2 * H), __ldg(zc + 3 * H), cc);
         cs[(DEC_XR + r) * UPC + uu] = cc;
         a.h1[((size_t)(t & 1) * B + rb) * H + c * UPC + uu] = h;
-        a.hout[((size_t)rb * N + t) * 2 * H + H + c * UPC + uu] = h;
+        a.hout[hrow(rb, t) * 2 * H + H + c * UPC + uu] = h;
+        if constexpr (RESUME) {
+          if (t == rtab[rb].z - 1) {   // the row's last step: carry h1, c1
+            float* s = a.state + (size_t)rtab[rb].x * 4 * H + 2 * H + c * UPC + uu;
+            s[0] = h;
+            s[H] = cc;
+          }
+        }
       }
       // earlier groups: h0_t's product for frame t+1 while the rows are staged
       if (rg < lastg && more) dec_matmul<SLH>(xs + vc::PRENET, w0h, ngroups, part, zp0 + rg * DEC_XR * NCOL, nullptr);
@@ -946,6 +1017,9 @@ constexpr size_t dec_scan_smem() {
           (2 * vc::DEC_H + vc::PRENET) * DEC_PCOL) * 4;
 }
 static_assert(dec_scan_smem() <= 227 * 1024, "decoder scan shared memory exceeds the 227 KB of an sm_90 CTA");
+// the RESUME instantiation adds its row table after the prenet weights
+constexpr size_t dec_resume_smem() { return dec_scan_smem() + (size_t)MAX_ROWS * sizeof(int4); }
+static_assert(dec_resume_smem() <= 227 * 1024, "resumable decoder scan shared memory exceeds the 227 KB of an sm_90 CTA");
 
 // Slot layout shared by the acoustic and the duration model: the TokenEncoder's derived tensors and packed convs
 // come first in both, so that run_token_encoder reads either slot.
@@ -1094,7 +1168,8 @@ int vtts_acoustic_prepare(vtts_ctx* ctx) {
   if (rc) return rc;
   VTTS_CUDA(cudaDeviceSynchronize());
   VTTS_CUDA(cudaFuncSetAttribute(enc_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc_scan_smem()));
-  VTTS_CUDA(cudaFuncSetAttribute(decoder_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dec_scan_smem()));
+  VTTS_CUDA(cudaFuncSetAttribute(decoder_scan_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dec_scan_smem()));
+  VTTS_CUDA(cudaFuncSetAttribute(decoder_scan_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dec_resume_smem()));
   VTTS_CUDA(cudaFuncSetAttribute(decoder_tf_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tf_scan_smem()));
   return VTTS_OK;
 }
@@ -1116,27 +1191,37 @@ static int run_upsample(vtts_ctx* ctx, const float* enc, const float* dur, const
 // copied to mel1 if given; sub-stage mark `proj_mark` (if >= 0); then AcousticModel.postnet (model.py:113-121,
 // is_training=False) + the residual add (:143-144 / :169): mel = melpre + conv5(tanh(bn(conv5(...)))).
 // q0/q1 are [B*N][512] scratch.
-static int run_projection_postnet(vtts_ctx* ctx, const float* hout, const int32_t* n_frames, int B, int N, float* melpre,
-                                  float* q0, float* q1, float* mel1, int proj_mark, float* mel, cudaStream_t st) {
+int vtts_acoustic_project(vtts_ctx* ctx, const float* hout, const int32_t* len, int B, int T, float* melpre, cudaStream_t st) {
   const ModelWeights& m = ctx->ac;
-  const auto& T = m.t;
-  const ConvProb pp = conv_prob(hout, T[aci::PROJ_W], T[aci::PROJ_B], melpre);
-  int rc = run_convs(ctx, &pp, 1, 1024, 80, B, N, n_frames, 0, m.tiles(PK_PROJ), st);
-  if (rc) return rc;
-  if (mel1) VTTS_CUDA(cudaMemcpyAsync(mel1, melpre, (size_t)B * N * 80 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  if (proj_mark >= 0) ctx->sub_mark(proj_mark, st);
+  const ConvProb pp = conv_prob(hout, m.t[aci::PROJ_W], m.t[aci::PROJ_B], melpre);
+  return run_convs(ctx, &pp, 1, 1024, 80, B, T, len, 0, m.tiles(PK_PROJ), st);
+}
+
+int vtts_acoustic_postnet(vtts_ctx* ctx, const float* melpre, const int32_t* len, int B, int T, float* q0, float* q1, float* mel,
+                          cudaStream_t st) {
+  const ModelWeights& m = ctx->ac;
+  const auto& W = m.t;
   const float* pin = melpre;
   float* pout = q0;
   for (int i = 0; i < 5; ++i) {
-    ConvProb p = conv_prob(pin, T[aci::POST_CONV(i, 0)], T[aci::POST_CONV(i, 1)], i < 4 ? pout : mel, 5);
-    if (i < 4) { p.bn_mean = T[aci::POST_CONV(i, 4)]; p.bn_inv = m.d[D_POST_BNINV0 + i]; p.bn_off = T[aci::POST_CONV(i, 3)]; }
+    ConvProb p = conv_prob(pin, W[aci::POST_CONV(i, 0)], W[aci::POST_CONV(i, 1)], i < 4 ? pout : mel, 5);
+    if (i < 4) { p.bn_mean = W[aci::POST_CONV(i, 4)]; p.bn_inv = m.d[D_POST_BNINV0 + i]; p.bn_off = W[aci::POST_CONV(i, 3)]; }
     else p.resid = melpre;
-    rc = run_convs(ctx, &p, 1, i == 0 ? 80 : 512, i < 4 ? 512 : 80, B, N, n_frames, i < 4 ? 1 : 0, m.tiles(PK_POST0 + i), st);
+    const int rc = run_convs(ctx, &p, 1, i == 0 ? 80 : 512, i < 4 ? 512 : 80, B, T, len, i < 4 ? 1 : 0, m.tiles(PK_POST0 + i), st);
     if (rc) return rc;
     pin = pout;
     pout = (pout == q0) ? q1 : q0;
   }
   return VTTS_OK;
+}
+
+static int run_projection_postnet(vtts_ctx* ctx, const float* hout, const int32_t* n_frames, int B, int N, float* melpre,
+                                  float* q0, float* q1, float* mel1, int proj_mark, float* mel, cudaStream_t st) {
+  int rc = vtts_acoustic_project(ctx, hout, n_frames, B, N, melpre, st);
+  if (rc) return rc;
+  if (mel1) VTTS_CUDA(cudaMemcpyAsync(mel1, melpre, (size_t)B * N * 80 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (proj_mark >= 0) ctx->sub_mark(proj_mark, st);
+  return vtts_acoustic_postnet(ctx, melpre, n_frames, B, N, q0, q1, mel, st);
 }
 
 namespace {
@@ -1213,6 +1298,67 @@ size_t vtts_acoustic_ws_bytes(int B, int L, int N) { return ws_bytes<AcBufs>(B, 
 size_t vtts_acoustic_teacher_ws_bytes(int B, int L, int N) { return ws_bytes<TfBufs>(B, L, N); }
 size_t vtts_duration_ws_bytes(int B, int L) { return ws_bytes<DuBufs>(B, L, 0); }
 
+// TokenEncoder -> upsample -> hoisted cond projections zc0 / zc1 of the decoder LSTMs (sub-stage marks 0..3)
+static int run_acoustic_front(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const float* dur, const int32_t* n_frames,
+                              int B, int L, int N, const AcBufs& w, cudaStream_t st) {
+  const ModelWeights& m = ctx->ac;
+  const auto& T = m.t;
+  const size_t BN = (size_t)B * N;
+  VTTS_CUDA(cudaMemsetAsync(w.cond, 0, BN * 512 * sizeof(float), st));
+  ctx->sub_mark(0, st);
+  int rc = run_token_encoder(ctx, m, tokens, lengths, B, L, w.e, st);
+  if (rc) return rc;
+  ctx->sub_mark(1, st);
+  rc = run_upsample(ctx, w.e.enc, dur, lengths, n_frames, B, L, N, w.cond, vc::ENC_OUT, st);
+  if (rc) return rc;
+  ctx->sub_mark(2, st);
+  const ConvProb hp[2] = {conv_prob(w.cond, T[aci::DEC_L0_W], T[aci::DEC_L0_B], w.zc0), conv_prob(w.cond, T[aci::DEC_L1_W], T[aci::DEC_L1_B], w.zc1)};
+  rc = run_convs(ctx, hp, 2, 512, 2048, 1, (int)BN, nullptr, 0, m.tiles(PK_DEC_L0), st);
+  if (rc) return rc;
+  ctx->sub_mark(3, st);
+  return VTTS_OK;
+}
+
+int vtts_acoustic_front(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const float* dur, const int32_t* n_frames, int B,
+                        int L, int N, const float** zc0, const float** zc1, cudaStream_t st) {
+  if (!ctx->ac.loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "acoustic weights not loaded");
+  if (B < 1 || L < 1 || N < 1 || B > MAX_ROWS) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic: B=%d L=%d N=%d", B, L, N);
+  const AcBufs w = carve_ws<AcBufs>(ctx, B, L, N);
+  *zc0 = w.zc0;
+  *zc1 = w.zc1;
+  return run_acoustic_front(ctx, tokens, lengths, dur, n_frames, B, L, N, w, st);
+}
+
+int vtts_ref_subkeys(vtts_ctx* ctx, uint64_t seed, int n, uint2* out, cudaStream_t st) {
+  ref_subkey_chain_kernel<<<1, 32, 0, st>>>(seed, n, out);
+  ctx->launches++;
+  VTTS_CUDA(cudaGetLastError());
+  return VTTS_OK;
+}
+
+int vtts_decoder_scan_resume(vtts_ctx* ctx, const DecResume& r, cudaStream_t st) {
+  if (r.B < 1 || r.B > MAX_ROWS || r.nmax < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "decoder_scan_resume: B=%d nmax=%d", r.B, r.nmax);
+  if (ctx->sm_count < DEC_CTAS) return ctx->fail(VTTS_ERR_NO_DEVICE, "scan kernels need %d SMs, device has %d", DEC_CTAS, ctx->sm_count);
+  const ModelWeights& m = ctx->ac;
+  const auto& D = m.d;
+  DecScanArgs da;
+  memset(&da, 0, sizeof(da));
+  da.zc0 = r.zc0; da.zc1 = r.zc1;
+  da.w0r = D[D_DEC_W0R]; da.w1r = D[D_DEC_W1R]; da.wc = D[D_DEC_WC]; da.bc = D[D_DEC_BC]; da.wp2 = D[D_DEC_WP2];
+  da.keep = r.keep; da.subkeys = r.subkeys; da.seed = r.seed; da.mode = r.mode;
+  da.p1 = r.p1; da.p2 = r.p2; da.h0 = r.h0; da.h1 = r.h1; da.hout = r.hout;
+  da.bar = r.bar; da.err = ctx->d_err;
+  da.B = r.B; da.N = r.nmax; da.row_base = 0;
+  da.rows = r.rows; da.state = r.state; da.zstride = r.zstride; da.hstride = r.hstride;
+  VTTS_CUDA(cudaMemsetAsync(r.bar, 0, sizeof(unsigned int), st));
+  void* args[] = {&da};
+  VTTS_CUDA(cudaLaunchCooperativeKernel((void*)decoder_scan_kernel<true>, dim3(DEC_CTAS), dim3(SCAN_THREADS), args, dec_resume_smem(), st));
+  ctx->launches++;
+  return VTTS_OK;
+}
+
+int vtts_acoustic_max_tokens() { return (200 * 1024) / (int)((1 + UP_F) * sizeof(float)); }
+
 int vtts_acoustic_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const float* dur,
                       const int32_t* n_frames, const uint8_t* keep, int mode, uint64_t seed, int B, int L, int N,
                       float* mel, cudaStream_t st) {
@@ -1225,27 +1371,15 @@ int vtts_acoustic_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengt
   const AcBufs w = carve_ws<AcBufs>(ctx, B, L, N);
   const size_t BL = (size_t)B * L, BN = (size_t)B * N;
   const ModelWeights& m = ctx->ac;
-  const auto& T = m.t;
   const auto& D = m.d;
   ctx->tap_enc = w.e.enc; ctx->tap_enc_n = BL * 512;
   ctx->tap_cond = w.cond; ctx->tap_cond_n = BN * 512;
   ctx->tap_melpre = w.melpre; ctx->tap_melpre_n = BN * 80;
 
   VTTS_CUDA(cudaMemsetAsync(mel, 0, BN * 80 * sizeof(float), st));
-  VTTS_CUDA(cudaMemsetAsync(w.cond, 0, BN * 512 * sizeof(float), st));
   VTTS_CUDA(cudaMemsetAsync(w.melpre, 0, BN * 80 * sizeof(float), st));
-  ctx->sub_mark(0, st);
-  int rc = run_token_encoder(ctx, m, tokens, lengths, B, L, w.e, st);
+  int rc = run_acoustic_front(ctx, tokens, lengths, dur, n_frames, B, L, N, w, st);
   if (rc) return rc;
-  ctx->sub_mark(1, st);
-  rc = run_upsample(ctx, w.e.enc, dur, lengths, n_frames, B, L, N, w.cond, vc::ENC_OUT, st);
-  if (rc) return rc;
-  ctx->sub_mark(2, st);
-  // ---- hoisted cond projections of the decoder LSTMs ----
-  const ConvProb hp[2] = {conv_prob(w.cond, T[aci::DEC_L0_W], T[aci::DEC_L0_B], w.zc0), conv_prob(w.cond, T[aci::DEC_L1_W], T[aci::DEC_L1_B], w.zc1)};
-  rc = run_convs(ctx, hp, 2, 512, 2048, 1, (int)BN, nullptr, 0, m.tiles(PK_DEC_L0), st);
-  if (rc) return rc;
-  ctx->sub_mark(3, st);
   // ---- REFERENCE: the 2N prenet sub-keys of the reference's chain, stream-ordered into the workspace ----
   if (mode == VTTS_DROPOUT_REFERENCE) {
     ref_subkey_chain_kernel<<<1, 32, 0, st>>>(seed, 2 * N, w.subkeys);
@@ -1265,7 +1399,7 @@ int vtts_acoustic_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengt
     VTTS_CUDA(cudaMemsetAsync(w.dec_bar, 0, sizeof(unsigned int), st));
     da.B = nb; da.N = N; da.row_base = b0; da.dbg = ctx->tc_dbg_on ? ctx->d_tc_dbg : nullptr;
     void* args[] = {&da};
-    VTTS_CUDA(cudaLaunchCooperativeKernel((void*)decoder_scan_kernel, dim3(DEC_CTAS), dim3(SCAN_THREADS), args, dec_scan_smem(), st));
+    VTTS_CUDA(cudaLaunchCooperativeKernel((void*)decoder_scan_kernel<false>, dim3(DEC_CTAS), dim3(SCAN_THREADS), args, dec_scan_smem(), st));
     ctx->launches++;
   }
   ctx->sub_mark(4, st);

@@ -294,6 +294,37 @@ int vtts_teacher_mode_check(vtts_ctx* ctx, int mode, int B, int N);
 int vtts_acoustic_teacher_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const float* dur,
                               const int32_t* n_frames, const float* mels_in, const uint8_t* keep, const uint8_t* zone, int mode,
                               uint64_t seed, int B, int L, int N, float* mel1, float* mel2, cudaStream_t st);
+// pieces of vtts_acoustic_run that the acoustic stream (acoustic_stream.cu) runs on its own:
+// the front half (encoder, upsample, hoisted cond projections) into ctx->ws, sized by vtts_acoustic_ws_bytes(B, L, N);
+// zc0 / zc1 receive the [B][N][2048] results inside the workspace
+int vtts_acoustic_front(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const float* dur, const int32_t* n_frames, int B,
+                        int L, int N, const float** zc0, const float** zc1, cudaStream_t st);
+// output projection melpre = hout . Wo + bo over B rows of T frames (rows at or past len[b] not written)
+int vtts_acoustic_project(vtts_ctx* ctx, const float* hout, const int32_t* len, int B, int T, float* melpre, cudaStream_t st);
+// postnet + residual over B rows of T frames, frames at or past len[b] read as zero and are not written; q0 / q1 [B][T][512]
+int vtts_acoustic_postnet(vtts_ctx* ctx, const float* melpre, const int32_t* len, int B, int T, float* q0, float* q1, float* mel,
+                          cudaStream_t st);
+// the first n REFERENCE sub-keys of key `seed`, stream-ordered into out[n]
+int vtts_ref_subkeys(vtts_ctx* ctx, uint64_t seed, int n, uint2* out, cudaStream_t st);
+// the longest token row the upsample kernel takes (the acoustic entry points reject longer ones)
+int vtts_acoustic_max_tokens();
+// one launch of the resumable decoder scan (decoder_scan_kernel<true>, see DecScanArgs)
+struct DecResume {
+  const float* zc0;        // [S][zstride][2048]
+  const float* zc1;
+  const uint8_t* keep;     // MASK: [S][zstride][2][256]
+  const uint2* subkeys;    // REFERENCE: [2 * zstride]
+  uint64_t seed;
+  int mode;
+  const int4* rows;        // device [B] (slot, t0, n, -)
+  int B, nmax;             // launch rows (<= 128), largest n
+  float* state;            // [S][4][512]
+  int zstride, hstride;
+  float *p1, *p2, *h0, *h1; // [128][256] x2, [2][128][512] x2
+  float* hout;             // [B][hstride][1024]
+  unsigned int* bar;
+};
+int vtts_decoder_scan_resume(vtts_ctx* ctx, const DecResume& r, cudaStream_t st);
 int vtts_duration_prepare(vtts_ctx* ctx);
 size_t vtts_duration_ws_bytes(int B, int L);
 // DurationModel.__call__ (model.py:64-70); dur_sec [B][L] seconds, 0 past lengths[b]

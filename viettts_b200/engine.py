@@ -256,6 +256,42 @@ class Engine:
         precision mode, fused pairs off).  Needs the generator weights and the 'bf16x3' or 'fp16' mode."""
         return VocoderStream(self, max_streams, max_chunk_frames)
 
+    def open_acoustic_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
+                             masks: bool = False) -> "AcousticStream":
+        """Streaming acoustic model with `max_streams` (<= 128) independent slots (vtts_acoustic_stream_*): `begin`
+        starts utterances in free slots, each `push` advances every open slot by up to `max_chunk_frames` decoder steps
+        in one scan launch and returns the mel frames that are final.  Each utterance's frames equal `predict_mel` of
+        that utterance alone bit for bit.  Dropout, fixed for the stream: `masks=True` (MASK, masks given to `begin`),
+        else `seed` (SEED, slot s draws as row s of `predict_mel(seed=)`), else `rng` (REFERENCE), else off."""
+        return AcousticStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, masks=masks)
+
+    def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
+                        rng=None) -> "TtsStream":
+        """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
+        device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
+        With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  Needs the 'bf16x3' or 'fp16'
+        mode (the vocoder stream has no strict fp32 path)."""
+        return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng)
+
+    def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
+        """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
+        in frames [B,L], acoustic frames n_frames [B], frames kept after the trailing-silence trim n_emit [B])."""
+        tokens = _np(tokens, np.int32)
+        if tokens.ndim != 2:
+            raise ValueError("tokens must be [B,L]")
+        B, L = tokens.shape
+        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
+        sec = np.empty((B, L), np.float32)
+        frames = np.empty((B, L), np.float32)
+        nf = np.empty(B, np.int32)
+        ne = np.empty(B, np.int32)
+        self._ck(self.lib.vtts_tts_plan(self.h, _ptr(tokens), _ptr(lens), B, L, float(silence_duration), _ptr(sec), _ptr(frames),
+                                        _ptr(nf), _ptr(ne)))
+        return sec, frames, nf, ne
+
+    def get_precision(self) -> int:
+        return int(self.lib.vtts_get_precision(self.h))
+
     def _acoustic_args(self, tokens, dur_frames, lengths, n_frames, masks, seed, rng=None):
         ref_seed = None if rng is None else _rng_seed(rng, masks, seed)
         tokens = _np(tokens, np.int32)
@@ -653,6 +689,192 @@ class VocoderStream:
             self.close()
         except Exception:
             pass
+
+
+def acoustic_stream_schedule(n_frames: int, n_emit: int | None, chunk: int, lookahead: int = 10) -> list:
+    """Frames an acoustic stream slot emits per push: it scans min(n_frames, n_emit + lookahead) frames, `chunk` per
+    push; after P frames scanned it has emitted min(n_emit, max(0, P - lookahead)), and its last push emits the rest."""
+    n_emit = n_frames if n_emit is None else n_emit
+    end = min(n_frames, n_emit + lookahead)
+    P, E, out = 0, 0, []
+    while P < end:
+        P = min(end, P + chunk)
+        e = n_emit if P == end else min(n_emit, max(0, P - lookahead))
+        out.append(e - E)
+        E = e
+    return out
+
+
+class AcousticStream:
+    """Handle of a streaming acoustic model (Engine.open_acoustic_stream)."""
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
+                 masks: bool = False):
+        self.eng = eng
+        self.max_streams, self.max_chunk_frames = int(max_streams), int(max_chunk_frames)
+        self.max_frames, self.max_tokens = int(max_frames), int(max_tokens)
+        if rng is not None:
+            self.mode, self.seed = DROPOUT_REFERENCE, _rng_seed(rng, seed, True if masks else None)
+        elif masks:
+            if seed is not None:
+                raise ValueError("masks=True selects MASK mode; it cannot be combined with seed=")
+            self.mode, self.seed = DROPOUT_MASK, 0
+        else:
+            self.mode, self.seed = (DROPOUT_SEED if seed is not None else DROPOUT_OFF), int(seed or 0)
+        self.lookahead = int(eng.lib.vtts_acoustic_stream_lookahead())
+        self.out_frames = self.max_chunk_frames + self.lookahead   # frames per slot of a push's output buffer
+        self.open = np.zeros(self.max_streams, bool)               # host mirror of the library's slot state
+        self._left = np.zeros(self.max_streams, np.int64)          # pushes left per open slot
+        h = C.c_void_p()
+        eng._ck(eng.lib.vtts_acoustic_stream_create(eng.h, self.max_streams, self.max_chunk_frames, self.max_frames, self.max_tokens,
+                                                    self.mode, self.seed, C.byref(h)))
+        self.h = h
+
+    def begin(self, slots, tokens, dur_frames, lengths=None, n_frames=None, n_emit=None, masks=None):
+        """Start one utterance per entry of `slots` (closed slots): tokens int [nb,L], durations in frames [nb,L],
+        lengths / n_frames as for `predict_mel`, n_emit int [nb] (frames to emit, <= n_frames; default all), masks uint8
+        [nb,>=N,2,256] in MASK mode."""
+        slots = _np(np.atleast_1d(slots), np.int32)
+        if (masks is not None) != (self.mode == DROPOUT_MASK):
+            raise ValueError("masks are given to begin exactly when the stream was opened with masks=True")
+        tokens, dur, lens, nf, N, masks, _, _ = self.eng._acoustic_args(tokens, dur_frames, lengths, n_frames, masks, None)
+        nb, L = tokens.shape
+        if slots.shape != (nb,):
+            raise ValueError(f"slots must hold one slot per token row ({nb}), got {slots.shape}")
+        ne = None if n_emit is None else _np(n_emit, np.int32, (nb,), "n_emit")
+        self.eng._ck(self.eng.lib.vtts_acoustic_stream_begin(self.eng.h, self.h, nb, _ptr(slots), _ptr(tokens), _ptr(lens), _ptr(dur),
+                                                             _ptr(nf), _ptr(ne), _ptr(masks), L))
+        for i, s in enumerate(slots):
+            self.open[s] = True
+            self._left[s] = len(acoustic_stream_schedule(int(nf[i]), None if ne is None else int(ne[i]), self.max_chunk_frames,
+                                                         self.lookahead))
+
+    def _advance(self):
+        """slots that close with this push"""
+        closing = self.open & (self._left == 1)
+        self._left[self.open] -= 1
+        self.open &= ~closing
+        return closing
+
+    def push(self) -> list:
+        """Advance every open slot; returns one float32 [n, 80] array per slot with the frames it emits now."""
+        S = self.max_streams
+        mel = np.empty((S, self.out_frames, config.MEL_DIM), np.float32)
+        n_out = np.zeros(S, np.int32)
+        self.eng._ck(self.eng.lib.vtts_acoustic_stream_push_host(self.eng.h, self.h, _ptr(mel), _ptr(n_out)))
+        self._advance()
+        return [mel[s, : int(n_out[s])].copy() for s in range(S)]
+
+    def push_device(self, out_t, stream=None) -> np.ndarray:
+        """Device output: out_t f32 CUDA [S, F + lookahead, 80].  Stream-ordered; returns n_out int32 [S] (frames slot s
+        got at the start of its row of out_t)."""
+        import torch
+        S = self.max_streams
+        if tuple(out_t.shape) != (S, self.out_frames, config.MEL_DIM) or out_t.dtype != torch.float32 or not out_t.is_contiguous():
+            raise ValueError(f"out_t must be contiguous float32 [{S}, {self.out_frames}, {config.MEL_DIM}]")
+        n_out = np.zeros(S, np.int32)
+        st = torch.cuda.current_stream(out_t.device).cuda_stream if stream is None else stream
+        self.eng._ck(self.eng.lib.vtts_acoustic_stream_push(self.eng.h, self.h, _ptr(out_t), _ptr(n_out), st))
+        self._advance()
+        return n_out
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.eng, "h", None):
+            self.eng._ck(self.eng.lib.vtts_acoustic_stream_destroy(self.eng.h, self.h))
+        self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class TtsStream:
+    """Handle of a text-to-speech stream (Engine.open_tts_stream): an acoustic stream of max_chunk_frames F feeding a
+    vocoder stream of F + the acoustic lookahead frames per push."""
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None):
+        import torch
+        if eng.get_precision() == PRECISION_FP32:
+            raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
+        self.eng = eng
+        self.ac = AcousticStream(eng, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng)
+        try:
+            self.voc = VocoderStream(eng, max_streams, self.ac.out_frames)
+        except Exception:
+            self.ac.close()
+            raise
+        dev = torch.device("cuda", eng.device)
+        self._mel = torch.zeros((max_streams, self.ac.out_frames, config.MEL_DIM), dtype=torch.float32, device=dev)
+        self._wav = torch.zeros((max_streams, self.voc.wav_ld), dtype=torch.float32, device=dev)
+        self._fresh = np.zeros(max_streams, bool)   # begun, no push yet: the next vocoder push carries BEGIN
+        self._empty = set()                         # begun with nothing left after the trim: reported empty at the next step
+
+    @property
+    def max_streams(self):
+        return self.ac.max_streams
+
+    def begin(self, slot: int, tokens, silence_duration=-1.0):
+        """Start `tokens` (one row of phoneme ids) in a free slot: durations, the text2mel fix-ups and the trim are
+        planned exactly as `Engine.tts` plans them (vtts_tts_plan).  Returns the number of frames the slot will vocode."""
+        slot = int(slot)
+        if self.ac.open[slot] or slot in self._empty:
+            raise ValueError(f"slot {slot} is still open")
+        tok = _np(tokens, np.int32).reshape(1, -1)
+        _, frames, nf, ne = self.eng.tts_plan(tok, silence_duration=silence_duration)
+        if nf[0] < 1:
+            raise ValueError("tts stream: predicted durations sum to less than one frame")
+        if ne[0] == 0:
+            self._empty.add(slot)
+            return 0
+        self.ac.begin([slot], tok, frames, n_frames=nf, n_emit=ne)
+        self._fresh[slot] = True
+        return int(ne[0])
+
+    def busy(self) -> np.ndarray:
+        """bool [S]: slots with an utterance still running"""
+        b = self.ac.open.copy()
+        for s in self._empty:
+            b[s] = True
+        return b
+
+    def step(self) -> dict:
+        """One acoustic push into a device buffer, then one vocoder push of the frames it emitted (BEGIN on a slot's
+        first push, END on its last); one synchronisation.  Returns {slot: float32 samples} for every slot that was
+        running (possibly empty); a slot whose utterance finished this step is free afterwards."""
+        active = self.ac.open.copy()
+        closing_before = active.copy()
+        n_out = self.ac.push_device(self._mel) if active.any() else np.zeros(self.max_streams, np.int32)
+        closed = closing_before & ~self.ac.open
+        flags = (self._fresh & active).astype(np.uint8) * STREAM_BEGIN | closed.astype(np.uint8) * STREAM_END
+        out = {s: np.zeros(0, np.float32) for s in self._empty}
+        self._empty = set()
+        if active.any():
+            n_wav = self.voc.push_device(self._mel, n_out, flags, self._wav)
+            wav = self._wav.cpu().numpy()
+            for s in np.flatnonzero(active):
+                out[int(s)] = wav[s, : int(n_wav[s]) * config.HOP].copy()
+        self._fresh &= ~active
+        return out
+
+    def close(self):
+        if getattr(self, "voc", None) is not None:
+            self.voc.close()
+        if getattr(self, "ac", None) is not None:
+            self.ac.close()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
 
 
 _engines: dict = {}

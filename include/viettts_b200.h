@@ -183,6 +183,24 @@ int vtts_debug_conv_dispatch(vtts_ctx* ctx, int precision, int nprob, const floa
 int vtts_debug_pair(vtts_ctx* ctx, const float* x_dev, const float* w1_dev, const float* b1_dev, const float* w2_dev,
                     const float* b2_dev, const int32_t* len_dev, int B, int T, int C, int k, int dil, float slope, float* out_dev);
 
+/* test hook: exactly one layer of the generator forward (vtts_hifigan_forward), on caller buffers, with the loaded
+ * weights, the context's precision mode and its fused-pair setting; the forward runs the same functions in order.
+ * T and n_frames (int32 [B] or NULL) are in mel frames as for the forward; stage i runs on T*S_i rows per batch row
+ * with S_0..S_4 = 1, 8, 64, 128, 256, and rows at or past n_frames[b]*S_i read as zero and are not written.
+ * x and out are host arrays of device pointers:
+ *   layer 0        conv_pre                 x[0] mel [B,T,80]                   -> out[0] [B,T,512]
+ *   layer 1        ConvTranspose of stage 0 x[0] conv_pre output [B,T,512]      -> out[0] [B,8T,256]
+ *   layer 1+i      ConvTranspose of stage i (i = 1..3): x[0..2] the three ResBlock chains of stage i-1, [B,T*S_i,C_i]
+ *                  (lrelu of their mean is the input)                            -> out[0] [B,T*S_{i+1},C_i/2]
+ *   layer 5+3i+m   ResBlock step m (0..2) of stage i (0..3), the three chains k = 3, 7, 11 in one launch (two unfused):
+ *                  x[j] [B,T*S_{i+1},C_i/2] -> out[j] = x[j] + conv2(lrelu(conv1(lrelu(x[j])))), same shape; out[j]
+ *                  must not alias x[j]
+ *   layer 17       conv_post                x[0..2] the three chains of stage 3 [B,256T,32] -> out[0] wav [B,256T]
+ *                  (tanh applied; zeros past n_frames[b]*256)
+ * with C_i = 512 >> i.  Synchronous. */
+int vtts_debug_hifigan_layer(vtts_ctx* ctx, int layer, const float* const* x, float* const* out, const int32_t* n_frames, int B,
+                             int T);
+
 /* test hook: the masks VTTS_DROPOUT_REFERENCE applies for key `seed`, drawn on the device by the scans' own draw
  * functions, as uint8 (1 = keep).  kind 0: the autoregressive prenet masks [N,2,256] (shared by every row; B ignored);
  * kind 1: the teacher-forced masks, keep [B,N,2,256] followed by zone [B,N,4,512].  Uses the context's workspace

@@ -66,9 +66,12 @@ def conv1d_transpose_nwc(x, w, b, stride: int):
     return y.transpose(1, 2)
 
 
-def resblock1(x, p, prefix: str, k: int, dtype):
-    """model.py:44-51"""
+def resblock1(x, p, prefix: str, k: int, dtype, taps: dict | None = None, tag: str = ""):
+    """model.py:44-51.  If `taps` is a dict, the input of step m is stored as taps[f"{tag}_{m}"] and the output as
+    taps[f"{tag}_3"]."""
     for m, d in enumerate(RB_DILATIONS):
+        if taps is not None:
+            taps[f"{tag}_{m}"] = x
         c1 = p[f"{prefix}/~/convs1_{m}"]
         c2 = p[f"{prefix}/~/convs2_{m}"]
         xt = F.leaky_relu(x, LRELU_SLOPE)
@@ -76,6 +79,8 @@ def resblock1(x, p, prefix: str, k: int, dtype):
         xt = F.leaky_relu(xt, LRELU_SLOPE)
         xt = conv1d_nwc(xt, _t(c2["w"], dtype), _t(c2["b"], dtype), dilation=1)
         x = xt + x
+    if taps is not None:
+        taps[f"{tag}_3"] = x
     return x
 
 
@@ -83,7 +88,7 @@ def generator_forward(params: dict, mel, dtype=torch.float32, taps: dict | None 
     """Generator.__call__ (model.py:109-125).  mel [B,T,80] -> wav [B,256T].
 
     If `taps` is a dict, intermediate activations are stored in it
-    ("pre", "ups_i", "stage_i", "post")."""
+    ("pre", "ups_i", "stage_i"; "rb_i_j_m": the input of ResBlock step m of chain j of stage i, m = 3 its output)."""
     x = _t(mel, dtype)
     g = "generator/~/"
     p0 = params[g + "conv1_d"]
@@ -98,7 +103,7 @@ def generator_forward(params: dict, mel, dtype=torch.float32, taps: dict | None 
             taps[f"ups_{i}"] = x
         xs = None
         for j, k in enumerate(RB_KERNELS):
-            r = resblock1(x, params, g + f"res_block1_{i * 3 + j}", k, dtype)
+            r = resblock1(x, params, g + f"res_block1_{i * 3 + j}", k, dtype, taps, f"rb_{i}_{j}")
             xs = r if xs is None else xs + r
         x = xs / 3
         if taps is not None:

@@ -35,6 +35,7 @@ SIGNATURES = {
     "vtts_debug_dropout_masks": (C.c_int, [c_ctx, C.c_int, C.c_uint64, C.c_int, C.c_int, C.c_void_p]),
     "vtts_debug_pair": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]),
+    "vtts_debug_hifigan_layer": (C.c_int, [c_ctx, C.c_int, ptrp, ptrp, C.c_void_p, C.c_int, C.c_int]),
     "vtts_hifigan_blob_floats": (C.c_int64, []),
     "vtts_acoustic_blob_floats": (C.c_int64, []),
     "vtts_duration_blob_floats": (C.c_int64, []),

@@ -143,196 +143,272 @@ int vtts_hifigan_prepare(vtts_ctx* ctx) {
   return VTTS_OK;
 }
 
-int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, int B, int T, float* wav, cudaStream_t st) {
-  if (!ctx->hg.loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "hifigan weights not loaded");
-  if (B < 1 || T < 1 || B > 65535) return ctx->fail(VTTS_ERR_BAD_ARG, "hifigan: B=%d T=%d", B, T);
-  if ((int64_t)T * 256 > (int64_t)INT32_MAX / 64) return ctx->fail(VTTS_ERR_BAD_ARG, "hifigan: T=%d too long", T);
-  size_t need = vtts_hifigan_ws_bytes(B, T);
-  int rc = ctx->ensure_ws(need);
-  if (rc) return rc;
-  Arena ar(ctx->ws, ctx->ws_bytes, false);
-  HgBufs hb;
-  carve(ar, B, T, hb);
+// ---- the generator's layers, one function each: vtts_hifigan_run calls them in order, vtts_debug_hifigan_layer one ----
+// Every layer derives its rows from T mel frames and its valid rows from n_frames[b]: stage i runs on T * hg_scale(i)
+// input rows per batch row, and rows at or past n_frames[b] * hg_scale(i) read as zero and are not written.
+
+namespace {
+
+// rows per mel frame entering stage i (i = 4: conv_post)
+int hg_scale(int i) {
+  int s = 1;
+  for (int q = 0; q < i; ++q) s *= vc::hg_rate(q);
+  return s;
+}
+
+// conv_pre: 80 -> 512, k7 pad 3.  mel [B][T][80] -> out [B][T][512]
+int hg_conv_pre(vtts_ctx* ctx, const float* mel, float* out, const int32_t* n_frames, int B, int T, cudaStream_t st) {
   const ModelWeights& M = ctx->hg;
   auto& W = M.t;
-
   ConvLaunch L;
   memset(&L, 0, sizeof(L));
   L.B = B;
   L.len = n_frames;
-
-  ctx->sub_mark(8, st);
-  // conv_pre: 80 -> 512, k7 pad 3
   L.nprob = 1;
   L.Cin = vc::MEL; L.Cout = vc::HG_C0;
   L.T_rows = T; L.rows_out = T; L.len_mul = 1;
   L.pre_mode = 0; L.pre_slope = 1.f; L.post_act = 0;
-  L.p[0] = ConvProb{mel, nullptr, nullptr, W[hgi::PRE_W], W[hgi::PRE_B], nullptr, nullptr, nullptr, nullptr, hb.P0, 7, 1, -3, 1, 0};
+  L.p[0] = ConvProb{mel, nullptr, nullptr, W[hgi::PRE_W], W[hgi::PRE_B], nullptr, nullptr, nullptr, nullptr, out, 7, 1, -3, 1, 0};
   // tensor-core modes: bf16x3 (BF16X3) or one fp16 product (FP16, the packing table's second half)
   const bool tc = ctx->precision != VTTS_PRECISION_FP32;
   const int f16 = ctx->precision == VTTS_PRECISION_FP16;
   const int pk = f16 ? PK_COUNT : 0;
-  if (tc) {
-    TcLaunch TL;
-    memset(&TL, 0, sizeof(TL));
-    TL.nprob = 2; TL.Cin = vc::MEL; TL.N = 256; TL.in_ld = vc::MEL; TL.out_ld = vc::HG_C0;
-    TL.B = B; TL.T_rows = T; TL.rows_out = T; TL.len = n_frames; TL.len_mul = 1; TL.pre_mode = 0; TL.pre_slope = 1.f; TL.f16 = f16;
-    for (int t = 0; t < 2; ++t)
-      TL.p[t] = TcProb{mel, nullptr, nullptr, M.tiles(pk + PK_PRE)[t], W[hgi::PRE_B] + 256 * t, nullptr, nullptr, nullptr, nullptr, hb.P0 + 256 * t, 7, 1, -3, 1, 0};
-    rc = vtts_launch_tc_conv(ctx, TL, st);
-  } else {
-    rc = vtts_launch_conv(ctx, L, st);
+  if (!tc) return vtts_launch_conv(ctx, L, st);
+  TcLaunch TL;
+  memset(&TL, 0, sizeof(TL));
+  TL.nprob = 2; TL.Cin = vc::MEL; TL.N = 256; TL.in_ld = vc::MEL; TL.out_ld = vc::HG_C0;
+  TL.B = B; TL.T_rows = T; TL.rows_out = T; TL.len = n_frames; TL.len_mul = 1; TL.pre_mode = 0; TL.pre_slope = 1.f; TL.f16 = f16;
+  for (int t = 0; t < 2; ++t)
+    TL.p[t] = TcProb{mel, nullptr, nullptr, M.tiles(pk + PK_PRE)[t], W[hgi::PRE_B] + 256 * t, nullptr, nullptr, nullptr, nullptr, out + 256 * t, 7, 1, -3, 1, 0};
+  return vtts_launch_tc_conv(ctx, TL, st);
+}
+
+// lrelu(0.1) [of the 3-way mean for i > 0] -> ConvTranspose of stage i as u two-tap phases.  x[0] (i = 0: conv_pre's
+// output) or x[0..2] (the previous stage's three ResBlock chains), [B][T*hg_scale(i)][C] -> out [B][T*hg_scale(i+1)][C/2]
+int hg_ups(vtts_ctx* ctx, int i, const float* const* x, float* out, const int32_t* n_frames, int B, int T, cudaStream_t st) {
+  const ModelWeights& M = ctx->hg;
+  auto& W = M.t;
+  const bool tc = ctx->precision != VTTS_PRECISION_FP32;
+  const int f16 = ctx->precision == VTTS_PRECISION_FP16;
+  const int pk = f16 ? PK_COUNT : 0;
+  const int C = vc::HG_C0 >> i, scale_in = hg_scale(i), rows_in = T * scale_in;
+  const int u = vc::hg_rate(i), K = vc::hg_upk(i), Co = C / 2;
+  const int a = (K + u - 2 + 1) / 2;
+  ConvLaunch L;
+  memset(&L, 0, sizeof(L));
+  L.B = B; L.len = n_frames; L.len_mul = scale_in;
+  L.nprob = u; L.Cin = C; L.Cout = Co;
+  L.T_rows = rows_in; L.rows_out = rows_in * u;
+  L.pre_mode = (i == 0) ? 1 : 2; L.pre_slope = 0.1f; L.post_act = 0;
+  for (int r = 0; r < u; ++r) {
+    int j0 = ((a - r) % u + u) % u;
+    int e = (r + j0 - a) / u;  // exact division, <= 0
+    ConvProb p;
+    memset(&p, 0, sizeof(p));
+    if (i == 0) { p.x0 = x[0]; } else { p.x0 = x[0]; p.x1 = x[1]; p.x2 = x[2]; }
+    p.w = M.d[i] + (size_t)r * 2 * C * Co;
+    p.bias = W[hgi::UPS_B(i)];
+    p.out = out;
+    p.k = 2; p.dil = 1; p.in_off = e; p.out_stride = u; p.out_off = r;
+    L.p[r] = p;
   }
+  if (!tc) return vtts_launch_conv(ctx, L, st);
+  // ConvTranspose phases share their input: for N <= 128 one converted activation tile feeds NPH phases
+  // (multi-phase tiles of tc_conv.cu); N = 256 keeps one problem per phase.
+  const int nph = Co == 256 ? 1 : (Co == 128 ? 4 : 2);
+  TcLaunch TL;
+  memset(&TL, 0, sizeof(TL));
+  TL.nprob = u / nph; TL.nphase = nph; TL.Cin = C; TL.N = Co; TL.in_ld = C; TL.out_ld = Co;
+  TL.B = B; TL.T_rows = rows_in; TL.rows_out = rows_in * u; TL.len = n_frames; TL.len_mul = scale_in;
+  TL.pre_mode = L.pre_mode; TL.pre_slope = 0.1f; TL.f16 = f16;
+  for (int g = 0; g < u / nph; ++g) {
+    const ConvProb& c0 = L.p[g * nph];
+    TcProb q;
+    memset(&q, 0, sizeof(q));
+    q.x0 = c0.x0; q.x1 = c0.x1; q.x2 = c0.x2; q.bias = c0.bias; q.out = c0.out;
+    q.k = 2; q.dil = 1; q.out_stride = u;
+    q.wpk = M.tiles(pk + PK_UPS(i, g * nph))[0]; q.in_off = c0.in_off; q.out_off = g * nph;
+    for (int ph = 0; ph < nph; ++ph) {
+      const int r = g * nph + ph;
+      q.wpk_ph[ph] = M.tiles(pk + PK_UPS(i, r))[0];
+      q.in_off_ph[ph] = L.p[r].in_off;
+      q.out_off_ph[ph] = r;
+    }
+    TL.p[g] = q;
+  }
+  return vtts_launch_tc_conv(ctx, TL, st);
+}
+
+// step m of the three ResBlock1 (k = 3, 7, 11) of stage i: chain j runs dst[j] = conv2(lrelu(conv1_d(lrelu(src[j])))) +
+// src[j], all [B][T*hg_scale(i+1)][C/2]; tmp[j] receives conv1's output when the pair is not fused
+int hg_resblock(vtts_ctx* ctx, int i, int m, const float* const* src, float* const* dst, float* const* tmp, const int32_t* n_frames,
+                int B, int T, cudaStream_t st) {
+  const ModelWeights& M = ctx->hg;
+  auto& W = M.t;
+  const bool tc = ctx->precision != VTTS_PRECISION_FP32;
+  const int f16 = ctx->precision == VTTS_PRECISION_FP16;
+  const int pk = f16 ? PK_COUNT : 0;
+  const int Co = vc::HG_C0 >> (i + 1), scale = hg_scale(i + 1), rows = T * scale;
+  const int d = vc::hg_dil(m);
+  if (tc && ctx->fuse_pairs && Co <= 64) {
+    // ---- fused pair: conv(d) -> lrelu -> conv(1) -> + x, intermediate kept on chip (tc_conv.cu) ----
+    TcPairLaunch PL;
+    memset(&PL, 0, sizeof(PL));
+    PL.nprob = 3; PL.N = Co; PL.B = B; PL.T_rows = rows; PL.len = n_frames; PL.len_mul = scale; PL.slope = 0.1f; PL.f16 = f16;
+    for (int j = 0; j < 3; ++j) {
+      const int kk = vc::hg_rbk(j), n = i * 3 + j;
+      PL.p[j] = TcPairProb{src[j], M.tiles(pk + PK_RB(n, 0, m))[0], M.tiles(pk + PK_RB(n, 1, m))[0], W[hgi::RB_B(n, 0, m)], W[hgi::RB_B(n, 1, m)],
+                           dst[j], kk, d};
+    }
+    return vtts_launch_tc_pair(ctx, PL, st);
+  }
+  if (tc) {
+    // ---- tensor-core path (tc_conv.cu) ----
+    TcLaunch TL;
+    for (int which = 0; which < 2; ++which) {
+      memset(&TL, 0, sizeof(TL));
+      TL.nprob = 3; TL.Cin = Co; TL.N = Co; TL.in_ld = Co; TL.out_ld = Co;
+      TL.B = B; TL.T_rows = rows; TL.rows_out = rows; TL.len = n_frames; TL.len_mul = scale;
+      TL.pre_mode = 1; TL.pre_slope = 0.1f; TL.f16 = f16;
+      for (int j = 0; j < 3; ++j) {
+        const int kk = vc::hg_rbk(j), n = i * 3 + j;
+        const int dd = which == 0 ? d : 1;
+        TcProb p;
+        memset(&p, 0, sizeof(p));
+        p.x0 = which == 0 ? src[j] : tmp[j];
+        p.wpk = M.tiles(pk + PK_RB(n, which, m))[0];
+        p.bias = W[hgi::RB_B(n, which, m)];
+        p.resid = which == 0 ? nullptr : src[j];
+        p.out = which == 0 ? tmp[j] : dst[j];
+        p.k = kk; p.dil = dd; p.in_off = -((kk - 1) * dd) / 2; p.out_stride = 1; p.out_off = 0;
+        TL.p[j] = p;
+      }
+      int rc = vtts_launch_tc_conv(ctx, TL, st);
+      if (rc) return rc;
+    }
+    return VTTS_OK;
+  }
+  // conv1 (dilated)
+  ConvLaunch L;
+  memset(&L, 0, sizeof(L));
+  L.B = B; L.len = n_frames; L.len_mul = scale;
+  L.nprob = 3; L.Cin = Co; L.Cout = Co; L.T_rows = rows; L.rows_out = rows;
+  L.pre_mode = 1; L.pre_slope = 0.1f; L.post_act = 0;
+  for (int j = 0; j < 3; ++j) {
+    const int kk = vc::hg_rbk(j), n = i * 3 + j;
+    ConvProb p;
+    memset(&p, 0, sizeof(p));
+    p.x0 = src[j];
+    p.w = W[hgi::RB_W(n, 0, m)]; p.bias = W[hgi::RB_B(n, 0, m)];
+    p.out = tmp[j];
+    p.k = kk; p.dil = d; p.in_off = -((kk - 1) * d) / 2; p.out_stride = 1; p.out_off = 0;
+    L.p[j] = p;
+  }
+  int rc = vtts_launch_conv(ctx, L, st);
+  if (rc) return rc;
+  // conv2 (dilation 1) + residual
+  for (int j = 0; j < 3; ++j) {
+    const int kk = vc::hg_rbk(j), n = i * 3 + j;
+    ConvProb p;
+    memset(&p, 0, sizeof(p));
+    p.x0 = tmp[j];
+    p.w = W[hgi::RB_W(n, 1, m)]; p.bias = W[hgi::RB_B(n, 1, m)];
+    p.resid = src[j];
+    p.out = dst[j];
+    p.k = kk; p.dil = 1; p.in_off = -(kk - 1) / 2; p.out_stride = 1; p.out_off = 0;
+    L.p[j] = p;
+  }
+  return vtts_launch_conv(ctx, L, st);
+}
+
+// mean of 3, lrelu(0.01), conv_post (32 -> 1, k7), tanh: x[0..2] [B][256T][32] -> wav [B][256T], zeros past
+// n_frames[b] * 256
+int hg_conv_post(vtts_ctx* ctx, const float* const* x, float* wav, const int32_t* n_frames, int B, int T, cudaStream_t st) {
+  auto& W = ctx->hg.t;
+  const int R = T * hg_scale(4);  // 256*T
+  dim3 grid((R + 255) / 256, B);
+  conv_post_kernel<<<grid, 256, 0, st>>>(x[0], x[1], x[2], W[hgi::POST_W], W[hgi::POST_B], n_frames, 256, R, wav);
+  ctx->launches++;
+  VTTS_CUDA(cudaGetLastError());
+  return VTTS_OK;
+}
+
+int hg_check(vtts_ctx* ctx, int B, int T) {
+  if (!ctx->hg.loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "hifigan weights not loaded");
+  if (B < 1 || T < 1 || B > 65535) return ctx->fail(VTTS_ERR_BAD_ARG, "hifigan: B=%d T=%d", B, T);
+  if ((int64_t)T * 256 > (int64_t)INT32_MAX / 64) return ctx->fail(VTTS_ERR_BAD_ARG, "hifigan: T=%d too long", T);
+  return VTTS_OK;
+}
+
+}  // namespace
+
+int vtts_hifigan_run(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, int B, int T, float* wav, cudaStream_t st) {
+  int rc = hg_check(ctx, B, T);
+  if (rc) return rc;
+  size_t need = vtts_hifigan_ws_bytes(B, T);
+  rc = ctx->ensure_ws(need);
+  if (rc) return rc;
+  Arena ar(ctx->ws, ctx->ws_bytes, false);
+  HgBufs hb;
+  carve(ar, B, T, hb);
+
+  ctx->sub_mark(8, st);
+  rc = hg_conv_pre(ctx, mel, hb.P0, n_frames, B, T, st);
   if (rc) return rc;
   ctx->sub_mark(9, st);
-
-  int C = vc::HG_C0;      // input channels of the stage
-  int rows_in = T;        // rows per batch item entering the stage
-  int scale_in = 1;       // rows_in = T*scale_in
   for (int i = 0; i < 4; ++i) {
-    const int u = vc::hg_rate(i), K = vc::hg_upk(i), Co = C / 2;
-    const int a = (K + u - 2 + 1) / 2;
-    const int par = i & 1;
-    // ---- lrelu(0.1) [of the 3-way mean for i>0] -> ConvTranspose as u two-tap phases ----
-    memset(&L, 0, sizeof(L));
-    L.B = B; L.len = n_frames; L.len_mul = scale_in;
-    L.nprob = u; L.Cin = C; L.Cout = Co;
-    L.T_rows = rows_in; L.rows_out = rows_in * u;
-    L.pre_mode = (i == 0) ? 1 : 2; L.pre_slope = 0.1f; L.post_act = 0;
-    for (int r = 0; r < u; ++r) {
-      int j0 = ((a - r) % u + u) % u;
-      int e = (r + j0 - a) / u;  // exact division, <= 0
-      ConvProb p;
-      memset(&p, 0, sizeof(p));
-      if (i == 0) { p.x0 = hb.P0; } else { p.x0 = hb.A[par ^ 1][0]; p.x1 = hb.A[par ^ 1][1]; p.x2 = hb.A[par ^ 1][2]; }
-      p.w = M.d[i] + (size_t)r * 2 * C * Co;
-      p.bias = W[hgi::UPS_B(i)];
-      p.out = hb.X;
-      p.k = 2; p.dil = 1; p.in_off = e; p.out_stride = u; p.out_off = r;
-      L.p[r] = p;
-    }
-    if (tc) {
-      // ConvTranspose phases share their input: for N <= 128 one converted activation tile feeds NPH phases
-      // (multi-phase tiles of tc_conv.cu); N = 256 keeps one problem per phase.
-      const int nph = Co == 256 ? 1 : (Co == 128 ? 4 : 2);
-      TcLaunch TL;
-      memset(&TL, 0, sizeof(TL));
-      TL.nprob = u / nph; TL.nphase = nph; TL.Cin = C; TL.N = Co; TL.in_ld = C; TL.out_ld = Co;
-      TL.B = B; TL.T_rows = rows_in; TL.rows_out = rows_in * u; TL.len = n_frames; TL.len_mul = scale_in;
-      TL.pre_mode = L.pre_mode; TL.pre_slope = 0.1f; TL.f16 = f16;
-      for (int g = 0; g < u / nph; ++g) {
-        const ConvProb& c0 = L.p[g * nph];
-        TcProb q;
-        memset(&q, 0, sizeof(q));
-        q.x0 = c0.x0; q.x1 = c0.x1; q.x2 = c0.x2; q.bias = c0.bias; q.out = c0.out;
-        q.k = 2; q.dil = 1; q.out_stride = u;
-        q.wpk = M.tiles(pk + PK_UPS(i, g * nph))[0]; q.in_off = c0.in_off; q.out_off = g * nph;
-        for (int ph = 0; ph < nph; ++ph) {
-          const int r = g * nph + ph;
-          q.wpk_ph[ph] = M.tiles(pk + PK_UPS(i, r))[0];
-          q.in_off_ph[ph] = L.p[r].in_off;
-          q.out_off_ph[ph] = r;
-        }
-        TL.p[g] = q;
-      }
-      rc = vtts_launch_tc_conv(ctx, TL, st);
-    } else {
-      rc = vtts_launch_conv(ctx, L, st);
-    }
+    const int par = i & 1;   // stage i's ResBlock chains end in A[par]; stage i - 1's in A[par ^ 1]
+    const float* const ups_in[3] = {i == 0 ? hb.P0 : hb.A[par ^ 1][0], i == 0 ? nullptr : hb.A[par ^ 1][1], i == 0 ? nullptr : hb.A[par ^ 1][2]};
+    rc = hg_ups(ctx, i, ups_in, hb.X, n_frames, B, T, st);
     if (rc) return rc;
-
-    // ---- three ResBlock1 (k = 3,7,11), each 3 x [lrelu, conv(d), lrelu, conv(1), +x] ----
-    const int rows = rows_in * u;
-    const int scale = scale_in * u;
     for (int m = 0; m < 3; ++m) {
-      const int d = vc::hg_dil(m);
       const float* src[3];
-      for (int j = 0; j < 3; ++j) src[j] = (m == 0) ? hb.X : (m == 1 ? hb.A[par][j] : hb.Bb[j]);
-      if (tc && ctx->fuse_pairs && Co <= 64) {
-        // ---- fused pair: conv(d) -> lrelu -> conv(1) -> + x, intermediate kept on chip (tc_conv.cu) ----
-        TcPairLaunch PL;
-        memset(&PL, 0, sizeof(PL));
-        PL.nprob = 3; PL.N = Co; PL.B = B; PL.T_rows = rows; PL.len = n_frames; PL.len_mul = scale; PL.slope = 0.1f; PL.f16 = f16;
-        for (int j = 0; j < 3; ++j) {
-          const int kk = vc::hg_rbk(j), n = i * 3 + j;
-          PL.p[j] = TcPairProb{src[j], M.tiles(pk + PK_RB(n, 0, m))[0], M.tiles(pk + PK_RB(n, 1, m))[0], W[hgi::RB_B(n, 0, m)], W[hgi::RB_B(n, 1, m)],
-                               (m == 1) ? hb.Bb[j] : hb.A[par][j], kk, d};
-        }
-        rc = vtts_launch_tc_pair(ctx, PL, st);
-        if (rc) return rc;
-        continue;
-      }
-      if (tc) {
-        // ---- tensor-core path (tc_conv.cu) ----
-        TcLaunch TL;
-        for (int which = 0; which < 2; ++which) {
-          memset(&TL, 0, sizeof(TL));
-          TL.nprob = 3; TL.Cin = Co; TL.N = Co; TL.in_ld = Co; TL.out_ld = Co;
-          TL.B = B; TL.T_rows = rows; TL.rows_out = rows; TL.len = n_frames; TL.len_mul = scale;
-          TL.pre_mode = 1; TL.pre_slope = 0.1f; TL.f16 = f16;
-          for (int j = 0; j < 3; ++j) {
-            const int kk = vc::hg_rbk(j), n = i * 3 + j;
-            const int dd = which == 0 ? d : 1;
-            TcProb p;
-            memset(&p, 0, sizeof(p));
-            p.x0 = which == 0 ? src[j] : hb.Tb[j];
-            p.wpk = M.tiles(pk + PK_RB(n, which, m))[0];
-            p.bias = W[hgi::RB_B(n, which, m)];
-            p.resid = which == 0 ? nullptr : src[j];
-            p.out = which == 0 ? hb.Tb[j] : ((m == 1) ? hb.Bb[j] : hb.A[par][j]);
-            p.k = kk; p.dil = dd; p.in_off = -((kk - 1) * dd) / 2; p.out_stride = 1; p.out_off = 0;
-            TL.p[j] = p;
-          }
-          rc = vtts_launch_tc_conv(ctx, TL, st);
-          if (rc) return rc;
-        }
-        continue;
-      }
-      // conv1 (dilated)
-      memset(&L, 0, sizeof(L));
-      L.B = B; L.len = n_frames; L.len_mul = scale;
-      L.nprob = 3; L.Cin = Co; L.Cout = Co; L.T_rows = rows; L.rows_out = rows;
-      L.pre_mode = 1; L.pre_slope = 0.1f; L.post_act = 0;
+      float* dst[3];
       for (int j = 0; j < 3; ++j) {
-        const int kk = vc::hg_rbk(j), n = i * 3 + j;
-        ConvProb p;
-        memset(&p, 0, sizeof(p));
-        p.x0 = src[j];
-        p.w = W[hgi::RB_W(n, 0, m)]; p.bias = W[hgi::RB_B(n, 0, m)];
-        p.out = hb.Tb[j];
-        p.k = kk; p.dil = d; p.in_off = -((kk - 1) * d) / 2; p.out_stride = 1; p.out_off = 0;
-        L.p[j] = p;
+        src[j] = (m == 0) ? hb.X : (m == 1 ? hb.A[par][j] : hb.Bb[j]);
+        dst[j] = (m == 1) ? hb.Bb[j] : hb.A[par][j];
       }
-      rc = vtts_launch_conv(ctx, L, st);
-      if (rc) return rc;
-      // conv2 (dilation 1) + residual
-      for (int j = 0; j < 3; ++j) {
-        const int kk = vc::hg_rbk(j), n = i * 3 + j;
-        ConvProb p;
-        memset(&p, 0, sizeof(p));
-        p.x0 = hb.Tb[j];
-        p.w = W[hgi::RB_W(n, 1, m)]; p.bias = W[hgi::RB_B(n, 1, m)];
-        p.resid = src[j];
-        p.out = (m == 1) ? hb.Bb[j] : hb.A[par][j];
-        p.k = kk; p.dil = 1; p.in_off = -(kk - 1) / 2; p.out_stride = 1; p.out_off = 0;
-        L.p[j] = p;
-      }
-      rc = vtts_launch_conv(ctx, L, st);
+      rc = hg_resblock(ctx, i, m, src, dst, hb.Tb, n_frames, B, T, st);
       if (rc) return rc;
     }
-    C = Co;
-    rows_in = rows;
-    scale_in = scale;
     ctx->sub_mark(10 + i, st);
   }
-  // ---- mean of 3, lrelu(0.01), conv_post (32 -> 1, k7), tanh ----
-  {
-    const int R = rows_in;  // 256*T
-    dim3 grid((R + 255) / 256, B);
-    conv_post_kernel<<<grid, 256, 0, st>>>(hb.A[1][0], hb.A[1][1], hb.A[1][2], W[hgi::POST_W], W[hgi::POST_B], n_frames, 256, R, wav);
-    ctx->launches++;
-    VTTS_CUDA(cudaGetLastError());
-  }
+  rc = hg_conv_post(ctx, hb.A[1], wav, n_frames, B, T, st);
+  if (rc) return rc;
   ctx->sub_mark(14, st);
+  return VTTS_OK;
+}
+
+int vtts_debug_hifigan_layer(vtts_ctx* ctx, int layer, const float* const* x, float* const* out, const int32_t* n_frames, int B, int T) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  int rc = hg_check(ctx, B, T);
+  if (rc) return rc;
+  if (layer < 0 || layer > 17 || !x || !out) return ctx->fail(VTTS_ERR_BAD_ARG, "debug_hifigan_layer: layer %d (0..17), x and out required", layer);
+  const int nx = layer <= 1 ? 1 : 3, nout = (layer >= 5 && layer <= 16) ? 3 : 1;
+  for (int j = 0; j < nx; ++j)
+    if (!x[j]) return ctx->fail(VTTS_ERR_BAD_ARG, "debug_hifigan_layer: layer %d needs %d inputs", layer, nx);
+  for (int j = 0; j < nout; ++j)
+    if (!out[j]) return ctx->fail(VTTS_ERR_BAD_ARG, "debug_hifigan_layer: layer %d needs %d outputs", layer, nout);
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  if (layer == 0) {
+    rc = hg_conv_pre(ctx, x[0], out[0], n_frames, B, T, nullptr);
+  } else if (layer <= 4) {
+    rc = hg_ups(ctx, layer - 1, x, out[0], n_frames, B, T, nullptr);
+  } else if (layer <= 16) {
+    // conv1's outputs of the unfused pair: three buffers of the step's shape
+    const int i = (layer - 5) / 3, m = (layer - 5) % 3;
+    const size_t n = (size_t)B * T * hg_scale(i + 1) * (vc::HG_C0 >> (i + 1));
+    float* tmp = nullptr;
+    VTTS_CUDA(cudaMalloc(&tmp, 3 * n * sizeof(float)));
+    float* const t3[3] = {tmp, tmp + n, tmp + 2 * n};
+    rc = hg_resblock(ctx, i, m, x, out, t3, n_frames, B, T, nullptr);
+    const cudaError_t e = cudaDeviceSynchronize();
+    cudaFree(tmp);
+    if (!rc && e != cudaSuccess) return ctx->fail(VTTS_ERR_CUDA, "debug_hifigan_layer: %s", cudaGetErrorString(e));
+  } else {
+    rc = hg_conv_post(ctx, x, out[0], n_frames, B, T, nullptr);
+  }
+  if (rc) return rc;
+  VTTS_CUDA(cudaDeviceSynchronize());
   return VTTS_OK;
 }

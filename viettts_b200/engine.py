@@ -145,6 +145,22 @@ class Engine:
                                           B, T, Cc, int(k), int(dil), float(slope), _ptr(out)))
         return out
 
+    HIFIGAN_LAYERS = 18   # 0 conv_pre, 1..4 ConvTranspose of stage i - 1, 5 + 3i + m ResBlock step (i, m), 17 conv_post
+
+    def debug_hifigan_layer(self, layer, xs, outs, n_frames_t=None, T=None):
+        """Test hook (vtts_debug_hifigan_layer): exactly one layer of the generator forward on torch CUDA tensors, with
+        the loaded weights, the engine's precision mode and fused-pair setting.  xs: one tensor (layers 0 and 1) or three
+        (the chains of a stage), [B, rows, C]; outs: one tensor (three for the ResBlock steps 5..16), written in place
+        except the rows at or past n_frames_t[b] times the stage's rows per mel frame.  T (mel frames) defaults to the
+        rows of xs[0] divided by the stage's rows per mel frame."""
+        scale = [1, 1, 8, 64, 128] + [8] * 3 + [64] * 3 + [128] * 3 + [256] * 3 + [256]
+        B, rows = xs[0].shape[:2]
+        if T is None:
+            T = rows // scale[layer]
+        arr = lambda ts: (C.c_void_p * len(ts))(*[_ptr(t) for t in ts])  # noqa: E731
+        self._ck(self.lib.vtts_debug_hifigan_layer(self.h, int(layer), arr(xs), arr(outs), _ptr(n_frames_t), int(B), int(T)))
+        return outs
+
     PAIR_KERNELS = {"smem": 0, "tmem": 1, "smem2": 2}
 
     def set_fused_pairs(self, on: bool, kind: str | None = None):

@@ -246,6 +246,47 @@ int vtts_vocoder_stream_push(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float
 int vtts_vocoder_stream_push_host(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float* mel, const int32_t* n_new,
                                   const uint8_t* flags, float* wav, int32_t* n_out);
 
+/* ---- resampling to the caller's output rate ------------------------------------------------------------------
+ * (in_rate, out_rate) reduce by their gcd to up / down; both must be positive and up, down <= 1024 (every pair of
+ * standard rates reachable from 16 kHz qualifies: 16000 -> 44100 is 441 / 160, 16000 -> 11025 is 441 / 640), else
+ * VTTS_ERR_BAD_ARG.  The output is scipy.signal.resample_poly(x, up, down) with its defaults:
+ *   half = 10 * max(up, down);  h[k] = up * w[k] / sum(w),  w[k] = fc * sinc(fc * (k - half)) * kaiser(2 * half + 1, 5)[k],
+ *   fc = 1 / max(up, down);  y[m] = sum of x[i] * h[m * down + half - i * up] over 0 <= i < n with the index in
+ *   [0, 2 * half];  len(y) = ceil(n * up / down).
+ * up == down is an exact copy.  The taps are designed in double and rounded to fp32 once (cached in the context per
+ * ratio); every output is an fp32 FMA sum in ascending input index, in every vtts_precision mode. */
+/* the double-precision filter h[0 .. 2 * half] of the ratio (a single 1.0 when up == down) into taps[capacity] if it
+ * fits; returns the tap count, or VTTS_ERR_BAD_ARG.  Needs no device. */
+int vtts_resample_filter(int in_rate, int out_rate, double* taps, int capacity);
+/* x_dev [B,S_in]; n_in_dev int32 [B] or NULL (= S_in); y_dev [B,S_out] with S_out = ceil(S_in * up / down); outputs
+ * past ceil(n_in[b] * up / down) are 0.  Stream-ordered. */
+int vtts_resample(vtts_ctx* ctx, const float* x_dev, const int32_t* n_in_dev, int B, int S_in, int in_rate, int out_rate,
+                  float* y_dev, void* stream);
+/* the same on host buffers */
+int vtts_resample_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S_in, int in_rate, int out_rate, float* y);
+/* Streaming resampler with max_streams independent slots: each slot carries its filter history (at most
+ * 2 * half / up + 1 input samples and a 64-bit position) across pushes, so the outputs a slot emits, concatenated, are
+ * bit-identical to vtts_resample of its whole input.  An output is emitted with the first push after which every input
+ * it reads has arrived: before END a slot that has received P samples has emitted
+ * min(ceil(P * up / down), max(0, floor((P * up - 1 - half) / down) + 1)) outputs; END emits the rest.
+ * vtts_resample_stream_lookahead = floor(half / up): how many input samples an output reads past its own time.
+ * flags and slot rules as for the vocoder stream: bit0 BEGIN (resets the slot, also an open one; may be combined with
+ * END), bit1 END; n_new = 0 without flags leaves a slot idle and untouched; frames or END to a slot that is not open
+ * fail with VTTS_ERR_BAD_ARG.  Every push issues the same two launches. */
+typedef struct vtts_resample_stream vtts_resample_stream;
+/* *out_pitch receives the outputs per slot of a push's output buffer */
+int vtts_resample_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int in_rate, int out_rate,
+                                vtts_resample_stream** out, int* out_pitch);
+int vtts_resample_stream_destroy(vtts_ctx* ctx, vtts_resample_stream* rs);
+int vtts_resample_stream_lookahead(int in_rate, int out_rate);
+/* x_dev [S][max_chunk_samples] (samples past n_new[s] ignored); n_new, flags, n_out HOST int32 / uint8 / int32 [S];
+ * y_dev [S][out_pitch], slot s gets n_out[s] outputs from its start.  Stream-ordered. */
+int vtts_resample_stream_push(vtts_ctx* ctx, vtts_resample_stream* rs, const float* x_dev, const int32_t* n_new,
+                              const uint8_t* flags, float* y_dev, int32_t* n_out, void* stream);
+/* the same on host buffers x [S][max_chunk_samples] and y [S][out_pitch]; returns when y is written */
+int vtts_resample_stream_push_host(vtts_ctx* ctx, vtts_resample_stream* rs, const float* x, const int32_t* n_new,
+                                   const uint8_t* flags, float* y, int32_t* n_out);
+
 /* ---- streaming acoustic model: every slot advances its decoder a few frames per push ---------------------------
  * A vtts_acoustic_stream holds max_streams (1..128) independent slots.  begin starts utterances in closed slots; each
  * push advances every open slot by min(F, frames left) decoder steps in ONE scan launch and returns the mel frames whose

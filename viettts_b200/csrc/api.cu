@@ -351,6 +351,7 @@ int vtts_destroy(vtts_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
   for (auto& m : kModels) vtts_free_weights(ctx->*m.w);
+  vtts_resample_free(ctx);
   cudaFree(ctx->mel_fb); cudaFree(ctx->mel_lo); cudaFree(ctx->mel_hi); cudaFree(ctx->fft_tw); cudaFree(ctx->hann);
   cudaFree(ctx->ws); cudaFree(ctx->dstage); cudaFree(ctx->d_err); cudaFree(ctx->d_tc_sched); cudaFree(ctx->d_tc_dbg);
   if (ctx->hpin) cudaFreeHost(ctx->hpin);

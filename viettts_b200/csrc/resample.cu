@@ -1,0 +1,462 @@
+// Rational-rate resampling of synthesized audio: exactly scipy.signal.resample_poly(x, up, down) with its defaults
+// (Kaiser beta = 5 low-pass of 2 * half + 1 taps, half = 10 * max(up, down), zero padding), in fp32 on the device.
+//
+// Filter.  Designed on the host in double precision (Kaiser window through an I0 series, cutoff 1 / max(up, down), unit
+// DC gain, times up), rounded to fp32 once and cached in the context per reduced ratio.  Polyphase layout [phase][tap]
+// with T = ceil((2 * half + 1) / up) taps per phase: output m has j = m * down + half, phase p = j mod up and top input
+// it = floor(j / up); tap t of phase p multiplies input it - (T - 1) + t and holds h[p + (T - 1 - t) * up] (0 past
+// 2 * half).  Every output is therefore the same T-term fp32 FMA sum in ascending input index, a function of m alone:
+// the one-shot call and every push pattern of the stream produce the same bits.  up == down is a copy (T = 1, h = 1).
+//
+// Windows.  A CTA computes a tile of consecutive outputs of one row; it stages the filter and the input span the tile
+// reads in shared memory.  Per-row bounds (RsRow) place the row's buffer in absolute time: element 0 is input x0, inputs
+// outside [lo, hi) read as zero, outputs m0 .. m0 + n_calc - 1 are computed and written from the row's start and the
+// outputs after them up to n_out are written as zero.  Absolute input and output indices are 64-bit: m * down + half
+// passes 2^31 after about 4.9 M input samples at 16000 -> 11025.
+//
+// Stream.  Per slot a window of K + F inputs (K = T - 1 carried, F = max chunk); one prep launch per push moves the last
+// K inputs of the previous push to the front and copies the new ones after them, then resample_kernel runs on the
+// windows with bounds built on the host.
+#include <algorithm>
+#include <cmath>
+
+#include "vtts_internal.cuh"
+
+namespace {
+
+constexpr int RS_MAX_FACTOR = 1024;   // largest reduced up / down
+constexpr int RS_THREADS = 256;
+constexpr int RS_SMEM_MAX = 227 * 1024;
+
+struct RsRatio {
+  int up, down, half, T;
+};
+
+long long gcd_ll(long long a, long long b) {
+  while (b) {
+    long long t = a % b;
+    a = b;
+    b = t;
+  }
+  return a;
+}
+
+// 0, or VTTS_ERR_BAD_ARG for a non-positive rate or a reduced ratio past RS_MAX_FACTOR
+int rs_ratio(int in_rate, int out_rate, RsRatio* r) {
+  if (in_rate <= 0 || out_rate <= 0) return VTTS_ERR_BAD_ARG;
+  const long long g = gcd_ll(in_rate, out_rate);
+  r->up = (int)(out_rate / g);
+  r->down = (int)(in_rate / g);
+  if (r->up > RS_MAX_FACTOR || r->down > RS_MAX_FACTOR) return VTTS_ERR_BAD_ARG;
+  r->half = r->up == r->down ? 0 : 10 * std::max(r->up, r->down);
+  r->T = (2 * r->half + r->up) / r->up;   // ceil((2 * half + 1) / up)
+  return VTTS_OK;
+}
+
+double bessel_i0(double x) {
+  double sum = 1.0, term = 1.0;
+  const double q = 0.25 * x * x;
+  for (int k = 1; k < 500; ++k) {
+    term *= q / ((double)k * k);
+    sum += term;
+    if (term < 1e-17 * sum) break;
+  }
+  return sum;
+}
+
+// h[0 .. 2 * half]: firwin(2 * half + 1, 1 / max(up, down), window=('kaiser', 5.0)) * up
+std::vector<double> rs_design(const RsRatio& r) {
+  if (r.half == 0) return {1.0};
+  const int L = 2 * r.half + 1;
+  const double fc = 1.0 / std::max(r.up, r.down), beta = 5.0, i0b = bessel_i0(beta), pi = 3.14159265358979323846;
+  std::vector<double> h(L);
+  double sum = 0.0;
+  for (int k = 0; k < L; ++k) {
+    const double a = (double)(k - r.half) / r.half;
+    const double w = bessel_i0(beta * std::sqrt(std::max(0.0, 1.0 - a * a))) / i0b;
+    const double t = fc * (k - r.half);
+    const double y = pi * (t == 0.0 ? 1e-20 : t);
+    h[k] = fc * (std::sin(y) / y) * w;
+    sum += h[k];
+  }
+  for (int k = 0; k < L; ++k) h[k] = h[k] / sum * r.up;
+  return h;
+}
+
+struct RsRow {
+  long long x0;       // absolute input index of buffer element 0
+  long long lo, hi;   // inputs outside [lo, hi) read as zero
+  long long m0;       // absolute index of the row's first output
+  long long n_calc;   // outputs computed
+  long long n_out;    // outputs written (the ones past n_calc as zero)
+};
+
+// rows == nullptr: the one-shot bounds of row b, inputs [0, n_b) with n_b = n_in[b] (or S_in), S_out outputs of which
+// the first ceil(n_b * up / down) are computed
+__global__ void __launch_bounds__(RS_THREADS) resample_kernel(const float* __restrict__ x, long long x_ld, int S_in,
+                                                              const int* __restrict__ n_in, const RsRow* __restrict__ rows,
+                                                              const float* __restrict__ taps, int up, int down, int half, int T,
+                                                              long long S_out, int TM, float* __restrict__ y, long long y_ld) {
+  extern __shared__ float rs_smem[];
+  const int b = blockIdx.y, tid = threadIdx.x;
+  RsRow r;
+  if (rows) {
+    r = rows[b];
+  } else {
+    const long long n = n_in ? (long long)min(max(n_in[b], 0), S_in) : (long long)S_in;
+    r.x0 = 0; r.lo = 0; r.hi = n; r.m0 = 0; r.n_out = S_out;
+    r.n_calc = min(S_out, (n * up + down - 1) / down);
+  }
+  const long long t0 = (long long)blockIdx.x * TM;
+  if (t0 >= r.n_out) return;
+  const int cnt = (int)min((long long)TM, r.n_out - t0);
+  const int cc = (int)max(0LL, min((long long)cnt, r.n_calc - t0));
+  float* yr = y + (size_t)b * y_ld + t0;
+  for (int q = cc + tid; q < cnt; q += RS_THREADS) yr[q] = 0.f;
+  if (cc == 0) return;
+
+  const long long mA = r.m0 + t0;
+  const long long i_lo = (mA * down + half) / up - (T - 1);
+  const long long i_hi = ((mA + cc - 1) * down + half) / up;
+  const int span = (int)(i_hi - i_lo + 1);
+  float* hs = rs_smem;
+  float* xs = rs_smem + up * T;
+  for (int e = tid; e < up * T; e += RS_THREADS) hs[e] = taps[e];
+  const long long lo = max(r.lo, r.x0), hi = r.hi;
+  const float* xr = x + (size_t)b * x_ld;
+  for (int e = tid; e < span; e += RS_THREADS) {
+    const long long i = i_lo + e;
+    xs[e] = (i >= lo && i < hi) ? __ldg(xr + (i - r.x0)) : 0.f;
+  }
+  __syncthreads();
+  for (int q = tid; q < cc; q += RS_THREADS) {
+    const long long j = (mA + q) * down + half;
+    const long long it = j / up;
+    const int p = (int)(j - it * up);
+    const float* xq = xs + (it - (T - 1) - i_lo);
+    const float* hq = hs + p * T;
+    float acc = xq[0] * hq[0];
+#pragma unroll 4
+    for (int t = 1; t < T; ++t) acc = fmaf(xq[t], hq[t], acc);
+    yr[q] = acc;
+  }
+}
+
+// per slot: tbl[2s] = inputs of the previous push (its window tail [shift, shift + K) moves to [0, K)), tbl[2s + 1] =
+// new inputs to copy to [K, K + n)
+__global__ void __launch_bounds__(RS_THREADS) resample_prep_kernel(float* __restrict__ win, int cap, int K, const int* __restrict__ tbl,
+                                                                   const float* __restrict__ x, int F) {
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int shift = tbl[2 * b], n = tbl[2 * b + 1];
+  float* w = win + (size_t)b * cap;
+  if (shift > 0) {
+    // source and destination overlap when the push was shorter than the carry: each block of 1024 values is read
+    // completely before it is written, in ascending order (the destination lies before the source)
+    constexpr int U = 4;
+    for (int i0 = 0; i0 < K; i0 += RS_THREADS * U) {
+      float v[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int i = i0 + u * RS_THREADS + tid;
+        if (i < K) v[u] = w[shift + i];
+      }
+      __syncthreads();
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int i = i0 + u * RS_THREADS + tid;
+        if (i < K) w[i] = v[u];
+      }
+      __syncthreads();
+    }
+  }
+  const float* src = x + (size_t)b * F;
+  for (int i = tid; i < n; i += RS_THREADS) w[K + i] = src[i];
+}
+
+// tile of outputs per CTA: 1024 unless the filter plus the input span do not fit in shared memory
+int rs_tile(const RsRatio& r, size_t* smem) {
+  int TM = 1024;
+  auto bytes = [&](int tm) { return ((size_t)r.up * r.T + ((size_t)(tm - 1) * r.down + r.up - 1) / r.up + r.T) * sizeof(float); };
+  while (TM > 1 && bytes(TM) > (size_t)RS_SMEM_MAX) TM /= 2;
+  *smem = bytes(TM);
+  return TM;
+}
+
+// the context's fp32 polyphase filter of ratio r (designed and uploaded at the first use)
+int rs_filter(vtts_ctx* ctx, const RsRatio& r, const float** out) {
+  for (const auto& f : ctx->rs_filters)
+    if (f.up == r.up && f.down == r.down) {
+      *out = f.taps;
+      return VTTS_OK;
+    }
+  const std::vector<double> h = rs_design(r);
+  std::vector<float> pp((size_t)r.up * r.T, 0.f);
+  for (int p = 0; p < r.up; ++p)
+    for (int t = 0; t < r.T; ++t) {
+      const long long k = p + (long long)(r.T - 1 - t) * r.up;
+      if (k <= 2 * r.half) pp[(size_t)p * r.T + t] = (float)h[k];
+    }
+  float* d = nullptr;
+  VTTS_CUDA(cudaMalloc(&d, pp.size() * sizeof(float)));
+  cudaError_t e = cudaMemcpy(d, pp.data(), pp.size() * sizeof(float), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    cudaFree(d);
+    return ctx->fail(VTTS_ERR_CUDA, "resample: filter upload: %s", cudaGetErrorString(e));
+  }
+  ctx->rs_filters.push_back({r.up, r.down, d});
+  *out = d;
+  return VTTS_OK;
+}
+
+int rs_launch(vtts_ctx* ctx, const RsRatio& r, const float* taps, const float* x, long long x_ld, int S_in, const int* n_in,
+              const RsRow* rows, int B, long long S_out, long long max_out, float* y, long long y_ld, cudaStream_t st) {
+  size_t smem = 0;
+  const int TM = rs_tile(r, &smem);
+  static bool attr_set[64] = {};
+  if (ctx->device < 64 && !attr_set[ctx->device]) {
+    VTTS_CUDA(cudaFuncSetAttribute(resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RS_SMEM_MAX));
+    attr_set[ctx->device] = true;
+  }
+  const long long tiles = std::max(1LL, (max_out + TM - 1) / TM);
+  resample_kernel<<<dim3((unsigned)tiles, B), RS_THREADS, smem, st>>>(x, x_ld, S_in, n_in, rows, taps, r.up, r.down, r.half, r.T, S_out, TM,
+                                                                     y, y_ld);
+  ctx->launches++;
+  VTTS_CUDA(cudaGetLastError());
+  return VTTS_OK;
+}
+
+long long ceil_div(long long a, long long b) { return (a + b - 1) / b; }
+
+}  // namespace
+
+void vtts_resample_free(vtts_ctx* ctx) {
+  for (auto& f : ctx->rs_filters) cudaFree(f.taps);
+  ctx->rs_filters.clear();
+}
+
+int vtts_resample_filter(int in_rate, int out_rate, double* taps, int capacity) {
+  RsRatio r;
+  if (rs_ratio(in_rate, out_rate, &r)) return VTTS_ERR_BAD_ARG;
+  const std::vector<double> h = rs_design(r);
+  if (taps && capacity >= (int)h.size()) std::copy(h.begin(), h.end(), taps);
+  return (int)h.size();
+}
+
+int vtts_resample(vtts_ctx* ctx, const float* x_dev, const int32_t* n_in_dev, int B, int S_in, int in_rate, int out_rate, float* y_dev,
+                  void* stream) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  RsRatio r;
+  if (rs_ratio(in_rate, out_rate, &r))
+    return ctx->fail(VTTS_ERR_BAD_ARG, "resample: rates %d -> %d (positive, reduced ratio up / down <= %d)", in_rate, out_rate, RS_MAX_FACTOR);
+  if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "resample: null pointer");
+  if (B < 1 || B > 65535 || S_in < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "resample: B=%d S_in=%d (1..65535, >= 1)", B, S_in);
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  const float* taps = nullptr;
+  int rc = rs_filter(ctx, r, &taps);
+  if (rc) return rc;
+  const long long S_out = ceil_div((long long)S_in * r.up, r.down);
+  return rs_launch(ctx, r, taps, x_dev, S_in, S_in, n_in_dev, nullptr, B, S_out, S_out, y_dev, S_out, (cudaStream_t)stream);
+}
+
+int vtts_resample_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S_in, int in_rate, int out_rate, float* y) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  RsRatio r;
+  if (rs_ratio(in_rate, out_rate, &r))
+    return ctx->fail(VTTS_ERR_BAD_ARG, "resample_host: rates %d -> %d (positive, reduced ratio up / down <= %d)", in_rate, out_rate,
+                     RS_MAX_FACTOR);
+  if (!x || !y || B < 1 || B > 65535 || S_in < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_host: bad argument");
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  const size_t x_b = (size_t)B * S_in * 4, n_b = (size_t)B * 4;
+  const size_t y_b = (size_t)B * ceil_div((long long)S_in * r.up, r.down) * 4;
+  const size_t o_n = (x_b + 255) & ~size_t(255), o_y = (o_n + n_b + 255) & ~size_t(255);
+  int rc = ctx->ensure_staging(o_y + y_b, o_y + y_b);
+  if (rc) return rc;
+  char* hp = (char*)ctx->hpin;
+  char* dp = (char*)ctx->dstage;
+  cudaStream_t st = ctx->own_stream;
+  memcpy(hp, x, x_b);
+  if (n_in) memcpy(hp + o_n, n_in, n_b);
+  VTTS_CUDA(cudaMemcpyAsync(dp, hp, n_in ? o_n + n_b : x_b, cudaMemcpyHostToDevice, st));
+  rc = vtts_resample(ctx, (const float*)dp, n_in ? (const int32_t*)(dp + o_n) : nullptr, B, S_in, in_rate, out_rate, (float*)(dp + o_y), st);
+  if (rc) {
+    cudaStreamSynchronize(st);   // the staging copy must not outlive the call
+    return rc;
+  }
+  VTTS_CUDA(cudaMemcpyAsync(hp + o_y, dp + o_y, y_b, cudaMemcpyDeviceToHost, st));
+  VTTS_CUDA(cudaStreamSynchronize(st));
+  memcpy(y, hp + o_y, y_b);
+  return VTTS_OK;
+}
+
+// ---- stream ---------------------------------------------------------------------------------------------------
+struct vtts_resample_stream {
+  vtts_ctx* ctx = nullptr;
+  RsRatio r{};
+  int S = 0, F = 0, K = 0, cap = 0, out_pitch = 0;
+  const float* taps = nullptr;
+  void* mem = nullptr;          // windows [S][cap], then the per-push tables
+  float* win = nullptr;
+  RsRow* d_rows = nullptr;
+  int* d_prep = nullptr;
+  // per slot: inputs received since BEGIN, outputs emitted, open, inputs of the last push whose tail has not moved yet
+  std::vector<long long> P, E;
+  std::vector<int> open, pending;
+  std::vector<char> tbl;        // host image of the per-push tables: RsRow [S], then int [S][2]
+};
+
+int vtts_resample_stream_lookahead(int in_rate, int out_rate) {
+  RsRatio r;
+  if (rs_ratio(in_rate, out_rate, &r)) return VTTS_ERR_BAD_ARG;
+  return r.half / r.up;
+}
+
+int vtts_resample_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int in_rate, int out_rate,
+                                vtts_resample_stream** out, int* out_pitch) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  if (!out || !out_pitch) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_create: null output pointer");
+  *out = nullptr;
+  RsRatio r;
+  if (rs_ratio(in_rate, out_rate, &r))
+    return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_create: rates %d -> %d (positive, reduced ratio up / down <= %d)", in_rate, out_rate,
+                     RS_MAX_FACTOR);
+  if (max_streams < 1 || max_streams > 65535 || max_chunk_samples < 1 || max_chunk_samples > (1 << 22))
+    return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_create: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", max_streams,
+                     max_chunk_samples, 1 << 22);
+  // outputs per push: fewer than (n_new * up + half + 1) / down + 1 (see the schedule in vtts_resample_stream_push)
+  const long long pitch = ceil_div((long long)max_chunk_samples * r.up + r.half + 1, r.down);
+  if (pitch > (1LL << 30)) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_create: %lld outputs per push", pitch);
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  const float* taps = nullptr;
+  int rc = rs_filter(ctx, r, &taps);
+  if (rc) return rc;
+  vtts_resample_stream* rs = new vtts_resample_stream;
+  rs->ctx = ctx;
+  rs->r = r;
+  rs->S = max_streams;
+  rs->F = max_chunk_samples;
+  rs->K = r.T - 1;
+  rs->cap = rs->K + max_chunk_samples;
+  rs->out_pitch = (int)pitch;
+  rs->taps = taps;
+  const size_t win_b = ((size_t)max_streams * rs->cap * sizeof(float) + 255) & ~size_t(255);
+  const size_t rows_b = ((size_t)max_streams * sizeof(RsRow) + 255) & ~size_t(255);
+  const size_t bytes = win_b + rows_b + (size_t)max_streams * 2 * sizeof(int);
+  cudaError_t e = cudaMalloc(&rs->mem, bytes);
+  if (e == cudaSuccess) e = cudaMemset(rs->mem, 0, bytes);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    if (rs->mem) cudaFree(rs->mem);
+    delete rs;
+    return ctx->fail(e == cudaErrorMemoryAllocation ? VTTS_ERR_OOM : VTTS_ERR_CUDA, "resample_stream_create: %zu bytes: %s", bytes,
+                     cudaGetErrorString(e));
+  }
+  rs->win = (float*)rs->mem;
+  rs->d_rows = (RsRow*)((char*)rs->mem + win_b);
+  rs->d_prep = (int*)((char*)rs->mem + win_b + rows_b);
+  rs->P.assign(max_streams, 0);
+  rs->E.assign(max_streams, 0);
+  rs->open.assign(max_streams, 0);
+  rs->pending.assign(max_streams, 0);
+  rs->tbl.assign((size_t)max_streams * (sizeof(RsRow) + 2 * sizeof(int)), 0);
+  *out = rs;
+  *out_pitch = rs->out_pitch;
+  return VTTS_OK;
+}
+
+int vtts_resample_stream_destroy(vtts_ctx* ctx, vtts_resample_stream* rs) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  if (!rs) return VTTS_OK;
+  if (rs->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_destroy: the stream belongs to another context");
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  VTTS_CUDA(cudaDeviceSynchronize());   // a push may still be running on the caller's stream
+  cudaFree(rs->mem);
+  delete rs;
+  return VTTS_OK;
+}
+
+int vtts_resample_stream_push(vtts_ctx* ctx, vtts_resample_stream* rs, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
+                              float* y_dev, int32_t* n_out, void* stream) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  if (!rs || rs->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_push: the stream belongs to another context");
+  if (!x_dev || !n_new || !flags || !y_dev || !n_out) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_push: null pointer");
+  const int S = rs->S, F = rs->F;
+  for (int s = 0; s < S; ++s) {
+    if (n_new[s] < 0 || n_new[s] > F) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_push: n_new[%d]=%d outside [0, %d]", s, n_new[s], F);
+    if (flags[s] & ~3u) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_push: flags[%d]=%u (bit0 BEGIN, bit1 END)", s, flags[s]);
+    const bool idle = n_new[s] == 0 && flags[s] == 0;
+    if (!idle && !(flags[s] & 1) && !rs->open[s])
+      return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_push: slot %d is not open (push BEGIN first, also after END)", s);
+  }
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const RsRatio& r = rs->r;
+
+  // ---- host bookkeeping: an output is emitted once every input it reads has arrived, i.e. after P inputs (before END)
+  // the slot has emitted min(ceil(P * up / down), max(0, floor((P * up - 1 - half) / down) + 1)) outputs ----
+  RsRow* rows = reinterpret_cast<RsRow*>(rs->tbl.data());
+  int* prep = reinterpret_cast<int*>(rs->tbl.data() + (size_t)S * sizeof(RsRow));
+  std::vector<long long> E1(S);
+  long long max_out = 0;
+  for (int s = 0; s < S; ++s) {
+    const bool act = n_new[s] > 0 || flags[s] != 0, begin = flags[s] & 1, end = flags[s] & 2;
+    const long long P0 = begin ? 0 : rs->P[s], E0 = begin ? 0 : rs->E[s], P1 = P0 + n_new[s];
+    long long e = E0;
+    if (act) {
+      const long long total = ceil_div(P1 * r.up, r.down), v = P1 * r.up - 1 - r.half;
+      e = end ? total : std::min(total, v < 0 ? 0 : v / r.down + 1);
+    }
+    E1[s] = e;
+    n_out[s] = (int32_t)(e - E0);
+    rows[s] = RsRow{P0 - rs->K, std::max(0LL, P0 - rs->K), P1, E0, e - E0, e - E0};
+    prep[2 * s] = act && !begin ? rs->pending[s] : 0;
+    prep[2 * s + 1] = act ? n_new[s] : 0;
+    max_out = std::max(max_out, e - E0);
+  }
+
+  // ---- device: one table copy, prep, resample ----
+  // pageable source: the call returns once the table is staged, so rs->tbl may be rewritten by the next push
+  VTTS_CUDA(cudaMemcpyAsync(rs->d_rows, rows, (size_t)S * sizeof(RsRow), cudaMemcpyHostToDevice, st));
+  VTTS_CUDA(cudaMemcpyAsync(rs->d_prep, prep, (size_t)S * 2 * sizeof(int), cudaMemcpyHostToDevice, st));
+  resample_prep_kernel<<<S, RS_THREADS, 0, st>>>(rs->win, rs->cap, rs->K, rs->d_prep, x_dev, F);
+  ctx->launches++;
+  VTTS_CUDA(cudaGetLastError());
+  int rc = rs_launch(ctx, r, rs->taps, rs->win, rs->cap, rs->cap, nullptr, rs->d_rows, S, 0, max_out, y_dev, rs->out_pitch, st);
+  if (rc) return rc;
+
+  // ---- commit the slot state ----
+  for (int s = 0; s < S; ++s) {
+    const bool act = n_new[s] > 0 || flags[s] != 0, begin = flags[s] & 1, end = flags[s] & 2;
+    if (!act) continue;
+    rs->P[s] = (begin ? 0 : rs->P[s]) + n_new[s];
+    rs->E[s] = E1[s];
+    rs->open[s] = !end;
+    rs->pending[s] = end ? 0 : n_new[s];
+  }
+  return VTTS_OK;
+}
+
+int vtts_resample_stream_push_host(vtts_ctx* ctx, vtts_resample_stream* rs, const float* x, const int32_t* n_new, const uint8_t* flags,
+                                   float* y, int32_t* n_out) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  if (!rs || rs->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_push_host: the stream belongs to another context");
+  if (!x || !y) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_push_host: null pointer");
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  const size_t x_b = (size_t)rs->S * rs->F * 4, y_b = (size_t)rs->S * rs->out_pitch * 4;
+  const size_t o_y = (x_b + 255) & ~size_t(255);
+  int rc = ctx->ensure_staging(o_y + y_b, o_y + y_b);
+  if (rc) return rc;
+  char* hp = (char*)ctx->hpin;
+  char* dp = (char*)ctx->dstage;
+  cudaStream_t st = ctx->own_stream;
+  memcpy(hp, x, x_b);
+  VTTS_CUDA(cudaMemcpyAsync(dp, hp, x_b, cudaMemcpyHostToDevice, st));
+  rc = vtts_resample_stream_push(ctx, rs, (const float*)dp, n_new, flags, (float*)(dp + o_y), n_out, st);
+  if (rc) {
+    cudaStreamSynchronize(st);   // the staging copy must not outlive the call
+    return rc;
+  }
+  VTTS_CUDA(cudaMemcpyAsync(hp + o_y, dp + o_y, y_b, cudaMemcpyDeviceToHost, st));
+  VTTS_CUDA(cudaStreamSynchronize(st));
+  memcpy(y, hp + o_y, y_b);
+  return VTTS_OK;
+}

@@ -201,6 +201,10 @@ struct vtts_ctx {
   void* dstage = nullptr;
   size_t dstage_bytes = 0;
 
+  // fp32 polyphase filters of the resampler (resample.cu), one per reduced ratio up / down, designed at first use
+  struct RsFilter { int up, down; float* taps; };
+  std::vector<RsFilter> rs_filters;
+
   // taps of the last acoustic forward (point into ws)
   float* tap_enc = nullptr; int64_t tap_enc_n = 0;
   float* tap_cond = nullptr; int64_t tap_cond_n = 0;
@@ -330,6 +334,8 @@ size_t vtts_duration_ws_bytes(int B, int L);
 // DurationModel.__call__ (model.py:64-70); dur_sec [B][L] seconds, 0 past lengths[b]
 int vtts_duration_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, int B, int L, float* dur_sec,
                       cudaStream_t st);
+// resample.cu: frees the context's cached resampling filters
+void vtts_resample_free(vtts_ctx* ctx);
 // melspec.cu
 int vtts_melspec_prepare(vtts_ctx* ctx);
 int vtts_melspec_run(vtts_ctx* ctx, const float* wav, int B, int S, float* mel, cudaStream_t st);

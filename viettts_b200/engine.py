@@ -35,6 +35,22 @@ PRECISIONS = {"fp32": PRECISION_FP32, "bf16x3": PRECISION_BF16X3, "fp16": PRECIS
 MAX_ACOUSTIC_ROWS = 128   # rows per vtts_acoustic_forward call (csrc/nat.cu MAX_ROWS)
 
 
+def resample_ratio(in_rate: int, out_rate: int):
+    """(up, down): out_rate / in_rate in lowest terms, as vtts_resample takes it (each must be <= 1024)"""
+    from math import gcd
+    in_rate, out_rate = int(in_rate), int(out_rate)
+    if in_rate <= 0 or out_rate <= 0:
+        raise ValueError(f"sample rates must be positive, got {in_rate} -> {out_rate}")
+    g = gcd(in_rate, out_rate)
+    return out_rate // g, in_rate // g
+
+
+def resample_length(n: int, in_rate: int, out_rate: int) -> int:
+    """ceil(n * up / down): the samples `Engine.resample` makes of n input samples"""
+    up, down = resample_ratio(in_rate, out_rate)
+    return -(-int(n) * up // down)
+
+
 def _ptr(a):
     if a is None:
         return None
@@ -282,12 +298,13 @@ class Engine:
         return AcousticStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, masks=masks)
 
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
-                        rng=None) -> "TtsStream":
+                        rng=None, output_rate=None) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
-        With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  Needs the 'bf16x3' or 'fp16'
-        mode (the vocoder stream has no strict fp32 path)."""
-        return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng)
+        With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  `output_rate`: a resample
+        stream follows the vocoder on the device and `step()` returns samples at that rate, equal to `resample` of the
+        `tts` audio bit for bit.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
+        return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -630,6 +647,46 @@ class Engine:
         self._ck(self.lib.vtts_melspec(self.h, _ptr(wav_t), B, S, _ptr(out), st))
         return out
 
+    # ---- resampling to an output rate (vtts_resample*: scipy.signal.resample_poly with its defaults, fp32) ----
+    def resample(self, wav, out_rate: int, in_rate: int = config.SAMPLE_RATE, lengths=None) -> np.ndarray:
+        """Host arrays: wav f32 [S] or [B,S] at `in_rate` -> [ceil(S * up / down)] or [B, that] at `out_rate`, where up /
+        down is out_rate / in_rate in lowest terms (each <= 1024).  lengths int [B]: row b holds lengths[b] samples,
+        and its outputs past ceil(lengths[b] * up / down) are 0.  Equals scipy.signal.resample_poly(x, up, down) up to
+        fp32 rounding; in_rate == out_rate is a copy."""
+        x = _np(wav, np.float32)
+        one = x.ndim == 1
+        x = x[None] if one else x
+        if x.ndim != 2 or x.shape[1] < 1:
+            raise ValueError(f"wav must be [S] or [B,S], got {np.shape(wav)}")
+        B, S = x.shape
+        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
+        y = np.empty((B, resample_length(S, in_rate, out_rate)), np.float32)
+        self._ck(self.lib.vtts_resample_host(self.h, _ptr(x), _ptr(lens), B, S, int(in_rate), int(out_rate), _ptr(y)))
+        return y[0] if one else y
+
+    def resample_forward(self, x_t, out_rate: int, in_rate: int = config.SAMPLE_RATE, lengths_t=None, out=None, stream=None):
+        """vtts_resample on torch CUDA tensors, stream-ordered: x_t f32 [B,S] -> [B, ceil(S * up / down)]; lengths_t
+        int32 CUDA [B] or None."""
+        import torch
+        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
+        B, S = x_t.shape
+        n = resample_length(S, in_rate, out_rate)
+        if out is None:
+            out = torch.empty((B, n), dtype=torch.float32, device=x_t.device)
+        elif tuple(out.shape) != (B, n) or out.dtype != torch.float32 or not out.is_contiguous():
+            raise ValueError(f"out must be contiguous float32 [{B}, {n}]")
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self._ck(self.lib.vtts_resample(self.h, _ptr(x_t), _ptr(lengths_t), B, S, int(in_rate), int(out_rate), _ptr(out), st))
+        return out
+
+    def open_resample_stream(self, max_streams: int, max_chunk_samples: int, out_rate: int,
+                             in_rate: int = config.SAMPLE_RATE) -> "ResampleStream":
+        """Streaming resampler with `max_streams` independent slots (vtts_resample_stream_*): each slot carries its
+        filter history across pushes, so its outputs, concatenated, equal `resample` of its whole input bit for bit.
+        An output is emitted as soon as every input it reads has arrived (at most `lookahead` samples after its own
+        time); END emits the rest."""
+        return ResampleStream(self, max_streams, max_chunk_samples, out_rate, in_rate)
+
 
 STREAM_BEGIN, STREAM_END = 1, 2
 
@@ -692,6 +749,78 @@ class VocoderStream:
     def close(self):
         if getattr(self, "h", None) and getattr(self.eng, "h", None):
             self.eng._ck(self.eng.lib.vtts_vocoder_stream_destroy(self.eng.h, self.h))
+        self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class ResampleStream:
+    """Handle of a streaming resampler (Engine.open_resample_stream).  Before END a slot that has received P samples
+    has emitted min(ceil(P up / down), max(0, floor((P up - 1 - half) / down) + 1)) outputs, half = 10 max(up, down);
+    a push with END emits the rest."""
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, out_rate: int, in_rate: int = config.SAMPLE_RATE):
+        self.eng = eng
+        self.max_streams, self.max_chunk_samples = int(max_streams), int(max_chunk_samples)
+        self.in_rate, self.out_rate = int(in_rate), int(out_rate)
+        resample_ratio(self.in_rate, self.out_rate)
+        h, pitch = C.c_void_p(), C.c_int()
+        eng._ck(eng.lib.vtts_resample_stream_create(eng.h, self.max_streams, self.max_chunk_samples, self.in_rate, self.out_rate,
+                                                    C.byref(h), C.byref(pitch)))
+        self.h = h
+        self.out_pitch = int(pitch.value)   # outputs per slot of a push's output buffer
+        self.lookahead = int(eng.lib.vtts_resample_stream_lookahead(self.in_rate, self.out_rate))
+
+    def push(self, x, n_new, begin=None, end=None) -> list:
+        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None.
+        Returns one float32 array per slot with the samples it emits now."""
+        S, F = self.max_streams, self.max_chunk_samples
+        x = _np(x, np.float32)
+        if x.ndim != 2 or x.shape[0] != S or x.shape[1] > F:
+            raise ValueError(f"x must be [{S}, <= {F}], got {x.shape}")
+        if x.shape[1] < F:
+            x = np.concatenate([x, np.zeros((S, F - x.shape[1]), np.float32)], axis=1)
+        flags = np.zeros(S, np.uint8)
+        if begin is not None:
+            flags |= np.asarray(begin, bool).astype(np.uint8) * STREAM_BEGIN
+        if end is not None:
+            flags |= np.asarray(end, bool).astype(np.uint8) * STREAM_END
+        n = _np(n_new, np.int32, (S,), "n_new")
+        y = np.empty((S, self.out_pitch), np.float32)
+        n_out = np.zeros(S, np.int32)
+        self.eng._ck(self.eng.lib.vtts_resample_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(flags), _ptr(y), _ptr(n_out)))
+        return [y[s, : int(n_out[s])].copy() for s in range(S)]
+
+    def push_device(self, x_t, n_new, flags, out_t, stream=None) -> np.ndarray:
+        """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S, out_pitch]; n_new int [S] and flags
+        uint8 [S] (bit0 BEGIN, bit1 END) on the host.  Stream-ordered; returns n_out int32 [S] (outputs slot s got at the
+        start of its row of out_t)."""
+        import torch
+        S, F = self.max_streams, self.max_chunk_samples
+        if tuple(x_t.shape) != (S, F) or x_t.dtype != torch.float32 or not x_t.is_contiguous():
+            raise ValueError(f"x_t must be contiguous float32 [{S}, {F}]")
+        if tuple(out_t.shape) != (S, self.out_pitch) or out_t.dtype != torch.float32 or not out_t.is_contiguous():
+            raise ValueError(f"out_t must be contiguous float32 [{S}, {self.out_pitch}]")
+        n = _np(n_new, np.int32, (S,), "n_new")
+        f = _np(flags, np.uint8, (S,), "flags")
+        n_out = np.zeros(S, np.int32)
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self.eng._ck(self.eng.lib.vtts_resample_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(out_t), _ptr(n_out), st))
+        return n_out
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.eng, "h", None):
+            self.eng._ck(self.eng.lib.vtts_resample_stream_destroy(self.eng.h, self.h))
         self.h = None
 
     def __enter__(self):
@@ -814,22 +943,32 @@ class AcousticStream:
 
 class TtsStream:
     """Handle of a text-to-speech stream (Engine.open_tts_stream): an acoustic stream of max_chunk_frames F feeding a
-    vocoder stream of F + the acoustic lookahead frames per push."""
+    vocoder stream of F + the acoustic lookahead frames per push, and with an output rate a resample stream after it."""
 
-    def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None):
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
+                 output_rate=None):
         import torch
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
+        if output_rate is not None:
+            resample_ratio(config.SAMPLE_RATE, output_rate)
         self.eng = eng
+        self.rs = None
         self.ac = AcousticStream(eng, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng)
         try:
             self.voc = VocoderStream(eng, max_streams, self.ac.out_frames)
+            if output_rate is not None:
+                # the vocoder's output buffer is the resampler's input: n_new = 256 * frames it emitted
+                self.rs = ResampleStream(eng, max_streams, self.voc.wav_ld, output_rate)
         except Exception:
+            if getattr(self, "voc", None) is not None:
+                self.voc.close()
             self.ac.close()
             raise
         dev = torch.device("cuda", eng.device)
         self._mel = torch.zeros((max_streams, self.ac.out_frames, config.MEL_DIM), dtype=torch.float32, device=dev)
         self._wav = torch.zeros((max_streams, self.voc.wav_ld), dtype=torch.float32, device=dev)
+        self._out = None if self.rs is None else torch.zeros((max_streams, self.rs.out_pitch), dtype=torch.float32, device=dev)
         self._fresh = np.zeros(max_streams, bool)   # begun, no push yet: the next vocoder push carries BEGIN
         self._empty = set()                         # begun with nothing left after the trim: reported empty at the next step
 
@@ -874,13 +1013,20 @@ class TtsStream:
         self._empty = set()
         if active.any():
             n_wav = self.voc.push_device(self._mel, n_out, flags, self._wav)
-            wav = self._wav.cpu().numpy()
+            n_wav = n_wav * config.HOP
+            src = self._wav
+            if self.rs is not None:
+                n_wav = self.rs.push_device(self._wav, n_wav, flags, self._out)
+                src = self._out
+            wav = src.cpu().numpy()
             for s in np.flatnonzero(active):
-                out[int(s)] = wav[s, : int(n_wav[s]) * config.HOP].copy()
+                out[int(s)] = wav[s, : int(n_wav[s])].copy()
         self._fresh &= ~active
         return out
 
     def close(self):
+        if getattr(self, "rs", None) is not None:
+            self.rs.close()
         if getattr(self, "voc", None) is not None:
             self.voc.close()
         if getattr(self, "ac", None) is not None:

@@ -5,6 +5,8 @@ pipeline (synthesizer.py:34-39): normalise -> text2mel -> mel2wave -> 16-bit PCM
 GPU path makes worthwhile: `--text-file` synthesises one utterance per input line as ragged batches through a
 single library call per batch (`Engine.tts`), and the WAV writer is built in (the reference needs `soundfile`).
 `--precision fp16` runs the generator in the fast fp16 mode (Engine.set_precision) for either input.
+`--output-rate R` resamples the audio on the device (Engine.resample) and writes R in the header; `--sample-rate` keeps
+the reference's meaning, the header rate of the unchanged 16 kHz samples.
 """
 from __future__ import annotations
 
@@ -101,7 +103,12 @@ def main(argv=None) -> int:
     parser.add_argument("--text", type=str)
     parser.add_argument("--text-file", type=Path, default=None, help="one utterance per line; outputs <output stem>_NNNN.wav")
     parser.add_argument("--output", default="clip.wav", type=Path)
-    parser.add_argument("--sample-rate", default=16000, type=int)
+    parser.add_argument("--sample-rate", default=None, type=int,
+                        help="rate written in the WAV header (default 16000); as in the reference it does not change the "
+                             "samples, which stay at the model's 16 kHz -- use --output-rate to resample")
+    parser.add_argument("--output-rate", default=None, type=int,
+                        help="resample the audio on the device to this rate (scipy.signal.resample_poly with its defaults) "
+                             "and write it in the header")
     parser.add_argument("--silence-duration", default=-1, type=float)
     parser.add_argument("--lexicon-file", default=None)
     parser.add_argument("--seed", default=None, type=int,
@@ -120,10 +127,28 @@ def main(argv=None) -> int:
         parser.error("--reference-dropout applies to --text-file (--text always uses the reference's stream)")
     if args.reference_dropout and args.seed is not None:
         parser.error("--reference-dropout and --seed select different dropout streams; give one")
+    if args.output_rate is not None:
+        if args.sample_rate is not None and args.sample_rate != args.output_rate:
+            parser.error("--sample-rate only labels the 16 kHz samples and --output-rate resamples them; they disagree")
+        from .engine import resample_ratio
+        try:
+            up, down = resample_ratio(config.SAMPLE_RATE, args.output_rate)
+        except ValueError as e:
+            parser.error(f"--output-rate: {e}")
+        if max(up, down) > 1024:
+            parser.error(f"--output-rate {args.output_rate}: {config.SAMPLE_RATE} -> {args.output_rate} reduces to {up}/{down} "
+                         "(at most 1024 each)")
+    header_rate = args.output_rate or args.sample_rate or config.SAMPLE_RATE
     lexicon = args.lexicon_file if args.lexicon_file is not None else config.LEXICON_FILE
     if args.precision is not None:
         from .engine import get_engine
         get_engine().set_precision(args.precision)      # the engine both the --text and the --text-file paths use
+
+    def to_output_rate(waves):
+        if args.output_rate is None:
+            return waves
+        from .engine import get_engine
+        return [get_engine().resample(w, args.output_rate) for w in waves]
 
     if args.text_file is not None:
         lines = [ln for ln in args.text_file.read_text().splitlines() if ln.strip()]
@@ -131,11 +156,11 @@ def main(argv=None) -> int:
         if args.reference_dropout:
             from .nat.text2mel import checkpoint_rng
             rng = checkpoint_rng()
-        waves = synthesize_lines(lines, lexicon, args.silence_duration, seed=args.seed, rng=rng)
+        waves = to_output_rate(synthesize_lines(lines, lexicon, args.silence_duration, seed=args.seed, rng=rng))
         for i, w in enumerate(waves):
             fn = args.output.with_name(f"{args.output.stem}_{i:04d}{args.output.suffix or '.wav'}")
             print("writing output to file", fn)
-            write_wav(fn, w, args.sample_rate)
+            write_wav(fn, w, header_rate)
         return 0
 
     if args.text is None:
@@ -145,9 +170,9 @@ def main(argv=None) -> int:
     text = nat_normalize_text(args.text)
     print("Normalized text input:", text)
     mel = text2mel(text, lexicon, args.silence_duration, seed=args.seed)
-    wave = mel2wave(mel)
+    wave = to_output_rate([np.ravel(mel2wave(mel))])[0]
     print("writing output to file", args.output)
-    write_wav(args.output, wave, args.sample_rate)
+    write_wav(args.output, wave, header_rate)
     return 0
 
 

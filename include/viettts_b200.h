@@ -287,6 +287,47 @@ int vtts_resample_stream_push(vtts_ctx* ctx, vtts_resample_stream* rs, const flo
 int vtts_resample_stream_push_host(vtts_ctx* ctx, vtts_resample_stream* rs, const float* x, const int32_t* n_new,
                                    const uint8_t* flags, float* y, int32_t* n_out);
 
+/* ---- bias denoiser: STFT spectral subtraction of the vocoder's hiss -------------------------------------------------
+ * One row x of n samples, strength s >= 0, bias beta[0..512] >= 0 (the WaveGlow / HiFiGAN `Denoiser` convention):
+ *   STFT n_fft 1024, hop 256, periodic Hann w, centered frames with reflect padding 512 (torch.stft(center=True,
+ *   pad_mode="reflect"), F = n / 256 + 1 frames);  |X| = sqrt(re^2 + im^2);  M' = max(|X| - s beta[k], 0);
+ *   Y = X M' / |X| where |X| > 0, else 0;  y = torch.istft(Y, 1024, 256, window=w, center=True, length=n).
+ * Rows of n <= 512 samples cannot be reflect-padded and are returned unchanged, bit for bit.  fp32 in every
+ * vtts_precision mode; s beta[k] is rounded to fp32 once.  Each frame is transformed on its own, so the bits of an
+ * output depend only on the input samples of the frames covering it: the same row gives the same bits alone, in any
+ * batch, and through the stream.  The usual bias is vtts_denoise_bias of the generator's output for an all-zero mel
+ * [1, 88, 80]. */
+/* x_dev [B,S]; n_dev int32 [B] or NULL (= S; values are clamped to [0, S]); bias_dev [513]; y_dev [B,S], not x_dev;
+ * outputs past n[b] are 0.  strength finite and >= 0, else VTTS_ERR_BAD_ARG.  Stream-ordered; uses the context's
+ * workspace (B * (S / 256 + 1) * 4 KiB). */
+int vtts_denoise(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, float strength, const float* bias_dev,
+                 float* y_dev, void* stream);
+/* the same on host buffers; n_in[b] must lie in [0, S] and the bias values be finite and >= 0 */
+int vtts_denoise_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, float strength, const float* bias, float* y);
+/* bias_dev[k] = |X_0[k]|, k = 0..512: the magnitude spectrum of frame 0 of the n-sample waveform wav_dev (n > 512),
+ * through the denoiser's own frame code.  Stream-ordered. */
+int vtts_denoise_bias(vtts_ctx* ctx, const float* wav_dev, int n, float* bias_dev, void* stream);
+/* Streaming denoiser with max_streams independent slots, strength and bias (host [513], finite and >= 0) fixed at
+ * create: each slot carries the last 2048 input samples and a 64-bit position, so the outputs a slot emits,
+ * concatenated, are bit-identical to vtts_denoise of its whole input (rows of <= 512 samples included).  An output t
+ * is emitted with the first push after which the frames covering it are final: before END a slot that has received P
+ * samples has emitted min(P, 256 * max(0, floor(P / 256) - 3)) outputs; END emits the rest (also with no new samples).
+ * vtts_denoise_stream_lookahead() = 1023: how many input samples an output reads past its own time.  flags and slot
+ * rules as for the resample stream.  Every push issues the same three launches (window step, frames, overlap-add). */
+typedef struct vtts_denoise_stream vtts_denoise_stream;
+/* *out_pitch receives the outputs per slot of a push's output buffer (max_chunk_samples + 1023) */
+int vtts_denoise_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, float strength, const float* bias,
+                               vtts_denoise_stream** out, int* out_pitch);
+int vtts_denoise_stream_destroy(vtts_ctx* ctx, vtts_denoise_stream* ds);
+int vtts_denoise_stream_lookahead(void);
+/* x_dev [S][max_chunk_samples] (samples past n_new[s] ignored); n_new, flags, n_out HOST int32 / uint8 / int32 [S];
+ * y_dev [S][out_pitch], slot s gets n_out[s] outputs from its start.  Stream-ordered. */
+int vtts_denoise_stream_push(vtts_ctx* ctx, vtts_denoise_stream* ds, const float* x_dev, const int32_t* n_new,
+                             const uint8_t* flags, float* y_dev, int32_t* n_out, void* stream);
+/* the same on host buffers x [S][max_chunk_samples] and y [S][out_pitch]; returns when y is written */
+int vtts_denoise_stream_push_host(vtts_ctx* ctx, vtts_denoise_stream* ds, const float* x, const int32_t* n_new,
+                                  const uint8_t* flags, float* y, int32_t* n_out);
+
 /* ---- streaming acoustic model: every slot advances its decoder a few frames per push ---------------------------
  * A vtts_acoustic_stream holds max_streams (1..128) independent slots.  begin starts utterances in closed slots; each
  * push advances every open slot by min(F, frames left) decoder steps in ONE scan launch and returns the mel frames whose

@@ -76,6 +76,14 @@ SIGNATURES = {
     "vtts_resample_stream_lookahead": (C.c_int, [C.c_int, C.c_int]),
     "vtts_resample_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtts_resample_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_denoise": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_denoise_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
+    "vtts_denoise_bias": (C.c_int, [c_ctx, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "vtts_denoise_stream_create": (C.c_int, [c_ctx, C.c_int, C.c_int, C.c_float, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int)]),
+    "vtts_denoise_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
+    "vtts_denoise_stream_lookahead": (C.c_int, []),
+    "vtts_denoise_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_denoise_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtts_acoustic_stream_create":(C.c_int, [c_ctx, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, C.POINTER(C.c_void_p)]),
     "vtts_acoustic_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
     "vtts_acoustic_stream_lookahead": (C.c_int, []),

@@ -10,38 +10,19 @@
 // every sample is read from HBM once.
 #include <math.h>
 
+#include "fft_common.cuh"
 #include "vtts_internal.cuh"
 
 namespace {
+
+using fftc::bitrev5;
+using fftc::cmul;
+using fftc::fft32;
 
 constexpr int NF = vc::NFFT;      // 1024
 constexpr int NB = vc::NBINS;     // 513
 constexpr int MEL_WARPS = 8;      // frame pairs per CTA
 constexpr int TP = 33;            // transpose pitch (float2)
-
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-
-// exp(-2 pi i k / 32), k = 0..15; k is a compile-time constant at every call site (fully unrolled loops)
-__device__ __forceinline__ float2 w32(int k) {
-  switch (k) {
-    case 0: return make_float2(1.f, 0.f);
-    case 1: return make_float2(0.98078528040323043f, -0.19509032201612825f);
-    case 2: return make_float2(0.92387953251128674f, -0.38268343236508978f);
-    case 3: return make_float2(0.83146961230254524f, -0.55557023301960218f);
-    case 4: return make_float2(0.70710678118654757f, -0.70710678118654757f);
-    case 5: return make_float2(0.55557023301960229f, -0.83146961230254524f);
-    case 6: return make_float2(0.38268343236508984f, -0.92387953251128674f);
-    case 7: return make_float2(0.19509032201612833f, -0.98078528040323043f);
-    case 8: return make_float2(0.f, -1.f);
-    case 9: return make_float2(-0.19509032201612819f, -0.98078528040323043f);
-    case 10: return make_float2(-0.38268343236508973f, -0.92387953251128674f);
-    case 11: return make_float2(-0.55557023301960196f, -0.83146961230254546f);
-    case 12: return make_float2(-0.70710678118654746f, -0.70710678118654757f);
-    case 13: return make_float2(-0.83146961230254535f, -0.55557023301960218f);
-    case 14: return make_float2(-0.92387953251128674f, -0.38268343236508989f);
-    default: return make_float2(-0.98078528040323043f, -0.19509032201612861f);
-  }
-}
 
 // sqrt.approx.f32: one MUFU op, max relative error 2^-23 (the IEEE sqrtf expands to ~10 instructions; 34 of them per
 // lane were a quarter of the kernel)
@@ -49,31 +30,6 @@ __device__ __forceinline__ float fast_sqrt(float x) {
   float r;
   asm("sqrt.approx.f32 %0, %1;" : "=f"(r) : "f"(x));
   return r;
-}
-
-__host__ __device__ constexpr int bitrev5(int x) {
-  return ((x & 1) << 4) | ((x & 2) << 2) | (x & 4) | ((x & 8) >> 2) | ((x & 16) >> 4);
-}
-
-// in-place 32-point DFT in registers: radix-2 decimation in frequency, natural-order input,
-// v[p] = X[bitrev5(p)] on return.  Every index and twiddle is a compile-time constant after unrolling.
-__device__ __forceinline__ void fft32(float2 (&v)[32]) {
-#pragma unroll
-  for (int half = 16; half >= 1; half >>= 1) {
-#pragma unroll
-    for (int g = 0; g < 32; g += 2 * half) {
-#pragma unroll
-      for (int j = 0; j < half; ++j) {
-        const float2 a = v[g + j], b = v[g + j + half];
-        v[g + j] = make_float2(a.x + b.x, a.y + b.y);
-        const float2 d = make_float2(a.x - b.x, a.y - b.y);
-        const int tk = j * (16 / half);            // W_{2 half}^j = W_32^{tk}
-        if (tk == 0) v[g + j + half] = d;
-        else if (tk == 8) v[g + j + half] = make_float2(d.y, -d.x);
-        else v[g + j + half] = cmul(d, w32(tk));
-      }
-    }
-  }
 }
 
 __global__ void __launch_bounds__(MEL_WARPS * 32) melspec_kernel(const float* __restrict__ wav, int S, int F,
@@ -197,7 +153,8 @@ __global__ void mel_span_kernel(const float* __restrict__ fb, int* lo, int* hi) 
 
 }  // namespace
 
-int vtts_melspec_prepare(vtts_ctx* ctx) {
+int vtts_fft_tables(vtts_ctx* ctx) {
+  if (ctx->fft_ready) return VTTS_OK;
   // twiddles exp(-2 pi i k / 1024) and the periodic Hann window, computed in double on the host
   std::vector<float> tw(2 * NF), hn(NF);
   for (int k = 0; k < NF; ++k) {
@@ -208,10 +165,17 @@ int vtts_melspec_prepare(vtts_ctx* ctx) {
   }
   if (!ctx->fft_tw) VTTS_CUDA(cudaMalloc(&ctx->fft_tw, tw.size() * sizeof(float)));
   if (!ctx->hann) VTTS_CUDA(cudaMalloc(&ctx->hann, hn.size() * sizeof(float)));
-  if (!ctx->mel_lo) VTTS_CUDA(cudaMalloc(&ctx->mel_lo, vc::MEL * sizeof(int)));
-  if (!ctx->mel_hi) VTTS_CUDA(cudaMalloc(&ctx->mel_hi, vc::MEL * sizeof(int)));
   VTTS_CUDA(cudaMemcpy(ctx->fft_tw, tw.data(), tw.size() * sizeof(float), cudaMemcpyHostToDevice));
   VTTS_CUDA(cudaMemcpy(ctx->hann, hn.data(), hn.size() * sizeof(float), cudaMemcpyHostToDevice));
+  ctx->fft_ready = true;
+  return VTTS_OK;
+}
+
+int vtts_melspec_prepare(vtts_ctx* ctx) {
+  int rc = vtts_fft_tables(ctx);
+  if (rc) return rc;
+  if (!ctx->mel_lo) VTTS_CUDA(cudaMalloc(&ctx->mel_lo, vc::MEL * sizeof(int)));
+  if (!ctx->mel_hi) VTTS_CUDA(cudaMalloc(&ctx->mel_hi, vc::MEL * sizeof(int)));
   mel_span_kernel<<<1, 128>>>(ctx->mel_fb, ctx->mel_lo, ctx->mel_hi);
   VTTS_CUDA(cudaGetLastError());
   VTTS_CUDA(cudaDeviceSynchronize());

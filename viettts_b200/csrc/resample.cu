@@ -229,6 +229,13 @@ long long ceil_div(long long a, long long b) { return (a + b - 1) / b; }
 
 }  // namespace
 
+int vtts_stream_window_prep(vtts_ctx* ctx, float* win, int cap, int K, const int* tbl, const float* x, int F, int S, cudaStream_t st) {
+  resample_prep_kernel<<<S, RS_THREADS, 0, st>>>(win, cap, K, tbl, x, F);
+  ctx->launches++;
+  VTTS_CUDA(cudaGetLastError());
+  return VTTS_OK;
+}
+
 void vtts_resample_free(vtts_ctx* ctx) {
   for (auto& f : ctx->rs_filters) cudaFree(f.taps);
   ctx->rs_filters.clear();
@@ -417,10 +424,9 @@ int vtts_resample_stream_push(vtts_ctx* ctx, vtts_resample_stream* rs, const flo
   // pageable source: the call returns once the table is staged, so rs->tbl may be rewritten by the next push
   VTTS_CUDA(cudaMemcpyAsync(rs->d_rows, rows, (size_t)S * sizeof(RsRow), cudaMemcpyHostToDevice, st));
   VTTS_CUDA(cudaMemcpyAsync(rs->d_prep, prep, (size_t)S * 2 * sizeof(int), cudaMemcpyHostToDevice, st));
-  resample_prep_kernel<<<S, RS_THREADS, 0, st>>>(rs->win, rs->cap, rs->K, rs->d_prep, x_dev, F);
-  ctx->launches++;
-  VTTS_CUDA(cudaGetLastError());
-  int rc = rs_launch(ctx, r, rs->taps, rs->win, rs->cap, rs->cap, nullptr, rs->d_rows, S, 0, max_out, y_dev, rs->out_pitch, st);
+  int rc = vtts_stream_window_prep(ctx, rs->win, rs->cap, rs->K, rs->d_prep, x_dev, F, S, st);
+  if (rc) return rc;
+  rc = rs_launch(ctx, r, rs->taps, rs->win, rs->cap, rs->cap, nullptr, rs->d_rows, S, 0, max_out, y_dev, rs->out_pitch, st);
   if (rc) return rc;
 
   // ---- commit the slot state ----

@@ -190,6 +190,7 @@ struct vtts_ctx {
   int* mel_hi = nullptr;        // [80] one past last non-zero bin
   float* fft_tw = nullptr;      // [1024][2] cos/sin(-2 pi k/1024)
   float* hann = nullptr;        // [1024]
+  bool fft_ready = false;       // fft_tw and hann uploaded (vtts_fft_tables)
   bool mel_loaded = false;
 
   // ---- workspace (device), grown on demand ----
@@ -336,7 +337,13 @@ int vtts_duration_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengt
                       cudaStream_t st);
 // resample.cu: frees the context's cached resampling filters
 void vtts_resample_free(vtts_ctx* ctx);
+// resample.cu: the stream window step shared by the resample and denoise streams.  Per slot s of a window buffer
+// win [S][cap]: tbl[2s] = inputs of the previous push (the window tail [tbl[2s], tbl[2s] + K) moves to [0, K)),
+// tbl[2s + 1] = new inputs copied from x [S][F] to [K, K + tbl[2s + 1]).  One launch.
+int vtts_stream_window_prep(vtts_ctx* ctx, float* win, int cap, int K, const int* tbl, const float* x, int F, int S, cudaStream_t st);
 // melspec.cu
+// twiddles exp(-2 pi i k / 1024) and the periodic Hann window into ctx->fft_tw / ctx->hann (once per context)
+int vtts_fft_tables(vtts_ctx* ctx);
 int vtts_melspec_prepare(vtts_ctx* ctx);
 int vtts_melspec_run(vtts_ctx* ctx, const float* wav, int B, int S, float* mel, cudaStream_t st);
 

@@ -51,6 +51,17 @@ def resample_length(n: int, in_rate: int, out_rate: int) -> int:
     return -(-int(n) * up // down)
 
 
+DENOISE_BINS = config.N_FFT // 2 + 1   # 513
+DENOISE_BIAS_FRAMES = 88                # the all-zero mel [1, 88, 80] the default denoiser bias is taken from
+
+
+def _strength(s) -> float:
+    s = float(s)
+    if not (np.isfinite(s) and s >= 0):
+        raise ValueError(f"denoise strength must be finite and >= 0, got {s}")
+    return s
+
+
 def _ptr(a):
     if a is None:
         return None
@@ -82,6 +93,7 @@ class Engine:
         self._acoustic_key = None
         self._duration_key = None
         self._mel_loaded = False
+        self._denoise_bias = None   # default denoiser bias of the loaded generator in the current mode (denoiser_bias)
 
     def close(self):
         if getattr(self, "h", None):
@@ -117,6 +129,7 @@ class Engine:
         synthetic weights; every other model runs as in 'bf16x3')."""
         m = PRECISIONS.get(mode, mode)
         self._ck(self.lib.vtts_set_precision(self.h, int(m)))
+        self._denoise_bias = None
 
     def debug_conv1d(self, precision, x_t, w_t, bias_t, k, dil, pre_slope=1.0, resid_t=None, len_t=None):
         """Test hook: one conv layer on torch CUDA tensors through either arithmetic path."""
@@ -187,6 +200,7 @@ class Engine:
         if kind is not None:
             flags |= 0x800 | (self.PAIR_KERNELS[kind] << 12)
         self._ck(self.lib.vtts_debug_tc_stats(self.h, flags, None))
+        self._denoise_bias = None   # the generator's output (and so the default bias) may change in its last bits
 
     def tc_stats(self, enable=True):
         """Per-CTA stall counters of the last tensor-core conv launch (see vtts_debug_tc_stats)."""
@@ -219,6 +233,7 @@ class Engine:
         tensor holding the blob (e.g. received through an NCCL broadcast)."""
         self._load(self.lib.vtts_load_hifigan, weights.pack_hifigan, params)
         self._hifigan_key = key if key is not None else object()
+        self._denoise_bias = None
 
     def load_acoustic(self, ckpt, key=None):
         self._load(self.lib.vtts_load_acoustic, weights.pack_acoustic, ckpt)
@@ -233,6 +248,7 @@ class Engine:
         """vtts_broadcast_weights: the root's loaded models reach every rank's context by one grouped ncclBroadcast.
         `nccl_comm`: an ncclComm_t as ctypes.c_void_p / int (e.g. parallel.NcclComm(...).handle)."""
         self._ck(self.lib.vtts_broadcast_weights(self.h, nccl_comm, int(root), 1 if is_root else 0, stream))
+        self._denoise_bias = None
         if not is_root:
             self._hifigan_key = self._acoustic_key = self._duration_key = object()
 
@@ -298,13 +314,16 @@ class Engine:
         return AcousticStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, masks=masks)
 
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
-                        rng=None, output_rate=None) -> "TtsStream":
+                        rng=None, output_rate=None, denoise=None) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
         With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  `output_rate`: a resample
         stream follows the vocoder on the device and `step()` returns samples at that rate, equal to `resample` of the
-        `tts` audio bit for bit.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
-        return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate)
+        `tts` audio bit for bit.  `denoise`: a strength; a denoise stream with the default bias (`denoiser_bias()`) sits
+        between the vocoder and the resampler, and the audio equals `denoise` of the `tts` audio (then resampled) bit for
+        bit.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
+        return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate,
+                         denoise=denoise)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -687,6 +706,80 @@ class Engine:
         time); END emits the rest."""
         return ResampleStream(self, max_streams, max_chunk_samples, out_rate, in_rate)
 
+    # ---- bias denoiser (vtts_denoise*: STFT spectral subtraction of the vocoder's bias spectrum, fp32) ----
+    def denoiser_bias(self, mel=None) -> np.ndarray:
+        """The denoiser's bias beta [513]: |X_0|, the magnitude spectrum of frame 0 of the loaded generator's output in
+        the current precision mode, for `mel` ([T,80] or [1,T,80]) or by default an all-zero mel [1, 88, 80].  The
+        default is computed on first use and kept until the generator or the precision mode changes."""
+        import torch
+        default = mel is None
+        if default and self._denoise_bias is not None:
+            return self._denoise_bias.copy()
+        m = np.zeros((1, DENOISE_BIAS_FRAMES, config.MEL_DIM), np.float32) if default else _np(mel, np.float32)
+        if m.ndim == 2:
+            m = m[None]
+        if m.ndim != 3 or m.shape[0] != 1 or m.shape[2] != config.MEL_DIM:
+            raise ValueError(f"mel must be [T,{config.MEL_DIM}] or [1,T,{config.MEL_DIM}], got {np.shape(mel)}")
+        wav = torch.from_numpy(self.mel2wave(m)[0]).to(torch.device("cuda", self.device))
+        out = torch.empty(DENOISE_BINS, dtype=torch.float32, device=wav.device)
+        st = torch.cuda.current_stream(wav.device).cuda_stream
+        self._ck(self.lib.vtts_denoise_bias(self.h, _ptr(wav), int(wav.numel()), _ptr(out), st))
+        beta = out.cpu().numpy()
+        if default:
+            self._denoise_bias = beta.copy()
+        return beta
+
+    def _bias_arg(self, bias) -> np.ndarray:
+        b = self.denoiser_bias() if bias is None else _np(bias, np.float32, (DENOISE_BINS,), "bias")
+        if not (np.all(np.isfinite(b)) and np.all(b >= 0)):
+            raise ValueError("bias values must be finite and >= 0")
+        return b
+
+    def denoise(self, wav, strength: float, lengths=None, bias=None) -> np.ndarray:
+        """Host arrays: wav f32 [S] or [B,S] -> the same shape with strength * bias subtracted from every STFT magnitude
+        (n_fft 1024, hop 256, Hann, reflect-padded centered frames), phase kept; rows of <= 512 samples are copied.
+        lengths int [B] in [0, S]: row b holds lengths[b] samples and its outputs past them are 0.  bias f32 [513]
+        (default: `denoiser_bias()`)."""
+        strength = _strength(strength)
+        x = _np(wav, np.float32)
+        one = x.ndim == 1
+        x = x[None] if one else x
+        if x.ndim != 2:
+            raise ValueError(f"wav must be [S] or [B,S], got {np.shape(wav)}")
+        B, S = x.shape
+        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
+        if S == 0 or B == 0:
+            return (x[0] if one else x).copy()          # nothing to transform: empty rows are short rows
+        b = self._bias_arg(bias)
+        y = np.empty((B, S), np.float32)
+        self._ck(self.lib.vtts_denoise_host(self.h, _ptr(x), _ptr(lens), B, S, strength, _ptr(b), _ptr(y)))
+        return y[0] if one else y
+
+    def denoise_forward(self, x_t, strength: float, lengths_t=None, bias_t=None, out=None, stream=None):
+        """vtts_denoise on torch CUDA tensors, stream-ordered: x_t f32 [B,S] -> [B,S]; lengths_t int32 CUDA [B] or None;
+        bias_t f32 CUDA [513] or None (`denoiser_bias()`)."""
+        import torch
+        strength = _strength(strength)
+        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
+        B, S = x_t.shape
+        if bias_t is None:
+            bias_t = torch.from_numpy(self._bias_arg(None)).to(x_t.device)
+        elif tuple(bias_t.shape) != (DENOISE_BINS,) or bias_t.dtype != torch.float32 or not bias_t.is_contiguous():
+            raise ValueError(f"bias_t must be contiguous float32 [{DENOISE_BINS}]")
+        if out is None:
+            out = torch.empty((B, S), dtype=torch.float32, device=x_t.device)
+        elif tuple(out.shape) != (B, S) or out.dtype != torch.float32 or not out.is_contiguous():
+            raise ValueError(f"out must be contiguous float32 [{B}, {S}]")
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self._ck(self.lib.vtts_denoise(self.h, _ptr(x_t), _ptr(lengths_t), B, S, strength, _ptr(bias_t), _ptr(out), st))
+        return out
+
+    def open_denoise_stream(self, max_streams: int, max_chunk_samples: int, strength: float, bias=None) -> "DenoiseStream":
+        """Streaming denoiser with `max_streams` independent slots (vtts_denoise_stream_*), strength and bias fixed:
+        each slot's outputs, concatenated, equal `denoise` of its whole input bit for bit.  An output is emitted once the
+        frames covering it are final (at most 1023 samples after its own time); END emits the rest."""
+        return DenoiseStream(self, max_streams, max_chunk_samples, strength, bias)
+
 
 STREAM_BEGIN, STREAM_END = 1, 2
 
@@ -836,6 +929,77 @@ class ResampleStream:
             pass
 
 
+class DenoiseStream:
+    """Handle of a streaming denoiser (Engine.open_denoise_stream).  Before END a slot that has received P samples has
+    emitted min(P, 256 max(0, floor(P / 256) - 3)) outputs; a push with END emits the rest."""
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, strength: float, bias=None):
+        self.eng = eng
+        self.max_streams, self.max_chunk_samples = int(max_streams), int(max_chunk_samples)
+        self.strength = _strength(strength)
+        self.bias = eng._bias_arg(bias)
+        h, pitch = C.c_void_p(), C.c_int()
+        eng._ck(eng.lib.vtts_denoise_stream_create(eng.h, self.max_streams, self.max_chunk_samples, self.strength, _ptr(self.bias),
+                                                   C.byref(h), C.byref(pitch)))
+        self.h = h
+        self.out_pitch = int(pitch.value)   # outputs per slot of a push's output buffer
+        self.lookahead = int(eng.lib.vtts_denoise_stream_lookahead())
+
+    def push(self, x, n_new, begin=None, end=None) -> list:
+        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None.
+        Returns one float32 array per slot with the samples it emits now."""
+        S, F = self.max_streams, self.max_chunk_samples
+        x = _np(x, np.float32)
+        if x.ndim != 2 or x.shape[0] != S or x.shape[1] > F:
+            raise ValueError(f"x must be [{S}, <= {F}], got {x.shape}")
+        if x.shape[1] < F:
+            x = np.concatenate([x, np.zeros((S, F - x.shape[1]), np.float32)], axis=1)
+        flags = np.zeros(S, np.uint8)
+        if begin is not None:
+            flags |= np.asarray(begin, bool).astype(np.uint8) * STREAM_BEGIN
+        if end is not None:
+            flags |= np.asarray(end, bool).astype(np.uint8) * STREAM_END
+        n = _np(n_new, np.int32, (S,), "n_new")
+        y = np.empty((S, self.out_pitch), np.float32)
+        n_out = np.zeros(S, np.int32)
+        self.eng._ck(self.eng.lib.vtts_denoise_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(flags), _ptr(y), _ptr(n_out)))
+        return [y[s, : int(n_out[s])].copy() for s in range(S)]
+
+    def push_device(self, x_t, n_new, flags, out_t, stream=None) -> np.ndarray:
+        """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S, out_pitch]; n_new int [S] and flags
+        uint8 [S] (bit0 BEGIN, bit1 END) on the host.  Stream-ordered; returns n_out int32 [S] (outputs slot s got at the
+        start of its row of out_t)."""
+        import torch
+        S, F = self.max_streams, self.max_chunk_samples
+        if tuple(x_t.shape) != (S, F) or x_t.dtype != torch.float32 or not x_t.is_contiguous():
+            raise ValueError(f"x_t must be contiguous float32 [{S}, {F}]")
+        if tuple(out_t.shape) != (S, self.out_pitch) or out_t.dtype != torch.float32 or not out_t.is_contiguous():
+            raise ValueError(f"out_t must be contiguous float32 [{S}, {self.out_pitch}]")
+        n = _np(n_new, np.int32, (S,), "n_new")
+        f = _np(flags, np.uint8, (S,), "flags")
+        n_out = np.zeros(S, np.int32)
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self.eng._ck(self.eng.lib.vtts_denoise_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(out_t), _ptr(n_out), st))
+        return n_out
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.eng, "h", None):
+            self.eng._ck(self.eng.lib.vtts_denoise_stream_destroy(self.eng.h, self.h))
+        self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 def acoustic_stream_schedule(n_frames: int, n_emit: int | None, chunk: int, lookahead: int = 10) -> list:
     """Frames an acoustic stream slot emits per push: it scans min(n_frames, n_emit + lookahead) frames, `chunk` per
     push; after P frames scanned it has emitted min(n_emit, max(0, P - lookahead)), and its last push emits the rest."""
@@ -943,24 +1107,35 @@ class AcousticStream:
 
 class TtsStream:
     """Handle of a text-to-speech stream (Engine.open_tts_stream): an acoustic stream of max_chunk_frames F feeding a
-    vocoder stream of F + the acoustic lookahead frames per push, and with an output rate a resample stream after it."""
+    vocoder stream of F + the acoustic lookahead frames per push, with a denoise strength a denoise stream after it, and
+    with an output rate a resample stream last."""
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
-                 output_rate=None):
+                 output_rate=None, denoise=None):
         import torch
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
         if output_rate is not None:
             resample_ratio(config.SAMPLE_RATE, output_rate)
+        if denoise is not None:
+            denoise = _strength(denoise)
         self.eng = eng
         self.rs = None
+        self.dn = None
         self.ac = AcousticStream(eng, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng)
         try:
             self.voc = VocoderStream(eng, max_streams, self.ac.out_frames)
+            pitch = self.voc.wav_ld
+            if denoise is not None:
+                # the vocoder's output buffer is the denoiser's input: n_new = 256 * frames it emitted
+                self.dn = DenoiseStream(eng, max_streams, pitch, denoise)
+                pitch = self.dn.out_pitch
             if output_rate is not None:
-                # the vocoder's output buffer is the resampler's input: n_new = 256 * frames it emitted
-                self.rs = ResampleStream(eng, max_streams, self.voc.wav_ld, output_rate)
+                # the previous stage's output buffer is the resampler's input
+                self.rs = ResampleStream(eng, max_streams, pitch, output_rate)
         except Exception:
+            if getattr(self, "dn", None) is not None:
+                self.dn.close()
             if getattr(self, "voc", None) is not None:
                 self.voc.close()
             self.ac.close()
@@ -968,6 +1143,7 @@ class TtsStream:
         dev = torch.device("cuda", eng.device)
         self._mel = torch.zeros((max_streams, self.ac.out_frames, config.MEL_DIM), dtype=torch.float32, device=dev)
         self._wav = torch.zeros((max_streams, self.voc.wav_ld), dtype=torch.float32, device=dev)
+        self._den = None if self.dn is None else torch.zeros((max_streams, self.dn.out_pitch), dtype=torch.float32, device=dev)
         self._out = None if self.rs is None else torch.zeros((max_streams, self.rs.out_pitch), dtype=torch.float32, device=dev)
         self._fresh = np.zeros(max_streams, bool)   # begun, no push yet: the next vocoder push carries BEGIN
         self._empty = set()                         # begun with nothing left after the trim: reported empty at the next step
@@ -1015,8 +1191,11 @@ class TtsStream:
             n_wav = self.voc.push_device(self._mel, n_out, flags, self._wav)
             n_wav = n_wav * config.HOP
             src = self._wav
+            if self.dn is not None:
+                n_wav = self.dn.push_device(src, n_wav, flags, self._den)
+                src = self._den
             if self.rs is not None:
-                n_wav = self.rs.push_device(self._wav, n_wav, flags, self._out)
+                n_wav = self.rs.push_device(src, n_wav, flags, self._out)
                 src = self._out
             wav = src.cpu().numpy()
             for s in np.flatnonzero(active):
@@ -1027,6 +1206,8 @@ class TtsStream:
     def close(self):
         if getattr(self, "rs", None) is not None:
             self.rs.close()
+        if getattr(self, "dn", None) is not None:
+            self.dn.close()
         if getattr(self, "voc", None) is not None:
             self.voc.close()
         if getattr(self, "ac", None) is not None:

@@ -6,7 +6,8 @@ GPU path makes worthwhile: `--text-file` synthesises one utterance per input lin
 single library call per batch (`Engine.tts`), and the WAV writer is built in (the reference needs `soundfile`).
 `--precision fp16` runs the generator in the fast fp16 mode (Engine.set_precision) for either input.
 `--output-rate R` resamples the audio on the device (Engine.resample) and writes R in the header; `--sample-rate` keeps
-the reference's meaning, the header rate of the unchanged 16 kHz samples.
+the reference's meaning, the header rate of the unchanged 16 kHz samples.  `--denoise S` removes the generator's bias
+hiss on the device (Engine.denoise, strength S, the default bias) at 16 kHz, before any resampling.
 """
 from __future__ import annotations
 
@@ -109,6 +110,9 @@ def main(argv=None) -> int:
     parser.add_argument("--output-rate", default=None, type=int,
                         help="resample the audio on the device to this rate (scipy.signal.resample_poly with its defaults) "
                              "and write it in the header")
+    parser.add_argument("--denoise", default=None, type=float, metavar="STRENGTH",
+                        help="subtract STRENGTH times the generator's bias spectrum (its output for an all-zero mel) from the "
+                             "STFT magnitude of the 16 kHz audio on the device, before any --output-rate resampling; >= 0")
     parser.add_argument("--silence-duration", default=-1, type=float)
     parser.add_argument("--lexicon-file", default=None)
     parser.add_argument("--seed", default=None, type=int,
@@ -127,6 +131,8 @@ def main(argv=None) -> int:
         parser.error("--reference-dropout applies to --text-file (--text always uses the reference's stream)")
     if args.reference_dropout and args.seed is not None:
         parser.error("--reference-dropout and --seed select different dropout streams; give one")
+    if args.denoise is not None and not (np.isfinite(args.denoise) and args.denoise >= 0):
+        parser.error(f"--denoise {args.denoise}: the strength must be finite and >= 0")
     if args.output_rate is not None:
         if args.sample_rate is not None and args.sample_rate != args.output_rate:
             parser.error("--sample-rate only labels the 16 kHz samples and --output-rate resamples them; they disagree")
@@ -145,9 +151,11 @@ def main(argv=None) -> int:
         get_engine().set_precision(args.precision)      # the engine both the --text and the --text-file paths use
 
     def to_output_rate(waves):
+        from .engine import get_engine
+        if args.denoise is not None:
+            waves = [get_engine().denoise(w, args.denoise) for w in waves]
         if args.output_rate is None:
             return waves
-        from .engine import get_engine
         return [get_engine().resample(w, args.output_rate) for w in waves]
 
     if args.text_file is not None:

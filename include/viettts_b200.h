@@ -328,6 +328,53 @@ int vtts_denoise_stream_push(vtts_ctx* ctx, vtts_denoise_stream* ds, const float
 int vtts_denoise_stream_push_host(vtts_ctx* ctx, vtts_denoise_stream* ds, const float* x, const int32_t* n_new,
                                   const uint8_t* flags, float* y, int32_t* n_out);
 
+/* ---- loudness: ITU-R BS.1770-4 gated loudness and true peak, and normalization to a target ------------------------
+ * One mono row x of n samples at rate r, a multiple of 10 in [8000, 192000] (else VTTS_ERR_BAD_ARG):
+ *   K-weighting: the libebur128 shelf and high-pass biquads for r, from zero state;  m = r / 10;  E_k = sum of y^2 over
+ *   sub-block k (whole sub-blocks only, K = floor(n / m));  blocks j < J = max(0, K - 3):
+ *   z_j = (E_j + E_j+1 + E_j+2 + E_j+3) / 4m,  l_j = -0.691 + 10 log10 z_j;  integrated: the mean z over blocks with
+ *   l_j > -70 gives Gamma = its loudness - 10, and L = -0.691 + 10 log10(mean z over blocks with l_j > -70 and
+ *   l_j > Gamma), -inf with no such block;  momentary l_J-1;  short-term -0.691 + 10 log10(sum of the last 30 E_k / 30m)
+ *   (-inf for K < 30);  true peak 20 log10 max(max |x|, max |resample_poly(x, 4, 1)|) dBTP (-inf for silence).
+ * fp32 in every vtts_precision mode; each E_k is a fixed function of the filter state entering sub-block k and its
+ * samples, and every reduction has an order fixed by the sub-block or block index, so a row gives the same bits alone,
+ * in any batch, and through the stream. */
+/* coeffs[10] = b0 b1 b2 a1 a2 of the shelf, then of the high-pass, in double (a0 = 1).  Needs no device. */
+int vtts_loudness_filter(int rate, double* coeffs);
+/* x_dev [B,S]; n_dev int32 [B] or NULL (= S; values clamped to [0, S]); out_dev [B][4] = integrated, momentary and
+ * short-term LUFS, true peak dBTP.  Stream-ordered; uses the context's workspace (the 4x oversampled rows, 16 bytes per sample). */
+int vtts_loudness(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, float* out_dev, void* stream);
+/* the same on host buffers; n_in[b] must lie in [0, S] */
+int vtts_loudness_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float* out);
+/* y = x * fp32(10^(g / 20)) per row, g = target - L, with a ceiling min(g, ceiling - true peak); g = 0 (a bit copy) when
+ * L = -inf; outputs past n[b] are 0.  target in [-70, 0] LUFS; ceiling +inf (none) or in [-20, 0] dBTP.  g and the factor
+ * are computed on the device (no host synchronisation).  y_dev may equal x_dev; gain_db_dev [B] receives g, or NULL. */
+int vtts_loudness_normalize(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, float target,
+                            float ceiling, float* y_dev, float* gain_db_dev, void* stream);
+/* the same on host buffers; gain_db [B] or NULL */
+int vtts_loudness_normalize_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float target,
+                                 float ceiling, float* y, float* gain_db);
+/* Streaming meter with max_streams independent slots: each slot carries the filter state at its last complete
+ * sub-block boundary, the samples of the incomplete one, its E_k history (10 * max_seconds sub-blocks), the 4x
+ * oversampler's window and the running peak.  After every push a slot's integrated, momentary and short-term values equal
+ * vtts_loudness of the samples it has received since BEGIN, bit for bit; its true peak covers the samples and the
+ * oversampled outputs whose inputs have all arrived (vtts_loudness_stream_lookahead = 10 samples), and equals the
+ * one-shot value after END.  A push that would overflow a slot's history fails with VTTS_ERR_BAD_ARG before anything is
+ * launched.  flags and slot rules as for the resample stream; idle and ended slots keep their last readings.  Every push
+ * issues the same seven launches. */
+typedef struct vtts_loudness_stream vtts_loudness_stream;
+int vtts_loudness_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int rate, int max_seconds,
+                                vtts_loudness_stream** out);
+int vtts_loudness_stream_destroy(vtts_ctx* ctx, vtts_loudness_stream* ls);
+int vtts_loudness_stream_lookahead(int rate);
+/* x_dev [S][max_chunk_samples] (samples past n_new[s] ignored); n_new, flags HOST int32 / uint8 [S]; out_dev [S][4]
+ * receives every slot's readings.  Stream-ordered. */
+int vtts_loudness_stream_push(vtts_ctx* ctx, vtts_loudness_stream* ls, const float* x_dev, const int32_t* n_new,
+                              const uint8_t* flags, float* out_dev, void* stream);
+/* the same on host buffers x [S][max_chunk_samples] and out [S][4]; returns when out is written */
+int vtts_loudness_stream_push_host(vtts_ctx* ctx, vtts_loudness_stream* ls, const float* x, const int32_t* n_new,
+                                   const uint8_t* flags, float* out);
+
 /* ---- streaming acoustic model: every slot advances its decoder a few frames per push ---------------------------
  * A vtts_acoustic_stream holds max_streams (1..128) independent slots.  begin starts utterances in closed slots; each
  * push advances every open slot by min(F, frames left) decoder steps in ONE scan launch and returns the mel frames whose

@@ -84,6 +84,18 @@ SIGNATURES = {
     "vtts_denoise_stream_lookahead": (C.c_int, []),
     "vtts_denoise_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtts_denoise_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_loudness_filter": (C.c_int, [C.c_int, C.c_void_p]),
+    "vtts_loudness": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vtts_loudness_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "vtts_loudness_normalize": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p,
+                                          C.c_void_p, C.c_void_p]),
+    "vtts_loudness_normalize_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                               C.c_void_p, C.c_void_p]),
+    "vtts_loudness_stream_create": (C.c_int, [c_ctx, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
+    "vtts_loudness_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
+    "vtts_loudness_stream_lookahead": (C.c_int, [C.c_int]),
+    "vtts_loudness_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_loudness_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtts_acoustic_stream_create":(C.c_int, [c_ctx, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, C.POINTER(C.c_void_p)]),
     "vtts_acoustic_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
     "vtts_acoustic_stream_lookahead": (C.c_int, []),

@@ -83,14 +83,6 @@ std::vector<double> rs_design(const RsRatio& r) {
   return h;
 }
 
-struct RsRow {
-  long long x0;       // absolute input index of buffer element 0
-  long long lo, hi;   // inputs outside [lo, hi) read as zero
-  long long m0;       // absolute index of the row's first output
-  long long n_calc;   // outputs computed
-  long long n_out;    // outputs written (the ones past n_calc as zero)
-};
-
 // rows == nullptr: the one-shot bounds of row b, inputs [0, n_b) with n_b = n_in[b] (or S_in), S_out outputs of which
 // the first ceil(n_b * up / down) are computed
 __global__ void __launch_bounds__(RS_THREADS) resample_kernel(const float* __restrict__ x, long long x_ld, int S_in,
@@ -234,6 +226,16 @@ int vtts_stream_window_prep(vtts_ctx* ctx, float* win, int cap, int K, const int
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   return VTTS_OK;
+}
+
+int vtts_resample_run(vtts_ctx* ctx, int in_rate, int out_rate, const float* x, long long x_ld, int S_in, const int* n_in,
+                      const RsRow* rows, int B, long long S_out, long long max_out, float* y, long long y_ld, cudaStream_t st) {
+  RsRatio r;
+  if (rs_ratio(in_rate, out_rate, &r)) return ctx->fail(VTTS_ERR_BAD_ARG, "resample: rates %d -> %d", in_rate, out_rate);
+  const float* taps = nullptr;
+  int rc = rs_filter(ctx, r, &taps);
+  if (rc) return rc;
+  return rs_launch(ctx, r, taps, x, x_ld, S_in, n_in, rows, B, S_out, max_out, y, y_ld, st);
 }
 
 void vtts_resample_free(vtts_ctx* ctx) {

@@ -205,6 +205,10 @@ struct vtts_ctx {
   // fp32 polyphase filters of the resampler (resample.cu), one per reduced ratio up / down, designed at first use
   struct RsFilter { int up, down; float* taps; };
   std::vector<RsFilter> rs_filters;
+  // fp32 K-weighting cascade of the loudness meter (loudness.cu), one per sample rate, designed at first use: the ten
+  // biquad coefficients, the segment transitions A^(seg d) (d = 1, 2, 4, 8, 16) and the sub-block transition A^m
+  struct LnFilter { int rate; float coef[10]; float seg[5][16]; float blk[16]; };
+  std::vector<LnFilter> ln_filters;
 
   // taps of the last acoustic forward (point into ws)
   float* tap_enc = nullptr; int64_t tap_enc_n = 0;
@@ -341,6 +345,19 @@ void vtts_resample_free(vtts_ctx* ctx);
 // win [S][cap]: tbl[2s] = inputs of the previous push (the window tail [tbl[2s], tbl[2s] + K) moves to [0, K)),
 // tbl[2s + 1] = new inputs copied from x [S][F] to [K, K + tbl[2s + 1]).  One launch.
 int vtts_stream_window_prep(vtts_ctx* ctx, float* win, int cap, int K, const int* tbl, const float* x, int F, int S, cudaStream_t st);
+// resample.cu: per-row bounds of resample_kernel, which place a row's buffer in absolute time
+struct RsRow {
+  long long x0;       // absolute input index of buffer element 0
+  long long lo, hi;   // inputs outside [lo, hi) read as zero
+  long long m0;       // absolute index of the row's first output
+  long long n_calc;   // outputs computed
+  long long n_out;    // outputs written (the ones past n_calc as zero)
+};
+// resample.cu: one resample_kernel launch at out_rate / in_rate (the context's cached filter).  rows == nullptr: the
+// one-shot bounds (row b holds n_in[b] or S_in inputs, S_out outputs written); else per-row bounds, max_out the most
+// outputs of a row.
+int vtts_resample_run(vtts_ctx* ctx, int in_rate, int out_rate, const float* x, long long x_ld, int S_in, const int* n_in,
+                      const RsRow* rows, int B, long long S_out, long long max_out, float* y, long long y_ld, cudaStream_t st);
 // melspec.cu
 // twiddles exp(-2 pi i k / 1024) and the periodic Hann window into ctx->fft_tw / ctx->hann (once per context)
 int vtts_fft_tables(vtts_ctx* ctx);

@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import threading
+from typing import NamedTuple
 
 import numpy as np
 
@@ -314,16 +315,18 @@ class Engine:
         return AcousticStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, masks=masks)
 
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
-                        rng=None, output_rate=None, denoise=None) -> "TtsStream":
+                        rng=None, output_rate=None, denoise=None, meter=False) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
         With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  `output_rate`: a resample
         stream follows the vocoder on the device and `step()` returns samples at that rate, equal to `resample` of the
         `tts` audio bit for bit.  `denoise`: a strength; a denoise stream with the default bias (`denoiser_bias()`) sits
         between the vocoder and the resampler, and the audio equals `denoise` of the `tts` audio (then resampled) bit for
-        bit.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
+        bit.  `meter=True`: a loudness meter runs last, on what `step()` returns at the output rate (a multiple of 10),
+        and `TtsStream.meter()` gives each stepped slot's readings, read back in the step's one synchronisation.  Needs the
+        'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
         return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate,
-                         denoise=denoise)
+                         denoise=denoise, meter=meter)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -780,6 +783,115 @@ class Engine:
         frames covering it are final (at most 1023 samples after its own time); END emits the rest."""
         return DenoiseStream(self, max_streams, max_chunk_samples, strength, bias)
 
+    # ---- loudness (vtts_loudness*: ITU-R BS.1770-4 gated loudness and true peak, fp32) ----
+    def loudness(self, wav, rate: int = config.SAMPLE_RATE, lengths=None) -> "Loudness":
+        """Host arrays: wav f32 [S] or [B,S] at `rate` (a multiple of 10 in [8000, 192000]) -> Loudness of float32 [B]
+        arrays (scalars for a 1-D input): integrated, momentary and short-term loudness in LUFS (-inf where undefined) and
+        the true peak in dBTP (4x oversampled by resample_poly).  lengths int [B] in [0, S]."""
+        rate = _loudness_rate(rate)
+        x = _np(wav, np.float32)
+        one = x.ndim == 1
+        x = x[None] if one else x
+        if x.ndim != 2:
+            raise ValueError(f"wav must be [S] or [B,S], got {np.shape(wav)}")
+        B, S = x.shape
+        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
+        out = np.full((B, 4), -np.inf, np.float32)
+        if B and S:                                # empty rows measure as silence
+            self._ck(self.lib.vtts_loudness_host(self.h, _ptr(x), _ptr(lens), B, S, rate, _ptr(out)))
+        cols = [out[:, i] for i in range(4)]
+        return Loudness(*(c[0] for c in cols)) if one else Loudness(*cols)
+
+    def normalize_loudness(self, wav, target: float, rate: int = config.SAMPLE_RATE, true_peak=None, lengths=None):
+        """Host arrays: (y, gain_db).  y = wav * fp32(10^(g / 20)) per row with g = target - integrated loudness, at most
+        true_peak - the true peak when a ceiling (dBTP, in [-20, 0]) is given; rows measuring -inf are copied (g = 0) and
+        outputs past lengths[b] are 0.  target in [-70, 0] LUFS."""
+        rate = _loudness_rate(rate)
+        target, ceiling = _loudness_target(target, true_peak)
+        x = _np(wav, np.float32)
+        one = x.ndim == 1
+        x = x[None] if one else x
+        if x.ndim != 2:
+            raise ValueError(f"wav must be [S] or [B,S], got {np.shape(wav)}")
+        B, S = x.shape
+        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
+        y = x.copy()
+        g = np.zeros(B, np.float32)
+        if B and S:
+            self._ck(self.lib.vtts_loudness_normalize_host(self.h, _ptr(x), _ptr(lens), B, S, rate, target, ceiling, _ptr(y), _ptr(g)))
+        return (y[0], g[0]) if one else (y, g)
+
+    def loudness_forward(self, x_t, rate: int = config.SAMPLE_RATE, lengths_t=None, out=None, stream=None):
+        """vtts_loudness on torch CUDA tensors, stream-ordered: x_t f32 [B,S] -> f32 [B,4] (integrated, momentary,
+        short-term LUFS, true peak dBTP); lengths_t int32 CUDA [B] or None."""
+        import torch
+        rate = _loudness_rate(rate)
+        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
+        B, S = x_t.shape
+        if out is None:
+            out = torch.empty((B, 4), dtype=torch.float32, device=x_t.device)
+        elif tuple(out.shape) != (B, 4) or out.dtype != torch.float32 or not out.is_contiguous():
+            raise ValueError(f"out must be contiguous float32 [{B}, 4]")
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self._ck(self.lib.vtts_loudness(self.h, _ptr(x_t), _ptr(lengths_t), B, S, rate, _ptr(out), st))
+        return out
+
+    def normalize_loudness_forward(self, x_t, target: float, rate: int = config.SAMPLE_RATE, true_peak=None, lengths_t=None, out=None,
+                                   gain_db=None, stream=None):
+        """vtts_loudness_normalize on torch CUDA tensors, stream-ordered and without a host synchronisation: returns
+        (y [B,S], gain_db [B]).  `out` may be x_t (in place)."""
+        import torch
+        rate = _loudness_rate(rate)
+        target, ceiling = _loudness_target(target, true_peak)
+        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
+        B, S = x_t.shape
+        if out is None:
+            out = torch.empty((B, S), dtype=torch.float32, device=x_t.device)
+        elif tuple(out.shape) != (B, S) or out.dtype != torch.float32 or not out.is_contiguous():
+            raise ValueError(f"out must be contiguous float32 [{B}, {S}]")
+        if gain_db is None:
+            gain_db = torch.empty(B, dtype=torch.float32, device=x_t.device)
+        elif tuple(gain_db.shape) != (B,) or gain_db.dtype != torch.float32 or not gain_db.is_contiguous():
+            raise ValueError(f"gain_db must be contiguous float32 [{B}]")
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self._ck(self.lib.vtts_loudness_normalize(self.h, _ptr(x_t), _ptr(lengths_t), B, S, rate, target, ceiling, _ptr(out),
+                                                  _ptr(gain_db), st))
+        return out, gain_db
+
+    def open_loudness_meter(self, max_streams: int, max_chunk_samples: int, rate: int = config.SAMPLE_RATE,
+                            max_seconds: int = 600) -> "LoudnessMeter":
+        """Streaming loudness meter with `max_streams` independent slots (vtts_loudness_stream_*): after every push a
+        slot's integrated, momentary and short-term readings equal `loudness` of what it has received, bit for bit; its
+        true peak lags `lookahead` samples and equals the one-shot value after END.  A slot holds up to `max_seconds`."""
+        return LoudnessMeter(self, max_streams, max_chunk_samples, rate, max_seconds)
+
+
+class Loudness(NamedTuple):
+    integrated: np.ndarray     # LUFS (gated, BS.1770-4)
+    momentary: np.ndarray      # LUFS, the last 400 ms block
+    short_term: np.ndarray     # LUFS, the last 3 s
+    true_peak: np.ndarray      # dBTP
+
+
+def _loudness_rate(rate) -> int:
+    r = int(rate)
+    if r != rate or r % 10 or not 8000 <= r <= 192000:
+        raise ValueError(f"loudness: rate {rate} must be a multiple of 10 in [8000, 192000] (100 ms a whole number of samples)")
+    return r
+
+
+def _loudness_target(target, true_peak):
+    """(target, ceiling) as vtts_loudness_normalize takes them: ceiling +inf for none"""
+    t = float(target)
+    if not -70.0 <= t <= 0.0:
+        raise ValueError(f"loudness target {target} LUFS must lie in [-70, 0]")
+    if true_peak is None:
+        return t, float("inf")
+    c = float(true_peak)
+    if not (np.isfinite(c) and -20.0 <= c <= 0.0):
+        raise ValueError(f"true-peak ceiling {true_peak} dBTP must be finite and lie in [-20, 0]")
+    return t, c
+
 
 STREAM_BEGIN, STREAM_END = 1, 2
 
@@ -1000,6 +1112,72 @@ class DenoiseStream:
             pass
 
 
+class LoudnessMeter:
+    """Handle of a streaming loudness meter (Engine.open_loudness_meter).  Every push returns every slot's readings
+    [S,4]: integrated, momentary, short-term LUFS and true peak dBTP of the samples it has received since BEGIN."""
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, rate: int = config.SAMPLE_RATE, max_seconds: int = 600):
+        self.eng = eng
+        self.max_streams, self.max_chunk_samples = int(max_streams), int(max_chunk_samples)
+        self.rate, self.max_seconds = _loudness_rate(rate), int(max_seconds)
+        h = C.c_void_p()
+        eng._ck(eng.lib.vtts_loudness_stream_create(eng.h, self.max_streams, self.max_chunk_samples, self.rate, self.max_seconds,
+                                                    C.byref(h)))
+        self.h = h
+        self.lookahead = int(eng.lib.vtts_loudness_stream_lookahead(self.rate))
+
+    def push(self, x, n_new, begin=None, end=None) -> np.ndarray:
+        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None.
+        Returns float32 [S,4]."""
+        S, F = self.max_streams, self.max_chunk_samples
+        x = _np(x, np.float32)
+        if x.ndim != 2 or x.shape[0] != S or x.shape[1] > F:
+            raise ValueError(f"x must be [{S}, <= {F}], got {x.shape}")
+        if x.shape[1] < F:
+            x = np.concatenate([x, np.zeros((S, F - x.shape[1]), np.float32)], axis=1)
+        flags = np.zeros(S, np.uint8)
+        if begin is not None:
+            flags |= np.asarray(begin, bool).astype(np.uint8) * STREAM_BEGIN
+        if end is not None:
+            flags |= np.asarray(end, bool).astype(np.uint8) * STREAM_END
+        n = _np(n_new, np.int32, (S,), "n_new")
+        out = np.empty((S, 4), np.float32)
+        self.eng._ck(self.eng.lib.vtts_loudness_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(flags), _ptr(out)))
+        return out
+
+    def push_device(self, x_t, n_new, flags, out_t, stream=None):
+        """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S,4]; n_new int [S] and flags uint8 [S]
+        (bit0 BEGIN, bit1 END) on the host.  Stream-ordered."""
+        import torch
+        S, F = self.max_streams, self.max_chunk_samples
+        if tuple(x_t.shape) != (S, F) or x_t.dtype != torch.float32 or not x_t.is_contiguous():
+            raise ValueError(f"x_t must be contiguous float32 [{S}, {F}]")
+        if tuple(out_t.shape) != (S, 4) or out_t.dtype != torch.float32 or not out_t.is_contiguous():
+            raise ValueError(f"out_t must be contiguous float32 [{S}, 4]")
+        n = _np(n_new, np.int32, (S,), "n_new")
+        f = _np(flags, np.uint8, (S,), "flags")
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self.eng._ck(self.eng.lib.vtts_loudness_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(out_t), st))
+        return out_t
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.eng, "h", None):
+            self.eng._ck(self.eng.lib.vtts_loudness_stream_destroy(self.eng.h, self.h))
+        self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 def acoustic_stream_schedule(n_frames: int, n_emit: int | None, chunk: int, lookahead: int = 10) -> list:
     """Frames an acoustic stream slot emits per push: it scans min(n_frames, n_emit + lookahead) frames, `chunk` per
     push; after P frames scanned it has emitted min(n_emit, max(0, P - lookahead)), and its last push emits the rest."""
@@ -1107,11 +1285,11 @@ class AcousticStream:
 
 class TtsStream:
     """Handle of a text-to-speech stream (Engine.open_tts_stream): an acoustic stream of max_chunk_frames F feeding a
-    vocoder stream of F + the acoustic lookahead frames per push, with a denoise strength a denoise stream after it, and
-    with an output rate a resample stream last."""
+    vocoder stream of F + the acoustic lookahead frames per push, with a denoise strength a denoise stream after it,
+    with an output rate a resample stream, and with meter=True a loudness meter of the audio `step()` returns last."""
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
-                 output_rate=None, denoise=None):
+                 output_rate=None, denoise=None, meter=False):
         import torch
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
@@ -1119,9 +1297,12 @@ class TtsStream:
             resample_ratio(config.SAMPLE_RATE, output_rate)
         if denoise is not None:
             denoise = _strength(denoise)
+        if meter:
+            _loudness_rate(output_rate or config.SAMPLE_RATE)
         self.eng = eng
         self.rs = None
         self.dn = None
+        self.mt = None
         self.ac = AcousticStream(eng, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng)
         try:
             self.voc = VocoderStream(eng, max_streams, self.ac.out_frames)
@@ -1133,7 +1314,14 @@ class TtsStream:
             if output_rate is not None:
                 # the previous stage's output buffer is the resampler's input
                 self.rs = ResampleStream(eng, max_streams, pitch, output_rate)
+                pitch = self.rs.out_pitch
+            if meter:
+                # the last stage's output buffer is the meter's input; a slot holds at most max_frames of audio
+                seconds = -(-int(max_frames) * config.HOP // config.SAMPLE_RATE) + 1
+                self.mt = LoudnessMeter(eng, max_streams, pitch, output_rate or config.SAMPLE_RATE, seconds)
         except Exception:
+            if getattr(self, "rs", None) is not None:
+                self.rs.close()
             if getattr(self, "dn", None) is not None:
                 self.dn.close()
             if getattr(self, "voc", None) is not None:
@@ -1145,6 +1333,9 @@ class TtsStream:
         self._wav = torch.zeros((max_streams, self.voc.wav_ld), dtype=torch.float32, device=dev)
         self._den = None if self.dn is None else torch.zeros((max_streams, self.dn.out_pitch), dtype=torch.float32, device=dev)
         self._out = None if self.rs is None else torch.zeros((max_streams, self.rs.out_pitch), dtype=torch.float32, device=dev)
+        self._mout = None if self.mt is None else torch.zeros((max_streams, 4), dtype=torch.float32, device=dev)
+        self._mout_h = None if self.mt is None else torch.zeros((max_streams, 4), dtype=torch.float32).pin_memory()
+        self._meter = {}
         self._fresh = np.zeros(max_streams, bool)   # begun, no push yet: the next vocoder push carries BEGIN
         self._empty = set()                         # begun with nothing left after the trim: reported empty at the next step
 
@@ -1197,13 +1388,28 @@ class TtsStream:
             if self.rs is not None:
                 n_wav = self.rs.push_device(src, n_wav, flags, self._out)
                 src = self._out
+            if self.mt is not None:
+                self.mt.push_device(src, n_wav, flags, self._mout)
+                self._mout_h.copy_(self._mout, non_blocking=True)   # ready once the blocking copy below returns
             wav = src.cpu().numpy()
             for s in np.flatnonzero(active):
                 out[int(s)] = wav[s, : int(n_wav[s])].copy()
+            if self.mt is not None:
+                m = self._mout_h.numpy()
+                self._meter = {int(s): tuple(float(v) for v in m[s]) for s in np.flatnonzero(active)}
         self._fresh &= ~active
         return out
 
+    def meter(self) -> dict:
+        """{slot: (integrated, momentary, short_term, true_peak)} of the audio each slot stepped last has produced since
+        its BEGIN (meter=True): equal to `Engine.loudness` of that audio, bit for bit, once the slot's last step ran."""
+        if self.mt is None:
+            raise ValueError("the stream was opened without meter=True")
+        return dict(self._meter)
+
     def close(self):
+        if getattr(self, "mt", None) is not None:
+            self.mt.close()
         if getattr(self, "rs", None) is not None:
             self.rs.close()
         if getattr(self, "dn", None) is not None:

@@ -7,7 +7,9 @@ single library call per batch (`Engine.tts`), and the WAV writer is built in (th
 `--precision fp16` runs the generator in the fast fp16 mode (Engine.set_precision) for either input.
 `--output-rate R` resamples the audio on the device (Engine.resample) and writes R in the header; `--sample-rate` keeps
 the reference's meaning, the header rate of the unchanged 16 kHz samples.  `--denoise S` removes the generator's bias
-hiss on the device (Engine.denoise, strength S, the default bias) at 16 kHz, before any resampling.
+hiss on the device (Engine.denoise, strength S, the default bias) at 16 kHz, before any resampling.  `--loudness L`
+normalizes every output to L LUFS (ITU-R BS.1770-4, Engine.normalize_loudness) at the rate it is written, after
+--denoise and --output-rate, under a true-peak ceiling (`--true-peak`, default -1 dBTP as EBU R128 asks).
 """
 from __future__ import annotations
 
@@ -113,6 +115,13 @@ def main(argv=None) -> int:
     parser.add_argument("--denoise", default=None, type=float, metavar="STRENGTH",
                         help="subtract STRENGTH times the generator's bias spectrum (its output for an all-zero mel) from the "
                              "STFT magnitude of the 16 kHz audio on the device, before any --output-rate resampling; >= 0")
+    parser.add_argument("--loudness", default=None, type=float, metavar="LUFS",
+                        help="normalize every output (each --text-file line separately) to this integrated loudness, "
+                             "ITU-R BS.1770-4, in [-70, 0]; measured on the device at the output rate, after --denoise and "
+                             "--output-rate (e.g. -23 broadcast, -16 podcasts)")
+    parser.add_argument("--true-peak", default=None, type=float, metavar="DBTP",
+                        help="with --loudness: the true-peak ceiling in dBTP, in [-20, 0] (default -1.0, EBU R128); the gain is "
+                             "lowered until the 4x-oversampled peak stays below it")
     parser.add_argument("--silence-duration", default=-1, type=float)
     parser.add_argument("--lexicon-file", default=None)
     parser.add_argument("--seed", default=None, type=int,
@@ -144,6 +153,17 @@ def main(argv=None) -> int:
         if max(up, down) > 1024:
             parser.error(f"--output-rate {args.output_rate}: {config.SAMPLE_RATE} -> {args.output_rate} reduces to {up}/{down} "
                          "(at most 1024 each)")
+    if args.true_peak is not None and args.loudness is None:
+        parser.error("--true-peak is the ceiling of --loudness normalization; give --loudness too")
+    if args.loudness is not None:
+        from .engine import _loudness_rate, _loudness_target
+        if args.true_peak is None:
+            args.true_peak = -1.0
+        try:
+            _loudness_target(args.loudness, args.true_peak)
+            _loudness_rate(args.output_rate or config.SAMPLE_RATE)
+        except ValueError as e:
+            parser.error(f"--loudness: {e}")
     header_rate = args.output_rate or args.sample_rate or config.SAMPLE_RATE
     lexicon = args.lexicon_file if args.lexicon_file is not None else config.LEXICON_FILE
     if args.precision is not None:
@@ -154,9 +174,12 @@ def main(argv=None) -> int:
         from .engine import get_engine
         if args.denoise is not None:
             waves = [get_engine().denoise(w, args.denoise) for w in waves]
-        if args.output_rate is None:
-            return waves
-        return [get_engine().resample(w, args.output_rate) for w in waves]
+        if args.output_rate is not None:
+            waves = [get_engine().resample(w, args.output_rate) for w in waves]
+        if args.loudness is not None:
+            rate = args.output_rate or config.SAMPLE_RATE
+            waves = [get_engine().normalize_loudness(w, args.loudness, rate, true_peak=args.true_peak)[0] for w in waves]
+        return waves
 
     if args.text_file is not None:
         lines = [ln for ln in args.text_file.read_text().splitlines() if ln.strip()]

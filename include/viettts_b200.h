@@ -207,6 +207,14 @@ int vtts_debug_hifigan_layer(vtts_ctx* ctx, int layer, const float* const* x, fl
  * (later debug_read taps are invalid).  Synchronous. */
 int vtts_debug_dropout_masks(vtts_ctx* ctx, int kind, uint64_t seed, int B, int N, uint8_t* host_out);
 
+/* test hook: the discrete decisions of vtts_pitch_shift for the same arguments, as the device takes them:
+ * dec_dev int32 [B][S / 256 + 1][513], for frame t and bin k 1 | (e < 0) << 1 where k is a peak of frame t and e its
+ * wrapped phase deviation princarg(theta_t[k] - theta_t-1[k] - 2 pi k H / N) (which side of the princarg cut it took;
+ * 0 in frame 0), and 0 elsewhere (no peak, frames past the row's, copied rows).  Runs the analysis and phase kernels of
+ * the call.  Stream-ordered; uses the context's workspace. */
+int vtts_debug_pitch_decisions(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const float* semitones,
+                               int32_t* dec_dev, void* stream);
+
 /* profiling aid: per-CTA stall counters (SM clocks) of the LAST tensor-core conv launch.
  * Row = CTA, columns: 0 MMA-role total, 1 MMA wait accumulator-free, 2 MMA wait activations, 3 MMA wait
  * weights, 4 weight-producer wait slot, 5 converter wait slot, 6 converter fill, 7 epilogue wait
@@ -327,6 +335,50 @@ int vtts_denoise_stream_push(vtts_ctx* ctx, vtts_denoise_stream* ds, const float
 /* the same on host buffers x [S][max_chunk_samples] and y [S][out_pitch]; returns when y is written */
 int vtts_denoise_stream_push_host(vtts_ctx* ctx, vtts_denoise_stream* ds, const float* x, const int32_t* n_new,
                                   const uint8_t* flags, float* y, int32_t* n_out);
+
+/* ---- pitch shift: a peak-locked phase vocoder on the denoiser's STFT --------------------------------------------------
+ * One row x of n samples, a shift of s semitones (finite, in [-12, 12], else VTTS_ERR_BAD_ARG before anything is
+ * launched), r = fp32(2^(s / 12)) computed in double (Laroche & Dolson 1999, "New phase-vocoder techniques for
+ * pitch-shifting, harmonizing and other exotic effects"):
+ *   the STFT of vtts_denoise (X_t[k], k = 0..512); a_t = |X_t|, theta_t = arg X_t (double);
+ *   peaks: a_t[k] > a_t[k-1], a_t[k] >= a_t[k+1], a_t[k] > 0, neighbours outside [0, 512] counting as -1; every bin
+ *   belongs to its nearest peak (the lower one on a tie);
+ *   omega_t[p] = 2 pi p / N + princarg(theta_t[p] - theta_t-1[p] - 2 pi p H / N) / H (2 pi p / N at t = 0);
+ *   psi_t(p) = princarg(psi_t-1[p] + H (r - 1) omega_t[p]), psi_t-1[k] the rotation of the peak that owned bin k in
+ *   frame t - 1 (0 before frame 0 and in a frame without peaks); princarg(x) = x - 2 pi rint(x / 2 pi); in double;
+ *   D_p = rint((r - 1) p); bin k of peak p adds X_t[k] (-1)^D_p e^(i psi_t(p)) to Z_t[k + D_p] (targets outside [0, 512]
+ *   dropped, sums in ascending k);  y = the denoiser's inverse and overlap-add of Z.
+ * Rows with s == 0 and rows of n <= 512 are returned unchanged, bit for bit.  fp32 in every vtts_precision mode apart
+ * from the double phase recurrence.  Each frame is analysed and synthesized on its own and the recurrence runs once per
+ * frame in frame order, so a row gives the same bits alone, in any batch, and through the stream. */
+/* x_dev [B,S]; n_dev int32 [B] or NULL (= S; values clamped to [0, S]); semitones HOST float [B]; y_dev [B,S], not x_dev;
+ * outputs past n[b] are 0.  Stream-ordered; uses the context's workspace (about 17 KiB per frame of 256 samples). */
+int vtts_pitch_shift(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const float* semitones, float* y_dev,
+                     void* stream);
+/* the same on host buffers; n_in[b] must lie in [0, S] */
+int vtts_pitch_shift_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, const float* semitones, float* y);
+/* Streaming pitch shifter with max_streams independent slots: each slot carries the denoise stream's window of 2048
+ * inputs and its 64-bit position, the index of its next unscanned frame, theta and psi (double) of the last scanned frame
+ * and the synthesized frames later outputs still overlap, so the outputs a slot emits, concatenated, are bit-identical
+ * to vtts_pitch_shift of its whole input.  Outputs are released on the denoise stream's schedule (before END
+ * min(P, 256 * max(0, floor(P / 256) - 3)) after P samples; END emits the rest) and vtts_pitch_shift_stream_lookahead()
+ * = 1023.  A slot's shift is read from semitones[s] with BEGIN and fixed until END.  flags and slot rules as for the
+ * resample stream.  Every push issues the same five launches (window step, analysis, phase, synthesis, overlap-add). */
+typedef struct vtts_pitch_shift_stream vtts_pitch_shift_stream;
+/* *out_pitch receives the outputs per slot of a push's output buffer (max_chunk_samples + 1023) */
+int vtts_pitch_shift_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, vtts_pitch_shift_stream** out, int* out_pitch);
+int vtts_pitch_shift_stream_destroy(vtts_ctx* ctx, vtts_pitch_shift_stream* ps);
+int vtts_pitch_shift_stream_lookahead(void);
+/* x_dev [S][max_chunk_samples] (samples past n_new[s] ignored); n_new, flags, n_out HOST int32 / uint8 / int32 [S];
+ * semitones HOST float [S]: read for the slots with BEGIN (finite, in [-12, 12]); for the other pushed slots it must
+ * hold the slot's shift, or semitones may be NULL when no slot begins.  y_dev [S][out_pitch], not x_dev, slot s gets
+ * n_out[s] outputs from its start.  Argument errors fail with VTTS_ERR_BAD_ARG before anything is launched.
+ * Stream-ordered. */
+int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x_dev, const int32_t* n_new,
+                                 const uint8_t* flags, const float* semitones, float* y_dev, int32_t* n_out, void* stream);
+/* the same on host buffers x [S][max_chunk_samples] and y [S][out_pitch]; returns when y is written */
+int vtts_pitch_shift_stream_push_host(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x, const int32_t* n_new,
+                                      const uint8_t* flags, const float* semitones, float* y, int32_t* n_out);
 
 /* ---- loudness: ITU-R BS.1770-4 gated loudness and true peak, and normalization to a target ------------------------
  * One mono row x of n samples at rate r, a multiple of 10 in [8000, 192000] (else VTTS_ERR_BAD_ARG):

@@ -35,6 +35,7 @@ SIGNATURES = {
     "vtts_debug_dropout_masks": (C.c_int, [c_ctx, C.c_int, C.c_uint64, C.c_int, C.c_int, C.c_void_p]),
     "vtts_debug_pair": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]),
+    "vtts_debug_pitch_decisions": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtts_debug_hifigan_layer": (C.c_int, [c_ctx, C.c_int, ptrp, ptrp, C.c_void_p, C.c_int, C.c_int]),
     "vtts_hifigan_blob_floats": (C.c_int64, []),
     "vtts_acoustic_blob_floats": (C.c_int64, []),
@@ -84,6 +85,15 @@ SIGNATURES = {
     "vtts_denoise_stream_lookahead": (C.c_int, []),
     "vtts_denoise_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtts_denoise_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_pitch_shift": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_pitch_shift_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vtts_pitch_shift_stream_create": (C.c_int, [c_ctx, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_int)]),
+    "vtts_pitch_shift_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
+    "vtts_pitch_shift_stream_lookahead": (C.c_int, []),
+    "vtts_pitch_shift_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_void_p]),
+    "vtts_pitch_shift_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                    C.c_void_p]),
     "vtts_loudness_filter": (C.c_int, [C.c_int, C.c_void_p]),
     "vtts_loudness": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "vtts_loudness_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),

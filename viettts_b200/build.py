@@ -11,7 +11,7 @@ PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 LIB = PKG / "libviettts_b200.so"
 SOURCES = ["api.cu", "conv1d.cu", "tc_conv.cu", "hifigan.cu", "vocoder_stream.cu", "acoustic_stream.cu", "nat.cu", "melspec.cu",
-           "resample.cu", "denoise.cu", "loudness.cu"]
+           "resample.cu", "denoise.cu", "loudness.cu", "pitch.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

@@ -26,35 +26,23 @@
 #include <cmath>
 #include <cstring>
 
-#include "fft_common.cuh"
+#include "stft_common.cuh"
 #include "vtts_internal.cuh"
 
 namespace {
 
 using fftc::bitrev5;
-using fftc::cmul;
-using fftc::fft32;
+using stftc::fft1024;
 
 constexpr int NF = vc::NFFT;      // 1024
 constexpr int NB = vc::NBINS;     // 513
 constexpr int HOP = vc::HOP;      // 256
 constexpr int PAD = NF / 2;       // 512
 constexpr int DN_WARPS = 4;       // frames per CTA
-constexpr int TP = 33;            // transpose pitch (float2)
+constexpr int TP = stftc::TP;     // transpose pitch (float2)
 constexpr int OLA_THREADS = 256;
 constexpr int DN_K = 2048;        // carried inputs per stream slot (the frames of a push start at most 1791 before P0)
 constexpr int DN_LOOKAHEAD = 1023;
-constexpr long long DN_OPEN = 1LL << 60;   // row length not known yet (stream slot before END)
-
-struct DnRow {
-  long long x0;       // absolute index of buffer element 0
-  long long n;        // row length (DN_OPEN while a stream slot is open)
-  long long g0;       // first frame computed (workspace row 0)
-  long long e0;       // absolute index of the first output written
-  long long cnt;      // outputs written
-  int nfr;            // frames computed
-  int copy;           // row of <= 512 samples: the outputs are the inputs
-};
 
 // rows == nullptr: the one-shot bounds of row b: n = n_in[b] clamped to [0, S] (or S), all S outputs written (zeros
 // past n), frames 0 .. n / 256 when n > 512
@@ -69,21 +57,6 @@ __device__ __forceinline__ DnRow dn_row(const DnRow* rows, const int* n_in, int 
   r.copy = r.n <= PAD;
   r.nfr = r.copy ? 0 : (int)(r.n / HOP + 1);
   return r;
-}
-
-// forward four-step FFT-1024 of v (v[m] = sample lane + 32 m): on return v[p] = X[lane + 32 bitrev5(p)].  sw is the
-// warp's 32 x TP transpose buffer; the caller syncs the warp before sw is reused.
-__device__ __forceinline__ void fft1024(float2 (&v)[32], float2* sw, const float2* __restrict__ tw, int lane) {
-  fft32(v);                                              // over m: v[bitrev5(k1)] = sum_m x[lane + 32 m] W32^(m k1)
-#pragma unroll
-  for (int p = 0; p < 32; ++p) {
-    const int k1 = bitrev5(p);
-    sw[k1 * TP + lane] = k1 == 0 ? v[p] : cmul(v[p], __ldg(tw + lane * k1));   // W1024^(lane k1), lane k1 <= 961
-  }
-  __syncwarp();
-#pragma unroll
-  for (int t = 0; t < 32; ++t) v[t] = sw[lane * TP + t];  // lane = k1, t = the first pass's lane
-  fft32(v);                                              // over t: X[k1 + 32 k2]
 }
 
 // MAG: write |X_0[k]| of frame 0 of row 0 to mag_out[k] (the bias of a waveform) and stop
@@ -105,18 +78,7 @@ __global__ void __launch_bounds__(DN_WARPS * 32) denoise_frame_kernel(const floa
 
   // ---- windowed frame: sample j0 + lane + 32 m, reflected at 0 and n - 1 of the row ----
   float2 v[32];
-  if (j0 >= 0 && j0 + NF <= r.n) {
-    const float* src = xr + (j0 - r.x0) + lane;
-#pragma unroll
-    for (int m = 0; m < 32; ++m) v[m] = make_float2(__ldg(src + 32 * m) * __ldg(hann + lane + 32 * m), 0.f);
-  } else {
-#pragma unroll
-    for (int m = 0; m < 32; ++m) {
-      long long j = j0 + lane + 32 * m;
-      j = j < 0 ? -j : (j >= r.n ? 2 * (r.n - 1) - j : j);
-      v[m] = make_float2(__ldg(xr + (j - r.x0)) * __ldg(hann + lane + 32 * m), 0.f);
-    }
-  }
+  stftc::read_frame(v, xr, r.x0, r.n, j0, hann, lane);
   fft1024(v, sw, tw, lane);
 
   // ---- gain on bins k = lane + 32 k2 <= 512 ----
@@ -139,25 +101,9 @@ __global__ void __launch_bounds__(DN_WARPS * 32) denoise_frame_kernel(const floa
   if (MAG) return;
   __syncwarp();
 
-  // ---- inverse: Re FFT(conj Y) of the Hermitian spectrum, element i = lane + 32 m is conj Y[i] (i <= 512) or Y[1024 - i] ----
-#pragma unroll
-  for (int m = 0; m < 32; ++m) {
-    const int i = lane + 32 * m;
-    if (m < 16 || i == NB - 1) {
-      const float2 y = sw[i];
-      v[m] = make_float2(y.x, -y.y);
-    } else {
-      v[m] = sw[NF - i];
-    }
-  }
-  __syncwarp();                                          // every lane has read the spectrum
-  fft1024(v, sw, tw, lane);
-  float* out = ws + ((size_t)b * ws_frames + fl) * NF;
-#pragma unroll
-  for (int p = 0; p < 32; ++p) {
-    const int i = lane + 32 * bitrev5(p);
-    out[i] = v[p].x * (1.f / NF) * __ldg(hann + i);
-  }
+  // ---- inverse: w * irfft(Y) of the gained spectrum ----
+  stftc::inverse_frame(v, sw, tw, lane);
+  stftc::write_frame(v, hann, lane, ws + ((size_t)b * ws_frames + fl) * NF);
 }
 
 __global__ void __launch_bounds__(OLA_THREADS) denoise_ola_kernel(const float* __restrict__ x, long long x_ld, int S,
@@ -209,14 +155,19 @@ int dn_launch(vtts_ctx* ctx, const float* x, long long x_ld, int S, const int* n
                                                                       nullptr);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
+  return vtts_denoise_ola(ctx, x, x_ld, S, n_in, rows, B, max_out, ws, ws_frames, y, y_ld, st);
+}
+
+}  // namespace
+
+int vtts_denoise_ola(vtts_ctx* ctx, const float* x, long long x_ld, int S, const int* n_in, const DnRow* rows, int B, long long max_out,
+                     const float* ws, int ws_frames, float* y, long long y_ld, cudaStream_t st) {
   const unsigned ogrid = (unsigned)std::max(1LL, (max_out + OLA_THREADS - 1) / OLA_THREADS);
   denoise_ola_kernel<<<dim3(ogrid, B), OLA_THREADS, 0, st>>>(x, x_ld, S, n_in, rows, ctx->hann, ws, ws_frames, y, y_ld);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   return VTTS_OK;
 }
-
-}  // namespace
 
 int vtts_denoise_stream_lookahead(void) { return DN_LOOKAHEAD; }
 

@@ -358,6 +358,22 @@ struct RsRow {
 // outputs of a row.
 int vtts_resample_run(vtts_ctx* ctx, int in_rate, int out_rate, const float* x, long long x_ld, int S_in, const int* n_in,
                       const RsRow* rows, int B, long long S_out, long long max_out, float* y, long long y_ld, cudaStream_t st);
+// denoise.cu: per-row bounds of the STFT frame and overlap-add kernels, which place a row's buffers in absolute time
+constexpr long long DN_OPEN = 1LL << 60;   // row length not known yet (stream slot before END)
+struct DnRow {
+  long long x0;       // absolute index of buffer element 0
+  long long n;        // row length (DN_OPEN while a stream slot is open)
+  long long g0;       // frame held in workspace row 0 of the row
+  long long e0;       // absolute index of the first output written
+  long long cnt;      // outputs written
+  int nfr;            // frames computed
+  int copy;           // the outputs are the inputs (a row of <= 512 samples)
+};
+// denoise.cu: one launch of the overlap-add kernel (denoise_ola_kernel): output t of row b is the sum of the covering
+// windowed time frames ws [B][ws_frames][1024] (frame g at row g - g0) in ascending order over the envelope sum w^2, the
+// input itself for copy rows, 0 past n.  rows == nullptr: the one-shot bounds (n_in[b] or S samples, S outputs written).
+int vtts_denoise_ola(vtts_ctx* ctx, const float* x, long long x_ld, int S, const int* n_in, const DnRow* rows, int B, long long max_out,
+                     const float* ws, int ws_frames, float* y, long long y_ld, cudaStream_t st);
 // melspec.cu
 // twiddles exp(-2 pi i k / 1024) and the periodic Hann window into ctx->fft_tw / ctx->hann (once per context)
 int vtts_fft_tables(vtts_ctx* ctx);

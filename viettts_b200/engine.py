@@ -63,6 +63,20 @@ def _strength(s) -> float:
     return s
 
 
+MAX_SEMITONES = 12.0
+
+
+def _semitones(v, n: int) -> np.ndarray:
+    """float32 [n]: a scalar shift for every row, or one per row, each finite and in [-12, 12]"""
+    a = np.asarray(v, np.float32)
+    a = np.full(n, a, np.float32) if a.ndim == 0 else np.ascontiguousarray(a.reshape(-1), np.float32)
+    if a.shape != (n,):
+        raise ValueError(f"semitones: one value or one per row ({n}), got {np.shape(v)}")
+    if not (np.all(np.isfinite(a)) and np.all(np.abs(a) <= MAX_SEMITONES)):
+        raise ValueError(f"semitones must be finite and lie in [-12, 12], got {v}")
+    return a
+
+
 def _ptr(a):
     if a is None:
         return None
@@ -315,18 +329,20 @@ class Engine:
         return AcousticStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, masks=masks)
 
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
-                        rng=None, output_rate=None, denoise=None, meter=False) -> "TtsStream":
+                        rng=None, output_rate=None, denoise=None, meter=False, semitones=None) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
         With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  `output_rate`: a resample
         stream follows the vocoder on the device and `step()` returns samples at that rate, equal to `resample` of the
         `tts` audio bit for bit.  `denoise`: a strength; a denoise stream with the default bias (`denoiser_bias()`) sits
         between the vocoder and the resampler, and the audio equals `denoise` of the `tts` audio (then resampled) bit for
-        bit.  `meter=True`: a loudness meter runs last, on what `step()` returns at the output rate (a multiple of 10),
-        and `TtsStream.meter()` gives each stepped slot's readings, read back in the step's one synchronisation.  Needs the
-        'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
+        bit.  `semitones`: a pitch-shift stream follows the denoiser (before the resampler) with this shift as every slot's
+        default (`begin(..., semitones=)` overrides it per slot), and the audio equals `pitch_shift` of the (denoised)
+        `tts` audio bit for bit.  `meter=True`: a loudness meter runs last, on what `step()` returns at the output rate (a
+        multiple of 10), and `TtsStream.meter()` gives each stepped slot's readings, read back in the step's one
+        synchronisation.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
         return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate,
-                         denoise=denoise, meter=meter)
+                         denoise=denoise, meter=meter, semitones=semitones)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -783,6 +799,59 @@ class Engine:
         frames covering it are final (at most 1023 samples after its own time); END emits the rest."""
         return DenoiseStream(self, max_streams, max_chunk_samples, strength, bias)
 
+    # ---- pitch shift (vtts_pitch_shift*: a peak-locked phase vocoder on the denoiser's STFT, fp32, double phases) ----
+    def pitch_shift(self, wav, semitones, lengths=None) -> np.ndarray:
+        """Host arrays: wav f32 [S] or [B,S] -> the same shape, every spectral peak's region moved by the ratio
+        fp32(2^(s / 12)) with its phase kept coherent across frames (n_fft 1024, hop 256); the timing of every sample is
+        kept.  semitones: a scalar or one value per row, finite and in [-12, 12]; rows with 0 and rows of <= 512 samples
+        are copied.  lengths int [B] in [0, S]: row b holds lengths[b] samples and its outputs past them are 0."""
+        x = _np(wav, np.float32)
+        one = x.ndim == 1
+        x = x[None] if one else x
+        if x.ndim != 2:
+            raise ValueError(f"wav must be [S] or [B,S], got {np.shape(wav)}")
+        B, S = x.shape
+        sem = _semitones(semitones, B)
+        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
+        if S == 0 or B == 0:
+            return (x[0] if one else x).copy()          # nothing to transform: empty rows are short rows
+        y = np.empty((B, S), np.float32)
+        self._ck(self.lib.vtts_pitch_shift_host(self.h, _ptr(x), _ptr(lens), B, S, _ptr(sem), _ptr(y)))
+        return y[0] if one else y
+
+    def pitch_shift_forward(self, x_t, semitones, lengths_t=None, out=None, stream=None):
+        """vtts_pitch_shift on torch CUDA tensors, stream-ordered: x_t f32 [B,S] -> [B,S] (not x_t); semitones a scalar or
+        one host value per row; lengths_t int32 CUDA [B] or None."""
+        import torch
+        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
+        B, S = x_t.shape
+        sem = _semitones(semitones, B)
+        if out is None:
+            out = torch.empty((B, S), dtype=torch.float32, device=x_t.device)
+        elif tuple(out.shape) != (B, S) or out.dtype != torch.float32 or not out.is_contiguous():
+            raise ValueError(f"out must be contiguous float32 [{B}, {S}]")
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self._ck(self.lib.vtts_pitch_shift(self.h, _ptr(x_t), _ptr(lengths_t), B, S, _ptr(sem), _ptr(out), st))
+        return out
+
+    def debug_pitch_decisions(self, x_t, semitones, lengths_t=None) -> np.ndarray:
+        """Test hook (vtts_debug_pitch_decisions): int32 [B, S // 256 + 1, 513], the device's peak flags (bit 0) and the
+        side of the princarg cut each peak's phase deviation took (bit 1: negative) for `pitch_shift_forward` of the
+        same arguments."""
+        import torch
+        B, S = x_t.shape
+        sem = _semitones(semitones, B)
+        out = torch.empty((B, S // config.HOP + 1, DENOISE_BINS), dtype=torch.int32, device=x_t.device)
+        st = torch.cuda.current_stream(x_t.device).cuda_stream
+        self._ck(self.lib.vtts_debug_pitch_decisions(self.h, _ptr(x_t), _ptr(lengths_t), B, S, _ptr(sem), _ptr(out), st))
+        return out.cpu().numpy()
+
+    def open_pitch_shift_stream(self, max_streams: int, max_chunk_samples: int) -> "PitchShiftStream":
+        """Streaming pitch shifter with `max_streams` independent slots (vtts_pitch_shift_stream_*): a slot's shift is
+        given with BEGIN and fixed until END, and its outputs, concatenated, equal `pitch_shift` of its whole input bit
+        for bit.  Outputs are released on the denoise stream's schedule (at most 1023 samples after their own time)."""
+        return PitchShiftStream(self, max_streams, max_chunk_samples)
+
     # ---- loudness (vtts_loudness*: ITU-R BS.1770-4 gated loudness and true peak, fp32) ----
     def loudness(self, wav, rate: int = config.SAMPLE_RATE, lengths=None) -> "Loudness":
         """Host arrays: wav f32 [S] or [B,S] at `rate` (a multiple of 10 in [8000, 192000]) -> Loudness of float32 [B]
@@ -1112,6 +1181,100 @@ class DenoiseStream:
             pass
 
 
+class PitchShiftStream:
+    """Handle of a streaming pitch shifter (Engine.open_pitch_shift_stream).  Before END a slot that has received P samples
+    has emitted min(P, 256 max(0, floor(P / 256) - 3)) outputs; a push with END emits the rest."""
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int):
+        self.eng = eng
+        self.max_streams, self.max_chunk_samples = int(max_streams), int(max_chunk_samples)
+        h, pitch = C.c_void_p(), C.c_int()
+        eng._ck(eng.lib.vtts_pitch_shift_stream_create(eng.h, self.max_streams, self.max_chunk_samples, C.byref(h), C.byref(pitch)))
+        self.h = h
+        self.out_pitch = int(pitch.value)   # outputs per slot of a push's output buffer
+        self.lookahead = int(eng.lib.vtts_pitch_shift_stream_lookahead())
+        self.shift = np.zeros(self.max_streams, np.float32)   # each slot's shift since its BEGIN
+
+    def _shifts(self, flags, semitones) -> np.ndarray:
+        """the semitones array of a push: the given values for the slots that begin, the slots' own shifts elsewhere"""
+        sem = self.shift.copy()
+        begin = (np.asarray(flags) & STREAM_BEGIN) != 0
+        if begin.any():
+            if semitones is None:
+                raise ValueError("semitones= is required for the slots a push begins")
+            given = np.asarray(semitones, np.float32)
+            given = np.full(self.max_streams, given, np.float32) if given.ndim == 0 else given
+            if given.shape != (self.max_streams,):
+                raise ValueError(f"semitones: one value or one per slot ({self.max_streams}), got {np.shape(semitones)}")
+            sem[begin] = given[begin]
+        return np.ascontiguousarray(sem, np.float32)
+
+    def _commit(self, flags, sem):
+        begin = (np.asarray(flags) & STREAM_BEGIN) != 0
+        self.shift[begin] = sem[begin]
+
+    def push(self, x, n_new, begin=None, end=None, semitones=None) -> list:
+        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None,
+        semitones: a scalar or [S], read for the slots that begin.  Returns one float32 array per slot with the samples
+        it emits now."""
+        S, F = self.max_streams, self.max_chunk_samples
+        x = _np(x, np.float32)
+        if x.ndim != 2 or x.shape[0] != S or x.shape[1] > F:
+            raise ValueError(f"x must be [{S}, <= {F}], got {x.shape}")
+        if x.shape[1] < F:
+            x = np.concatenate([x, np.zeros((S, F - x.shape[1]), np.float32)], axis=1)
+        flags = np.zeros(S, np.uint8)
+        if begin is not None:
+            flags |= np.asarray(begin, bool).astype(np.uint8) * STREAM_BEGIN
+        if end is not None:
+            flags |= np.asarray(end, bool).astype(np.uint8) * STREAM_END
+        n = _np(n_new, np.int32, (S,), "n_new")
+        sem = self._shifts(flags, semitones)
+        y = np.empty((S, self.out_pitch), np.float32)
+        n_out = np.zeros(S, np.int32)
+        self.eng._ck(self.eng.lib.vtts_pitch_shift_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(flags), _ptr(sem), _ptr(y),
+                                                                    _ptr(n_out)))
+        self._commit(flags, sem)
+        return [y[s, : int(n_out[s])].copy() for s in range(S)]
+
+    def push_device(self, x_t, n_new, flags, out_t, semitones=None, stream=None) -> np.ndarray:
+        """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S, out_pitch]; n_new int [S], flags
+        uint8 [S] (bit0 BEGIN, bit1 END) and semitones (scalar or [S], read for the slots that begin) on the host.
+        Stream-ordered; returns n_out int32 [S] (outputs slot s got at the start of its row of out_t)."""
+        import torch
+        S, F = self.max_streams, self.max_chunk_samples
+        if tuple(x_t.shape) != (S, F) or x_t.dtype != torch.float32 or not x_t.is_contiguous():
+            raise ValueError(f"x_t must be contiguous float32 [{S}, {F}]")
+        if tuple(out_t.shape) != (S, self.out_pitch) or out_t.dtype != torch.float32 or not out_t.is_contiguous():
+            raise ValueError(f"out_t must be contiguous float32 [{S}, {self.out_pitch}]")
+        n = _np(n_new, np.int32, (S,), "n_new")
+        f = _np(flags, np.uint8, (S,), "flags")
+        sem = self._shifts(f, semitones)
+        n_out = np.zeros(S, np.int32)
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self.eng._ck(self.eng.lib.vtts_pitch_shift_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(sem), _ptr(out_t),
+                                                               _ptr(n_out), st))
+        self._commit(f, sem)
+        return n_out
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.eng, "h", None):
+            self.eng._ck(self.eng.lib.vtts_pitch_shift_stream_destroy(self.eng.h, self.h))
+        self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class LoudnessMeter:
     """Handle of a streaming loudness meter (Engine.open_loudness_meter).  Every push returns every slot's readings
     [S,4]: integrated, momentary, short-term LUFS and true peak dBTP of the samples it has received since BEGIN."""
@@ -1286,10 +1449,11 @@ class AcousticStream:
 class TtsStream:
     """Handle of a text-to-speech stream (Engine.open_tts_stream): an acoustic stream of max_chunk_frames F feeding a
     vocoder stream of F + the acoustic lookahead frames per push, with a denoise strength a denoise stream after it,
-    with an output rate a resample stream, and with meter=True a loudness meter of the audio `step()` returns last."""
+    with semitones a pitch-shift stream, with an output rate a resample stream, and with meter=True a loudness meter of
+    the audio `step()` returns last."""
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
-                 output_rate=None, denoise=None, meter=False):
+                 output_rate=None, denoise=None, meter=False, semitones=None):
         import torch
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
@@ -1299,9 +1463,12 @@ class TtsStream:
             denoise = _strength(denoise)
         if meter:
             _loudness_rate(output_rate or config.SAMPLE_RATE)
+        if semitones is not None:
+            semitones = float(_semitones(semitones, 1)[0])
         self.eng = eng
         self.rs = None
         self.dn = None
+        self.ps = None
         self.mt = None
         self.ac = AcousticStream(eng, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng)
         try:
@@ -1311,6 +1478,10 @@ class TtsStream:
                 # the vocoder's output buffer is the denoiser's input: n_new = 256 * frames it emitted
                 self.dn = DenoiseStream(eng, max_streams, pitch, denoise)
                 pitch = self.dn.out_pitch
+            if semitones is not None:
+                # the previous stage's output buffer is the pitch shifter's input
+                self.ps = PitchShiftStream(eng, max_streams, pitch)
+                pitch = self.ps.out_pitch
             if output_rate is not None:
                 # the previous stage's output buffer is the resampler's input
                 self.rs = ResampleStream(eng, max_streams, pitch, output_rate)
@@ -1322,6 +1493,8 @@ class TtsStream:
         except Exception:
             if getattr(self, "rs", None) is not None:
                 self.rs.close()
+            if getattr(self, "ps", None) is not None:
+                self.ps.close()
             if getattr(self, "dn", None) is not None:
                 self.dn.close()
             if getattr(self, "voc", None) is not None:
@@ -1332,6 +1505,9 @@ class TtsStream:
         self._mel = torch.zeros((max_streams, self.ac.out_frames, config.MEL_DIM), dtype=torch.float32, device=dev)
         self._wav = torch.zeros((max_streams, self.voc.wav_ld), dtype=torch.float32, device=dev)
         self._den = None if self.dn is None else torch.zeros((max_streams, self.dn.out_pitch), dtype=torch.float32, device=dev)
+        self._psout = None if self.ps is None else torch.zeros((max_streams, self.ps.out_pitch), dtype=torch.float32, device=dev)
+        self._semitones = semitones                    # every slot's default shift
+        self._shift = np.zeros(max_streams, np.float32)  # the shift of each slot's utterance
         self._out = None if self.rs is None else torch.zeros((max_streams, self.rs.out_pitch), dtype=torch.float32, device=dev)
         self._mout = None if self.mt is None else torch.zeros((max_streams, 4), dtype=torch.float32, device=dev)
         self._mout_h = None if self.mt is None else torch.zeros((max_streams, 4), dtype=torch.float32).pin_memory()
@@ -1343,12 +1519,16 @@ class TtsStream:
     def max_streams(self):
         return self.ac.max_streams
 
-    def begin(self, slot: int, tokens, silence_duration=-1.0):
+    def begin(self, slot: int, tokens, silence_duration=-1.0, semitones=None):
         """Start `tokens` (one row of phoneme ids) in a free slot: durations, the text2mel fix-ups and the trim are
-        planned exactly as `Engine.tts` plans them (vtts_tts_plan).  Returns the number of frames the slot will vocode."""
+        planned exactly as `Engine.tts` plans them (vtts_tts_plan).  `semitones` overrides the stream's shift for this
+        utterance.  Returns the number of frames the slot will vocode."""
         slot = int(slot)
         if self.ac.open[slot] or slot in self._empty:
             raise ValueError(f"slot {slot} is still open")
+        if semitones is not None and self.ps is None:
+            raise ValueError("the stream was opened without semitones= (no pitch-shift stage)")
+        shift = self._semitones if semitones is None else float(_semitones(semitones, 1)[0])
         tok = _np(tokens, np.int32).reshape(1, -1)
         _, frames, nf, ne = self.eng.tts_plan(tok, silence_duration=silence_duration)
         if nf[0] < 1:
@@ -1358,6 +1538,8 @@ class TtsStream:
             return 0
         self.ac.begin([slot], tok, frames, n_frames=nf, n_emit=ne)
         self._fresh[slot] = True
+        if self.ps is not None:
+            self._shift[slot] = shift
         return int(ne[0])
 
     def busy(self) -> np.ndarray:
@@ -1385,6 +1567,9 @@ class TtsStream:
             if self.dn is not None:
                 n_wav = self.dn.push_device(src, n_wav, flags, self._den)
                 src = self._den
+            if self.ps is not None:
+                n_wav = self.ps.push_device(src, n_wav, flags, self._psout, semitones=self._shift)
+                src = self._psout
             if self.rs is not None:
                 n_wav = self.rs.push_device(src, n_wav, flags, self._out)
                 src = self._out
@@ -1412,6 +1597,8 @@ class TtsStream:
             self.mt.close()
         if getattr(self, "rs", None) is not None:
             self.rs.close()
+        if getattr(self, "ps", None) is not None:
+            self.ps.close()
         if getattr(self, "dn", None) is not None:
             self.dn.close()
         if getattr(self, "voc", None) is not None:

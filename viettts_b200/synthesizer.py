@@ -7,7 +7,9 @@ single library call per batch (`Engine.tts`), and the WAV writer is built in (th
 `--precision fp16` runs the generator in the fast fp16 mode (Engine.set_precision) for either input.
 `--output-rate R` resamples the audio on the device (Engine.resample) and writes R in the header; `--sample-rate` keeps
 the reference's meaning, the header rate of the unchanged 16 kHz samples.  `--denoise S` removes the generator's bias
-hiss on the device (Engine.denoise, strength S, the default bias) at 16 kHz, before any resampling.  `--loudness L`
+hiss on the device (Engine.denoise, strength S, the default bias) at 16 kHz, before any resampling.  `--pitch P` shifts
+the voice by P semitones on the device (Engine.pitch_shift) at 16 kHz, after --denoise and before any resampling.
+`--loudness L`
 normalizes every output to L LUFS (ITU-R BS.1770-4, Engine.normalize_loudness) at the rate it is written, after
 --denoise and --output-rate, under a true-peak ceiling (`--true-peak`, default -1 dBTP as EBU R128 asks).
 """
@@ -115,6 +117,9 @@ def main(argv=None) -> int:
     parser.add_argument("--denoise", default=None, type=float, metavar="STRENGTH",
                         help="subtract STRENGTH times the generator's bias spectrum (its output for an all-zero mel) from the "
                              "STFT magnitude of the 16 kHz audio on the device, before any --output-rate resampling; >= 0")
+    parser.add_argument("--pitch", default=None, type=float, metavar="SEMITONES",
+                        help="shift the voice's pitch by this many semitones on the device (a peak-locked phase vocoder that "
+                             "keeps the timing), in [-12, 12]; at 16 kHz, after --denoise and before --output-rate")
     parser.add_argument("--loudness", default=None, type=float, metavar="LUFS",
                         help="normalize every output (each --text-file line separately) to this integrated loudness, "
                              "ITU-R BS.1770-4, in [-70, 0]; measured on the device at the output rate, after --denoise and "
@@ -142,6 +147,8 @@ def main(argv=None) -> int:
         parser.error("--reference-dropout and --seed select different dropout streams; give one")
     if args.denoise is not None and not (np.isfinite(args.denoise) and args.denoise >= 0):
         parser.error(f"--denoise {args.denoise}: the strength must be finite and >= 0")
+    if args.pitch is not None and not (np.isfinite(args.pitch) and abs(args.pitch) <= 12.0):
+        parser.error(f"--pitch {args.pitch}: the shift must be finite and lie in [-12, 12] semitones")
     if args.output_rate is not None:
         if args.sample_rate is not None and args.sample_rate != args.output_rate:
             parser.error("--sample-rate only labels the 16 kHz samples and --output-rate resamples them; they disagree")
@@ -174,6 +181,8 @@ def main(argv=None) -> int:
         from .engine import get_engine
         if args.denoise is not None:
             waves = [get_engine().denoise(w, args.denoise) for w in waves]
+        if args.pitch is not None:
+            waves = [get_engine().pitch_shift(w, args.pitch) for w in waves]
         if args.output_rate is not None:
             waves = [get_engine().resample(w, args.output_rate) for w in waves]
         if args.loudness is not None:

@@ -216,7 +216,8 @@ int vtts_debug_pitch_decisions(vtts_ctx* ctx, const float* x_dev, const int32_t*
                                int32_t* dec_dev, void* stream);
 
 /* profiling aid: per-CTA stall counters (SM clocks) of the LAST tensor-core conv launch.
- * Row = CTA, columns: 0 MMA-role total, 1 MMA wait accumulator-free, 2 MMA wait activations, 3 MMA wait
+ * Row = CTA, columns: 0 MMA-role total, 1 epilogue (tc_conv_kernel: after the last wgmma of a tile retires until its
+ * outputs are stored), 2 MMA wait activations, 3 MMA wait
  * weights, 4 weight-producer wait slot, 5 converter wait slot, 6 converter fill, 7 epilogue wait
  * accumulator, 8 epilogue drain.  enable!=0 turns collection on for later launches; the call
  * synchronises, copies (if host_out != NULL) and clears the counters. */

@@ -20,7 +20,7 @@
 //
 // One persistent CTA per SM, 12 warps:
 //   warps 0-7  two consumer warpgroups: each owns MW x 64 rows of the tile, issues the wgmmas of its rows and runs the
-//              epilogue straight from its accumulator registers (+ bias (+ BN/act) (+ residual), fp32 NWC store)
+//              epilogue (+ bias (+ BN/act) (+ residual), fp32 NWC store; the plain one staged through shared memory)
 //   warp  8    weight producer (one lane, cp.async.bulk + expect_tx)
 //   warps 9-11 activation converters: fp32 global -> [mean3] -> leaky_relu -> hi/lo bf16 -> smem
 // A consumer keeps one wgmma group in flight: it releases a ring stage when the NEXT group has been issued and the
@@ -52,7 +52,7 @@ constexpr int PAIR_OVERLAP = 16;              // pair kernel: rows per tile that
 constexpr int NQ = 2;                         // tile-id ring slots
 constexpr int NREADERS = (NCONS + NCONV) / 32;  // warps that read the tile-id ring
 
-template <int N, int MW, int PAIRF>
+template <int N, int MW, int PAIRF, bool STAGED = false>
 struct TcCfg {
   static constexpr int R = 64 * MW * NCWG;                  // rows computed per tile
   static constexpr int R_OUT = R - PAIR_OVERLAP;             // rows stored per tile of the pair kernel
@@ -61,7 +61,15 @@ struct TcCfg {
   static constexpr int W_STAGE = N * 64;                    // bytes of one packed (chunk, tap) weight block
   static constexpr int NW = N == 256 ? 4 : 8;               // weight stages
   static constexpr int NCH2 = PAIRF ? N / 16 : 0;           // 16-channel chunks of the on-chip intermediate
-  static constexpr int SMEM_BYTES = NA * A_STAGE + NW * W_STAGE + NCH2 * A_STAGE + (2 * NA + 2 * NW + 2 * NQ) * 8 + NQ * 4 + 1024;
+  // STAGED: tc_conv_kernel's plain-epilogue staging, per consumer warpgroup: one 64-row block of up to 128 columns
+  // (EPI_NC), rows EPI_LD floats apart, then the N bias values.  EPI_LD = 8 (mod 32) words puts the 4 rows x 8 columns
+  // of a half-warp's accumulator float2 accesses on 32 distinct banks.
+  static constexpr int EPI_NC = N < 128 ? N : 128;
+  static constexpr int EPI_LD = EPI_NC + 8;
+  static constexpr int EPI_WG = 64 * EPI_LD + N;             // floats
+  static constexpr int EPI_STAGE = STAGED ? NCWG * EPI_WG * 4 : 0;   // the register epilogue keeps the L1 it would take
+  static constexpr int SMEM_BYTES =
+      NA * A_STAGE + NW * W_STAGE + NCH2 * A_STAGE + EPI_STAGE + (2 * NA + 2 * NW + 2 * NQ) * 8 + NQ * 4 + 1024;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one CTA");
 };
 
@@ -286,6 +294,13 @@ __device__ __forceinline__ void consume(float (&acc)[MW][N / 2], int wg, uint32_
   }
 }
 
+// 16-byte global -> shared copy that bypasses the registers (cp.async, L1 not allocated)
+__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
 // barriers: a_full[NA] a_empty[NA] w_full[nw] w_empty[nw] q_full[NQ] q_empty[NQ], then the NQ tile ids
 __device__ __forceinline__ void init_barriers(uint64_t* bars, int nw) {
   uint64_t* a_full = bars;
@@ -326,13 +341,15 @@ __device__ __forceinline__ TileQueue tile_queue(uint64_t* bars, int nw) {
 // tanh / relu, residual, partial N tile (acoustic model convs and GEMMs).
 template <int N, int EPI, int MW, bool F16>
 __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_constant__ TcLaunch L) {
-  using Cfg = TcCfg<N, MW, 0>;
+  using Cfg = TcCfg<N, MW, 0, EPI == 0>;
   constexpr int R = Cfg::R, RA = Cfg::RA, NW = Cfg::NW;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* a_st = smem;
   uint8_t* w_st = smem + NA * Cfg::A_STAGE;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(w_st + NW * Cfg::W_STAGE);
+  // [NCWG][EPI_WG]; indexed from smem_raw so that its accesses compile to shared-memory instructions
+  float* epi_st = reinterpret_cast<float*>(smem_raw + (w_st + NW * Cfg::W_STAGE - smem_raw));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(w_st + NW * Cfg::W_STAGE + Cfg::EPI_STAGE);
   uint64_t* a_full = bars;
   uint64_t* a_empty = bars + NA;
   uint64_t* w_full = bars + 2 * NA;
@@ -408,50 +425,130 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
     const int wg = warp >> 2, lane = tid & 31;
     float acc[MW][N / 2];
     Ring ra, rw;
-    long long w_a = 0, w_w = 0;
+    long long w_a = 0, w_w = 0, t_epi = 0;
     const long long t_begin = clock64();
     const int n_valid = (EPI && L.n_valid > 0) ? L.n_valid : N;
     const int post_act = EPI ? L.post_act : 0;
+    // plain epilogue (EPI = 0): this warpgroup's staging rows; the accumulator fragment's row and first column; a
+    // thread's first staged row and float4 column when the warpgroup walks the rows (RPS rows per step, NQ4 steps)
+    constexpr int EPI_NC = Cfg::EPI_NC, EPI_LD = Cfg::EPI_LD, RPS = 128 / (EPI_NC / 4), NQ4 = 64 / RPS;
+    float* stg = epi_st + wg * Cfg::EPI_WG;
+    float* stg_bias = stg + 64 * EPI_LD;
+    const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);
+    const int dr = (tid & 127) / (EPI_NC / 4), dq = (tid & 127) % (EPI_NC / 4);
     READER_TILES
     TILE_LOOP_BEGIN
-      consume<N, MW, RA, NW, true, false, F16>(acc, wg, smem_u32(a_st), a_full, a_empty, ra, smem_u32(w_st), w_full, w_empty, rw, nch, P.k,
-                                               P.dil, L.err, w_a, w_w);
       const size_t out_base = (size_t)b * L.rows_out * L.out_ld;
       const int ostride = P.out_stride, ooff = P.out_off_ph[ph];
-      const int row_w = tau0 + wg * MW * 64 + (warp & 3) * 16 + (lane >> 2);
+      // output row tau is stored while it is valid; the condition is monotone in tau
+      auto row_ok = [&](int tau) { return (ROW_BOUNDS && P.rb) ? tau * ostride + ooff < out_hi : tau < valid; };
+      // cp.async the residual of pass (mt, nh) -- rows tau0 + (wg * MW + mt) * 64..., columns nh * EPI_NC... -- into
+      // the staging rows; wait_pass makes every thread's copies visible to the warpgroup
+      auto fetch_pass = [&](int mt, int nh) {
+        if (P.resid) {
+          const int blk = tau0 + (wg * MW + mt) * 64;
 #pragma unroll
-      for (int mt = 0; mt < MW; ++mt)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int tau = row_w + mt * 64 + 8 * h;
-          if ((ROW_BOUNDS && P.rb) ? tau * ostride + ooff >= out_hi : tau >= valid) continue;
-          const size_t orow = out_base + (size_t)(tau * ostride + ooff) * L.out_ld;
-#pragma unroll
-          for (int jn = 0; jn < N / 8; ++jn) {
-            const int col = jn * 8 + 2 * (lane & 3);
-            if (EPI && col >= n_valid) continue;
-            float2 o = make_float2(acc[mt][jn * 4 + 2 * h], acc[mt][jn * 4 + 2 * h + 1]);
-            const float2 bi = __ldg(reinterpret_cast<const float2*>(P.bias + col));
-            o.x += bi.x; o.y += bi.y;
-            if (EPI && P.bn_mean) {
-              const float2 mu = __ldg(reinterpret_cast<const float2*>(P.bn_mean + col));
-              const float2 iv = __ldg(reinterpret_cast<const float2*>(P.bn_inv + col));
-              const float2 of = __ldg(reinterpret_cast<const float2*>(P.bn_off + col));
-              o.x = (o.x - mu.x) * iv.x + of.x; o.y = (o.y - mu.y) * iv.y + of.y;
-            }
-            if (EPI && post_act == 1) { o.x = tanhf(o.x); o.y = tanhf(o.y); }
-            else if (EPI && post_act == 2) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
-            if (P.resid) {
-              const float2 r = __ldg(reinterpret_cast<const float2*>(P.resid + orow + col));
-              o.x += r.x; o.y += r.y;
-            }
-            *reinterpret_cast<float2*>(P.out + orow + col) = o;
+          for (int i = 0; i < NQ4; ++i) {
+            const int row = i * RPS + dr, tau = blk + row;
+            if (row_ok(tau))
+              cp_async16(stg + row * EPI_LD + dq * 4, P.resid + out_base + ((tau * ostride + ooff) * L.out_ld + nh * EPI_NC + dq * 4));
           }
         }
+        cp_async_commit();
+      };
+      auto wait_pass = [&]() {
+        cp_async_wait_all();
+        named_bar(2 + wg, 128);
+      };
+      if constexpr (EPI == 0) {
+        // the tile's bias (read by the fragments from shared memory, so the compiler keeps no copy of it in registers)
+        // and the first pass's residual are requested before the wgmmas
+        if ((tid & 127) < N / 4) cp_async16(stg_bias + (tid & 127) * 4, P.bias + (tid & 127) * 4);
+        fetch_pass(0, 0);
+      }
+      consume<N, MW, RA, NW, true, false, F16>(acc, wg, smem_u32(a_st), a_full, a_empty, ra, smem_u32(w_st), w_full, w_empty, rw, nch, P.k,
+                                               P.dil, L.err, w_a, w_w);
+      const long long t_epi0 = clock64();
+      if constexpr (EPI == 0) {
+        // Staged through shared memory, one pass per 64-row block of the warpgroup and EPI_NC columns: the pass's
+        // residual rows are copied into the staging rows with cp.async (pass 0's at tile start, so they arrive under
+        // the wgmmas; a later pass's as soon as the previous one has left), the accumulator fragments add bias and the
+        // staged residual in place, and the warpgroup stores the rows in float4 units.  The residual is the layer's
+        // input, read from DRAM: this way a tile waits for it at most once per pass instead of once per fragment pair.
+        wait_pass();
+#pragma unroll
+        for (int mt = 0; mt < MW; ++mt) {
+          if (!row_ok(tau0 + (wg * MW + mt) * 64)) break;   // uniform over the warpgroup: no later row of it is stored
+#pragma unroll
+          for (int nh = 0; nh < N / EPI_NC; ++nh) {
+            if (mt + nh > 0 && P.resid) {
+              fetch_pass(mt, nh);
+              wait_pass();
+            }
+#pragma unroll
+            for (int jn = 0; jn < EPI_NC / 8; ++jn) {
+              const int col = jn * 8 + fc, e = (nh * (EPI_NC / 8) + jn) * 4;
+              const float2 bi = *reinterpret_cast<const float2*>(stg_bias + nh * EPI_NC + col);
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                float2* s = reinterpret_cast<float2*>(stg + (fr + 8 * h) * EPI_LD + col);
+                float2 o = make_float2(acc[mt][e + 2 * h] + bi.x, acc[mt][e + 2 * h + 1] + bi.y);
+                if (P.resid) {
+                  const float2 r = *s;
+                  o.x += r.x; o.y += r.y;
+                }
+                *s = o;
+              }
+            }
+            named_bar(2 + wg, 128);
+            const int blk = tau0 + (wg * MW + mt) * 64;
+#pragma unroll
+            for (int i = 0; i < NQ4; ++i) {
+              const int row = i * RPS + dr, tau = blk + row;
+              if (row_ok(tau))
+                *reinterpret_cast<float4*>(P.out + out_base + ((tau * ostride + ooff) * L.out_ld + nh * EPI_NC + dq * 4)) =
+                    *reinterpret_cast<const float4*>(stg + row * EPI_LD + dq * 4);
+            }
+            named_bar(2 + wg, 128);   // stored before the next pass or tile rewrites the staging rows
+          }
+        }
+      } else {
+        const int row_w = tau0 + wg * MW * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+        for (int mt = 0; mt < MW; ++mt)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int tau = row_w + mt * 64 + 8 * h;
+            if (!row_ok(tau)) continue;
+            const size_t orow = out_base + (size_t)(tau * ostride + ooff) * L.out_ld;
+#pragma unroll
+            for (int jn = 0; jn < N / 8; ++jn) {
+              const int col = jn * 8 + 2 * (lane & 3);
+              if (col >= n_valid) continue;
+              float2 o = make_float2(acc[mt][jn * 4 + 2 * h], acc[mt][jn * 4 + 2 * h + 1]);
+              const float2 bi = __ldg(reinterpret_cast<const float2*>(P.bias + col));
+              o.x += bi.x; o.y += bi.y;
+              if (P.bn_mean) {
+                const float2 mu = __ldg(reinterpret_cast<const float2*>(P.bn_mean + col));
+                const float2 iv = __ldg(reinterpret_cast<const float2*>(P.bn_inv + col));
+                const float2 of = __ldg(reinterpret_cast<const float2*>(P.bn_off + col));
+                o.x = (o.x - mu.x) * iv.x + of.x; o.y = (o.y - mu.y) * iv.y + of.y;
+              }
+              if (post_act == 1) { o.x = tanhf(o.x); o.y = tanhf(o.y); }
+              else if (post_act == 2) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+              if (P.resid) {
+                const float2 r = __ldg(reinterpret_cast<const float2*>(P.resid + orow + col));
+                o.x += r.x; o.y += r.y;
+              }
+              *reinterpret_cast<float2*>(P.out + orow + col) = o;
+            }
+          }
+      }
+      t_epi += clock64() - t_epi0;
     TILE_LOOP_END
     if (L.dbg && tid == 0) {
       long long* d = L.dbg + (size_t)blockIdx.x * 16;
-      d[0] = clock64() - t_begin; d[2] = w_a; d[3] = w_w;
+      d[0] = clock64() - t_begin; d[1] = t_epi; d[2] = w_a; d[3] = w_w;
     }
   }
 #undef TILE_LOOP_BEGIN
@@ -627,7 +724,7 @@ __global__ void pack_w_kernel(const float* __restrict__ w, uint16_t* __restrict_
 
 template <int N, int EPI, int MW, bool F16>
 int launch_cfg(vtts_ctx* ctx, TcLaunch& L, cudaStream_t st) {
-  using Cfg = TcCfg<N, MW, 0>;
+  using Cfg = TcCfg<N, MW, 0, EPI == 0>;
   static bool attr_done_dev[64] = {};   // function attributes are per device (a process may hold contexts on several GPUs)
   if (!attr_done_dev[ctx->device & 63]) {
     VTTS_CUDA(cudaFuncSetAttribute(tc_conv_kernel<N, EPI, MW, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -664,6 +761,14 @@ int launch_n(vtts_ctx* ctx, TcLaunch& L, cudaStream_t st) {
     rb |= L.p[i].rb != nullptr;
   }
   if (rb && generic) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: per-row bounds use the plain epilogue");
+  if (!generic) {
+    // the plain epilogue copies the bias and the residual and stores the output in float4 row segments, at 32-bit
+    // offsets within a batch row
+    if ((int64_t)L.rows_out * L.out_ld > INT32_MAX) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: %d output rows of %d", L.rows_out, L.out_ld);
+    bool aligned = L.out_ld % 4 == 0;
+    for (int i = 0; i < L.nprob; ++i) aligned &= (((uintptr_t)L.p[i].out | (uintptr_t)L.p[i].resid | (uintptr_t)L.p[i].bias) & 15) == 0;
+    if (!aligned) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: the plain epilogue needs 16-byte aligned out / resid rows and bias (out_ld %d)", L.out_ld);
+  }
   if (L.nphase > 4) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: %d phases", L.nphase);
   if (L.nphase > 1 && generic) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: multi-phase tiles use the plain epilogue");
   // fp16 operands serve the generator, whose convs all use the plain epilogue

@@ -12,7 +12,7 @@
 //        sums each output element in a fixed order whatever the window length, so they get the same bits.
 #include <algorithm>
 
-#include "vtts_internal.cuh"
+#include "stream_common.cuh"
 
 namespace {
 
@@ -198,29 +198,18 @@ int vtts_acoustic_stream_begin(vtts_ctx* ctx, vtts_acoustic_stream* as, int nb, 
   VTTS_CUDA(cudaSetDevice(ctx->device));
   VTTS_CUDA(cudaDeviceSynchronize());   // earlier pushes may still read the slots' memory
   // ---- stage the rows, run the one-shot front half, keep each row's zc0 / zc1 in its slot ----
-  const size_t tok_b = (size_t)nb * L * 4, len_b = (size_t)nb * 4, dur_b = (size_t)nb * L * 4, nf_b = (size_t)nb * 4;
-  size_t off = 0;
-  auto take = [&](size_t b) { off = (off + 255) & ~size_t(255); const size_t o = off; off += b; return o; };
-  const size_t o_tok = take(tok_b), o_len = take(len_b), o_dur = take(dur_b), o_nf = take(nf_b);
-  int rc = ctx->ensure_staging(off, off);
+  int rc = ctx->ensure_ws(vtts_acoustic_ws_bytes(nb, L, N));
   if (rc) return rc;
-  rc = ctx->ensure_ws(vtts_acoustic_ws_bytes(nb, L, N));
+  HostStage hs(ctx);
+  const size_t o_tok = hs.in(tokens, (size_t)nb * L * 4), o_len = hs.in(lengths, (size_t)nb * 4);
+  const size_t o_dur = hs.in(dur_frames, (size_t)nb * L * 4), o_nf = hs.in(n_frames, (size_t)nb * 4);
+  rc = hs.upload();
   if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp + o_tok, tokens, tok_b);
-  if (lengths) memcpy(hp + o_len, lengths, len_b);
-  memcpy(hp + o_dur, dur_frames, dur_b);
-  memcpy(hp + o_nf, n_frames, nf_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp, hp, off, cudaMemcpyHostToDevice, st));
+  cudaStream_t st = hs.st;
   const float *zc0 = nullptr, *zc1 = nullptr;
-  rc = vtts_acoustic_front(ctx, (const int32_t*)(dp + o_tok), lengths ? (const int32_t*)(dp + o_len) : nullptr, (const float*)(dp + o_dur),
-                           (const int32_t*)(dp + o_nf), nb, L, N, &zc0, &zc1, st);
-  if (rc) {
-    cudaStreamSynchronize(st);
-    return rc;
-  }
+  rc = vtts_acoustic_front(ctx, hs.dev<const int32_t>(o_tok), lengths ? hs.dev<const int32_t>(o_len) : nullptr, hs.dev<const float>(o_dur),
+                           hs.dev<const int32_t>(o_nf), nb, L, N, &zc0, &zc1, st);
+  if (rc) return rc;
   std::vector<int> pend(nb);
   for (int i = 0; i < nb; ++i) {
     const int s = slots[i], ne = n_emit ? n_emit[i] : n_frames[i];
@@ -234,7 +223,8 @@ int vtts_acoustic_stream_begin(vtts_ctx* ctx, vtts_acoustic_stream* as, int nb, 
       VTTS_CUDA(cudaMemcpyAsync(as->keep + (size_t)s * as->NF * 2 * vc::PRENET, keep + (size_t)i * N * 2 * vc::PRENET,
                                 (size_t)pend[i] * 2 * vc::PRENET, cudaMemcpyHostToDevice, st));
   }
-  VTTS_CUDA(cudaStreamSynchronize(st));
+  rc = hs.finish();
+  if (rc) return rc;
   for (int i = 0; i < nb; ++i) {
     const int s = slots[i];
     as->open[s] = 1;
@@ -318,27 +308,15 @@ int vtts_acoustic_stream_push_host(vtts_ctx* ctx, vtts_acoustic_stream* as, floa
   if (!as || as->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic_stream_push_host: the stream belongs to another context");
   if (!mel || !n_out) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic_stream_push_host: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t mel_b = (size_t)as->S * (as->F + D_A) * vc::MEL * sizeof(float);
-  int rc = ctx->ensure_staging(mel_b, mel_b);
-  if (rc) return rc;
-  cudaStream_t st = ctx->own_stream;
-  rc = vtts_acoustic_stream_push(ctx, as, (float*)ctx->dstage, n_out, st);
-  if (rc) {
-    cudaStreamSynchronize(st);
-    return rc;
-  }
+  const size_t row_b = (size_t)(as->F + D_A) * vc::MEL * sizeof(float);
+  HostStage hs(ctx);
+  const size_t o_mel = hs.out((size_t)as->S * row_b);
+  int rc = hs.upload();
+  if (!rc) rc = vtts_acoustic_stream_push(ctx, as, hs.dev<float>(o_mel), n_out, hs.st);
   // only the rows that received frames are copied back
-  for (int s = 0; s < as->S; ++s) {
-    if (n_out[s] == 0) continue;
-    const size_t o = (size_t)s * (as->F + D_A) * vc::MEL * sizeof(float);
-    VTTS_CUDA(cudaMemcpyAsync((char*)ctx->hpin + o, (char*)ctx->dstage + o, (size_t)n_out[s] * vc::MEL * sizeof(float), cudaMemcpyDeviceToHost, st));
-  }
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  for (int s = 0; s < as->S; ++s) {
-    const size_t o = (size_t)s * (as->F + D_A) * vc::MEL * sizeof(float);
-    if (n_out[s]) memcpy((char*)mel + o, (char*)ctx->hpin + o, (size_t)n_out[s] * vc::MEL * sizeof(float));
-  }
-  return VTTS_OK;
+  for (int s = 0; s < as->S && !rc; ++s)
+    if (n_out[s]) rc = hs.fetch(o_mel + s * row_b, (char*)mel + s * row_b, (size_t)n_out[s] * vc::MEL * sizeof(float));
+  return rc ? rc : hs.finish();
 }
 
 }  // extern "C"

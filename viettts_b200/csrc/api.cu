@@ -6,7 +6,7 @@
 
 #include <dlfcn.h>
 
-#include "vtts_internal.cuh"
+#include "stream_common.cuh"
 
 std::string g_vtts_create_error;
 
@@ -701,9 +701,7 @@ int vtts_debug_read(vtts_ctx* ctx, const char* name, float* host_out, int64_t n_
   return VTTS_OK;
 }
 
-// ---- host-buffer entry points -------------------------------------------------------------------
-// Layout of the staging areas: inputs first, outputs after, every block 256B aligned; the same
-// offsets are used in the pinned host buffer and in the device staging buffer.
+// ---- host-buffer entry points (staged through HostStage) ------------------------------------------
 namespace {
 // true if `p` is page-locked host memory known to CUDA (cudaHostAlloc / cudaHostRegister / torch pin_memory):
 // results can then be copied D2H straight into the caller's buffer instead of through the context's staging area
@@ -715,40 +713,21 @@ bool is_pinned_host(const void* p) {
   }
   return at.type == cudaMemoryTypeHost;
 }
-
-struct Stager {
-  size_t off = 0;
-  size_t take(size_t bytes) {
-    off = (off + 255) & ~size_t(255);
-    size_t o = off;
-    off += bytes;
-    return o;
-  }
-};
 }  // namespace
 
 int vtts_mel2wave_host(vtts_ctx* ctx, const float* mel, const int32_t* n_frames, int B, int T, float* wav) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   if (!mel || !wav || B < 1 || T < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "mel2wave_host: bad argument");
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  Stager s;
-  const size_t mel_b = (size_t)B * T * vc::MEL * 4, nf_b = (size_t)B * 4, wav_b = (size_t)B * T * vc::HOP * 4;
-  const size_t o_mel = s.take(mel_b), o_nf = s.take(nf_b), o_wav = s.take(wav_b);
-  int rc = ctx->ensure_staging(s.off, s.off);
-  if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp + o_mel, mel, mel_b);
-  if (n_frames) memcpy(hp + o_nf, n_frames, nf_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp + o_mel, hp + o_mel, (n_frames ? o_nf + nf_b : mel_b) - o_mel, cudaMemcpyHostToDevice, st));
-  rc = vtts_hifigan_forward(ctx, (const float*)(dp + o_mel), n_frames ? (const int32_t*)(dp + o_nf) : nullptr, B, T, (float*)(dp + o_wav), st);
-  if (rc) return rc;
-  const bool direct = is_pinned_host(wav);
-  VTTS_CUDA(cudaMemcpyAsync(direct ? (void*)wav : (void*)(hp + o_wav), dp + o_wav, wav_b, cudaMemcpyDeviceToHost, st));
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  if (!direct) memcpy(wav, hp + o_wav, wav_b);
-  return VTTS_OK;
+  const size_t wav_b = (size_t)B * T * vc::HOP * 4;
+  HostStage hs(ctx);
+  const size_t o_mel = hs.in(mel, (size_t)B * T * vc::MEL * 4), o_nf = hs.in(n_frames, (size_t)B * 4), o_wav = hs.out(wav_b);
+  int rc = hs.upload();
+  if (!rc)
+    rc = vtts_hifigan_forward(ctx, hs.dev<const float>(o_mel), n_frames ? hs.dev<const int32_t>(o_nf) : nullptr, B, T, hs.dev<float>(o_wav),
+                              hs.st);
+  if (!rc) rc = hs.fetch(o_wav, wav, wav_b, is_pinned_host(wav));
+  return rc ? rc : hs.finish();
 }
 
 static int synth_common(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const float* dur, const int32_t* n_frames,
@@ -759,48 +738,31 @@ static int synth_common(vtts_ctx* ctx, const int32_t* tokens, const int32_t* len
   if (!tokens || !dur || B < 1 || L < 1 || N < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "predict_mel/synthesize_host: bad argument");
   if (mode == VTTS_DROPOUT_MASK && !keep) return ctx->fail(VTTS_ERR_BAD_ARG, "dropout_mode MASK needs keep_mask");
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  Stager s;
-  const size_t tok_b = (size_t)B * L * 4, len_b = (size_t)B * 4, dur_b = (size_t)B * L * 4, nf_b = (size_t)B * 4;
+  const size_t nf_b = (size_t)B * 4;
   const size_t keep_b = mode == VTTS_DROPOUT_MASK ? (size_t)B * N * 2 * vc::PRENET : 0;
   const size_t mel_b = (size_t)B * N * vc::MEL * 4, wav_b = wav_out ? (size_t)B * N * vc::HOP * 4 : 0;
-  const size_t o_tok = s.take(tok_b), o_len = s.take(len_b), o_dur = s.take(dur_b), o_nf = s.take(nf_b), o_keep = s.take(keep_b);
-  const size_t o_nfv = s.take(n_frames_voc ? nf_b : 0);
-  const size_t in_end = s.off;
-  const size_t o_mel = s.take(mel_b), o_wav = s.take(wav_b);
-  int rc = ctx->ensure_staging(s.off, s.off);
+  HostStage hs(ctx);
+  const size_t o_tok = hs.in(tokens, (size_t)B * L * 4), o_len = hs.in(lengths, nf_b), o_dur = hs.in(dur, (size_t)B * L * 4);
+  const size_t o_nf = hs.in(n_frames, nf_b), o_keep = hs.in(keep_b ? keep : nullptr, keep_b), o_nfv = hs.in(n_frames_voc, n_frames_voc ? nf_b : 0);
+  const size_t o_mel = hs.out(mel_b), o_wav = hs.out(wav_b);
+  int rc = hs.upload();
   if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp + o_tok, tokens, tok_b);
-  if (lengths) memcpy(hp + o_len, lengths, len_b);
-  memcpy(hp + o_dur, dur, dur_b);
-  if (n_frames) memcpy(hp + o_nf, n_frames, nf_b);
-  if (keep_b) memcpy(hp + o_keep, keep, keep_b);
-  if (n_frames_voc) memcpy(hp + o_nfv, n_frames_voc, nf_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp, hp, in_end, cudaMemcpyHostToDevice, st));
-  const int32_t* d_len = lengths ? (const int32_t*)(dp + o_len) : nullptr;
-  const int32_t* d_nf = n_frames ? (const int32_t*)(dp + o_nf) : nullptr;
-  rc = vtts_acoustic_forward(ctx, (const int32_t*)(dp + o_tok), d_len, (const float*)(dp + o_dur), d_nf,
-                             keep_b ? (const uint8_t*)(dp + o_keep) : nullptr, mode, seed, B, L, N, (float*)(dp + o_mel), st);
+  const int32_t* d_nf = n_frames ? hs.dev<const int32_t>(o_nf) : nullptr;
+  rc = vtts_acoustic_forward(ctx, hs.dev<const int32_t>(o_tok), lengths ? hs.dev<const int32_t>(o_len) : nullptr, hs.dev<const float>(o_dur),
+                             d_nf, keep_b ? hs.dev<const uint8_t>(o_keep) : nullptr, mode, seed, B, L, N, hs.dev<float>(o_mel), hs.st);
+  if (!rc && mel_out) rc = hs.fetch(o_mel, mel_out, mel_b, is_pinned_host(mel_out));
   if (rc) return rc;
-  const bool mel_direct = mel_out && is_pinned_host(mel_out);
-  const bool wav_direct = wav_out && is_pinned_host(wav_out);
-  if (mel_out) VTTS_CUDA(cudaMemcpyAsync(mel_direct ? (void*)mel_out : (void*)(hp + o_mel), dp + o_mel, mel_b, cudaMemcpyDeviceToHost, st));
   if (wav_out) {
     // the hifigan workspace replaces the acoustic one: its kernels are stream-ordered after the acoustic ones,
     // but growing the workspace frees memory -> make sure `mel` (in dstage) is complete first
     size_t need = vtts_hifigan_ws_bytes(B, N);
-    if (need > ctx->ws_bytes) VTTS_CUDA(cudaStreamSynchronize(st));
-    rc = vtts_hifigan_forward(ctx, (const float*)(dp + o_mel), n_frames_voc ? (const int32_t*)(dp + o_nfv) : d_nf, B, N,
-                              (float*)(dp + o_wav), st);
+    if (need > ctx->ws_bytes) VTTS_CUDA(cudaStreamSynchronize(hs.st));
+    rc = vtts_hifigan_forward(ctx, hs.dev<const float>(o_mel), n_frames_voc ? hs.dev<const int32_t>(o_nfv) : d_nf, B, N, hs.dev<float>(o_wav),
+                              hs.st);
+    if (!rc) rc = hs.fetch(o_wav, wav_out, wav_b, is_pinned_host(wav_out));
     if (rc) return rc;
-    VTTS_CUDA(cudaMemcpyAsync(wav_direct ? (void*)wav_out : (void*)(hp + o_wav), dp + o_wav, wav_b, cudaMemcpyDeviceToHost, st));
   }
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  if (mel_out && !mel_direct) memcpy(mel_out, hp + o_mel, mel_b);
-  if (wav_out && !wav_direct) memcpy(wav_out, hp + o_wav, wav_b);
-  return VTTS_OK;
+  return hs.finish();
 }
 
 int vtts_predict_mel_host(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, const float* dur_frames,
@@ -823,25 +785,15 @@ int vtts_predict_duration_host(vtts_ctx* ctx, const int32_t* tokens, const int32
   if (!ctx) return VTTS_ERR_BAD_ARG;
   if (!tokens || !dur_sec || B < 1 || L < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "predict_duration_host: bad argument");
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  Stager s;
-  const size_t tok_b = (size_t)B * L * 4, len_b = (size_t)B * 4, dur_b = (size_t)B * L * 4;
-  const size_t o_tok = s.take(tok_b), o_len = s.take(len_b), o_dur = s.take(dur_b);
-  int rc = ctx->ensure_staging(s.off, s.off);
-  if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp + o_tok, tokens, tok_b);
-  if (lengths) memcpy(hp + o_len, lengths, len_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp + o_tok, hp + o_tok, tok_b, cudaMemcpyHostToDevice, st));
-  if (lengths) VTTS_CUDA(cudaMemcpyAsync(dp + o_len, hp + o_len, len_b, cudaMemcpyHostToDevice, st));
-  rc = vtts_duration_forward(ctx, (const int32_t*)(dp + o_tok), lengths ? (const int32_t*)(dp + o_len) : nullptr, B, L,
-                             (float*)(dp + o_dur), st);
-  if (rc) return rc;
-  VTTS_CUDA(cudaMemcpyAsync(hp + o_dur, dp + o_dur, dur_b, cudaMemcpyDeviceToHost, st));
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  memcpy(dur_sec, hp + o_dur, dur_b);
-  return VTTS_OK;
+  const size_t dur_b = (size_t)B * L * 4;
+  HostStage hs(ctx);
+  const size_t o_tok = hs.in(tokens, (size_t)B * L * 4), o_len = hs.in(lengths, (size_t)B * 4), o_dur = hs.out(dur_b);
+  int rc = hs.upload();
+  if (!rc)
+    rc = vtts_duration_forward(ctx, hs.dev<const int32_t>(o_tok), lengths ? hs.dev<const int32_t>(o_len) : nullptr, B, L,
+                               hs.dev<float>(o_dur), hs.st);
+  if (!rc) rc = hs.fetch(o_dur, dur_sec, dur_b);
+  return rc ? rc : hs.finish();
 }
 
 namespace {
@@ -865,57 +817,43 @@ int vtts_gta_host(vtts_ctx* ctx, const int16_t* wav_i16, const int32_t* wav_leng
   int rc = vtts_teacher_mode_check(ctx, dropout_mode, B, N);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  Stager s;
-  const size_t wav_b = (size_t)B * S * 2, tok_b = (size_t)B * L * 4, len_b = (size_t)B * 4, dur_b = (size_t)B * L * 4, nf_b = (size_t)B * 4;
+  std::vector<float> dur((size_t)B * L);                              // gta.py:37  durations * sample_rate / (n_fft // 4), float32
+  for (size_t i = 0; i < dur.size(); ++i) dur[i] = (dur_sec[i] * 16000.0f) / 256.0f;
+  std::vector<int32_t> nf(B);                                         // gta.py:74  l = wav_length // hop
+  for (int b = 0; b < B; ++b) {
+    int n = wav_lengths ? wav_lengths[b] / vc::HOP : N;
+    nf[b] = n < 1 ? 1 : (n > N ? N : n);
+  }
   const size_t keep_b = dropout_mode == VTTS_DROPOUT_MASK ? (size_t)B * N * 2 * vc::PRENET : 0;
   const size_t zone_b = dropout_mode == VTTS_DROPOUT_MASK ? (size_t)B * N * 4 * vc::DEC_H : 0;
   const size_t mel_b = (size_t)B * N * vc::MEL * 4;
-  const size_t o_wav = s.take(wav_b), o_tok = s.take(tok_b), o_len = s.take(len_b), o_dur = s.take(dur_b), o_nf = s.take(nf_b);
-  const size_t o_keep = s.take(keep_b), o_zone = s.take(zone_b);
-  const size_t in_end = s.off;
-  const size_t o_gt = s.take(mel_b), o_out = s.take(mel_b);
-  const size_t host_end = s.off;
-  const size_t o_wavf = s.take((size_t)B * S * 4), o_in = s.take(mel_b);      // device-only scratch
-  rc = ctx->ensure_staging(host_end, s.off);
+  HostStage hs(ctx);
+  const size_t o_wav = hs.in(wav_i16, (size_t)B * S * 2), o_tok = hs.in(tokens, (size_t)B * L * 4), o_len = hs.in(lengths, (size_t)B * 4);
+  const size_t o_dur = hs.in(dur.data(), dur.size() * 4), o_nf = hs.in(nf.data(), (size_t)B * 4);
+  const size_t o_keep = hs.in(keep_b ? keep_mask : nullptr, keep_b), o_zone = hs.in(zone_b ? zone_mask : nullptr, zone_b);
+  const size_t o_gt = hs.out(mel_b), o_out = hs.out(mel_b);
+  const size_t o_wavf = hs.scratch((size_t)B * S * 4), o_in = hs.scratch(mel_b);
+  rc = hs.upload();
   if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp + o_wav, wav_i16, wav_b);
-  memcpy(hp + o_tok, tokens, tok_b);
-  if (lengths) memcpy(hp + o_len, lengths, len_b);
-  {
-    float* d = (float*)(hp + o_dur);                                  // gta.py:37  durations * sample_rate / (n_fft // 4), float32
-    for (size_t i = 0; i < (size_t)B * L; ++i) d[i] = (dur_sec[i] * 16000.0f) / 256.0f;
-    int32_t* nf = (int32_t*)(hp + o_nf);                              // gta.py:74  l = wav_length // hop
-    for (int b = 0; b < B; ++b) {
-      int n = wav_lengths ? wav_lengths[b] / vc::HOP : N;
-      nf[b] = n < 1 ? 1 : (n > N ? N : n);
-    }
-  }
-  if (keep_b) memcpy(hp + o_keep, keep_mask, keep_b);
-  if (zone_b) memcpy(hp + o_zone, zone_mask, zone_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp, hp, in_end, cudaMemcpyHostToDevice, st));
-  pcm16_to_float_kernel<<<ctx->sm_count * 4, 256, 0, st>>>((const int16_t*)(dp + o_wav), (float*)(dp + o_wavf), (size_t)B * S);
+  cudaStream_t st = hs.st;
+  pcm16_to_float_kernel<<<ctx->sm_count * 4, 256, 0, st>>>(hs.dev<const int16_t>(o_wav), hs.dev<float>(o_wavf), (size_t)B * S);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
-  rc = vtts_melspec(ctx, (const float*)(dp + o_wavf), B, S, (float*)(dp + o_gt), st);
+  rc = vtts_melspec(ctx, hs.dev<const float>(o_wavf), B, S, hs.dev<float>(o_gt), st);
   if (rc) return rc;
   // inp_mels = concat(zeros[B,1,D], mels[:, :-1]) (gta.py:34-36)
-  VTTS_CUDA(cudaMemsetAsync(dp + o_in, 0, mel_b, st));
+  char* d_in = hs.dev<char>(o_in);
+  VTTS_CUDA(cudaMemsetAsync(d_in, 0, mel_b, st));
   if (N > 1)
-    VTTS_CUDA(cudaMemcpy2DAsync(dp + o_in + vc::MEL * 4, (size_t)N * vc::MEL * 4, dp + o_gt, (size_t)N * vc::MEL * 4,
+    VTTS_CUDA(cudaMemcpy2DAsync(d_in + vc::MEL * 4, (size_t)N * vc::MEL * 4, hs.dev<char>(o_gt), (size_t)N * vc::MEL * 4,
                                 (size_t)(N - 1) * vc::MEL * 4, B, cudaMemcpyDeviceToDevice, st));
-  rc = vtts_acoustic_teacher_forward(ctx, (const int32_t*)(dp + o_tok), lengths ? (const int32_t*)(dp + o_len) : nullptr,
-                                     (const float*)(dp + o_dur), (const int32_t*)(dp + o_nf), (const float*)(dp + o_in),
-                                     keep_b ? (const uint8_t*)(dp + o_keep) : nullptr, zone_b ? (const uint8_t*)(dp + o_zone) : nullptr,
-                                     dropout_mode, seed, B, L, N, nullptr, (float*)(dp + o_out), st);
-  if (rc) return rc;
-  VTTS_CUDA(cudaMemcpyAsync(hp + o_gt, dp + o_gt, 2 * mel_b + (o_out - o_gt - mel_b), cudaMemcpyDeviceToHost, st));
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  if (mel_gt_out_or_null) memcpy(mel_gt_out_or_null, hp + o_gt, mel_b);
-  memcpy(mel2_out, hp + o_out, mel_b);
-  return VTTS_OK;
+  rc = vtts_acoustic_teacher_forward(ctx, hs.dev<const int32_t>(o_tok), lengths ? hs.dev<const int32_t>(o_len) : nullptr,
+                                     hs.dev<const float>(o_dur), hs.dev<const int32_t>(o_nf), hs.dev<const float>(o_in),
+                                     keep_b ? hs.dev<const uint8_t>(o_keep) : nullptr, zone_b ? hs.dev<const uint8_t>(o_zone) : nullptr,
+                                     dropout_mode, seed, B, L, N, nullptr, hs.dev<float>(o_out), st);
+  if (!rc && mel_gt_out_or_null) rc = hs.fetch(o_gt, mel_gt_out_or_null, mel_b);
+  if (!rc) rc = hs.fetch(o_out, mel2_out, mel_b);
+  return rc ? rc : hs.finish();
 }
 
 // text2mel (vietTTS/nat/text2mel.py:85-103) + mel2wave for a batch of token rows, in one call:
@@ -986,22 +924,13 @@ int vtts_melspec_host(vtts_ctx* ctx, const float* wav, int B, int S, float* mel)
   if (!ctx) return VTTS_ERR_BAD_ARG;
   if (!wav || !mel || B < 1 || S < 512 || S % vc::HOP) return ctx->fail(VTTS_ERR_BAD_ARG, "melspec_host: bad argument");
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  Stager s;
-  const size_t wav_b = (size_t)B * S * 4, mel_b = (size_t)B * (S / vc::HOP) * vc::MEL * 4;
-  const size_t o_wav = s.take(wav_b), o_mel = s.take(mel_b);
-  int rc = ctx->ensure_staging(s.off, s.off);
-  if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp + o_wav, wav, wav_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp + o_wav, hp + o_wav, wav_b, cudaMemcpyHostToDevice, st));
-  rc = vtts_melspec(ctx, (const float*)(dp + o_wav), B, S, (float*)(dp + o_mel), st);
-  if (rc) return rc;
-  VTTS_CUDA(cudaMemcpyAsync(hp + o_mel, dp + o_mel, mel_b, cudaMemcpyDeviceToHost, st));
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  memcpy(mel, hp + o_mel, mel_b);
-  return VTTS_OK;
+  const size_t mel_b = (size_t)B * (S / vc::HOP) * vc::MEL * 4;
+  HostStage hs(ctx);
+  const size_t o_wav = hs.in(wav, (size_t)B * S * 4), o_mel = hs.out(mel_b);
+  int rc = hs.upload();
+  if (!rc) rc = vtts_melspec(ctx, hs.dev<const float>(o_wav), B, S, hs.dev<float>(o_mel), hs.st);
+  if (!rc) rc = hs.fetch(o_mel, mel, mel_b);
+  return rc ? rc : hs.finish();
 }
 
 int64_t vtts_launch_count(vtts_ctx* ctx) { return ctx ? ctx->launches : 0; }

@@ -27,7 +27,7 @@
 #include <cstring>
 
 #include "stft_common.cuh"
-#include "vtts_internal.cuh"
+#include "stream_common.cuh"
 
 namespace {
 
@@ -198,27 +198,15 @@ int vtts_denoise_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B,
     for (int b = 0; b < B; ++b)
       if (n_in[b] < 0 || n_in[b] > S) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_host: n[%d]=%d outside [0, %d]", b, n_in[b], S);
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4, n_b = (size_t)B * 4, b_b = (size_t)NB * 4;
-  const size_t o_n = (x_b + 255) & ~size_t(255), o_b = (o_n + n_b + 255) & ~size_t(255), o_y = (o_b + b_b + 255) & ~size_t(255);
-  rc = ctx->ensure_staging(o_y + x_b, o_y + x_b);
-  if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp, x, x_b);
-  if (n_in) memcpy(hp + o_n, n_in, n_b);
-  memcpy(hp + o_b, bias, b_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp, hp, o_b + b_b, cudaMemcpyHostToDevice, st));
-  rc = vtts_denoise(ctx, (const float*)dp, n_in ? (const int32_t*)(dp + o_n) : nullptr, B, S, strength, (const float*)(dp + o_b),
-                    (float*)(dp + o_y), st);
-  if (rc) {
-    cudaStreamSynchronize(st);   // the staging copy must not outlive the call
-    return rc;
-  }
-  VTTS_CUDA(cudaMemcpyAsync(hp + o_y, dp + o_y, x_b, cudaMemcpyDeviceToHost, st));
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  memcpy(y, hp + o_y, x_b);
-  return VTTS_OK;
+  const size_t x_b = (size_t)B * S * 4;
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, (size_t)B * 4), o_b = hs.in(bias, (size_t)NB * 4), o_y = hs.out(x_b);
+  rc = hs.upload();
+  if (!rc)
+    rc = vtts_denoise(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, strength, hs.dev<const float>(o_b),
+                      hs.dev<float>(o_y), hs.st);
+  if (!rc) rc = hs.fetch(o_y, y, x_b);
+  return rc ? rc : hs.finish();
 }
 
 int vtts_denoise_bias(vtts_ctx* ctx, const float* wav_dev, int n, float* bias_dev, void* stream) {
@@ -236,20 +224,15 @@ int vtts_denoise_bias(vtts_ctx* ctx, const float* wav_dev, int n, float* bias_de
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
-struct vtts_denoise_stream {
-  vtts_ctx* ctx = nullptr;
-  int S = 0, F = 0, cap = 0, out_pitch = 0, ws_frames = 0;
+struct vtts_denoise_stream : StreamBase {
+  using StreamBase::StreamBase;
+  int cap = 0, out_pitch = 0, ws_frames = 0;
   float strength = 0.f;
-  void* mem = nullptr;          // windows [S][cap], frame workspace [S][ws_frames][1024], bias [513], then the per-push tables
-  float* win = nullptr;
-  float* ws = nullptr;
-  float* bias = nullptr;
-  DnRow* d_rows = nullptr;
-  int* d_prep = nullptr;
-  // per slot: inputs received since BEGIN, outputs emitted, open, inputs of the last push whose tail has not moved yet
-  std::vector<long long> P, E;
-  std::vector<int> open, pending;
-  std::vector<char> tbl;        // host image of the per-push tables: DnRow [S], then int [S][2]
+  float* win = nullptr;         // windows [S][cap]
+  float* ws = nullptr;          // frame workspace [S][ws_frames][1024]
+  float* bias = nullptr;        // [513]
+  char* d_tbl = nullptr;        // the per-push tables, laid out as their host image tbl: DnRow [S], then int [S][2]
+  std::vector<char> tbl;
 };
 
 int vtts_denoise_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, float strength, const float* bias,
@@ -266,73 +249,39 @@ int vtts_denoise_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_sam
   VTTS_CUDA(cudaSetDevice(ctx->device));
   rc = vtts_fft_tables(ctx);
   if (rc) return rc;
-  vtts_denoise_stream* ds = new vtts_denoise_stream;
-  ds->ctx = ctx;
-  ds->S = max_streams;
-  ds->F = max_chunk_samples;
+  std::unique_ptr<vtts_denoise_stream> ds(new vtts_denoise_stream(ctx, max_streams, max_chunk_samples));
   ds->cap = DN_K + max_chunk_samples;
   // outputs per push: fewer than n_new + 256 before END, at most n_new + 1023 with it (E(P0) >= P0 - 1023)
   ds->out_pitch = max_chunk_samples + DN_LOOKAHEAD;
   // frames per push: outputs [E0, E1) read frames floor((E0 - 511) / 256) .. floor((E1 + 511) / 256)
   ds->ws_frames = (ds->out_pitch + 2 * PAD) / HOP + 2;
   ds->strength = strength;
-  const size_t win_b = ((size_t)max_streams * ds->cap * sizeof(float) + 255) & ~size_t(255);
-  const size_t ws_b = (size_t)max_streams * ds->ws_frames * NF * sizeof(float);
-  const size_t bias_b = ((size_t)NB * sizeof(float) + 255) & ~size_t(255);
-  const size_t rows_b = ((size_t)max_streams * sizeof(DnRow) + 255) & ~size_t(255);
-  const size_t bytes = win_b + ws_b + bias_b + rows_b + (size_t)max_streams * 2 * sizeof(int);
-  cudaError_t e = cudaMalloc(&ds->mem, bytes);
-  if (e == cudaSuccess) e = cudaMemset(ds->mem, 0, bytes);
-  char* base = (char*)ds->mem;
-  if (e == cudaSuccess) e = cudaMemcpy(base + win_b + ws_b, bias, (size_t)NB * sizeof(float), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    if (ds->mem) cudaFree(ds->mem);
-    delete ds;
-    return ctx->fail(e == cudaErrorMemoryAllocation ? VTTS_ERR_OOM : VTTS_ERR_CUDA, "denoise_stream_create: %zu bytes: %s", bytes,
-                     cudaGetErrorString(e));
-  }
-  ds->win = (float*)base;
-  ds->ws = (float*)(base + win_b);
-  ds->bias = (float*)(base + win_b + ws_b);
-  ds->d_rows = (DnRow*)(base + win_b + ws_b + bias_b);
-  ds->d_prep = (int*)(base + win_b + ws_b + bias_b + rows_b);
-  ds->P.assign(max_streams, 0);
-  ds->E.assign(max_streams, 0);
-  ds->open.assign(max_streams, 0);
-  ds->pending.assign(max_streams, 0);
   ds->tbl.assign((size_t)max_streams * (sizeof(DnRow) + 2 * sizeof(int)), 0);
-  *out = ds;
+  rc = stream_alloc(ctx, "denoise_stream_create", *ds, [&](Arena& a) {
+    ds->win = a.take<float>((size_t)max_streams * ds->cap);
+    ds->ws = a.take<float>((size_t)max_streams * ds->ws_frames * NF);
+    ds->bias = a.take<float>(NB);
+    ds->d_tbl = a.take<char>(ds->tbl.size());
+  });
+  if (rc) return rc;
+  VTTS_CUDA(cudaMemcpy(ds->bias, bias, (size_t)NB * sizeof(float), cudaMemcpyHostToDevice));
   *out_pitch = ds->out_pitch;
+  *out = ds.release();
   return VTTS_OK;
 }
 
-int vtts_denoise_stream_destroy(vtts_ctx* ctx, vtts_denoise_stream* ds) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!ds) return VTTS_OK;
-  if (ds->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_stream_destroy: the stream belongs to another context");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  VTTS_CUDA(cudaDeviceSynchronize());   // a push may still be running on the caller's stream
-  cudaFree(ds->mem);
-  delete ds;
-  return VTTS_OK;
-}
+int vtts_denoise_stream_destroy(vtts_ctx* ctx, vtts_denoise_stream* ds) { return stream_destroy(ctx, "denoise_stream_destroy", ds); }
 
 int vtts_denoise_stream_push(vtts_ctx* ctx, vtts_denoise_stream* ds, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
                              float* y_dev, int32_t* n_out, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!ds || ds->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_stream_push: the stream belongs to another context");
-  if (!x_dev || !n_new || !flags || !y_dev || !n_out) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_stream_push: null pointer");
-  const int S = ds->S, F = ds->F;
-  for (int s = 0; s < S; ++s) {
-    if (n_new[s] < 0 || n_new[s] > F) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_stream_push: n_new[%d]=%d outside [0, %d]", s, n_new[s], F);
-    if (flags[s] & ~3u) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_stream_push: flags[%d]=%u (bit0 BEGIN, bit1 END)", s, flags[s]);
-    const bool idle = n_new[s] == 0 && flags[s] == 0;
-    if (!idle && !(flags[s] & 1) && !ds->open[s])
-      return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_stream_push: slot %d is not open (push BEGIN first, also after END)", s);
-  }
+  int rc = stream_args(ctx, "denoise_stream_push", ds, x_dev && n_new && flags && y_dev && n_out);
+  if (!rc) rc = ds->slots.check(ctx, "denoise_stream_push", ds->F, n_new, flags);
+  if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
+  const int S = ds->S;
+  const SlotState& sl = ds->slots;
 
   // ---- host bookkeeping: outputs [E0, E1) of this push and the frames they read ----
   DnRow* rows = reinterpret_cast<DnRow*>(ds->tbl.data());
@@ -340,8 +289,8 @@ int vtts_denoise_stream_push(vtts_ctx* ctx, vtts_denoise_stream* ds, const float
   std::vector<long long> E1(S);
   long long max_out = 0, max_frames = 0;
   for (int s = 0; s < S; ++s) {
-    const bool act = n_new[s] > 0 || flags[s] != 0, begin = flags[s] & 1, end = flags[s] & 2;
-    const long long P0 = begin ? 0 : ds->P[s], E0 = begin ? 0 : ds->E[s], P1 = P0 + n_new[s];
+    const bool act = SlotState::active(n_new, flags, s), begin = flags[s] & 1, end = flags[s] & 2;
+    const long long P0 = begin ? 0 : sl.P[s], E0 = begin ? 0 : sl.E[s], P1 = P0 + n_new[s];
     long long e = E0;
     if (act) e = end ? P1 : std::min(P1, (long long)HOP * std::max(0LL, P1 / HOP - 3));
     E1[s] = e;
@@ -361,56 +310,32 @@ int vtts_denoise_stream_push(vtts_ctx* ctx, vtts_denoise_stream* ds, const float
       return ctx->fail(VTTS_ERR_CUDA, "denoise_stream_push: slot %d needs %d frames / %lld outputs (internal bound %d / %d)", s, r.nfr,
                        r.cnt, ds->ws_frames, ds->out_pitch);
     rows[s] = r;
-    prep[2 * s] = act && !begin ? ds->pending[s] : 0;
-    prep[2 * s + 1] = act ? n_new[s] : 0;
     max_out = std::max(max_out, r.cnt);
     max_frames = std::max(max_frames, (long long)r.nfr);
   }
+  sl.prep(n_new, flags, prep);
 
-  // ---- device: table copies, prep, frames, overlap-add (three launches) ----
+  // ---- device: one table copy, prep, frames, overlap-add (three launches) ----
   // pageable source: the call returns once the table is staged, so ds->tbl may be rewritten by the next push
-  VTTS_CUDA(cudaMemcpyAsync(ds->d_rows, rows, (size_t)S * sizeof(DnRow), cudaMemcpyHostToDevice, st));
-  VTTS_CUDA(cudaMemcpyAsync(ds->d_prep, prep, (size_t)S * 2 * sizeof(int), cudaMemcpyHostToDevice, st));
-  int rc = vtts_stream_window_prep(ctx, ds->win, ds->cap, DN_K, ds->d_prep, x_dev, F, S, st);
+  VTTS_CUDA(cudaMemcpyAsync(ds->d_tbl, ds->tbl.data(), ds->tbl.size(), cudaMemcpyHostToDevice, st));
+  const DnRow* d_rows = reinterpret_cast<const DnRow*>(ds->d_tbl);
+  const int* d_prep = reinterpret_cast<const int*>(ds->d_tbl + (size_t)S * sizeof(DnRow));
+  rc = vtts_stream_window_prep(ctx, ds->win, ds->cap, DN_K, d_prep, x_dev, ds->F, S, st);
   if (rc) return rc;
-  rc = dn_launch(ctx, ds->win, ds->cap, ds->cap, nullptr, ds->d_rows, S, max_frames, max_out, ds->strength, ds->bias, ds->ws, ds->ws_frames,
+  rc = dn_launch(ctx, ds->win, ds->cap, ds->cap, nullptr, d_rows, S, max_frames, max_out, ds->strength, ds->bias, ds->ws, ds->ws_frames,
                  y_dev, ds->out_pitch, st);
   if (rc) return rc;
-
-  // ---- commit the slot state ----
-  for (int s = 0; s < S; ++s) {
-    const bool act = n_new[s] > 0 || flags[s] != 0, begin = flags[s] & 1, end = flags[s] & 2;
-    if (!act) continue;
-    ds->P[s] = (begin ? 0 : ds->P[s]) + n_new[s];
-    ds->E[s] = E1[s];
-    ds->open[s] = !end;
-    ds->pending[s] = end ? 0 : n_new[s];
-  }
+  ds->slots.commit(n_new, flags, E1.data());
   return VTTS_OK;
 }
 
 int vtts_denoise_stream_push_host(vtts_ctx* ctx, vtts_denoise_stream* ds, const float* x, const int32_t* n_new, const uint8_t* flags,
                                   float* y, int32_t* n_out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!ds || ds->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_stream_push_host: the stream belongs to another context");
-  if (!x || !y) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_stream_push_host: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)ds->S * ds->F * 4, y_b = (size_t)ds->S * ds->out_pitch * 4;
-  const size_t o_y = (x_b + 255) & ~size_t(255);
-  int rc = ctx->ensure_staging(o_y + y_b, o_y + y_b);
+  int rc = stream_args(ctx, "denoise_stream_push_host", ds, x && y);
   if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp, x, x_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp, hp, x_b, cudaMemcpyHostToDevice, st));
-  rc = vtts_denoise_stream_push(ctx, ds, (const float*)dp, n_new, flags, (float*)(dp + o_y), n_out, st);
-  if (rc) {
-    cudaStreamSynchronize(st);   // the staging copy must not outlive the call
-    return rc;
-  }
-  VTTS_CUDA(cudaMemcpyAsync(hp + o_y, dp + o_y, y_b, cudaMemcpyDeviceToHost, st));
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  memcpy(y, hp + o_y, y_b);
-  return VTTS_OK;
+  return stream_push_host(ctx, x, (size_t)ds->S * ds->F * 4, y, (size_t)ds->S * ds->out_pitch * 4,
+                          [&](const float* x_dev, float* y_dev, cudaStream_t st) {
+                            return vtts_denoise_stream_push(ctx, ds, x_dev, n_new, flags, y_dev, n_out, st);
+                          });
 }

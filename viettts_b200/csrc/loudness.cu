@@ -31,7 +31,7 @@
 #include <cmath>
 #include <cstring>
 
-#include "vtts_internal.cuh"
+#include "stream_common.cuh"
 
 namespace {
 
@@ -526,25 +526,13 @@ int vtts_loudness_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B
   if (rc) return rc;
   if (!x || !out) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_host: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4, n_b = (size_t)B * 4, o_b = (size_t)B * 16;
-  const size_t o_n = al(x_b), o_o = al(o_n + n_b);
-  rc = ctx->ensure_staging(o_o + o_b, o_o + o_b);
-  if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp, x, x_b);
-  if (n_in) memcpy(hp + o_n, n_in, n_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp, hp, n_in ? o_n + n_b : x_b, cudaMemcpyHostToDevice, st));
-  rc = vtts_loudness(ctx, (const float*)dp, n_in ? (const int32_t*)(dp + o_n) : nullptr, B, S, rate, (float*)(dp + o_o), st);
-  if (rc) {
-    cudaStreamSynchronize(st);   // the staging copy must not outlive the call
-    return rc;
-  }
-  VTTS_CUDA(cudaMemcpyAsync(hp + o_o, dp + o_o, o_b, cudaMemcpyDeviceToHost, st));
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  memcpy(out, hp + o_o, o_b);
-  return VTTS_OK;
+  const size_t o_b = (size_t)B * 16;
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, (size_t)B * S * 4), o_n = hs.in(n_in, (size_t)B * 4), o_o = hs.out(o_b);
+  rc = hs.upload();
+  if (!rc) rc = vtts_loudness(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, rate, hs.dev<float>(o_o), hs.st);
+  if (!rc) rc = hs.fetch(o_o, out, o_b);
+  return rc ? rc : hs.finish();
 }
 
 int vtts_loudness_normalize_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float target, float ceiling,
@@ -557,43 +545,26 @@ int vtts_loudness_normalize_host(vtts_ctx* ctx, const float* x, const int32_t* n
   if (!x || !y) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_normalize_host: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
   const size_t x_b = (size_t)B * S * 4, n_b = (size_t)B * 4;
-  const size_t o_n = al(x_b), o_g = al(o_n + n_b), o_y = al(o_g + n_b);
-  rc = ctx->ensure_staging(o_y + x_b, o_y + x_b);
-  if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp, x, x_b);
-  if (n_in) memcpy(hp + o_n, n_in, n_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp, hp, n_in ? o_n + n_b : x_b, cudaMemcpyHostToDevice, st));
-  rc = vtts_loudness_normalize(ctx, (const float*)dp, n_in ? (const int32_t*)(dp + o_n) : nullptr, B, S, rate, target, ceiling,
-                               (float*)(dp + o_y), (float*)(dp + o_g), st);
-  if (rc) {
-    cudaStreamSynchronize(st);   // the staging copy must not outlive the call
-    return rc;
-  }
-  VTTS_CUDA(cudaMemcpyAsync(hp + o_g, dp + o_g, o_y - o_g + x_b, cudaMemcpyDeviceToHost, st));
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  memcpy(y, hp + o_y, x_b);
-  if (gain_db) memcpy(gain_db, hp + o_g, n_b);
-  return VTTS_OK;
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, n_b), o_g = hs.out(n_b), o_y = hs.out(x_b);
+  rc = hs.upload();
+  if (!rc)
+    rc = vtts_loudness_normalize(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, rate, target, ceiling,
+                                 hs.dev<float>(o_y), hs.dev<float>(o_g), hs.st);
+  if (!rc) rc = hs.fetch(o_y, y, x_b);
+  if (!rc && gain_db) rc = hs.fetch(o_g, gain_db, n_b);
+  return rc ? rc : hs.finish();
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
-struct vtts_loudness_stream {
-  vtts_ctx* ctx = nullptr;
-  int rate = 0, m = 0, S = 0, F = 0, cap = 0, hcap = 0, kpush = 0, upitch = 0, ptiles = 0;
-  void* mem = nullptr;          // windows, e, s, history, state, peak, u, tile maxima, then the per-push tables
-  float* win = nullptr;
+// The shared slot state counts samples in P and, in E, the oversampled outputs the running peak covers.
+struct vtts_loudness_stream : StreamBase {
+  using StreamBase::StreamBase;
+  int rate = 0, m = 0, cap = 0, hcap = 0, kpush = 0, upitch = 0, ptiles = 0;
+  float* win = nullptr;         // windows [S][cap]
   LnBufs w{};
-  LnRow* d_rows = nullptr;
-  RsRow* d_rs = nullptr;
-  int* d_prep = nullptr;
-  // per slot: samples received since BEGIN, oversampled outputs covered by the peak, open, samples of the last push
-  // whose tail has not moved yet
-  std::vector<long long> P, U;
-  std::vector<int> open, pending;
-  std::vector<char> tbl;        // host image of the per-push tables: LnRow [S], RsRow [S], int [S][2]
+  char* d_tbl = nullptr;        // the per-push tables, laid out as their host image tbl: LnRow [S], RsRow [S], int [S][2]
+  std::vector<char> tbl;
 };
 
 int vtts_loudness_stream_lookahead(int rate) {
@@ -612,86 +583,54 @@ int vtts_loudness_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_sa
                      max_streams, max_chunk_samples, max_seconds, 1 << 22, 1 << 20);
   VTTS_CUDA(cudaSetDevice(ctx->device));
   ln_filter(ctx, rate);
-  vtts_loudness_stream* ls = new vtts_loudness_stream;
-  ls->ctx = ctx;
+  std::unique_ptr<vtts_loudness_stream> ls(new vtts_loudness_stream(ctx, max_streams, max_chunk_samples));
   ls->rate = rate;
   ls->m = rate / 10;
-  ls->S = max_streams;
-  ls->F = max_chunk_samples;
   ls->cap = ls->m + max_chunk_samples;
   ls->hcap = 10 * max_seconds;
   ls->kpush = (ls->m - 1 + max_chunk_samples) / ls->m;            // complete sub-blocks one push can bring
   ls->upitch = OS * max_chunk_samples + 10 * OS + 1;              // oversampled outputs one push can cover
   ls->ptiles = (max_chunk_samples + ls->upitch + PEAK_TILE - 1) / PEAK_TILE;
   const size_t S = max_streams, kp = std::max(1, ls->kpush);
-  const size_t win_b = al(S * ls->cap * 4), e_b = al(S * kp * 16), h_b = al(S * ls->hcap * 4), c_b = al(S * 16), pk_b = al(S * 4),
-               u_b = al(S * ls->upitch * 4), pt_b = al(S * ls->ptiles * 4);
-  // the per-push tables follow each other without padding, as in their host image (one copy per push)
-  const size_t r_b = S * sizeof(LnRow), rs_b = S * sizeof(RsRow);
   static_assert(sizeof(LnRow) % 16 == 0 && sizeof(RsRow) % 16 == 0, "table entries keep 16-byte alignment");
-  const size_t bytes = win_b + 2 * e_b + h_b + c_b + pk_b + u_b + pt_b + r_b + rs_b + S * 2 * sizeof(int);
-  cudaError_t e = cudaMalloc(&ls->mem, bytes);
-  if (e == cudaSuccess) e = cudaMemset(ls->mem, 0, bytes);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    if (ls->mem) cudaFree(ls->mem);
-    delete ls;
-    return ctx->fail(e == cudaErrorMemoryAllocation ? VTTS_ERR_OOM : VTTS_ERR_CUDA, "loudness_stream_create: %zu bytes: %s", bytes,
-                     cudaGetErrorString(e));
-  }
-  char* p = (char*)ls->mem;
-  ls->win = (float*)p;                      p += win_b;
-  ls->w.e = (float*)p;                      p += e_b;
-  ls->w.s = (float*)p;                      p += e_b;
-  ls->w.E = (float*)p;                      p += h_b;
-  ls->w.carry = (float*)p;                  p += c_b;
-  ls->w.peak = (float*)p;                   p += pk_b;
-  ls->w.u = (float*)p;                      p += u_b;
-  ls->w.part = (float*)p;                   p += pt_b;
-  ls->d_rows = (LnRow*)p;                   p += r_b;
-  ls->d_rs = (RsRow*)p;                     p += rs_b;
-  ls->d_prep = (int*)p;
+  ls->tbl.assign(S * (sizeof(LnRow) + sizeof(RsRow) + 2 * sizeof(int)), 0);
+  int rc = stream_alloc(ctx, "loudness_stream_create", *ls, [&](Arena& a) {
+    ls->win = a.take<float>(S * ls->cap);
+    ls->w.e = a.take<float>(S * kp * 4);
+    ls->w.s = a.take<float>(S * kp * 4);
+    ls->w.E = a.take<float>(S * ls->hcap);
+    ls->w.carry = a.take<float>(S * 4);
+    ls->w.peak = a.take<float>(S);
+    ls->w.u = a.take<float>(S * ls->upitch);
+    ls->w.part = a.take<float>(S * ls->ptiles);
+    ls->d_tbl = a.take<char>(ls->tbl.size());
+  });
+  if (rc) return rc;
   ls->w.ld_k = (int)kp;
   ls->w.E_ld = ls->hcap;
   ls->w.u_ld = ls->upitch;
   ls->w.part_ld = ls->ptiles;
-  ls->P.assign(S, 0);
-  ls->U.assign(S, 0);
-  ls->open.assign(S, 0);
-  ls->pending.assign(S, 0);
-  ls->tbl.assign(S * (sizeof(LnRow) + sizeof(RsRow) + 2 * sizeof(int)), 0);
-  *out = ls;
+  *out = ls.release();
   return VTTS_OK;
 }
 
-int vtts_loudness_stream_destroy(vtts_ctx* ctx, vtts_loudness_stream* ls) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!ls) return VTTS_OK;
-  if (ls->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_stream_destroy: the stream belongs to another context");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  VTTS_CUDA(cudaDeviceSynchronize());   // a push may still be running on the caller's stream
-  cudaFree(ls->mem);
-  delete ls;
-  return VTTS_OK;
-}
+int vtts_loudness_stream_destroy(vtts_ctx* ctx, vtts_loudness_stream* ls) { return stream_destroy(ctx, "loudness_stream_destroy", ls); }
 
 int vtts_loudness_stream_push(vtts_ctx* ctx, vtts_loudness_stream* ls, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
                               float* out_dev, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!ls || ls->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_stream_push: the stream belongs to another context");
-  if (!x_dev || !n_new || !flags || !out_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_stream_push: null pointer");
-  const int S = ls->S, F = ls->F, m = ls->m;
-  for (int s = 0; s < S; ++s) {
-    if (n_new[s] < 0 || n_new[s] > F) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_stream_push: n_new[%d]=%d outside [0, %d]", s, n_new[s], F);
-    if (flags[s] & ~3u) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_stream_push: flags[%d]=%u (bit0 BEGIN, bit1 END)", s, flags[s]);
-    const bool idle = n_new[s] == 0 && flags[s] == 0;
-    if (!idle && !(flags[s] & 1) && !ls->open[s])
-      return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_stream_push: slot %d is not open (push BEGIN first, also after END)", s);
-    const long long P1 = ((flags[s] & 1) ? 0 : ls->P[s]) + n_new[s];
+  int rc = stream_args(ctx, "loudness_stream_push", ls, x_dev && n_new && flags && out_dev);
+  if (rc) return rc;
+  const int S = ls->S, m = ls->m;
+  const SlotState& sl = ls->slots;
+  rc = sl.check(ctx, "loudness_stream_push", ls->F, n_new, flags, [&](int s) -> int {
+    const long long P1 = ((flags[s] & 1) ? 0 : sl.P[s]) + n_new[s];
     if (P1 / m > ls->hcap)
       return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_stream_push: slot %d would hold %lld samples, more than max_seconds (%d sub-blocks)", s,
                        P1, ls->hcap);
-  }
+    return VTTS_OK;
+  });
+  if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
 
@@ -704,9 +643,9 @@ int vtts_loudness_stream_push(vtts_ctx* ctx, vtts_loudness_stream* ls, const flo
   std::vector<long long> U1(S);
   long long max_k = 0, max_u = 0, max_peak = 0;
   for (int s = 0; s < S; ++s) {
-    const bool act = n_new[s] > 0 || flags[s] != 0, begin = flags[s] & 1, end = flags[s] & 2;
-    const long long P0 = begin ? 0 : ls->P[s], P1 = P0 + (act ? n_new[s] : 0);
-    const long long U0 = begin ? 0 : ls->U[s];
+    const bool act = SlotState::active(n_new, flags, s), begin = flags[s] & 1, end = flags[s] & 2;
+    const long long P0 = begin ? 0 : sl.P[s], P1 = P0 + (act ? n_new[s] : 0);
+    const long long U0 = begin ? 0 : sl.E[s];
     U1[s] = act ? (end ? OS * P1 : std::max(0LL, OS * P1 - half)) : U0;
     LnRow r{};
     r.x0 = P0 - m;
@@ -719,59 +658,36 @@ int vtts_loudness_stream_push(vtts_ctx* ctx, vtts_loudness_stream* ls, const flo
     r.begin = begin;
     rows[s] = r;
     rs[s] = RsRow{P0 - m, std::max(0LL, P0 - m), P1, U0, r.nu, r.nu};
-    prep[2 * s] = act && !begin ? ls->pending[s] : 0;
-    prep[2 * s + 1] = act ? n_new[s] : 0;
     max_k = std::max(max_k, (long long)r.nk);
     max_u = std::max(max_u, r.nu);
     max_peak = std::max(max_peak, r.nx + r.nu);
   }
+  sl.prep(n_new, flags, prep);
   if (max_u > ls->upitch || max_k > ls->w.ld_k)
     return ctx->fail(VTTS_ERR_CUDA, "loudness_stream_push: %lld outputs / %lld sub-blocks (internal bound %d / %d)", max_u, max_k, ls->upitch,
                      ls->w.ld_k);
 
-  // ---- device: table copies, window step, the six measuring launches (seven in all) ----
+  // ---- device: one table copy, window step, the six measuring launches (seven in all) ----
   // pageable source: the call returns once the tables are staged, so ls->tbl may be rewritten by the next push
-  VTTS_CUDA(cudaMemcpyAsync(ls->d_rows, ls->tbl.data(), ls->tbl.size(), cudaMemcpyHostToDevice, st));
-  int rc = vtts_stream_window_prep(ctx, ls->win, ls->cap, m, ls->d_prep, x_dev, F, S, st);
+  VTTS_CUDA(cudaMemcpyAsync(ls->d_tbl, ls->tbl.data(), ls->tbl.size(), cudaMemcpyHostToDevice, st));
+  const LnRow* d_rows = reinterpret_cast<const LnRow*>(ls->d_tbl);
+  const RsRow* d_rs = reinterpret_cast<const RsRow*>(ls->d_tbl + (size_t)S * sizeof(LnRow));
+  const int* d_prep = reinterpret_cast<const int*>(ls->d_tbl + (size_t)S * (sizeof(LnRow) + sizeof(RsRow)));
+  rc = vtts_stream_window_prep(ctx, ls->win, ls->cap, m, d_prep, x_dev, ls->F, S, st);
   if (rc) return rc;
-  rc = ln_measure(ctx, ln_filter(ctx, ls->rate), ls->win, ls->cap, ls->cap, nullptr, ls->d_rows, ls->d_rs, S, max_k, max_u, max_peak, ls->w,
+  rc = ln_measure(ctx, ln_filter(ctx, ls->rate), ls->win, ls->cap, ls->cap, nullptr, d_rows, d_rs, S, max_k, max_u, max_peak, ls->w,
                   out_dev, 0.f, INFINITY, nullptr, nullptr, st);
   if (rc) return rc;
-
-  // ---- commit the slot state ----
-  for (int s = 0; s < S; ++s) {
-    const bool act = n_new[s] > 0 || flags[s] != 0, begin = flags[s] & 1, end = flags[s] & 2;
-    if (!act) continue;
-    ls->P[s] = (begin ? 0 : ls->P[s]) + n_new[s];
-    ls->U[s] = U1[s];
-    ls->open[s] = !end;
-    ls->pending[s] = end ? 0 : n_new[s];
-  }
+  ls->slots.commit(n_new, flags, U1.data());
   return VTTS_OK;
 }
 
 int vtts_loudness_stream_push_host(vtts_ctx* ctx, vtts_loudness_stream* ls, const float* x, const int32_t* n_new, const uint8_t* flags,
                                    float* out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!ls || ls->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_stream_push_host: the stream belongs to another context");
-  if (!x || !out) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_stream_push_host: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)ls->S * ls->F * 4, o_b = (size_t)ls->S * 16;
-  const size_t o_o = al(x_b);
-  int rc = ctx->ensure_staging(o_o + o_b, o_o + o_b);
+  int rc = stream_args(ctx, "loudness_stream_push_host", ls, x && out);
   if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp, x, x_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp, hp, x_b, cudaMemcpyHostToDevice, st));
-  rc = vtts_loudness_stream_push(ctx, ls, (const float*)dp, n_new, flags, (float*)(dp + o_o), st);
-  if (rc) {
-    cudaStreamSynchronize(st);   // the staging copy must not outlive the call
-    return rc;
-  }
-  VTTS_CUDA(cudaMemcpyAsync(hp + o_o, dp + o_o, o_b, cudaMemcpyDeviceToHost, st));
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  memcpy(out, hp + o_o, o_b);
-  return VTTS_OK;
+  return stream_push_host(ctx, x, (size_t)ls->S * ls->F * 4, out, (size_t)ls->S * 16, [&](const float* x_dev, float* out_dev, cudaStream_t st) {
+    return vtts_loudness_stream_push(ctx, ls, x_dev, n_new, flags, out_dev, st);
+  });
 }

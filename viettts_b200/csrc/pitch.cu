@@ -29,7 +29,7 @@
 #include <vector>
 
 #include "stft_common.cuh"
-#include "vtts_internal.cuh"
+#include "stream_common.cuh"
 
 namespace {
 
@@ -397,42 +397,31 @@ int vtts_pitch_shift_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, in
     for (int b = 0; b < B; ++b)
       if (n_in[b] < 0 || n_in[b] > S) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_host: n[%d]=%d outside [0, %d]", b, n_in[b], S);
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4, n_b = (size_t)B * 4;
-  const size_t o_n = (x_b + 255) & ~size_t(255), o_y = (o_n + n_b + 255) & ~size_t(255);
-  rc = ctx->ensure_staging(o_y + x_b, o_y + x_b);
-  if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp, x, x_b);
-  if (n_in) memcpy(hp + o_n, n_in, n_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp, hp, o_n + n_b, cudaMemcpyHostToDevice, st));
-  rc = vtts_pitch_shift(ctx, (const float*)dp, n_in ? (const int32_t*)(dp + o_n) : nullptr, B, S, semitones, (float*)(dp + o_y), st);
-  if (rc) {
-    cudaStreamSynchronize(st);   // the staging copy must not outlive the call
-    return rc;
-  }
-  VTTS_CUDA(cudaMemcpyAsync(hp + o_y, dp + o_y, x_b, cudaMemcpyDeviceToHost, st));
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  memcpy(y, hp + o_y, x_b);
-  return VTTS_OK;
+  const size_t x_b = (size_t)B * S * 4;
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, (size_t)B * 4), o_y = hs.out(x_b);
+  rc = hs.upload();
+  if (!rc)
+    rc = vtts_pitch_shift(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, semitones, hs.dev<float>(o_y),
+                          hs.st);
+  if (!rc) rc = hs.fetch(o_y, y, x_b);
+  return rc ? rc : hs.finish();
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
-struct vtts_pitch_shift_stream {
-  vtts_ctx* ctx = nullptr;
-  int S = 0, F = 0, cap = 0, out_pitch = 0;
+struct vtts_pitch_shift_stream : StreamBase {
+  using StreamBase::StreamBase;
+  int cap = 0, out_pitch = 0;
   PsWs w{};
-  void* mem = nullptr;          // windows [S][cap], the workspace, state [S][2][513], then the per-push tables
-  float* win = nullptr;
-  double* state = nullptr;
-  DnRow* d_rows = nullptr;      // tables: DnRow [S], PsRow [S], int [S][2], one copy per push
-  // per slot: inputs received since BEGIN, outputs emitted, next unscanned frame, first frame and half of the last
-  // push's synthesized-frame buffer, open, inputs of the last push whose tail has not moved yet, shift since BEGIN
-  std::vector<long long> P, E, q, fb;
-  std::vector<int> open, pending, half;
+  float* win = nullptr;         // windows [S][cap]
+  double* state = nullptr;      // [S][2][513]
+  char* d_tbl = nullptr;        // the per-push tables, laid out as their host image tbl: DnRow [S], PsRow [S], int [S][2]
+  // per slot besides the shared state: next unscanned frame, first frame and half of the last push's synthesized-frame
+  // buffer, shift since BEGIN
+  std::vector<long long> q, fb;
+  std::vector<int> half;
   std::vector<float> semis;
-  std::vector<char> tbl;        // host image of the per-push tables
+  std::vector<char> tbl;
 };
 
 int vtts_pitch_shift_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, vtts_pitch_shift_stream** out, int* out_pitch) {
@@ -445,79 +434,42 @@ int vtts_pitch_shift_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk
   VTTS_CUDA(cudaSetDevice(ctx->device));
   int rc = vtts_fft_tables(ctx);
   if (rc) return rc;
-  vtts_pitch_shift_stream* ps = new vtts_pitch_shift_stream;
   const int S = max_streams;
-  ps->ctx = ctx;
-  ps->S = S;
-  ps->F = max_chunk_samples;
+  std::unique_ptr<vtts_pitch_shift_stream> ps(new vtts_pitch_shift_stream(ctx, S, max_chunk_samples));
   ps->cap = PS_K + max_chunk_samples;
   ps->out_pitch = max_chunk_samples + PS_LOOKAHEAD;    // as the denoise stream
   // frames scanned per push: at most n_new / 256 + 3 (with END); the buffer also holds the <= 3 carried frames
   ps->w.fr = max_chunk_samples / HOP + 4;
   ps->w.nbuf = ps->w.fr + 4;
   ps->w.halves = 2;
-  const size_t tbl_b = (size_t)S * (sizeof(DnRow) + sizeof(PsRow) + 2 * sizeof(int));
-  Arena m(nullptr, 0, true);
-  m.take<float>((size_t)S * ps->cap);
-  PsWs w = ps->w;
-  ps_carve(m, w, S);
-  m.take<double>((size_t)S * 2 * NB);
-  m.take<char>(tbl_b);
-  const size_t bytes = m.off;
-  cudaError_t e = cudaMalloc(&ps->mem, bytes);
-  if (e == cudaSuccess) e = cudaMemset(ps->mem, 0, bytes);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    if (ps->mem) cudaFree(ps->mem);
-    delete ps;
-    return ctx->fail(e == cudaErrorMemoryAllocation ? VTTS_ERR_OOM : VTTS_ERR_CUDA, "pitch_shift_stream_create: %zu bytes: %s", bytes,
-                     cudaGetErrorString(e));
-  }
-  Arena a(ps->mem, bytes, false);
-  ps->win = a.take<float>((size_t)S * ps->cap);
-  ps_carve(a, ps->w, S);
-  ps->state = a.take<double>((size_t)S * 2 * NB);
-  ps->d_rows = reinterpret_cast<DnRow*>(a.take<char>(tbl_b));
-  ps->P.assign(S, 0);
-  ps->E.assign(S, 0);
   ps->q.assign(S, 0);
   ps->fb.assign(S, 0);
-  ps->open.assign(S, 0);
-  ps->pending.assign(S, 0);
   ps->half.assign(S, 0);
   ps->semis.assign(S, 0.f);
-  ps->tbl.assign(tbl_b, 0);
-  *out = ps;
+  ps->tbl.assign((size_t)S * (sizeof(DnRow) + sizeof(PsRow) + 2 * sizeof(int)), 0);
+  rc = stream_alloc(ctx, "pitch_shift_stream_create", *ps, [&](Arena& a) {
+    ps->win = a.take<float>((size_t)S * ps->cap);
+    ps_carve(a, ps->w, S);
+    ps->state = a.take<double>((size_t)S * 2 * NB);
+    ps->d_tbl = a.take<char>(ps->tbl.size());
+  });
+  if (rc) return rc;
   *out_pitch = ps->out_pitch;
+  *out = ps.release();
   return VTTS_OK;
 }
 
 int vtts_pitch_shift_stream_destroy(vtts_ctx* ctx, vtts_pitch_shift_stream* ps) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!ps) return VTTS_OK;
-  if (ps->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_destroy: the stream belongs to another context");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  VTTS_CUDA(cudaDeviceSynchronize());   // a push may still be running on the caller's stream
-  cudaFree(ps->mem);
-  delete ps;
-  return VTTS_OK;
+  return stream_destroy(ctx, "pitch_shift_stream_destroy", ps);
 }
 
 int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
                                  const float* semitones, float* y_dev, int32_t* n_out, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!ps || ps->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_push: the stream belongs to another context");
-  if (!x_dev || !n_new || !flags || !y_dev || !n_out) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_push: null pointer");
+  int rc = stream_args(ctx, "pitch_shift_stream_push", ps, x_dev && n_new && flags && y_dev && n_out);
+  if (rc) return rc;
   if (x_dev == y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_push: y must not alias x");
-  const int S = ps->S, F = ps->F;
-  for (int s = 0; s < S; ++s) {
-    if (n_new[s] < 0 || n_new[s] > F)
-      return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_push: n_new[%d]=%d outside [0, %d]", s, n_new[s], F);
-    if (flags[s] & ~3u) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_push: flags[%d]=%u (bit0 BEGIN, bit1 END)", s, flags[s]);
-    const bool idle = n_new[s] == 0 && flags[s] == 0;
-    if (idle) continue;
-    if (!(flags[s] & 1) && !ps->open[s])
-      return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_push: slot %d is not open (push BEGIN first, also after END)", s);
+  rc = ps->slots.check(ctx, "pitch_shift_stream_push", ps->F, n_new, flags, [&](int s) -> int {
     if (flags[s] & 1) {
       if (!semitones) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_push: BEGIN needs the semitones array");
       if (!shift_ok(semitones[s]))
@@ -526,9 +478,13 @@ int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, con
       return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_push: semitones[%d] = %g, but slot %d shifts by %g until END (BEGIN to change it)",
                        s, (double)semitones[s], s, (double)ps->semis[s]);
     }
-  }
+    return VTTS_OK;
+  });
+  if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
+  const int S = ps->S;
+  const SlotState& sl = ps->slots;
 
   // ---- host bookkeeping: outputs [E0, E1), frames [q0, q1) scanned, synthesized-frame buffer [fb, q1) ----
   DnRow* rows = reinterpret_cast<DnRow*>(ps->tbl.data());
@@ -537,8 +493,8 @@ int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, con
   std::vector<long long> E1(S), Q1(S);
   long long max_out = 0, max_nq = 0, max_nsyn = 0;
   for (int s = 0; s < S; ++s) {
-    const bool act = n_new[s] > 0 || flags[s] != 0, begin = flags[s] & 1, end = flags[s] & 2;
-    const long long P0 = begin ? 0 : ps->P[s], E0 = begin ? 0 : ps->E[s], P1 = P0 + n_new[s];
+    const bool act = SlotState::active(n_new, flags, s), begin = flags[s] & 1, end = flags[s] & 2;
+    const long long P0 = begin ? 0 : sl.P[s], E0 = begin ? 0 : sl.E[s], P1 = P0 + n_new[s];
     const float sm = begin ? semitones[s] : ps->semis[s];
     long long e = E0;
     if (act) e = end ? P1 : std::min(P1, (long long)HOP * std::max(0LL, P1 / HOP - 3));
@@ -575,30 +531,29 @@ int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, con
       return ctx->fail(VTTS_ERR_CUDA, "pitch_shift_stream_push: slot %d needs %lld outputs (internal bound %d)", s, r.cnt, ps->out_pitch);
     rows[s] = r;
     prow[s] = p;
-    prep[2 * s] = act && !begin ? ps->pending[s] : 0;
-    prep[2 * s + 1] = act ? n_new[s] : 0;
     max_out = std::max(max_out, r.cnt);
     max_nq = std::max(max_nq, (long long)p.nq);
     max_nsyn = std::max(max_nsyn, (long long)p.nsyn);
   }
+  sl.prep(n_new, flags, prep);
 
   // ---- device: table copy, window step, analysis, phase, synthesis, overlap-add (five launches) ----
   // pageable source: the call returns once the table is staged, so ps->tbl may be rewritten by the next push
-  VTTS_CUDA(cudaMemcpyAsync(ps->d_rows, ps->tbl.data(), ps->tbl.size(), cudaMemcpyHostToDevice, st));
-  const PsRow* d_prow = reinterpret_cast<const PsRow*>(reinterpret_cast<const char*>(ps->d_rows) + (size_t)S * sizeof(DnRow));
-  const int* d_prep = reinterpret_cast<const int*>(reinterpret_cast<const char*>(ps->d_rows) + (size_t)S * (sizeof(DnRow) + sizeof(PsRow)));
-  int rc = vtts_stream_window_prep(ctx, ps->win, ps->cap, PS_K, d_prep, x_dev, F, S, st);
+  VTTS_CUDA(cudaMemcpyAsync(ps->d_tbl, ps->tbl.data(), ps->tbl.size(), cudaMemcpyHostToDevice, st));
+  const DnRow* d_rows = reinterpret_cast<const DnRow*>(ps->d_tbl);
+  const PsRow* d_prow = reinterpret_cast<const PsRow*>(ps->d_tbl + (size_t)S * sizeof(DnRow));
+  const int* d_prep = reinterpret_cast<const int*>(ps->d_tbl + (size_t)S * (sizeof(DnRow) + sizeof(PsRow)));
+  rc = vtts_stream_window_prep(ctx, ps->win, ps->cap, PS_K, d_prep, x_dev, ps->F, S, st);
   if (rc) return rc;
   rc = ps_launch(ctx, ps->win, ps->cap, ps->cap, nullptr, nullptr, d_prow, S, max_nq, max_nsyn, ps->w, ps->state, nullptr, nullptr, 0, st);
   if (rc) return rc;
-  rc = vtts_denoise_ola(ctx, ps->win, ps->cap, ps->cap, nullptr, ps->d_rows, S, max_out, ps->w.syn, 2 * ps->w.nbuf, y_dev, ps->out_pitch,
-                        st);
+  rc = vtts_denoise_ola(ctx, ps->win, ps->cap, ps->cap, nullptr, d_rows, S, max_out, ps->w.syn, 2 * ps->w.nbuf, y_dev, ps->out_pitch, st);
   if (rc) return rc;
 
   // ---- commit the slot state ----
   for (int s = 0; s < S; ++s) {
-    const bool act = n_new[s] > 0 || flags[s] != 0, begin = flags[s] & 1, end = flags[s] & 2;
-    if (!act) continue;
+    if (!SlotState::active(n_new, flags, s)) continue;
+    const bool begin = flags[s] & 1;
     if (begin) ps->semis[s] = semitones[s];
     if (prow[s].nsyn > 0 || prow[s].nq > 0) {
       ps->fb[s] = prow[s].fb;
@@ -608,36 +563,18 @@ int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, con
       ps->half[s] = 0;
     }
     ps->q[s] = Q1[s];
-    ps->P[s] = (begin ? 0 : ps->P[s]) + n_new[s];
-    ps->E[s] = E1[s];
-    ps->open[s] = !end;
-    ps->pending[s] = end ? 0 : n_new[s];
   }
+  ps->slots.commit(n_new, flags, E1.data());
   return VTTS_OK;
 }
 
 int vtts_pitch_shift_stream_push_host(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x, const int32_t* n_new, const uint8_t* flags,
                                       const float* semitones, float* y, int32_t* n_out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!ps || ps->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_push_host: the stream belongs to another context");
-  if (!x || !y) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_push_host: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)ps->S * ps->F * 4, y_b = (size_t)ps->S * ps->out_pitch * 4;
-  const size_t o_y = (x_b + 255) & ~size_t(255);
-  int rc = ctx->ensure_staging(o_y + y_b, o_y + y_b);
+  int rc = stream_args(ctx, "pitch_shift_stream_push_host", ps, x && y);
   if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp, x, x_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp, hp, x_b, cudaMemcpyHostToDevice, st));
-  rc = vtts_pitch_shift_stream_push(ctx, ps, (const float*)dp, n_new, flags, semitones, (float*)(dp + o_y), n_out, st);
-  if (rc) {
-    cudaStreamSynchronize(st);   // the staging copy must not outlive the call
-    return rc;
-  }
-  VTTS_CUDA(cudaMemcpyAsync(hp + o_y, dp + o_y, y_b, cudaMemcpyDeviceToHost, st));
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  memcpy(y, hp + o_y, y_b);
-  return VTTS_OK;
+  return stream_push_host(ctx, x, (size_t)ps->S * ps->F * 4, y, (size_t)ps->S * ps->out_pitch * 4,
+                          [&](const float* x_dev, float* y_dev, cudaStream_t st) {
+                            return vtts_pitch_shift_stream_push(ctx, ps, x_dev, n_new, flags, semitones, y_dev, n_out, st);
+                          });
 }

@@ -20,7 +20,7 @@
 #include <algorithm>
 #include <cmath>
 
-#include "vtts_internal.cuh"
+#include "stream_common.cuh"
 
 namespace {
 
@@ -275,42 +275,26 @@ int vtts_resample_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B
                      RS_MAX_FACTOR);
   if (!x || !y || B < 1 || B > 65535 || S_in < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_host: bad argument");
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S_in * 4, n_b = (size_t)B * 4;
   const size_t y_b = (size_t)B * ceil_div((long long)S_in * r.up, r.down) * 4;
-  const size_t o_n = (x_b + 255) & ~size_t(255), o_y = (o_n + n_b + 255) & ~size_t(255);
-  int rc = ctx->ensure_staging(o_y + y_b, o_y + y_b);
-  if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp, x, x_b);
-  if (n_in) memcpy(hp + o_n, n_in, n_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp, hp, n_in ? o_n + n_b : x_b, cudaMemcpyHostToDevice, st));
-  rc = vtts_resample(ctx, (const float*)dp, n_in ? (const int32_t*)(dp + o_n) : nullptr, B, S_in, in_rate, out_rate, (float*)(dp + o_y), st);
-  if (rc) {
-    cudaStreamSynchronize(st);   // the staging copy must not outlive the call
-    return rc;
-  }
-  VTTS_CUDA(cudaMemcpyAsync(hp + o_y, dp + o_y, y_b, cudaMemcpyDeviceToHost, st));
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  memcpy(y, hp + o_y, y_b);
-  return VTTS_OK;
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, (size_t)B * S_in * 4), o_n = hs.in(n_in, (size_t)B * 4), o_y = hs.out(y_b);
+  int rc = hs.upload();
+  if (!rc)
+    rc = vtts_resample(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S_in, in_rate, out_rate,
+                       hs.dev<float>(o_y), hs.st);
+  if (!rc) rc = hs.fetch(o_y, y, y_b);
+  return rc ? rc : hs.finish();
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
-struct vtts_resample_stream {
-  vtts_ctx* ctx = nullptr;
+struct vtts_resample_stream : StreamBase {
+  using StreamBase::StreamBase;
   RsRatio r{};
-  int S = 0, F = 0, K = 0, cap = 0, out_pitch = 0;
+  int K = 0, cap = 0, out_pitch = 0;
   const float* taps = nullptr;
-  void* mem = nullptr;          // windows [S][cap], then the per-push tables
-  float* win = nullptr;
-  RsRow* d_rows = nullptr;
-  int* d_prep = nullptr;
-  // per slot: inputs received since BEGIN, outputs emitted, open, inputs of the last push whose tail has not moved yet
-  std::vector<long long> P, E;
-  std::vector<int> open, pending;
-  std::vector<char> tbl;        // host image of the per-push tables: RsRow [S], then int [S][2]
+  float* win = nullptr;         // windows [S][cap]
+  char* d_tbl = nullptr;        // the per-push tables, laid out as their host image tbl: RsRow [S], then int [S][2]
+  std::vector<char> tbl;
 };
 
 int vtts_resample_stream_lookahead(int in_rate, int out_rate) {
@@ -338,67 +322,36 @@ int vtts_resample_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_sa
   const float* taps = nullptr;
   int rc = rs_filter(ctx, r, &taps);
   if (rc) return rc;
-  vtts_resample_stream* rs = new vtts_resample_stream;
-  rs->ctx = ctx;
+  std::unique_ptr<vtts_resample_stream> rs(new vtts_resample_stream(ctx, max_streams, max_chunk_samples));
   rs->r = r;
-  rs->S = max_streams;
-  rs->F = max_chunk_samples;
   rs->K = r.T - 1;
   rs->cap = rs->K + max_chunk_samples;
   rs->out_pitch = (int)pitch;
   rs->taps = taps;
-  const size_t win_b = ((size_t)max_streams * rs->cap * sizeof(float) + 255) & ~size_t(255);
-  const size_t rows_b = ((size_t)max_streams * sizeof(RsRow) + 255) & ~size_t(255);
-  const size_t bytes = win_b + rows_b + (size_t)max_streams * 2 * sizeof(int);
-  cudaError_t e = cudaMalloc(&rs->mem, bytes);
-  if (e == cudaSuccess) e = cudaMemset(rs->mem, 0, bytes);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    if (rs->mem) cudaFree(rs->mem);
-    delete rs;
-    return ctx->fail(e == cudaErrorMemoryAllocation ? VTTS_ERR_OOM : VTTS_ERR_CUDA, "resample_stream_create: %zu bytes: %s", bytes,
-                     cudaGetErrorString(e));
-  }
-  rs->win = (float*)rs->mem;
-  rs->d_rows = (RsRow*)((char*)rs->mem + win_b);
-  rs->d_prep = (int*)((char*)rs->mem + win_b + rows_b);
-  rs->P.assign(max_streams, 0);
-  rs->E.assign(max_streams, 0);
-  rs->open.assign(max_streams, 0);
-  rs->pending.assign(max_streams, 0);
   rs->tbl.assign((size_t)max_streams * (sizeof(RsRow) + 2 * sizeof(int)), 0);
-  *out = rs;
+  rc = stream_alloc(ctx, "resample_stream_create", *rs, [&](Arena& a) {
+    rs->win = a.take<float>((size_t)max_streams * rs->cap);
+    rs->d_tbl = a.take<char>(rs->tbl.size());
+  });
+  if (rc) return rc;
   *out_pitch = rs->out_pitch;
+  *out = rs.release();
   return VTTS_OK;
 }
 
-int vtts_resample_stream_destroy(vtts_ctx* ctx, vtts_resample_stream* rs) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!rs) return VTTS_OK;
-  if (rs->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_destroy: the stream belongs to another context");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  VTTS_CUDA(cudaDeviceSynchronize());   // a push may still be running on the caller's stream
-  cudaFree(rs->mem);
-  delete rs;
-  return VTTS_OK;
-}
+int vtts_resample_stream_destroy(vtts_ctx* ctx, vtts_resample_stream* rs) { return stream_destroy(ctx, "resample_stream_destroy", rs); }
 
 int vtts_resample_stream_push(vtts_ctx* ctx, vtts_resample_stream* rs, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
                               float* y_dev, int32_t* n_out, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!rs || rs->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_push: the stream belongs to another context");
-  if (!x_dev || !n_new || !flags || !y_dev || !n_out) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_push: null pointer");
-  const int S = rs->S, F = rs->F;
-  for (int s = 0; s < S; ++s) {
-    if (n_new[s] < 0 || n_new[s] > F) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_push: n_new[%d]=%d outside [0, %d]", s, n_new[s], F);
-    if (flags[s] & ~3u) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_push: flags[%d]=%u (bit0 BEGIN, bit1 END)", s, flags[s]);
-    const bool idle = n_new[s] == 0 && flags[s] == 0;
-    if (!idle && !(flags[s] & 1) && !rs->open[s])
-      return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_push: slot %d is not open (push BEGIN first, also after END)", s);
-  }
+  int rc = stream_args(ctx, "resample_stream_push", rs, x_dev && n_new && flags && y_dev && n_out);
+  if (!rc) rc = rs->slots.check(ctx, "resample_stream_push", rs->F, n_new, flags);
+  if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
+  const int S = rs->S;
   const RsRatio& r = rs->r;
+  const SlotState& sl = rs->slots;
 
   // ---- host bookkeeping: an output is emitted once every input it reads has arrived, i.e. after P inputs (before END)
   // the slot has emitted min(ceil(P * up / down), max(0, floor((P * up - 1 - half) / down) + 1)) outputs ----
@@ -407,8 +360,8 @@ int vtts_resample_stream_push(vtts_ctx* ctx, vtts_resample_stream* rs, const flo
   std::vector<long long> E1(S);
   long long max_out = 0;
   for (int s = 0; s < S; ++s) {
-    const bool act = n_new[s] > 0 || flags[s] != 0, begin = flags[s] & 1, end = flags[s] & 2;
-    const long long P0 = begin ? 0 : rs->P[s], E0 = begin ? 0 : rs->E[s], P1 = P0 + n_new[s];
+    const bool act = SlotState::active(n_new, flags, s), begin = flags[s] & 1, end = flags[s] & 2;
+    const long long P0 = begin ? 0 : sl.P[s], E0 = begin ? 0 : sl.E[s], P1 = P0 + n_new[s];
     long long e = E0;
     if (act) {
       const long long total = ceil_div(P1 * r.up, r.down), v = P1 * r.up - 1 - r.half;
@@ -417,54 +370,30 @@ int vtts_resample_stream_push(vtts_ctx* ctx, vtts_resample_stream* rs, const flo
     E1[s] = e;
     n_out[s] = (int32_t)(e - E0);
     rows[s] = RsRow{P0 - rs->K, std::max(0LL, P0 - rs->K), P1, E0, e - E0, e - E0};
-    prep[2 * s] = act && !begin ? rs->pending[s] : 0;
-    prep[2 * s + 1] = act ? n_new[s] : 0;
     max_out = std::max(max_out, e - E0);
   }
+  sl.prep(n_new, flags, prep);
 
   // ---- device: one table copy, prep, resample ----
   // pageable source: the call returns once the table is staged, so rs->tbl may be rewritten by the next push
-  VTTS_CUDA(cudaMemcpyAsync(rs->d_rows, rows, (size_t)S * sizeof(RsRow), cudaMemcpyHostToDevice, st));
-  VTTS_CUDA(cudaMemcpyAsync(rs->d_prep, prep, (size_t)S * 2 * sizeof(int), cudaMemcpyHostToDevice, st));
-  int rc = vtts_stream_window_prep(ctx, rs->win, rs->cap, rs->K, rs->d_prep, x_dev, F, S, st);
+  VTTS_CUDA(cudaMemcpyAsync(rs->d_tbl, rs->tbl.data(), rs->tbl.size(), cudaMemcpyHostToDevice, st));
+  const RsRow* d_rows = reinterpret_cast<const RsRow*>(rs->d_tbl);
+  const int* d_prep = reinterpret_cast<const int*>(rs->d_tbl + (size_t)S * sizeof(RsRow));
+  rc = vtts_stream_window_prep(ctx, rs->win, rs->cap, rs->K, d_prep, x_dev, rs->F, S, st);
   if (rc) return rc;
-  rc = rs_launch(ctx, r, rs->taps, rs->win, rs->cap, rs->cap, nullptr, rs->d_rows, S, 0, max_out, y_dev, rs->out_pitch, st);
+  rc = rs_launch(ctx, r, rs->taps, rs->win, rs->cap, rs->cap, nullptr, d_rows, S, 0, max_out, y_dev, rs->out_pitch, st);
   if (rc) return rc;
-
-  // ---- commit the slot state ----
-  for (int s = 0; s < S; ++s) {
-    const bool act = n_new[s] > 0 || flags[s] != 0, begin = flags[s] & 1, end = flags[s] & 2;
-    if (!act) continue;
-    rs->P[s] = (begin ? 0 : rs->P[s]) + n_new[s];
-    rs->E[s] = E1[s];
-    rs->open[s] = !end;
-    rs->pending[s] = end ? 0 : n_new[s];
-  }
+  rs->slots.commit(n_new, flags, E1.data());
   return VTTS_OK;
 }
 
 int vtts_resample_stream_push_host(vtts_ctx* ctx, vtts_resample_stream* rs, const float* x, const int32_t* n_new, const uint8_t* flags,
                                    float* y, int32_t* n_out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!rs || rs->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_push_host: the stream belongs to another context");
-  if (!x || !y) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_push_host: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)rs->S * rs->F * 4, y_b = (size_t)rs->S * rs->out_pitch * 4;
-  const size_t o_y = (x_b + 255) & ~size_t(255);
-  int rc = ctx->ensure_staging(o_y + y_b, o_y + y_b);
+  int rc = stream_args(ctx, "resample_stream_push_host", rs, x && y);
   if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp, x, x_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp, hp, x_b, cudaMemcpyHostToDevice, st));
-  rc = vtts_resample_stream_push(ctx, rs, (const float*)dp, n_new, flags, (float*)(dp + o_y), n_out, st);
-  if (rc) {
-    cudaStreamSynchronize(st);   // the staging copy must not outlive the call
-    return rc;
-  }
-  VTTS_CUDA(cudaMemcpyAsync(hp + o_y, dp + o_y, y_b, cudaMemcpyDeviceToHost, st));
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  memcpy(y, hp + o_y, y_b);
-  return VTTS_OK;
+  return stream_push_host(ctx, x, (size_t)rs->S * rs->F * 4, y, (size_t)rs->S * rs->out_pitch * 4,
+                          [&](const float* x_dev, float* y_dev, cudaStream_t st) {
+                            return vtts_resample_stream_push(ctx, rs, x_dev, n_new, flags, y_dev, n_out, st);
+                          });
 }

@@ -16,7 +16,7 @@
 // and copies the new mel frames in.
 #include <algorithm>
 
-#include "vtts_internal.cuh"
+#include "stream_common.cuh"
 
 using namespace hgpk;
 
@@ -194,16 +194,12 @@ int ci_rb(int i, int m, int which, int j) { return 1 + 19 * i + 1 + m * 6 + whic
 
 }  // namespace
 
-struct vtts_vocoder_stream {
-  vtts_ctx* ctx = nullptr;
-  int S = 0, F = 0;
+// The shared slot state counts mel frames: received since BEGIN in P, emitted in E.
+struct vtts_vocoder_stream : StreamBase {
+  using StreamBase::StreamBase;
   int cap[NRATE] = {};
-  void* mem = nullptr;          // every window, then the tensor table
-  StreamTen ten[NTEN];
+  StreamTen ten[NTEN];          // every window, then their device copy d_ten in the same allocation
   StreamTen* d_ten = nullptr;
-  // per slot: frames received since BEGIN, frames emitted, open (BEGIN seen, END not yet), frames of the last push whose
-  // tail has not been moved to the front yet
-  std::vector<int> P, emitted, open, pending;
   std::vector<int> tbl;         // host image of the per-push bounds table
 };
 
@@ -219,10 +215,7 @@ int vtts_vocoder_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_fra
                      max_chunk_frames);
   VTTS_CUDA(cudaSetDevice(ctx->device));
   const Plan& pl = plan();
-  vtts_vocoder_stream* vs = new vtts_vocoder_stream;
-  vs->ctx = ctx;
-  vs->S = max_streams;
-  vs->F = max_chunk_frames;
+  std::unique_ptr<vtts_vocoder_stream> vs(new vtts_vocoder_stream(ctx, max_streams, max_chunk_frames));
   for (int r = 0; r < NRATE; ++r) vs->cap[r] = pl.lead[r] + pl.rate[r] * max_chunk_frames;
   // window shapes: channels, rate index, lag
   auto shape = [&](int t, int C, int ri, int lag) { vs->ten[t] = StreamTen{nullptr, C, vs->cap[ri], pl.lead[ri] - lag, pl.rate[ri]}; };
@@ -236,65 +229,32 @@ int vtts_vocoder_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_fra
         shape(ti_y(i, j, m), C, i + 1, pl.lag_y[i][j][m]);
       }
   }
-  size_t bytes = 0;
-  std::vector<size_t> off(NTEN);
-  for (int t = 0; t < NTEN; ++t) {
-    off[t] = bytes;
-    bytes += ((size_t)max_streams * vs->ten[t].cap * vs->ten[t].C * sizeof(float) + 255) & ~size_t(255);
-  }
-  const size_t ten_off = bytes;
-  bytes += sizeof(vs->ten);
-  cudaError_t e = cudaMalloc(&vs->mem, bytes);
-  if (e == cudaSuccess) e = cudaMemset(vs->mem, 0, bytes);
-  if (e == cudaSuccess) {
-    for (int t = 0; t < NTEN; ++t) vs->ten[t].p = reinterpret_cast<float*>((char*)vs->mem + off[t]);
-    vs->d_ten = reinterpret_cast<StreamTen*>((char*)vs->mem + ten_off);
-    e = cudaMemcpy(vs->d_ten, vs->ten, sizeof(vs->ten), cudaMemcpyHostToDevice);
-  }
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    if (vs->mem) cudaFree(vs->mem);
-    delete vs;
-    return ctx->fail(e == cudaErrorMemoryAllocation ? VTTS_ERR_OOM : VTTS_ERR_CUDA, "vocoder_stream_create: %zu bytes of windows: %s", bytes,
-                     cudaGetErrorString(e));
-  }
-  vs->P.assign(max_streams, 0);
-  vs->emitted.assign(max_streams, 0);
-  vs->open.assign(max_streams, 0);
-  vs->pending.assign(max_streams, 0);
-  *out = vs;
+  int rc = stream_alloc(ctx, "vocoder_stream_create", *vs, [&](Arena& a) {
+    for (int t = 0; t < NTEN; ++t) vs->ten[t].p = a.take<float>((size_t)max_streams * vs->ten[t].cap * vs->ten[t].C);
+    vs->d_ten = a.take<StreamTen>(NTEN);
+  });
+  if (rc) return rc;
+  VTTS_CUDA(cudaMemcpy(vs->d_ten, vs->ten, sizeof(vs->ten), cudaMemcpyHostToDevice));
+  *out = vs.release();
   return VTTS_OK;
 }
 
-int vtts_vocoder_stream_destroy(vtts_ctx* ctx, vtts_vocoder_stream* vs) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!vs) return VTTS_OK;
-  if (vs->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "vocoder_stream_destroy: the stream belongs to another context");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  VTTS_CUDA(cudaDeviceSynchronize());   // a push may still be running on the caller's stream
-  cudaFree(vs->mem);
-  delete vs;
-  return VTTS_OK;
-}
+int vtts_vocoder_stream_destroy(vtts_ctx* ctx, vtts_vocoder_stream* vs) { return stream_destroy(ctx, "vocoder_stream_destroy", vs); }
 
 int vtts_vocoder_stream_push(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float* mel_dev, const int32_t* n_new, const uint8_t* flags,
                              float* wav_dev, int32_t* n_out, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!vs || vs->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "vocoder_stream_push: the stream belongs to another context");
-  if (!mel_dev || !n_new || !flags || !wav_dev || !n_out) return ctx->fail(VTTS_ERR_BAD_ARG, "vocoder_stream_push: null pointer");
+  int rc = stream_args(ctx, "vocoder_stream_push", vs, mel_dev && n_new && flags && wav_dev && n_out);
+  if (rc) return rc;
   if (!ctx->hg.loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "vocoder_stream_push: hifigan weights not loaded");
   if (ctx->precision == VTTS_PRECISION_FP32)
     return ctx->fail(VTTS_ERR_BAD_ARG, "vocoder_stream_push: the strict fp32 mode has no streaming path; use bf16x3 or fp16");
   const int S = vs->S, F = vs->F;
   const Plan& pl = plan();
   const int D = pl.D, wav_ld = vc::HOP * (F + D);
-  for (int s = 0; s < S; ++s) {
-    if (n_new[s] < 0 || n_new[s] > F) return ctx->fail(VTTS_ERR_BAD_ARG, "vocoder_stream_push: n_new[%d]=%d outside [0, %d]", s, n_new[s], F);
-    if (flags[s] & ~3u) return ctx->fail(VTTS_ERR_BAD_ARG, "vocoder_stream_push: flags[%d]=%u (bit0 BEGIN, bit1 END)", s, flags[s]);
-    const bool idle = n_new[s] == 0 && flags[s] == 0;
-    if (!idle && !(flags[s] & 1) && !vs->open[s])
-      return ctx->fail(VTTS_ERR_BAD_ARG, "vocoder_stream_push: slot %d is not open (push BEGIN first, also after END)", s);
-  }
+  SlotState& sl = vs->slots;
+  rc = sl.check(ctx, "vocoder_stream_push", F, n_new, flags);
+  if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
 
@@ -304,7 +264,7 @@ int vtts_vocoder_stream_push(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float
     act[s] = n_new[s] > 0 || flags[s] != 0;
     end[s] = (flags[s] & 2) != 0;
     nn[s] = n_new[s];
-    P0[s] = (flags[s] & 1) ? 0 : vs->P[s];
+    P0[s] = (flags[s] & 1) ? 0 : (int)sl.P[s];
   }
   // table layout: [NCONV][S][3] conv bounds, [S][4] conv_post, [S][3] prep
   const size_t o_post = (size_t)NCONV * S * 3, o_prep = o_post + (size_t)S * 4, n_tbl = o_prep + (size_t)S * 3;
@@ -336,12 +296,14 @@ int vtts_vocoder_stream_push(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float
       }
   }
   std::vector<int> emit(S, 0), P1(S);
+  std::vector<long long> E1(S);
   int post_max = 0;
   for (int s = 0; s < S; ++s) {
     P1[s] = P0[s] + nn[s];
-    const int e_old = (flags[s] & 1) ? 0 : vs->emitted[s];
+    const int e_old = (flags[s] & 1) ? 0 : (int)sl.E[s];
     const int e_new = !act[s] ? e_old : (end[s] ? P1[s] : std::max(e_old, P1[s] - D));
     emit[s] = e_new - e_old;
+    E1[s] = e_new;
     if (act[s]) {
       const int L = pl.lead[4];
       int* r = tb + o_post + (size_t)s * 4;
@@ -353,12 +315,12 @@ int vtts_vocoder_stream_push(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float
     }
     int* q = tb + o_prep + (size_t)s * 3;
     if (flags[s] & 1) q[0] = 1;
-    else if (act[s] && vs->pending[s] > 0) { q[0] = 2; q[1] = vs->pending[s]; }
+    else if (act[s] && sl.pending[s] > 0) { q[0] = 2; q[1] = sl.pending[s]; }
     q[2] = nn[s];
   }
 
   // ---- device: one table copy, prep, conv_pre, four stages, conv_post ----
-  int rc = ctx->ensure_ws(n_tbl * sizeof(int) + 256);
+  rc = ctx->ensure_ws(n_tbl * sizeof(int) + 256);
   if (rc) return rc;
   int* dtb = reinterpret_cast<int*>(ctx->ws);
   // pageable source: the call returns once the table is staged, so vs->tbl may be rewritten by the next push
@@ -448,41 +410,18 @@ int vtts_vocoder_stream_push(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float
     VTTS_CUDA(cudaGetLastError());
   }
 
-  // ---- commit the slot state ----
-  for (int s = 0; s < S; ++s) {
-    n_out[s] = emit[s];
-    if (!act[s]) continue;
-    vs->P[s] = P1[s];
-    vs->emitted[s] = ((flags[s] & 1) ? 0 : vs->emitted[s]) + emit[s];
-    vs->open[s] = !end[s];
-    vs->pending[s] = end[s] ? 0 : nn[s];
-  }
+  for (int s = 0; s < S; ++s) n_out[s] = emit[s];
+  sl.commit(n_new, flags, E1.data());
   return VTTS_OK;
 }
 
 int vtts_vocoder_stream_push_host(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float* mel, const int32_t* n_new, const uint8_t* flags,
                                   float* wav, int32_t* n_out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!vs || vs->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "vocoder_stream_push_host: the stream belongs to another context");
-  if (!mel || !wav) return ctx->fail(VTTS_ERR_BAD_ARG, "vocoder_stream_push_host: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t mel_b = (size_t)vs->S * vs->F * vc::MEL * 4;
-  const size_t wav_b = (size_t)vs->S * vc::HOP * (vs->F + plan().D) * 4;
-  const size_t o_wav = (mel_b + 255) & ~size_t(255);
-  int rc = ctx->ensure_staging(o_wav + wav_b, o_wav + wav_b);
+  int rc = stream_args(ctx, "vocoder_stream_push_host", vs, mel && wav);
   if (rc) return rc;
-  char* hp = (char*)ctx->hpin;
-  char* dp = (char*)ctx->dstage;
-  cudaStream_t st = ctx->own_stream;
-  memcpy(hp, mel, mel_b);
-  VTTS_CUDA(cudaMemcpyAsync(dp, hp, mel_b, cudaMemcpyHostToDevice, st));
-  rc = vtts_vocoder_stream_push(ctx, vs, (const float*)dp, n_new, flags, (float*)(dp + o_wav), n_out, st);
-  if (rc) {
-    cudaStreamSynchronize(st);   // the staging copy must not outlive the call
-    return rc;
-  }
-  VTTS_CUDA(cudaMemcpyAsync(hp + o_wav, dp + o_wav, wav_b, cudaMemcpyDeviceToHost, st));
-  VTTS_CUDA(cudaStreamSynchronize(st));
-  memcpy(wav, hp + o_wav, wav_b);
-  return VTTS_OK;
+  return stream_push_host(ctx, mel, (size_t)vs->S * vs->F * vc::MEL * 4, wav, (size_t)vs->S * vc::HOP * (vs->F + plan().D) * 4,
+                          [&](const float* mel_dev, float* wav_dev, cudaStream_t st) {
+                            return vtts_vocoder_stream_push(ctx, vs, mel_dev, n_new, flags, wav_dev, n_out, st);
+                          });
 }

@@ -92,6 +92,26 @@ def _np(a, dtype, shape=None, what="array"):
     return a
 
 
+def _wav_rows(wav):
+    """(x f32 [B,S], one): a host [S] or [B,S] array as rows, and whether it was a single row"""
+    x = _np(wav, np.float32)
+    one = x.ndim == 1
+    x = x[None] if one else x
+    if x.ndim != 2:
+        raise ValueError(f"wav must be [S] or [B,S], got {np.shape(wav)}")
+    return x, one
+
+
+def _out_tensor(out, shape, device, what="out"):
+    """`out` checked to be a contiguous float32 tensor of `shape`, or a new one on `device`"""
+    import torch
+    if out is None:
+        return torch.empty(shape, dtype=torch.float32, device=device)
+    if tuple(out.shape) != shape or out.dtype != torch.float32 or not out.is_contiguous():
+        raise ValueError(f"{what} must be contiguous float32 [{', '.join(map(str, shape))}]")
+    return out
+
+
 class Engine:
     """A context on one H100.  Not thread-safe (like the C context)."""
 
@@ -691,10 +711,8 @@ class Engine:
         down is out_rate / in_rate in lowest terms (each <= 1024).  lengths int [B]: row b holds lengths[b] samples,
         and its outputs past ceil(lengths[b] * up / down) are 0.  Equals scipy.signal.resample_poly(x, up, down) up to
         fp32 rounding; in_rate == out_rate is a copy."""
-        x = _np(wav, np.float32)
-        one = x.ndim == 1
-        x = x[None] if one else x
-        if x.ndim != 2 or x.shape[1] < 1:
+        x, one = _wav_rows(wav)
+        if x.shape[1] < 1:
             raise ValueError(f"wav must be [S] or [B,S], got {np.shape(wav)}")
         B, S = x.shape
         lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
@@ -709,10 +727,7 @@ class Engine:
         assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
         B, S = x_t.shape
         n = resample_length(S, in_rate, out_rate)
-        if out is None:
-            out = torch.empty((B, n), dtype=torch.float32, device=x_t.device)
-        elif tuple(out.shape) != (B, n) or out.dtype != torch.float32 or not out.is_contiguous():
-            raise ValueError(f"out must be contiguous float32 [{B}, {n}]")
+        out = _out_tensor(out, (B, n), x_t.device)
         st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
         self._ck(self.lib.vtts_resample(self.h, _ptr(x_t), _ptr(lengths_t), B, S, int(in_rate), int(out_rate), _ptr(out), st))
         return out
@@ -760,11 +775,7 @@ class Engine:
         lengths int [B] in [0, S]: row b holds lengths[b] samples and its outputs past them are 0.  bias f32 [513]
         (default: `denoiser_bias()`)."""
         strength = _strength(strength)
-        x = _np(wav, np.float32)
-        one = x.ndim == 1
-        x = x[None] if one else x
-        if x.ndim != 2:
-            raise ValueError(f"wav must be [S] or [B,S], got {np.shape(wav)}")
+        x, one = _wav_rows(wav)
         B, S = x.shape
         lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
         if S == 0 or B == 0:
@@ -785,10 +796,7 @@ class Engine:
             bias_t = torch.from_numpy(self._bias_arg(None)).to(x_t.device)
         elif tuple(bias_t.shape) != (DENOISE_BINS,) or bias_t.dtype != torch.float32 or not bias_t.is_contiguous():
             raise ValueError(f"bias_t must be contiguous float32 [{DENOISE_BINS}]")
-        if out is None:
-            out = torch.empty((B, S), dtype=torch.float32, device=x_t.device)
-        elif tuple(out.shape) != (B, S) or out.dtype != torch.float32 or not out.is_contiguous():
-            raise ValueError(f"out must be contiguous float32 [{B}, {S}]")
+        out = _out_tensor(out, (B, S), x_t.device)
         st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
         self._ck(self.lib.vtts_denoise(self.h, _ptr(x_t), _ptr(lengths_t), B, S, strength, _ptr(bias_t), _ptr(out), st))
         return out
@@ -805,11 +813,7 @@ class Engine:
         fp32(2^(s / 12)) with its phase kept coherent across frames (n_fft 1024, hop 256); the timing of every sample is
         kept.  semitones: a scalar or one value per row, finite and in [-12, 12]; rows with 0 and rows of <= 512 samples
         are copied.  lengths int [B] in [0, S]: row b holds lengths[b] samples and its outputs past them are 0."""
-        x = _np(wav, np.float32)
-        one = x.ndim == 1
-        x = x[None] if one else x
-        if x.ndim != 2:
-            raise ValueError(f"wav must be [S] or [B,S], got {np.shape(wav)}")
+        x, one = _wav_rows(wav)
         B, S = x.shape
         sem = _semitones(semitones, B)
         lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
@@ -826,10 +830,7 @@ class Engine:
         assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
         B, S = x_t.shape
         sem = _semitones(semitones, B)
-        if out is None:
-            out = torch.empty((B, S), dtype=torch.float32, device=x_t.device)
-        elif tuple(out.shape) != (B, S) or out.dtype != torch.float32 or not out.is_contiguous():
-            raise ValueError(f"out must be contiguous float32 [{B}, {S}]")
+        out = _out_tensor(out, (B, S), x_t.device)
         st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
         self._ck(self.lib.vtts_pitch_shift(self.h, _ptr(x_t), _ptr(lengths_t), B, S, _ptr(sem), _ptr(out), st))
         return out
@@ -858,11 +859,7 @@ class Engine:
         arrays (scalars for a 1-D input): integrated, momentary and short-term loudness in LUFS (-inf where undefined) and
         the true peak in dBTP (4x oversampled by resample_poly).  lengths int [B] in [0, S]."""
         rate = _loudness_rate(rate)
-        x = _np(wav, np.float32)
-        one = x.ndim == 1
-        x = x[None] if one else x
-        if x.ndim != 2:
-            raise ValueError(f"wav must be [S] or [B,S], got {np.shape(wav)}")
+        x, one = _wav_rows(wav)
         B, S = x.shape
         lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
         out = np.full((B, 4), -np.inf, np.float32)
@@ -877,11 +874,7 @@ class Engine:
         outputs past lengths[b] are 0.  target in [-70, 0] LUFS."""
         rate = _loudness_rate(rate)
         target, ceiling = _loudness_target(target, true_peak)
-        x = _np(wav, np.float32)
-        one = x.ndim == 1
-        x = x[None] if one else x
-        if x.ndim != 2:
-            raise ValueError(f"wav must be [S] or [B,S], got {np.shape(wav)}")
+        x, one = _wav_rows(wav)
         B, S = x.shape
         lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
         y = x.copy()
@@ -897,10 +890,7 @@ class Engine:
         rate = _loudness_rate(rate)
         assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
         B, S = x_t.shape
-        if out is None:
-            out = torch.empty((B, 4), dtype=torch.float32, device=x_t.device)
-        elif tuple(out.shape) != (B, 4) or out.dtype != torch.float32 or not out.is_contiguous():
-            raise ValueError(f"out must be contiguous float32 [{B}, 4]")
+        out = _out_tensor(out, (B, 4), x_t.device)
         st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
         self._ck(self.lib.vtts_loudness(self.h, _ptr(x_t), _ptr(lengths_t), B, S, rate, _ptr(out), st))
         return out
@@ -914,14 +904,8 @@ class Engine:
         target, ceiling = _loudness_target(target, true_peak)
         assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
         B, S = x_t.shape
-        if out is None:
-            out = torch.empty((B, S), dtype=torch.float32, device=x_t.device)
-        elif tuple(out.shape) != (B, S) or out.dtype != torch.float32 or not out.is_contiguous():
-            raise ValueError(f"out must be contiguous float32 [{B}, {S}]")
-        if gain_db is None:
-            gain_db = torch.empty(B, dtype=torch.float32, device=x_t.device)
-        elif tuple(gain_db.shape) != (B,) or gain_db.dtype != torch.float32 or not gain_db.is_contiguous():
-            raise ValueError(f"gain_db must be contiguous float32 [{B}]")
+        out = _out_tensor(out, (B, S), x_t.device)
+        gain_db = _out_tensor(gain_db, (B,), x_t.device, "gain_db")
         st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
         self._ck(self.lib.vtts_loudness_normalize(self.h, _ptr(x_t), _ptr(lengths_t), B, S, rate, target, ceiling, _ptr(out),
                                                   _ptr(gain_db), st))
@@ -965,233 +949,182 @@ def _loudness_target(target, true_peak):
 STREAM_BEGIN, STREAM_END = 1, 2
 
 
-class VocoderStream:
-    """Handle of a streaming generator (Engine.open_vocoder_stream).  A slot that has received P frames since BEGIN
-    has emitted max(0, P - lookahead) frames; a push with END emits the rest."""
+class _SlotStream:
+    """What every per-slot stream handle shares: the library handle `h` of one stream of `eng`'s context, the marshalling
+    of a push (zero padding of short chunks, the BEGIN / END flag bits, the n_new / flags arrays, the device-buffer checks
+    and the CUDA stream) and the lifecycle.  A subclass opens its stream, names its input and pushes."""
+    _kind = ""       # the library's vtts_<kind>_destroy closes the stream
+    _x = "x"         # the input's name in error messages
+    _row = ()        # shape of one input element past [S, F]: () for samples, (80,) for mel frames
+    h = None
 
-    def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int):
+    def __init__(self, eng: Engine, max_streams: int, max_chunk: int):
         self.eng = eng
-        self.max_streams, self.max_chunk_frames = int(max_streams), int(max_chunk_frames)
-        self.lookahead = int(eng.lib.vtts_vocoder_stream_lookahead())
-        self.wav_ld = config.HOP * (self.max_chunk_frames + self.lookahead)   # samples per slot of the output buffer
-        h = C.c_void_p()
-        eng._ck(eng.lib.vtts_vocoder_stream_create(eng.h, self.max_streams, self.max_chunk_frames, C.byref(h)))
+        self.max_streams, self._chunk = int(max_streams), int(max_chunk)
+
+    def _create(self, fn, *args, pitch=False):
+        """calls vtts_<kind>_create(ctx, *args, &h[, &pitch]); sets `h` and, with pitch, `out_pitch`"""
+        h, p = C.c_void_p(), C.c_int()
+        self.eng._ck(fn(self.eng.h, *args, C.byref(h), *((C.byref(p),) if pitch else ())))
         self.h = h
+        if pitch:
+            self.out_pitch = int(p.value)   # outputs per slot of a push's output buffer
 
-    def _host_args(self, n_new, flags):
-        S = self.max_streams
-        n = _np(n_new, np.int32, (S,), "n_new")
-        f = _np(flags, np.uint8, (S,), "flags")
-        return n, f
-
-    def push(self, mel, n_new, begin=None, end=None) -> list:
-        """mel f32 [S,F',80] (F' <= max_chunk_frames; rows past n_new[s] ignored), n_new int [S], begin / end bool [S]
-        or None.  Returns one float32 array per slot with the samples it emits now (256 per frame)."""
-        S, F = self.max_streams, self.max_chunk_frames
-        mel = _np(mel, np.float32)
-        if mel.ndim != 3 or mel.shape[0] != S or mel.shape[1] > F or mel.shape[2] != config.MEL_DIM:
-            raise ValueError(f"mel must be [{S}, <= {F}, {config.MEL_DIM}], got {mel.shape}")
-        if mel.shape[1] < F:
-            mel = np.concatenate([mel, np.zeros((S, F - mel.shape[1], config.MEL_DIM), np.float32)], axis=1)
+    def _host_in(self, x, n_new, begin, end):
+        """(x f32 [S, F, *row] zero-padded, n_new int32 [S], flags uint8 [S]) of a host push"""
+        S, F, row = self.max_streams, self._chunk, self._row
+        x = _np(x, np.float32)
+        if x.ndim != 2 + len(row) or x.shape[0] != S or x.shape[1] > F or x.shape[2:] != row:
+            raise ValueError(f"{self._x} must be [{S}, <= {F}{''.join(f', {d}' for d in row)}], got {x.shape}")
+        if x.shape[1] < F:
+            x = np.concatenate([x, np.zeros((S, F - x.shape[1]) + row, np.float32)], axis=1)
         flags = np.zeros(S, np.uint8)
         if begin is not None:
             flags |= np.asarray(begin, bool).astype(np.uint8) * STREAM_BEGIN
         if end is not None:
             flags |= np.asarray(end, bool).astype(np.uint8) * STREAM_END
-        n, f = self._host_args(n_new, flags)
-        wav = np.empty((S, self.wav_ld), np.float32)
-        n_out = np.zeros(S, np.int32)
+        return (x,) + self._args(n_new, flags)
+
+    def _args(self, n_new, flags):
+        S = self.max_streams
+        return _np(n_new, np.int32, (S,), "n_new"), _np(flags, np.uint8, (S,), "flags")
+
+    def _device_in(self, x_t, out_t, out_shape, n_new, flags, stream):
+        """(n_new int32 [S], flags uint8 [S], CUDA stream) of a device push, after checking both buffers"""
+        import torch
+        for t, name, shape in ((x_t, self._x + "_t", (self.max_streams, self._chunk) + self._row), (out_t, "out_t", out_shape)):
+            if tuple(t.shape) != shape or t.dtype != torch.float32 or not t.is_contiguous():
+                raise ValueError(f"{name} must be contiguous float32 [{', '.join(map(str, shape))}]")
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        return self._args(n_new, flags) + (st,)
+
+    def _rows(self, y, n_out, scale=1):
+        return [y[s, : int(n_out[s]) * scale].copy() for s in range(self.max_streams)]
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.eng, "h", None):
+            self.eng._ck(getattr(self.eng.lib, f"vtts_{self._kind}_destroy")(self.eng.h, self.h))
+        self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class VocoderStream(_SlotStream):
+    """Handle of a streaming generator (Engine.open_vocoder_stream).  A slot that has received P frames since BEGIN
+    has emitted max(0, P - lookahead) frames; a push with END emits the rest."""
+    _kind, _x, _row = "vocoder_stream", "mel", (config.MEL_DIM,)
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int):
+        super().__init__(eng, max_streams, max_chunk_frames)
+        self.max_chunk_frames = self._chunk
+        self.lookahead = int(eng.lib.vtts_vocoder_stream_lookahead())
+        self.wav_ld = config.HOP * (self.max_chunk_frames + self.lookahead)   # samples per slot of the output buffer
+        self._create(eng.lib.vtts_vocoder_stream_create, self.max_streams, self.max_chunk_frames)
+
+    def push(self, mel, n_new, begin=None, end=None) -> list:
+        """mel f32 [S,F',80] (F' <= max_chunk_frames; rows past n_new[s] ignored), n_new int [S], begin / end bool [S]
+        or None.  Returns one float32 array per slot with the samples it emits now (256 per frame)."""
+        mel, n, f = self._host_in(mel, n_new, begin, end)
+        wav = np.empty((self.max_streams, self.wav_ld), np.float32)
+        n_out = np.zeros(self.max_streams, np.int32)
         self.eng._ck(self.eng.lib.vtts_vocoder_stream_push_host(self.eng.h, self.h, _ptr(mel), _ptr(n), _ptr(f), _ptr(wav), _ptr(n_out)))
-        return [wav[s, : int(n_out[s]) * config.HOP].copy() for s in range(S)]
+        return self._rows(wav, n_out, config.HOP)
 
     def push_device(self, mel_t, n_new, flags, out_t, stream=None) -> np.ndarray:
         """Device buffers: mel_t f32 CUDA [S,F,80], out_t f32 CUDA [S, 256*(F+lookahead)]; n_new int [S] and flags
         uint8 [S] (bit0 BEGIN, bit1 END) on the host.  Stream-ordered; returns n_out int32 [S] (frames slot s got at
         the start of its row of out_t)."""
-        import torch
-        S, F = self.max_streams, self.max_chunk_frames
-        if tuple(mel_t.shape) != (S, F, config.MEL_DIM) or mel_t.dtype != torch.float32 or not mel_t.is_contiguous():
-            raise ValueError(f"mel_t must be contiguous float32 [{S}, {F}, {config.MEL_DIM}]")
-        if tuple(out_t.shape) != (S, self.wav_ld) or out_t.dtype != torch.float32 or not out_t.is_contiguous():
-            raise ValueError(f"out_t must be contiguous float32 [{S}, {self.wav_ld}]")
-        n, f = self._host_args(n_new, flags)
-        n_out = np.zeros(S, np.int32)
-        st = torch.cuda.current_stream(mel_t.device).cuda_stream if stream is None else stream
+        n, f, st = self._device_in(mel_t, out_t, (self.max_streams, self.wav_ld), n_new, flags, stream)
+        n_out = np.zeros(self.max_streams, np.int32)
         self.eng._ck(self.eng.lib.vtts_vocoder_stream_push(self.eng.h, self.h, _ptr(mel_t), _ptr(n), _ptr(f), _ptr(out_t), _ptr(n_out), st))
         return n_out
 
-    def close(self):
-        if getattr(self, "h", None) and getattr(self.eng, "h", None):
-            self.eng._ck(self.eng.lib.vtts_vocoder_stream_destroy(self.eng.h, self.h))
-        self.h = None
 
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class ResampleStream:
+class ResampleStream(_SlotStream):
     """Handle of a streaming resampler (Engine.open_resample_stream).  Before END a slot that has received P samples
     has emitted min(ceil(P up / down), max(0, floor((P up - 1 - half) / down) + 1)) outputs, half = 10 max(up, down);
     a push with END emits the rest."""
+    _kind = "resample_stream"
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, out_rate: int, in_rate: int = config.SAMPLE_RATE):
-        self.eng = eng
-        self.max_streams, self.max_chunk_samples = int(max_streams), int(max_chunk_samples)
+        super().__init__(eng, max_streams, max_chunk_samples)
+        self.max_chunk_samples = self._chunk
         self.in_rate, self.out_rate = int(in_rate), int(out_rate)
         resample_ratio(self.in_rate, self.out_rate)
-        h, pitch = C.c_void_p(), C.c_int()
-        eng._ck(eng.lib.vtts_resample_stream_create(eng.h, self.max_streams, self.max_chunk_samples, self.in_rate, self.out_rate,
-                                                    C.byref(h), C.byref(pitch)))
-        self.h = h
-        self.out_pitch = int(pitch.value)   # outputs per slot of a push's output buffer
+        self._create(eng.lib.vtts_resample_stream_create, self.max_streams, self.max_chunk_samples, self.in_rate, self.out_rate, pitch=True)
         self.lookahead = int(eng.lib.vtts_resample_stream_lookahead(self.in_rate, self.out_rate))
 
     def push(self, x, n_new, begin=None, end=None) -> list:
         """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None.
         Returns one float32 array per slot with the samples it emits now."""
-        S, F = self.max_streams, self.max_chunk_samples
-        x = _np(x, np.float32)
-        if x.ndim != 2 or x.shape[0] != S or x.shape[1] > F:
-            raise ValueError(f"x must be [{S}, <= {F}], got {x.shape}")
-        if x.shape[1] < F:
-            x = np.concatenate([x, np.zeros((S, F - x.shape[1]), np.float32)], axis=1)
-        flags = np.zeros(S, np.uint8)
-        if begin is not None:
-            flags |= np.asarray(begin, bool).astype(np.uint8) * STREAM_BEGIN
-        if end is not None:
-            flags |= np.asarray(end, bool).astype(np.uint8) * STREAM_END
-        n = _np(n_new, np.int32, (S,), "n_new")
-        y = np.empty((S, self.out_pitch), np.float32)
-        n_out = np.zeros(S, np.int32)
-        self.eng._ck(self.eng.lib.vtts_resample_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(flags), _ptr(y), _ptr(n_out)))
-        return [y[s, : int(n_out[s])].copy() for s in range(S)]
+        x, n, f = self._host_in(x, n_new, begin, end)
+        y = np.empty((self.max_streams, self.out_pitch), np.float32)
+        n_out = np.zeros(self.max_streams, np.int32)
+        self.eng._ck(self.eng.lib.vtts_resample_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(y), _ptr(n_out)))
+        return self._rows(y, n_out)
 
     def push_device(self, x_t, n_new, flags, out_t, stream=None) -> np.ndarray:
         """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S, out_pitch]; n_new int [S] and flags
         uint8 [S] (bit0 BEGIN, bit1 END) on the host.  Stream-ordered; returns n_out int32 [S] (outputs slot s got at the
         start of its row of out_t)."""
-        import torch
-        S, F = self.max_streams, self.max_chunk_samples
-        if tuple(x_t.shape) != (S, F) or x_t.dtype != torch.float32 or not x_t.is_contiguous():
-            raise ValueError(f"x_t must be contiguous float32 [{S}, {F}]")
-        if tuple(out_t.shape) != (S, self.out_pitch) or out_t.dtype != torch.float32 or not out_t.is_contiguous():
-            raise ValueError(f"out_t must be contiguous float32 [{S}, {self.out_pitch}]")
-        n = _np(n_new, np.int32, (S,), "n_new")
-        f = _np(flags, np.uint8, (S,), "flags")
-        n_out = np.zeros(S, np.int32)
-        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        n, f, st = self._device_in(x_t, out_t, (self.max_streams, self.out_pitch), n_new, flags, stream)
+        n_out = np.zeros(self.max_streams, np.int32)
         self.eng._ck(self.eng.lib.vtts_resample_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(out_t), _ptr(n_out), st))
         return n_out
 
-    def close(self):
-        if getattr(self, "h", None) and getattr(self.eng, "h", None):
-            self.eng._ck(self.eng.lib.vtts_resample_stream_destroy(self.eng.h, self.h))
-        self.h = None
 
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class DenoiseStream:
+class DenoiseStream(_SlotStream):
     """Handle of a streaming denoiser (Engine.open_denoise_stream).  Before END a slot that has received P samples has
     emitted min(P, 256 max(0, floor(P / 256) - 3)) outputs; a push with END emits the rest."""
+    _kind = "denoise_stream"
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, strength: float, bias=None):
-        self.eng = eng
-        self.max_streams, self.max_chunk_samples = int(max_streams), int(max_chunk_samples)
+        super().__init__(eng, max_streams, max_chunk_samples)
+        self.max_chunk_samples = self._chunk
         self.strength = _strength(strength)
         self.bias = eng._bias_arg(bias)
-        h, pitch = C.c_void_p(), C.c_int()
-        eng._ck(eng.lib.vtts_denoise_stream_create(eng.h, self.max_streams, self.max_chunk_samples, self.strength, _ptr(self.bias),
-                                                   C.byref(h), C.byref(pitch)))
-        self.h = h
-        self.out_pitch = int(pitch.value)   # outputs per slot of a push's output buffer
+        self._create(eng.lib.vtts_denoise_stream_create, self.max_streams, self.max_chunk_samples, self.strength, _ptr(self.bias),
+                     pitch=True)
         self.lookahead = int(eng.lib.vtts_denoise_stream_lookahead())
 
     def push(self, x, n_new, begin=None, end=None) -> list:
         """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None.
         Returns one float32 array per slot with the samples it emits now."""
-        S, F = self.max_streams, self.max_chunk_samples
-        x = _np(x, np.float32)
-        if x.ndim != 2 or x.shape[0] != S or x.shape[1] > F:
-            raise ValueError(f"x must be [{S}, <= {F}], got {x.shape}")
-        if x.shape[1] < F:
-            x = np.concatenate([x, np.zeros((S, F - x.shape[1]), np.float32)], axis=1)
-        flags = np.zeros(S, np.uint8)
-        if begin is not None:
-            flags |= np.asarray(begin, bool).astype(np.uint8) * STREAM_BEGIN
-        if end is not None:
-            flags |= np.asarray(end, bool).astype(np.uint8) * STREAM_END
-        n = _np(n_new, np.int32, (S,), "n_new")
-        y = np.empty((S, self.out_pitch), np.float32)
-        n_out = np.zeros(S, np.int32)
-        self.eng._ck(self.eng.lib.vtts_denoise_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(flags), _ptr(y), _ptr(n_out)))
-        return [y[s, : int(n_out[s])].copy() for s in range(S)]
+        x, n, f = self._host_in(x, n_new, begin, end)
+        y = np.empty((self.max_streams, self.out_pitch), np.float32)
+        n_out = np.zeros(self.max_streams, np.int32)
+        self.eng._ck(self.eng.lib.vtts_denoise_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(y), _ptr(n_out)))
+        return self._rows(y, n_out)
 
     def push_device(self, x_t, n_new, flags, out_t, stream=None) -> np.ndarray:
         """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S, out_pitch]; n_new int [S] and flags
         uint8 [S] (bit0 BEGIN, bit1 END) on the host.  Stream-ordered; returns n_out int32 [S] (outputs slot s got at the
         start of its row of out_t)."""
-        import torch
-        S, F = self.max_streams, self.max_chunk_samples
-        if tuple(x_t.shape) != (S, F) or x_t.dtype != torch.float32 or not x_t.is_contiguous():
-            raise ValueError(f"x_t must be contiguous float32 [{S}, {F}]")
-        if tuple(out_t.shape) != (S, self.out_pitch) or out_t.dtype != torch.float32 or not out_t.is_contiguous():
-            raise ValueError(f"out_t must be contiguous float32 [{S}, {self.out_pitch}]")
-        n = _np(n_new, np.int32, (S,), "n_new")
-        f = _np(flags, np.uint8, (S,), "flags")
-        n_out = np.zeros(S, np.int32)
-        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        n, f, st = self._device_in(x_t, out_t, (self.max_streams, self.out_pitch), n_new, flags, stream)
+        n_out = np.zeros(self.max_streams, np.int32)
         self.eng._ck(self.eng.lib.vtts_denoise_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(out_t), _ptr(n_out), st))
         return n_out
 
-    def close(self):
-        if getattr(self, "h", None) and getattr(self.eng, "h", None):
-            self.eng._ck(self.eng.lib.vtts_denoise_stream_destroy(self.eng.h, self.h))
-        self.h = None
 
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class PitchShiftStream:
+class PitchShiftStream(_SlotStream):
     """Handle of a streaming pitch shifter (Engine.open_pitch_shift_stream).  Before END a slot that has received P samples
     has emitted min(P, 256 max(0, floor(P / 256) - 3)) outputs; a push with END emits the rest."""
+    _kind = "pitch_shift_stream"
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int):
-        self.eng = eng
-        self.max_streams, self.max_chunk_samples = int(max_streams), int(max_chunk_samples)
-        h, pitch = C.c_void_p(), C.c_int()
-        eng._ck(eng.lib.vtts_pitch_shift_stream_create(eng.h, self.max_streams, self.max_chunk_samples, C.byref(h), C.byref(pitch)))
-        self.h = h
-        self.out_pitch = int(pitch.value)   # outputs per slot of a push's output buffer
+        super().__init__(eng, max_streams, max_chunk_samples)
+        self.max_chunk_samples = self._chunk
+        self._create(eng.lib.vtts_pitch_shift_stream_create, self.max_streams, self.max_chunk_samples, pitch=True)
         self.lookahead = int(eng.lib.vtts_pitch_shift_stream_lookahead())
         self.shift = np.zeros(self.max_streams, np.float32)   # each slot's shift since its BEGIN
 
@@ -1217,128 +1150,54 @@ class PitchShiftStream:
         """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None,
         semitones: a scalar or [S], read for the slots that begin.  Returns one float32 array per slot with the samples
         it emits now."""
-        S, F = self.max_streams, self.max_chunk_samples
-        x = _np(x, np.float32)
-        if x.ndim != 2 or x.shape[0] != S or x.shape[1] > F:
-            raise ValueError(f"x must be [{S}, <= {F}], got {x.shape}")
-        if x.shape[1] < F:
-            x = np.concatenate([x, np.zeros((S, F - x.shape[1]), np.float32)], axis=1)
-        flags = np.zeros(S, np.uint8)
-        if begin is not None:
-            flags |= np.asarray(begin, bool).astype(np.uint8) * STREAM_BEGIN
-        if end is not None:
-            flags |= np.asarray(end, bool).astype(np.uint8) * STREAM_END
-        n = _np(n_new, np.int32, (S,), "n_new")
-        sem = self._shifts(flags, semitones)
-        y = np.empty((S, self.out_pitch), np.float32)
-        n_out = np.zeros(S, np.int32)
-        self.eng._ck(self.eng.lib.vtts_pitch_shift_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(flags), _ptr(sem), _ptr(y),
+        x, n, f = self._host_in(x, n_new, begin, end)
+        sem = self._shifts(f, semitones)
+        y = np.empty((self.max_streams, self.out_pitch), np.float32)
+        n_out = np.zeros(self.max_streams, np.int32)
+        self.eng._ck(self.eng.lib.vtts_pitch_shift_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(sem), _ptr(y),
                                                                     _ptr(n_out)))
-        self._commit(flags, sem)
-        return [y[s, : int(n_out[s])].copy() for s in range(S)]
+        self._commit(f, sem)
+        return self._rows(y, n_out)
 
     def push_device(self, x_t, n_new, flags, out_t, semitones=None, stream=None) -> np.ndarray:
         """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S, out_pitch]; n_new int [S], flags
         uint8 [S] (bit0 BEGIN, bit1 END) and semitones (scalar or [S], read for the slots that begin) on the host.
         Stream-ordered; returns n_out int32 [S] (outputs slot s got at the start of its row of out_t)."""
-        import torch
-        S, F = self.max_streams, self.max_chunk_samples
-        if tuple(x_t.shape) != (S, F) or x_t.dtype != torch.float32 or not x_t.is_contiguous():
-            raise ValueError(f"x_t must be contiguous float32 [{S}, {F}]")
-        if tuple(out_t.shape) != (S, self.out_pitch) or out_t.dtype != torch.float32 or not out_t.is_contiguous():
-            raise ValueError(f"out_t must be contiguous float32 [{S}, {self.out_pitch}]")
-        n = _np(n_new, np.int32, (S,), "n_new")
-        f = _np(flags, np.uint8, (S,), "flags")
+        n, f, st = self._device_in(x_t, out_t, (self.max_streams, self.out_pitch), n_new, flags, stream)
         sem = self._shifts(f, semitones)
-        n_out = np.zeros(S, np.int32)
-        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        n_out = np.zeros(self.max_streams, np.int32)
         self.eng._ck(self.eng.lib.vtts_pitch_shift_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(sem), _ptr(out_t),
                                                                _ptr(n_out), st))
         self._commit(f, sem)
         return n_out
 
-    def close(self):
-        if getattr(self, "h", None) and getattr(self.eng, "h", None):
-            self.eng._ck(self.eng.lib.vtts_pitch_shift_stream_destroy(self.eng.h, self.h))
-        self.h = None
 
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class LoudnessMeter:
+class LoudnessMeter(_SlotStream):
     """Handle of a streaming loudness meter (Engine.open_loudness_meter).  Every push returns every slot's readings
     [S,4]: integrated, momentary, short-term LUFS and true peak dBTP of the samples it has received since BEGIN."""
+    _kind = "loudness_stream"
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, rate: int = config.SAMPLE_RATE, max_seconds: int = 600):
-        self.eng = eng
-        self.max_streams, self.max_chunk_samples = int(max_streams), int(max_chunk_samples)
+        super().__init__(eng, max_streams, max_chunk_samples)
+        self.max_chunk_samples = self._chunk
         self.rate, self.max_seconds = _loudness_rate(rate), int(max_seconds)
-        h = C.c_void_p()
-        eng._ck(eng.lib.vtts_loudness_stream_create(eng.h, self.max_streams, self.max_chunk_samples, self.rate, self.max_seconds,
-                                                    C.byref(h)))
-        self.h = h
+        self._create(eng.lib.vtts_loudness_stream_create, self.max_streams, self.max_chunk_samples, self.rate, self.max_seconds)
         self.lookahead = int(eng.lib.vtts_loudness_stream_lookahead(self.rate))
 
     def push(self, x, n_new, begin=None, end=None) -> np.ndarray:
         """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None.
         Returns float32 [S,4]."""
-        S, F = self.max_streams, self.max_chunk_samples
-        x = _np(x, np.float32)
-        if x.ndim != 2 or x.shape[0] != S or x.shape[1] > F:
-            raise ValueError(f"x must be [{S}, <= {F}], got {x.shape}")
-        if x.shape[1] < F:
-            x = np.concatenate([x, np.zeros((S, F - x.shape[1]), np.float32)], axis=1)
-        flags = np.zeros(S, np.uint8)
-        if begin is not None:
-            flags |= np.asarray(begin, bool).astype(np.uint8) * STREAM_BEGIN
-        if end is not None:
-            flags |= np.asarray(end, bool).astype(np.uint8) * STREAM_END
-        n = _np(n_new, np.int32, (S,), "n_new")
-        out = np.empty((S, 4), np.float32)
-        self.eng._ck(self.eng.lib.vtts_loudness_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(flags), _ptr(out)))
+        x, n, f = self._host_in(x, n_new, begin, end)
+        out = np.empty((self.max_streams, 4), np.float32)
+        self.eng._ck(self.eng.lib.vtts_loudness_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(out)))
         return out
 
     def push_device(self, x_t, n_new, flags, out_t, stream=None):
         """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S,4]; n_new int [S] and flags uint8 [S]
         (bit0 BEGIN, bit1 END) on the host.  Stream-ordered."""
-        import torch
-        S, F = self.max_streams, self.max_chunk_samples
-        if tuple(x_t.shape) != (S, F) or x_t.dtype != torch.float32 or not x_t.is_contiguous():
-            raise ValueError(f"x_t must be contiguous float32 [{S}, {F}]")
-        if tuple(out_t.shape) != (S, 4) or out_t.dtype != torch.float32 or not out_t.is_contiguous():
-            raise ValueError(f"out_t must be contiguous float32 [{S}, 4]")
-        n = _np(n_new, np.int32, (S,), "n_new")
-        f = _np(flags, np.uint8, (S,), "flags")
-        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        n, f, st = self._device_in(x_t, out_t, (self.max_streams, 4), n_new, flags, stream)
         self.eng._ck(self.eng.lib.vtts_loudness_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(out_t), st))
         return out_t
-
-    def close(self):
-        if getattr(self, "h", None) and getattr(self.eng, "h", None):
-            self.eng._ck(self.eng.lib.vtts_loudness_stream_destroy(self.eng.h, self.h))
-        self.h = None
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def acoustic_stream_schedule(n_frames: int, n_emit: int | None, chunk: int, lookahead: int = 10) -> list:
@@ -1355,13 +1214,14 @@ def acoustic_stream_schedule(n_frames: int, n_emit: int | None, chunk: int, look
     return out
 
 
-class AcousticStream:
+class AcousticStream(_SlotStream):
     """Handle of a streaming acoustic model (Engine.open_acoustic_stream)."""
+    _kind = "acoustic_stream"
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
                  masks: bool = False):
-        self.eng = eng
-        self.max_streams, self.max_chunk_frames = int(max_streams), int(max_chunk_frames)
+        super().__init__(eng, max_streams, max_chunk_frames)
+        self.max_chunk_frames = self._chunk
         self.max_frames, self.max_tokens = int(max_frames), int(max_tokens)
         if rng is not None:
             self.mode, self.seed = DROPOUT_REFERENCE, _rng_seed(rng, seed, True if masks else None)
@@ -1428,23 +1288,6 @@ class AcousticStream:
         self._advance()
         return n_out
 
-    def close(self):
-        if getattr(self, "h", None) and getattr(self.eng, "h", None):
-            self.eng._ck(self.eng.lib.vtts_acoustic_stream_destroy(self.eng.h, self.h))
-        self.h = None
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 class TtsStream:
     """Handle of a text-to-speech stream (Engine.open_tts_stream): an acoustic stream of max_chunk_frames F feeding a
@@ -1466,51 +1309,40 @@ class TtsStream:
         if semitones is not None:
             semitones = float(_semitones(semitones, 1)[0])
         self.eng = eng
-        self.rs = None
-        self.dn = None
-        self.ps = None
-        self.mt = None
-        self.ac = AcousticStream(eng, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng)
+        self.rs = self.dn = self.ps = self.mt = None
+        S, sr = max_streams, output_rate or config.SAMPLE_RATE
+        # the stages after the vocoder, in push order; each takes the previous stage's output buffer as its input
+        # (the vocoder's: n_new = 256 * frames it emitted) and a slot of the meter holds at most max_frames of audio
+        seconds = -(-int(max_frames) * config.HOP // config.SAMPLE_RATE) + 1
+        plan = (("dn", denoise is not None, lambda p: DenoiseStream(eng, S, p, denoise)),
+                ("ps", semitones is not None, lambda p: PitchShiftStream(eng, S, p)),
+                ("rs", output_rate is not None, lambda p: ResampleStream(eng, S, p, output_rate)),
+                ("mt", meter, lambda p: LoudnessMeter(eng, S, p, sr, seconds)))
+        self._built = []   # every stream handle, in construction order
         try:
-            self.voc = VocoderStream(eng, max_streams, self.ac.out_frames)
+            self.ac = AcousticStream(eng, S, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng)
+            self._built.append(self.ac)
+            self.voc = VocoderStream(eng, S, self.ac.out_frames)
+            self._built.append(self.voc)
             pitch = self.voc.wav_ld
-            if denoise is not None:
-                # the vocoder's output buffer is the denoiser's input: n_new = 256 * frames it emitted
-                self.dn = DenoiseStream(eng, max_streams, pitch, denoise)
-                pitch = self.dn.out_pitch
-            if semitones is not None:
-                # the previous stage's output buffer is the pitch shifter's input
-                self.ps = PitchShiftStream(eng, max_streams, pitch)
-                pitch = self.ps.out_pitch
-            if output_rate is not None:
-                # the previous stage's output buffer is the resampler's input
-                self.rs = ResampleStream(eng, max_streams, pitch, output_rate)
-                pitch = self.rs.out_pitch
-            if meter:
-                # the last stage's output buffer is the meter's input; a slot holds at most max_frames of audio
-                seconds = -(-int(max_frames) * config.HOP // config.SAMPLE_RATE) + 1
-                self.mt = LoudnessMeter(eng, max_streams, pitch, output_rate or config.SAMPLE_RATE, seconds)
+            for name, on, make in plan:
+                if on:
+                    st = make(pitch)
+                    self._built.append(st)
+                    setattr(self, name, st)
+                    pitch = getattr(st, "out_pitch", pitch)
         except Exception:
-            if getattr(self, "rs", None) is not None:
-                self.rs.close()
-            if getattr(self, "ps", None) is not None:
-                self.ps.close()
-            if getattr(self, "dn", None) is not None:
-                self.dn.close()
-            if getattr(self, "voc", None) is not None:
-                self.voc.close()
-            self.ac.close()
+            self.close()
             raise
         dev = torch.device("cuda", eng.device)
-        self._mel = torch.zeros((max_streams, self.ac.out_frames, config.MEL_DIM), dtype=torch.float32, device=dev)
-        self._wav = torch.zeros((max_streams, self.voc.wav_ld), dtype=torch.float32, device=dev)
-        self._den = None if self.dn is None else torch.zeros((max_streams, self.dn.out_pitch), dtype=torch.float32, device=dev)
-        self._psout = None if self.ps is None else torch.zeros((max_streams, self.ps.out_pitch), dtype=torch.float32, device=dev)
+        self._mel = torch.zeros((S, self.ac.out_frames, config.MEL_DIM), dtype=torch.float32, device=dev)
+        self._wav = torch.zeros((S, self.voc.wav_ld), dtype=torch.float32, device=dev)
+        self._shift = np.zeros(S, np.float32)  # the shift of each slot's utterance
+        # (handle, device output buffer, extra push arguments) of the stages after the vocoder
+        self._stages = [(st, torch.zeros((S, 4 if st is self.mt else st.out_pitch), dtype=torch.float32, device=dev),
+                         {"semitones": self._shift} if st is self.ps else {}) for st in self._built[2:]]
+        self._mout_h = None if self.mt is None else torch.zeros((S, 4), dtype=torch.float32).pin_memory()
         self._semitones = semitones                    # every slot's default shift
-        self._shift = np.zeros(max_streams, np.float32)  # the shift of each slot's utterance
-        self._out = None if self.rs is None else torch.zeros((max_streams, self.rs.out_pitch), dtype=torch.float32, device=dev)
-        self._mout = None if self.mt is None else torch.zeros((max_streams, 4), dtype=torch.float32, device=dev)
-        self._mout_h = None if self.mt is None else torch.zeros((max_streams, 4), dtype=torch.float32).pin_memory()
         self._meter = {}
         self._fresh = np.zeros(max_streams, bool)   # begun, no push yet: the next vocoder push carries BEGIN
         self._empty = set()                         # begun with nothing left after the trim: reported empty at the next step
@@ -1564,18 +1396,12 @@ class TtsStream:
             n_wav = self.voc.push_device(self._mel, n_out, flags, self._wav)
             n_wav = n_wav * config.HOP
             src = self._wav
-            if self.dn is not None:
-                n_wav = self.dn.push_device(src, n_wav, flags, self._den)
-                src = self._den
-            if self.ps is not None:
-                n_wav = self.ps.push_device(src, n_wav, flags, self._psout, semitones=self._shift)
-                src = self._psout
-            if self.rs is not None:
-                n_wav = self.rs.push_device(src, n_wav, flags, self._out)
-                src = self._out
-            if self.mt is not None:
-                self.mt.push_device(src, n_wav, flags, self._mout)
-                self._mout_h.copy_(self._mout, non_blocking=True)   # ready once the blocking copy below returns
+            for st, buf, kw in self._stages:
+                r = st.push_device(src, n_wav, flags, buf, **kw)
+                if st is self.mt:
+                    self._mout_h.copy_(buf, non_blocking=True)   # ready once the blocking copy below returns
+                else:
+                    n_wav, src = r, buf
             wav = src.cpu().numpy()
             for s in np.flatnonzero(active):
                 out[int(s)] = wav[s, : int(n_wav[s])].copy()
@@ -1593,18 +1419,8 @@ class TtsStream:
         return dict(self._meter)
 
     def close(self):
-        if getattr(self, "mt", None) is not None:
-            self.mt.close()
-        if getattr(self, "rs", None) is not None:
-            self.rs.close()
-        if getattr(self, "ps", None) is not None:
-            self.ps.close()
-        if getattr(self, "dn", None) is not None:
-            self.dn.close()
-        if getattr(self, "voc", None) is not None:
-            self.voc.close()
-        if getattr(self, "ac", None) is not None:
-            self.ac.close()
+        for st in reversed(getattr(self, "_built", [])):
+            st.close()
 
     def __enter__(self):
         return self

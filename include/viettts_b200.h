@@ -381,6 +381,59 @@ int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, con
 int vtts_pitch_shift_stream_push_host(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x, const int32_t* n_new,
                                       const uint8_t* flags, const float* semitones, float* y, int32_t* n_out);
 
+/* ---- time stretch: the pitch shifter's phase vocoder with moving analysis frames ------------------------------------
+ * One row x of n samples, a tempo alpha (fp32, finite, in [0.5, 2], else VTTS_ERR_BAD_ARG before anything is launched;
+ * alpha > 1 is faster), after Laroche & Dolson, "Improved phase vocoder time-scale modification of audio" (IEEE TSAP
+ * 7(3), 1999):
+ *   M = floor(n / (double)alpha + 0.5) outputs;  T = M / 256 + 1 synthesis frames at hop H = 256;
+ *   analysis frame t centred at a_t = min(rint(256 t (double)alpha), n - 1), read with the denoiser's window and its
+ *   reflection at 0 and n - 1;  h_t = a_t - a_t-1 (>= 1);  peaks and owners as for vtts_pitch_shift;
+ *   omega_t[p] = 2 pi p / N + princarg(theta_t[p] - theta_t-1[p] - 2 pi p h_t / N) / h_t;
+ *   psi_t(p) = princarg(psi_t-1[p] + (H - h_t) omega_t[p]), psi_0 = 0, in double;
+ *   Y_t[k] = X_t[k] e^(i psi_t(owner_t(k)));  y = the denoiser's inverse and overlap-add of Y over T frames, length M.
+ * This is vtts_pitch_shift's recurrence with a per-frame h_t and r = 1.  Rows with alpha == 1 and rows of n <= 512 give
+ * their first min(n, M) samples, then zeros up to M (so alpha == 1 is a bit copy).  fp32 in every vtts_precision mode
+ * apart from the double phase recurrence; a row gives the same bits alone, in any batch, and through the stream. */
+/* M for n samples at `tempo`, or -1 for n < 0 or a tempo outside [0.5, 2].  Needs no device. */
+int64_t vtts_time_stretch_length(int64_t n, float tempo);
+/* x_dev [B,S]; n_dev int32 [B] or NULL (= S; values clamped to [0, S]); tempo HOST float [B]; y_dev [B,Sy], not x_dev:
+ * row b gets its first min(M_b, Sy) outputs, zeros past M_b.  Stream-ordered; uses the context's workspace (about
+ * 17 KiB per synthesis frame of the longest row). */
+int vtts_time_stretch(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const float* tempo, float* y_dev, int Sy,
+                      void* stream);
+/* the same on host buffers x [B,S] and y [B,Sy]; n_in[b] must lie in [0, S] */
+int vtts_time_stretch_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, const float* tempo, float* y, int Sy);
+/* test hook: the discrete decisions of vtts_time_stretch, encoded as vtts_debug_pitch_decisions does:
+ * dec_dev int32 [B][T_max][513], T_max = max over b of vtts_time_stretch_length(S, tempo[b]) / 256 + 1.  Stream-ordered;
+ * uses the context's workspace. */
+int vtts_debug_time_stretch_decisions(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const float* tempo,
+                                      int32_t* dec_dev, void* stream);
+/* Streaming time stretcher with max_streams independent slots, laid out as the pitch-shift stream (2048 carried inputs
+ * and a 64-bit position, the next unscanned frame, theta and psi of the last scanned frame, two halves of synthesized
+ * frames), so the outputs a slot emits, concatenated, are bit-identical to vtts_time_stretch of its whole input.
+ * Schedule: before END, frame t is scanned once a_t + 512 <= P (P inputs received) and P > 512; after Q frames are
+ * scanned the slot has released max(0, 256 Q - 511) outputs, those whose every weighing synthesis frame (256 g <
+ * u + 512 <= 256 g + 1023) is synthesized (a slot at tempo 1 releases every input it has received); END releases the
+ * rest, up to M.  So n_out is known on the host before launch.  vtts_time_stretch_stream_lookahead() = 1536: before
+ * END a slot holding P inputs has released more than P / alpha - 1536 outputs.  A slot's tempo is read from tempo[s] with BEGIN and fixed until END.
+ * flags and slot rules as for the resample stream.  Every push issues the same five launches (window step, analysis,
+ * phase, synthesis, overlap-add). */
+typedef struct vtts_time_stretch_stream vtts_time_stretch_stream;
+/* *out_pitch receives the outputs per slot of a push's output buffer (2 * max_chunk_samples + 2048) */
+int vtts_time_stretch_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, vtts_time_stretch_stream** out,
+                                    int* out_pitch);
+int vtts_time_stretch_stream_destroy(vtts_ctx* ctx, vtts_time_stretch_stream* ts);
+int vtts_time_stretch_stream_lookahead(void);
+/* x_dev [S][max_chunk_samples] (samples past n_new[s] ignored); n_new, flags, n_out HOST int32 / uint8 / int32 [S];
+ * tempo HOST float [S]: read for the slots with BEGIN (finite, in [0.5, 2]); for the other pushed slots it must hold the
+ * slot's tempo, or tempo may be NULL when no slot begins.  y_dev [S][out_pitch], not x_dev, slot s gets n_out[s]
+ * outputs from its start.  Argument errors fail with VTTS_ERR_BAD_ARG before anything is launched.  Stream-ordered. */
+int vtts_time_stretch_stream_push(vtts_ctx* ctx, vtts_time_stretch_stream* ts, const float* x_dev, const int32_t* n_new,
+                                  const uint8_t* flags, const float* tempo, float* y_dev, int32_t* n_out, void* stream);
+/* the same on host buffers x [S][max_chunk_samples] and y [S][out_pitch]; returns when y is written */
+int vtts_time_stretch_stream_push_host(vtts_ctx* ctx, vtts_time_stretch_stream* ts, const float* x, const int32_t* n_new,
+                                       const uint8_t* flags, const float* tempo, float* y, int32_t* n_out);
+
 /* ---- loudness: ITU-R BS.1770-4 gated loudness and true peak, and normalization to a target ------------------------
  * One mono row x of n samples at rate r, a multiple of 10 in [8000, 192000] (else VTTS_ERR_BAD_ARG):
  *   K-weighting: the libebur128 shelf and high-pass biquads for r, from zero state;  m = r / 10;  E_k = sum of y^2 over

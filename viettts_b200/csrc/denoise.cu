@@ -120,10 +120,12 @@ __global__ void __launch_bounds__(OLA_THREADS) denoise_ola_kernel(const float* _
     if (r.copy) {
       out = x[(size_t)b * x_ld + (t - r.x0)];
     } else {
-      // frames g with 256 g <= t + 512 <= 256 g + 1023 that exist (g <= n / 256), ascending
+      // frames g with 256 g < t + 512 <= 256 g + 1023 that exist (g <= n / 256), ascending.  A frame's sample 0 is
+      // windowed by w[0] = 0 and adds exactly nothing, so it is not read: a stream may release an output before the
+      // frame that starts at it is synthesized.
       const long long p = t + PAD;
       const long long g_lo = p >= NF - 1 ? (p - (NF - 1) + HOP - 1) / HOP : 0;
-      const long long g_hi = min(r.n / HOP, p / HOP);
+      const long long g_hi = min(r.n / HOP, (p - 1) / HOP);
       const float* wr = ws + (size_t)b * ws_frames * NF;
       float num = 0.f, env = 0.f;
       for (long long g = g_lo; g <= g_hi; ++g) {

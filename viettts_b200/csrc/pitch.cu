@@ -1,13 +1,20 @@
-// Pitch shifter: a peak-locked phase vocoder (Laroche & Dolson 1999) on the denoiser's STFT, fp32 on the device in every
-// vtts_precision mode, with the phase recurrence in double:
-//   STFT n_fft 1024 / hop 256 / periodic Hann / reflect padding 512 (F = n / 256 + 1 frames) | a = |X|, theta = arg X |
-//   peaks: a[k] > a[k-1], a[k] >= a[k+1], a[k] > 0 (neighbours outside [0, 512] count as -1) | every bin belongs to its
-//   nearest peak, the lower one on a tie | omega_t[p] = 2 pi p / N + princarg(theta_t[p] - theta_t-1[p] - 2 pi p H / N) / H
-//   (2 pi p / N at t = 0) | psi_t(p) = princarg(psi_t-1[p] + H (r - 1) omega_t[p]), psi_t-1[k] the rotation of the peak
+// Phase vocoder: a peak-locked phase vocoder (Laroche & Dolson 1999) on the denoiser's STFT, fp32 on the device in every
+// vtts_precision mode, with the phase recurrence in double.  It serves two calls, the pitch shifter and the time
+// stretcher, which differ in where the analysis frames sit, in one coefficient of the recurrence and in the bin remap.
+//   STFT n_fft 1024 / periodic Hann / reflect padding 512; analysis frame t centred at a_t | X_t, a = |X_t|, theta =
+//   arg X_t | peaks: a[k] > a[k-1], a[k] >= a[k+1], a[k] > 0 (neighbours outside [0, 512] count as -1) | every bin
+//   belongs to its nearest peak, the lower one on a tie | h_t = a_t - a_t-1 |
+//   omega_t[p] = 2 pi p / N + princarg(theta_t[p] - theta_t-1[p] - 2 pi p h_t / N) / h_t (2 pi p / N at t = 0) |
+//   psi_t(p) = princarg(psi_t-1[p] + (H r - h_t) omega_t[p]) with h_0 = H = 256, psi_t-1[k] the rotation of the peak
 //   that owned bin k in frame t - 1 (0 before frame 0 and in a frame without peaks) | bin k of peak p moves to
 //   k + D_p, D_p = rint((r - 1) p), times (-1)^D_p e^(i psi_t(p)), targets outside [0, 512] dropped, contributions summed
-//   in ascending k | the denoiser's inverse and overlap-add.
-// r = fp32(2^(s / 12)), s in [-12, 12].  Rows with s == 0, and rows of <= 512 samples, are copied.
+//   in ascending k | the denoiser's inverse and overlap-add over the synthesis frames at hop H.
+// Pitch shift: a_t = 256 t, F = n / 256 + 1 frames, r = fp32(2^(s / 12)), s in [-12, 12]; n outputs.  (H r - 256) equals
+//   H (r - 1) exactly in double.  Rows with s == 0, and rows of <= 512 samples, are copied.
+// Time stretch: tempo alpha (fp32, in [0.5, 2], > 1 faster); M = floor(n / (double)alpha + 0.5) outputs, T = M / 256 + 1
+//   frames, a_t = min(rint(256 t (double)alpha), n - 1), r = 1 (so D_p = 0 and psi_0 = 0).  h_t >= 1: a_t rises by at
+//   least 128 until the clamp, and only the last frame can reach it (256 (T - 2) alpha <= n + 1 - 128).  Rows with
+//   alpha == 1, and rows of <= 512 samples, give their first min(n, M) samples, then zeros up to M.
 //
 // Analysis kernel.  One warp per frame, as denoise_frame_kernel: the frame is read and transformed ALONE, so its
 // outputs (X, theta in double, the owner map) are a function of its own 1024 input samples.
@@ -16,13 +23,18 @@
 // the shared rotations makes that one barrier per frame.
 // Synthesis kernel.  One warp per frame: the rotated bins and their targets go to shared memory, lane l then sums the
 // targets [16 l, 16 l + 16) over the sources in ascending order, and the denoiser's inverse transform windows the frame.
-// Overlap-add.  denoise_ola_kernel itself (vtts_denoise_ola).
+// Overlap-add.  denoise_ola_kernel itself (vtts_denoise_ola), over the synthesis frames into the outputs.
 //
-// Stream.  Per slot the denoiser's window (2048 carried inputs plus one chunk), the 64-bit position, the next unscanned
+// Streams.  Per slot the denoiser's window (2048 carried inputs plus one chunk), the 64-bit position, the next unscanned
 // frame, theta and psi (double) of the last scanned frame, and the synthesized frames later outputs still overlap, in
 // two halves that alternate per push (the carried frames are copied from the other half by the synthesis kernel).  A
-// frame is scanned once it reads no input past the ones received (256 g + 512 <= P, and P > 512 for frame 0's
-// reflection), or at END; outputs are released on the denoiser's schedule.
+// frame is scanned once it reads no input past the ones received (a_t + 512 <= P, and P > 512 for frame 0's
+// reflection), or at END; such frames never reach the end clamp or the far reflection, so they equal the one-shot
+// call's.  A frame scanned in a push starts past P0 - 1024 (it was not scannable at P0), so 2048 carried inputs cover
+// every tempo, alpha = 2 included.  The pitch shifter releases outputs on the denoiser's schedule; the time stretcher
+// releases output u once every synthesis frame that weighs it (256 g < u + 512 <= 256 g + 1023; the overlap-add skips
+// the zero-weight sample 0 of a frame) is synthesized: max(0, 256 Q - 511) after Q scanned frames (frame Q - 1 exists
+// in the final row, M >= 256 Q), everything at END, and alpha == 1 slots (copies) everything received.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -43,16 +55,19 @@ constexpr int PH_THREADS = 544;   // phase kernel: one thread per bin (17 warps)
 constexpr int OWN_LD = 514;       // pitch of the int16 owner rows
 constexpr int PS_K = 2048;        // carried inputs per stream slot (as the denoise stream)
 constexpr int PS_LOOKAHEAD = 1023;
+constexpr int TS_LOOKAHEAD = 1536;  // before END a time-stretch slot has released more than P / alpha - 1536 outputs
 constexpr double TWO_PI = 6.283185307179586;
 
 struct PsShift {
-  float r;            // fp32(2^(s / 12))
-  int copy;           // s == 0
+  float r;            // pitch: fp32(2^(s / 12)); time stretch: 1
+  float tempo;        // time stretch: alpha; pitch: 0 (frames at 256 t, no end clamp)
+  int copy;           // s == 0 or alpha == 1
 };
 
 struct PsRow {
   long long x0;       // absolute index of input buffer element 0
   long long n;        // row length (DN_OPEN while a stream slot is open)
+  long long m;        // outputs of the row: n (pitch) or M (time stretch)
   long long q0;       // first frame this call scans (analysis, phase step, synthesis)
   long long fb;       // first frame of the synthesized-frame buffer this call fills
   long long fb_prev;  // stream: first frame of the slot's other half; frames [fb, q0) are copied from it
@@ -61,7 +76,7 @@ struct PsRow {
   int half;           // stream: the half of the slot's frame buffer this call fills
   int copy;           // the outputs are the inputs
   float r;            // ratio
-  int pad_;
+  float tempo;        // as PsShift::tempo
 };
 
 // workspace of one call: per row `fr` analysed frames and `halves` x `nbuf` synthesized frames
@@ -74,6 +89,16 @@ struct PsWs {
   int fr, nbuf, halves;
 };
 
+// M = floor(n / (double)alpha + 0.5): the time stretcher's output length
+__host__ __device__ __forceinline__ long long ts_len(long long n, float tempo) { return (long long)floor((double)n / (double)tempo + 0.5); }
+// rint(256 g (double)alpha): the unclamped centre of analysis frame g of the time stretcher
+__host__ __device__ __forceinline__ long long ts_centre(long long g, float tempo) { return (long long)rint(256.0 * (double)g * (double)tempo); }
+
+// centre a_g of analysis frame g
+__device__ __forceinline__ long long ps_centre(const PsRow& r, long long g) {
+  return r.tempo == 0.f ? g * HOP : min(ts_centre(g, r.tempo), r.n - 1);
+}
+
 // rows == nullptr: the one-shot bounds of row b, n = n_in[b] clamped to [0, S] (or S), every frame scanned in this call
 __device__ __forceinline__ PsRow ps_row(const PsRow* rows, const int* n_in, const PsShift* shifts, int S, int b) {
   if (rows) return rows[b];
@@ -85,10 +110,11 @@ __device__ __forceinline__ PsRow ps_row(const PsRow* rows, const int* n_in, cons
   r.fb_prev = 0;
   r.half = 0;
   r.r = shifts[b].r;
+  r.tempo = shifts[b].tempo;
+  r.m = r.tempo == 0.f ? r.n : ts_len(r.n, r.tempo);
   r.copy = r.n <= PAD || shifts[b].copy;
-  r.nq = r.copy ? 0 : (int)(r.n / HOP + 1);
+  r.nq = r.copy ? 0 : (int)(r.m / HOP + 1);
   r.nsyn = r.nq;
-  r.pad_ = 0;
   return r;
 }
 
@@ -105,7 +131,7 @@ __global__ void __launch_bounds__(PS_WARPS * 32) pitch_analysis_kernel(const flo
   if (fl >= r.nq) return;                                // warps are independent: no block-level barrier below
   float2* sw = smem + (size_t)warp * 32 * TP;
   float2 v[32];
-  stftc::read_frame(v, x + (size_t)b * x_ld, r.x0, r.n, (r.q0 + fl) * HOP - PAD, hann, lane);
+  stftc::read_frame(v, x + (size_t)b * x_ld, r.x0, r.n, ps_centre(r, r.q0 + fl) - PAD, hann, lane);
   stftc::fft1024(v, sw, tw, lane);
 
   // ---- X, theta = atan2 in double, |X| into shared memory ----
@@ -171,28 +197,28 @@ __global__ void __launch_bounds__(PS_WARPS * 32) pitch_analysis_kernel(const flo
 }
 
 // state: stream [rows][2][513] (theta, psi of the last scanned frame) or nullptr; ola: one-shot, receives the rows'
-// overlap-add bounds; dec: [rows][dec_fr][513] decisions, 1 | (e < 0) << 1 at a peak whose wrapped phase deviation is e,
-// 0 elsewhere (test hook)
+// overlap-add bounds (y_cnt outputs per row); dec: [rows][dec_fr][513] decisions, 1 | (e < 0) << 1 at a peak whose
+// wrapped phase deviation is e, 0 elsewhere (test hook)
 __global__ void __launch_bounds__(PH_THREADS) pitch_phase_kernel(const int* __restrict__ n_in, const PsShift* __restrict__ shifts,
                                                                 const PsRow* __restrict__ rows, int S, PsWs w, double* __restrict__ state,
-                                                                DnRow* __restrict__ ola, int* __restrict__ dec, int dec_fr) {
+                                                                DnRow* __restrict__ ola, long long y_cnt, int* __restrict__ dec, int dec_fr) {
   __shared__ double ps_sh[2][NB];
   const int b = blockIdx.x, k = threadIdx.x;
   const PsRow r = ps_row(rows, n_in, shifts, S, b);
   if (ola && k == 0) {
     DnRow d;
     d.x0 = 0;
-    d.n = r.n;
+    d.n = r.copy ? min(r.n, r.m) : r.m;
     d.g0 = 0;
     d.e0 = 0;
-    d.cnt = S;
+    d.cnt = y_cnt;
     d.nfr = r.nq;
     d.copy = r.copy;
     ola[b] = d;
   }
   if (r.nq == 0) return;                                 // uniform over the CTA
   const bool bin = k < NB;
-  const double hr1 = HOP * ((double)r.r - 1.0);
+  const double hr = HOP * (double)r.r;                   // the rotation advances by (H r - h_t) omega
   double thp = 0.0, psp = 0.0;
   if (state && bin) {
     thp = state[(size_t)b * 2 * NB + k];
@@ -201,8 +227,10 @@ __global__ void __launch_bounds__(PH_THREADS) pitch_phase_kernel(const int* __re
   const size_t f0 = (size_t)b * w.fr;
   int own = bin ? w.own[f0 * OWN_LD + k] : -1;
   double th = bin ? w.th[f0 * NB + k] : 0.0;
+  long long a_prev = ps_centre(r, r.q0 - 1);
   for (int i = 0; i < r.nq; ++i) {
     const long long g = r.q0 + i;
+    const long long a = ps_centre(r, g);
     int own_n = -1;
     double th_n = 0.0;
     if (bin && i + 1 < r.nq) {                           // the next frame's loads fly under this frame's step
@@ -211,14 +239,15 @@ __global__ void __launch_bounds__(PH_THREADS) pitch_phase_kernel(const int* __re
     }
     int neg = 0;
     if (own == k) {
+      const double h = g > 0 ? (double)(a - a_prev) : (double)HOP;
       double om = TWO_PI * k / NF, prev = 0.0;
       if (g > 0) {
-        const double e = princarg(th - thp - TWO_PI * k * HOP / NF);
+        const double e = princarg(th - thp - TWO_PI * k * h / NF);
         neg = e < 0.0;
-        om += e / HOP;
+        om += e / h;
         prev = psp;
       }
-      ps_sh[i & 1][k] = princarg(prev + hr1 * om);
+      ps_sh[i & 1][k] = princarg(prev + (hr - h) * om);
     }
     __syncthreads();
     const double ps = own >= 0 ? ps_sh[i & 1][own] : 0.0;
@@ -230,6 +259,7 @@ __global__ void __launch_bounds__(PH_THREADS) pitch_phase_kernel(const int* __re
     thp = th;
     own = own_n;
     th = th_n;
+    a_prev = a;
   }
   if (state && bin) {
     state[(size_t)b * 2 * NB + k] = thp;
@@ -293,6 +323,7 @@ __global__ void __launch_bounds__(PS_WARPS * 32) pitch_synth_kernel(const int* _
 }
 
 bool shift_ok(float s) { return std::isfinite(s) && s >= -12.f && s <= 12.f; }
+bool tempo_ok(float a) { return std::isfinite(a) && a >= 0.5f && a <= 2.f; }
 
 int ps_check_shifts(vtts_ctx* ctx, const char* who, const float* semitones, int n) {
   if (!semitones) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: null semitones", who);
@@ -302,8 +333,17 @@ int ps_check_shifts(vtts_ctx* ctx, const char* who, const float* semitones, int 
   return VTTS_OK;
 }
 
+int ts_check_tempos(vtts_ctx* ctx, const char* who, const float* tempo, int n) {
+  if (!tempo) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: null tempo", who);
+  for (int i = 0; i < n; ++i)
+    if (!tempo_ok(tempo[i])) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: tempo[%d] = %g (finite, in [0.5, 2])", who, i, (double)tempo[i]);
+  return VTTS_OK;
+}
+
 // fp32(2^(s / 12)), computed in double and rounded once
 float ps_ratio(float s) { return (float)std::pow(2.0, (double)s / 12.0); }
+PsShift ps_params(float s) { return PsShift{ps_ratio(s), 0.f, s == 0.f}; }
+PsShift ts_params(float tempo) { return PsShift{1.f, tempo, tempo == 1.f}; }
 
 void ps_carve(Arena& a, PsWs& w, int rows) {
   w.X = a.take<float2>((size_t)rows * w.fr * NB);
@@ -315,13 +355,14 @@ void ps_carve(Arena& a, PsWs& w, int rows) {
 
 // analysis, phase, synthesis (three launches); the synthesis is skipped when only the decisions are wanted
 int ps_launch(vtts_ctx* ctx, const float* x, long long x_ld, int S, const int* n_in, const PsShift* shifts, const PsRow* rows, int B,
-              long long max_nq, long long max_nsyn, const PsWs& w, double* state, DnRow* ola, int* dec, int dec_fr, cudaStream_t st) {
+              long long max_nq, long long max_nsyn, const PsWs& w, double* state, DnRow* ola, long long y_cnt, int* dec, int dec_fr,
+              cudaStream_t st) {
   const float2* tw = reinterpret_cast<const float2*>(ctx->fft_tw);
   const unsigned agrid = (unsigned)std::max(1LL, (max_nq + PS_WARPS - 1) / PS_WARPS);
   pitch_analysis_kernel<<<dim3(agrid, B), PS_WARPS * 32, 0, st>>>(x, x_ld, S, n_in, shifts, rows, ctx->hann, tw, w);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
-  pitch_phase_kernel<<<B, PH_THREADS, 0, st>>>(n_in, shifts, rows, S, w, state, ola, dec, dec_fr);
+  pitch_phase_kernel<<<B, PH_THREADS, 0, st>>>(n_in, shifts, rows, S, w, state, ola, y_cnt, dec, dec_fr);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   if (dec) return VTTS_OK;
@@ -332,22 +373,24 @@ int ps_launch(vtts_ctx* ctx, const float* x, long long x_ld, int S, const int* n
   return VTTS_OK;
 }
 
-// one-shot call (dec == nullptr) or the decisions test hook
-int ps_one_shot(vtts_ctx* ctx, const char* who, const float* x_dev, const int32_t* n_dev, int B, int S, const float* semitones, float* y_dev,
-                int* dec_dev, cudaStream_t st) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!x_dev || !(y_dev || dec_dev)) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: null pointer", who);
+// the pointer and shape rejections of a one-shot call, before its parameters are looked at
+int ps_check_call(vtts_ctx* ctx, const char* who, const float* x_dev, const void* out_dev, const float* y_dev, int B, int S) {
+  if (!x_dev || !out_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: null pointer", who);
   if (x_dev == y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: y must not alias x", who);
   if (B < 1 || B > 65535 || S < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: B=%d S=%d (1..65535, >= 1)", who, B, S);
-  int rc = ps_check_shifts(ctx, who, semitones, B);
-  if (rc) return rc;
+  return VTTS_OK;
+}
+
+// one-shot call (dec == nullptr) or the decisions test hook, on checked arguments: rows with the parameters h, F
+// analysis frames for the longest row, Sy outputs per row
+int ps_one_shot(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const std::vector<PsShift>& h, long long F, int Sy,
+                float* y_dev, int* dec_dev, cudaStream_t st) {
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  rc = vtts_fft_tables(ctx);
+  int rc = vtts_fft_tables(ctx);
   if (rc) return rc;
-  const int F = S / HOP + 1;
   PsWs w{};
-  w.fr = F;
-  w.nbuf = F;
+  w.fr = (int)F;
+  w.nbuf = (int)F;
   w.halves = 1;
   Arena m(nullptr, 0, true);
   m.take<PsShift>(B);
@@ -359,17 +402,45 @@ int ps_one_shot(vtts_ctx* ctx, const char* who, const float* x_dev, const int32_
   PsShift* shifts = a.take<PsShift>(B);
   DnRow* ola = a.take<DnRow>(B);
   ps_carve(a, w, B);
-  std::vector<PsShift> h(B);
-  for (int b = 0; b < B; ++b) h[b] = PsShift{ps_ratio(semitones[b]), semitones[b] == 0.f};
   // pageable source: the call returns once the table is staged
   VTTS_CUDA(cudaMemcpyAsync(shifts, h.data(), (size_t)B * sizeof(PsShift), cudaMemcpyHostToDevice, st));
   if (dec_dev) {
     VTTS_CUDA(cudaMemsetAsync(dec_dev, 0, (size_t)B * F * NB * sizeof(int), st));
-    return ps_launch(ctx, x_dev, S, S, n_dev, shifts, nullptr, B, F, F, w, nullptr, nullptr, dec_dev, F, st);
+    return ps_launch(ctx, x_dev, S, S, n_dev, shifts, nullptr, B, F, F, w, nullptr, nullptr, 0, dec_dev, (int)F, st);
   }
-  rc = ps_launch(ctx, x_dev, S, S, n_dev, shifts, nullptr, B, F, F, w, nullptr, ola, nullptr, 0, st);
+  rc = ps_launch(ctx, x_dev, S, S, n_dev, shifts, nullptr, B, F, F, w, nullptr, ola, Sy, nullptr, 0, st);
   if (rc) return rc;
-  return vtts_denoise_ola(ctx, x_dev, S, S, nullptr, ola, B, S, w.syn, w.nbuf, y_dev, S, st);
+  return vtts_denoise_ola(ctx, x_dev, S, S, nullptr, ola, B, Sy, w.syn, w.nbuf, y_dev, Sy, st);
+}
+
+int ps_call(vtts_ctx* ctx, const char* who, const float* x_dev, const int32_t* n_dev, int B, int S, const float* semitones, float* y_dev,
+            int* dec_dev, cudaStream_t st) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  int rc = ps_check_call(ctx, who, x_dev, y_dev ? (const void*)y_dev : (const void*)dec_dev, y_dev, B, S);
+  if (!rc) rc = ps_check_shifts(ctx, who, semitones, B);
+  if (rc) return rc;
+  std::vector<PsShift> h(B);
+  for (int b = 0; b < B; ++b) h[b] = ps_params(semitones[b]);
+  return ps_one_shot(ctx, x_dev, n_dev, B, S, h, S / HOP + 1, S, y_dev, dec_dev, st);
+}
+
+// frames of the longest time-stretched row of S samples: max over the rows of M(S) / 256 + 1
+long long ts_frames(const float* tempo, int B, int S) {
+  long long F = 1;
+  for (int b = 0; b < B; ++b) F = std::max(F, ts_len(S, tempo[b]) / HOP + 1);
+  return F;
+}
+
+int ts_call(vtts_ctx* ctx, const char* who, const float* x_dev, const int32_t* n_dev, int B, int S, const float* tempo, float* y_dev, int Sy,
+            int* dec_dev, cudaStream_t st) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  int rc = ps_check_call(ctx, who, x_dev, y_dev ? (const void*)y_dev : (const void*)dec_dev, y_dev, B, S);
+  if (!rc && y_dev && Sy < 1) rc = ctx->fail(VTTS_ERR_BAD_ARG, "%s: Sy=%d (>= 1)", who, Sy);
+  if (!rc) rc = ts_check_tempos(ctx, who, tempo, B);
+  if (rc) return rc;
+  std::vector<PsShift> h(B);
+  for (int b = 0; b < B; ++b) h[b] = ts_params(tempo[b]);
+  return ps_one_shot(ctx, x_dev, n_dev, B, S, h, ts_frames(tempo, B, S), Sy, y_dev, dec_dev, st);
 }
 
 }  // namespace
@@ -379,13 +450,13 @@ int vtts_pitch_shift_stream_lookahead(void) { return PS_LOOKAHEAD; }
 int vtts_pitch_shift(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const float* semitones, float* y_dev,
                      void* stream) {
   if (ctx && !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift: null pointer");
-  return ps_one_shot(ctx, "pitch_shift", x_dev, n_dev, B, S, semitones, y_dev, nullptr, (cudaStream_t)stream);
+  return ps_call(ctx, "pitch_shift", x_dev, n_dev, B, S, semitones, y_dev, nullptr, (cudaStream_t)stream);
 }
 
 int vtts_debug_pitch_decisions(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const float* semitones, int32_t* dec_dev,
                                void* stream) {
   if (ctx && !dec_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "debug_pitch_decisions: null pointer");
-  return ps_one_shot(ctx, "debug_pitch_decisions", x_dev, n_dev, B, S, semitones, nullptr, dec_dev, (cudaStream_t)stream);
+  return ps_call(ctx, "debug_pitch_decisions", x_dev, n_dev, B, S, semitones, nullptr, dec_dev, (cudaStream_t)stream);
 }
 
 int vtts_pitch_shift_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, const float* semitones, float* y) {
@@ -408,46 +479,103 @@ int vtts_pitch_shift_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, in
   return rc ? rc : hs.finish();
 }
 
-// ---- stream ---------------------------------------------------------------------------------------------------
-struct vtts_pitch_shift_stream : StreamBase {
+int64_t vtts_time_stretch_length(int64_t n, float tempo) { return n < 0 || !tempo_ok(tempo) ? -1 : ts_len(n, tempo); }
+
+int vtts_time_stretch_stream_lookahead(void) { return TS_LOOKAHEAD; }
+
+int vtts_time_stretch(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const float* tempo, float* y_dev, int Sy,
+                      void* stream) {
+  if (ctx && !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "time_stretch: null pointer");
+  return ts_call(ctx, "time_stretch", x_dev, n_dev, B, S, tempo, y_dev, Sy, nullptr, (cudaStream_t)stream);
+}
+
+int vtts_debug_time_stretch_decisions(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const float* tempo,
+                                      int32_t* dec_dev, void* stream) {
+  if (ctx && !dec_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "debug_time_stretch_decisions: null pointer");
+  return ts_call(ctx, "debug_time_stretch_decisions", x_dev, n_dev, B, S, tempo, nullptr, 0, dec_dev, (cudaStream_t)stream);
+}
+
+int vtts_time_stretch_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, const float* tempo, float* y, int Sy) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  if (!x || !y || B < 1 || B > 65535 || S < 1 || Sy < 1)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "time_stretch_host: bad argument (B=%d S=%d Sy=%d)", B, S, Sy);
+  int rc = ts_check_tempos(ctx, "time_stretch_host", tempo, B);
+  if (rc) return rc;
+  if (n_in)
+    for (int b = 0; b < B; ++b)
+      if (n_in[b] < 0 || n_in[b] > S) return ctx->fail(VTTS_ERR_BAD_ARG, "time_stretch_host: n[%d]=%d outside [0, %d]", b, n_in[b], S);
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  const size_t x_b = (size_t)B * S * 4, y_b = (size_t)B * Sy * 4;
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, (size_t)B * 4), o_y = hs.out(y_b);
+  rc = hs.upload();
+  if (!rc)
+    rc = vtts_time_stretch(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, tempo, hs.dev<float>(o_y), Sy,
+                           hs.st);
+  if (!rc) rc = hs.fetch(o_y, y, y_b);
+  return rc ? rc : hs.finish();
+}
+
+// ---- streams ---------------------------------------------------------------------------------------------------
+// One implementation serves both vocoder streams; `stretch` selects the time stretcher's frame positions and schedule.
+struct PvStream : StreamBase {
   using StreamBase::StreamBase;
   int cap = 0, out_pitch = 0;
+  bool stretch = false;
   PsWs w{};
   float* win = nullptr;         // windows [S][cap]
   double* state = nullptr;      // [S][2][513]
   char* d_tbl = nullptr;        // the per-push tables, laid out as their host image tbl: DnRow [S], PsRow [S], int [S][2]
   // per slot besides the shared state: next unscanned frame, first frame and half of the last push's synthesized-frame
-  // buffer, shift since BEGIN
+  // buffer, shift or tempo since BEGIN
   std::vector<long long> q, fb;
   std::vector<int> half;
-  std::vector<float> semis;
+  std::vector<float> par;
   std::vector<char> tbl;
 };
+struct vtts_pitch_shift_stream : PvStream {
+  using PvStream::PvStream;
+};
+struct vtts_time_stretch_stream : PvStream {
+  using PvStream::PvStream;
+};
 
-int vtts_pitch_shift_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, vtts_pitch_shift_stream** out, int* out_pitch) {
+namespace {
+
+// frames scanned per push (at most fr), outputs per push (out_pitch) and the slots' neutral parameter
+template <class Stream>
+int pv_create(vtts_ctx* ctx, const char* who, int max_streams, int max_chunk_samples, bool stretch, Stream** out, int* out_pitch) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out || !out_pitch) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_create: null pointer");
+  if (!out || !out_pitch) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: null pointer", who);
   *out = nullptr;
   if (max_streams < 1 || max_streams > 65535 || max_chunk_samples < 1 || max_chunk_samples > (1 << 22))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_create: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", max_streams,
-                     max_chunk_samples, 1 << 22);
+    return ctx->fail(VTTS_ERR_BAD_ARG, "%s: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", who, max_streams, max_chunk_samples,
+                     1 << 22);
   VTTS_CUDA(cudaSetDevice(ctx->device));
   int rc = vtts_fft_tables(ctx);
   if (rc) return rc;
   const int S = max_streams;
-  std::unique_ptr<vtts_pitch_shift_stream> ps(new vtts_pitch_shift_stream(ctx, S, max_chunk_samples));
+  std::unique_ptr<Stream> ps(new Stream(ctx, S, max_chunk_samples));
+  ps->stretch = stretch;
   ps->cap = PS_K + max_chunk_samples;
-  ps->out_pitch = max_chunk_samples + PS_LOOKAHEAD;    // as the denoise stream
-  // frames scanned per push: at most n_new / 256 + 3 (with END); the buffer also holds the <= 3 carried frames
-  ps->w.fr = max_chunk_samples / HOP + 4;
+  if (!stretch) {
+    ps->out_pitch = max_chunk_samples + PS_LOOKAHEAD;  // as the denoise stream
+    // frames scanned per push: at most n_new / 256 + 3 (with END); the buffer also holds the <= 3 carried frames
+    ps->w.fr = max_chunk_samples / HOP + 4;
+  } else {
+    // outputs per push: at most 2 n_new + 256 before END, (n_new + 512.5) / alpha + 512.5 with it; frames scanned: at
+    // most n_new / 128 + 1 before END, (n_new + 512.5) / (256 alpha) + 2.01 with it
+    ps->out_pitch = 2 * max_chunk_samples + 2048;
+    ps->w.fr = max_chunk_samples / 128 + 8;
+  }
   ps->w.nbuf = ps->w.fr + 4;
   ps->w.halves = 2;
   ps->q.assign(S, 0);
   ps->fb.assign(S, 0);
   ps->half.assign(S, 0);
-  ps->semis.assign(S, 0.f);
+  ps->par.assign(S, stretch ? 1.f : 0.f);
   ps->tbl.assign((size_t)S * (sizeof(DnRow) + sizeof(PsRow) + 2 * sizeof(int)), 0);
-  rc = stream_alloc(ctx, "pitch_shift_stream_create", *ps, [&](Arena& a) {
+  rc = stream_alloc(ctx, who, *ps, [&](Arena& a) {
     ps->win = a.take<float>((size_t)S * ps->cap);
     ps_carve(a, ps->w, S);
     ps->state = a.take<double>((size_t)S * 2 * NB);
@@ -459,24 +587,31 @@ int vtts_pitch_shift_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk
   return VTTS_OK;
 }
 
-int vtts_pitch_shift_stream_destroy(vtts_ctx* ctx, vtts_pitch_shift_stream* ps) {
-  return stream_destroy(ctx, "pitch_shift_stream_destroy", ps);
-}
-
-int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
-                                 const float* semitones, float* y_dev, int32_t* n_out, void* stream) {
+// par: semitones (pitch) or tempo (time stretch) per slot, read with BEGIN
+int pv_push(vtts_ctx* ctx, const char* who, PvStream* ps, const float* x_dev, const int32_t* n_new, const uint8_t* flags, const float* par,
+            float* y_dev, int32_t* n_out, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = stream_args(ctx, "pitch_shift_stream_push", ps, x_dev && n_new && flags && y_dev && n_out);
+  int rc = stream_args(ctx, who, ps, x_dev && n_new && flags && y_dev && n_out);
   if (rc) return rc;
-  if (x_dev == y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_push: y must not alias x");
-  rc = ps->slots.check(ctx, "pitch_shift_stream_push", ps->F, n_new, flags, [&](int s) -> int {
+  if (x_dev == y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: y must not alias x", who);
+  const bool stretch = ps->stretch;
+  rc = ps->slots.check(ctx, who, ps->F, n_new, flags, [&](int s) -> int {
+    if (stretch) {
+      if (flags[s] & 1) {
+        if (!par) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: BEGIN needs the tempo array", who);
+        if (!tempo_ok(par[s])) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: tempo[%d] = %g (finite, in [0.5, 2])", who, s, (double)par[s]);
+      } else if (par && !(par[s] == ps->par[s])) {
+        return ctx->fail(VTTS_ERR_BAD_ARG, "%s: tempo[%d] = %g, but slot %d runs at tempo %g until END (BEGIN to change it)", who, s,
+                         (double)par[s], s, (double)ps->par[s]);
+      }
+      return VTTS_OK;
+    }
     if (flags[s] & 1) {
-      if (!semitones) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_push: BEGIN needs the semitones array");
-      if (!shift_ok(semitones[s]))
-        return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_push: semitones[%d] = %g (finite, in [-12, 12])", s, (double)semitones[s]);
-    } else if (semitones && !(semitones[s] == ps->semis[s])) {
-      return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_stream_push: semitones[%d] = %g, but slot %d shifts by %g until END (BEGIN to change it)",
-                       s, (double)semitones[s], s, (double)ps->semis[s]);
+      if (!par) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: BEGIN needs the semitones array", who);
+      if (!shift_ok(par[s])) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: semitones[%d] = %g (finite, in [-12, 12])", who, s, (double)par[s]);
+    } else if (par && !(par[s] == ps->par[s])) {
+      return ctx->fail(VTTS_ERR_BAD_ARG, "%s: semitones[%d] = %g, but slot %d shifts by %g until END (BEGIN to change it)", who, s,
+                       (double)par[s], s, (double)ps->par[s]);
     }
     return VTTS_OK;
   });
@@ -495,23 +630,41 @@ int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, con
   for (int s = 0; s < S; ++s) {
     const bool act = SlotState::active(n_new, flags, s), begin = flags[s] & 1, end = flags[s] & 2;
     const long long P0 = begin ? 0 : sl.P[s], E0 = begin ? 0 : sl.E[s], P1 = P0 + n_new[s];
-    const float sm = begin ? semitones[s] : ps->semis[s];
-    long long e = E0;
-    if (act) e = end ? P1 : std::min(P1, (long long)HOP * std::max(0LL, P1 / HOP - 3));
-    E1[s] = e;
-    n_out[s] = (int32_t)(e - E0);
+    const float pv = begin ? par[s] : ps->par[s];
+    const PsShift h = stretch ? ts_params(pv) : ps_params(pv);
+    const long long M1 = end ? (stretch ? ts_len(P1, pv) : P1) : DN_OPEN;   // the row's outputs, once known
     DnRow r{};
     PsRow p{};
     r.x0 = p.x0 = P0 - PS_K;
-    r.n = p.n = end ? P1 : DN_OPEN;
+    p.n = end ? P1 : DN_OPEN;
+    p.m = M1;
+    r.copy = p.copy = h.copy || (end && P1 <= PAD);
+    r.n = end && r.copy ? std::min(P1, M1) : M1;
+    p.r = h.r;
+    p.tempo = h.tempo;
+    const long long q0 = begin ? 0 : ps->q[s];
+    long long q1 = q0;
+    if (act && !p.copy) {
+      if (end) {
+        q1 = M1 / HOP + 1;
+      } else if (!stretch) {
+        q1 = P1 > PAD ? (P1 - PAD) / HOP + 1 : 0;
+      } else {
+        while (P1 > PAD && ts_centre(q1, pv) + PAD <= P1) ++q1;
+      }
+    }
+    long long e = E0;
+    if (act) {
+      if (end) e = M1;
+      else if (!stretch) e = std::min(P1, (long long)HOP * std::max(0LL, P1 / HOP - 3));
+      else e = h.copy ? P1 : std::max(0LL, HOP * q1 - (PAD - 1));
+    }
+    E1[s] = e;
+    n_out[s] = (int32_t)(e - E0);
     r.e0 = E0;
     r.cnt = e - E0;
-    r.copy = p.copy = sm == 0.f || (end && P1 <= PAD);
-    p.r = ps_ratio(sm);
-    const long long q0 = begin ? 0 : ps->q[s];
     Q1[s] = q0;
     if (act && !p.copy) {
-      const long long q1 = end ? P1 / HOP + 1 : (P1 > PAD ? (P1 - PAD) / HOP + 1 : 0);
       const long long p0 = E0 + PAD;
       const long long fb = p0 >= NF - 1 ? (p0 - (NF - 1) + HOP - 1) / HOP : 0;
       p.q0 = q0;
@@ -524,11 +677,11 @@ int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, con
       if (r.cnt > 0) r.nfr = (int)(std::min(r.n / HOP, (e - 1 + PAD) / HOP) - fb + 1);
       Q1[s] = q1;
       if (fb > q0 || q1 < q0 || (!begin && fb < ps->fb[s]) || p.nq > ps->w.fr || p.nsyn > ps->w.nbuf)
-        return ctx->fail(VTTS_ERR_CUDA, "pitch_shift_stream_push: slot %d frames [%lld, %lld) buffer from %lld (internal bound %d / %d)", s, q0,
-                         q1, fb, ps->w.fr, ps->w.nbuf);
+        return ctx->fail(VTTS_ERR_CUDA, "%s: slot %d frames [%lld, %lld) buffer from %lld (internal bound %d / %d)", who, s, q0, q1, fb,
+                         ps->w.fr, ps->w.nbuf);
     }
     if (r.cnt > ps->out_pitch)
-      return ctx->fail(VTTS_ERR_CUDA, "pitch_shift_stream_push: slot %d needs %lld outputs (internal bound %d)", s, r.cnt, ps->out_pitch);
+      return ctx->fail(VTTS_ERR_CUDA, "%s: slot %d needs %lld outputs (internal bound %d)", who, s, r.cnt, ps->out_pitch);
     rows[s] = r;
     prow[s] = p;
     max_out = std::max(max_out, r.cnt);
@@ -545,7 +698,7 @@ int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, con
   const int* d_prep = reinterpret_cast<const int*>(ps->d_tbl + (size_t)S * (sizeof(DnRow) + sizeof(PsRow)));
   rc = vtts_stream_window_prep(ctx, ps->win, ps->cap, PS_K, d_prep, x_dev, ps->F, S, st);
   if (rc) return rc;
-  rc = ps_launch(ctx, ps->win, ps->cap, ps->cap, nullptr, nullptr, d_prow, S, max_nq, max_nsyn, ps->w, ps->state, nullptr, nullptr, 0, st);
+  rc = ps_launch(ctx, ps->win, ps->cap, ps->cap, nullptr, nullptr, d_prow, S, max_nq, max_nsyn, ps->w, ps->state, nullptr, 0, nullptr, 0, st);
   if (rc) return rc;
   rc = vtts_denoise_ola(ctx, ps->win, ps->cap, ps->cap, nullptr, d_rows, S, max_out, ps->w.syn, 2 * ps->w.nbuf, y_dev, ps->out_pitch, st);
   if (rc) return rc;
@@ -554,7 +707,7 @@ int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, con
   for (int s = 0; s < S; ++s) {
     if (!SlotState::active(n_new, flags, s)) continue;
     const bool begin = flags[s] & 1;
-    if (begin) ps->semis[s] = semitones[s];
+    if (begin) ps->par[s] = par[s];
     if (prow[s].nsyn > 0 || prow[s].nq > 0) {
       ps->fb[s] = prow[s].fb;
       ps->half[s] = prow[s].half;
@@ -568,13 +721,51 @@ int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, con
   return VTTS_OK;
 }
 
-int vtts_pitch_shift_stream_push_host(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x, const int32_t* n_new, const uint8_t* flags,
-                                      const float* semitones, float* y, int32_t* n_out) {
+int pv_push_host(vtts_ctx* ctx, const char* who, PvStream* ps, const float* x, const int32_t* n_new, const uint8_t* flags, const float* par,
+                 float* y, int32_t* n_out, const char* push_who) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = stream_args(ctx, "pitch_shift_stream_push_host", ps, x && y);
+  int rc = stream_args(ctx, who, ps, x && y);
   if (rc) return rc;
   return stream_push_host(ctx, x, (size_t)ps->S * ps->F * 4, y, (size_t)ps->S * ps->out_pitch * 4,
                           [&](const float* x_dev, float* y_dev, cudaStream_t st) {
-                            return vtts_pitch_shift_stream_push(ctx, ps, x_dev, n_new, flags, semitones, y_dev, n_out, st);
+                            return pv_push(ctx, push_who, ps, x_dev, n_new, flags, par, y_dev, n_out, st);
                           });
+}
+
+}  // namespace
+
+int vtts_pitch_shift_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, vtts_pitch_shift_stream** out, int* out_pitch) {
+  return pv_create(ctx, "pitch_shift_stream_create", max_streams, max_chunk_samples, false, out, out_pitch);
+}
+
+int vtts_pitch_shift_stream_destroy(vtts_ctx* ctx, vtts_pitch_shift_stream* ps) {
+  return stream_destroy(ctx, "pitch_shift_stream_destroy", ps);
+}
+
+int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
+                                 const float* semitones, float* y_dev, int32_t* n_out, void* stream) {
+  return pv_push(ctx, "pitch_shift_stream_push", ps, x_dev, n_new, flags, semitones, y_dev, n_out, stream);
+}
+
+int vtts_pitch_shift_stream_push_host(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x, const int32_t* n_new, const uint8_t* flags,
+                                      const float* semitones, float* y, int32_t* n_out) {
+  return pv_push_host(ctx, "pitch_shift_stream_push_host", ps, x, n_new, flags, semitones, y, n_out, "pitch_shift_stream_push");
+}
+
+int vtts_time_stretch_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, vtts_time_stretch_stream** out, int* out_pitch) {
+  return pv_create(ctx, "time_stretch_stream_create", max_streams, max_chunk_samples, true, out, out_pitch);
+}
+
+int vtts_time_stretch_stream_destroy(vtts_ctx* ctx, vtts_time_stretch_stream* ts) {
+  return stream_destroy(ctx, "time_stretch_stream_destroy", ts);
+}
+
+int vtts_time_stretch_stream_push(vtts_ctx* ctx, vtts_time_stretch_stream* ts, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
+                                  const float* tempo, float* y_dev, int32_t* n_out, void* stream) {
+  return pv_push(ctx, "time_stretch_stream_push", ts, x_dev, n_new, flags, tempo, y_dev, n_out, stream);
+}
+
+int vtts_time_stretch_stream_push_host(vtts_ctx* ctx, vtts_time_stretch_stream* ts, const float* x, const int32_t* n_new,
+                                       const uint8_t* flags, const float* tempo, float* y, int32_t* n_out) {
+  return pv_push_host(ctx, "time_stretch_stream_push_host", ts, x, n_new, flags, tempo, y, n_out, "time_stretch_stream_push");
 }

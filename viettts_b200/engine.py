@@ -77,6 +77,20 @@ def _semitones(v, n: int) -> np.ndarray:
     return a
 
 
+MIN_TEMPO, MAX_TEMPO = 0.5, 2.0
+
+
+def _tempo(v, n: int) -> np.ndarray:
+    """float32 [n]: a scalar tempo for every row, or one per row, each finite and in [0.5, 2]"""
+    a = np.asarray(v, np.float32)
+    a = np.full(n, a, np.float32) if a.ndim == 0 else np.ascontiguousarray(a.reshape(-1), np.float32)
+    if a.shape != (n,):
+        raise ValueError(f"tempo: one value or one per row ({n}), got {np.shape(v)}")
+    if not (np.all(np.isfinite(a)) and np.all((a >= MIN_TEMPO) & (a <= MAX_TEMPO))):
+        raise ValueError(f"tempo must be finite and lie in [0.5, 2], got {v}")
+    return a
+
+
 def _ptr(a):
     if a is None:
         return None
@@ -349,7 +363,7 @@ class Engine:
         return AcousticStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, masks=masks)
 
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
-                        rng=None, output_rate=None, denoise=None, meter=False, semitones=None) -> "TtsStream":
+                        rng=None, output_rate=None, denoise=None, meter=False, semitones=None, tempo=None) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
         With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  `output_rate`: a resample
@@ -358,11 +372,13 @@ class Engine:
         between the vocoder and the resampler, and the audio equals `denoise` of the `tts` audio (then resampled) bit for
         bit.  `semitones`: a pitch-shift stream follows the denoiser (before the resampler) with this shift as every slot's
         default (`begin(..., semitones=)` overrides it per slot), and the audio equals `pitch_shift` of the (denoised)
-        `tts` audio bit for bit.  `meter=True`: a loudness meter runs last, on what `step()` returns at the output rate (a
+        `tts` audio bit for bit.  `tempo`: a time-stretch stream follows the pitch shifter (before the resampler) with this
+        tempo as every slot's default (`begin(..., tempo=)` overrides it per slot), and the audio equals `time_stretch` of
+        the (denoised, pitch-shifted) `tts` audio bit for bit.  `meter=True`: a loudness meter runs last, on what `step()` returns at the output rate (a
         multiple of 10), and `TtsStream.meter()` gives each stepped slot's readings, read back in the step's one
         synchronisation.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
         return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate,
-                         denoise=denoise, meter=meter, semitones=semitones)
+                         denoise=denoise, meter=meter, semitones=semitones, tempo=tempo)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -853,6 +869,69 @@ class Engine:
         for bit.  Outputs are released on the denoise stream's schedule (at most 1023 samples after their own time)."""
         return PitchShiftStream(self, max_streams, max_chunk_samples)
 
+    # ---- time stretch (vtts_time_stretch*: the pitch shifter's phase vocoder with analysis frames at 256 t alpha) ----
+    def time_stretch_length(self, n: int, tempo: float) -> int:
+        """M = floor(n / alpha + 0.5) (in double, alpha the fp32 tempo): the samples `time_stretch` makes of n"""
+        m = int(self.lib.vtts_time_stretch_length(int(n), float(_tempo(tempo, 1)[0])))
+        if m < 0:
+            raise ValueError(f"time_stretch_length: n={n} must be >= 0")
+        return m
+
+    def time_stretch(self, wav, tempo, lengths=None) -> np.ndarray:
+        """Host arrays: wav f32 [S] -> [M], or [B,S] -> [B, max_b M_b], played `tempo` times as fast with the pitch kept
+        (a peak-locked phase vocoder, n_fft 1024, synthesis hop 256); M_b = floor(n_b / tempo_b + 0.5) and row b is zero
+        past M_b.  tempo: a scalar or one value per row, finite and in [0.5, 2]; rows at 1 and rows of <= 512 samples
+        give their first min(n, M) samples.  lengths int [B] in [0, S]: row b holds lengths[b] samples."""
+        x, one = _wav_rows(wav)
+        B, S = x.shape
+        tp = _tempo(tempo, B)
+        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
+        n = np.full(B, S) if lens is None else lens
+        Sy = max((self.time_stretch_length(int(n[b]), tp[b]) for b in range(B)), default=0)
+        if S == 0 or B == 0 or Sy == 0:
+            y = np.zeros((B, Sy), np.float32)
+            for b in range(B):
+                k = min(int(n[b]), Sy)
+                y[b, :k] = x[b, :k]                     # nothing to transform: empty rows are short rows
+            return y[0] if one else y
+        y = np.empty((B, Sy), np.float32)
+        self._ck(self.lib.vtts_time_stretch_host(self.h, _ptr(x), _ptr(lens), B, S, _ptr(tp), _ptr(y), Sy))
+        return y[0] if one else y
+
+    def time_stretch_forward(self, x_t, tempo, lengths_t=None, out=None, stream=None):
+        """vtts_time_stretch on torch CUDA tensors, stream-ordered: x_t f32 [B,S] -> [B, Sy] (not x_t), Sy = out's width or
+        max_b time_stretch_length(S, tempo_b); tempo a scalar or one host value per row; lengths_t int32 CUDA [B] or None."""
+        import torch
+        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
+        B, S = x_t.shape
+        tp = _tempo(tempo, B)
+        if out is None:
+            out = _out_tensor(None, (B, max(self.time_stretch_length(S, a) for a in tp)), x_t.device)
+        elif out.dim() != 2 or out.shape[0] != B or out.shape[1] < 1 or out.dtype != torch.float32 or not out.is_contiguous():
+            raise ValueError(f"out must be contiguous float32 [{B}, Sy >= 1]")
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self._ck(self.lib.vtts_time_stretch(self.h, _ptr(x_t), _ptr(lengths_t), B, S, _ptr(tp), _ptr(out), int(out.shape[1]), st))
+        return out
+
+    def debug_time_stretch_decisions(self, x_t, tempo, lengths_t=None) -> np.ndarray:
+        """Test hook (vtts_debug_time_stretch_decisions): int32 [B, T_max, 513], T_max = max_b time_stretch_length(S,
+        tempo_b) // 256 + 1, the device's peak flags (bit 0) and princarg sides (bit 1: negative), as
+        `debug_pitch_decisions` encodes them, for `time_stretch_forward` of the same arguments."""
+        import torch
+        B, S = x_t.shape
+        tp = _tempo(tempo, B)
+        T = max(self.time_stretch_length(S, a) for a in tp) // config.HOP + 1
+        out = torch.empty((B, T, DENOISE_BINS), dtype=torch.int32, device=x_t.device)
+        st = torch.cuda.current_stream(x_t.device).cuda_stream
+        self._ck(self.lib.vtts_debug_time_stretch_decisions(self.h, _ptr(x_t), _ptr(lengths_t), B, S, _ptr(tp), _ptr(out), st))
+        return out.cpu().numpy()
+
+    def open_time_stretch_stream(self, max_streams: int, max_chunk_samples: int) -> "TimeStretchStream":
+        """Streaming time stretcher with `max_streams` independent slots (vtts_time_stretch_stream_*): a slot's tempo is
+        given with BEGIN and fixed until END, and its outputs, concatenated, equal `time_stretch` of its whole input bit
+        for bit.  An output is released once every synthesis frame overlapping it is synthesized; END releases the rest."""
+        return TimeStretchStream(self, max_streams, max_chunk_samples)
+
     # ---- loudness (vtts_loudness*: ITU-R BS.1770-4 gated loudness and true peak, fp32) ----
     def loudness(self, wav, rate: int = config.SAMPLE_RATE, lengths=None) -> "Loudness":
         """Host arrays: wav f32 [S] or [B,S] at `rate` (a multiple of 10 in [8000, 192000]) -> Loudness of float32 [B]
@@ -1116,6 +1195,21 @@ class DenoiseStream(_SlotStream):
         return n_out
 
 
+def _begin_values(carry, flags, given, name) -> np.ndarray:
+    """float32 [S] of a push: `given` (a scalar or [S]) for the slots that begin, each slot's `carry` elsewhere"""
+    out = carry.copy()
+    begin = (np.asarray(flags) & STREAM_BEGIN) != 0
+    if begin.any():
+        if given is None:
+            raise ValueError(f"{name}= is required for the slots a push begins")
+        g = np.asarray(given, np.float32)
+        g = np.full(carry.size, g, np.float32) if g.ndim == 0 else g
+        if g.shape != (carry.size,):
+            raise ValueError(f"{name}: one value or one per slot ({carry.size}), got {np.shape(given)}")
+        out[begin] = g[begin]
+    return np.ascontiguousarray(out, np.float32)
+
+
 class PitchShiftStream(_SlotStream):
     """Handle of a streaming pitch shifter (Engine.open_pitch_shift_stream).  Before END a slot that has received P samples
     has emitted min(P, 256 max(0, floor(P / 256) - 3)) outputs; a push with END emits the rest."""
@@ -1130,17 +1224,7 @@ class PitchShiftStream(_SlotStream):
 
     def _shifts(self, flags, semitones) -> np.ndarray:
         """the semitones array of a push: the given values for the slots that begin, the slots' own shifts elsewhere"""
-        sem = self.shift.copy()
-        begin = (np.asarray(flags) & STREAM_BEGIN) != 0
-        if begin.any():
-            if semitones is None:
-                raise ValueError("semitones= is required for the slots a push begins")
-            given = np.asarray(semitones, np.float32)
-            given = np.full(self.max_streams, given, np.float32) if given.ndim == 0 else given
-            if given.shape != (self.max_streams,):
-                raise ValueError(f"semitones: one value or one per slot ({self.max_streams}), got {np.shape(semitones)}")
-            sem[begin] = given[begin]
-        return np.ascontiguousarray(sem, np.float32)
+        return _begin_values(self.shift, flags, semitones, "semitones")
 
     def _commit(self, flags, sem):
         begin = (np.asarray(flags) & STREAM_BEGIN) != 0
@@ -1169,6 +1253,49 @@ class PitchShiftStream(_SlotStream):
         self.eng._ck(self.eng.lib.vtts_pitch_shift_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(sem), _ptr(out_t),
                                                                _ptr(n_out), st))
         self._commit(f, sem)
+        return n_out
+
+
+class TimeStretchStream(_SlotStream):
+    """Handle of a streaming time stretcher (Engine.open_time_stretch_stream).  Before END a slot at tempo alpha that has
+    scanned Q frames (frame t once rint(256 t alpha) + 512 <= P, P > 512) has released max(0, 256 Q - 511) outputs (all
+    P at tempo 1); a push with END releases the rest."""
+    _kind = "time_stretch_stream"
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int):
+        super().__init__(eng, max_streams, max_chunk_samples)
+        self.max_chunk_samples = self._chunk
+        self._create(eng.lib.vtts_time_stretch_stream_create, self.max_streams, self.max_chunk_samples, pitch=True)
+        self.lookahead = int(eng.lib.vtts_time_stretch_stream_lookahead())
+        self.tempo = np.ones(self.max_streams, np.float32)   # each slot's tempo since its BEGIN
+
+    def _commit(self, flags, tp):
+        begin = (np.asarray(flags) & STREAM_BEGIN) != 0
+        self.tempo[begin] = tp[begin]
+
+    def push(self, x, n_new, begin=None, end=None, tempo=None) -> list:
+        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None,
+        tempo: a scalar or [S], read for the slots that begin.  Returns one float32 array per slot with the samples it
+        releases now."""
+        x, n, f = self._host_in(x, n_new, begin, end)
+        tp = _begin_values(self.tempo, f, tempo, "tempo")
+        y = np.empty((self.max_streams, self.out_pitch), np.float32)
+        n_out = np.zeros(self.max_streams, np.int32)
+        self.eng._ck(self.eng.lib.vtts_time_stretch_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(tp), _ptr(y),
+                                                                     _ptr(n_out)))
+        self._commit(f, tp)
+        return self._rows(y, n_out)
+
+    def push_device(self, x_t, n_new, flags, out_t, tempo=None, stream=None) -> np.ndarray:
+        """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S, out_pitch]; n_new int [S], flags
+        uint8 [S] (bit0 BEGIN, bit1 END) and tempo (scalar or [S], read for the slots that begin) on the host.
+        Stream-ordered; returns n_out int32 [S] (outputs slot s got at the start of its row of out_t)."""
+        n, f, st = self._device_in(x_t, out_t, (self.max_streams, self.out_pitch), n_new, flags, stream)
+        tp = _begin_values(self.tempo, f, tempo, "tempo")
+        n_out = np.zeros(self.max_streams, np.int32)
+        self.eng._ck(self.eng.lib.vtts_time_stretch_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(tp), _ptr(out_t),
+                                                                _ptr(n_out), st))
+        self._commit(f, tp)
         return n_out
 
 
@@ -1292,11 +1419,11 @@ class AcousticStream(_SlotStream):
 class TtsStream:
     """Handle of a text-to-speech stream (Engine.open_tts_stream): an acoustic stream of max_chunk_frames F feeding a
     vocoder stream of F + the acoustic lookahead frames per push, with a denoise strength a denoise stream after it,
-    with semitones a pitch-shift stream, with an output rate a resample stream, and with meter=True a loudness meter of
-    the audio `step()` returns last."""
+    with semitones a pitch-shift stream, with a tempo a time-stretch stream, with an output rate a resample stream, and
+    with meter=True a loudness meter of the audio `step()` returns last."""
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
-                 output_rate=None, denoise=None, meter=False, semitones=None):
+                 output_rate=None, denoise=None, meter=False, semitones=None, tempo=None):
         import torch
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
@@ -1308,14 +1435,19 @@ class TtsStream:
             _loudness_rate(output_rate or config.SAMPLE_RATE)
         if semitones is not None:
             semitones = float(_semitones(semitones, 1)[0])
+        if tempo is not None:
+            tempo = float(_tempo(tempo, 1)[0])
         self.eng = eng
-        self.rs = self.dn = self.ps = self.mt = None
+        self.rs = self.dn = self.ps = self.ts = self.mt = None
         S, sr = max_streams, output_rate or config.SAMPLE_RATE
         # the stages after the vocoder, in push order; each takes the previous stage's output buffer as its input
-        # (the vocoder's: n_new = 256 * frames it emitted) and a slot of the meter holds at most max_frames of audio
-        seconds = -(-int(max_frames) * config.HOP // config.SAMPLE_RATE) + 1
+        # (the vocoder's: n_new = 256 * frames it emitted) and a slot of the meter holds at most max_frames of audio,
+        # slowed down at most 1 / MIN_TEMPO times by the time stretcher
+        slow = int(1 / MIN_TEMPO) if tempo is not None else 1
+        seconds = -(-int(max_frames) * config.HOP * slow // config.SAMPLE_RATE) + 1
         plan = (("dn", denoise is not None, lambda p: DenoiseStream(eng, S, p, denoise)),
                 ("ps", semitones is not None, lambda p: PitchShiftStream(eng, S, p)),
+                ("ts", tempo is not None, lambda p: TimeStretchStream(eng, S, p)),
                 ("rs", output_rate is not None, lambda p: ResampleStream(eng, S, p, output_rate)),
                 ("mt", meter, lambda p: LoudnessMeter(eng, S, p, sr, seconds)))
         self._built = []   # every stream handle, in construction order
@@ -1338,11 +1470,14 @@ class TtsStream:
         self._mel = torch.zeros((S, self.ac.out_frames, config.MEL_DIM), dtype=torch.float32, device=dev)
         self._wav = torch.zeros((S, self.voc.wav_ld), dtype=torch.float32, device=dev)
         self._shift = np.zeros(S, np.float32)  # the shift of each slot's utterance
+        self._tempo = np.ones(S, np.float32)   # the tempo of each slot's utterance
+        extra = {"ps": {"semitones": self._shift}, "ts": {"tempo": self._tempo}}
         # (handle, device output buffer, extra push arguments) of the stages after the vocoder
         self._stages = [(st, torch.zeros((S, 4 if st is self.mt else st.out_pitch), dtype=torch.float32, device=dev),
-                         {"semitones": self._shift} if st is self.ps else {}) for st in self._built[2:]]
+                         next((kw for name, kw in extra.items() if st is getattr(self, name)), {})) for st in self._built[2:]]
         self._mout_h = None if self.mt is None else torch.zeros((S, 4), dtype=torch.float32).pin_memory()
         self._semitones = semitones                    # every slot's default shift
+        self._tempo_default = tempo                    # every slot's default tempo
         self._meter = {}
         self._fresh = np.zeros(max_streams, bool)   # begun, no push yet: the next vocoder push carries BEGIN
         self._empty = set()                         # begun with nothing left after the trim: reported empty at the next step
@@ -1351,16 +1486,19 @@ class TtsStream:
     def max_streams(self):
         return self.ac.max_streams
 
-    def begin(self, slot: int, tokens, silence_duration=-1.0, semitones=None):
+    def begin(self, slot: int, tokens, silence_duration=-1.0, semitones=None, tempo=None):
         """Start `tokens` (one row of phoneme ids) in a free slot: durations, the text2mel fix-ups and the trim are
-        planned exactly as `Engine.tts` plans them (vtts_tts_plan).  `semitones` overrides the stream's shift for this
-        utterance.  Returns the number of frames the slot will vocode."""
+        planned exactly as `Engine.tts` plans them (vtts_tts_plan).  `semitones` and `tempo` override the stream's shift
+        and tempo for this utterance.  Returns the number of frames the slot will vocode."""
         slot = int(slot)
         if self.ac.open[slot] or slot in self._empty:
             raise ValueError(f"slot {slot} is still open")
         if semitones is not None and self.ps is None:
             raise ValueError("the stream was opened without semitones= (no pitch-shift stage)")
+        if tempo is not None and self.ts is None:
+            raise ValueError("the stream was opened without tempo= (no time-stretch stage)")
         shift = self._semitones if semitones is None else float(_semitones(semitones, 1)[0])
+        pace = self._tempo_default if tempo is None else float(_tempo(tempo, 1)[0])
         tok = _np(tokens, np.int32).reshape(1, -1)
         _, frames, nf, ne = self.eng.tts_plan(tok, silence_duration=silence_duration)
         if nf[0] < 1:
@@ -1372,6 +1510,8 @@ class TtsStream:
         self._fresh[slot] = True
         if self.ps is not None:
             self._shift[slot] = shift
+        if self.ts is not None:
+            self._tempo[slot] = pace
         return int(ne[0])
 
     def busy(self) -> np.ndarray:

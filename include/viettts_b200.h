@@ -481,6 +481,59 @@ int vtts_loudness_stream_push(vtts_ctx* ctx, vtts_loudness_stream* ls, const flo
 int vtts_loudness_stream_push_host(vtts_ctx* ctx, vtts_loudness_stream* ls, const float* x, const int32_t* n_new,
                                    const uint8_t* flags, float* out);
 
+/* ---- lookahead true-peak limiter ------------------------------------------------------------------------------------
+ * One mono row x of n samples at rate r (a multiple of 10 in [8000, 192000]); pre-gain G dB in [-70, 70]; ceiling C dBTP
+ * in [-20, 0], c = 10^(C / 20); lookahead A ms in [1, 20], W = max(1, rint(A r / 1000)); release R ms in [1, 2000],
+ * beta = exp(-1000 / (R r)):
+ *   v = fp32(10^(G / 20)) x;  u = resample_poly(v, 4, 1);  p[t] = max(|v[t]|, max |u[j]| over j in [4(t - 10),
+ *   4(t + 10) + 3] inside [0, 4n));  tau = min(1, c / p) (1 where p = 0);  hold h[t] = min tau[t .. t + W - 1] (tau = 1
+ *   past n);  attack a[t] = mean of 1 - h over [t - W + 1, t] (h = 1 before 0; over integers 2^32 (1 - h), rounded up);
+ *   release d[t] = max(a[t], beta d[t - 1] + (1 - beta) a[t]);  y = v min(tau, 1 - d);  reduction_db = 20 log10 of the
+ *   least applied gain (<= 0).  |y| <= c; rows whose peaks stay under c come back as v bit for bit.
+ * fp32 in every vtts_precision mode; every value is a fixed function of the samples and of state at boundaries fixed by
+ * absolute sample index, so a row gives the same bits alone, in any batch, and through the stream. */
+/* x_dev [B,S]; n_dev int32 [B] or NULL (= S; values clamped to [0, S]); gain_db_dev float [B] or NULL (0 dB), read on
+ * the device (clamped to [-70, 70], non-finite as 0); y_dev [B,S] (may equal x_dev), 0 past n[b]; reduction_db_dev [B]
+ * or NULL.  Stream-ordered, no host synchronisation, eight launches; uses the context's workspace (about 28 bytes per
+ * sample). */
+int vtts_limit(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, const float* gain_db_dev, int B, int S, int rate,
+               float ceiling, float lookahead_ms, float release_ms, float* y_dev, float* reduction_db_dev, void* stream);
+/* the same on host buffers; n_in[b] must lie in [0, S] and gain_db[b] in [-70, 70] */
+int vtts_limit_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, const float* gain_db, int B, int S, int rate, float ceiling,
+                    float lookahead_ms, float release_ms, float* y, float* reduction_db);
+/* Loudness normalization that reaches the target under a true-peak ceiling with the limiter instead of lowering the
+ * gain: measure L (vtts_loudness), limit x at G = T - L, measure the result L_y, limit x again at G + (T - L_y); G is
+ * clamped to [-70, 70] and kept where a reading is -inf (silence: G = 0, y = x).  gain_db_dev [B] receives the final G,
+ * or NULL.  All on the device with no host synchronisation, 30 launches; y_dev may equal x_dev. */
+int vtts_loudness_normalize_limited(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, float target,
+                                    float ceiling, float lookahead_ms, float release_ms, float* y_dev, float* gain_db_dev,
+                                    void* stream);
+/* the same on host buffers; gain_db [B] or NULL */
+int vtts_loudness_normalize_limited_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float target,
+                                         float ceiling, float lookahead_ms, float release_ms, float* y, float* gain_db);
+/* Streaming limiter with max_streams independent slots; ceiling, lookahead and release are fixed at create, a slot's
+ * pre-gain is read from gain_db[s] (host, [-70, 70]) at its BEGIN.  Before END sample t is released once sample
+ * t + L has arrived, L = vtts_limiter_stream_lookahead(rate, lookahead_ms) = W + 19; END releases the rest.  A slot's
+ * outputs, concatenated, equal vtts_limit of its whole input bit for bit.  Each slot carries H = 2W + 64 input samples,
+ * the release scan's partial map and d_in of the block holding its next output, and its least gain.  flags and slot
+ * rules as for the resample stream.  Every push issues the same nine launches. */
+typedef struct vtts_limiter_stream vtts_limiter_stream;
+/* *out_pitch = max_chunk_samples + L, the outputs per slot of a push's output buffer */
+int vtts_limiter_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int rate, float ceiling, float lookahead_ms,
+                               float release_ms, vtts_limiter_stream** out, int* out_pitch);
+int vtts_limiter_stream_destroy(vtts_ctx* ctx, vtts_limiter_stream* ls);
+/* L, or VTTS_ERR_BAD_ARG for a bad rate or lookahead.  Needs no device. */
+int vtts_limiter_stream_lookahead(int rate, float lookahead_ms);
+/* x_dev [S][max_chunk_samples] (samples past n_new[s] ignored); n_new, flags, gain_db HOST int32 / uint8 / float [S];
+ * y_dev [S][out_pitch]: slot s gets n_out[s] (HOST int32 [S]) outputs from its start; reduction_db_dev [S] receives each
+ * slot's reduction over what it has released since BEGIN.  Argument errors fail with VTTS_ERR_BAD_ARG before anything is
+ * launched.  Stream-ordered. */
+int vtts_limiter_stream_push(vtts_ctx* ctx, vtts_limiter_stream* ls, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
+                             const float* gain_db, float* y_dev, int32_t* n_out, float* reduction_db_dev, void* stream);
+/* the same on host buffers x [S][max_chunk_samples], y [S][out_pitch] and reduction_db [S]; returns when they are written */
+int vtts_limiter_stream_push_host(vtts_ctx* ctx, vtts_limiter_stream* ls, const float* x, const int32_t* n_new, const uint8_t* flags,
+                                  const float* gain_db, float* y, int32_t* n_out, float* reduction_db);
+
 /* ---- streaming acoustic model: every slot advances its decoder a few frames per push ---------------------------
  * A vtts_acoustic_stream holds max_streams (1..128) independent slots.  begin starts utterances in closed slots; each
  * push advances every open slot by min(F, frames left) decoder steps in ONE scan launch and returns the mel frames whose

@@ -118,6 +118,22 @@ SIGNATURES = {
     "vtts_loudness_stream_lookahead": (C.c_int, [C.c_int]),
     "vtts_loudness_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtts_loudness_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_limit": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float,
+                             C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_limit_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float,
+                                  C.c_void_p, C.c_void_p]),
+    "vtts_loudness_normalize_limited": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                                  C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_loudness_normalize_limited_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                                       C.c_float, C.c_float, C.c_void_p, C.c_void_p]),
+    "vtts_limiter_stream_create": (C.c_int, [c_ctx, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.POINTER(C.c_void_p),
+                                             C.POINTER(C.c_int)]),
+    "vtts_limiter_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
+    "vtts_limiter_stream_lookahead": (C.c_int, [C.c_int, C.c_float]),
+    "vtts_limiter_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p]),
+    "vtts_limiter_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_void_p]),
     "vtts_acoustic_stream_create":(C.c_int, [c_ctx, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, C.POINTER(C.c_void_p)]),
     "vtts_acoustic_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
     "vtts_acoustic_stream_lookahead": (C.c_int, []),

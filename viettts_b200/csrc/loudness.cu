@@ -472,6 +472,12 @@ int ln_check_lengths(vtts_ctx* ctx, const char* who, const int32_t* n_in, int B,
 
 }  // namespace
 
+size_t vtts_loudness_ws_bytes(int B, int S, int rate) {
+  const int m = rate / 10;
+  const long long K = std::max(1, S / m), U = (long long)OS * S, T = (S + U + PEAK_TILE - 1) / PEAK_TILE;
+  return 2 * al((size_t)B * K * 16) + al((size_t)B * K * 4) + al((size_t)B * U * 4) + al((size_t)B * T * 4) + al((size_t)B * 8);
+}
+
 int vtts_loudness_filter(int rate, double* coeffs) {
   if (!rate_ok(rate) || !coeffs) return VTTS_ERR_BAD_ARG;
   ln_design(rate, coeffs);

@@ -358,6 +358,9 @@ struct RsRow {
 // outputs of a row.
 int vtts_resample_run(vtts_ctx* ctx, int in_rate, int out_rate, const float* x, long long x_ld, int S_in, const int* n_in,
                       const RsRow* rows, int B, long long S_out, long long max_out, float* y, long long y_ld, cudaStream_t st);
+// loudness.cu: the context workspace vtts_loudness / vtts_loudness_normalize use for B rows of S samples at `rate`
+// (from the start of ctx->ws)
+size_t vtts_loudness_ws_bytes(int B, int S, int rate);
 // denoise.cu: per-row bounds of the STFT frame and overlap-add kernels, which place a row's buffers in absolute time
 constexpr long long DN_OPEN = 1LL << 60;   // row length not known yet (stream slot before END)
 struct DnRow {

@@ -363,7 +363,8 @@ class Engine:
         return AcousticStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, masks=masks)
 
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
-                        rng=None, output_rate=None, denoise=None, meter=False, semitones=None, tempo=None) -> "TtsStream":
+                        rng=None, output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None,
+                        gain_db=0.0) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
         With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  `output_rate`: a resample
@@ -374,11 +375,14 @@ class Engine:
         default (`begin(..., semitones=)` overrides it per slot), and the audio equals `pitch_shift` of the (denoised)
         `tts` audio bit for bit.  `tempo`: a time-stretch stream follows the pitch shifter (before the resampler) with this
         tempo as every slot's default (`begin(..., tempo=)` overrides it per slot), and the audio equals `time_stretch` of
-        the (denoised, pitch-shifted) `tts` audio bit for bit.  `meter=True`: a loudness meter runs last, on what `step()` returns at the output rate (a
+        the (denoised, pitch-shifted) `tts` audio bit for bit.  `limit=CEILING_DBTP`: a limiter stream follows the
+        resampler, at the output rate (a multiple of 10), with pre-gain `gain_db` as every slot's default
+        (`begin(..., gain_db=)` overrides it per slot); its audio equals `limit` of the unlimited stream audio bit for bit.
+        `meter=True`: a loudness meter runs last, on what `step()` returns at the output rate (a
         multiple of 10), and `TtsStream.meter()` gives each stepped slot's readings, read back in the step's one
         synchronisation.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
         return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate,
-                         denoise=denoise, meter=meter, semitones=semitones, tempo=tempo)
+                         denoise=denoise, meter=meter, semitones=semitones, tempo=tempo, limit=limit, gain_db=gain_db)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -947,18 +951,29 @@ class Engine:
         cols = [out[:, i] for i in range(4)]
         return Loudness(*(c[0] for c in cols)) if one else Loudness(*cols)
 
-    def normalize_loudness(self, wav, target: float, rate: int = config.SAMPLE_RATE, true_peak=None, lengths=None):
+    def normalize_loudness(self, wav, target: float, rate: int = config.SAMPLE_RATE, true_peak=None, lengths=None, limit=False,
+                           lookahead_ms: float = 5.0, release_ms: float = 100.0):
         """Host arrays: (y, gain_db).  y = wav * fp32(10^(g / 20)) per row with g = target - integrated loudness, at most
         true_peak - the true peak when a ceiling (dBTP, in [-20, 0]) is given; rows measuring -inf are copied (g = 0) and
-        outputs past lengths[b] are 0.  target in [-70, 0] LUFS."""
+        outputs past lengths[b] are 0.  target in [-70, 0] LUFS.
+        limit=True (needs true_peak): reach the target and hold the ceiling with the limiter instead of lowering the
+        gain: measure, limit at g = target - L, measure the result L_y, limit again at g + (target - L_y); gain_db is that
+        final g (vtts_loudness_normalize_limited)."""
         rate = _loudness_rate(rate)
         target, ceiling = _loudness_target(target, true_peak)
+        if limit:
+            if true_peak is None:
+                raise ValueError("normalize_loudness(limit=True) needs a true_peak ceiling")
+            _limit_args(ceiling, rate, lookahead_ms, release_ms)
         x, one = _wav_rows(wav)
         B, S = x.shape
         lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
         y = x.copy()
         g = np.zeros(B, np.float32)
-        if B and S:
+        if B and S and limit:
+            self._ck(self.lib.vtts_loudness_normalize_limited_host(self.h, _ptr(x), _ptr(lens), B, S, rate, target, ceiling,
+                                                                   float(lookahead_ms), float(release_ms), _ptr(y), _ptr(g)))
+        elif B and S:
             self._ck(self.lib.vtts_loudness_normalize_host(self.h, _ptr(x), _ptr(lens), B, S, rate, target, ceiling, _ptr(y), _ptr(g)))
         return (y[0], g[0]) if one else (y, g)
 
@@ -975,19 +990,28 @@ class Engine:
         return out
 
     def normalize_loudness_forward(self, x_t, target: float, rate: int = config.SAMPLE_RATE, true_peak=None, lengths_t=None, out=None,
-                                   gain_db=None, stream=None):
-        """vtts_loudness_normalize on torch CUDA tensors, stream-ordered and without a host synchronisation: returns
-        (y [B,S], gain_db [B]).  `out` may be x_t (in place)."""
+                                   gain_db=None, stream=None, limit=False, lookahead_ms: float = 5.0, release_ms: float = 100.0):
+        """vtts_loudness_normalize (limit=True: vtts_loudness_normalize_limited, see normalize_loudness) on torch CUDA
+        tensors, stream-ordered and without a host synchronisation: returns (y [B,S], gain_db [B]).  `out` may be x_t
+        (in place)."""
         import torch
         rate = _loudness_rate(rate)
         target, ceiling = _loudness_target(target, true_peak)
+        if limit:
+            if true_peak is None:
+                raise ValueError("normalize_loudness_forward(limit=True) needs a true_peak ceiling")
+            _limit_args(ceiling, rate, lookahead_ms, release_ms)
         assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
         B, S = x_t.shape
         out = _out_tensor(out, (B, S), x_t.device)
         gain_db = _out_tensor(gain_db, (B,), x_t.device, "gain_db")
         st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
-        self._ck(self.lib.vtts_loudness_normalize(self.h, _ptr(x_t), _ptr(lengths_t), B, S, rate, target, ceiling, _ptr(out),
-                                                  _ptr(gain_db), st))
+        if limit:
+            self._ck(self.lib.vtts_loudness_normalize_limited(self.h, _ptr(x_t), _ptr(lengths_t), B, S, rate, target, ceiling,
+                                                              float(lookahead_ms), float(release_ms), _ptr(out), _ptr(gain_db), st))
+        else:
+            self._ck(self.lib.vtts_loudness_normalize(self.h, _ptr(x_t), _ptr(lengths_t), B, S, rate, target, ceiling, _ptr(out),
+                                                      _ptr(gain_db), st))
         return out, gain_db
 
     def open_loudness_meter(self, max_streams: int, max_chunk_samples: int, rate: int = config.SAMPLE_RATE,
@@ -996,6 +1020,60 @@ class Engine:
         slot's integrated, momentary and short-term readings equal `loudness` of what it has received, bit for bit; its
         true peak lags `lookahead` samples and equals the one-shot value after END.  A slot holds up to `max_seconds`."""
         return LoudnessMeter(self, max_streams, max_chunk_samples, rate, max_seconds)
+
+    # ---- limiter (vtts_limit*: lookahead true-peak limiter, fp32) ----
+    def limit(self, wav, ceiling: float = -1.0, rate: int = config.SAMPLE_RATE, gain_db=0.0, lookahead_ms: float = 5.0,
+              release_ms: float = 100.0, lengths=None):
+        """Host arrays: (y, reduction_db).  wav f32 [S] or [B,S] at `rate` (a multiple of 10 in [8000, 192000]) times the
+        pre-gain gain_db (a scalar or one per row, in [-70, 70] dB), held under `ceiling` dBTP (in [-20, 0]) by a
+        lookahead limiter: the gain dips ahead of every 4x-oversampled peak over `lookahead_ms` (in [1, 20]) and
+        recovers with `release_ms` (in [1, 2000]).  reduction_db: the deepest gain reduction per row (<= 0).  Rows whose
+        peaks stay under the ceiling come back exactly as wav times the pre-gain.  lengths int [B] in [0, S]."""
+        ceiling, rate, lookahead_ms, release_ms = _limit_args(ceiling, rate, lookahead_ms, release_ms)
+        x, one = _wav_rows(wav)
+        B, S = x.shape
+        g = _gain_db(gain_db, B)
+        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
+        y = np.zeros((B, S), np.float32)
+        red = np.zeros(B, np.float32)
+        if B and S:
+            self._ck(self.lib.vtts_limit_host(self.h, _ptr(x), _ptr(lens), _ptr(g), B, S, rate, ceiling, lookahead_ms, release_ms, _ptr(y),
+                                              _ptr(red)))
+        return (y[0], red[0]) if one else (y, red)
+
+    def limit_forward(self, x_t, ceiling: float = -1.0, rate: int = config.SAMPLE_RATE, gain_db=0.0, lookahead_ms: float = 5.0,
+                      release_ms: float = 100.0, lengths_t=None, out=None, reduction_db=None, stream=None):
+        """vtts_limit on torch CUDA tensors, stream-ordered and without a host synchronisation: returns (y [B,S],
+        reduction_db [B]).  gain_db: a host scalar or [B] (validated as in `limit`), or a float32 CUDA tensor [B] read on
+        the device.  `out` may be x_t (in place)."""
+        import torch
+        ceiling, rate, lookahead_ms, release_ms = _limit_args(ceiling, rate, lookahead_ms, release_ms)
+        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
+        B, S = x_t.shape
+        if isinstance(gain_db, torch.Tensor):
+            if tuple(gain_db.shape) != (B,) or gain_db.dtype != torch.float32 or not gain_db.is_cuda or not gain_db.is_contiguous():
+                raise ValueError(f"gain_db must be a contiguous float32 CUDA tensor [{B}] or host values")
+            g_t = gain_db
+        else:
+            g_t = torch.from_numpy(_gain_db(gain_db, B)).to(x_t.device, non_blocking=False)
+        out = _out_tensor(out, (B, S), x_t.device)
+        reduction_db = _out_tensor(reduction_db, (B,), x_t.device, "reduction_db")
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self._ck(self.lib.vtts_limit(self.h, _ptr(x_t), _ptr(lengths_t), _ptr(g_t), B, S, rate, ceiling, lookahead_ms, release_ms,
+                                     _ptr(out), _ptr(reduction_db), st))
+        return out, reduction_db
+
+    def limiter_stream_lookahead(self, rate: int, lookahead_ms: float = 5.0) -> int:
+        """inputs past sample t a limiter stream needs before it releases t: W + 19, W = max(1, rint(lookahead_ms rate / 1000))"""
+        _, rate, lookahead_ms, _ = _limit_args(-1.0, rate, lookahead_ms, 100.0)
+        return int(self.lib.vtts_limiter_stream_lookahead(rate, lookahead_ms))
+
+    def open_limiter_stream(self, max_streams: int, max_chunk_samples: int, rate: int = config.SAMPLE_RATE, ceiling: float = -1.0,
+                            lookahead_ms: float = 5.0, release_ms: float = 100.0) -> "LimiterStream":
+        """Streaming limiter with `max_streams` independent slots (vtts_limiter_stream_*): a slot's pre-gain is given with
+        BEGIN; its outputs, concatenated, equal `limit` of its whole input bit for bit.  Sample t is released once
+        `lookahead` more samples have arrived; END releases the rest."""
+        return LimiterStream(self, max_streams, max_chunk_samples, rate, ceiling, lookahead_ms, release_ms)
 
 
 class Loudness(NamedTuple):
@@ -1023,6 +1101,34 @@ def _loudness_target(target, true_peak):
     if not (np.isfinite(c) and -20.0 <= c <= 0.0):
         raise ValueError(f"true-peak ceiling {true_peak} dBTP must be finite and lie in [-20, 0]")
     return t, c
+
+
+LIMIT_MAX_GAIN_DB = 70.0
+
+
+def _limit_args(ceiling, rate, lookahead_ms, release_ms):
+    """(ceiling, rate, lookahead_ms, release_ms) as vtts_limit takes them, each checked"""
+    c = float(ceiling)
+    if not (np.isfinite(c) and -20.0 <= c <= 0.0):
+        raise ValueError(f"limiter ceiling {ceiling} dBTP must be finite and lie in [-20, 0]")
+    r = _loudness_rate(rate)
+    a, rel = float(lookahead_ms), float(release_ms)
+    if not (np.isfinite(a) and 1.0 <= a <= 20.0):
+        raise ValueError(f"limiter lookahead {lookahead_ms} ms must lie in [1, 20]")
+    if not (np.isfinite(rel) and 1.0 <= rel <= 2000.0):
+        raise ValueError(f"limiter release {release_ms} ms must lie in [1, 2000]")
+    return c, r, a, rel
+
+
+def _gain_db(v, n: int) -> np.ndarray:
+    """float32 [n]: a scalar pre-gain for every row, or one per row, each finite and in [-70, 70] dB"""
+    a = np.asarray(v, np.float32)
+    a = np.full(n, a, np.float32) if a.ndim == 0 else np.ascontiguousarray(a.reshape(-1), np.float32)
+    if a.shape != (n,):
+        raise ValueError(f"gain_db: one value or one per row ({n}), got {np.shape(v)}")
+    if not (np.all(np.isfinite(a)) and np.all(np.abs(a) <= LIMIT_MAX_GAIN_DB)):
+        raise ValueError(f"gain_db must be finite and lie in [-70, 70], got {v}")
+    return a
 
 
 STREAM_BEGIN, STREAM_END = 1, 2
@@ -1327,6 +1433,65 @@ class LoudnessMeter(_SlotStream):
         return out_t
 
 
+class LimiterStream(_SlotStream):
+    """Handle of a streaming limiter (Engine.open_limiter_stream).  Before END a slot that has received P samples has
+    released max(0, P - lookahead) outputs; a push with END releases the rest.  After every push `reduction_db` holds
+    each slot's deepest reduction over what it has released since BEGIN."""
+    _kind = "limiter_stream"
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, rate: int = config.SAMPLE_RATE, ceiling: float = -1.0,
+                 lookahead_ms: float = 5.0, release_ms: float = 100.0):
+        super().__init__(eng, max_streams, max_chunk_samples)
+        self.max_chunk_samples = self._chunk
+        self.ceiling, self.rate, self.lookahead_ms, self.release_ms = _limit_args(ceiling, rate, lookahead_ms, release_ms)
+        self._create(eng.lib.vtts_limiter_stream_create, self.max_streams, self.max_chunk_samples, self.rate, self.ceiling,
+                     self.lookahead_ms, self.release_ms, pitch=True)
+        self.lookahead = int(eng.lib.vtts_limiter_stream_lookahead(self.rate, self.lookahead_ms))
+        self.gain_db = np.zeros(self.max_streams, np.float32)        # each slot's pre-gain since its BEGIN
+        self.reduction_db = np.zeros(self.max_streams, np.float32)   # host pushes: each slot's reduction so far
+
+    def _gains(self, flags, gain_db):
+        g = _begin_values(self.gain_db, flags, gain_db, "gain_db")
+        if not (np.all(np.isfinite(g)) and np.all(np.abs(g) <= LIMIT_MAX_GAIN_DB)):
+            raise ValueError(f"gain_db must be finite and lie in [-70, 70], got {gain_db}")
+        return g
+
+    def _commit(self, flags, g):
+        begin = (np.asarray(flags) & STREAM_BEGIN) != 0
+        self.gain_db[begin] = g[begin]
+
+    def push(self, x, n_new, begin=None, end=None, gain_db=None) -> list:
+        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None,
+        gain_db: a scalar or [S], read for the slots that begin (default 0 dB).  Returns one float32 array per slot with
+        the samples it releases now."""
+        x, n, f = self._host_in(x, n_new, begin, end)
+        g = self._gains(f, 0.0 if gain_db is None else gain_db)
+        y = np.empty((self.max_streams, self.out_pitch), np.float32)
+        n_out = np.zeros(self.max_streams, np.int32)
+        red = np.empty(self.max_streams, np.float32)
+        self.eng._ck(self.eng.lib.vtts_limiter_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(g), _ptr(y),
+                                                                _ptr(n_out), _ptr(red)))
+        self._commit(f, g)
+        self.reduction_db = red
+        return self._rows(y, n_out)
+
+    def push_device(self, x_t, n_new, flags, out_t, reduction_t, gain_db=None, stream=None) -> np.ndarray:
+        """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S, out_pitch], reduction_t f32 CUDA [S];
+        n_new int [S], flags uint8 [S] (bit0 BEGIN, bit1 END) and gain_db (scalar or [S], read for the slots that begin,
+        default 0 dB) on the host.  Stream-ordered; returns n_out int32 [S] (outputs slot s got at the start of its row of
+        out_t)."""
+        import torch
+        n, f, st = self._device_in(x_t, out_t, (self.max_streams, self.out_pitch), n_new, flags, stream)
+        if tuple(reduction_t.shape) != (self.max_streams,) or reduction_t.dtype != torch.float32 or not reduction_t.is_contiguous():
+            raise ValueError(f"reduction_t must be contiguous float32 [{self.max_streams}]")
+        g = self._gains(f, 0.0 if gain_db is None else gain_db)
+        n_out = np.zeros(self.max_streams, np.int32)
+        self.eng._ck(self.eng.lib.vtts_limiter_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(g), _ptr(out_t),
+                                                           _ptr(n_out), _ptr(reduction_t), st))
+        self._commit(f, g)
+        return n_out
+
+
 def acoustic_stream_schedule(n_frames: int, n_emit: int | None, chunk: int, lookahead: int = 10) -> list:
     """Frames an acoustic stream slot emits per push: it scans min(n_frames, n_emit + lookahead) frames, `chunk` per
     push; after P frames scanned it has emitted min(n_emit, max(0, P - lookahead)), and its last push emits the rest."""
@@ -1423,7 +1588,7 @@ class TtsStream:
     with meter=True a loudness meter of the audio `step()` returns last."""
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
-                 output_rate=None, denoise=None, meter=False, semitones=None, tempo=None):
+                 output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None, gain_db=0.0):
         import torch
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
@@ -1437,8 +1602,11 @@ class TtsStream:
             semitones = float(_semitones(semitones, 1)[0])
         if tempo is not None:
             tempo = float(_tempo(tempo, 1)[0])
+        if limit is not None:
+            limit = _limit_args(limit, output_rate or config.SAMPLE_RATE, 5.0, 100.0)[0]
+            gain_db = float(_gain_db(gain_db, 1)[0])
         self.eng = eng
-        self.rs = self.dn = self.ps = self.ts = self.mt = None
+        self.rs = self.dn = self.ps = self.ts = self.lm = self.mt = None
         S, sr = max_streams, output_rate or config.SAMPLE_RATE
         # the stages after the vocoder, in push order; each takes the previous stage's output buffer as its input
         # (the vocoder's: n_new = 256 * frames it emitted) and a slot of the meter holds at most max_frames of audio,
@@ -1449,6 +1617,7 @@ class TtsStream:
                 ("ps", semitones is not None, lambda p: PitchShiftStream(eng, S, p)),
                 ("ts", tempo is not None, lambda p: TimeStretchStream(eng, S, p)),
                 ("rs", output_rate is not None, lambda p: ResampleStream(eng, S, p, output_rate)),
+                ("lm", limit is not None, lambda p: LimiterStream(eng, S, p, sr, limit)),
                 ("mt", meter, lambda p: LoudnessMeter(eng, S, p, sr, seconds)))
         self._built = []   # every stream handle, in construction order
         try:
@@ -1471,13 +1640,16 @@ class TtsStream:
         self._wav = torch.zeros((S, self.voc.wav_ld), dtype=torch.float32, device=dev)
         self._shift = np.zeros(S, np.float32)  # the shift of each slot's utterance
         self._tempo = np.ones(S, np.float32)   # the tempo of each slot's utterance
-        extra = {"ps": {"semitones": self._shift}, "ts": {"tempo": self._tempo}}
+        self._gain = np.zeros(S, np.float32)   # the limiter pre-gain of each slot's utterance
+        self._red = None if self.lm is None else torch.zeros(S, dtype=torch.float32, device=dev)
+        extra = {"ps": {"semitones": self._shift}, "ts": {"tempo": self._tempo}, "lm": {"reduction_t": self._red, "gain_db": self._gain}}
         # (handle, device output buffer, extra push arguments) of the stages after the vocoder
         self._stages = [(st, torch.zeros((S, 4 if st is self.mt else st.out_pitch), dtype=torch.float32, device=dev),
                          next((kw for name, kw in extra.items() if st is getattr(self, name)), {})) for st in self._built[2:]]
         self._mout_h = None if self.mt is None else torch.zeros((S, 4), dtype=torch.float32).pin_memory()
         self._semitones = semitones                    # every slot's default shift
         self._tempo_default = tempo                    # every slot's default tempo
+        self._gain_default = gain_db                   # every slot's default limiter pre-gain
         self._meter = {}
         self._fresh = np.zeros(max_streams, bool)   # begun, no push yet: the next vocoder push carries BEGIN
         self._empty = set()                         # begun with nothing left after the trim: reported empty at the next step
@@ -1486,10 +1658,10 @@ class TtsStream:
     def max_streams(self):
         return self.ac.max_streams
 
-    def begin(self, slot: int, tokens, silence_duration=-1.0, semitones=None, tempo=None):
+    def begin(self, slot: int, tokens, silence_duration=-1.0, semitones=None, tempo=None, gain_db=None):
         """Start `tokens` (one row of phoneme ids) in a free slot: durations, the text2mel fix-ups and the trim are
         planned exactly as `Engine.tts` plans them (vtts_tts_plan).  `semitones` and `tempo` override the stream's shift
-        and tempo for this utterance.  Returns the number of frames the slot will vocode."""
+        and tempo for this utterance, `gain_db` the limiter's pre-gain.  Returns the number of frames the slot will vocode."""
         slot = int(slot)
         if self.ac.open[slot] or slot in self._empty:
             raise ValueError(f"slot {slot} is still open")
@@ -1497,6 +1669,9 @@ class TtsStream:
             raise ValueError("the stream was opened without semitones= (no pitch-shift stage)")
         if tempo is not None and self.ts is None:
             raise ValueError("the stream was opened without tempo= (no time-stretch stage)")
+        if gain_db is not None and self.lm is None:
+            raise ValueError("the stream was opened without limit= (no limiter stage)")
+        gain = self._gain_default if gain_db is None else float(_gain_db(gain_db, 1)[0])
         shift = self._semitones if semitones is None else float(_semitones(semitones, 1)[0])
         pace = self._tempo_default if tempo is None else float(_tempo(tempo, 1)[0])
         tok = _np(tokens, np.int32).reshape(1, -1)
@@ -1512,6 +1687,8 @@ class TtsStream:
             self._shift[slot] = shift
         if self.ts is not None:
             self._tempo[slot] = pace
+        if self.lm is not None:
+            self._gain[slot] = gain
         return int(ne[0])
 
     def busy(self) -> np.ndarray:

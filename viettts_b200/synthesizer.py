@@ -14,6 +14,9 @@ before any resampling.
 `--loudness L`
 normalizes every output to L LUFS (ITU-R BS.1770-4, Engine.normalize_loudness) at the rate it is written, after
 --denoise and --output-rate, under a true-peak ceiling (`--true-peak`, default -1 dBTP as EBU R128 asks).
+`--limiter` holds that ceiling with a lookahead true-peak limiter (Engine.limit) instead of lowering the gain: with
+--loudness the target is reached (Engine.normalize_loudness(limit=True)), without it every output is limited to
+--true-peak at the rate it is written, after --output-rate.
 """
 from __future__ import annotations
 
@@ -132,6 +135,10 @@ def main(argv=None) -> int:
     parser.add_argument("--true-peak", default=None, type=float, metavar="DBTP",
                         help="with --loudness: the true-peak ceiling in dBTP, in [-20, 0] (default -1.0, EBU R128); the gain is "
                              "lowered until the 4x-oversampled peak stays below it")
+    parser.add_argument("--limiter", action="store_true",
+                        help="hold the --true-peak ceiling (default -1 dBTP) with a lookahead limiter on the device (5 ms "
+                             "lookahead, 100 ms release): with --loudness the target is reached instead of the gain being "
+                             "lowered; without it every output is limited at the output rate, after --output-rate")
     parser.add_argument("--silence-duration", default=-1, type=float)
     parser.add_argument("--lexicon-file", default=None)
     parser.add_argument("--seed", default=None, type=int,
@@ -167,8 +174,16 @@ def main(argv=None) -> int:
         if max(up, down) > 1024:
             parser.error(f"--output-rate {args.output_rate}: {config.SAMPLE_RATE} -> {args.output_rate} reduces to {up}/{down} "
                          "(at most 1024 each)")
-    if args.true_peak is not None and args.loudness is None:
-        parser.error("--true-peak is the ceiling of --loudness normalization; give --loudness too")
+    if args.true_peak is not None and args.loudness is None and not args.limiter:
+        parser.error("--true-peak is the ceiling of --loudness normalization or of --limiter; give one of them too")
+    if args.limiter and args.loudness is None:
+        from .engine import _limit_args
+        if args.true_peak is None:
+            args.true_peak = -1.0
+        try:
+            _limit_args(args.true_peak, args.output_rate or config.SAMPLE_RATE, 5.0, 100.0)
+        except ValueError as e:
+            parser.error(f"--limiter: {e}")
     if args.loudness is not None:
         from .engine import _loudness_rate, _loudness_target
         if args.true_peak is None:
@@ -196,7 +211,11 @@ def main(argv=None) -> int:
             waves = [get_engine().resample(w, args.output_rate) for w in waves]
         if args.loudness is not None:
             rate = args.output_rate or config.SAMPLE_RATE
-            waves = [get_engine().normalize_loudness(w, args.loudness, rate, true_peak=args.true_peak)[0] for w in waves]
+            waves = [get_engine().normalize_loudness(w, args.loudness, rate, true_peak=args.true_peak, limit=args.limiter)[0]
+                     for w in waves]
+        elif args.limiter:
+            rate = args.output_rate or config.SAMPLE_RATE
+            waves = [get_engine().limit(w, args.true_peak, rate)[0] for w in waves]
         return waves
 
     if args.text_file is not None:

@@ -534,6 +534,49 @@ int vtts_limiter_stream_push(vtts_ctx* ctx, vtts_limiter_stream* ls, const float
 int vtts_limiter_stream_push_host(vtts_ctx* ctx, vtts_limiter_stream* ls, const float* x, const int32_t* n_new, const uint8_t* flags,
                                   const float* gain_db, float* y, int32_t* n_out, float* reduction_db);
 
+/* ---- equalizer: a cascade of second-order IIR sections -------------------------------------------------------------
+ * A filter is sos, HOST float64 [K][6], rows b0 b1 b2 a0 a1 a2 (scipy's layout), 1 <= K <= 8.  For one mono row x of n
+ * samples, y = scipy.signal.sosfilt(sos, x) from zero state at sample 0; y is not clipped and outputs past n are 0.
+ * Each section, normalized by a0 (a0 != 0), must be finite and strictly stable with every pole radius <= 1 - 1e-6
+ * (|a2| < 1, |a1| < 1 + a2); anything else fails with VTTS_ERR_BAD_ARG before anything is launched.
+ * Every section runs as the trapezoidal state-variable filter of its bilinear transform, fp32 in every vtts_precision
+ * mode; every output is a fixed function of the samples and of the cascade state at boundaries of 1024 samples fixed by
+ * absolute sample index, so a row gives the same bits alone, in any batch, and through the stream. */
+typedef enum vtts_eq_kind {
+  VTTS_EQ_HIGHPASS = 0,   /* Butterworth of `order` 1..8, bilinear prewarped to f0: ceil(order / 2) sections */
+  VTTS_EQ_LOWPASS = 1,
+  VTTS_EQ_LOWSHELF = 2,   /* RBJ Audio EQ Cookbook shelves, q = the shelf slope S in (0, 1], gain_db in [-24, 24]: 1 section */
+  VTTS_EQ_HIGHSHELF = 3,
+  VTTS_EQ_PEAKING = 4,    /* RBJ peaking EQ, q in [0.1, 30], gain_db in [-24, 24]: 1 section */
+  VTTS_EQ_NOTCH = 5       /* RBJ notch, q in [0.1, 30]: 1 section */
+} vtts_eq_kind;
+/* sos [8][6] receives *n_sections rows with a0 = 1, designed in double for rate in [8000, 192000] and f0 in
+ * [10, 0.45 rate] Hz; parameters a kind does not use are ignored.  VTTS_ERR_BAD_ARG for anything out of range.  Needs
+ * no device. */
+int vtts_eq_design(int kind, int rate, double f0, double q, double gain_db, int order, double* sos, int* n_sections);
+/* x_dev [B,S]; n_dev int32 [B] or NULL (= S; values clamped to [0, S]); y_dev [B,S] (may equal x_dev).  Stream-ordered,
+ * no host synchronisation, three launches; uses the context's workspace (128 bytes per 1024 samples). */
+int vtts_eq(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const double* sos, int K, float* y_dev,
+            void* stream);
+/* the same on host buffers; n_in[b] must lie in [0, S] */
+int vtts_eq_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, const double* sos, int K, float* y);
+/* Streaming equalizer with max_streams independent slots; the filter is fixed at create.  Every sample is released by
+ * the push that brings it (no lookahead): n_out[s] = n_new[s], and a slot's outputs, concatenated, equal vtts_eq of its
+ * whole input bit for bit.  Each slot carries the cascade state at its last complete 1024-sample block boundary and the
+ * samples of its incomplete block.  flags and slot rules as for the resample stream.  Every push issues the same four
+ * launches. */
+typedef struct vtts_eq_stream vtts_eq_stream;
+int vtts_eq_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, const double* sos, int K, vtts_eq_stream** out);
+int vtts_eq_stream_destroy(vtts_ctx* ctx, vtts_eq_stream* es);
+/* x_dev [S][max_chunk_samples] (samples past n_new[s] ignored); n_new, flags, n_out HOST int32 / uint8 / int32 [S];
+ * y_dev [S][max_chunk_samples] (may equal x_dev): slot s gets n_out[s] outputs from its start.  Argument errors fail
+ * with VTTS_ERR_BAD_ARG before anything is launched.  Stream-ordered. */
+int vtts_eq_stream_push(vtts_ctx* ctx, vtts_eq_stream* es, const float* x_dev, const int32_t* n_new, const uint8_t* flags, float* y_dev,
+                        int32_t* n_out, void* stream);
+/* the same on host buffers x and y [S][max_chunk_samples]; returns when y is written */
+int vtts_eq_stream_push_host(vtts_ctx* ctx, vtts_eq_stream* es, const float* x, const int32_t* n_new, const uint8_t* flags, float* y,
+                             int32_t* n_out);
+
 /* ---- streaming acoustic model: every slot advances its decoder a few frames per push ---------------------------
  * A vtts_acoustic_stream holds max_streams (1..128) independent slots.  begin starts utterances in closed slots; each
  * push advances every open slot by min(F, frames left) decoder steps in ONE scan launch and returns the mel frames whose

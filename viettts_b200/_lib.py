@@ -134,6 +134,13 @@ SIGNATURES = {
                                            C.c_void_p, C.c_void_p]),
     "vtts_limiter_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                 C.c_void_p, C.c_void_p]),
+    "vtts_eq_design": (C.c_int, [C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, C.c_void_p, C.POINTER(C.c_int)]),
+    "vtts_eq": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "vtts_eq_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
+    "vtts_eq_stream_create": (C.c_int, [c_ctx, C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]),
+    "vtts_eq_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
+    "vtts_eq_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_eq_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtts_acoustic_stream_create":(C.c_int, [c_ctx, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, C.POINTER(C.c_void_p)]),
     "vtts_acoustic_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
     "vtts_acoustic_stream_lookahead": (C.c_int, []),

@@ -324,30 +324,6 @@ void ln_design(int rate, double* c) {
   }
 }
 
-void mat_mul(const double* X, const double* Y, double* Z) {   // Z = X Y (4 x 4, Z may alias neither)
-  for (int i = 0; i < 4; ++i)
-    for (int j = 0; j < 4; ++j) {
-      double a = 0.0;
-      for (int k = 0; k < 4; ++k) a += X[i * 4 + k] * Y[k * 4 + j];
-      Z[i * 4 + j] = a;
-    }
-}
-
-void mat_pow(const double* A, long long e, double* R) {
-  double P[16], T[16];
-  std::memcpy(P, A, sizeof(P));
-  for (int i = 0; i < 16; ++i) R[i] = i % 5 == 0 ? 1.0 : 0.0;
-  while (e > 0) {
-    if (e & 1) {
-      mat_mul(R, P, T);
-      std::memcpy(R, T, sizeof(T));
-    }
-    mat_mul(P, P, T);
-    std::memcpy(P, T, sizeof(T));
-    e >>= 1;
-  }
-}
-
 int seg_of(int m) { return (m + 31) / 32; }
 
 // the context's fp32 cascade of `rate` (designed at the first use).  The high-pass b = [1, -2, 1] / a equals a0 times
@@ -378,10 +354,10 @@ const LnFilter& ln_filter(vtts_ctx* ctx, int rate) {
   const int m = rate / 10, seg = seg_of(m);
   double P[16];
   for (int d = 0; d < 5; ++d) {
-    mat_pow(A, (long long)seg << d, P);
+    vtts_mat_pow(A, (long long)seg << d, P, 4);
     for (int i = 0; i < 16; ++i) f.seg[d][i] = (float)P[i];
   }
-  mat_pow(A, m, P);
+  vtts_mat_pow(A, m, P, 4);
   for (int i = 0; i < 16; ++i) f.blk[i] = (float)P[i];
   ctx->ln_filters.push_back(f);
   return ctx->ln_filters.back();

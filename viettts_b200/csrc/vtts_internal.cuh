@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -258,6 +259,30 @@ struct Arena {
     return p;
   }
 };
+
+// R = A^e of an n x n row-major matrix in double (R aliases nothing): square and multiply, every product summed in index
+// order.  The loudness meter and the equalizer power their state transitions with it.
+inline void vtts_mat_pow(const double* A, long long e, double* R, int n) {
+  std::vector<double> P(A, A + (size_t)n * n), T((size_t)n * n);
+  const auto mul = [n](const double* X, const double* Y, double* Z) {
+    for (int i = 0; i < n; ++i)
+      for (int j = 0; j < n; ++j) {
+        double a = 0.0;
+        for (int k = 0; k < n; ++k) a += X[i * n + k] * Y[k * n + j];
+        Z[i * n + j] = a;
+      }
+  };
+  for (int i = 0; i < n * n; ++i) R[i] = i % (n + 1) == 0 ? 1.0 : 0.0;
+  while (e > 0) {
+    if (e & 1) {
+      mul(R, P.data(), T.data());
+      std::copy(T.begin(), T.end(), R);
+    }
+    mul(P.data(), P.data(), T.data());
+    P.swap(T);
+    e >>= 1;
+  }
+}
 
 // conv1d.cu
 int vtts_launch_conv(vtts_ctx* ctx, const ConvLaunch& L, cudaStream_t st);

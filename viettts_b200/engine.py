@@ -91,6 +91,80 @@ def _tempo(v, n: int) -> np.ndarray:
     return a
 
 
+EQ_MAX_SECTIONS = 8
+EQ_PRESETS = {"telephone": "hp:300:4,lp:3400:4"}   # the ITU-T G.712 telephone band
+# band name -> (vtts_eq_kind, its value names, how many of them may be left out)
+_EQ_BANDS = {"hp": (0, ("F", "ORDER"), 1), "lp": (1, ("F", "ORDER"), 1), "ls": (2, ("F", "GAIN", "S"), 1),
+             "hs": (3, ("F", "GAIN", "S"), 1), "pk": (4, ("F", "Q", "GAIN"), 0), "notch": (5, ("F", "Q"), 0)}
+
+
+def _eq_stable(row) -> bool:
+    """a section b0 b1 b2 a0 a1 a2 is finite, a0 != 0 and strictly stable with every pole radius <= 1 - 1e-6"""
+    if not np.all(np.isfinite(row)) or row[3] == 0:
+        return False
+    a1, a2 = row[4] / row[3], row[5] / row[3]
+    if not (abs(a2) < 1 and abs(a1) < 1 + a2):
+        return False
+    disc = a1 * a1 - 4 * a2      # the poles of z^2 + a1 z + a2
+    return (np.sqrt(a2) if disc < 0 else (abs(a1) + np.sqrt(disc)) / 2) <= 1 - 1e-6
+
+
+def eq_sections(spec, rate: int) -> np.ndarray:
+    """float64 [K,6] (rows b0 b1 b2 a0 a1 a2, 1 <= K <= 8) of an equalizer `spec` at `rate` Hz, designed by the library
+    (vtts_eq_design; needs no device).  `spec` is an sos array, or comma-separated bands: hp:F[:ORDER] and lp:F[:ORDER]
+    (Butterworth, order 1..8, default 2), ls:F:GAIN[:S] and hs:F:GAIN[:S] (RBJ shelves, slope S in (0, 1], default 1),
+    pk:F:Q:GAIN (RBJ peaking), notch:F:Q, or the preset `telephone` (hp:300:4,lp:3400:4).  F in [10, 0.45 rate] Hz, Q in
+    [0.1, 30], GAIN in [-24, 24] dB, rate in [8000, 192000].  Raises ValueError for anything else, for more than 8
+    sections, and for a section that is not finite and strictly stable."""
+    try:
+        r = float(rate)
+    except (TypeError, ValueError):
+        r = None
+    if r is None or not (8000 <= r <= 192000 and r == int(r)):
+        raise ValueError(f"eq: rate {rate} must be an integer in [8000, 192000]")
+    r = int(r)
+    if not isinstance(spec, str):
+        sos = np.array(spec, np.float64, order="C")   # a copy in the [K][6] row-major layout the library reads
+        if sos.ndim != 2 or sos.shape[1] != 6 or not 1 <= sos.shape[0] <= EQ_MAX_SECTIONS:
+            raise ValueError(f"eq: an sos array must be [K,6] with 1 <= K <= {EQ_MAX_SECTIONS}, got {np.shape(spec)}")
+        for j, row in enumerate(sos):
+            if not _eq_stable(row):
+                raise ValueError(f"eq: section {j} {row.tolist()} must be finite with a0 != 0 and strictly stable")
+        return sos
+    lib = _lib.load()
+    rows = []
+    for band in spec.split(","):
+        band = band.strip().lower()
+        if band in EQ_PRESETS:
+            rows.append(eq_sections(EQ_PRESETS[band], r))
+            continue
+        name, *vals = band.split(":")
+        if name not in _EQ_BANDS:
+            raise ValueError(f"eq: unknown band {band!r} (hp, lp, ls, hs, pk, notch or {', '.join(EQ_PRESETS)})")
+        kind, names, optional = _EQ_BANDS[name]
+        if not len(names) - optional <= len(vals) <= len(names):
+            raise ValueError(f"eq: band {band!r} takes {name}:{':'.join(names[:len(names) - optional])}"
+                             + "".join(f"[:{n}]" for n in names[len(names) - optional:]))
+        try:
+            v = dict(zip(names, (float(s) for s in vals)))
+        except ValueError:
+            raise ValueError(f"eq: band {band!r} has a value that is not a number") from None
+        order = v.get("ORDER", 2.0)
+        if not (np.isfinite(order) and order == int(order)):
+            raise ValueError(f"eq: band {band!r}: the order must be an integer in [1, 8]")
+        buf = np.zeros((EQ_MAX_SECTIONS, 6), np.float64)
+        k = C.c_int()
+        rc = lib.vtts_eq_design(kind, r, v["F"], v.get("Q", v.get("S", 1.0)), v.get("GAIN", 0.0), int(order), _ptr(buf), C.byref(k))
+        if rc != 0:
+            raise ValueError(f"eq: band {band!r} at {r} Hz is out of range (F in [10, {0.45 * r:g}] Hz, ORDER in [1, 8], "
+                             "Q in [0.1, 30], S in (0, 1], GAIN in [-24, 24] dB)")
+        rows.append(buf[:k.value])
+    sos = np.concatenate(rows) if rows else np.zeros((0, 6))
+    if not 1 <= sos.shape[0] <= EQ_MAX_SECTIONS:
+        raise ValueError(f"eq: {spec!r} makes {sos.shape[0]} sections (1 to {EQ_MAX_SECTIONS})")
+    return sos
+
+
 def _ptr(a):
     if a is None:
         return None
@@ -364,7 +438,7 @@ class Engine:
 
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
                         rng=None, output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None,
-                        gain_db=0.0) -> "TtsStream":
+                        gain_db=0.0, eq=None) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
         With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  `output_rate`: a resample
@@ -378,11 +452,14 @@ class Engine:
         the (denoised, pitch-shifted) `tts` audio bit for bit.  `limit=CEILING_DBTP`: a limiter stream follows the
         resampler, at the output rate (a multiple of 10), with pre-gain `gain_db` as every slot's default
         (`begin(..., gain_db=)` overrides it per slot); its audio equals `limit` of the unlimited stream audio bit for bit.
+        `eq`: an equalizer spec or sos array (`eq_sections`), designed at the output rate; an equalizer stream follows the
+        resampler (before the limiter and the meter) and the audio equals `equalize` of the (resampled) `tts` audio bit
+        for bit.  It releases every sample it receives, so it adds no delay.
         `meter=True`: a loudness meter runs last, on what `step()` returns at the output rate (a
         multiple of 10), and `TtsStream.meter()` gives each stepped slot's readings, read back in the step's one
         synchronisation.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
         return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate,
-                         denoise=denoise, meter=meter, semitones=semitones, tempo=tempo, limit=limit, gain_db=gain_db)
+                         denoise=denoise, meter=meter, semitones=semitones, tempo=tempo, limit=limit, gain_db=gain_db, eq=eq)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -1075,6 +1152,37 @@ class Engine:
         `lookahead` more samples have arrived; END releases the rest."""
         return LimiterStream(self, max_streams, max_chunk_samples, rate, ceiling, lookahead_ms, release_ms)
 
+    # ---- equalizer (vtts_eq*: a cascade of second-order sections, fp32) ----
+    def equalize(self, wav, eq, rate: int = config.SAMPLE_RATE, lengths=None) -> np.ndarray:
+        """Host arrays: wav f32 [S] or [B,S] at `rate` through the equalizer `eq` (a spec or an sos array, see
+        `eq_sections`), equal to scipy.signal.sosfilt of each row from zero state up to fp32 rounding; not clipped.
+        lengths int [B] in [0, S]: outputs past lengths[b] are 0."""
+        sos = eq_sections(eq, rate)
+        x, one = _wav_rows(wav)
+        B, S = x.shape
+        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
+        y = np.zeros((B, S), np.float32)
+        if B and S:
+            self._ck(self.lib.vtts_eq_host(self.h, _ptr(x), _ptr(lens), B, S, _ptr(sos), sos.shape[0], _ptr(y)))
+        return y[0] if one else y
+
+    def equalize_forward(self, x_t, eq, rate: int = config.SAMPLE_RATE, lengths_t=None, out=None, stream=None):
+        """vtts_eq on torch CUDA tensors, stream-ordered and without a host synchronisation: x_t f32 [B,S] -> [B,S];
+        lengths_t int32 CUDA [B] or None.  `out` may be x_t (in place)."""
+        import torch
+        sos = eq_sections(eq, rate)
+        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
+        B, S = x_t.shape
+        out = _out_tensor(out, (B, S), x_t.device)
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self._ck(self.lib.vtts_eq(self.h, _ptr(x_t), _ptr(lengths_t), B, S, _ptr(sos), sos.shape[0], _ptr(out), st))
+        return out
+
+    def open_eq_stream(self, max_streams: int, max_chunk_samples: int, eq, rate: int = config.SAMPLE_RATE) -> "EqStream":
+        """Streaming equalizer with `max_streams` independent slots (vtts_eq_stream_*): every push releases every sample
+        it brings (no lookahead), and a slot's outputs, concatenated, equal `equalize` of its whole input bit for bit."""
+        return EqStream(self, max_streams, max_chunk_samples, eq, rate)
+
 
 class Loudness(NamedTuple):
     integrated: np.ndarray     # LUFS (gated, BS.1770-4)
@@ -1492,6 +1600,36 @@ class LimiterStream(_SlotStream):
         return n_out
 
 
+class EqStream(_SlotStream):
+    """Handle of a streaming equalizer (Engine.open_eq_stream).  Every push releases every sample it brings:
+    n_out = n_new."""
+    _kind = "eq_stream"
+    lookahead = 0
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, eq, rate: int = config.SAMPLE_RATE):
+        super().__init__(eng, max_streams, max_chunk_samples)
+        self.max_chunk_samples = self.out_pitch = self._chunk
+        self.sos = eq_sections(eq, rate)
+        self._create(eng.lib.vtts_eq_stream_create, self.max_streams, self.max_chunk_samples, _ptr(self.sos), self.sos.shape[0])
+
+    def push(self, x, n_new, begin=None, end=None) -> list:
+        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None.
+        Returns one float32 array per slot with its n_new[s] outputs."""
+        x, n, f = self._host_in(x, n_new, begin, end)
+        y = np.empty((self.max_streams, self.out_pitch), np.float32)
+        n_out = np.zeros(self.max_streams, np.int32)
+        self.eng._ck(self.eng.lib.vtts_eq_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(y), _ptr(n_out)))
+        return self._rows(y, n_out)
+
+    def push_device(self, x_t, n_new, flags, out_t, stream=None) -> np.ndarray:
+        """Device buffers: x_t and out_t f32 CUDA [S, max_chunk_samples] (out_t may be x_t); n_new int [S] and flags
+        uint8 [S] (bit0 BEGIN, bit1 END) on the host.  Stream-ordered; returns n_out int32 [S] (= n_new)."""
+        n, f, st = self._device_in(x_t, out_t, (self.max_streams, self.out_pitch), n_new, flags, stream)
+        n_out = np.zeros(self.max_streams, np.int32)
+        self.eng._ck(self.eng.lib.vtts_eq_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(out_t), _ptr(n_out), st))
+        return n_out
+
+
 def acoustic_stream_schedule(n_frames: int, n_emit: int | None, chunk: int, lookahead: int = 10) -> list:
     """Frames an acoustic stream slot emits per push: it scans min(n_frames, n_emit + lookahead) frames, `chunk` per
     push; after P frames scanned it has emitted min(n_emit, max(0, P - lookahead)), and its last push emits the rest."""
@@ -1584,11 +1722,12 @@ class AcousticStream(_SlotStream):
 class TtsStream:
     """Handle of a text-to-speech stream (Engine.open_tts_stream): an acoustic stream of max_chunk_frames F feeding a
     vocoder stream of F + the acoustic lookahead frames per push, with a denoise strength a denoise stream after it,
-    with semitones a pitch-shift stream, with a tempo a time-stretch stream, with an output rate a resample stream, and
-    with meter=True a loudness meter of the audio `step()` returns last."""
+    with semitones a pitch-shift stream, with a tempo a time-stretch stream, with an output rate a resample stream, with
+    eq an equalizer stream, with limit a limiter stream, and with meter=True a loudness meter of the audio `step()`
+    returns last."""
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
-                 output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None, gain_db=0.0):
+                 output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None, gain_db=0.0, eq=None):
         import torch
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
@@ -1605,8 +1744,10 @@ class TtsStream:
         if limit is not None:
             limit = _limit_args(limit, output_rate or config.SAMPLE_RATE, 5.0, 100.0)[0]
             gain_db = float(_gain_db(gain_db, 1)[0])
+        if eq is not None:
+            eq = eq_sections(eq, output_rate or config.SAMPLE_RATE)
         self.eng = eng
-        self.rs = self.dn = self.ps = self.ts = self.lm = self.mt = None
+        self.rs = self.dn = self.ps = self.ts = self.eq = self.lm = self.mt = None
         S, sr = max_streams, output_rate or config.SAMPLE_RATE
         # the stages after the vocoder, in push order; each takes the previous stage's output buffer as its input
         # (the vocoder's: n_new = 256 * frames it emitted) and a slot of the meter holds at most max_frames of audio,
@@ -1617,6 +1758,7 @@ class TtsStream:
                 ("ps", semitones is not None, lambda p: PitchShiftStream(eng, S, p)),
                 ("ts", tempo is not None, lambda p: TimeStretchStream(eng, S, p)),
                 ("rs", output_rate is not None, lambda p: ResampleStream(eng, S, p, output_rate)),
+                ("eq", eq is not None, lambda p: EqStream(eng, S, p, eq, sr)),
                 ("lm", limit is not None, lambda p: LimiterStream(eng, S, p, sr, limit)),
                 ("mt", meter, lambda p: LoudnessMeter(eng, S, p, sr, seconds)))
         self._built = []   # every stream handle, in construction order

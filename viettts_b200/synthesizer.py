@@ -17,6 +17,8 @@ normalizes every output to L LUFS (ITU-R BS.1770-4, Engine.normalize_loudness) a
 `--limiter` holds that ceiling with a lookahead true-peak limiter (Engine.limit) instead of lowering the gain: with
 --loudness the target is reached (Engine.normalize_loudness(limit=True)), without it every output is limited to
 --true-peak at the rate it is written, after --output-rate.
+`--eq SPEC` equalizes every output on the device (Engine.equalize: high / low-pass, shelves, peaking and notch bands,
+or the `telephone` preset) at the rate it is written, after --output-rate and before --loudness / --limiter.
 """
 from __future__ import annotations
 
@@ -139,6 +141,11 @@ def main(argv=None) -> int:
                         help="hold the --true-peak ceiling (default -1 dBTP) with a lookahead limiter on the device (5 ms "
                              "lookahead, 100 ms release): with --loudness the target is reached instead of the gain being "
                              "lowered; without it every output is limited at the output rate, after --output-rate")
+    parser.add_argument("--eq", default=None, metavar="SPEC",
+                        help="equalize every output on the device at the output rate, after --output-rate and before "
+                             "--loudness / --limiter: comma-separated bands hp:F[:ORDER], lp:F[:ORDER], ls:F:GAIN[:S], "
+                             "hs:F:GAIN[:S], pk:F:Q:GAIN, notch:F:Q, or 'telephone' (hp:300:4,lp:3400:4, the 300-3400 Hz "
+                             "band); at most 8 second-order sections in all")
     parser.add_argument("--silence-duration", default=-1, type=float)
     parser.add_argument("--lexicon-file", default=None)
     parser.add_argument("--seed", default=None, type=int,
@@ -193,6 +200,13 @@ def main(argv=None) -> int:
             _loudness_rate(args.output_rate or config.SAMPLE_RATE)
         except ValueError as e:
             parser.error(f"--loudness: {e}")
+    eq_sos = None
+    if args.eq is not None:
+        from .engine import eq_sections
+        try:
+            eq_sos = eq_sections(args.eq, args.output_rate or config.SAMPLE_RATE)
+        except ValueError as e:
+            parser.error(f"--eq: {e}")
     header_rate = args.output_rate or args.sample_rate or config.SAMPLE_RATE
     lexicon = args.lexicon_file if args.lexicon_file is not None else config.LEXICON_FILE
     if args.precision is not None:
@@ -209,6 +223,9 @@ def main(argv=None) -> int:
             waves = [get_engine().time_stretch(w, args.tempo) for w in waves]
         if args.output_rate is not None:
             waves = [get_engine().resample(w, args.output_rate) for w in waves]
+        if eq_sos is not None:
+            rate = args.output_rate or config.SAMPLE_RATE
+            waves = [get_engine().equalize(w, eq_sos, rate) for w in waves]
         if args.loudness is not None:
             rate = args.output_rate or config.SAMPLE_RATE
             waves = [get_engine().normalize_loudness(w, args.loudness, rate, true_peak=args.true_peak, limit=args.limiter)[0]

@@ -195,8 +195,8 @@ def _out_tensor(out, shape, device, what="out"):
     import torch
     if out is None:
         return torch.empty(shape, dtype=torch.float32, device=device)
-    if tuple(out.shape) != shape or out.dtype != torch.float32 or not out.is_contiguous():
-        raise ValueError(f"{what} must be contiguous float32 [{', '.join(map(str, shape))}]")
+    if tuple(out.shape) != shape or out.dtype != torch.float32 or not out.is_contiguous() or out.device != torch.device(device):
+        raise ValueError(f"{what} must be contiguous float32 [{', '.join(map(str, shape))}] on {device}")
     return out
 
 
@@ -215,7 +215,7 @@ class Engine:
         self._hifigan_key = None
         self._acoustic_key = None
         self._duration_key = None
-        self._mel_loaded = False
+        self._mel_fb = None         # host copy of the filterbank on the device (None: none loaded)
         self._denoise_bias = None   # default denoiser bias of the loaded generator in the current mode (denoiser_bias)
 
     def close(self):
@@ -376,9 +376,12 @@ class Engine:
             self._hifigan_key = self._acoustic_key = self._duration_key = object()
 
     def load_mel_filterbank(self, fb=None):
-        fb = _np(weights.mel_filterbank() if fb is None else fb, np.float32, (config.MEL_DIM, config.N_FFT // 2 + 1), "filterbank")
+        """The filterbank f32 [80,513] of `melspec` and `melspec_forward` (by default the Slaney bank of
+        weights.mel_filterbank(), what MelFilter(16000, 1024, 80) builds).  `gta` always uses the default bank."""
+        fb = _np(weights.mel_filterbank() if fb is None else fb, np.float32, (config.MEL_DIM, config.N_FFT // 2 + 1), "filterbank").copy()
+        self._mel_fb = None
         self._ck(self.lib.vtts_load_mel_filterbank(self.h, _ptr(fb), fb.shape[0], fb.shape[1]))
-        self._mel_loaded = True
+        self._mel_fb = fb
 
     # ---- host-buffer calls -----------------------------------------------------------
     def mel2wave(self, mel, n_frames=None, out=None) -> np.ndarray:
@@ -702,9 +705,10 @@ class Engine:
     def gta(self, wav_i16, tokens, dur_sec, lengths=None, wav_lengths=None, keep_masks=None, zone_masks=None, seed=None, return_gt=False,
             rng=None):
         """forward_fn of nat/gta.py:28-44 in one library call: int16 wavs [B,S] + aligned phonemes -> mel2_hat
-        f32 [B,S/256,80] (rows past wav_lengths[b]//256 are 0).  Masks as in `teacher_forced`."""
-        if not self._mel_loaded:
-            self.load_mel_filterbank()
+        f32 [B,S/256,80] (rows past wav_lengths[b]//256 are 0).  Masks as in `teacher_forced`.  The ground-truth mel
+        (returned first with return_gt) is MelFilter(16000, 1024, 80)(wav / 2**15) with the default filterbank, as the
+        reference builds its own MelFilter (gta.py:29-31), whatever bank `load_mel_filterbank` last loaded; that bank
+        stays loaded for `melspec`."""
         wav = np.ascontiguousarray(np.asarray(wav_i16))
         if wav.dtype != np.int16 or wav.ndim != 2:
             raise ValueError("wav_i16 must be int16 [B,S]")
@@ -719,15 +723,25 @@ class Engine:
         km, zm, mode, seed = self._tf_masks(B, N, keep_masks, zone_masks, seed, rng)
         lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
         wl = None if wav_lengths is None else _np(wav_lengths, np.int32, (B,), "wav_lengths")
+        dur = _np(dur_sec, np.float32, (B, L), "durations")
         gt = np.empty((B, N, config.MEL_DIM), np.float32) if return_gt else None
         out = np.empty((B, N, config.MEL_DIM), np.float32)
-        self._ck(self.lib.vtts_gta_host(self.h, _ptr(wav), _ptr(wl), _ptr(tokens), _ptr(lens), _ptr(_np(dur_sec, np.float32, (B, L), "durations")),
-                                        _ptr(km), _ptr(zm), mode, seed, B, L, S, _ptr(gt), _ptr(out)))
+        kept = self._mel_fb
+        swap = kept is None or not np.array_equal(kept, weights.mel_filterbank())
+        if swap:
+            self.load_mel_filterbank()
+        try:
+            self._ck(self.lib.vtts_gta_host(self.h, _ptr(wav), _ptr(wl), _ptr(tokens), _ptr(lens), _ptr(dur), _ptr(km), _ptr(zm), mode, seed,
+                                            B, L, S, _ptr(gt), _ptr(out)))
+        finally:
+            if swap and kept is not None:
+                self.load_mel_filterbank(kept)
         return (out, gt) if return_gt else out
 
     def melspec(self, wav) -> np.ndarray:
-        """MelFilter.__call__ (nat/dsp.py:115-128): wav f32 [B,S] -> log-mel [B,S/256,80]."""
-        if not self._mel_loaded:
+        """MelFilter.__call__ (nat/dsp.py:115-128): wav f32 [B,S] -> log-mel [B,S/256,80], with the filterbank
+        `load_mel_filterbank` last loaded (the default bank if none)."""
+        if self._mel_fb is None:
             self.load_mel_filterbank()
         wav = _np(wav, np.float32)
         assert wav.ndim == 2, "MelFilter expects [B,S] (dsp.py:118)"
@@ -792,12 +806,13 @@ class Engine:
         return out
 
     def melspec_forward(self, wav_t, out=None, stream=None):
+        """vtts_melspec on torch CUDA tensors, stream-ordered: wav_t f32 [B,S] -> log-mel [B,S/256,80], as `melspec`."""
         import torch
-        if not self._mel_loaded:
-            self.load_mel_filterbank()
+        assert wav_t.is_cuda and wav_t.dtype == torch.float32 and wav_t.is_contiguous() and wav_t.dim() == 2
         B, S = wav_t.shape
-        if out is None:
-            out = torch.empty((B, S // config.HOP, config.MEL_DIM), dtype=torch.float32, device=wav_t.device)
+        out = _out_tensor(out, (B, S // config.HOP, config.MEL_DIM), wav_t.device)
+        if self._mel_fb is None:
+            self.load_mel_filterbank()
         st = torch.cuda.current_stream(wav_t.device).cuda_stream if stream is None else stream
         self._ck(self.lib.vtts_melspec(self.h, _ptr(wav_t), B, S, _ptr(out), st))
         return out

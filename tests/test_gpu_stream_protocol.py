@@ -1,5 +1,5 @@
-"""GPU: the slot protocol every per-slot stream shares (resample, denoise, pitch shift, loudness, vocoder), called
-through the C ABI on device buffers, and the error paths of the host-buffer entry points.
+"""GPU: the slot protocol every per-slot stream shares (resample, denoise, pitch shift, time stretch, loudness, limiter,
+equalizer, vocoder), called through the C ABI on device buffers, and the error paths of the host-buffer entry points.
 
 A rejected push names the entry point and the first bad slot, launches nothing and leaves the stream as it was: the
 valid pushes around it produce the bits of a stream that never saw it."""
@@ -42,9 +42,24 @@ def _pitch(eng):
     return st, "pitch_shift_stream_push", (S, 512), (S, st.out_pitch)
 
 
+def _time_stretch(eng):
+    st = eng.open_time_stretch_stream(S, 512)
+    return st, "time_stretch_stream_push", (S, 512), (S, st.out_pitch)
+
+
 def _loudness(eng):
     st = eng.open_loudness_meter(S, 1600)
     return st, "loudness_stream_push", (S, 1600), (S, 4)
+
+
+def _limiter(eng):
+    st = eng.open_limiter_stream(S, 64)
+    return st, "limiter_stream_push", (S, 64), (S, st.out_pitch)
+
+
+def _eq(eng):
+    st = eng.open_eq_stream(S, 64, "hp:100,pk:1000:1:3")
+    return st, "eq_stream_push", (S, 64), (S, st.out_pitch)
 
 
 def _vocoder(eng):
@@ -52,7 +67,8 @@ def _vocoder(eng):
     return st, "vocoder_stream_push", (S, 8, 80), (S, st.wav_ld)
 
 
-STREAMS = {"resample": _resample, "denoise": _denoise, "pitch": _pitch, "loudness": _loudness, "vocoder": _vocoder}
+STREAMS = {"resample": _resample, "denoise": _denoise, "pitch": _pitch, "time_stretch": _time_stretch, "loudness": _loudness,
+           "limiter": _limiter, "eq": _eq, "vocoder": _vocoder}
 
 
 def _push(eng, name, st, ctx, x, n_new, flags, y, n_out):
@@ -62,9 +78,12 @@ def _push(eng, name, st, ctx, x, n_new, flags, y, n_out):
     f = None if flags is None else np.ascontiguousarray(flags, np.uint8)
     ptr = lambda a: None if a is None else a.ctypes.data
     no = None if n_out is None else n_out.ctypes.data
-    if name == "pitch_shift_stream_push":
-        sem = np.full(S, 3.0, np.float32)
-        rc = lib.vtts_pitch_shift_stream_push(ctx, st.h, _p(x), ptr(n), ptr(f), sem.ctypes.data, _p(y), no, s)
+    if name in ("pitch_shift_stream_push", "time_stretch_stream_push"):
+        par = np.full(S, 3.0 if name == "pitch_shift_stream_push" else 1.5, np.float32)   # semitones / tempo
+        rc = getattr(lib, "vtts_" + name)(ctx, st.h, _p(x), ptr(n), ptr(f), par.ctypes.data, _p(y), no, s)
+    elif name == "limiter_stream_push":
+        gain, red = np.full(S, 6.0, np.float32), torch.zeros(S, device="cuda")
+        rc = lib.vtts_limiter_stream_push(ctx, st.h, _p(x), ptr(n), ptr(f), gain.ctypes.data, _p(y), no, _p(red), s)
     elif name == "loudness_stream_push":
         rc = lib.vtts_loudness_stream_push(ctx, st.h, _p(x), ptr(n), ptr(f), _p(y), s)
     else:

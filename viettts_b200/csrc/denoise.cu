@@ -195,10 +195,8 @@ int vtts_denoise_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B,
   if (!x || !y || !bias || B < 1 || B > 65535 || S < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_host: bad argument (B=%d S=%d)", B, S);
   if (!finite_nonneg(strength)) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_host: strength %g (finite and >= 0)", (double)strength);
   int rc = dn_check_bias(ctx, "denoise_host", bias);
+  if (!rc) rc = host_lengths_check(ctx, "denoise_host", n_in, B, S);
   if (rc) return rc;
-  if (n_in)
-    for (int b = 0; b < B; ++b)
-      if (n_in[b] < 0 || n_in[b] > S) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_host: n[%d]=%d outside [0, %d]", b, n_in[b], S);
   VTTS_CUDA(cudaSetDevice(ctx->device));
   const size_t x_b = (size_t)B * S * 4;
   HostStage hs(ctx);
@@ -226,15 +224,12 @@ int vtts_denoise_bias(vtts_ctx* ctx, const float* wav_dev, int n, float* bias_de
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
-struct vtts_denoise_stream : StreamBase {
-  using StreamBase::StreamBase;
-  int cap = 0, out_pitch = 0, ws_frames = 0;
+struct vtts_denoise_stream : SampleStream<DnRow> {
+  using SampleStream::SampleStream;
+  int out_pitch = 0, ws_frames = 0;
   float strength = 0.f;
-  float* win = nullptr;         // windows [S][cap]
   float* ws = nullptr;          // frame workspace [S][ws_frames][1024]
   float* bias = nullptr;        // [513]
-  char* d_tbl = nullptr;        // the per-push tables, laid out as their host image tbl: DnRow [S], then int [S][2]
-  std::vector<char> tbl;
 };
 
 int vtts_denoise_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, float strength, const float* bias,
@@ -251,19 +246,17 @@ int vtts_denoise_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_sam
   VTTS_CUDA(cudaSetDevice(ctx->device));
   rc = vtts_fft_tables(ctx);
   if (rc) return rc;
-  std::unique_ptr<vtts_denoise_stream> ds(new vtts_denoise_stream(ctx, max_streams, max_chunk_samples));
-  ds->cap = DN_K + max_chunk_samples;
+  std::unique_ptr<vtts_denoise_stream> ds(new vtts_denoise_stream(ctx, max_streams, max_chunk_samples, DN_K));
   // outputs per push: fewer than n_new + 256 before END, at most n_new + 1023 with it (E(P0) >= P0 - 1023)
   ds->out_pitch = max_chunk_samples + DN_LOOKAHEAD;
   // frames per push: outputs [E0, E1) read frames floor((E0 - 511) / 256) .. floor((E1 + 511) / 256)
   ds->ws_frames = (ds->out_pitch + 2 * PAD) / HOP + 2;
   ds->strength = strength;
-  ds->tbl.assign((size_t)max_streams * (sizeof(DnRow) + 2 * sizeof(int)), 0);
   rc = stream_alloc(ctx, "denoise_stream_create", *ds, [&](Arena& a) {
-    ds->win = a.take<float>((size_t)max_streams * ds->cap);
+    ds->carve_window(a);
     ds->ws = a.take<float>((size_t)max_streams * ds->ws_frames * NF);
     ds->bias = a.take<float>(NB);
-    ds->d_tbl = a.take<char>(ds->tbl.size());
+    ds->carve_tables(a);
   });
   if (rc) return rc;
   VTTS_CUDA(cudaMemcpy(ds->bias, bias, (size_t)NB * sizeof(float), cudaMemcpyHostToDevice));
@@ -286,8 +279,7 @@ int vtts_denoise_stream_push(vtts_ctx* ctx, vtts_denoise_stream* ds, const float
   const SlotState& sl = ds->slots;
 
   // ---- host bookkeeping: outputs [E0, E1) of this push and the frames they read ----
-  DnRow* rows = reinterpret_cast<DnRow*>(ds->tbl.data());
-  int* prep = reinterpret_cast<int*>(ds->tbl.data() + (size_t)S * sizeof(DnRow));
+  DnRow* rows = ds->rows<0>();
   std::vector<long long> E1(S);
   long long max_out = 0, max_frames = 0;
   for (int s = 0; s < S; ++s) {
@@ -315,16 +307,11 @@ int vtts_denoise_stream_push(vtts_ctx* ctx, vtts_denoise_stream* ds, const float
     max_out = std::max(max_out, r.cnt);
     max_frames = std::max(max_frames, (long long)r.nfr);
   }
-  sl.prep(n_new, flags, prep);
 
   // ---- device: one table copy, prep, frames, overlap-add (three launches) ----
-  // pageable source: the call returns once the table is staged, so ds->tbl may be rewritten by the next push
-  VTTS_CUDA(cudaMemcpyAsync(ds->d_tbl, ds->tbl.data(), ds->tbl.size(), cudaMemcpyHostToDevice, st));
-  const DnRow* d_rows = reinterpret_cast<const DnRow*>(ds->d_tbl);
-  const int* d_prep = reinterpret_cast<const int*>(ds->d_tbl + (size_t)S * sizeof(DnRow));
-  rc = vtts_stream_window_prep(ctx, ds->win, ds->cap, DN_K, d_prep, x_dev, ds->F, S, st);
+  rc = ds->upload(n_new, flags, x_dev, st);
   if (rc) return rc;
-  rc = dn_launch(ctx, ds->win, ds->cap, ds->cap, nullptr, d_rows, S, max_frames, max_out, ds->strength, ds->bias, ds->ws, ds->ws_frames,
+  rc = dn_launch(ctx, ds->win, ds->cap, ds->cap, nullptr, ds->d_rows<0>(), S, max_frames, max_out, ds->strength, ds->bias, ds->ws, ds->ws_frames,
                  y_dev, ds->out_pitch, st);
   if (rc) return rc;
   ds->slots.commit(n_new, flags, E1.data());

@@ -424,10 +424,8 @@ int vtts_eq_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int 
   EqFilter f;
   int rc = eq_check(ctx, "eq_host", B, S);
   if (!rc) rc = eq_filter(ctx, "eq_host", sos, K, &f);
+  if (!rc) rc = host_lengths_check(ctx, "eq_host", n_in, B, S);
   if (rc) return rc;
-  if (n_in)
-    for (int b = 0; b < B; ++b)
-      if (n_in[b] < 0 || n_in[b] > S) return ctx->fail(VTTS_ERR_BAD_ARG, "eq_host: n[%d]=%d outside [0, %d]", b, n_in[b], S);
   if (!x || !y) return ctx->fail(VTTS_ERR_BAD_ARG, "eq_host: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
   const size_t x_b = (size_t)B * S * 4, n_b = (size_t)B * 4;
@@ -441,13 +439,11 @@ int vtts_eq_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int 
 
 // ---- stream ---------------------------------------------------------------------------------------------------
 // The shared slot state counts samples received in P and released in E (the same: no lookahead).
-struct vtts_eq_stream : StreamBase {
-  using StreamBase::StreamBase;
+struct vtts_eq_stream : SampleStream<EqRow> {
+  using SampleStream::SampleStream;
   EqFilter f{};
-  int cap = 0, ld_k = 0;
-  float *win = nullptr, *e = nullptr, *s = nullptr, *carry = nullptr;
-  char* d_tbl = nullptr;        // the per-push tables, laid out as their host image tbl: EqRow [S], int [S][2]
-  std::vector<char> tbl;
+  int ld_k = 0;
+  float *e = nullptr, *s = nullptr, *carry = nullptr;
 };
 
 int vtts_eq_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, const double* sos, int K, vtts_eq_stream** out) {
@@ -461,18 +457,16 @@ int vtts_eq_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples,
   int rc = eq_filter(ctx, "eq_stream_create", sos, K, &f);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  std::unique_ptr<vtts_eq_stream> es(new vtts_eq_stream(ctx, max_streams, max_chunk_samples));
+  std::unique_ptr<vtts_eq_stream> es(new vtts_eq_stream(ctx, max_streams, max_chunk_samples, Q));
   es->f = f;
-  es->cap = Q + max_chunk_samples;
   es->ld_k = (Q - 1 + max_chunk_samples + Q - 1) / Q;     // blocks one push can touch
   const size_t S = max_streams;
-  es->tbl.assign(S * (sizeof(EqRow) + 2 * sizeof(int)), 0);
   rc = stream_alloc(ctx, "eq_stream_create", *es, [&](Arena& a) {
-    es->win = a.take<float>(S * es->cap);
+    es->carve_window(a);
     es->e = a.take<float>(S * es->ld_k * NS);
     es->s = a.take<float>(S * es->ld_k * NS);
     es->carry = a.take<float>(S * NS);
-    es->d_tbl = a.take<char>(es->tbl.size());
+    es->carve_tables(a);
   });
   if (rc) return rc;
   *out = es.release();
@@ -494,8 +488,7 @@ int vtts_eq_stream_push(vtts_ctx* ctx, vtts_eq_stream* es, const float* x_dev, c
   const int S = es->S;
 
   // ---- host bookkeeping: every sample is released in the push that brings it ----
-  EqRow* rows = reinterpret_cast<EqRow*>(es->tbl.data());
-  int* prep = reinterpret_cast<int*>(es->tbl.data() + (size_t)S * sizeof(EqRow));
+  EqRow* rows = es->rows<0>();
   std::vector<long long> E1(S);
   long long max_k = 0;
   for (int s = 0; s < S; ++s) {
@@ -514,17 +507,12 @@ int vtts_eq_stream_push(vtts_ctx* ctx, vtts_eq_stream* es, const float* x_dev, c
     n_out[s] = (int32_t)(P1 - P0);
     max_k = std::max(max_k, (long long)r.nk);
   }
-  sl.prep(n_new, flags, prep);
   if (max_k > es->ld_k) return ctx->fail(VTTS_ERR_CUDA, "eq_stream_push: %lld blocks (internal bound %d)", max_k, es->ld_k);
 
   // ---- device: one table copy, window step, the three filter launches (four in all) ----
-  // pageable source: the call returns once the tables are staged, so es->tbl may be rewritten by the next push
-  VTTS_CUDA(cudaMemcpyAsync(es->d_tbl, es->tbl.data(), es->tbl.size(), cudaMemcpyHostToDevice, st));
-  const EqRow* d_rows = reinterpret_cast<const EqRow*>(es->d_tbl);
-  const int* d_prep = reinterpret_cast<const int*>(es->d_tbl + (size_t)S * sizeof(EqRow));
-  rc = vtts_stream_window_prep(ctx, es->win, es->cap, Q, d_prep, x_dev, es->F, S, st);
+  rc = es->upload(n_new, flags, x_dev, st);
   if (rc) return rc;
-  rc = eq_run(ctx, es->f, es->win, es->cap, es->cap, nullptr, d_rows, S, max_k, es->ld_k, es->e, es->s, es->carry, y_dev, es->F, st);
+  rc = eq_run(ctx, es->f, es->win, es->cap, es->cap, nullptr, es->d_rows<0>(), S, max_k, es->ld_k, es->e, es->s, es->carry, y_dev, es->F, st);
   if (rc) return rc;
   es->slots.commit(n_new, flags, E1.data());
   return VTTS_OK;

@@ -339,9 +339,8 @@ int lm_check(vtts_ctx* ctx, const char* who, int B, int S) {
 }
 
 int lm_check_host(vtts_ctx* ctx, const char* who, const int32_t* n_in, const float* gain_db, int B, int S) {
-  if (n_in)
-    for (int b = 0; b < B; ++b)
-      if (n_in[b] < 0 || n_in[b] > S) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: n[%d]=%d outside [0, %d]", who, b, n_in[b], S);
+  const int rc = host_lengths_check(ctx, who, n_in, B, S);
+  if (rc) return rc;
   if (gain_db)
     for (int b = 0; b < B; ++b)
       if (!(gain_db[b] >= -70.f && gain_db[b] <= 70.f))
@@ -535,15 +534,14 @@ int vtts_loudness_normalize_limited_host(vtts_ctx* ctx, const float* x, const in
 
 // ---- stream ---------------------------------------------------------------------------------------------------
 // The shared slot state counts samples received in P and samples released in E.
-struct vtts_limiter_stream : StreamBase {
-  using StreamBase::StreamBase;
-  int rate = 0, H = 0, cap = 0, look = 0, pitch = 0;
+// The window carries H = 2 W + 64 samples: tau of the earliest sample a push needs reads inputs from t - W + 1 - 2 D - 1
+// on, t >= P0 - look, that is 2 W + 40 back.
+struct vtts_limiter_stream : SampleStream<LmRow, RsRow> {
+  using SampleStream::SampleStream;
+  int rate = 0, look = 0, pitch = 0;
   LmParams p{};
-  float* win = nullptr;              // windows [S][cap]
   LmBufs w{};
   std::vector<float> gain;           // each slot's pre-gain since its BEGIN
-  char* d_tbl = nullptr;             // the per-push tables, laid out as their host image tbl: LmRow [S], RsRow [S], int [S][2]
-  std::vector<char> tbl;
 };
 
 int vtts_limiter_stream_lookahead(int rate, float lookahead_ms) {
@@ -565,19 +563,15 @@ int vtts_limiter_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_sam
     return ctx->fail(VTTS_ERR_BAD_ARG, "limiter_stream_create: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", max_streams,
                      max_chunk_samples, 1 << 22);
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  std::unique_ptr<vtts_limiter_stream> ls(new vtts_limiter_stream(ctx, max_streams, max_chunk_samples));
+  std::unique_ptr<vtts_limiter_stream> ls(new vtts_limiter_stream(ctx, max_streams, max_chunk_samples, 2 * p.W + 64));
   ls->rate = rate;
   ls->p = p;
   ls->look = vtts_limiter_stream_lookahead(rate, lookahead_ms);
-  // tau of the earliest sample a push needs reads inputs from t - W + 1 - 2 D - 1 on, t >= P0 - look: 2 W + 40 back
-  ls->H = 2 * p.W + 64;
-  ls->cap = ls->H + max_chunk_samples;
   ls->pitch = max_chunk_samples + ls->look;   // END releases at most n_new + look
   ls->gain.assign(max_streams, 0.f);
   const size_t S = max_streams, nb = lm_blocks_max(ls->pitch);
-  ls->tbl.assign(S * (sizeof(LmRow) + sizeof(RsRow) + 2 * sizeof(int)), 0);
   rc = stream_alloc(ctx, "limiter_stream_create", *ls, [&](Arena& a) {
-    ls->win = a.take<float>(S * ls->cap);
+    ls->carve_window(a);
     ls->w.v = a.take<float>(S * ls->cap);
     ls->w.tau = a.take<float>(S * ls->cap);
     ls->w.alpha = a.take<float>(S * ls->cap);
@@ -589,7 +583,7 @@ int vtts_limiter_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_sam
     ls->w.carry_map = a.take<float4>(S);
     ls->w.carry_din = a.take<float>(S);
     ls->w.carry_min = a.take<float>(S);
-    ls->d_tbl = a.take<char>(ls->tbl.size());
+    ls->carve_tables(a);
   });
   if (rc) return rc;
   const std::vector<float> ones(S, 1.f);   // no reduction yet
@@ -621,9 +615,8 @@ int vtts_limiter_stream_push(vtts_ctx* ctx, vtts_limiter_stream* ls, const float
   const int S = ls->S;
 
   // ---- host bookkeeping: before END sample t is released once P > t + look; END releases the rest ----
-  LmRow* rows = reinterpret_cast<LmRow*>(ls->tbl.data());
-  RsRow* rs = reinterpret_cast<RsRow*>(ls->tbl.data() + (size_t)S * sizeof(LmRow));
-  int* prep = reinterpret_cast<int*>(ls->tbl.data() + (size_t)S * (sizeof(LmRow) + sizeof(RsRow)));
+  LmRow* rows = ls->rows<0>();
+  RsRow* rs = ls->rows<1>();
   std::vector<long long> E1(S);
   long long max_u = 0, max_tn = 0, max_rn = 0;
   for (int s = 0; s < S; ++s) {
@@ -632,7 +625,7 @@ int vtts_limiter_stream_push(vtts_ctx* ctx, vtts_limiter_stream* ls, const float
     const long long R1 = act ? (end ? P1 : std::max(R0, P1 - ls->look)) : R0;
     const float g = begin ? gain_db[s] : ls->gain[s];
     LmRow r{};
-    r.x0 = P0 - ls->H;
+    r.x0 = P0 - ls->K;
     r.u0 = std::max(0LL, OS * r.x0);
     r.n = P1;
     r.r0 = R0;
@@ -650,24 +643,19 @@ int vtts_limiter_stream_push(vtts_ctx* ctx, vtts_limiter_stream* ls, const float
     max_tn = std::max(max_tn, r.tn);
     max_rn = std::max(max_rn, r.rn);
   }
-  sl.prep(n_new, flags, prep);
   if (max_rn > ls->pitch || max_u > ls->w.u_ld)
     return ctx->fail(VTTS_ERR_CUDA, "limiter_stream_push: %lld outputs / %lld oversampled (internal bound %d / %lld)", max_rn, max_u, ls->pitch,
                      ls->w.u_ld);
 
   // ---- device: one table copy, window step, gain, then the limiter's seven launches (nine in all) ----
-  // pageable source: the call returns once the tables are staged, so ls->tbl may be rewritten by the next push
-  VTTS_CUDA(cudaMemcpyAsync(ls->d_tbl, ls->tbl.data(), ls->tbl.size(), cudaMemcpyHostToDevice, st));
-  const LmRow* d_rows = reinterpret_cast<const LmRow*>(ls->d_tbl);
-  const RsRow* d_rs = reinterpret_cast<const RsRow*>(ls->d_tbl + (size_t)S * sizeof(LmRow));
-  const int* d_prep = reinterpret_cast<const int*>(ls->d_tbl + (size_t)S * (sizeof(LmRow) + sizeof(RsRow)));
-  rc = vtts_stream_window_prep(ctx, ls->win, ls->cap, ls->H, d_prep, x_dev, ls->F, S, st);
+  rc = ls->upload(n_new, flags, x_dev, st);
   if (rc) return rc;
+  const LmRow* d_rows = ls->d_rows<0>();
   lm_gain_kernel<<<dim3((ls->cap + THREADS - 1) / THREADS, S), THREADS, 0, st>>>(ls->win, ls->cap, ls->cap, nullptr, nullptr, d_rows, ls->cap,
                                                                                   ls->w.v, ls->w.v_ld, nullptr);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
-  rc = lm_run(ctx, ls->p, ls->rate, ls->cap, nullptr, d_rows, d_rs, S, max_u, max_tn, max_rn, ls->w, y_dev, ls->pitch, reduction_db_dev, st);
+  rc = lm_run(ctx, ls->p, ls->rate, ls->cap, nullptr, d_rows, ls->d_rows<1>(), S, max_u, max_tn, max_rn, ls->w, y_dev, ls->pitch, reduction_db_dev, st);
   if (rc) return rc;
   for (int s = 0; s < S; ++s)
     if (flags[s] & 1) ls->gain[s] = gain_db[s];

@@ -439,13 +439,6 @@ int ln_check_target(vtts_ctx* ctx, const char* who, float target, float ceiling)
   return VTTS_OK;
 }
 
-int ln_check_lengths(vtts_ctx* ctx, const char* who, const int32_t* n_in, int B, int S) {
-  if (n_in)
-    for (int b = 0; b < B; ++b)
-      if (n_in[b] < 0 || n_in[b] > S) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: n[%d]=%d outside [0, %d]", who, b, n_in[b], S);
-  return VTTS_OK;
-}
-
 }  // namespace
 
 size_t vtts_loudness_ws_bytes(int B, int S, int rate) {
@@ -504,7 +497,7 @@ int vtts_loudness_normalize(vtts_ctx* ctx, const float* x_dev, const int32_t* n_
 int vtts_loudness_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float* out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   int rc = ln_check(ctx, "loudness_host", rate, B, S);
-  if (!rc) rc = ln_check_lengths(ctx, "loudness_host", n_in, B, S);
+  if (!rc) rc = host_lengths_check(ctx, "loudness_host", n_in, B, S);
   if (rc) return rc;
   if (!x || !out) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_host: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
@@ -522,7 +515,7 @@ int vtts_loudness_normalize_host(vtts_ctx* ctx, const float* x, const int32_t* n
   if (!ctx) return VTTS_ERR_BAD_ARG;
   int rc = ln_check(ctx, "loudness_normalize_host", rate, B, S);
   if (!rc) rc = ln_check_target(ctx, "loudness_normalize_host", target, ceiling);
-  if (!rc) rc = ln_check_lengths(ctx, "loudness_normalize_host", n_in, B, S);
+  if (!rc) rc = host_lengths_check(ctx, "loudness_normalize_host", n_in, B, S);
   if (rc) return rc;
   if (!x || !y) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_normalize_host: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
@@ -540,13 +533,10 @@ int vtts_loudness_normalize_host(vtts_ctx* ctx, const float* x, const int32_t* n
 
 // ---- stream ---------------------------------------------------------------------------------------------------
 // The shared slot state counts samples in P and, in E, the oversampled outputs the running peak covers.
-struct vtts_loudness_stream : StreamBase {
-  using StreamBase::StreamBase;
-  int rate = 0, m = 0, cap = 0, hcap = 0, kpush = 0, upitch = 0, ptiles = 0;
-  float* win = nullptr;         // windows [S][cap]
+struct vtts_loudness_stream : SampleStream<LnRow, RsRow> {
+  using SampleStream::SampleStream;
+  int rate = 0, m = 0, hcap = 0, kpush = 0, upitch = 0, ptiles = 0;
   LnBufs w{};
-  char* d_tbl = nullptr;        // the per-push tables, laid out as their host image tbl: LnRow [S], RsRow [S], int [S][2]
-  std::vector<char> tbl;
 };
 
 int vtts_loudness_stream_lookahead(int rate) {
@@ -565,19 +555,17 @@ int vtts_loudness_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_sa
                      max_streams, max_chunk_samples, max_seconds, 1 << 22, 1 << 20);
   VTTS_CUDA(cudaSetDevice(ctx->device));
   ln_filter(ctx, rate);
-  std::unique_ptr<vtts_loudness_stream> ls(new vtts_loudness_stream(ctx, max_streams, max_chunk_samples));
+  std::unique_ptr<vtts_loudness_stream> ls(new vtts_loudness_stream(ctx, max_streams, max_chunk_samples, rate / 10));
   ls->rate = rate;
   ls->m = rate / 10;
-  ls->cap = ls->m + max_chunk_samples;
   ls->hcap = 10 * max_seconds;
   ls->kpush = (ls->m - 1 + max_chunk_samples) / ls->m;            // complete sub-blocks one push can bring
   ls->upitch = OS * max_chunk_samples + 10 * OS + 1;              // oversampled outputs one push can cover
   ls->ptiles = (max_chunk_samples + ls->upitch + PEAK_TILE - 1) / PEAK_TILE;
   const size_t S = max_streams, kp = std::max(1, ls->kpush);
   static_assert(sizeof(LnRow) % 16 == 0 && sizeof(RsRow) % 16 == 0, "table entries keep 16-byte alignment");
-  ls->tbl.assign(S * (sizeof(LnRow) + sizeof(RsRow) + 2 * sizeof(int)), 0);
   int rc = stream_alloc(ctx, "loudness_stream_create", *ls, [&](Arena& a) {
-    ls->win = a.take<float>(S * ls->cap);
+    ls->carve_window(a);
     ls->w.e = a.take<float>(S * kp * 4);
     ls->w.s = a.take<float>(S * kp * 4);
     ls->w.E = a.take<float>(S * ls->hcap);
@@ -585,7 +573,7 @@ int vtts_loudness_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_sa
     ls->w.peak = a.take<float>(S);
     ls->w.u = a.take<float>(S * ls->upitch);
     ls->w.part = a.take<float>(S * ls->ptiles);
-    ls->d_tbl = a.take<char>(ls->tbl.size());
+    ls->carve_tables(a);
   });
   if (rc) return rc;
   ls->w.ld_k = (int)kp;
@@ -618,9 +606,8 @@ int vtts_loudness_stream_push(vtts_ctx* ctx, vtts_loudness_stream* ls, const flo
 
   // ---- host bookkeeping: the sub-blocks this push completes and the oversampled outputs whose inputs have all arrived
   // (resample stream schedule of 4 / 1: max(0, 4 P - 40) before END, 4 P with it) ----
-  LnRow* rows = reinterpret_cast<LnRow*>(ls->tbl.data());
-  RsRow* rs = reinterpret_cast<RsRow*>(ls->tbl.data() + (size_t)S * sizeof(LnRow));
-  int* prep = reinterpret_cast<int*>(ls->tbl.data() + (size_t)S * (sizeof(LnRow) + sizeof(RsRow)));
+  LnRow* rows = ls->rows<0>();
+  RsRow* rs = ls->rows<1>();
   const long long half = (long long)vtts_resample_stream_lookahead(1, OS) * OS;
   std::vector<long long> U1(S);
   long long max_k = 0, max_u = 0, max_peak = 0;
@@ -644,20 +631,14 @@ int vtts_loudness_stream_push(vtts_ctx* ctx, vtts_loudness_stream* ls, const flo
     max_u = std::max(max_u, r.nu);
     max_peak = std::max(max_peak, r.nx + r.nu);
   }
-  sl.prep(n_new, flags, prep);
   if (max_u > ls->upitch || max_k > ls->w.ld_k)
     return ctx->fail(VTTS_ERR_CUDA, "loudness_stream_push: %lld outputs / %lld sub-blocks (internal bound %d / %d)", max_u, max_k, ls->upitch,
                      ls->w.ld_k);
 
   // ---- device: one table copy, window step, the six measuring launches (seven in all) ----
-  // pageable source: the call returns once the tables are staged, so ls->tbl may be rewritten by the next push
-  VTTS_CUDA(cudaMemcpyAsync(ls->d_tbl, ls->tbl.data(), ls->tbl.size(), cudaMemcpyHostToDevice, st));
-  const LnRow* d_rows = reinterpret_cast<const LnRow*>(ls->d_tbl);
-  const RsRow* d_rs = reinterpret_cast<const RsRow*>(ls->d_tbl + (size_t)S * sizeof(LnRow));
-  const int* d_prep = reinterpret_cast<const int*>(ls->d_tbl + (size_t)S * (sizeof(LnRow) + sizeof(RsRow)));
-  rc = vtts_stream_window_prep(ctx, ls->win, ls->cap, m, d_prep, x_dev, ls->F, S, st);
+  rc = ls->upload(n_new, flags, x_dev, st);
   if (rc) return rc;
-  rc = ln_measure(ctx, ln_filter(ctx, ls->rate), ls->win, ls->cap, ls->cap, nullptr, d_rows, d_rs, S, max_k, max_u, max_peak, ls->w,
+  rc = ln_measure(ctx, ln_filter(ctx, ls->rate), ls->win, ls->cap, ls->cap, nullptr, ls->d_rows<0>(), ls->d_rows<1>(), S, max_k, max_u, max_peak, ls->w,
                   out_dev, 0.f, INFINITY, nullptr, nullptr, st);
   if (rc) return rc;
   ls->slots.commit(n_new, flags, U1.data());

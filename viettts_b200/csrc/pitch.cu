@@ -463,10 +463,8 @@ int vtts_pitch_shift_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, in
   if (!ctx) return VTTS_ERR_BAD_ARG;
   if (!x || !y || B < 1 || B > 65535 || S < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_host: bad argument (B=%d S=%d)", B, S);
   int rc = ps_check_shifts(ctx, "pitch_shift_host", semitones, B);
+  if (!rc) rc = host_lengths_check(ctx, "pitch_shift_host", n_in, B, S);
   if (rc) return rc;
-  if (n_in)
-    for (int b = 0; b < B; ++b)
-      if (n_in[b] < 0 || n_in[b] > S) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_host: n[%d]=%d outside [0, %d]", b, n_in[b], S);
   VTTS_CUDA(cudaSetDevice(ctx->device));
   const size_t x_b = (size_t)B * S * 4;
   HostStage hs(ctx);
@@ -500,10 +498,8 @@ int vtts_time_stretch_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, i
   if (!x || !y || B < 1 || B > 65535 || S < 1 || Sy < 1)
     return ctx->fail(VTTS_ERR_BAD_ARG, "time_stretch_host: bad argument (B=%d S=%d Sy=%d)", B, S, Sy);
   int rc = ts_check_tempos(ctx, "time_stretch_host", tempo, B);
+  if (!rc) rc = host_lengths_check(ctx, "time_stretch_host", n_in, B, S);
   if (rc) return rc;
-  if (n_in)
-    for (int b = 0; b < B; ++b)
-      if (n_in[b] < 0 || n_in[b] > S) return ctx->fail(VTTS_ERR_BAD_ARG, "time_stretch_host: n[%d]=%d outside [0, %d]", b, n_in[b], S);
   VTTS_CUDA(cudaSetDevice(ctx->device));
   const size_t x_b = (size_t)B * S * 4, y_b = (size_t)B * Sy * 4;
   HostStage hs(ctx);
@@ -518,20 +514,17 @@ int vtts_time_stretch_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, i
 
 // ---- streams ---------------------------------------------------------------------------------------------------
 // One implementation serves both vocoder streams; `stretch` selects the time stretcher's frame positions and schedule.
-struct PvStream : StreamBase {
-  using StreamBase::StreamBase;
-  int cap = 0, out_pitch = 0;
+struct PvStream : SampleStream<DnRow, PsRow> {
+  using SampleStream::SampleStream;
+  int out_pitch = 0;
   bool stretch = false;
   PsWs w{};
-  float* win = nullptr;         // windows [S][cap]
   double* state = nullptr;      // [S][2][513]
-  char* d_tbl = nullptr;        // the per-push tables, laid out as their host image tbl: DnRow [S], PsRow [S], int [S][2]
   // per slot besides the shared state: next unscanned frame, first frame and half of the last push's synthesized-frame
   // buffer, shift or tempo since BEGIN
   std::vector<long long> q, fb;
   std::vector<int> half;
   std::vector<float> par;
-  std::vector<char> tbl;
 };
 struct vtts_pitch_shift_stream : PvStream {
   using PvStream::PvStream;
@@ -555,9 +548,8 @@ int pv_create(vtts_ctx* ctx, const char* who, int max_streams, int max_chunk_sam
   int rc = vtts_fft_tables(ctx);
   if (rc) return rc;
   const int S = max_streams;
-  std::unique_ptr<Stream> ps(new Stream(ctx, S, max_chunk_samples));
+  std::unique_ptr<Stream> ps(new Stream(ctx, S, max_chunk_samples, PS_K));
   ps->stretch = stretch;
-  ps->cap = PS_K + max_chunk_samples;
   if (!stretch) {
     ps->out_pitch = max_chunk_samples + PS_LOOKAHEAD;  // as the denoise stream
     // frames scanned per push: at most n_new / 256 + 3 (with END); the buffer also holds the <= 3 carried frames
@@ -574,12 +566,11 @@ int pv_create(vtts_ctx* ctx, const char* who, int max_streams, int max_chunk_sam
   ps->fb.assign(S, 0);
   ps->half.assign(S, 0);
   ps->par.assign(S, stretch ? 1.f : 0.f);
-  ps->tbl.assign((size_t)S * (sizeof(DnRow) + sizeof(PsRow) + 2 * sizeof(int)), 0);
   rc = stream_alloc(ctx, who, *ps, [&](Arena& a) {
-    ps->win = a.take<float>((size_t)S * ps->cap);
+    ps->carve_window(a);
     ps_carve(a, ps->w, S);
     ps->state = a.take<double>((size_t)S * 2 * NB);
-    ps->d_tbl = a.take<char>(ps->tbl.size());
+    ps->carve_tables(a);
   });
   if (rc) return rc;
   *out_pitch = ps->out_pitch;
@@ -622,9 +613,8 @@ int pv_push(vtts_ctx* ctx, const char* who, PvStream* ps, const float* x_dev, co
   const SlotState& sl = ps->slots;
 
   // ---- host bookkeeping: outputs [E0, E1), frames [q0, q1) scanned, synthesized-frame buffer [fb, q1) ----
-  DnRow* rows = reinterpret_cast<DnRow*>(ps->tbl.data());
-  PsRow* prow = reinterpret_cast<PsRow*>(ps->tbl.data() + (size_t)S * sizeof(DnRow));
-  int* prep = reinterpret_cast<int*>(ps->tbl.data() + (size_t)S * (sizeof(DnRow) + sizeof(PsRow)));
+  DnRow* rows = ps->rows<0>();
+  PsRow* prow = ps->rows<1>();
   std::vector<long long> E1(S), Q1(S);
   long long max_out = 0, max_nq = 0, max_nsyn = 0;
   for (int s = 0; s < S; ++s) {
@@ -688,19 +678,13 @@ int pv_push(vtts_ctx* ctx, const char* who, PvStream* ps, const float* x_dev, co
     max_nq = std::max(max_nq, (long long)p.nq);
     max_nsyn = std::max(max_nsyn, (long long)p.nsyn);
   }
-  sl.prep(n_new, flags, prep);
 
   // ---- device: table copy, window step, analysis, phase, synthesis, overlap-add (five launches) ----
-  // pageable source: the call returns once the table is staged, so ps->tbl may be rewritten by the next push
-  VTTS_CUDA(cudaMemcpyAsync(ps->d_tbl, ps->tbl.data(), ps->tbl.size(), cudaMemcpyHostToDevice, st));
-  const DnRow* d_rows = reinterpret_cast<const DnRow*>(ps->d_tbl);
-  const PsRow* d_prow = reinterpret_cast<const PsRow*>(ps->d_tbl + (size_t)S * sizeof(DnRow));
-  const int* d_prep = reinterpret_cast<const int*>(ps->d_tbl + (size_t)S * (sizeof(DnRow) + sizeof(PsRow)));
-  rc = vtts_stream_window_prep(ctx, ps->win, ps->cap, PS_K, d_prep, x_dev, ps->F, S, st);
+  rc = ps->upload(n_new, flags, x_dev, st);
   if (rc) return rc;
-  rc = ps_launch(ctx, ps->win, ps->cap, ps->cap, nullptr, nullptr, d_prow, S, max_nq, max_nsyn, ps->w, ps->state, nullptr, 0, nullptr, 0, st);
+  rc = ps_launch(ctx, ps->win, ps->cap, ps->cap, nullptr, nullptr, ps->d_rows<1>(), S, max_nq, max_nsyn, ps->w, ps->state, nullptr, 0, nullptr, 0, st);
   if (rc) return rc;
-  rc = vtts_denoise_ola(ctx, ps->win, ps->cap, ps->cap, nullptr, d_rows, S, max_out, ps->w.syn, 2 * ps->w.nbuf, y_dev, ps->out_pitch, st);
+  rc = vtts_denoise_ola(ctx, ps->win, ps->cap, ps->cap, nullptr, ps->d_rows<0>(), S, max_out, ps->w.syn, 2 * ps->w.nbuf, y_dev, ps->out_pitch, st);
   if (rc) return rc;
 
   // ---- commit the slot state ----

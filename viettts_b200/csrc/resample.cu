@@ -287,14 +287,11 @@ int vtts_resample_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
-struct vtts_resample_stream : StreamBase {
-  using StreamBase::StreamBase;
+struct vtts_resample_stream : SampleStream<RsRow> {
+  using SampleStream::SampleStream;
   RsRatio r{};
-  int K = 0, cap = 0, out_pitch = 0;
+  int out_pitch = 0;
   const float* taps = nullptr;
-  float* win = nullptr;         // windows [S][cap]
-  char* d_tbl = nullptr;        // the per-push tables, laid out as their host image tbl: RsRow [S], then int [S][2]
-  std::vector<char> tbl;
 };
 
 int vtts_resample_stream_lookahead(int in_rate, int out_rate) {
@@ -322,16 +319,13 @@ int vtts_resample_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_sa
   const float* taps = nullptr;
   int rc = rs_filter(ctx, r, &taps);
   if (rc) return rc;
-  std::unique_ptr<vtts_resample_stream> rs(new vtts_resample_stream(ctx, max_streams, max_chunk_samples));
+  std::unique_ptr<vtts_resample_stream> rs(new vtts_resample_stream(ctx, max_streams, max_chunk_samples, r.T - 1));
   rs->r = r;
-  rs->K = r.T - 1;
-  rs->cap = rs->K + max_chunk_samples;
   rs->out_pitch = (int)pitch;
   rs->taps = taps;
-  rs->tbl.assign((size_t)max_streams * (sizeof(RsRow) + 2 * sizeof(int)), 0);
   rc = stream_alloc(ctx, "resample_stream_create", *rs, [&](Arena& a) {
-    rs->win = a.take<float>((size_t)max_streams * rs->cap);
-    rs->d_tbl = a.take<char>(rs->tbl.size());
+    rs->carve_window(a);
+    rs->carve_tables(a);
   });
   if (rc) return rc;
   *out_pitch = rs->out_pitch;
@@ -355,8 +349,7 @@ int vtts_resample_stream_push(vtts_ctx* ctx, vtts_resample_stream* rs, const flo
 
   // ---- host bookkeeping: an output is emitted once every input it reads has arrived, i.e. after P inputs (before END)
   // the slot has emitted min(ceil(P * up / down), max(0, floor((P * up - 1 - half) / down) + 1)) outputs ----
-  RsRow* rows = reinterpret_cast<RsRow*>(rs->tbl.data());
-  int* prep = reinterpret_cast<int*>(rs->tbl.data() + (size_t)S * sizeof(RsRow));
+  RsRow* rows = rs->rows<0>();
   std::vector<long long> E1(S);
   long long max_out = 0;
   for (int s = 0; s < S; ++s) {
@@ -372,16 +365,11 @@ int vtts_resample_stream_push(vtts_ctx* ctx, vtts_resample_stream* rs, const flo
     rows[s] = RsRow{P0 - rs->K, std::max(0LL, P0 - rs->K), P1, E0, e - E0, e - E0};
     max_out = std::max(max_out, e - E0);
   }
-  sl.prep(n_new, flags, prep);
 
   // ---- device: one table copy, prep, resample ----
-  // pageable source: the call returns once the table is staged, so rs->tbl may be rewritten by the next push
-  VTTS_CUDA(cudaMemcpyAsync(rs->d_tbl, rs->tbl.data(), rs->tbl.size(), cudaMemcpyHostToDevice, st));
-  const RsRow* d_rows = reinterpret_cast<const RsRow*>(rs->d_tbl);
-  const int* d_prep = reinterpret_cast<const int*>(rs->d_tbl + (size_t)S * sizeof(RsRow));
-  rc = vtts_stream_window_prep(ctx, rs->win, rs->cap, rs->K, d_prep, x_dev, rs->F, S, st);
+  rc = rs->upload(n_new, flags, x_dev, st);
   if (rc) return rc;
-  rc = rs_launch(ctx, r, rs->taps, rs->win, rs->cap, rs->cap, nullptr, d_rows, S, 0, max_out, y_dev, rs->out_pitch, st);
+  rc = rs_launch(ctx, r, rs->taps, rs->win, rs->cap, rs->cap, nullptr, rs->d_rows<0>(), S, 0, max_out, y_dev, rs->out_pitch, st);
   if (rc) return rc;
   rs->slots.commit(n_new, flags, E1.data());
   return VTTS_OK;

@@ -1,7 +1,8 @@
-// Host-side pieces shared by the per-slot streams (resample, denoise, pitch, loudness, vocoder) and the *_host entry
-// points: the slot protocol of a push, the device memory of a stream, and the staging of host buffers.
+// Host-side pieces shared by the per-slot streams and the *_host entry points: the slot protocol of a push, the device
+// memory of a stream, the window and push tables of a sample stream, and the staging of host buffers.
 #pragma once
 #include <memory>
+#include <tuple>
 
 #include "vtts_internal.cuh"
 
@@ -68,6 +69,51 @@ struct StreamBase {
   SlotState slots;
   StreamBase(vtts_ctx* c, int s, int f) : ctx(c), S(s), F(f), slots(s) {}
   ~StreamBase() { cudaFree(mem); }
+};
+
+// ---- sample streams ----------------------------------------------------------------------------------------------
+// What a stream of samples adds: its window, per slot the K samples carried from earlier pushes and then the push's new
+// ones ([S][cap]), and its per-push tables, one host image and its device copy laid out as Rows [S] for each row type in
+// turn, then the int [S][2] window step table of vtts_stream_window_prep.  A push fills rows<I>() and then upload()s.
+template <class... Rows>
+struct SampleStream : StreamBase {
+  template <int I>
+  using Row = std::tuple_element_t<I, std::tuple<Rows...>>;
+
+  const int K, cap;
+  float* win = nullptr;
+
+  SampleStream(vtts_ctx* c, int s, int f, int k)
+      : StreamBase(c, s, f), K(k), cap(k + f), tbl((size_t)s * (offset(sizeof...(Rows)) + 2 * sizeof(int)), 0) {}
+
+  // stream_alloc: the window comes first and the device tables last, around the stream's own buffers
+  void carve_window(Arena& a) { win = a.take<float>((size_t)S * cap); }
+  void carve_tables(Arena& a) { d_tbl = a.take<char>(tbl.size()); }
+
+  template <int I>
+  Row<I>* rows() { return reinterpret_cast<Row<I>*>(tbl.data() + (size_t)S * offset(I)); }
+  template <int I>
+  const Row<I>* d_rows() const { return reinterpret_cast<const Row<I>*>(d_tbl + (size_t)S * offset(I)); }
+
+  // after the rows are filled, on the caller's stream: the window step table, the push's one table copy (from pageable
+  // memory: the call returns once it is staged, so the next push may rewrite the image) and the window step of x
+  int upload(const int32_t* n_new, const uint8_t* flags, const float* x, cudaStream_t st) {
+    const size_t steps = (size_t)S * offset(sizeof...(Rows));
+    slots.prep(n_new, flags, reinterpret_cast<int*>(tbl.data() + steps));
+    VTTS_CUDA(cudaMemcpyAsync(d_tbl, tbl.data(), tbl.size(), cudaMemcpyHostToDevice, st));
+    return vtts_stream_window_prep(ctx, win, cap, K, reinterpret_cast<const int*>(d_tbl + steps), x, F, S, st);
+  }
+
+ private:
+  // bytes per slot of the row types before the n-th
+  static constexpr size_t offset(int n) {
+    constexpr size_t sz[] = {sizeof(Rows)...};
+    size_t b = 0;
+    for (int i = 0; i < n; ++i) b += sz[i];
+    return b;
+  }
+  std::vector<char> tbl;
+  char* d_tbl = nullptr;
 };
 
 // `carve(Arena&)` hands out the stream's buffers; it runs once to measure and once more on the zero-filled allocation
@@ -178,6 +224,14 @@ class HostStage {
   std::vector<In> ins;
   std::vector<Out> outs;
 };
+
+// the row lengths n[b] of a *_host entry point `who` (null: every row full), each in [0, S]
+inline int host_lengths_check(vtts_ctx* ctx, const char* who, const int32_t* n, int B, int S) {
+  if (n)
+    for (int b = 0; b < B; ++b)
+      if (n[b] < 0 || n[b] > S) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: n[%d]=%d outside [0, %d]", who, b, n[b], S);
+  return VTTS_OK;
+}
 
 // push_host of a stream: the x_bytes of host input x are staged, push(x_dev, y_dev, stream) runs the stream's device
 // push on the staged buffers, and the y_bytes of its output come back to host memory y

@@ -63,32 +63,37 @@ def _strength(s) -> float:
     return s
 
 
+def _per_row(v, n: int, name: str, lo: float, hi: float, shown=None) -> np.ndarray:
+    """float32 [n]: a scalar for every row, or one value per row, each finite and in [lo, hi] (errors show `shown`, by
+    default v)"""
+    a = np.asarray(v, np.float32)
+    a = np.full(n, a, np.float32) if a.ndim == 0 else np.ascontiguousarray(a.reshape(-1), np.float32)
+    if a.shape != (n,):
+        raise ValueError(f"{name}: one value or one per row ({n}), got {np.shape(v)}")
+    if not (np.all(np.isfinite(a)) and np.all((a >= lo) & (a <= hi))):
+        raise ValueError(f"{name} must be finite and lie in [{lo:g}, {hi:g}], got {v if shown is None else shown}")
+    return a
+
+
+class _BeginParam(NamedTuple):
+    """A per-row effect parameter that a stream slot takes with BEGIN and keeps until END."""
+    name: str                       # keyword of the calls and of `TtsStream.begin`
+    neutral: float                  # a slot's value before its first BEGIN
+    lo: float
+    hi: float
+    default: float | None = None    # a push's value when the keyword is left out (None: required with BEGIN)
+    host_check: bool = False        # a push checks the range here (else the library rejects a bad BEGIN value)
+
+    def rows(self, v, n: int) -> np.ndarray:
+        return _per_row(v, n, self.name, self.lo, self.hi)
+
+
 MAX_SEMITONES = 12.0
-
-
-def _semitones(v, n: int) -> np.ndarray:
-    """float32 [n]: a scalar shift for every row, or one per row, each finite and in [-12, 12]"""
-    a = np.asarray(v, np.float32)
-    a = np.full(n, a, np.float32) if a.ndim == 0 else np.ascontiguousarray(a.reshape(-1), np.float32)
-    if a.shape != (n,):
-        raise ValueError(f"semitones: one value or one per row ({n}), got {np.shape(v)}")
-    if not (np.all(np.isfinite(a)) and np.all(np.abs(a) <= MAX_SEMITONES)):
-        raise ValueError(f"semitones must be finite and lie in [-12, 12], got {v}")
-    return a
-
-
 MIN_TEMPO, MAX_TEMPO = 0.5, 2.0
-
-
-def _tempo(v, n: int) -> np.ndarray:
-    """float32 [n]: a scalar tempo for every row, or one per row, each finite and in [0.5, 2]"""
-    a = np.asarray(v, np.float32)
-    a = np.full(n, a, np.float32) if a.ndim == 0 else np.ascontiguousarray(a.reshape(-1), np.float32)
-    if a.shape != (n,):
-        raise ValueError(f"tempo: one value or one per row ({n}), got {np.shape(v)}")
-    if not (np.all(np.isfinite(a)) and np.all((a >= MIN_TEMPO) & (a <= MAX_TEMPO))):
-        raise ValueError(f"tempo must be finite and lie in [0.5, 2], got {v}")
-    return a
+LIMIT_MAX_GAIN_DB = 70.0
+SEMITONES = _BeginParam("semitones", 0.0, -MAX_SEMITONES, MAX_SEMITONES)
+TEMPO = _BeginParam("tempo", 1.0, MIN_TEMPO, MAX_TEMPO)
+GAIN_DB = _BeginParam("gain_db", 0.0, -LIMIT_MAX_GAIN_DB, LIMIT_MAX_GAIN_DB, default=0.0, host_check=True)
 
 
 EQ_MAX_SECTIONS = 8
@@ -180,14 +185,15 @@ def _np(a, dtype, shape=None, what="array"):
     return a
 
 
-def _wav_rows(wav):
-    """(x f32 [B,S], one): a host [S] or [B,S] array as rows, and whether it was a single row"""
+def _wav_rows(wav, lengths=None):
+    """(x f32 [B,S], lengths int32 [B] or None, one) of a one-shot host call: a host [S] or [B,S] array as rows, its
+    row lengths, and whether it was a single row"""
     x = _np(wav, np.float32)
     one = x.ndim == 1
     x = x[None] if one else x
     if x.ndim != 2:
         raise ValueError(f"wav must be [S] or [B,S], got {np.shape(wav)}")
-    return x, one
+    return x, None if lengths is None else _np(lengths, np.int32, (x.shape[0],), "lengths"), one
 
 
 def _out_tensor(out, shape, device, what="out"):
@@ -198,6 +204,16 @@ def _out_tensor(out, shape, device, what="out"):
     if tuple(out.shape) != shape or out.dtype != torch.float32 or not out.is_contiguous() or out.device != torch.device(device):
         raise ValueError(f"{what} must be contiguous float32 [{', '.join(map(str, shape))}] on {device}")
     return out
+
+
+def _dev_rows(x_t, out, stream, width=None):
+    """(B, S, out, CUDA stream) of a one-shot device call on x_t, a contiguous float32 CUDA tensor [B,S]: `out` checked
+    or made as [B, width] (default S), and the caller's stream or else the current one"""
+    import torch
+    assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
+    B, S = x_t.shape
+    out = _out_tensor(out, (B, S if width is None else width), x_t.device)
+    return B, S, out, torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
 
 
 class Engine:
@@ -823,11 +839,10 @@ class Engine:
         down is out_rate / in_rate in lowest terms (each <= 1024).  lengths int [B]: row b holds lengths[b] samples,
         and its outputs past ceil(lengths[b] * up / down) are 0.  Equals scipy.signal.resample_poly(x, up, down) up to
         fp32 rounding; in_rate == out_rate is a copy."""
-        x, one = _wav_rows(wav)
+        x, lens, one = _wav_rows(wav, lengths)
         if x.shape[1] < 1:
             raise ValueError(f"wav must be [S] or [B,S], got {np.shape(wav)}")
         B, S = x.shape
-        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
         y = np.empty((B, resample_length(S, in_rate, out_rate)), np.float32)
         self._ck(self.lib.vtts_resample_host(self.h, _ptr(x), _ptr(lens), B, S, int(in_rate), int(out_rate), _ptr(y)))
         return y[0] if one else y
@@ -835,12 +850,7 @@ class Engine:
     def resample_forward(self, x_t, out_rate: int, in_rate: int = config.SAMPLE_RATE, lengths_t=None, out=None, stream=None):
         """vtts_resample on torch CUDA tensors, stream-ordered: x_t f32 [B,S] -> [B, ceil(S * up / down)]; lengths_t
         int32 CUDA [B] or None."""
-        import torch
-        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
-        B, S = x_t.shape
-        n = resample_length(S, in_rate, out_rate)
-        out = _out_tensor(out, (B, n), x_t.device)
-        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        B, S, out, st = _dev_rows(x_t, out, stream, resample_length(x_t.shape[-1], in_rate, out_rate))
         self._ck(self.lib.vtts_resample(self.h, _ptr(x_t), _ptr(lengths_t), B, S, int(in_rate), int(out_rate), _ptr(out), st))
         return out
 
@@ -887,9 +897,8 @@ class Engine:
         lengths int [B] in [0, S]: row b holds lengths[b] samples and its outputs past them are 0.  bias f32 [513]
         (default: `denoiser_bias()`)."""
         strength = _strength(strength)
-        x, one = _wav_rows(wav)
+        x, lens, one = _wav_rows(wav, lengths)
         B, S = x.shape
-        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
         if S == 0 or B == 0:
             return (x[0] if one else x).copy()          # nothing to transform: empty rows are short rows
         b = self._bias_arg(bias)
@@ -902,14 +911,11 @@ class Engine:
         bias_t f32 CUDA [513] or None (`denoiser_bias()`)."""
         import torch
         strength = _strength(strength)
-        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
-        B, S = x_t.shape
+        B, S, out, st = _dev_rows(x_t, out, stream)
         if bias_t is None:
             bias_t = torch.from_numpy(self._bias_arg(None)).to(x_t.device)
         elif tuple(bias_t.shape) != (DENOISE_BINS,) or bias_t.dtype != torch.float32 or not bias_t.is_contiguous():
             raise ValueError(f"bias_t must be contiguous float32 [{DENOISE_BINS}]")
-        out = _out_tensor(out, (B, S), x_t.device)
-        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
         self._ck(self.lib.vtts_denoise(self.h, _ptr(x_t), _ptr(lengths_t), B, S, strength, _ptr(bias_t), _ptr(out), st))
         return out
 
@@ -925,10 +931,9 @@ class Engine:
         fp32(2^(s / 12)) with its phase kept coherent across frames (n_fft 1024, hop 256); the timing of every sample is
         kept.  semitones: a scalar or one value per row, finite and in [-12, 12]; rows with 0 and rows of <= 512 samples
         are copied.  lengths int [B] in [0, S]: row b holds lengths[b] samples and its outputs past them are 0."""
-        x, one = _wav_rows(wav)
+        x, lens, one = _wav_rows(wav, lengths)
         B, S = x.shape
-        sem = _semitones(semitones, B)
-        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
+        sem = SEMITONES.rows(semitones, B)
         if S == 0 or B == 0:
             return (x[0] if one else x).copy()          # nothing to transform: empty rows are short rows
         y = np.empty((B, S), np.float32)
@@ -938,12 +943,8 @@ class Engine:
     def pitch_shift_forward(self, x_t, semitones, lengths_t=None, out=None, stream=None):
         """vtts_pitch_shift on torch CUDA tensors, stream-ordered: x_t f32 [B,S] -> [B,S] (not x_t); semitones a scalar or
         one host value per row; lengths_t int32 CUDA [B] or None."""
-        import torch
-        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
-        B, S = x_t.shape
-        sem = _semitones(semitones, B)
-        out = _out_tensor(out, (B, S), x_t.device)
-        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        B, S, out, st = _dev_rows(x_t, out, stream)
+        sem = SEMITONES.rows(semitones, B)
         self._ck(self.lib.vtts_pitch_shift(self.h, _ptr(x_t), _ptr(lengths_t), B, S, _ptr(sem), _ptr(out), st))
         return out
 
@@ -953,7 +954,7 @@ class Engine:
         same arguments."""
         import torch
         B, S = x_t.shape
-        sem = _semitones(semitones, B)
+        sem = SEMITONES.rows(semitones, B)
         out = torch.empty((B, S // config.HOP + 1, DENOISE_BINS), dtype=torch.int32, device=x_t.device)
         st = torch.cuda.current_stream(x_t.device).cuda_stream
         self._ck(self.lib.vtts_debug_pitch_decisions(self.h, _ptr(x_t), _ptr(lengths_t), B, S, _ptr(sem), _ptr(out), st))
@@ -968,7 +969,7 @@ class Engine:
     # ---- time stretch (vtts_time_stretch*: the pitch shifter's phase vocoder with analysis frames at 256 t alpha) ----
     def time_stretch_length(self, n: int, tempo: float) -> int:
         """M = floor(n / alpha + 0.5) (in double, alpha the fp32 tempo): the samples `time_stretch` makes of n"""
-        m = int(self.lib.vtts_time_stretch_length(int(n), float(_tempo(tempo, 1)[0])))
+        m = int(self.lib.vtts_time_stretch_length(int(n), float(TEMPO.rows(tempo, 1)[0])))
         if m < 0:
             raise ValueError(f"time_stretch_length: n={n} must be >= 0")
         return m
@@ -978,10 +979,9 @@ class Engine:
         (a peak-locked phase vocoder, n_fft 1024, synthesis hop 256); M_b = floor(n_b / tempo_b + 0.5) and row b is zero
         past M_b.  tempo: a scalar or one value per row, finite and in [0.5, 2]; rows at 1 and rows of <= 512 samples
         give their first min(n, M) samples.  lengths int [B] in [0, S]: row b holds lengths[b] samples."""
-        x, one = _wav_rows(wav)
+        x, lens, one = _wav_rows(wav, lengths)
         B, S = x.shape
-        tp = _tempo(tempo, B)
-        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
+        tp = TEMPO.rows(tempo, B)
         n = np.full(B, S) if lens is None else lens
         Sy = max((self.time_stretch_length(int(n[b]), tp[b]) for b in range(B)), default=0)
         if S == 0 or B == 0 or Sy == 0:
@@ -1000,7 +1000,7 @@ class Engine:
         import torch
         assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
         B, S = x_t.shape
-        tp = _tempo(tempo, B)
+        tp = TEMPO.rows(tempo, B)
         if out is None:
             out = _out_tensor(None, (B, max(self.time_stretch_length(S, a) for a in tp)), x_t.device)
         elif out.dim() != 2 or out.shape[0] != B or out.shape[1] < 1 or out.dtype != torch.float32 or not out.is_contiguous():
@@ -1015,7 +1015,7 @@ class Engine:
         `debug_pitch_decisions` encodes them, for `time_stretch_forward` of the same arguments."""
         import torch
         B, S = x_t.shape
-        tp = _tempo(tempo, B)
+        tp = TEMPO.rows(tempo, B)
         T = max(self.time_stretch_length(S, a) for a in tp) // config.HOP + 1
         out = torch.empty((B, T, DENOISE_BINS), dtype=torch.int32, device=x_t.device)
         st = torch.cuda.current_stream(x_t.device).cuda_stream
@@ -1034,9 +1034,8 @@ class Engine:
         arrays (scalars for a 1-D input): integrated, momentary and short-term loudness in LUFS (-inf where undefined) and
         the true peak in dBTP (4x oversampled by resample_poly).  lengths int [B] in [0, S]."""
         rate = _loudness_rate(rate)
-        x, one = _wav_rows(wav)
+        x, lens, one = _wav_rows(wav, lengths)
         B, S = x.shape
-        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
         out = np.full((B, 4), -np.inf, np.float32)
         if B and S:                                # empty rows measure as silence
             self._ck(self.lib.vtts_loudness_host(self.h, _ptr(x), _ptr(lens), B, S, rate, _ptr(out)))
@@ -1057,9 +1056,8 @@ class Engine:
             if true_peak is None:
                 raise ValueError("normalize_loudness(limit=True) needs a true_peak ceiling")
             _limit_args(ceiling, rate, lookahead_ms, release_ms)
-        x, one = _wav_rows(wav)
+        x, lens, one = _wav_rows(wav, lengths)
         B, S = x.shape
-        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
         y = x.copy()
         g = np.zeros(B, np.float32)
         if B and S and limit:
@@ -1072,12 +1070,8 @@ class Engine:
     def loudness_forward(self, x_t, rate: int = config.SAMPLE_RATE, lengths_t=None, out=None, stream=None):
         """vtts_loudness on torch CUDA tensors, stream-ordered: x_t f32 [B,S] -> f32 [B,4] (integrated, momentary,
         short-term LUFS, true peak dBTP); lengths_t int32 CUDA [B] or None."""
-        import torch
         rate = _loudness_rate(rate)
-        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
-        B, S = x_t.shape
-        out = _out_tensor(out, (B, 4), x_t.device)
-        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        B, S, out, st = _dev_rows(x_t, out, stream, 4)
         self._ck(self.lib.vtts_loudness(self.h, _ptr(x_t), _ptr(lengths_t), B, S, rate, _ptr(out), st))
         return out
 
@@ -1086,18 +1080,14 @@ class Engine:
         """vtts_loudness_normalize (limit=True: vtts_loudness_normalize_limited, see normalize_loudness) on torch CUDA
         tensors, stream-ordered and without a host synchronisation: returns (y [B,S], gain_db [B]).  `out` may be x_t
         (in place)."""
-        import torch
         rate = _loudness_rate(rate)
         target, ceiling = _loudness_target(target, true_peak)
         if limit:
             if true_peak is None:
                 raise ValueError("normalize_loudness_forward(limit=True) needs a true_peak ceiling")
             _limit_args(ceiling, rate, lookahead_ms, release_ms)
-        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
-        B, S = x_t.shape
-        out = _out_tensor(out, (B, S), x_t.device)
+        B, S, out, st = _dev_rows(x_t, out, stream)
         gain_db = _out_tensor(gain_db, (B,), x_t.device, "gain_db")
-        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
         if limit:
             self._ck(self.lib.vtts_loudness_normalize_limited(self.h, _ptr(x_t), _ptr(lengths_t), B, S, rate, target, ceiling,
                                                               float(lookahead_ms), float(release_ms), _ptr(out), _ptr(gain_db), st))
@@ -1122,10 +1112,9 @@ class Engine:
         recovers with `release_ms` (in [1, 2000]).  reduction_db: the deepest gain reduction per row (<= 0).  Rows whose
         peaks stay under the ceiling come back exactly as wav times the pre-gain.  lengths int [B] in [0, S]."""
         ceiling, rate, lookahead_ms, release_ms = _limit_args(ceiling, rate, lookahead_ms, release_ms)
-        x, one = _wav_rows(wav)
+        x, lens, one = _wav_rows(wav, lengths)
         B, S = x.shape
-        g = _gain_db(gain_db, B)
-        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
+        g = GAIN_DB.rows(gain_db, B)
         y = np.zeros((B, S), np.float32)
         red = np.zeros(B, np.float32)
         if B and S:
@@ -1140,17 +1129,14 @@ class Engine:
         the device.  `out` may be x_t (in place)."""
         import torch
         ceiling, rate, lookahead_ms, release_ms = _limit_args(ceiling, rate, lookahead_ms, release_ms)
-        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
-        B, S = x_t.shape
+        B, S, out, st = _dev_rows(x_t, out, stream)
         if isinstance(gain_db, torch.Tensor):
             if tuple(gain_db.shape) != (B,) or gain_db.dtype != torch.float32 or not gain_db.is_cuda or not gain_db.is_contiguous():
                 raise ValueError(f"gain_db must be a contiguous float32 CUDA tensor [{B}] or host values")
             g_t = gain_db
         else:
-            g_t = torch.from_numpy(_gain_db(gain_db, B)).to(x_t.device, non_blocking=False)
-        out = _out_tensor(out, (B, S), x_t.device)
+            g_t = torch.from_numpy(GAIN_DB.rows(gain_db, B)).to(x_t.device, non_blocking=False)
         reduction_db = _out_tensor(reduction_db, (B,), x_t.device, "reduction_db")
-        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
         self._ck(self.lib.vtts_limit(self.h, _ptr(x_t), _ptr(lengths_t), _ptr(g_t), B, S, rate, ceiling, lookahead_ms, release_ms,
                                      _ptr(out), _ptr(reduction_db), st))
         return out, reduction_db
@@ -1173,9 +1159,8 @@ class Engine:
         `eq_sections`), equal to scipy.signal.sosfilt of each row from zero state up to fp32 rounding; not clipped.
         lengths int [B] in [0, S]: outputs past lengths[b] are 0."""
         sos = eq_sections(eq, rate)
-        x, one = _wav_rows(wav)
+        x, lens, one = _wav_rows(wav, lengths)
         B, S = x.shape
-        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
         y = np.zeros((B, S), np.float32)
         if B and S:
             self._ck(self.lib.vtts_eq_host(self.h, _ptr(x), _ptr(lens), B, S, _ptr(sos), sos.shape[0], _ptr(y)))
@@ -1184,12 +1169,8 @@ class Engine:
     def equalize_forward(self, x_t, eq, rate: int = config.SAMPLE_RATE, lengths_t=None, out=None, stream=None):
         """vtts_eq on torch CUDA tensors, stream-ordered and without a host synchronisation: x_t f32 [B,S] -> [B,S];
         lengths_t int32 CUDA [B] or None.  `out` may be x_t (in place)."""
-        import torch
         sos = eq_sections(eq, rate)
-        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
-        B, S = x_t.shape
-        out = _out_tensor(out, (B, S), x_t.device)
-        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        B, S, out, st = _dev_rows(x_t, out, stream)
         self._ck(self.lib.vtts_eq(self.h, _ptr(x_t), _ptr(lengths_t), B, S, _ptr(sos), sos.shape[0], _ptr(out), st))
         return out
 
@@ -1226,9 +1207,6 @@ def _loudness_target(target, true_peak):
     return t, c
 
 
-LIMIT_MAX_GAIN_DB = 70.0
-
-
 def _limit_args(ceiling, rate, lookahead_ms, release_ms):
     """(ceiling, rate, lookahead_ms, release_ms) as vtts_limit takes them, each checked"""
     c = float(ceiling)
@@ -1245,13 +1223,7 @@ def _limit_args(ceiling, rate, lookahead_ms, release_ms):
 
 def _gain_db(v, n: int) -> np.ndarray:
     """float32 [n]: a scalar pre-gain for every row, or one per row, each finite and in [-70, 70] dB"""
-    a = np.asarray(v, np.float32)
-    a = np.full(n, a, np.float32) if a.ndim == 0 else np.ascontiguousarray(a.reshape(-1), np.float32)
-    if a.shape != (n,):
-        raise ValueError(f"gain_db: one value or one per row ({n}), got {np.shape(v)}")
-    if not (np.all(np.isfinite(a)) and np.all(np.abs(a) <= LIMIT_MAX_GAIN_DB)):
-        raise ValueError(f"gain_db must be finite and lie in [-70, 70], got {v}")
-    return a
+    return GAIN_DB.rows(v, n)
 
 
 STREAM_BEGIN, STREAM_END = 1, 2
@@ -1259,16 +1231,27 @@ STREAM_BEGIN, STREAM_END = 1, 2
 
 class _SlotStream:
     """What every per-slot stream handle shares: the library handle `h` of one stream of `eng`'s context, the marshalling
-    of a push (zero padding of short chunks, the BEGIN / END flag bits, the n_new / flags arrays, the device-buffer checks
-    and the CUDA stream) and the lifecycle.  A subclass opens its stream, names its input and pushes."""
-    _kind = ""       # the library's vtts_<kind>_destroy closes the stream
+    of a push (zero padding of short chunks, the BEGIN / END flag bits, the n_new / flags arrays, the device-buffer checks,
+    the CUDA stream, the per-slot BEGIN parameter), the push itself and the lifecycle.  A subclass opens its stream and
+    declares its kind, its input, its output width and at most one BEGIN parameter."""
+    _kind = ""       # the library's vtts_<kind>_push[_host] pushes and vtts_<kind>_destroy closes the stream
     _x = "x"         # the input's name in error messages
     _row = ()        # shape of one input element past [S, F]: () for samples, (80,) for mel frames
+    _scale = 1       # output samples per unit of n_out
+    _param = None    # the _BeginParam a push takes for the slots it begins, or None
+    _carried = ""    # with a _param: the attribute holding each slot's value since its BEGIN
     h = None
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk: int):
         self.eng = eng
         self.max_streams, self._chunk = int(max_streams), int(max_chunk)
+        if self._param is not None:
+            setattr(self, self._carried, np.full(self.max_streams, self._param.neutral, np.float32))
+
+    @property
+    def _width(self):
+        """outputs per slot of a push's output buffer"""
+        return self.out_pitch
 
     def _create(self, fn, *args, pitch=False):
         """calls vtts_<kind>_create(ctx, *args, &h[, &pitch]); sets `h` and, with pitch, `out_pitch`"""
@@ -1297,14 +1280,76 @@ class _SlotStream:
         S = self.max_streams
         return _np(n_new, np.int32, (S,), "n_new"), _np(flags, np.uint8, (S,), "flags")
 
-    def _device_in(self, x_t, out_t, out_shape, n_new, flags, stream):
+    def _device_in(self, x_t, out_t, n_new, flags, stream):
         """(n_new int32 [S], flags uint8 [S], CUDA stream) of a device push, after checking both buffers"""
         import torch
-        for t, name, shape in ((x_t, self._x + "_t", (self.max_streams, self._chunk) + self._row), (out_t, "out_t", out_shape)):
+        for t, name, shape in ((x_t, self._x + "_t", (self.max_streams, self._chunk) + self._row),
+                               (out_t, "out_t", (self.max_streams, self._width))):
             if tuple(t.shape) != shape or t.dtype != torch.float32 or not t.is_contiguous():
                 raise ValueError(f"{name} must be contiguous float32 [{', '.join(map(str, shape))}]")
         st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
         return self._args(n_new, flags) + (st,)
+
+    def _values(self, flags, v) -> tuple:
+        """() without a BEGIN parameter, else (float32 [S],): the push's value `v` (a scalar or [S]) for the slots it
+        begins and each slot's carried value elsewhere, which the library checks is unchanged"""
+        p = self._param
+        if p is None:
+            return ()
+        out = getattr(self, self._carried).copy()
+        begin = (flags & STREAM_BEGIN) != 0
+        v = p.default if v is None else v
+        if begin.any():
+            if v is None:
+                raise ValueError(f"{p.name}= is required for the slots a push begins")
+            g = np.asarray(v, np.float32)
+            g = np.full(out.size, g, np.float32) if g.ndim == 0 else g
+            if g.shape != (out.size,):
+                raise ValueError(f"{p.name}: one value or one per slot ({out.size}), got {np.shape(v)}")
+            out[begin] = g[begin]
+        if p.host_check:
+            _per_row(out, out.size, p.name, p.lo, p.hi, shown=v)
+        return (out,)
+
+    def _outs(self):
+        """the push call's outputs after y: n_out int32 [S] (a subclass adds its own)"""
+        return (np.zeros(self.max_streams, np.int32),)
+
+    def _result(self, y, outs, host: bool):
+        """what a push returns: each slot's new outputs (host) or n_out (device)"""
+        return self._rows(y, outs[0], self._scale) if host else outs[0]
+
+    def _push(self, host: bool, x, n, f, values, y, outs, st=None):
+        fn = getattr(self.eng.lib, f"vtts_{self._kind}_push" + ("_host" if host else ""))
+        self.eng._ck(fn(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), *map(_ptr, values), _ptr(y), *map(_ptr, outs),
+                        *(() if host else (st,))))
+        if values:
+            begin = (f & STREAM_BEGIN) != 0
+            getattr(self, self._carried)[begin] = values[0][begin]
+        return self._result(y, outs, host)
+
+    def _push_host(self, x, n_new, begin, end, value=None):
+        x, n, f = self._host_in(x, n_new, begin, end)
+        values = self._values(f, value)
+        y = np.empty((self.max_streams, self._width), np.float32)
+        return self._push(True, x, n, f, values, y, self._outs())
+
+    def _push_device(self, x_t, n_new, flags, out_t, stream, value=None, dev=()):
+        """`dev`: the stream's own device outputs after n_out"""
+        n, f, st = self._device_in(x_t, out_t, n_new, flags, stream)
+        values = self._values(f, value)
+        return self._push(False, x_t, n, f, values, out_t, self._outs(*dev), st)
+
+    def push(self, x, n_new, begin=None, end=None) -> list:
+        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None.
+        Returns one float32 array per slot with the samples it emits now."""
+        return self._push_host(x, n_new, begin, end)
+
+    def push_device(self, x_t, n_new, flags, out_t, stream=None) -> np.ndarray:
+        """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S, out_pitch]; n_new int [S] and flags
+        uint8 [S] (bit0 BEGIN, bit1 END) on the host.  Stream-ordered; returns n_out int32 [S] (outputs slot s got at the
+        start of its row of out_t)."""
+        return self._push_device(x_t, n_new, flags, out_t, stream)
 
     def _rows(self, y, n_out, scale=1):
         return [y[s, : int(n_out[s]) * scale].copy() for s in range(self.max_streams)]
@@ -1328,9 +1373,10 @@ class _SlotStream:
 
 
 class VocoderStream(_SlotStream):
-    """Handle of a streaming generator (Engine.open_vocoder_stream).  A slot that has received P frames since BEGIN
-    has emitted max(0, P - lookahead) frames; a push with END emits the rest."""
-    _kind, _x, _row = "vocoder_stream", "mel", (config.MEL_DIM,)
+    """Handle of a streaming generator (Engine.open_vocoder_stream): push mel f32 [S, F', 80], get 256 samples per
+    frame.  A slot that has received P frames since BEGIN has emitted max(0, P - lookahead) frames; a push with END
+    emits the rest.  `push_device` takes out_t [S, wav_ld] and returns n_out in frames."""
+    _kind, _x, _row, _scale = "vocoder_stream", "mel", (config.MEL_DIM,), config.HOP
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int):
         super().__init__(eng, max_streams, max_chunk_frames)
@@ -1339,23 +1385,20 @@ class VocoderStream(_SlotStream):
         self.wav_ld = config.HOP * (self.max_chunk_frames + self.lookahead)   # samples per slot of the output buffer
         self._create(eng.lib.vtts_vocoder_stream_create, self.max_streams, self.max_chunk_frames)
 
+    @property
+    def _width(self):
+        return self.wav_ld
+
     def push(self, mel, n_new, begin=None, end=None) -> list:
         """mel f32 [S,F',80] (F' <= max_chunk_frames; rows past n_new[s] ignored), n_new int [S], begin / end bool [S]
         or None.  Returns one float32 array per slot with the samples it emits now (256 per frame)."""
-        mel, n, f = self._host_in(mel, n_new, begin, end)
-        wav = np.empty((self.max_streams, self.wav_ld), np.float32)
-        n_out = np.zeros(self.max_streams, np.int32)
-        self.eng._ck(self.eng.lib.vtts_vocoder_stream_push_host(self.eng.h, self.h, _ptr(mel), _ptr(n), _ptr(f), _ptr(wav), _ptr(n_out)))
-        return self._rows(wav, n_out, config.HOP)
+        return self._push_host(mel, n_new, begin, end)
 
     def push_device(self, mel_t, n_new, flags, out_t, stream=None) -> np.ndarray:
         """Device buffers: mel_t f32 CUDA [S,F,80], out_t f32 CUDA [S, 256*(F+lookahead)]; n_new int [S] and flags
         uint8 [S] (bit0 BEGIN, bit1 END) on the host.  Stream-ordered; returns n_out int32 [S] (frames slot s got at
         the start of its row of out_t)."""
-        n, f, st = self._device_in(mel_t, out_t, (self.max_streams, self.wav_ld), n_new, flags, stream)
-        n_out = np.zeros(self.max_streams, np.int32)
-        self.eng._ck(self.eng.lib.vtts_vocoder_stream_push(self.eng.h, self.h, _ptr(mel_t), _ptr(n), _ptr(f), _ptr(out_t), _ptr(n_out), st))
-        return n_out
+        return self._push_device(mel_t, n_new, flags, out_t, stream)
 
 
 class ResampleStream(_SlotStream):
@@ -1372,24 +1415,6 @@ class ResampleStream(_SlotStream):
         self._create(eng.lib.vtts_resample_stream_create, self.max_streams, self.max_chunk_samples, self.in_rate, self.out_rate, pitch=True)
         self.lookahead = int(eng.lib.vtts_resample_stream_lookahead(self.in_rate, self.out_rate))
 
-    def push(self, x, n_new, begin=None, end=None) -> list:
-        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None.
-        Returns one float32 array per slot with the samples it emits now."""
-        x, n, f = self._host_in(x, n_new, begin, end)
-        y = np.empty((self.max_streams, self.out_pitch), np.float32)
-        n_out = np.zeros(self.max_streams, np.int32)
-        self.eng._ck(self.eng.lib.vtts_resample_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(y), _ptr(n_out)))
-        return self._rows(y, n_out)
-
-    def push_device(self, x_t, n_new, flags, out_t, stream=None) -> np.ndarray:
-        """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S, out_pitch]; n_new int [S] and flags
-        uint8 [S] (bit0 BEGIN, bit1 END) on the host.  Stream-ordered; returns n_out int32 [S] (outputs slot s got at the
-        start of its row of out_t)."""
-        n, f, st = self._device_in(x_t, out_t, (self.max_streams, self.out_pitch), n_new, flags, stream)
-        n_out = np.zeros(self.max_streams, np.int32)
-        self.eng._ck(self.eng.lib.vtts_resample_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(out_t), _ptr(n_out), st))
-        return n_out
-
 
 class DenoiseStream(_SlotStream):
     """Handle of a streaming denoiser (Engine.open_denoise_stream).  Before END a slot that has received P samples has
@@ -1405,133 +1430,55 @@ class DenoiseStream(_SlotStream):
                      pitch=True)
         self.lookahead = int(eng.lib.vtts_denoise_stream_lookahead())
 
-    def push(self, x, n_new, begin=None, end=None) -> list:
-        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None.
-        Returns one float32 array per slot with the samples it emits now."""
-        x, n, f = self._host_in(x, n_new, begin, end)
-        y = np.empty((self.max_streams, self.out_pitch), np.float32)
-        n_out = np.zeros(self.max_streams, np.int32)
-        self.eng._ck(self.eng.lib.vtts_denoise_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(y), _ptr(n_out)))
-        return self._rows(y, n_out)
-
-    def push_device(self, x_t, n_new, flags, out_t, stream=None) -> np.ndarray:
-        """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S, out_pitch]; n_new int [S] and flags
-        uint8 [S] (bit0 BEGIN, bit1 END) on the host.  Stream-ordered; returns n_out int32 [S] (outputs slot s got at the
-        start of its row of out_t)."""
-        n, f, st = self._device_in(x_t, out_t, (self.max_streams, self.out_pitch), n_new, flags, stream)
-        n_out = np.zeros(self.max_streams, np.int32)
-        self.eng._ck(self.eng.lib.vtts_denoise_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(out_t), _ptr(n_out), st))
-        return n_out
-
-
-def _begin_values(carry, flags, given, name) -> np.ndarray:
-    """float32 [S] of a push: `given` (a scalar or [S]) for the slots that begin, each slot's `carry` elsewhere"""
-    out = carry.copy()
-    begin = (np.asarray(flags) & STREAM_BEGIN) != 0
-    if begin.any():
-        if given is None:
-            raise ValueError(f"{name}= is required for the slots a push begins")
-        g = np.asarray(given, np.float32)
-        g = np.full(carry.size, g, np.float32) if g.ndim == 0 else g
-        if g.shape != (carry.size,):
-            raise ValueError(f"{name}: one value or one per slot ({carry.size}), got {np.shape(given)}")
-        out[begin] = g[begin]
-    return np.ascontiguousarray(out, np.float32)
-
 
 class PitchShiftStream(_SlotStream):
-    """Handle of a streaming pitch shifter (Engine.open_pitch_shift_stream).  Before END a slot that has received P samples
-    has emitted min(P, 256 max(0, floor(P / 256) - 3)) outputs; a push with END emits the rest."""
-    _kind = "pitch_shift_stream"
+    """Handle of a streaming pitch shifter (Engine.open_pitch_shift_stream): `semitones=` with BEGIN.  Before END a slot
+    that has received P samples has emitted min(P, 256 max(0, floor(P / 256) - 3)) outputs; a push with END emits the
+    rest.  `shift` holds each slot's shift since its BEGIN."""
+    _kind, _param, _carried = "pitch_shift_stream", SEMITONES, "shift"
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int):
         super().__init__(eng, max_streams, max_chunk_samples)
         self.max_chunk_samples = self._chunk
         self._create(eng.lib.vtts_pitch_shift_stream_create, self.max_streams, self.max_chunk_samples, pitch=True)
         self.lookahead = int(eng.lib.vtts_pitch_shift_stream_lookahead())
-        self.shift = np.zeros(self.max_streams, np.float32)   # each slot's shift since its BEGIN
-
-    def _shifts(self, flags, semitones) -> np.ndarray:
-        """the semitones array of a push: the given values for the slots that begin, the slots' own shifts elsewhere"""
-        return _begin_values(self.shift, flags, semitones, "semitones")
-
-    def _commit(self, flags, sem):
-        begin = (np.asarray(flags) & STREAM_BEGIN) != 0
-        self.shift[begin] = sem[begin]
 
     def push(self, x, n_new, begin=None, end=None, semitones=None) -> list:
-        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None,
-        semitones: a scalar or [S], read for the slots that begin.  Returns one float32 array per slot with the samples
-        it emits now."""
-        x, n, f = self._host_in(x, n_new, begin, end)
-        sem = self._shifts(f, semitones)
-        y = np.empty((self.max_streams, self.out_pitch), np.float32)
-        n_out = np.zeros(self.max_streams, np.int32)
-        self.eng._ck(self.eng.lib.vtts_pitch_shift_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(sem), _ptr(y),
-                                                                    _ptr(n_out)))
-        self._commit(f, sem)
-        return self._rows(y, n_out)
+        """As `_SlotStream.push`, with semitones: a scalar or [S], read for the slots that begin."""
+        return self._push_host(x, n_new, begin, end, semitones)
 
     def push_device(self, x_t, n_new, flags, out_t, semitones=None, stream=None) -> np.ndarray:
-        """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S, out_pitch]; n_new int [S], flags
-        uint8 [S] (bit0 BEGIN, bit1 END) and semitones (scalar or [S], read for the slots that begin) on the host.
-        Stream-ordered; returns n_out int32 [S] (outputs slot s got at the start of its row of out_t)."""
-        n, f, st = self._device_in(x_t, out_t, (self.max_streams, self.out_pitch), n_new, flags, stream)
-        sem = self._shifts(f, semitones)
-        n_out = np.zeros(self.max_streams, np.int32)
-        self.eng._ck(self.eng.lib.vtts_pitch_shift_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(sem), _ptr(out_t),
-                                                               _ptr(n_out), st))
-        self._commit(f, sem)
-        return n_out
+        """As `_SlotStream.push_device`, with semitones (host scalar or [S], read for the slots that begin)."""
+        return self._push_device(x_t, n_new, flags, out_t, stream, semitones)
 
 
 class TimeStretchStream(_SlotStream):
-    """Handle of a streaming time stretcher (Engine.open_time_stretch_stream).  Before END a slot at tempo alpha that has
-    scanned Q frames (frame t once rint(256 t alpha) + 512 <= P, P > 512) has released max(0, 256 Q - 511) outputs (all
-    P at tempo 1); a push with END releases the rest."""
-    _kind = "time_stretch_stream"
+    """Handle of a streaming time stretcher (Engine.open_time_stretch_stream): `tempo=` with BEGIN.  Before END a slot at
+    tempo alpha that has scanned Q frames (frame t once rint(256 t alpha) + 512 <= P, P > 512) has released
+    max(0, 256 Q - 511) outputs (all P at tempo 1); a push with END releases the rest.  `tempo` holds each slot's tempo
+    since its BEGIN."""
+    _kind, _param, _carried = "time_stretch_stream", TEMPO, "tempo"
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int):
         super().__init__(eng, max_streams, max_chunk_samples)
         self.max_chunk_samples = self._chunk
         self._create(eng.lib.vtts_time_stretch_stream_create, self.max_streams, self.max_chunk_samples, pitch=True)
         self.lookahead = int(eng.lib.vtts_time_stretch_stream_lookahead())
-        self.tempo = np.ones(self.max_streams, np.float32)   # each slot's tempo since its BEGIN
-
-    def _commit(self, flags, tp):
-        begin = (np.asarray(flags) & STREAM_BEGIN) != 0
-        self.tempo[begin] = tp[begin]
 
     def push(self, x, n_new, begin=None, end=None, tempo=None) -> list:
-        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None,
-        tempo: a scalar or [S], read for the slots that begin.  Returns one float32 array per slot with the samples it
-        releases now."""
-        x, n, f = self._host_in(x, n_new, begin, end)
-        tp = _begin_values(self.tempo, f, tempo, "tempo")
-        y = np.empty((self.max_streams, self.out_pitch), np.float32)
-        n_out = np.zeros(self.max_streams, np.int32)
-        self.eng._ck(self.eng.lib.vtts_time_stretch_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(tp), _ptr(y),
-                                                                     _ptr(n_out)))
-        self._commit(f, tp)
-        return self._rows(y, n_out)
+        """As `_SlotStream.push`, with tempo: a scalar or [S], read for the slots that begin."""
+        return self._push_host(x, n_new, begin, end, tempo)
 
     def push_device(self, x_t, n_new, flags, out_t, tempo=None, stream=None) -> np.ndarray:
-        """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S, out_pitch]; n_new int [S], flags
-        uint8 [S] (bit0 BEGIN, bit1 END) and tempo (scalar or [S], read for the slots that begin) on the host.
-        Stream-ordered; returns n_out int32 [S] (outputs slot s got at the start of its row of out_t)."""
-        n, f, st = self._device_in(x_t, out_t, (self.max_streams, self.out_pitch), n_new, flags, stream)
-        tp = _begin_values(self.tempo, f, tempo, "tempo")
-        n_out = np.zeros(self.max_streams, np.int32)
-        self.eng._ck(self.eng.lib.vtts_time_stretch_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(tp), _ptr(out_t),
-                                                                _ptr(n_out), st))
-        self._commit(f, tp)
-        return n_out
+        """As `_SlotStream.push_device`, with tempo (host scalar or [S], read for the slots that begin)."""
+        return self._push_device(x_t, n_new, flags, out_t, stream, tempo)
 
 
 class LoudnessMeter(_SlotStream):
     """Handle of a streaming loudness meter (Engine.open_loudness_meter).  Every push returns every slot's readings
-    [S,4]: integrated, momentary, short-term LUFS and true peak dBTP of the samples it has received since BEGIN."""
-    _kind = "loudness_stream"
+    [S,4] (`push_device`: fills out_t [S,4] and returns it): integrated, momentary, short-term LUFS and true peak dBTP of
+    the samples it has received since BEGIN."""
+    _kind, _width = "loudness_stream", 4
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, rate: int = config.SAMPLE_RATE, max_seconds: int = 600):
         super().__init__(eng, max_streams, max_chunk_samples)
@@ -1540,27 +1487,18 @@ class LoudnessMeter(_SlotStream):
         self._create(eng.lib.vtts_loudness_stream_create, self.max_streams, self.max_chunk_samples, self.rate, self.max_seconds)
         self.lookahead = int(eng.lib.vtts_loudness_stream_lookahead(self.rate))
 
-    def push(self, x, n_new, begin=None, end=None) -> np.ndarray:
-        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None.
-        Returns float32 [S,4]."""
-        x, n, f = self._host_in(x, n_new, begin, end)
-        out = np.empty((self.max_streams, 4), np.float32)
-        self.eng._ck(self.eng.lib.vtts_loudness_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(out)))
-        return out
+    def _outs(self):
+        return ()
 
-    def push_device(self, x_t, n_new, flags, out_t, stream=None):
-        """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S,4]; n_new int [S] and flags uint8 [S]
-        (bit0 BEGIN, bit1 END) on the host.  Stream-ordered."""
-        n, f, st = self._device_in(x_t, out_t, (self.max_streams, 4), n_new, flags, stream)
-        self.eng._ck(self.eng.lib.vtts_loudness_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(out_t), st))
-        return out_t
+    def _result(self, y, outs, host: bool):
+        return y
 
 
 class LimiterStream(_SlotStream):
-    """Handle of a streaming limiter (Engine.open_limiter_stream).  Before END a slot that has received P samples has
-    released max(0, P - lookahead) outputs; a push with END releases the rest.  After every push `reduction_db` holds
-    each slot's deepest reduction over what it has released since BEGIN."""
-    _kind = "limiter_stream"
+    """Handle of a streaming limiter (Engine.open_limiter_stream): `gain_db=` with BEGIN (default 0 dB).  Before END a slot that has received P samples has released
+    max(0, P - lookahead) outputs; a push with END releases the rest.  After every host push `reduction_db` holds each
+    slot's deepest reduction over what it has released since BEGIN; `gain_db` holds each slot's pre-gain."""
+    _kind, _param, _carried = "limiter_stream", GAIN_DB, "gain_db"
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, rate: int = config.SAMPLE_RATE, ceiling: float = -1.0,
                  lookahead_ms: float = 5.0, release_ms: float = 100.0):
@@ -1570,54 +1508,37 @@ class LimiterStream(_SlotStream):
         self._create(eng.lib.vtts_limiter_stream_create, self.max_streams, self.max_chunk_samples, self.rate, self.ceiling,
                      self.lookahead_ms, self.release_ms, pitch=True)
         self.lookahead = int(eng.lib.vtts_limiter_stream_lookahead(self.rate, self.lookahead_ms))
-        self.gain_db = np.zeros(self.max_streams, np.float32)        # each slot's pre-gain since its BEGIN
         self.reduction_db = np.zeros(self.max_streams, np.float32)   # host pushes: each slot's reduction so far
 
-    def _gains(self, flags, gain_db):
-        g = _begin_values(self.gain_db, flags, gain_db, "gain_db")
-        if not (np.all(np.isfinite(g)) and np.all(np.abs(g) <= LIMIT_MAX_GAIN_DB)):
-            raise ValueError(f"gain_db must be finite and lie in [-70, 70], got {gain_db}")
-        return g
-
-    def _commit(self, flags, g):
-        begin = (np.asarray(flags) & STREAM_BEGIN) != 0
-        self.gain_db[begin] = g[begin]
-
     def push(self, x, n_new, begin=None, end=None, gain_db=None) -> list:
-        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None,
-        gain_db: a scalar or [S], read for the slots that begin (default 0 dB).  Returns one float32 array per slot with
-        the samples it releases now."""
-        x, n, f = self._host_in(x, n_new, begin, end)
-        g = self._gains(f, 0.0 if gain_db is None else gain_db)
-        y = np.empty((self.max_streams, self.out_pitch), np.float32)
-        n_out = np.zeros(self.max_streams, np.int32)
-        red = np.empty(self.max_streams, np.float32)
-        self.eng._ck(self.eng.lib.vtts_limiter_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(g), _ptr(y),
-                                                                _ptr(n_out), _ptr(red)))
-        self._commit(f, g)
-        self.reduction_db = red
-        return self._rows(y, n_out)
+        """As `_SlotStream.push`, with gain_db: a scalar or [S], read for the slots that begin (default 0 dB)."""
+        return self._push_host(x, n_new, begin, end, gain_db)
 
     def push_device(self, x_t, n_new, flags, out_t, reduction_t, gain_db=None, stream=None) -> np.ndarray:
-        """Device buffers: x_t f32 CUDA [S, max_chunk_samples], out_t f32 CUDA [S, out_pitch], reduction_t f32 CUDA [S];
-        n_new int [S], flags uint8 [S] (bit0 BEGIN, bit1 END) and gain_db (scalar or [S], read for the slots that begin,
-        default 0 dB) on the host.  Stream-ordered; returns n_out int32 [S] (outputs slot s got at the start of its row of
-        out_t)."""
+        """As `_SlotStream.push_device`, with reduction_t f32 CUDA [S] (each slot's reduction so far, written on the
+        device) and gain_db (host scalar or [S], read for the slots that begin, default 0 dB)."""
+        return self._push_device(x_t, n_new, flags, out_t, stream, gain_db, (reduction_t,))
+
+    def _outs(self, *dev):
+        """a host push: n_out and a new host reduction array; a device push: n_out and reduction_t, which must be a tensor"""
         import torch
-        n, f, st = self._device_in(x_t, out_t, (self.max_streams, self.out_pitch), n_new, flags, stream)
-        if tuple(reduction_t.shape) != (self.max_streams,) or reduction_t.dtype != torch.float32 or not reduction_t.is_contiguous():
-            raise ValueError(f"reduction_t must be contiguous float32 [{self.max_streams}]")
-        g = self._gains(f, 0.0 if gain_db is None else gain_db)
-        n_out = np.zeros(self.max_streams, np.int32)
-        self.eng._ck(self.eng.lib.vtts_limiter_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(g), _ptr(out_t),
-                                                           _ptr(n_out), _ptr(reduction_t), st))
-        self._commit(f, g)
-        return n_out
+        if not dev:
+            return super()._outs() + (np.empty(self.max_streams, np.float32),)
+        (red,) = dev
+        if (not isinstance(red, torch.Tensor) or tuple(red.shape) != (self.max_streams,) or red.dtype != torch.float32
+                or not red.is_contiguous()):
+            raise ValueError(f"reduction_t must be a contiguous float32 tensor [{self.max_streams}]")
+        return super()._outs() + (red,)
+
+    def _result(self, y, outs, host: bool):
+        if host:
+            self.reduction_db = outs[1]
+        return super()._result(y, outs, host)
 
 
 class EqStream(_SlotStream):
     """Handle of a streaming equalizer (Engine.open_eq_stream).  Every push releases every sample it brings:
-    n_out = n_new."""
+    n_out = n_new (`push_device`: out_t may be x_t)."""
     _kind = "eq_stream"
     lookahead = 0
 
@@ -1626,23 +1547,6 @@ class EqStream(_SlotStream):
         self.max_chunk_samples = self.out_pitch = self._chunk
         self.sos = eq_sections(eq, rate)
         self._create(eng.lib.vtts_eq_stream_create, self.max_streams, self.max_chunk_samples, _ptr(self.sos), self.sos.shape[0])
-
-    def push(self, x, n_new, begin=None, end=None) -> list:
-        """x f32 [S, <= max_chunk_samples] (samples past n_new[s] ignored), n_new int [S], begin / end bool [S] or None.
-        Returns one float32 array per slot with its n_new[s] outputs."""
-        x, n, f = self._host_in(x, n_new, begin, end)
-        y = np.empty((self.max_streams, self.out_pitch), np.float32)
-        n_out = np.zeros(self.max_streams, np.int32)
-        self.eng._ck(self.eng.lib.vtts_eq_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(y), _ptr(n_out)))
-        return self._rows(y, n_out)
-
-    def push_device(self, x_t, n_new, flags, out_t, stream=None) -> np.ndarray:
-        """Device buffers: x_t and out_t f32 CUDA [S, max_chunk_samples] (out_t may be x_t); n_new int [S] and flags
-        uint8 [S] (bit0 BEGIN, bit1 END) on the host.  Stream-ordered; returns n_out int32 [S] (= n_new)."""
-        n, f, st = self._device_in(x_t, out_t, (self.max_streams, self.out_pitch), n_new, flags, stream)
-        n_out = np.zeros(self.max_streams, np.int32)
-        self.eng._ck(self.eng.lib.vtts_eq_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(out_t), _ptr(n_out), st))
-        return n_out
 
 
 def acoustic_stream_schedule(n_frames: int, n_emit: int | None, chunk: int, lookahead: int = 10) -> list:
@@ -1734,79 +1638,135 @@ class AcousticStream(_SlotStream):
         return n_out
 
 
+def _output_rate(rate) -> int:
+    """an output rate the resampler reaches from 16 kHz (reduced ratio at most 1024 each way)"""
+    up, down = resample_ratio(config.SAMPLE_RATE, rate)
+    if max(up, down) > 1024:
+        raise ValueError(f"output rate {rate}: {config.SAMPLE_RATE} -> {rate} reduces to {up}/{down} (at most 1024 each)")
+    return int(rate)
+
+
+class OptionError(ValueError):
+    """A bad AudioChain option; `option` is its keyword."""
+
+    def __init__(self, option: str, msg: str):
+        super().__init__(msg)
+        self.option = option
+
+
+class AudioChain:
+    """The audio stages after the vocoder, their options validated, in the one order every caller runs them: denoise,
+    pitch shift and time stretch at 16 kHz, then resample, equalize, limit (or normalize loudness) and meter at the
+    output rate.  `run` applies the chain to one waveform with the one-shot host calls; `streams` opens it as stream
+    stages.  `loudness` (a target in LUFS, reached under `true_peak`, or under the limiter's ceiling with `limit`) has no
+    streaming form, and `meter` only measures, so `run` leaves the audio as it is for it.  Raises OptionError (a
+    ValueError naming the option) for an option out of range."""
+
+    def __init__(self, denoise=None, semitones=None, tempo=None, output_rate=None, eq=None, limit=None, gain_db=0.0,
+                 loudness=None, true_peak=None, meter=False):
+        def checked(option, check, *args):
+            try:
+                return check(*args)
+            except ValueError as e:
+                raise OptionError(option, str(e)) from None
+
+        self.output_rate = None if output_rate is None else checked("output_rate", _output_rate, output_rate)
+        self.rate = self.output_rate or config.SAMPLE_RATE
+        self.denoise = None if denoise is None else checked("denoise", _strength, denoise)
+        self.semitones = None if semitones is None else float(checked("semitones", SEMITONES.rows, semitones, 1)[0])
+        self.tempo = None if tempo is None else float(checked("tempo", TEMPO.rows, tempo, 1)[0])
+        self.eq = None if eq is None else checked("eq", eq_sections, eq, self.rate)
+        self.limit = None if limit is None else checked("limit", _limit_args, limit, self.rate, 5.0, 100.0)[0]
+        self.gain_db = float(checked("gain_db", GAIN_DB.rows, gain_db, 1)[0]) if limit is not None else 0.0
+        self.loudness = self.true_peak = None
+        if loudness is not None:
+            self.loudness, self.true_peak = checked("loudness", _loudness_target, loudness, self.limit if limit is not None else true_peak)
+        if meter or loudness is not None:
+            checked("meter" if loudness is None else "loudness", _loudness_rate, self.rate)
+        self.meter = bool(meter)
+
+    def _stages(self):
+        """(TtsStream attribute, one-shot call or None, stream factory or None) of each stage that is on, in order"""
+        r = self.rate
+        stages = (
+            (self.denoise is not None, "dn", lambda e, w: e.denoise(w, self.denoise),
+             lambda e, S, p, sec: DenoiseStream(e, S, p, self.denoise)),
+            (self.semitones is not None, "ps", lambda e, w: e.pitch_shift(w, self.semitones), lambda e, S, p, sec: PitchShiftStream(e, S, p)),
+            (self.tempo is not None, "ts", lambda e, w: e.time_stretch(w, self.tempo), lambda e, S, p, sec: TimeStretchStream(e, S, p)),
+            (self.output_rate is not None, "rs", lambda e, w: e.resample(w, self.output_rate),
+             lambda e, S, p, sec: ResampleStream(e, S, p, self.output_rate)),
+            (self.eq is not None, "eq", lambda e, w: e.equalize(w, self.eq, r), lambda e, S, p, sec: EqStream(e, S, p, self.eq, r)),
+            (self.loudness is not None, "lm",
+             lambda e, w: e.normalize_loudness(w, self.loudness, r, true_peak=self.true_peak, limit=self.limit is not None)[0], None),
+            (self.loudness is None and self.limit is not None, "lm", lambda e, w: e.limit(w, self.limit, r, self.gain_db)[0],
+             lambda e, S, p, sec: LimiterStream(e, S, p, r, self.limit)),
+            (self.meter, "mt", None, lambda e, S, p, sec: LoudnessMeter(e, S, p, r, sec)),
+        )
+        return [s[1:] for s in stages if s[0]]
+
+    def run(self, eng: Engine, wav) -> np.ndarray:
+        """the one-shot host calls of every stage on `wav` ([S] or [B,S] at 16 kHz), in order"""
+        for _, call, _ in self._stages():
+            if call is not None:
+                wav = call(eng, wav)
+        return wav
+
+    def streams(self, eng: Engine, max_streams: int, pitch: int, max_frames: int):
+        """Opens the stream stages in order, yielding (TtsStream attribute, handle) as each opens: the first takes
+        `pitch` samples per slot and push, each next one the previous one's output width; a meter slot holds the audio of
+        `max_frames` vocoder frames, slowed down at most 1 / MIN_TEMPO times by the time stretcher."""
+        if self.loudness is not None:
+            raise ValueError("loudness normalization has no streaming form (use limit= and gain_db=, or meter=True)")
+        slow = int(1 / MIN_TEMPO) if self.tempo is not None else 1
+        seconds = -(-int(max_frames) * config.HOP * slow // config.SAMPLE_RATE) + 1
+        for name, _, make in self._stages():
+            st = make(eng, max_streams, pitch, seconds)
+            yield name, st
+            pitch = getattr(st, "out_pitch", pitch)
+
+
+_OPENED_WITH = {"semitones": "semitones", "tempo": "tempo", "gain_db": "limit"}   # the open_tts_stream option of each stage
+
+
 class TtsStream:
     """Handle of a text-to-speech stream (Engine.open_tts_stream): an acoustic stream of max_chunk_frames F feeding a
-    vocoder stream of F + the acoustic lookahead frames per push, with a denoise strength a denoise stream after it,
-    with semitones a pitch-shift stream, with a tempo a time-stretch stream, with an output rate a resample stream, with
-    eq an equalizer stream, with limit a limiter stream, and with meter=True a loudness meter of the audio `step()`
-    returns last."""
+    vocoder stream of F + the acoustic lookahead frames per push, then the stream stages of the AudioChain of the
+    options, each taking the previous one's output buffer, with a loudness meter of the audio `step()` returns last."""
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
                  output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None, gain_db=0.0, eq=None):
         import torch
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
-        if output_rate is not None:
-            resample_ratio(config.SAMPLE_RATE, output_rate)
-        if denoise is not None:
-            denoise = _strength(denoise)
-        if meter:
-            _loudness_rate(output_rate or config.SAMPLE_RATE)
-        if semitones is not None:
-            semitones = float(_semitones(semitones, 1)[0])
-        if tempo is not None:
-            tempo = float(_tempo(tempo, 1)[0])
-        if limit is not None:
-            limit = _limit_args(limit, output_rate or config.SAMPLE_RATE, 5.0, 100.0)[0]
-            gain_db = float(_gain_db(gain_db, 1)[0])
-        if eq is not None:
-            eq = eq_sections(eq, output_rate or config.SAMPLE_RATE)
+        self._chain = AudioChain(denoise=denoise, semitones=semitones, tempo=tempo, output_rate=output_rate, eq=eq, limit=limit,
+                                 gain_db=gain_db, meter=meter)
         self.eng = eng
         self.rs = self.dn = self.ps = self.ts = self.eq = self.lm = self.mt = None
-        S, sr = max_streams, output_rate or config.SAMPLE_RATE
-        # the stages after the vocoder, in push order; each takes the previous stage's output buffer as its input
-        # (the vocoder's: n_new = 256 * frames it emitted) and a slot of the meter holds at most max_frames of audio,
-        # slowed down at most 1 / MIN_TEMPO times by the time stretcher
-        slow = int(1 / MIN_TEMPO) if tempo is not None else 1
-        seconds = -(-int(max_frames) * config.HOP * slow // config.SAMPLE_RATE) + 1
-        plan = (("dn", denoise is not None, lambda p: DenoiseStream(eng, S, p, denoise)),
-                ("ps", semitones is not None, lambda p: PitchShiftStream(eng, S, p)),
-                ("ts", tempo is not None, lambda p: TimeStretchStream(eng, S, p)),
-                ("rs", output_rate is not None, lambda p: ResampleStream(eng, S, p, output_rate)),
-                ("eq", eq is not None, lambda p: EqStream(eng, S, p, eq, sr)),
-                ("lm", limit is not None, lambda p: LimiterStream(eng, S, p, sr, limit)),
-                ("mt", meter, lambda p: LoudnessMeter(eng, S, p, sr, seconds)))
+        S = max_streams
         self._built = []   # every stream handle, in construction order
         try:
             self.ac = AcousticStream(eng, S, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng)
             self._built.append(self.ac)
             self.voc = VocoderStream(eng, S, self.ac.out_frames)
             self._built.append(self.voc)
-            pitch = self.voc.wav_ld
-            for name, on, make in plan:
-                if on:
-                    st = make(pitch)
-                    self._built.append(st)
-                    setattr(self, name, st)
-                    pitch = getattr(st, "out_pitch", pitch)
+            for name, st in self._chain.streams(eng, S, self.voc.wav_ld, max_frames):
+                self._built.append(st)
+                setattr(self, name, st)
         except Exception:
             self.close()
             raise
         dev = torch.device("cuda", eng.device)
         self._mel = torch.zeros((S, self.ac.out_frames, config.MEL_DIM), dtype=torch.float32, device=dev)
         self._wav = torch.zeros((S, self.voc.wav_ld), dtype=torch.float32, device=dev)
-        self._shift = np.zeros(S, np.float32)  # the shift of each slot's utterance
-        self._tempo = np.ones(S, np.float32)   # the tempo of each slot's utterance
-        self._gain = np.zeros(S, np.float32)   # the limiter pre-gain of each slot's utterance
-        self._red = None if self.lm is None else torch.zeros(S, dtype=torch.float32, device=dev)
-        extra = {"ps": {"semitones": self._shift}, "ts": {"tempo": self._tempo}, "lm": {"reduction_t": self._red, "gain_db": self._gain}}
-        # (handle, device output buffer, extra push arguments) of the stages after the vocoder
-        self._stages = [(st, torch.zeros((S, 4 if st is self.mt else st.out_pitch), dtype=torch.float32, device=dev),
-                         next((kw for name, kw in extra.items() if st is getattr(self, name)), {})) for st in self._built[2:]]
+        # (handle, device output buffer, extra push arguments) of the stages after the vocoder; a stage's BEGIN
+        # parameter is the array of each slot's utterance value, set by `begin`
+        self._stages = []
+        for st in self._built[2:]:
+            kw = {} if st._param is None else {st._param.name: np.full(S, st._param.neutral, np.float32)}
+            if st is self.lm:
+                kw["reduction_t"] = torch.zeros(S, dtype=torch.float32, device=dev)
+            self._stages.append((st, torch.zeros((S, st._width), dtype=torch.float32, device=dev), kw))
         self._mout_h = None if self.mt is None else torch.zeros((S, 4), dtype=torch.float32).pin_memory()
-        self._semitones = semitones                    # every slot's default shift
-        self._tempo_default = tempo                    # every slot's default tempo
-        self._gain_default = gain_db                   # every slot's default limiter pre-gain
         self._meter = {}
         self._fresh = np.zeros(max_streams, bool)   # begun, no push yet: the next vocoder push carries BEGIN
         self._empty = set()                         # begun with nothing left after the trim: reported empty at the next step
@@ -1822,15 +1782,15 @@ class TtsStream:
         slot = int(slot)
         if self.ac.open[slot] or slot in self._empty:
             raise ValueError(f"slot {slot} is still open")
-        if semitones is not None and self.ps is None:
-            raise ValueError("the stream was opened without semitones= (no pitch-shift stage)")
-        if tempo is not None and self.ts is None:
-            raise ValueError("the stream was opened without tempo= (no time-stretch stage)")
-        if gain_db is not None and self.lm is None:
-            raise ValueError("the stream was opened without limit= (no limiter stage)")
-        gain = self._gain_default if gain_db is None else float(_gain_db(gain_db, 1)[0])
-        shift = self._semitones if semitones is None else float(_semitones(semitones, 1)[0])
-        pace = self._tempo_default if tempo is None else float(_tempo(tempo, 1)[0])
+        given = {"semitones": semitones, "tempo": tempo, "gain_db": gain_db}
+        values = []   # (a stage's per-slot array, this utterance's value)
+        for st, _, kw in self._stages:
+            if st._param is not None:
+                v = given.pop(st._param.name)
+                values.append((kw[st._param.name], getattr(self._chain, st._param.name) if v is None else float(st._param.rows(v, 1)[0])))
+        for name, v in given.items():
+            if v is not None:
+                raise ValueError(f"the stream was opened without {_OPENED_WITH[name]}= (no stage takes {name}=)")
         tok = _np(tokens, np.int32).reshape(1, -1)
         _, frames, nf, ne = self.eng.tts_plan(tok, silence_duration=silence_duration)
         if nf[0] < 1:
@@ -1840,12 +1800,8 @@ class TtsStream:
             return 0
         self.ac.begin([slot], tok, frames, n_frames=nf, n_emit=ne)
         self._fresh[slot] = True
-        if self.ps is not None:
-            self._shift[slot] = shift
-        if self.ts is not None:
-            self._tempo[slot] = pace
-        if self.lm is not None:
-            self._gain[slot] = gain
+        for a, v in values:
+            a[slot] = v
         return int(ne[0])
 
     def busy(self) -> np.ndarray:

@@ -110,6 +110,11 @@ def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_
     return out
 
 
+# the command-line flag of each AudioChain option the CLI sets
+_FLAGS = {"denoise": "--denoise", "semitones": "--pitch", "tempo": "--tempo", "output_rate": "--output-rate", "eq": "--eq",
+          "limit": "--limiter", "loudness": "--loudness"}
+
+
 def main(argv=None) -> int:
     parser = ArgumentParser(description="H100-native vietTTS synthesizer")
     parser.add_argument("--text", type=str)
@@ -164,49 +169,17 @@ def main(argv=None) -> int:
         parser.error("--reference-dropout applies to --text-file (--text always uses the reference's stream)")
     if args.reference_dropout and args.seed is not None:
         parser.error("--reference-dropout and --seed select different dropout streams; give one")
-    if args.denoise is not None and not (np.isfinite(args.denoise) and args.denoise >= 0):
-        parser.error(f"--denoise {args.denoise}: the strength must be finite and >= 0")
-    if args.pitch is not None and not (np.isfinite(args.pitch) and abs(args.pitch) <= 12.0):
-        parser.error(f"--pitch {args.pitch}: the shift must be finite and lie in [-12, 12] semitones")
-    if args.tempo is not None and not (np.isfinite(args.tempo) and 0.5 <= args.tempo <= 2.0):
-        parser.error(f"--tempo {args.tempo}: the tempo must be finite and lie in [0.5, 2]")
-    if args.output_rate is not None:
-        if args.sample_rate is not None and args.sample_rate != args.output_rate:
-            parser.error("--sample-rate only labels the 16 kHz samples and --output-rate resamples them; they disagree")
-        from .engine import resample_ratio
-        try:
-            up, down = resample_ratio(config.SAMPLE_RATE, args.output_rate)
-        except ValueError as e:
-            parser.error(f"--output-rate: {e}")
-        if max(up, down) > 1024:
-            parser.error(f"--output-rate {args.output_rate}: {config.SAMPLE_RATE} -> {args.output_rate} reduces to {up}/{down} "
-                         "(at most 1024 each)")
+    if args.output_rate is not None and args.sample_rate is not None and args.sample_rate != args.output_rate:
+        parser.error("--sample-rate only labels the 16 kHz samples and --output-rate resamples them; they disagree")
     if args.true_peak is not None and args.loudness is None and not args.limiter:
         parser.error("--true-peak is the ceiling of --loudness normalization or of --limiter; give one of them too")
-    if args.limiter and args.loudness is None:
-        from .engine import _limit_args
-        if args.true_peak is None:
-            args.true_peak = -1.0
-        try:
-            _limit_args(args.true_peak, args.output_rate or config.SAMPLE_RATE, 5.0, 100.0)
-        except ValueError as e:
-            parser.error(f"--limiter: {e}")
-    if args.loudness is not None:
-        from .engine import _loudness_rate, _loudness_target
-        if args.true_peak is None:
-            args.true_peak = -1.0
-        try:
-            _loudness_target(args.loudness, args.true_peak)
-            _loudness_rate(args.output_rate or config.SAMPLE_RATE)
-        except ValueError as e:
-            parser.error(f"--loudness: {e}")
-    eq_sos = None
-    if args.eq is not None:
-        from .engine import eq_sections
-        try:
-            eq_sos = eq_sections(args.eq, args.output_rate or config.SAMPLE_RATE)
-        except ValueError as e:
-            parser.error(f"--eq: {e}")
+    from .engine import AudioChain, OptionError
+    ceiling = -1.0 if args.true_peak is None else args.true_peak
+    try:
+        chain = AudioChain(denoise=args.denoise, semitones=args.pitch, tempo=args.tempo, output_rate=args.output_rate, eq=args.eq,
+                           limit=ceiling if args.limiter else None, loudness=args.loudness, true_peak=ceiling)
+    except OptionError as e:
+        parser.error(f"{_FLAGS[e.option]}: {e}")
     header_rate = args.output_rate or args.sample_rate or config.SAMPLE_RATE
     lexicon = args.lexicon_file if args.lexicon_file is not None else config.LEXICON_FILE
     if args.precision is not None:
@@ -215,25 +188,7 @@ def main(argv=None) -> int:
 
     def to_output_rate(waves):
         from .engine import get_engine
-        if args.denoise is not None:
-            waves = [get_engine().denoise(w, args.denoise) for w in waves]
-        if args.pitch is not None:
-            waves = [get_engine().pitch_shift(w, args.pitch) for w in waves]
-        if args.tempo is not None:
-            waves = [get_engine().time_stretch(w, args.tempo) for w in waves]
-        if args.output_rate is not None:
-            waves = [get_engine().resample(w, args.output_rate) for w in waves]
-        if eq_sos is not None:
-            rate = args.output_rate or config.SAMPLE_RATE
-            waves = [get_engine().equalize(w, eq_sos, rate) for w in waves]
-        if args.loudness is not None:
-            rate = args.output_rate or config.SAMPLE_RATE
-            waves = [get_engine().normalize_loudness(w, args.loudness, rate, true_peak=args.true_peak, limit=args.limiter)[0]
-                     for w in waves]
-        elif args.limiter:
-            rate = args.output_rate or config.SAMPLE_RATE
-            waves = [get_engine().limit(w, args.true_peak, rate)[0] for w in waves]
-        return waves
+        return [chain.run(get_engine(), w) for w in waves]
 
     if args.text_file is not None:
         lines = [ln for ln in args.text_file.read_text().splitlines() if ln.strip()]

@@ -152,9 +152,13 @@ int vtts_duration_forward(vtts_ctx* ctx, const int32_t* tokens_dev, const int32_
 int vtts_melspec(vtts_ctx* ctx, const float* wav_dev, int B, int S, float* mel_dev, void* stream);
 
 /* optional taps for tests: copy an internal activation of the LAST forward call to host.
- * name: "enc" [B,L,512] (of the last acoustic OR duration call), "cond" [B,N,512], "mel_pre" [B,N,80] (before the postnet;
- * after an acoustic stream push: the stream's [max_streams, max_frames, 80] projection outputs, valid for the frames
- * each slot has scanned). */
+ * name: "enc" [B,L,512] (of the last acoustic, teacher-forced OR duration call), "cond" [B,N,512] (autoregressive pass),
+ * "mel_pre" [B,N,80] (before the postnet, = mel1 of the teacher-forced pass; after an acoustic stream push: the stream's
+ * [max_streams, max_frames, 80] projection outputs, valid for the frames each slot has scanned), "dec_in" [B,N,768]
+ * (teacher-forced decoder input [cond | prenet(mels_in)]), "dec_out" [B,N,1024] (decoder scan output [h0 | h1], before
+ * zoneout; autoregressive and teacher-forced pass).  Each call sets every tap, to nothing where it produces none; a
+ * call that grows the workspace, and destroying the stream a mel_pre tap points into, clear them all.  Reading a tap
+ * that is not set fails with VTTS_ERR_BAD_ARG before any copy. */
 int vtts_debug_read(vtts_ctx* ctx, const char* name, float* host_out, int64_t n_floats);
 
 /* test hook: one hk.Conv1D (SAME padding, dilation, optional leaky_relu on the input and residual

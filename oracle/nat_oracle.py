@@ -265,37 +265,62 @@ def teacher_forced(ckpt, tokens, lengths, durations_frames, mels_in, keep_masks=
     P, S = ckpt["params"], ckpt["aux"]
     with torch.no_grad():
         mels_in = _t(mels_in, dtype)
-        B, N, _ = mels_in.shape
+        N = mels_in.shape[1]
         enc = token_encoder(P, S, tokens, lengths, dtype)
         cond, _ = upsample(enc, _t(durations_frames, dtype), N)
-        if keep_masks is None:
-            p = prenet(P, mels_in, None, dtype)
-        else:
-            km = torch.as_tensor(np.asarray(keep_masks)).bool()          # [B,N,2,256] -> prenet wants [...,2,256] on dim 1
-            w1 = _t(P[A + "linear_1"]["w"], dtype)
-            w2 = _t(P[A + "linear_2"]["w"], dtype)
-            p = km[:, :, 0].to(dtype) * torch.relu(mels_in @ w1) / 0.5
-            p = km[:, :, 1].to(dtype) * torch.relu(p @ w2) / 0.5
-        x = torch.cat([cond, p], dim=-1)
+        x = torch.cat([cond, tf_prenet(P, mels_in, keep_masks, dtype)], dim=-1)
+        mel1 = project(P, zoneout_decode(P, x, zone_masks, dtype), dtype)
+        mel2 = mel1 + postnet(P, S, mel1, dtype)
+        return mel1.numpy(), mel2.numpy()
+
+
+def tf_prenet(P, mels_in, keep=None, dtype=torch.float32):
+    """The prenet of the teacher-forced pass over whole sequences (model.py:95-100,149).  mels_in [B,N,80] (any float
+    array); keep uint8 [B,N,2,256] or None (dropout off, scale 1).  Returns p2 [B,N,256]."""
+    with torch.no_grad():
+        x = _t(mels_in, dtype)
+        w1 = _t(P[A + "linear_1"]["w"], dtype)
+        w2 = _t(P[A + "linear_2"]["w"], dtype)
+        km = None if keep is None else torch.as_tensor(np.asarray(keep)).bool()
+        x = torch.relu(x @ w1)
+        if km is not None:
+            x = km[:, :, 0].to(dtype) * x / 0.5
+        x = torch.relu(x @ w2)
+        if km is not None:
+            x = km[:, :, 1].to(dtype) * x / 0.5
+        return x
+
+
+def zoneout_decode(P, x, zone=None, dtype=torch.float32):
+    """The zoneout decoder of the teacher-forced pass (model.py:150-166): x [B,N,768] = [cond | p2] (any float array);
+    zone uint8 [B,N,4,512] in the state-tree order (layer0.hidden, layer0.cell, layer1.hidden, layer1.cell), 1 = keep
+    the previous state (`s1 * m + s2 * (1 - m)`, model.py:157-159), or None.  Returns the decoder output [B,N,1024] =
+    [h0 | h1], the cores' new (un-zoned) hidden states."""
+    with torch.no_grad():
+        x = _t(x, dtype)
+        B, N, _ = x.shape
         w0, b0 = _t(P[A + "lstm/linear"]["w"], dtype), _t(P[A + "lstm/linear"]["b"], dtype)
-        w1_, b1 = _t(P[A + "lstm_1/linear"]["w"], dtype), _t(P[A + "lstm_1/linear"]["b"], dtype)
-        wo, bo = _t(P[A + "linear"]["w"], dtype), _t(P[A + "linear"]["b"], dtype)
+        w1, b1 = _t(P[A + "lstm_1/linear"]["w"], dtype), _t(P[A + "lstm_1/linear"]["b"], dtype)
         H = w0.shape[1] // 4
         h0 = x.new_zeros(B, H); c0 = x.new_zeros(B, H); h1 = x.new_zeros(B, H); c1 = x.new_zeros(B, H)
-        zm = None if zone_masks is None else torch.as_tensor(np.asarray(zone_masks)).bool()
+        zm = None if zone is None else torch.as_tensor(np.asarray(zone)).bool()
         outs = []
         for t in range(N):
             nh0, nc0 = lstm_step(x[:, t], h0, c0, w0, b0)
-            nh1, nc1 = lstm_step(torch.cat([x[:, t], nh0], dim=-1), h1, c1, w1_, b1)   # skip connection feeds the NEW h0
-            outs.append(torch.cat([nh0, nh1], dim=-1))                                  # decoder output = un-zoned states
+            nh1, nc1 = lstm_step(torch.cat([x[:, t], nh0], dim=-1), h1, c1, w1, b1)   # skip connection feeds the NEW h0
+            outs.append(torch.cat([nh0, nh1], dim=-1))                                 # decoder output = un-zoned states
             if zm is None:
                 h0, c0, h1, c1 = nh0, nc0, nh1, nc1
             else:
                 h0 = torch.where(zm[:, t, 0], h0, nh0); c0 = torch.where(zm[:, t, 1], c0, nc0)
                 h1 = torch.where(zm[:, t, 2], h1, nh1); c1 = torch.where(zm[:, t, 3], c1, nc1)
-        mel1 = torch.stack(outs, 1) @ wo + bo
-        mel2 = mel1 + postnet(P, S, mel1, dtype)
-        return mel1.numpy(), mel2.numpy()
+        return torch.stack(outs, 1)
+
+
+def project(P, hout, dtype=torch.float32):
+    """The output projection (model.py:167): hout [B,N,1024] (any float array) -> mel1 [B,N,80]."""
+    with torch.no_grad():
+        return _t(hout, dtype) @ _t(P[A + "linear"]["w"], dtype) + _t(P[A + "linear"]["b"], dtype)
 
 
 def gta_forward(ckpt, wav_i16, tokens, lengths, durations_sec, keep_masks=None, zone_masks=None, dtype=torch.float32):

@@ -166,6 +166,7 @@ int vtts_acoustic_stream_destroy(vtts_ctx* ctx, vtts_acoustic_stream* as) {
   if (as->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic_stream_destroy: the stream belongs to another context");
   VTTS_CUDA(cudaSetDevice(ctx->device));
   VTTS_CUDA(cudaDeviceSynchronize());   // a push may still be running on the caller's stream
+  if (ctx->tap_melpre == as->melpre) ctx->clear_taps();
   cudaFree(as->mem);
   delete as;
   return VTTS_OK;
@@ -291,6 +292,7 @@ int vtts_acoustic_stream_push(vtts_ctx* ctx, vtts_acoustic_stream* as, float* me
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   // the stream's projection outputs so far are the mel_pre tap of this push ([S][max_frames][80])
+  ctx->clear_taps();
   ctx->tap_melpre = as->melpre;
   ctx->tap_melpre_n = (int64_t)S * as->NF * vc::MEL;
   // ---- commit ----

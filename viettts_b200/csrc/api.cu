@@ -23,6 +23,7 @@ int vtts_ctx::fail(int code, const char* fmt, ...) {
 int vtts_ctx::ensure_ws(size_t bytes) {
   vtts_ctx* ctx = this;
   if (bytes <= ws_bytes) return VTTS_OK;
+  clear_taps();   // they point into the workspace freed here
   if (ws) {
     VTTS_CUDA(cudaDeviceSynchronize());
     cudaFree(ws);
@@ -693,8 +694,13 @@ int vtts_debug_read(vtts_ctx* ctx, const char* name, float* host_out, int64_t n_
   if (!strcmp(name, "enc")) { src = ctx->tap_enc; n = ctx->tap_enc_n; }
   else if (!strcmp(name, "cond")) { src = ctx->tap_cond; n = ctx->tap_cond_n; }
   else if (!strcmp(name, "mel_pre")) { src = ctx->tap_melpre; n = ctx->tap_melpre_n; }
+  else if (!strcmp(name, "dec_in")) { src = ctx->tap_decin; n = ctx->tap_decin_n; }
+  else if (!strcmp(name, "dec_out")) { src = ctx->tap_decout; n = ctx->tap_decout_n; }
   else return ctx->fail(VTTS_ERR_BAD_ARG, "debug_read: unknown tap %s", name);
-  if (!src || n_floats != n) return ctx->fail(VTTS_ERR_BAD_ARG, "debug_read: tap %s has %lld floats, asked %lld", name, (long long)n, (long long)n_floats);
+  if (!src)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "debug_read: tap %s is not set (the last call did not produce it, or the workspace it pointed into "
+                     "was freed)", name);
+  if (n_floats != n) return ctx->fail(VTTS_ERR_BAD_ARG, "debug_read: tap %s has %lld floats, asked %lld", name, (long long)n, (long long)n_floats);
   VTTS_CUDA(cudaSetDevice(ctx->device));
   VTTS_CUDA(cudaDeviceSynchronize());
   VTTS_CUDA(cudaMemcpy(host_out, src, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost));

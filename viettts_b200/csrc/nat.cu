@@ -1372,9 +1372,11 @@ int vtts_acoustic_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengt
   const size_t BL = (size_t)B * L, BN = (size_t)B * N;
   const ModelWeights& m = ctx->ac;
   const auto& D = m.d;
+  ctx->clear_taps();
   ctx->tap_enc = w.e.enc; ctx->tap_enc_n = BL * 512;
   ctx->tap_cond = w.cond; ctx->tap_cond_n = BN * 512;
   ctx->tap_melpre = w.melpre; ctx->tap_melpre_n = BN * 80;
+  ctx->tap_decout = w.hout; ctx->tap_decout_n = BN * 1024;
 
   VTTS_CUDA(cudaMemsetAsync(mel, 0, BN * 80 * sizeof(float), st));
   VTTS_CUDA(cudaMemsetAsync(w.melpre, 0, BN * 80 * sizeof(float), st));
@@ -1447,9 +1449,11 @@ int vtts_acoustic_teacher_run(vtts_ctx* ctx, const int32_t* tokens, const int32_
   const ModelWeights& m = ctx->ac;
   const auto& T = m.t;
   const auto& D = m.d;
+  ctx->clear_taps();   // cond: the first 512 columns of dec_in
   ctx->tap_enc = w.e.enc; ctx->tap_enc_n = BL * 512;
-  ctx->tap_cond = nullptr; ctx->tap_cond_n = 0;
   ctx->tap_melpre = w.melpre; ctx->tap_melpre_n = BN * 80;
+  ctx->tap_decin = w.xin; ctx->tap_decin_n = BN * XW;
+  ctx->tap_decout = w.hout; ctx->tap_decout_n = BN * 1024;
   VTTS_CUDA(cudaMemsetAsync(mel2, 0, BN * 80 * sizeof(float), st));
   if (mel1) VTTS_CUDA(cudaMemsetAsync(mel1, 0, BN * 80 * sizeof(float), st));
   VTTS_CUDA(cudaMemsetAsync(w.xin, 0, BN * XW * sizeof(float), st));
@@ -1612,11 +1616,12 @@ int vtts_duration_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengt
   const DuBufs w = carve_ws<DuBufs>(ctx, B, L, 0);
   const size_t BL = (size_t)B * L;
   const ModelWeights& m = ctx->du;
+  ctx->clear_taps();
+  ctx->tap_enc = w.e.enc; ctx->tap_enc_n = BL * 512;
   // padded encoder rows are never written by the scan: clear them so the projection reads zeros, not stale workspace
   VTTS_CUDA(cudaMemsetAsync(w.e.enc, 0, BL * 512 * sizeof(float), st));
   int rc = run_token_encoder(ctx, m, tokens, lengths, B, L, w.e, st);
   if (rc) return rc;
-  ctx->tap_enc = w.e.enc; ctx->tap_enc_n = BL * 512;
   // ---- projection head ----
   const ConvProb p = conv_prob(w.e.enc, m.t[dui::FC1_W], m.t[dui::FC1_B], w.y);
   rc = run_convs(ctx, &p, 1, 512, 256, 1, (int)BL, nullptr, 0, m.tiles(PK_DU_FC1), st);

@@ -211,10 +211,18 @@ struct vtts_ctx {
   struct LnFilter { int rate; float coef[10]; float seg[5][16]; float blk[16]; };
   std::vector<LnFilter> ln_filters;
 
-  // taps of the last acoustic forward (point into ws)
+  // taps of the last acoustic, teacher-forced or duration call or acoustic stream push (vtts_debug_read).  They point
+  // into ws (the stream's mel_pre into the stream's memory): every call that sets one sets all of them, null where it
+  // produces none, and ensure_ws / the stream's destroy clear them before freeing what they point into.
   float* tap_enc = nullptr; int64_t tap_enc_n = 0;
   float* tap_cond = nullptr; int64_t tap_cond_n = 0;
   float* tap_melpre = nullptr; int64_t tap_melpre_n = 0;
+  float* tap_decin = nullptr; int64_t tap_decin_n = 0;     // teacher-forced decoder input [B,N,768] = [cond | p2]
+  float* tap_decout = nullptr; int64_t tap_decout_n = 0;   // decoder scan output [B,N,1024] = [h0 | h1] (un-zoned)
+  void clear_taps() {
+    tap_enc = tap_cond = tap_melpre = tap_decin = tap_decout = nullptr;
+    tap_enc_n = tap_cond_n = tap_melpre_n = tap_decin_n = tap_decout_n = 0;
+  }
 
   static constexpr int NSTAGE = 4;   // 0 hifigan, 1 acoustic, 2 melspec, 3 duration
   cudaEvent_t ev0[NSTAGE] = {nullptr, nullptr, nullptr, nullptr};

@@ -581,6 +581,45 @@ int vtts_eq_stream_push(vtts_ctx* ctx, vtts_eq_stream* es, const float* x_dev, c
 int vtts_eq_stream_push_host(vtts_ctx* ctx, vtts_eq_stream* es, const float* x, const int32_t* n_new, const uint8_t* flags, float* y,
                              int32_t* n_out);
 
+/* ---- feed-forward dynamic range compressor ------------------------------------------------------------------------
+ * One mono row x of n samples at rate r (an integer in [8000, 192000]); threshold T dBFS in [-60, 0], ratio R in
+ * [1, 20], knee W dB in [0, 24], attack A ms in [0.5, 200], release Rel ms in [5, 5000], makeup M dB in [-24, 24]
+ * (anything else, NaN included, fails with VTTS_ERR_BAD_ARG before anything is launched):
+ *   L = 20 log10 |x|;  x_L = L - G(L) >= 0 with the soft-knee gain computer G (Giannoulis, Massberg & Reiss 2012,
+ *   eq. 4: 0 where 2 (L - T) < -W, (1 - 1/R) (L - T + W/2)^2 / (2W) where 2 |L - T| <= W, (1 - 1/R) (L - T) above);
+ *   release y1[t] = max(x_L[t], a_R y1[t - 1] + b_R x_L[t]);  attack y_L[t] = a_A y_L[t - 1] + b_A y1[t] (both from
+ *   0), a = fp32(exp(-1000 / (tau r))), b = 1 - a;  y = (x m) 10^(-y_L / 20), m = fp32(10^(M / 20));
+ *   reduction_db = -max y_L (<= 0, makeup excluded).  Rows that stay below the knee (and R = 1) come back as x m bit
+ *   for bit.
+ * fp32 in every vtts_precision mode; every value is a fixed function of the samples and of state at boundaries of 256
+ * samples fixed by absolute sample index, so a row gives the same bits alone, in any batch, and through the stream. */
+/* x_dev [B,S]; n_dev int32 [B] or NULL (= S; values clamped to [0, S]); y_dev [B,S] (may equal x_dev), 0 past n[b];
+ * reduction_db_dev [B] or NULL.  Stream-ordered, no host synchronisation, six launches; uses the context's workspace
+ * (about 0.2 bytes per sample). */
+int vtts_compress(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, float threshold_db, float ratio,
+                  float knee_db, float attack_ms, float release_ms, float makeup_db, float* y_dev, float* reduction_db_dev, void* stream);
+/* the same on host buffers; n_in[b] must lie in [0, S]; reduction_db [B] or NULL */
+int vtts_compress_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float threshold_db, float ratio,
+                       float knee_db, float attack_ms, float release_ms, float makeup_db, float* y, float* reduction_db);
+/* Streaming compressor with max_streams independent slots; every parameter is fixed at create.  Every sample is released
+ * by the push that brings it (no lookahead): n_out[s] = n_new[s], and a slot's outputs, concatenated, equal
+ * vtts_compress of its whole input bit for bit.  Each slot carries the partial release and attack maps of the block
+ * holding its next sample, that block's entering y1 and y_L, and its largest y_L.  flags and slot rules as for the
+ * resample stream.  Every push issues the same six launches. */
+typedef struct vtts_compressor_stream vtts_compressor_stream;
+int vtts_compressor_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int rate, float threshold_db, float ratio,
+                                  float knee_db, float attack_ms, float release_ms, float makeup_db, vtts_compressor_stream** out);
+int vtts_compressor_stream_destroy(vtts_ctx* ctx, vtts_compressor_stream* cs);
+/* x_dev [S][max_chunk_samples] (samples past n_new[s] ignored); n_new, flags, n_out HOST int32 / uint8 / int32 [S];
+ * y_dev [S][max_chunk_samples] (may equal x_dev): slot s gets n_out[s] outputs from its start; reduction_db_dev [S]
+ * receives each slot's reduction over what it has released since BEGIN.  Argument errors fail with VTTS_ERR_BAD_ARG
+ * before anything is launched.  Stream-ordered. */
+int vtts_compressor_stream_push(vtts_ctx* ctx, vtts_compressor_stream* cs, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
+                                float* y_dev, int32_t* n_out, float* reduction_db_dev, void* stream);
+/* the same on host buffers x and y [S][max_chunk_samples] and reduction_db [S]; returns when they are written */
+int vtts_compressor_stream_push_host(vtts_ctx* ctx, vtts_compressor_stream* cs, const float* x, const int32_t* n_new, const uint8_t* flags,
+                                     float* y, int32_t* n_out, float* reduction_db);
+
 /* ---- streaming acoustic model: every slot advances its decoder a few frames per push ---------------------------
  * A vtts_acoustic_stream holds max_streams (1..128) independent slots.  begin starts utterances in closed slots; each
  * push advances every open slot by min(F, frames left) decoder steps in ONE scan launch and returns the mel frames whose

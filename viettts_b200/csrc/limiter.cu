@@ -182,17 +182,7 @@ __global__ void __launch_bounds__(THREADS) lm_attack_kernel(const float* __restr
   }
 }
 
-struct Map {
-  float c, m, k;
-};
-__device__ __forceinline__ Map map_id() { return Map{-INFINITY, 1.f, 0.f}; }
-__device__ __forceinline__ void map_fold(Map& M, float a, float beta, float omb) {
-  const float e = omb * a;
-  M.c = fmaxf(a, fmaf(beta, M.c, e));
-  M.m = beta * M.m;
-  M.k = fmaf(beta, M.k, e);
-}
-__device__ __forceinline__ float map_apply(const Map& M, float d) { return fmaxf(M.c, fmaf(M.m, d, M.k)); }
+// the release maps (Map, map_fold, map_apply) live in vtts_internal.cuh, shared with the compressor
 
 // the samples [lo, hi) of call block i of row r
 __device__ __forceinline__ void lm_block_span(const LmRow& r, int i, long long& lo, long long& hi) {

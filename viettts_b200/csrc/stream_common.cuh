@@ -104,6 +104,12 @@ struct SampleStream : StreamBase {
     return vtts_stream_window_prep(ctx, win, cap, K, reinterpret_cast<const int*>(d_tbl + steps), x, F, S, st);
   }
 
+  // a stream that reads each push's inputs where they are (K = 0, no window carved): only the push's one table copy
+  int upload_rows(cudaStream_t st) {
+    VTTS_CUDA(cudaMemcpyAsync(d_tbl, tbl.data(), (size_t)S * offset(sizeof...(Rows)), cudaMemcpyHostToDevice, st));
+    return VTTS_OK;
+  }
+
  private:
   // bytes per slot of the row types before the n-th
   static constexpr size_t offset(int n) {

@@ -391,6 +391,19 @@ struct RsRow {
 // outputs of a row.
 int vtts_resample_run(vtts_ctx* ctx, int in_rate, int out_rate, const float* x, long long x_ld, int S_in, const int* n_in,
                       const RsRow* rows, int B, long long S_out, long long max_out, float* y, long long y_ld, cudaStream_t st);
+// limiter.cu, compressor.cu: the monotone maps M(d) = max(c, fma(m, d, k)) of a release scan in the form of the
+// limiter's.  map_fold composes f_t(d) = max(a, fma(beta, d, e)), e = omb a, after M; the identity is (-inf, 1, 0).
+struct Map {
+  float c, m, k;
+};
+__device__ __forceinline__ Map map_id() { return Map{-INFINITY, 1.f, 0.f}; }
+__device__ __forceinline__ void map_fold(Map& M, float a, float beta, float omb) {
+  const float e = omb * a;
+  M.c = fmaxf(a, fmaf(beta, M.c, e));
+  M.m = beta * M.m;
+  M.k = fmaf(beta, M.k, e);
+}
+__device__ __forceinline__ float map_apply(const Map& M, float d) { return fmaxf(M.c, fmaf(M.m, d, M.k)); }
 // loudness.cu: the context workspace vtts_loudness / vtts_loudness_normalize use for B rows of S samples at `rate`
 // (from the start of ctx->ws)
 size_t vtts_loudness_ws_bytes(int B, int S, int rate);

@@ -170,6 +170,53 @@ def eq_sections(spec, rate: int) -> np.ndarray:
     return sos
 
 
+# the compressor's parameters in vtts_compress's order, with their ranges and the `voice` preset
+COMPRESSOR_RANGES = {"threshold": (-60.0, 0.0), "ratio": (1.0, 20.0), "knee": (0.0, 24.0), "attack": (0.5, 200.0),
+                     "release": (5.0, 5000.0), "makeup": (-24.0, 24.0)}
+COMPRESSOR_PRESETS = {"voice": {"threshold": -24.0, "ratio": 3.0, "knee": 6.0, "attack": 5.0, "release": 80.0, "makeup": 0.0}}
+
+
+def compressor_params(spec, rate: int) -> dict:
+    """{threshold, ratio, knee, attack, release, makeup} (float32 values, in vtts_compress's order) of a compressor
+    `spec` at `rate` Hz (an integer in [8000, 192000]).  `spec` is the preset `voice` (-24 dBFS threshold, 3:1 ratio,
+    6 dB knee, 5 ms attack, 80 ms release, 0 dB makeup), comma-separated key=value pairs over those six keys, or a dict
+    of them; keys left out take the voice preset.  threshold dBFS in [-60, 0], ratio in [1, 20], knee dB in [0, 24],
+    attack ms in [0.5, 200], release ms in [5, 5000], makeup dB in [-24, 24].  Raises ValueError naming the key."""
+    try:
+        r = float(rate)
+    except (TypeError, ValueError):
+        r = None
+    if r is None or not (8000 <= r <= 192000 and r == int(r)):
+        raise ValueError(f"compress: rate {rate} must be an integer in [8000, 192000]")
+    if isinstance(spec, str):
+        given = {}
+        s = spec.strip().lower()
+        if s not in COMPRESSOR_PRESETS:
+            for item in s.split(","):
+                key, eq, val = item.strip().partition("=")
+                if not eq:
+                    raise ValueError(f"compress: {item.strip()!r} is not key=value (keys {', '.join(COMPRESSOR_RANGES)}) "
+                                     f"or a preset ({', '.join(COMPRESSOR_PRESETS)})")
+                given[key.strip()] = val.strip()
+    elif isinstance(spec, dict):
+        given = dict(spec)
+    else:
+        raise ValueError(f"compress: a spec is a string or a dict, got {type(spec).__name__}")
+    out = dict(COMPRESSOR_PRESETS["voice"])
+    for key, val in given.items():
+        if key not in COMPRESSOR_RANGES:
+            raise ValueError(f"compress: unknown key {key!r} (keys {', '.join(COMPRESSOR_RANGES)})")
+        try:
+            v = float(np.float32(float(val)))
+        except (TypeError, ValueError):
+            raise ValueError(f"compress: {key}={val!r} is not a number") from None
+        lo, hi = COMPRESSOR_RANGES[key]
+        if not (np.isfinite(v) and lo <= v <= hi):
+            raise ValueError(f"compress: {key}={val} must lie in [{lo:g}, {hi:g}]")
+        out[key] = v
+    return out
+
+
 def _ptr(a):
     if a is None:
         return None
@@ -457,7 +504,7 @@ class Engine:
 
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
                         rng=None, output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None,
-                        gain_db=0.0, eq=None) -> "TtsStream":
+                        gain_db=0.0, eq=None, compress=None) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
         With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  `output_rate`: a resample
@@ -474,11 +521,15 @@ class Engine:
         `eq`: an equalizer spec or sos array (`eq_sections`), designed at the output rate; an equalizer stream follows the
         resampler (before the limiter and the meter) and the audio equals `equalize` of the (resampled) `tts` audio bit
         for bit.  It releases every sample it receives, so it adds no delay.
+        `compress`: a compressor spec (`compressor_params`); a compressor stream follows the equalizer (before the
+        limiter and the meter) at the output rate, and the audio equals `compress` of the (resampled, equalized) `tts`
+        audio bit for bit.  It also adds no delay.
         `meter=True`: a loudness meter runs last, on what `step()` returns at the output rate (a
         multiple of 10), and `TtsStream.meter()` gives each stepped slot's readings, read back in the step's one
         synchronisation.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
         return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate,
-                         denoise=denoise, meter=meter, semitones=semitones, tempo=tempo, limit=limit, gain_db=gain_db, eq=eq)
+                         denoise=denoise, meter=meter, semitones=semitones, tempo=tempo, limit=limit, gain_db=gain_db, eq=eq,
+                         compress=compress)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -1179,6 +1230,39 @@ class Engine:
         it brings (no lookahead), and a slot's outputs, concatenated, equal `equalize` of its whole input bit for bit."""
         return EqStream(self, max_streams, max_chunk_samples, eq, rate)
 
+    # ---- compressor (vtts_compress*: feed-forward soft-knee compressor, fp32) ----
+    def compress(self, wav, spec="voice", rate: int = config.SAMPLE_RATE, lengths=None):
+        """Host arrays: (y, reduction_db).  wav f32 [S] or [B,S] at `rate` through the compressor `spec` (see
+        `compressor_params`): a soft-knee gain computer on the log level, a smooth decoupled peak detector (release, then
+        attack) and the makeup gain.  reduction_db: the deepest gain reduction per row (<= 0, makeup excluded).  Rows
+        that stay below the knee come back exactly as wav times the makeup factor.  lengths int [B] in [0, S]: outputs
+        past lengths[b] are 0."""
+        p = compressor_params(spec, rate)
+        x, lens, one = _wav_rows(wav, lengths)
+        B, S = x.shape
+        y = np.zeros((B, S), np.float32)
+        red = np.zeros(B, np.float32)
+        if B and S:
+            self._ck(self.lib.vtts_compress_host(self.h, _ptr(x), _ptr(lens), B, S, int(rate), *p.values(), _ptr(y), _ptr(red)))
+        return (y[0], red[0]) if one else (y, red)
+
+    def compress_forward(self, x_t, spec="voice", rate: int = config.SAMPLE_RATE, lengths_t=None, out=None, reduction_db=None,
+                         stream=None):
+        """vtts_compress on torch CUDA tensors, stream-ordered and without a host synchronisation: returns (y [B,S],
+        reduction_db [B]), both on the device.  lengths_t int32 CUDA [B] or None.  `out` may be x_t (in place)."""
+        p = compressor_params(spec, rate)
+        B, S, out, st = _dev_rows(x_t, out, stream)
+        reduction_db = _out_tensor(reduction_db, (B,), x_t.device, "reduction_db")
+        self._ck(self.lib.vtts_compress(self.h, _ptr(x_t), _ptr(lengths_t), B, S, int(rate), *p.values(), _ptr(out), _ptr(reduction_db), st))
+        return out, reduction_db
+
+    def open_compressor_stream(self, max_streams: int, max_chunk_samples: int, spec="voice",
+                               rate: int = config.SAMPLE_RATE) -> "CompressorStream":
+        """Streaming compressor with `max_streams` independent slots (vtts_compressor_stream_*): every push releases every
+        sample it brings (no lookahead), and a slot's outputs, concatenated, equal `compress` of its whole input bit for
+        bit."""
+        return CompressorStream(self, max_streams, max_chunk_samples, spec, rate)
+
 
 class Loudness(NamedTuple):
     integrated: np.ndarray     # LUFS (gated, BS.1770-4)
@@ -1494,7 +1578,28 @@ class LoudnessMeter(_SlotStream):
         return y
 
 
-class LimiterStream(_SlotStream):
+class _ReductionStream(_SlotStream):
+    """A stream handle that also reports each slot's gain reduction so far: `reduction_db` after a host push, the
+    required reduction_t f32 CUDA [S] of a device push."""
+
+    def _outs(self, *dev):
+        """a host push: n_out and a new host reduction array; a device push: n_out and reduction_t, which must be a tensor"""
+        import torch
+        if not dev:
+            return super()._outs() + (np.empty(self.max_streams, np.float32),)
+        (red,) = dev
+        if (not isinstance(red, torch.Tensor) or tuple(red.shape) != (self.max_streams,) or red.dtype != torch.float32
+                or not red.is_contiguous()):
+            raise ValueError(f"reduction_t must be a contiguous float32 tensor [{self.max_streams}]")
+        return super()._outs() + (red,)
+
+    def _result(self, y, outs, host: bool):
+        if host:
+            self.reduction_db = outs[1]
+        return super()._result(y, outs, host)
+
+
+class LimiterStream(_ReductionStream):
     """Handle of a streaming limiter (Engine.open_limiter_stream): `gain_db=` with BEGIN (default 0 dB).  Before END a slot that has received P samples has released
     max(0, P - lookahead) outputs; a push with END releases the rest.  After every host push `reduction_db` holds each
     slot's deepest reduction over what it has released since BEGIN; `gain_db` holds each slot's pre-gain."""
@@ -1519,22 +1624,6 @@ class LimiterStream(_SlotStream):
         device) and gain_db (host scalar or [S], read for the slots that begin, default 0 dB)."""
         return self._push_device(x_t, n_new, flags, out_t, stream, gain_db, (reduction_t,))
 
-    def _outs(self, *dev):
-        """a host push: n_out and a new host reduction array; a device push: n_out and reduction_t, which must be a tensor"""
-        import torch
-        if not dev:
-            return super()._outs() + (np.empty(self.max_streams, np.float32),)
-        (red,) = dev
-        if (not isinstance(red, torch.Tensor) or tuple(red.shape) != (self.max_streams,) or red.dtype != torch.float32
-                or not red.is_contiguous()):
-            raise ValueError(f"reduction_t must be a contiguous float32 tensor [{self.max_streams}]")
-        return super()._outs() + (red,)
-
-    def _result(self, y, outs, host: bool):
-        if host:
-            self.reduction_db = outs[1]
-        return super()._result(y, outs, host)
-
 
 class EqStream(_SlotStream):
     """Handle of a streaming equalizer (Engine.open_eq_stream).  Every push releases every sample it brings:
@@ -1547,6 +1636,26 @@ class EqStream(_SlotStream):
         self.max_chunk_samples = self.out_pitch = self._chunk
         self.sos = eq_sections(eq, rate)
         self._create(eng.lib.vtts_eq_stream_create, self.max_streams, self.max_chunk_samples, _ptr(self.sos), self.sos.shape[0])
+
+
+class CompressorStream(_ReductionStream):
+    """Handle of a streaming compressor (Engine.open_compressor_stream).  Every push releases every sample it brings:
+    n_out = n_new (`push_device`: out_t may be x_t).  After every host push `reduction_db` holds each slot's deepest
+    reduction over what it has released since BEGIN."""
+    _kind = "compressor_stream"
+    lookahead = 0
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, spec="voice", rate: int = config.SAMPLE_RATE):
+        super().__init__(eng, max_streams, max_chunk_samples)
+        self.max_chunk_samples = self.out_pitch = self._chunk
+        self.params, self.rate = compressor_params(spec, rate), int(rate)
+        self._create(eng.lib.vtts_compressor_stream_create, self.max_streams, self.max_chunk_samples, self.rate, *self.params.values())
+        self.reduction_db = np.zeros(self.max_streams, np.float32)   # host pushes: each slot's reduction so far
+
+    def push_device(self, x_t, n_new, flags, out_t, reduction_t, stream=None) -> np.ndarray:
+        """As `_SlotStream.push_device`, with reduction_t f32 CUDA [S] (each slot's reduction so far, written on the
+        device)."""
+        return self._push_device(x_t, n_new, flags, out_t, stream, dev=(reduction_t,))
 
 
 def acoustic_stream_schedule(n_frames: int, n_emit: int | None, chunk: int, lookahead: int = 10) -> list:
@@ -1656,14 +1765,14 @@ class OptionError(ValueError):
 
 class AudioChain:
     """The audio stages after the vocoder, their options validated, in the one order every caller runs them: denoise,
-    pitch shift and time stretch at 16 kHz, then resample, equalize, limit (or normalize loudness) and meter at the
-    output rate.  `run` applies the chain to one waveform with the one-shot host calls; `streams` opens it as stream
+    pitch shift and time stretch at 16 kHz, then resample, equalize, compress, limit (or normalize loudness) and meter at
+    the output rate.  `run` applies the chain to one waveform with the one-shot host calls; `streams` opens it as stream
     stages.  `loudness` (a target in LUFS, reached under `true_peak`, or under the limiter's ceiling with `limit`) has no
     streaming form, and `meter` only measures, so `run` leaves the audio as it is for it.  Raises OptionError (a
     ValueError naming the option) for an option out of range."""
 
     def __init__(self, denoise=None, semitones=None, tempo=None, output_rate=None, eq=None, limit=None, gain_db=0.0,
-                 loudness=None, true_peak=None, meter=False):
+                 loudness=None, true_peak=None, meter=False, compress=None):
         def checked(option, check, *args):
             try:
                 return check(*args)
@@ -1676,6 +1785,7 @@ class AudioChain:
         self.semitones = None if semitones is None else float(checked("semitones", SEMITONES.rows, semitones, 1)[0])
         self.tempo = None if tempo is None else float(checked("tempo", TEMPO.rows, tempo, 1)[0])
         self.eq = None if eq is None else checked("eq", eq_sections, eq, self.rate)
+        self.compress = None if compress is None else checked("compress", compressor_params, compress, self.rate)
         self.limit = None if limit is None else checked("limit", _limit_args, limit, self.rate, 5.0, 100.0)[0]
         self.gain_db = float(checked("gain_db", GAIN_DB.rows, gain_db, 1)[0]) if limit is not None else 0.0
         self.loudness = self.true_peak = None
@@ -1696,6 +1806,8 @@ class AudioChain:
             (self.output_rate is not None, "rs", lambda e, w: e.resample(w, self.output_rate),
              lambda e, S, p, sec: ResampleStream(e, S, p, self.output_rate)),
             (self.eq is not None, "eq", lambda e, w: e.equalize(w, self.eq, r), lambda e, S, p, sec: EqStream(e, S, p, self.eq, r)),
+            (self.compress is not None, "cp", lambda e, w: e.compress(w, self.compress, r)[0],
+             lambda e, S, p, sec: CompressorStream(e, S, p, self.compress, r)),
             (self.loudness is not None, "lm",
              lambda e, w: e.normalize_loudness(w, self.loudness, r, true_peak=self.true_peak, limit=self.limit is not None)[0], None),
             (self.loudness is None and self.limit is not None, "lm", lambda e, w: e.limit(w, self.limit, r, self.gain_db)[0],
@@ -1734,14 +1846,15 @@ class TtsStream:
     options, each taking the previous one's output buffer, with a loudness meter of the audio `step()` returns last."""
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
-                 output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None, gain_db=0.0, eq=None):
+                 output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None, gain_db=0.0, eq=None,
+                 compress=None):
         import torch
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
         self._chain = AudioChain(denoise=denoise, semitones=semitones, tempo=tempo, output_rate=output_rate, eq=eq, limit=limit,
-                                 gain_db=gain_db, meter=meter)
+                                 gain_db=gain_db, meter=meter, compress=compress)
         self.eng = eng
-        self.rs = self.dn = self.ps = self.ts = self.eq = self.lm = self.mt = None
+        self.rs = self.dn = self.ps = self.ts = self.eq = self.cp = self.lm = self.mt = None
         S = max_streams
         self._built = []   # every stream handle, in construction order
         try:
@@ -1763,7 +1876,7 @@ class TtsStream:
         self._stages = []
         for st in self._built[2:]:
             kw = {} if st._param is None else {st._param.name: np.full(S, st._param.neutral, np.float32)}
-            if st is self.lm:
+            if isinstance(st, _ReductionStream):
                 kw["reduction_t"] = torch.zeros(S, dtype=torch.float32, device=dev)
             self._stages.append((st, torch.zeros((S, st._width), dtype=torch.float32, device=dev), kw))
         self._mout_h = None if self.mt is None else torch.zeros((S, 4), dtype=torch.float32).pin_memory()

@@ -19,6 +19,9 @@ normalizes every output to L LUFS (ITU-R BS.1770-4, Engine.normalize_loudness) a
 --true-peak at the rate it is written, after --output-rate.
 `--eq SPEC` equalizes every output on the device (Engine.equalize: high / low-pass, shelves, peaking and notch bands,
 or the `telephone` preset) at the rate it is written, after --output-rate and before --loudness / --limiter.
+`--compress SPEC` lowers the dynamic range of every output on the device (Engine.compress: a soft-knee feed-forward
+compressor, the `voice` preset or key=value settings) at the rate it is written, after --eq and before --loudness /
+--limiter, so the limiter only catches what the compressor leaves.
 """
 from __future__ import annotations
 
@@ -112,7 +115,7 @@ def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_
 
 # the command-line flag of each AudioChain option the CLI sets
 _FLAGS = {"denoise": "--denoise", "semitones": "--pitch", "tempo": "--tempo", "output_rate": "--output-rate", "eq": "--eq",
-          "limit": "--limiter", "loudness": "--loudness"}
+          "limit": "--limiter", "loudness": "--loudness", "compress": "--compress"}
 
 
 def main(argv=None) -> int:
@@ -151,6 +154,11 @@ def main(argv=None) -> int:
                              "--loudness / --limiter: comma-separated bands hp:F[:ORDER], lp:F[:ORDER], ls:F:GAIN[:S], "
                              "hs:F:GAIN[:S], pk:F:Q:GAIN, notch:F:Q, or 'telephone' (hp:300:4,lp:3400:4, the 300-3400 Hz "
                              "band); at most 8 second-order sections in all")
+    parser.add_argument("--compress", default=None, metavar="SPEC",
+                        help="compress the dynamic range of every output on the device at the output rate, after --eq and "
+                             "before --loudness / --limiter: 'voice' (-24 dBFS threshold, 3:1, 6 dB knee, 5 ms attack, 80 ms "
+                             "release, 0 dB makeup) or comma-separated threshold=, ratio=, knee=, attack=, release=, makeup= "
+                             "(keys left out keep the voice values)")
     parser.add_argument("--silence-duration", default=-1, type=float)
     parser.add_argument("--lexicon-file", default=None)
     parser.add_argument("--seed", default=None, type=int,
@@ -177,7 +185,7 @@ def main(argv=None) -> int:
     ceiling = -1.0 if args.true_peak is None else args.true_peak
     try:
         chain = AudioChain(denoise=args.denoise, semitones=args.pitch, tempo=args.tempo, output_rate=args.output_rate, eq=args.eq,
-                           limit=ceiling if args.limiter else None, loudness=args.loudness, true_peak=ceiling)
+                           limit=ceiling if args.limiter else None, loudness=args.loudness, true_peak=ceiling, compress=args.compress)
     except OptionError as e:
         parser.error(f"{_FLAGS[e.option]}: {e}")
     header_rate = args.output_rate or args.sample_rate or config.SAMPLE_RATE

@@ -2,7 +2,8 @@
 // conv kernel (strict fp32) or the tensor-core kernels of tc_conv.cu (bf16x3, or fp16 in VTTS_PRECISION_FP16).
 //
 //   conv_pre                              model.py:110
-//   per stage: lrelu(0.1) -> ups[i]       model.py:112-114   (u output phases, 2 taps each)
+//   per stage: lrelu(0.1) -> ups[i]       model.py:112-114   (u output phases, 2 taps each; one dense conv over blocks of
+//                                                               u output rows on the tensor cores)
 //              3 x ResBlock1, mean        model.py:115-121   (mean fused into the next consumer)
 //   lrelu(0.01) -> conv_post -> tanh      model.py:122-124   (conv_post_kernel below)
 #include "vtts_internal.cuh"
@@ -112,17 +113,30 @@ size_t vtts_hifigan_ws_bytes(int B, int T) {
 
 int vtts_hifigan_prepare(vtts_ctx* ctx) {
   ModelWeights& m = ctx->hg;
-  // derived: the transposed-conv weights of stage i repacked per output phase, [u][2][C][C/2]
-  std::vector<size_t> dn;
-  for (int i = 0, C = vc::HG_C0; i < 4; ++i, C /= 2) dn.push_back((size_t)vc::hg_rate(i) * 2 * C * (C / 2));
+  // derived, per stage i: the transposed-conv weights repacked per output phase, [u][2][C][C/2] (D_UPS_PH, the strict
+  // fp32 path), the same stacked per block of u output rows, [2][C][u][C/2] (D_UPS_BLK, see hg_ups), and the bias
+  // repeated per output row of the block, [u][C/2] (D_UPS_BLK_B)
+  std::vector<size_t> dn(12);
+  for (int i = 0, C = vc::HG_C0; i < 4; ++i, C /= 2) {
+    dn[D_UPS_PH(i)] = dn[D_UPS_BLK(i)] = (size_t)vc::hg_rate(i) * 2 * C * (C / 2);
+    dn[D_UPS_BLK_B(i)] = (size_t)vc::hg_rate(i) * (C / 2);
+  }
   int rc = vtts_alloc_tensors(ctx, dn, &m.derived, m.d);
   if (rc) return rc;
   std::vector<PackSpec> pk(2 * PK_COUNT);
   for (int i = 0, C = vc::HG_C0; i < 4; ++i, C /= 2) {
-    const int u = vc::hg_rate(i), K = vc::hg_upk(i);
-    repack_ups_kernel<<<256, 256>>>(m.t[hgi::UPS_W(i)], m.d[i], u, K, C, C / 2, (K + u - 2 + 1) / 2);
+    const int u = vc::hg_rate(i), K = vc::hg_upk(i), Co = C / 2;
+    repack_ups_kernel<<<256, 256>>>(m.t[hgi::UPS_W(i)], m.d[D_UPS_PH(i)], u, K, C, Co, (K + u - 2 + 1) / 2);
     VTTS_CUDA(cudaGetLastError());
-    for (int r = 0; r < u; ++r) pk[PK_UPS(i, r)] = {m.d[i] + (size_t)r * 2 * C * (C / 2), 2, C, C / 2};
+    // column block mm of the block weights is phase (mm + u/2) mod u: the first half of a block holds the late phases
+    // of one input row, the second half the early phases of the next
+    for (int mm = 0; mm < u; ++mm) {
+      const int r = (mm + u / 2) % u;
+      VTTS_CUDA(cudaMemcpy2D(m.d[D_UPS_BLK(i)] + (size_t)mm * Co, (size_t)u * Co * 4, m.d[D_UPS_PH(i)] + (size_t)r * 2 * C * Co, (size_t)Co * 4,
+                             (size_t)Co * 4, 2 * C, cudaMemcpyDeviceToDevice));
+      VTTS_CUDA(cudaMemcpy(m.d[D_UPS_BLK_B(i)] + (size_t)mm * Co, m.t[hgi::UPS_B(i)], (size_t)Co * 4, cudaMemcpyDeviceToDevice));
+    }
+    pk[PK_UPS(i)] = {m.d[D_UPS_BLK(i)], 2, C, u * Co};
   }
   for (int n = 0; n < 12; ++n)
     for (int which = 0; which < 2; ++which)
@@ -136,7 +150,7 @@ int vtts_hifigan_prepare(vtts_ctx* ctx) {
     pk[PK_COUNT + e].f16 = true;
   }
   // ---- tensor-core path: bf16 hi/lo split (and fp16) + canonical K-major packing of every dense conv ----
-  VTTS_CUDA(cudaDeviceSynchronize());  // the phase weights are packed from the repacked transposed-conv weights
+  VTTS_CUDA(cudaDeviceSynchronize());  // the block weights are packed from the repacked transposed-conv weights
   rc = vtts_pack_convs(ctx, m, pk);
   if (rc) return rc;
   VTTS_CUDA(cudaDeviceSynchronize());
@@ -206,35 +220,29 @@ int hg_ups(vtts_ctx* ctx, int i, const float* const* x, float* out, const int32_
     ConvProb p;
     memset(&p, 0, sizeof(p));
     if (i == 0) { p.x0 = x[0]; } else { p.x0 = x[0]; p.x1 = x[1]; p.x2 = x[2]; }
-    p.w = M.d[i] + (size_t)r * 2 * C * Co;
+    p.w = M.d[D_UPS_PH(i)] + (size_t)r * 2 * C * Co;
     p.bias = W[hgi::UPS_B(i)];
     p.out = out;
     p.k = 2; p.dil = 1; p.in_off = e; p.out_stride = u; p.out_off = r;
     L.p[r] = p;
   }
   if (!tc) return vtts_launch_conv(ctx, L, st);
-  // ConvTranspose phases share their input: for N <= 128 one converted activation tile feeds NPH phases
-  // (multi-phase tiles of tc_conv.cu); N = 256 keeps one problem per phase.
-  const int nph = Co == 256 ? 1 : (Co == 128 ? 4 : 2);
+  // Tensor cores: one dense two-tap conv over blocks of u output rows, so that every output phase shares one converted
+  // activation tile.  Phase r of input row tau reads x[tau - 1 + q] for r < u/2 and x[tau + q] for r >= u/2 (q = 0, 1),
+  // so block s, output rows u*s - u/2 .. u*s + u/2 - 1 (phases u/2.. of row s - 1, then phases ..u/2 - 1 of row s),
+  // reads x[s - 1] and x[s] with the stacked weights D_UPS_BLK: in_off = -1 over s = 0..rows_in.  In the [B][u*rows_in]
+  // [Co] output a block is one row of u*Co floats starting u/2 output rows early (out_e0); N <= 256 columns per problem.
+  const int N = vtts_tc_tile_n(u * Co), nt = u * Co / N;
   TcLaunch TL;
   memset(&TL, 0, sizeof(TL));
-  TL.nprob = u / nph; TL.nphase = nph; TL.Cin = C; TL.N = Co; TL.in_ld = C; TL.out_ld = Co;
-  TL.B = B; TL.T_rows = rows_in; TL.rows_out = rows_in * u; TL.len = n_frames; TL.len_mul = scale_in;
+  TL.nprob = nt; TL.Cin = C; TL.N = N; TL.in_ld = C; TL.out_ld = u * Co; TL.out_sub = Co;
+  TL.B = B; TL.T_rows = rows_in; TL.rows_out = rows_in * u; TL.tile_rows = rows_in + 1; TL.len = n_frames; TL.len_mul = scale_in;
   TL.pre_mode = L.pre_mode; TL.pre_slope = 0.1f; TL.f16 = f16;
-  for (int g = 0; g < u / nph; ++g) {
-    const ConvProb& c0 = L.p[g * nph];
-    TcProb q;
-    memset(&q, 0, sizeof(q));
-    q.x0 = c0.x0; q.x1 = c0.x1; q.x2 = c0.x2; q.bias = c0.bias; q.out = c0.out;
-    q.k = 2; q.dil = 1; q.out_stride = u;
-    q.wpk = M.tiles(pk + PK_UPS(i, g * nph))[0]; q.in_off = c0.in_off; q.out_off = g * nph;
-    for (int ph = 0; ph < nph; ++ph) {
-      const int r = g * nph + ph;
-      q.wpk_ph[ph] = M.tiles(pk + PK_UPS(i, r))[0];
-      q.in_off_ph[ph] = L.p[r].in_off;
-      q.out_off_ph[ph] = r;
-    }
-    TL.p[g] = q;
+  for (int g = 0; g < nt; ++g) {
+    TcProb& q = TL.p[g];
+    q.x0 = L.p[0].x0; q.x1 = L.p[0].x1; q.x2 = L.p[0].x2;
+    q.wpk = M.tiles(pk + PK_UPS(i))[g]; q.bias = M.d[D_UPS_BLK_B(i)] + g * N; q.out = out;
+    q.k = 2; q.dil = 1; q.in_off = -1; q.out_stride = 1; q.out_off = 0; q.out_e0 = -(u / 2) * Co + g * N;
   }
   return vtts_launch_tc_conv(ctx, TL, st);
 }

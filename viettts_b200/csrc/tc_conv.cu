@@ -84,15 +84,14 @@ struct Ring {
 // would run one problem only.  The weight-producer lane of each CTA takes tickets from a launch-wide counter and passes
 // every ticket on to the CTA's other roles through the NQ-slot tile-id ring (-1 ends the launch).
 //
-// Ticket order is (batch row, row tile) major, problem, then output phase minor, with the problems sorted by k,
-// descending: CTAs running at the same time work on the same rows, so an input several problems share (the first pair
-// of a ResBlock stage, the ConvTranspose problems) is read from DRAM once and served from L2 to the others.
+// Ticket order is (batch row, row tile) major, problem minor, with the problems sorted by k, descending: CTAs running at
+// the same time work on the same rows, so an input several problems share (the first pair of a ResBlock stage, the
+// column groups of a ConvTranspose) is read from DRAM once and served from L2 to the others.
 struct Tile {
-  int pi, b, tt, ph;   // problem, batch row, row tile, output phase
+  int pi, b, tt;   // problem, batch row, row tile
 };
-__device__ __forceinline__ Tile decode_tile(int t, int nph, int nprob, int tiles_per_row) {
+__device__ __forceinline__ Tile decode_tile(int t, int nprob, int tiles_per_row) {
   Tile d;
-  d.ph = t % nph; t /= nph;
   d.pi = t % nprob; t /= nprob;
   d.tt = t % tiles_per_row;
   d.b = t / tiles_per_row;
@@ -320,6 +319,12 @@ __device__ __forceinline__ TileQueue tile_queue(uint64_t* bars, int nw) {
   return TileQueue{reinterpret_cast<int*>(q_full + 2 * NQ), q_full, q_full + NQ, Ring{}};
 }
 
+// sub-row output (TcLaunch::out_sub): the element of the batch row's output that column col of tile row tau of problem
+// P goes to
+__device__ __forceinline__ int sub_elem(const TcLaunch& L, const TcProb& P, int tau, int col) {
+  return (tau * P.out_stride + P.out_off) * L.out_ld + P.out_e0 + col;
+}
+
 // Tile loops of the roles.  The producer lane takes tickets one tile ahead of the tile it streams weights for, so the
 // converters learn their next tile before they finish the current one.
 #define PRODUCER_TILES                                                                     \
@@ -338,9 +343,11 @@ __device__ __forceinline__ TileQueue tile_queue(uint64_t* bars, int nw) {
   auto next_tile = [&]() { return q.get(L.err, w_q); };
 
 // EPI = 0: bias (+ residual) only -- the HiFiGAN generator's hot path.  EPI = 1: bias, eval BatchNorm,
-// tanh / relu, residual, partial N tile (acoustic model convs and GEMMs).
-template <int N, int EPI, int MW, bool F16>
+// tanh / relu, residual, partial N tile (acoustic model convs and GEMMs).  SUB: sub-row output (TcLaunch::out_sub, EPI 0
+// only, the ConvTranspose); a template flag so that the ResBlock launches keep their epilogue as it is.
+template <int N, int EPI, int MW, bool F16, bool SUB>
 __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_constant__ TcLaunch L) {
+  static_assert(!SUB || EPI == 0, "sub-row output uses the plain epilogue");
   using Cfg = TcCfg<N, MW, 0, EPI == 0>;
   constexpr int R = Cfg::R, RA = Cfg::RA, NW = Cfg::NW;
   extern __shared__ uint8_t smem_raw[];
@@ -361,29 +368,32 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
   __syncthreads();
 
   const int nch = L.Cin / 16;
-  const int nph = L.nphase > 1 ? L.nphase : 1;
 
-  // every role walks the same tile sequence (next_tile); a tile is (problem, batch row, row tile, output phase).
+  // every role walks the same tile sequence (next_tile); a tile is (problem, batch row, row tile).
   // Input rows outside [in_lo, valid) read as zero.  Output row tau is written while tau < valid, or, with per-row
   // bounds (TcProb::rb, plain epilogue only), while its output row tau * out_stride + out_off stays below out_hi.
+  // SUB bounds each out_sub-float output row of a tile row instead: an element e of the batch row's output is written
+  // iff 0 <= e < e_lim, e_lim = out_sub x (the first output row not written).
   constexpr bool ROW_BOUNDS = EPI == 0;
 #define TILE_LOOP_BEGIN                                                           \
   for (int tile; (tile = next_tile()) >= 0;) {                                    \
-    const Tile td = decode_tile(tile, nph, L.nprob, L.tiles_per_row);              \
-    const int ph = td.ph, b = td.b;                                                 \
+    const Tile td = decode_tile(tile, L.nprob, L.tiles_per_row);                   \
+    const int b = td.b;                                                            \
     const int tau0 = td.tt * R;                                                    \
     const TcProb& P = L.p[td.pi];                                                  \
     int valid = L.T_rows, in_lo = 0, out_hi = 0;                                  \
     if (ROW_BOUNDS && P.rb) {                                                     \
       in_lo = P.rb[3 * b]; valid = P.rb[3 * b + 1]; out_hi = P.rb[3 * b + 2];     \
-      if (tau0 * P.out_stride + P.out_off_ph[ph] >= out_hi) continue;             \
+      if (!SUB && tau0 * P.out_stride + P.out_off >= out_hi) continue;            \
     } else {                                                                      \
       if (L.len) {                                                                \
         const int v = L.len[b] * L.len_mul;                                       \
         valid = v < valid ? v : valid;                                            \
       }                                                                           \
-      if (tau0 >= valid) continue;                                                \
-    }
+      if (!SUB && tau0 >= valid) continue;                                        \
+    }                                                                             \
+    const int e_lim = SUB ? (P.rb ? out_hi * L.out_sub : valid * L.out_ld) : 0;   \
+    if (SUB && sub_elem(L, P, tau0, 0) >= e_lim) continue;
 #define TILE_LOOP_END }
 
   if (warp == PROD_WARP) {
@@ -393,8 +403,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
       long long w_e = 0;
       PRODUCER_TILES
       TILE_LOOP_BEGIN
-        (void)b; (void)tau0; (void)in_lo; (void)valid; (void)out_hi;
-        produce_weights<N, NW, F16>(w_st, w_full, w_empty, rw, P.wpk_ph[ph], nch, P.k, L.err, w_e);
+        (void)b; (void)tau0; (void)in_lo; (void)valid; (void)out_hi; (void)e_lim;
+        produce_weights<N, NW, F16>(w_st, w_full, w_empty, rw, P.wpk, nch, P.k, L.err, w_e);
       TILE_LOOP_END
       if (L.dbg) L.dbg[(size_t)blockIdx.x * 16 + 4] = w_e;
     }
@@ -411,13 +421,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
       const float* x2 = L.pre_mode == 2 ? P.x2 + in_base : nullptr;
       for (int c = 0; c < nch; ++c) {
         mbar_wait_t(&a_empty[ra.s], ra.p ^ 1, L.err, 5, w_ae);
-        convert_chunk<RA, F16>(a_st + ra.s * Cfg::A_STAGE, ct, P.x0 + in_base, x1, x2, L.in_ld, c, tau0 + P.in_off_ph[ph], R + (k - 1) * dil,
+        convert_chunk<RA, F16>(a_st + ra.s * Cfg::A_STAGE, ct, P.x0 + in_base, x1, x2, L.in_ld, c, tau0 + P.in_off, R + (k - 1) * dil,
                           in_lo, valid, L.pre_mode, L.pre_slope);
         fence_proxy_async();
         mbar_arrive(&a_full[ra.s]);
         ra.next<NA>();
       }
-      (void)out_hi;
+      (void)out_hi; (void)e_lim;
     TILE_LOOP_END
     if (L.dbg && ct == 0) L.dbg[(size_t)blockIdx.x * 16 + 5] = w_ae;
   } else {
@@ -438,10 +448,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
     const int dr = (tid & 127) / (EPI_NC / 4), dq = (tid & 127) % (EPI_NC / 4);
     READER_TILES
     TILE_LOOP_BEGIN
-      const size_t out_base = (size_t)b * L.rows_out * L.out_ld;
-      const int ostride = P.out_stride, ooff = P.out_off_ph[ph];
+      const size_t out_base = (size_t)b * L.rows_out * (SUB ? L.out_sub : L.out_ld);
+      const int ostride = P.out_stride, ooff = P.out_off, oe0 = SUB ? P.out_e0 : 0;
       // output row tau is stored while it is valid; the condition is monotone in tau
       auto row_ok = [&](int tau) { return (ROW_BOUNDS && P.rb) ? tau * ostride + ooff < out_hi : tau < valid; };
+      // ... and the float4 at element e (of tile row tau) of the batch row's output (plain epilogue); with sub-row output
+      // it lies in one output row (out_sub % 4 == 0)
+      auto elem_ok = [&](int tau, int e) { return SUB ? e >= 0 && e < e_lim : row_ok(tau); };
       // cp.async the residual of pass (mt, nh) -- rows tau0 + (wg * MW + mt) * 64..., columns nh * EPI_NC... -- into
       // the staging rows; wait_pass makes every thread's copies visible to the warpgroup
       auto fetch_pass = [&](int mt, int nh) {
@@ -450,8 +463,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
 #pragma unroll
           for (int i = 0; i < NQ4; ++i) {
             const int row = i * RPS + dr, tau = blk + row;
-            if (row_ok(tau))
-              cp_async16(stg + row * EPI_LD + dq * 4, P.resid + out_base + ((tau * ostride + ooff) * L.out_ld + nh * EPI_NC + dq * 4));
+            const int e = (tau * ostride + ooff) * L.out_ld + oe0 + nh * EPI_NC + dq * 4;
+            if (elem_ok(tau, e)) cp_async16(stg + row * EPI_LD + dq * 4, P.resid + out_base + e);
           }
         }
         cp_async_commit();
@@ -478,7 +491,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
         wait_pass();
 #pragma unroll
         for (int mt = 0; mt < MW; ++mt) {
-          if (!row_ok(tau0 + (wg * MW + mt) * 64)) break;   // uniform over the warpgroup: no later row of it is stored
+          // uniform over the warpgroup: past the last output row, so no later row of it is stored
+          const int blk = tau0 + (wg * MW + mt) * 64;
+          if (SUB ? sub_elem(L, P, blk, 0) >= e_lim : !row_ok(blk)) break;
 #pragma unroll
           for (int nh = 0; nh < N / EPI_NC; ++nh) {
             if (mt + nh > 0 && P.resid) {
@@ -501,13 +516,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
               }
             }
             named_bar(2 + wg, 128);
-            const int blk = tau0 + (wg * MW + mt) * 64;
 #pragma unroll
             for (int i = 0; i < NQ4; ++i) {
               const int row = i * RPS + dr, tau = blk + row;
-              if (row_ok(tau))
-                *reinterpret_cast<float4*>(P.out + out_base + ((tau * ostride + ooff) * L.out_ld + nh * EPI_NC + dq * 4)) =
-                    *reinterpret_cast<const float4*>(stg + row * EPI_LD + dq * 4);
+              const int e = (tau * ostride + ooff) * L.out_ld + oe0 + nh * EPI_NC + dq * 4;
+              if (elem_ok(tau, e))
+                *reinterpret_cast<float4*>(P.out + out_base + e) = *reinterpret_cast<const float4*>(stg + row * EPI_LD + dq * 4);
             }
             named_bar(2 + wg, 128);   // stored before the next pass or tile rewrites the staging rows
           }
@@ -582,7 +596,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_pair_kernel(const __grid_const
 
 #define TILE_LOOP_BEGIN                                                   \
   for (int tile; (tile = next_tile()) >= 0;) {                            \
-    const Tile td = decode_tile(tile, 1, L.nprob, L.tiles_per_row);        \
+    const Tile td = decode_tile(tile, L.nprob, L.tiles_per_row);        \
     const int b = td.b;                                                    \
     const int tau0 = td.tt * R_OUT;                                        \
     int valid = L.T_rows;                                                 \
@@ -722,29 +736,22 @@ __global__ void pack_w_kernel(const float* __restrict__ w, uint16_t* __restrict_
   }
 }
 
-template <int N, int EPI, int MW, bool F16>
+template <int N, int EPI, int MW, bool F16, bool SUB = false>
 int launch_cfg(vtts_ctx* ctx, TcLaunch& L, cudaStream_t st) {
   using Cfg = TcCfg<N, MW, 0, EPI == 0>;
   static bool attr_done_dev[64] = {};   // function attributes are per device (a process may hold contexts on several GPUs)
   if (!attr_done_dev[ctx->device & 63]) {
-    VTTS_CUDA(cudaFuncSetAttribute(tc_conv_kernel<N, EPI, MW, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    VTTS_CUDA(cudaFuncSetAttribute(tc_conv_kernel<N, EPI, MW, F16, SUB>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_done_dev[ctx->device & 63] = true;
   }
-  const int nph = L.nphase > 1 ? L.nphase : 1;
-  for (int i = 0; i < L.nprob; ++i) {
-    if (nph == 1) {   // single-phase problems describe themselves with the scalar fields
-      L.p[i].wpk_ph[0] = L.p[i].wpk;
-      L.p[i].in_off_ph[0] = L.p[i].in_off;
-      L.p[i].out_off_ph[0] = L.p[i].out_off;
-    }
+  for (int i = 0; i < L.nprob; ++i)
     if ((L.p[i].k - 1) * L.p[i].dil > HALO) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: halo too large");
-  }
   // the expensive problems (large k) first: within each row tile they are handed out before the cheap ones
   std::stable_sort(L.p, L.p + L.nprob, [](const TcProb& a, const TcProb& b) { return a.k > b.k; });
   L.tiles_per_row = ((L.tile_rows > 0 ? L.tile_rows : L.T_rows) + Cfg::R - 1) / Cfg::R;
-  L.ntiles = L.nprob * L.tiles_per_row * L.B * nph;
+  L.ntiles = L.nprob * L.tiles_per_row * L.B;
   const int grid = L.ntiles < ctx->sm_count ? L.ntiles : ctx->sm_count;
-  tc_conv_kernel<N, EPI, MW, F16><<<grid, NTHREADS, Cfg::SMEM_BYTES, st>>>(L);
+  tc_conv_kernel<N, EPI, MW, F16, SUB><<<grid, NTHREADS, Cfg::SMEM_BYTES, st>>>(L);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   return VTTS_OK;
@@ -760,21 +767,24 @@ int launch_n(vtts_ctx* ctx, TcLaunch& L, cudaStream_t st) {
     generic |= L.p[i].bn_mean != nullptr;
     rb |= L.p[i].rb != nullptr;
   }
-  if (rb && generic) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: per-row bounds use the plain epilogue");
+  if ((rb || L.out_sub) && generic) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: per-row bounds and sub-row output use the plain epilogue");
+  // a float4 of the plain epilogue lies in one output row
+  if (L.out_sub < 0 || (L.out_sub && (L.out_sub % 4 || L.out_ld % L.out_sub)))
+    return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: output rows of %d floats in tile rows of %d", L.out_sub, L.out_ld);
   if (!generic) {
     // the plain epilogue copies the bias and the residual and stores the output in float4 row segments, at 32-bit
     // offsets within a batch row
-    if ((int64_t)L.rows_out * L.out_ld > INT32_MAX) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: %d output rows of %d", L.rows_out, L.out_ld);
+    const int row_w = L.out_sub ? L.out_sub : L.out_ld;
+    if ((int64_t)L.rows_out * row_w > INT32_MAX) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: %d output rows of %d", L.rows_out, row_w);
     bool aligned = L.out_ld % 4 == 0;
     for (int i = 0; i < L.nprob; ++i) aligned &= (((uintptr_t)L.p[i].out | (uintptr_t)L.p[i].resid | (uintptr_t)L.p[i].bias) & 15) == 0;
     if (!aligned) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: the plain epilogue needs 16-byte aligned out / resid rows and bias (out_ld %d)", L.out_ld);
   }
-  if (L.nphase > 4) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: %d phases", L.nphase);
-  if (L.nphase > 1 && generic) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: multi-phase tiles use the plain epilogue");
   // fp16 operands serve the generator, whose convs all use the plain epilogue
   if (L.f16 && generic) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: fp16 operands use the plain epilogue");
-  if (L.f16) return launch_cfg<N, 0, MW, true>(ctx, L, st);
-  return generic ? launch_cfg<N, 1, MW, false>(ctx, L, st) : launch_cfg<N, 0, MW, false>(ctx, L, st);
+  if (L.f16) return L.out_sub ? launch_cfg<N, 0, MW, true, true>(ctx, L, st) : launch_cfg<N, 0, MW, true>(ctx, L, st);
+  if (generic) return launch_cfg<N, 1, MW, false>(ctx, L, st);
+  return L.out_sub ? launch_cfg<N, 0, MW, false, true>(ctx, L, st) : launch_cfg<N, 0, MW, false>(ctx, L, st);
 }
 
 template <int N, int MW, bool A2_REGS, bool F16 = false>

@@ -272,11 +272,17 @@ int vtts_vocoder_stream_push(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float
   int* tb = vs->tbl.data();
   int tile_rows[NCONV];
   std::fill(tile_rows, tile_rows + NCONV, 1);   // every launch is issued every push (a fixed launch count); idle rows skip their tiles
+  // ConvTranspose of stage i in block form (hifigan.cu hg_ups): block tau covers rows ups_out0(i) + u * tau .. + u - 1,
+  // phases u/2.. of input row tau - 1 and ..u/2 - 1 of input row tau, and reads both.  Input row tau <-> input time
+  // rate * P_old - lag_in - 1 + tau.  Block 0 also rewrites rows already final in the last push, from the same input
+  // rows: same bits.
+  auto ups_out0 = [&](int i) { return pl.lead[i + 1] - pl.lag_x[i] + pl.late[i] - vc::hg_rate(i) - vc::hg_rate(i) / 2; };
+  auto ups_in_off = [&](int i) { return pl.lead[i] - pl.lag_in[i] - 2; };
   // conv c reads rate ri_in (inputs final up to lag_in) and writes rate ri_out with lag lag_out; its output tau <-> row
-  // out_off + tau (phases: out_off + u * tau + r, r < u)
+  // out0 + tau (ConvTranspose: the block of rows out0 + u * tau .. + u - 1)
   auto bounds = [&](int c, int ri_in, int lag_in, int ri_out, int lag_out, int u) {
     const int sin = pl.rate[ri_in], sout = pl.rate[ri_out];
-    const int out0 = u > 1 ? pl.lead[ri_out] - lag_out + pl.late[ri_in] - u : pl.lead[ri_out] - lag_out;   // first row written by tau = 0
+    const int out0 = u > 1 ? ups_out0(ri_in) : pl.lead[ri_out] - lag_out;   // first row written by tau = 0
     for (int s = 0; s < S; ++s) {
       if (!act[s]) continue;
       int* r = tb + ((size_t)c * S + s) * 3;
@@ -349,28 +355,22 @@ int vtts_vocoder_stream_push(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float
 
   for (int i = 0, C = vc::HG_C0; i < 4; ++i, C /= 2) {
     const int u = vc::hg_rate(i), Co = C / 2;
-    // ---- lrelu(0.1) [of the 3-way mean for i > 0] -> ConvTranspose phases; tau <-> input time rate * P_old - lag_in - 1 + tau ----
-    const int nph = Co == 256 ? 1 : (Co == 128 ? 4 : 2);
+    // ---- lrelu(0.1) [of the 3-way mean for i > 0] -> ConvTranspose as one conv over blocks of u output rows ----
+    const int N = vtts_tc_tile_n(u * Co), nt = u * Co / N;
     memset(&TL, 0, sizeof(TL));
-    TL.nprob = u / nph; TL.nphase = nph; TL.Cin = C; TL.N = Co; TL.in_ld = C; TL.out_ld = Co;
+    TL.nprob = nt; TL.Cin = C; TL.N = N; TL.in_ld = C; TL.out_ld = u * Co; TL.out_sub = Co;
     TL.B = S; TL.T_rows = vs->cap[i]; TL.rows_out = vs->cap[i + 1]; TL.tile_rows = tile_rows[ci_ups(i)];
     TL.pre_mode = i == 0 ? 1 : 2; TL.pre_slope = 0.1f; TL.f16 = f16;
-    for (int g = 0; g < u / nph; ++g) {
+    for (int g = 0; g < nt; ++g) {
       TcProb& q = TL.p[g];
       if (i == 0) {
         q.x0 = T[1].p;
       } else {
         q.x0 = T[ti_y(i - 1, 0, 2)].p; q.x1 = T[ti_y(i - 1, 1, 2)].p; q.x2 = T[ti_y(i - 1, 2, 2)].p;
       }
-      q.bias = W[hgi::UPS_B(i)]; q.out = T[ti_x(i)].p; q.k = 2; q.dil = 1; q.out_stride = u; q.rb = rb(ci_ups(i));
-      for (int ph = 0; ph < nph; ++ph) {
-        const int r = g * nph + ph;
-        q.wpk_ph[ph] = M.tiles(pk + PK_UPS(i, r))[0];
-        q.in_off_ph[ph] = pl.lead[i] - pl.lag_in[i] - 1 + ups_e(i, r);
-        // tau = 0 also rewrites the u - late phases already final in the last push, with the same inputs: same bits
-        q.out_off_ph[ph] = pl.lead[i + 1] - pl.lag_x[i] + pl.late[i] - u + r;
-      }
-      q.wpk = q.wpk_ph[0]; q.in_off = q.in_off_ph[0]; q.out_off = q.out_off_ph[0];
+      q.wpk = M.tiles(pk + PK_UPS(i))[g]; q.bias = M.d[D_UPS_BLK_B(i)] + g * N; q.out = T[ti_x(i)].p;
+      q.k = 2; q.dil = 1; q.in_off = ups_in_off(i); q.out_stride = 1; q.out_off = 0; q.out_e0 = ups_out0(i) * Co + g * N;
+      q.rb = rb(ci_ups(i));
     }
     if ((rc = vtts_launch_tc_conv(ctx, TL, st))) return rc;
 

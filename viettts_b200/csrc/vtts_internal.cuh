@@ -84,12 +84,7 @@ struct TcProb {
   const float* bn_off;
   float* out;
   int k, dil, in_off, out_stride, out_off;
-  // multi-phase tiles (TcLaunch::nphase > 1): phase ph of this problem uses weights wpk_ph[ph], reads input rows
-  // shifted by in_off_ph[ph] and writes output rows tau*out_stride + out_off_ph[ph]; one converted activation
-  // tile feeds all phases (ConvTranspose output phases share their input)
-  const void* wpk_ph[4];
-  int in_off_ph[4];
-  int out_off_ph[4];
+  int out_e0;            // signed element offset of the output and residual addresses (TcLaunch::out_sub)
   // optional per-batch-row bounds [B][3] (device int32): input rows outside [rb[3b], rb[3b+1]) read as zero, and output
   // row tau*out_stride + out_off is written only below rb[3b+2].  Null: rows [0, valid) of the launch for both
   // (vocoder_stream.cu runs "valid" convs over per-slot windows, whose input and output ranges differ)
@@ -106,7 +101,12 @@ struct TcLaunch {
   int len_mul;
   int pre_mode;
   float pre_slope;
-  int nphase;            // phases per tile (1, 2 or 4); 0 means 1
+  // sub-row output (plain epilogue only; 0 = off): a tile row is a block of out_ld / out_sub output rows of out_sub
+  // floats, and rows_out counts such rows.  Column col of tile row tau of a problem is element
+  // e = (tau*out_stride + out_off)*out_ld + out_e0 + col of the batch row's output, i.e. output row e / out_sub; it is
+  // written only if e >= 0 and that row is below valid * out_ld / out_sub (or below rb[3b+2]).  The ConvTranspose runs
+  // as such a dense conv over blocks of output rows (hifigan.cu hg_ups).
+  int out_sub;
   int post_act;          // 0 none, 1 tanh, 2 relu (after BN, before the residual)
   int n_valid;           // real output channels of this N tile (<= N); 0 means N
   int f16;               // operand format: 0 = bf16 hi/lo planes, three products (bf16x3); 1 = one fp16 plane, one product
@@ -447,13 +447,19 @@ constexpr int POST_W = 10 + 12 * 12, POST_B = POST_W + 1;
 constexpr int COUNT = POST_B + 1;
 }  // namespace hgi
 
-// packing table of the generator (ctx->hg.tiles): the 72 ResBlock convs in hgi order, the ConvTranspose output phases
-// of the four stages, conv_pre (two N = 256 tiles) as bf16 hi/lo planes; then the same PK_COUNT entries again as fp16
+// packing table of the generator (ctx->hg.tiles): the 72 ResBlock convs in hgi order, the ConvTranspose of the four
+// stages in block form (hifigan.cu hg_ups: a two-tap conv of hg_rate(i) * C/2 columns, N = 256 / 256 / 128 / 64, so
+// 8 / 4 / 1 / 1 tiles), conv_pre (two N = 256 tiles) as bf16 hi/lo planes; then the same PK_COUNT entries again as fp16
 // planes (VTTS_PRECISION_FP16): entry e + PK_COUNT is the fp16 copy of entry e
 namespace hgpk {
 constexpr int PK_RB(int n, int which, int m) { return n * 6 + which * 3 + m; }
-constexpr int PK_UPS(int i, int r) { return i == 0 ? 72 + r : PK_UPS(i - 1, vc::hg_rate(i - 1)) + r; }
-constexpr int PK_PRE = PK_UPS(4, 0), PK_COUNT = PK_PRE + 1;
+constexpr int PK_UPS(int i) { return 72 + i; }
+constexpr int PK_PRE = PK_UPS(4), PK_COUNT = PK_PRE + 1;
+// derived tensors (ctx->hg.d) of stage i's ConvTranspose: weights per output phase, the same stacked per block of
+// output rows, and the bias of a block (vtts_hifigan_prepare)
+constexpr int D_UPS_PH(int i) { return i; }
+constexpr int D_UPS_BLK(int i) { return 4 + i; }
+constexpr int D_UPS_BLK_B(int i) { return 8 + i; }
 }  // namespace hgpk
 
 // indices into ctx->ac.t

@@ -156,8 +156,9 @@ int vtts_melspec(vtts_ctx* ctx, const float* wav_dev, int B, int S, float* mel_d
  * "mel_pre" [B,N,80] (before the postnet, = mel1 of the teacher-forced pass; after an acoustic stream push: the stream's
  * [max_streams, max_frames, 80] projection outputs, valid for the frames each slot has scanned), "dec_in" [B,N,768]
  * (teacher-forced decoder input [cond | prenet(mels_in)]), "dec_out" [B,N,1024] (decoder scan output [h0 | h1], before
- * zoneout; autoregressive and teacher-forced pass).  Each call sets every tap, to nothing where it produces none; a
- * call that grows the workspace, and destroying the stream a mel_pre tap points into, clear them all.  Reading a tap
+ * zoneout; autoregressive and teacher-forced pass), "dur_hidden" [B,L,256] (duration call: the first Linear's output,
+ * bias included, before gelu: the duration head's input; like "enc", unspecified past lengths[b]).  Each call sets
+ * every tap, to nothing where it produces none; a call that grows the workspace, and destroying the stream a mel_pre tap points into, clear them all.  Reading a tap
  * that is not set fails with VTTS_ERR_BAD_ARG before any copy. */
 int vtts_debug_read(vtts_ctx* ctx, const char* name, float* host_out, int64_t n_floats);
 

@@ -175,10 +175,20 @@ def inference(ckpt, tokens, durations_frames, n_frames: int, masks=None, dtype=t
         return x + res
 
 
+def frame_count(frames):
+    """n_frames = int(sum(durations)) of text2mel.py:79 for one row of float32 frame durations: the sum in float64,
+    term by term in token order, rounded to float32 once, truncated.  The reference's `jnp.sum` leaves the order to
+    XLA; the float64 sum of float32 terms is exact for any realistic row, so this count does not depend on it."""
+    total = 0.0
+    for f in np.asarray(frames, np.float32).ravel().tolist():
+        total += f
+    return int(np.float32(total))
+
+
 def seconds_to_frames(durations_sec):
-    """text2mel.py:78-79: float32 `durations * 16000 / 256`, n_frames=int(sum)."""
+    """text2mel.py:78-79: float32 `durations * 16000 / 256`, n_frames = frame_count."""
     d = (np.asarray(durations_sec, np.float32) * np.float32(16000)) / np.float32(256)
-    return d, int(np.sum(d, dtype=np.float32))
+    return d, frame_count(d)
 
 
 def predict_mel(ckpt, tokens, durations_sec, masks=None, dtype=torch.float32):
@@ -194,7 +204,7 @@ def inference_ragged(ckpt, tokens_list, dur_frames_list, masks_list=None, dtype=
     outs = []
     for b, (tk, d) in enumerate(zip(tokens_list, dur_frames_list)):
         d = np.asarray(d, np.float32)[None, :]
-        n = int(np.sum(d, dtype=np.float32))
+        n = frame_count(d)
         m = None if masks_list is None else np.asarray(masks_list[b])[None, :n]
         outs.append(inference(ckpt, np.asarray(tk, np.int32)[None, :], d, n, m, dtype)[0].numpy())
     return outs

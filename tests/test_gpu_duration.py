@@ -2,8 +2,10 @@
 (SURVEY.md §8f row 1: the callers of predict_mel).
 
 Oracle status: pinned to the reference's own source (tests/test_reference_goldens.py; the CUDA path is also compared
-with the reference-produced durations directly in tests/test_gpu_reference_goldens.py).  Tolerance: predicted durations are
-O(0.1 s); |gpu - float64 oracle| <= 2e-5 s in both arithmetic modes (the recurrent part is fp32 in both)."""
+with the reference-produced durations directly in tests/test_gpu_reference_goldens.py).  Tolerance, per token:
+|gpu - float64 oracle| <= E2E_UNITS[mode] units of 2^-24 (sigmoid(s) sum_i |gelu(y_i) w2_i| + softplus(s)), the unit of
+the head's own bound (tests/test_gpu_duration_stages.py), at most 1.1e-5 s on these rows; tests/test_duration_bounds.py
+derives it from the plain fp32 oracle.  The stages one by one are pinned in tests/test_gpu_duration_stages.py."""
 import json
 import pickle
 
@@ -13,10 +15,19 @@ import torch
 
 from oracle import hifigan_oracle as ho
 from oracle import nat_oracle as no
+from test_gpu_duration_stages import E2E_UNITS, e2e_ref
 from viettts_b200 import config, synthetic
 
 pytestmark = pytest.mark.gpu
-DUR_TOL = 2e-5
+
+
+def within_bound(eng, ckpt, tokens, lengths, got):
+    """|got - float64| <= E2E_UNITS units on every token < lengths[b] of tokens [B,L]; returns the worst in units"""
+    ref, unit = e2e_ref(ckpt, tokens, np.asarray(lengths))
+    valid = np.arange(tokens.shape[1])[None, :] < np.asarray(lengths)[:, None]
+    u = np.where(valid, np.abs(got - ref) / unit, 0.0)
+    assert (u <= E2E_UNITS[eng.mode]).all(), (np.argwhere(u > E2E_UNITS[eng.mode])[:4], float(u.max()))
+    return float(u.max())
 
 
 @pytest.fixture(scope="module")
@@ -32,6 +43,7 @@ def eng(duration_ckpt, acoustic_ckpt, hifigan_params, request):
     e.load_acoustic(acoustic_ckpt)
     e.load_hifigan(hifigan_params)
     e.set_precision(request.param)
+    e.mode = request.param
     yield e
     e.close()
 
@@ -52,16 +64,16 @@ def test_single_utterance_vs_oracle(eng, duration_ckpt):
     print(f"duration: gpu-vs-f64 {np.abs(got-ref64).max():.3e}  f32-vs-f64 {np.abs(ref32-ref64).max():.3e}  enc {np.abs(enc-enc_ref).max():.3e}")
     assert got.shape == (1, 100) and got.dtype == np.float32
     assert np.abs(enc - enc_ref).max() < 1e-4
-    assert np.abs(got - ref64).max() < DUR_TOL
+    print(f"duration: gpu-vs-f64 {within_bound(eng, duration_ckpt, tk[None], [100], got):.2f} units")
 
 
 def test_reference_shape_case(eng, duration_ckpt):
     """tests/test_nat_duration.py's input (all-zero tokens, B=2, L=10)."""
     tok = np.zeros((2, 10), np.int32)
     got = eng.predict_duration(tok)
-    ref = no.duration_model(duration_ckpt, tok, np.array([10, 10]), dtype=torch.float64)
     assert got.shape == (2, 10)
-    assert np.abs(got - ref).max() < DUR_TOL and np.array_equal(got[0], got[1])
+    within_bound(eng, duration_ckpt, tok, [10, 10], got)
+    assert np.array_equal(got[0], got[1])
 
 
 def test_ragged_batch_rows_equal_single_runs(eng, duration_ckpt):
@@ -76,8 +88,7 @@ def test_ragged_batch_rows_equal_single_runs(eng, duration_ckpt):
     got = eng.predict_duration(tok, lengths=lens)
     for b, n in enumerate(lens):
         assert np.all(got[b, n:] == 0.0)
-        ref = no.duration_model(duration_ckpt, rows[b][None], np.array([n]), dtype=torch.float64)
-        assert np.abs(got[b, :n] - ref[0]).max() < DUR_TOL, (b, n)
+        within_bound(eng, duration_ckpt, rows[b][None], [n], got[b : b + 1, :n])
         alone = eng.predict_duration(rows[b][None])
         assert np.abs(alone[0] - got[b, :n]).max() < 1e-6
 
@@ -87,8 +98,7 @@ def test_batch_larger_than_one_launch(eng, duration_ckpt):
     tok = np.stack([_tokens(300 + b, 12) for b in range(B)])
     got = eng.predict_duration(tok)
     for b in (0, 127, 128, 129):
-        ref = no.duration_model(duration_ckpt, tok[b : b + 1], np.array([12]), dtype=torch.float64)
-        assert np.abs(got[b] - ref[0]).max() < DUR_TOL
+        within_bound(eng, duration_ckpt, tok[b : b + 1], [12], got[b : b + 1])
 
 
 def test_device_pointer_entry_point(eng):
@@ -178,12 +188,13 @@ def test_tts_vs_oracle_end_to_end(eng, duration_ckpt, acoustic_ckpt, hifigan_par
     """Whole chain against the CPU restatement for one short utterance (dropout off)."""
     tk = _tokens(7, 14)
     tokens = [int(t) for t in tk]
-    d = no.adjust_durations(tokens, no.predict_duration(duration_ckpt, tk, dtype=torch.float64), 0.05)
+    raw64, unit = e2e_ref(duration_ckpt, tk[None], np.array([len(tk)]))
+    d = no.adjust_durations(tokens, raw64, 0.05)
     mel_ref = no.predict_mel(acoustic_ckpt, tokens, d, None)[None]
     mel_ref = no.trim_end_silence(tokens, d, mel_ref)
     wav_ref = ho.mel2wave(hifigan_params, mel_ref)
     waves, dur = eng.tts(tk[None], silence_duration=0.05)
-    assert np.abs(dur[0] - d[0]).max() < DUR_TOL
+    assert (np.abs(dur[0] - d[0]) <= E2E_UNITS[eng.mode] * unit[0]).all()     # the clip and word-end zeroing add no error
     assert waves[0].shape == wav_ref.shape, (waves[0].shape, wav_ref.shape)
     err = waves[0] - wav_ref
     print(f"tts e2e: Linf {np.abs(err).max():.3e} rms {np.sqrt(np.mean(err**2)):.3e}")

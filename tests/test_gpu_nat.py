@@ -150,7 +150,7 @@ def test_mixed_length_bucketed_synthesis(eng, hifigan_params):
     assert len(wavs) == len(utts)
     for i in (0, 3, 7, 9):
         tk, d = utts[i]
-        n = int(np.sum(d, dtype=np.float32))
+        n = no.frame_count(d)
         alone = eng.synthesize(tk[None], d[None], n_frames=[n])
         assert wavs[i].shape == (n * 256,)
         assert np.abs(wavs[i] - alone[0]).max() < 1e-5

@@ -696,6 +696,7 @@ int vtts_debug_read(vtts_ctx* ctx, const char* name, float* host_out, int64_t n_
   else if (!strcmp(name, "mel_pre")) { src = ctx->tap_melpre; n = ctx->tap_melpre_n; }
   else if (!strcmp(name, "dec_in")) { src = ctx->tap_decin; n = ctx->tap_decin_n; }
   else if (!strcmp(name, "dec_out")) { src = ctx->tap_decout; n = ctx->tap_decout_n; }
+  else if (!strcmp(name, "dur_hidden")) { src = ctx->tap_durhid; n = ctx->tap_durhid_n; }
   else return ctx->fail(VTTS_ERR_BAD_ARG, "debug_read: unknown tap %s", name);
   if (!src)
     return ctx->fail(VTTS_ERR_BAD_ARG, "debug_read: tap %s is not set (the last call did not produce it, or the workspace it pointed into "

@@ -1618,6 +1618,7 @@ int vtts_duration_run(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengt
   const ModelWeights& m = ctx->du;
   ctx->clear_taps();
   ctx->tap_enc = w.e.enc; ctx->tap_enc_n = BL * 512;
+  ctx->tap_durhid = w.y; ctx->tap_durhid_n = BL * 256;
   // padded encoder rows are never written by the scan: clear them so the projection reads zeros, not stale workspace
   VTTS_CUDA(cudaMemsetAsync(w.e.enc, 0, BL * 512 * sizeof(float), st));
   int rc = run_token_encoder(ctx, m, tokens, lengths, B, L, w.e, st);

@@ -219,9 +219,10 @@ struct vtts_ctx {
   float* tap_melpre = nullptr; int64_t tap_melpre_n = 0;
   float* tap_decin = nullptr; int64_t tap_decin_n = 0;     // teacher-forced decoder input [B,N,768] = [cond | p2]
   float* tap_decout = nullptr; int64_t tap_decout_n = 0;   // decoder scan output [B,N,1024] = [h0 | h1] (un-zoned)
+  float* tap_durhid = nullptr; int64_t tap_durhid_n = 0;   // duration head input [B,L,256]: first Linear + bias, pre-gelu
   void clear_taps() {
-    tap_enc = tap_cond = tap_melpre = tap_decin = tap_decout = nullptr;
-    tap_enc_n = tap_cond_n = tap_melpre_n = tap_decin_n = tap_decout_n = 0;
+    tap_enc = tap_cond = tap_melpre = tap_decin = tap_decout = tap_durhid = nullptr;
+    tap_enc_n = tap_cond_n = tap_melpre_n = tap_decin_n = tap_decout_n = tap_durhid_n = 0;
   }
 
   static constexpr int NSTAGE = 4;   // 0 hifigan, 1 acoustic, 2 melspec, 3 duration

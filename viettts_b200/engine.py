@@ -559,7 +559,8 @@ class Engine:
         dur = _np(dur_frames, np.float32, (B, L), "durations")
         lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
         if n_frames is None:
-            nf = np.array([int(np.sum(dur[b, : (L if lens is None else lens[b])], dtype=np.float32)) for b in range(B)], np.int32)
+            from .nat.text2mel import frame_count
+            nf = np.array([frame_count(dur[b, : (L if lens is None else lens[b])]) for b in range(B)], np.int32)
         else:
             nf = _np(n_frames, np.int32, (B,), "n_frames")
         N = int(nf.max())
@@ -701,10 +702,11 @@ class Engine:
         `max_pad_frac`, each bucket runs as one ragged batch, and the waveforms come back in input order
         (list of np.float32 [256*n_frames_i]).  Row i of any bucket equals utterance i run alone (with `rng`, the
         reference's own dropout stream, that includes its masks)."""
+        from .nat.text2mel import frame_count
         from .parallel import bucket_by_length
         if rng is not None:
             _rng_seed(rng, masks, seed)
-        nfs = [int(np.sum(np.asarray(d, np.float32), dtype=np.float32)) for _, d in utterances]
+        nfs = [frame_count(d) for _, d in utterances]
         out = [None] * len(utterances)
         for bucket in bucket_by_length(nfs, max_pad_frac, max_rows):
             Lmax = max(len(utterances[i][0]) for i in bucket)

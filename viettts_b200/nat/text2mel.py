@@ -60,10 +60,21 @@ def checkpoint_rng(ckpt_file=None) -> np.ndarray:
     return _rng_keys[key]
 
 
+def frame_count(frames) -> int:
+    """The acoustic frame count of one utterance, `int(sum(durations))` of text2mel.py:79, from its float32 per-token
+    durations in frames: summed in float64 in token order, rounded to float32 once, then truncated.  This is the
+    library's one definition (vtts_tts_plan, so `Engine.tts` and the TTS stream, computes the same).  For any realistic
+    row the float64 sum is exact, so it does not depend on the order of the terms; a float32 sum does, and near an
+    integer it can land one frame off."""
+    f = np.asarray(frames, np.float32).ravel()
+    total = float(np.cumsum(f, dtype=np.float64)[-1]) if f.size else 0.0
+    return int(np.float32(total))
+
+
 def seconds_to_frames(durations):
-    """text2mel.py:78-79 in float32: durations * sample_rate / (n_fft // 4)."""
+    """text2mel.py:78-79: durations * sample_rate / (n_fft // 4) in float32, and the frame count (`frame_count`)."""
     d = (np.asarray(durations, np.float32) * np.float32(config.SAMPLE_RATE)) / np.float32(config.N_FFT // 4)
-    return d, int(np.sum(d, dtype=np.float32))
+    return d, frame_count(d)
 
 
 def predict_mel(tokens, durations, masks=None, dropout=True, seed=None):

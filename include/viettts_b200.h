@@ -621,6 +621,45 @@ int vtts_compressor_stream_push(vtts_ctx* ctx, vtts_compressor_stream* cs, const
 int vtts_compressor_stream_push_host(vtts_ctx* ctx, vtts_compressor_stream* cs, const float* x, const int32_t* n_new, const uint8_t* flags,
                                      float* y, int32_t* n_out, float* reduction_db);
 
+/* ---- split-band de-esser ------------------------------------------------------------------------------------------
+ * One mono row x of n samples at rate r (an integer in [8000, 192000]); crossover freq_hz in [1000, 0.45 r]; threshold,
+ * ratio, knee, attack and release as for vtts_compress; range_db in [0, 24] (anything else, NaN included, fails with
+ * VTTS_ERR_BAD_ARG before anything is launched):
+ *   h = the one second-order Butterworth high-pass section of vtts_eq_design(VTTS_EQ_HIGHPASS, r, freq_hz, order 2)
+ *   over x from zero state (the equalizer's filter);  y_L = vtts_compress's detector on L = 20 log10 |h| (no makeup);
+ *   y^_L = min(y_L, range_db);  g = 10^(-y^_L / 20);  y = x - (1 - g) h, evaluated as fmaf(g - 1, h, x) where
+ *   y^_L > 0 and as x where it is 0: the band below the crossover passes untouched and only the high band is turned
+ *   down, by at most range_db.  reduction_db = -max y^_L (<= 0).  Rows whose high band stays below the knee (and
+ *   ratio 1, and range 0) come back as x bit for bit.
+ * fp32 in every vtts_precision mode; the sidechain keeps the equalizer's 1024-sample blocks and the detector the
+ * compressor's 256-sample blocks, both fixed by absolute sample index, so a row gives the same bits alone, in any
+ * batch, and through the stream. */
+/* x_dev [B,S]; n_dev int32 [B] or NULL (= S; values clamped to [0, S]); y_dev [B,S] (may equal x_dev), 0 past n[b];
+ * reduction_db_dev [B] or NULL.  Stream-ordered, no host synchronisation, nine launches (the equalizer's three, then
+ * the compressor's six); uses the context's workspace (about 4.3 bytes per sample). */
+int vtts_deess(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, float freq_hz, float threshold_db, float ratio,
+               float knee_db, float attack_ms, float release_ms, float range_db, float* y_dev, float* reduction_db_dev, void* stream);
+/* the same on host buffers; n_in[b] must lie in [0, S]; reduction_db [B] or NULL */
+int vtts_deess_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float freq_hz, float threshold_db, float ratio,
+                    float knee_db, float attack_ms, float release_ms, float range_db, float* y, float* reduction_db);
+/* Streaming de-esser with max_streams independent slots; every parameter is fixed at create.  Every sample is released by
+ * the push that brings it (no lookahead): n_out[s] = n_new[s], and a slot's outputs, concatenated, and its reduction
+ * equal vtts_deess of its whole input bit for bit.  Each slot carries the equalizer stream's state (the samples of its
+ * incomplete 1024-sample block and the filter state at the block's start) and the compressor stream's (partial maps,
+ * entering values, largest y^_L).  flags and slot rules as for the resample stream.  Every push issues the same ten
+ * launches (the window step, the equalizer's three, the compressor's six). */
+typedef struct vtts_deesser_stream vtts_deesser_stream;
+int vtts_deesser_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int rate, float freq_hz, float threshold_db, float ratio,
+                               float knee_db, float attack_ms, float release_ms, float range_db, vtts_deesser_stream** out);
+int vtts_deesser_stream_destroy(vtts_ctx* ctx, vtts_deesser_stream* ds);
+/* as vtts_compressor_stream_push: x_dev, y_dev [S][max_chunk_samples] (y_dev may equal x_dev), n_new, flags, n_out HOST
+ * [S], reduction_db_dev [S] each slot's reduction over what it has released since BEGIN.  Stream-ordered. */
+int vtts_deesser_stream_push(vtts_ctx* ctx, vtts_deesser_stream* ds, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
+                             float* y_dev, int32_t* n_out, float* reduction_db_dev, void* stream);
+/* the same on host buffers x and y [S][max_chunk_samples] and reduction_db [S]; returns when they are written */
+int vtts_deesser_stream_push_host(vtts_ctx* ctx, vtts_deesser_stream* ds, const float* x, const int32_t* n_new, const uint8_t* flags,
+                                  float* y, int32_t* n_out, float* reduction_db);
+
 /* ---- streaming acoustic model: every slot advances its decoder a few frames per push ---------------------------
  * A vtts_acoustic_stream holds max_streams (1..128) independent slots.  begin starts utterances in closed slots; each
  * push advances every open slot by min(F, frames left) decoder steps in ONE scan launch and returns the mel frames whose

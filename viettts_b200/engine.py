@@ -182,38 +182,72 @@ def compressor_params(spec, rate: int) -> dict:
     6 dB knee, 5 ms attack, 80 ms release, 0 dB makeup), comma-separated key=value pairs over those six keys, or a dict
     of them; keys left out take the voice preset.  threshold dBFS in [-60, 0], ratio in [1, 20], knee dB in [0, 24],
     attack ms in [0.5, 200], release ms in [5, 5000], makeup dB in [-24, 24].  Raises ValueError naming the key."""
+    _check_rate("compress", rate)
+    return _keyed_params("compress", spec, COMPRESSOR_RANGES, COMPRESSOR_PRESETS)
+
+
+# the de-esser's parameters in vtts_deess's order, with their ranges and the `voice` preset; freq's upper end is a
+# fraction of the rate (deesser_params puts in 0.45 rate), and the detector's ranges are the compressor's
+DEESSER_RANGES = {"freq": (1000.0, 0.45), "threshold": (-60.0, 0.0), "ratio": (1.0, 20.0), "knee": (0.0, 24.0), "attack": (0.5, 200.0),
+                  "release": (5.0, 5000.0), "range": (0.0, 24.0)}
+DEESSER_PRESETS = {"voice": {"freq": 5000.0, "threshold": -30.0, "ratio": 4.0, "knee": 6.0, "attack": 1.0, "release": 60.0,
+                             "range": 12.0}}
+
+
+def deesser_params(spec, rate: int) -> dict:
+    """{freq, threshold, ratio, knee, attack, release, range} (float32 values, in vtts_deess's order) of a de-esser
+    `spec` at `rate` Hz (an integer in [8000, 192000]).  `spec` is the preset `voice` (5000 Hz crossover, -30 dBFS
+    threshold, 4:1 ratio, 6 dB knee, 1 ms attack, 60 ms release, 12 dB range), comma-separated key=value pairs over
+    those seven keys, or a dict of them; keys left out take the voice preset.  freq Hz in [1000, 0.45 rate] (so the voice
+    preset needs rate >= 11112 Hz), range dB in [0, 24], the others in the compressor's ranges.  Raises ValueError
+    naming the key."""
+    _check_rate("deess", rate)
+    ranges = dict(DEESSER_RANGES, freq=(1000.0, 0.45 * float(rate)))
+    return _keyed_params("deess", spec, ranges, DEESSER_PRESETS)
+
+
+def _check_rate(what: str, rate):
     try:
         r = float(rate)
     except (TypeError, ValueError):
         r = None
     if r is None or not (8000 <= r <= 192000 and r == int(r)):
-        raise ValueError(f"compress: rate {rate} must be an integer in [8000, 192000]")
+        raise ValueError(f"{what}: rate {rate} must be an integer in [8000, 192000]")
+
+
+def _keyed_params(what: str, spec, ranges: dict, presets: dict) -> dict:
+    """the float32 values of a `spec` (a preset name, comma-separated key=value pairs, or a dict) over `ranges`, keys
+    left out taking presets["voice"]; every value must lie in its range.  Raises ValueError naming the key."""
     if isinstance(spec, str):
         given = {}
         s = spec.strip().lower()
-        if s not in COMPRESSOR_PRESETS:
+        if s not in presets:
             for item in s.split(","):
                 key, eq, val = item.strip().partition("=")
                 if not eq:
-                    raise ValueError(f"compress: {item.strip()!r} is not key=value (keys {', '.join(COMPRESSOR_RANGES)}) "
-                                     f"or a preset ({', '.join(COMPRESSOR_PRESETS)})")
+                    raise ValueError(f"{what}: {item.strip()!r} is not key=value (keys {', '.join(ranges)}) "
+                                     f"or a preset ({', '.join(presets)})")
                 given[key.strip()] = val.strip()
     elif isinstance(spec, dict):
         given = dict(spec)
     else:
-        raise ValueError(f"compress: a spec is a string or a dict, got {type(spec).__name__}")
-    out = dict(COMPRESSOR_PRESETS["voice"])
+        raise ValueError(f"{what}: a spec is a string or a dict, got {type(spec).__name__}")
+    out = dict(presets["voice"])
     for key, val in given.items():
-        if key not in COMPRESSOR_RANGES:
-            raise ValueError(f"compress: unknown key {key!r} (keys {', '.join(COMPRESSOR_RANGES)})")
+        if key not in ranges:
+            raise ValueError(f"{what}: unknown key {key!r} (keys {', '.join(ranges)})")
         try:
             v = float(np.float32(float(val)))
         except (TypeError, ValueError):
-            raise ValueError(f"compress: {key}={val!r} is not a number") from None
-        lo, hi = COMPRESSOR_RANGES[key]
+            raise ValueError(f"{what}: {key}={val!r} is not a number") from None
+        lo, hi = ranges[key]
         if not (np.isfinite(v) and lo <= v <= hi):
-            raise ValueError(f"compress: {key}={val} must lie in [{lo:g}, {hi:g}]")
+            raise ValueError(f"{what}: {key}={val} must lie in [{lo:g}, {hi:g}]")
         out[key] = v
+    for key, v in out.items():       # the preset's values too: a range may depend on the rate
+        lo, hi = ranges[key]
+        if not lo <= v <= hi:
+            raise ValueError(f"{what}: {key}={v:g} (the voice preset's) must lie in [{lo:g}, {hi:g}] at this rate")
     return out
 
 
@@ -504,7 +538,7 @@ class Engine:
 
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
                         rng=None, output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None,
-                        gain_db=0.0, eq=None, compress=None) -> "TtsStream":
+                        gain_db=0.0, eq=None, compress=None, deess=None) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
         With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  `output_rate`: a resample
@@ -524,12 +558,15 @@ class Engine:
         `compress`: a compressor spec (`compressor_params`); a compressor stream follows the equalizer (before the
         limiter and the meter) at the output rate, and the audio equals `compress` of the (resampled, equalized) `tts`
         audio bit for bit.  It also adds no delay.
+        `deess`: a de-esser spec (`deesser_params`); a de-esser stream follows the compressor (before the limiter and the
+        meter) at the output rate, and the audio equals `deess` of the (resampled, equalized, compressed) `tts` audio bit
+        for bit.  It also adds no delay.
         `meter=True`: a loudness meter runs last, on what `step()` returns at the output rate (a
         multiple of 10), and `TtsStream.meter()` gives each stepped slot's readings, read back in the step's one
         synchronisation.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
         return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate,
                          denoise=denoise, meter=meter, semitones=semitones, tempo=tempo, limit=limit, gain_db=gain_db, eq=eq,
-                         compress=compress)
+                         compress=compress, deess=deess)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -1265,6 +1302,39 @@ class Engine:
         bit."""
         return CompressorStream(self, max_streams, max_chunk_samples, spec, rate)
 
+    # ---- de-esser (vtts_deess*: split-band sibilance compressor, fp32) ----
+    def deess(self, wav, spec="voice", rate: int = config.SAMPLE_RATE, lengths=None):
+        """Host arrays: (y, reduction_db).  wav f32 [S] or [B,S] at `rate` through the de-esser `spec` (see
+        `deesser_params`): the compressor's detector keyed by the band above the crossover `freq` (the second-order
+        Butterworth high-pass h of `equalize`), and y = x - (1 - g) h, so only that band is turned down, by at most
+        `range` dB.  reduction_db: the deepest reduction of the band per row (<= 0).  Rows whose high band stays below the
+        knee come back exactly as wav.  lengths int [B] in [0, S]: outputs past lengths[b] are 0."""
+        p = deesser_params(spec, rate)
+        x, lens, one = _wav_rows(wav, lengths)
+        B, S = x.shape
+        y = np.zeros((B, S), np.float32)
+        red = np.zeros(B, np.float32)
+        if B and S:
+            self._ck(self.lib.vtts_deess_host(self.h, _ptr(x), _ptr(lens), B, S, int(rate), *p.values(), _ptr(y), _ptr(red)))
+        return (y[0], red[0]) if one else (y, red)
+
+    def deess_forward(self, x_t, spec="voice", rate: int = config.SAMPLE_RATE, lengths_t=None, out=None, reduction_db=None,
+                      stream=None):
+        """vtts_deess on torch CUDA tensors, stream-ordered and without a host synchronisation: returns (y [B,S],
+        reduction_db [B]), both on the device.  lengths_t int32 CUDA [B] or None.  `out` may be x_t (in place)."""
+        p = deesser_params(spec, rate)
+        B, S, out, st = _dev_rows(x_t, out, stream)
+        reduction_db = _out_tensor(reduction_db, (B,), x_t.device, "reduction_db")
+        self._ck(self.lib.vtts_deess(self.h, _ptr(x_t), _ptr(lengths_t), B, S, int(rate), *p.values(), _ptr(out), _ptr(reduction_db), st))
+        return out, reduction_db
+
+    def open_deesser_stream(self, max_streams: int, max_chunk_samples: int, spec="voice",
+                            rate: int = config.SAMPLE_RATE) -> "DeesserStream":
+        """Streaming de-esser with `max_streams` independent slots (vtts_deesser_stream_*): every push releases every
+        sample it brings (no lookahead), and a slot's outputs, concatenated, and its reduction equal `deess` of its whole
+        input bit for bit."""
+        return DeesserStream(self, max_streams, max_chunk_samples, spec, rate)
+
 
 class Loudness(NamedTuple):
     integrated: np.ndarray     # LUFS (gated, BS.1770-4)
@@ -1660,6 +1730,26 @@ class CompressorStream(_ReductionStream):
         return self._push_device(x_t, n_new, flags, out_t, stream, dev=(reduction_t,))
 
 
+class DeesserStream(_ReductionStream):
+    """Handle of a streaming de-esser (Engine.open_deesser_stream).  Every push releases every sample it brings:
+    n_out = n_new (`push_device`: out_t may be x_t).  After every host push `reduction_db` holds each slot's deepest
+    reduction of its high band over what it has released since BEGIN."""
+    _kind = "deesser_stream"
+    lookahead = 0
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, spec="voice", rate: int = config.SAMPLE_RATE):
+        super().__init__(eng, max_streams, max_chunk_samples)
+        self.max_chunk_samples = self.out_pitch = self._chunk
+        self.params, self.rate = deesser_params(spec, rate), int(rate)
+        self._create(eng.lib.vtts_deesser_stream_create, self.max_streams, self.max_chunk_samples, self.rate, *self.params.values())
+        self.reduction_db = np.zeros(self.max_streams, np.float32)   # host pushes: each slot's reduction so far
+
+    def push_device(self, x_t, n_new, flags, out_t, reduction_t, stream=None) -> np.ndarray:
+        """As `_SlotStream.push_device`, with reduction_t f32 CUDA [S] (each slot's reduction so far, written on the
+        device)."""
+        return self._push_device(x_t, n_new, flags, out_t, stream, dev=(reduction_t,))
+
+
 def acoustic_stream_schedule(n_frames: int, n_emit: int | None, chunk: int, lookahead: int = 10) -> list:
     """Frames an acoustic stream slot emits per push: it scans min(n_frames, n_emit + lookahead) frames, `chunk` per
     push; after P frames scanned it has emitted min(n_emit, max(0, P - lookahead)), and its last push emits the rest."""
@@ -1767,14 +1857,14 @@ class OptionError(ValueError):
 
 class AudioChain:
     """The audio stages after the vocoder, their options validated, in the one order every caller runs them: denoise,
-    pitch shift and time stretch at 16 kHz, then resample, equalize, compress, limit (or normalize loudness) and meter at
-    the output rate.  `run` applies the chain to one waveform with the one-shot host calls; `streams` opens it as stream
+    pitch shift and time stretch at 16 kHz, then resample, equalize, compress, de-ess, limit (or normalize loudness) and
+    meter at the output rate.  `run` applies the chain to one waveform with the one-shot host calls; `streams` opens it as stream
     stages.  `loudness` (a target in LUFS, reached under `true_peak`, or under the limiter's ceiling with `limit`) has no
     streaming form, and `meter` only measures, so `run` leaves the audio as it is for it.  Raises OptionError (a
     ValueError naming the option) for an option out of range."""
 
     def __init__(self, denoise=None, semitones=None, tempo=None, output_rate=None, eq=None, limit=None, gain_db=0.0,
-                 loudness=None, true_peak=None, meter=False, compress=None):
+                 loudness=None, true_peak=None, meter=False, compress=None, deess=None):
         def checked(option, check, *args):
             try:
                 return check(*args)
@@ -1788,6 +1878,7 @@ class AudioChain:
         self.tempo = None if tempo is None else float(checked("tempo", TEMPO.rows, tempo, 1)[0])
         self.eq = None if eq is None else checked("eq", eq_sections, eq, self.rate)
         self.compress = None if compress is None else checked("compress", compressor_params, compress, self.rate)
+        self.deess = None if deess is None else checked("deess", deesser_params, deess, self.rate)
         self.limit = None if limit is None else checked("limit", _limit_args, limit, self.rate, 5.0, 100.0)[0]
         self.gain_db = float(checked("gain_db", GAIN_DB.rows, gain_db, 1)[0]) if limit is not None else 0.0
         self.loudness = self.true_peak = None
@@ -1810,6 +1901,7 @@ class AudioChain:
             (self.eq is not None, "eq", lambda e, w: e.equalize(w, self.eq, r), lambda e, S, p, sec: EqStream(e, S, p, self.eq, r)),
             (self.compress is not None, "cp", lambda e, w: e.compress(w, self.compress, r)[0],
              lambda e, S, p, sec: CompressorStream(e, S, p, self.compress, r)),
+            (self.deess is not None, "ds", lambda e, w: e.deess(w, self.deess, r)[0], lambda e, S, p, sec: DeesserStream(e, S, p, self.deess, r)),
             (self.loudness is not None, "lm",
              lambda e, w: e.normalize_loudness(w, self.loudness, r, true_peak=self.true_peak, limit=self.limit is not None)[0], None),
             (self.loudness is None and self.limit is not None, "lm", lambda e, w: e.limit(w, self.limit, r, self.gain_db)[0],
@@ -1849,14 +1941,14 @@ class TtsStream:
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
                  output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None, gain_db=0.0, eq=None,
-                 compress=None):
+                 compress=None, deess=None):
         import torch
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
         self._chain = AudioChain(denoise=denoise, semitones=semitones, tempo=tempo, output_rate=output_rate, eq=eq, limit=limit,
-                                 gain_db=gain_db, meter=meter, compress=compress)
+                                 gain_db=gain_db, meter=meter, compress=compress, deess=deess)
         self.eng = eng
-        self.rs = self.dn = self.ps = self.ts = self.eq = self.cp = self.lm = self.mt = None
+        self.rs = self.dn = self.ps = self.ts = self.eq = self.cp = self.ds = self.lm = self.mt = None
         S = max_streams
         self._built = []   # every stream handle, in construction order
         try:

@@ -22,6 +22,8 @@ or the `telephone` preset) at the rate it is written, after --output-rate and be
 `--compress SPEC` lowers the dynamic range of every output on the device (Engine.compress: a soft-knee feed-forward
 compressor, the `voice` preset or key=value settings) at the rate it is written, after --eq and before --loudness /
 --limiter, so the limiter only catches what the compressor leaves.
+`--deess SPEC` turns down harsh sibilants of every output on the device (Engine.deess: the band above a crossover,
+only while it is loud) at the rate it is written, after --compress and before --loudness / --limiter.
 """
 from __future__ import annotations
 
@@ -115,7 +117,8 @@ def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_
 
 # the command-line flag of each AudioChain option the CLI sets
 _FLAGS = {"denoise": "--denoise", "semitones": "--pitch", "tempo": "--tempo", "output_rate": "--output-rate", "eq": "--eq",
-          "limit": "--limiter", "loudness": "--loudness", "compress": "--compress"}
+          "limit": "--limiter", "loudness": "--loudness", "compress": "--compress",
+          "deess": "--deess"}
 
 
 def main(argv=None) -> int:
@@ -159,6 +162,12 @@ def main(argv=None) -> int:
                              "before --loudness / --limiter: 'voice' (-24 dBFS threshold, 3:1, 6 dB knee, 5 ms attack, 80 ms "
                              "release, 0 dB makeup) or comma-separated threshold=, ratio=, knee=, attack=, release=, makeup= "
                              "(keys left out keep the voice values)")
+    parser.add_argument("--deess", default=None, metavar="SPEC",
+                        help="de-ess every output on the device at the output rate, after --compress and before --loudness / "
+                             "--limiter: only the band above the crossover is turned down, only while it is loud. 'voice' "
+                             "(5000 Hz crossover, -30 dBFS threshold, 4:1, 6 dB knee, 1 ms attack, 60 ms release, 12 dB range; "
+                             "needs an output rate of at least 11112 Hz) or comma-separated freq=, threshold=, ratio=, knee=, "
+                             "attack=, release=, range= (keys left out keep the voice values)")
     parser.add_argument("--silence-duration", default=-1, type=float)
     parser.add_argument("--lexicon-file", default=None)
     parser.add_argument("--seed", default=None, type=int,
@@ -185,7 +194,8 @@ def main(argv=None) -> int:
     ceiling = -1.0 if args.true_peak is None else args.true_peak
     try:
         chain = AudioChain(denoise=args.denoise, semitones=args.pitch, tempo=args.tempo, output_rate=args.output_rate, eq=args.eq,
-                           limit=ceiling if args.limiter else None, loudness=args.loudness, true_peak=ceiling, compress=args.compress)
+                           limit=ceiling if args.limiter else None, loudness=args.loudness, true_peak=ceiling, compress=args.compress,
+                           deess=args.deess)
     except OptionError as e:
         parser.error(f"{_FLAGS[e.option]}: {e}")
     header_rate = args.output_rate or args.sample_rate or config.SAMPLE_RATE

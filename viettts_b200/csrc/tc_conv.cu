@@ -23,6 +23,8 @@
 //              epilogue (+ bias (+ BN/act) (+ residual), fp32 NWC store; the plain one staged through shared memory)
 //   warp  8    weight producer (one lane, cp.async.bulk + expect_tx)
 //   warps 9-11 activation converters: fp32 global -> [mean3] -> leaky_relu -> hi/lo bf16 -> smem
+// The ConvTranspose instantiation (SUB) walks a tile in row steps of NCWG x 64 rows instead: its ring stages hold a row
+// step over several chunks (the row-block ring, SUB_* below), so each input row is read once per tile.
 // A consumer keeps one wgmma group in flight: it releases a ring stage when the NEXT group has been issued and the
 // previous one has retired (wgmma.wait_group 1), so issue and tensor-core execution overlap.
 //
@@ -52,12 +54,28 @@ constexpr int PAIR_OVERLAP = 16;              // pair kernel: rows per tile that
 constexpr int NQ = 2;                         // tile-id ring slots
 constexpr int NREADERS = (NCONS + NCONV) / 32;  // warps that read the tile-id ring
 
-template <int N, int MW, int PAIRF, bool STAGED = false>
+// Row-block ring of the sub-row (ConvTranspose) instantiation.  Its input is the 3-way mean of three chain tensors, so a
+// tile's live input is three times that of a ResBlock conv; converted chunk by chunk, every row of it would be revisited
+// Cin/16 times and fall out of L2 in between.  Instead a ring stage holds one row step of the tile -- NCWG x 64 rows, one
+// 64-row block per consumer warpgroup, plus the tap halo -- over SUB_CG 16-channel chunks, so each pass reads contiguous
+// SUB_CG x 64 B row segments of x0 (x1, x2) and every input element is read once per tile.  Layout per chunk:
+// [plane hi|lo][k-half][SUB_RS rows][16 B], chunks SUB_CSB bytes apart.  SUB_RS = 129 (k-half stride = 4 words mod 32)
+// and SUB_CSB = 24 words mod 32 put the 16 float4 columns of a converted row on 32 distinct banks.
+constexpr int SUB_CG = 4;                          // chunks per stage (64 channels)
+constexpr int SUB_HALO = 1;                        // (k - 1) * dilation of the ConvTranspose's two taps
+constexpr int SUB_RS = NCWG * 64 + SUB_HALO;       // rows per stage
+constexpr int SUB_CSB = SUB_RS * 64 + 32;          // bytes per chunk
+constexpr int SUB_STAGE = SUB_CG * SUB_CSB;
+static_assert(SUB_RS * 4 % 32 == 4 && SUB_CSB / 4 % 32 == 24, "bank-conflict-free converter stores");
+
+template <int N, int MW, int PAIRF, bool STAGED = false, bool SUB = false>
 struct TcCfg {
   static constexpr int R = 64 * MW * NCWG;                  // rows computed per tile
   static constexpr int R_OUT = R - PAIR_OVERLAP;             // rows stored per tile of the pair kernel
   static constexpr int RA = R + HALO;                       // allocated activation rows per stage
   static constexpr int A_STAGE = RA * 64;                   // bytes: 2 planes x 2 k-halves x RA rows x 16 B
+  static constexpr int NAS = SUB ? (N == 64 ? 4 : 2) : NA;  // activation stages (SUB: row-block stages, as many as fit)
+  static constexpr int A_BYTES = SUB ? NAS * SUB_STAGE : NA * A_STAGE;
   static constexpr int W_STAGE = N * 64;                    // bytes of one packed (chunk, tap) weight block
   static constexpr int NW = N == 256 ? 4 : 8;               // weight stages
   static constexpr int NCH2 = PAIRF ? N / 16 : 0;           // 16-channel chunks of the on-chip intermediate
@@ -69,7 +87,7 @@ struct TcCfg {
   static constexpr int EPI_WG = 64 * EPI_LD + N;             // floats
   static constexpr int EPI_STAGE = STAGED ? NCWG * EPI_WG * 4 : 0;   // the register epilogue keeps the L1 it would take
   static constexpr int SMEM_BYTES =
-      NA * A_STAGE + NW * W_STAGE + NCH2 * A_STAGE + EPI_STAGE + (2 * NA + 2 * NW + 2 * NQ) * 8 + NQ * 4 + 1024;
+      A_BYTES + NW * W_STAGE + NCH2 * A_STAGE + EPI_STAGE + (2 * NA + 2 * NW + 2 * NQ) * 8 + NQ * 4 + 1024;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one CTA");
 };
 
@@ -139,34 +157,80 @@ struct TileQueue {
   }
 };
 
-// converters: fill A stage `stage` with rows [row_base, row_base + rows) of channels [c*16, c*16+16) of x0 (+x1+x2)/3,
-// leaky_relu'd (pre_mode >= 1), zero outside [lo, valid); bf16 hi/lo planes, or one saturated fp16 plane (F16)
-template <int RA, bool F16>
-__device__ __forceinline__ void convert_chunk(uint8_t* stage, int ct, const float* x0, const float* x1, const float* x2, int ld, int c,
-                                              int row_base, int rows, int lo, int valid, int pre_mode, float slope) {
-  constexpr int RSTEP = NCONV / 4;
-  const int q = ct & 3;                     // 4-channel group inside the 16-channel chunk
-  const int r0 = ct >> 2;
-  uint8_t* st = stage + ((q >> 1) * RA) * 16 + (q & 1) * 8;
-  const int coff = c * 16 + q * 4;
+// s / 3, rounded to nearest like the IEEE division s / 3.0f, without its branch to a slow path: q0 = s * RN(1/3), then one
+// correction by the exact residual s - 3 q0 (Markstein).  Bit-equal to s / 3.0f for every float except +-0 and +-inf,
+// where it would give +0 and NaN; for those s / 3 is s itself (scripts/check_div3.c checks all 2^32 inputs).
+__device__ __forceinline__ float div3_rn(float s) {
+  constexpr float y = 0x1.555556p-2f;   // RN(1/3)
+  const float q0 = __fmul_rn(s, y);
+  const float q1 = __fmaf_rn(__fmaf_rn(-q0, 3.0f, s), y, q0);
+  return (s == 0.f || fabsf(s) == __int_as_float(0x7f800000)) ? s : q1;
+}
+
+// converters: fill A stage `stage` with rows [row_base, row_base + rows) of channels [ch0, ch0 + 4 * QN) of
+// x0 (+x1+x2)/3, leaky_relu'd (pre_mode >= 1), zero outside [lo, valid); bf16 hi/lo planes, or one saturated fp16 plane
+// (F16).  The stage holds QN / 4 chunks of [plane][k-half][RS rows][16 B], CSB bytes apart; thread ct converts float4
+// column ct % QN of every (NCONV / QN)-th row.
+// LOADS_FIRST: all 3 x U loads of a step are issued before the first mean, and the mean divides with div3_rn.  The IEEE
+// division by 3 branches to a slow path; the compiler does not hoist later loads above that branch (in source order, row
+// u + 1's loads would wait for row u's data, one memory round trip per row), and the 4 U branches serialize the step's
+// arithmetic.
+template <int QN, int RS, int CSB, bool F16, bool LOADS_FIRST = false>
+__device__ __forceinline__ void convert_rows(uint8_t* stage, int ct, const float* x0, const float* x1, const float* x2, int ld, int ch0,
+                                             int row_base, int rows, int lo, int valid, int pre_mode, float slope) {
+  static_assert(NCONV % QN == 0, "whole rows per converter step");
+  constexpr int RSTEP = NCONV / QN, RA = RS;
+  const int q = ct % QN;                    // 4-channel group
+  const int r0 = ct / QN;
+  uint8_t* st = stage + (q >> 2) * CSB + (((q >> 1) & 1) * RA) * 16 + (q & 1) * 8;
+  const int coff = ch0 + q * 4;
   constexpr int U = 8;                      // loads in flight per thread
   for (int rr0 = r0; rr0 < rows; rr0 += RSTEP * U) {
     float4 v[U];
+    if constexpr (LOADS_FIRST) {
+      float4 a[U], bb[U];
+      bool in[U];
 #pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int rr = rr0 + u * RSTEP;
-      const int t = row_base + rr;
-      v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (rr < rows && t >= lo && t < valid) {
-        const size_t off = (size_t)t * ld + coff;
-        v[u] = ldg_pf256(x0 + off);
-        if (pre_mode == 2) {
-          const float4 a = ldg_pf256(x1 + off);
-          const float4 bb = ldg_pf256(x2 + off);
-          v[u].x = ((v[u].x + a.x) + bb.x) / 3.0f;
-          v[u].y = ((v[u].y + a.y) + bb.y) / 3.0f;
-          v[u].z = ((v[u].z + a.z) + bb.z) / 3.0f;
-          v[u].w = ((v[u].w + a.w) + bb.w) / 3.0f;
+      for (int u = 0; u < U; ++u) {
+        const int rr = rr0 + u * RSTEP;
+        const int t = row_base + rr;
+        in[u] = rr < rows && t >= lo && t < valid;
+        v[u] = a[u] = bb[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (in[u]) {
+          const size_t off = (size_t)t * ld + coff;
+          v[u] = ldg_pf256(x0 + off);
+          if (pre_mode == 2) {
+            a[u] = ldg_pf256(x1 + off);
+            bb[u] = ldg_pf256(x2 + off);
+          }
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        if (in[u] && pre_mode == 2) {
+          v[u].x = div3_rn((v[u].x + a[u].x) + bb[u].x);
+          v[u].y = div3_rn((v[u].y + a[u].y) + bb[u].y);
+          v[u].z = div3_rn((v[u].z + a[u].z) + bb[u].z);
+          v[u].w = div3_rn((v[u].w + a[u].w) + bb[u].w);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int rr = rr0 + u * RSTEP;
+        const int t = row_base + rr;
+        v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (rr < rows && t >= lo && t < valid) {
+          const size_t off = (size_t)t * ld + coff;
+          v[u] = ldg_pf256(x0 + off);
+          if (pre_mode == 2) {
+            const float4 a = ldg_pf256(x1 + off);
+            const float4 bb = ldg_pf256(x2 + off);
+            v[u].x = ((v[u].x + a.x) + bb.x) / 3.0f;
+            v[u].y = ((v[u].y + a.y) + bb.y) / 3.0f;
+            v[u].z = ((v[u].z + a.z) + bb.z) / 3.0f;
+            v[u].w = ((v[u].w + a.w) + bb.w) / 3.0f;
+          }
         }
       }
     }
@@ -189,6 +253,13 @@ __device__ __forceinline__ void convert_chunk(uint8_t* stage, int ct, const floa
       }
     }
   }
+}
+
+// one 16-channel chunk c over RA-row stages
+template <int RA, bool F16>
+__device__ __forceinline__ void convert_chunk(uint8_t* stage, int ct, const float* x0, const float* x1, const float* x2, int ld, int c,
+                                              int row_base, int rows, int lo, int valid, int pre_mode, float slope) {
+  convert_rows<4, RA, 0, F16>(stage, ct, x0, x1, x2, ld, c * 16, row_base, rows, lo, valid, pre_mode, slope);
 }
 
 // weight producer: the k packed (chunk, tap) blocks of chunks [0, nch) of one conv, one ring stage each
@@ -293,6 +364,58 @@ __device__ __forceinline__ void consume(float (&acc)[MW][N / 2], int wg, uint32_
   }
 }
 
+// consumer warpgroup, row-block ring (SUB): acc (+)= sum over chunks c < nch and taps j < k of A(row wg * 64 + j * dil
+// of the row step) . W(c, j) for the warpgroup's one 64-row block of a row step, whose chunks arrive SUB_CG per ring
+// stage.  Per accumulator the (chunk, tap, plane product) sequence is the one consume() issues.
+template <int N, int NW, int NAS, bool F16>
+__device__ __forceinline__ void consume_rows(float (&acc)[N / 2], int wg, uint32_t a_st_u32, uint64_t* a_full, uint64_t* a_empty, Ring& ra,
+                                             uint32_t w_st_u32, uint64_t* w_full, uint64_t* w_empty, Ring& rw, int nch, int k, int dil,
+                                             int* err, long long& w_a, long long& w_w) {
+  const uint64_t a_tmpl = make_desc(0, SUB_RS * 16, 128);
+  const uint64_t b_tmpl = make_desc(0, (F16 ? 1 : 2) * N * 16, 128);
+  const bool lane0 = (threadIdx.x & 31) == 0;
+  int pend_w = -1, pend_a = -1;
+  for (int c0 = 0; c0 < nch; c0 += SUB_CG) {
+    mbar_wait_t(&a_full[ra.s], ra.p, err, 2, w_a);
+    const uint32_t a_blk = a_st_u32 + ra.s * SUB_STAGE + wg * 64 * 16;
+    for (int cl = 0; cl < SUB_CG; ++cl) {
+      for (int j = 0; j < k; ++j) {
+        mbar_wait_t(&w_full[rw.s], rw.p, err, 3, w_w);
+        const uint32_t w_base = w_st_u32 + rw.s * (N * 64);
+        const uint64_t b_hi = b_tmpl | (uint64_t)(w_base >> 4);
+        const uint64_t b_lo = b_tmpl | (uint64_t)((w_base + N * 16) >> 4);
+        const uint32_t first = ((c0 + cl) | j) != 0 ? 1u : 0u;
+        const uint32_t row = a_blk + cl * SUB_CSB + j * dil * 16;
+        const uint64_t a_hi = a_tmpl | (uint64_t)(row >> 4);
+        const uint64_t a_lo = a_tmpl | (uint64_t)((row + 2 * SUB_RS * 16) >> 4);
+        wgmma_fence();
+        if constexpr (F16) {
+          wgmma<N, true>(acc, a_hi, b_hi, first);
+        } else {
+          wgmma<N>(acc, a_hi, b_hi, first);
+          wgmma<N>(acc, a_hi, b_lo, 1u);
+          wgmma<N>(acc, a_lo, b_hi, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();          // the previous group has retired: its stages may be refilled
+        if (lane0) {
+          if (pend_w >= 0) mbar_arrive(&w_empty[pend_w]);
+          if (pend_a >= 0) mbar_arrive(&a_empty[pend_a]);
+        }
+        pend_w = (int)rw.s;
+        pend_a = (cl == SUB_CG - 1 && j == k - 1) ? (int)ra.s : -1;
+        rw.next<NW>();
+      }
+    }
+    ra.next<NAS>();
+  }
+  wgmma_wait<0>();
+  if (lane0) {
+    if (pend_w >= 0) mbar_arrive(&w_empty[pend_w]);
+    if (pend_a >= 0) mbar_arrive(&a_empty[pend_a]);
+  }
+}
+
 // 16-byte global -> shared copy that bypasses the registers (cp.async, L1 not allocated)
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
@@ -348,12 +471,12 @@ __device__ __forceinline__ int sub_elem(const TcLaunch& L, const TcProb& P, int 
 template <int N, int EPI, int MW, bool F16, bool SUB>
 __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_constant__ TcLaunch L) {
   static_assert(!SUB || EPI == 0, "sub-row output uses the plain epilogue");
-  using Cfg = TcCfg<N, MW, 0, EPI == 0>;
-  constexpr int R = Cfg::R, RA = Cfg::RA, NW = Cfg::NW;
+  using Cfg = TcCfg<N, MW, 0, EPI == 0, SUB>;
+  constexpr int R = Cfg::R, RA = Cfg::RA, NW = Cfg::NW, NAS = Cfg::NAS;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* a_st = smem;
-  uint8_t* w_st = smem + NA * Cfg::A_STAGE;
+  uint8_t* w_st = smem + Cfg::A_BYTES;
   // [NCWG][EPI_WG]; indexed from smem_raw so that its accesses compile to shared-memory instructions
   float* epi_st = reinterpret_cast<float*>(smem_raw + (w_st + NW * Cfg::W_STAGE - smem_raw));
   uint64_t* bars = reinterpret_cast<uint64_t*>(w_st + NW * Cfg::W_STAGE + Cfg::EPI_STAGE);
@@ -404,7 +527,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
       PRODUCER_TILES
       TILE_LOOP_BEGIN
         (void)b; (void)tau0; (void)in_lo; (void)valid; (void)out_hi; (void)e_lim;
-        produce_weights<N, NW, F16>(w_st, w_full, w_empty, rw, P.wpk, nch, P.k, L.err, w_e);
+        // SUB: the consumers run the tile's MW row steps one after another, each over all (chunk, tap) blocks
+        for (int mt = 0; mt < (SUB ? MW : 1); ++mt) produce_weights<N, NW, F16>(w_st, w_full, w_empty, rw, P.wpk, nch, P.k, L.err, w_e);
       TILE_LOOP_END
       if (L.dbg) L.dbg[(size_t)blockIdx.x * 16 + 4] = w_e;
     }
@@ -419,13 +543,27 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
       const size_t in_base = (size_t)b * L.T_rows * L.in_ld;
       const float* x1 = L.pre_mode == 2 ? P.x1 + in_base : nullptr;
       const float* x2 = L.pre_mode == 2 ? P.x2 + in_base : nullptr;
-      for (int c = 0; c < nch; ++c) {
-        mbar_wait_t(&a_empty[ra.s], ra.p ^ 1, L.err, 5, w_ae);
-        convert_chunk<RA, F16>(a_st + ra.s * Cfg::A_STAGE, ct, P.x0 + in_base, x1, x2, L.in_ld, c, tau0 + P.in_off, R + (k - 1) * dil,
-                          in_lo, valid, L.pre_mode, L.pre_slope);
-        fence_proxy_async();
-        mbar_arrive(&a_full[ra.s]);
-        ra.next<NA>();
+      if constexpr (SUB) {
+        // row step mt (NCWG x 64 rows + halo), SUB_CG chunks per stage
+        for (int mt = 0; mt < MW; ++mt)
+          for (int c0 = 0; c0 < nch; c0 += SUB_CG) {
+            mbar_wait_t(&a_empty[ra.s], ra.p ^ 1, L.err, 5, w_ae);
+            convert_rows<SUB_CG * 4, SUB_RS, SUB_CSB, F16, true>(a_st + ra.s * SUB_STAGE, ct, P.x0 + in_base, x1, x2, L.in_ld, c0 * 16,
+                                                            tau0 + P.in_off + mt * NCWG * 64, NCWG * 64 + (k - 1) * dil, in_lo, valid,
+                                                            L.pre_mode, L.pre_slope);
+            fence_proxy_async();
+            mbar_arrive(&a_full[ra.s]);
+            ra.next<NAS>();
+          }
+      } else {
+        for (int c = 0; c < nch; ++c) {
+          mbar_wait_t(&a_empty[ra.s], ra.p ^ 1, L.err, 5, w_ae);
+          convert_chunk<RA, F16>(a_st + ra.s * Cfg::A_STAGE, ct, P.x0 + in_base, x1, x2, L.in_ld, c, tau0 + P.in_off, R + (k - 1) * dil,
+                            in_lo, valid, L.pre_mode, L.pre_slope);
+          fence_proxy_async();
+          mbar_arrive(&a_full[ra.s]);
+          ra.next<NA>();
+        }
       }
       (void)out_hi; (void)e_lim;
     TILE_LOOP_END
@@ -455,11 +593,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
       // ... and the float4 at element e (of tile row tau) of the batch row's output (plain epilogue); with sub-row output
       // it lies in one output row (out_sub % 4 == 0)
       auto elem_ok = [&](int tau, int e) { return SUB ? e >= 0 && e < e_lim : row_ok(tau); };
+      // first row of the warpgroup's 64-row block mt: the warpgroup's MW blocks are adjacent, or (SUB) block mt of each
+      // warpgroup lies in row step mt
+      auto blk_row = [&](int mt) { return tau0 + (SUB ? mt * NCWG + wg : wg * MW + mt) * 64; };
       // cp.async the residual of pass (mt, nh) -- rows tau0 + (wg * MW + mt) * 64..., columns nh * EPI_NC... -- into
       // the staging rows; wait_pass makes every thread's copies visible to the warpgroup
       auto fetch_pass = [&](int mt, int nh) {
         if (P.resid) {
-          const int blk = tau0 + (wg * MW + mt) * 64;
+          const int blk = blk_row(mt);
 #pragma unroll
           for (int i = 0; i < NQ4; ++i) {
             const int row = i * RPS + dr, tau = blk + row;
@@ -479,8 +620,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
         if ((tid & 127) < N / 4) cp_async16(stg_bias + (tid & 127) * 4, P.bias + (tid & 127) * 4);
         fetch_pass(0, 0);
       }
-      consume<N, MW, RA, NW, true, false, F16>(acc, wg, smem_u32(a_st), a_full, a_empty, ra, smem_u32(w_st), w_full, w_empty, rw, nch, P.k,
-                                               P.dil, L.err, w_a, w_w);
+      if constexpr (SUB) {
+#pragma unroll
+        for (int mt = 0; mt < MW; ++mt)
+          consume_rows<N, NW, NAS, F16>(acc[mt], wg, smem_u32(a_st), a_full, a_empty, ra, smem_u32(w_st), w_full, w_empty, rw, nch, P.k,
+                                        P.dil, L.err, w_a, w_w);
+      } else {
+        consume<N, MW, RA, NW, true, false, F16>(acc, wg, smem_u32(a_st), a_full, a_empty, ra, smem_u32(w_st), w_full, w_empty, rw, nch,
+                                                 P.k, P.dil, L.err, w_a, w_w);
+      }
       const long long t_epi0 = clock64();
       if constexpr (EPI == 0) {
         // Staged through shared memory, one pass per 64-row block of the warpgroup and EPI_NC columns: the pass's
@@ -492,7 +640,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) tc_conv_kernel(const __grid_const
 #pragma unroll
         for (int mt = 0; mt < MW; ++mt) {
           // uniform over the warpgroup: past the last output row, so no later row of it is stored
-          const int blk = tau0 + (wg * MW + mt) * 64;
+          const int blk = blk_row(mt);
           if (SUB ? sub_elem(L, P, blk, 0) >= e_lim : !row_ok(blk)) break;
 #pragma unroll
           for (int nh = 0; nh < N / EPI_NC; ++nh) {
@@ -738,14 +886,15 @@ __global__ void pack_w_kernel(const float* __restrict__ w, uint16_t* __restrict_
 
 template <int N, int EPI, int MW, bool F16, bool SUB = false>
 int launch_cfg(vtts_ctx* ctx, TcLaunch& L, cudaStream_t st) {
-  using Cfg = TcCfg<N, MW, 0, EPI == 0>;
+  using Cfg = TcCfg<N, MW, 0, EPI == 0, SUB>;
   static bool attr_done_dev[64] = {};   // function attributes are per device (a process may hold contexts on several GPUs)
   if (!attr_done_dev[ctx->device & 63]) {
     VTTS_CUDA(cudaFuncSetAttribute(tc_conv_kernel<N, EPI, MW, F16, SUB>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_done_dev[ctx->device & 63] = true;
   }
   for (int i = 0; i < L.nprob; ++i)
-    if ((L.p[i].k - 1) * L.p[i].dil > HALO) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: halo too large");
+    if ((L.p[i].k - 1) * L.p[i].dil > (SUB ? SUB_HALO : HALO)) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: halo too large");
+  if (SUB && L.Cin % (SUB_CG * 16)) return ctx->fail(VTTS_ERR_BAD_ARG, "tc_conv: sub-row output needs Cin %% %d == 0, not %d", SUB_CG * 16, L.Cin);
   // the expensive problems (large k) first: within each row tile they are handed out before the cheap ones
   std::stable_sort(L.p, L.p + L.nprob, [](const TcProb& a, const TcProb& b) { return a.k > b.k; });
   L.tiles_per_row = ((L.tile_rows > 0 ? L.tile_rows : L.T_rows) + Cfg::R - 1) / Cfg::R;

@@ -660,6 +660,47 @@ int vtts_deesser_stream_push(vtts_ctx* ctx, vtts_deesser_stream* ds, const float
 int vtts_deesser_stream_push_host(vtts_ctx* ctx, vtts_deesser_stream* ds, const float* x, const int32_t* n_new, const uint8_t* flags,
                                   float* y, int32_t* n_out, float* reduction_db);
 
+/* ---- convolution reverb: a uniformly partitioned overlap-save FIR -------------------------------------------------
+ * One mono row x of n samples at rate r (an integer in [8000, 192000]), an impulse response h of L taps (1 <= L <= 5 r,
+ * finite) and mix in [0, 1] (anything else, NaN included, fails with VTTS_ERR_BAD_ARG before anything is launched):
+ *   c[t] = sum_{i=0}^{min(t, L-1)} h[i] x[t - i]  (causal, from zero state);  y[t] = (1 - mix) x[t] + mix c[t], t < n.
+ * The tail past the row's end is not emitted (pad x with zeros to hear it); mix = 0 returns x bit for bit.
+ * fp32 in every vtts_precision mode, evaluated as y = fmaf(fp32(mix), c, fp32(1 - mix) x) over 512-sample blocks and
+ * partitions fixed by absolute sample index: H_k = FFT-1024 of [h[512k .. 512k + 511], 0 x 512], X_j = FFT-1024 of x
+ * over [512 (j - 1), 512 (j + 1)) (zeros before 0 and from n on), and block j of c is samples 512..1023 of
+ * irfft(sum_{k <= min(j, K-1)} X_{j-k} H_k), K = ceil(L / 512), each bin summed in ascending k.  So a row gives the same
+ * bits alone, in any batch, and through the stream. */
+/* x_dev [B,S]; n_dev int32 [B] or NULL (= S; values clamped to [0, S]); ir_dev [L] on the device (its values are the
+ * caller's to check: vtts_reverb_host and the stream check them); y_dev [B,S] (may equal x_dev), 0 past n[b].
+ * Stream-ordered, no host synchronisation, four launches (IR spectra, input spectra, multiply-accumulate, inverse and
+ * mix); uses the context's workspace: 8 K * 513 bytes for the IR spectra plus about 16 bytes per sample. */
+int vtts_reverb(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, const float* ir_dev, int L, float mix,
+                float* y_dev, void* stream);
+/* the same on host buffers; n_in[b] must lie in [0, S] and every ir[i] be finite */
+int vtts_reverb_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, const float* ir, int L, float mix, float* y);
+/* Streaming reverb with max_streams independent slots; the IR (host [L]) and mix are fixed at create, where the IR's
+ * spectra are computed once.  Each slot carries a window of up to 1023 input samples (its last complete block and the
+ * incomplete one) and a frequency-domain delay line, the ring of its last R = K + ceil((max_chunk_samples + 511) / 512) - 1
+ * input spectra: S * R * 513 * 8 bytes in all (at 48 kHz with a 1.8 s IR, K = 172, about 0.7 MB per slot plus the
+ * chunk's share).  Block j is released with the push after which the slot has received 512 (j + 1) samples: before END
+ * a slot that has received p samples has emitted 512 floor(p / 512); END emits the rest (also with no new samples).
+ * vtts_reverb_stream_lookahead() = 511.  A slot's outputs, concatenated, equal vtts_reverb of its whole input bit for
+ * bit.  flags and slot rules as for the resample stream.  Every push issues the same four launches (window step,
+ * input spectra into the ring, multiply-accumulate over the ring, inverse and mix). */
+typedef struct vtts_reverb_stream vtts_reverb_stream;
+/* *out_pitch receives the outputs per slot of a push's output buffer (max_chunk_samples + 511) */
+int vtts_reverb_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int rate, const float* ir, int L, float mix,
+                              vtts_reverb_stream** out, int* out_pitch);
+int vtts_reverb_stream_destroy(vtts_ctx* ctx, vtts_reverb_stream* rs);
+int vtts_reverb_stream_lookahead(void);
+/* x_dev [S][max_chunk_samples] (samples past n_new[s] ignored); n_new, flags, n_out HOST int32 / uint8 / int32 [S];
+ * y_dev [S][out_pitch], slot s gets n_out[s] outputs from its start.  Stream-ordered. */
+int vtts_reverb_stream_push(vtts_ctx* ctx, vtts_reverb_stream* rs, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
+                            float* y_dev, int32_t* n_out, void* stream);
+/* the same on host buffers x [S][max_chunk_samples] and y [S][out_pitch]; returns when y is written */
+int vtts_reverb_stream_push_host(vtts_ctx* ctx, vtts_reverb_stream* rs, const float* x, const int32_t* n_new, const uint8_t* flags,
+                                 float* y, int32_t* n_out);
+
 /* ---- streaming acoustic model: every slot advances its decoder a few frames per push ---------------------------
  * A vtts_acoustic_stream holds max_streams (1..128) independent slots.  begin starts utterances in closed slots; each
  * push advances every open slot by min(F, frames left) decoder steps in ONE scan launch and returns the mel frames whose

@@ -206,6 +206,57 @@ def deesser_params(spec, rate: int) -> dict:
     return _keyed_params("deess", spec, ranges, DEESSER_PRESETS)
 
 
+# the synthetic room's parameters with their ranges (seed: an integer) and the presets; an IR may be at most 5 s long
+REVERB_RANGES = {"rt60": (0.1, 4.0), "predelay": (0.0, 200.0), "mix": (0.0, 1.0), "seed": (0.0, float(2 ** 24))}
+REVERB_PRESETS = {"room": {"rt60": 0.35, "predelay": 8.0, "mix": 0.15, "seed": 0.0},
+                  "hall": {"rt60": 1.8, "predelay": 25.0, "mix": 0.22, "seed": 0.0}}
+REVERB_MAX_IR_SECONDS = 5
+
+
+def reverb_ir(rt60: float, predelay_ms: float, seed: int, rate: int) -> np.ndarray:
+    """The synthetic room's impulse response (float32 [d + N]): d = round(predelay_ms rate / 1000) zeros, then Gaussian
+    noise e = default_rng(seed).standard_normal(N), N = ceil(rt60 rate), under the envelope 10^(-3 i / (rt60 rate)) (60 dB
+    down after rt60 seconds), scaled to unit energy in float64 and cast once."""
+    d = int(np.round(float(predelay_ms) * rate / 1000.0))
+    n = int(np.ceil(float(rt60) * rate))
+    e = np.random.default_rng(int(seed)).standard_normal(n)
+    h = np.zeros(d + n)
+    h[d:] = e * 10.0 ** (-3.0 * np.arange(n) / (float(rt60) * rate))
+    return (h / np.sqrt(np.sum(h * h))).astype(np.float32)
+
+
+def reverb_params(spec, rate: int) -> dict:
+    """{ir: float32 [L], mix: float32 value} of a reverb `spec` at `rate` Hz (an integer in [8000, 192000]).  `spec` is
+    a preset (`room`: rt60 0.35 s, predelay 8 ms, mix 0.15; `hall`: rt60 1.8 s, predelay 25 ms, mix 0.22; seed 0),
+    comma-separated key=value pairs over rt60, predelay, mix and seed (keys left out keep the room values), or a dict of
+    them; these give the synthetic room of `reverb_ir`, and the dict also carries rt60, predelay and seed.  rt60 s in
+    [0.1, 4], predelay ms in [0, 200], mix in [0, 1], seed an integer >= 0.  A dict may instead give `ir` (a float
+    array of 1 to 5 rate finite taps, used as given, not normalized) and `mix` (default the room's).  Raises ValueError
+    naming the key."""
+    _check_rate("reverb", rate)
+    rate = int(rate)
+    if isinstance(spec, dict) and "ir" in spec:
+        extra = set(spec) - {"ir", "mix"}
+        if extra:
+            raise ValueError(f"reverb: with ir= the only other key is mix, got {', '.join(sorted(extra))}")
+        try:
+            ir = np.ascontiguousarray(np.asarray(spec["ir"], np.float64).astype(np.float32)).ravel()
+        except (TypeError, ValueError):
+            raise ValueError("reverb: ir= must be an array of numbers") from None
+        if not 1 <= ir.size <= REVERB_MAX_IR_SECONDS * rate:
+            raise ValueError(f"reverb: ir has {ir.size} taps (1 to {REVERB_MAX_IR_SECONDS} s = {REVERB_MAX_IR_SECONDS * rate} at {rate} Hz)")
+        if not np.all(np.isfinite(ir)):
+            raise ValueError("reverb: ir taps must be finite")
+        mix = float(np.float32(_keyed_params("reverb", {"mix": spec.get("mix", REVERB_PRESETS["room"]["mix"])}, REVERB_RANGES,
+                                             REVERB_PRESETS, "room")["mix"]))
+        return {"ir": ir, "mix": mix}
+    p = {k: float(np.float32(v)) for k, v in _keyed_params("reverb", spec, REVERB_RANGES, REVERB_PRESETS, "room").items()}
+    if p["seed"] != int(p["seed"]):
+        raise ValueError(f"reverb: seed={p['seed']:g} must be an integer")
+    p["seed"] = int(p["seed"])
+    return dict(ir=reverb_ir(p["rt60"], p["predelay"], p["seed"], rate), **p)
+
+
 def _check_rate(what: str, rate):
     try:
         r = float(rate)
@@ -215,9 +266,9 @@ def _check_rate(what: str, rate):
         raise ValueError(f"{what}: rate {rate} must be an integer in [8000, 192000]")
 
 
-def _keyed_params(what: str, spec, ranges: dict, presets: dict) -> dict:
+def _keyed_params(what: str, spec, ranges: dict, presets: dict, default: str = "voice") -> dict:
     """the float32 values of a `spec` (a preset name, comma-separated key=value pairs, or a dict) over `ranges`, keys
-    left out taking presets["voice"]; every value must lie in its range.  Raises ValueError naming the key."""
+    left out taking presets[default]; every value must lie in its range.  Raises ValueError naming the key."""
     if isinstance(spec, str):
         given = {}
         s = spec.strip().lower()
@@ -232,7 +283,7 @@ def _keyed_params(what: str, spec, ranges: dict, presets: dict) -> dict:
         given = dict(spec)
     else:
         raise ValueError(f"{what}: a spec is a string or a dict, got {type(spec).__name__}")
-    out = dict(presets["voice"])
+    out = dict(presets[s] if isinstance(spec, str) and s in presets else presets[default])
     for key, val in given.items():
         if key not in ranges:
             raise ValueError(f"{what}: unknown key {key!r} (keys {', '.join(ranges)})")
@@ -247,7 +298,7 @@ def _keyed_params(what: str, spec, ranges: dict, presets: dict) -> dict:
     for key, v in out.items():       # the preset's values too: a range may depend on the rate
         lo, hi = ranges[key]
         if not lo <= v <= hi:
-            raise ValueError(f"{what}: {key}={v:g} (the voice preset's) must lie in [{lo:g}, {hi:g}] at this rate")
+            raise ValueError(f"{what}: {key}={v:g} (the {default} preset's) must lie in [{lo:g}, {hi:g}] at this rate")
     return out
 
 
@@ -314,6 +365,7 @@ class Engine:
         self._duration_key = None
         self._mel_fb = None         # host copy of the filterbank on the device (None: none loaded)
         self._denoise_bias = None   # default denoiser bias of the loaded generator in the current mode (denoiser_bias)
+        self._reverb_irs = {}       # (string spec, rate, device) -> (IR on the device, mix) of reverb_forward
 
     def close(self):
         if getattr(self, "h", None):
@@ -538,7 +590,7 @@ class Engine:
 
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
                         rng=None, output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None,
-                        gain_db=0.0, eq=None, compress=None, deess=None) -> "TtsStream":
+                        gain_db=0.0, eq=None, compress=None, deess=None, reverb=None) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
         With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  `output_rate`: a resample
@@ -561,12 +613,15 @@ class Engine:
         `deess`: a de-esser spec (`deesser_params`); a de-esser stream follows the compressor (before the limiter and the
         meter) at the output rate, and the audio equals `deess` of the (resampled, equalized, compressed) `tts` audio bit
         for bit.  It also adds no delay.
+        `reverb`: a reverb spec (`reverb_params`, presets and keys); a reverb stream follows the de-esser (before the
+        limiter and the meter) at the output rate, and the audio equals `reverb` of the (resampled, ..., de-essed) `tts`
+        audio bit for bit.  It holds back up to 511 samples until the next block of 512 is complete.
         `meter=True`: a loudness meter runs last, on what `step()` returns at the output rate (a
         multiple of 10), and `TtsStream.meter()` gives each stepped slot's readings, read back in the step's one
         synchronisation.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
         return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate,
                          denoise=denoise, meter=meter, semitones=semitones, tempo=tempo, limit=limit, gain_db=gain_db, eq=eq,
-                         compress=compress, deess=deess)
+                         compress=compress, deess=deess, reverb=reverb)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -1335,6 +1390,44 @@ class Engine:
         input bit for bit."""
         return DeesserStream(self, max_streams, max_chunk_samples, spec, rate)
 
+    # ---- convolution reverb (vtts_reverb*: partitioned overlap-save FIR, fp32) ----
+    def reverb(self, wav, spec="room", rate: int = config.SAMPLE_RATE, lengths=None) -> np.ndarray:
+        """Host array y: wav f32 [S] or [B,S] at `rate` through the reverb `spec` (see `reverb_params`): y = (1 - mix) x
+        + mix (h * x), the causal convolution with the IR h from zero state, its tail past each row's end not emitted.
+        mix = 0 returns wav exactly.  lengths int [B] in [0, S]: outputs past lengths[b] are 0."""
+        p = reverb_params(spec, rate)
+        x, lens, one = _wav_rows(wav, lengths)
+        B, S = x.shape
+        y = np.zeros((B, S), np.float32)
+        if B and S:
+            ir = p["ir"]
+            self._ck(self.lib.vtts_reverb_host(self.h, _ptr(x), _ptr(lens), B, S, int(rate), _ptr(ir), ir.size, p["mix"], _ptr(y)))
+        return y[0] if one else y
+
+    def reverb_forward(self, x_t, spec="room", rate: int = config.SAMPLE_RATE, lengths_t=None, out=None, stream=None):
+        """vtts_reverb on torch CUDA tensors, stream-ordered: returns y [B,S] on the device.  lengths_t int32 CUDA [B] or
+        None.  `out` may be x_t (in place).  The IR is copied to the device before the launches (once per string spec
+        and rate: it is kept for later calls)."""
+        import torch
+        B, S, out, st = _dev_rows(x_t, out, stream)
+        key = (spec, int(rate), x_t.device) if isinstance(spec, str) else None
+        cached = self._reverb_irs.get(key) if key else None
+        if cached is None:
+            p = reverb_params(spec, rate)
+            cached = (torch.from_numpy(p["ir"]).to(x_t.device), p["mix"])
+            if key:
+                self._reverb_irs[key] = cached
+        ir_t, mix = cached
+        self._ck(self.lib.vtts_reverb(self.h, _ptr(x_t), _ptr(lengths_t), B, S, int(rate), _ptr(ir_t), ir_t.numel(), mix, _ptr(out), st))
+        return out
+
+    def open_reverb_stream(self, max_streams: int, max_chunk_samples: int, spec="room",
+                           rate: int = config.SAMPLE_RATE) -> "ReverbStream":
+        """Streaming reverb with `max_streams` independent slots (vtts_reverb_stream_*): before END a slot that has
+        received p samples has emitted 512 floor(p / 512), and a slot's outputs, concatenated, equal `reverb` of its
+        whole input bit for bit."""
+        return ReverbStream(self, max_streams, max_chunk_samples, spec, rate)
+
 
 class Loudness(NamedTuple):
     integrated: np.ndarray     # LUFS (gated, BS.1770-4)
@@ -1750,6 +1843,26 @@ class DeesserStream(_ReductionStream):
         return self._push_device(x_t, n_new, flags, out_t, stream, dev=(reduction_t,))
 
 
+class ReverbStream(_SlotStream):
+    """Handle of a streaming reverb (Engine.open_reverb_stream).  Before END a slot that has received p samples has
+    emitted 512 floor(p / 512) outputs (`lookahead` = 511); a push with END emits the rest."""
+    _kind = "reverb_stream"
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, spec="room", rate: int = config.SAMPLE_RATE):
+        super().__init__(eng, max_streams, max_chunk_samples)
+        self.max_chunk_samples = self._chunk
+        self.params, self.rate = reverb_params(spec, rate), int(rate)
+        ir = self.params["ir"]
+        self._create(eng.lib.vtts_reverb_stream_create, self.max_streams, self.max_chunk_samples, self.rate, _ptr(ir), ir.size,
+                     self.params["mix"], pitch=True)
+        self.lookahead = int(eng.lib.vtts_reverb_stream_lookahead())
+
+
+def reverb_stream_emitted(p: int, end: bool = False) -> int:
+    """outputs a reverb stream slot has emitted after receiving p samples: 512 floor(p / 512), or p once END is pushed"""
+    return int(p) if end else 512 * (int(p) // 512)
+
+
 def acoustic_stream_schedule(n_frames: int, n_emit: int | None, chunk: int, lookahead: int = 10) -> list:
     """Frames an acoustic stream slot emits per push: it scans min(n_frames, n_emit + lookahead) frames, `chunk` per
     push; after P frames scanned it has emitted min(n_emit, max(0, P - lookahead)), and its last push emits the rest."""
@@ -1857,14 +1970,14 @@ class OptionError(ValueError):
 
 class AudioChain:
     """The audio stages after the vocoder, their options validated, in the one order every caller runs them: denoise,
-    pitch shift and time stretch at 16 kHz, then resample, equalize, compress, de-ess, limit (or normalize loudness) and
-    meter at the output rate.  `run` applies the chain to one waveform with the one-shot host calls; `streams` opens it as stream
+    pitch shift and time stretch at 16 kHz, then resample, equalize, compress, de-ess, reverb, limit (or normalize
+    loudness) and meter at the output rate.  `run` applies the chain to one waveform with the one-shot host calls; `streams` opens it as stream
     stages.  `loudness` (a target in LUFS, reached under `true_peak`, or under the limiter's ceiling with `limit`) has no
     streaming form, and `meter` only measures, so `run` leaves the audio as it is for it.  Raises OptionError (a
     ValueError naming the option) for an option out of range."""
 
     def __init__(self, denoise=None, semitones=None, tempo=None, output_rate=None, eq=None, limit=None, gain_db=0.0,
-                 loudness=None, true_peak=None, meter=False, compress=None, deess=None):
+                 loudness=None, true_peak=None, meter=False, compress=None, deess=None, reverb=None):
         def checked(option, check, *args):
             try:
                 return check(*args)
@@ -1879,6 +1992,9 @@ class AudioChain:
         self.eq = None if eq is None else checked("eq", eq_sections, eq, self.rate)
         self.compress = None if compress is None else checked("compress", compressor_params, compress, self.rate)
         self.deess = None if deess is None else checked("deess", deesser_params, deess, self.rate)
+        if reverb is not None:
+            checked("reverb", reverb_params, reverb, self.rate)
+        self.reverb = reverb           # the spec: the stages synthesize its IR where they open
         self.limit = None if limit is None else checked("limit", _limit_args, limit, self.rate, 5.0, 100.0)[0]
         self.gain_db = float(checked("gain_db", GAIN_DB.rows, gain_db, 1)[0]) if limit is not None else 0.0
         self.loudness = self.true_peak = None
@@ -1902,6 +2018,7 @@ class AudioChain:
             (self.compress is not None, "cp", lambda e, w: e.compress(w, self.compress, r)[0],
              lambda e, S, p, sec: CompressorStream(e, S, p, self.compress, r)),
             (self.deess is not None, "ds", lambda e, w: e.deess(w, self.deess, r)[0], lambda e, S, p, sec: DeesserStream(e, S, p, self.deess, r)),
+            (self.reverb is not None, "rv", lambda e, w: e.reverb(w, self.reverb, r), lambda e, S, p, sec: ReverbStream(e, S, p, self.reverb, r)),
             (self.loudness is not None, "lm",
              lambda e, w: e.normalize_loudness(w, self.loudness, r, true_peak=self.true_peak, limit=self.limit is not None)[0], None),
             (self.loudness is None and self.limit is not None, "lm", lambda e, w: e.limit(w, self.limit, r, self.gain_db)[0],
@@ -1941,14 +2058,14 @@ class TtsStream:
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
                  output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None, gain_db=0.0, eq=None,
-                 compress=None, deess=None):
+                 compress=None, deess=None, reverb=None):
         import torch
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
         self._chain = AudioChain(denoise=denoise, semitones=semitones, tempo=tempo, output_rate=output_rate, eq=eq, limit=limit,
-                                 gain_db=gain_db, meter=meter, compress=compress, deess=deess)
+                                 gain_db=gain_db, meter=meter, compress=compress, deess=deess, reverb=reverb)
         self.eng = eng
-        self.rs = self.dn = self.ps = self.ts = self.eq = self.cp = self.ds = self.lm = self.mt = None
+        self.rs = self.dn = self.ps = self.ts = self.eq = self.cp = self.ds = self.rv = self.lm = self.mt = None
         S = max_streams
         self._built = []   # every stream handle, in construction order
         try:

@@ -24,6 +24,9 @@ compressor, the `voice` preset or key=value settings) at the rate it is written,
 --limiter, so the limiter only catches what the compressor leaves.
 `--deess SPEC` turns down harsh sibilants of every output on the device (Engine.deess: the band above a crossover,
 only while it is loud) at the rate it is written, after --compress and before --loudness / --limiter.
+`--reverb SPEC` places every output in a synthetic room on the device (Engine.reverb: a convolution with a decaying
+noise impulse response, the `room` or `hall` preset or key=value settings) at the rate it is written, after --deess and
+before --loudness / --limiter.
 """
 from __future__ import annotations
 
@@ -118,7 +121,7 @@ def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_
 # the command-line flag of each AudioChain option the CLI sets
 _FLAGS = {"denoise": "--denoise", "semitones": "--pitch", "tempo": "--tempo", "output_rate": "--output-rate", "eq": "--eq",
           "limit": "--limiter", "loudness": "--loudness", "compress": "--compress",
-          "deess": "--deess"}
+          "deess": "--deess", "reverb": "--reverb"}
 
 
 def main(argv=None) -> int:
@@ -168,6 +171,11 @@ def main(argv=None) -> int:
                              "(5000 Hz crossover, -30 dBFS threshold, 4:1, 6 dB knee, 1 ms attack, 60 ms release, 12 dB range; "
                              "needs an output rate of at least 11112 Hz) or comma-separated freq=, threshold=, ratio=, knee=, "
                              "attack=, release=, range= (keys left out keep the voice values)")
+    parser.add_argument("--reverb", default=None, metavar="SPEC",
+                        help="add a synthetic room to every output on the device at the output rate, after --deess and "
+                             "before --loudness / --limiter: 'room' (rt60 0.35 s, 8 ms predelay, mix 0.15), 'hall' (rt60 "
+                             "1.8 s, 25 ms predelay, mix 0.22) or comma-separated rt60=, predelay=, mix=, seed= (keys left "
+                             "out keep the room values)")
     parser.add_argument("--silence-duration", default=-1, type=float)
     parser.add_argument("--lexicon-file", default=None)
     parser.add_argument("--seed", default=None, type=int,
@@ -195,7 +203,7 @@ def main(argv=None) -> int:
     try:
         chain = AudioChain(denoise=args.denoise, semitones=args.pitch, tempo=args.tempo, output_rate=args.output_rate, eq=args.eq,
                            limit=ceiling if args.limiter else None, loudness=args.loudness, true_peak=ceiling, compress=args.compress,
-                           deess=args.deess)
+                           deess=args.deess, reverb=args.reverb)
     except OptionError as e:
         parser.error(f"{_FLAGS[e.option]}: {e}")
     header_rate = args.output_rate or args.sample_rate or config.SAMPLE_RATE

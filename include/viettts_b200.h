@@ -701,6 +701,55 @@ int vtts_reverb_stream_push(vtts_ctx* ctx, vtts_reverb_stream* rs, const float* 
 int vtts_reverb_stream_push_host(vtts_ctx* ctx, vtts_reverb_stream* rs, const float* x, const int32_t* n_new, const uint8_t* flags,
                                  float* y, int32_t* n_out);
 
+/* ---- watermark: a keyed spread-spectrum mark and its batched detector ---------------------------------------------
+ * Embed, one mono 16 kHz row x of n samples, a key (any uint64) and a strength eps in [0, 0.3] (anything else, NaN
+ * included, fails with VTTS_ERR_BAD_ARG before anything is launched): the denoiser's STFT (n_fft 1024, hop 256, periodic
+ * Hann, centered frames with reflect padding), Y_f[k] = X_f[k] (1 + eps c(key, j, k)) for k in [20, 219) (312..3422 Hz),
+ * every other bin unchanged, j = floor(f / 4) mod 64, then the denoiser's overlap-add.  c = -1 where the top bit of word 0
+ * of threefry2x32(key_lo, key_hi, j, k) is set, else +1.  The pattern repeats every 65536 samples (4.096 s).  Digital
+ * silence stays silence; eps = 0 and rows of <= 512 samples return x bit for bit.  fp32 in every vtts_precision mode.
+ * Detect, per row and key: resample to 16 kHz (vtts_resample) when rate differs; log power of hop-64 frames whitened by
+ * its 9-bin moving mean across frequency; per frame phase q in [0, 16) the sums of groups of 4 hop-256 frames less half
+ * of each neighbouring group, folded onto the 64-group period (S_j); z = sum_{j,k} S_j[k] c(key, (j + p) mod 64, k) /
+ * sqrt(sum S^2) (0 when that is 0).  Aligned (search = 0): p = q = 0, offset 0.  Search: the largest z over the 1024
+ * (p, q) and its offset (1024 p - 64 q) mod 65536, where the row's sample 0 sits in the mark's period at 16 kHz (a crop
+ * starting at sample c of a marked row reports c mod 65536).  For audio that does not carry the key, z at one (p, q) is
+ * a Rademacher sum: P(z >= tau) <= exp(-tau^2 / 2) whatever the audio, so z >= 5 aligned (3.7e-6) and z >= 6.5 in search
+ * (1024 exp(-21.1) = 7e-7) are the library's thresholds.  Rows of <= 512 samples at 16 kHz give z = 0. */
+/* x_dev [B,S] at 16 kHz; n_dev int32 [B] or NULL (= S; values clamped to [0, S]); y_dev [B,S] (not x_dev), 0 past
+ * n[b].  Stream-ordered, no host synchronisation: two launches (frames, overlap-add), one with eps = 0 (the copy). */
+int vtts_watermark(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, uint64_t key, float strength, float* y_dev,
+                   void* stream);
+/* the same on host buffers; n_in[b] must lie in [0, S] */
+int vtts_watermark_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, uint64_t key, float strength, float* y);
+/* Streaming embedder with max_streams independent slots on the denoise stream's window and schedule: before END a slot
+ * that has received P samples has emitted min(P, 256 max(0, floor(P / 256) - 3)); END emits the rest.
+ * vtts_watermark_stream_lookahead() = 1023.  Key and strength are fixed at create.  A slot's outputs, concatenated, equal
+ * vtts_watermark of its whole input bit for bit.  flags and slot rules as for the resample stream; every push is one
+ * table copy plus three launches. */
+typedef struct vtts_watermark_stream vtts_watermark_stream;
+/* *out_pitch receives the outputs per slot of a push's output buffer (max_chunk_samples + 1023) */
+int vtts_watermark_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, uint64_t key, float strength,
+                                 vtts_watermark_stream** out, int* out_pitch);
+int vtts_watermark_stream_destroy(vtts_ctx* ctx, vtts_watermark_stream* ws);
+int vtts_watermark_stream_lookahead(void);
+/* x_dev [S][max_chunk_samples] (samples past n_new[s] ignored); n_new, flags, n_out HOST int32 / uint8 / int32 [S];
+ * y_dev [S][out_pitch], slot s gets n_out[s] outputs from its start.  Stream-ordered. */
+int vtts_watermark_stream_push(vtts_ctx* ctx, vtts_watermark_stream* ws, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
+                               float* y_dev, int32_t* n_out, void* stream);
+/* the same on host buffers x [S][max_chunk_samples] and y [S][out_pitch]; returns when y is written */
+int vtts_watermark_stream_push_host(vtts_ctx* ctx, vtts_watermark_stream* ws, const float* x, const int32_t* n_new, const uint8_t* flags,
+                                    float* y, int32_t* n_out);
+/* x_dev [B,S] at `rate` (an integer in [8000, 192000] whose ratio to 16000 the resampler takes); n_dev int32 [B] or
+ * NULL; keys_dev uint64 [K] on the device, 1 <= K <= 4096; search 0 (aligned) or not; z_dev float [B][K], offset_dev
+ * int32 [B][K].  Stream-ordered, no host synchronisation: three launches (four with the resampler); uses the context's
+ * workspace, about 3.2 bytes per 16 kHz sample plus 0.8 MB (search) or 51 KB (aligned) per row. */
+int vtts_watermark_detect(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, const uint64_t* keys_dev, int K,
+                          int search, float* z_dev, int32_t* offset_dev, void* stream);
+/* the same on host buffers; n_in[b] must lie in [0, S] */
+int vtts_watermark_detect_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, const uint64_t* keys, int K,
+                               int search, float* z, int32_t* offset);
+
 /* ---- streaming acoustic model: every slot advances its decoder a few frames per push ---------------------------
  * A vtts_acoustic_stream holds max_streams (1..128) independent slots.  begin starts utterances in closed slots; each
  * push advances every open slot by min(F, frames left) decoder steps in ONE scan launch and returns the mel frames whose

@@ -172,6 +172,17 @@ SIGNATURES = {
     "vtts_reverb_stream_lookahead": (C.c_int, []),
     "vtts_reverb_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtts_reverb_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_watermark": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint64, C.c_float, C.c_void_p, C.c_void_p]),
+    "vtts_watermark_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint64, C.c_float, C.c_void_p]),
+    "vtts_watermark_stream_create": (C.c_int, [c_ctx, C.c_int, C.c_int, C.c_uint64, C.c_float, C.POINTER(C.c_void_p), C.POINTER(C.c_int)]),
+    "vtts_watermark_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
+    "vtts_watermark_stream_lookahead": (C.c_int, []),
+    "vtts_watermark_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_watermark_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_watermark_detect": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                        C.c_void_p, C.c_void_p]),
+    "vtts_watermark_detect_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                             C.c_void_p, C.c_void_p]),
     "vtts_acoustic_stream_create":(C.c_int, [c_ctx, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, C.POINTER(C.c_void_p)]),
     "vtts_acoustic_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
     "vtts_acoustic_stream_lookahead": (C.c_int, []),

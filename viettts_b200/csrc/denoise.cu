@@ -3,7 +3,8 @@
 //   STFT n_fft 1024 / hop 256 / periodic Hann, centered frames with reflect padding 512 (F = n / 256 + 1 frames, frame f
 //   covers samples 256 f - 512 .. 256 f + 511) | |X| = sqrt(re^2 + im^2) | M' = max(|X| - s beta[k], 0) |
 //   Y = X M' / |X| (0 where |X| = 0) | ISTFT: overlap-add of w * irfft(Y_f) over the envelope sum_f w^2.
-// Rows of <= 512 samples cannot be reflect-padded and are copied.
+// Rows of <= 512 samples cannot be reflect-padded and are copied.  The frame kernel (with the gain below as its policy)
+// and the stream's schedule are stft_gain.cuh's, shared with the watermark embedder (watermark.cu).
 //
 // Frame kernel.  One warp per frame.  The frame is transformed ALONE: a complex FFT-1024 of the windowed real frame
 // (imaginary part zero), four-step 32 x 32 with both 32-point passes in registers (fftc::fft32) and exact table
@@ -26,84 +27,41 @@
 #include <cmath>
 #include <cstring>
 
-#include "stft_common.cuh"
-#include "stream_common.cuh"
+#include "stft_gain.cuh"
 
 namespace {
 
-using fftc::bitrev5;
-using stftc::fft1024;
-
-constexpr int NF = vc::NFFT;      // 1024
-constexpr int NB = vc::NBINS;     // 513
-constexpr int HOP = vc::HOP;      // 256
-constexpr int PAD = NF / 2;       // 512
-constexpr int DN_WARPS = 4;       // frames per CTA
-constexpr int TP = stftc::TP;     // transpose pitch (float2)
+using stftg::HOP;
+using stftg::NB;
+using stftg::NF;
+using stftg::PAD;
 constexpr int OLA_THREADS = 256;
-constexpr int DN_K = 2048;        // carried inputs per stream slot (the frames of a push start at most 1791 before P0)
-constexpr int DN_LOOKAHEAD = 1023;
 
-// rows == nullptr: the one-shot bounds of row b: n = n_in[b] clamped to [0, S] (or S), all S outputs written (zeros
-// past n), frames 0 .. n / 256 when n > 512
-__device__ __forceinline__ DnRow dn_row(const DnRow* rows, const int* n_in, int S, int b) {
-  if (rows) return rows[b];
-  DnRow r;
-  r.n = n_in ? (long long)min(max(n_in[b], 0), S) : (long long)S;
-  r.x0 = 0;
-  r.g0 = 0;
-  r.e0 = 0;
-  r.cnt = S;
-  r.copy = r.n <= PAD;
-  r.nfr = r.copy ? 0 : (int)(r.n / HOP + 1);
-  return r;
-}
+// spectral subtraction: |X| less strength * bias[k], floored at 0, with X's phase
+struct DnGain {
+  const float* __restrict__ bias;
+  float strength;
+  __device__ __forceinline__ float2 operator()(int k, long long, float2 X) const {
+    const float mag = sqrtf(X.x * X.x + X.y * X.y);
+    const float keep = fmaxf(mag - strength * __ldg(bias + k), 0.f);
+    const float gain = mag > 0.f ? keep / mag : 0.f;
+    return make_float2(X.x * gain, X.y * gain);
+  }
+};
 
-// MAG: write |X_0[k]| of frame 0 of row 0 to mag_out[k] (the bias of a waveform) and stop
-template <bool MAG>
-__global__ void __launch_bounds__(DN_WARPS * 32) denoise_frame_kernel(const float* __restrict__ x, long long x_ld, int S,
-                                                                      const int* __restrict__ n_in, const DnRow* __restrict__ rows,
-                                                                      const float* __restrict__ hann, const float2* __restrict__ tw,
-                                                                      const float* __restrict__ bias, float strength,
-                                                                      float* __restrict__ ws, int ws_frames, float* __restrict__ mag_out) {
-  __shared__ float2 smem[DN_WARPS * 32 * TP];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int b = blockIdx.y, fl = blockIdx.x * DN_WARPS + warp;
-  const DnRow r = dn_row(rows, n_in, S, b);
-  if (fl >= r.nfr || (MAG && fl > 0)) return;            // warps are independent: no block-level barrier below
-  float2* sw = smem + (size_t)warp * 32 * TP;
-  const float* xr = x + (size_t)b * x_ld;
-  const long long g = r.g0 + fl;
-  const long long j0 = g * HOP - PAD;
-
-  // ---- windowed frame: sample j0 + lane + 32 m, reflected at 0 and n - 1 of the row ----
+// |X_0[k]| of frame 0 of a row of n > 512 samples into mag_out[k] (the bias of a waveform); one warp
+__global__ void __launch_bounds__(32) denoise_mag_kernel(const float* __restrict__ x, long long n, const float* __restrict__ hann,
+                                                         const float2* __restrict__ tw, float* __restrict__ mag_out) {
+  __shared__ float2 sw[32 * stftc::TP];
+  const int lane = threadIdx.x;
   float2 v[32];
-  stftc::read_frame(v, xr, r.x0, r.n, j0, hann, lane);
-  fft1024(v, sw, tw, lane);
-
-  // ---- gain on bins k = lane + 32 k2 <= 512 ----
-  __syncwarp();                                          // every lane has read sw
+  stftc::read_frame(v, x, 0, n, -PAD, hann, lane);
+  stftc::fft1024(v, sw, tw, lane);
 #pragma unroll
   for (int p = 0; p < 32; ++p) {
-    const int k = lane + 32 * bitrev5(p);
-    if (k <= NB - 1) {
-      const float2 X = v[p];
-      const float mag = sqrtf(X.x * X.x + X.y * X.y);
-      if (MAG) {
-        mag_out[k] = mag;
-      } else {
-        const float keep = fmaxf(mag - strength * __ldg(bias + k), 0.f);
-        const float gain = mag > 0.f ? keep / mag : 0.f;
-        sw[k] = make_float2(X.x * gain, X.y * gain);
-      }
-    }
+    const int k = lane + 32 * fftc::bitrev5(p);
+    if (k <= NB - 1) mag_out[k] = sqrtf(v[p].x * v[p].x + v[p].y * v[p].y);
   }
-  if (MAG) return;
-  __syncwarp();
-
-  // ---- inverse: w * irfft(Y) of the gained spectrum ----
-  stftc::inverse_frame(v, sw, tw, lane);
-  stftc::write_frame(v, hann, lane, ws + ((size_t)b * ws_frames + fl) * NF);
 }
 
 __global__ void __launch_bounds__(OLA_THREADS) denoise_ola_kernel(const float* __restrict__ x, long long x_ld, int S,
@@ -112,7 +70,7 @@ __global__ void __launch_bounds__(OLA_THREADS) denoise_ola_kernel(const float* _
                                                                   int ws_frames, float* __restrict__ y, long long y_ld) {
   const int b = blockIdx.y;
   const long long q = (long long)blockIdx.x * OLA_THREADS + threadIdx.x;
-  const DnRow r = dn_row(rows, n_in, S, b);
+  const DnRow r = stftg::frame_row(rows, n_in, S, b);
   if (q >= r.cnt) return;
   const long long t = r.e0 + q;
   float out = 0.f;
@@ -148,18 +106,6 @@ int dn_check_bias(vtts_ctx* ctx, const char* who, const float* bias) {
   return VTTS_OK;
 }
 
-// frames then overlap-add: two launches
-int dn_launch(vtts_ctx* ctx, const float* x, long long x_ld, int S, const int* n_in, const DnRow* rows, int B, long long max_frames,
-              long long max_out, float strength, const float* bias, float* ws, int ws_frames, float* y, long long y_ld, cudaStream_t st) {
-  const float2* tw = reinterpret_cast<const float2*>(ctx->fft_tw);
-  const unsigned fgrid = (unsigned)std::max(1LL, (max_frames + DN_WARPS - 1) / DN_WARPS);
-  denoise_frame_kernel<false><<<dim3(fgrid, B), DN_WARPS * 32, 0, st>>>(x, x_ld, S, n_in, rows, ctx->hann, tw, bias, strength, ws, ws_frames,
-                                                                      nullptr);
-  ctx->launches++;
-  VTTS_CUDA(cudaGetLastError());
-  return vtts_denoise_ola(ctx, x, x_ld, S, n_in, rows, B, max_out, ws, ws_frames, y, y_ld, st);
-}
-
 }  // namespace
 
 int vtts_denoise_ola(vtts_ctx* ctx, const float* x, long long x_ld, int S, const int* n_in, const DnRow* rows, int B, long long max_out,
@@ -171,7 +117,7 @@ int vtts_denoise_ola(vtts_ctx* ctx, const float* x, long long x_ld, int S, const
   return VTTS_OK;
 }
 
-int vtts_denoise_stream_lookahead(void) { return DN_LOOKAHEAD; }
+int vtts_denoise_stream_lookahead(void) { return stftg::LOOKAHEAD; }
 
 int vtts_denoise(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, float strength, const float* bias_dev, float* y_dev,
                  void* stream) {
@@ -186,8 +132,8 @@ int vtts_denoise(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B,
   const int ws_frames = S / HOP + 1;
   rc = ctx->ensure_ws((size_t)B * ws_frames * NF * sizeof(float));
   if (rc) return rc;
-  return dn_launch(ctx, x_dev, S, S, n_dev, nullptr, B, ws_frames, S, strength, bias_dev, (float*)ctx->ws, ws_frames, y_dev, S,
-                   (cudaStream_t)stream);
+  return stftg::launch(ctx, x_dev, S, S, n_dev, nullptr, B, ws_frames, S, DnGain{bias_dev, strength}, (float*)ctx->ws, ws_frames, y_dev, S,
+                       (cudaStream_t)stream);
 }
 
 int vtts_denoise_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, float strength, const float* bias, float* y) {
@@ -216,19 +162,16 @@ int vtts_denoise_bias(vtts_ctx* ctx, const float* wav_dev, int n, float* bias_de
   VTTS_CUDA(cudaSetDevice(ctx->device));
   int rc = vtts_fft_tables(ctx);
   if (rc) return rc;
-  denoise_frame_kernel<true><<<dim3(1, 1), DN_WARPS * 32, 0, (cudaStream_t)stream>>>(
-      wav_dev, n, n, nullptr, nullptr, ctx->hann, reinterpret_cast<const float2*>(ctx->fft_tw), nullptr, 0.f, nullptr, 0, bias_dev);
+  denoise_mag_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(wav_dev, n, ctx->hann, reinterpret_cast<const float2*>(ctx->fft_tw), bias_dev);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   return VTTS_OK;
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
-struct vtts_denoise_stream : SampleStream<DnRow> {
-  using SampleStream::SampleStream;
-  int out_pitch = 0, ws_frames = 0;
+struct vtts_denoise_stream : stftg::Stream {
+  using Stream::Stream;
   float strength = 0.f;
-  float* ws = nullptr;          // frame workspace [S][ws_frames][1024]
   float* bias = nullptr;        // [513]
 };
 
@@ -246,15 +189,11 @@ int vtts_denoise_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_sam
   VTTS_CUDA(cudaSetDevice(ctx->device));
   rc = vtts_fft_tables(ctx);
   if (rc) return rc;
-  std::unique_ptr<vtts_denoise_stream> ds(new vtts_denoise_stream(ctx, max_streams, max_chunk_samples, DN_K));
-  // outputs per push: fewer than n_new + 256 before END, at most n_new + 1023 with it (E(P0) >= P0 - 1023)
-  ds->out_pitch = max_chunk_samples + DN_LOOKAHEAD;
-  // frames per push: outputs [E0, E1) read frames floor((E0 - 511) / 256) .. floor((E1 + 511) / 256)
-  ds->ws_frames = (ds->out_pitch + 2 * PAD) / HOP + 2;
+  std::unique_ptr<vtts_denoise_stream> ds(new vtts_denoise_stream(ctx, max_streams, max_chunk_samples));
   ds->strength = strength;
   rc = stream_alloc(ctx, "denoise_stream_create", *ds, [&](Arena& a) {
     ds->carve_window(a);
-    ds->ws = a.take<float>((size_t)max_streams * ds->ws_frames * NF);
+    ds->carve_ws(a);
     ds->bias = a.take<float>(NB);
     ds->carve_tables(a);
   });
@@ -274,48 +213,7 @@ int vtts_denoise_stream_push(vtts_ctx* ctx, vtts_denoise_stream* ds, const float
   if (!rc) rc = ds->slots.check(ctx, "denoise_stream_push", ds->F, n_new, flags);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int S = ds->S;
-  const SlotState& sl = ds->slots;
-
-  // ---- host bookkeeping: outputs [E0, E1) of this push and the frames they read ----
-  DnRow* rows = ds->rows<0>();
-  std::vector<long long> E1(S);
-  long long max_out = 0, max_frames = 0;
-  for (int s = 0; s < S; ++s) {
-    const bool act = SlotState::active(n_new, flags, s), begin = flags[s] & 1, end = flags[s] & 2;
-    const long long P0 = begin ? 0 : sl.P[s], E0 = begin ? 0 : sl.E[s], P1 = P0 + n_new[s];
-    long long e = E0;
-    if (act) e = end ? P1 : std::min(P1, (long long)HOP * std::max(0LL, P1 / HOP - 3));
-    E1[s] = e;
-    n_out[s] = (int32_t)(e - E0);
-    DnRow r{};
-    r.x0 = P0 - DN_K;
-    r.n = end ? P1 : DN_OPEN;
-    r.e0 = E0;
-    r.cnt = e - E0;
-    r.copy = end && P1 <= PAD;
-    if (r.cnt > 0 && !r.copy) {
-      const long long p0 = E0 + PAD, p1 = e - 1 + PAD;
-      r.g0 = p0 >= NF - 1 ? (p0 - (NF - 1) + HOP - 1) / HOP : 0;
-      r.nfr = (int)(std::min(r.n / HOP, p1 / HOP) - r.g0 + 1);
-    }
-    if (r.nfr > ds->ws_frames || r.cnt > ds->out_pitch)
-      return ctx->fail(VTTS_ERR_CUDA, "denoise_stream_push: slot %d needs %d frames / %lld outputs (internal bound %d / %d)", s, r.nfr,
-                       r.cnt, ds->ws_frames, ds->out_pitch);
-    rows[s] = r;
-    max_out = std::max(max_out, r.cnt);
-    max_frames = std::max(max_frames, (long long)r.nfr);
-  }
-
-  // ---- device: one table copy, prep, frames, overlap-add (three launches) ----
-  rc = ds->upload(n_new, flags, x_dev, st);
-  if (rc) return rc;
-  rc = dn_launch(ctx, ds->win, ds->cap, ds->cap, nullptr, ds->d_rows<0>(), S, max_frames, max_out, ds->strength, ds->bias, ds->ws, ds->ws_frames,
-                 y_dev, ds->out_pitch, st);
-  if (rc) return rc;
-  ds->slots.commit(n_new, flags, E1.data());
-  return VTTS_OK;
+  return ds->push("denoise_stream_push", x_dev, n_new, flags, y_dev, n_out, DnGain{ds->bias, ds->strength}, false, (cudaStream_t)stream);
 }
 
 int vtts_denoise_stream_push_host(vtts_ctx* ctx, vtts_denoise_stream* ds, const float* x, const int32_t* n_new, const uint8_t* flags,

@@ -14,6 +14,7 @@
 // are exchanged with one grid barrier per dependent phase.
 #include <cooperative_groups.h>
 
+#include "threefry.cuh"
 #include "vtts_internal.cuh"
 
 namespace cg = cooperative_groups;
@@ -29,28 +30,6 @@ constexpr int NSLICE = 64;    // K slices (SCAN_THREADS / 4 column groups)
 constexpr int MAX_ROWS = 128; // batch rows per scan launch
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
-
-// ---- threefry2x32 (20 rounds), the counter-based generator used for VTTS_DROPOUT_SEED ----------
-__host__ __device__ inline void threefry2x32(uint32_t k0, uint32_t k1, uint32_t c0, uint32_t c1, uint32_t& o0, uint32_t& o1) {
-  const uint32_t ks2 = 0x1BD11BDAu ^ k0 ^ k1;
-  uint32_t x0 = c0 + k0, x1 = c1 + k1;
-  const int R0[4] = {13, 15, 26, 6}, R1[4] = {17, 29, 16, 24};
-  const uint32_t ks[3] = {k0, k1, ks2};
-#pragma unroll
-  for (int blk = 0; blk < 5; ++blk) {
-    const int* R = (blk & 1) ? R1 : R0;
-#pragma unroll
-    for (int r = 0; r < 4; ++r) {
-      x0 += x1;
-      x1 = (x1 << R[r]) | (x1 >> (32 - R[r]));
-      x1 ^= x0;
-    }
-    x0 += ks[(blk + 1) % 3];
-    x1 += ks[(blk + 2) % 3] + (uint32_t)(blk + 1);
-  }
-  o0 = x0;
-  o1 = x1;
-}
 
 // jax split(key) in the classic layout: (next key, sub-key) = ((a0, b0), (a1, b1)) with (a0, a1) = threefry(key, (0, 2)),
 // (b0, b1) = threefry(key, (1, 3)); one hk.next_rng_key() call returns the sub-key

@@ -257,6 +257,71 @@ def reverb_params(spec, rate: int) -> dict:
     return dict(ir=reverb_ir(p["rt60"], p["predelay"], p["seed"], rate), **p)
 
 
+WATERMARK_MAX_STRENGTH = 0.3
+WATERMARK_STRENGTH = 0.1                           # the default strength
+WATERMARK_ALIGNED_THRESHOLD = 5.0                  # P(z >= 5) <= exp(-12.5) = 3.7e-6 for audio without the key
+WATERMARK_SEARCH_THRESHOLD = 6.5                   # 1024 offsets: P(max z >= 6.5) <= 1024 exp(-21.1) = 7e-7
+WATERMARK_MAX_KEYS = 4096                          # keys per detect call
+
+
+def _watermark_key(v) -> int:
+    """an integer in [0, 2^64) (a bool, a float or a string of anything else raises ValueError)"""
+    if isinstance(v, (bool, np.bool_)) or isinstance(v, (float, np.floating)):
+        raise ValueError(f"watermark: key {v!r} must be an integer in [0, 2^64)")
+    try:
+        k = int(v, 0) if isinstance(v, str) else int(v)
+    except (TypeError, ValueError):
+        raise ValueError(f"watermark: key {v!r} must be an integer in [0, 2^64)") from None
+    if not 0 <= k < 2 ** 64:
+        raise ValueError(f"watermark: key {k} must be an integer in [0, 2^64)")
+    return k
+
+
+def watermark_params(spec) -> dict:
+    """{key: int, strength: float32 value} of a watermark `spec`: a bare integer key (an int or a string such as
+    "12345" or "0x3039"), comma-separated `key=…,strength=…`, or a dict of them.  The key is an integer in [0, 2^64);
+    strength lies in [0, 0.3] (default 0.1; 0 leaves the audio exactly as it is).  Raises ValueError naming the key."""
+    if isinstance(spec, dict):
+        given = dict(spec)
+    elif isinstance(spec, str) and "=" in spec:
+        given = {}
+        for part in spec.split(","):
+            k, eq, v = part.partition("=")
+            k = k.strip().lower()
+            if not eq or not k:
+                raise ValueError(f"watermark: {part.strip()!r} is not key=value")
+            given[k] = v.strip()
+    else:
+        given = {"key": spec}
+    extra = set(given) - {"key", "strength"}
+    if extra:
+        raise ValueError(f"watermark: unknown key {sorted(extra)[0]!r} (keys key, strength)")
+    if "key" not in given:
+        raise ValueError("watermark: key= is required")
+    key = _watermark_key(given["key"])
+    try:
+        eps = float(given.get("strength", WATERMARK_STRENGTH))
+    except (TypeError, ValueError):
+        raise ValueError(f"watermark: strength={given['strength']!r} must be a number") from None
+    if not 0.0 <= np.float32(eps) <= np.float32(WATERMARK_MAX_STRENGTH):      # NaN fails too; as the library compares
+        raise ValueError(f"watermark: strength={eps:g} must lie in [0, {WATERMARK_MAX_STRENGTH:g}]")
+    return {"key": key, "strength": float(np.float32(eps))}
+
+
+def watermark_keys(keys) -> np.ndarray:
+    """uint64 [K] of one key or a list of 1 to 4096 keys, each an integer in [0, 2^64)"""
+    ks = [keys] if np.ndim(keys) == 0 else list(np.asarray(keys, object).ravel())
+    if not 1 <= len(ks) <= WATERMARK_MAX_KEYS:
+        raise ValueError(f"watermark: {len(ks)} keys (1 to {WATERMARK_MAX_KEYS})")
+    return np.array([_watermark_key(k) for k in ks], np.uint64)
+
+
+class WatermarkDetection(NamedTuple):
+    z: np.ndarray          # float32 [B, K] (or [K] for one row): the detection score
+    offset: np.ndarray     # int32, same shape: where sample 0 sits in the mark's 65536-sample period at 16 kHz
+    detected: np.ndarray   # bool, same shape: z at or above the mode's threshold
+
+
 def _check_rate(what: str, rate):
     try:
         r = float(rate)
@@ -590,7 +655,7 @@ class Engine:
 
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
                         rng=None, output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None,
-                        gain_db=0.0, eq=None, compress=None, deess=None, reverb=None) -> "TtsStream":
+                        gain_db=0.0, eq=None, compress=None, deess=None, reverb=None, watermark=None) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
         With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  `output_rate`: a resample
@@ -616,12 +681,15 @@ class Engine:
         `reverb`: a reverb spec (`reverb_params`, presets and keys); a reverb stream follows the de-esser (before the
         limiter and the meter) at the output rate, and the audio equals `reverb` of the (resampled, ..., de-essed) `tts`
         audio bit for bit.  It holds back up to 511 samples until the next block of 512 is complete.
+        `watermark`: a watermark spec (`watermark_params`: a key, or key=…,strength=…); a watermark stream follows the
+        time stretcher (before the resampler) at 16 kHz, and the audio equals `watermark` of the (denoised, shifted,
+        stretched) `tts` audio bit for bit.  Every slot carries the same key.  It holds back up to 1023 samples.
         `meter=True`: a loudness meter runs last, on what `step()` returns at the output rate (a
         multiple of 10), and `TtsStream.meter()` gives each stepped slot's readings, read back in the step's one
         synchronisation.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
         return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate,
                          denoise=denoise, meter=meter, semitones=semitones, tempo=tempo, limit=limit, gain_db=gain_db, eq=eq,
-                         compress=compress, deess=deess, reverb=reverb)
+                         compress=compress, deess=deess, reverb=reverb, watermark=watermark)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -1428,6 +1496,69 @@ class Engine:
         whole input bit for bit."""
         return ReverbStream(self, max_streams, max_chunk_samples, spec, rate)
 
+    # ---- watermark (vtts_watermark*: a keyed spread-spectrum mark on the denoiser's STFT, fp32) ----
+    def watermark(self, wav, spec, lengths=None) -> np.ndarray:
+        """Host array y: wav f32 [S] or [B,S] at 16 kHz marked with the key of `spec` (see `watermark_params`): every
+        STFT bin from 312 to 3422 Hz scaled by 1 +- strength after the key's chip pattern.  strength 0 and rows of <= 512
+        samples return wav exactly.  lengths int [B] in [0, S]: outputs past lengths[b] are 0."""
+        p = watermark_params(spec)
+        x, lens, one = _wav_rows(wav, lengths)
+        B, S = x.shape
+        y = np.zeros((B, S), np.float32)
+        if B and S:
+            self._ck(self.lib.vtts_watermark_host(self.h, _ptr(x), _ptr(lens), B, S, p["key"], p["strength"], _ptr(y)))
+        return y[0] if one else y
+
+    def watermark_forward(self, x_t, spec, lengths_t=None, out=None, stream=None):
+        """vtts_watermark on torch CUDA tensors, stream-ordered: x_t f32 [B,S] at 16 kHz -> [B,S] (not x_t itself);
+        lengths_t int32 CUDA [B] or None."""
+        p = watermark_params(spec)
+        B, S, out, st = _dev_rows(x_t, out, stream)
+        self._ck(self.lib.vtts_watermark(self.h, _ptr(x_t), _ptr(lengths_t), B, S, p["key"], p["strength"], _ptr(out), st))
+        return out
+
+    def open_watermark_stream(self, max_streams: int, max_chunk_samples: int, spec) -> "WatermarkStream":
+        """Streaming watermark with `max_streams` independent slots (vtts_watermark_stream_*), key and strength fixed:
+        each slot's outputs, concatenated, equal `watermark` of its whole input bit for bit, on the denoise stream's
+        schedule (at most 1023 samples of lookahead)."""
+        return WatermarkStream(self, max_streams, max_chunk_samples, spec)
+
+    def detect_watermark(self, wav, keys, rate: int = config.SAMPLE_RATE, lengths=None, search: bool = True) -> WatermarkDetection:
+        """Scores host audio wav f32 [S] or [B,S] at `rate` against every key of `keys` (one or up to 4096 integers).
+        search=True: the largest score over the 1024 offsets of the mark's period, so a crop is found wherever it
+        starts; search=False: the score at offset 0, for audio that starts where the mark started.  `detected` is
+        z >= 6.5 (search) or z >= 5 (aligned); for audio without the key these are crossed with probability at most
+        7e-7 and 3.7e-6 per row and key.  Returns (z, offset, detected), each [B,K] (or [K] for one row)."""
+        rate = _output_rate(rate)
+        ks = watermark_keys(keys)
+        x, lens, one = _wav_rows(wav, lengths)
+        B, S = x.shape
+        K = ks.size
+        z = np.zeros((B, K), np.float32)
+        off = np.zeros((B, K), np.int32)
+        if B and S:
+            self._ck(self.lib.vtts_watermark_detect_host(self.h, _ptr(x), _ptr(lens), B, S, rate, _ptr(ks), K, int(bool(search)),
+                                                         _ptr(z), _ptr(off)))
+        det = z >= (WATERMARK_SEARCH_THRESHOLD if search else WATERMARK_ALIGNED_THRESHOLD)
+        return WatermarkDetection(z[0], off[0], det[0]) if one else WatermarkDetection(z, off, det)
+
+    def detect_watermark_forward(self, x_t, keys, rate: int = config.SAMPLE_RATE, lengths_t=None, search: bool = True,
+                                 stream=None) -> WatermarkDetection:
+        """vtts_watermark_detect on torch CUDA tensors, stream-ordered: x_t f32 [B,S] at `rate`; keys a uint64 CUDA
+        tensor [K] (torch.uint64) or host keys, copied to the device.  Returns (z f32 [B,K], offset int32 [B,K], detected
+        bool [B,K]) as CUDA tensors."""
+        import torch
+        rate = _output_rate(rate)
+        if not (isinstance(keys, torch.Tensor) and keys.is_cuda):
+            keys = torch.from_numpy(watermark_keys(keys)).to(x_t.device)
+        if keys.dtype != torch.uint64 or keys.dim() != 1 or not keys.is_contiguous() or not 1 <= keys.numel() <= WATERMARK_MAX_KEYS:
+            raise ValueError(f"keys must be a contiguous uint64 tensor of 1 to {WATERMARK_MAX_KEYS} keys")
+        B, S, z, st = _dev_rows(x_t, None, stream, keys.numel())
+        off = torch.empty((B, keys.numel()), dtype=torch.int32, device=x_t.device)
+        self._ck(self.lib.vtts_watermark_detect(self.h, _ptr(x_t), _ptr(lengths_t), B, S, rate, _ptr(keys), keys.numel(), int(bool(search)),
+                                                _ptr(z), _ptr(off), st))
+        return WatermarkDetection(z, off, z >= (WATERMARK_SEARCH_THRESHOLD if search else WATERMARK_ALIGNED_THRESHOLD))
+
 
 class Loudness(NamedTuple):
     integrated: np.ndarray     # LUFS (gated, BS.1770-4)
@@ -1858,6 +1989,20 @@ class ReverbStream(_SlotStream):
         self.lookahead = int(eng.lib.vtts_reverb_stream_lookahead())
 
 
+class WatermarkStream(_SlotStream):
+    """Handle of a streaming watermark (Engine.open_watermark_stream).  Before END a slot that has received P samples
+    has emitted min(P, 256 max(0, floor(P / 256) - 3)) outputs; a push with END emits the rest."""
+    _kind = "watermark_stream"
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, spec):
+        super().__init__(eng, max_streams, max_chunk_samples)
+        self.max_chunk_samples = self._chunk
+        self.params = watermark_params(spec)
+        self._create(eng.lib.vtts_watermark_stream_create, self.max_streams, self.max_chunk_samples, self.params["key"],
+                     self.params["strength"], pitch=True)
+        self.lookahead = int(eng.lib.vtts_watermark_stream_lookahead())
+
+
 def reverb_stream_emitted(p: int, end: bool = False) -> int:
     """outputs a reverb stream slot has emitted after receiving p samples: 512 floor(p / 512), or p once END is pushed"""
     return int(p) if end else 512 * (int(p) // 512)
@@ -1970,14 +2115,15 @@ class OptionError(ValueError):
 
 class AudioChain:
     """The audio stages after the vocoder, their options validated, in the one order every caller runs them: denoise,
-    pitch shift and time stretch at 16 kHz, then resample, equalize, compress, de-ess, reverb, limit (or normalize
-    loudness) and meter at the output rate.  `run` applies the chain to one waveform with the one-shot host calls; `streams` opens it as stream
+    pitch shift, time stretch and watermark at 16 kHz, then resample, equalize, compress, de-ess, reverb, limit (or
+    normalize loudness) and meter at the output rate.  The watermark is the last 16 kHz stage, after everything that
+    moves time or pitch.  `run` applies the chain to one waveform with the one-shot host calls; `streams` opens it as stream
     stages.  `loudness` (a target in LUFS, reached under `true_peak`, or under the limiter's ceiling with `limit`) has no
     streaming form, and `meter` only measures, so `run` leaves the audio as it is for it.  Raises OptionError (a
     ValueError naming the option) for an option out of range."""
 
     def __init__(self, denoise=None, semitones=None, tempo=None, output_rate=None, eq=None, limit=None, gain_db=0.0,
-                 loudness=None, true_peak=None, meter=False, compress=None, deess=None, reverb=None):
+                 loudness=None, true_peak=None, meter=False, compress=None, deess=None, reverb=None, watermark=None):
         def checked(option, check, *args):
             try:
                 return check(*args)
@@ -1989,6 +2135,7 @@ class AudioChain:
         self.denoise = None if denoise is None else checked("denoise", _strength, denoise)
         self.semitones = None if semitones is None else float(checked("semitones", SEMITONES.rows, semitones, 1)[0])
         self.tempo = None if tempo is None else float(checked("tempo", TEMPO.rows, tempo, 1)[0])
+        self.watermark = None if watermark is None else checked("watermark", watermark_params, watermark)
         self.eq = None if eq is None else checked("eq", eq_sections, eq, self.rate)
         self.compress = None if compress is None else checked("compress", compressor_params, compress, self.rate)
         self.deess = None if deess is None else checked("deess", deesser_params, deess, self.rate)
@@ -2012,6 +2159,8 @@ class AudioChain:
              lambda e, S, p, sec: DenoiseStream(e, S, p, self.denoise)),
             (self.semitones is not None, "ps", lambda e, w: e.pitch_shift(w, self.semitones), lambda e, S, p, sec: PitchShiftStream(e, S, p)),
             (self.tempo is not None, "ts", lambda e, w: e.time_stretch(w, self.tempo), lambda e, S, p, sec: TimeStretchStream(e, S, p)),
+            (self.watermark is not None, "wm", lambda e, w: e.watermark(w, self.watermark),
+             lambda e, S, p, sec: WatermarkStream(e, S, p, self.watermark)),
             (self.output_rate is not None, "rs", lambda e, w: e.resample(w, self.output_rate),
              lambda e, S, p, sec: ResampleStream(e, S, p, self.output_rate)),
             (self.eq is not None, "eq", lambda e, w: e.equalize(w, self.eq, r), lambda e, S, p, sec: EqStream(e, S, p, self.eq, r)),
@@ -2058,14 +2207,15 @@ class TtsStream:
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
                  output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None, gain_db=0.0, eq=None,
-                 compress=None, deess=None, reverb=None):
+                 compress=None, deess=None, reverb=None, watermark=None):
         import torch
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
         self._chain = AudioChain(denoise=denoise, semitones=semitones, tempo=tempo, output_rate=output_rate, eq=eq, limit=limit,
-                                 gain_db=gain_db, meter=meter, compress=compress, deess=deess, reverb=reverb)
+                                 gain_db=gain_db, meter=meter, compress=compress, deess=deess, reverb=reverb,
+                                 watermark=watermark)
         self.eng = eng
-        self.rs = self.dn = self.ps = self.ts = self.eq = self.cp = self.ds = self.rv = self.lm = self.mt = None
+        self.rs = self.dn = self.ps = self.ts = self.wm = self.eq = self.cp = self.ds = self.rv = self.lm = self.mt = None
         S = max_streams
         self._built = []   # every stream handle, in construction order
         try:

@@ -27,6 +27,9 @@ only while it is loud) at the rate it is written, after --compress and before --
 `--reverb SPEC` places every output in a synthetic room on the device (Engine.reverb: a convolution with a decaying
 noise impulse response, the `room` or `hall` preset or key=value settings) at the rate it is written, after --deess and
 before --loudness / --limiter.
+`--watermark SPEC` marks every output with a key on the device (Engine.watermark: a keyed spread-spectrum mark, a bare
+integer key or key=…,strength=…) at 16 kHz, after --tempo and before any resampling; `python -m viettts_b200.watermark
+detect --key K FILE.wav` checks a written file for it.
 """
 from __future__ import annotations
 
@@ -121,7 +124,7 @@ def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_
 # the command-line flag of each AudioChain option the CLI sets
 _FLAGS = {"denoise": "--denoise", "semitones": "--pitch", "tempo": "--tempo", "output_rate": "--output-rate", "eq": "--eq",
           "limit": "--limiter", "loudness": "--loudness", "compress": "--compress",
-          "deess": "--deess", "reverb": "--reverb"}
+          "deess": "--deess", "reverb": "--reverb", "watermark": "--watermark"}
 
 
 def main(argv=None) -> int:
@@ -176,6 +179,10 @@ def main(argv=None) -> int:
                              "before --loudness / --limiter: 'room' (rt60 0.35 s, 8 ms predelay, mix 0.15), 'hall' (rt60 "
                              "1.8 s, 25 ms predelay, mix 0.22) or comma-separated rt60=, predelay=, mix=, seed= (keys left "
                              "out keep the room values)")
+    parser.add_argument("--watermark", default=None, metavar="SPEC",
+                        help="mark every output with a key on the device at 16 kHz, after --tempo and before --output-rate: "
+                             "an integer key in [0, 2^64) or key=K,strength=S (S in [0, 0.3], default 0.1); "
+                             "`python -m viettts_b200.watermark detect --key K FILE.wav` detects it")
     parser.add_argument("--silence-duration", default=-1, type=float)
     parser.add_argument("--lexicon-file", default=None)
     parser.add_argument("--seed", default=None, type=int,
@@ -203,7 +210,7 @@ def main(argv=None) -> int:
     try:
         chain = AudioChain(denoise=args.denoise, semitones=args.pitch, tempo=args.tempo, output_rate=args.output_rate, eq=args.eq,
                            limit=ceiling if args.limiter else None, loudness=args.loudness, true_peak=ceiling, compress=args.compress,
-                           deess=args.deess, reverb=args.reverb)
+                           deess=args.deess, reverb=args.reverb, watermark=args.watermark)
     except OptionError as e:
         parser.error(f"{_FLAGS[e.option]}: {e}")
     header_rate = args.output_rate or args.sample_rate or config.SAMPLE_RATE

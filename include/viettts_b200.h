@@ -750,6 +750,25 @@ int vtts_watermark_detect(vtts_ctx* ctx, const float* x_dev, const int32_t* n_de
 int vtts_watermark_detect_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, const uint64_t* keys, int K,
                                int search, float* z, int32_t* offset);
 
+/* ---- wire encodings: PCM-16 and G.711 mu-law / A-law -----------------------------------------------------------
+ * Encode, per float32 sample x: v = clip(rint(x * 32767), -32768, 32767), the product in double and rint rounding half
+ * to even (NaN gives 0, +-Inf clip): the float -> PCM_16 conversion of libsndfile.  VTTS_ENC_PCM16 stores v as int16;
+ * VTTS_ENC_ULAW stores the G.711 mu-law code of v >> 2 and VTTS_ENC_ALAW the G.711 A-law code of v >> 3, one uint8
+ * each (the codes of CPython's audioop.lin2ulaw / lin2alaw at width 2).  Decode is the G.711 expansion of a code to
+ * int16 (mu-law 0x00 -> -32124), or the int16 itself, divided by 32767 in fp32.  Bit-exact in every vtts_precision
+ * mode.  Any other encoding, B outside [1, 65535], S < 1, a null buffer or an output that overlaps the input fails with
+ * VTTS_ERR_BAD_ARG before anything is launched. */
+typedef enum vtts_encoding { VTTS_ENC_PCM16 = 0, VTTS_ENC_ULAW = 1, VTTS_ENC_ALAW = 2 } vtts_encoding;
+/* x_dev float [B,S]; n_dev int32 [B] or NULL (= S; values clamped to [0, S]); y_dev [B,S] int16 (PCM16) or uint8
+ * (ULAW, ALAW), the code of 0 past n[b] (0, 0xFF, 0xD5).  Stream-ordered, no host synchronisation: one launch. */
+int vtts_encode(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int encoding, void* y_dev, void* stream);
+/* the same on host buffers; n_in[b] must lie in [0, S] */
+int vtts_encode_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int encoding, void* y);
+/* c_dev [B,S] int16 (PCM16) or uint8 codes; n_dev as above; y_dev float [B,S], 0 past n[b].  One launch. */
+int vtts_decode(vtts_ctx* ctx, const void* c_dev, const int32_t* n_dev, int B, int S, int encoding, float* y_dev, void* stream);
+/* the same on host buffers; n_in[b] must lie in [0, S] */
+int vtts_decode_host(vtts_ctx* ctx, const void* c, const int32_t* n_in, int B, int S, int encoding, float* y);
+
 /* ---- streaming acoustic model: every slot advances its decoder a few frames per push ---------------------------
  * A vtts_acoustic_stream holds max_streams (1..128) independent slots.  begin starts utterances in closed slots; each
  * push advances every open slot by min(F, frames left) decoder steps in ONE scan launch and returns the mel frames whose

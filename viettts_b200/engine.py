@@ -316,6 +316,17 @@ def watermark_keys(keys) -> np.ndarray:
     return np.array([_watermark_key(k) for k in ks], np.uint64)
 
 
+ENCODINGS = {"pcm16": 0, "ulaw": 1, "alaw": 2}       # vtts_encoding
+ENCODING_DTYPES = {"pcm16": np.int16, "ulaw": np.uint8, "alaw": np.uint8}
+
+
+def encoding_name(encoding) -> str:
+    """the name of a wire encoding ('pcm16', 'ulaw' or 'alaw'; anything else raises ValueError)"""
+    if encoding not in ENCODINGS:
+        raise ValueError(f"encoding {encoding!r} must be one of {', '.join(ENCODINGS)}")
+    return encoding
+
+
 class WatermarkDetection(NamedTuple):
     z: np.ndarray          # float32 [B, K] (or [K] for one row): the detection score
     offset: np.ndarray     # int32, same shape: where sample 0 sits in the mark's 65536-sample period at 16 kHz
@@ -400,6 +411,22 @@ def _out_tensor(out, shape, device, what="out"):
         return torch.empty(shape, dtype=torch.float32, device=device)
     if tuple(out.shape) != shape or out.dtype != torch.float32 or not out.is_contiguous() or out.device != torch.device(device):
         raise ValueError(f"{what} must be contiguous float32 [{', '.join(map(str, shape))}] on {device}")
+    return out
+
+
+def _torch_code_dtype(encoding: str):
+    import torch
+    return torch.int16 if encoding == "pcm16" else torch.uint8
+
+
+def _code_tensor(out, shape, encoding: str, device):
+    """`out` checked to be a contiguous code tensor of `shape` for `encoding`, or a new one on `device`"""
+    import torch
+    dt = _torch_code_dtype(encoding)
+    if out is None:
+        return torch.empty(shape, dtype=dt, device=device)
+    if tuple(out.shape) != shape or out.dtype != dt or not out.is_contiguous() or out.device != torch.device(device):
+        raise ValueError(f"out must be contiguous {dt} [{', '.join(map(str, shape))}] on {device}")
     return out
 
 
@@ -655,7 +682,8 @@ class Engine:
 
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
                         rng=None, output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None,
-                        gain_db=0.0, eq=None, compress=None, deess=None, reverb=None, watermark=None) -> "TtsStream":
+                        gain_db=0.0, eq=None, compress=None, deess=None, reverb=None, watermark=None,
+                        encoding=None) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
         With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  `output_rate`: a resample
@@ -684,12 +712,15 @@ class Engine:
         `watermark`: a watermark spec (`watermark_params`: a key, or key=…,strength=…); a watermark stream follows the
         time stretcher (before the resampler) at 16 kHz, and the audio equals `watermark` of the (denoised, shifted,
         stretched) `tts` audio bit for bit.  Every slot carries the same key.  It holds back up to 1023 samples.
+        `encoding`: 'pcm16', 'ulaw' or 'alaw'; after the meter the last stage's buffer is encoded on the device
+        (`encode_forward` over the whole buffer) and `step()` copies and returns those codes (2 or 1 bytes per sample
+        instead of 4), equal to `encode` of the float audio bit for bit.
         `meter=True`: a loudness meter runs last, on what `step()` returns at the output rate (a
         multiple of 10), and `TtsStream.meter()` gives each stepped slot's readings, read back in the step's one
         synchronisation.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
         return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate,
                          denoise=denoise, meter=meter, semitones=semitones, tempo=tempo, limit=limit, gain_db=gain_db, eq=eq,
-                         compress=compress, deess=deess, reverb=reverb, watermark=watermark)
+                         compress=compress, deess=deess, reverb=reverb, watermark=watermark, encoding=encoding)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -1559,6 +1590,63 @@ class Engine:
                                                 _ptr(z), _ptr(off), st))
         return WatermarkDetection(z, off, z >= (WATERMARK_SEARCH_THRESHOLD if search else WATERMARK_ALIGNED_THRESHOLD))
 
+    # ---- wire encodings (vtts_encode / vtts_decode: PCM-16, G.711 mu-law and A-law, bit-exact) ----
+    def encode(self, wav, encoding, lengths=None) -> np.ndarray:
+        """Codes of host audio wav f32 [S] or [B,S] in `encoding` (see `encoding_name`): np.int16 for 'pcm16' (as
+        synthesizer.float_to_pcm16, NaN as 0), np.uint8 G.711 codes for 'ulaw' and 'alaw'; the same shape.  lengths int
+        [B] in [0, S]: outputs past lengths[b] are the code of 0."""
+        enc = encoding_name(encoding)
+        x, lens, one = _wav_rows(wav, lengths)
+        B, S = x.shape
+        y = np.zeros((B, S), ENCODING_DTYPES[enc])
+        if B and S:
+            self._ck(self.lib.vtts_encode_host(self.h, _ptr(x), _ptr(lens), B, S, ENCODINGS[enc], _ptr(y)))
+        return y[0] if one else y
+
+    def encode_forward(self, x_t, encoding, lengths_t=None, out=None, stream=None):
+        """vtts_encode on torch CUDA tensors, stream-ordered: x_t f32 [B,S] -> an int16 ('pcm16') or uint8 tensor [B,S]
+        (`out`, contiguous, of that dtype and shape, or a new one); lengths_t int32 CUDA [B] or None."""
+        import torch
+        enc = encoding_name(encoding)
+        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
+        B, S = x_t.shape
+        out = _code_tensor(out, (B, S), enc, x_t.device)
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self._ck(self.lib.vtts_encode(self.h, _ptr(x_t), _ptr(lengths_t), B, S, ENCODINGS[enc], _ptr(out), st))
+        return out
+
+    def decode(self, codes, encoding, lengths=None) -> np.ndarray:
+        """Host float32 audio of codes [S] or [B,S] in `encoding` (int16 for 'pcm16', uint8 otherwise): the G.711
+        expansion to int16 (or the int16 itself) over 32767, as synthesizer.read_wav scales.  Outputs past lengths[b]
+        are 0."""
+        enc = encoding_name(encoding)
+        c = np.ascontiguousarray(codes)
+        if c.dtype != ENCODING_DTYPES[enc]:
+            raise ValueError(f"{enc} codes must be {np.dtype(ENCODING_DTYPES[enc]).name}, got {c.dtype}")
+        one = c.ndim == 1
+        c = c[None] if one else c
+        if c.ndim != 2:
+            raise ValueError(f"codes must be [S] or [B,S], got {np.shape(codes)}")
+        B, S = c.shape
+        lens = None if lengths is None else _np(lengths, np.int32, (B,), "lengths")
+        y = np.zeros((B, S), np.float32)
+        if B and S:
+            self._ck(self.lib.vtts_decode_host(self.h, _ptr(c), _ptr(lens), B, S, ENCODINGS[enc], _ptr(y)))
+        return y[0] if one else y
+
+    def decode_forward(self, c_t, encoding, lengths_t=None, out=None, stream=None):
+        """vtts_decode on torch CUDA tensors, stream-ordered: codes c_t [B,S] (int16 for 'pcm16', uint8 otherwise) -> f32
+        [B,S]; lengths_t int32 CUDA [B] or None."""
+        import torch
+        enc = encoding_name(encoding)
+        if not (c_t.is_cuda and c_t.is_contiguous() and c_t.dim() == 2 and c_t.dtype == _torch_code_dtype(enc)):
+            raise ValueError(f"{enc} codes must be a contiguous {_torch_code_dtype(enc)} CUDA tensor [B,S]")
+        B, S = c_t.shape
+        out = _out_tensor(out, (B, S), c_t.device)
+        st = torch.cuda.current_stream(c_t.device).cuda_stream if stream is None else stream
+        self._ck(self.lib.vtts_decode(self.h, _ptr(c_t), _ptr(lengths_t), B, S, ENCODINGS[enc], _ptr(out), st))
+        return out
+
 
 class Loudness(NamedTuple):
     integrated: np.ndarray     # LUFS (gated, BS.1770-4)
@@ -2117,13 +2205,15 @@ class AudioChain:
     """The audio stages after the vocoder, their options validated, in the one order every caller runs them: denoise,
     pitch shift, time stretch and watermark at 16 kHz, then resample, equalize, compress, de-ess, reverb, limit (or
     normalize loudness) and meter at the output rate.  The watermark is the last 16 kHz stage, after everything that
-    moves time or pitch.  `run` applies the chain to one waveform with the one-shot host calls; `streams` opens it as stream
-    stages.  `loudness` (a target in LUFS, reached under `true_peak`, or under the limiter's ceiling with `limit`) has no
+    moves time or pitch.  `encoding` ('pcm16', 'ulaw' or 'alaw') turns the float audio into the codes of that wire format
+    last, after the meter; it has no state, so it is not a stream stage (TtsStream encodes its last buffer itself).
+    `run` applies the chain to one waveform with the one-shot host calls; `streams` opens it as stream stages.  `loudness` (a target in LUFS, reached under `true_peak`, or under the limiter's ceiling with `limit`) has no
     streaming form, and `meter` only measures, so `run` leaves the audio as it is for it.  Raises OptionError (a
     ValueError naming the option) for an option out of range."""
 
     def __init__(self, denoise=None, semitones=None, tempo=None, output_rate=None, eq=None, limit=None, gain_db=0.0,
-                 loudness=None, true_peak=None, meter=False, compress=None, deess=None, reverb=None, watermark=None):
+                 loudness=None, true_peak=None, meter=False, compress=None, deess=None, reverb=None, watermark=None,
+                 encoding=None):
         def checked(option, check, *args):
             try:
                 return check(*args)
@@ -2150,6 +2240,7 @@ class AudioChain:
         if meter or loudness is not None:
             checked("meter" if loudness is None else "loudness", _loudness_rate, self.rate)
         self.meter = bool(meter)
+        self.encoding = None if encoding is None else checked("encoding", encoding_name, encoding)
 
     def _stages(self):
         """(TtsStream attribute, one-shot call or None, stream factory or None) of each stage that is on, in order"""
@@ -2177,11 +2268,12 @@ class AudioChain:
         return [s[1:] for s in stages if s[0]]
 
     def run(self, eng: Engine, wav) -> np.ndarray:
-        """the one-shot host calls of every stage on `wav` ([S] or [B,S] at 16 kHz), in order"""
+        """the one-shot host calls of every stage on `wav` ([S] or [B,S] at 16 kHz), in order, then `Engine.encode`
+        with `encoding` (float32 audio without one)"""
         for _, call, _ in self._stages():
             if call is not None:
                 wav = call(eng, wav)
-        return wav
+        return wav if self.encoding is None else eng.encode(wav, self.encoding)
 
     def streams(self, eng: Engine, max_streams: int, pitch: int, max_frames: int):
         """Opens the stream stages in order, yielding (TtsStream attribute, handle) as each opens: the first takes
@@ -2207,13 +2299,13 @@ class TtsStream:
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
                  output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None, gain_db=0.0, eq=None,
-                 compress=None, deess=None, reverb=None, watermark=None):
+                 compress=None, deess=None, reverb=None, watermark=None, encoding=None):
         import torch
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
         self._chain = AudioChain(denoise=denoise, semitones=semitones, tempo=tempo, output_rate=output_rate, eq=eq, limit=limit,
                                  gain_db=gain_db, meter=meter, compress=compress, deess=deess, reverb=reverb,
-                                 watermark=watermark)
+                                 watermark=watermark, encoding=encoding)
         self.eng = eng
         self.rs = self.dn = self.ps = self.ts = self.wm = self.eq = self.cp = self.ds = self.rv = self.lm = self.mt = None
         S = max_streams
@@ -2241,6 +2333,10 @@ class TtsStream:
                 kw["reduction_t"] = torch.zeros(S, dtype=torch.float32, device=dev)
             self._stages.append((st, torch.zeros((S, st._width), dtype=torch.float32, device=dev), kw))
         self._mout_h = None if self.mt is None else torch.zeros((S, 4), dtype=torch.float32).pin_memory()
+        # the codes of the last audio buffer (the meter's input), the one buffer `step` copies to the host when encoding
+        last = ([b for st, b, _ in self._stages if st is not self.mt] or [self._wav])[-1]
+        self._codes = None if self._chain.encoding is None else _code_tensor(None, tuple(last.shape), self._chain.encoding, dev)
+        self._empty_out = np.zeros(0, np.float32 if self._codes is None else ENCODING_DTYPES[self._chain.encoding])
         self._meter = {}
         self._fresh = np.zeros(max_streams, bool)   # begun, no push yet: the next vocoder push carries BEGIN
         self._empty = set()                         # begun with nothing left after the trim: reported empty at the next step
@@ -2288,13 +2384,14 @@ class TtsStream:
     def step(self) -> dict:
         """One acoustic push into a device buffer, then one vocoder push of the frames it emitted (BEGIN on a slot's
         first push, END on its last); one synchronisation.  Returns {slot: float32 samples} for every slot that was
-        running (possibly empty); a slot whose utterance finished this step is free afterwards."""
+        running (possibly empty), or {slot: codes} (int16 or uint8, `Engine.encode` of those samples) when the stream
+        was opened with `encoding`; a slot whose utterance finished this step is free afterwards."""
         active = self.ac.open.copy()
         closing_before = active.copy()
         n_out = self.ac.push_device(self._mel) if active.any() else np.zeros(self.max_streams, np.int32)
         closed = closing_before & ~self.ac.open
         flags = (self._fresh & active).astype(np.uint8) * STREAM_BEGIN | closed.astype(np.uint8) * STREAM_END
-        out = {s: np.zeros(0, np.float32) for s in self._empty}
+        out = {s: self._empty_out.copy() for s in self._empty}
         self._empty = set()
         if active.any():
             n_wav = self.voc.push_device(self._mel, n_out, flags, self._wav)
@@ -2306,6 +2403,8 @@ class TtsStream:
                     self._mout_h.copy_(buf, non_blocking=True)   # ready once the blocking copy below returns
                 else:
                     n_wav, src = r, buf
+            if self._codes is not None:
+                src = self.eng.encode_forward(src, self._chain.encoding, out=self._codes)
             wav = src.cpu().numpy()
             for s in np.flatnonzero(active):
                 out[int(s)] = wav[s, : int(n_wav[s])].copy()

@@ -30,6 +30,9 @@ before --loudness / --limiter.
 `--watermark SPEC` marks every output with a key on the device (Engine.watermark: a keyed spread-spectrum mark, a bare
 integer key or key=…,strength=…) at 16 kHz, after --tempo and before any resampling; `python -m viettts_b200.watermark
 detect --key K FILE.wav` checks a written file for it.
+`--encoding E` encodes every output on the device (Engine.encode) at the rate it is written, after every other stage,
+and writes that WAVE format: `pcm16` (the same bytes as without the flag), `ulaw` or `alaw` (8-bit G.711, format 7 or
+6, the wire format of telephony, e.g. with `--output-rate 8000 --eq telephone`).
 """
 from __future__ import annotations
 
@@ -70,25 +73,68 @@ def float_to_pcm16(wave) -> np.ndarray:
     return np.clip(np.rint(x), -32768, 32767).astype("<i2")
 
 
-def write_wav(path, wave, sample_rate: int = config.SAMPLE_RATE) -> None:
-    """Mono 16-bit PCM RIFF/WAVE file with the canonical 44-byte header (synthesizer.py:39)."""
-    pcm = float_to_pcm16(np.ravel(wave))
-    data = pcm.tobytes()
-    header = b"RIFF" + struct.pack("<I", 36 + len(data)) + b"WAVE"
-    header += b"fmt " + struct.pack("<IHHIIHH", 16, 1, 1, int(sample_rate), int(sample_rate) * 2, 2, 16)
-    header += b"data" + struct.pack("<I", len(data))
+# WAVE format tag and bits per sample of each wire encoding (Engine.encode)
+WAV_FORMATS = {"pcm16": (1, 16), "ulaw": (7, 8), "alaw": (6, 8)}
+
+
+def write_wav(path, wave, sample_rate: int = config.SAMPLE_RATE, encoding=None) -> None:
+    """Mono RIFF/WAVE file.  Without `encoding`: float audio quantized by float_to_pcm16 into 16-bit PCM with the
+    canonical 44-byte header (synthesizer.py:39).  With `encoding`, `wave` holds codes already encoded in it
+    (Engine.encode): 'pcm16' int16 samples under the same 44-byte header; 'ulaw' (format 7) or 'alaw' (format 6) uint8
+    codes under an 18-byte fmt chunk (cbSize 0, 8 bits, block align 1, byte rate = rate) and a fact chunk holding the
+    sample count, as non-PCM WAVE files carry."""
+    rate = int(sample_rate)
+    if encoding is None:
+        codes, encoding = float_to_pcm16(np.ravel(wave)), "pcm16"
+    else:
+        if encoding not in WAV_FORMATS:
+            raise ValueError(f"encoding {encoding!r} must be one of {', '.join(WAV_FORMATS)}")
+        codes = np.ravel(wave)
+        want = np.int16 if encoding == "pcm16" else np.uint8
+        if codes.dtype != want:
+            raise ValueError(f"{encoding} samples must be {np.dtype(want).name}, got {codes.dtype}")
+    fmt, bits = WAV_FORMATS[encoding]
+    data = codes.astype("<i2" if bits == 16 else np.uint8).tobytes()
+    if fmt == 1:
+        chunks = b"fmt " + struct.pack("<IHHIIHH", 16, 1, 1, rate, rate * 2, 2, 16)
+    else:
+        chunks = b"fmt " + struct.pack("<IHHIIHHH", 18, fmt, 1, rate, rate, 1, 8, 0)
+        chunks += b"fact" + struct.pack("<II", 4, codes.size)
+    chunks += b"data" + struct.pack("<I", len(data)) + data + b"\0" * (len(data) % 2)   # chunks are word aligned
     with open(path, "wb") as f:
-        f.write(header + data)
+        f.write(b"RIFF" + struct.pack("<I", 4 + len(chunks)) + b"WAVE" + chunks)
+
+
+def read_wav_codes(path):
+    """(codes, sample_rate, encoding) of a mono WAVE file in one of the wire encodings: int16 samples for 'pcm16'
+    (format 1, 16 bits), uint8 codes for 'ulaw' (format 7) and 'alaw' (format 6, both 8 bits).  Chunks other than fmt
+    and data are skipped.  Raises ValueError for anything else."""
+    raw = Path(path).read_bytes()
+    if raw[:4] != b"RIFF" or raw[8:12] != b"WAVE":
+        raise ValueError(f"{path}: not a RIFF/WAVE file")
+    pos, fmt = 12, None
+    while pos + 8 <= len(raw):
+        cid, size = raw[pos:pos + 4], struct.unpack("<I", raw[pos + 4:pos + 8])[0]
+        body = raw[pos + 8:pos + 8 + size]
+        if cid == b"fmt " and size >= 16:
+            fmt = struct.unpack("<HHIIHH", body[:16])
+        elif cid == b"data":
+            if fmt is None:
+                raise ValueError(f"{path}: data before the fmt chunk")
+            tag, ch, sr, _, _, bits = fmt
+            enc = next((e for e, f in WAV_FORMATS.items() if f == (tag, bits)), None)
+            if ch != 1 or enc is None:
+                raise ValueError(f"{path}: format {tag}, {ch} channels, {bits} bits (mono PCM-16, mu-law or A-law)")
+            return np.frombuffer(body, "<i2" if bits == 16 else np.uint8).astype(np.int16 if bits == 16 else np.uint8), sr, enc
+        pos += 8 + size + size % 2
+    raise ValueError(f"{path}: no data chunk")
 
 
 def read_wav(path):
-    """Inverse of write_wav for tests: (float32 wave in [-1,1), sample_rate)."""
-    raw = Path(path).read_bytes()
-    assert raw[:4] == b"RIFF" and raw[8:12] == b"WAVE" and raw[12:16] == b"fmt "
-    fmt, ch, sr, _, _, bits = struct.unpack("<HHIIHH", raw[20:36])
-    assert (fmt, ch, bits) == (1, 1, 16) and raw[36:40] == b"data"
-    n = struct.unpack("<I", raw[40:44])[0]
-    return np.frombuffer(raw[44:44 + n], "<i2").astype(np.float32) / 32767.0, sr
+    """Inverse of write_wav for tests: (float32 wave in [-1,1), sample_rate) of a 16-bit PCM file."""
+    codes, sr, encoding = read_wav_codes(path)
+    assert encoding == "pcm16"
+    return codes.astype(np.float32) / 32767.0, sr
 
 
 def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_rows=32, engine=None, rng=None):
@@ -124,7 +170,7 @@ def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_
 # the command-line flag of each AudioChain option the CLI sets
 _FLAGS = {"denoise": "--denoise", "semitones": "--pitch", "tempo": "--tempo", "output_rate": "--output-rate", "eq": "--eq",
           "limit": "--limiter", "loudness": "--loudness", "compress": "--compress",
-          "deess": "--deess", "reverb": "--reverb", "watermark": "--watermark"}
+          "deess": "--deess", "reverb": "--reverb", "watermark": "--watermark", "encoding": "--encoding"}
 
 
 def main(argv=None) -> int:
@@ -183,6 +229,10 @@ def main(argv=None) -> int:
                         help="mark every output with a key on the device at 16 kHz, after --tempo and before --output-rate: "
                              "an integer key in [0, 2^64) or key=K,strength=S (S in [0, 0.3], default 0.1); "
                              "`python -m viettts_b200.watermark detect --key K FILE.wav` detects it")
+    parser.add_argument("--encoding", default=None, metavar="{pcm16,ulaw,alaw}",
+                        help="encode every output on the device at the output rate, after every other stage, and write it "
+                             "in that WAVE format: pcm16 (16-bit PCM, the default file), ulaw or alaw (8-bit G.711, e.g. "
+                             "with --output-rate 8000 --eq telephone for telephony)")
     parser.add_argument("--silence-duration", default=-1, type=float)
     parser.add_argument("--lexicon-file", default=None)
     parser.add_argument("--seed", default=None, type=int,
@@ -210,7 +260,7 @@ def main(argv=None) -> int:
     try:
         chain = AudioChain(denoise=args.denoise, semitones=args.pitch, tempo=args.tempo, output_rate=args.output_rate, eq=args.eq,
                            limit=ceiling if args.limiter else None, loudness=args.loudness, true_peak=ceiling, compress=args.compress,
-                           deess=args.deess, reverb=args.reverb, watermark=args.watermark)
+                           deess=args.deess, reverb=args.reverb, watermark=args.watermark, encoding=args.encoding)
     except OptionError as e:
         parser.error(f"{_FLAGS[e.option]}: {e}")
     header_rate = args.output_rate or args.sample_rate or config.SAMPLE_RATE
@@ -233,7 +283,7 @@ def main(argv=None) -> int:
         for i, w in enumerate(waves):
             fn = args.output.with_name(f"{args.output.stem}_{i:04d}{args.output.suffix or '.wav'}")
             print("writing output to file", fn)
-            write_wav(fn, w, header_rate)
+            write_wav(fn, w, header_rate, encoding=chain.encoding)
         return 0
 
     if args.text is None:
@@ -245,7 +295,7 @@ def main(argv=None) -> int:
     mel = text2mel(text, lexicon, args.silence_duration, seed=args.seed)
     wave = to_output_rate([np.ravel(mel2wave(mel))])[0]
     print("writing output to file", args.output)
-    write_wav(args.output, wave, header_rate)
+    write_wav(args.output, wave, header_rate, encoding=chain.encoding)
     return 0
 
 

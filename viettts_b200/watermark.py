@@ -1,7 +1,8 @@
 """Watermark detection from the command line (`python -m viettts_b200.watermark detect --key K [--key ...] FILE.wav ...`).
 
-Reads each 16-bit PCM WAV file the synthesizer writes (any rate the resampler reaches from 16 kHz), scores it against
-every key on the device (Engine.detect_watermark) and prints one line per file and key: the score z, the offset in
+Reads each WAV file the synthesizer writes (16-bit PCM, or 8-bit G.711 mu-law or A-law from --encoding, expanded on the
+device by Engine.decode; any rate the resampler reaches from 16 kHz), scores it against every key on the device
+(Engine.detect_watermark) and prints one line per file and key: the score z, the offset in
 16 kHz samples where the file's first sample sits in the mark's 4.096 s period, and the verdict.  Search mode (the
 default) finds the mark wherever a crop starts and calls z >= 6.5 marked; `--aligned` scores only offset 0, for files
 that start where the mark started, and calls z >= 5 marked.  For audio without the key either verdict is wrong with
@@ -24,7 +25,7 @@ def main(argv=None) -> int:
     args = parser.parse_args(argv)
 
     from .engine import get_engine, watermark_keys
-    from .synthesizer import read_wav
+    from .synthesizer import read_wav_codes
     try:
         keys = watermark_keys(args.key)
     except ValueError as e:
@@ -33,9 +34,10 @@ def main(argv=None) -> int:
     all_marked = True
     for fn in args.files:
         try:
-            wav, rate = read_wav(fn)
-        except (OSError, AssertionError, ValueError):
-            parser.error(f"{fn}: not a mono 16-bit PCM WAV file")
+            codes, rate, encoding = read_wav_codes(fn)
+        except (OSError, ValueError):
+            parser.error(f"{fn}: not a mono 16-bit PCM, mu-law or A-law WAV file")
+        wav = eng.decode(codes, encoding)
         r = eng.detect_watermark(wav, keys, rate=rate, search=not args.aligned)
         for k, z, off, hit in zip(keys, r.z, r.offset, r.detected):
             print(f"{fn}\tkey={int(k)}\tz={float(z):.2f}\toffset={int(off)}\t{'marked' if hit else 'not marked'}")

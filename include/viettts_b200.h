@@ -701,6 +701,56 @@ int vtts_reverb_stream_push(vtts_ctx* ctx, vtts_reverb_stream* rs, const float* 
 int vtts_reverb_stream_push_host(vtts_ctx* ctx, vtts_reverb_stream* rs, const float* x, const int32_t* n_new, const uint8_t* flags,
                                  float* y, int32_t* n_out);
 
+/* ---- background bed: a music or ambience bed under the voice, ducked by it ---------------------------------------
+ * One mono speech row x of n samples at rate r (an integer in [8000, 192000]) and a bank of K <= 8 beds, each Nb
+ * samples at r (0.5 r <= Nb <= 600 r) already at its level: bed k is bank_dev[offsets[k] .. offsets[k] + lengths[k]).
+ * duck_db D in [0, 40]; threshold, attack and release as for vtts_compress; fade_in Fi in [0, 5 r], tail Tt in
+ * [0, 10 r], xfade C in [0, r] with 2 C < Nb of every bed, offset o in [0, Nb) of every bed, all in samples (anything
+ * else, NaN included, fails with VTTS_ERR_BAD_ARG before anything is launched):
+ *   y_L = vtts_compress's detector (ratio 20, knee 6 dB) on L = 20 log10 |x|, x = 0 from n on;  y^_L = min(y_L, D);
+ *   g = 10^(-y^_L / 20);  bl[t] = b[u], u = (t + o) mod P, P = Nb - C, and for u < C the equal-power seam crossfade
+ *   sin(pi u / 2C) b[u] + cos(pi u / 2C) b[P + u];  e[t] = (1 - cos(pi t / Fi)) / 2 for t < Fi (else 1) times
+ *   (1 + cos(pi (t - n + 1) / Tt)) / 2 for t >= n (else 1);  y[t] = x[t] + g e bl, evaluated as fmaf(g e, bl, x), for
+ *   t < n + Tt;  reduction = -max y^_L (<= 0).  A row with bed index -1 comes back as x bit for bit, without a tail
+ *   (reduction 0).
+ * fp32 in every vtts_precision mode; the detector keeps the compressor's 256-sample blocks fixed by absolute sample index
+ * and the bed and envelopes are functions of that index, so a row gives the same bits alone, in any batch, and through
+ * the stream. */
+/* x_dev [B,S]; n_dev int32 [B] or NULL (= S; values clamped to [0, S]); bank_dev on the device, offsets int64 and lengths
+ * int32 HOST [K]; bed HOST int32 [B] in [-1, K); y_dev [B][S + tail] (not x_dev), 0 from n[b] + tail (n[b] without a
+ * bed); reduction_db_dev [B] or NULL.  Stream-ordered, no host synchronisation: one table copy, the key gather and the
+ * compressor's six launches; uses the context's workspace (about 4.3 bytes per sample of S + tail). */
+int vtts_bed_mix(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, const float* bank_dev,
+                 const long long* offsets, const int32_t* lengths, int K, const int32_t* bed, float duck_db, float threshold_db,
+                 float attack_ms, float release_ms, int fade_in, int tail, int xfade, long long offset, float* y_dev,
+                 float* reduction_db_dev, void* stream);
+/* the same on host buffers x [B,S] and y [B][S + tail] (the bank stays on the device); n_in[b] must lie in [0, S];
+ * reduction_db [B] or NULL */
+int vtts_bed_mix_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, const float* bank_dev,
+                      const long long* offsets, const int32_t* lengths, int K, const int32_t* bed, float duck_db, float threshold_db,
+                      float attack_ms, float release_ms, int fade_in, int tail, int xfade, long long offset, float* y, float* reduction_db);
+/* Streaming bed with max_streams independent slots; the bank and every parameter are fixed at create (bank_dev must stay
+ * valid until destroy; offsets and lengths are copied).  No lookahead: a push releases every sample it brings, and the
+ * push with END also releases the slot's tail (n_out[s] = n_new[s], + tail with END and a bed).  A slot's bed index is
+ * read with BEGIN and kept until END; a push that changes it for an open slot without BEGIN fails.  A slot's outputs,
+ * concatenated, and its reduction equal vtts_bed_mix of its whole input bit for bit.  Each slot carries the compressor
+ * stream's state.  flags and slot rules as for the resample stream.  Every push issues one table copy, the key gather
+ * and the compressor's six launches. */
+typedef struct vtts_bed_stream vtts_bed_stream;
+/* *out_pitch receives the outputs per slot of a push's output buffer (max_chunk_samples + tail) */
+int vtts_bed_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int rate, const float* bank_dev, const long long* offsets,
+                           const int32_t* lengths, int K, float duck_db, float threshold_db, float attack_ms, float release_ms, int fade_in,
+                           int tail, int xfade, long long offset, vtts_bed_stream** out, int* out_pitch);
+int vtts_bed_stream_destroy(vtts_ctx* ctx, vtts_bed_stream* bs);
+/* x_dev [S][max_chunk_samples] (samples past n_new[s] ignored); n_new, flags, bed (each slot's bed index, read where
+ * BEGIN is set), n_out HOST [S]; y_dev [S][out_pitch], slot s gets n_out[s] outputs from its start; reduction_db_dev [S]
+ * each slot's reduction over what it has released since BEGIN.  Stream-ordered. */
+int vtts_bed_stream_push(vtts_ctx* ctx, vtts_bed_stream* bs, const float* x_dev, const int32_t* n_new, const uint8_t* flags, const int32_t* bed,
+                         float* y_dev, int32_t* n_out, float* reduction_db_dev, void* stream);
+/* the same on host buffers x [S][max_chunk_samples], y [S][out_pitch] and reduction_db [S]; returns when they are written */
+int vtts_bed_stream_push_host(vtts_ctx* ctx, vtts_bed_stream* bs, const float* x, const int32_t* n_new, const uint8_t* flags, const int32_t* bed,
+                              float* y, int32_t* n_out, float* reduction_db);
+
 /* ---- watermark: a keyed spread-spectrum mark and its batched detector ---------------------------------------------
  * Embed, one mono 16 kHz row x of n samples, a key (any uint64) and a strength eps in [0, 0.3] (anything else, NaN
  * included, fails with VTTS_ERR_BAD_ARG before anything is launched): the denoiser's STFT (n_fft 1024, hop 256, periodic

@@ -172,6 +172,20 @@ SIGNATURES = {
     "vtts_reverb_stream_lookahead": (C.c_int, []),
     "vtts_reverb_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtts_reverb_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_bed_mix": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                               C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int,
+                               C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_bed_mix_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int,
+                                    C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]),
+    "vtts_bed_stream_create": (C.c_int, [c_ctx, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                         C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_int, C.c_int,
+                                         C.c_longlong, C.POINTER(C.c_void_p), C.POINTER(C.c_int)]),
+    "vtts_bed_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
+    "vtts_bed_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_bed_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p]),
     "vtts_watermark": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint64, C.c_float, C.c_void_p, C.c_void_p]),
     "vtts_watermark_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint64, C.c_float, C.c_void_p]),
     "vtts_watermark_stream_create": (C.c_int, [c_ctx, C.c_int, C.c_int, C.c_uint64, C.c_float, C.POINTER(C.c_void_p), C.POINTER(C.c_int)]),

@@ -1,6 +1,7 @@
 // The compressor's parameters, scan kernels and launch sequence (compressor.cu states the definition and the block
-// invariant), shared by the compressor and the de-esser (deesser.cu), whose detector reads its high band as the level
-// source.  Internal to each translation unit that includes it.
+// invariant), shared by the compressor, the de-esser (deesser.cu), whose detector reads its high band as the level
+// source, and the bed ducker (bed.cu), whose gain acts on a second signal.  Internal to each translation unit that
+// includes it.
 #pragma once
 #include <algorithm>
 #include <cmath>
@@ -154,13 +155,14 @@ __global__ void __launch_bounds__(SCAN_THREADS) cp_attack_fold_kernel(const floa
 }
 
 // The output rule of the apply kernel, a template parameter so that each user compiles only its own: where the
-// detector reads its level (the fold kernels read the same source), the cap on y_L, and y from the sample x, its level
-// sample l and g = 10^(-y_L / 20) (1 exactly where the capped y_L is 0).
+// detector reads its level (the fold kernels read the same source), the cap on y_L of row b, and y of row b at absolute
+// sample t from the sample x, its level sample l and g = 10^(-y_L / 20) (1 exactly where the capped y_L is 0).  The
+// compressor and the de-esser ignore the row and the sample index.
 struct CpMakeup {                   // the compressor: level source x, y = (x m) g
   __host__ __device__ const float* source(const float* x) const { return x; }
   __device__ __forceinline__ float level(const float* xr, long long t, float v) const { return v; }
-  __device__ __forceinline__ float cap(float yl) const { return yl; }
-  __device__ __forceinline__ float out(const CpParams& p, float v, float l, float yl, float g) const { return (v * p.m) * g; }
+  __device__ __forceinline__ float cap(int, float yl) const { return yl; }
+  __device__ __forceinline__ float out(const CpParams& p, int, long long, float v, float l, float yl, float g) const { return (v * p.m) * g; }
 };
 
 struct CpSplit {                    // the de-esser: level source its high band h (x's layout), y = x - (1 - g) h
@@ -168,8 +170,8 @@ struct CpSplit {                    // the de-esser: level source its high band 
   float range;                      // the cap on y_L, dB
   __host__ __device__ const float* source(const float*) const { return h; }
   __device__ __forceinline__ float level(const float* xr, long long t, float) const { return xr[t]; }
-  __device__ __forceinline__ float cap(float yl) const { return fminf(yl, range); }
-  __device__ __forceinline__ float out(const CpParams&, float v, float l, float yl, float g) const {
+  __device__ __forceinline__ float cap(int, float yl) const { return fminf(yl, range); }
+  __device__ __forceinline__ float out(const CpParams&, int, long long, float v, float l, float yl, float g) const {
     return yl > 0.f ? fmaf(g - 1.f, l, v) : v;
   }
 };
@@ -211,9 +213,9 @@ __global__ void __launch_bounds__(SCAN_THREADS) cp_apply_kernel(const float* x, 
     const float v = xr[t], l = o.level(lr, t, v);
     map_fold(R, cp_reduction(p, l), p.aR, p.bR);
     cp_attack_fold(A, map_apply(R, y1_in), p.aA, p.bA);
-    const float yl = o.cap(map_apply(A, yl_in));
+    const float yl = o.cap(b, map_apply(A, yl_in));
     const float g = yl > 0.f ? exp10f(-yl / 20.f) : 1.f;
-    yr[t] = o.out(p, v, l, yl, g);
+    yr[t] = o.out(p, b, t, v, l, yl, g);
     mx = fmaxf(mx, yl);
   }
   bmax[(size_t)b * ld_blk + i] = mx;

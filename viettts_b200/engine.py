@@ -94,6 +94,7 @@ LIMIT_MAX_GAIN_DB = 70.0
 SEMITONES = _BeginParam("semitones", 0.0, -MAX_SEMITONES, MAX_SEMITONES)
 TEMPO = _BeginParam("tempo", 1.0, MIN_TEMPO, MAX_TEMPO)
 GAIN_DB = _BeginParam("gain_db", 0.0, -LIMIT_MAX_GAIN_DB, LIMIT_MAX_GAIN_DB, default=0.0, host_check=True)
+BED = _BeginParam("bed", -1.0, -1.0, 7.0, default=0, host_check=True)     # a bank entry; the bank's size bounds it
 
 
 EQ_MAX_SECTIONS = 8
@@ -255,6 +256,149 @@ def reverb_params(spec, rate: int) -> dict:
         raise ValueError(f"reverb: seed={p['seed']:g} must be an integer")
     p["seed"] = int(p["seed"])
     return dict(ir=reverb_ir(p["rt60"], p["predelay"], p["seed"], rate), **p)
+
+
+# the bed's parameters with their ranges; `offset` is checked against the bed's length, and seed / length belong to
+# the pink preset
+BED_RANGES = {"level": (-60.0, -10.0), "duck": (0.0, 40.0), "threshold": (-60.0, 0.0), "attack": (0.5, 200.0),
+              "release": (5.0, 5000.0), "fade_in": (0.0, 5000.0), "tail": (0.0, 10000.0), "xfade": (0.0, 1000.0),
+              "offset": (0.0, 600.0)}
+BED_DEFAULTS = {"level": -30.0, "duck": 12.0, "threshold": -40.0, "attack": 10.0, "release": 500.0, "fade_in": 250.0,
+                "tail": 1000.0, "xfade": 50.0, "offset": 0.0}
+BED_PINK_RANGES = {"seed": (0.0, float(2 ** 24)), "length": (0.5, 600.0)}
+BED_PINK_DEFAULTS = {"seed": 0.0, "length": 8.0}
+BED_MAX_SECONDS = 600
+BED_MAX_BEDS = 8
+# the keys a bank's beds may differ in: every other one is a parameter of the call
+_BED_OWN = ("audio", "audio_rate", "level", "seed", "length")
+
+
+def pink_bed(seed: int, seconds: float, rate: int) -> np.ndarray:
+    """The `pink` preset's bed (float32 [round(seconds rate)]): white Gaussian noise default_rng(seed) shaped to a 1/f
+    power spectrum in the frequency domain (bin k scaled by 1 / sqrt(k), DC removed), scaled to unit RMS in float64 and
+    cast once.  The shaping is circular, so the bed loops without a seam of its own."""
+    n = int(round(float(seconds) * rate))
+    X = np.fft.rfft(np.random.default_rng(int(seed)).standard_normal(n))
+    k = np.arange(X.size)
+    X[0] = 0.0
+    X[1:] /= np.sqrt(k[1:])
+    v = np.fft.irfft(X, n)
+    return (v / np.sqrt(np.mean(v * v))).astype(np.float32)
+
+
+def bed_params(spec, rate: int) -> dict:
+    """The bed of a `spec` at the chain rate `rate` (an integer in [8000, 192000] and a multiple of 10, where the bed's
+    loudness is measured): {audio: float32, audio_rate, level, duck, threshold, attack, release, fade_in, tail, xfade,
+    offset (float32 values), Nb: samples at `rate`, Fi, Tt, C, o: fade_in, tail, xfade and offset in samples at `rate`
+    (rint)}.  `spec` is the preset `pink` with comma-separated key=value pairs after it (`pink,seed=3,duck=18`: seeded
+    pink noise of `length` s, default 8, see `pink_bed`), or a dict that gives `audio` (a mono float array at
+    `audio_rate`, default `rate`; any ratio the resampler takes, each reduced term at most 1024) or leaves it out for
+    the pink preset.  level LUFS in [-60, -10] (default -30), duck dB in [0, 40] (12), threshold dBFS in [-60, 0] (-40),
+    attack ms in [0.5, 200] (10), release ms in [5, 5000] (500), fade_in ms in [0, 5000] (250), tail ms in [0, 10000]
+    (1000), xfade ms in [0, 1000] (50) with 2 C below the bed's samples, offset s in [0, the bed's length) (0).  The bed
+    lasts 0.5 s at `rate` to 600 s.  Raises ValueError naming the key."""
+    _check_rate("bed", rate)
+    rate = int(rate)
+    if rate % 10:
+        raise ValueError(f"bed: rate {rate} must be a multiple of 10 (the bed's loudness is measured at it)")
+    if isinstance(spec, str):
+        head, *items = [t.strip() for t in spec.split(",")]
+        if head.lower() != "pink":
+            raise ValueError(f"bed: a string spec is the preset 'pink' with key=value pairs after it, got {head!r} "
+                             "(pass a dict with audio= for a bed of your own)")
+        given = {}
+        for item in items:
+            key, eq, val = item.partition("=")
+            if not eq:
+                raise ValueError(f"bed: {item!r} is not key=value (keys {', '.join([*BED_RANGES, *BED_PINK_RANGES])})")
+            given[key.strip().lower()] = val.strip()
+    elif isinstance(spec, dict):
+        given = dict(spec)
+    else:
+        raise ValueError(f"bed: a spec is a string or a dict, got {type(spec).__name__}")
+    audio, audio_rate = given.pop("audio", None), given.pop("audio_rate", None)
+    pink = audio is None
+    if pink and audio_rate is not None:
+        raise ValueError("bed: audio_rate= goes with audio=")
+    ranges = dict(BED_RANGES, **(BED_PINK_RANGES if pink else {}))
+    p = _keyed_params("bed", given, ranges, {"pink": dict(BED_DEFAULTS, **(BED_PINK_DEFAULTS if pink else {}))}, "pink")
+    if pink:
+        if p["seed"] != int(p["seed"]):
+            raise ValueError(f"bed: seed={p['seed']:g} must be an integer")
+        p["seed"] = int(p["seed"])
+        audio, audio_rate = pink_bed(p["seed"], p["length"], rate), rate
+    else:
+        try:
+            audio = np.ascontiguousarray(np.asarray(audio, np.float64).astype(np.float32))
+        except (TypeError, ValueError):
+            raise ValueError("bed: audio= must be an array of numbers") from None
+        if audio.ndim != 1:
+            raise ValueError(f"bed: audio must be mono [N], got {audio.shape}")
+        if not np.all(np.isfinite(audio)):
+            raise ValueError("bed: audio samples must be finite")
+        try:
+            audio_rate = rate if audio_rate is None else int(audio_rate)
+            up, down = resample_ratio(audio_rate, rate)
+        except (TypeError, ValueError):
+            raise ValueError(f"bed: audio_rate={audio_rate!r} must be a positive integer") from None
+        if max(up, down) > 1024:
+            raise ValueError(f"bed: audio_rate {audio_rate} -> {rate} reduces to {up}/{down} (at most 1024 each)")
+    nb = resample_length(audio.size, audio_rate, rate)
+    if not (2 * nb >= rate and audio.size <= BED_MAX_SECONDS * audio_rate):
+        raise ValueError(f"bed: audio lasts {audio.size / audio_rate:g} s (0.5 s at {rate} Hz to {BED_MAX_SECONDS} s)")
+    n = {k: int(np.rint(p[k] * rate / 1000.0)) for k in ("fade_in", "tail", "xfade")}
+    o = int(np.rint(p["offset"] * rate))
+    if 2 * n["xfade"] >= nb:
+        raise ValueError(f"bed: xfade={p['xfade']:g} ms makes 2 x {n['xfade']} samples, not below the bed's {nb}")
+    if o >= nb:
+        raise ValueError(f"bed: offset={p['offset']:g} s lies past the bed's {nb / rate:g} s")
+    return dict(audio=audio, audio_rate=audio_rate, **p, Nb=nb, Fi=n["fade_in"], Tt=n["tail"], C=n["xfade"], o=o)
+
+
+def bed_specs(spec, rate: int) -> list:
+    """`bed_params` of a spec or of a list of 1 to 8 specs (a bank), which may differ only in their audio, level and
+    pink seed and length"""
+    specs = list(spec) if isinstance(spec, (list, tuple)) else [spec]
+    if not 1 <= len(specs) <= BED_MAX_BEDS:
+        raise ValueError(f"bed: {len(specs)} beds (1 to {BED_MAX_BEDS})")
+    ps = [bed_params(s, rate) for s in specs]
+    shared = [k for k in BED_RANGES if k not in _BED_OWN]
+    for i, q in enumerate(ps[1:], 1):
+        for k in shared:
+            if q[k] != ps[0][k]:
+                raise ValueError(f"bed: bed {i} has {k}={q[k]:g} and bed 0 {k}={ps[0][k]:g} (the beds of a bank share every "
+                                 f"key but {', '.join(_BED_OWN)})")
+        if 2 * ps[0]["C"] >= q["Nb"] or ps[0]["o"] >= q["Nb"]:
+            raise ValueError(f"bed: bed {i}'s {q['Nb']} samples do not hold the xfade and offset")
+    return ps
+
+
+class BedBank(NamedTuple):
+    """The prepared beds of a bank on the device (Engine.prepare_beds): each resampled to `rate` and scaled to its level."""
+    audio: "object"          # float32 CUDA tensor [sum of lengths], bed k at offsets[k]
+    offsets: np.ndarray      # int64 [K]
+    lengths: np.ndarray      # int32 [K]
+    params: list             # bed_params of each bed
+    rate: int
+
+    def args(self) -> tuple:
+        """the bank and call parameters of vtts_bed_* after the rate: bank, offsets, lengths, K, duck, threshold, attack,
+        release, fade_in, tail, xfade, offset"""
+        p = self.params[0]
+        return (_ptr(self.audio), _ptr(self.offsets), _ptr(self.lengths), len(self.params), p["duck"], p["threshold"],
+                p["attack"], p["release"], p["Fi"], p["Tt"], p["C"], p["o"])
+
+    def index(self, bed, n: int) -> np.ndarray:
+        """int32 [n]: a bank entry for every row, or one per row, each in [-1, K)"""
+        a = np.asarray(bed)
+        if a.dtype.kind not in "iu" and not (a.dtype.kind == "f" and np.all(np.isfinite(a)) and np.all(a == np.round(a))):
+            raise ValueError(f"bed index must be integers, got {bed!r}")
+        a = np.full(n, a, np.int64) if a.ndim == 0 else a.reshape(-1).astype(np.int64)
+        if a.shape != (n,):
+            raise ValueError(f"bed index: one value or one per row ({n}), got {np.shape(bed)}")
+        if np.any((a < -1) | (a >= len(self.params))):
+            raise ValueError(f"bed index must lie in [-1, {len(self.params) - 1}], got {bed!r}")
+        return a.astype(np.int32)
 
 
 WATERMARK_MAX_STRENGTH = 0.3
@@ -458,6 +602,7 @@ class Engine:
         self._mel_fb = None         # host copy of the filterbank on the device (None: none loaded)
         self._denoise_bias = None   # default denoiser bias of the loaded generator in the current mode (denoiser_bias)
         self._reverb_irs = {}       # (string spec, rate, device) -> (IR on the device, mix) of reverb_forward
+        self._bed_banks = {}        # (string spec(s), rate) -> BedBank of mix_bed / mix_bed_forward
 
     def close(self):
         if getattr(self, "h", None):
@@ -683,7 +828,7 @@ class Engine:
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
                         rng=None, output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None,
                         gain_db=0.0, eq=None, compress=None, deess=None, reverb=None, watermark=None,
-                        encoding=None) -> "TtsStream":
+                        encoding=None, bed=None) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
         With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  `output_rate`: a resample
@@ -709,6 +854,10 @@ class Engine:
         `reverb`: a reverb spec (`reverb_params`, presets and keys); a reverb stream follows the de-esser (before the
         limiter and the meter) at the output rate, and the audio equals `reverb` of the (resampled, ..., de-essed) `tts`
         audio bit for bit.  It holds back up to 511 samples until the next block of 512 is complete.
+        `bed`: a bed spec or a list of up to 8 (`bed_specs`); a bed stream follows the reverb (before the limiter and the
+        meter) at the output rate, its bank prepared once here, and each slot's audio equals `mix_bed` of the
+        (resampled, ..., reverberated) `tts` audio with the slot's bank entry (`begin(..., bed=)`, default 0, -1 for
+        none) bit for bit.  It adds no delay; a slot's last step also returns its `tail`.
         `watermark`: a watermark spec (`watermark_params`: a key, or key=…,strength=…); a watermark stream follows the
         time stretcher (before the resampler) at 16 kHz, and the audio equals `watermark` of the (denoised, shifted,
         stretched) `tts` audio bit for bit.  Every slot carries the same key.  It holds back up to 1023 samples.
@@ -720,7 +869,7 @@ class Engine:
         synchronisation.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
         return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate,
                          denoise=denoise, meter=meter, semitones=semitones, tempo=tempo, limit=limit, gain_db=gain_db, eq=eq,
-                         compress=compress, deess=deess, reverb=reverb, watermark=watermark, encoding=encoding)
+                         compress=compress, deess=deess, reverb=reverb, watermark=watermark, encoding=encoding, bed=bed)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -1527,6 +1676,87 @@ class Engine:
         whole input bit for bit."""
         return ReverbStream(self, max_streams, max_chunk_samples, spec, rate)
 
+    # ---- background bed (vtts_bed*: a looped bed ducked by the compressor's detector on the voice, fp32) ----
+    def prepare_beds(self, bed, rate: int = config.SAMPLE_RATE) -> BedBank:
+        """The bank of a bed spec or a list of up to 8 (`bed_specs`) prepared on the device once: each bed resampled from
+        its audio_rate to `rate` (vtts_resample) and scaled to its integrated loudness `level` (vtts_loudness_normalize;
+        a silent bed stays silent).  A BedBank passes through unchanged (its rate must be `rate`)."""
+        import torch
+        if isinstance(bed, BedBank):
+            if bed.rate != int(rate):
+                raise ValueError(f"bed: the bank was prepared at {bed.rate} Hz, not {rate}")
+            return bed
+        ps = bed_specs(bed, rate)
+        lengths = np.array([p["Nb"] for p in ps], np.int32)
+        offsets = np.concatenate([[0], np.cumsum(lengths[:-1], dtype=np.int64)]).astype(np.int64)
+        dev = torch.device("cuda", self.device)
+        audio = torch.empty(int(lengths.sum()), dtype=torch.float32, device=dev)
+        for p, o, n in zip(ps, offsets, lengths):
+            row = audio[int(o):int(o) + int(n)].view(1, -1)
+            a = torch.from_numpy(p["audio"]).to(dev).view(1, -1)
+            if p["audio_rate"] != int(rate):
+                a = self.resample_forward(a, int(rate), p["audio_rate"])
+            self.normalize_loudness_forward(a, p["level"], int(rate), out=row)
+        torch.cuda.current_stream(dev).synchronize()
+        return BedBank(audio, offsets, lengths, ps, int(rate))
+
+    def _bed_bank(self, bed, rate) -> BedBank:
+        """prepare_beds, kept for later calls when the spec is a string or a list of strings"""
+        key = None
+        if isinstance(bed, str) or (isinstance(bed, (list, tuple)) and all(isinstance(b, str) for b in bed)):
+            key = (bed if isinstance(bed, str) else tuple(bed), int(rate))
+        bank = self._bed_banks.get(key) if key else None
+        if bank is None:
+            bank = self.prepare_beds(bed, rate)
+            if key:
+                self._bed_banks[key] = bank
+        return bank
+
+    def mix_bed(self, wav, bed="pink", rate: int = config.SAMPLE_RATE, lengths=None, index=0):
+        """Host arrays: (y, reduction_db).  wav f32 [S] or [B,S] at `rate` over the bed `bed` (a spec, a list of up to 8
+        or a BedBank, see `bed_params` and `prepare_beds`): the bank entry `index` (one for every row or one per row, -1
+        for none) looped from its offset with an equal-power crossfade at the seam, under a raised-cosine fade-in, ducked
+        by up to `duck` dB while the voice is above the threshold (the compressor's detector, ratio 20, knee 6 dB), and
+        carried `tail` ms past each row's end, where the voice is silent, the bed swells back and a raised-cosine fade
+        brings it to zero.  y is [B, S + tail samples]: row b holds n[b] + tail samples (n[b] as wav without a bed), then
+        zeros; a single row comes back as [S + tail] ([S] without a bed).  reduction_db: the deepest duck per row (<= 0).
+        lengths int [B] in [0, S]."""
+        bank = self._bed_bank(bed, rate)
+        x, lens, one = _wav_rows(wav, lengths)
+        B, S = x.shape
+        idx = bank.index(index, B)
+        W = S + bank.params[0]["Tt"]
+        if B and not S:                            # empty rows still carry the bed's tail
+            x, lens = np.zeros((B, 1), np.float32), np.zeros(B, np.int32)
+        y = np.zeros((B, x.shape[1] + bank.params[0]["Tt"]), np.float32)
+        red = np.zeros(B, np.float32)
+        if B:
+            self._ck(self.lib.vtts_bed_mix_host(self.h, _ptr(x), _ptr(lens), B, x.shape[1], int(rate), *bank.args()[:4], _ptr(idx),
+                                                *bank.args()[4:], _ptr(y), _ptr(red)))
+        y = y[:, :W]
+        if one:
+            return (y[0] if idx[0] >= 0 else y[0, :S]), red[0]
+        return y, red
+
+    def mix_bed_forward(self, x_t, bed="pink", rate: int = config.SAMPLE_RATE, lengths_t=None, index=0, out=None, reduction_db=None,
+                        stream=None):
+        """vtts_bed_mix on torch CUDA tensors, stream-ordered and without a host synchronisation: returns (y [B, S + tail],
+        reduction_db [B]), both on the device, as `mix_bed`.  lengths_t int32 CUDA [B] or None; `index` host values.
+        The bank is prepared once per string spec and rate and kept for later calls."""
+        bank = self._bed_bank(bed, rate)
+        B, S, out, st = _dev_rows(x_t, out, stream, x_t.shape[1] + bank.params[0]["Tt"])
+        idx = bank.index(index, B)
+        reduction_db = _out_tensor(reduction_db, (B,), x_t.device, "reduction_db")
+        self._ck(self.lib.vtts_bed_mix(self.h, _ptr(x_t), _ptr(lengths_t), B, S, int(rate), *bank.args()[:4], _ptr(idx),
+                                       *bank.args()[4:], _ptr(out), _ptr(reduction_db), st))
+        return out, reduction_db
+
+    def open_bed_stream(self, max_streams: int, max_chunk_samples: int, bed="pink", rate: int = config.SAMPLE_RATE) -> "BedStream":
+        """Streaming bed with `max_streams` independent slots (vtts_bed_stream_*): a slot's bank entry is given with
+        BEGIN (`bed=`, default 0, -1 for none); every push releases every sample it brings, the push with END also the
+        tail, and a slot's outputs, concatenated, and its reduction equal `mix_bed` of its whole input bit for bit."""
+        return BedStream(self, max_streams, max_chunk_samples, bed, rate)
+
     # ---- watermark (vtts_watermark*: a keyed spread-spectrum mark on the denoiser's STFT, fp32) ----
     def watermark(self, wav, spec, lengths=None) -> np.ndarray:
         """Host array y: wav f32 [S] or [B,S] at 16 kHz marked with the key of `spec` (see `watermark_params`): every
@@ -2077,6 +2307,43 @@ class ReverbStream(_SlotStream):
         self.lookahead = int(eng.lib.vtts_reverb_stream_lookahead())
 
 
+class BedStream(_ReductionStream):
+    """Handle of a streaming bed (Engine.open_bed_stream): `bed=` with BEGIN, the slot's bank entry (default 0, -1 for
+    none).  Every push releases every sample it brings, and the push with END also the slot's `tail` samples
+    (n_out = n_new, + tail at END with a bed; out_pitch = max_chunk_samples + tail).  After every host push
+    `reduction_db` holds each slot's deepest duck over what it has released since BEGIN; `bed` holds each slot's entry."""
+    _kind, _param, _carried = "bed_stream", BED, "bed"
+    lookahead = 0
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, bed="pink", rate: int = config.SAMPLE_RATE):
+        super().__init__(eng, max_streams, max_chunk_samples)
+        self.max_chunk_samples = self._chunk
+        self.rate = int(rate)
+        self.bank = eng.prepare_beds(bed, self.rate)    # held: the stream reads it until it closes
+        self.tail = self.bank.params[0]["Tt"]
+        self.bed = np.full(self.max_streams, -1, np.int32)
+        self._create(eng.lib.vtts_bed_stream_create, self.max_streams, self.max_chunk_samples, self.rate, *self.bank.args(), pitch=True)
+        self.reduction_db = np.zeros(self.max_streams, np.float32)   # host pushes: each slot's reduction so far
+
+    def _values(self, flags, v) -> tuple:
+        """(int32 [S],): the push's entry `v` (default 0; one or one per slot) for the slots it begins, each slot's own
+        elsewhere"""
+        out = self.bed.copy()
+        begin = (flags & STREAM_BEGIN) != 0
+        if begin.any():
+            out[begin] = self.bank.index(BED.default if v is None else v, out.size)[begin]
+        return (out,)
+
+    def push(self, x, n_new, begin=None, end=None, bed=None) -> list:
+        """As `_SlotStream.push`, with bed: a bank entry or one per slot, read for the slots that begin (default 0)."""
+        return self._push_host(x, n_new, begin, end, bed)
+
+    def push_device(self, x_t, n_new, flags, out_t, reduction_t, bed=None, stream=None) -> np.ndarray:
+        """As `_SlotStream.push_device`, with reduction_t f32 CUDA [S] (each slot's reduction so far, written on the
+        device) and bed (host, read for the slots that begin, default 0)."""
+        return self._push_device(x_t, n_new, flags, out_t, stream, bed, (reduction_t,))
+
+
 class WatermarkStream(_SlotStream):
     """Handle of a streaming watermark (Engine.open_watermark_stream).  Before END a slot that has received P samples
     has emitted min(P, 256 max(0, floor(P / 256) - 3)) outputs; a push with END emits the rest."""
@@ -2203,9 +2470,10 @@ class OptionError(ValueError):
 
 class AudioChain:
     """The audio stages after the vocoder, their options validated, in the one order every caller runs them: denoise,
-    pitch shift, time stretch and watermark at 16 kHz, then resample, equalize, compress, de-ess, reverb, limit (or
-    normalize loudness) and meter at the output rate.  The watermark is the last 16 kHz stage, after everything that
-    moves time or pitch.  `encoding` ('pcm16', 'ulaw' or 'alaw') turns the float audio into the codes of that wire format
+    pitch shift, time stretch and watermark at 16 kHz, then resample, equalize, compress, de-ess, reverb, bed, limit
+    (or normalize loudness) and meter at the output rate.  The bed sits under the limiter and the meter, so it counts in
+    the program loudness and stays under the true-peak ceiling; its tail makes each row `tail` samples longer.  The
+    watermark is the last 16 kHz stage, after everything that moves time or pitch.  `encoding` ('pcm16', 'ulaw' or 'alaw') turns the float audio into the codes of that wire format
     last, after the meter; it has no state, so it is not a stream stage (TtsStream encodes its last buffer itself).
     `run` applies the chain to one waveform with the one-shot host calls; `streams` opens it as stream stages.  `loudness` (a target in LUFS, reached under `true_peak`, or under the limiter's ceiling with `limit`) has no
     streaming form, and `meter` only measures, so `run` leaves the audio as it is for it.  Raises OptionError (a
@@ -2213,7 +2481,7 @@ class AudioChain:
 
     def __init__(self, denoise=None, semitones=None, tempo=None, output_rate=None, eq=None, limit=None, gain_db=0.0,
                  loudness=None, true_peak=None, meter=False, compress=None, deess=None, reverb=None, watermark=None,
-                 encoding=None):
+                 encoding=None, bed=None):
         def checked(option, check, *args):
             try:
                 return check(*args)
@@ -2232,6 +2500,8 @@ class AudioChain:
         if reverb is not None:
             checked("reverb", reverb_params, reverb, self.rate)
         self.reverb = reverb           # the spec: the stages synthesize its IR where they open
+        self.bed = None if bed is None else checked("bed", bed_specs, bed, self.rate)
+        self._bed_spec, self._banks = bed, {}   # the bank is prepared once per engine, where a stage first runs or opens
         self.limit = None if limit is None else checked("limit", _limit_args, limit, self.rate, 5.0, 100.0)[0]
         self.gain_db = float(checked("gain_db", GAIN_DB.rows, gain_db, 1)[0]) if limit is not None else 0.0
         self.loudness = self.true_peak = None
@@ -2259,6 +2529,8 @@ class AudioChain:
              lambda e, S, p, sec: CompressorStream(e, S, p, self.compress, r)),
             (self.deess is not None, "ds", lambda e, w: e.deess(w, self.deess, r)[0], lambda e, S, p, sec: DeesserStream(e, S, p, self.deess, r)),
             (self.reverb is not None, "rv", lambda e, w: e.reverb(w, self.reverb, r), lambda e, S, p, sec: ReverbStream(e, S, p, self.reverb, r)),
+            (self.bed is not None, "bd", lambda e, w: e.mix_bed(w, self._bank(e), r)[0],
+             lambda e, S, p, sec: BedStream(e, S, p, self._bank(e), r)),
             (self.loudness is not None, "lm",
              lambda e, w: e.normalize_loudness(w, self.loudness, r, true_peak=self.true_peak, limit=self.limit is not None)[0], None),
             (self.loudness is None and self.limit is not None, "lm", lambda e, w: e.limit(w, self.limit, r, self.gain_db)[0],
@@ -2266,6 +2538,11 @@ class AudioChain:
             (self.meter, "mt", None, lambda e, S, p, sec: LoudnessMeter(e, S, p, r, sec)),
         )
         return [s[1:] for s in stages if s[0]]
+
+    def _bank(self, eng: Engine) -> BedBank:
+        if eng not in self._banks:
+            self._banks[eng] = eng.prepare_beds(self._bed_spec, self.rate)
+        return self._banks[eng]
 
     def run(self, eng: Engine, wav) -> np.ndarray:
         """the one-shot host calls of every stage on `wav` ([S] or [B,S] at 16 kHz), in order, then `Engine.encode`
@@ -2283,13 +2560,15 @@ class AudioChain:
             raise ValueError("loudness normalization has no streaming form (use limit= and gain_db=, or meter=True)")
         slow = int(1 / MIN_TEMPO) if self.tempo is not None else 1
         seconds = -(-int(max_frames) * config.HOP * slow // config.SAMPLE_RATE) + 1
+        if self.bed is not None:
+            seconds += -(-self.bed[0]["Tt"] // self.rate)       # the bed's tail
         for name, _, make in self._stages():
             st = make(eng, max_streams, pitch, seconds)
             yield name, st
             pitch = getattr(st, "out_pitch", pitch)
 
 
-_OPENED_WITH = {"semitones": "semitones", "tempo": "tempo", "gain_db": "limit"}   # the open_tts_stream option of each stage
+_OPENED_WITH = {"semitones": "semitones", "tempo": "tempo", "gain_db": "limit", "bed": "bed"}   # the open_tts_stream option of each stage
 
 
 class TtsStream:
@@ -2299,15 +2578,15 @@ class TtsStream:
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
                  output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None, gain_db=0.0, eq=None,
-                 compress=None, deess=None, reverb=None, watermark=None, encoding=None):
+                 compress=None, deess=None, reverb=None, watermark=None, encoding=None, bed=None):
         import torch
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
         self._chain = AudioChain(denoise=denoise, semitones=semitones, tempo=tempo, output_rate=output_rate, eq=eq, limit=limit,
                                  gain_db=gain_db, meter=meter, compress=compress, deess=deess, reverb=reverb,
-                                 watermark=watermark, encoding=encoding)
+                                 watermark=watermark, encoding=encoding, bed=bed)
         self.eng = eng
-        self.rs = self.dn = self.ps = self.ts = self.wm = self.eq = self.cp = self.ds = self.rv = self.lm = self.mt = None
+        self.rs = self.dn = self.ps = self.ts = self.wm = self.eq = self.cp = self.ds = self.rv = self.bd = self.lm = self.mt = None
         S = max_streams
         self._built = []   # every stream handle, in construction order
         try:
@@ -2345,17 +2624,21 @@ class TtsStream:
     def max_streams(self):
         return self.ac.max_streams
 
-    def begin(self, slot: int, tokens, silence_duration=-1.0, semitones=None, tempo=None, gain_db=None):
+    def begin(self, slot: int, tokens, silence_duration=-1.0, semitones=None, tempo=None, gain_db=None, bed=None):
         """Start `tokens` (one row of phoneme ids) in a free slot: durations, the text2mel fix-ups and the trim are
         planned exactly as `Engine.tts` plans them (vtts_tts_plan).  `semitones` and `tempo` override the stream's shift
-        and tempo for this utterance, `gain_db` the limiter's pre-gain.  Returns the number of frames the slot will vocode."""
+        and tempo for this utterance, `gain_db` the limiter's pre-gain, `bed` the bank entry of the stream's beds (default
+        0, -1 for none).  Returns the number of frames the slot will vocode."""
         slot = int(slot)
         if self.ac.open[slot] or slot in self._empty:
             raise ValueError(f"slot {slot} is still open")
-        given = {"semitones": semitones, "tempo": tempo, "gain_db": gain_db}
+        given = {"semitones": semitones, "tempo": tempo, "gain_db": gain_db, "bed": bed}
         values = []   # (a stage's per-slot array, this utterance's value)
         for st, _, kw in self._stages:
-            if st._param is not None:
+            if st is self.bd:
+                v = given.pop("bed")
+                values.append((kw["bed"], int(st.bank.index(BED.default if v is None else v, 1)[0])))
+            elif st._param is not None:
                 v = given.pop(st._param.name)
                 values.append((kw[st._param.name], getattr(self._chain, st._param.name) if v is None else float(st._param.rows(v, 1)[0])))
         for name, v in given.items():

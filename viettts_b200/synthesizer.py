@@ -27,6 +27,10 @@ only while it is loud) at the rate it is written, after --compress and before --
 `--reverb SPEC` places every output in a synthetic room on the device (Engine.reverb: a convolution with a decaying
 noise impulse response, the `room` or `hall` preset or key=value settings) at the rate it is written, after --deess and
 before --loudness / --limiter.
+`--bed FILE.wav[,key=value…]` mixes a background bed under every output on the device (Engine.mix_bed: a mono or stereo
+PCM-16 file, stereo averaged, or `pink` noise, looped with a crossfaded seam, ducked under the voice and carried on for
+a tail) at the rate it is written, after --reverb and before --loudness / --limiter, so the bed counts in the loudness
+and stays under the ceiling.
 `--watermark SPEC` marks every output with a key on the device (Engine.watermark: a keyed spread-spectrum mark, a bare
 integer key or key=…,strength=…) at 16 kHz, after --tempo and before any resampling; `python -m viettts_b200.watermark
 detect --key K FILE.wav` checks a written file for it.
@@ -105,10 +109,11 @@ def write_wav(path, wave, sample_rate: int = config.SAMPLE_RATE, encoding=None) 
         f.write(b"RIFF" + struct.pack("<I", 4 + len(chunks)) + b"WAVE" + chunks)
 
 
-def read_wav_codes(path):
+def read_wav_codes(path, stereo: bool = False):
     """(codes, sample_rate, encoding) of a mono WAVE file in one of the wire encodings: int16 samples for 'pcm16'
-    (format 1, 16 bits), uint8 codes for 'ulaw' (format 7) and 'alaw' (format 6, both 8 bits).  Chunks other than fmt
-    and data are skipped.  Raises ValueError for anything else."""
+    (format 1, 16 bits), uint8 codes for 'ulaw' (format 7) and 'alaw' (format 6, both 8 bits).  With `stereo` a
+    2-channel PCM-16 file is read too, as int16 [N, 2].  Chunks other than fmt and data are skipped.  Raises ValueError
+    for anything else."""
     raw = Path(path).read_bytes()
     if raw[:4] != b"RIFF" or raw[8:12] != b"WAVE":
         raise ValueError(f"{path}: not a RIFF/WAVE file")
@@ -123,9 +128,12 @@ def read_wav_codes(path):
                 raise ValueError(f"{path}: data before the fmt chunk")
             tag, ch, sr, _, _, bits = fmt
             enc = next((e for e, f in WAV_FORMATS.items() if f == (tag, bits)), None)
-            if ch != 1 or enc is None:
-                raise ValueError(f"{path}: format {tag}, {ch} channels, {bits} bits (mono PCM-16, mu-law or A-law)")
-            return np.frombuffer(body, "<i2" if bits == 16 else np.uint8).astype(np.int16 if bits == 16 else np.uint8), sr, enc
+            two = stereo and ch == 2 and enc == "pcm16"
+            if (ch != 1 and not two) or enc is None:
+                raise ValueError(f"{path}: format {tag}, {ch} channels, {bits} bits (mono PCM-16, mu-law or A-law"
+                                 + (", or stereo PCM-16)" if stereo else ")"))
+            codes = np.frombuffer(body, "<i2" if bits == 16 else np.uint8).astype(np.int16 if bits == 16 else np.uint8)
+            return (codes[: codes.size // 2 * 2].reshape(-1, 2) if two else codes), sr, enc
         pos += 8 + size + size % 2
     raise ValueError(f"{path}: no data chunk")
 
@@ -135,6 +143,36 @@ def read_wav(path):
     codes, sr, encoding = read_wav_codes(path)
     assert encoding == "pcm16"
     return codes.astype(np.float32) / 32767.0, sr
+
+
+def read_bed_wav(path):
+    """(float32 mono samples, sample_rate) of a PCM-16 WAVE file for a background bed: a stereo file is downmixed by
+    averaging its two channels (in float64, cast once); samples scale as read_wav's, by 1 / 32767."""
+    codes, sr, enc = read_wav_codes(path, stereo=True)
+    if enc != "pcm16":
+        raise ValueError(f"{path}: a bed is a PCM-16 file, got {enc}")
+    v = codes.astype(np.float64)
+    v = v.mean(axis=1) if v.ndim == 2 else v
+    return (v / 32767.0).astype(np.float32), sr
+
+
+def bed_arg(arg: str):
+    """The bed spec of a `--bed` value: `pink[,key=value…]` as it is, or `FILE.wav[,key=value…]` as a dict holding the
+    file's samples (read_bed_wav) and rate and the keys after it.  Raises ValueError for a file it cannot read."""
+    head, *items = [t.strip() for t in arg.split(",")]
+    if head.lower() == "pink":
+        return arg
+    try:
+        audio, rate = read_bed_wav(head)
+    except OSError as e:
+        raise ValueError(f"cannot read {head}: {e.strerror or e}") from None
+    spec = {"audio": audio, "audio_rate": rate}
+    for item in items:
+        key, eq, val = item.partition("=")
+        if not eq or key.strip() in ("audio", "audio_rate"):
+            raise ValueError(f"{item!r} is not key=value over the bed's keys")
+        spec[key.strip().lower()] = val.strip()
+    return spec
 
 
 def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_rows=32, engine=None, rng=None):
@@ -170,7 +208,7 @@ def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_
 # the command-line flag of each AudioChain option the CLI sets
 _FLAGS = {"denoise": "--denoise", "semitones": "--pitch", "tempo": "--tempo", "output_rate": "--output-rate", "eq": "--eq",
           "limit": "--limiter", "loudness": "--loudness", "compress": "--compress",
-          "deess": "--deess", "reverb": "--reverb", "watermark": "--watermark", "encoding": "--encoding"}
+          "deess": "--deess", "reverb": "--reverb", "watermark": "--watermark", "encoding": "--encoding", "bed": "--bed"}
 
 
 def main(argv=None) -> int:
@@ -225,6 +263,13 @@ def main(argv=None) -> int:
                              "before --loudness / --limiter: 'room' (rt60 0.35 s, 8 ms predelay, mix 0.15), 'hall' (rt60 "
                              "1.8 s, 25 ms predelay, mix 0.22) or comma-separated rt60=, predelay=, mix=, seed= (keys left "
                              "out keep the room values)")
+    parser.add_argument("--bed", default=None, metavar="FILE.wav[,KEY=VALUE...]",
+                        help="mix a background bed under every output on the device at the output rate, after --reverb and "
+                             "before --loudness / --limiter: a mono or stereo PCM-16 WAV file (stereo is averaged; any rate "
+                             "the resampler reaches) or 'pink' (seeded pink noise, seed=, length= s), looped with a crossfade, "
+                             "ducked under the voice and carried on for a tail; keys level= LUFS (-30), duck= dB (12), "
+                             "threshold= dBFS (-40), attack= ms (10), release= ms (500), fade_in= ms (250), tail= ms (1000), "
+                             "xfade= ms (50), offset= s (0)")
     parser.add_argument("--watermark", default=None, metavar="SPEC",
                         help="mark every output with a key on the device at 16 kHz, after --tempo and before --output-rate: "
                              "an integer key in [0, 2^64) or key=K,strength=S (S in [0, 0.3], default 0.1); "
@@ -258,9 +303,13 @@ def main(argv=None) -> int:
     from .engine import AudioChain, OptionError
     ceiling = -1.0 if args.true_peak is None else args.true_peak
     try:
+        bed = None if args.bed is None else bed_arg(args.bed)
+    except ValueError as e:
+        parser.error(f"--bed: {e}")
+    try:
         chain = AudioChain(denoise=args.denoise, semitones=args.pitch, tempo=args.tempo, output_rate=args.output_rate, eq=args.eq,
                            limit=ceiling if args.limiter else None, loudness=args.loudness, true_peak=ceiling, compress=args.compress,
-                           deess=args.deess, reverb=args.reverb, watermark=args.watermark, encoding=args.encoding)
+                           deess=args.deess, reverb=args.reverb, watermark=args.watermark, encoding=args.encoding, bed=bed)
     except OptionError as e:
         parser.error(f"{_FLAGS[e.option]}: {e}")
     header_rate = args.output_rate or args.sample_rate or config.SAMPLE_RATE

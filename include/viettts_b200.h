@@ -864,6 +864,7 @@ int vtts_predict_mel_host(vtts_ctx* ctx, const int32_t* tokens, const int32_t* l
                           const float* dur_frames, const int32_t* n_frames,
                           const uint8_t* keep_mask, int dropout_mode, uint64_t seed,
                           int B, int L, int N, float* mel);
+/* any B: the rows run in launches of at most 128 inside the one call (a row's durations do not depend on the others) */
 int vtts_predict_duration_host(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, int B, int L, float* dur_sec);
 /* predict_mel -> mel2wave without leaving the device: tokens/durations in, waveform out */
 int vtts_synthesize_host(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths,
@@ -882,6 +883,23 @@ int vtts_synthesize_host(vtts_ctx* ctx, const int32_t* tokens, const int32_t* le
 int vtts_tts_host(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, int B, int L, float silence_duration,
                   int dropout_mode, uint64_t seed, int max_frames, float* dur_sec_out, int32_t* n_frames_out,
                   int32_t* n_max_out, float* wav);
+/* Joined utterances: G texts of several sentences each, every sentence one token row, in one call.  Each sentence is
+ * planned as vtts_tts_host plans it alone (vtts_tts_plan, one host round trip for all rows) and run through the acoustic
+ * model; its first n_emit frames are kept.  A text's kept frames, in sentence order, form one mel row, and the
+ * generator runs once over the G rows, so the seams are ordinary context to it.
+ * tokens int32 [B,L] sentence rows (B is not limited: the acoustic model runs them in launches of at most 128 rows);
+ * lengths int32 [B] or NULL; group_start int32 [G+1]: text g owns rows group_start[g] .. group_start[g+1]-1 (0 first,
+ * strictly increasing, B last).  dropout_mode OFF, SEED or REFERENCE (MASK is rejected); in SEED mode the rows of launch
+ * c draw with key seed ^ (c * 0x9E3779B97F4A7C15), so row r draws as row r of predict_mel's chunked calls.
+ * Outputs: dur_sec_out [B,L] as vtts_tts_host (may be NULL); sent_start_out int32 [B] each sentence's first frame in its
+ * text's row (a zero-frame sentence gets the next sentence's start); n_frames_out int32 [G] frames of each text;
+ * *n_max_out the row pitch in frames; wav dense [G][256 * n_max] (zero past 256 * n_frames_out[g]), capacity
+ * G*256*max_frames floats.  If n_max > max_frames nothing is launched after the plan: the call fails with
+ * VTTS_ERR_BAD_ARG after setting the frame outputs, so the caller can retry with that size.  Every bad argument fails
+ * before any launch. */
+int vtts_tts_joined_host(vtts_ctx* ctx, const int32_t* tokens, const int32_t* lengths, int B, int L, const int32_t* group_start, int G,
+                         float silence_duration, int dropout_mode, uint64_t seed, int max_frames, float* dur_sec_out,
+                         int32_t* sent_start_out, int32_t* n_frames_out, int32_t* n_max_out, float* wav);
 int vtts_melspec_host(vtts_ctx* ctx, const float* wav, int B, int S, float* mel);
 /* forward_fn_ of vietTTS/nat/gta.py:28-41 (ground-truth-aligned mels for vocoder fine-tuning): wav_i16 int16 [B,S]
  * (S % 256 == 0) -> /2^15 -> MelFilter -> shift by one frame -> teacher-forced acoustic model -> mel2_out [B,S/256,80].

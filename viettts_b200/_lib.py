@@ -59,6 +59,8 @@ SIGNATURES = {
                                        C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "vtts_tts_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int, C.c_uint64, C.c_int,
                                 C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p]),
+    "vtts_tts_joined_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_int,
+                                       C.c_uint64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p]),
     "vtts_acoustic_teacher_forward": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                 C.c_int, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtts_gta_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,

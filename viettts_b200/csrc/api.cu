@@ -796,9 +796,10 @@ int vtts_predict_duration_host(vtts_ctx* ctx, const int32_t* tokens, const int32
   HostStage hs(ctx);
   const size_t o_tok = hs.in(tokens, (size_t)B * L * 4), o_len = hs.in(lengths, (size_t)B * 4), o_dur = hs.out(dur_b);
   int rc = hs.upload();
-  if (!rc)
-    rc = vtts_duration_forward(ctx, hs.dev<const int32_t>(o_tok), lengths ? hs.dev<const int32_t>(o_len) : nullptr, B, L,
-                               hs.dev<float>(o_dur), hs.st);
+  // launches of at most 128 rows (a row's durations do not depend on the rows launched with it), one round trip
+  for (size_t b0 = 0; b0 < (size_t)B && !rc; b0 += vc::LAUNCH_ROWS)
+    rc = vtts_duration_forward(ctx, hs.dev<const int32_t>(o_tok) + b0 * L, lengths ? hs.dev<const int32_t>(o_len) + b0 : nullptr,
+                               std::min(B - (int)b0, vc::LAUNCH_ROWS), L, hs.dev<float>(o_dur) + b0 * L, hs.st);
   if (!rc) rc = hs.fetch(o_dur, dur_sec, dur_b);
   return rc ? rc : hs.finish();
 }

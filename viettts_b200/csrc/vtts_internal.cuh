@@ -24,6 +24,7 @@ constexpr int POSTNET = 512;
 constexpr int VOCAB = 256;
 constexpr int SIL_INDEX = 0;      // nat/config.py:26 special_phonemes.index("sil")
 constexpr int WORD_END_INDEX = 3; // nat/config.py:28 special_phonemes.index(" ")
+constexpr int LAUNCH_ROWS = 128;  // token rows per acoustic or duration launch (the decoder scan's row limit, nat.cu)
 constexpr int HG_C0 = 512;        // upsample_initial_channel
 constexpr int HG_NSTAGE = 4;
 __host__ __device__ constexpr int hg_rate(int i) { return i < 2 ? 8 : 2; }

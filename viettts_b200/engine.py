@@ -828,10 +828,15 @@ class Engine:
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
                         rng=None, output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None,
                         gain_db=0.0, eq=None, compress=None, deess=None, reverb=None, watermark=None,
-                        encoding=None, bed=None) -> "TtsStream":
+                        encoding=None, bed=None, max_joined_frames=None) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
-        With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.  `output_rate`: a resample
+        With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.
+        `begin(..., more=True)` keeps the slot open after its sentence, and `append(slot, tokens)` adds the next one (a
+        voice agent's text arrives a sentence at a time): the slot's audio is then `tts_joined` of its sentences, one
+        utterance through every stage, bit for bit.  `max_frames` and `max_tokens` bound one sentence;
+        `max_joined_frames` (default `max_frames`) bounds the frames a slot vocodes over all its sentences, and sizes the
+        meter's history.  `output_rate`: a resample
         stream follows the vocoder on the device and `step()` returns samples at that rate, equal to `resample` of the
         `tts` audio bit for bit.  `denoise`: a strength; a denoise stream with the default bias (`denoiser_bias()`) sits
         between the vocoder and the resampler, and the audio equals `denoise` of the `tts` audio (then resampled) bit for
@@ -869,7 +874,8 @@ class Engine:
         synchronisation.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
         return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate,
                          denoise=denoise, meter=meter, semitones=semitones, tempo=tempo, limit=limit, gain_db=gain_db, eq=eq,
-                         compress=compress, deess=deess, reverb=reverb, watermark=watermark, encoding=encoding, bed=bed)
+                         compress=compress, deess=deess, reverb=reverb, watermark=watermark, encoding=encoding, bed=bed,
+                         max_joined_frames=max_joined_frames)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -1035,6 +1041,55 @@ class Engine:
         n = int(nmax.value)
         wav = wav[: B * n * config.HOP].reshape(B, n * config.HOP)
         return [wav[b, : int(nf[b]) * config.HOP].copy() for b in range(B)], dur
+
+    def tts_joined(self, texts, silence_duration=-1.0, seed=None, rng=None, max_frames=None):
+        """Texts of several sentences -> one waveform per text, in ONE library call (vtts_tts_joined_host).  `texts` is a
+        list of texts, each a list of 1-D token rows (its sentences).  Every sentence is planned and run through the
+        acoustic model as `tts` runs it alone; the frames it keeps after its trailing-silence trim are joined in order
+        and the generator runs once per text, so a text sounds as one utterance with no seam to hear.  Any number of
+        sentences per call (the acoustic model runs 128 rows per launch).  Returns (list of f32 waveforms, list of int64
+        arrays: each sentence's first sample in its text's waveform at 16 kHz).  Dropout as `tts`: `seed` (row r draws
+        as row r of `predict_mel(seed=)` on the same rows), else `rng`, else off."""
+        ref_seed = None if rng is None else _rng_seed(rng, seed)
+        rows, bounds = [], [0]
+        for i, text in enumerate(texts):
+            sent = [np.asarray(r) for r in text]
+            if not sent:
+                raise ValueError(f"tts_joined: text {i} has no sentence")
+            for r in sent:
+                if r.ndim != 1 or r.size < 1 or not np.issubdtype(r.dtype, np.integer):
+                    raise ValueError(f"tts_joined: every sentence of text {i} must be a non-empty 1-D row of token ids")
+            rows += sent
+            bounds.append(len(rows))
+        if not rows:
+            raise ValueError("tts_joined: no texts")
+        B, G, L = len(rows), len(bounds) - 1, max(r.size for r in rows)
+        tokens = np.zeros((B, L), np.int32)
+        lens = np.array([r.size for r in rows], np.int32)
+        for b, r in enumerate(rows):
+            tokens[b, : r.size] = r
+        gs = np.asarray(bounds, np.int32)
+        dur = np.empty((B, L), np.float32)
+        starts = np.zeros(B, np.int32)
+        nf = np.zeros(G, np.int32)
+        nmax = C.c_int32(0)
+        text_tokens = int(np.add.reduceat(lens, gs[:-1]).max())
+        cap = int(max_frames) if max_frames else max(16, int(text_tokens * 0.12 * config.SAMPLE_RATE / config.HOP))
+        mode = DROPOUT_SEED if seed is not None else DROPOUT_OFF
+        if ref_seed is not None:
+            mode, seed = DROPOUT_REFERENCE, ref_seed
+        for _ in range(2):
+            wav = np.empty(G * cap * config.HOP, np.float32)
+            rc = self.lib.vtts_tts_joined_host(self.h, _ptr(tokens), _ptr(lens), B, L, _ptr(gs), G, float(silence_duration), mode,
+                                               int(seed or 0), cap, _ptr(dur), _ptr(starts), _ptr(nf), C.byref(nmax), _ptr(wav))
+            if rc == 0 or not (0 < cap < nmax.value):
+                break
+            cap = int(nmax.value)       # buffer too small: the call reported the size it needs
+        self._ck(rc)
+        n = int(nmax.value)
+        wav = wav[: G * n * config.HOP].reshape(G, n * config.HOP)
+        return ([wav[g, : int(nf[g]) * config.HOP].copy() for g in range(G)],
+                [starts[gs[g]: gs[g + 1]].astype(np.int64) * config.HOP for g in range(G)])
 
     def synthesize_many(self, utterances, seed=None, masks=None, max_pad_frac=0.08, max_rows=32, rng=None):
         """Mixed-length workload (BASELINE configs[4]): `utterances` is a list of (tokens list[int],
@@ -2578,8 +2633,11 @@ class TtsStream:
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
                  output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None, gain_db=0.0, eq=None,
-                 compress=None, deess=None, reverb=None, watermark=None, encoding=None, bed=None):
+                 compress=None, deess=None, reverb=None, watermark=None, encoding=None, bed=None, max_joined_frames=None):
         import torch
+        self.max_joined_frames = int(max_frames if max_joined_frames is None else max_joined_frames)
+        if self.max_joined_frames < 1:
+            raise ValueError(f"max_joined_frames must be >= 1, got {self.max_joined_frames}")
         if eng.get_precision() == PRECISION_FP32:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
         self._chain = AudioChain(denoise=denoise, semitones=semitones, tempo=tempo, output_rate=output_rate, eq=eq, limit=limit,
@@ -2594,7 +2652,7 @@ class TtsStream:
             self._built.append(self.ac)
             self.voc = VocoderStream(eng, S, self.ac.out_frames)
             self._built.append(self.voc)
-            for name, st in self._chain.streams(eng, S, self.voc.wav_ld, max_frames):
+            for name, st in self._chain.streams(eng, S, self.voc.wav_ld, self.max_joined_frames):
                 self._built.append(st)
                 setattr(self, name, st)
         except Exception:
@@ -2617,20 +2675,48 @@ class TtsStream:
         self._codes = None if self._chain.encoding is None else _code_tensor(None, tuple(last.shape), self._chain.encoding, dev)
         self._empty_out = np.zeros(0, np.float32 if self._codes is None else ENCODING_DTYPES[self._chain.encoding])
         self._meter = {}
-        self._fresh = np.zeros(max_streams, bool)   # begun, no push yet: the next vocoder push carries BEGIN
+        self._fresh = np.zeros(max_streams, bool)   # begun, no acoustic push yet: the next vocoder push carries BEGIN
         self._empty = set()                         # begun with nothing left after the trim: reported empty at the next step
+        # a slot's utterance, from `begin` until END is pushed: live; another sentence may be appended: more; the
+        # sentence on the acoustic stream ends the utterance: last; what is planned and not started yet, in order (a
+        # (tokens, frames, n_frames, n_emit, last) sentence, or None where the utterance ends without one): queue;
+        # frames vocoded over all its sentences: joined; begin's silence_duration: sil
+        self._live = np.zeros(max_streams, bool)
+        self._more = np.zeros(max_streams, bool)
+        self._last = np.zeros(max_streams, bool)
+        self._queue = [[] for _ in range(max_streams)]
+        self._joined = np.zeros(max_streams, np.int64)
+        self._sil = np.full(max_streams, -1.0)
 
     @property
     def max_streams(self):
         return self.ac.max_streams
 
-    def begin(self, slot: int, tokens, silence_duration=-1.0, semitones=None, tempo=None, gain_db=None, bed=None):
+    def _plan(self, slot: int, tokens, silence_duration, joined: int, queued: bool):
+        """tts_plan of one sentence for `slot`: (tokens [1,L], frames, n_frames, n_emit); raises ValueError if it would
+        take the slot past max_joined_frames, or, for a sentence `queued` to start later, if the acoustic stream would
+        refuse it then"""
+        tok = _np(tokens, np.int32).reshape(1, -1)
+        if queued and tok.shape[1] > self.ac.max_tokens:
+            raise ValueError(f"tts stream: {tok.shape[1]} tokens, the stream takes at most max_tokens={self.ac.max_tokens} per sentence")
+        _, frames, nf, ne = self.eng.tts_plan(tok, silence_duration=silence_duration)
+        if nf[0] < 1:
+            raise ValueError("tts stream: predicted durations sum to less than one frame")
+        if queued and nf[0] > self.ac.max_frames:
+            raise ValueError(f"tts stream: {int(nf[0])} frames, the stream takes at most max_frames={self.ac.max_frames} per sentence")
+        if joined + int(ne[0]) > self.max_joined_frames:
+            raise ValueError(f"tts stream: slot {slot} would vocode {joined + int(ne[0])} frames, more than "
+                             f"max_joined_frames={self.max_joined_frames}")
+        return tok, frames, nf, ne
+
+    def begin(self, slot: int, tokens, silence_duration=-1.0, semitones=None, tempo=None, gain_db=None, bed=None, more=False):
         """Start `tokens` (one row of phoneme ids) in a free slot: durations, the text2mel fix-ups and the trim are
         planned exactly as `Engine.tts` plans them (vtts_tts_plan).  `semitones` and `tempo` override the stream's shift
         and tempo for this utterance, `gain_db` the limiter's pre-gain, `bed` the bank entry of the stream's beds (default
-        0, -1 for none).  Returns the number of frames the slot will vocode."""
+        0, -1 for none).  `more=True` keeps the slot open after this sentence for `append` (or `finish`); every sentence
+        of the slot keeps these values.  Returns the number of frames the slot will vocode."""
         slot = int(slot)
-        if self.ac.open[slot] or slot in self._empty:
+        if self._live[slot] or slot in self._empty:
             raise ValueError(f"slot {slot} is still open")
         given = {"semitones": semitones, "tempo": tempo, "gain_db": gain_db, "bed": bed}
         values = []   # (a stage's per-slot array, this utterance's value)
@@ -2644,39 +2730,93 @@ class TtsStream:
         for name, v in given.items():
             if v is not None:
                 raise ValueError(f"the stream was opened without {_OPENED_WITH[name]}= (no stage takes {name}=)")
-        tok = _np(tokens, np.int32).reshape(1, -1)
-        _, frames, nf, ne = self.eng.tts_plan(tok, silence_duration=silence_duration)
-        if nf[0] < 1:
-            raise ValueError("tts stream: predicted durations sum to less than one frame")
-        if ne[0] == 0:
+        tok, frames, nf, ne = self._plan(slot, tokens, silence_duration, 0, queued=False)
+        if ne[0] == 0 and not more:
             self._empty.add(slot)
             return 0
-        self.ac.begin([slot], tok, frames, n_frames=nf, n_emit=ne)
+        if ne[0] > 0:
+            self.ac.begin([slot], tok, frames, n_frames=nf, n_emit=ne)
+        self._live[slot], self._more[slot], self._last[slot] = True, bool(more), not more
         self._fresh[slot] = True
+        self._joined[slot], self._sil[slot] = int(ne[0]), float(silence_duration)
         for a, v in values:
             a[slot] = v
         return int(ne[0])
 
+    def append(self, slot: int, tokens, more=False):
+        """Add the next sentence to a slot whose last `begin` or `append` had more=True.  It is planned now (with
+        begin's silence_duration), so errors surface here, and queued: it starts on the acoustic stream at the first
+        step where the slot's previous sentence has made its last acoustic push.  The vocoder and every stage see the
+        sentences as one utterance (no flags between them, every state carried), so the slot's audio is `tts_joined` of
+        its sentences.  `more=False` makes it the last.  Returns the number of frames it will vocode."""
+        slot = int(slot)
+        if not self._more[slot]:
+            raise ValueError(f"slot {slot} takes no more sentences (begin it with more=True; append after more=False "
+                             f"or finish is not possible)")
+        tok, frames, nf, ne = self._plan(slot, tokens, self._sil[slot], int(self._joined[slot]), queued=True)
+        self._joined[slot] += int(ne[0])
+        self._more[slot] = bool(more)
+        if ne[0] > 0:
+            self._queue[slot].append((tok, frames, nf, ne, not more))
+        elif not more:
+            self._queue[slot].append(None)
+        return int(ne[0])
+
+    def finish(self, slot: int):
+        """End a slot that still takes sentences (open or waiting) without another one: END goes out in the step after
+        its queued sentences have made their last acoustic push."""
+        slot = int(slot)
+        if not self._more[slot]:
+            raise ValueError(f"slot {slot} takes no more sentences: nothing to finish")
+        self._more[slot] = False
+        self._queue[slot].append(None)
+
     def busy(self) -> np.ndarray:
-        """bool [S]: slots with an utterance still running"""
-        b = self.ac.open.copy()
+        """bool [S]: slots with an utterance still running, including a slot waiting for its next sentence"""
+        b = self._live.copy()
         for s in self._empty:
             b[s] = True
         return b
 
+    def _start_queued(self) -> np.ndarray:
+        """starts the next queued sentence of every slot whose acoustic side is closed; returns the slots whose
+        utterance ends without another sentence (END in this step)"""
+        end_now = np.zeros(self.max_streams, bool)
+        for s in np.flatnonzero(self._live & ~self.ac.open):
+            if not self._queue[s]:
+                continue
+            item = self._queue[s].pop(0)
+            if item is None:
+                end_now[s] = True
+                continue
+            tok, frames, nf, ne, last = item
+            self.ac.begin([int(s)], tok, frames, n_frames=nf, n_emit=ne)
+            self._last[s] = last
+        return end_now
+
     def step(self) -> dict:
         """One acoustic push into a device buffer, then one vocoder push of the frames it emitted (BEGIN on a slot's
-        first push, END on its last); one synchronisation.  Returns {slot: float32 samples} for every slot that was
-        running (possibly empty), or {slot: codes} (int16 or uint8, `Engine.encode` of those samples) when the stream
-        was opened with `encoding`; a slot whose utterance finished this step is free afterwards."""
+        first push, END on its last sentence's last one); one synchronisation.  Returns {slot: float32 samples} for every
+        slot that was running (possibly empty), or {slot: codes} (int16 or uint8, `Engine.encode` of those samples) when
+        the stream was opened with `encoding`; a slot whose utterance finished this step is free afterwards.
+        A slot waiting for its next sentence gets an empty array, and its vocoder and stages get no frames and no flags:
+        each keeps its lookahead (the vocoder's 13 frames, a stage's held samples) until the next sentence or `finish`.
+        That held audio is the cost of a seamless join."""
+        end_now = self._start_queued()
+        never = end_now & self._fresh          # every sentence planned zero frames: nothing was ever pushed
+        live = self._live.copy()
+        self._live &= ~never
         active = self.ac.open.copy()
         closing_before = active.copy()
         n_out = self.ac.push_device(self._mel) if active.any() else np.zeros(self.max_streams, np.int32)
         closed = closing_before & ~self.ac.open
-        flags = (self._fresh & active).astype(np.uint8) * STREAM_BEGIN | closed.astype(np.uint8) * STREAM_END
-        out = {s: self._empty_out.copy() for s in self._empty}
+        end = (closed & self._last) | (end_now & ~never)
+        flags = (self._fresh & active).astype(np.uint8) * STREAM_BEGIN | end.astype(np.uint8) * STREAM_END
+        pushed = active | end
+        self._live &= ~end
+        out = {s: self._empty_out.copy() for s in sorted(self._empty | set(np.flatnonzero(live).tolist()))}
         self._empty = set()
-        if active.any():
+        if pushed.any():
             n_wav = self.voc.push_device(self._mel, n_out, flags, self._wav)
             n_wav = n_wav * config.HOP
             src = self._wav
@@ -2689,11 +2829,11 @@ class TtsStream:
             if self._codes is not None:
                 src = self.eng.encode_forward(src, self._chain.encoding, out=self._codes)
             wav = src.cpu().numpy()
-            for s in np.flatnonzero(active):
+            for s in np.flatnonzero(pushed):
                 out[int(s)] = wav[s, : int(n_wav[s])].copy()
             if self.mt is not None:
                 m = self._mout_h.numpy()
-                self._meter = {int(s): tuple(float(v) for v in m[s]) for s in np.flatnonzero(active)}
+                self._meter = {int(s): tuple(float(v) for v in m[s]) for s in np.flatnonzero(pushed)}
         self._fresh &= ~active
         return out
 

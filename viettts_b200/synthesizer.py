@@ -37,6 +37,9 @@ detect --key K FILE.wav` checks a written file for it.
 `--encoding E` encodes every output on the device (Engine.encode) at the rate it is written, after every other stage,
 and writes that WAVE format: `pcm16` (the same bytes as without the flag), `ulaw` or `alaw` (8-bit G.711, format 7 or
 6, the wire format of telephony, e.g. with `--output-rate 8000 --eq telephone`).
+`--split-sentences` splits `--text` and each `--text-file` line at its sentence ends (split_sentences) and synthesizes
+the sentences as one joined utterance (Engine.tts_joined): a long text runs as a batch of short rows instead of one long
+scan, with one waveform, one output file, as before.
 """
 from __future__ import annotations
 
@@ -175,24 +178,58 @@ def bed_arg(arg: str):
     return spec
 
 
-def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_rows=32, engine=None, rng=None):
-    """Batched text -> list of waveforms (input order).  Lines are sorted by token count and cut into batches of
-    at most `max_rows` rows so the padding inside a batch stays small; every batch is one `Engine.tts` call.
-    Dropout: `rng` (the checkpoint's uint32[2], `text2mel.checkpoint_rng()`) draws the reference's own mask stream on
-    the device, so each line sounds as it does alone through `text2mel`; otherwise the on-device counter stream keyed
-    by `seed` (default: the checkpoint's rng words), whose masks depend on the line's row in its batch."""
+_SENTENCE_END = re.compile(r"[.!?…]+(?=\s|$)|\n")
+
+
+def split_sentences(text: str) -> list:
+    """The sentences of a raw text: it is split after each run of `.`, `!`, `?` or `…` followed by whitespace or the
+    end (so `3.5` stays whole), and at newlines; the run itself is dropped, and so is a piece with no letter or digit.
+    Each piece then goes through nat_normalize_text and text2tokens as a whole text does, so two joined sentences have
+    one silence token between them (the next one's leading sil) where the whole text had the punctuation's one."""
+    return [p for p in _SENTENCE_END.split(text) if any(ch.isalnum() for ch in p)]
+
+
+def _load_models(engine):
+    """the engine with the duration, acoustic and generator checkpoints loaded, and the acoustic checkpoint's rng words"""
     from .nat import text2mel as t2m
     from .hifigan.mel2wave import load_generator
     engine = t2m.load_duration(engine)
     _, ck_seed = t2m.load_acoustic(engine)
+    load_generator(engine)
+    return engine, ck_seed
+
+
+def synthesize_joined(texts, lexicon_file, silence_duration=-1.0, seed=None, rng=None, engine=None):
+    """`texts` split into sentences (split_sentences; a text without one is taken whole) -> one `Engine.tts_joined`
+    call -> one waveform per text, in order"""
+    from .nat import text2mel as t2m
+    sentences = [split_sentences(t) or [t] for t in texts]
+    toks = [[t2m.text2tokens(nat_normalize_text(s), lexicon_file) for s in sent] for sent in sentences]
+    waves, _ = engine.tts_joined(toks, silence_duration=silence_duration, seed=seed, rng=rng)
+    return waves
+
+
+def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_rows=32, engine=None, rng=None, split_sentences=False):
+    """Batched text -> list of waveforms (input order).  Lines are sorted by token count and cut into batches of
+    at most `max_rows` rows so the padding inside a batch stays small; every batch is one `Engine.tts` call.
+    Dropout: `rng` (the checkpoint's uint32[2], `text2mel.checkpoint_rng()`) draws the reference's own mask stream on
+    the device, so each line sounds as it does alone through `text2mel`; otherwise the on-device counter stream keyed
+    by `seed` (default: the checkpoint's rng words), whose masks depend on the line's row in its batch.
+    `split_sentences`: each line is split into its sentences and joined back into one utterance (`Engine.tts_joined`),
+    `max_rows` lines per call."""
+    from .nat import text2mel as t2m
+    engine, ck_seed = _load_models(engine)
     if seed is None and rng is None:
         seed = ck_seed          # default stream key: the checkpoint's rng words
-    load_generator(engine)
     toks = [t2m.text2tokens(nat_normalize_text(line), lexicon_file) for line in lines]
     order = sorted(range(len(toks)), key=lambda i: len(toks[i]))
     out = [None] * len(toks)
     for s in range(0, len(order), max_rows):
         idx = order[s:s + max_rows]
+        if split_sentences:
+            for i, w in zip(idx, synthesize_joined([lines[i] for i in idx], lexicon_file, silence_duration, seed, rng, engine)):
+                out[i] = w
+            continue
         L = max(len(toks[i]) for i in idx)
         tok = np.zeros((len(idx), L), np.int32)
         lens = np.zeros(len(idx), np.int32)
@@ -278,6 +315,10 @@ def main(argv=None) -> int:
                         help="encode every output on the device at the output rate, after every other stage, and write it "
                              "in that WAVE format: pcm16 (16-bit PCM, the default file), ulaw or alaw (8-bit G.711, e.g. "
                              "with --output-rate 8000 --eq telephone for telephony)")
+    parser.add_argument("--split-sentences", action="store_true",
+                        help="split --text, and each --text-file line, at its sentence ends (. ! ? … before a space or the end, "
+                             "and newlines), run the sentences as separate rows and join their frames into one utterance "
+                             "before the vocoder (Engine.tts_joined): long texts run as a batch of short rows")
     parser.add_argument("--silence-duration", default=-1, type=float)
     parser.add_argument("--lexicon-file", default=None)
     parser.add_argument("--seed", default=None, type=int,
@@ -328,7 +369,8 @@ def main(argv=None) -> int:
         if args.reference_dropout:
             from .nat.text2mel import checkpoint_rng
             rng = checkpoint_rng()
-        waves = to_output_rate(synthesize_lines(lines, lexicon, args.silence_duration, seed=args.seed, rng=rng))
+        waves = to_output_rate(synthesize_lines(lines, lexicon, args.silence_duration, seed=args.seed, rng=rng,
+                                                split_sentences=args.split_sentences))
         for i, w in enumerate(waves):
             fn = args.output.with_name(f"{args.output.stem}_{i:04d}{args.output.suffix or '.wav'}")
             print("writing output to file", fn)
@@ -337,6 +379,15 @@ def main(argv=None) -> int:
 
     if args.text is None:
         parser.error("--text or --text-file is required")
+    if args.split_sentences:
+        from .engine import get_engine
+        from .nat.text2mel import checkpoint_rng
+        engine, _ = _load_models(get_engine())
+        rng = checkpoint_rng() if args.seed is None else None
+        wave = to_output_rate(synthesize_joined([args.text], lexicon, args.silence_duration, seed=args.seed, rng=rng, engine=engine))[0]
+        print("writing output to file", args.output)
+        write_wav(args.output, wave, header_rate, encoding=chain.encoding)
+        return 0
     from .hifigan.mel2wave import mel2wave
     from .nat.text2mel import text2mel
     text = nat_normalize_text(args.text)

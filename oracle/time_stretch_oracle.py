@@ -181,10 +181,14 @@ def stretch_scanned(P: int, tempo) -> int:
     if P <= PAD:
         return 0
     a = tempo_of(tempo)
-    q = 0
-    while int(np.rint(256.0 * q * a)) + PAD <= P:
-        q += 1
-    return q
+    lo, hi = 0, int(P)                  # a_q >= 128 q, so q = P is never scanned; bisect the monotone a_q
+    while lo < hi:
+        q = (lo + hi) // 2
+        if int(np.rint(256.0 * q * a)) + PAD <= P:
+            lo = q + 1
+        else:
+            hi = q
+    return lo
 
 
 def stretch_emitted(P: int, tempo, end: bool = False) -> int:

@@ -65,14 +65,15 @@ def chips(key: int) -> np.ndarray:
     return _chip_cache[key]
 
 
-def embed(x, key: int, eps: float) -> np.ndarray:
-    """y of one row in float64 (x taken as float64)"""
+def embed(x, key: int, eps: float, frame0: int = 0) -> np.ndarray:
+    """y of one row in float64 (x taken as float64).  `frame0` is the absolute index of the row's frame 0: a row that
+    starts at sample 256 frame0 of a stream slot, so chip group j = floor((frame0 + f) / 4) mod 64 keys its frame f"""
     x = np.asarray(x, np.float64)
     n = x.size
     if n <= dn.PAD or eps == 0:
         return x.copy()
     X = dn.stft(x)
-    f = np.arange(X.shape[0])
+    f = int(frame0) + np.arange(X.shape[0], dtype=np.int64)
     X[:, K0:K1] *= 1.0 + float(eps) * chips(key)[(f // G) % P]
     y = np.fft.irfft(X, dn.N_FFT, axis=1) * dn.window()[None, :]
     return dn.overlap_add(y, n) / dn.envelope(n)

@@ -386,6 +386,38 @@ int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, con
 int vtts_pitch_shift_stream_push_host(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x, const int32_t* n_new,
                                       const uint8_t* flags, const float* semitones, float* y, int32_t* n_out);
 
+/* ---- voice shift: the pitch shift with the formants kept or moved on their own -----------------------------------------
+ * vtts_pitch_shift with a formant shift phi per row (finite, in [-12, 12], else VTTS_ERR_BAD_ARG before anything is
+ * launched), f = fp32(2^(phi / 12)) computed in double.  Per analysis frame, the real cepstrum of the log magnitudes
+ * (floored 80 dB under the frame's peak) liftered to its first 27 coefficients gives the envelope E[k]:
+ *   m = max_k a[k];  l[k] = ln max(a[k], 1e-4 m, 1e-30);
+ *   c[q] = (l[0] + (-1)^q l[512] + 2 sum_k=1..511 l[k] cos(2 pi k q / 1024)) / 1024, q = 0..26;
+ *   E[k] = c[0] + 2 sum_q=1..26 c[q] cos(2 pi k q / 1024).
+ * Bin k of peak p, landing on t = k + D_p, is multiplied after its rotation by exp(min(E(t / f) - E[k], ln 10^(24/20))),
+ * E(u) linear between E[floor u] and E[floor u + 1] (E[512] past 512), u = t / f in double.  phi = 0 keeps the formants
+ * where they are while the pitch moves; phi != 0 moves them by f whatever the pitch does.  Rows with s == 0 and phi == 0,
+ * and rows of n <= 512, are copied bit for bit; s == 0 with phi != 0 filters the row's STFT by the gains (r = 1, no phase
+ * change).  formants NULL: every row follows the pitch, which is vtts_pitch_shift bit for bit (the vtts_pitch_shift*
+ * functions are these calls with formants = NULL).  The envelope is a function of one frame, so a row gives the same bits
+ * alone, in any batch, and through the stream. */
+/* as vtts_pitch_shift; formants HOST float [B] or NULL.  The workspace grows by 2 KiB per frame of 256 samples. */
+int vtts_voice_shift(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const float* semitones, const float* formants,
+                     float* y_dev, void* stream);
+/* the same on host buffers; n_in[b] must lie in [0, S] */
+int vtts_voice_shift_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, const float* semitones, const float* formants,
+                          float* y);
+/* vtts_pitch_shift_stream_push with formants HOST float [S] or NULL, on a vtts_pitch_shift_stream: a slot's formant shift
+ * is read with BEGIN (NULL: the slots that begin follow the pitch) and fixed until END; for the other pushed slots
+ * formants[s] must hold the slot's formant shift, or NaN for a slot that follows the pitch, or formants may be NULL.  A
+ * different value for an open slot fails with VTTS_ERR_BAD_ARG before anything is launched.  Schedule, lookahead and
+ * launches are the pitch stream's; the outputs a slot emits, concatenated, equal vtts_voice_shift of its whole input. */
+int vtts_voice_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x_dev, const int32_t* n_new,
+                                 const uint8_t* flags, const float* semitones, const float* formants, float* y_dev, int32_t* n_out,
+                                 void* stream);
+/* the same on host buffers x [S][max_chunk_samples] and y [S][out_pitch]; returns when y is written */
+int vtts_voice_shift_stream_push_host(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x, const int32_t* n_new,
+                                      const uint8_t* flags, const float* semitones, const float* formants, float* y, int32_t* n_out);
+
 /* ---- time stretch: the pitch shifter's phase vocoder with moving analysis frames ------------------------------------
  * One row x of n samples, a tempo alpha (fp32, finite, in [0.5, 2], else VTTS_ERR_BAD_ARG before anything is launched;
  * alpha > 1 is faster), after Laroche & Dolson, "Improved phase vocoder time-scale modification of audio" (IEEE TSAP

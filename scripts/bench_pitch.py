@@ -1,6 +1,6 @@
 """Pitch shifter (Engine.pitch_shift_forward, Engine.open_tts_stream(semitones=)) against the generator.
 
-    python scripts/bench_pitch.py [--out FILE.json]
+    python scripts/bench_pitch.py [--formant PHI] [--out FILE.json]
 
   * device time (CUDA events, 20 calls after a warm-up) of shifting the 32 x 5 s batch (B = 32, 313 frames = 80128
     samples at 16 kHz) by +3 semitones, beside the generator's time for that batch in the same process;
@@ -9,7 +9,8 @@
   * TTS stream step time (host clock around step(), which ends in the step's one synchronisation) at S in {1, 32},
     F = 16, with and without semitones=3, the two streams stepped alternately in one process.
 
-Synthetic weights, bf16x3.  The card name and power limit are read (nvidia-smi, read-only) in the same run.  Prints one
+`--formant PHI` adds the voice shift (formant=PHI, the cepstral-envelope kernels) to each case, measured beside the
+pitch shift in the same process (a third TTS stream with semitones=3, formant=PHI).  Synthetic weights, bf16x3.  The card name and power limit are read (nvidia-smi, read-only) in the same run.  Prints one
 JSON object; `--out` also writes it."""
 from __future__ import annotations
 
@@ -29,6 +30,7 @@ from viettts_b200 import synthetic  # noqa: E402
 from viettts_b200.engine import Engine  # noqa: E402
 
 SEMITONES = 3.0
+FORMANT = None     # --formant
 
 
 def kernel_split(fn, reps=5):
@@ -62,8 +64,14 @@ def shift_ms(eng, B, n, reps=20):
     ms = device_ms(fn, reps=reps)
     split = kernel_split(fn)
     frames = B * (n // HOP + 1)
-    return {"B": B, "samples": n, "stft_frames": frames, "ms": ms, "us_per_frame": ms * 1e3 / frames, "kernel_ms": split,
-            "phase_share": split.get("pitch_phase_kernel", 0.0) / max(sum(split.values()), 1e-9)}
+    res = {"B": B, "samples": n, "stft_frames": frames, "ms": ms, "us_per_frame": ms * 1e3 / frames, "kernel_ms": split,
+           "phase_share": split.get("pitch_phase_kernel", 0.0) / max(sum(split.values()), 1e-9)}
+    if FORMANT is not None:
+        fv = lambda: eng.pitch_shift_forward(x, SEMITONES, out=out, formant=FORMANT)   # noqa: E731
+        vms = device_ms(fv, reps=reps)
+        res["voice_shift"] = {"formant": FORMANT, "ms": vms, "us_per_frame": vms * 1e3 / frames, "over_pitch_shift": vms / ms,
+                              "kernel_ms": kernel_split(fv)}
+    return res
 
 
 def batch(eng, B=32, T=313):
@@ -80,6 +88,12 @@ def batch(eng, B=32, T=313):
     res["pitch_shift"] = {"semitones": SEMITONES, "ms": ms, "stft_frames": frames, "us_per_frame": ms * 1e3 / frames,
                           "share_of_generator_time": ms / res["generator_ms"], "kernel_ms": split,
                           "phase_share": split.get("pitch_phase_kernel", 0.0) / max(sum(split.values()), 1e-9)}
+    if FORMANT is not None:
+        fv = lambda: eng.pitch_shift_forward(wav, SEMITONES, out=out, formant=FORMANT)   # noqa: E731
+        vms = device_ms(fv)
+        res["voice_shift"] = {"semitones": SEMITONES, "formant": FORMANT, "ms": vms, "us_per_frame": vms * 1e3 / frames,
+                              "share_of_generator_time": vms / res["generator_ms"], "over_pitch_shift": vms / ms,
+                              "kernel_ms": kernel_split(fv)}
     return res
 
 
@@ -87,13 +101,17 @@ def tts_steps(eng, S, F=16, reps=2):
     tok = [np.asarray(synthetic.utterance(300 + s, 120, None)[0], np.int32) for s in range(S)]
     res = {"S": S, "F": F}
     times = {"plain": [], "pitch": []}
-    with eng.open_tts_stream(S, F, 4000, 1024) as a, eng.open_tts_stream(S, F, 4000, 1024, semitones=SEMITONES) as b:
+    if FORMANT is not None:
+        times["voice"] = []
+    with eng.open_tts_stream(S, F, 4000, 1024) as a, eng.open_tts_stream(S, F, 4000, 1024, semitones=SEMITONES) as b, \
+            eng.open_tts_stream(S, F, 4000, 1024, semitones=SEMITONES, formant=0.0 if FORMANT is None else FORMANT) as c:
+        streams = [("plain", a), ("pitch", b)] + ([("voice", c)] if FORMANT is not None else [])
         for rep in range(reps + 1):            # the first run warms up
             for s in range(S):
-                a.begin(s, tok[s])
-                b.begin(s, tok[s])
-            while a.busy().any() or b.busy().any():
-                for key, ts in (("plain", a), ("pitch", b)):
+                for _, ts in streams:
+                    ts.begin(s, tok[s])
+            while any(ts.busy().any() for _, ts in streams):
+                for key, ts in streams:
                     if ts.busy().any():
                         t0 = time.perf_counter()
                         ts.step()
@@ -104,19 +122,24 @@ def tts_steps(eng, S, F=16, reps=2):
         res[f"step_ms_{key}"] = {"steps": int(t.size), "mean": float(t.mean()), "p50": float(np.percentile(t, 50)),
                                  "p90": float(np.percentile(t, 90))}
     res["mean_step_overhead_ms"] = res["step_ms_pitch"]["mean"] - res["step_ms_plain"]["mean"]
+    if FORMANT is not None:
+        res["mean_step_overhead_ms_voice"] = res["step_ms_voice"]["mean"] - res["step_ms_plain"]["mean"]
     return res
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
+    ap.add_argument("--formant", default=None, type=float)
     args = ap.parse_args()
+    global FORMANT
+    FORMANT = args.formant
     eng = Engine(0)
     eng.load_acoustic(synthetic.acoustic_ckpt(1234))
     eng.load_hifigan(synthetic.hifigan_params(1234))
     eng.load_duration(synthetic.duration_ckpt(1234))
     eng.set_precision("bf16x3")
-    res = {"card": card(), "precision": "bf16x3", "batch": batch(eng), "three_minute_row": shift_ms(eng, 1, 3 * 60 * 16000, reps=5),
+    res = {"card": card(), "precision": "bf16x3", "formant": FORMANT, "batch": batch(eng), "three_minute_row": shift_ms(eng, 1, 3 * 60 * 16000, reps=5),
            "tts_stream": [tts_steps(eng, S) for S in (1, 32)]}
     s = json.dumps(res, indent=1)
     print(s)

@@ -11,6 +11,13 @@
 //   in ascending k | the denoiser's inverse and overlap-add over the synthesis frames at hop H.
 // Pitch shift: a_t = 256 t, F = n / 256 + 1 frames, r = fp32(2^(s / 12)), s in [-12, 12]; n outputs.  (H r - 256) equals
 //   H (r - 1) exactly in double.  Rows with s == 0, and rows of <= 512 samples, are copied.
+// Voice shift: the pitch shift with a formant shift phi (finite, in [-12, 12]) or none (the formants follow the pitch,
+//   the pitch shift above bit for bit).  f = fp32(2^(phi / 12)).  Per analysis frame the cepstral envelope of a = |X_t|:
+//   m = max a, l[k] = ln max(a[k], 1e-4 m, 1e-30), c[q] = (l[0] + (-1)^q l[512] + 2 sum_k=1..511 l[k] cos(2 pi k q / N)) / N
+//   for q = 0..26, E[k] = c[0] + 2 sum_q=1..26 c[q] cos(2 pi k q / N) (cosines from the FFT twiddle table at k q mod N);
+//   bin k landing on t = k + D_p is multiplied after its rotation by exp(min(E(t / f) - E[k], ln 10^(24 / 20))), E(u)
+//   linear between E[floor u] and E[floor u + 1], E[512] past 512, u = t / f in double.  Rows with s == 0 and phi in
+//   {none, 0}, and rows of <= 512 samples, are copied; s == 0 with phi != 0 runs the vocoder at r = 1.
 // Time stretch: tempo alpha (fp32, in [0.5, 2], > 1 faster); M = floor(n / (double)alpha + 0.5) outputs, T = M / 256 + 1
 //   frames, a_t = min(rint(256 t (double)alpha), n - 1), r = 1 (so D_p = 0 and psi_0 = 0).  h_t >= 1: a_t rises by at
 //   least 128 until the clamp, and only the last frame can reach it (256 (T - 2) alpha <= n + 1 - 128).  Rows with
@@ -24,6 +31,12 @@
 // Synthesis kernel.  One warp per frame: the rotated bins and their targets go to shared memory, lane l then sums the
 // targets [16 l, 16 l + 16) over the sources in ascending order, and the denoiser's inverse transform windows the frame.
 // Overlap-add.  denoise_ola_kernel itself (vtts_denoise_ola), over the synthesis frames into the outputs.
+// Envelope.  The analysis and synthesis kernels take a compile-time flag; the legacy instantiations (no row has a formant
+// shift) compile as before.  With it, the analysis warp of a row with f != 0 forms E after the owners: lane l takes the
+// bins [16 l, 16 l + 16) (lane 31 also 512); m by a max-shuffle; each c[q] is the lane's fmaf sum over its bins in
+// ascending order of weight * l[k] * cos (weight 1 at k = 0 and 512, else 2), then an xor-shuffle tree at distances 16,
+// 8, 4, 2, 1, times 1 / 1024; each E[k] is c[0] + 2 s, s the fmaf sum over q = 1..26 ascending.  The synthesis warp
+// multiplies each rotated bin by its gain (fp32 interpolation fmaf(frac, E[i + 1] - E[i], E[i]), expf) before the scatter.
 //
 // Streams.  Per slot the denoiser's window (2048 carried inputs plus one chunk), the 64-bit position, the next unscanned
 // frame, theta and psi (double) of the last scanned frame, and the synthesized frames later outputs still overlap, in
@@ -57,11 +70,13 @@ constexpr int PS_K = 2048;        // carried inputs per stream slot (as the deno
 constexpr int PS_LOOKAHEAD = 1023;
 constexpr int TS_LOOKAHEAD = 1536;  // before END a time-stretch slot has released more than P / alpha - 1536 outputs
 constexpr double TWO_PI = 6.283185307179586;
+constexpr int ENV_Q = 26;                          // cepstral lifter: c[0..26]
+constexpr float ENV_CAP = 2.7631021115928547f;     // ln 10^(24 / 20): the largest boost of a bin
 
 struct PsShift {
   float r;            // pitch: fp32(2^(s / 12)); time stretch: 1
   float tempo;        // time stretch: alpha; pitch: 0 (frames at 256 t, no end clamp)
-  int copy;           // s == 0 or alpha == 1
+  int copy;           // s == 0 with the formants following the pitch or unmoved, or alpha == 1
 };
 
 struct PsRow {
@@ -87,6 +102,13 @@ struct PsWs {
   double* psi;        // [rows][fr][513]: the owner's rotation
   float* syn;         // [rows][halves][nbuf][1024]: windowed time frames
   int fr, nbuf, halves;
+};
+
+// the voice shift's per-call additions, read only by the envelope instantiations (a separate argument, so the legacy
+// kernels keep their parameter layout)
+struct PsEnv {
+  const float* ratio; // [rows]: f = fp32(2^(phi / 12)), or 0 where the formants follow the pitch
+  float* env;         // [rows][fr][513]: E of each analysed frame
 };
 
 // M = floor(n / (double)alpha + 0.5): the time stretcher's output length
@@ -120,10 +142,66 @@ __device__ __forceinline__ PsRow ps_row(const PsRow* rows, const int* n_in, cons
 
 __device__ __forceinline__ double princarg(double x) { return x - TWO_PI * rint(x / TWO_PI); }
 
+// E[0..512] of one frame into env from its magnitudes mag[0..512] (shared, synced over the warp), in the order the
+// header states
+__device__ __forceinline__ void ps_envelope(const float* mag, const float2* __restrict__ tw, int lane, float* __restrict__ env) {
+  const int k0 = 16 * lane, cnt = lane == 31 ? 17 : 16;
+  float m = 0.f;
+#pragma unroll
+  for (int i = 0; i < 17; ++i)
+    if (i < cnt) m = fmaxf(m, mag[k0 + i]);
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, d));
+  const float lo = fmaxf(1e-4f * m, 1e-30f);
+  float l[17];
+#pragma unroll
+  for (int i = 0; i < 17; ++i) {
+    const int k = k0 + i;
+    const float v = i < cnt ? logf(fmaxf(mag[k], lo)) : 0.f;
+    l[i] = k == 0 || k == NB - 1 ? v : 2.f * v;
+  }
+  float c[ENV_Q + 1];
+#pragma unroll
+  for (int q = 0; q <= ENV_Q; ++q) {
+    float p = 0.f;
+#pragma unroll
+    for (int i = 0; i < 17; ++i)
+      if (i < cnt) p = fmaf(l[i], __ldg(&tw[((k0 + i) * q) & (NF - 1)].x), p);
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) p += __shfl_xor_sync(0xffffffffu, p, d);
+    c[q] = p * (1.f / NF);
+  }
+#pragma unroll
+  for (int i = 0; i < 17; ++i) {
+    if (i < cnt) {
+      const int k = k0 + i;
+      float s = 0.f;
+#pragma unroll
+      for (int q = 1; q <= ENV_Q; ++q) s = fmaf(c[q], __ldg(&tw[(k * q) & (NF - 1)].x), s);
+      env[k] = c[0] + 2.f * s;
+    }
+  }
+}
+
+// the gain of a bin k landing on t: exp(min(E(t / f) - E[k], ln 10^(24 / 20)))
+__device__ __forceinline__ float ps_gain(const float* __restrict__ env, int k, int t, float ratio) {
+  const double u = (double)t / (double)ratio;
+  float eu;
+  if (u >= (double)(NB - 1)) {
+    eu = env[NB - 1];
+  } else {
+    const int i = (int)u;
+    const float e0 = env[i];
+    eu = fmaf((float)(u - i), env[i + 1] - e0, e0);
+  }
+  return expf(fminf(eu - env[k], ENV_CAP));
+}
+
+template <bool ENV>
 __global__ void __launch_bounds__(PS_WARPS * 32) pitch_analysis_kernel(const float* __restrict__ x, long long x_ld, int S,
                                                                       const int* __restrict__ n_in, const PsShift* __restrict__ shifts,
                                                                       const PsRow* __restrict__ rows, const float* __restrict__ hann,
-                                                                      const float2* __restrict__ tw, PsWs w) {
+                                                                      const float2* __restrict__ tw, PsWs w, PsEnv e) {
   __shared__ float2 smem[PS_WARPS * 32 * TP];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.y, fl = blockIdx.x * PS_WARPS + warp;
@@ -193,6 +271,9 @@ __global__ void __launch_bounds__(PS_WARPS * 32) pitch_analysis_kernel(const flo
       else o = (rrun == NONE_R || k - L <= rrun - k) ? L : rrun;
       own[k] = (short)o;
     }
+  }
+  if constexpr (ENV) {
+    if (e.ratio[b] != 0.f) ps_envelope(mag, tw, lane, e.env + f * NB);
   }
 }
 
@@ -267,9 +348,10 @@ __global__ void __launch_bounds__(PH_THREADS) pitch_phase_kernel(const int* __re
   }
 }
 
+template <bool ENV>
 __global__ void __launch_bounds__(PS_WARPS * 32) pitch_synth_kernel(const int* __restrict__ n_in, const PsShift* __restrict__ shifts,
                                                                    const PsRow* __restrict__ rows, int S, const float* __restrict__ hann,
-                                                                   const float2* __restrict__ tw, PsWs w) {
+                                                                   const float2* __restrict__ tw, PsWs w, PsEnv e) {
   __shared__ float2 smem[PS_WARPS * 32 * TP];            // per warp: Z[0..512], then the rotated bins [513..1025]
   __shared__ short tg_sh[PS_WARPS][NB + 1];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -289,6 +371,12 @@ __global__ void __launch_bounds__(PS_WARPS * 32) pitch_synth_kernel(const int* _
   float2* rot = sw + NB;
   short* tg = tg_sh[warp];
   const double r1 = (double)r.r - 1.0;
+  float fr = 0.f;
+  const float* env = nullptr;
+  if constexpr (ENV) {
+    fr = e.ratio[b];
+    env = e.env + f * NB;
+  }
   for (int k = lane; k < NB; k += 32) {
     const int p = w.own[f * OWN_LD + k];
     int t = -1;
@@ -301,6 +389,12 @@ __global__ void __launch_bounds__(PS_WARPS * 32) pitch_synth_kernel(const int* _
         sincos(w.psi[f * NB + k], &sn, &cs);
         z = fftc::cmul(w.X[f * NB + k], make_float2((float)cs, (float)sn));
         if (d & 1) z = make_float2(-z.x, -z.y);          // (-1)^D: the phase referred to the frame centre
+        if constexpr (ENV) {
+          if (fr != 0.f) {
+            const float g = ps_gain(env, k, t, fr);
+            z = make_float2(z.x * g, z.y * g);
+          }
+        }
       }
     }
     rot[k] = z;
@@ -333,6 +427,15 @@ int ps_check_shifts(vtts_ctx* ctx, const char* who, const float* semitones, int 
   return VTTS_OK;
 }
 
+// formants: null (every row follows the pitch) or n formant shifts, finite and in [-12, 12]
+int ps_check_formants(vtts_ctx* ctx, const char* who, const float* formants, int n) {
+  if (formants)
+    for (int i = 0; i < n; ++i)
+      if (!shift_ok(formants[i]))
+        return ctx->fail(VTTS_ERR_BAD_ARG, "%s: formants[%d] = %g (finite, in [-12, 12])", who, i, (double)formants[i]);
+  return VTTS_OK;
+}
+
 int ts_check_tempos(vtts_ctx* ctx, const char* who, const float* tempo, int n) {
   if (!tempo) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: null tempo", who);
   for (int i = 0; i < n; ++i)
@@ -342,8 +445,11 @@ int ts_check_tempos(vtts_ctx* ctx, const char* who, const float* tempo, int n) {
 
 // fp32(2^(s / 12)), computed in double and rounded once
 float ps_ratio(float s) { return (float)std::pow(2.0, (double)s / 12.0); }
-PsShift ps_params(float s) { return PsShift{ps_ratio(s), 0.f, s == 0.f}; }
+// phi: the formant shift, NaN where the formants follow the pitch; s == 0 copies unless the formants move
+PsShift ps_params(float s, float phi = NAN) { return PsShift{ps_ratio(s), 0.f, s == 0.f && (std::isnan(phi) || phi == 0.f)}; }
 PsShift ts_params(float tempo) { return PsShift{1.f, tempo, tempo == 1.f}; }
+// the envelope ratio f of a row: 0 (no envelope) where the formants follow the pitch or the row is a copy
+float ps_env_ratio(float phi, const PsShift& h) { return std::isnan(phi) || h.copy ? 0.f : ps_ratio(phi); }
 
 void ps_carve(Arena& a, PsWs& w, int rows) {
   w.X = a.take<float2>((size_t)rows * w.fr * NB);
@@ -352,14 +458,18 @@ void ps_carve(Arena& a, PsWs& w, int rows) {
   w.psi = a.take<double>((size_t)rows * w.fr * NB);
   w.syn = a.take<float>((size_t)rows * w.halves * w.nbuf * NF);
 }
+float* ps_carve_env(Arena& a, const PsWs& w, int rows) { return a.take<float>((size_t)rows * w.fr * NB); }
 
-// analysis, phase, synthesis (three launches); the synthesis is skipped when only the decisions are wanted
+// analysis, phase, synthesis (three launches); the synthesis is skipped when only the decisions are wanted.  env: the
+// envelope instantiations with these buffers, or null for the legacy ones
 int ps_launch(vtts_ctx* ctx, const float* x, long long x_ld, int S, const int* n_in, const PsShift* shifts, const PsRow* rows, int B,
               long long max_nq, long long max_nsyn, const PsWs& w, double* state, DnRow* ola, long long y_cnt, int* dec, int dec_fr,
-              cudaStream_t st) {
+              const PsEnv* env, cudaStream_t st) {
   const float2* tw = reinterpret_cast<const float2*>(ctx->fft_tw);
+  const PsEnv e = env ? *env : PsEnv{};
   const unsigned agrid = (unsigned)std::max(1LL, (max_nq + PS_WARPS - 1) / PS_WARPS);
-  pitch_analysis_kernel<<<dim3(agrid, B), PS_WARPS * 32, 0, st>>>(x, x_ld, S, n_in, shifts, rows, ctx->hann, tw, w);
+  if (env) pitch_analysis_kernel<true><<<dim3(agrid, B), PS_WARPS * 32, 0, st>>>(x, x_ld, S, n_in, shifts, rows, ctx->hann, tw, w, e);
+  else pitch_analysis_kernel<false><<<dim3(agrid, B), PS_WARPS * 32, 0, st>>>(x, x_ld, S, n_in, shifts, rows, ctx->hann, tw, w, e);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   pitch_phase_kernel<<<B, PH_THREADS, 0, st>>>(n_in, shifts, rows, S, w, state, ola, y_cnt, dec, dec_fr);
@@ -367,7 +477,8 @@ int ps_launch(vtts_ctx* ctx, const float* x, long long x_ld, int S, const int* n
   VTTS_CUDA(cudaGetLastError());
   if (dec) return VTTS_OK;
   const unsigned sgrid = (unsigned)std::max(1LL, (max_nsyn + PS_WARPS - 1) / PS_WARPS);
-  pitch_synth_kernel<<<dim3(sgrid, B), PS_WARPS * 32, 0, st>>>(n_in, shifts, rows, S, ctx->hann, tw, w);
+  if (env) pitch_synth_kernel<true><<<dim3(sgrid, B), PS_WARPS * 32, 0, st>>>(n_in, shifts, rows, S, ctx->hann, tw, w, e);
+  else pitch_synth_kernel<false><<<dim3(sgrid, B), PS_WARPS * 32, 0, st>>>(n_in, shifts, rows, S, ctx->hann, tw, w, e);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   return VTTS_OK;
@@ -382,12 +493,14 @@ int ps_check_call(vtts_ctx* ctx, const char* who, const float* x_dev, const void
 }
 
 // one-shot call (dec == nullptr) or the decisions test hook, on checked arguments: rows with the parameters h, F
-// analysis frames for the longest row, Sy outputs per row
+// analysis frames for the longest row, Sy outputs per row; ratio: each row's envelope ratio (ps_env_ratio), or empty
+// for the legacy kernels
 int ps_one_shot(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const std::vector<PsShift>& h, long long F, int Sy,
-                float* y_dev, int* dec_dev, cudaStream_t st) {
+                float* y_dev, int* dec_dev, cudaStream_t st, const std::vector<float>& ratio = {}) {
   VTTS_CUDA(cudaSetDevice(ctx->device));
   int rc = vtts_fft_tables(ctx);
   if (rc) return rc;
+  const bool use_env = !ratio.empty();
   PsWs w{};
   w.fr = (int)F;
   w.nbuf = (int)F;
@@ -396,32 +509,70 @@ int ps_one_shot(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, 
   m.take<PsShift>(B);
   m.take<DnRow>(B);
   ps_carve(m, w, B);
+  if (use_env) {
+    m.take<float>(B);
+    ps_carve_env(m, w, B);
+  }
   rc = ctx->ensure_ws(m.off);
   if (rc) return rc;
   Arena a(ctx->ws, ctx->ws_bytes, false);
   PsShift* shifts = a.take<PsShift>(B);
   DnRow* ola = a.take<DnRow>(B);
   ps_carve(a, w, B);
+  PsEnv env{};
+  if (use_env) {
+    float* r = a.take<float>(B);
+    env.ratio = r;
+    env.env = ps_carve_env(a, w, B);
+    VTTS_CUDA(cudaMemcpyAsync(r, ratio.data(), (size_t)B * sizeof(float), cudaMemcpyHostToDevice, st));
+  }
   // pageable source: the call returns once the table is staged
   VTTS_CUDA(cudaMemcpyAsync(shifts, h.data(), (size_t)B * sizeof(PsShift), cudaMemcpyHostToDevice, st));
   if (dec_dev) {
     VTTS_CUDA(cudaMemsetAsync(dec_dev, 0, (size_t)B * F * NB * sizeof(int), st));
-    return ps_launch(ctx, x_dev, S, S, n_dev, shifts, nullptr, B, F, F, w, nullptr, nullptr, 0, dec_dev, (int)F, st);
+    return ps_launch(ctx, x_dev, S, S, n_dev, shifts, nullptr, B, F, F, w, nullptr, nullptr, 0, dec_dev, (int)F, nullptr, st);
   }
-  rc = ps_launch(ctx, x_dev, S, S, n_dev, shifts, nullptr, B, F, F, w, nullptr, ola, Sy, nullptr, 0, st);
+  rc = ps_launch(ctx, x_dev, S, S, n_dev, shifts, nullptr, B, F, F, w, nullptr, ola, Sy, nullptr, 0, use_env ? &env : nullptr, st);
   if (rc) return rc;
   return vtts_denoise_ola(ctx, x_dev, S, S, nullptr, ola, B, Sy, w.syn, w.nbuf, y_dev, Sy, st);
 }
 
-int ps_call(vtts_ctx* ctx, const char* who, const float* x_dev, const int32_t* n_dev, int B, int S, const float* semitones, float* y_dev,
-            int* dec_dev, cudaStream_t st) {
+// formants: null (the pitch shift: legacy kernels) or one formant shift per row (the envelope kernels)
+int ps_call(vtts_ctx* ctx, const char* who, const float* x_dev, const int32_t* n_dev, int B, int S, const float* semitones,
+            const float* formants, float* y_dev, int* dec_dev, cudaStream_t st) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   int rc = ps_check_call(ctx, who, x_dev, y_dev ? (const void*)y_dev : (const void*)dec_dev, y_dev, B, S);
   if (!rc) rc = ps_check_shifts(ctx, who, semitones, B);
+  if (!rc) rc = ps_check_formants(ctx, who, formants, B);
   if (rc) return rc;
   std::vector<PsShift> h(B);
-  for (int b = 0; b < B; ++b) h[b] = ps_params(semitones[b]);
-  return ps_one_shot(ctx, x_dev, n_dev, B, S, h, S / HOP + 1, S, y_dev, dec_dev, st);
+  std::vector<float> ratio(formants ? B : 0);
+  for (int b = 0; b < B; ++b) {
+    const float phi = formants ? formants[b] : NAN;
+    h[b] = ps_params(semitones[b], phi);
+    if (formants) ratio[b] = ps_env_ratio(phi, h[b]);
+  }
+  return ps_one_shot(ctx, x_dev, n_dev, B, S, h, S / HOP + 1, S, y_dev, dec_dev, st, ratio);
+}
+
+int ps_call_host(vtts_ctx* ctx, const char* who, const char* dev_who, const float* x, const int32_t* n_in, int B, int S,
+                 const float* semitones, const float* formants, float* y) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  if (!x || !y || B < 1 || B > 65535 || S < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: bad argument (B=%d S=%d)", who, B, S);
+  int rc = ps_check_shifts(ctx, who, semitones, B);
+  if (!rc) rc = ps_check_formants(ctx, who, formants, B);
+  if (!rc) rc = host_lengths_check(ctx, who, n_in, B, S);
+  if (rc) return rc;
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  const size_t x_b = (size_t)B * S * 4;
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, (size_t)B * 4), o_y = hs.out(x_b);
+  rc = hs.upload();
+  if (!rc)
+    rc = ps_call(ctx, dev_who, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, semitones, formants,
+                 hs.dev<float>(o_y), nullptr, hs.st);
+  if (!rc) rc = hs.fetch(o_y, y, x_b);
+  return rc ? rc : hs.finish();
 }
 
 // frames of the longest time-stretched row of S samples: max over the rows of M(S) / 256 + 1
@@ -450,31 +601,28 @@ int vtts_pitch_shift_stream_lookahead(void) { return PS_LOOKAHEAD; }
 int vtts_pitch_shift(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const float* semitones, float* y_dev,
                      void* stream) {
   if (ctx && !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift: null pointer");
-  return ps_call(ctx, "pitch_shift", x_dev, n_dev, B, S, semitones, y_dev, nullptr, (cudaStream_t)stream);
+  return ps_call(ctx, "pitch_shift", x_dev, n_dev, B, S, semitones, nullptr, y_dev, nullptr, (cudaStream_t)stream);
+}
+
+int vtts_voice_shift(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const float* semitones, const float* formants,
+                     float* y_dev, void* stream) {
+  if (ctx && !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "voice_shift: null pointer");
+  return ps_call(ctx, "voice_shift", x_dev, n_dev, B, S, semitones, formants, y_dev, nullptr, (cudaStream_t)stream);
 }
 
 int vtts_debug_pitch_decisions(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const float* semitones, int32_t* dec_dev,
                                void* stream) {
   if (ctx && !dec_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "debug_pitch_decisions: null pointer");
-  return ps_call(ctx, "debug_pitch_decisions", x_dev, n_dev, B, S, semitones, nullptr, dec_dev, (cudaStream_t)stream);
+  return ps_call(ctx, "debug_pitch_decisions", x_dev, n_dev, B, S, semitones, nullptr, nullptr, dec_dev, (cudaStream_t)stream);
 }
 
 int vtts_pitch_shift_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, const float* semitones, float* y) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!x || !y || B < 1 || B > 65535 || S < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "pitch_shift_host: bad argument (B=%d S=%d)", B, S);
-  int rc = ps_check_shifts(ctx, "pitch_shift_host", semitones, B);
-  if (!rc) rc = host_lengths_check(ctx, "pitch_shift_host", n_in, B, S);
-  if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4;
-  HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, (size_t)B * 4), o_y = hs.out(x_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = vtts_pitch_shift(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, semitones, hs.dev<float>(o_y),
-                          hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, x_b);
-  return rc ? rc : hs.finish();
+  return ps_call_host(ctx, "pitch_shift_host", "pitch_shift", x, n_in, B, S, semitones, nullptr, y);
+}
+
+int vtts_voice_shift_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, const float* semitones, const float* formants,
+                          float* y) {
+  return ps_call_host(ctx, "voice_shift_host", "voice_shift", x, n_in, B, S, semitones, formants, y);
 }
 
 int64_t vtts_time_stretch_length(int64_t n, float tempo) { return n < 0 || !tempo_ok(tempo) ? -1 : ts_len(n, tempo); }
@@ -514,17 +662,19 @@ int vtts_time_stretch_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, i
 
 // ---- streams ---------------------------------------------------------------------------------------------------
 // One implementation serves both vocoder streams; `stretch` selects the time stretcher's frame positions and schedule.
-struct PvStream : SampleStream<DnRow, PsRow> {
+// Push tables: the overlap-add rows, the vocoder rows and each slot's envelope ratio (PsEnv::ratio).
+struct PvStream : SampleStream<DnRow, PsRow, float> {
   using SampleStream::SampleStream;
   int out_pitch = 0;
   bool stretch = false;
   PsWs w{};
   double* state = nullptr;      // [S][2][513]
+  float* env = nullptr;         // pitch: [S][fr][513] (PsEnv::env)
   // per slot besides the shared state: next unscanned frame, first frame and half of the last push's synthesized-frame
-  // buffer, shift or tempo since BEGIN
+  // buffer, shift or tempo since BEGIN, formant shift since BEGIN (NaN: the formants follow the pitch)
   std::vector<long long> q, fb;
   std::vector<int> half;
-  std::vector<float> par;
+  std::vector<float> par, fpar;
 };
 struct vtts_pitch_shift_stream : PvStream {
   using PvStream::PvStream;
@@ -566,9 +716,11 @@ int pv_create(vtts_ctx* ctx, const char* who, int max_streams, int max_chunk_sam
   ps->fb.assign(S, 0);
   ps->half.assign(S, 0);
   ps->par.assign(S, stretch ? 1.f : 0.f);
+  ps->fpar.assign(S, NAN);
   rc = stream_alloc(ctx, who, *ps, [&](Arena& a) {
     ps->carve_window(a);
     ps_carve(a, ps->w, S);
+    if (!stretch) ps->env = ps_carve_env(a, ps->w, S);
     ps->state = a.take<double>((size_t)S * 2 * NB);
     ps->carve_tables(a);
   });
@@ -578,9 +730,11 @@ int pv_create(vtts_ctx* ctx, const char* who, int max_streams, int max_chunk_sam
   return VTTS_OK;
 }
 
-// par: semitones (pitch) or tempo (time stretch) per slot, read with BEGIN
+// par: semitones (pitch) or tempo (time stretch) per slot, read with BEGIN; fmt (pitch only): formant shifts per slot,
+// read with BEGIN (null: the slots that begin follow the pitch), for an open slot its formant shift or NaN where it
+// follows the pitch
 int pv_push(vtts_ctx* ctx, const char* who, PvStream* ps, const float* x_dev, const int32_t* n_new, const uint8_t* flags, const float* par,
-            float* y_dev, int32_t* n_out, void* stream) {
+            const float* fmt, float* y_dev, int32_t* n_out, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   int rc = stream_args(ctx, who, ps, x_dev && n_new && flags && y_dev && n_out);
   if (rc) return rc;
@@ -600,9 +754,13 @@ int pv_push(vtts_ctx* ctx, const char* who, PvStream* ps, const float* x_dev, co
     if (flags[s] & 1) {
       if (!par) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: BEGIN needs the semitones array", who);
       if (!shift_ok(par[s])) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: semitones[%d] = %g (finite, in [-12, 12])", who, s, (double)par[s]);
+      if (fmt && !shift_ok(fmt[s])) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: formants[%d] = %g (finite, in [-12, 12])", who, s, (double)fmt[s]);
     } else if (par && !(par[s] == ps->par[s])) {
       return ctx->fail(VTTS_ERR_BAD_ARG, "%s: semitones[%d] = %g, but slot %d shifts by %g until END (BEGIN to change it)", who, s,
                        (double)par[s], s, (double)ps->par[s]);
+    } else if (fmt && !(fmt[s] == ps->fpar[s] || (std::isnan(fmt[s]) && std::isnan(ps->fpar[s])))) {
+      return ctx->fail(VTTS_ERR_BAD_ARG, "%s: formants[%d] = %g, but slot %d has formant shift %g until END (NaN: it follows the pitch; "
+                       "BEGIN to change it)", who, s, (double)fmt[s], s, (double)ps->fpar[s]);
     }
     return VTTS_OK;
   });
@@ -615,13 +773,17 @@ int pv_push(vtts_ctx* ctx, const char* who, PvStream* ps, const float* x_dev, co
   // ---- host bookkeeping: outputs [E0, E1), frames [q0, q1) scanned, synthesized-frame buffer [fb, q1) ----
   DnRow* rows = ps->rows<0>();
   PsRow* prow = ps->rows<1>();
+  float* eratio = ps->rows<2>();
   std::vector<long long> E1(S), Q1(S);
   long long max_out = 0, max_nq = 0, max_nsyn = 0;
+  bool use_env = false;
   for (int s = 0; s < S; ++s) {
     const bool act = SlotState::active(n_new, flags, s), begin = flags[s] & 1, end = flags[s] & 2;
     const long long P0 = begin ? 0 : sl.P[s], E0 = begin ? 0 : sl.E[s], P1 = P0 + n_new[s];
     const float pv = begin ? par[s] : ps->par[s];
-    const PsShift h = stretch ? ts_params(pv) : ps_params(pv);
+    const float fv = begin ? (fmt ? fmt[s] : NAN) : ps->fpar[s];
+    const PsShift h = stretch ? ts_params(pv) : ps_params(pv, fv);
+    eratio[s] = act && !stretch ? ps_env_ratio(fv, h) : 0.f;
     const long long M1 = end ? (stretch ? ts_len(P1, pv) : P1) : DN_OPEN;   // the row's outputs, once known
     DnRow r{};
     PsRow p{};
@@ -677,12 +839,16 @@ int pv_push(vtts_ctx* ctx, const char* who, PvStream* ps, const float* x_dev, co
     max_out = std::max(max_out, r.cnt);
     max_nq = std::max(max_nq, (long long)p.nq);
     max_nsyn = std::max(max_nsyn, (long long)p.nsyn);
+    use_env |= eratio[s] != 0.f && p.nq > 0;
   }
 
   // ---- device: table copy, window step, analysis, phase, synthesis, overlap-add (five launches) ----
   rc = ps->upload(n_new, flags, x_dev, st);
   if (rc) return rc;
-  rc = ps_launch(ctx, ps->win, ps->cap, ps->cap, nullptr, nullptr, ps->d_rows<1>(), S, max_nq, max_nsyn, ps->w, ps->state, nullptr, 0, nullptr, 0, st);
+  // the envelope kernels only when a slot scans a frame with its formants moved: the other slots' bits are the same in both
+  const PsEnv env{ps->d_rows<2>(), ps->env};
+  rc = ps_launch(ctx, ps->win, ps->cap, ps->cap, nullptr, nullptr, ps->d_rows<1>(), S, max_nq, max_nsyn, ps->w, ps->state, nullptr, 0, nullptr, 0,
+                 use_env ? &env : nullptr, st);
   if (rc) return rc;
   rc = vtts_denoise_ola(ctx, ps->win, ps->cap, ps->cap, nullptr, ps->d_rows<0>(), S, max_out, ps->w.syn, 2 * ps->w.nbuf, y_dev, ps->out_pitch, st);
   if (rc) return rc;
@@ -691,7 +857,10 @@ int pv_push(vtts_ctx* ctx, const char* who, PvStream* ps, const float* x_dev, co
   for (int s = 0; s < S; ++s) {
     if (!SlotState::active(n_new, flags, s)) continue;
     const bool begin = flags[s] & 1;
-    if (begin) ps->par[s] = par[s];
+    if (begin) {
+      ps->par[s] = par[s];
+      ps->fpar[s] = fmt ? fmt[s] : NAN;
+    }
     if (prow[s].nsyn > 0 || prow[s].nq > 0) {
       ps->fb[s] = prow[s].fb;
       ps->half[s] = prow[s].half;
@@ -706,13 +875,13 @@ int pv_push(vtts_ctx* ctx, const char* who, PvStream* ps, const float* x_dev, co
 }
 
 int pv_push_host(vtts_ctx* ctx, const char* who, PvStream* ps, const float* x, const int32_t* n_new, const uint8_t* flags, const float* par,
-                 float* y, int32_t* n_out, const char* push_who) {
+                 const float* fmt, float* y, int32_t* n_out, const char* push_who) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   int rc = stream_args(ctx, who, ps, x && y);
   if (rc) return rc;
   return stream_push_host(ctx, x, (size_t)ps->S * ps->F * 4, y, (size_t)ps->S * ps->out_pitch * 4,
                           [&](const float* x_dev, float* y_dev, cudaStream_t st) {
-                            return pv_push(ctx, push_who, ps, x_dev, n_new, flags, par, y_dev, n_out, st);
+                            return pv_push(ctx, push_who, ps, x_dev, n_new, flags, par, fmt, y_dev, n_out, st);
                           });
 }
 
@@ -728,12 +897,22 @@ int vtts_pitch_shift_stream_destroy(vtts_ctx* ctx, vtts_pitch_shift_stream* ps) 
 
 int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
                                  const float* semitones, float* y_dev, int32_t* n_out, void* stream) {
-  return pv_push(ctx, "pitch_shift_stream_push", ps, x_dev, n_new, flags, semitones, y_dev, n_out, stream);
+  return pv_push(ctx, "pitch_shift_stream_push", ps, x_dev, n_new, flags, semitones, nullptr, y_dev, n_out, stream);
 }
 
 int vtts_pitch_shift_stream_push_host(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x, const int32_t* n_new, const uint8_t* flags,
                                       const float* semitones, float* y, int32_t* n_out) {
-  return pv_push_host(ctx, "pitch_shift_stream_push_host", ps, x, n_new, flags, semitones, y, n_out, "pitch_shift_stream_push");
+  return pv_push_host(ctx, "pitch_shift_stream_push_host", ps, x, n_new, flags, semitones, nullptr, y, n_out, "pitch_shift_stream_push");
+}
+
+int vtts_voice_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
+                                 const float* semitones, const float* formants, float* y_dev, int32_t* n_out, void* stream) {
+  return pv_push(ctx, "voice_shift_stream_push", ps, x_dev, n_new, flags, semitones, formants, y_dev, n_out, stream);
+}
+
+int vtts_voice_shift_stream_push_host(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x, const int32_t* n_new, const uint8_t* flags,
+                                      const float* semitones, const float* formants, float* y, int32_t* n_out) {
+  return pv_push_host(ctx, "voice_shift_stream_push_host", ps, x, n_new, flags, semitones, formants, y, n_out, "voice_shift_stream_push");
 }
 
 int vtts_time_stretch_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, vtts_time_stretch_stream** out, int* out_pitch) {
@@ -746,10 +925,10 @@ int vtts_time_stretch_stream_destroy(vtts_ctx* ctx, vtts_time_stretch_stream* ts
 
 int vtts_time_stretch_stream_push(vtts_ctx* ctx, vtts_time_stretch_stream* ts, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
                                   const float* tempo, float* y_dev, int32_t* n_out, void* stream) {
-  return pv_push(ctx, "time_stretch_stream_push", ts, x_dev, n_new, flags, tempo, y_dev, n_out, stream);
+  return pv_push(ctx, "time_stretch_stream_push", ts, x_dev, n_new, flags, tempo, nullptr, y_dev, n_out, stream);
 }
 
 int vtts_time_stretch_stream_push_host(vtts_ctx* ctx, vtts_time_stretch_stream* ts, const float* x, const int32_t* n_new,
                                        const uint8_t* flags, const float* tempo, float* y, int32_t* n_out) {
-  return pv_push_host(ctx, "time_stretch_stream_push_host", ts, x, n_new, flags, tempo, y, n_out, "time_stretch_stream_push");
+  return pv_push_host(ctx, "time_stretch_stream_push_host", ts, x, n_new, flags, tempo, nullptr, y, n_out, "time_stretch_stream_push");
 }

@@ -83,6 +83,7 @@ class _BeginParam(NamedTuple):
     hi: float
     default: float | None = None    # a push's value when the keyword is left out (None: required with BEGIN)
     host_check: bool = False        # a push checks the range here (else the library rejects a bad BEGIN value)
+    optional: bool = False          # may be left out with BEGIN: the library gets NULL and the slots take `neutral`
 
     def rows(self, v, n: int) -> np.ndarray:
         return _per_row(v, n, self.name, self.lo, self.hi)
@@ -92,6 +93,8 @@ MAX_SEMITONES = 12.0
 MIN_TEMPO, MAX_TEMPO = 0.5, 2.0
 LIMIT_MAX_GAIN_DB = 70.0
 SEMITONES = _BeginParam("semitones", 0.0, -MAX_SEMITONES, MAX_SEMITONES)
+# the formant shift of the voice shifter; NaN (a slot's value without one): the formants follow the pitch
+FORMANT = _BeginParam("formant", float("nan"), -MAX_SEMITONES, MAX_SEMITONES, optional=True)
 TEMPO = _BeginParam("tempo", 1.0, MIN_TEMPO, MAX_TEMPO)
 GAIN_DB = _BeginParam("gain_db", 0.0, -LIMIT_MAX_GAIN_DB, LIMIT_MAX_GAIN_DB, default=0.0, host_check=True)
 BED = _BeginParam("bed", -1.0, -1.0, 7.0, default=0, host_check=True)     # a bank entry; the bank's size bounds it
@@ -828,7 +831,7 @@ class Engine:
     def open_tts_stream(self, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int = 1024, seed=None,
                         rng=None, output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None,
                         gain_db=0.0, eq=None, compress=None, deess=None, reverb=None, watermark=None,
-                        encoding=None, bed=None, max_joined_frames=None) -> "TtsStream":
+                        encoding=None, bed=None, max_joined_frames=None, formant=None) -> "TtsStream":
         """Text-to-speech per slot as a stream: one acoustic stream feeding one vocoder stream, the mel never leaving the
         device.  `begin(slot, tokens)` plans the utterance as `tts` does; each `step()` returns the new audio per slot.
         With fused pairs off a slot's audio equals `tts` of the same tokens bit for bit.
@@ -842,7 +845,9 @@ class Engine:
         between the vocoder and the resampler, and the audio equals `denoise` of the `tts` audio (then resampled) bit for
         bit.  `semitones`: a pitch-shift stream follows the denoiser (before the resampler) with this shift as every slot's
         default (`begin(..., semitones=)` overrides it per slot), and the audio equals `pitch_shift` of the (denoised)
-        `tts` audio bit for bit.  `tempo`: a time-stretch stream follows the pitch shifter (before the resampler) with this
+        `tts` audio bit for bit.  `formant`: the pitch-shift stream (on with `semitones` or `formant`) moves the formants
+        by this many semitones as every slot's default (`begin(..., formant=)` overrides it per slot; 0 keeps them), and
+        the audio equals `pitch_shift(..., formant=)` bit for bit.  `tempo`: a time-stretch stream follows the pitch shifter (before the resampler) with this
         tempo as every slot's default (`begin(..., tempo=)` overrides it per slot), and the audio equals `time_stretch` of
         the (denoised, pitch-shifted) `tts` audio bit for bit.  `limit=CEILING_DBTP`: a limiter stream follows the
         resampler, at the output rate (a multiple of 10), with pre-gain `gain_db` as every slot's default
@@ -875,7 +880,7 @@ class Engine:
         return TtsStream(self, max_streams, max_chunk_frames, max_frames, max_tokens, seed=seed, rng=rng, output_rate=output_rate,
                          denoise=denoise, meter=meter, semitones=semitones, tempo=tempo, limit=limit, gain_db=gain_db, eq=eq,
                          compress=compress, deess=deess, reverb=reverb, watermark=watermark, encoding=encoding, bed=bed,
-                         max_joined_frames=max_joined_frames)
+                         max_joined_frames=max_joined_frames, formant=formant)
 
     def tts_plan(self, tokens, lengths=None, silence_duration=-1.0):
         """vtts_tts_plan: the duration half of `tts` for token rows [B,L].  Returns (durations in seconds [B,L], durations
@@ -1374,26 +1379,38 @@ class Engine:
         return DenoiseStream(self, max_streams, max_chunk_samples, strength, bias)
 
     # ---- pitch shift (vtts_pitch_shift*: a peak-locked phase vocoder on the denoiser's STFT, fp32, double phases) ----
-    def pitch_shift(self, wav, semitones, lengths=None) -> np.ndarray:
+    def pitch_shift(self, wav, semitones, lengths=None, formant=None) -> np.ndarray:
         """Host arrays: wav f32 [S] or [B,S] -> the same shape, every spectral peak's region moved by the ratio
         fp32(2^(s / 12)) with its phase kept coherent across frames (n_fft 1024, hop 256); the timing of every sample is
         kept.  semitones: a scalar or one value per row, finite and in [-12, 12]; rows with 0 and rows of <= 512 samples
-        are copied.  lengths int [B] in [0, S]: row b holds lengths[b] samples and its outputs past them are 0."""
+        are copied.  lengths int [B] in [0, S]: row b holds lengths[b] samples and its outputs past them are 0.
+        formant (vtts_voice_shift): None, the formants move with the pitch; else a scalar or one value per row, finite
+        and in [-12, 12], the shift of the spectral envelope in semitones whatever the pitch does (0 keeps the voice's
+        formants where they are); rows with semitones 0 and formant 0 are copied."""
         x, lens, one = _wav_rows(wav, lengths)
         B, S = x.shape
         sem = SEMITONES.rows(semitones, B)
+        fmt = None if formant is None else FORMANT.rows(formant, B)
         if S == 0 or B == 0:
             return (x[0] if one else x).copy()          # nothing to transform: empty rows are short rows
         y = np.empty((B, S), np.float32)
-        self._ck(self.lib.vtts_pitch_shift_host(self.h, _ptr(x), _ptr(lens), B, S, _ptr(sem), _ptr(y)))
+        if fmt is None:
+            self._ck(self.lib.vtts_pitch_shift_host(self.h, _ptr(x), _ptr(lens), B, S, _ptr(sem), _ptr(y)))
+        else:
+            self._ck(self.lib.vtts_voice_shift_host(self.h, _ptr(x), _ptr(lens), B, S, _ptr(sem), _ptr(fmt), _ptr(y)))
         return y[0] if one else y
 
-    def pitch_shift_forward(self, x_t, semitones, lengths_t=None, out=None, stream=None):
-        """vtts_pitch_shift on torch CUDA tensors, stream-ordered: x_t f32 [B,S] -> [B,S] (not x_t); semitones a scalar or
-        one host value per row; lengths_t int32 CUDA [B] or None."""
+    def pitch_shift_forward(self, x_t, semitones, lengths_t=None, out=None, stream=None, formant=None):
+        """vtts_pitch_shift (vtts_voice_shift with `formant`, as `pitch_shift` takes it) on torch CUDA tensors,
+        stream-ordered: x_t f32 [B,S] -> [B,S] (not x_t); semitones a scalar or one host value per row; lengths_t int32
+        CUDA [B] or None."""
         B, S, out, st = _dev_rows(x_t, out, stream)
         sem = SEMITONES.rows(semitones, B)
-        self._ck(self.lib.vtts_pitch_shift(self.h, _ptr(x_t), _ptr(lengths_t), B, S, _ptr(sem), _ptr(out), st))
+        if formant is None:
+            self._ck(self.lib.vtts_pitch_shift(self.h, _ptr(x_t), _ptr(lengths_t), B, S, _ptr(sem), _ptr(out), st))
+        else:
+            fmt = FORMANT.rows(formant, B)
+            self._ck(self.lib.vtts_voice_shift(self.h, _ptr(x_t), _ptr(lengths_t), B, S, _ptr(sem), _ptr(fmt), _ptr(out), st))
         return out
 
     def debug_pitch_decisions(self, x_t, semitones, lengths_t=None) -> np.ndarray:
@@ -1413,6 +1430,12 @@ class Engine:
         given with BEGIN and fixed until END, and its outputs, concatenated, equal `pitch_shift` of its whole input bit
         for bit.  Outputs are released on the denoise stream's schedule (at most 1023 samples after their own time)."""
         return PitchShiftStream(self, max_streams, max_chunk_samples)
+
+    def open_voice_shift_stream(self, max_streams: int, max_chunk_samples: int) -> "VoiceShiftStream":
+        """The pitch-shift stream with a formant shift per slot (vtts_voice_shift_stream_push): `semitones=` and
+        `formant=` with BEGIN, fixed until END; a slot's outputs, concatenated, equal `pitch_shift(..., formant=)` of its
+        whole input bit for bit.  Schedule and lookahead are the pitch-shift stream's."""
+        return VoiceShiftStream(self, max_streams, max_chunk_samples)
 
     # ---- time stretch (vtts_time_stretch*: the pitch shifter's phase vocoder with analysis frames at 256 t alpha) ----
     def time_stretch_length(self, n: int, tempo: float) -> int:
@@ -1985,21 +2008,22 @@ STREAM_BEGIN, STREAM_END = 1, 2
 class _SlotStream:
     """What every per-slot stream handle shares: the library handle `h` of one stream of `eng`'s context, the marshalling
     of a push (zero padding of short chunks, the BEGIN / END flag bits, the n_new / flags arrays, the device-buffer checks,
-    the CUDA stream, the per-slot BEGIN parameter), the push itself and the lifecycle.  A subclass opens its stream and
-    declares its kind, its input, its output width and at most one BEGIN parameter."""
+    the CUDA stream, the per-slot BEGIN parameters), the push itself and the lifecycle.  A subclass opens its stream and
+    declares its kind, its input, its output width and its BEGIN parameters."""
     _kind = ""       # the library's vtts_<kind>_push[_host] pushes and vtts_<kind>_destroy closes the stream
+    _push_kind = ""  # the push's own kind where it differs from _kind
     _x = "x"         # the input's name in error messages
     _row = ()        # shape of one input element past [S, F]: () for samples, (80,) for mel frames
     _scale = 1       # output samples per unit of n_out
-    _param = None    # the _BeginParam a push takes for the slots it begins, or None
-    _carried = ""    # with a _param: the attribute holding each slot's value since its BEGIN
+    _params = ()     # the _BeginParams a push takes for the slots it begins, in the push's argument order
+    _carried = ()    # per _param: the attribute holding each slot's value since its BEGIN
     h = None
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk: int):
         self.eng = eng
         self.max_streams, self._chunk = int(max_streams), int(max_chunk)
-        if self._param is not None:
-            setattr(self, self._carried, np.full(self.max_streams, self._param.neutral, np.float32))
+        for p, name in zip(self._params, self._carried):
+            setattr(self, name, np.full(self.max_streams, p.neutral, np.float32))
 
     @property
     def _width(self):
@@ -2043,15 +2067,18 @@ class _SlotStream:
         st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
         return self._args(n_new, flags) + (st,)
 
-    def _values(self, flags, v) -> tuple:
-        """() without a BEGIN parameter, else (float32 [S],): the push's value `v` (a scalar or [S]) for the slots it
-        begins and each slot's carried value elsewhere, which the library checks is unchanged"""
-        p = self._param
-        if p is None:
-            return ()
-        out = getattr(self, self._carried).copy()
+    def _values(self, flags, vs) -> tuple:
+        """per BEGIN parameter, float32 [S]: the push's value (a scalar or [S]) in `vs` for the slots it begins and each
+        slot's carried value elsewhere, which the library checks is unchanged; None for an optional parameter left out
+        (the slots that begin take its neutral value)"""
+        return tuple(self._value(p, name, flags, v) for p, name, v in zip(self._params, self._carried, vs))
+
+    def _value(self, p, carried, flags, v):
+        out = getattr(self, carried).copy()
         begin = (flags & STREAM_BEGIN) != 0
         v = p.default if v is None else v
+        if v is None and p.optional:
+            return None
         if begin.any():
             if v is None:
                 raise ValueError(f"{p.name}= is required for the slots a push begins")
@@ -2062,7 +2089,7 @@ class _SlotStream:
             out[begin] = g[begin]
         if p.host_check:
             _per_row(out, out.size, p.name, p.lo, p.hi, shown=v)
-        return (out,)
+        return out
 
     def _outs(self):
         """the push call's outputs after y: n_out int32 [S] (a subclass adds its own)"""
@@ -2073,24 +2100,24 @@ class _SlotStream:
         return self._rows(y, outs[0], self._scale) if host else outs[0]
 
     def _push(self, host: bool, x, n, f, values, y, outs, st=None):
-        fn = getattr(self.eng.lib, f"vtts_{self._kind}_push" + ("_host" if host else ""))
+        fn = getattr(self.eng.lib, f"vtts_{self._push_kind or self._kind}_push" + ("_host" if host else ""))
         self.eng._ck(fn(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), *map(_ptr, values), _ptr(y), *map(_ptr, outs),
                         *(() if host else (st,))))
-        if values:
-            begin = (f & STREAM_BEGIN) != 0
-            getattr(self, self._carried)[begin] = values[0][begin]
+        begin = (f & STREAM_BEGIN) != 0
+        for p, name, v in zip(self._params, self._carried, values):
+            getattr(self, name)[begin] = p.neutral if v is None else v[begin]
         return self._result(y, outs, host)
 
-    def _push_host(self, x, n_new, begin, end, value=None):
+    def _push_host(self, x, n_new, begin, end, *vs):
         x, n, f = self._host_in(x, n_new, begin, end)
-        values = self._values(f, value)
+        values = self._values(f, vs)
         y = np.empty((self.max_streams, self._width), np.float32)
         return self._push(True, x, n, f, values, y, self._outs())
 
-    def _push_device(self, x_t, n_new, flags, out_t, stream, value=None, dev=()):
+    def _push_device(self, x_t, n_new, flags, out_t, stream, *vs, dev=()):
         """`dev`: the stream's own device outputs after n_out"""
         n, f, st = self._device_in(x_t, out_t, n_new, flags, stream)
-        values = self._values(f, value)
+        values = self._values(f, vs)
         return self._push(False, x_t, n, f, values, out_t, self._outs(*dev), st)
 
     def push(self, x, n_new, begin=None, end=None) -> list:
@@ -2188,7 +2215,7 @@ class PitchShiftStream(_SlotStream):
     """Handle of a streaming pitch shifter (Engine.open_pitch_shift_stream): `semitones=` with BEGIN.  Before END a slot
     that has received P samples has emitted min(P, 256 max(0, floor(P / 256) - 3)) outputs; a push with END emits the
     rest.  `shift` holds each slot's shift since its BEGIN."""
-    _kind, _param, _carried = "pitch_shift_stream", SEMITONES, "shift"
+    _kind, _params, _carried = "pitch_shift_stream", (SEMITONES,), ("shift",)
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int):
         super().__init__(eng, max_streams, max_chunk_samples)
@@ -2205,12 +2232,27 @@ class PitchShiftStream(_SlotStream):
         return self._push_device(x_t, n_new, flags, out_t, stream, semitones)
 
 
+class VoiceShiftStream(PitchShiftStream):
+    """Handle of a streaming voice shifter (Engine.open_voice_shift_stream): the pitch-shift stream with `semitones=`
+    and `formant=` with BEGIN.  `formant` holds each slot's formant shift since its BEGIN (NaN: the formants follow the
+    pitch, as a push that leaves `formant=` out begins its slots)."""
+    _push_kind, _params, _carried = "voice_shift_stream", (SEMITONES, FORMANT), ("shift", "formant")
+
+    def push(self, x, n_new, begin=None, end=None, semitones=None, formant=None) -> list:
+        """As `_SlotStream.push`, with semitones and formant: each a scalar or [S], read for the slots that begin."""
+        return self._push_host(x, n_new, begin, end, semitones, formant)
+
+    def push_device(self, x_t, n_new, flags, out_t, semitones=None, formant=None, stream=None) -> np.ndarray:
+        """As `_SlotStream.push_device`, with semitones and formant (host scalars or [S], read for the slots that begin)."""
+        return self._push_device(x_t, n_new, flags, out_t, stream, semitones, formant)
+
+
 class TimeStretchStream(_SlotStream):
     """Handle of a streaming time stretcher (Engine.open_time_stretch_stream): `tempo=` with BEGIN.  Before END a slot at
     tempo alpha that has scanned Q frames (frame t once rint(256 t alpha) + 512 <= P, P > 512) has released
     max(0, 256 Q - 511) outputs (all P at tempo 1); a push with END releases the rest.  `tempo` holds each slot's tempo
     since its BEGIN."""
-    _kind, _param, _carried = "time_stretch_stream", TEMPO, "tempo"
+    _kind, _params, _carried = "time_stretch_stream", (TEMPO,), ("tempo",)
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int):
         super().__init__(eng, max_streams, max_chunk_samples)
@@ -2272,7 +2314,7 @@ class LimiterStream(_ReductionStream):
     """Handle of a streaming limiter (Engine.open_limiter_stream): `gain_db=` with BEGIN (default 0 dB).  Before END a slot that has received P samples has released
     max(0, P - lookahead) outputs; a push with END releases the rest.  After every host push `reduction_db` holds each
     slot's deepest reduction over what it has released since BEGIN; `gain_db` holds each slot's pre-gain."""
-    _kind, _param, _carried = "limiter_stream", GAIN_DB, "gain_db"
+    _kind, _params, _carried = "limiter_stream", (GAIN_DB,), ("gain_db",)
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, rate: int = config.SAMPLE_RATE, ceiling: float = -1.0,
                  lookahead_ms: float = 5.0, release_ms: float = 100.0):
@@ -2291,7 +2333,7 @@ class LimiterStream(_ReductionStream):
     def push_device(self, x_t, n_new, flags, out_t, reduction_t, gain_db=None, stream=None) -> np.ndarray:
         """As `_SlotStream.push_device`, with reduction_t f32 CUDA [S] (each slot's reduction so far, written on the
         device) and gain_db (host scalar or [S], read for the slots that begin, default 0 dB)."""
-        return self._push_device(x_t, n_new, flags, out_t, stream, gain_db, (reduction_t,))
+        return self._push_device(x_t, n_new, flags, out_t, stream, gain_db, dev=(reduction_t,))
 
 
 class EqStream(_SlotStream):
@@ -2367,7 +2409,7 @@ class BedStream(_ReductionStream):
     none).  Every push releases every sample it brings, and the push with END also the slot's `tail` samples
     (n_out = n_new, + tail at END with a bed; out_pitch = max_chunk_samples + tail).  After every host push
     `reduction_db` holds each slot's deepest duck over what it has released since BEGIN; `bed` holds each slot's entry."""
-    _kind, _param, _carried = "bed_stream", BED, "bed"
+    _kind, _params, _carried = "bed_stream", (BED,), ("bed",)
     lookahead = 0
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, bed="pink", rate: int = config.SAMPLE_RATE):
@@ -2380,9 +2422,10 @@ class BedStream(_ReductionStream):
         self._create(eng.lib.vtts_bed_stream_create, self.max_streams, self.max_chunk_samples, self.rate, *self.bank.args(), pitch=True)
         self.reduction_db = np.zeros(self.max_streams, np.float32)   # host pushes: each slot's reduction so far
 
-    def _values(self, flags, v) -> tuple:
-        """(int32 [S],): the push's entry `v` (default 0; one or one per slot) for the slots it begins, each slot's own
-        elsewhere"""
+    def _values(self, flags, vs) -> tuple:
+        """(int32 [S],): the push's entry `vs[0]` (default 0; one or one per slot) for the slots it begins, each slot's
+        own elsewhere"""
+        (v,) = vs
         out = self.bed.copy()
         begin = (flags & STREAM_BEGIN) != 0
         if begin.any():
@@ -2396,7 +2439,7 @@ class BedStream(_ReductionStream):
     def push_device(self, x_t, n_new, flags, out_t, reduction_t, bed=None, stream=None) -> np.ndarray:
         """As `_SlotStream.push_device`, with reduction_t f32 CUDA [S] (each slot's reduction so far, written on the
         device) and bed (host, read for the slots that begin, default 0)."""
-        return self._push_device(x_t, n_new, flags, out_t, stream, bed, (reduction_t,))
+        return self._push_device(x_t, n_new, flags, out_t, stream, bed, dev=(reduction_t,))
 
 
 class WatermarkStream(_SlotStream):
@@ -2536,7 +2579,7 @@ class AudioChain:
 
     def __init__(self, denoise=None, semitones=None, tempo=None, output_rate=None, eq=None, limit=None, gain_db=0.0,
                  loudness=None, true_peak=None, meter=False, compress=None, deess=None, reverb=None, watermark=None,
-                 encoding=None, bed=None):
+                 encoding=None, bed=None, formant=None):
         def checked(option, check, *args):
             try:
                 return check(*args)
@@ -2547,6 +2590,8 @@ class AudioChain:
         self.rate = self.output_rate or config.SAMPLE_RATE
         self.denoise = None if denoise is None else checked("denoise", _strength, denoise)
         self.semitones = None if semitones is None else float(checked("semitones", SEMITONES.rows, semitones, 1)[0])
+        # the formant shift of the pitch stage (which runs when semitones or formant is given; None follows the pitch)
+        self.formant = None if formant is None else float(checked("formant", FORMANT.rows, formant, 1)[0])
         self.tempo = None if tempo is None else float(checked("tempo", TEMPO.rows, tempo, 1)[0])
         self.watermark = None if watermark is None else checked("watermark", watermark_params, watermark)
         self.eq = None if eq is None else checked("eq", eq_sections, eq, self.rate)
@@ -2573,7 +2618,9 @@ class AudioChain:
         stages = (
             (self.denoise is not None, "dn", lambda e, w: e.denoise(w, self.denoise),
              lambda e, S, p, sec: DenoiseStream(e, S, p, self.denoise)),
-            (self.semitones is not None, "ps", lambda e, w: e.pitch_shift(w, self.semitones), lambda e, S, p, sec: PitchShiftStream(e, S, p)),
+            (self.semitones is not None or self.formant is not None, "ps",
+             lambda e, w: e.pitch_shift(w, self.semitones or 0.0, formant=self.formant),
+             lambda e, S, p, sec: PitchShiftStream(e, S, p) if self.formant is None else VoiceShiftStream(e, S, p)),
             (self.tempo is not None, "ts", lambda e, w: e.time_stretch(w, self.tempo), lambda e, S, p, sec: TimeStretchStream(e, S, p)),
             (self.watermark is not None, "wm", lambda e, w: e.watermark(w, self.watermark),
              lambda e, S, p, sec: WatermarkStream(e, S, p, self.watermark)),
@@ -2623,7 +2670,8 @@ class AudioChain:
             pitch = getattr(st, "out_pitch", pitch)
 
 
-_OPENED_WITH = {"semitones": "semitones", "tempo": "tempo", "gain_db": "limit", "bed": "bed"}   # the open_tts_stream option of each stage
+# the open_tts_stream option of each stage's BEGIN parameter
+_OPENED_WITH = {"semitones": "semitones", "formant": "formant", "tempo": "tempo", "gain_db": "limit", "bed": "bed"}
 
 
 class TtsStream:
@@ -2633,7 +2681,8 @@ class TtsStream:
 
     def __init__(self, eng: Engine, max_streams: int, max_chunk_frames: int, max_frames: int, max_tokens: int, seed=None, rng=None,
                  output_rate=None, denoise=None, meter=False, semitones=None, tempo=None, limit=None, gain_db=0.0, eq=None,
-                 compress=None, deess=None, reverb=None, watermark=None, encoding=None, bed=None, max_joined_frames=None):
+                 compress=None, deess=None, reverb=None, watermark=None, encoding=None, bed=None, max_joined_frames=None,
+                 formant=None):
         import torch
         self.max_joined_frames = int(max_frames if max_joined_frames is None else max_joined_frames)
         if self.max_joined_frames < 1:
@@ -2642,7 +2691,7 @@ class TtsStream:
             raise ValueError("the tts stream needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)")
         self._chain = AudioChain(denoise=denoise, semitones=semitones, tempo=tempo, output_rate=output_rate, eq=eq, limit=limit,
                                  gain_db=gain_db, meter=meter, compress=compress, deess=deess, reverb=reverb,
-                                 watermark=watermark, encoding=encoding, bed=bed)
+                                 watermark=watermark, encoding=encoding, bed=bed, formant=formant)
         self.eng = eng
         self.rs = self.dn = self.ps = self.ts = self.wm = self.eq = self.cp = self.ds = self.rv = self.bd = self.lm = self.mt = None
         S = max_streams
@@ -2665,7 +2714,7 @@ class TtsStream:
         # parameter is the array of each slot's utterance value, set by `begin`
         self._stages = []
         for st in self._built[2:]:
-            kw = {} if st._param is None else {st._param.name: np.full(S, st._param.neutral, np.float32)}
+            kw = {p.name: np.full(S, p.neutral, np.float32) for p in st._params}
             if isinstance(st, _ReductionStream):
                 kw["reduction_t"] = torch.zeros(S, dtype=torch.float32, device=dev)
             self._stages.append((st, torch.zeros((S, st._width), dtype=torch.float32, device=dev), kw))
@@ -2709,24 +2758,26 @@ class TtsStream:
                              f"max_joined_frames={self.max_joined_frames}")
         return tok, frames, nf, ne
 
-    def begin(self, slot: int, tokens, silence_duration=-1.0, semitones=None, tempo=None, gain_db=None, bed=None, more=False):
+    def begin(self, slot: int, tokens, silence_duration=-1.0, semitones=None, tempo=None, gain_db=None, bed=None, more=False,
+              formant=None):
         """Start `tokens` (one row of phoneme ids) in a free slot: durations, the text2mel fix-ups and the trim are
         planned exactly as `Engine.tts` plans them (vtts_tts_plan).  `semitones` and `tempo` override the stream's shift
         and tempo for this utterance, `gain_db` the limiter's pre-gain, `bed` the bank entry of the stream's beds (default
-        0, -1 for none).  `more=True` keeps the slot open after this sentence for `append` (or `finish`); every sentence
+        0, -1 for none), `formant` the formant shift (a stream opened with formant=).  `more=True` keeps the slot open after this sentence for `append` (or `finish`); every sentence
         of the slot keeps these values.  Returns the number of frames the slot will vocode."""
         slot = int(slot)
         if self._live[slot] or slot in self._empty:
             raise ValueError(f"slot {slot} is still open")
-        given = {"semitones": semitones, "tempo": tempo, "gain_db": gain_db, "bed": bed}
+        given = {"semitones": semitones, "formant": formant, "tempo": tempo, "gain_db": gain_db, "bed": bed}
         values = []   # (a stage's per-slot array, this utterance's value)
         for st, _, kw in self._stages:
             if st is self.bd:
                 v = given.pop("bed")
                 values.append((kw["bed"], int(st.bank.index(BED.default if v is None else v, 1)[0])))
-            elif st._param is not None:
-                v = given.pop(st._param.name)
-                values.append((kw[st._param.name], getattr(self._chain, st._param.name) if v is None else float(st._param.rows(v, 1)[0])))
+            else:
+                for p in st._params:
+                    v, dflt = given.pop(p.name), getattr(self._chain, p.name)
+                    values.append((kw[p.name], (p.neutral if dflt is None else dflt) if v is None else float(p.rows(v, 1)[0])))
         for name, v in given.items():
             if v is not None:
                 raise ValueError(f"the stream was opened without {_OPENED_WITH[name]}= (no stage takes {name}=)")

@@ -9,6 +9,8 @@ single library call per batch (`Engine.tts`), and the WAV writer is built in (th
 the reference's meaning, the header rate of the unchanged 16 kHz samples.  `--denoise S` removes the generator's bias
 hiss on the device (Engine.denoise, strength S, the default bias) at 16 kHz, before any resampling.  `--pitch P` shifts
 the voice by P semitones on the device (Engine.pitch_shift) at 16 kHz, after --denoise and before any resampling.
+`--formant F` moves the voice's formants by F semitones whatever the pitch does, in the same stage (with or without
+--pitch): `--pitch 4 --formant 0` is a higher voice from the same throat, `--formant -3` alone a deeper throat.
 `--tempo T` plays the speech T times as fast with its pitch kept (Engine.time_stretch) at 16 kHz, after --pitch and
 before any resampling.
 `--loudness L`
@@ -243,7 +245,7 @@ def synthesize_lines(lines, lexicon_file, silence_duration=-1.0, seed=None, max_
 
 
 # the command-line flag of each AudioChain option the CLI sets
-_FLAGS = {"denoise": "--denoise", "semitones": "--pitch", "tempo": "--tempo", "output_rate": "--output-rate", "eq": "--eq",
+_FLAGS = {"denoise": "--denoise", "semitones": "--pitch", "formant": "--formant", "tempo": "--tempo", "output_rate": "--output-rate", "eq": "--eq",
           "limit": "--limiter", "loudness": "--loudness", "compress": "--compress",
           "deess": "--deess", "reverb": "--reverb", "watermark": "--watermark", "encoding": "--encoding", "bed": "--bed"}
 
@@ -265,6 +267,10 @@ def main(argv=None) -> int:
     parser.add_argument("--pitch", default=None, type=float, metavar="SEMITONES",
                         help="shift the voice's pitch by this many semitones on the device (a peak-locked phase vocoder that "
                              "keeps the timing), in [-12, 12]; at 16 kHz, after --denoise and before --output-rate")
+    parser.add_argument("--formant", default=None, type=float, metavar="SEMITONES",
+                        help="move the voice's formants (its spectral envelope) by this many semitones on the device, in "
+                             "[-12, 12], independently of --pitch (0 keeps them where they are while --pitch moves the "
+                             "pitch); in the --pitch stage")
     parser.add_argument("--tempo", default=None, type=float, metavar="T",
                         help="speak T times as fast with the pitch kept (a peak-locked phase-vocoder time stretch on the "
                              "device), in [0.5, 2]; at 16 kHz, after --pitch and before --output-rate")
@@ -348,7 +354,8 @@ def main(argv=None) -> int:
     except ValueError as e:
         parser.error(f"--bed: {e}")
     try:
-        chain = AudioChain(denoise=args.denoise, semitones=args.pitch, tempo=args.tempo, output_rate=args.output_rate, eq=args.eq,
+        chain = AudioChain(denoise=args.denoise, semitones=args.pitch, formant=args.formant, tempo=args.tempo, output_rate=args.output_rate,
+                           eq=args.eq,
                            limit=ceiling if args.limiter else None, loudness=args.loudness, true_peak=ceiling, compress=args.compress,
                            deess=args.deess, reverb=args.reverb, watermark=args.watermark, encoding=args.encoding, bed=bed)
     except OptionError as e:

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import slot_streams as ss
 from oracle import bed_oracle as bo
 from oracle import watermark_oracle as wo
 from test_bed_cpu import TOL, cases, error_units
@@ -120,82 +121,30 @@ def test_same_bits_in_every_mode_batch_position_and_entry_point(eng):
     assert np.array_equal(eng.mix_bed(x, BANK[0], rate, lengths=lengths)[0][0], ref[0])             # bank entry 0 alone
 
 
-def run_stream(eng, x, lengths, idx, bank, chunk, rate, S, pattern, device=False):
-    """(per row its outputs concatenated, per row its reduction at END); rows go to the slots in turn, so a slot takes
-    its next row with BEGIN in the push after its last row's END"""
-    Tt = bank.params[0]["Tt"]
-    st = eng.open_bed_stream(S, chunk, bank, rate)
-    assert st.lookahead == 0 and st.out_pitch == chunk + Tt and st.tail == Tt
-    R = len(lengths)
-    queue = [[r for r in range(R) if r % S == s] for s in range(S)]
-    out = [[] for _ in range(R)]
-    cur, pos = [None] * S, [0] * S
-    rng = np.random.default_rng(11)
-    x_t = torch.zeros((S, chunk), dtype=torch.float32, device="cuda")
-    y_t = torch.zeros((S, st.out_pitch), dtype=torch.float32, device="cuda")
-    red_t = torch.zeros(S, dtype=torch.float32, device="cuda")
-    reds = {}
-    try:
-        while any(queue[s] or cur[s] is not None for s in range(S)):
-            n_new = np.zeros(S, np.int32)
-            buf = np.zeros((S, chunk), np.float32)
-            begin, end = np.zeros(S, bool), np.zeros(S, bool)
-            bed = np.zeros(S, np.int32)
-            for s in range(S):
-                if cur[s] is None:
-                    if not queue[s]:
-                        continue
-                    cur[s], pos[s], begin[s] = queue[s].pop(0), 0, True
-                r = cur[s]
-                k = chunk if pattern == "full" else int(rng.integers(0, chunk + 1))
-                k = min(k, lengths[r] - pos[s])
-                buf[s, :k] = x[r, pos[s]:pos[s] + k]
-                n_new[s], pos[s] = k, pos[s] + k
-                end[s] = pos[s] >= lengths[r]
-                bed[s] = idx[r] if begin[s] else st.bed[s]
-            if device:
-                x_t.copy_(torch.from_numpy(buf))
-                flags = begin.astype(np.uint8) | (end.astype(np.uint8) << 1)
-                n_out = st.push_device(x_t, n_new, flags, y_t, red_t, bed=bed)
-                y = y_t.cpu().numpy()
-                ys, red = [y[s, :n_out[s]].copy() for s in range(S)], red_t.cpu().numpy()
-            else:
-                ys, red = st.push(buf, n_new, begin, end, bed=bed), st.reduction_db
-            for s in range(S):
-                if cur[s] is None:
-                    assert ys[s].size == 0
-                    continue
-                tail = Tt if end[s] and idx[cur[s]] >= 0 else 0
-                assert ys[s].size == n_new[s] + tail, (s, ys[s].size, n_new[s], tail)      # the tail only at END
-                out[cur[s]].append(ys[s])
-                if end[s]:
-                    reds[cur[s]] = float(red[s])
-                    cur[s] = None
-    finally:
-        st.close()
-    return [np.concatenate(o) for o in out], reds
-
-
 @pytest.mark.parametrize("S", [1, 3, 32])
 @pytest.mark.parametrize("pattern,device", [("full", False), ("random", False), ("random", True)])
 def test_stream_equals_one_shot(eng, S, pattern, device):
+    """rows go to the slots in turn (a slot takes its next row with BEGIN in the push after its last row's END), each
+    with its own bank entry, pushed in `pattern` chunks and held to the stream's contract on every push
+    (tests/helpers/slot_streams.py)"""
     rate = 48000
     bank = eng.prepare_beds(BANK, rate)
+    Tt = bank.params[0]["Tt"]
     R = 2 * S
     rng = np.random.default_rng(S)
     lengths = [int(v) for v in rng.integers(0, 30000, size=R)]
     lengths[0] = 0                                       # BEGIN and END in one push, with nothing in it
     if R > 2:
         lengths[1] = 300                                 # BEGIN and END in one push
-    idx = np.array([(r % 3) - 1 for r in range(R)], np.int32)
+    idx = [(r % 3) - 1 for r in range(R)]
     x = rows(rate, lengths, S)
-    ref, rr = eng.mix_bed(x, bank, rate, lengths=lengths, index=idx)
+    rng = np.random.default_rng(11)
     for chunk in (700, 4096):
-        got, reds = run_stream(eng, x, lengths, idx, bank, chunk, rate, S, pattern, device=device)
-        for r in range(R):
-            m = lengths[r] + (bank.params[0]["Tt"] if idx[r] >= 0 else 0)
-            assert got[r].shape == (m,) and np.array_equal(got[r], ref[r, :m]), (chunk, r)
-            assert reds[r] == rr[r], (chunk, r)
+        stage = ss.stage(eng, "bed", S, chunk, rate, bed=bank)
+        with stage.open() as st:
+            assert st.lookahead == 0 and st.out_pitch == chunk + Tt and st.tail == Tt
+        plans = [[ss.pattern(pattern, lengths[r], chunk, rng) for r in range(s, R, S)] for s in range(S)]
+        ss.run(stage, plans, lambda s, u, n: x[s + u * S, :n], [idx[s::S] for s in range(S)], host=not device)
 
 
 def test_launch_counts(eng):

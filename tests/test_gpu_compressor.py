@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import slot_streams as ss
 from oracle import compressor_oracle as co
 from test_compressor_cpu import PARAMS, TOL, cases, error_units, speech_like
 from viettts_b200 import config, synthetic
@@ -110,64 +111,19 @@ def test_forward_in_place_and_device_reduction(eng):
     assert np.array_equal(y_t.cpu().numpy(), ref) and np.array_equal(r_t.cpu().numpy(), rr)
 
 
-def run_stream(eng, x, lengths, spec, chunk, rate, S, pattern, device=False):
-    st = eng.open_compressor_stream(S, chunk, spec, rate)
-    out = [[] for _ in range(S)]
-    pos = [0] * S
-    rng = np.random.default_rng(7)
-    begun = [False] * S
-    x_t = torch.zeros((S, chunk), dtype=torch.float32, device="cuda")
-    r_t = torch.zeros(S, dtype=torch.float32, device="cuda")
-    try:
-        while any(pos[s] < lengths[s] or not begun[s] for s in range(S)):
-            n_new = np.zeros(S, np.int32)
-            buf = np.zeros((S, chunk), np.float32)
-            begin = np.zeros(S, bool)
-            end = np.zeros(S, bool)
-            for s in range(S):
-                if begun[s] and pos[s] >= lengths[s]:
-                    continue
-                k = 1 if pattern == "one" else (chunk if pattern == "full" else int(rng.integers(0, chunk + 1)))
-                k = min(k, lengths[s] - pos[s])
-                buf[s, :k] = x[s, pos[s]:pos[s] + k]
-                n_new[s] = k
-                begin[s] = not begun[s]
-                begun[s] = True
-                pos[s] += k
-                end[s] = pos[s] >= lengths[s]
-            if device:
-                x_t.copy_(torch.from_numpy(buf))
-                flags = begin.astype(np.uint8) | (end.astype(np.uint8) << 1)
-                n_out = st.push_device(x_t, n_new, flags, x_t, r_t)       # in place
-                assert np.array_equal(n_out, n_new)
-                y = x_t.cpu().numpy()
-                ys = [y[s, :n_out[s]].copy() for s in range(S)]
-                red = r_t.cpu().numpy()
-            else:
-                ys = st.push(buf, n_new, begin, end)
-                red = st.reduction_db.copy()
-            for s, y in enumerate(ys):
-                assert y.size == n_new[s]
-                out[s].append(y)
-    finally:
-        st.close()
-    return [np.concatenate(o) for o in out], red
-
-
 @pytest.mark.parametrize("S", [1, 3, 32])
 @pytest.mark.parametrize("pattern", ["one", "full", "random"])
 def test_stream_equals_one_shot(eng, S, pattern):
+    """rows pushed in `pattern` chunks (through push_device, in place, for "random") and held to the stream's
+    contract on every push (tests/helpers/slot_streams.py)"""
     rate = 16000
     if pattern == "one" and S == 32:
         pytest.skip("one-sample pushes run at S = 1 and 3")
     lengths = [int(v) for v in np.random.default_rng(S).integers(1, 2500 if pattern == "one" else 9000, size=S)]
     x = rows(rate, lengths, S)
-    spec = "attack=1,release=40,threshold=-30"
-    got, red = run_stream(eng, x, lengths, spec, 700, rate, S, pattern, device=pattern == "random")
-    ref, rref = eng.compress(x, spec, rate, lengths=lengths)
-    for s in range(S):
-        assert got[s].shape == (lengths[s],) and np.array_equal(got[s], ref[s, :lengths[s]]), s
-    assert np.array_equal(red, rref)
+    rng = np.random.default_rng(7)
+    stage = ss.stage(eng, "compressor", S, 700, rate, spec="attack=1,release=40,threshold=-30")
+    ss.run(stage, [[ss.pattern(pattern, n, 700, rng)] for n in lengths], lambda s, u, n: x[s, :n], host=pattern != "random")
 
 
 def test_launch_counts(eng):

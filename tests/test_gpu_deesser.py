@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import slot_streams as ss
 from oracle import deesser_oracle as do
 from test_deesser_cpu import PARAMS, TOL, cases, clear_of_bursts, error_units, parts, sibilant_speech
 from viettts_b200 import config, synthetic
@@ -121,67 +122,22 @@ def test_forward_in_place_and_device_reduction(eng):
     assert np.array_equal(y_t.cpu().numpy(), ref) and np.array_equal(r_t.cpu().numpy(), rr)
 
 
-def run_stream(eng, x, lengths, spec, chunk, rate, S, pattern, device=False):
-    st = eng.open_deesser_stream(S, chunk, spec, rate)
-    out = [[] for _ in range(S)]
-    pos = [0] * S
-    rng = np.random.default_rng(7)
-    begun = [False] * S
-    x_t = torch.zeros((S, chunk), dtype=torch.float32, device="cuda")
-    r_t = torch.zeros(S, dtype=torch.float32, device="cuda")
-    try:
-        while any(pos[s] < lengths[s] or not begun[s] for s in range(S)):
-            n_new = np.zeros(S, np.int32)
-            buf = np.zeros((S, chunk), np.float32)
-            begin = np.zeros(S, bool)
-            end = np.zeros(S, bool)
-            for s in range(S):
-                if begun[s] and pos[s] >= lengths[s]:
-                    continue
-                k = 1 if pattern == "one" else (chunk if pattern == "full" else int(rng.integers(0, chunk + 1)))
-                k = min(k, lengths[s] - pos[s])
-                buf[s, :k] = x[s, pos[s]:pos[s] + k]
-                n_new[s] = k
-                begin[s] = not begun[s]
-                begun[s] = True
-                pos[s] += k
-                end[s] = pos[s] >= lengths[s]
-            if device:
-                x_t.copy_(torch.from_numpy(buf))
-                flags = begin.astype(np.uint8) | (end.astype(np.uint8) << 1)
-                n_out = st.push_device(x_t, n_new, flags, x_t, r_t)       # in place
-                assert np.array_equal(n_out, n_new)
-                y = x_t.cpu().numpy()
-                ys = [y[s, :n_out[s]].copy() for s in range(S)]
-                red = r_t.cpu().numpy()
-            else:
-                ys = st.push(buf, n_new, begin, end)
-                red = st.reduction_db.copy()
-            for s, y in enumerate(ys):
-                assert y.size == n_new[s]
-                out[s].append(y)
-    finally:
-        st.close()
-    return [np.concatenate(o) for o in out], red
-
-
 @pytest.mark.parametrize("S", [1, 3, 32])
 @pytest.mark.parametrize("pattern,device", [("one", False), ("full", False), ("full", True), ("random", False), ("random", True)])
 def test_stream_equals_one_shot(eng, S, pattern, device):
+    """rows pushed in `pattern` chunks (device pushes in place) and held to the stream's contract on every push
+    (tests/helpers/slot_streams.py)"""
     rate = 48000
     if pattern == "one" and S == 32:
         pytest.skip("one-sample pushes run at S = 1 and 3")
     # lengths and chunks across both block sizes (256 and 1024)
     lengths = [int(v) for v in np.random.default_rng(S).integers(1, 2500 if pattern == "one" else 12000, size=S)]
     x = rows(rate, lengths, S)
-    spec = "attack=0.5,release=20,threshold=-40"
+    rng = np.random.default_rng(7)
     for chunk in (700, 1500):
-        got, red = run_stream(eng, x, lengths, spec, chunk, rate, S, pattern, device=device)
-        ref, rref = eng.deess(x, spec, rate, lengths=lengths)
-        for s in range(S):
-            assert got[s].shape == (lengths[s],) and np.array_equal(got[s], ref[s, :lengths[s]]), (chunk, s)
-        assert np.array_equal(red, rref), chunk
-        assert rref.min() < 0
+        stage = ss.stage(eng, "deesser", S, chunk, rate, spec="attack=0.5,release=20,threshold=-40")
+        out = ss.run(stage, [[ss.pattern(pattern, n, chunk, rng)] for n in lengths], lambda s, u, n: x[s, :n], host=not device)
+        assert min(row[0][3] for row in out) < 0
         if pattern == "one":
             break
 

@@ -12,10 +12,10 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import slot_streams as ss
 from oracle import denoise_oracle as do
 from test_denoise_cpu import STRENGTHS, TOL, hiss_bias, signal_of
 from viettts_b200 import config, synthetic
-from viettts_b200.engine import STREAM_BEGIN, STREAM_END
 
 pytestmark = pytest.mark.gpu
 KEY = np.array([7, 1234567], np.uint32)
@@ -95,91 +95,26 @@ def test_zero_strength_reconstructs(eng):
 
 # ---- stream ------------------------------------------------------------------------------------------------------
 
-def push_plans(kind, F, rng):
-    """utterances of one slot, each a list of push sizes (END with the last one)"""
-    if kind == "ones":
-        return [[1] * int(rng.integers(1100, 1500))]
-    if kind in (255, 256, 1000):
-        return [[min(kind, F)] * int(rng.integers(4, 12))]
-    if kind == "max":
-        return [[F] * int(rng.integers(2, 5)) + [int(rng.integers(1, F))]]
-    if kind == "end_empty":
-        return [[int(v) for v in rng.integers(1, F + 1, size=4)] + [0]]
-    if kind == "short":
-        return [[int(rng.integers(1, 200)), int(rng.integers(0, 200))], [512], [513]]
-    if kind == "reuse":
-        return [[int(v) for v in rng.integers(1, F + 1, size=3)], [int(v) for v in rng.integers(1, F + 1, size=5)]]
-    return []    # idle
+KINDS = [k for k in ss.KINDS if k != "late"]
 
 
-KINDS = ["ones", 255, 256, 1000, "max", "end_empty", "short", "reuse", "idle"]
-
-
-def run_stream(eng, S, F, kinds, strength, bias, seed):
+def run_stream(eng, S, F, kinds, strength, seed):
+    """slot s runs plan kinds[s]; every push is held to the stream's contract (tests/helpers/slot_streams.py)"""
     rng = np.random.default_rng(seed)
-    dev = torch.device("cuda", 0)
-    plans = []
-    for k in kinds:
-        flat = []
-        for u, sizes in enumerate(push_plans(k, F, rng)):
-            for q, n in enumerate(sizes):
-                flat.append((n, (STREAM_BEGIN if q == 0 else 0) | (STREAM_END if q == len(sizes) - 1 else 0), u))
-        plans.append(flat)
-    data = [dict() for _ in range(S)]
-    got = [dict() for _ in range(S)]
-    P = np.zeros(S, np.int64)
-    E = np.zeros(S, np.int64)
-    with eng.open_denoise_stream(S, F, strength, bias=bias) as ds:
+    stage = ss.stage(eng, "denoise", S, F, strength=strength, bias=hiss_bias())
+    with stage.open() as ds:
         assert ds.lookahead == do.LOOKAHEAD
-        xt = torch.zeros((S, F), device=dev)
-        yt = torch.empty((S, ds.out_pitch), device=dev)
-        for c in range(max(len(p) for p in plans)):
-            n_new = np.zeros(S, np.int32)
-            flags = np.zeros(S, np.uint8)
-            x = np.full((S, F), np.nan, np.float32)          # past n_new: never read
-            for s in range(S):
-                if c >= len(plans[s]):
-                    continue
-                n, f, u = plans[s][c]
-                n_new[s], flags[s] = n, f
-                chunk = signal_of(max(n, 1), 1000 * s + 10 * c + u)[:n]
-                x[s, :n] = chunk
-                if f & STREAM_BEGIN:
-                    data[s][u], got[s][u] = [], []
-                    P[s] = E[s] = 0
-                data[s][u].append(chunk)
-            xt.copy_(torch.from_numpy(x))
-            yt.fill_(12345.0)
-            before = eng.launch_count()
-            n_out = ds.push_device(xt, n_new, flags, yt)
-            assert eng.launch_count() - before == 3
-            y = yt.cpu().numpy()
-            for s in range(S):
-                if n_new[s] == 0 and flags[s] == 0:
-                    assert n_out[s] == 0 and np.all(y[s] == 12345.0), (s, c)     # idle: untouched
-                    continue
-                P[s] += n_new[s]
-                e = int(P[s]) if flags[s] & STREAM_END else do.emitted_closed_form(int(P[s]))
-                assert n_out[s] == e - E[s], (kinds[s], s, c, int(P[s]), int(n_out[s]), e - E[s])
-                E[s] = e
-                got[s][plans[s][c][2]].append(y[s, : n_out[s]].copy())
-    for s in range(S):
-        for u, chunks in data[s].items():
-            xs = np.concatenate(chunks)
-            out = np.concatenate(got[s][u])
-            ref = eng.denoise(xs, strength, bias=bias)
-            assert out.shape == ref.shape and np.array_equal(out, ref), (kinds[s], s, u, xs.size)
+    ss.run(stage, [ss.push_plan(k, F, rng) for k in kinds], lambda s, u, n: signal_of(n, 1000 * s + u))
 
 
 @pytest.mark.parametrize("S", [1, 3, 32])
 def test_stream_equals_one_shot(eng, S):
-    F = 1000
     kinds = ["max"] if S == 1 else [KINDS[(s + S) % len(KINDS)] for s in range(S)]
-    run_stream(eng, S, F, kinds, 0.3, hiss_bias(), seed=S)
+    run_stream(eng, S, 1000, kinds, 0.3, seed=S)
 
 
 def test_stream_one_sample_pushes_and_edges(eng):
-    run_stream(eng, 4, 1024, ["ones", 255, 256, "short"], 1.0, hiss_bias(), seed=99)
+    run_stream(eng, 4, 1024, ["ones", 255, 256, "short"], 1.0, seed=99)
 
 
 def test_stream_host_push_equals_device_push(eng):

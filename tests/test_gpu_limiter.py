@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import slot_streams as ss
 from oracle import limiter_oracle as lm
 from oracle import loudness_oracle as lo
 from test_limiter_cpu import TP_MARGIN, Y_TOL, clicks, error_units, fs4_sine, noise, speech_like
@@ -113,51 +114,21 @@ def test_forward_in_place_and_device_gain(eng):
     assert np.array_equal(y_t.cpu().numpy(), ref) and np.array_equal(r_t.cpu().numpy(), rr)
 
 
-def run_stream(eng, x, lengths, gains, chunk, rate, S, pattern):
-    st = eng.open_limiter_stream(S, chunk, rate, -1.0, 3.0, 60.0)
-    out = [[] for _ in range(S)]
-    pos = [0] * S
-    rng = np.random.default_rng(7)
-    begun = [False] * S
-    try:
-        while any(pos[s] < lengths[s] or not begun[s] for s in range(S)):
-            n_new = np.zeros(S, np.int32)
-            buf = np.zeros((S, chunk), np.float32)
-            begin = np.zeros(S, bool)
-            end = np.zeros(S, bool)
-            for s in range(S):
-                if begun[s] and pos[s] >= lengths[s]:
-                    continue
-                k = 1 if pattern == "one" else (chunk if pattern == "full" else int(rng.integers(0, chunk + 1)))
-                k = min(k, lengths[s] - pos[s])
-                buf[s, :k] = x[s, pos[s]:pos[s] + k]
-                n_new[s] = k
-                begin[s] = not begun[s]
-                begun[s] = True
-                pos[s] += k
-                end[s] = pos[s] >= lengths[s]
-            for s, y in enumerate(st.push(buf, n_new, begin, end, gain_db=gains)):
-                out[s].append(y)
-        red = st.reduction_db.copy()
-    finally:
-        st.close()
-    return [np.concatenate(o) for o in out], red
-
-
 @pytest.mark.parametrize("S", [1, 3, 32])
 @pytest.mark.parametrize("pattern", ["one", "full", "random"])
 def test_stream_equals_one_shot(eng, S, pattern):
+    """rows pushed in `pattern` chunks through the host push, each slot at its own pre-gain, and held to the stream's
+    contract on every push (tests/helpers/slot_streams.py)"""
     rate = 16000
     if pattern == "one" and S == 32:
         pytest.skip("one-sample pushes run at S = 1 and 3")
     lengths = [int(v) for v in np.random.default_rng(S).integers(1, 2500 if pattern == "one" else 9000, size=S)]
     x = rows(rate, lengths, S)
     gains = np.linspace(-6, 24, S).astype(np.float32)
-    got, red = run_stream(eng, x, lengths, gains, 700, rate, S, pattern)
-    ref, rref = eng.limit(x, -1.0, rate, gain_db=gains, lookahead_ms=3.0, release_ms=60.0, lengths=lengths)
-    for s in range(S):
-        assert got[s].shape == (lengths[s],) and np.array_equal(got[s], ref[s, :lengths[s]]), s
-    assert np.array_equal(red, rref)
+    rng = np.random.default_rng(7)
+    stage = ss.stage(eng, "limiter", S, 700, rate, ceiling=-1.0, lookahead_ms=3.0, release_ms=60.0)
+    ss.run(stage, [[ss.pattern(pattern, n, 700, rng)] for n in lengths], lambda s, u, n: x[s, :n],
+           [[float(g)] for g in gains], host=True)
 
 
 def test_stream_schedule_and_launch_counts(eng):

@@ -28,6 +28,7 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import slot_streams as ss
 from oracle import bed_oracle as bo
 from oracle import loudness_oracle as lo
 from oracle import pitch_oracle as po
@@ -41,7 +42,7 @@ from test_resample_cpu import TOL as RS_TOL
 from test_time_stretch_cpu import TOL as TS_TOL
 from test_watermark_cpu import KEY, TOL_EMBED, embed_scale, speech
 from viettts_b200 import config
-from viettts_b200.engine import STREAM_BEGIN, STREAM_END, reverb_stream_emitted
+from viettts_b200.engine import STREAM_BEGIN, STREAM_END
 
 pytestmark = pytest.mark.gpu
 SR = config.SAMPLE_RATE
@@ -70,37 +71,6 @@ def probe_chunks():
     return CHUNKS + out
 
 
-def hop_emitted(P, end):
-    return P if end else min(P, 256 * max(0, P // 256 - 3))
-
-
-def rs_emitted(up, down):
-    half = 10 * max(up, down)
-
-    def f(P, end):
-        total = -(-P * up // down)
-        return total if end else min(total, max(0, (P * up - 1 - half) // down + 1))
-    return f
-
-
-class Stage:
-    """one sample stream: how to open and push it, its counting formula E(P, end) (outputs after P inputs), its
-    period and its BEGIN value"""
-
-    def __init__(self, name, open_, emitted, period, value=None, reduction=False, meter=False):
-        self.name, self.open, self.emitted, self.period = name, open_, emitted, period
-        self.value, self.reduction, self.meter = value, reduction, meter
-
-    def push(self, st, x_t, n_new, flags, y_t, red_t):
-        kw = {} if self.value is None else {self.value[0]: self.value[1]}
-        if self.meter:
-            st.push_device(x_t, n_new, flags, y_t)
-            return None
-        if self.reduction:
-            return st.push_device(x_t, n_new, flags, y_t, red_t, **kw)
-        return st.push_device(x_t, n_new, flags, y_t, **kw)
-
-
 def ts_period(tempo):
     """input samples and frames after which the time stretcher's frame centres rint(256 t alpha) repeat exactly"""
     r = Fraction(float(np.float32(tempo))) * 256
@@ -115,31 +85,25 @@ def bed_period(eng):
     return P * 256 // gcd(P, 256)
 
 
-def stages(eng):
-    up, down, _ = ro.ratio(SR, OUT_RATE)
-    tail = eng.prepare_beds(BANK, SR).params[0]["Tt"]
-    la = eng.limiter_stream_lookahead(SR)
-    out = [
-        Stage("resample", lambda e: e.open_resample_stream(2, F, OUT_RATE), rs_emitted(up, down), down),
-        Stage("denoise", lambda e: e.open_denoise_stream(2, F, 0.5, bias=np.full(513, 1e-3, np.float32)), hop_emitted, 256),
-        Stage("pitch", lambda e: e.open_pitch_shift_stream(2, F), hop_emitted, 256, ("semitones", 3.0)),
-    ]
-    for tempo in (1.25, 0.9):
-        out.append(Stage(f"time_stretch_{tempo}", lambda e: e.open_time_stretch_stream(2, F),
-                         lambda P, end, t=tempo: tso.stretch_emitted(P, t, end), ts_period(tempo)[0], ("tempo", tempo)))
-    out += [
-        Stage("limiter", lambda e: e.open_limiter_stream(2, F, SR, -1.0), lambda P, end: P if end else max(0, P - la),
-              1024, ("gain_db", 12.0), reduction=True),
-        Stage("eq", lambda e: e.open_eq_stream(2, F, "telephone", SR), lambda P, end: P, 1024),
-        Stage("compressor", lambda e: e.open_compressor_stream(2, F, "voice", SR), lambda P, end: P, 256, reduction=True),
-        Stage("deesser", lambda e: e.open_deesser_stream(2, F, "voice", SR), lambda P, end: P, 1024, reduction=True),
-        Stage("reverb", lambda e: e.open_reverb_stream(2, F, "room", SR), reverb_stream_emitted, 512),
-        Stage("watermark", lambda e: e.open_watermark_stream(2, F, KEY), hop_emitted, wo.PERIOD),
-        Stage("bed", lambda e: e.open_bed_stream(2, F, BANK, SR), lambda P, end: P + (tail if end else 0),
-              bed_period(eng), ("bed", 0), reduction=True),
-        Stage("loudness", lambda e: e.open_loudness_meter(2, F, SR, max_seconds=1 << 20), None, SR // 10, meter=True),
-    ]
-    return out
+def long_stage(eng, name):
+    """(stage, BEGIN value, period) of stream `name` as the probe runs it: two slots of chunk F from the table"""
+    if name.startswith("time_stretch_"):
+        tempo = float(name.rsplit("_", 1)[1])
+        return ss.stage(eng, "time_stretch", 2, F), tempo, ts_period(tempo)[0]
+    spec, value, period = {
+        "resample": (dict(out_rate=OUT_RATE), None, ro.ratio(SR, OUT_RATE)[1]),
+        "denoise": (dict(strength=0.5, bias=np.full(513, 1e-3, np.float32)), None, 256),
+        "pitch": ({}, 3.0, 256),
+        "limiter": (dict(ceiling=-1.0), 12.0, 1024),
+        "eq": (dict(eq="telephone"), None, 1024),
+        "compressor": (dict(spec="voice"), None, 256),
+        "deesser": (dict(spec="voice"), None, 1024),
+        "reverb": (dict(spec="room"), None, 512),
+        "watermark": (dict(spec=KEY), None, wo.PERIOD),
+        "bed": (dict(bed=BANK), 0, None),
+        "loudness": (dict(max_seconds=1 << 20), None, SR // 10),
+    }[name]
+    return ss.stage(eng, name, 2, F, **spec), value, bed_period(eng) if name == "bed" else period
 
 
 def plan(mark):
@@ -153,12 +117,13 @@ def plan(mark):
     return p
 
 
-def run(eng, stage, marks):
-    """runs both slots of one stream to their marks and through the probe; per slot: the probe pushes' outputs (a list
-    of arrays), the last reduction (or meter reading) and the wall time"""
+def run(eng, stage, value, marks):
+    """runs both slots of one stream, BEGIN value `value`, to their marks and through the probe; per slot: the probe
+    pushes' outputs (a list of arrays), the last reduction (or meter reading) and the wall time"""
     dev = torch.device("cuda", 0)
     t0 = time.perf_counter()
-    st = stage.open(eng)
+    st = stage.open()
+    kw = stage.begin([value] * 2)[0]
     S = 2
     width = 4 if stage.meter else st.out_pitch
     x_t = torch.zeros((S, F), dtype=torch.float32, device=dev)
@@ -180,14 +145,14 @@ def run(eng, stage, marks):
                     x_t[s, :n].copy_(probe_t[off:off + n])
                 n_new[s] = n
                 flags[s] = (STREAM_BEGIN if i == 0 else 0) | (STREAM_END if end else 0)
-            n_out = stage.push(st, x_t, n_new, flags, y_t, red_t)
+            n_out = stage.push_device(st, x_t, n_new, flags, y_t, red_t, kw)
             for s in range(S):
                 if i >= len(plans[s]):
                     continue
                 n, off, end = plans[s][i]
                 P0, P[s] = P[s], P[s] + n
                 if n_out is not None:
-                    want = stage.emitted(P[s], end) - (0 if i == 0 else stage.emitted(P0, False))
+                    want = stage.emitted(P[s], end, value) - (0 if i == 0 else stage.emitted(P0, False, value))
                     assert int(n_out[s]) == want, (stage.name, marks[s], i, P[s], int(n_out[s]), want)
                 if off is not None:
                     if n_out is not None:
@@ -266,7 +231,7 @@ def oracle_stretch(eng, stage, mark, y):
     M = tso.stretch_length(w.size, tempo)
     dec = eng.debug_time_stretch_decisions(torch.from_numpy(w[None]).cuda(), tempo)[0, :M // 256 + 1]
     ref = tso.time_stretch(w, tempo, decisions=dec)
-    u0 = stage.emitted(mark, False) - s0 * q * 256 // p
+    u0 = stage.emitted(mark, False, tempo) - s0 * q * 256 // p
     assert u0 + y.size == M, (u0, y.size, M)
     return rel(y, ref[u0:], tso.stretch_error_scale(w, tempo)[u0:]), TS_TOL
 
@@ -312,11 +277,11 @@ STAGE_NAMES = ["resample", "denoise", "pitch", "time_stretch_1.25", "time_stretc
 @pytest.mark.parametrize("session", [0, 1], ids=["2^24,2^31-", "2^31+,2^32+"])
 @pytest.mark.parametrize("name", STAGE_NAMES)
 def test_probe_deep_in_a_slot(eng, name, session):
-    stage = {s.name: s for s in stages(eng)}[name]
+    stage, value, period = long_stage(eng, name)
     marks = SESSIONS[session]
-    outs, last, secs = run(eng, stage, marks)
-    ref_marks = [short(m, stage.period) for m in marks]
-    routs, rlast, _ = run(eng, stage, ref_marks)
+    outs, last, secs = run(eng, stage, value, marks)
+    ref_marks = [short(m, period) for m in marks]
+    routs, rlast, _ = run(eng, stage, value, ref_marks)
     for s, mark in enumerate(marks):
         what = (name, mark, ref_marks[s])
         if stage.meter:

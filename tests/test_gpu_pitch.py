@@ -13,12 +13,12 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import slot_streams as ss
 from oracle import denoise_oracle as do
 from oracle import pitch_oracle as po
 from test_denoise_cpu import signal_of
 from test_pitch_cpu import DEC_MARGIN, TOL, decision_margins, voiced_of
 from viettts_b200 import config, synthetic
-from viettts_b200.engine import STREAM_BEGIN, STREAM_END
 
 pytestmark = pytest.mark.gpu
 KEY = np.array([7, 1234567], np.uint32)
@@ -125,100 +125,28 @@ def test_zero_shift_is_the_input(eng):
 
 # ---- stream ------------------------------------------------------------------------------------------------------
 
-def push_plans(kind, F, rng):
-    """utterances of one slot, each a list of push sizes (END with the last one)"""
-    if kind == "ones":
-        return [[1] * int(rng.integers(1100, 1500))]
-    if kind in (255, 256, 1000):
-        return [[min(kind, F)] * int(rng.integers(4, 12))]
-    if kind == "max":
-        return [[F] * int(rng.integers(2, 5)) + [int(rng.integers(1, F))]]
-    if kind == "end_empty":
-        return [[int(v) for v in rng.integers(1, F + 1, size=4)] + [0]]
-    if kind == "short":
-        return [[int(rng.integers(1, 200)), int(rng.integers(0, 200))], [512], [513]]
-    if kind == "reuse":
-        return [[int(v) for v in rng.integers(1, F + 1, size=3)], [int(v) for v in rng.integers(1, F + 1, size=5)]]
-    if kind == "late":
-        return [[0] * int(rng.integers(2, 6))] + [[int(v) for v in rng.integers(1, F + 1, size=6)]]
-    return []    # idle
-
-
-KINDS = ["ones", 255, 256, 1000, "max", "end_empty", "short", "reuse", "late", "idle"]
 STREAM_SHIFTS = [3.0, -5.0, 0.0, 12.0, -12.0, 7.5, -1.0]
 
 
 def run_stream(eng, S, F, kinds, seed):
-    """each slot runs its plan (a slot's "late" plan starts it some pushes after the others), every utterance with its
-    own shift; the concatenated outputs must equal the one-shot call and each push must issue five launches"""
+    """slot s runs plan kinds[s], every utterance with its own shift, held to the stream's contract on every push
+    (tests/helpers/slot_streams.py); at shift 0 the stream is the input"""
     rng = np.random.default_rng(seed)
-    dev = torch.device("cuda", 0)
-    plans = []
-    for k in kinds:
-        flat = []
-        for u, sizes in enumerate(push_plans(k, F, rng)):
-            if k == "late" and u == 0:
-                flat += [(0, 0, None)] * len(sizes)                     # idle pushes before the slot begins
-                continue
-            for q, n in enumerate(sizes):
-                flat.append((n, (STREAM_BEGIN if q == 0 else 0) | (STREAM_END if q == len(sizes) - 1 else 0), u))
-        plans.append(flat)
-    data = [dict() for _ in range(S)]
-    got = [dict() for _ in range(S)]
-    shift = [dict() for _ in range(S)]
-    P = np.zeros(S, np.int64)
-    E = np.zeros(S, np.int64)
-    with eng.open_pitch_shift_stream(S, F) as ps:
+    plans = [ss.push_plan(k, F, rng) for k in kinds]
+    shifts = [[STREAM_SHIFTS[int(rng.integers(len(STREAM_SHIFTS)))] for _ in p] for p in plans]
+    stage = ss.stage(eng, "pitch", S, F)
+    with stage.open() as ps:
         assert ps.lookahead == do.LOOKAHEAD
-        xt = torch.zeros((S, F), device=dev)
-        yt = torch.empty((S, ps.out_pitch), device=dev)
-        for c in range(max(len(p) for p in plans)):
-            n_new = np.zeros(S, np.int32)
-            flags = np.zeros(S, np.uint8)
-            sem = np.full(S, np.nan, np.float32)                       # read only for the slots that begin
-            x = np.full((S, F), np.nan, np.float32)                    # past n_new: never read
-            for s in range(S):
-                if c >= len(plans[s]) or plans[s][c][2] is None:
-                    continue
-                n, f, u = plans[s][c]
-                n_new[s], flags[s] = n, f
-                chunk = voiced_of(max(n, 1), 1000 * s + 10 * c + u)[:n]
-                x[s, :n] = chunk
-                if f & STREAM_BEGIN:
-                    data[s][u], got[s][u] = [], []
-                    shift[s][u] = sem[s] = STREAM_SHIFTS[int(rng.integers(len(STREAM_SHIFTS)))]
-                    P[s] = E[s] = 0
-                data[s][u].append(chunk)
-            xt.copy_(torch.from_numpy(x))
-            yt.fill_(12345.0)
-            before = eng.launch_count()
-            n_out = ps.push_device(xt, n_new, flags, yt, semitones=sem)
-            assert eng.launch_count() - before == 5
-            y = yt.cpu().numpy()
-            for s in range(S):
-                if n_new[s] == 0 and flags[s] == 0:
-                    assert n_out[s] == 0 and np.all(y[s] == 12345.0), (s, c)     # idle: untouched
-                    continue
-                P[s] += n_new[s]
-                e = int(P[s]) if flags[s] & STREAM_END else po.emitted_closed_form(int(P[s]))
-                assert n_out[s] == e - E[s], (kinds[s], s, c, int(P[s]), int(n_out[s]), e - E[s])
-                E[s] = e
-                got[s][plans[s][c][2]].append(y[s, : n_out[s]].copy())
-    for s in range(S):
-        for u, chunks in data[s].items():
-            xs = np.concatenate(chunks)
-            out = np.concatenate(got[s][u])
-            ref = eng.pitch_shift(xs, shift[s][u])
-            assert out.shape == ref.shape and np.array_equal(out, ref), (kinds[s], s, u, xs.size, shift[s][u])
-            if shift[s][u] == 0:
-                assert np.array_equal(out, xs)
+    for row in ss.run(stage, plans, lambda s, u, n: voiced_of(n, 1000 * s + u), shifts):
+        for x, shift, y, _ in filter(None, row):
+            if shift == 0:
+                assert np.array_equal(y, x)
 
 
 @pytest.mark.parametrize("S", [1, 3, 32])
 def test_stream_equals_one_shot(eng, S):
-    F = 1000
-    kinds = ["max"] if S == 1 else [KINDS[(s + S) % len(KINDS)] for s in range(S)]
-    run_stream(eng, S, F, kinds, seed=S)
+    kinds = ["max"] if S == 1 else [ss.KINDS[(s + S) % len(ss.KINDS)] for s in range(S)]
+    run_stream(eng, S, 1000, kinds, seed=S)
 
 
 def test_stream_one_sample_pushes_and_edges(eng):

@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import slot_streams as ss
 from oracle import reverb_oracle as ro
 from test_reverb_cpu import TOL, cases, error_units
 from viettts_b200 import config, synthetic
@@ -122,66 +123,22 @@ def test_forward_in_place(eng):
     assert np.array_equal(eng.reverb_forward(torch.from_numpy(x).cuda(), ir, rate).cpu().numpy(), eng.reverb(x, ir, rate))
 
 
-def run_stream(eng, x, lengths, spec, chunk, rate, S, pattern, device=False):
-    from viettts_b200.engine import reverb_stream_emitted
-    st = eng.open_reverb_stream(S, chunk, spec, rate)
-    assert st.lookahead == 511 and st.out_pitch == chunk + 511
-    out = [[] for _ in range(S)]
-    pos = [0] * S
-    rng = np.random.default_rng(7)
-    begun = [False] * S
-    x_t = torch.zeros((S, chunk), dtype=torch.float32, device="cuda")
-    y_t = torch.zeros((S, st.out_pitch), dtype=torch.float32, device="cuda")
-    try:
-        while any(pos[s] < lengths[s] or not begun[s] for s in range(S)):
-            n_new = np.zeros(S, np.int32)
-            buf = np.zeros((S, chunk), np.float32)
-            begin = np.zeros(S, bool)
-            end = np.zeros(S, bool)
-            for s in range(S):
-                if begun[s] and pos[s] >= lengths[s]:
-                    continue
-                k = 1 if pattern == "one" else (chunk if pattern == "full" else int(rng.integers(0, chunk + 1)))
-                k = min(k, lengths[s] - pos[s])
-                buf[s, :k] = x[s, pos[s]:pos[s] + k]
-                n_new[s] = k
-                begin[s] = not begun[s]
-                begun[s] = True
-                pos[s] += k
-                end[s] = pos[s] >= lengths[s]
-            if device:
-                x_t.copy_(torch.from_numpy(buf))
-                flags = begin.astype(np.uint8) | (end.astype(np.uint8) << 1)
-                n_out = st.push_device(x_t, n_new, flags, y_t)
-                y = y_t.cpu().numpy()
-                ys = [y[s, :n_out[s]].copy() for s in range(S)]
-            else:
-                ys = st.push(buf, n_new, begin, end)
-            for s, y in enumerate(ys):
-                if n_new[s] or begin[s] or end[s]:
-                    out[s].append(y)
-                    assert sum(v.size for v in out[s]) == reverb_stream_emitted(pos[s], end[s]), (s, pos[s])
-                else:
-                    assert y.size == 0
-    finally:
-        st.close()
-    return [np.concatenate(o) for o in out]
-
-
 @pytest.mark.parametrize("S", [1, 3, 32])
 @pytest.mark.parametrize("pattern,device", [("one", False), ("full", False), ("full", True), ("random", False), ("random", True)])
 def test_stream_equals_one_shot(eng, S, pattern, device):
+    """rows pushed in `pattern` chunks and held to the stream's contract on every push (tests/helpers/slot_streams.py)"""
     rate = 48000
     if pattern == "one" and S == 32:
         pytest.skip("one-sample pushes run at S = 1 and 3")
     lengths = [int(v) for v in np.random.default_rng(S).integers(1, 2500 if pattern == "one" else 30000, size=S)]
     x = rows(rate, lengths, S)
+    rng = np.random.default_rng(7)
     for spec in ("hall", {"ir": user_ir(1500, rate), "mix": 0.7}):
         for chunk in (300, 1500):
-            got = run_stream(eng, x, lengths, spec, chunk, rate, S, pattern, device=device)
-            ref = eng.reverb(x, spec, rate, lengths=lengths)
-            for s in range(S):
-                assert got[s].shape == (lengths[s],) and np.array_equal(got[s], ref[s, :lengths[s]]), (chunk, s)
+            stage = ss.stage(eng, "reverb", S, chunk, rate, spec=spec)
+            with stage.open() as st:
+                assert st.lookahead == 511 and st.out_pitch == chunk + 511
+            ss.run(stage, [[ss.pattern(pattern, n, chunk, rng)] for n in lengths], lambda s, u, n: x[s, :n], host=not device)
             if pattern == "one":
                 break
 

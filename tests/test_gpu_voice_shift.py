@@ -10,15 +10,16 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import slot_streams as ss
 from oracle import denoise_oracle as do
 from oracle import pitch_oracle as po
 from oracle import voice_shift_oracle as vo
 from test_denoise_cpu import signal_of
-from test_gpu_pitch import check_decisions, decisions, push_plans, tts_tokens
+from test_gpu_pitch import check_decisions, decisions, tts_tokens
 from test_pitch_cpu import voiced_of
 from test_voice_shift_cpu import KEEP_MOVE, LEGACY, SIGNALS, SR, TOL_F, expected_steps, f0_of, warp_steps
 from viettts_b200 import synthetic
-from viettts_b200.engine import STREAM_BEGIN, STREAM_END, AudioChain
+from viettts_b200.engine import AudioChain
 
 pytestmark = pytest.mark.gpu
 RAGGED = [0, 1, 512, 513, 1023, 1025, 80128, 30000, 24000]
@@ -139,87 +140,21 @@ STREAM_CASES = [(3.0, 0.0), (-5.0, 4.0), (0.0, -3.0), (12.0, None), (-12.0, 2.0)
 
 
 def run_stream(eng, S, F, kinds, seed, host=False):
-    """each slot runs its plan with its own (s, phi) per utterance (phi None: the slot follows the pitch); the
-    concatenated outputs must equal the one-shot call and each push must issue the pitch stream's five launches"""
+    """slot s runs plan kinds[s] with its own (s, phi) per utterance (phi None: the formants follow the pitch), held to
+    the stream's contract and the pitch stream's five launches on every push (tests/helpers/slot_streams.py); without a
+    formant the stream is the pitch shifter"""
     rng = np.random.default_rng(seed)
-    dev = torch.device("cuda", 0)
-    plans = []
-    for k in kinds:
-        flat = []
-        for u, sizes in enumerate(push_plans(k, F, rng)):
-            if k == "late" and u == 0:
-                flat += [(0, 0, None)] * len(sizes)
-                continue
-            for q, n in enumerate(sizes):
-                flat.append((n, (STREAM_BEGIN if q == 0 else 0) | (STREAM_END if q == len(sizes) - 1 else 0), u))
-        plans.append(flat)
-    data = [dict() for _ in range(S)]
-    got = [dict() for _ in range(S)]
-    case = [dict() for _ in range(S)]
-    with eng.open_voice_shift_stream(S, F) as ps:
-        xt = torch.zeros((S, F), device=dev)
-        yt = torch.empty((S, ps.out_pitch), device=dev)
-        for c in range(max(len(p) for p in plans)):
-            n_new = np.zeros(S, np.int32)
-            flags = np.zeros(S, np.uint8)
-            sem = np.zeros(S, np.float32)
-            fmt = np.full(S, np.nan, np.float32)
-            x = np.full((S, F), np.nan, np.float32)
-            any_fmt = False
-            for s in range(S):
-                if c >= len(plans[s]) or plans[s][c][2] is None:
-                    continue
-                n, f, u = plans[s][c]
-                n_new[s], flags[s] = n, f
-                chunk = voiced_of(max(n, 1), 1000 * s + 10 * c + u)[:n]
-                x[s, :n] = chunk
-                if f & STREAM_BEGIN:
-                    data[s][u], got[s][u] = [], []
-                    case[s][u] = STREAM_CASES[int(rng.integers(len(STREAM_CASES)))]
-                    sem[s] = case[s][u][0]
-                    if case[s][u][1] is not None:
-                        fmt[s] = case[s][u][1]
-                data[s][u].append(chunk)
-                any_fmt |= bool(f & STREAM_BEGIN) and case[s][u][1] is not None
-            if any_fmt:
-                # a push that passes formants gives one to every slot it begins (NaN is rejected with BEGIN): slots
-                # drawn to follow the pitch keep their formants instead
-                for s in np.flatnonzero(flags & STREAM_BEGIN):
-                    u = plans[s][c][2]
-                    if case[s][u][1] is None:
-                        case[s][u] = (case[s][u][0], 0.0)
-                        fmt[s] = 0.0
-            begin = (flags & STREAM_BEGIN) != 0
-            fmt_arg = fmt if any_fmt else None
-            before = eng.launch_count()
-            if host:
-                ys = ps.push(x[:, : max(1, int(n_new.max()))], n_new, begin=begin, end=(flags & STREAM_END) != 0,
-                             semitones=sem, formant=fmt_arg)
-                n_out = [len(v) for v in ys]
-            else:
-                xt.copy_(torch.from_numpy(x))
-                n_out = ps.push_device(xt, n_new, flags, yt, semitones=sem, formant=fmt_arg)
-                y = yt.cpu().numpy()
-                ys = [y[s, : n_out[s]] for s in range(S)]
-            assert eng.launch_count() - before == 5
-            for s in range(S):
-                if n_new[s] or flags[s]:
-                    got[s][plans[s][c][2]].append(ys[s].copy())
-    for s in range(S):
-        for u, chunks in data[s].items():
-            xs = np.concatenate(chunks)
-            out = np.concatenate(got[s][u])
-            sh, phi = case[s][u]
-            ref = eng.pitch_shift(xs, sh, formant=phi)
-            assert out.shape == ref.shape and np.array_equal(out, ref), (kinds[s], s, u, xs.size, sh, phi)
+    plans = [ss.push_plan(k, F, rng) for k in kinds]
+    cases = [[STREAM_CASES[int(rng.integers(len(STREAM_CASES)))] for _ in p] for p in plans]
+    for row in ss.run(ss.stage(eng, "voice_shift", S, F), plans, lambda s, u, n: voiced_of(n, 1000 * s + u), cases, host=host):
+        for x, (sh, phi), y, _ in filter(None, row):
             if phi is None:
-                assert np.array_equal(out, eng.pitch_shift(xs, sh)), (s, u)
+                assert np.array_equal(y, eng.pitch_shift(x, sh))
 
 
 @pytest.mark.parametrize("S", [1, 3, 16])
 def test_stream_equals_one_shot(eng, S):
-    kinds = ["max"] if S == 1 else [["ones", 255, 256, 1000, "max", "end_empty", "short", "reuse", "late", "idle"][(s + S) % 10]
-                                    for s in range(S)]
+    kinds = ["max"] if S == 1 else [ss.KINDS[(s + S) % len(ss.KINDS)] for s in range(S)]
     run_stream(eng, S, 1000, kinds, seed=S)
 
 

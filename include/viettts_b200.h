@@ -851,6 +851,50 @@ int vtts_decode(vtts_ctx* ctx, const void* c_dev, const int32_t* n_dev, int B, i
 /* the same on host buffers; n_in[b] must lie in [0, S] */
 int vtts_decode_host(vtts_ctx* ctx, const void* c, const int32_t* n_in, int B, int S, int encoding, float* y);
 
+/* ---- FLAC: lossless compression of the PCM-16 codes --------------------------------------------------------------
+ * A row of n samples becomes a native FLAC stream (RFC 9639, streamable subset): mono, 16 bits, the PCM-16 codes of
+ * vtts_encode(VTTS_ENC_PCM16), so a decoder gives those codes back exactly.  "fLaC" and one STREAMINFO block (42
+ * bytes: block size, min / max frame size, rate, total samples n, MD5 0 = unknown), then ceil(n / block) frames of fixed
+ * blocking, each the cheapest of CONSTANT, FIXED 0..4, LPC 1..12 (Rice-coded residuals) and VERBATIM by exact bit count.
+ * oracle/flac_oracle.py is the definition: the bytes are the same in every vtts_precision mode.
+ * block: 256, 512, 1024, 2048 or 4096.  rate: any rate a frame header can state (a table rate, kHz <= 255, Hz <= 65535,
+ * tens of Hz <= 655350).  A bad block or rate, B outside [1, 65535], S < 0, a pitch below vtts_flac_bound, a null
+ * buffer or overlapping buffers fail with VTTS_ERR_BAD_ARG before anything is launched.  S = 0 gives every row the
+ * 42-byte header alone. */
+/* bytes per row that no output of a row of S samples exceeds (VERBATIM frames with the longest headers); -1 for a
+ * bad block or S < 0 */
+int64_t vtts_flac_bound(int S, int block);
+/* x_dev float [B,S]; n_dev int32 [B] or NULL (= S; clamped to [0, S]); row b's stream goes to y_dev + b * y_pitch
+ * (y_pitch >= vtts_flac_bound(S, block)) and its byte count to nbytes_dev[b]; nothing past it is written.  A row of
+ * n = 0 gives the 42-byte header only.  Stream-ordered, no host synchronisation: five launches (three when S = 0). */
+int vtts_flac_encode(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, int block, uint8_t* y_dev,
+                     int64_t y_pitch, int32_t* nbytes_dev, void* stream);
+/* the same on host buffers; n_in[b] must lie in [0, S].  One copy of the longest row's byte count from every row
+ * comes back, and each row's nbytes[b] bytes go to y + b * y_pitch. */
+int vtts_flac_encode_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, int block, uint8_t* y,
+                          int64_t y_pitch, int32_t* nbytes);
+/* the 4-bit rate code a frame header gives `rate` (1..14), or -1 for a rate FLAC cannot state */
+int vtts_flac_rate_code(int rate);
+/* Per-slot FLAC stream on the slot protocol of the sample streams (BEGIN / END flags): max_streams 1..65535 slots,
+ * pushes of up to max_chunk_samples (1..2^22) new samples per slot.  A slot carries its P mod block samples that no
+ * frame holds yet.  A push emits per slot: with BEGIN the 42-byte stream header (total samples and min / max frame size
+ * 0, "unknown"), then the frames its samples complete (after P samples since BEGIN, floor(P / block) frames in all),
+ * and with END the short last frame (ceil(P / block) in all).  A slot's bytes, concatenated from BEGIN to END, are the
+ * one-shot stream of its samples with those three STREAMINFO fields 0.  *out_bytes: the bytes of a push's output
+ * buffer.  Frame numbers past 2^31 - 1 are refused. */
+typedef struct vtts_flac_stream vtts_flac_stream;
+int vtts_flac_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int rate, int block, vtts_flac_stream** out,
+                            int64_t* out_bytes);
+int vtts_flac_stream_destroy(vtts_ctx* ctx, vtts_flac_stream* fs);
+/* x_dev float [S][max_chunk_samples]; n_new, flags host [S]; y_dev uint8 [out_bytes]: every slot's bytes packed one after
+ * another from y_dev; tbl_dev int32 [S][2]: each slot's (offset, count) in y_dev.  Stream-ordered, no host
+ * synchronisation; buffers must not overlap. */
+int vtts_flac_stream_push(vtts_ctx* ctx, vtts_flac_stream* fs, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
+                          uint8_t* y_dev, int32_t* tbl_dev, void* stream);
+/* the same on host buffers: the table comes back first, then only the bytes the slots produced */
+int vtts_flac_stream_push_host(vtts_ctx* ctx, vtts_flac_stream* fs, const float* x, const int32_t* n_new, const uint8_t* flags,
+                               uint8_t* y, int32_t* tbl);
+
 /* ---- streaming acoustic model: every slot advances its decoder a few frames per push ---------------------------
  * A vtts_acoustic_stream holds max_streams (1..128) independent slots.  begin starts utterances in closed slots; each
  * push advances every open slot by min(F, frames left) decoder steps in ONE scan launch and returns the mel frames whose

@@ -209,6 +209,16 @@ SIGNATURES = {
     "vtts_encode_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "vtts_decode": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "vtts_decode_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "vtts_flac_bound": (C.c_int64, [C.c_int, C.c_int]),
+    "vtts_flac_encode": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64,
+                                   C.c_void_p, C.c_void_p]),
+    "vtts_flac_encode_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64,
+                                        C.c_void_p]),
+    "vtts_flac_rate_code": (C.c_int, [C.c_int]),
+    "vtts_flac_stream_create": (C.c_int, [c_ctx, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]),
+    "vtts_flac_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
+    "vtts_flac_stream_push": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtts_flac_stream_push_host": (C.c_int, [c_ctx, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtts_acoustic_stream_create":(C.c_int, [c_ctx, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, C.POINTER(C.c_void_p)]),
     "vtts_acoustic_stream_destroy": (C.c_int, [c_ctx, C.c_void_p]),
     "vtts_acoustic_stream_lookahead": (C.c_int, []),

@@ -12,6 +12,7 @@
 // addresses reach that alignment at different samples (a caller's offset view) runs every group element by element.
 #include <type_traits>
 
+#include "pcm16.cuh"
 #include "stream_common.cuh"
 
 namespace {
@@ -33,8 +34,7 @@ __device__ __forceinline__ int bit_length(int p) { return 32 - __clz(p); }
 
 template <int E>
 __device__ __forceinline__ Code<E> encode_one(float x) {
-  // cvt.rni.s32.f64 rounds half to even and saturates +-Inf; NaN is mapped to 0 by the definition
-  const int v = x != x ? 0 : min(max(__double2int_rn((double)x * 32767.0), -32768), 32767);
+  const int v = VTTS_PCM16_OF(x);
   if (E == VTTS_ENC_PCM16) return (Code<E>)v;
   if (E == VTTS_ENC_ULAW) {
     int p = v >> 2, mask = 0xFF;

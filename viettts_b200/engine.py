@@ -470,8 +470,51 @@ ENCODING_DTYPES = {"pcm16": np.int16, "ulaw": np.uint8, "alaw": np.uint8}
 def encoding_name(encoding) -> str:
     """the name of a wire encoding ('pcm16', 'ulaw' or 'alaw'; anything else raises ValueError)"""
     if encoding not in ENCODINGS:
+        if isinstance(encoding, str) and encoding.split(",")[0] == "flac":
+            raise ValueError(f"encoding {encoding!r}: FLAC codes frames, not samples; use Engine.encode_flac")
         raise ValueError(f"encoding {encoding!r} must be one of {', '.join(ENCODINGS)}")
     return encoding
+
+
+FLAC_BLOCKS = (256, 512, 1024, 2048, 4096)
+FLAC_HEADER_BYTES = 42
+
+
+def flac_rate(rate) -> int:
+    """`rate` if a FLAC frame header can state it (vtts_flac_rate_code: a table rate, kHz <= 255, Hz <= 65535, tens of Hz
+    <= 655350)"""
+    r = int(rate)
+    if r != rate or not 0 < r < 2**31 or _lib.load().vtts_flac_rate_code(r) < 0:
+        raise ValueError(f"flac: rate {rate} has no frame-header code (kHz <= 255, Hz <= 65535 or tens of Hz <= 655350)")
+    return r
+
+
+def flac_block(block) -> int:
+    if block not in FLAC_BLOCKS:
+        raise ValueError(f"flac: block {block} must be one of {', '.join(map(str, FLAC_BLOCKS))}")
+    return int(block)
+
+
+def flac_params(spec) -> dict:
+    """{'block': N} of a FLAC spec: 'flac' (block 4096) or 'flac,block=N' with N in FLAC_BLOCKS (ValueError otherwise)"""
+    parts = str(spec).split(",") if isinstance(spec, str) else [None]
+    if parts[0] != "flac":
+        raise ValueError(f"flac spec {spec!r} must be 'flac' or 'flac,block=N'")
+    out = {"block": 4096}
+    for kv in parts[1:]:
+        k, eq, v = kv.partition("=")
+        if k.strip() != "block" or not eq:
+            raise ValueError(f"flac spec {spec!r}: unknown setting {kv!r} (block=N)")
+        try:
+            out["block"] = flac_block(int(v))
+        except ValueError:
+            raise ValueError(f"flac spec {spec!r}: block must be one of {', '.join(map(str, FLAC_BLOCKS))}") from None
+    return out
+
+
+def flac_bound(S: int, block: int = 4096) -> int:
+    """bytes per row that no FLAC stream of a row of S samples exceeds (vtts_flac_bound)"""
+    return int(_lib.load().vtts_flac_bound(int(S), flac_block(block)))
 
 
 class WatermarkDetection(NamedTuple):
@@ -874,6 +917,8 @@ class Engine:
         `encoding`: 'pcm16', 'ulaw' or 'alaw'; after the meter the last stage's buffer is encoded on the device
         (`encode_forward` over the whole buffer) and `step()` copies and returns those codes (2 or 1 bytes per sample
         instead of 4), equal to `encode` of the float audio bit for bit.
+        'flac' or 'flac,block=N': a per-slot FLAC stream (FlacStream) runs after the meter, and `step()` copies the
+        per-slot (offset, count) table and then only the packed bytes, returning {slot: bytes}.
         `meter=True`: a loudness meter runs last, on what `step()` returns at the output rate (a
         multiple of 10), and `TtsStream.meter()` gives each stepped slot's readings, read back in the step's one
         synchronisation.  Needs the 'bf16x3' or 'fp16' mode (the vocoder stream has no strict fp32 path)."""
@@ -1956,6 +2001,49 @@ class Engine:
         return out
 
 
+    # ---- FLAC (vtts_flac_encode: lossless frames of the PCM-16 codes, oracle/flac_oracle.py byte for byte) ----
+    def encode_flac(self, wav, rate=config.SAMPLE_RATE, lengths=None, block=4096):
+        """Native FLAC streams (mono, 16 bits, streamable subset) of host audio wav f32 [S] or [B,S] at `rate`: bytes
+        for [S], a list of bytes per row for [B,S].  The samples are the PCM-16 codes of `encode(wav, 'pcm16')`, so a
+        decoder gives those back exactly.  lengths int [B] in [0, S]: row b holds its first lengths[b] samples."""
+        rate, block = flac_rate(rate), flac_block(block)
+        x, lens, one = _wav_rows(wav, lengths)
+        B, S = x.shape
+        out = []
+        if B:
+            pitch = flac_bound(S, block)
+            y = np.empty((B, pitch), np.uint8)
+            nb = np.zeros(B, np.int32)
+            self._ck(self.lib.vtts_flac_encode_host(self.h, _ptr(x) if S else None, _ptr(lens), B, S, rate, block, _ptr(y),
+                                                    pitch, _ptr(nb)))
+            out = [y[b, : nb[b]].tobytes() for b in range(B)]
+        return out[0] if one else out
+
+    def open_flac_stream(self, max_streams: int, max_chunk_samples: int, rate=config.SAMPLE_RATE, block=4096) -> "FlacStream":
+        """Per-slot FLAC streams (FlacStream): push samples as they arrive, get each slot's finished frames."""
+        return FlacStream(self, max_streams, max_chunk_samples, rate, block)
+
+    def encode_flac_forward(self, x_t, rate=config.SAMPLE_RATE, lengths_t=None, block=4096, out=None, stream=None):
+        """vtts_flac_encode on torch CUDA tensors, stream-ordered: x_t f32 [B,S] -> (uint8 [B, flac_bound(S, block)],
+        int32 nbytes [B]): row b's stream is out[b, :nbytes[b]], and nothing past it is written.  `out`: a contiguous
+        uint8 CUDA tensor [B, >= the bound] (its row stride is the pitch) or None."""
+        import torch
+        rate, block = flac_rate(rate), flac_block(block)
+        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous() and x_t.dim() == 2
+        B, S = x_t.shape
+        bound = flac_bound(S, block)
+        if out is None:
+            out = torch.empty((B, bound), dtype=torch.uint8, device=x_t.device)
+        elif not (out.is_cuda and out.dtype == torch.uint8 and out.dim() == 2 and out.shape[0] == B and out.shape[1] >= bound
+                  and out.is_contiguous()):
+            raise ValueError(f"out must be a contiguous uint8 CUDA tensor [{B}, >= {bound}]")
+        nbytes = torch.empty(B, dtype=torch.int32, device=x_t.device)
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self._ck(self.lib.vtts_flac_encode(self.h, _ptr(x_t), _ptr(lengths_t), B, S, rate, block, _ptr(out), out.shape[1],
+                                           _ptr(nbytes), st))
+        return out, nbytes
+
+
 class Loudness(NamedTuple):
     integrated: np.ndarray     # LUFS (gated, BS.1770-4)
     momentary: np.ndarray      # LUFS, the last 400 ms block
@@ -2456,6 +2544,53 @@ class WatermarkStream(_SlotStream):
         self.lookahead = int(eng.lib.vtts_watermark_stream_lookahead())
 
 
+def flac_stream_frames(p: int, block: int, end: bool = False) -> int:
+    """frames a FLAC stream slot has emitted after p samples since BEGIN: floor(p / block), ceil(p / block) once END"""
+    return -(-int(p) // block) if end else int(p) // block
+
+
+class FlacStream(_SlotStream):
+    """Handle of a per-slot FLAC stream (Engine.open_flac_stream).  A slot's bytes from BEGIN to END are
+    `Engine.encode_flac` of its samples with STREAMINFO's total samples and min / max frame size 0 ("unknown"): the
+    stream header with BEGIN, then each frame once its block of samples has arrived, and the short last frame with END
+    (flac_stream_frames).  `push` returns one `bytes` per slot; `push_device` writes every slot's bytes packed into out_t
+    (uint8 [out_bytes]) and their (offset, count) into tbl_t (int32 [S, 2])."""
+    _kind = "flac_stream"
+
+    def __init__(self, eng: Engine, max_streams: int, max_chunk_samples: int, rate=config.SAMPLE_RATE, block=4096):
+        super().__init__(eng, max_streams, max_chunk_samples)
+        self.max_chunk_samples = self._chunk
+        self.rate, self.block = flac_rate(rate), flac_block(block)
+        h, nb = C.c_void_p(), C.c_int64()
+        eng._ck(eng.lib.vtts_flac_stream_create(eng.h, self.max_streams, self._chunk, self.rate, self.block, C.byref(h),
+                                                C.byref(nb)))
+        self.h, self.out_bytes = h, int(nb.value)
+
+    def push(self, x, n_new, begin=None, end=None) -> list:
+        """x f32 [S, <= max_chunk_samples], n_new int [S], begin / end bool [S] or None; one `bytes` per slot"""
+        x, n, f = self._host_in(x, n_new, begin, end)
+        y = np.empty(self.out_bytes, np.uint8)
+        tbl = np.zeros((self.max_streams, 2), np.int32)
+        self.eng._ck(self.eng.lib.vtts_flac_stream_push_host(self.eng.h, self.h, _ptr(x), _ptr(n), _ptr(f), _ptr(y), _ptr(tbl)))
+        return [y[o:o + c].tobytes() for o, c in tbl]
+
+    def push_device(self, x_t, n_new, flags, out_t, tbl_t, stream=None):
+        """x_t f32 CUDA [S, max_chunk_samples], out_t uint8 CUDA [out_bytes], tbl_t int32 CUDA [S, 2]; n_new and flags
+        on the host.  Stream-ordered."""
+        import torch
+        S, F = self.max_streams, self._chunk
+        if tuple(x_t.shape) != (S, F) or x_t.dtype != torch.float32 or not x_t.is_contiguous():
+            raise ValueError(f"x_t must be contiguous float32 [{S}, {F}]")
+        if tuple(out_t.shape) != (self.out_bytes,) or out_t.dtype != torch.uint8:
+            raise ValueError(f"out_t must be uint8 [{self.out_bytes}]")
+        if tuple(tbl_t.shape) != (S, 2) or tbl_t.dtype != torch.int32 or not tbl_t.is_contiguous():
+            raise ValueError(f"tbl_t must be contiguous int32 [{S}, 2]")
+        n, f = self._args(n_new, flags)
+        st = torch.cuda.current_stream(x_t.device).cuda_stream if stream is None else stream
+        self.eng._ck(self.eng.lib.vtts_flac_stream_push(self.eng.h, self.h, _ptr(x_t), _ptr(n), _ptr(f), _ptr(out_t), _ptr(tbl_t),
+                                                        st))
+
+
 def reverb_stream_emitted(p: int, end: bool = False) -> int:
     """outputs a reverb stream slot has emitted after receiving p samples: 512 floor(p / 512), or p once END is pushed"""
     return int(p) if end else 512 * (int(p) // 512)
@@ -2573,6 +2708,7 @@ class AudioChain:
     the program loudness and stays under the true-peak ceiling; its tail makes each row `tail` samples longer.  The
     watermark is the last 16 kHz stage, after everything that moves time or pitch.  `encoding` ('pcm16', 'ulaw' or 'alaw') turns the float audio into the codes of that wire format
     last, after the meter; it has no state, so it is not a stream stage (TtsStream encodes its last buffer itself).
+    'flac' or 'flac,block=N' makes `run` return a FLAC stream of the PCM-16 codes (Engine.encode_flac at the output rate).
     `run` applies the chain to one waveform with the one-shot host calls; `streams` opens it as stream stages.  `loudness` (a target in LUFS, reached under `true_peak`, or under the limiter's ceiling with `limit`) has no
     streaming form, and `meter` only measures, so `run` leaves the audio as it is for it.  Raises OptionError (a
     ValueError naming the option) for an option out of range."""
@@ -2610,7 +2746,13 @@ class AudioChain:
         if meter or loudness is not None:
             checked("meter" if loudness is None else "loudness", _loudness_rate, self.rate)
         self.meter = bool(meter)
-        self.encoding = None if encoding is None else checked("encoding", encoding_name, encoding)
+        self.encoding = self.flac = None
+        if isinstance(encoding, str) and encoding.split(",")[0] == "flac":
+            self.flac = checked("encoding", flac_params, encoding)
+            checked("encoding", flac_rate, self.rate)
+            self.encoding = "flac"
+        elif encoding is not None:
+            self.encoding = checked("encoding", encoding_name, encoding)
 
     def _stages(self):
         """(TtsStream attribute, one-shot call or None, stream factory or None) of each stage that is on, in order"""
@@ -2648,10 +2790,12 @@ class AudioChain:
 
     def run(self, eng: Engine, wav) -> np.ndarray:
         """the one-shot host calls of every stage on `wav` ([S] or [B,S] at 16 kHz), in order, then `Engine.encode`
-        with `encoding` (float32 audio without one)"""
+        with `encoding` (float32 audio without one; FLAC stream bytes, or a list of them for [B,S], with 'flac')"""
         for _, call, _ in self._stages():
             if call is not None:
                 wav = call(eng, wav)
+        if self.flac is not None:
+            return eng.encode_flac(wav, self.rate, block=self.flac["block"])
         return wav if self.encoding is None else eng.encode(wav, self.encoding)
 
     def streams(self, eng: Engine, max_streams: int, pitch: int, max_frames: int):
@@ -2721,8 +2865,18 @@ class TtsStream:
         self._mout_h = None if self.mt is None else torch.zeros((S, 4), dtype=torch.float32).pin_memory()
         # the codes of the last audio buffer (the meter's input), the one buffer `step` copies to the host when encoding
         last = ([b for st, b, _ in self._stages if st is not self.mt] or [self._wav])[-1]
-        self._codes = None if self._chain.encoding is None else _code_tensor(None, tuple(last.shape), self._chain.encoding, dev)
-        self._empty_out = np.zeros(0, np.float32 if self._codes is None else ENCODING_DTYPES[self._chain.encoding])
+        self._codes = self._flac = None
+        if self._chain.flac is not None:
+            # FLAC is a stateful last stage: a slot's frames leave as its blocks complete
+            self._flac = FlacStream(eng, S, last.shape[1], self._chain.rate, self._chain.flac["block"])
+            self._built.append(self._flac)
+            self._flac_out = torch.zeros(self._flac.out_bytes, dtype=torch.uint8, device=dev)
+            self._flac_tbl = torch.zeros((S, 2), dtype=torch.int32, device=dev)
+            self._empty_out = b""
+        elif self._chain.encoding is not None:
+            self._codes = _code_tensor(None, tuple(last.shape), self._chain.encoding, dev)
+        if self._flac is None:
+            self._empty_out = np.zeros(0, np.float32 if self._codes is None else ENCODING_DTYPES[self._chain.encoding])
         self._meter = {}
         self._fresh = np.zeros(max_streams, bool)   # begun, no acoustic push yet: the next vocoder push carries BEGIN
         self._empty = set()                         # begun with nothing left after the trim: reported empty at the next step
@@ -2849,7 +3003,8 @@ class TtsStream:
         """One acoustic push into a device buffer, then one vocoder push of the frames it emitted (BEGIN on a slot's
         first push, END on its last sentence's last one); one synchronisation.  Returns {slot: float32 samples} for every
         slot that was running (possibly empty), or {slot: codes} (int16 or uint8, `Engine.encode` of those samples) when
-        the stream was opened with `encoding`; a slot whose utterance finished this step is free afterwards.
+        the stream was opened with `encoding`, or {slot: bytes} with 'flac' (the FLAC stream of the slot's samples, the
+        stream header with its first step and each frame once its block is complete, the short last frame at its end); a slot whose utterance finished this step is free afterwards.
         A slot waiting for its next sentence gets an empty array, and its vocoder and stages get no frames and no flags:
         each keeps its lookahead (the vocoder's 13 frames, a stage's held samples) until the next sentence or `finish`.
         That held audio is the cost of a seamless join."""
@@ -2865,7 +3020,7 @@ class TtsStream:
         flags = (self._fresh & active).astype(np.uint8) * STREAM_BEGIN | end.astype(np.uint8) * STREAM_END
         pushed = active | end
         self._live &= ~end
-        out = {s: self._empty_out.copy() for s in sorted(self._empty | set(np.flatnonzero(live).tolist()))}
+        out = {s: (self._empty_out.copy() if self._flac is None else b"") for s in sorted(self._empty | set(np.flatnonzero(live).tolist()))}
         self._empty = set()
         if pushed.any():
             n_wav = self.voc.push_device(self._mel, n_out, flags, self._wav)
@@ -2877,11 +3032,20 @@ class TtsStream:
                     self._mout_h.copy_(buf, non_blocking=True)   # ready once the blocking copy below returns
                 else:
                     n_wav, src = r, buf
-            if self._codes is not None:
-                src = self.eng.encode_forward(src, self._chain.encoding, out=self._codes)
-            wav = src.cpu().numpy()
-            for s in np.flatnonzero(pushed):
-                out[int(s)] = wav[s, : int(n_wav[s])].copy()
+            if self._flac is not None:
+                self._flac.push_device(src, n_wav, flags, self._flac_out, self._flac_tbl)
+                tbl = self._flac_tbl.cpu().numpy()        # the per-slot (offset, count), then only the bytes produced
+                total = int(tbl[:, 1].sum())
+                data = self._flac_out[:total].cpu().numpy().tobytes() if total else b""
+                for s in np.flatnonzero(pushed):
+                    o, c = tbl[s]
+                    out[int(s)] = data[o:o + c]
+            else:
+                if self._codes is not None:
+                    src = self.eng.encode_forward(src, self._chain.encoding, out=self._codes)
+                wav = src.cpu().numpy()
+                for s in np.flatnonzero(pushed):
+                    out[int(s)] = wav[s, : int(n_wav[s])].copy()
             if self.mt is not None:
                 m = self._mout_h.numpy()
                 self._meter = {int(s): tuple(float(v) for v in m[s]) for s in np.flatnonzero(pushed)}

@@ -276,7 +276,7 @@ int vtts_resample_filter(int in_rate, int out_rate, double* taps, int capacity);
  * past ceil(n_in[b] * up / down) are 0.  Stream-ordered. */
 int vtts_resample(vtts_ctx* ctx, const float* x_dev, const int32_t* n_in_dev, int B, int S_in, int in_rate, int out_rate,
                   float* y_dev, void* stream);
-/* the same on host buffers */
+/* the same on host buffers; n_in[b] must lie in [0, S_in] */
 int vtts_resample_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S_in, int in_rate, int out_rate, float* y);
 /* Streaming resampler with max_streams independent slots: each slot carries its filter history (at most
  * 2 * half / up + 1 input samples and a 64-bit position) across pushes, so the outputs a slot emits, concatenated, are

@@ -87,12 +87,9 @@ int vtts_acoustic_stream_lookahead(void) { return D_A; }
 int vtts_acoustic_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_frames, int max_frames, int max_tokens, int dropout_mode,
                                 uint64_t seed, vtts_acoustic_stream** out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic_stream_create: null output pointer");
-  *out = nullptr;
+  int rc = create_check(ctx, "acoustic_stream_create", out, true, max_streams, max_chunk_frames, 4096, "max_chunk_frames", MAX_SLOTS);
+  if (rc) return rc;
   if (!ctx->ac.loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "acoustic_stream_create: acoustic weights not loaded");
-  if (max_streams < 1 || max_streams > MAX_SLOTS || max_chunk_frames < 1 || max_chunk_frames > 4096)
-    return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic_stream_create: max_streams=%d max_chunk_frames=%d (1..%d, 1..4096)", max_streams,
-                     max_chunk_frames, MAX_SLOTS);
   if (max_frames < 1 || max_frames > (1 << 24) || max_tokens < 1 || max_tokens > vtts_acoustic_max_tokens())
     return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic_stream_create: max_frames=%d max_tokens=%d (1..%d, 1..%d)", max_frames, max_tokens, 1 << 24,
                      vtts_acoustic_max_tokens());
@@ -143,7 +140,7 @@ int vtts_acoustic_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_fr
   carve(ar);
   if (dropout_mode == VTTS_DROPOUT_REFERENCE) {
     // frame t, prenet layer l of every slot draws with sub-key 2t + l of the checkpoint key's chain
-    int rc = vtts_ref_subkeys(ctx, seed, 2 * max_frames, as->subkeys, nullptr);
+    rc = vtts_ref_subkeys(ctx, seed, 2 * max_frames, as->subkeys, nullptr);
     if (rc == VTTS_OK && cudaDeviceSynchronize() != cudaSuccess) rc = ctx->fail(VTTS_ERR_CUDA, "acoustic_stream_create: sub-key chain failed");
     if (rc) {
       cudaFree(as->mem);
@@ -309,16 +306,16 @@ int vtts_acoustic_stream_push_host(vtts_ctx* ctx, vtts_acoustic_stream* as, floa
   if (!ctx) return VTTS_ERR_BAD_ARG;
   if (!as || as->ctx != ctx) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic_stream_push_host: the stream belongs to another context");
   if (!mel || !n_out) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic_stream_push_host: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
   const size_t row_b = (size_t)(as->F + D_A) * vc::MEL * sizeof(float);
   HostStage hs(ctx);
   const size_t o_mel = hs.out((size_t)as->S * row_b);
-  int rc = hs.upload();
-  if (!rc) rc = vtts_acoustic_stream_push(ctx, as, hs.dev<float>(o_mel), n_out, hs.st);
-  // only the rows that received frames are copied back
-  for (int s = 0; s < as->S && !rc; ++s)
-    if (n_out[s]) rc = hs.fetch(o_mel + s * row_b, (char*)mel + s * row_b, (size_t)n_out[s] * vc::MEL * sizeof(float));
-  return rc ? rc : hs.finish();
+  return hs.run([&](cudaStream_t st) {
+    int rc = vtts_acoustic_stream_push(ctx, as, hs.dev<float>(o_mel), n_out, st);
+    // only the rows that received frames are copied back
+    for (int s = 0; s < as->S && !rc; ++s)
+      if (n_out[s]) rc = hs.fetch(o_mel + s * row_b, (char*)mel + s * row_b, (size_t)n_out[s] * vc::MEL * sizeof(float));
+    return rc;
+  });
 }
 
 }  // extern "C"

@@ -169,6 +169,34 @@ void bd_carve(Arena& a, int B, int W, BdBufs* d) {
   cpk::cp_carve(a, B, cpk::cp_blocks_max(W), &d->w);
 }
 
+// the parameters, batch shape and bed indices of a one-shot call of entry point `who`
+int bd_args(vtts_ctx* ctx, const char* who, int B, int S, int rate, const float* bank_dev, const long long* offsets, const int32_t* lengths,
+            int K, const int32_t* bed, float duck_db, float threshold_db, float attack_ms, float release_ms, int fade_in, int tail, int xfade,
+            long long offset, BdParams* d) {
+  int rc = bd_params(ctx, who, rate, bank_dev, offsets, lengths, K, duck_db, threshold_db, attack_ms, release_ms, fade_in, tail, xfade, offset, d);
+  if (!rc) rc = batch_check(ctx, who, B, S, cpk::S_MAX);
+  if (!rc && (long long)S + tail > cpk::S_MAX) rc = ctx->fail(VTTS_ERR_BAD_ARG, "%s: S + tail = %lld (at most 2^30)", who, (long long)S + tail);
+  return rc ? rc : bd_bed_check(ctx, who, bed, B, K);
+}
+
+int bd_launch(vtts_ctx* ctx, const BdParams& d, const float* x, const int32_t* n_in, int B, int S, const float* bank_dev, const long long* offsets,
+              const int32_t* lengths, const int32_t* bed, float* y, float* reduction_db, cudaStream_t st) {
+  const int W = S + d.Tt;
+  Arena m(nullptr, 0, true);
+  BdBufs w;
+  bd_carve(m, B, W, &w);
+  int rc = ctx->ensure_ws(m.off);
+  if (rc) return rc;
+  Arena a(ctx->ws, SIZE_MAX, false);
+  bd_carve(a, B, W, &w);
+  std::vector<BdRow> rows(B);
+  for (int b = 0; b < B; ++b) rows[b] = bd_row(bed[b], offsets, lengths);
+  VTTS_CUDA(cudaMemcpyAsync(w.rows, rows.data(), (size_t)B * sizeof(BdRow), cudaMemcpyHostToDevice, st));
+  rc = bd_gather(ctx, x, S, S, n_in, d.Tt, w.rows, w.n2, w.key, W, B, st);
+  if (rc) return rc;
+  return cpk::cp_run(ctx, d.p, w.key, W, W, w.n2, nullptr, B, W, W, w.w, y, W, reduction_db, st, bd_rule(d, w.rows, bank_dev));
+}
+
 }  // namespace
 
 int vtts_bed_mix(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, const float* bank_dev,
@@ -177,29 +205,12 @@ int vtts_bed_mix(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B,
                  float* reduction_db_dev, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   BdParams d;
-  int rc = bd_params(ctx, "bed_mix", rate, bank_dev, offsets, lengths, K, duck_db, threshold_db, attack_ms, release_ms, fade_in, tail, xfade,
-                     offset, &d);
-  if (!rc) rc = cpk::cp_check(ctx, "bed_mix", B, S);
-  if (!rc && (long long)S + tail > (1 << 30)) rc = ctx->fail(VTTS_ERR_BAD_ARG, "bed_mix: S + tail = %lld (at most 2^30)", (long long)S + tail);
-  if (!rc) rc = bd_bed_check(ctx, "bed_mix", bed, B, K);
+  const int rc = bd_args(ctx, "bed_mix", B, S, rate, bank_dev, offsets, lengths, K, bed, duck_db, threshold_db, attack_ms, release_ms, fade_in,
+                         tail, xfade, offset, &d);
   if (rc) return rc;
   if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "bed_mix: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  const int W = S + tail;
-  Arena m(nullptr, 0, true);
-  BdBufs w;
-  bd_carve(m, B, W, &w);
-  rc = ctx->ensure_ws(m.off);
-  if (rc) return rc;
-  Arena a(ctx->ws, SIZE_MAX, false);
-  bd_carve(a, B, W, &w);
-  const cudaStream_t st = (cudaStream_t)stream;
-  std::vector<BdRow> rows(B);
-  for (int b = 0; b < B; ++b) rows[b] = bd_row(bed[b], offsets, lengths);
-  VTTS_CUDA(cudaMemcpyAsync(w.rows, rows.data(), (size_t)B * sizeof(BdRow), cudaMemcpyHostToDevice, st));
-  rc = bd_gather(ctx, x_dev, S, S, n_dev, tail, w.rows, w.n2, w.key, W, B, st);
-  if (rc) return rc;
-  return cpk::cp_run(ctx, d.p, w.key, W, W, w.n2, nullptr, B, W, W, w.w, y_dev, W, reduction_db_dev, st, bd_rule(d, w.rows, bank_dev));
+  return bd_launch(ctx, d, x_dev, n_dev, B, S, bank_dev, offsets, lengths, bed, y_dev, reduction_db_dev, (cudaStream_t)stream);
 }
 
 int vtts_bed_mix_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, const float* bank_dev,
@@ -207,25 +218,16 @@ int vtts_bed_mix_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B,
                       float attack_ms, float release_ms, int fade_in, int tail, int xfade, long long offset, float* y, float* reduction_db) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   BdParams d;
-  int rc = bd_params(ctx, "bed_mix_host", rate, bank_dev, offsets, lengths, K, duck_db, threshold_db, attack_ms, release_ms, fade_in, tail,
-                     xfade, offset, &d);
-  if (!rc) rc = cpk::cp_check(ctx, "bed_mix_host", B, S);
-  if (!rc) rc = host_lengths_check(ctx, "bed_mix_host", n_in, B, S);
-  if (!rc) rc = bd_bed_check(ctx, "bed_mix_host", bed, B, K);
+  int rc = bd_args(ctx, "bed_mix_host", B, S, rate, bank_dev, offsets, lengths, K, bed, duck_db, threshold_db, attack_ms, release_ms, fade_in,
+                   tail, xfade, offset, &d);
   if (rc) return rc;
-  if (!x || !y) return ctx->fail(VTTS_ERR_BAD_ARG, "bed_mix_host: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4, y_b = (size_t)B * ((size_t)S + tail) * 4, r_b = (size_t)B * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, r_b), o_r = hs.out(r_b), o_y = hs.out(y_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = vtts_bed_mix(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, rate, bank_dev, offsets, lengths, K,
-                      bed, duck_db, threshold_db, attack_ms, release_ms, fade_in, tail, xfade, offset, hs.dev<float>(o_y), hs.dev<float>(o_r),
-                      hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, y_b);
-  if (!rc && reduction_db) rc = hs.fetch(o_r, reduction_db, r_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("bed_mix_host", x, n_in, B, S, y != nullptr);
+  if (rc) return rc;
+  const size_t o_r = hs.out((size_t)B * 4, reduction_db), o_y = hs.out((size_t)B * ((size_t)S + tail) * 4, y);
+  return hs.run([&](cudaStream_t st) {
+    return bd_launch(ctx, d, hs.x(), hs.n(), B, S, bank_dev, offsets, lengths, bed, hs.dev<float>(o_y), hs.dev<float>(o_r), st);
+  });
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
@@ -246,15 +248,12 @@ int vtts_bed_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples
                            const int32_t* lengths, int K, float duck_db, float threshold_db, float attack_ms, float release_ms, int fade_in,
                            int tail, int xfade, long long offset, vtts_bed_stream** out, int* out_pitch) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out || !out_pitch) return ctx->fail(VTTS_ERR_BAD_ARG, "bed_stream_create: null output pointer");
-  *out = nullptr;
+  int rc = create_check(ctx, "bed_stream_create", out, out_pitch != nullptr, max_streams, max_chunk_samples);
+  if (rc) return rc;
   BdParams d;
-  int rc = bd_params(ctx, "bed_stream_create", rate, bank_dev, offsets, lengths, K, duck_db, threshold_db, attack_ms, release_ms, fade_in,
+  rc = bd_params(ctx, "bed_stream_create", rate, bank_dev, offsets, lengths, K, duck_db, threshold_db, attack_ms, release_ms, fade_in,
                      tail, xfade, offset, &d);
   if (rc) return rc;
-  if (max_streams < 1 || max_streams > 65535 || max_chunk_samples < 1 || max_chunk_samples > (1 << 22))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "bed_stream_create: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", max_streams,
-                     max_chunk_samples, 1 << 22);
   VTTS_CUDA(cudaSetDevice(ctx->device));
   std::unique_ptr<vtts_bed_stream> bs(new vtts_bed_stream(ctx, max_streams, max_chunk_samples, 0));
   bs->d = d;
@@ -341,13 +340,10 @@ int vtts_bed_stream_push_host(vtts_ctx* ctx, vtts_bed_stream* bs, const float* x
   if (!ctx) return VTTS_ERR_BAD_ARG;
   int rc = stream_args(ctx, "bed_stream_push_host", bs, x && y && reduction_db);
   if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)bs->S * bs->F * 4, y_b = (size_t)bs->S * ((size_t)bs->F + bs->d.Tt) * 4, r_b = (size_t)bs->S * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_y = hs.out(y_b), o_r = hs.out(r_b);
-  rc = hs.upload();
-  if (!rc) rc = vtts_bed_stream_push(ctx, bs, hs.dev<const float>(o_x), n_new, flags, bed, hs.dev<float>(o_y), n_out, hs.dev<float>(o_r), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, y_b);
-  if (!rc) rc = hs.fetch(o_r, reduction_db, r_b);
-  return rc ? rc : hs.finish();
+  const size_t o_x = hs.in(x, (size_t)bs->S * bs->F * 4), o_y = hs.out((size_t)bs->S * ((size_t)bs->F + bs->d.Tt) * 4, y),
+               o_r = hs.out((size_t)bs->S * 4, reduction_db);
+  return hs.run([&](cudaStream_t st) {
+    return vtts_bed_stream_push(ctx, bs, hs.dev<const float>(o_x), n_new, flags, bed, hs.dev<float>(o_y), n_out, hs.dev<float>(o_r), st);
+  });
 }

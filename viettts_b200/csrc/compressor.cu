@@ -23,43 +23,48 @@
 
 using namespace cpk;
 
-int vtts_compress(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, float threshold_db, float ratio,
-                  float knee_db, float attack_ms, float release_ms, float makeup_db, float* y_dev, float* reduction_db_dev, void* stream) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  CpParams p;
-  int rc = cp_params(ctx, "compress", rate, threshold_db, ratio, knee_db, attack_ms, release_ms, makeup_db, &p);
-  if (!rc) rc = cp_check(ctx, "compress", B, S);
-  if (rc) return rc;
-  if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "compress: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  rc = ctx->ensure_ws(cp_oneshot_bytes(B, S));
+namespace {
+
+// the parameters and batch shape of a one-shot call of entry point `who`
+int cp_args(vtts_ctx* ctx, const char* who, int B, int S, int rate, float threshold_db, float ratio, float knee_db, float attack_ms,
+            float release_ms, float makeup_db, CpParams* p) {
+  const int rc = cp_params(ctx, who, rate, threshold_db, ratio, knee_db, attack_ms, release_ms, makeup_db, p);
+  return rc ? rc : batch_check(ctx, who, B, S, S_MAX);
+}
+
+int cp_launch(vtts_ctx* ctx, const CpParams& p, const float* x, const int32_t* n_in, int B, int S, float* y, float* reduction_db, cudaStream_t st) {
+  const int rc = ctx->ensure_ws(cp_oneshot_bytes(B, S));
   if (rc) return rc;
   CpBufs w{};
   Arena a(ctx->ws, SIZE_MAX, false);
   cp_carve(a, B, cp_blocks_max(S), &w);
-  return cp_run(ctx, p, x_dev, S, S, n_dev, nullptr, B, S, S, w, y_dev, S, reduction_db_dev, (cudaStream_t)stream);
+  return cp_run(ctx, p, x, S, S, n_in, nullptr, B, S, S, w, y, S, reduction_db, st);
+}
+
+}  // namespace
+
+int vtts_compress(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, float threshold_db, float ratio,
+                  float knee_db, float attack_ms, float release_ms, float makeup_db, float* y_dev, float* reduction_db_dev, void* stream) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  CpParams p;
+  const int rc = cp_args(ctx, "compress", B, S, rate, threshold_db, ratio, knee_db, attack_ms, release_ms, makeup_db, &p);
+  if (rc) return rc;
+  if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "compress: null pointer");
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  return cp_launch(ctx, p, x_dev, n_dev, B, S, y_dev, reduction_db_dev, (cudaStream_t)stream);
 }
 
 int vtts_compress_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float threshold_db, float ratio,
                        float knee_db, float attack_ms, float release_ms, float makeup_db, float* y, float* reduction_db) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   CpParams p;
-  int rc = cp_params(ctx, "compress_host", rate, threshold_db, ratio, knee_db, attack_ms, release_ms, makeup_db, &p);
-  if (!rc) rc = cp_check(ctx, "compress_host", B, S);
-  if (!rc) rc = host_lengths_check(ctx, "compress_host", n_in, B, S);
+  int rc = cp_args(ctx, "compress_host", B, S, rate, threshold_db, ratio, knee_db, attack_ms, release_ms, makeup_db, &p);
   if (rc) return rc;
-  if (!x || !y) return ctx->fail(VTTS_ERR_BAD_ARG, "compress_host: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4, r_b = (size_t)B * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, r_b), o_r = hs.out(r_b), o_y = hs.out(x_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = vtts_compress(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, rate, threshold_db, ratio, knee_db,
-                       attack_ms, release_ms, makeup_db, hs.dev<float>(o_y), hs.dev<float>(o_r), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, x_b);
-  if (!rc && reduction_db) rc = hs.fetch(o_r, reduction_db, r_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("compress_host", x, n_in, B, S, y != nullptr);
+  if (rc) return rc;
+  const size_t o_r = hs.out((size_t)B * 4, reduction_db), o_y = hs.out((size_t)B * S * 4, y);
+  return hs.run([&](cudaStream_t st) { return cp_launch(ctx, p, hs.x(), hs.n(), B, S, hs.dev<float>(o_y), hs.dev<float>(o_r), st); });
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
@@ -74,14 +79,11 @@ struct vtts_compressor_stream : SampleStream<CpRow> {
 int vtts_compressor_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int rate, float threshold_db, float ratio,
                                   float knee_db, float attack_ms, float release_ms, float makeup_db, vtts_compressor_stream** out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out) return ctx->fail(VTTS_ERR_BAD_ARG, "compressor_stream_create: null output pointer");
-  *out = nullptr;
-  CpParams p;
-  int rc = cp_params(ctx, "compressor_stream_create", rate, threshold_db, ratio, knee_db, attack_ms, release_ms, makeup_db, &p);
+  int rc = create_check(ctx, "compressor_stream_create", out, true, max_streams, max_chunk_samples);
   if (rc) return rc;
-  if (max_streams < 1 || max_streams > 65535 || max_chunk_samples < 1 || max_chunk_samples > (1 << 22))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "compressor_stream_create: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", max_streams,
-                     max_chunk_samples, 1 << 22);
+  CpParams p;
+  rc = cp_params(ctx, "compressor_stream_create", rate, threshold_db, ratio, knee_db, attack_ms, release_ms, makeup_db, &p);
+  if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
   std::unique_ptr<vtts_compressor_stream> cs(new vtts_compressor_stream(ctx, max_streams, max_chunk_samples, 0));
   cs->p = p;
@@ -140,15 +142,11 @@ int vtts_compressor_stream_push(vtts_ctx* ctx, vtts_compressor_stream* cs, const
 int vtts_compressor_stream_push_host(vtts_ctx* ctx, vtts_compressor_stream* cs, const float* x, const int32_t* n_new, const uint8_t* flags,
                                      float* y, int32_t* n_out, float* reduction_db) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = stream_args(ctx, "compressor_stream_push_host", cs, x && y && reduction_db);
+  const int rc = stream_args(ctx, "compressor_stream_push_host", cs, x && y && reduction_db);
   if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)cs->S * cs->F * 4, r_b = (size_t)cs->S * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_y = hs.out(x_b), o_r = hs.out(r_b);
-  rc = hs.upload();
-  if (!rc) rc = vtts_compressor_stream_push(ctx, cs, hs.dev<const float>(o_x), n_new, flags, hs.dev<float>(o_y), n_out, hs.dev<float>(o_r), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, x_b);
-  if (!rc) rc = hs.fetch(o_r, reduction_db, r_b);
-  return rc ? rc : hs.finish();
+  const size_t o_x = hs.in(x, (size_t)cs->S * cs->F * 4), o_y = hs.out((size_t)cs->S * cs->F * 4, y), o_r = hs.out((size_t)cs->S * 4, reduction_db);
+  return hs.run([&](cudaStream_t st) {
+    return vtts_compressor_stream_push(ctx, cs, hs.dev<const float>(o_x), n_new, flags, hs.dev<float>(o_y), n_out, hs.dev<float>(o_r), st);
+  });
 }

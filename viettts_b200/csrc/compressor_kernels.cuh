@@ -13,6 +13,7 @@ namespace cpk {
 
 constexpr int Q = 256;                // block of both scans
 constexpr int SCAN_THREADS = 128;     // one thread per block or row
+constexpr long long S_MAX = 1 << 30;  // one-shot row length: int sample indices one block past the row stay exact
 
 struct CpRow {
   long long x0;      // absolute index of x buffer element 0
@@ -258,11 +259,6 @@ int cp_params(vtts_ctx* ctx, const char* who, int rate, float threshold_db, floa
   p->aA = (float)std::exp(-1000.0 / ((double)attack_ms * rate));
   p->bA = 1.f - p->aA;
   p->m = (float)std::pow(10.0, (double)makeup_db / 20.0);
-  return VTTS_OK;
-}
-
-int cp_check(vtts_ctx* ctx, const char* who, int B, int S) {
-  if (B < 1 || B > 65535 || S < 1 || S > (1 << 30)) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: B=%d S=%d (1..65535, 1..2^30)", who, B, S);
   return VTTS_OK;
 }
 

@@ -58,51 +58,51 @@ void ds_carve(Arena& a, int B, int S, DsBufs* d) {
   cpk::cp_carve(a, B, cpk::cp_blocks_max(S), &d->w);
 }
 
+// the parameters and batch shape of a one-shot call of entry point `who`
+int ds_args(vtts_ctx* ctx, const char* who, int B, int S, int rate, float freq_hz, float threshold_db, float ratio, float knee_db,
+            float attack_ms, float release_ms, float range_db, DsParams* d) {
+  const int rc = ds_params(ctx, who, rate, freq_hz, threshold_db, ratio, knee_db, attack_ms, release_ms, range_db, d);
+  return rc ? rc : batch_check(ctx, who, B, S, cpk::S_MAX);
+}
+
+int ds_launch(vtts_ctx* ctx, const DsParams& d, const float* x, const int32_t* n_in, int B, int S, float* y, float* reduction_db, cudaStream_t st) {
+  Arena m(nullptr, 0, true);
+  DsBufs w;
+  ds_carve(m, B, S, &w);
+  int rc = ctx->ensure_ws(m.off);
+  if (rc) return rc;
+  Arena a(ctx->ws, SIZE_MAX, false);
+  ds_carve(a, B, S, &w);
+  const int nb = (S + eqk::Q - 1) / eqk::Q;
+  rc = eqk::eq_run(ctx, d.f, x, S, S, n_in, nullptr, B, nb, nb, w.e, w.s, nullptr, w.h, S, st);
+  if (rc) return rc;
+  return cpk::cp_run(ctx, d.p, x, S, S, n_in, nullptr, B, S, S, w.w, y, S, reduction_db, st, cpk::CpSplit{w.h, d.range});
+}
+
 }  // namespace
 
 int vtts_deess(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, float freq_hz, float threshold_db, float ratio,
                float knee_db, float attack_ms, float release_ms, float range_db, float* y_dev, float* reduction_db_dev, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   DsParams d;
-  int rc = ds_params(ctx, "deess", rate, freq_hz, threshold_db, ratio, knee_db, attack_ms, release_ms, range_db, &d);
-  if (!rc) rc = cpk::cp_check(ctx, "deess", B, S);
+  const int rc = ds_args(ctx, "deess", B, S, rate, freq_hz, threshold_db, ratio, knee_db, attack_ms, release_ms, range_db, &d);
   if (rc) return rc;
   if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "deess: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  Arena m(nullptr, 0, true);
-  DsBufs w;
-  ds_carve(m, B, S, &w);
-  rc = ctx->ensure_ws(m.off);
-  if (rc) return rc;
-  Arena a(ctx->ws, SIZE_MAX, false);
-  ds_carve(a, B, S, &w);
-  const cudaStream_t st = (cudaStream_t)stream;
-  const int nb = (S + eqk::Q - 1) / eqk::Q;
-  rc = eqk::eq_run(ctx, d.f, x_dev, S, S, n_dev, nullptr, B, nb, nb, w.e, w.s, nullptr, w.h, S, st);
-  if (rc) return rc;
-  return cpk::cp_run(ctx, d.p, x_dev, S, S, n_dev, nullptr, B, S, S, w.w, y_dev, S, reduction_db_dev, st, cpk::CpSplit{w.h, d.range});
+  return ds_launch(ctx, d, x_dev, n_dev, B, S, y_dev, reduction_db_dev, (cudaStream_t)stream);
 }
 
 int vtts_deess_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float freq_hz, float threshold_db, float ratio,
                     float knee_db, float attack_ms, float release_ms, float range_db, float* y, float* reduction_db) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   DsParams d;
-  int rc = ds_params(ctx, "deess_host", rate, freq_hz, threshold_db, ratio, knee_db, attack_ms, release_ms, range_db, &d);
-  if (!rc) rc = cpk::cp_check(ctx, "deess_host", B, S);
-  if (!rc) rc = host_lengths_check(ctx, "deess_host", n_in, B, S);
+  int rc = ds_args(ctx, "deess_host", B, S, rate, freq_hz, threshold_db, ratio, knee_db, attack_ms, release_ms, range_db, &d);
   if (rc) return rc;
-  if (!x || !y) return ctx->fail(VTTS_ERR_BAD_ARG, "deess_host: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4, r_b = (size_t)B * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, r_b), o_r = hs.out(r_b), o_y = hs.out(x_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = vtts_deess(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, rate, freq_hz, threshold_db, ratio,
-                    knee_db, attack_ms, release_ms, range_db, hs.dev<float>(o_y), hs.dev<float>(o_r), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, x_b);
-  if (!rc && reduction_db) rc = hs.fetch(o_r, reduction_db, r_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("deess_host", x, n_in, B, S, y != nullptr);
+  if (rc) return rc;
+  const size_t o_r = hs.out((size_t)B * 4, reduction_db), o_y = hs.out((size_t)B * S * 4, y);
+  return hs.run([&](cudaStream_t st) { return ds_launch(ctx, d, hs.x(), hs.n(), B, S, hs.dev<float>(o_y), hs.dev<float>(o_r), st); });
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
@@ -120,14 +120,11 @@ struct vtts_deesser_stream : SampleStream<eqk::EqRow, cpk::CpRow> {
 int vtts_deesser_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int rate, float freq_hz, float threshold_db, float ratio,
                                float knee_db, float attack_ms, float release_ms, float range_db, vtts_deesser_stream** out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out) return ctx->fail(VTTS_ERR_BAD_ARG, "deesser_stream_create: null output pointer");
-  *out = nullptr;
-  DsParams d;
-  int rc = ds_params(ctx, "deesser_stream_create", rate, freq_hz, threshold_db, ratio, knee_db, attack_ms, release_ms, range_db, &d);
+  int rc = create_check(ctx, "deesser_stream_create", out, true, max_streams, max_chunk_samples);
   if (rc) return rc;
-  if (max_streams < 1 || max_streams > 65535 || max_chunk_samples < 1 || max_chunk_samples > (1 << 22))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "deesser_stream_create: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", max_streams,
-                     max_chunk_samples, 1 << 22);
+  DsParams d;
+  rc = ds_params(ctx, "deesser_stream_create", rate, freq_hz, threshold_db, ratio, knee_db, attack_ms, release_ms, range_db, &d);
+  if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
   std::unique_ptr<vtts_deesser_stream> ds(new vtts_deesser_stream(ctx, max_streams, max_chunk_samples, eqk::Q));
   ds->d = d;
@@ -199,15 +196,11 @@ int vtts_deesser_stream_push(vtts_ctx* ctx, vtts_deesser_stream* ds, const float
 int vtts_deesser_stream_push_host(vtts_ctx* ctx, vtts_deesser_stream* ds, const float* x, const int32_t* n_new, const uint8_t* flags,
                                   float* y, int32_t* n_out, float* reduction_db) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = stream_args(ctx, "deesser_stream_push_host", ds, x && y && reduction_db);
+  const int rc = stream_args(ctx, "deesser_stream_push_host", ds, x && y && reduction_db);
   if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)ds->S * ds->F * 4, r_b = (size_t)ds->S * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_y = hs.out(x_b), o_r = hs.out(r_b);
-  rc = hs.upload();
-  if (!rc) rc = vtts_deesser_stream_push(ctx, ds, hs.dev<const float>(o_x), n_new, flags, hs.dev<float>(o_y), n_out, hs.dev<float>(o_r), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, x_b);
-  if (!rc) rc = hs.fetch(o_r, reduction_db, r_b);
-  return rc ? rc : hs.finish();
+  const size_t o_x = hs.in(x, (size_t)ds->S * ds->F * 4), o_y = hs.out((size_t)ds->S * ds->F * 4, y), o_r = hs.out((size_t)ds->S * 4, reduction_db);
+  return hs.run([&](cudaStream_t st) {
+    return vtts_deesser_stream_push(ctx, ds, hs.dev<const float>(o_x), n_new, flags, hs.dev<float>(o_y), n_out, hs.dev<float>(o_r), st);
+  });
 }

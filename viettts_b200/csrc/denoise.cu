@@ -119,40 +119,48 @@ int vtts_denoise_ola(vtts_ctx* ctx, const float* x, long long x_ld, int S, const
 
 int vtts_denoise_stream_lookahead(void) { return stftg::LOOKAHEAD; }
 
-int vtts_denoise(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, float strength, const float* bias_dev, float* y_dev,
-                 void* stream) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!x_dev || !y_dev || !bias_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise: null pointer");
-  if (x_dev == y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise: y must not alias x");
-  if (B < 1 || B > 65535 || S < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise: B=%d S=%d (1..65535, >= 1)", B, S);
-  if (!finite_nonneg(strength)) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise: strength %g (finite and >= 0)", (double)strength);
-  VTTS_CUDA(cudaSetDevice(ctx->device));
+namespace {
+
+// the parameters and batch shape of a one-shot call of entry point `who`
+int dn_args(vtts_ctx* ctx, const char* who, int B, int S, float strength) {
+  const int rc = batch_check(ctx, who, B, S, S_ANY);
+  if (rc) return rc;
+  if (!finite_nonneg(strength)) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: strength %g (finite and >= 0)", who, (double)strength);
+  return VTTS_OK;
+}
+
+int dn_launch(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, float strength, const float* bias, float* y, cudaStream_t st) {
   int rc = vtts_fft_tables(ctx);
   if (rc) return rc;
   const int ws_frames = S / HOP + 1;
   rc = ctx->ensure_ws((size_t)B * ws_frames * NF * sizeof(float));
   if (rc) return rc;
-  return stftg::launch(ctx, x_dev, S, S, n_dev, nullptr, B, ws_frames, S, DnGain{bias_dev, strength}, (float*)ctx->ws, ws_frames, y_dev, S,
-                       (cudaStream_t)stream);
+  return stftg::launch(ctx, x, S, S, n_in, nullptr, B, ws_frames, S, DnGain{bias, strength}, (float*)ctx->ws, ws_frames, y, S, st);
+}
+
+}  // namespace
+
+int vtts_denoise(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, float strength, const float* bias_dev, float* y_dev,
+                 void* stream) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  const int rc = dn_args(ctx, "denoise", B, S, strength);
+  if (rc) return rc;
+  if (!x_dev || !y_dev || !bias_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise: null pointer");
+  if (x_dev == y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise: y must not alias x");
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  return dn_launch(ctx, x_dev, n_dev, B, S, strength, bias_dev, y_dev, (cudaStream_t)stream);
 }
 
 int vtts_denoise_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, float strength, const float* bias, float* y) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!x || !y || !bias || B < 1 || B > 65535 || S < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_host: bad argument (B=%d S=%d)", B, S);
-  if (!finite_nonneg(strength)) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_host: strength %g (finite and >= 0)", (double)strength);
-  int rc = dn_check_bias(ctx, "denoise_host", bias);
-  if (!rc) rc = host_lengths_check(ctx, "denoise_host", n_in, B, S);
+  int rc = dn_args(ctx, "denoise_host", B, S, strength);
   if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, (size_t)B * 4), o_b = hs.in(bias, (size_t)NB * 4), o_y = hs.out(x_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = vtts_denoise(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, strength, hs.dev<const float>(o_b),
-                      hs.dev<float>(o_y), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, x_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("denoise_host", x, n_in, B, S, y && bias);
+  if (!rc) rc = dn_check_bias(ctx, "denoise_host", bias);
+  if (rc) return rc;
+  const size_t o_b = hs.in(bias, (size_t)NB * 4), o_y = hs.out((size_t)B * S * 4, y);
+  return hs.run([&](cudaStream_t st) { return dn_launch(ctx, hs.x(), hs.n(), B, S, strength, hs.dev<const float>(o_b), hs.dev<float>(o_y), st); });
 }
 
 int vtts_denoise_bias(vtts_ctx* ctx, const float* wav_dev, int n, float* bias_dev, void* stream) {
@@ -178,13 +186,10 @@ struct vtts_denoise_stream : stftg::Stream {
 int vtts_denoise_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, float strength, const float* bias,
                                vtts_denoise_stream** out, int* out_pitch) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out || !out_pitch || !bias) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_stream_create: null pointer");
-  *out = nullptr;
-  if (max_streams < 1 || max_streams > 65535 || max_chunk_samples < 1 || max_chunk_samples > (1 << 22))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_stream_create: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", max_streams,
-                     max_chunk_samples, 1 << 22);
+  int rc = create_check(ctx, "denoise_stream_create", out, out_pitch && bias, max_streams, max_chunk_samples);
+  if (rc) return rc;
   if (!finite_nonneg(strength)) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_stream_create: strength %g (finite and >= 0)", (double)strength);
-  int rc = dn_check_bias(ctx, "denoise_stream_create", bias);
+  rc = dn_check_bias(ctx, "denoise_stream_create", bias);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
   rc = vtts_fft_tables(ctx);
@@ -219,10 +224,11 @@ int vtts_denoise_stream_push(vtts_ctx* ctx, vtts_denoise_stream* ds, const float
 int vtts_denoise_stream_push_host(vtts_ctx* ctx, vtts_denoise_stream* ds, const float* x, const int32_t* n_new, const uint8_t* flags,
                                   float* y, int32_t* n_out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = stream_args(ctx, "denoise_stream_push_host", ds, x && y);
+  const int rc = stream_args(ctx, "denoise_stream_push_host", ds, x && y);
   if (rc) return rc;
-  return stream_push_host(ctx, x, (size_t)ds->S * ds->F * 4, y, (size_t)ds->S * ds->out_pitch * 4,
-                          [&](const float* x_dev, float* y_dev, cudaStream_t st) {
-                            return vtts_denoise_stream_push(ctx, ds, x_dev, n_new, flags, y_dev, n_out, st);
-                          });
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, (size_t)ds->S * ds->F * 4), o_y = hs.out((size_t)ds->S * ds->out_pitch * 4, y);
+  return hs.run([&](cudaStream_t st) {
+    return vtts_denoise_stream_push(ctx, ds, hs.dev<const float>(o_x), n_new, flags, hs.dev<float>(o_y), n_out, st);
+  });
 }

@@ -132,11 +132,15 @@ __global__ void __launch_bounds__(THREADS) decode_kernel(const Code<E>* __restri
 
 size_t code_bytes(int encoding) { return encoding == VTTS_ENC_PCM16 ? 2 : 1; }
 
-// the argument rules of every entry point: a known encoding, 1 <= B <= 65535, S >= 1, both buffers given and apart
-int coder_args(vtts_ctx* ctx, const char* who, const void* f32, const void* codes, int B, int S, int encoding) {
+// the encoding and batch shape of a call of entry point `who`
+int coder_args(vtts_ctx* ctx, const char* who, int B, int S, int encoding) {
   if (encoding != VTTS_ENC_PCM16 && encoding != VTTS_ENC_ULAW && encoding != VTTS_ENC_ALAW)
     return ctx->fail(VTTS_ERR_BAD_ARG, "%s: encoding %d (VTTS_ENC_PCM16, _ULAW or _ALAW)", who, encoding);
-  if (B < 1 || B > 65535 || S < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: B=%d S=%d (1..65535, >= 1)", who, B, S);
+  return batch_check(ctx, who, B, S, S_ANY);
+}
+
+// both buffers given and apart
+int coder_apart(vtts_ctx* ctx, const char* who, const void* f32, const void* codes, int B, int S, int encoding) {
   if (!f32 || !codes) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: null pointer", who);
   const uintptr_t a = (uintptr_t)f32, c = (uintptr_t)codes;
   const size_t n = (size_t)B * S;
@@ -149,72 +153,72 @@ dim3 coder_grid(int B, int S) {
   return dim3((unsigned)((groups + THREADS - 1) / THREADS), (unsigned)B);
 }
 
+int encode_launch(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int encoding, void* y, cudaStream_t st) {
+  const dim3 grid = coder_grid(B, S);
+  if (encoding == VTTS_ENC_PCM16)
+    encode_kernel<VTTS_ENC_PCM16><<<grid, THREADS, 0, st>>>(x, n_in, S, (int16_t*)y);
+  else if (encoding == VTTS_ENC_ULAW)
+    encode_kernel<VTTS_ENC_ULAW><<<grid, THREADS, 0, st>>>(x, n_in, S, (uint8_t*)y);
+  else
+    encode_kernel<VTTS_ENC_ALAW><<<grid, THREADS, 0, st>>>(x, n_in, S, (uint8_t*)y);
+  ctx->launches++;
+  VTTS_CUDA(cudaGetLastError());
+  return VTTS_OK;
+}
+
+int decode_launch(vtts_ctx* ctx, const void* c, const int32_t* n_in, int B, int S, int encoding, float* y, cudaStream_t st) {
+  const dim3 grid = coder_grid(B, S);
+  if (encoding == VTTS_ENC_PCM16)
+    decode_kernel<VTTS_ENC_PCM16><<<grid, THREADS, 0, st>>>((const int16_t*)c, n_in, S, y);
+  else if (encoding == VTTS_ENC_ULAW)
+    decode_kernel<VTTS_ENC_ULAW><<<grid, THREADS, 0, st>>>((const uint8_t*)c, n_in, S, y);
+  else
+    decode_kernel<VTTS_ENC_ALAW><<<grid, THREADS, 0, st>>>((const uint8_t*)c, n_in, S, y);
+  ctx->launches++;
+  VTTS_CUDA(cudaGetLastError());
+  return VTTS_OK;
+}
+
 }  // namespace
 
 int vtts_encode(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int encoding, void* y_dev, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = coder_args(ctx, "encode", x_dev, y_dev, B, S, encoding);
+  int rc = coder_args(ctx, "encode", B, S, encoding);
+  if (!rc) rc = coder_apart(ctx, "encode", x_dev, y_dev, B, S, encoding);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  const dim3 grid = coder_grid(B, S);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (encoding == VTTS_ENC_PCM16)
-    encode_kernel<VTTS_ENC_PCM16><<<grid, THREADS, 0, st>>>(x_dev, n_dev, S, (int16_t*)y_dev);
-  else if (encoding == VTTS_ENC_ULAW)
-    encode_kernel<VTTS_ENC_ULAW><<<grid, THREADS, 0, st>>>(x_dev, n_dev, S, (uint8_t*)y_dev);
-  else
-    encode_kernel<VTTS_ENC_ALAW><<<grid, THREADS, 0, st>>>(x_dev, n_dev, S, (uint8_t*)y_dev);
-  ctx->launches++;
-  VTTS_CUDA(cudaGetLastError());
-  return VTTS_OK;
+  return encode_launch(ctx, x_dev, n_dev, B, S, encoding, y_dev, (cudaStream_t)stream);
 }
 
 int vtts_encode_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int encoding, void* y) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = coder_args(ctx, "encode_host", x, y, B, S, encoding);
-  if (!rc) rc = host_lengths_check(ctx, "encode_host", n_in, B, S);
+  int rc = coder_args(ctx, "encode_host", B, S, encoding);
+  if (!rc) rc = coder_apart(ctx, "encode_host", x, y, B, S, encoding);
   if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4, y_b = (size_t)B * S * code_bytes(encoding);
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, (size_t)B * 4), o_y = hs.out(y_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = vtts_encode(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, encoding, hs.dev<void>(o_y), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, y_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("encode_host", x, n_in, B, S);
+  if (rc) return rc;
+  const size_t o_y = hs.out((size_t)B * S * code_bytes(encoding), y);
+  return hs.run([&](cudaStream_t st) { return encode_launch(ctx, hs.x(), hs.n(), B, S, encoding, hs.dev<void>(o_y), st); });
 }
 
 int vtts_decode(vtts_ctx* ctx, const void* c_dev, const int32_t* n_dev, int B, int S, int encoding, float* y_dev, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = coder_args(ctx, "decode", y_dev, c_dev, B, S, encoding);
+  int rc = coder_args(ctx, "decode", B, S, encoding);
+  if (!rc) rc = coder_apart(ctx, "decode", y_dev, c_dev, B, S, encoding);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  const dim3 grid = coder_grid(B, S);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (encoding == VTTS_ENC_PCM16)
-    decode_kernel<VTTS_ENC_PCM16><<<grid, THREADS, 0, st>>>((const int16_t*)c_dev, n_dev, S, y_dev);
-  else if (encoding == VTTS_ENC_ULAW)
-    decode_kernel<VTTS_ENC_ULAW><<<grid, THREADS, 0, st>>>((const uint8_t*)c_dev, n_dev, S, y_dev);
-  else
-    decode_kernel<VTTS_ENC_ALAW><<<grid, THREADS, 0, st>>>((const uint8_t*)c_dev, n_dev, S, y_dev);
-  ctx->launches++;
-  VTTS_CUDA(cudaGetLastError());
-  return VTTS_OK;
+  return decode_launch(ctx, c_dev, n_dev, B, S, encoding, y_dev, (cudaStream_t)stream);
 }
 
 int vtts_decode_host(vtts_ctx* ctx, const void* c, const int32_t* n_in, int B, int S, int encoding, float* y) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = coder_args(ctx, "decode_host", y, c, B, S, encoding);
-  if (!rc) rc = host_lengths_check(ctx, "decode_host", n_in, B, S);
+  int rc = coder_args(ctx, "decode_host", B, S, encoding);
+  if (!rc) rc = coder_apart(ctx, "decode_host", y, c, B, S, encoding);
   if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t c_b = (size_t)B * S * code_bytes(encoding), y_b = (size_t)B * S * 4;
   HostStage hs(ctx);
-  const size_t o_c = hs.in(c, c_b), o_n = hs.in(n_in, (size_t)B * 4), o_y = hs.out(y_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = vtts_decode(ctx, hs.dev<const void>(o_c), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, encoding, hs.dev<float>(o_y), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, y_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("decode_host", c, n_in, B, S, true, code_bytes(encoding));
+  if (rc) return rc;
+  const size_t o_y = hs.out((size_t)B * S * 4, y);
+  return hs.run([&](cudaStream_t st) { return decode_launch(ctx, hs.x<void>(), hs.n(), B, S, encoding, hs.dev<float>(o_y), st); });
 }

@@ -115,39 +115,46 @@ int vtts_eq_design(int kind, int rate, double f0, double q, double gain_db, int 
   }
 }
 
-int vtts_eq(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const double* sos, int K, float* y_dev, void* stream) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  EqFilter f;
-  int rc = eq_check(ctx, "eq", B, S);
-  if (!rc) rc = eq_filter(ctx, "eq", sos, K, &f);
-  if (rc) return rc;
-  if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "eq: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
+namespace {
+
+// the batch shape and filter of a one-shot call of entry point `who`
+int eq_args(vtts_ctx* ctx, const char* who, int B, int S, const double* sos, int K, EqFilter* f) {
+  const int rc = batch_check(ctx, who, B, S, S_MAX);
+  return rc ? rc : eq_filter(ctx, who, sos, K, f);
+}
+
+int eq_launch(vtts_ctx* ctx, const EqFilter& f, const float* x, const int32_t* n_in, int B, int S, float* y, cudaStream_t st) {
   const int nb = (S + Q - 1) / Q;
   const size_t es_b = al((size_t)B * nb * NS * 4);
-  rc = ctx->ensure_ws(2 * es_b);
+  const int rc = ctx->ensure_ws(2 * es_b);
   if (rc) return rc;
   float* e = (float*)ctx->ws;
   float* s = (float*)((char*)ctx->ws + es_b);
-  return eq_run(ctx, f, x_dev, S, S, n_dev, nullptr, B, nb, nb, e, s, nullptr, y_dev, S, (cudaStream_t)stream);
+  return eq_run(ctx, f, x, S, S, n_in, nullptr, B, nb, nb, e, s, nullptr, y, S, st);
+}
+
+}  // namespace
+
+int vtts_eq(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const double* sos, int K, float* y_dev, void* stream) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  EqFilter f;
+  const int rc = eq_args(ctx, "eq", B, S, sos, K, &f);
+  if (rc) return rc;
+  if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "eq: null pointer");
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  return eq_launch(ctx, f, x_dev, n_dev, B, S, y_dev, (cudaStream_t)stream);
 }
 
 int vtts_eq_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, const double* sos, int K, float* y) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   EqFilter f;
-  int rc = eq_check(ctx, "eq_host", B, S);
-  if (!rc) rc = eq_filter(ctx, "eq_host", sos, K, &f);
-  if (!rc) rc = host_lengths_check(ctx, "eq_host", n_in, B, S);
+  int rc = eq_args(ctx, "eq_host", B, S, sos, K, &f);
   if (rc) return rc;
-  if (!x || !y) return ctx->fail(VTTS_ERR_BAD_ARG, "eq_host: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4, n_b = (size_t)B * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, n_b), o_y = hs.out(x_b);
-  rc = hs.upload();
-  if (!rc) rc = vtts_eq(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, sos, K, hs.dev<float>(o_y), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, x_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("eq_host", x, n_in, B, S, y != nullptr);
+  if (rc) return rc;
+  const size_t o_y = hs.out((size_t)B * S * 4, y);
+  return hs.run([&](cudaStream_t st) { return eq_launch(ctx, f, hs.x(), hs.n(), B, S, hs.dev<float>(o_y), st); });
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
@@ -161,13 +168,10 @@ struct vtts_eq_stream : SampleStream<EqRow> {
 
 int vtts_eq_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, const double* sos, int K, vtts_eq_stream** out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out) return ctx->fail(VTTS_ERR_BAD_ARG, "eq_stream_create: null output pointer");
-  *out = nullptr;
-  if (max_streams < 1 || max_streams > 65535 || max_chunk_samples < 1 || max_chunk_samples > (1 << 22))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "eq_stream_create: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", max_streams,
-                     max_chunk_samples, 1 << 22);
+  int rc = create_check(ctx, "eq_stream_create", out, true, max_streams, max_chunk_samples);
+  if (rc) return rc;
   EqFilter f;
-  int rc = eq_filter(ctx, "eq_stream_create", sos, K, &f);
+  rc = eq_filter(ctx, "eq_stream_create", sos, K, &f);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
   std::unique_ptr<vtts_eq_stream> es(new vtts_eq_stream(ctx, max_streams, max_chunk_samples, Q));
@@ -227,10 +231,10 @@ int vtts_eq_stream_push(vtts_ctx* ctx, vtts_eq_stream* es, const float* x_dev, c
 int vtts_eq_stream_push_host(vtts_ctx* ctx, vtts_eq_stream* es, const float* x, const int32_t* n_new, const uint8_t* flags, float* y,
                              int32_t* n_out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = stream_args(ctx, "eq_stream_push_host", es, x && y);
+  const int rc = stream_args(ctx, "eq_stream_push_host", es, x && y);
   if (rc) return rc;
   const size_t b = (size_t)es->S * es->F * 4;
-  return stream_push_host(ctx, x, b, y, b, [&](const float* x_dev, float* y_dev, cudaStream_t st) {
-    return vtts_eq_stream_push(ctx, es, x_dev, n_new, flags, y_dev, n_out, st);
-  });
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, b), o_y = hs.out(b, y);
+  return hs.run([&](cudaStream_t st) { return vtts_eq_stream_push(ctx, es, hs.dev<const float>(o_x), n_new, flags, hs.dev<float>(o_y), n_out, st); });
 }

@@ -15,6 +15,7 @@ constexpr int NS = 2 * KMAX;          // cascade state
 constexpr int SEG = 32;               // samples per lane
 constexpr int Q = 32 * SEG;           // samples per block (one warp)
 constexpr int WARPS = 4;              // blocks per CTA
+constexpr long long S_MAX = 1 << 30;  // one-shot row length: int sample indices one block past the row stay exact
 constexpr int CHAIN_WARPS = 4;        // rows per CTA of the chain kernel
 constexpr double POLE_MARGIN = 1e-6;  // every pole radius <= 1 - POLE_MARGIN
 constexpr unsigned FULL = 0xffffffffu;
@@ -288,12 +289,6 @@ int eq_run(vtts_ctx* ctx, const EqFilter& f, const float* x, long long x_ld, int
 }
 
 size_t al(size_t b) { return (b + 255) & ~size_t(255); }
-
-int eq_check(vtts_ctx* ctx, const char* who, int B, int S) {
-  if (B < 1 || B > 65535 || S < 1 || S > (1 << 30))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "%s: B=%d S=%d (1..65535, 1..2^30)", who, B, S);
-  return VTTS_OK;
-}
 
 // the stream row of a slot that holds P0 samples before the push and P1 after it: its window carries the samples from
 // P0 - Q on (the incomplete block), it re-runs the blocks from P0's, and it releases every sample the push brings

@@ -676,15 +676,22 @@ bool overlaps(const void* a, size_t an, const void* b, size_t bn) {
   return x < y + bn && y < x + an;
 }
 
-int flac_args(vtts_ctx* ctx, const char* who, const void* x, const void* y, const void* nb, int B, int S, int rate, int block,
-              long long pitch, RateCode* rc) {
+// the block, rate and batch shape of a one-shot call of entry point `who` (an empty row is a valid stream), and the
+// bytes a row can take
+int flac_args(vtts_ctx* ctx, const char* who, int B, int S, int rate, int block, RateCode* rc, long long* bound) {
   if (!block_ok(block)) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: block %d (256, 512, 1024, 2048 or 4096)", who, block);
   if (!rate_code(rate, rc))
     return ctx->fail(VTTS_ERR_BAD_ARG, "%s: rate %d has no FLAC frame-header code (a table rate, kHz <= 255, Hz <= 65535 or "
                      "tens of Hz <= 655350)", who, rate);
-  if (B < 1 || B > 65535 || S < 0) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: B=%d S=%d (1..65535, >= 0)", who, B, S);
-  const long long bound = flac_bound(S, block);
-  if (bound > INT_MAX) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: S=%d: a row's bound of %lld bytes exceeds 2^31 - 1", who, S, bound);
+  const int r = batch_check(ctx, who, B, S, S_ANY, 0);
+  if (r) return r;
+  *bound = flac_bound(S, block);
+  if (*bound > INT_MAX) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: S=%d: a row's bound of %lld bytes exceeds 2^31 - 1", who, S, *bound);
+  return VTTS_OK;
+}
+
+// the device buffers of a one-shot call: y rows `pitch` bytes apart, each at least the bound, all three apart
+int flac_buffers(vtts_ctx* ctx, const char* who, const void* x, const void* y, const void* nb, int B, int S, long long pitch, long long bound) {
   if (pitch < bound) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: y_pitch %lld below the bound %lld (vtts_flac_bound)", who, pitch, bound);
   if ((S && !x) || !y || !nb) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: null pointer", who);
   const size_t xb = (size_t)B * S * 4, yb = (size_t)(B - 1) * pitch + bound, nbb = (size_t)B * 4;
@@ -737,13 +744,10 @@ int vtts_flac_rate_code(int rate) {
   return rate_code(rate, &rc) ? rc.code : -1;
 }
 
-int vtts_flac_encode(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, int block, uint8_t* y_dev,
-                     int64_t y_pitch, int32_t* nbytes_dev, void* stream) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  RateCode rc;
-  int r = flac_args(ctx, "flac_encode", x_dev, y_dev, nbytes_dev, B, S, rate, block, y_pitch, &rc);
-  if (r) return r;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
+namespace {
+
+int flac_oneshot(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, int block, const RateCode& rc, uint8_t* y,
+                 int64_t y_pitch, int32_t* nbytes, cudaStream_t st) {
   const int nf = (S + block - 1) / block;
   const auto carve = [&](Arena& a, FrameDesc** d, FlacRow** rows, RowOut** ro) {
     *d = a.take<FrameDesc>((size_t)B * nf);
@@ -755,34 +759,45 @@ int vtts_flac_encode(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, in
   RowOut* ro;
   Arena m(nullptr, 0, true);
   carve(m, &d, &rows, &ro);
-  if ((r = ctx->ensure_ws(m.off))) return r;
+  if (const int r = ctx->ensure_ws(m.off)) return r;
   Arena a(ctx->ws, ctx->ws_bytes, false);
   carve(a, &d, &rows, &ro);
-  cudaStream_t st = (cudaStream_t)stream;
-  flac_rows_oneshot<<<(B + 255) / 256, 256, 0, st>>>(x_dev, n_dev, S, B, block, rows);
+  flac_rows_oneshot<<<(B + 255) / 256, 256, 0, st>>>(x, n_in, S, B, block, rows);
   ctx->launches++;
-  const FlacArgs A{rows, B, block, rc, rate, nf, d, ro, y_dev, y_pitch, nbytes_dev, nullptr};
+  const FlacArgs A{rows, B, block, rc, rate, nf, d, ro, y, y_pitch, nbytes, nullptr};
   return flac_launch(ctx, A, st);
 }
 
+}  // namespace
+
+int vtts_flac_encode(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, int block, uint8_t* y_dev,
+                     int64_t y_pitch, int32_t* nbytes_dev, void* stream) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  RateCode rc;
+  long long bound;
+  int r = flac_args(ctx, "flac_encode", B, S, rate, block, &rc, &bound);
+  if (!r) r = flac_buffers(ctx, "flac_encode", x_dev, y_dev, nbytes_dev, B, S, y_pitch, bound);
+  if (r) return r;
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  return flac_oneshot(ctx, x_dev, n_dev, B, S, rate, block, rc, y_dev, y_pitch, nbytes_dev, (cudaStream_t)stream);
+}
+
+// two fetches: each row's byte count, then as many bytes of every row as the longest one took
 int vtts_flac_encode_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, int block, uint8_t* y,
                           int64_t y_pitch, int32_t* nbytes) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   RateCode rc;
-  int r = flac_args(ctx, "flac_encode_host", x, y, nbytes, B, S, rate, block, y_pitch, &rc);
-  if (!r) r = host_lengths_check(ctx, "flac_encode_host", n_in, B, S);
+  long long pitch;
+  int r = flac_args(ctx, "flac_encode_host", B, S, rate, block, &rc, &pitch);
   if (r) return r;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const long long pitch = flac_bound(S, block);
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, (size_t)B * S * 4), o_n = hs.in(n_in, (size_t)B * 4), o_y = hs.out((size_t)B * pitch),
-               o_nb = hs.out((size_t)B * 4);
-  r = hs.upload();
-  if (!r)
-    r = vtts_flac_encode(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, rate, block,
-                         hs.dev<uint8_t>(o_y), pitch, hs.dev<int32_t>(o_nb), hs.st);
-  if (!r) r = hs.fetch(o_nb, nbytes, (size_t)B * 4);
-  if (!r) r = hs.finish();
+  r = flac_buffers(ctx, "flac_encode_host", x, y, nbytes, B, S, y_pitch, pitch);
+  if (!r) r = hs.rows("flac_encode_host", x, n_in, B, S);
+  if (r) return r;
+  const size_t o_y = hs.out((size_t)B * pitch), o_nb = hs.out((size_t)B * 4, nbytes);
+  r = hs.run([&](cudaStream_t st) {
+    return flac_oneshot(ctx, hs.x(), hs.n(), B, S, rate, block, rc, hs.dev<uint8_t>(o_y), pitch, hs.dev<int32_t>(o_nb), st);
+  });
   if (r) return r;
   // then one copy of the longest row's bytes from every row, and each row's own bytes out of it
   int width = 0;
@@ -830,18 +845,16 @@ struct vtts_flac_stream : StreamBase {
 int vtts_flac_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int rate, int block, vtts_flac_stream** out,
                             int64_t* out_bytes) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out || !out_bytes) return ctx->fail(VTTS_ERR_BAD_ARG, "flac_stream_create: null pointer");
+  int r = create_check(ctx, "flac_stream_create", out, out_bytes != nullptr, max_streams, max_chunk_samples);
+  if (r) return r;
   RateCode rc;
   if (!block_ok(block)) return ctx->fail(VTTS_ERR_BAD_ARG, "flac_stream_create: block %d (256, 512, 1024, 2048 or 4096)", block);
   if (!rate_code(rate, &rc)) return ctx->fail(VTTS_ERR_BAD_ARG, "flac_stream_create: rate %d has no FLAC frame-header code", rate);
-  if (max_streams < 1 || max_streams > 65535 || max_chunk_samples < 1 || max_chunk_samples > (1 << 22))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "flac_stream_create: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", max_streams,
-                     max_chunk_samples, 1 << 22);
   VTTS_CUDA(cudaSetDevice(ctx->device));
   std::unique_ptr<vtts_flac_stream> fs(new vtts_flac_stream(ctx, max_streams, max_chunk_samples, block, rate, rc));
   if ((long long)fs->out_cap > INT_MAX)
     return ctx->fail(VTTS_ERR_BAD_ARG, "flac_stream_create: a push's output of %lld bytes exceeds 2^31 - 1", fs->out_cap);
-  int r = stream_alloc(ctx, "flac_stream_create", *fs, [&](Arena& a) { fs->carve(a); });
+  r = stream_alloc(ctx, "flac_stream_create", *fs, [&](Arena& a) { fs->carve(a); });
   if (r) return r;
   *out_bytes = fs->out_cap;
   *out = fs.release();
@@ -901,13 +914,11 @@ int vtts_flac_stream_push_host(vtts_ctx* ctx, vtts_flac_stream* fs, const float*
   if (!ctx) return VTTS_ERR_BAD_ARG;
   int r = stream_args(ctx, "flac_stream_push_host", fs, x && n_new && flags && y && tbl);
   if (r) return r;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, (size_t)fs->S * fs->F * 4), o_y = hs.out(fs->out_cap), o_t = hs.out((size_t)fs->S * 8);
-  r = hs.upload();
-  if (!r) r = vtts_flac_stream_push(ctx, fs, hs.dev<const float>(o_x), n_new, flags, hs.dev<uint8_t>(o_y), hs.dev<int32_t>(o_t), hs.st);
-  if (!r) r = hs.fetch(o_t, tbl, (size_t)fs->S * 8);
-  if (!r) r = hs.finish();
+  const size_t o_x = hs.in(x, (size_t)fs->S * fs->F * 4), o_y = hs.out(fs->out_cap), o_t = hs.out((size_t)fs->S * 8, tbl);
+  r = hs.run([&](cudaStream_t st) {
+    return vtts_flac_stream_push(ctx, fs, hs.dev<const float>(o_x), n_new, flags, hs.dev<uint8_t>(o_y), hs.dev<int32_t>(o_t), st);
+  });
   if (r) return r;
   long long total = 0;   // the slots' bytes lie one after another from the start of the buffer
   for (int s = 0; s < fs->S; ++s) total += tbl[2 * s + 1];

@@ -322,20 +322,13 @@ int lm_params(vtts_ctx* ctx, const char* who, int rate, float ceiling, float loo
   return VTTS_OK;
 }
 
-int lm_check(vtts_ctx* ctx, const char* who, int B, int S) {
-  if (B < 1 || B > 65535 || S < 1 || (long long)S * OS > (1LL << 31) - 1)
-    return ctx->fail(VTTS_ERR_BAD_ARG, "%s: B=%d S=%d (1..65535, 1..2^29)", who, B, S);
-  return VTTS_OK;
-}
+// the oversampled index S * OS of a one-shot row must fit an int
+constexpr long long S_MAX = INT_MAX / OS;
 
-int lm_check_host(vtts_ctx* ctx, const char* who, const int32_t* n_in, const float* gain_db, int B, int S) {
-  const int rc = host_lengths_check(ctx, who, n_in, B, S);
-  if (rc) return rc;
-  if (gain_db)
-    for (int b = 0; b < B; ++b)
-      if (!(gain_db[b] >= -70.f && gain_db[b] <= 70.f))
-        return ctx->fail(VTTS_ERR_BAD_ARG, "%s: gain_db[%d]=%g outside [-70, 70]", who, b, (double)gain_db[b]);
-  return VTTS_OK;
+// the parameters and batch shape of a one-shot call of entry point `who`
+int lm_args(vtts_ctx* ctx, const char* who, int B, int S, int rate, float ceiling, float lookahead_ms, float release_ms, LmParams* p) {
+  const int rc = lm_params(ctx, who, rate, ceiling, lookahead_ms, release_ms, p);
+  return rc ? rc : batch_check(ctx, who, B, S, S_MAX);
 }
 
 size_t al(size_t b) { return (b + 255) & ~size_t(255); }
@@ -425,101 +418,103 @@ int lm_oneshot(vtts_ctx* ctx, void* ws, const LmParams& p, int rate, const float
   return lm_run(ctx, p, rate, S, n_in, nullptr, nullptr, B, (long long)OS * S, S, S, w, y, S, red, st);
 }
 
+// the one-shot limiter in the context workspace
+int lm_launch(vtts_ctx* ctx, const LmParams& p, int rate, const float* x, const int* n_in, const float* gain_db, int B, int S, float* y, float* red,
+              cudaStream_t st) {
+  const int rc = ctx->ensure_ws(lm_oneshot_bytes(B, S));
+  return rc ? rc : lm_oneshot(ctx, ctx->ws, p, rate, x, n_in, gain_db, B, S, y, red, st);
+}
+
+// the normalizer and limiter of a loudness_normalize_limited call whose arguments hold
+int lnl_launch(vtts_ctx* ctx, const LmParams& p, const float* x, const int32_t* n_in, int B, int S, int rate, float target, float* y,
+               float* gain_db, cudaStream_t st) {
+  // the meter and the limiter each use the workspace from its start; the first pass's output, the readings and the
+  // gains live past both
+  const size_t front = al(std::max(vtts_loudness_ws_bytes(B, S, rate), lm_oneshot_bytes(B, S)));
+  const size_t y1_b = al((size_t)B * S * 4), rd_b = al((size_t)B * 16);
+  int rc = ctx->ensure_ws(front + y1_b + rd_b + al((size_t)B * 4));
+  if (rc) return rc;
+  char* base = (char*)ctx->ws;
+  float* y1 = (float*)(base + front);
+  float* rd = (float*)(base + front + y1_b);
+  float* g = gain_db ? gain_db : (float*)(base + front + y1_b + rd_b);
+  const unsigned gg = (unsigned)((B + 127) / 128);
+  rc = vtts_loudness_launch(ctx, x, n_in, B, S, rate, rd, st);
+  if (rc) return rc;
+  lm_norm_gain_kernel<<<gg, 128, 0, st>>>(rd, B, target, true, g);
+  ctx->launches++;
+  VTTS_CUDA(cudaGetLastError());
+  rc = lm_oneshot(ctx, base, p, rate, x, n_in, g, B, S, y1, nullptr, st);
+  if (!rc) rc = vtts_loudness_launch(ctx, y1, n_in, B, S, rate, rd, st);
+  if (rc) return rc;
+  lm_norm_gain_kernel<<<gg, 128, 0, st>>>(rd, B, target, false, g);
+  ctx->launches++;
+  VTTS_CUDA(cudaGetLastError());
+  return lm_oneshot(ctx, base, p, rate, x, n_in, g, B, S, y, nullptr, st);
+}
+
+int lnl_args(vtts_ctx* ctx, const char* who, int B, int S, int rate, float target, float ceiling, float lookahead_ms, float release_ms,
+             LmParams* p) {
+  const int rc = lm_args(ctx, who, B, S, rate, ceiling, lookahead_ms, release_ms, p);
+  if (rc) return rc;
+  if (!(target >= -70.f && target <= 0.f)) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: target %g LUFS (in [-70, 0])", who, (double)target);
+  return VTTS_OK;
+}
+
 }  // namespace
 
 int vtts_limit(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, const float* gain_db_dev, int B, int S, int rate, float ceiling,
                float lookahead_ms, float release_ms, float* y_dev, float* reduction_db_dev, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   LmParams p;
-  int rc = lm_params(ctx, "limit", rate, ceiling, lookahead_ms, release_ms, &p);
-  if (!rc) rc = lm_check(ctx, "limit", B, S);
+  const int rc = lm_args(ctx, "limit", B, S, rate, ceiling, lookahead_ms, release_ms, &p);
   if (rc) return rc;
   if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "limit: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  rc = ctx->ensure_ws(lm_oneshot_bytes(B, S));
-  if (rc) return rc;
-  return lm_oneshot(ctx, ctx->ws, p, rate, x_dev, n_dev, gain_db_dev, B, S, y_dev, reduction_db_dev, (cudaStream_t)stream);
+  return lm_launch(ctx, p, rate, x_dev, n_dev, gain_db_dev, B, S, y_dev, reduction_db_dev, (cudaStream_t)stream);
 }
 
 int vtts_limit_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, const float* gain_db, int B, int S, int rate, float ceiling,
                     float lookahead_ms, float release_ms, float* y, float* reduction_db) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   LmParams p;
-  int rc = lm_params(ctx, "limit_host", rate, ceiling, lookahead_ms, release_ms, &p);
-  if (!rc) rc = lm_check(ctx, "limit_host", B, S);
-  if (!rc) rc = lm_check_host(ctx, "limit_host", n_in, gain_db, B, S);
+  int rc = lm_args(ctx, "limit_host", B, S, rate, ceiling, lookahead_ms, release_ms, &p);
   if (rc) return rc;
-  if (!x || !y) return ctx->fail(VTTS_ERR_BAD_ARG, "limit_host: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4, r_b = (size_t)B * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, r_b), o_g = hs.in(gain_db, r_b), o_r = hs.out(r_b), o_y = hs.out(x_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = vtts_limit(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, gain_db ? hs.dev<const float>(o_g) : nullptr,
-                    B, S, rate, ceiling, lookahead_ms, release_ms, hs.dev<float>(o_y), hs.dev<float>(o_r), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, x_b);
-  if (!rc && reduction_db) rc = hs.fetch(o_r, reduction_db, r_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("limit_host", x, n_in, B, S, y != nullptr);
+  if (rc) return rc;
+  if (gain_db)
+    for (int b = 0; b < B; ++b)
+      if (!(gain_db[b] >= -70.f && gain_db[b] <= 70.f))
+        return ctx->fail(VTTS_ERR_BAD_ARG, "limit_host: gain_db[%d]=%g outside [-70, 70]", b, (double)gain_db[b]);
+  const size_t o_g = hs.in(gain_db, (size_t)B * 4), o_r = hs.out((size_t)B * 4, reduction_db), o_y = hs.out((size_t)B * S * 4, y);
+  return hs.run([&](cudaStream_t st) {
+    return lm_launch(ctx, p, rate, hs.x(), hs.n(), gain_db ? hs.dev<const float>(o_g) : nullptr, B, S, hs.dev<float>(o_y), hs.dev<float>(o_r), st);
+  });
 }
 
 int vtts_loudness_normalize_limited(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, float target,
                                     float ceiling, float lookahead_ms, float release_ms, float* y_dev, float* gain_db_dev, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   LmParams p;
-  int rc = lm_params(ctx, "loudness_normalize_limited", rate, ceiling, lookahead_ms, release_ms, &p);
-  if (!rc) rc = lm_check(ctx, "loudness_normalize_limited", B, S);
+  const int rc = lnl_args(ctx, "loudness_normalize_limited", B, S, rate, target, ceiling, lookahead_ms, release_ms, &p);
   if (rc) return rc;
-  if (!(target >= -70.f && target <= 0.f))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_normalize_limited: target %g LUFS (in [-70, 0])", (double)target);
   if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_normalize_limited: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = (cudaStream_t)stream;
-  // the meter and the limiter each use the workspace from its start; the first pass's output, the readings and the
-  // gains live past both
-  const size_t front = al(std::max(vtts_loudness_ws_bytes(B, S, rate), lm_oneshot_bytes(B, S)));
-  const size_t y1_b = al((size_t)B * S * 4), rd_b = al((size_t)B * 16);
-  rc = ctx->ensure_ws(front + y1_b + rd_b + al((size_t)B * 4));
-  if (rc) return rc;
-  char* base = (char*)ctx->ws;
-  float* y1 = (float*)(base + front);
-  float* rd = (float*)(base + front + y1_b);
-  float* g = gain_db_dev ? gain_db_dev : (float*)(base + front + y1_b + rd_b);
-  const unsigned gg = (unsigned)((B + 127) / 128);
-  rc = vtts_loudness(ctx, x_dev, n_dev, B, S, rate, rd, st);
-  if (rc) return rc;
-  lm_norm_gain_kernel<<<gg, 128, 0, st>>>(rd, B, target, true, g);
-  ctx->launches++;
-  VTTS_CUDA(cudaGetLastError());
-  rc = lm_oneshot(ctx, base, p, rate, x_dev, n_dev, g, B, S, y1, nullptr, st);
-  if (!rc) rc = vtts_loudness(ctx, y1, n_dev, B, S, rate, rd, st);
-  if (rc) return rc;
-  lm_norm_gain_kernel<<<gg, 128, 0, st>>>(rd, B, target, false, g);
-  ctx->launches++;
-  VTTS_CUDA(cudaGetLastError());
-  return lm_oneshot(ctx, base, p, rate, x_dev, n_dev, g, B, S, y_dev, nullptr, st);
+  return lnl_launch(ctx, p, x_dev, n_dev, B, S, rate, target, y_dev, gain_db_dev, (cudaStream_t)stream);
 }
 
 int vtts_loudness_normalize_limited_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float target,
                                          float ceiling, float lookahead_ms, float release_ms, float* y, float* gain_db) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   LmParams p;
-  int rc = lm_params(ctx, "loudness_normalize_limited_host", rate, ceiling, lookahead_ms, release_ms, &p);
-  if (!rc) rc = lm_check(ctx, "loudness_normalize_limited_host", B, S);
-  if (!rc) rc = lm_check_host(ctx, "loudness_normalize_limited_host", n_in, nullptr, B, S);
+  int rc = lnl_args(ctx, "loudness_normalize_limited_host", B, S, rate, target, ceiling, lookahead_ms, release_ms, &p);
   if (rc) return rc;
-  if (!x || !y) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_normalize_limited_host: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4, n_b = (size_t)B * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, n_b), o_g = hs.out(n_b), o_y = hs.out(x_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = vtts_loudness_normalize_limited(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, rate, target,
-                                         ceiling, lookahead_ms, release_ms, hs.dev<float>(o_y), hs.dev<float>(o_g), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, x_b);
-  if (!rc && gain_db) rc = hs.fetch(o_g, gain_db, n_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("loudness_normalize_limited_host", x, n_in, B, S, y != nullptr);
+  if (rc) return rc;
+  const size_t o_g = hs.out((size_t)B * 4, gain_db), o_y = hs.out((size_t)B * S * 4, y);
+  return hs.run([&](cudaStream_t st) { return lnl_launch(ctx, p, hs.x(), hs.n(), B, S, rate, target, hs.dev<float>(o_y), hs.dev<float>(o_g), st); });
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
@@ -544,14 +539,11 @@ int vtts_limiter_stream_lookahead(int rate, float lookahead_ms) {
 int vtts_limiter_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int rate, float ceiling, float lookahead_ms,
                                float release_ms, vtts_limiter_stream** out, int* out_pitch) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out || !out_pitch) return ctx->fail(VTTS_ERR_BAD_ARG, "limiter_stream_create: null output pointer");
-  *out = nullptr;
-  LmParams p;
-  int rc = lm_params(ctx, "limiter_stream_create", rate, ceiling, lookahead_ms, release_ms, &p);
+  int rc = create_check(ctx, "limiter_stream_create", out, out_pitch != nullptr, max_streams, max_chunk_samples);
   if (rc) return rc;
-  if (max_streams < 1 || max_streams > 65535 || max_chunk_samples < 1 || max_chunk_samples > (1 << 22))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "limiter_stream_create: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", max_streams,
-                     max_chunk_samples, 1 << 22);
+  LmParams p;
+  rc = lm_params(ctx, "limiter_stream_create", rate, ceiling, lookahead_ms, release_ms, &p);
+  if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
   std::unique_ptr<vtts_limiter_stream> ls(new vtts_limiter_stream(ctx, max_streams, max_chunk_samples, 2 * p.W + 64));
   ls->rate = rate;
@@ -658,13 +650,10 @@ int vtts_limiter_stream_push_host(vtts_ctx* ctx, vtts_limiter_stream* ls, const 
   if (!ctx) return VTTS_ERR_BAD_ARG;
   int rc = stream_args(ctx, "limiter_stream_push_host", ls, x && y && reduction_db);
   if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)ls->S * ls->F * 4, y_b = (size_t)ls->S * ls->pitch * 4, r_b = (size_t)ls->S * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_y = hs.out(y_b), o_r = hs.out(r_b);
-  rc = hs.upload();
-  if (!rc) rc = vtts_limiter_stream_push(ctx, ls, hs.dev<const float>(o_x), n_new, flags, gain_db, hs.dev<float>(o_y), n_out, hs.dev<float>(o_r), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, y_b);
-  if (!rc) rc = hs.fetch(o_r, reduction_db, r_b);
-  return rc ? rc : hs.finish();
+  const size_t o_x = hs.in(x, (size_t)ls->S * ls->F * 4), o_y = hs.out((size_t)ls->S * ls->pitch * 4, y),
+               o_r = hs.out((size_t)ls->S * 4, reduction_db);
+  return hs.run([&](cudaStream_t st) {
+    return vtts_limiter_stream_push(ctx, ls, hs.dev<const float>(o_x), n_new, flags, gain_db, hs.dev<float>(o_y), n_out, hs.dev<float>(o_r), st);
+  });
 }

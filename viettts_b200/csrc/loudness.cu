@@ -425,17 +425,40 @@ int ln_oneshot_ws(vtts_ctx* ctx, int B, int S, int m, LnBufs* w, float** gains) 
   return VTTS_OK;
 }
 
-int ln_check(vtts_ctx* ctx, const char* who, int rate, int B, int S) {
+// the oversampled index S * OS of a one-shot row must fit an int
+constexpr long long S_MAX = INT_MAX / OS;
+
+// the rate and batch shape of a one-shot call of entry point `who`
+int ln_args(vtts_ctx* ctx, const char* who, int B, int S, int rate) {
   if (!rate_ok(rate)) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: rate %d (a multiple of 10 in [8000, 192000])", who, rate);
-  if (B < 1 || B > 65535 || S < 1 || (long long)S * OS > (1LL << 31) - 1)
-    return ctx->fail(VTTS_ERR_BAD_ARG, "%s: B=%d S=%d (1..65535, 1..2^29)", who, B, S);
-  return VTTS_OK;
+  return batch_check(ctx, who, B, S, S_MAX);
 }
 
-int ln_check_target(vtts_ctx* ctx, const char* who, float target, float ceiling) {
+// ... and of a normalize call
+int ln_norm_args(vtts_ctx* ctx, const char* who, int B, int S, int rate, float target, float ceiling) {
+  const int rc = ln_args(ctx, who, B, S, rate);
+  if (rc) return rc;
   if (!(target >= -70.f && target <= 0.f)) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: target %g LUFS (in [-70, 0])", who, (double)target);
   if (!(ceiling == INFINITY || (ceiling >= -20.f && ceiling <= 0.f)))
     return ctx->fail(VTTS_ERR_BAD_ARG, "%s: ceiling %g dBTP (in [-20, 0], or +inf for none)", who, (double)ceiling);
+  return VTTS_OK;
+}
+
+int ln_norm_launch(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float target, float ceiling, float* y,
+                   float* gain_db, cudaStream_t st) {
+  const LnFilter& f = ln_filter(ctx, rate);
+  LnBufs w;
+  float* gains = nullptr;
+  int rc = ln_oneshot_ws(ctx, B, S, rate / 10, &w, &gains);
+  if (rc) return rc;
+  const long long U = (long long)OS * S;
+  // the meter rows land in the e buffer, which the gate no longer reads
+  float* g_db = gain_db ? gain_db : gains;
+  rc = ln_measure(ctx, f, x, S, S, n_in, nullptr, nullptr, B, S / (rate / 10), U, S + U, w, w.e, target, ceiling, g_db, gains + B, st);
+  if (rc) return rc;
+  gain_apply_kernel<<<dim3((S + APPLY_THREADS - 1) / APPLY_THREADS, B), APPLY_THREADS, 0, st>>>(x, S, n_in, gains + B, y);
+  ctx->launches++;
+  VTTS_CUDA(cudaGetLastError());
   return VTTS_OK;
 }
 
@@ -453,82 +476,58 @@ int vtts_loudness_filter(int rate, double* coeffs) {
   return VTTS_OK;
 }
 
-int vtts_loudness(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, float* out_dev, void* stream) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = ln_check(ctx, "loudness", rate, B, S);
-  if (rc) return rc;
-  if (!x_dev || !out_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
+int vtts_loudness_launch(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float* out, cudaStream_t st) {
   const LnFilter& f = ln_filter(ctx, rate);
   LnBufs w;
   float* gains = nullptr;
-  rc = ln_oneshot_ws(ctx, B, S, rate / 10, &w, &gains);
+  const int rc = ln_oneshot_ws(ctx, B, S, rate / 10, &w, &gains);
   if (rc) return rc;
   const long long U = (long long)OS * S;
-  return ln_measure(ctx, f, x_dev, S, S, n_dev, nullptr, nullptr, B, S / (rate / 10), U, S + U, w, out_dev, 0.f, INFINITY, nullptr,
-                    nullptr, (cudaStream_t)stream);
+  return ln_measure(ctx, f, x, S, S, n_in, nullptr, nullptr, B, S / (rate / 10), U, S + U, w, out, 0.f, INFINITY, nullptr, nullptr, st);
+}
+
+int vtts_loudness(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, float* out_dev, void* stream) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  const int rc = ln_args(ctx, "loudness", B, S, rate);
+  if (rc) return rc;
+  if (!x_dev || !out_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness: null pointer");
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  return vtts_loudness_launch(ctx, x_dev, n_dev, B, S, rate, out_dev, (cudaStream_t)stream);
 }
 
 int vtts_loudness_normalize(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, float target, float ceiling,
                             float* y_dev, float* gain_db_dev, void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = ln_check(ctx, "loudness_normalize", rate, B, S);
-  if (!rc) rc = ln_check_target(ctx, "loudness_normalize", target, ceiling);
+  const int rc = ln_norm_args(ctx, "loudness_normalize", B, S, rate, target, ceiling);
   if (rc) return rc;
   if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_normalize: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  const LnFilter& f = ln_filter(ctx, rate);
-  LnBufs w;
-  float* gains = nullptr;
-  rc = ln_oneshot_ws(ctx, B, S, rate / 10, &w, &gains);
-  if (rc) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  const long long U = (long long)OS * S;
-  // the meter rows land in the e buffer, which the gate no longer reads
-  float* g_db = gain_db_dev ? gain_db_dev : gains;
-  rc = ln_measure(ctx, f, x_dev, S, S, n_dev, nullptr, nullptr, B, S / (rate / 10), U, S + U, w, w.e, target, ceiling, g_db, gains + B, st);
-  if (rc) return rc;
-  gain_apply_kernel<<<dim3((S + APPLY_THREADS - 1) / APPLY_THREADS, B), APPLY_THREADS, 0, st>>>(x_dev, S, n_dev, gains + B, y_dev);
-  ctx->launches++;
-  VTTS_CUDA(cudaGetLastError());
-  return VTTS_OK;
+  return ln_norm_launch(ctx, x_dev, n_dev, B, S, rate, target, ceiling, y_dev, gain_db_dev, (cudaStream_t)stream);
 }
 
 int vtts_loudness_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float* out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = ln_check(ctx, "loudness_host", rate, B, S);
-  if (!rc) rc = host_lengths_check(ctx, "loudness_host", n_in, B, S);
+  int rc = ln_args(ctx, "loudness_host", B, S, rate);
   if (rc) return rc;
-  if (!x || !out) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_host: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t o_b = (size_t)B * 16;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, (size_t)B * S * 4), o_n = hs.in(n_in, (size_t)B * 4), o_o = hs.out(o_b);
-  rc = hs.upload();
-  if (!rc) rc = vtts_loudness(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, rate, hs.dev<float>(o_o), hs.st);
-  if (!rc) rc = hs.fetch(o_o, out, o_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("loudness_host", x, n_in, B, S, out != nullptr);
+  if (rc) return rc;
+  const size_t o_o = hs.out((size_t)B * 16, out);
+  return hs.run([&](cudaStream_t st) { return vtts_loudness_launch(ctx, hs.x(), hs.n(), B, S, rate, hs.dev<float>(o_o), st); });
 }
 
 int vtts_loudness_normalize_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float target, float ceiling,
                                  float* y, float* gain_db) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = ln_check(ctx, "loudness_normalize_host", rate, B, S);
-  if (!rc) rc = ln_check_target(ctx, "loudness_normalize_host", target, ceiling);
-  if (!rc) rc = host_lengths_check(ctx, "loudness_normalize_host", n_in, B, S);
+  int rc = ln_norm_args(ctx, "loudness_normalize_host", B, S, rate, target, ceiling);
   if (rc) return rc;
-  if (!x || !y) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_normalize_host: null pointer");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4, n_b = (size_t)B * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, n_b), o_g = hs.out(n_b), o_y = hs.out(x_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = vtts_loudness_normalize(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, rate, target, ceiling,
-                                 hs.dev<float>(o_y), hs.dev<float>(o_g), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, x_b);
-  if (!rc && gain_db) rc = hs.fetch(o_g, gain_db, n_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("loudness_normalize_host", x, n_in, B, S, y != nullptr);
+  if (rc) return rc;
+  const size_t o_g = hs.out((size_t)B * 4, gain_db), o_y = hs.out((size_t)B * S * 4, y);
+  return hs.run([&](cudaStream_t st) {
+    return ln_norm_launch(ctx, hs.x(), hs.n(), B, S, rate, target, ceiling, hs.dev<float>(o_y), hs.dev<float>(o_g), st);
+  });
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
@@ -546,13 +545,11 @@ int vtts_loudness_stream_lookahead(int rate) {
 
 int vtts_loudness_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int rate, int max_seconds, vtts_loudness_stream** out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_stream_create: null output pointer");
-  *out = nullptr;
+  int rc = create_check(ctx, "loudness_stream_create", out, true, max_streams, max_chunk_samples);
+  if (rc) return rc;
   if (!rate_ok(rate)) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_stream_create: rate %d (a multiple of 10 in [8000, 192000])", rate);
-  if (max_streams < 1 || max_streams > 65535 || max_chunk_samples < 1 || max_chunk_samples > (1 << 22) || max_seconds < 1 ||
-      max_seconds > (1 << 20))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_stream_create: max_streams=%d max_chunk_samples=%d max_seconds=%d (1..65535, 1..%d, 1..%d)",
-                     max_streams, max_chunk_samples, max_seconds, 1 << 22, 1 << 20);
+  if (max_seconds < 1 || max_seconds > (1 << 20))
+    return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_stream_create: max_seconds=%d (1..%d)", max_seconds, 1 << 20);
   VTTS_CUDA(cudaSetDevice(ctx->device));
   ln_filter(ctx, rate);
   std::unique_ptr<vtts_loudness_stream> ls(new vtts_loudness_stream(ctx, max_streams, max_chunk_samples, rate / 10));
@@ -564,7 +561,7 @@ int vtts_loudness_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_sa
   ls->ptiles = (max_chunk_samples + ls->upitch + PEAK_TILE - 1) / PEAK_TILE;
   const size_t S = max_streams, kp = std::max(1, ls->kpush);
   static_assert(sizeof(LnRow) % 16 == 0 && sizeof(RsRow) % 16 == 0, "table entries keep 16-byte alignment");
-  int rc = stream_alloc(ctx, "loudness_stream_create", *ls, [&](Arena& a) {
+  rc = stream_alloc(ctx, "loudness_stream_create", *ls, [&](Arena& a) {
     ls->carve_window(a);
     ls->w.e = a.take<float>(S * kp * 4);
     ls->w.s = a.take<float>(S * kp * 4);
@@ -648,9 +645,9 @@ int vtts_loudness_stream_push(vtts_ctx* ctx, vtts_loudness_stream* ls, const flo
 int vtts_loudness_stream_push_host(vtts_ctx* ctx, vtts_loudness_stream* ls, const float* x, const int32_t* n_new, const uint8_t* flags,
                                    float* out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = stream_args(ctx, "loudness_stream_push_host", ls, x && out);
+  const int rc = stream_args(ctx, "loudness_stream_push_host", ls, x && out);
   if (rc) return rc;
-  return stream_push_host(ctx, x, (size_t)ls->S * ls->F * 4, out, (size_t)ls->S * 16, [&](const float* x_dev, float* out_dev, cudaStream_t st) {
-    return vtts_loudness_stream_push(ctx, ls, x_dev, n_new, flags, out_dev, st);
-  });
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, (size_t)ls->S * ls->F * 4), o_o = hs.out((size_t)ls->S * 16, out);
+  return hs.run([&](cudaStream_t st) { return vtts_loudness_stream_push(ctx, ls, hs.dev<const float>(o_x), n_new, flags, hs.dev<float>(o_o), st); });
 }

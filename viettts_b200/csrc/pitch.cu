@@ -484,11 +484,10 @@ int ps_launch(vtts_ctx* ctx, const float* x, long long x_ld, int S, const int* n
   return VTTS_OK;
 }
 
-// the pointer and shape rejections of a one-shot call, before its parameters are looked at
-int ps_check_call(vtts_ctx* ctx, const char* who, const float* x_dev, const void* out_dev, const float* y_dev, int B, int S) {
-  if (!x_dev || !out_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: null pointer", who);
+// the pointer rejections of a one-shot call into y_dev, or dec_dev for the decisions test hook
+int ps_pointers(vtts_ctx* ctx, const char* who, const float* x_dev, const float* y_dev, const int* dec_dev) {
+  if (!x_dev || (!y_dev && !dec_dev)) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: null pointer", who);
   if (x_dev == y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: y must not alias x", who);
-  if (B < 1 || B > 65535 || S < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: B=%d S=%d (1..65535, >= 1)", who, B, S);
   return VTTS_OK;
 }
 
@@ -497,7 +496,6 @@ int ps_check_call(vtts_ctx* ctx, const char* who, const float* x_dev, const void
 // for the legacy kernels
 int ps_one_shot(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, const std::vector<PsShift>& h, long long F, int Sy,
                 float* y_dev, int* dec_dev, cudaStream_t st, const std::vector<float>& ratio = {}) {
-  VTTS_CUDA(cudaSetDevice(ctx->device));
   int rc = vtts_fft_tables(ctx);
   if (rc) return rc;
   const bool use_env = !ratio.empty();
@@ -537,42 +535,48 @@ int ps_one_shot(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, 
   return vtts_denoise_ola(ctx, x_dev, S, S, nullptr, ola, B, Sy, w.syn, w.nbuf, y_dev, Sy, st);
 }
 
-// formants: null (the pitch shift: legacy kernels) or one formant shift per row (the envelope kernels)
-int ps_call(vtts_ctx* ctx, const char* who, const float* x_dev, const int32_t* n_dev, int B, int S, const float* semitones,
-            const float* formants, float* y_dev, int* dec_dev, cudaStream_t st) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = ps_check_call(ctx, who, x_dev, y_dev ? (const void*)y_dev : (const void*)dec_dev, y_dev, B, S);
+// the batch shape and per-row parameters h of a one-shot call of entry point `who`; formants: null (the pitch shift:
+// legacy kernels) or one formant shift per row (the envelope kernels, each row's envelope ratio in `ratio`)
+int ps_args(vtts_ctx* ctx, const char* who, int B, int S, const float* semitones, const float* formants, std::vector<PsShift>* h,
+            std::vector<float>* ratio) {
+  int rc = batch_check(ctx, who, B, S, S_ANY);
   if (!rc) rc = ps_check_shifts(ctx, who, semitones, B);
   if (!rc) rc = ps_check_formants(ctx, who, formants, B);
   if (rc) return rc;
-  std::vector<PsShift> h(B);
-  std::vector<float> ratio(formants ? B : 0);
+  h->resize(B);
+  ratio->resize(formants ? B : 0);
   for (int b = 0; b < B; ++b) {
     const float phi = formants ? formants[b] : NAN;
-    h[b] = ps_params(semitones[b], phi);
-    if (formants) ratio[b] = ps_env_ratio(phi, h[b]);
+    (*h)[b] = ps_params(semitones[b], phi);
+    if (formants) (*ratio)[b] = ps_env_ratio(phi, (*h)[b]);
   }
+  return VTTS_OK;
+}
+
+int ps_call(vtts_ctx* ctx, const char* who, const float* x_dev, const int32_t* n_dev, int B, int S, const float* semitones,
+            const float* formants, float* y_dev, int* dec_dev, cudaStream_t st) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  std::vector<PsShift> h;
+  std::vector<float> ratio;
+  int rc = ps_args(ctx, who, B, S, semitones, formants, &h, &ratio);
+  if (!rc) rc = ps_pointers(ctx, who, x_dev, y_dev, dec_dev);
+  if (rc) return rc;
+  VTTS_CUDA(cudaSetDevice(ctx->device));
   return ps_one_shot(ctx, x_dev, n_dev, B, S, h, S / HOP + 1, S, y_dev, dec_dev, st, ratio);
 }
 
-int ps_call_host(vtts_ctx* ctx, const char* who, const char* dev_who, const float* x, const int32_t* n_in, int B, int S,
-                 const float* semitones, const float* formants, float* y) {
+int ps_call_host(vtts_ctx* ctx, const char* who, const float* x, const int32_t* n_in, int B, int S, const float* semitones,
+                 const float* formants, float* y) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!x || !y || B < 1 || B > 65535 || S < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: bad argument (B=%d S=%d)", who, B, S);
-  int rc = ps_check_shifts(ctx, who, semitones, B);
-  if (!rc) rc = ps_check_formants(ctx, who, formants, B);
-  if (!rc) rc = host_lengths_check(ctx, who, n_in, B, S);
+  std::vector<PsShift> h;
+  std::vector<float> ratio;
+  int rc = ps_args(ctx, who, B, S, semitones, formants, &h, &ratio);
   if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, (size_t)B * 4), o_y = hs.out(x_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = ps_call(ctx, dev_who, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, semitones, formants,
-                 hs.dev<float>(o_y), nullptr, hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, x_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows(who, x, n_in, B, S, y != nullptr);
+  if (rc) return rc;
+  const size_t o_y = hs.out((size_t)B * S * 4, y);
+  return hs.run([&](cudaStream_t st) { return ps_one_shot(ctx, hs.x(), hs.n(), B, S, h, S / HOP + 1, S, hs.dev<float>(o_y), nullptr, st, ratio); });
 }
 
 // frames of the longest time-stretched row of S samples: max over the rows of M(S) / 256 + 1
@@ -582,15 +586,25 @@ long long ts_frames(const float* tempo, int B, int S) {
   return F;
 }
 
+// the batch shape, output row length Sy and per-row parameters h of a one-shot call of entry point `who`
+int ts_args(vtts_ctx* ctx, const char* who, int B, int S, const float* tempo, int Sy, std::vector<PsShift>* h) {
+  int rc = batch_check(ctx, who, B, S, S_ANY);
+  if (!rc && Sy < 1) rc = ctx->fail(VTTS_ERR_BAD_ARG, "%s: Sy=%d (>= 1)", who, Sy);
+  if (!rc) rc = ts_check_tempos(ctx, who, tempo, B);
+  if (rc) return rc;
+  h->resize(B);
+  for (int b = 0; b < B; ++b) (*h)[b] = ts_params(tempo[b]);
+  return VTTS_OK;
+}
+
 int ts_call(vtts_ctx* ctx, const char* who, const float* x_dev, const int32_t* n_dev, int B, int S, const float* tempo, float* y_dev, int Sy,
             int* dec_dev, cudaStream_t st) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = ps_check_call(ctx, who, x_dev, y_dev ? (const void*)y_dev : (const void*)dec_dev, y_dev, B, S);
-  if (!rc && y_dev && Sy < 1) rc = ctx->fail(VTTS_ERR_BAD_ARG, "%s: Sy=%d (>= 1)", who, Sy);
-  if (!rc) rc = ts_check_tempos(ctx, who, tempo, B);
+  std::vector<PsShift> h;
+  int rc = ts_args(ctx, who, B, S, tempo, y_dev ? Sy : 1, &h);   // the decisions hook has no output rows
+  if (!rc) rc = ps_pointers(ctx, who, x_dev, y_dev, dec_dev);
   if (rc) return rc;
-  std::vector<PsShift> h(B);
-  for (int b = 0; b < B; ++b) h[b] = ts_params(tempo[b]);
+  VTTS_CUDA(cudaSetDevice(ctx->device));
   return ps_one_shot(ctx, x_dev, n_dev, B, S, h, ts_frames(tempo, B, S), Sy, y_dev, dec_dev, st);
 }
 
@@ -617,12 +631,12 @@ int vtts_debug_pitch_decisions(vtts_ctx* ctx, const float* x_dev, const int32_t*
 }
 
 int vtts_pitch_shift_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, const float* semitones, float* y) {
-  return ps_call_host(ctx, "pitch_shift_host", "pitch_shift", x, n_in, B, S, semitones, nullptr, y);
+  return ps_call_host(ctx, "pitch_shift_host", x, n_in, B, S, semitones, nullptr, y);
 }
 
 int vtts_voice_shift_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, const float* semitones, const float* formants,
                           float* y) {
-  return ps_call_host(ctx, "voice_shift_host", "voice_shift", x, n_in, B, S, semitones, formants, y);
+  return ps_call_host(ctx, "voice_shift_host", x, n_in, B, S, semitones, formants, y);
 }
 
 int64_t vtts_time_stretch_length(int64_t n, float tempo) { return n < 0 || !tempo_ok(tempo) ? -1 : ts_len(n, tempo); }
@@ -643,21 +657,16 @@ int vtts_debug_time_stretch_decisions(vtts_ctx* ctx, const float* x_dev, const i
 
 int vtts_time_stretch_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, const float* tempo, float* y, int Sy) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!x || !y || B < 1 || B > 65535 || S < 1 || Sy < 1)
-    return ctx->fail(VTTS_ERR_BAD_ARG, "time_stretch_host: bad argument (B=%d S=%d Sy=%d)", B, S, Sy);
-  int rc = ts_check_tempos(ctx, "time_stretch_host", tempo, B);
-  if (!rc) rc = host_lengths_check(ctx, "time_stretch_host", n_in, B, S);
+  std::vector<PsShift> h;
+  int rc = ts_args(ctx, "time_stretch_host", B, S, tempo, Sy, &h);
   if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4, y_b = (size_t)B * Sy * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, (size_t)B * 4), o_y = hs.out(y_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = vtts_time_stretch(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, tempo, hs.dev<float>(o_y), Sy,
-                           hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, y_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("time_stretch_host", x, n_in, B, S, y != nullptr);
+  if (rc) return rc;
+  const size_t o_y = hs.out((size_t)B * Sy * 4, y);
+  return hs.run([&](cudaStream_t st) {
+    return ps_one_shot(ctx, hs.x(), hs.n(), B, S, h, ts_frames(tempo, B, S), Sy, hs.dev<float>(o_y), nullptr, st);
+  });
 }
 
 // ---- streams ---------------------------------------------------------------------------------------------------
@@ -689,13 +698,10 @@ namespace {
 template <class Stream>
 int pv_create(vtts_ctx* ctx, const char* who, int max_streams, int max_chunk_samples, bool stretch, Stream** out, int* out_pitch) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out || !out_pitch) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: null pointer", who);
-  *out = nullptr;
-  if (max_streams < 1 || max_streams > 65535 || max_chunk_samples < 1 || max_chunk_samples > (1 << 22))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "%s: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", who, max_streams, max_chunk_samples,
-                     1 << 22);
+  int rc = create_check(ctx, who, out, out_pitch != nullptr, max_streams, max_chunk_samples);
+  if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
-  int rc = vtts_fft_tables(ctx);
+  rc = vtts_fft_tables(ctx);
   if (rc) return rc;
   const int S = max_streams;
   std::unique_ptr<Stream> ps(new Stream(ctx, S, max_chunk_samples, PS_K));
@@ -874,17 +880,6 @@ int pv_push(vtts_ctx* ctx, const char* who, PvStream* ps, const float* x_dev, co
   return VTTS_OK;
 }
 
-int pv_push_host(vtts_ctx* ctx, const char* who, PvStream* ps, const float* x, const int32_t* n_new, const uint8_t* flags, const float* par,
-                 const float* fmt, float* y, int32_t* n_out, const char* push_who) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = stream_args(ctx, who, ps, x && y);
-  if (rc) return rc;
-  return stream_push_host(ctx, x, (size_t)ps->S * ps->F * 4, y, (size_t)ps->S * ps->out_pitch * 4,
-                          [&](const float* x_dev, float* y_dev, cudaStream_t st) {
-                            return pv_push(ctx, push_who, ps, x_dev, n_new, flags, par, fmt, y_dev, n_out, st);
-                          });
-}
-
 }  // namespace
 
 int vtts_pitch_shift_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, vtts_pitch_shift_stream** out, int* out_pitch) {
@@ -902,7 +897,14 @@ int vtts_pitch_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, con
 
 int vtts_pitch_shift_stream_push_host(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x, const int32_t* n_new, const uint8_t* flags,
                                       const float* semitones, float* y, int32_t* n_out) {
-  return pv_push_host(ctx, "pitch_shift_stream_push_host", ps, x, n_new, flags, semitones, nullptr, y, n_out, "pitch_shift_stream_push");
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  const int rc = stream_args(ctx, "pitch_shift_stream_push_host", ps, x && y);
+  if (rc) return rc;
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, (size_t)ps->S * ps->F * 4), o_y = hs.out((size_t)ps->S * ps->out_pitch * 4, y);
+  return hs.run([&](cudaStream_t st) {
+    return pv_push(ctx, "pitch_shift_stream_push", ps, hs.dev<const float>(o_x), n_new, flags, semitones, nullptr, hs.dev<float>(o_y), n_out, st);
+  });
 }
 
 int vtts_voice_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x_dev, const int32_t* n_new, const uint8_t* flags,
@@ -912,7 +914,14 @@ int vtts_voice_shift_stream_push(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, con
 
 int vtts_voice_shift_stream_push_host(vtts_ctx* ctx, vtts_pitch_shift_stream* ps, const float* x, const int32_t* n_new, const uint8_t* flags,
                                       const float* semitones, const float* formants, float* y, int32_t* n_out) {
-  return pv_push_host(ctx, "voice_shift_stream_push_host", ps, x, n_new, flags, semitones, formants, y, n_out, "voice_shift_stream_push");
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  const int rc = stream_args(ctx, "voice_shift_stream_push_host", ps, x && y);
+  if (rc) return rc;
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, (size_t)ps->S * ps->F * 4), o_y = hs.out((size_t)ps->S * ps->out_pitch * 4, y);
+  return hs.run([&](cudaStream_t st) {
+    return pv_push(ctx, "voice_shift_stream_push", ps, hs.dev<const float>(o_x), n_new, flags, semitones, formants, hs.dev<float>(o_y), n_out, st);
+  });
 }
 
 int vtts_time_stretch_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, vtts_time_stretch_stream** out, int* out_pitch) {
@@ -930,5 +939,12 @@ int vtts_time_stretch_stream_push(vtts_ctx* ctx, vtts_time_stretch_stream* ts, c
 
 int vtts_time_stretch_stream_push_host(vtts_ctx* ctx, vtts_time_stretch_stream* ts, const float* x, const int32_t* n_new,
                                        const uint8_t* flags, const float* tempo, float* y, int32_t* n_out) {
-  return pv_push_host(ctx, "time_stretch_stream_push_host", ts, x, n_new, flags, tempo, nullptr, y, n_out, "time_stretch_stream_push");
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  const int rc = stream_args(ctx, "time_stretch_stream_push_host", ts, x && y);
+  if (rc) return rc;
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, (size_t)ts->S * ts->F * 4), o_y = hs.out((size_t)ts->S * ts->out_pitch * 4, y);
+  return hs.run([&](cudaStream_t st) {
+    return pv_push(ctx, "time_stretch_stream_push", ts, hs.dev<const float>(o_x), n_new, flags, tempo, nullptr, hs.dev<float>(o_y), n_out, st);
+  });
 }

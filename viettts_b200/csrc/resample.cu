@@ -251,39 +251,48 @@ int vtts_resample_filter(int in_rate, int out_rate, double* taps, int capacity) 
   return (int)h.size();
 }
 
+namespace {
+
+// the rates and batch shape of a one-shot call of entry point `who`
+int rs_args(vtts_ctx* ctx, const char* who, int B, int S_in, int in_rate, int out_rate, RsRatio* r) {
+  if (rs_ratio(in_rate, out_rate, r))
+    return ctx->fail(VTTS_ERR_BAD_ARG, "%s: rates %d -> %d (positive, reduced ratio up / down <= %d)", who, in_rate, out_rate, RS_MAX_FACTOR);
+  return batch_check(ctx, who, B, S_in, S_ANY);
+}
+
+long long rs_out_samples(const RsRatio& r, int S_in) { return ceil_div((long long)S_in * r.up, r.down); }
+
+int rs_oneshot(vtts_ctx* ctx, const RsRatio& r, const float* x, const int32_t* n_in, int B, int S_in, float* y, cudaStream_t st) {
+  const float* taps = nullptr;
+  const int rc = rs_filter(ctx, r, &taps);
+  if (rc) return rc;
+  const long long S_out = rs_out_samples(r, S_in);
+  return rs_launch(ctx, r, taps, x, S_in, S_in, n_in, nullptr, B, S_out, S_out, y, S_out, st);
+}
+
+}  // namespace
+
 int vtts_resample(vtts_ctx* ctx, const float* x_dev, const int32_t* n_in_dev, int B, int S_in, int in_rate, int out_rate, float* y_dev,
                   void* stream) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   RsRatio r;
-  if (rs_ratio(in_rate, out_rate, &r))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "resample: rates %d -> %d (positive, reduced ratio up / down <= %d)", in_rate, out_rate, RS_MAX_FACTOR);
-  if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "resample: null pointer");
-  if (B < 1 || B > 65535 || S_in < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "resample: B=%d S_in=%d (1..65535, >= 1)", B, S_in);
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const float* taps = nullptr;
-  int rc = rs_filter(ctx, r, &taps);
+  const int rc = rs_args(ctx, "resample", B, S_in, in_rate, out_rate, &r);
   if (rc) return rc;
-  const long long S_out = ceil_div((long long)S_in * r.up, r.down);
-  return rs_launch(ctx, r, taps, x_dev, S_in, S_in, n_in_dev, nullptr, B, S_out, S_out, y_dev, S_out, (cudaStream_t)stream);
+  if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "resample: null pointer");
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  return rs_oneshot(ctx, r, x_dev, n_in_dev, B, S_in, y_dev, (cudaStream_t)stream);
 }
 
 int vtts_resample_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S_in, int in_rate, int out_rate, float* y) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   RsRatio r;
-  if (rs_ratio(in_rate, out_rate, &r))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "resample_host: rates %d -> %d (positive, reduced ratio up / down <= %d)", in_rate, out_rate,
-                     RS_MAX_FACTOR);
-  if (!x || !y || B < 1 || B > 65535 || S_in < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_host: bad argument");
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t y_b = (size_t)B * ceil_div((long long)S_in * r.up, r.down) * 4;
+  int rc = rs_args(ctx, "resample_host", B, S_in, in_rate, out_rate, &r);
+  if (rc) return rc;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, (size_t)B * S_in * 4), o_n = hs.in(n_in, (size_t)B * 4), o_y = hs.out(y_b);
-  int rc = hs.upload();
-  if (!rc)
-    rc = vtts_resample(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S_in, in_rate, out_rate,
-                       hs.dev<float>(o_y), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, y_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("resample_host", x, n_in, B, S_in, y != nullptr);
+  if (rc) return rc;
+  const size_t o_y = hs.out((size_t)B * rs_out_samples(r, S_in) * 4, y);
+  return hs.run([&](cudaStream_t st) { return rs_oneshot(ctx, r, hs.x(), hs.n(), B, S_in, hs.dev<float>(o_y), st); });
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
@@ -303,21 +312,18 @@ int vtts_resample_stream_lookahead(int in_rate, int out_rate) {
 int vtts_resample_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int in_rate, int out_rate,
                                 vtts_resample_stream** out, int* out_pitch) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out || !out_pitch) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_create: null output pointer");
-  *out = nullptr;
+  int rc = create_check(ctx, "resample_stream_create", out, out_pitch != nullptr, max_streams, max_chunk_samples);
+  if (rc) return rc;
   RsRatio r;
   if (rs_ratio(in_rate, out_rate, &r))
     return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_create: rates %d -> %d (positive, reduced ratio up / down <= %d)", in_rate, out_rate,
                      RS_MAX_FACTOR);
-  if (max_streams < 1 || max_streams > 65535 || max_chunk_samples < 1 || max_chunk_samples > (1 << 22))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_create: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", max_streams,
-                     max_chunk_samples, 1 << 22);
   // outputs per push: fewer than (n_new * up + half + 1) / down + 1 (see the schedule in vtts_resample_stream_push)
   const long long pitch = ceil_div((long long)max_chunk_samples * r.up + r.half + 1, r.down);
   if (pitch > (1LL << 30)) return ctx->fail(VTTS_ERR_BAD_ARG, "resample_stream_create: %lld outputs per push", pitch);
   VTTS_CUDA(cudaSetDevice(ctx->device));
   const float* taps = nullptr;
-  int rc = rs_filter(ctx, r, &taps);
+  rc = rs_filter(ctx, r, &taps);
   if (rc) return rc;
   std::unique_ptr<vtts_resample_stream> rs(new vtts_resample_stream(ctx, max_streams, max_chunk_samples, r.T - 1));
   rs->r = r;
@@ -378,10 +384,11 @@ int vtts_resample_stream_push(vtts_ctx* ctx, vtts_resample_stream* rs, const flo
 int vtts_resample_stream_push_host(vtts_ctx* ctx, vtts_resample_stream* rs, const float* x, const int32_t* n_new, const uint8_t* flags,
                                    float* y, int32_t* n_out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = stream_args(ctx, "resample_stream_push_host", rs, x && y);
+  const int rc = stream_args(ctx, "resample_stream_push_host", rs, x && y);
   if (rc) return rc;
-  return stream_push_host(ctx, x, (size_t)rs->S * rs->F * 4, y, (size_t)rs->S * rs->out_pitch * 4,
-                          [&](const float* x_dev, float* y_dev, cudaStream_t st) {
-                            return vtts_resample_stream_push(ctx, rs, x_dev, n_new, flags, y_dev, n_out, st);
-                          });
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, (size_t)rs->S * rs->F * 4), o_y = hs.out((size_t)rs->S * rs->out_pitch * 4, y);
+  return hs.run([&](cudaStream_t st) {
+    return vtts_resample_stream_push(ctx, rs, hs.dev<const float>(o_x), n_new, flags, hs.dev<float>(o_y), n_out, st);
+  });
 }

@@ -258,19 +258,14 @@ int rv_launch(vtts_ctx* ctx, const float* x, long long x_ld, int S, const int* n
   return VTTS_OK;
 }
 
-}  // namespace
+// the parameters and batch shape of a one-shot call of entry point `who`
+int rv_args(vtts_ctx* ctx, const char* who, int B, int S, int rate, int L, float mix) {
+  const int rc = batch_check(ctx, who, B, S, S_ANY);
+  return rc ? rc : rv_check(ctx, who, rate, L, mix);
+}
 
-int vtts_reverb_stream_lookahead(void) { return RV_LOOKAHEAD; }
-
-int vtts_reverb(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, const float* ir_dev, int L, float mix,
-                float* y_dev, void* stream) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!x_dev || !y_dev || !ir_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "reverb: null pointer");
-  if (B < 1 || B > 65535 || S < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "reverb: B=%d S=%d (1..65535, >= 1)", B, S);
-  int rc = rv_check(ctx, "reverb", rate, L, mix);
-  if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  rc = vtts_fft_tables(ctx);
+int rv_oneshot(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, const float* ir, int L, float mix, float* y, cudaStream_t st) {
+  int rc = vtts_fft_tables(ctx);
   if (rc) return rc;
   const int K = partitions(L);
   const long long nbS = ((long long)S + BLK - 1) / BLK;
@@ -287,29 +282,35 @@ int vtts_reverb(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, 
   if (rc) return rc;
   Arena a(ctx->ws, m.off, false);
   carve(a, &H, &X, &Y);
-  cudaStream_t st = (cudaStream_t)stream;
-  rc = rv_ir(ctx, ir_dev, L, H, st);
+  rc = rv_ir(ctx, ir, L, H, st);
   if (rc) return rc;
-  return rv_launch(ctx, x_dev, S, S, n_dev, nullptr, B, nbS, S, H, K, X, R, Y, ycap, mix, y_dev, S, st);
+  return rv_launch(ctx, x, S, S, n_in, nullptr, B, nbS, S, H, K, X, R, Y, ycap, mix, y, S, st);
+}
+
+}  // namespace
+
+int vtts_reverb_stream_lookahead(void) { return RV_LOOKAHEAD; }
+
+int vtts_reverb(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, const float* ir_dev, int L, float mix,
+                float* y_dev, void* stream) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  const int rc = rv_args(ctx, "reverb", B, S, rate, L, mix);
+  if (rc) return rc;
+  if (!x_dev || !y_dev || !ir_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "reverb: null pointer");
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  return rv_oneshot(ctx, x_dev, n_dev, B, S, ir_dev, L, mix, y_dev, (cudaStream_t)stream);
 }
 
 int vtts_reverb_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, const float* ir, int L, float mix, float* y) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!x || !y || !ir || B < 1 || B > 65535 || S < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "reverb_host: bad argument (B=%d S=%d)", B, S);
-  int rc = rv_check(ctx, "reverb_host", rate, L, mix);
-  if (!rc) rc = rv_check_ir(ctx, "reverb_host", ir, L);
-  if (!rc) rc = host_lengths_check(ctx, "reverb_host", n_in, B, S);
+  int rc = rv_args(ctx, "reverb_host", B, S, rate, L, mix);
   if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, (size_t)B * 4), o_h = hs.in(ir, (size_t)L * 4), o_y = hs.out(x_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = vtts_reverb(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, rate, hs.dev<const float>(o_h), L,
-                     mix, hs.dev<float>(o_y), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, x_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("reverb_host", x, n_in, B, S, y && ir);
+  if (!rc) rc = rv_check_ir(ctx, "reverb_host", ir, L);
+  if (rc) return rc;
+  const size_t o_h = hs.in(ir, (size_t)L * 4), o_y = hs.out((size_t)B * S * 4, y);
+  return hs.run([&](cudaStream_t st) { return rv_oneshot(ctx, hs.x(), hs.n(), B, S, hs.dev<const float>(o_h), L, mix, hs.dev<float>(o_y), st); });
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
@@ -326,12 +327,9 @@ struct vtts_reverb_stream : SampleStream<RvRow> {
 int vtts_reverb_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, int rate, const float* ir, int L, float mix,
                               vtts_reverb_stream** out, int* out_pitch) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out || !out_pitch || !ir) return ctx->fail(VTTS_ERR_BAD_ARG, "reverb_stream_create: null pointer");
-  *out = nullptr;
-  if (max_streams < 1 || max_streams > 65535 || max_chunk_samples < 1 || max_chunk_samples > (1 << 22))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "reverb_stream_create: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", max_streams,
-                     max_chunk_samples, 1 << 22);
-  int rc = rv_check(ctx, "reverb_stream_create", rate, L, mix);
+  int rc = create_check(ctx, "reverb_stream_create", out, out_pitch && ir, max_streams, max_chunk_samples);
+  if (rc) return rc;
+  rc = rv_check(ctx, "reverb_stream_create", rate, L, mix);
   if (!rc) rc = rv_check_ir(ctx, "reverb_stream_create", ir, L);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
@@ -414,10 +412,11 @@ int vtts_reverb_stream_push(vtts_ctx* ctx, vtts_reverb_stream* rs, const float* 
 int vtts_reverb_stream_push_host(vtts_ctx* ctx, vtts_reverb_stream* rs, const float* x, const int32_t* n_new, const uint8_t* flags, float* y,
                                  int32_t* n_out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = stream_args(ctx, "reverb_stream_push_host", rs, x && y);
+  const int rc = stream_args(ctx, "reverb_stream_push_host", rs, x && y);
   if (rc) return rc;
-  return stream_push_host(ctx, x, (size_t)rs->S * rs->F * 4, y, (size_t)rs->S * rs->out_pitch * 4,
-                          [&](const float* x_dev, float* y_dev, cudaStream_t st) {
-                            return vtts_reverb_stream_push(ctx, rs, x_dev, n_new, flags, y_dev, n_out, st);
-                          });
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, (size_t)rs->S * rs->F * 4), o_y = hs.out((size_t)rs->S * rs->out_pitch * 4, y);
+  return hs.run([&](cudaStream_t st) {
+    return vtts_reverb_stream_push(ctx, rs, hs.dev<const float>(o_x), n_new, flags, hs.dev<float>(o_y), n_out, st);
+  });
 }

@@ -1,6 +1,7 @@
 // Host-side pieces shared by the per-slot streams and the *_host entry points: the slot protocol of a push, the device
 // memory of a stream, the window and push tables of a sample stream, and the staging of host buffers.
 #pragma once
+#include <climits>
 #include <memory>
 #include <tuple>
 
@@ -145,6 +146,18 @@ inline int stream_args(vtts_ctx* ctx, const char* who, const StreamBase* sb, boo
   return VTTS_OK;
 }
 
+// the rejections every stream create shares: a null handle or other pointer the create needs (pointers_ok false), then
+// the slot count and the largest chunk; *out is null on every failure
+template <class Stream>
+int create_check(vtts_ctx* ctx, const char* who, Stream** out, bool pointers_ok, int max_streams, int max_chunk, int chunk_max = 1 << 22,
+                 const char* chunk = "max_chunk_samples", int streams_max = 65535) {
+  if (!out || !pointers_ok) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: null pointer", who);
+  *out = nullptr;
+  if (max_streams < 1 || max_streams > streams_max || max_chunk < 1 || max_chunk > chunk_max)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "%s: max_streams=%d %s=%d (1..%d, 1..%d)", who, max_streams, chunk, max_chunk, streams_max, chunk_max);
+  return VTTS_OK;
+}
+
 template <class Stream>
 int stream_destroy(vtts_ctx* ctx, const char* who, Stream* sb) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
@@ -156,12 +169,24 @@ int stream_destroy(vtts_ctx* ctx, const char* who, Stream* sb) {
   return VTTS_OK;
 }
 
+// ---- batch shape -------------------------------------------------------------------------------------------------
+// The one-shot audio entry points take B rows of S samples.  B rides on a grid's y dimension (at most 65535).  S runs
+// from S_min (1, or 0 where an empty row has a meaning) to the stage's S_max, given by the stage beside its reason.
+constexpr long long S_ANY = INT_MAX;   // no ceiling beyond an int sample count
+
+inline int batch_check(vtts_ctx* ctx, const char* who, int B, int S, long long S_max, int S_min = 1) {
+  if (B < 1 || B > 65535 || S < S_min || S > S_max)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "%s: B=%d S=%d (B in 1..65535, S in %d..%lld)", who, B, S, S_min, S_max);
+  return VTTS_OK;
+}
+
 // ---- host staging ------------------------------------------------------------------------------------------------
 // The *_host entry points run the device call on the context's own stream with their buffers staged at the same
 // offsets in the pinned host buffer (ctx->hpin) and the device staging buffer (ctx->dstage): inputs first, then
-// outputs, then device-only scratch, each block 256 B aligned.  Declare every block, then upload(): it sizes the
-// buffers, packs the inputs and queues one H2D of the input span.  From then on the stream is synchronised on every
-// exit, so no copy from or into the pinned buffer outlives the call (the next call rewrites it).
+// outputs, then device-only scratch, each block 256 B aligned.  Declare every block, then run(launch): it sizes the
+// buffers, packs the inputs, queues one H2D of the input span, launch(stream), the D2H of every output that has a host
+// destination, and waits.  From upload() on the stream is synchronised on every exit, so no copy from or into the
+// pinned buffer outlives the call (the next call rewrites it).
 class HostStage {
  public:
   explicit HostStage(vtts_ctx* c) : ctx(c), st(c->own_stream) {}
@@ -178,13 +203,47 @@ class HostStage {
     in_end = off;
     return o;
   }
-  size_t out(size_t bytes) {
+  // an output block of `bytes`, fetched into `dst` by run() (null: not fetched)
+  size_t out(size_t bytes, void* dst = nullptr) {
     const size_t o = take(bytes);
     host_end = off;
+    if (dst) fetched.push_back({o, dst, bytes});
     return o;
   }
   size_t scratch(size_t bytes) { return take(bytes); }
 
+  // the batch x [B][S] of `elem`-byte samples and its row lengths n [B] (null: every row full) of host entry point
+  // `who`, staged as the first inputs: a null x with samples to stage, any other null pointer the call needs
+  // (pointers_ok false) and any n[b] outside [0, S] are rejected
+  int rows(const char* who, const void* x, const int32_t* n, int B, int S, bool pointers_ok = true, size_t elem = 4) {
+    if ((!x && S) || !pointers_ok) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: null pointer", who);
+    if (n)
+      for (int b = 0; b < B; ++b)
+        if (n[b] < 0 || n[b] > S) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: n[%d]=%d outside [0, %d]", who, b, n[b], S);
+    o_x = in(x, (size_t)B * S * elem);
+    o_n = n ? in(n, (size_t)B * 4) : SIZE_MAX;
+    return VTTS_OK;
+  }
+  // the staged batch and lengths (null when the call has none)
+  template <class T = float>
+  const T* x() const { return dev<const T>(o_x); }
+  const int32_t* n() const { return o_n == SIZE_MAX ? nullptr : dev<const int32_t>(o_n); }
+
+  template <class T>
+  T* dev(size_t o) const { return reinterpret_cast<T*>((char*)ctx->dstage + o); }
+
+  template <class Launch>
+  int run(Launch&& launch) {
+    VTTS_CUDA(cudaSetDevice(ctx->device));
+    int rc = upload();
+    if (!rc) rc = launch(st);
+    for (const Out& u : fetched)
+      if (!rc) rc = fetch(u.o, u.dst, u.bytes);
+    return rc ? rc : finish();
+  }
+
+  // the explicit steps, for calls that wait or fetch between launches (fetch and finish may follow run, for outputs
+  // whose size the launch decides)
   int upload() {
     int rc = ctx->ensure_staging(std::max(in_end, host_end), off);
     if (rc) return rc;
@@ -195,14 +254,11 @@ class HostStage {
     if (in_end) VTTS_CUDA(cudaMemcpyAsync(ctx->dstage, hp, in_end, cudaMemcpyHostToDevice, st));
     return VTTS_OK;
   }
-
-  template <class T>
-  T* dev(size_t o) const { return reinterpret_cast<T*>((char*)ctx->dstage + o); }
-
   // queues the D2H of `bytes` at output offset o into dst: straight into it when `direct` (page-locked caller memory),
   // else through the pinned buffer, copied out by finish()
   int fetch(size_t o, void* dst, size_t bytes, bool direct = false) {
     VTTS_CUDA(cudaMemcpyAsync(direct ? dst : (char*)ctx->hpin + o, (char*)ctx->dstage + o, bytes, cudaMemcpyDeviceToHost, st));
+    queued = true;
     if (!direct) outs.push_back({o, dst, bytes});
     return VTTS_OK;
   }
@@ -210,6 +266,7 @@ class HostStage {
     VTTS_CUDA(cudaStreamSynchronize(st));
     queued = false;
     for (const Out& u : outs) memcpy(u.dst, (char*)ctx->hpin + u.o, u.bytes);
+    outs.clear();
     return VTTS_OK;
   }
 
@@ -225,29 +282,8 @@ class HostStage {
     off += bytes;
     return o;
   }
-  size_t off = 0, in_end = 0, host_end = 0;
+  size_t off = 0, in_end = 0, host_end = 0, o_x = 0, o_n = SIZE_MAX;
   bool queued = false;
   std::vector<In> ins;
-  std::vector<Out> outs;
+  std::vector<Out> fetched, outs;   // declared by out(), queued by fetch()
 };
-
-// the row lengths n[b] of a *_host entry point `who` (null: every row full), each in [0, S]
-inline int host_lengths_check(vtts_ctx* ctx, const char* who, const int32_t* n, int B, int S) {
-  if (n)
-    for (int b = 0; b < B; ++b)
-      if (n[b] < 0 || n[b] > S) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: n[%d]=%d outside [0, %d]", who, b, n[b], S);
-  return VTTS_OK;
-}
-
-// push_host of a stream: the x_bytes of host input x are staged, push(x_dev, y_dev, stream) runs the stream's device
-// push on the staged buffers, and the y_bytes of its output come back to host memory y
-template <class Push>
-int stream_push_host(vtts_ctx* ctx, const float* x, size_t x_bytes, float* y, size_t y_bytes, Push&& push) {
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_bytes), o_y = hs.out(y_bytes);
-  int rc = hs.upload();
-  if (!rc) rc = push(hs.dev<const float>(o_x), hs.dev<float>(o_y), hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, y_bytes);
-  return rc ? rc : hs.finish();
-}

@@ -207,12 +207,9 @@ int vtts_vocoder_stream_lookahead(void) { return plan().D; }
 
 int vtts_vocoder_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_frames, vtts_vocoder_stream** out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out) return ctx->fail(VTTS_ERR_BAD_ARG, "vocoder_stream_create: null output pointer");
-  *out = nullptr;
+  int rc = create_check(ctx, "vocoder_stream_create", out, true, max_streams, max_chunk_frames, 4096, "max_chunk_frames");
+  if (rc) return rc;
   if (!ctx->hg.loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "vocoder_stream_create: hifigan weights not loaded");
-  if (max_streams < 1 || max_streams > 65535 || max_chunk_frames < 1 || max_chunk_frames > 4096)
-    return ctx->fail(VTTS_ERR_BAD_ARG, "vocoder_stream_create: max_streams=%d max_chunk_frames=%d (1..65535, 1..4096)", max_streams,
-                     max_chunk_frames);
   VTTS_CUDA(cudaSetDevice(ctx->device));
   const Plan& pl = plan();
   std::unique_ptr<vtts_vocoder_stream> vs(new vtts_vocoder_stream(ctx, max_streams, max_chunk_frames));
@@ -229,7 +226,7 @@ int vtts_vocoder_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_fra
         shape(ti_y(i, j, m), C, i + 1, pl.lag_y[i][j][m]);
       }
   }
-  int rc = stream_alloc(ctx, "vocoder_stream_create", *vs, [&](Arena& a) {
+  rc = stream_alloc(ctx, "vocoder_stream_create", *vs, [&](Arena& a) {
     for (int t = 0; t < NTEN; ++t) vs->ten[t].p = a.take<float>((size_t)max_streams * vs->ten[t].cap * vs->ten[t].C);
     vs->d_ten = a.take<StreamTen>(NTEN);
   });
@@ -418,10 +415,11 @@ int vtts_vocoder_stream_push(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float
 int vtts_vocoder_stream_push_host(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float* mel, const int32_t* n_new, const uint8_t* flags,
                                   float* wav, int32_t* n_out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = stream_args(ctx, "vocoder_stream_push_host", vs, mel && wav);
+  const int rc = stream_args(ctx, "vocoder_stream_push_host", vs, mel && wav);
   if (rc) return rc;
-  return stream_push_host(ctx, mel, (size_t)vs->S * vs->F * vc::MEL * 4, wav, (size_t)vs->S * vc::HOP * (vs->F + plan().D) * 4,
-                          [&](const float* mel_dev, float* wav_dev, cudaStream_t st) {
-                            return vtts_vocoder_stream_push(ctx, vs, mel_dev, n_new, flags, wav_dev, n_out, st);
-                          });
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(mel, (size_t)vs->S * vs->F * vc::MEL * 4), o_y = hs.out((size_t)vs->S * vc::HOP * (vs->F + plan().D) * 4, wav);
+  return hs.run([&](cudaStream_t st) {
+    return vtts_vocoder_stream_push(ctx, vs, hs.dev<const float>(o_x), n_new, flags, hs.dev<float>(o_y), n_out, st);
+  });
 }

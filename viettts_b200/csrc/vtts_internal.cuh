@@ -409,6 +409,8 @@ __device__ __forceinline__ float map_apply(const Map& M, float d) { return fmaxf
 // loudness.cu: the context workspace vtts_loudness / vtts_loudness_normalize use for B rows of S samples at `rate`
 // (from the start of ctx->ws)
 size_t vtts_loudness_ws_bytes(int B, int S, int rate);
+// the meter of vtts_loudness on arguments it has checked, on the current device
+int vtts_loudness_launch(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, float* out, cudaStream_t st);
 // denoise.cu: per-row bounds of the STFT frame and overlap-add kernels, which place a row's buffers in absolute time
 constexpr long long DN_OPEN = 1LL << 60;   // row length not known yet (stream slot before END)
 struct DnRow {

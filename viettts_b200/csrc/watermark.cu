@@ -219,68 +219,51 @@ int wm_check_strength(vtts_ctx* ctx, const char* who, float eps) {
   return VTTS_OK;
 }
 
-}  // namespace
+// a row of S samples at `rate` resampled to the detector's rate
+long long det_samples(int S, int rate) {
+  const long long g = std::gcd(rate, DET_RATE);
+  return ((long long)S * (DET_RATE / g) + rate / g - 1) / (rate / g);
+}
 
-int vtts_watermark_stream_lookahead(void) { return stftg::LOOKAHEAD; }
+// the parameters and batch shape of a watermark call of entry point `who`
+int wm_args(vtts_ctx* ctx, const char* who, int B, int S, float strength) {
+  const int rc = batch_check(ctx, who, B, S, S_ANY);
+  return rc ? rc : wm_check_strength(ctx, who, strength);
+}
 
-int vtts_watermark(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, uint64_t key, float strength, float* y_dev,
-                   void* stream) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "watermark: null pointer");
-  if (x_dev == y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "watermark: y must not alias x");
-  if (B < 1 || B > 65535 || S < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "watermark: B=%d S=%d (1..65535, >= 1)", B, S);
-  int rc = wm_check_strength(ctx, "watermark", strength);
-  if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = (cudaStream_t)stream;
+int wm_launch(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, uint64_t key, float strength, float* y, cudaStream_t st) {
   if (strength == 0.f) {
-    wm_copy_kernel<<<dim3((unsigned)((S + 255) / 256), B), 256, 0, st>>>(x_dev, n_dev, S, y_dev);
+    wm_copy_kernel<<<dim3((unsigned)((S + 255) / 256), B), 256, 0, st>>>(x, n_in, S, y);
     ctx->launches++;
     VTTS_CUDA(cudaGetLastError());
     return VTTS_OK;
   }
-  rc = vtts_fft_tables(ctx);
+  int rc = vtts_fft_tables(ctx);
   if (rc) return rc;
   const int ws_frames = S / stftg::HOP + 1;
   rc = ctx->ensure_ws((size_t)B * ws_frames * NF * sizeof(float));
   if (rc) return rc;
-  return stftg::launch(ctx, x_dev, S, S, n_dev, nullptr, B, ws_frames, S, wm_gain(key, strength), (float*)ctx->ws, ws_frames, y_dev, S, st);
+  return stftg::launch(ctx, x, S, S, n_in, nullptr, B, ws_frames, S, wm_gain(key, strength), (float*)ctx->ws, ws_frames, y, S, st);
 }
 
-int vtts_watermark_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, uint64_t key, float strength, float* y) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!x || !y || B < 1 || B > 65535 || S < 1) return ctx->fail(VTTS_ERR_BAD_ARG, "watermark_host: bad argument (B=%d S=%d)", B, S);
-  int rc = wm_check_strength(ctx, "watermark_host", strength);
-  if (!rc) rc = host_lengths_check(ctx, "watermark_host", n_in, B, S);
+// ... and of a detect call; the row at the detector's rate must stay within 2^30 samples
+int det_args(vtts_ctx* ctx, const char* who, int B, int S, int rate, int K) {
+  const int rc = batch_check(ctx, who, B, S, S_ANY);
   if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t x_b = (size_t)B * S * 4;
-  HostStage hs(ctx);
-  const size_t o_x = hs.in(x, x_b), o_n = hs.in(n_in, (size_t)B * 4), o_y = hs.out(x_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = vtts_watermark(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, key, strength, hs.dev<float>(o_y),
-                        hs.st);
-  if (!rc) rc = hs.fetch(o_y, y, x_b);
-  return rc ? rc : hs.finish();
+  if (K < 1 || K > WM_MAX_KEYS) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: K=%d keys (1..%d)", who, K, WM_MAX_KEYS);
+  if (rate < 8000 || rate > 192000 || vtts_resample_filter(rate, DET_RATE, nullptr, 0) < 0)
+    return ctx->fail(VTTS_ERR_BAD_ARG, "%s: rate %d (8000..192000, a ratio to 16000 the resampler takes)", who, rate);
+  if (det_samples(S, rate) > (1LL << 30)) return ctx->fail(VTTS_ERR_BAD_ARG, "%s: S=%d at %d Hz is too long", who, S, rate);
+  return VTTS_OK;
 }
 
-int vtts_watermark_detect(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, const uint64_t* keys_dev, int K,
-                          int search, float* z_dev, int32_t* offset_dev, void* stream) {
-  if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!x_dev || !keys_dev || !z_dev || !offset_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "watermark_detect: null pointer");
-  if (B < 1 || B > 65535 || S < 1 || K < 1 || K > WM_MAX_KEYS)
-    return ctx->fail(VTTS_ERR_BAD_ARG, "watermark_detect: B=%d S=%d K=%d (1..65535, >= 1, 1..%d)", B, S, K, WM_MAX_KEYS);
-  if (rate < 8000 || rate > 192000 || vtts_resample_filter(rate, DET_RATE, nullptr, 0) < 0)
-    return ctx->fail(VTTS_ERR_BAD_ARG, "watermark_detect: rate %d (8000..192000, a ratio to 16000 the resampler takes)", rate);
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = (cudaStream_t)stream;
+int det_launch(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, const uint64_t* keys, int K, int search, float* z,
+               int32_t* offset, cudaStream_t st) {
   int rc = vtts_fft_tables(ctx);
   if (rc) return rc;
   const long long g = std::gcd(rate, DET_RATE);
   const int up = (int)(DET_RATE / g), down = (int)(rate / g);
-  const long long S16 = ((long long)S * up + down - 1) / down;
-  if (S16 > (1LL << 30)) return ctx->fail(VTTS_ERR_BAD_ARG, "watermark_detect: S=%d at %d Hz is too long", S, rate);
+  const long long S16 = det_samples(S, rate);
   const int T_ld = (int)(S16 / DET_HOP + 1), nq = search ? WM_Q : 1, np = search ? WM_P : 1;
   Arena m(nullptr, 0, true);
   auto carve = [&](Arena& a, float** x16, float** D, float** Sf) {
@@ -294,45 +277,74 @@ int vtts_watermark_detect(vtts_ctx* ctx, const float* x_dev, const int32_t* n_de
   if (rc) return rc;
   Arena a((char*)ctx->ws, ctx->ws_bytes, false);
   carve(a, &x16, &D, &Sf);
-  const float* src = x_dev;
+  const float* src = x;
   if (x16) {
-    rc = vtts_resample(ctx, x_dev, n_dev, B, S, rate, DET_RATE, x16, st);
+    rc = vtts_resample_run(ctx, rate, DET_RATE, x, S, S, n_in, nullptr, B, S16, S16, x16, S16, st);
     if (rc) return rc;
     src = x16;
   }
   wm_spec_kernel<<<dim3((unsigned)((T_ld + SPEC_WARPS - 1) / SPEC_WARPS), B), SPEC_WARPS * 32, 0, st>>>(
-      src, x16 ? S16 : S, n_dev, S, up, down, ctx->hann, reinterpret_cast<const float2*>(ctx->fft_tw), D, T_ld);
+      src, x16 ? S16 : S, n_in, S, up, down, ctx->hann, reinterpret_cast<const float2*>(ctx->fft_tw), D, T_ld);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
-  wm_fold_kernel<<<dim3(WM_P, nq, B), FOLD_THREADS, 0, st>>>(D, T_ld, n_dev, S, up, down, Sf);
+  wm_fold_kernel<<<dim3(WM_P, nq, B), FOLD_THREADS, 0, st>>>(D, T_ld, n_in, S, up, down, Sf);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   VTTS_CUDA(cudaFuncSetAttribute(wm_corr_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CORR_SMEM));
-  wm_corr_kernel<<<dim3(K, B), CORR_THREADS, CORR_SMEM, st>>>(Sf, nq, np, keys_dev, z_dev, offset_dev);
+  wm_corr_kernel<<<dim3(K, B), CORR_THREADS, CORR_SMEM, st>>>(Sf, nq, np, keys, z, offset);
   ctx->launches++;
   VTTS_CUDA(cudaGetLastError());
   return VTTS_OK;
 }
 
+}  // namespace
+
+int vtts_watermark_stream_lookahead(void) { return stftg::LOOKAHEAD; }
+
+int vtts_watermark(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, uint64_t key, float strength, float* y_dev,
+                   void* stream) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  const int rc = wm_args(ctx, "watermark", B, S, strength);
+  if (rc) return rc;
+  if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "watermark: null pointer");
+  if (x_dev == y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "watermark: y must not alias x");
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  return wm_launch(ctx, x_dev, n_dev, B, S, key, strength, y_dev, (cudaStream_t)stream);
+}
+
+int vtts_watermark_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, uint64_t key, float strength, float* y) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  int rc = wm_args(ctx, "watermark_host", B, S, strength);
+  if (rc) return rc;
+  HostStage hs(ctx);
+  rc = hs.rows("watermark_host", x, n_in, B, S, y != nullptr);
+  if (rc) return rc;
+  const size_t o_y = hs.out((size_t)B * S * 4, y);
+  return hs.run([&](cudaStream_t st) { return wm_launch(ctx, hs.x(), hs.n(), B, S, key, strength, hs.dev<float>(o_y), st); });
+}
+
+int vtts_watermark_detect(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int S, int rate, const uint64_t* keys_dev, int K,
+                          int search, float* z_dev, int32_t* offset_dev, void* stream) {
+  if (!ctx) return VTTS_ERR_BAD_ARG;
+  const int rc = det_args(ctx, "watermark_detect", B, S, rate, K);
+  if (rc) return rc;
+  if (!x_dev || !keys_dev || !z_dev || !offset_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "watermark_detect: null pointer");
+  VTTS_CUDA(cudaSetDevice(ctx->device));
+  return det_launch(ctx, x_dev, n_dev, B, S, rate, keys_dev, K, search, z_dev, offset_dev, (cudaStream_t)stream);
+}
+
 int vtts_watermark_detect_host(vtts_ctx* ctx, const float* x, const int32_t* n_in, int B, int S, int rate, const uint64_t* keys, int K,
                                int search, float* z, int32_t* offset) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!x || !keys || !z || !offset || B < 1 || B > 65535 || S < 1 || K < 1 || K > WM_MAX_KEYS)
-    return ctx->fail(VTTS_ERR_BAD_ARG, "watermark_detect_host: bad argument (B=%d S=%d K=%d)", B, S, K);
-  int rc = host_lengths_check(ctx, "watermark_detect_host", n_in, B, S);
+  int rc = det_args(ctx, "watermark_detect_host", B, S, rate, K);
   if (rc) return rc;
-  VTTS_CUDA(cudaSetDevice(ctx->device));
-  const size_t out_b = (size_t)B * K * 4;
   HostStage hs(ctx);
-  const size_t o_x = hs.in(x, (size_t)B * S * 4), o_n = hs.in(n_in, (size_t)B * 4), o_k = hs.in(keys, (size_t)K * 8), o_z = hs.out(out_b),
-               o_o = hs.out(out_b);
-  rc = hs.upload();
-  if (!rc)
-    rc = vtts_watermark_detect(ctx, hs.dev<const float>(o_x), n_in ? hs.dev<const int32_t>(o_n) : nullptr, B, S, rate,
-                               hs.dev<const uint64_t>(o_k), K, search, hs.dev<float>(o_z), hs.dev<int32_t>(o_o), hs.st);
-  if (!rc) rc = hs.fetch(o_z, z, out_b);
-  if (!rc) rc = hs.fetch(o_o, offset, out_b);
-  return rc ? rc : hs.finish();
+  rc = hs.rows("watermark_detect_host", x, n_in, B, S, keys && z && offset);
+  if (rc) return rc;
+  const size_t out_b = (size_t)B * K * 4, o_k = hs.in(keys, (size_t)K * 8), o_z = hs.out(out_b, z), o_o = hs.out(out_b, offset);
+  return hs.run([&](cudaStream_t st) {
+    return det_launch(ctx, hs.x(), hs.n(), B, S, rate, hs.dev<const uint64_t>(o_k), K, search, hs.dev<float>(o_z), hs.dev<int32_t>(o_o), st);
+  });
 }
 
 // ---- stream ---------------------------------------------------------------------------------------------------
@@ -345,12 +357,9 @@ struct vtts_watermark_stream : stftg::Stream {
 int vtts_watermark_stream_create(vtts_ctx* ctx, int max_streams, int max_chunk_samples, uint64_t key, float strength,
                                  vtts_watermark_stream** out, int* out_pitch) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  if (!out || !out_pitch) return ctx->fail(VTTS_ERR_BAD_ARG, "watermark_stream_create: null pointer");
-  *out = nullptr;
-  if (max_streams < 1 || max_streams > 65535 || max_chunk_samples < 1 || max_chunk_samples > (1 << 22))
-    return ctx->fail(VTTS_ERR_BAD_ARG, "watermark_stream_create: max_streams=%d max_chunk_samples=%d (1..65535, 1..%d)", max_streams,
-                     max_chunk_samples, 1 << 22);
-  int rc = wm_check_strength(ctx, "watermark_stream_create", strength);
+  int rc = create_check(ctx, "watermark_stream_create", out, out_pitch != nullptr, max_streams, max_chunk_samples);
+  if (rc) return rc;
+  rc = wm_check_strength(ctx, "watermark_stream_create", strength);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
   rc = vtts_fft_tables(ctx);
@@ -385,10 +394,11 @@ int vtts_watermark_stream_push(vtts_ctx* ctx, vtts_watermark_stream* ws, const f
 int vtts_watermark_stream_push_host(vtts_ctx* ctx, vtts_watermark_stream* ws, const float* x, const int32_t* n_new, const uint8_t* flags,
                                     float* y, int32_t* n_out) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
-  int rc = stream_args(ctx, "watermark_stream_push_host", ws, x && y);
+  const int rc = stream_args(ctx, "watermark_stream_push_host", ws, x && y);
   if (rc) return rc;
-  return stream_push_host(ctx, x, (size_t)ws->S * ws->F * 4, y, (size_t)ws->S * ws->out_pitch * 4,
-                          [&](const float* x_dev, float* y_dev, cudaStream_t st) {
-                            return vtts_watermark_stream_push(ctx, ws, x_dev, n_new, flags, y_dev, n_out, st);
-                          });
+  HostStage hs(ctx);
+  const size_t o_x = hs.in(x, (size_t)ws->S * ws->F * 4), o_y = hs.out((size_t)ws->S * ws->out_pitch * 4, y);
+  return hs.run([&](cudaStream_t st) {
+    return vtts_watermark_stream_push(ctx, ws, hs.dev<const float>(o_x), n_new, flags, hs.dev<float>(o_y), n_out, st);
+  });
 }

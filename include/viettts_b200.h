@@ -23,6 +23,14 @@
  *   - one context per GPU; a context is not thread-safe; `*_forward` calls are
  *     stream-ordered and asynchronous, `*_host` calls copy H2D/D2H through pinned
  *     staging owned by the context and return after the result is in host memory.
+ *   - the calls on one context run on the device in the order they are issued,
+ *     whatever stream each is given: a call waits for the context's previous call
+ *     before its first launch (it shares the context's workspace and tile counters),
+ *     so a `*_host` call or a push on one stream may follow a `*_forward` call on
+ *     another without a synchronisation.  A call issued while its stream captures
+ *     a CUDA graph is not ordered this way: order the graph's replays against the
+ *     context's other calls on the stream they run on.  Ordering is not thread
+ *     safety: calls from several threads still need the caller's lock.
  *   - "dev" pointers are device memory owned by the caller (e.g. torch tensors'
  *     data_ptr()), float32 unless stated, dense row-major in the documented shape.
  *   - tensors are NWC ([batch, time, channels]) exactly like the Haiku models.

@@ -240,6 +240,7 @@ int vtts_acoustic_stream_push(vtts_ctx* ctx, vtts_acoustic_stream* as, float* me
   if (!mel_dev || !n_out) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic_stream_push: null pointer");
   if (!ctx->ac.loaded) return ctx->fail(VTTS_ERR_NOT_LOADED, "acoustic_stream_push: acoustic weights not loaded");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
   const int S = as->S, F = as->F;
   // ---- host schedule, fixed before anything is launched ----

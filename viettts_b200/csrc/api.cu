@@ -327,6 +327,11 @@ int vtts_create(int device, vtts_ctx** out) {
     cudaEventCreate(&ctx->ev0[i]);
     cudaEventCreate(&ctx->ev1[i]);
   }
+  if ((e = cudaEventCreateWithFlags(&ctx->tail, cudaEventDisableTiming)) != cudaSuccess) {
+    g_vtts_create_error = std::string("vtts_create: ") + cudaGetErrorString(e);
+    delete ctx;
+    return VTTS_ERR_CUDA;
+  }
   if (cudaMalloc(&ctx->d_err, sizeof(int)) != cudaSuccess || cudaMemset(ctx->d_err, 0, sizeof(int)) != cudaSuccess) {
     g_vtts_create_error = "vtts_create: cannot allocate the error flag";
     delete ctx;
@@ -360,6 +365,7 @@ int vtts_destroy(vtts_ctx* ctx) {
     cudaEventDestroy(ctx->ev0[i]);
     cudaEventDestroy(ctx->ev1[i]);
   }
+  if (ctx->tail) cudaEventDestroy(ctx->tail);
   if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);
   delete ctx;
   return VTTS_OK;
@@ -419,6 +425,7 @@ int vtts_debug_conv1d(vtts_ctx* ctx, int precision, const float* x_dev, const fl
                       float pre_slope, float* out_dev) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, nullptr);
   if (precision == VTTS_PRECISION_FP32) {
     ConvLaunch L;
     memset(&L, 0, sizeof(L));
@@ -493,6 +500,7 @@ int vtts_debug_conv_dispatch(vtts_ctx* ctx, int precision, int nprob, const floa
     return ctx->fail(VTTS_ERR_BAD_ARG, "debug_conv_dispatch: B=%d T=%d Cin=%d Cout=%d k=%d dil=%d post_act=%d", B, T, Cin, Cout, k, dil,
                      post_act);
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, nullptr);
   const size_t inv_bytes = ((size_t)nprob * Cout * sizeof(float) + 255) & ~size_t(255);
   char* tmp = nullptr;
   VTTS_CUDA(cudaMalloc(&tmp, inv_bytes + nprob * vtts_tc_conv_packed_bytes(k, Cin, Cout, false)));
@@ -511,6 +519,7 @@ int vtts_debug_pair(vtts_ctx* ctx, const float* x_dev, const float* w1_dev, cons
                     const float* b2_dev, const int32_t* len_dev, int B, int T, int C, int k, int dil, float slope, float* out_dev) {
   if (!ctx) return VTTS_ERR_BAD_ARG;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, nullptr);
   const bool f16 = ctx->precision == VTTS_PRECISION_FP16;   // the generator's operand format of the context's mode
   void* wpk = nullptr;
   const size_t bytes = vtts_tc_packed_elems(k, C, C, f16) * 2;
@@ -543,6 +552,7 @@ int vtts_broadcast_weights(vtts_ctx* ctx, void* nccl_comm, int root, int is_root
   if (!ctx) return VTTS_ERR_BAD_ARG;
   if (!nccl_comm) return ctx->fail(VTTS_ERR_BAD_ARG, "broadcast_weights: null communicator");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   if (const char* e = nccl_bind()) return ctx->fail(VTTS_ERR_NCCL, "broadcast_weights: %s", e);
   cudaStream_t st = (cudaStream_t)stream;
   auto nccl_ck = [&](int r, const char* what) -> int {
@@ -618,6 +628,7 @@ int vtts_hifigan_forward(vtts_ctx* ctx, const float* mel_dev, const int32_t* n_f
   if (!ctx) return VTTS_ERR_BAD_ARG;
   if (!mel_dev || !wav_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "hifigan_forward: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
   stage_begin(ctx, 0, st);
   int rc = vtts_hifigan_run(ctx, mel_dev, n_frames_dev, B, T, wav_dev, st);
@@ -631,6 +642,7 @@ int vtts_acoustic_forward(vtts_ctx* ctx, const int32_t* tokens_dev, const int32_
   if (!ctx) return VTTS_ERR_BAD_ARG;
   if (!tokens_dev || !dur_frames_dev || !mel_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "acoustic_forward: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
   // the acoustic workspace lives after the hifigan one is released: both share ctx->ws, so a
   // synthesize call sizes it for the larger of the two (see vtts_synthesize_host)
@@ -652,6 +664,7 @@ int vtts_acoustic_teacher_forward(vtts_ctx* ctx, const int32_t* tokens_dev, cons
   int rc = vtts_teacher_mode_check(ctx, dropout_mode, B, N);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
   rc = ctx->ensure_ws(vtts_acoustic_teacher_ws_bytes(B, L, N));
   if (rc) return rc;
@@ -667,6 +680,7 @@ int vtts_duration_forward(vtts_ctx* ctx, const int32_t* tokens_dev, const int32_
   if (!ctx) return VTTS_ERR_BAD_ARG;
   if (!tokens_dev || !dur_sec_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "duration_forward: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
   int rc = ctx->ensure_ws(vtts_duration_ws_bytes(B, L));
   if (rc) return rc;
@@ -680,6 +694,7 @@ int vtts_melspec(vtts_ctx* ctx, const float* wav_dev, int B, int S, float* mel_d
   if (!ctx) return VTTS_ERR_BAD_ARG;
   if (!wav_dev || !mel_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "melspec: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
   stage_begin(ctx, 2, st);
   int rc = vtts_melspec_run(ctx, wav_dev, B, S, mel_dev, st);

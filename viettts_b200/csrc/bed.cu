@@ -210,6 +210,7 @@ int vtts_bed_mix(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B,
   if (rc) return rc;
   if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "bed_mix: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return bd_launch(ctx, d, x_dev, n_dev, B, S, bank_dev, offsets, lengths, bed, y_dev, reduction_db_dev, (cudaStream_t)stream);
 }
 
@@ -297,6 +298,7 @@ int vtts_bed_stream_push(vtts_ctx* ctx, vtts_bed_stream* bs, const float* x_dev,
   });
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
   const int S = bs->S, W = bs->F + bs->d.Tt;
 

@@ -51,6 +51,7 @@ int vtts_compress(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B
   if (rc) return rc;
   if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "compress: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return cp_launch(ctx, p, x_dev, n_dev, B, S, y_dev, reduction_db_dev, (cudaStream_t)stream);
 }
 
@@ -113,6 +114,7 @@ int vtts_compressor_stream_push(vtts_ctx* ctx, vtts_compressor_stream* cs, const
   rc = sl.check(ctx, "compressor_stream_push", cs->F, n_new, flags);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
   const int S = cs->S;
 

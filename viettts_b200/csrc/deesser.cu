@@ -89,6 +89,7 @@ int vtts_deess(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, i
   if (rc) return rc;
   if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "deess: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return ds_launch(ctx, d, x_dev, n_dev, B, S, y_dev, reduction_db_dev, (cudaStream_t)stream);
 }
 
@@ -160,6 +161,7 @@ int vtts_deesser_stream_push(vtts_ctx* ctx, vtts_deesser_stream* ds, const float
   rc = sl.check(ctx, "deesser_stream_push", ds->F, n_new, flags);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
   const int S = ds->S;
 

@@ -148,6 +148,7 @@ int vtts_denoise(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B,
   if (!x_dev || !y_dev || !bias_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise: null pointer");
   if (x_dev == y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise: y must not alias x");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return dn_launch(ctx, x_dev, n_dev, B, S, strength, bias_dev, y_dev, (cudaStream_t)stream);
 }
 
@@ -168,6 +169,7 @@ int vtts_denoise_bias(vtts_ctx* ctx, const float* wav_dev, int n, float* bias_de
   if (!wav_dev || !bias_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_bias: null pointer");
   if (n <= PAD) return ctx->fail(VTTS_ERR_BAD_ARG, "denoise_bias: n=%d (more than %d samples)", n, PAD);
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   int rc = vtts_fft_tables(ctx);
   if (rc) return rc;
   denoise_mag_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(wav_dev, n, ctx->hann, reinterpret_cast<const float2*>(ctx->fft_tw), bias_dev);
@@ -218,6 +220,7 @@ int vtts_denoise_stream_push(vtts_ctx* ctx, vtts_denoise_stream* ds, const float
   if (!rc) rc = ds->slots.check(ctx, "denoise_stream_push", ds->F, n_new, flags);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return ds->push("denoise_stream_push", x_dev, n_new, flags, y_dev, n_out, DnGain{ds->bias, ds->strength}, false, (cudaStream_t)stream);
 }
 

@@ -187,6 +187,7 @@ int vtts_encode(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, 
   if (!rc) rc = coder_apart(ctx, "encode", x_dev, y_dev, B, S, encoding);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return encode_launch(ctx, x_dev, n_dev, B, S, encoding, y_dev, (cudaStream_t)stream);
 }
 
@@ -208,6 +209,7 @@ int vtts_decode(vtts_ctx* ctx, const void* c_dev, const int32_t* n_dev, int B, i
   if (!rc) rc = coder_apart(ctx, "decode", y_dev, c_dev, B, S, encoding);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return decode_launch(ctx, c_dev, n_dev, B, S, encoding, y_dev, (cudaStream_t)stream);
 }
 

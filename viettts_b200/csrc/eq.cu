@@ -142,6 +142,7 @@ int vtts_eq(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, int 
   if (rc) return rc;
   if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "eq: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return eq_launch(ctx, f, x_dev, n_dev, B, S, y_dev, (cudaStream_t)stream);
 }
 
@@ -201,6 +202,7 @@ int vtts_eq_stream_push(vtts_ctx* ctx, vtts_eq_stream* es, const float* x_dev, c
   rc = sl.check(ctx, "eq_stream_push", es->F, n_new, flags);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
   const int S = es->S;
 

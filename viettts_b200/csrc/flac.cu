@@ -779,6 +779,7 @@ int vtts_flac_encode(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, in
   if (!r) r = flac_buffers(ctx, "flac_encode", x_dev, y_dev, nbytes_dev, B, S, y_pitch, bound);
   if (r) return r;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return flac_oneshot(ctx, x_dev, n_dev, B, S, rate, block, rc, y_dev, y_pitch, nbytes_dev, (cudaStream_t)stream);
 }
 
@@ -879,6 +880,7 @@ int vtts_flac_stream_push(vtts_ctx* ctx, vtts_flac_stream* fs, const float* x_de
   });
   if (r) return r;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   std::vector<long long> E1(fs->S);
   for (int s = 0; s < fs->S; ++s) {
     const bool act = SlotState::active(n_new, flags, s), begin = act && (flags[s] & 1), end = act && (flags[s] & 2);

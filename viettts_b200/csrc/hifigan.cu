@@ -398,6 +398,7 @@ int vtts_debug_hifigan_layer(vtts_ctx* ctx, int layer, const float* const* x, fl
   for (int j = 0; j < nout; ++j)
     if (!out[j]) return ctx->fail(VTTS_ERR_BAD_ARG, "debug_hifigan_layer: layer %d needs %d outputs", layer, nout);
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, nullptr);
   if (layer == 0) {
     rc = hg_conv_pre(ctx, x[0], out[0], n_frames, B, T, nullptr);
   } else if (layer <= 4) {

@@ -471,6 +471,7 @@ int vtts_limit(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, const fl
   if (rc) return rc;
   if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "limit: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return lm_launch(ctx, p, rate, x_dev, n_dev, gain_db_dev, B, S, y_dev, reduction_db_dev, (cudaStream_t)stream);
 }
 
@@ -501,6 +502,7 @@ int vtts_loudness_normalize_limited(vtts_ctx* ctx, const float* x_dev, const int
   if (rc) return rc;
   if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_normalize_limited: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return lnl_launch(ctx, p, x_dev, n_dev, B, S, rate, target, y_dev, gain_db_dev, (cudaStream_t)stream);
 }
 
@@ -593,6 +595,7 @@ int vtts_limiter_stream_push(vtts_ctx* ctx, vtts_limiter_stream* ls, const float
   });
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
   const int S = ls->S;
 

@@ -492,6 +492,7 @@ int vtts_loudness(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B
   if (rc) return rc;
   if (!x_dev || !out_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return vtts_loudness_launch(ctx, x_dev, n_dev, B, S, rate, out_dev, (cudaStream_t)stream);
 }
 
@@ -502,6 +503,7 @@ int vtts_loudness_normalize(vtts_ctx* ctx, const float* x_dev, const int32_t* n_
   if (rc) return rc;
   if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "loudness_normalize: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return ln_norm_launch(ctx, x_dev, n_dev, B, S, rate, target, ceiling, y_dev, gain_db_dev, (cudaStream_t)stream);
 }
 
@@ -599,6 +601,7 @@ int vtts_loudness_stream_push(vtts_ctx* ctx, vtts_loudness_stream* ls, const flo
   });
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
 
   // ---- host bookkeeping: the sub-blocks this push completes and the oversampled outputs whose inputs have all arrived

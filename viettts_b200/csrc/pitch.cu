@@ -562,6 +562,7 @@ int ps_call(vtts_ctx* ctx, const char* who, const float* x_dev, const int32_t* n
   if (!rc) rc = ps_pointers(ctx, who, x_dev, y_dev, dec_dev);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, st);
   return ps_one_shot(ctx, x_dev, n_dev, B, S, h, S / HOP + 1, S, y_dev, dec_dev, st, ratio);
 }
 
@@ -605,6 +606,7 @@ int ts_call(vtts_ctx* ctx, const char* who, const float* x_dev, const int32_t* n
   if (!rc) rc = ps_pointers(ctx, who, x_dev, y_dev, dec_dev);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, st);
   return ps_one_shot(ctx, x_dev, n_dev, B, S, h, ts_frames(tempo, B, S), Sy, y_dev, dec_dev, st);
 }
 
@@ -772,6 +774,7 @@ int pv_push(vtts_ctx* ctx, const char* who, PvStream* ps, const float* x_dev, co
   });
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
   const int S = ps->S;
   const SlotState& sl = ps->slots;

@@ -280,6 +280,7 @@ int vtts_resample(vtts_ctx* ctx, const float* x_dev, const int32_t* n_in_dev, in
   if (rc) return rc;
   if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "resample: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return rs_oneshot(ctx, r, x_dev, n_in_dev, B, S_in, y_dev, (cudaStream_t)stream);
 }
 
@@ -348,6 +349,7 @@ int vtts_resample_stream_push(vtts_ctx* ctx, vtts_resample_stream* rs, const flo
   if (!rc) rc = rs->slots.check(ctx, "resample_stream_push", rs->F, n_new, flags);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
   const int S = rs->S;
   const RsRatio& r = rs->r;

@@ -298,6 +298,7 @@ int vtts_reverb(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int B, 
   if (rc) return rc;
   if (!x_dev || !y_dev || !ir_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "reverb: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return rv_oneshot(ctx, x_dev, n_dev, B, S, ir_dev, L, mix, y_dev, (cudaStream_t)stream);
 }
 
@@ -370,6 +371,7 @@ int vtts_reverb_stream_push(vtts_ctx* ctx, vtts_reverb_stream* rs, const float* 
   if (!rc) rc = rs->slots.check(ctx, "reverb_stream_push", rs->F, n_new, flags);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
   const int S = rs->S;
   const SlotState& sl = rs->slots;

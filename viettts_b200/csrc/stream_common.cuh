@@ -186,10 +186,11 @@ inline int batch_check(vtts_ctx* ctx, const char* who, int B, int S, long long S
 // outputs, then device-only scratch, each block 256 B aligned.  Declare every block, then run(launch): it sizes the
 // buffers, packs the inputs, queues one H2D of the input span, launch(stream), the D2H of every output that has a host
 // destination, and waits.  From upload() on the stream is synchronised on every exit, so no copy from or into the
-// pinned buffer outlives the call (the next call rewrites it).
+// pinned buffer outlives the call (the next call rewrites it).  A HostStage is the call's CallOrder scope on the own
+// stream, from its construction, before the first copy, to its destruction, after the last wait.
 class HostStage {
  public:
-  explicit HostStage(vtts_ctx* c) : ctx(c), st(c->own_stream) {}
+  explicit HostStage(vtts_ctx* c) : ctx(c), st(c->own_stream), order(c, c->own_stream) {}
   ~HostStage() {
     if (queued) cudaStreamSynchronize(st);
   }
@@ -282,6 +283,7 @@ class HostStage {
     off += bytes;
     return o;
   }
+  const CallOrder order;
   size_t off = 0, in_end = 0, host_end = 0, o_x = 0, o_n = SIZE_MAX;
   bool queued = false;
   std::vector<In> ins;

@@ -253,6 +253,7 @@ int vtts_vocoder_stream_push(vtts_ctx* ctx, vtts_vocoder_stream* vs, const float
   rc = sl.check(ctx, "vocoder_stream_push", F, n_new, flags);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   cudaStream_t st = (cudaStream_t)stream;
 
   // ---- host bookkeeping: per slot the frames before and after this push; per conv and slot the row bounds ----

@@ -167,7 +167,8 @@ struct vtts_ctx {
   int* d_err = nullptr;
   // tile scheduler counters of the tensor-core launches: [0] next ticket, [1] CTAs done taking tickets.  Each launch
   // leaves them at zero.  One pair serves every launch of the context because a context's tensor-core launches never
-  // overlap: they run in order on the one stream of the call that issues them (calls share the workspace, too).
+  // overlap: a call issues its launches in order on its one stream, and CallOrder puts each call after the one issued
+  // before it, whatever stream that one ran on (calls share the workspace and the error flag, too).
   int* d_tc_sched = nullptr;
   long long* d_tc_dbg = nullptr;   // [256][16] profiling counters of the last tensor-core conv launch
   bool tc_dbg_on = false;
@@ -180,6 +181,8 @@ struct vtts_ctx {
   std::string err;
   int64_t launches = 0;
   cudaStream_t own_stream = nullptr;   // used by the *_host entry points
+  cudaEvent_t tail = nullptr;          // recorded at the end of every call, on its stream (CallOrder)
+  int order_depth = 0;                 // CallOrder scopes open: a call made inside another adds no wait or record
 
   // ---- weights (device) ----
   ModelWeights hg;              // HiFiGAN generator
@@ -253,6 +256,38 @@ struct vtts_ctx {
 };
 
 extern std::string g_vtts_create_error;
+
+// The calls of one context run in the order they are issued, whatever stream each is given: every call shares the
+// workspace, the tile-scheduler counters and the error flag, so two calls' launches must never overlap.  Every entry
+// point that takes a stream, and every host-buffer call (HostStage), opens one CallOrder on its stream after its
+// argument checks and before its first launch or copy: the stream waits for ctx->tail, the end of the context's last
+// call, and ctx->tail is recorded on the stream when the scope closes.  The event, not a remembered stream, carries the
+// order, so a caller may destroy a stream as soon as its call has returned.  A call made from inside another call runs
+// on that call's stream and adds nothing.  On a stream that is capturing a CUDA graph neither step runs: a wait on a
+// record made outside the capture cannot join the graph, and a record inside it would leave ctx->tail pointing into a
+// graph.  The caller orders a graph's replays against the context's other calls.
+class CallOrder {
+ public:
+  CallOrder(vtts_ctx* c, void* stream) : ctx(c), st((cudaStream_t)stream) {
+    if (ctx->order_depth++) return;
+    cudaSetDevice(ctx->device);
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    on = cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone;
+    // a failed wait (a bad stream handle) stays the runtime's last error, which the call's first launch check reports
+    if (on) cudaStreamWaitEvent(st, ctx->tail, 0);
+  }
+  ~CallOrder() {
+    --ctx->order_depth;
+    if (on) cudaEventRecord(ctx->tail, st);
+  }
+  CallOrder(const CallOrder&) = delete;
+  CallOrder& operator=(const CallOrder&) = delete;
+
+ private:
+  vtts_ctx* const ctx;
+  const cudaStream_t st;
+  bool on = false;
+};
 
 // bump allocator over the context workspace
 struct Arena {

@@ -309,6 +309,7 @@ int vtts_watermark(vtts_ctx* ctx, const float* x_dev, const int32_t* n_dev, int 
   if (!x_dev || !y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "watermark: null pointer");
   if (x_dev == y_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "watermark: y must not alias x");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return wm_launch(ctx, x_dev, n_dev, B, S, key, strength, y_dev, (cudaStream_t)stream);
 }
 
@@ -330,6 +331,7 @@ int vtts_watermark_detect(vtts_ctx* ctx, const float* x_dev, const int32_t* n_de
   if (rc) return rc;
   if (!x_dev || !keys_dev || !z_dev || !offset_dev) return ctx->fail(VTTS_ERR_BAD_ARG, "watermark_detect: null pointer");
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return det_launch(ctx, x_dev, n_dev, B, S, rate, keys_dev, K, search, z_dev, offset_dev, (cudaStream_t)stream);
 }
 
@@ -387,6 +389,7 @@ int vtts_watermark_stream_push(vtts_ctx* ctx, vtts_watermark_stream* ws, const f
   if (!rc) rc = ws->slots.check(ctx, "watermark_stream_push", ws->F, n_new, flags);
   if (rc) return rc;
   VTTS_CUDA(cudaSetDevice(ctx->device));
+  const CallOrder order(ctx, stream);
   return ws->push("watermark_stream_push", x_dev, n_new, flags, y_dev, n_out, wm_gain(ws->key, ws->strength), ws->strength == 0.f,
                   (cudaStream_t)stream);
 }
